@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- BA windows/s of the B200 window solver on BASELINE.json's headline configuration, plus one sub-record per
+"""bench.py -- BA windows/s of the H100 window solver on BASELINE.json's headline configuration, plus one sub-record per
 other BASELINE configuration.
 
 Headline: one "step" = one complete trimmed bundle-adjustment solve (all LM iterations + trimming round, Ceres-equivalent
@@ -15,7 +15,7 @@ than L2 or stated otherwise; each with the CPU oracle beside it):
   config5         100 KF / 20k LM / 300k obs window: one GPU, and -- when launched on N > 1 ranks -- the landmark-sharded
                   solve with the NCCL all-reduce of the reduced system, checked against the one-GPU solve (row 5)
 
-  python bench.py [--gpus N] [--steps K] [--warmup W] [--batch B] [--impl reference] [--no-sub]
+  python bench.py [--gpus N] [--steps K] [--warmup W] [--batch B] [--impl reference] [--no-sub] [--dump-outputs DIR]
 """
 import argparse
 import json
@@ -41,15 +41,11 @@ FUSED = os.environ.get("KBA_FUSED", "1") != "0"
 # bytes of such a fused kernel: reads 16 + 2.7, writes E_ij 144 per observation + (C_j 48 + g_j 24) per landmark = 5.4 -> 168 B.
 LIN1 = FUSED and os.environ.get("KBA_LINEARIZE", "1") != "0"
 B_OBS_ALGORITHMIC = 168.0 if LIN1 else (187.0 if FUSED else 259.0)
-# dram__bytes_read.sum + dram__bytes_write.sum of one launch of that kernel / its observations, from the ncu --set full
-# capture summarised in profiles/ (re-measured whenever the kernel changes)
-B_OBS_DRAM_MEASURED = 184.6 if LIN1 else (199.0 if FUSED else 277.0)
-TRAFFIC_SOURCE = ("ncu --set full, profiles/r02_ncu_summary.md (k_linearize)" if LIN1 else
-                  "ncu --set full, profiles/r02_ncu_summary.md (k_eval_obs<true>, J_landmark not materialised)" if FUSED else
-                  "ncu --set full, profiles/r01_v11_ncu_summary.md: (0.200 GB read + 1.293 GB written) / 5.39 M observations")
+# the kernel's DRAM traffic is not measured (no hardware-counter profiler): "traffic" is the algorithmic bytes of its launches
+TRAFFIC_SOURCE = "algorithmic bytes per observation x observations per launch (DRAM traffic not measured)"
 KERNEL_NAME = ("k_linearize (residual/Jacobian + landmark blocks + V rows, one kernel)" if LIN1 else "k_eval_obs<true> (residual/Jacobian)")
 ALG_NOTE = ("SURVEY 8(d), fused Hessian kernel: 18.7 B read + 144 B (E_ij) written per observation + 72 B per landmark; the Jacobian "
-            "stays in registers.  The kernel is bound by instruction latency at 16 warps per SM (issue slots 31 % used, FP64 pipe 24 % busy), not by HBM: see profiles/r02_ncu_summary.md" if LIN1 else
+            "stays in registers, so the kernel is bound by FP64 instruction latency rather than by HBM" if LIN1 else
             "19 B read + 168 B written (residual 24 + J_pose 144); J_landmark (72 B) is not materialised" if FUSED else "SURVEY 8(d): 259 B/obs")
 CONFIG2 = "config 2: 30 KF / 3000 LM / 40000 obs, mono + lidar depth, FP64"
 
@@ -67,7 +63,7 @@ def make_windows(n_distinct, rank, config=2):
 
 
 class ClockSampler:
-    """nvidia-smi clock / throttle-reason sampling during the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clock / throttle-reason sampling during the timed region (read-only queries)."""
 
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
@@ -116,11 +112,8 @@ class ClockSampler:
 
 
 def measured_peak():
-    p = os.path.join(ROOT, "MEASURED_PEAKS.json")
-    if os.path.exists(p):
-        with open(p) as f:
-            return float(json.load(f)["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    """HBM bandwidth the roofline fractions are taken against: NVIDIA's H100 SXM data sheet figure (HBM3, 80 GB)"""
+    return 3350.0, "H100 SXM data sheet (3.35 TB/s), not measured"
 
 
 # ---------------------------------------------------------------------------------------------------------------------
@@ -145,9 +138,9 @@ def cpu_threads_all():
 
 
 def thread_candidates(cores):
-    """OpenMP thread counts probed for the CPU legs.  The oracle parallelises over observations and is memory-bound: on the
-    128-core, two-socket GPU hosts 128 threads measured 25x SLOWER than 32 (profiles/r02_bench.md), so the probe stays
-    within one socket's worth of threads and picks the fastest."""
+    """OpenMP thread counts probed for the CPU legs.  The oracle parallelises over observations and is memory-bound: on a
+    two-socket host, threads beyond one socket slow it down, so the probe stays within one socket's worth of threads and
+    picks the fastest."""
     return sorted({t for t in (16, 32, 64) if t <= cores} or {cores})
 
 
@@ -260,7 +253,7 @@ def sub_config2_batches(torch, capi, h, stream, base, opt, cpu_ws):
 def sub_config3(torch, capi, h, stream, rank):
     """config 3: + ground-plane residuals, plane blocks and the regularisation chain; FP64 and FP32 linearisation"""
     wins = make_windows(8, rank, config=3)
-    batch_n = 148
+    batch_n = 132  # one window per SM of an H100
     tiled = [wins[i % len(wins)] for i in range(batch_n)]
     rec = {"workload": "config 3: 30 KF / 3000 LM / 40000 obs + ground-plane prior + plane chain, trimmed", "batch": batch_n}
     results = {}
@@ -385,18 +378,50 @@ def sub_config5(torch, capi, h, stream, rank, local_rank, world):
     return rec
 
 
+DUMP_LIMIT_BYTES = 64 << 20
+
+
+def dump_outputs(out_dir, windows, results):
+    """The results of one batch solve as the caller receives them, concatenated over the windows in batch order (float64;
+    lm_rejected as float32).  When the whole batch exceeds DUMP_LIMIT_BYTES a fixed, seeded sample of windows is written;
+    window_index.npy says which."""
+    def nbytes(w):
+        return 8 * (11 * w.n_kf + 3 * w.n_lm + 4) + 4 * w.n_lm
+    idx = np.arange(len(windows))
+    if sum(nbytes(w) for w in windows) > DUMP_LIMIT_BYTES:
+        idx = np.random.default_rng(0).permutation(len(windows))
+        keep = np.cumsum([nbytes(windows[i]) for i in idx]) <= DUMP_LIMIT_BYTES - 8 * len(windows)
+        idx = np.sort(idx[keep])
+    rs, ws = [results[i] for i in idx], [windows[i] for i in idx]
+    arrays = {
+        "window_index": idx.astype(np.float64),
+        "kf_pose": np.concatenate([r.kf_pose for r in rs]),
+        "kf_plane": np.concatenate([r.kf_plane for r in rs]),
+        "lm_pos": np.concatenate([r.lm_pos[:w.n_lm] for r, w in zip(rs, ws)]),
+        "lm_rejected": np.concatenate([r.lm_rejected[:w.n_lm] for r, w in zip(rs, ws)]).astype(np.float32),
+        "initial_cost": np.array([r.c.initial_cost for r in rs], dtype=np.float64),
+        "final_cost": np.array([r.c.final_cost for r in rs], dtype=np.float64),
+        "status": np.array([r.c.status for r in rs], dtype=np.float64),
+        "lm_iterations": np.array([sum(s.num_iterations for s in r.solves) for r in rs], dtype=np.float64),
+    }
+    os.makedirs(out_dir, exist_ok=True)
+    for name, a in arrays.items():
+        np.save(os.path.join(out_dir, name + ".npy"), a)
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
     ap.add_argument("--steps", type=int, default=5)
     ap.add_argument("--warmup", type=int, default=3)
-    ap.add_argument("--batch", type=int, default=296, help="windows per GPU per step (two per SM: the windows of a batch\n"
+    ap.add_argument("--batch", type=int, default=264, help="windows per GPU per step (two per SM of an H100: the windows of a batch\n"
                     "advance in lock-step passes, a larger batch amortises the passes in which only the slowest windows are left)")
     ap.add_argument("--distinct", type=int, default=16, help="distinct synthetic windows per GPU (tiled to --batch)")
     ap.add_argument("--impl", default="b200", choices=["b200", "reference"])
     ap.add_argument("--cpu-sample", type=int, default=6, help="window solves timed for cpu_baseline (~0.5 s each); 0 = skip the CPU legs")
     ap.add_argument("--in-flight", type=int, default=4, help="steps in flight of the end-to-end measurement (handles / streams)")
     ap.add_argument("--no-sub", action="store_true", help="headline only: skip the sub-records of configs 3, 4, 5 and the batch sweep")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write what the last timed step returned to its caller as DIR/<name>.npy")
     args = ap.parse_args()
 
     from limo_b200 import parallel
@@ -450,6 +475,8 @@ def main():
     cnt = h.counters(reset=True)
     h.enable_kernel_timing(False)
     results = batch.download()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, windows, results)
     done = all(r.c.status == 0 for r in results)
     converged = all(r.solves[r.c.num_solves - 1].termination == 0 for r in results)  # KBA_TERM_CONVERGENCE of the final solve
     iters = [sum(s.num_iterations for s in r.solves) for r in results]
@@ -573,7 +600,7 @@ def main():
             "roofline": {"kernel": KERNEL_NAME, "bound": "hbm", "achieved": jac_gbs,
                          "peak": peak, "unit": "GB/s", "frac": (jac_gbs / peak) if jac_gbs else None,
                          "peak_source": peak_src,
-                         "traffic": B_OBS_DRAM_MEASURED * cnt.jacobian_obs / max(cnt.launches_jacobian, 1),
+                         "traffic": B_OBS_ALGORITHMIC * cnt.jacobian_obs / max(cnt.launches_jacobian, 1),
                          "traffic_unit": "bytes per launch", "traffic_source": TRAFFIC_SOURCE,
                          "algorithmic_bytes_per_obs": B_OBS_ALGORITHMIC,
                          "algorithmic_note": ALG_NOTE,

@@ -1,5 +1,5 @@
 /*
- * kba_b200.h -- C ABI of the B200-native keyframe bundle-adjustment hot path.
+ * kba_b200.h -- C ABI of the H100-native (sm_90a) keyframe bundle-adjustment hot path.
  *
  * This is the drop-in boundary for limo's `keyframe_bundle_adjustment` window solve.
  * The reference has no FFI: its "operator API" is the C++ class
@@ -16,7 +16,7 @@
  * the kba_batch_* entry points keep a batch of windows resident in HBM.
  *
  * The library has NO CPU fallback: every entry point that computes returns KBA_ERR_CUDA if no
- * sm_100-class device is usable.
+ * sm_90 (H100-class) device is usable.
  */
 #ifndef KBA_B200_H
 #define KBA_B200_H

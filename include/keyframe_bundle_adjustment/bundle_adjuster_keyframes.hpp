@@ -1,6 +1,6 @@
 // bundle_adjuster_keyframes.hpp -- source-compatible facade of limo's BundleAdjusterKeyframes (reference:
 // keyframe_bundle_adjustment/include/keyframe_bundle_adjustment/bundle_adjuster_keyframes.hpp:40-335) whose solve() /
-// adjustPoseOnly() run on the B200 through the C ABI of kba_b200.h instead of Ceres.  Same namespace, class name, public
+// adjustPoseOnly() run on the H100 through the C ABI of kba_b200.h instead of Ceres.  Same namespace, class name, public
 // members, method signatures and exceptions; the private ceres::Problem member is replaced by a kba_handle.  The types
 // around it live where the reference keeps them: internal/definitions.hpp, keyframe.hpp, landmark_selector.hpp,
 // landmark_selection_schemes.hpp, matches_msg_types/*.hpp.

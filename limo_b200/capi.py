@@ -1,7 +1,7 @@
 """ctypes binding of the CUDA library limo_b200/libkba_b200.so (C ABI: include/kba_b200.h).
 
 The product path: there is no CPU fallback.  Importing works without a GPU (symbols can be inspected), but every
-computing call fails with KBA_ERR_CUDA when no sm_100 device is present.
+computing call fails with KBA_ERR_CUDA when no sm_90 (H100) device is present.
 """
 import ctypes as C
 import os

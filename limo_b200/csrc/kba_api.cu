@@ -39,7 +39,7 @@ struct kba_handle {
     cudaEvent_t ev0 = nullptr, ev1 = nullptr;
     std::vector<cudaEvent_t> ev_pool;  // event pairs around every residual/Jacobian launch (kernel timing)
     int ev_used = 0;
-    int sm_count = 148;
+    int sm_count = 132;
     cudaEvent_t ev_block = nullptr;  // blocking-sync event: waiting host threads sleep instead of spinning on a core
     bool blocking_sync = false;      // KBA_BLOCKING_SYNC=1 at kba_create
     // grow-only device workspace of the single-shot entry points (kba_lidar_depth): no cudaMalloc / cudaFree per call
@@ -553,7 +553,11 @@ int kba_create(kba_handle** out, int device) {
     CU(cudaSetDevice(device));
     cudaDeviceProp prop;
     CU(cudaGetDeviceProperties(&prop, device));
-    if (prop.major < 10) return fail(KBA_ERR_CUDA, "kba_b200 kernels are built for sm_100a only");
+    // the library holds sm_90a code only (TMA bulk copies, mbarrier transaction counts, setmaxnreg), which no other compute
+    // capability can load
+    if (prop.major != 9 || prop.minor != 0)
+        return fail(KBA_ERR_CUDA, "kba_b200 kernels are built for sm_90a (H100) only, device " + std::to_string(device) +
+                                      " is sm_" + std::to_string(prop.major) + std::to_string(prop.minor));
     kba_handle* h = new kba_handle();
     h->device = device;
     h->sm_count = prop.multiProcessorCount;
@@ -654,6 +658,7 @@ int kba_batch_create(kba_handle* h, int32_t n_windows, const kba_window* w, kba_
     bd.tot_groups = (int)groups;
     bd.nr_cap_max = nr_cap_max;
     b->lc.nr_cap_max = nr_cap_max;
+    b->lc.sm_count = h->sm_count;
     // split the landmark chunks of each window over several CTAs when the batch alone cannot fill the GPU
     {
         const int nb = nr_cap_max / 64, pairs = nb * (nb + 1) / 2;
@@ -681,7 +686,7 @@ int kba_batch_create(kba_handle* h, int32_t n_windows, const kba_window* w, kba_
     { const char* le = std::getenv("KBA_LIN_BLOCKS"); if (le && std::atoi(le) == 3) b->lc.lin_blocks = 3; }
     { const char* le = std::getenv("KBA_LIN_GRID"); if (le) b->lc.lin_grid = std::max(-1, std::atoi(le)); }
     { const char* le = std::getenv("KBA_BS_GRID"); if (le) b->lc.bs_grid = std::max(-1, std::atoi(le)); }
-    {  // tuning knobs of the residual/Jacobian kernel (defaults measured on B200, see DESIGN.md)
+    {  // tuning knobs of the residual/Jacobian kernel (see DESIGN.md)
         auto knob = [](const char* name, int dflt) { const char* e = std::getenv(name); return e ? std::atoi(e) : dflt; };
         bd.eval_tiles_jac = std::max(1, knob("KBA_EVAL_TILES_JAC", 8));
         bd.eval_tiles_cost = std::max(1, knob("KBA_EVAL_TILES_COST", 8));
@@ -1024,7 +1029,7 @@ int kba_batch_solve(kba_batch* b, const kba_options* opt) {
         }
         // Completion check without draining the queue: every `check_every` passes the active-window count is copied out behind an
         // event, the next passes are enqueued at once, and the count is READ one check later.  The device never waits for the
-        // host (a synchronous poll emptied the queue 12-15 times per solve: ~1 ms of a 14 ms single-window solve); the price is
+        // host (a synchronous poll would empty the queue a dozen times per solve); the price is
         // up to `check_every` passes enqueued after the last window finished, in which every kernel exits at once.  In a sharded
         // solve the state -- hence the count -- is identical on all ranks, so they still issue the same passes.
         if ((pass + 1) % check_every == 0 || pass + 1 == max_passes) {

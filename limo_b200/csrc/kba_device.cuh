@@ -1,4 +1,4 @@
-// kba_device.cuh -- device-side data model and per-observation math of the B200 window solver.
+// kba_device.cuh -- device-side data model and per-observation math of the H100 window solver.
 //
 // Layout rule: everything that is streamed per observation is SoA over the whole batch (component-major), so that
 // a warp touching 32 consecutive observations issues fully coalesced 128-/256-byte transactions; everything that is

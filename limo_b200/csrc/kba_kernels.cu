@@ -1,4 +1,4 @@
-// kba_kernels.cu -- sm_100a kernels of the window solver.  One LM "pass" over a batch of windows is, for small windows
+// kba_kernels.cu -- sm_90a kernels of the window solver.  One LM "pass" over a batch of windows is, for small windows
 // (every window <= 184 reduced rows and <= 32 keyframes: BASELINE configs 1-3),
 //   k_solve_begin [-> k_gp_eval<true>] -> k_linearize (kba_linearize.cuh: evaluation + landmark blocks + V rows, Jacobian in registers)
 //   -> k_pose_hessian -> k_schur_fused (kba_schur_fused.cuh: warp-specialised FP64 tensor-core SYRK over bulk-copied V columns)
@@ -30,8 +30,8 @@ namespace kba {
 // =====================================================================================================================
 // solve begin: program layout (which parameter blocks are in the reduced program) + LM state reset
 // =====================================================================================================================
-// 1024 threads: the layout tables of a solve's first pass are dependent-load chains per landmark / observation (0.2 ms per
-// solve begin with 256 threads, three to four per trimmed solve: 5 % of a single-window solve)
+// 1024 threads: the layout tables of a solve's first pass are dependent-load chains per landmark / observation, and a trimmed
+// solve begins three to four times
 constexpr int kBeginThreads = 1024;
 __global__ void __launch_bounds__(kBeginThreads) k_solve_begin(BatchDev bd, SolveParams sp) {
     const int w = blockIdx.x;
@@ -959,8 +959,8 @@ __global__ void __launch_bounds__(256) k_sred_reduce(BatchDev bd, int mode) {
 
 // stage 0: the whole solve in this one CTA.  Large reduced systems of small batches split it (launch_pass): stage 1 =
 // assembly, Jacobi scaling and damping only; then per 32-column block k_chol_diag / k_chol_panel / k_chol_trail spread
-// the factorisation over many SMs (one SM's FP64 throughput bounds the n^3/3 trailing flops of a 594-row system at
-// 0.55 ms); stage 2 = back substitution and candidate state only.
+// the factorisation over many SMs (one SM's FP64 throughput bounds the n^3/3 trailing flops of a 594-row system);
+// stage 2 = back substitution and candidate state only.
 template <bool kTiled>
 __global__ void __launch_bounds__(512, 1) k_reduced_solve(BatchDev bd, SolveParams sp, int stage) {
     const int w = blockIdx.x;
@@ -1264,7 +1264,7 @@ __global__ void __launch_bounds__(512, 1) k_reduced_solve(BatchDev bd, SolvePara
         // Four lanes per row: lane a of a quad owns the columns c = 4 e + a.  Step q: the owner of column q scales it and
         // hands it to the quad (one shuffle), every lane eliminates it from its own later columns -- the same operations on the
         // same values in the same order as one thread per row, but 572 instead of 143 busy threads and a quarter of the
-        // dependent chain per thread (51 k -> cycles per solve of a 174-row system, profiles/).
+        // dependent chain per thread.
         {
             const int quad = tid >> 2, qa = tid & 3;
             const volatile double* vD = s_D;  // volatile: keeps the factor entries from being hoisted out of the row loop
@@ -1687,9 +1687,8 @@ __global__ void __launch_bounds__(256) k_backsub(BatchDev bd) {
 
 // Fused path: sum_i V_i^T delta_f,i from the compact per-observation V (k_obs_v2; landmark-column-major): each lane reads
 // its observation's three 48-byte column segments with nine 128-bit loads, consecutive lanes consecutive segments.
-// Measured and dropped (profiles/r02_graph_and_ab.md): requesting the V segments before obs_row has come back and the landmark's
-// L^-1 / z / g / lambda before the reduction (one round of memory latency instead of three) made a 296-window step 1.6 ms SLOWER --
-// not profiled further; the kernel stays as it is.
+// Tried and dropped: requesting the V segments before obs_row has come back and the landmark's L^-1 / z / g / lambda before the
+// reduction (one round of memory latency instead of three) made the headline step slower -- not profiled further.
 // kLoop: the CTAs of a window stride over its 16-landmark units (grid.x < n_units, LaunchCfg::bs_grid); unit = partial-sum slot
 template <bool kLoop>
 __global__ void __launch_bounds__(256) k_backsub_v(BatchDev bd, int n_units) {
@@ -1999,7 +1998,7 @@ __global__ void __launch_bounds__(256) k_trim_eval(BatchDev bd, SolveParams sp) 
     __syncthreads();
     const int lane = threadIdx.x & 31;
     // 64 landmarks per CTA (8 rounds of one landmark per warp): the kernel is launched in every pass and idles in all but the one or
-    // two trimming passes of a solve -- with 8 landmarks per CTA the idle launch of a 148-window batch alone cost 49 us per pass
+    // two trimming passes of a solve, so its idle launch over a large batch should be few CTAs
     for (int it = 0; it < 8; ++it) {
     const int j = (blockIdx.x * 8 + it) * 8 + (threadIdx.x >> 5);
     if (j >= wd.n_lm) continue;
@@ -2138,7 +2137,7 @@ __global__ void __launch_bounds__(512) k_trim_select(BatchDev bd, SolveParams sp
         const unsigned long long pivot = s_prefix;  // bit pattern of the value with rank `num`
         const int tie_keep = s_k;                   // ties with fewer than tie_keep smaller-index ties stay
         // how many values equal the pivot?  Normally one (the pivot itself): then the O(n) index count below -- one thread walking
-        // every value, 50-100 us per group -- is not needed
+        // every value -- is not needed
         __syncthreads();
         if (threadIdx.x == 0) s_n = 0;
         __syncthreads();
@@ -2294,17 +2293,18 @@ cudaError_t configure_kernels(int nr_cap_max) {
 
 // grid.x of a kernel whose CTAs stride over a window's units (k_linearize: 8 warp tiles, k_backsub_v: 16 landmarks).  Every pass is
 // launched for every window of the batch and the unit count is an upper bound, so with one CTA per unit most CTAs of a large batch
-// only find out that they have nothing to do; num/den of the units per window from the sweep on the headline workload
-// (profiles/r02_graph_and_ab.md: 296-window step 211.2 -> 202.9 ms at 3/10 and 1/3, 199.5 ms at 1/5 for k_linearize; k_backsub_v is
-// flat between 1/6 and 1/2).  Small batches keep one CTA per unit (latency: every SM busy).
+// only find out that they have nothing to do; num/den of the units per window come from a sweep on the headline workload
+// (k_linearize: 1/5, k_backsub_v: 1/3; any grid gives bit-identical results).  Small batches keep one CTA per unit (latency: every
+// SM busy).
 // `cfg`: -1 = this rule, 0 = one CTA per unit, > 0 = that many (KBA_LIN_GRID / KBA_BS_GRID).
-static int strided_grid(int cfg, int n_units, int num, int den, int n_win) {
+static int strided_grid(int cfg, int n_units, int num, int den, int n_win, int sm_count) {
     if (cfg == 0) return n_units;
     if (cfg > 0) return cfg < n_units ? cfg : n_units;
     const int g = (n_units * num + den - 1) / den;
-    return ((long long)g * n_win >= 8 * 296 && g >= 1) ? g : n_units;  // at least eight waves of 2 CTAs x 148 SMs remain (a CTA
-                                                                        // now runs several units back to back: keep the last,
-                                                                        // partly filled wave a small share of the launch)
+    return ((long long)g * n_win >= 8LL * 2 * sm_count && g >= 1) ? g : n_units;  // at least eight waves of 2 CTAs per SM remain
+                                                                                   // (a CTA now runs several units back to back:
+                                                                                   // keep the last, partly filled wave a small
+                                                                                   // share of the launch)
 }
 
 void launch_reset(const BatchDev& bd, const LaunchCfg& lc, cudaStream_t s) {
@@ -2326,7 +2326,7 @@ int launch_pass(const BatchDev& bd, const SolveParams& sp, const LaunchCfg& lc, 
         LCHK("k_gp_eval");
         if (timed) cudaEventRecord(lc.ev_pool[(*lc.ev_used)++], s);
         const int n_units = (lin_tile_bound(bd.max_obs, bd.max_lm) + kLinWarps - 1) / kLinWarps;
-        const dim3 g_lin(strided_grid(lc.lin_grid, n_units, 1, 5, B), B);  // CTAs of a window stride over its units
+        const dim3 g_lin(strided_grid(lc.lin_grid, n_units, 1, 5, B, lc.sm_count), B);  // CTAs of a window stride over its units
         if ((int)g_lin.x < n_units) k_linearize<2, true><<<g_lin, kLinThreads, 0, s>>>(bd, sp, n_units);
         else if (lc.lin_blocks == 3) k_linearize<3, false><<<g_lin, kLinThreads, 0, s>>>(bd, sp, n_units);
         else k_linearize<2, false><<<g_lin, kLinThreads, 0, s>>>(bd, sp, n_units);
@@ -2396,7 +2396,7 @@ int launch_pass(const BatchDev& bd, const SolveParams& sp, const LaunchCfg& lc, 
     }
     if (bd.fused) {
         const int n_units = (bd.max_lm + 15) / 16;
-        const int gx = strided_grid(lc.bs_grid, n_units, 1, 3, B);
+        const int gx = strided_grid(lc.bs_grid, n_units, 1, 3, B, lc.sm_count);
         if (gx < n_units) k_backsub_v<true><<<dim3(gx, B), 256, 0, s>>>(bd, n_units);
         else k_backsub_v<false><<<dim3(n_units, B), 256, 0, s>>>(bd, n_units);
     }

@@ -36,6 +36,7 @@ struct Exchange {
 
 struct LaunchCfg {
     int nr_cap_max = 64;
+    int sm_count = 132;       // SMs of the device the batch runs on (strided_grid: waves of CTAs)
     int max_rank = 0;         // largest observation rank in the batch (multi-camera rigs)
     bool small_syrk = false;  // every window has <= 184 reduced rows: register-resident Schur kernel
     bool lin_fused = true;    // fused path: evaluation + landmark blocks + V rows in one kernel (k_linearize); KBA_LINEARIZE=0: three kernels

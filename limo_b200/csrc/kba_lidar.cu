@@ -1,4 +1,4 @@
-// kba_lidar.cu -- lidar depth extraction on sm_100a (BASELINE config 4; C ABI: kba_lidar_depth in kba_b200.h).
+// kba_lidar.cu -- lidar depth extraction on sm_90a (BASELINE config 4; C ABI: kba_lidar_depth in kba_b200.h).
 //   k_lidar_bin<false>: project the cloud (coalesced float loads), count points per 16x16-pixel image cell
 //   k_lidar_scan      : exclusive scan of the cell counts (one CTA)
 //   k_lidar_bin<true> : project again and scatter (u, v, x, y, z, index) into cell-sorted order

@@ -5,7 +5,7 @@
 //               + V_i = (J_p^T J_l) L^-T of every observation (as k_obs_v2)
 //
 // Round 1 / early round 2 ran these as three kernels around a materialised J_p (168 B per observation written, then read
-// twice: 0.93 ms and 634 B of DRAM traffic per observation for a 148-window batch).  Here nothing of the Jacobian reaches
+// twice).  Here nothing of the Jacobian reaches
 // memory: a lane evaluates its observation, keeps J_p (18 doubles) in registers and writes only what the Schur kernel and
 // the back substitution consume -- V_i (144 B per observation) and the landmark's L^-1, z, g, lambda.  A rejected LM
 // step (new radius, same x) simply runs the kernel again: re-evaluating is cheaper than re-reading.
@@ -17,7 +17,7 @@
 // leave their block contributions in the warp's shared-memory strip, lane (landmark, component) sums its segment in
 // observation order (the order of the CPU oracle; fixed -> bit-reproducible), every lane then factors its landmark's
 // damped block redundantly (it needs L^-1 anyway) -- no CTA barrier between evaluation and V.  A first version with CTA-wide tiles and one thread per landmark for the block sums stalled 256
-// threads on two barriers around a serial sqrt / divide chain: 0.72 ms per pass of a 148-window batch (profiles/).
+// threads on two barriers around a serial sqrt / divide chain.
 #pragma once
 #include "kba_device.cuh"
 
@@ -34,12 +34,12 @@ __device__ __forceinline__ size_t lin_tile_offset(const WinDesc& wd, int w) {
     return (size_t)(wd.obs_off / 16) + (size_t)(wd.lm_off / 32) + 4 * (size_t)w;
 }
 
-// Measured and dropped (profiles/r02_graph_and_ab.md): a descriptor that also carries the first landmark and a segment-start mask,
+// Tried and dropped: a descriptor that also carries the first landmark and a segment-start mask,
 // so that a lane requests its landmark's data together with its observation's (no obs_lm -> lm_ptr round first), made the kernel
-// 1.5 % slower -- the bit arithmetic costs more than the dependent loads, which mostly hit L2.
+// slower -- the bit arithmetic costs more than the dependent loads, which mostly hit L2.
 // called by k_solve_begin (one CTA per window).  The tiling depends on the CSR only.  Greedy packing is sequential, so the
 // landmarks are cut into <= 512 chunks that are packed independently by one thread each (pass 1 counts, a scan places the
-// chunks, pass 2 writes): a serial pass over 3000 landmarks cost 270 us per solve begin, this one a few.
+// chunks, pass 2 writes): one thread walking thousands of landmarks would be a long serial chain in every solve begin.
 __device__ inline void build_lin_tiles(const BatchDev& bd, const WinDesc& wd, WinState& st, int w, int* s_chunk /* [513] */) {
     const int* lm_ptr = bd.lm_ptr + wd.lm_off + w;
     int2* tiles = bd.lin_tile + lin_tile_offset(wd, w);
@@ -81,11 +81,11 @@ __device__ inline void build_lin_tiles(const BatchDev& bd, const WinDesc& wd, Wi
 }
 
 // kMinBlocks: CTAs per SM the register allocation is sized for.  2: everything in registers (128 per thread); 3: 80 registers, the
-// Jacobian rows spill to local memory across the segment sums (KBA_LIN_BLOCKS, measured in profiles/r02_linearize.md)
+// Jacobian rows spill to local memory across the segment sums (KBA_LIN_BLOCKS)
 // n_units = ceil(lin_tile_bound / kLinWarps): a unit is 8 consecutive warp tiles and owns cost slot `unit`.  The CTAs of a window
 // stride over the units (grid.x <= n_units; grid.x == n_units: one unit per CTA, the original launch): the tile bound is 1.7x the
 // tiles a window really has and every pass is launched for every window, so a smaller grid saves the CTAs that would only find out
-// that they have nothing to do (profiles/r02_ncu_summary.md, addendum) and stages the poses once for several units.
+// that they have nothing to do and stages the poses once for several units.
 // kLoop = false: grid.x == n_units, compiled without the loop (no loop-carried registers: the loop form spills 120 bytes).
 template <int kMinBlocks, bool kLoop>
 __global__ void __launch_bounds__(kLinThreads, kMinBlocks) k_linearize(BatchDev bd, SolveParams sp, int n_units) {

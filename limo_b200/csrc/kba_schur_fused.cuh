@@ -8,9 +8,9 @@
 //                          landmark-column-major, and a track without gaps sits on consecutive rows, so a landmark's panel
 //                          column is ONE bulk copy (cp.async.bulk, 48 B per observation, complete_tx on the stage's "full"
 //                          mbarrier): 24 bulk copies + the z rows per group, nobody waits for data and the ring runs five
-//                          groups ahead.  Measured alternatives (profiles/r02_schur_fused.md): zero segments as bulk copies too
-//                          (no stores by the SM at all: slower, a warp issues its bulk copies one lane after the other, ~65
-//                          cycles each), 16-byte cp.async per lane instead of bulk copies (equal or slower).  Landmarks whose rows are not one run fall back to nine 16-byte
+//                          groups ahead.  Alternatives tried and dropped: zero segments as bulk copies too (no stores by the
+//                          SM at all, but a warp issues its bulk copies one lane after the other), 16-byte cp.async per lane
+//                          instead of bulk copies.  Landmarks whose rows are not one run fall back to nine 16-byte
 //                          cp.async per observation; windows with ground-plane rows or several cameras per keyframe (rows
 //                          that ADD onto others) take a synchronous variant of the same loop.
 //   consumers (12 warps) : Sred += V V^T on the FP64 tensor cores (mma.sync m8n8k4).  The whole lower triangle lives in
@@ -19,10 +19,10 @@
 //   ring                 : 6 panel stages with full / empty mbarriers, so warps drift up to five groups apart and the
 //                          per-group imbalance of the static block -> warp map (scripts/syrk_map_search.py) averages out.
 //
-// Replaces k_obs_v + k_gp_panel + k_schur_syrk_tma of round 1 (2.2 GB of zero-padded panels written and re-read per pass of
-// a 148-window batch; now 144 B per observation).  Forming V inside the producer warps was measured too: with only four
-// warps the ~250 dependent instructions per observation are latency-bound (5400 cycles per group against 1900 of tensor
-// work), see profiles/.  Included by kba_kernels.cu after dmma(), the mbarrier helpers and gp_row().
+// Replaces k_obs_v + k_gp_panel + k_schur_syrk_tma of round 1 (zero-padded panels written and re-read every pass; now 144 B
+// per observation).  Forming V inside the producer warps was tried too: with only four warps the ~250 dependent instructions
+// per observation are latency-bound next to the tensor work.  Included by kba_kernels.cu after dmma(), the mbarrier helpers
+// and gp_row().
 #pragma once
 
 namespace kba {
@@ -91,7 +91,7 @@ constexpr size_t schur_fused_smem() { return (size_t)kFStages * kFStageDoubles *
 
 // Landmark groups per CTA and CTAs that own groups, for a window with n_groups groups in a batch launched with p_split CTAs per
 // window.  At least 8 groups per CTA: every CTA writes a whole partial triangle (up to 295 KB) that k_sred_reduce folds again --
-// one window alone spread over 148 CTAs spent 47 us per pass folding 148 partials.  Because of the floor the partition of a small
+// one window alone spread over every SM would leave one partial per SM to fold in every pass.  Because of the floor the partition of a small
 // window is the same whether it is solved alone, in a batch or inside the capacity-sized batch of a persistent window
 // (kba_track_*), which keeps those paths bit-identical.
 __device__ __forceinline__ void schur_split(int n_groups, int p_split, int& per, int& used) {

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""A/B of library builds on the headline workload (resident batch of 296 config-2 windows):
+"""A/B of library builds on the headline workload (resident batch of 264 config-2 windows):
    python scripts/ab_variants.py lib1.so[:KBA_GRAPH[:NAME=VALUE,...]] lib2.so ...  -- each in its own process (the library and its
    switches are read once), two repetitions of 5 steps; prints a digest of the results (equal digests = bit-identical solves)."""
 import json
@@ -17,7 +17,7 @@ if len(sys.argv) > 1 and sys.argv[1] == "--child":
     base = parallel.windows_for_rank(16, 0, 2)
     h = capi.Handle(0, stream=stream.cuda_stream)
     opt = capi.default_options()
-    batch = h.batch([base[i % 16] for i in range(296)])
+    batch = h.batch([base[i % 16] for i in range(264)])
     out = []
     for rep in range(2):
         for _ in range(3 if rep == 0 else 1):
@@ -34,7 +34,7 @@ if len(sys.argv) > 1 and sys.argv[1] == "--child":
     digest = hashlib.sha1(b"".join(r.kf_pose.tobytes() + r.lm_pos.tobytes() for r in res[:16])).hexdigest()[:12]
     print(json.dumps({"lib": os.path.basename(os.environ.get("KBA_LIB_PATH", "default")),
                       "env": {k: v for k, v in os.environ.items() if k.startswith("KBA_") and k != "KBA_LIB_PATH"},
-                      "ms_per_step": out, "windows_per_s": round(296 / (min(out) * 1e-3), 1),
+                      "ms_per_step": out, "windows_per_s": round(264 / (min(out) * 1e-3), 1),
                       "results_sha1": digest, "cost0": res[0].c.final_cost, "done": all(r.c.status == 0 for r in res)}))
     sys.exit(0)
 

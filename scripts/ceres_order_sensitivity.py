@@ -7,7 +7,7 @@ pins neither (it holds no golden vectors for the iterate sequence and Ceres cann
 solves BASELINE configs 1-3 with the oracle in both orders (oracle/kba_oracle.c, kbo_set_tolerance_order) and prints the
 largest differences: the error bar that "parity with the oracle" carries as a statement about Ceres.
 
-  python scripts/ceres_order_sensitivity.py [--seeds 4] > profiles/r02_ceres_order_sensitivity.md
+  python scripts/ceres_order_sensitivity.py [--seeds 4] > ceres_order_sensitivity.md
 """
 import argparse
 import ctypes as C

@@ -19,9 +19,9 @@ a = h.evaluate(win); b = h.evaluate(win, o32)
 print("eval: cost rel %.2e  |dr| %.2e  |djp|/max %.2e  |djl|/max %.2e" % (abs(a[3] - b[3]) / a[3], np.abs(a[0] - b[0]).max(),
       np.abs(a[1] - b[1]).max() / np.abs(a[1]).max(), np.abs(a[2] - b[2]).max() / np.abs(a[2]).max()))
 wins = [synth.make_window(2, seed=0xBA5E0000 + i) for i in range(16)]
-batch = h.batch([wins[i % 16] for i in range(148)])
+batch = h.batch([wins[i % 16] for i in range(132)])
 for opt, nm in ((capi.default_options(), "fp64"), (o32, "fp32-lin")):
     for _ in range(2): batch.solve(opt)
     t = time.time(); batch.solve(opt); batch.solve(opt); dtm = (time.time() - t) / 2
-    print(nm, "148-window batch: %.1f ms per solve -> %.0f windows/s" % (1e3 * dtm, 148 / dtm))
+    print(nm, "132-window batch: %.1f ms per solve -> %.0f windows/s" % (1e3 * dtm, 132 / dtm))
 batch.close(); h.close()

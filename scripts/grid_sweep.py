@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """Sweep of the CTAs per window of k_linearize / k_backsub_v (KBA_LIN_GRID / KBA_BS_GRID are read when a batch is created) on the
-headline workload, in one process: ms per step of a resident batch of 296 config-2 windows, 5 steps after 2 warm-ups each."""
+headline workload, in one process: ms per step of a resident batch of 264 config-2 windows, 5 steps after 2 warm-ups each."""
 import json
 import os
 import sys
@@ -13,7 +13,7 @@ from limo_b200 import capi, parallel  # noqa: E402
 torch.cuda.set_stream(torch.cuda.Stream())
 stream = torch.cuda.current_stream()
 base = parallel.windows_for_rank(16, 0, 2)
-wins = [base[i % 16] for i in range(296)]
+wins = [base[i % 16] for i in range(264)]
 h = capi.Handle(0, stream=stream.cuda_stream)
 opt = capi.default_options()
 configs = [(-1, -1), (64, 63), (128, 63), (160, 63), (80, 63), (112, 63), (98, 32), (98, 94), (98, 126), (-1, -1)]
@@ -31,6 +31,6 @@ for lin, bs in configs:
     e1.record(stream)
     torch.cuda.synchronize()
     ms = e0.elapsed_time(e1) / 5
-    print(json.dumps({"lin_grid": lin, "bs_grid": bs, "ms_per_step": round(ms, 2), "windows_per_s": round(296 / (ms * 1e-3), 1)}), flush=True)
+    print(json.dumps({"lin_grid": lin, "bs_grid": bs, "ms_per_step": round(ms, 2), "windows_per_s": round(264 / (ms * 1e-3), 1)}), flush=True)
     batch.close()
 h.close()

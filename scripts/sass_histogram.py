@@ -28,7 +28,7 @@ for line in out.splitlines():
         for label, pat in COLS:
             if re.match(pat, op):
                 kern[name][label] += 1
-print("# SASS opcode histogram of `%s` (`cuobjdump -sass`, sm_100a)\n" % so)
+print("# SASS opcode histogram of `%s` (`cuobjdump -sass`, sm_90a)\n" % so)
 print("| kernel | instructions | " + " | ".join(c for c, _ in COLS) + " |")
 print("|---|---|" + "---|" * len(COLS))
 for k in sorted(kern):

@@ -9,7 +9,7 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100)")
 
 
 def pytest_collection_modifyitems(config, items):
@@ -21,7 +21,7 @@ def pytest_collection_modifyitems(config, items):
         have_gpu = False
     if have_gpu:
         return
-    skip = pytest.mark.skip(reason="needs a CUDA device (B200 box)")
+    skip = pytest.mark.skip(reason="needs a CUDA device (an H100)")
     for item in items:
         if "gpu" in item.keywords:
             item.add_marker(skip)

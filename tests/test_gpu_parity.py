@@ -340,7 +340,7 @@ def test_config5_full_window_matches_oracle(handle, oracle):
 
 def test_sharded_solve_with_one_rank_equals_plain_solve(handle):
     """the landmark-sharded multi-GPU path (NCCL exchange points, window-wide trimming) run with a single rank must
-    reproduce the plain solve bit for bit; with 2 GPUs it is exercised by scripts/config5_sharded.py (profiles/)"""
+    reproduce the plain solve bit for bit; with 2 GPUs it is exercised by scripts/config5_sharded.py"""
     from limo_b200 import capi, parallel
     win = synth.make_window(5, n_kf=40, n_lm=3000, n_obs=45000)
     sub, j0, j1 = parallel.shard_window(win, 0, 1)
