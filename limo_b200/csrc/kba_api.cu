@@ -683,7 +683,6 @@ int kba_batch_create(kba_handle* h, int32_t n_windows, const kba_window* w, kba_
     // cost partials: one per CTA of k_linearize (8 warp tiles each, kba_linearize.cuh: lin_tile_bound) or per 256-observation tile of k_eval_obs
     bd.cost_parts = std::max((bd.max_obs + 255) / 256, (bd.max_obs / 16 + bd.max_lm / 32 + 4 + 7) / 8);
     { const char* le = std::getenv("KBA_LINEARIZE"); b->lc.lin_fused = !(le && std::atoi(le) == 0); }
-    { const char* le = std::getenv("KBA_LIN_BLOCKS"); if (le && std::atoi(le) == 3) b->lc.lin_blocks = 3; }
     { const char* le = std::getenv("KBA_LIN_GRID"); if (le) b->lc.lin_grid = std::max(-1, std::atoi(le)); }
     { const char* le = std::getenv("KBA_BS_GRID"); if (le) b->lc.bs_grid = std::max(-1, std::atoi(le)); }
     {  // tuning knobs of the residual/Jacobian kernel (see DESIGN.md)
@@ -967,7 +966,7 @@ int kba_batch_solve(kba_batch* b, const kba_options* opt) {
         key.reserve(sizeof(BatchDev) + sizeof(SolveParams) + 64);
         key_append(key, b->bd); key_append(key, sp); key_append(key, gmode); key_append(key, max_passes); key_append(key, s);
         key_append(key, lc.nr_cap_max); key_append(key, lc.max_rank); key_append(key, (int)lc.small_syrk); key_append(key, (int)lc.lin_fused);
-        key_append(key, lc.lin_blocks); key_append(key, lc.fused_slots); key_append(key, lc.xchg.user);
+        key_append(key, lc.fused_slots); key_append(key, lc.xchg.user);
         key_append(key, lc.lin_grid); key_append(key, lc.bs_grid);
         if (!(b->sg.exec && b->sg.key == key) && !build_solve_graph(b, sp, lc, gmode, max_passes, check_every, key)) gmode = 0;
     }

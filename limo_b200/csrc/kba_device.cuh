@@ -266,22 +266,26 @@ __device__ inline void cauchy(T b, T w, T s, T& half_rho, T& sqrt_rho1) {
     sqrt_rho1 = sqrt(w / sum);
 }
 
-// One observation: reprojection (2 rows) + optional lidar depth row, robustified.
-// pose: staged R(9)+t(3); cam: staged Rc(9)+tc(3)+f,cx,cy.  Jacobian rows: d/d(delta_rot) = -2 (m x a), d/d(delta_t) = m,
-// d/d(p) = m R, with m = (row of Pi) * Rc and a = R p   (reference cost_functors_ceres.hpp:91-155,193-212).
+// One observation: reprojection (2 rows) + optional lidar depth row, robustified, in the factored form of its Jacobian.
+// pose: staged R(9)+t(3); cam: staged Rc(9)+tc(3)+f,cx,cy.  With m = (rows of d Pi / d x_cam, robustified) * Rc (3x3, row-major)
+// and a = R p, the Jacobian rows are d/d(delta_rot) = -2 (m_i x a), d/d(delta_t) = m_i, d/d(p) = m_i R, i.e.
+//   J_pose = m [K | I] with K = -2 [a]x,   J_landmark = m R      (reference cost_functors_ceres.hpp:91-155,193-212),
+// so every Gauss-Newton product follows from M = m^T m, m^T r and a.  kM: also form m.
 // Returns false when |z_cam| < 0.01 (evaluation failure, cost_functors_ceres.hpp:78-83).
-template <typename T, bool kJac, bool kCost = true>
-__device__ inline bool eval_observation(const T* __restrict__ pose, const T* __restrict__ cam, const T p[3], T u, T v,
-                                        T d, T wt, T b_repr, T b_depth, T r[3], T jp[18], T jl[9], T& half_rho_sum,
-                                        T raw[2]) {
-    const T a0 = pose[0] * p[0] + pose[1] * p[1] + pose[2] * p[2];
-    const T a1 = pose[3] * p[0] + pose[4] * p[1] + pose[5] * p[2];
-    const T a2 = pose[6] * p[0] + pose[7] * p[1] + pose[8] * p[2];
-    const T x0 = a0 + pose[9], x1 = a1 + pose[10], x2 = a2 + pose[11];
+template <typename T, bool kM, bool kCost = true>
+__device__ __forceinline__ bool eval_factored(const T* __restrict__ pose, const T* __restrict__ cam, const T p[3], T u, T v,
+                                              T d, T wt, T b_repr, T b_depth, T r[3], T m[9], T a[3], T& half_rho_sum,
+                                              T raw[2]) {
+    a[0] = pose[0] * p[0] + pose[1] * p[1] + pose[2] * p[2];
+    a[1] = pose[3] * p[0] + pose[4] * p[1] + pose[5] * p[2];
+    a[2] = pose[6] * p[0] + pose[7] * p[1] + pose[8] * p[2];
+    const T x0 = a[0] + pose[9], x1 = a[1] + pose[10], x2 = a[2] + pose[11];
     const T c0 = cam[0] * x0 + cam[1] * x1 + cam[2] * x2 + cam[9];
     const T c1 = cam[3] * x0 + cam[4] * x1 + cam[5] * x2 + cam[10];
     const T c2 = cam[6] * x0 + cam[7] * x1 + cam[8] * x2 + cam[11];
     if (!(fabs(c2) >= T(0.01))) return false;
+    const bool has_d = d > T(0);
+    const T rd = has_d ? c2 - d : T(0);  // formed first: c2 and d need not outlive the divisions below
     const T f = cam[12], iz = T(1) / c2;
     const T xn = c0 * iz, yn = c1 * iz;
     const T ru = f * xn + cam[13] - u, rv = f * yn + cam[14] - v;
@@ -292,36 +296,61 @@ __device__ inline bool eval_observation(const T* __restrict__ pose, const T* __r
     raw[0] = sqrt(s);
     raw[1] = T(-1);
     r[0] = sq * ru; r[1] = sq * rv; r[2] = T(0);
-    T sqd = T(0), rd = T(0);
-    const bool has_d = d > T(0);
+    T sqd = T(0);
     if (has_d) {
-        rd = c2 - d;
         T hrd;
         cauchy<T, kCost>(b_depth, wt, rd * rd, hrd, sqd);
         half_rho_sum += hrd;
         raw[1] = fabs(rd);
         r[2] = sqd * rd;
     }
-    if (kJac) {
+    if (kM) {
         const T fz = f * iz * sq;  // robustified
         // m rows: (fz * Rc[0,:] - fz*xn * Rc[2,:]), (fz * Rc[1,:] - fz*yn * Rc[2,:]), sqd * Rc[2,:]
-        T m[3][3];
 #pragma unroll
         for (int c = 0; c < 3; ++c) {
-            m[0][c] = fz * (cam[c] - xn * cam[6 + c]);
-            m[1][c] = fz * (cam[3 + c] - yn * cam[6 + c]);
-            m[2][c] = sqd * cam[6 + c];
+            m[c] = fz * (cam[c] - xn * cam[6 + c]);
+            m[3 + c] = fz * (cam[3 + c] - yn * cam[6 + c]);
+            m[6 + c] = sqd * cam[6 + c];
         }
+    }
+    return true;
+}
+
+// index of entry (i, j) of a symmetric 3x3 matrix stored upper, row-major: 00 01 02 11 12 22
+__host__ __device__ constexpr int sym3(int i, int j) {
+    return i <= j ? 3 * i + j - i * (i + 1) / 2 : 3 * j + i - j * (j + 1) / 2;
+}
+
+// M = m^T m (sym3 layout) of a factored evaluation
+__device__ __forceinline__ void gram_factored(const double m[9], double M[6]) {
+    M[0] = m[0] * m[0] + m[3] * m[3] + m[6] * m[6];
+    M[1] = m[0] * m[1] + m[3] * m[4] + m[6] * m[7];
+    M[2] = m[0] * m[2] + m[3] * m[5] + m[6] * m[8];
+    M[3] = m[1] * m[1] + m[4] * m[4] + m[7] * m[7];
+    M[4] = m[1] * m[2] + m[4] * m[5] + m[7] * m[8];
+    M[5] = m[2] * m[2] + m[5] * m[5] + m[8] * m[8];
+}
+
+// eval_factored with the Jacobian rows spelled out: J_pose (3x6, row-major) and J_landmark (3x3)
+template <typename T, bool kJac, bool kCost = true>
+__device__ inline bool eval_observation(const T* __restrict__ pose, const T* __restrict__ cam, const T p[3], T u, T v,
+                                        T d, T wt, T b_repr, T b_depth, T r[3], T jp[18], T jl[9], T& half_rho_sum,
+                                        T raw[2]) {
+    T m[9], a[3];
+    if (!eval_factored<T, kJac, kCost>(pose, cam, p, u, v, d, wt, b_repr, b_depth, r, m, a, half_rho_sum, raw)) return false;
+    if (kJac) {
 #pragma unroll
         for (int i = 0; i < 3; ++i) {
-            jp[6 * i + 0] = T(-2) * (m[i][1] * a2 - m[i][2] * a1);
-            jp[6 * i + 1] = T(-2) * (m[i][2] * a0 - m[i][0] * a2);
-            jp[6 * i + 2] = T(-2) * (m[i][0] * a1 - m[i][1] * a0);
-            jp[6 * i + 3] = m[i][0];
-            jp[6 * i + 4] = m[i][1];
-            jp[6 * i + 5] = m[i][2];
+            const T* mi = m + 3 * i;
+            jp[6 * i + 0] = T(-2) * (mi[1] * a[2] - mi[2] * a[1]);
+            jp[6 * i + 1] = T(-2) * (mi[2] * a[0] - mi[0] * a[2]);
+            jp[6 * i + 2] = T(-2) * (mi[0] * a[1] - mi[1] * a[0]);
+            jp[6 * i + 3] = mi[0];
+            jp[6 * i + 4] = mi[1];
+            jp[6 * i + 5] = mi[2];
 #pragma unroll
-            for (int c = 0; c < 3; ++c) jl[3 * i + c] = m[i][0] * pose[c] + m[i][1] * pose[3 + c] + m[i][2] * pose[6 + c];
+            for (int c = 0; c < 3; ++c) jl[3 * i + c] = mi[0] * pose[c] + mi[1] * pose[3 + c] + mi[2] * pose[6 + c];
         }
     }
     return true;

@@ -458,7 +458,13 @@ __global__ void __launch_bounds__(256, 2) k_pose_hessian(BatchDev bd, SolveParam
     __shared__ double s_pose[kPoseStride];
     __shared__ double s_cam[kMaxCam * kCamStride];
     __shared__ double s_red[8][27];
+    // per thread: the sums of M = m^T m (6) and m^T r (3).  In registers, next to the 18 other sums and the prefetched loads,
+    // they would be spilled at 128 registers; every observation adds to them once
+    __shared__ double s_acc[9][256];
+    __shared__ long long s_ob;                              // the window's first observation, its landmark offset, the end of
+    __shared__ int s_lm_off, s_e1;                          // this keyframe's observations: re-read in every iteration (below)
     if (threadIdx.x == 0) {
+        s_ob = wd.obs_off; s_lm_off = wd.lm_off; s_e1 = bd.kf_ptr[wd.kf_off + w + k + 1];
         const double* p = bd.pose[st.cur] + 7 * (size_t)(wd.kf_off + k);
         double R[9];
         quat_to_rot<double>(p, R);
@@ -467,9 +473,12 @@ __global__ void __launch_bounds__(256, 2) k_pose_hessian(BatchDev bd, SolveParam
     }
     for (int i = threadIdx.x; i < wd.n_cam * kCamStride; i += blockDim.x) s_cam[i] = bd.cam[(size_t)wd.cam_off * kCamStride + i];
     __syncthreads();
-    double acc[27];
+    // outputs 0..14 (the rotation rows of B_k) and 21..23 (K^T h) in registers: acc[0..17]; 15..20 and 24..26 in s_acc
+    double acc[18];
 #pragma unroll
-    for (int q = 0; q < 27; ++q) acc[q] = 0.0;
+    for (int q = 0; q < 18; ++q) acc[q] = 0.0;
+#pragma unroll
+    for (int q = 0; q < 9; ++q) s_acc[q][threadIdx.x] = 0.0;
     const int* kp = bd.kf_ptr + wd.kf_off + w;
     const int e0 = kp[k], e1 = kp[k + 1];
     // two-deep software pipeline like k_eval_obs: the landmark index of iteration i+2 and the measurement / landmark
@@ -490,42 +499,64 @@ __global__ void __launch_bounds__(256, 2) k_pose_hessian(BatchDev bd, SolveParam
         wgt = bd.lm_weight[L]; act = bd.lm_active[L];
     }
 #pragma unroll 1
-    for (; e < e1; e += blockDim.x) {
+    for (; e < s_e1; e += blockDim.x) {
+        // the staged pose and the window's offsets are read from shared memory in every iteration: hoisted out of the loop,
+        // they would be spilled
+        asm volatile("" ::: "memory");
+        const size_t obs0 = (size_t)s_ob;
+        const int e_end = s_e1, lm0 = s_lm_off;
         const int en = e + blockDim.x;
         int Ln = -1, camn = 0;
         float un = 0.f, vn = 0.f, dn = 0.f;
         double q0 = 0, q1 = 0, q2 = 0, wn = 0;
         unsigned char actn = 0;
         if (idx_a >= 0) {
-            Ln = wd.lm_off + idx_a;
-            camn = bd.pm_cam[ob + en]; un = bd.pm_u[ob + en]; vn = bd.pm_v[ob + en]; dn = bd.pm_d[ob + en];
+            Ln = lm0 + idx_a;
+            camn = bd.pm_cam[obs0 + en]; un = bd.pm_u[obs0 + en]; vn = bd.pm_v[obs0 + en]; dn = bd.pm_d[obs0 + en];
             q0 = lm_buf[3 * (size_t)Ln]; q1 = lm_buf[3 * (size_t)Ln + 1]; q2 = lm_buf[3 * (size_t)Ln + 2];
             wn = bd.lm_weight[Ln]; actn = bd.lm_active[Ln];
         }
-        idx_a = (en + (int)blockDim.x < e1) ? bd.pm_lm[ob + en + blockDim.x] : -1;
+        idx_a = (en + (int)blockDim.x < e_end) ? bd.pm_lm[obs0 + en + blockDim.x] : -1;
         if (act) {
             const double p[3] = {p0, p1, p2};
-            double r[3], jp[18], jl[9], raw[2], hr;
-            if (eval_observation<double, true, false>(s_pose, s_cam + kCamStride * cam, p, (double)u, (double)v, (double)d,
-                                                      wgt, sp.reprojection_thres * sp.reprojection_thres,
-                                                      sp.depth_thres * sp.depth_thres, r, jp, jl, hr, raw)) {
-                int q = 0;
+            double r[3], m[9], a[3], raw[2], hr;
+            if (eval_factored<double, true, false>(s_pose, s_cam + kCamStride * cam, p, (double)u, (double)v, (double)d,
+                                                   wgt, sp.reprojection_thres * sp.reprojection_thres,
+                                                   sp.depth_thres * sp.depth_thres, r, m, a, hr, raw)) {
+                // J_p = m [K | I] with K = -2 [a]x (kba_device.cuh: eval_factored), so with M = m^T m and h = m^T r
+                //   J_p^T J_p = [K^T M K, K^T M; M K, M],  J_p^T r = [K^T h; h],  K^T v = 2 a x v,  (row_i(P) K) = 2 a x row_i(P)
+                double mm[6], h[3];
+                gram_factored(m, mm);
 #pragma unroll
-                for (int a = 0; a < 6; ++a)
+                for (int c = 0; c < 3; ++c) h[c] = m[c] * r[0] + m[3 + c] * r[1] + m[6 + c] * r[2];
 #pragma unroll
-                    for (int b = a; b < 6; ++b) {
-                        acc[q] += jp[a] * jp[b] + jp[6 + a] * jp[6 + b] + jp[12 + a] * jp[12 + b];
-                        ++q;
+                for (int i = 0; i < 3; ++i) {  // row i of P = K^T M: P[i][c] = 2 (a x M_c)_i
+                    const int i1 = (i + 1) % 3, i2 = (i + 2) % 3;
+                    double pr[3];
+#pragma unroll
+                    for (int c = 0; c < 3; ++c) pr[c] = 2.0 * (a[i1] * mm[sym3(i2, c)] - a[i2] * mm[sym3(i1, c)]);
+                    const int qd = 6 * i - i * (i - 1) / 2;  // packed index of (i, i) in the upper 6x6
+#pragma unroll
+                    for (int j = i; j < 3; ++j) {  // (K^T M K)[i][j] = 2 (a x row_i(P))_j
+                        const int j1 = (j + 1) % 3, j2 = (j + 2) % 3;
+                        acc[qd + j - i] += 2.0 * (a[j1] * pr[j2] - a[j2] * pr[j1]);
                     }
 #pragma unroll
-                for (int a = 0; a < 6; ++a) acc[21 + a] += jp[a] * r[0] + jp[6 + a] * r[1] + jp[12 + a] * r[2];
+                    for (int c = 0; c < 3; ++c) acc[qd + 3 - i + c] += pr[c];
+                    acc[15 + i] += 2.0 * (a[i1] * h[i2] - a[i2] * h[i1]);
+                }
+#pragma unroll
+                for (int q = 0; q < 6; ++q) s_acc[q][threadIdx.x] += mm[q];
+#pragma unroll
+                for (int c = 0; c < 3; ++c) s_acc[6 + c][threadIdx.x] += h[c];
             }  // an evaluation failure is flagged by k_eval_obs
         }
         L = Ln; cam = camn; u = un; v = vn; d = dn; p0 = q0; p1 = q1; p2 = q2; wgt = wn; act = actn;
     }
 #pragma unroll
     for (int q = 0; q < 27; ++q) {
-        const double v = warp_sum(acc[q]);
+        const double t = q < 15 ? acc[q] : q < 21 ? s_acc[q - 15][threadIdx.x] : q < 24 ? acc[q - 6] : s_acc[q - 18][threadIdx.x];
+        const double v = warp_sum(t);
         if ((threadIdx.x & 31) == 0) s_red[threadIdx.x >> 5][q] = v;
     }
     __syncthreads();
@@ -2294,17 +2325,16 @@ cudaError_t configure_kernels(int nr_cap_max) {
 // grid.x of a kernel whose CTAs stride over a window's units (k_linearize: 8 warp tiles, k_backsub_v: 16 landmarks).  Every pass is
 // launched for every window of the batch and the unit count is an upper bound, so with one CTA per unit most CTAs of a large batch
 // only find out that they have nothing to do; num/den of the units per window come from a sweep on the headline workload
-// (k_linearize: 1/5, k_backsub_v: 1/3; any grid gives bit-identical results).  Small batches keep one CTA per unit (latency: every
-// SM busy).
+// (k_linearize: 1/8, k_backsub_v: 1/3; any grid gives bit-identical results), as long as the strided grid still fills `waves` waves
+// of the kernel's resident CTAs (k_linearize: six of three CTAs per SM -- a batch of 64 config-2 windows strides; k_backsub_v: eight
+// of two): a CTA then runs several units back to back, and the last, partly filled wave stays a small share of the launch.  Smaller
+// batches keep one CTA per unit (latency: every SM busy).
 // `cfg`: -1 = this rule, 0 = one CTA per unit, > 0 = that many (KBA_LIN_GRID / KBA_BS_GRID).
-static int strided_grid(int cfg, int n_units, int num, int den, int n_win, int sm_count) {
+static int strided_grid(int cfg, int n_units, int num, int den, int n_win, int sm_count, int ctas_per_sm, int waves) {
     if (cfg == 0) return n_units;
     if (cfg > 0) return cfg < n_units ? cfg : n_units;
     const int g = (n_units * num + den - 1) / den;
-    return ((long long)g * n_win >= 8LL * 2 * sm_count && g >= 1) ? g : n_units;  // at least eight waves of 2 CTAs per SM remain
-                                                                                   // (a CTA now runs several units back to back:
-                                                                                   // keep the last, partly filled wave a small
-                                                                                   // share of the launch)
+    return ((long long)g * n_win >= (long long)waves * ctas_per_sm * sm_count && g >= 1) ? g : n_units;
 }
 
 void launch_reset(const BatchDev& bd, const LaunchCfg& lc, cudaStream_t s) {
@@ -2326,10 +2356,9 @@ int launch_pass(const BatchDev& bd, const SolveParams& sp, const LaunchCfg& lc, 
         LCHK("k_gp_eval");
         if (timed) cudaEventRecord(lc.ev_pool[(*lc.ev_used)++], s);
         const int n_units = (lin_tile_bound(bd.max_obs, bd.max_lm) + kLinWarps - 1) / kLinWarps;
-        const dim3 g_lin(strided_grid(lc.lin_grid, n_units, 1, 5, B, lc.sm_count), B);  // CTAs of a window stride over its units
-        if ((int)g_lin.x < n_units) k_linearize<2, true><<<g_lin, kLinThreads, 0, s>>>(bd, sp, n_units);
-        else if (lc.lin_blocks == 3) k_linearize<3, false><<<g_lin, kLinThreads, 0, s>>>(bd, sp, n_units);
-        else k_linearize<2, false><<<g_lin, kLinThreads, 0, s>>>(bd, sp, n_units);
+        const dim3 g_lin(strided_grid(lc.lin_grid, n_units, 1, 8, B, lc.sm_count, kLinMinBlocks, 6), B);  // CTAs of a window stride over its units
+        if ((int)g_lin.x < n_units) k_linearize<true><<<g_lin, kLinThreads, 0, s>>>(bd, sp, n_units);
+        else k_linearize<false><<<g_lin, kLinThreads, 0, s>>>(bd, sp, n_units);
         LCHK("k_linearize");
         if (timed) cudaEventRecord(lc.ev_pool[(*lc.ev_used)++], s);
         k_pose_hessian<<<dim3(bd.max_kf, B), 256, 0, s>>>(bd, sp); LCHK("k_pose_hessian");
@@ -2396,7 +2425,7 @@ int launch_pass(const BatchDev& bd, const SolveParams& sp, const LaunchCfg& lc, 
     }
     if (bd.fused) {
         const int n_units = (bd.max_lm + 15) / 16;
-        const int gx = strided_grid(lc.bs_grid, n_units, 1, 3, B, lc.sm_count);
+        const int gx = strided_grid(lc.bs_grid, n_units, 1, 3, B, lc.sm_count, 2, 8);
         if (gx < n_units) k_backsub_v<true><<<dim3(gx, B), 256, 0, s>>>(bd, n_units);
         else k_backsub_v<false><<<dim3(n_units, B), 256, 0, s>>>(bd, n_units);
     }

@@ -40,7 +40,6 @@ struct LaunchCfg {
     int max_rank = 0;         // largest observation rank in the batch (multi-camera rigs)
     bool small_syrk = false;  // every window has <= 184 reduced rows: register-resident Schur kernel
     bool lin_fused = true;    // fused path: evaluation + landmark blocks + V rows in one kernel (k_linearize); KBA_LINEARIZE=0: three kernels
-    int lin_blocks = 2;       // CTAs per SM k_linearize is compiled for (KBA_LIN_BLOCKS: 2 or 3)
     int lin_grid = -1;        // CTAs per window of k_linearize striding over its tile units (KBA_LIN_GRID; -1: by batch size, 0: one CTA per unit)
     int bs_grid = -1;         // the same for k_backsub_v (KBA_BS_GRID; 0: one CTA per 16 landmarks)
     int fused_slots = 6;      // fused Schur kernel instance: 6 accumulator blocks per warp (<= 176 rows) or 7 (<= 184)

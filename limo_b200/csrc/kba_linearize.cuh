@@ -6,9 +6,11 @@
 //
 // Round 1 / early round 2 ran these as three kernels around a materialised J_p (168 B per observation written, then read
 // twice).  Here nothing of the Jacobian reaches
-// memory: a lane evaluates its observation, keeps J_p (18 doubles) in registers and writes only what the Schur kernel and
-// the back substitution consume -- V_i (144 B per observation) and the landmark's L^-1, z, g, lambda.  A rejected LM
-// step (new radius, same x) simply runs the kernel again: re-evaluating is cheaper than re-reading.
+// memory: a lane evaluates its observation in factored form (kba_device.cuh: eval_factored), parks M = m^T m and a = R p in
+// the warp's shared-memory strip (9 doubles, where J_p took 18 registers: this is what fits three CTAs per SM), forms V from
+// them and writes only what the Schur kernel and the back substitution consume -- V_i (144 B per observation) and the
+// landmark's L^-1, z, g, lambda.  A rejected LM step (new radius, same x) simply runs the kernel again: re-evaluating is
+// cheaper than re-reading.
 //
 // Work split: lane = observation, WARP = tile.  k_solve_begin cuts the window's landmark-major observation stream into
 // tiles of whole, consecutive landmarks with at most 32 observations together (a landmark has at most 32 on this path:
@@ -19,6 +21,7 @@
 // damped block redundantly (it needs L^-1 anyway) -- no CTA barrier between evaluation and V.  A first version with CTA-wide tiles and one thread per landmark for the block sums stalled 256
 // threads on two barriers around a serial sqrt / divide chain.
 #pragma once
+#include <type_traits>
 #include "kba_device.cuh"
 
 namespace kba {
@@ -80,38 +83,59 @@ __device__ inline void build_lin_tiles(const BatchDev& bd, const WinDesc& wd, Wi
     }
 }
 
-// kMinBlocks: CTAs per SM the register allocation is sized for.  2: everything in registers (128 per thread); 3: 80 registers, the
-// Jacobian rows spill to local memory across the segment sums (KBA_LIN_BLOCKS)
+// Three CTAs (24 warps) per SM: at most 80 registers per thread.  The kernel is bound by instruction latency, so the occupancy
+// pays (DESIGN.md section 9).  The FP64 division / square-root slow paths are calls: whatever is live across the evaluation is
+// saved around them, so what a lane needs later is parked in shared memory (s_ma, s_ix) or re-read where it is used.  The
+// form without the unit loop compiles to 78 registers without spills; the striding form keeps 8 B of spill stores.
 // n_units = ceil(lin_tile_bound / kLinWarps): a unit is 8 consecutive warp tiles and owns cost slot `unit`.  The CTAs of a window
 // stride over the units (grid.x <= n_units; grid.x == n_units: one unit per CTA, the original launch): the tile bound is 1.7x the
 // tiles a window really has and every pass is launched for every window, so a smaller grid saves the CTAs that would only find out
 // that they have nothing to do and stages the poses once for several units.
-// kLoop = false: grid.x == n_units, compiled without the loop (no loop-carried registers: the loop form spills 120 bytes).
-template <int kMinBlocks, bool kLoop>
-__global__ void __launch_bounds__(kLinThreads, kMinBlocks) k_linearize(BatchDev bd, SolveParams sp, int n_units) {
+// kLoop = false: grid.x == n_units, compiled without the loop (no loop-carried registers: the loop form spills more).
+constexpr int kLinMinBlocks = 3;
+// k_linearize's static shared memory (the arrays declared in the kernel, below): it has to stay within the 48 KB a kernel may
+// declare statically; a larger kFusedMaxKf or kMaxCam means dynamic shared memory (or thinner per-lane strips)
+constexpr size_t kLinStaticSmem = sizeof(double) * (kFusedMaxKf * kPoseStride + kMaxCam * kCamStride + kLinWarps * 9 * 33 +
+                                                    kLinWarps * 32 * 9 + kLinWarps) +
+                                  sizeof(int) * (kLinWarps * 6 * 32 + kLinWarps) + sizeof(uint64_t);
+static_assert(kLinStaticSmem <= 48 * 1024, "k_linearize: static shared memory over 48 KB");
+template <bool kLoop>
+__global__ void __launch_bounds__(kLinThreads, kLinMinBlocks) k_linearize(BatchDev bd, SolveParams sp, int n_units) {
     const int w = blockIdx.y;
     WinState& st = bd.state[w];
     if (st.phase != PH_ITERATE) return;
     const WinDesc& wd = bd.desc[w];
-    const int n_tiles = st.n_lin_tiles;
-    const bool lin = st.need_linearize != 0;            // x changed
-    // The cost at x is evaluated at iteration zero of a solve only: afterwards x is an accepted candidate whose cost the
-    // candidate pass (k_eval_obs<false>) has already summed, and k_lm_update carries it over (as ceres does) -- two FP64
-    // logarithms per observation less in every later pass.
-    const bool want_cost = lin && st.iter0;
-    if (wd.landmarks_fixed && !want_cost) return;       // motion-only window past iteration zero: the landmark blocks are constant
+    // The flags of the pass are read from the window state where they are used (volatile): carried in registers across the
+    // evaluation, they would be spilled at 80 registers.  lin: x changed.  want_cost: the cost at x is evaluated at iteration
+    // zero of a solve only -- afterwards x is an accepted candidate whose cost the candidate pass (k_eval_obs<false>) has
+    // already summed, and k_lm_update carries it over (as ceres does): two FP64 logarithms per observation less in every
+    // later pass.
+    const volatile WinState& vst = st;
+    const auto n_tiles = [&] { return vst.n_lin_tiles; };
+    const auto lin = [&] { return vst.need_linearize != 0; };
+    const auto want_cost = [&] { return vst.need_linearize != 0 && vst.iter0 != 0; };
+    if (wd.landmarks_fixed && !want_cost()) return;     // motion-only window past iteration zero: the landmark blocks are constant
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     __shared__ __align__(16) double s_pose[kFusedMaxKf * kPoseStride];
     __shared__ __align__(16) double s_cam[kMaxCam * kCamStride];
     __shared__ __align__(8) uint64_t s_bar;
     __shared__ double s_cg[kLinWarps][9][33];           // per warp: block contributions of its 32 observations; then, in place at the
                                                         // landmark's first lane, their sums
+    __shared__ double s_ma[kLinWarps][32][9];           // per lane: M (sym3 layout) and a of its observation, written as they are
+                                                        // formed and read back for V: in registers they would be live across the
+                                                        // FP64 division calls, the segment sums and the Cholesky (9 doubles per
+                                                        // lane, odd: conflict-free)
+    __shared__ int s_ix[kLinWarps][6][32];              // per lane: keyframe, pose row, first observation of the landmark (batch
+                                                        // index), its observation count, landmark, flags (1: lane holds an
+                                                        // observation, 2: of an active landmark; bits 2-6: the landmark's first
+                                                        // lane; 128: evaluated) -- parked across the evaluation, whose FP64
+                                                        // division calls would spill them
     __shared__ double s_red[kLinWarps];
     __shared__ int s_cnt[kLinWarps];
-    bool staged = false;
     for (int unit = blockIdx.x; unit < n_units; unit += gridDim.x) {
-    if (unit * kLinWarps >= n_tiles) {                  // no tile in this unit: its cost slot still has to read zero
-        if (tid == 0 && want_cost) bd.cost_part_x[(size_t)w * bd.cost_parts + unit] = 0.0;
+    asm volatile("" ::: "memory");  // the window's values are re-read per unit: hoisted out of the loop, they would be spilled
+    if (unit * kLinWarps >= n_tiles()) {                  // no tile in this unit: its cost slot still has to read zero
+        if (tid == 0 && want_cost()) bd.cost_part_x[(size_t)w * bd.cost_parts + unit] = 0.0;
         if constexpr (!kLoop) return;
         continue;
     }
@@ -120,7 +144,7 @@ __global__ void __launch_bounds__(kLinThreads, kMinBlocks) k_linearize(BatchDev 
     // my observation: the loads are issued before the staging barrier so that their latency overlaps the bulk copy
     const int t = unit * kLinWarps + warp;
     int2 tile = make_int2(0, 0);
-    if (t < n_tiles) tile = bd.lin_tile[lin_tile_offset(wd, w) + t];
+    if (t < n_tiles()) tile = bd.lin_tile[lin_tile_offset(wd, w) + t];
     const bool have = lane < tile.y;
     const int o = tile.x + lane;
     int j = 0, kf = 0, cam = 0, row0 = -1, p0 = 0, p1 = 0;
@@ -138,24 +162,44 @@ __global__ void __launch_bounds__(kLinThreads, kMinBlocks) k_linearize(BatchDev 
         p[0] = lmp[0]; p[1] = lmp[1]; p[2] = lmp[2];
         wgt = bd.lm_weight[wd.lm_off + j];
     }
-    const int L = wd.lm_off + j;
-    if (!staged) {  // (uniform per CTA) once: the poses do not change within a pass
-        stage_window_bulk(wd, bd.rt[st.cur], bd.cam, s_pose, s_cam, &s_bar);
-        staged = true;
-    }
+    int (*six)[32] = s_ix[warp];
+    // once, in the CTA's first unit (the poses do not change within a pass): units are taken in increasing order, so when the
+    // first one holds no tile, none does
+    if (unit == (int)blockIdx.x) stage_window_bulk(wd, bd.rt[st.cur], bd.cam, s_pose, s_cam, &s_bar);
+    six[0][lane] = kf; six[1][lane] = row0; six[2][lane] = wd.obs_off + p0; six[3][lane] = p1 - p0; six[4][lane] = wd.lm_off + j;
+    six[5][lane] = have ? 1 | (act ? 2 : 0) | ((p0 - tile.x) << 2) : 0;
     // ---- evaluate my observation; contributions to its landmark block
-    double jp[18];
-    bool ok = true;
+    double* sma = s_ma[warp][lane];
+    bool ok = false;                                    // my observation is active and evaluated
     double hr = 0.0;
     double cg[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0};
     if (act) {
-        double r[3], jl[9], raw[2];
-        const double* ps = s_pose + kPoseStride * kf;
-        const double* cs_ = s_cam + kCamStride * cam;
-        const double br = sp.reprojection_thres * sp.reprojection_thres, bdp = sp.depth_thres * sp.depth_thres;
-        if (want_cost) ok = eval_observation<double, true, true>(ps, cs_, p, (double)mu, (double)mv, (double)md, wgt, br, bdp, r, jp, jl, hr, raw);
-        else ok = eval_observation<double, true, false>(ps, cs_, p, (double)mu, (double)mv, (double)md, wgt, br, bdp, r, jp, jl, hr, raw);
-        if (ok) {
+        // the contributions are formed inside each of the two instantiations (with / without the cost terms): merged after
+        // them, m and r would be live across the join and spilled
+        const auto evaluate = [&](auto with_cost) {
+            double r[3], m[9], raw[2];
+            const double br = sp.reprojection_thres * sp.reprojection_thres, bdp = sp.depth_thres * sp.depth_thres;
+            ok = eval_factored<double, true, decltype(with_cost)::value>(s_pose + kPoseStride * kf, s_cam + kCamStride * cam, p,
+                                                                          (double)mu, (double)mv, (double)md, wgt, br, bdp, r, m,
+                                                                          sma + 6, hr, raw);
+            if (!ok) return;
+            {   // the flag word's address from a fresh read of the thread index: kept from before the evaluation, it would be spilled
+                unsigned t;
+                asm volatile("mov.u32 %0, %%tid.x;" : "=r"(t));
+                s_ix[t >> 5][5][t & 31] |= 128;
+            }
+            gram_factored(m, sma);
+            // C and g from J_l = m R, as the three-kernel path forms them.  R^T M R rounds no worse, but a landmark seen with
+            // almost no parallax (condition ~1e10) amplifies any change of rounding: in the parity tests' evaluation-failure
+            // window one then ended 17 cm from the oracle's solution (this form: 5 cm).  The keyframe is re-read from the
+            // strip: kept in a register, it would be spilled across the evaluation
+            const double* R = s_pose + kPoseStride * reinterpret_cast<volatile int*>(six[0])[lane];
+            double jl[9];
+#pragma unroll
+            for (int i = 0; i < 3; ++i) {
+#pragma unroll
+                for (int c = 0; c < 3; ++c) jl[3 * i + c] = m[3 * i] * R[c] + m[3 * i + 1] * R[3 + c] + m[3 * i + 2] * R[6 + c];
+            }
             cg[0] = jl[0] * jl[0] + jl[3] * jl[3] + jl[6] * jl[6];
             cg[1] = jl[0] * jl[1] + jl[3] * jl[4] + jl[6] * jl[7];
             cg[2] = jl[0] * jl[2] + jl[3] * jl[5] + jl[6] * jl[8];
@@ -164,14 +208,17 @@ __global__ void __launch_bounds__(kLinThreads, kMinBlocks) k_linearize(BatchDev 
             cg[5] = jl[2] * jl[2] + jl[5] * jl[5] + jl[8] * jl[8];
 #pragma unroll
             for (int c = 0; c < 3; ++c) cg[6 + c] = jl[c] * r[0] + jl[3 + c] * r[1] + jl[6 + c] * r[2];
-        } else {
+        };
+        if (want_cost()) evaluate(std::true_type{});
+        else evaluate(std::false_type{});
+        if (!ok) {
             hr = 0.0;
-            if (lin) st.eval_failed = 1;  // benign race
+            if (lin()) st.eval_failed = 1;  // benign race
         }
     }
     {   // cost partial of the CTA (fixed-shape reduction; the barrier is at the very end) and the observation count of the roofline report
         const double cs = warp_sum(hr);
-        const int dn = __reduce_add_sync(0xffffffffu, (act && ok) ? 1 : 0);
+        const int dn = __reduce_add_sync(0xffffffffu, ok ? 1 : 0);
         if (lane == 0) { s_red[warp] = cs; s_cnt[warp] = dn; }
     }
     if (!wd.landmarks_fixed) {  // (uniform per window) motion-only: the landmark blocks are constant, only the cost at x was needed
@@ -179,19 +226,21 @@ __global__ void __launch_bounds__(kLinThreads, kMinBlocks) k_linearize(BatchDev 
         double (*sw)[33] = s_cg[warp];  // row stride 33: the lanes summing different components below hit different banks
 #pragma unroll
         for (int q = 0; q < 9; ++q) sw[q][lane] = cg[q];
-        const int seg0 = p0 - tile.x;
-        const int klen = p1 - p0;
+        __syncwarp();
+        const int L = six[4][lane];
+        const bool in_tile = six[5][lane] & 1, active = six[5][lane] & 2;  // have, act of the loads above
+        const int seg0 = (six[5][lane] >> 2) & 31;
+        const int klen = six[3][lane];
         // the stored Jacobi scaling of my landmark (past iteration zero): requested here, consumed after the segment sums
         double tt_ld[3] = {0.0, 0.0, 0.0};
-        if (act && !st.iter0) {
+        if (active && !st.iter0) {
 #pragma unroll
             for (int e = 0; e < 3; ++e) tt_ld[e] = bd.lm_scale[3 * (size_t)L + e];
         }
-        __syncwarp();
         // lane seg0 + q of a landmark sums component q of its block in lane order (landmarks with fewer than 9 observations: several
         // components per lane) and leaves the sum at [q][first lane of the landmark] -- in place: component q of a landmark is read
         // and written by this one lane only
-        if (have) {
+        if (in_tile) {
             for (int q = lane - seg0; q < 9; q += klen) {
                 double sacc = 0.0;
                 for (int l = seg0; l < seg0 + klen; ++l) sacc += sw[q][l];
@@ -199,7 +248,7 @@ __global__ void __launch_bounds__(kLinThreads, kMinBlocks) k_linearize(BatchDev 
             }
         }
         __syncwarp();
-        if (act) {
+        if (active) {
             double c[6], g[3];
 #pragma unroll
             for (int q = 0; q < 6; ++q) c[q] = sw[q][seg0];
@@ -266,13 +315,15 @@ __global__ void __launch_bounds__(kLinThreads, kMinBlocks) k_linearize(BatchDev 
                         }
                     }
                 }
-                // ---- V_i = (J_p^T J_l) L^-T, J_l = M R(keyframe) with M = J_p[:, 3:6]; W = J_l L^-T first (short chains)
-                if (ok && row0 >= 0) {
-                    const double* R = s_pose + kPoseStride * kf;
+                // ---- V_i = (J_p^T J_l) L^-T = [K^T ; I] W with W = M R L^-T: the translation rows are W, the rotation rows
+                //      K^T W_c = 2 a x W_c (K = -2 [a]x)
+                if ((six[5][lane] & 128) && six[1][lane] >= 0) {
+                    const double* R = s_pose + kPoseStride * six[0][lane];
+                    const int g0 = six[2][lane];
                     double wm[9];
 #pragma unroll
                     for (int r = 0; r < 3; ++r) {
-                        const double m0 = jp[6 * r + 3], m1 = jp[6 * r + 4], m2 = jp[6 * r + 5];
+                        const double m0 = sma[sym3(r, 0)], m1 = sma[sym3(r, 1)], m2 = sma[sym3(r, 2)];
                         const double l0 = m0 * R[0] + m1 * R[3] + m2 * R[6], l1 = m0 * R[1] + m1 * R[4] + m2 * R[7], l2 = m0 * R[2] + m1 * R[5] + m2 * R[8];
                         wm[3 * r + 0] = l0 * i00;
                         wm[3 * r + 1] = l0 * i10 + l1 * i11;
@@ -280,13 +331,12 @@ __global__ void __launch_bounds__(kLinThreads, kMinBlocks) k_linearize(BatchDev 
                     }
 #pragma unroll
                     for (int cc = 0; cc < 3; ++cc) {  // 48 contiguous bytes per column; consecutive lanes = consecutive observations of the landmark
-                        double2* out = reinterpret_cast<double2*>(bd.vobs + vobs_index(base, p0, p1, o, cc));
-#pragma unroll
-                        for (int h = 0; h < 3; ++h) {
-                            const int r0 = 2 * h, r1 = 2 * h + 1;  // V[r][c] = sum_k J_p[k][r] W[k][c]
-                            out[h] = make_double2(jp[r0] * wm[cc] + jp[6 + r0] * wm[3 + cc] + jp[12 + r0] * wm[6 + cc],
-                                                  jp[r1] * wm[cc] + jp[6 + r1] * wm[3 + cc] + jp[12 + r1] * wm[6 + cc]);
-                        }
+                        double2* out = reinterpret_cast<double2*>(bd.vobs + vobs_index(0, g0, g0 + klen, g0 + lane - seg0, cc));
+                        const double w0 = wm[cc], w1 = wm[3 + cc], w2 = wm[6 + cc];
+                        const double a0 = sma[6], a1 = sma[7], a2 = sma[8];
+                        out[0] = make_double2(2.0 * (a1 * w2 - a2 * w1), 2.0 * (a2 * w0 - a0 * w2));
+                        out[1] = make_double2(2.0 * (a0 * w1 - a1 * w0), w0);
+                        out[2] = make_double2(w1, w2);
                     }
                 }
             }
@@ -297,7 +347,7 @@ __global__ void __launch_bounds__(kLinThreads, kMinBlocks) k_linearize(BatchDev 
         double s = 0.0;
         int cnt = 0;
         for (int q = 0; q < kLinWarps; ++q) { s += s_red[q]; cnt += s_cnt[q]; }
-        if (want_cost) bd.cost_part_x[(size_t)w * bd.cost_parts + unit] = s;
+        if (want_cost()) bd.cost_part_x[(size_t)w * bd.cost_parts + unit] = s;
         if (cnt) atomicAdd(bd.jac_obs, (unsigned long long)cnt);
     }
     if constexpr (!kLoop) break;
