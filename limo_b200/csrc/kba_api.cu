@@ -725,6 +725,7 @@ int kba_batch_create(kba_handle* h, int32_t n_windows, const kba_window* w, kba_
         bad |= b->dev_alloc(&b->raw.lm_inv, lm);
     }
     bad |= b->dev_alloc(&bd.grp_t0, groups); bad |= b->dev_alloc(&bd.grp_t1, groups); bad |= b->dev_alloc(&bd.grp_rs, groups);
+    bad |= b->dev_alloc(&bd.grp_tiles, groups);
     bad |= b->dev_alloc(&bd.lin_tile, (size_t)(obs / 16) + (size_t)(lm / 32) + 4 * (size_t)n_windows + 4);
 #ifdef KBA_PROF
     bad |= b->dev_alloc(&bd.prof, 16);

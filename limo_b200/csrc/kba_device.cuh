@@ -182,13 +182,15 @@ struct BatchDev {
     int tot_chunks;
     // fused small-window path (k_schur_fused): J_l is not materialised (J_l = translation columns of J_p times R), the V
     // panels exist only in shared memory; per 8-landmark group the keyframe range (host, static) and, per solve, the
-    // 8-row tile range of the reduced system it touches and the row stride of its shared-memory panel
+    // 8-row tile range of the reduced system it touches and the rows of its shared-memory panel
     int fused;                // 1: every window of the batch has <= 184 reduced rows -> fused path, jl / vpanel unused
     int* grp_k0;              // [tot_groups]
     int* grp_k1;
-    int* grp_t0;              // [tot_groups]
+    int* grp_t0;              // [tot_groups] tile range [t0, t1) aligned to 16-row blocks
     int* grp_t1;
-    int* grp_rs;              // [tot_groups] == 4 mod 16, 0: no free keyframe rows
+    int* grp_tiles;           // [tot_groups] t0 | t1 << 8 | e0 << 16 | e1 << 24: [e0, e1) = the exact tile range inside
+                              //   [t0, t1), right-hand-side tile included (what the consumer warps read, in one register)
+    int* grp_rs;              // [tot_groups] panel rows (multiple of 8), 0: no free keyframe rows
     double* vobs;             // [18 * tot_obs] V_i = (J_p^T J_l) L^-T of every observation, unpadded.  Per landmark with
                               //   observations [p0, p1), n = p1 - p0: column c of observation i at 18 (obs_off + p0) + 6 n c + 6 i
                               //   (6 rows each), so a whole panel column of the landmark is ONE contiguous run

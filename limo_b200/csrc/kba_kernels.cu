@@ -156,7 +156,7 @@ __global__ void __launch_bounds__(kBeginThreads) k_solve_begin(BatchDev bd, Solv
         }
     }
     if (bd.fused) build_lin_tiles(bd, wd, st, w, s_tile_chunk);  // warp tiles of k_linearize over the active landmarks
-    // fused path: 8-row tile range and shared-memory row stride (== 4 mod 16) of each 8-landmark group
+    // fused path: 16-row-aligned and exact 8-row tile ranges and shared-memory panel rows of each 8-landmark group
     if (bd.fused) {
         const int trhs = st.n_f >> 3;
         for (int c = threadIdx.x; c < wd.n_groups; c += blockDim.x) {
@@ -172,8 +172,17 @@ __global__ void __launch_bounds__(kBeginThreads) k_solve_begin(BatchDev bd, Solv
             const int t0 = (r1 < 0) ? 0 : (r0 / 16) * 2, t1 = (r1 < 0) ? 0 : ((r1 + 15) / 16) * 2;
             int rows = 0;  // rows of the group's shared-memory panel (the column stride is the constant kFMaxRs)
             if (t1 > t0) rows = 8 * (t1 - t0) + ((trhs >= t0 && trhs < t1) ? 0 : 8);
+            // tiles of [t0, t1) outside [e0, e1) are zero in the panel: the kernel skips the products against them.  The
+            // right-hand-side row, when it lies inside [t0, t1), is part of the panel too.
+            int e0 = 0, e1 = 0;
+            if (t1 > t0) {
+                e0 = r0 / 8;
+                e1 = (r1 + 7) / 8;
+                if (trhs >= t0 && trhs < t1) e1 = max(e1, trhs + 1);
+            }
             bd.grp_t0[wd.grp_off + c] = t0;
             bd.grp_t1[wd.grp_off + c] = t1;
+            bd.grp_tiles[wd.grp_off + c] = t0 | t1 << 8 | e0 << 16 | e1 << 24;
             bd.grp_rs[wd.grp_off + c] = rows;
         }
     }

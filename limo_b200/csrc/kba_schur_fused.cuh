@@ -13,16 +13,18 @@
 //                          instead of bulk copies.  Landmarks whose rows are not one run fall back to nine 16-byte
 //                          cp.async per observation; windows with ground-plane rows or several cameras per keyframe (rows
 //                          that ADD onto others) take a synchronous variant of the same loop.
-//   consumers (12 warps) : Sred += V V^T on the FP64 tensor cores (mma.sync m8n8k4).  The whole lower triangle lives in
-//                          the consumers' registers as 16x16 blocks (2x2 tiles: one shared-memory load per DMMA); only
-//                          the tile pairs inside the group's row range are multiplied.
+//   consumers (12 warps) : Sred += V V^T on the FP64 tensor cores (mma.sync m16n8k8 / m16n8k4: on sm_90 they issue at twice
+//                          the FLOP rate of m8n8k4, scripts/dmma_rate.cu).  The whole lower triangle lives in the consumers'
+//                          registers as 16x16 blocks, each two 16x8 halves (four shared-memory loads per k-step of both
+//                          halves, two for a diagonal block); only the blocks inside the group's 16-row-aligned range are
+//                          multiplied, and a half whose 8 columns lie outside the group's exact 8-row tile range is skipped.
 //   ring                 : 6 panel stages with full / empty mbarriers, so warps drift up to five groups apart and the
 //                          per-group imbalance of the static block -> warp map (scripts/syrk_map_search.py) averages out.
 //
 // Replaces k_obs_v + k_gp_panel + k_schur_syrk_tma of round 1 (zero-padded panels written and re-read every pass; now 144 B
 // per observation).  Forming V inside the producer warps was tried too: with only four warps the ~250 dependent instructions
-// per observation are latency-bound next to the tensor work.  Included by kba_kernels.cu after dmma(), the mbarrier helpers
-// and gp_row().
+// per observation are latency-bound next to the tensor work.  Included by kba_kernels.cu after the mbarrier helpers and
+// gp_row().
 #pragma once
 
 namespace kba {
@@ -36,12 +38,14 @@ constexpr int kFObs = 128;                       // observations staged per grou
 constexpr int kFConsumerWarps = 12;
 constexpr int kFMaxKf = 32;
 
-// 16x16 block (linear index bi (bi + 1) / 2 + bj of the 12-row block triangle) owned by each consumer warp: slot 0 is
-// the warp's block of row 11 (only systems of more than 176 rows have one), slots 1..6 blocks of rows <= 10.
-__constant__ signed char kSyrkMap12[12][7] = {
-    {72, 7, 22, 33, 36, 48, 65}, {67, 10, 12, 19, 40, 53, -1}, {73, 1, 13, 17, 42, 50, -1}, {77, 8, 21, 26, 39, 54, -1},
-    {75, 3, 18, 34, 49, 57, -1}, {69, 6, 23, 41, 58, 62, -1},  {66, 11, 27, 32, 38, 64, -1}, {74, 9, 20, 30, 37, 52, 55},
-    {68, 0, 14, 16, 31, 44, 51}, {76, 2, 24, 29, 43, 45, 60},  {71, 5, 25, 28, 46, 56, 63},  {70, 4, 15, 35, 47, 59, 61}};
+// 16x16 block (16 bi + bj: block row bi, block column bj <= bi of the 12-row block triangle; 0xff: none) owned by each
+// consumer warp: slot 0 is the warp's block of row 11 (only systems of more than 176 rows have one), slots 1..6 blocks of
+// rows <= 10.
+__constant__ unsigned char kSyrkMap12[12][7] = {
+    {0xb6, 0x31, 0x61, 0x75, 0x80, 0x93, 0xaa}, {0xb1, 0x40, 0x42, 0x54, 0x84, 0x98, 0xff}, {0xb7, 0x10, 0x43, 0x52, 0x86, 0x95, 0xff},
+    {0xbb, 0x32, 0x60, 0x65, 0x83, 0x99, 0xff}, {0xb9, 0x20, 0x53, 0x76, 0x94, 0xa2, 0xff}, {0xb3, 0x30, 0x62, 0x85, 0xa3, 0xa7, 0xff},
+    {0xb0, 0x41, 0x66, 0x74, 0x82, 0xa9, 0xff}, {0xb8, 0x33, 0x55, 0x72, 0x81, 0x97, 0xa0}, {0xb2, 0x00, 0x44, 0x51, 0x73, 0x88, 0x96},
+    {0xba, 0x11, 0x63, 0x71, 0x87, 0x90, 0xa5}, {0xb5, 0x22, 0x64, 0x70, 0x91, 0xa1, 0xa8}, {0xb4, 0x21, 0x50, 0x77, 0x92, 0xa4, 0xa6}};
 
 __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
     asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
@@ -99,6 +103,62 @@ __device__ __forceinline__ void schur_split(int n_groups, int p_split, int& per,
     used = max(1, min(p_split, (n_groups + per - 1) / per));
 }
 
+// D += A B on Hopper's 16x8 FP64 shapes (PTX ISA, mma.m16n8k4 / m16n8k8 .f64 fragments): a0 / a1 = rows fr / fr + 8 of A
+// in column fc, a2 / a3 the same in column fc + 4; b0 / b1 = rows fc / fc + 4 of B in column fr; c[0..1] = D[fr][2 fc + 0..1],
+// c[2..3] = D[fr + 8][2 fc + 0..1].  Both issue at twice the FLOP rate of m8n8k4 on sm_90 (scripts/dmma_rate.cu).
+__device__ __forceinline__ void dmma16k4(double (&c)[4], double a0, double a1, double b0) {
+    asm volatile("mma.sync.aligned.m16n8k4.row.col.f64.f64.f64.f64 {%0,%1,%2,%3}, {%4,%5}, {%6}, {%0,%1,%2,%3};\n"
+                 : "+d"(c[0]), "+d"(c[1]), "+d"(c[2]), "+d"(c[3])
+                 : "d"(a0), "d"(a1), "d"(b0));
+}
+__device__ __forceinline__ void dmma16k8(double (&c)[4], double a0, double a1, double a2, double a3, double b0, double b1) {
+    asm volatile("mma.sync.aligned.m16n8k8.row.col.f64.f64.f64.f64 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};\n"
+                 : "+d"(c[0]), "+d"(c[1]), "+d"(c[2]), "+d"(c[3])
+                 : "d"(a0), "d"(a1), "d"(a2), "d"(a3), "d"(b0), "d"(b1));
+}
+
+// One 16x16 accumulator block += (16 rows at pa) (16 rows at pb)^T over the 24 columns of a group panel (lane offset included,
+// column stride kFMaxRs).  c[h] is the 16x8 half of columns pb + 8 h; kL / kR multiply the left / right half.  kRhs: pa is
+// the 8-row right-hand-side tile, which lands in the upper (odd == false) or lower 8 rows of the block; the other 8 rows
+// get exact zero products.  kK8: three m16n8k8 per half instead of six m16n8k4 (same loads, half the dependent MMAs of an
+// accumulator); the seven-slot kernel keeps m16n8k4, its 112 accumulator registers leave no room for the wider fragments.
+template <bool kL, bool kR, bool kRhs, bool kK8>
+__device__ __forceinline__ void syrk_block(double (&c)[2][4], const double* pa, const double* pb, bool odd) {
+    if (kK8 && !kRhs) {
+#pragma unroll
+        for (int kk = 0; kk < kGC; kk += 8) {
+            const double* qa = pa + kk * kFMaxRs;
+            const double* qb = pb + kk * kFMaxRs;
+            const double a0 = qa[0], a1 = qa[8], a2 = qa[4 * kFMaxRs], a3 = qa[4 * kFMaxRs + 8];
+            if (kL) dmma16k8(c[0], a0, a1, a2, a3, qb[0], qb[4 * kFMaxRs]);
+            if (kR) dmma16k8(c[1], a0, a1, a2, a3, qb[8], qb[4 * kFMaxRs + 8]);
+        }
+    } else {
+#pragma unroll
+        for (int kk = 0; kk < kGC; kk += 4) {
+            double a0, a1;
+            if (kRhs) {
+                const double a = pa[kk * kFMaxRs];
+                a0 = odd ? 0.0 : a;
+                a1 = odd ? a : 0.0;
+            } else {
+                a0 = pa[kk * kFMaxRs];
+                a1 = pa[kk * kFMaxRs + 8];
+            }
+            if (kL) dmma16k4(c[0], a0, a1, pb[kk * kFMaxRs]);
+            if (kR) dmma16k4(c[1], a0, a1, pb[kk * kFMaxRs + 8]);
+        }
+    }
+}
+
+// the halves of a block that meet the group's exact rows: both, left only or right only
+template <bool kRhs, bool kK8>
+__device__ __forceinline__ void syrk_halves(double (&c)[2][4], const double* pa, const double* pb, bool odd, bool lo, bool hi) {
+    if (lo && hi) syrk_block<true, true, kRhs, kK8>(c, pa, pb, odd);
+    else if (lo) syrk_block<true, false, kRhs, kK8>(c, pa, pb, odd);
+    else if (hi) syrk_block<false, true, kRhs, kK8>(c, pa, pb, odd);
+}
+
 template <int kSlots>
 __global__ void __launch_bounds__(512, 1) k_schur_fused(BatchDev bd) {
     const int w = blockIdx.y;
@@ -119,6 +179,7 @@ __global__ void __launch_bounds__(512, 1) k_schur_fused(BatchDev bd) {
     const int* grs = bd.grp_rs + wd.grp_off;
     const int* gt0 = bd.grp_t0 + wd.grp_off;
     const int* gt1 = bd.grp_t1 + wd.grp_off;
+    const int* gtl = bd.grp_tiles + wd.grp_off;
     if (tid == 0) {
         for (int i = 0; i < kFStages; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], kFConsumerWarps); }
         asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // the barriers are armed by bulk copies (async proxy) too
@@ -128,7 +189,7 @@ __global__ void __launch_bounds__(512, 1) k_schur_fused(BatchDev bd) {
 
     if (warp >= kFConsumerWarps) {
         // =============================== producers ===============================
-        if (kSlots == 7) reg_dec<56>(); else reg_dec<104>();
+        reg_dec<56>();  // 4 x 56 + 12 x 152 = 16 x 128: the consumers' 16x8 accumulators need 152 without spills
 
         // Each producer warp assembles WHOLE groups on its own (group sequence number gi -> warp gi % 4), so four panels are
         // being built at any time and no CTA-level barrier is needed.  Lane roles inside a warp: lanes 0..23 own one panel
@@ -276,111 +337,67 @@ __global__ void __launch_bounds__(512, 1) k_schur_fused(BatchDev bd) {
     }
 
     // =============================== consumers ===============================
-    if (kSlots == 7) reg_inc<152>(); else reg_inc<136>();
+    reg_inc<152>();
     const int fr = lane >> 2, fc = lane & 3;
     const int nb2 = (nt + 1) >> 1, brhs = trhs >> 1;
-    double acc[kSlots][4][2];
-    int my_bi[kSlots], my_bj[kSlots];
+    double acc[kSlots][2][4];  // [slot][column half][rows fr: 0..1, rows fr + 8: 2..3]
+    const unsigned char* my_b = kSyrkMap12[warp] + (7 - kSlots);  // read in the group loop: the registers go to the accumulators
 #pragma unroll
-    for (int s = 0; s < kSlots; ++s) {
+    for (int s = 0; s < kSlots; ++s)
 #pragma unroll
-        for (int q = 0; q < 4; ++q) acc[s][q][0] = acc[s][q][1] = 0.0;
-        const int t = kSyrkMap12[warp][s + (7 - kSlots)];
-        int bi = 1 << 20, bj = 0;
-        if (t >= 0) {
-            bi = (int)((sqrtf(8.0f * (float)t + 1.0f) - 1.0f) * 0.5f);
-            while ((bi + 1) * (bi + 2) / 2 <= t) ++bi;
-            while (bi * (bi + 1) / 2 > t) --bi;
-            bj = t - bi * (bi + 1) / 2;
-        }
-        if (bi >= nb2) bi = 1 << 20;  // beyond this window's triangle
-        my_bi[s] = bi; my_bj[s] = bj;
-    }
+        for (int q = 0; q < 4; ++q) acc[s][0][q] = acc[s][1][q] = 0.0;
     {
-        // Group ranges are aligned to 16-row blocks (k_solve_begin), so a block inside the range has both its tiles and the
-        // only partial block is the one holding the right-hand-side tile when it lies outside the range: three straight-line
-        // variants, no predicate inside a tensor-core loop.  The column stride is the constant kFMaxRs, so every fragment
-        // load of a block is base + immediate.
+        // Group ranges are aligned to 16-row blocks (k_solve_begin), so a block inside the range has both its row tiles, and
+        // the only partial row block is the one holding the right-hand-side tile when it lies outside the range.  On the
+        // column side a block is two 16x8 products, and a half whose 8 rows lie outside the group's exact tile range
+        // [e0, e1) is zero in the panel and skipped.  Straight-line variants, no predicate inside a tensor-core loop; the
+        // column stride is the constant kFMaxRs, so every fragment load of a block is base + immediate.  A diagonal block
+        // passes the same pointer twice, so its B fragments are its A fragments (two loads per k-step instead of four).
         int gi = 0;
-        int g = next_group(g0), t0 = 0, t1 = 0;
-        if (g < g1) { t0 = gt0[g]; t1 = gt1[g]; }
+        int g = next_group(g0), tiles = 0;
+        if (g < g1) tiles = gtl[g];
         KBA_PROF_DECL;
         for (; g < g1; ++gi) {
             const int gn = next_group(g + 1);  // the next group's range is requested before this group's panel is awaited
-            int t0n = 0, t1n = 0;
-            if (gn < g1) { t0n = gt0[gn]; t1n = gt1[gn]; }
+            const int tiles_n = gn < g1 ? gtl[gn] : 0;
             const int slot = gi % kFStages;
             KBA_PROF_T0;
             mbar_wait(&full[slot], (gi / kFStages) & 1);
             KBA_PROF_ACC(0);
-            const int b0 = t0 >> 1, b1 = t1 >> 1;                         // block range [b0, b1) of the group
+            const int b0 = (tiles & 255) >> 1, b1 = ((tiles >> 8) & 255) >> 1;  // block range [b0, b1) of the group
+            const int e0 = (tiles >> 16) & 255, e1 = tiles >> 24;                // exact tile range [e0, e1)
             const bool rhs_in = brhs >= b0 && brhs < b1;
             const int rhs_row = 16 * (b1 - b0);  // panel row of the rhs tile when it lies outside the range
             const double* sb = stage + (size_t)slot * kFStageDoubles + (size_t)fc * kFMaxRs + fr;
 #pragma unroll
             for (int s = 0; s < kSlots; ++s) {
-                const int bi = my_bi[s], bj = my_bj[s];
+                const int b = my_b[s], bi = b >> 4, bj = b & 15;
                 if (bj < b0 || bj >= b1) continue;
-                if (bi >= b0 && bi < b1) {
-                    const double* pa = sb + 16 * (bi - b0);
-                    const double* pb = sb + 16 * (bj - b0);
-                    if (bi != bj) {
-#pragma unroll
-                        for (int kk = 0; kk < kGC; kk += 4) {
-                            const double a0 = pa[kk * kFMaxRs], a1 = pa[kk * kFMaxRs + 8], b0v = pb[kk * kFMaxRs], b1v = pb[kk * kFMaxRs + 8];
-                            dmma(acc[s][0][0], acc[s][0][1], a0, b0v);
-                            dmma(acc[s][1][0], acc[s][1][1], a0, b1v);
-                            dmma(acc[s][2][0], acc[s][2][1], a1, b0v);
-                            dmma(acc[s][3][0], acc[s][3][1], a1, b1v);
-                        }
-                    } else {
-#pragma unroll
-                        for (int kk = 0; kk < kGC; kk += 4) {
-                            const double a0 = pa[kk * kFMaxRs], a1 = pa[kk * kFMaxRs + 8];
-                            dmma(acc[s][0][0], acc[s][0][1], a0, a0);
-                            dmma(acc[s][2][0], acc[s][2][1], a1, a0);
-                            dmma(acc[s][3][0], acc[s][3][1], a1, a1);
-                        }
-                    }
-                } else if (bi == brhs && !rhs_in) {  // the right-hand-side tile against the group's rows
-                    const double* pa = sb + rhs_row;
-                    const double* pb = sb + 16 * (bj - b0);
-                    if (trhs & 1) {
-#pragma unroll
-                        for (int kk = 0; kk < kGC; kk += 4) {
-                            const double a1 = pa[kk * kFMaxRs], b0v = pb[kk * kFMaxRs], b1v = pb[kk * kFMaxRs + 8];
-                            dmma(acc[s][2][0], acc[s][2][1], a1, b0v);
-                            dmma(acc[s][3][0], acc[s][3][1], a1, b1v);
-                        }
-                    } else {
-#pragma unroll
-                        for (int kk = 0; kk < kGC; kk += 4) {
-                            const double a0 = pa[kk * kFMaxRs], b0v = pb[kk * kFMaxRs], b1v = pb[kk * kFMaxRs + 8];
-                            dmma(acc[s][0][0], acc[s][0][1], a0, b0v);
-                            dmma(acc[s][1][0], acc[s][1][1], a0, b1v);
-                        }
-                    }
-                }
+                const bool lo = 2 * bj >= e0, hi = 2 * bj + 1 < e1;  // column halves inside the exact range
+                const double* pb = sb + 16 * (bj - b0);
+                if (bi == bj) syrk_halves<false, kSlots == 6>(acc[s], pb, pb, false, lo, hi);
+                else if (bi >= b0 && bi < b1) syrk_halves<false, kSlots == 6>(acc[s], sb + 16 * (bi - b0), pb, false, lo, hi);
+                else if (bi == brhs && !rhs_in) syrk_halves<true, false>(acc[s], sb + rhs_row, pb, trhs & 1, lo, hi);
             }
             __syncwarp();
             if (lane == 0) mbar_arrive(&empty[slot]);
             KBA_PROF_ACC(1);
-            g = gn; t0 = t0n; t1 = t1n;
+            g = gn; tiles = tiles_n;
         }
         KBA_PROF_FLUSH(0);
     }
     double* out = bd.sred + wd.s_off * (size_t)bd.p_split + (size_t)blockIdx.x * wd.nr_cap * wd.nr_cap;
 #pragma unroll
     for (int s = 0; s < kSlots; ++s) {
-        const int bi = my_bi[s], bj = my_bj[s];
+        const int b = my_b[s], bi = b >> 4, bj = b & 15;
         if (bi >= nb2) continue;
 #pragma unroll
         for (int q = 0; q < 4; ++q) {
             const int i = 2 * bi + (q >> 1), j = 2 * bj + (q & 1);
             if (i >= nt || j > i) continue;
             double* o = out + (size_t)(8 * i + fr) * wd.nr_cap + 8 * j + 2 * fc;
-            o[0] = acc[s][q][0];
-            o[1] = acc[s][q][1];
+            o[0] = acc[s][q & 1][2 * (q >> 1)];
+            o[1] = acc[s][q & 1][2 * (q >> 1) + 1];
         }
     }
 }

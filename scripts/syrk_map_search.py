@@ -4,7 +4,9 @@
 The kernel keeps the lower triangle of the reduced system as 16x16 accumulator blocks in the registers of 12 consumer
 warps (3 per SM sub-partition), so ownership is static.  A landmark group (8 landmarks) only touches the blocks inside
 its keyframe row range plus the right-hand-side row; the FP64 tensor pipe is per sub-partition, so what a stage costs
-is the DMMA count of its busiest sub-partition.  The ring lets warps drift a few stages, so the long-run totals count
+is the MMA count of its busiest sub-partition.  A block is two 16x8 halves (mma.m16n8k4, 6 k-steps per group): a block
+costs its halves whose 8 columns meet the group's exact 8-row tile range, when its rows lie in the group's 16-row-aligned
+block range or hold the right-hand-side tile outside it.  The ring lets warps drift a few stages, so the long-run totals count
 too.  Objective: sum over groups of the busiest sub-partition + the long-run maximum, on config-2 windows (29 free
 keyframes) and on 30-free-keyframe windows (184 rows).
 
@@ -45,18 +47,13 @@ def groups_of(win, fixed_first):
 
 
 def block_cost(bi, bj, t0, t1, trhs):
-    """DMMA k-steps x tiles of one 16x16 block for a group (6 k-steps of 4 columns)"""
-    def present(t):
-        return (t0 <= t < t1) or t == trhs
-    ri = [present(2 * bi), present(2 * bi + 1)]
-    rj = [present(2 * bj), present(2 * bj + 1)]
-    n = 0
-    for a in range(2):
-        for b in range(2):
-            if bi == bj and a == 0 and b == 1:
-                continue
-            n += ri[a] and rj[b]
-    return 6 * n
+    """m16n8k4 MMAs of one 16x16 block for a group with exact tile range [t0, t1) (6 k-steps of 4 columns)"""
+    b0, b1 = t0 // 2, (t1 + 1) // 2                   # 16-row-aligned block range
+    rhs_in = b0 <= trhs // 2 < b1
+    e1 = max(t1, trhs + 1) if rhs_in else t1           # the rhs tile is part of the exact range when inside the blocks
+    if not b0 <= bj < b1 or not (b0 <= bi < b1 or (bi == trhs // 2 and not rhs_in)):
+        return 0
+    return 6 * (int(2 * bj >= t0) + int(2 * bj + 1 < e1))
 
 
 def build_costs(groups):
@@ -90,7 +87,7 @@ def main():
     for seed in (4,):
         g30 += groups_of(synth.make_window(2, seed=seed), False)
     C = np.concatenate([build_costs(groups), build_costs(g30)[::3]])
-    print("groups", C.shape[0], "mean DMMA per group", C.sum() / C.shape[0])
+    print("groups", C.shape[0], "mean MMA per group", C.sum() / C.shape[0])
     # start: rows dealt cyclically with a skew; every warp gets exactly one block of row 11 and at most one of row 10
     owner = np.zeros(len(BLOCKS), dtype=np.int64)
     cnt = [0] * NW
@@ -127,13 +124,14 @@ def main():
             if it % 50 == 0:
                 print(it, "score %.4f per-stage %.4f long-run %.4f" % (best, pb, lb), flush=True)
     print("final: per-stage busiest-subpartition / ideal = %.4f, long-run = %.4f" % (pb, lb))
-    # slot 0 = the warp's row-11 block, slots 1..6 = blocks of rows <= 10 (-1 padded)
-    print("__constant__ signed char kSyrkMap12[12][7] = {")
+    # slot 0 = the warp's row-11 block, slots 1..6 = blocks of rows <= 10 (0xff padded), as 16 bi + bj
+    code = lambda b: "0x%02x" % (16 * BLOCKS[b][0] + BLOCKS[b][1])
+    print("__constant__ unsigned char kSyrkMap12[12][7] = {")
     for w in range(NW):
-        r11 = [b for b in row11 if owner[b] == w]
-        rest = [b for b in low if owner[b] == w]
-        row = r11 + rest + [-1] * (NSLOT - 1 - len(rest))
-        print("    {%s}," % ", ".join(str(x) for x in row))
+        r11 = [code(b) for b in row11 if owner[b] == w]
+        rest = [code(b) for b in low if owner[b] == w]
+        row = r11 + rest + ["0xff"] * (NSLOT - 1 - len(rest))
+        print("    {%s}," % ", ".join(row))
     print("};")
 
 
