@@ -304,6 +304,45 @@ int kba_track_solve(kba_track* t, int32_t n_kf, const int32_t* kf_slot, const ui
                     const kba_window* sel, const kba_options* opt, kba_result* res);
 int kba_track_transfer_bytes(kba_track* t, int64_t* h2d_last_solve, int64_t* d2h_last_solve, int64_t* h2d_pushes_total);
 
+/* ---- many persistent windows in one launch: track groups -----------------------------------------------------------------
+ * kba_track_solve solves one window per call, which leaves the GPU mostly idle.  A group solves one window of each of its tracks
+ * as ONE batch (one kba_batch_solve: one CUDA graph launch), with the persistent store of every track: per solve only the
+ * selection lists travel, for all tracks together in one copy.  For several vehicles, offline reprocessing of many sequences or
+ * parameter sweeps over one recording.
+ *   - Membership: every track belongs to `h` (same device and stream) and appears once; an empty group, a duplicate or a track
+ *     of another handle is KBA_ERR_BAD_ARG.  Destroy a group before its tracks (as a batch before its handle).  A track of a
+ *     group may still be solved alone with kba_track_solve; between calls its store is the single source of truth.
+ *   - Memory: the group owns one capacity-shaped window per track, a copy of the allocations of the track's own batch (about
+ *     10 MB for a track sized like config 2, 30 keyframes / 3k landmarks / 40k observations).
+ *   - Validation: every request with n_kf != 0 is checked exactly as kba_track_solve checks its arguments.  If one fails, the
+ *     call returns that request's code before anything is uploaded or launched, kba_last_error names the track index, and no
+ *     store changes.
+ *   - Results: window i is the window kba_track_solve would build for track i; its results go to res[i] and into track i's
+ *     store exactly as for a single solve.  One kba_options applies to the whole group; solver_time_sec is checked on the
+ *     group's shared passes: each window's inner solves are timed on the device while the passes of the whole group run, so
+ *     a window's budget includes the time its group's other windows take.
+ *   - Launch configuration, decided per solve from the windows that are solved: the largest rig rank, the seven-slot Schur
+ *     kernel if any window needs more than 176 reduced rows, and from these the fused-linearisation switch, as kba_batch_solve
+ *     decides for any batch.  A window in a mixed group can therefore run a different kernel variant than alone (e.g. a
+ *     multi-camera rig turns the fused linearisation off for every window) and round differently in the last bits.
+ *   - Skipping: a request with n_kf == 0 sits the solve out: its store is untouched, res[i] gets status KBA_OK and
+ *     num_solves 0, its output arrays are not written.  A call in which every track sits out returns at once. */
+typedef struct kba_track_group kba_track_group;
+typedef struct kba_track_request {
+    int32_t n_kf;               /* 0: this track sits this solve out (store untouched, result status KBA_OK, num_solves 0) */
+    const int32_t* kf_slot;     /* the fields mean exactly what the arguments of kba_track_solve mean */
+    const uint8_t* kf_fixed;
+    int32_t n_lm;
+    const int32_t* lm_slot;
+    const kba_window* sel;      /* sizes, scalars and ground-plane lists, as for kba_track_solve */
+} kba_track_request;
+int kba_track_group_create(kba_handle* h, int32_t n_tracks, kba_track* const* tracks, kba_track_group** out);
+void kba_track_group_destroy(kba_track_group* g);
+/* req[n_tracks], res[n_tracks] */
+int kba_track_group_solve(kba_track_group* g, const kba_track_request* req, const kba_options* opt, kba_result* res);
+/* upload / download of the last group solve, counted as kba_track_transfer_bytes counts them */
+int kba_track_group_transfer_bytes(kba_track_group* g, int64_t* h2d_last_solve, int64_t* d2h_last_solve);
+
 /* ---- landmark initialisation of push() for a whole window (SURVEY 8(f) row 2) ------------------------------------------
  * Replaces, for all landmarks of `w` at once, what BundleAdjusterKeyframes::push() does per new landmark on the host:
  * the first observation with a lidar depth (d >= 0) is back-projected (bundle_adjuster_keyframes.cpp:332-355); without

@@ -8,8 +8,8 @@ import os
 
 import numpy as np
 
-from .capi_types import (KbaCounters, KbaEvalOut, KbaLidarOptions, KbaOptions, KbaResult, KbaTrackCaps, KbaWindow, Result, Window,
-                         c_double_p, c_int32_p)
+from .capi_types import (KbaCounters, KbaEvalOut, KbaLidarOptions, KbaOptions, KbaResult, KbaTrackCaps, KbaTrackRequest, KbaWindow,
+                         Result, Window, c_double_p, c_int32_p)
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("KBA_LIB_PATH") or os.path.join(_HERE, "libkba_b200.so")  # KBA_LIB_PATH: instrumented builds
@@ -21,7 +21,8 @@ SYMBOLS = ["kba_version", "kba_last_error", "kba_default_options", "kba_create",
            "kba_get_counters", "kba_enable_kernel_timing", "kba_lidar_default_options", "kba_lidar_depth",
            "kba_shard_unique_id", "kba_shard_comm_create", "kba_shard_comm_destroy", "kba_batch_set_shard",
            "kba_init_landmarks", "kba_track_create", "kba_track_destroy", "kba_track_push_keyframe", "kba_track_drop_keyframe",
-           "kba_track_set_landmarks", "kba_track_set_keyframe_pose", "kba_track_set_keyframe_poses", "kba_track_solve", "kba_track_transfer_bytes"]
+           "kba_track_set_landmarks", "kba_track_set_keyframe_pose", "kba_track_set_keyframe_poses", "kba_track_solve", "kba_track_transfer_bytes",
+           "kba_track_group_create", "kba_track_group_destroy", "kba_track_group_solve", "kba_track_group_transfer_bytes"]
 
 
 class KbaError(RuntimeError):
@@ -74,6 +75,11 @@ def lib():
         L.kba_track_set_keyframe_poses.argtypes = [vp, C.c_int32, ip, c_double_p, c_double_p]
         L.kba_track_solve.argtypes = [vp, C.c_int32, ip, u8p, C.c_int32, ip, C.POINTER(KbaWindow), C.POINTER(KbaOptions), C.POINTER(KbaResult)]
         L.kba_track_transfer_bytes.argtypes = [vp, C.POINTER(C.c_int64), C.POINTER(C.c_int64), C.POINTER(C.c_int64)]
+        L.kba_track_group_create.argtypes = [vp, C.c_int32, C.POINTER(vp), C.POINTER(vp)]
+        L.kba_track_group_destroy.argtypes = [vp]
+        L.kba_track_group_destroy.restype = None
+        L.kba_track_group_solve.argtypes = [vp, C.POINTER(KbaTrackRequest), C.POINTER(KbaOptions), C.POINTER(KbaResult)]
+        L.kba_track_group_transfer_bytes.argtypes = [vp, C.POINTER(C.c_int64), C.POINTER(C.c_int64)]
         L.kba_lidar_default_options.argtypes = [C.POINTER(KbaLidarOptions)]
         L.kba_lidar_default_options.restype = None
         fp = C.POINTER(C.c_float)
@@ -194,17 +200,30 @@ class Track:
         _check(lib().kba_track_set_landmarks(self._p, len(lm), lmp, C.cast(None, c_double_p) if p is None else p.ctypes.data_as(c_double_p),
                                              C.cast(None, c_double_p) if w is None else w.ctypes.data_as(c_double_p)))
 
-    def solve(self, kf_slots, kf_fixed, lm_slots, opt=None, **scalars):
-        """scalars: scale_kf0, scale_kf1, scale_weight, scale_value, plane_reg_weight, plane_dist_fixed, gp_lm, gp_kf, gp_weight"""
+    def set_keyframe_poses(self, kf_slots, pose7s, plane4s=None):
         kf, kfp = self._i32(kf_slots)
-        lm, lmp = self._i32(lm_slots)
+        p = np.ascontiguousarray(pose7s, dtype=np.float64).reshape(-1, 7)
+        pl = None if plane4s is None else np.ascontiguousarray(plane4s, dtype=np.float64).reshape(-1, 4)
+        _check(lib().kba_track_set_keyframe_poses(self._p, len(kf), kfp, p.ctypes.data_as(c_double_p),
+                                                  C.cast(None, c_double_p) if pl is None else pl.ctypes.data_as(c_double_p)))
+
+    @staticmethod
+    def _selection(kf_slots, kf_fixed, lm_slots, **scalars):
+        """the arrays of one solve and the `sel` window that carries its sizes, scalars and ground-plane lists"""
+        kf, _ = Track._i32(kf_slots)
+        lm, _ = Track._i32(lm_slots)
         fx = np.ascontiguousarray(kf_fixed, dtype=np.uint8)
         n_kf, n_lm = len(kf), len(lm)
         sel = Window(np.tile([1.0, 0, 0, 0, 0, 0, 0], (n_kf, 1)), fx, [[1.0, 0, 0]], [[1.0, 0, 0, 0, 0, 0, 0]], np.zeros((n_lm, 3)),
                      np.ones(n_lm), np.zeros(n_lm + 1, dtype=np.int32), [], [], [], [], **scalars)
+        return kf, fx, lm, sel
+
+    def solve(self, kf_slots, kf_fixed, lm_slots, opt=None, **scalars):
+        """scalars: scale_kf0, scale_kf1, scale_weight, scale_value, plane_reg_weight, plane_dist_fixed, gp_lm, gp_kf, gp_weight"""
+        kf, fx, lm, sel = self._selection(kf_slots, kf_fixed, lm_slots, **scalars)
         res = Result(sel, 256)
-        _check(lib().kba_track_solve(self._p, n_kf, kfp, fx.ctypes.data_as(C.POINTER(C.c_uint8)), n_lm, lmp, C.byref(sel.c),
-                                     C.byref(opt or default_options()), C.byref(res.c)))
+        _check(lib().kba_track_solve(self._p, len(kf), kf.ctypes.data_as(c_int32_p), fx.ctypes.data_as(C.POINTER(C.c_uint8)), len(lm),
+                                     lm.ctypes.data_as(c_int32_p), C.byref(sel.c), C.byref(opt or default_options()), C.byref(res.c)))
         return res
 
     def transfer_bytes(self):
@@ -215,6 +234,53 @@ class Track:
     def close(self):
         if self._p:
             lib().kba_track_destroy(self._p)
+            self._p = C.c_void_p()
+
+
+class TrackGroup:
+    """Several persistent windows solved as one batch (kba_track_group_*): one launch for a window of every track."""
+
+    def __init__(self, handle, tracks):
+        self.handle, self.tracks = handle, list(tracks)
+        arr = (C.c_void_p * len(self.tracks))(*[t._p.value for t in self.tracks])
+        self._p = C.c_void_p()
+        _check(lib().kba_track_group_create(handle._p, len(self.tracks), arr, C.byref(self._p)))
+
+    def solve(self, requests, opt=None, iterations_capacity=256):
+        """requests: one per track, None (the track sits this solve out) or a dict with the arguments of Track.solve
+        (kf_slots, kf_fixed, lm_slots and the scalar keywords).  Returns one Result per track."""
+        assert len(requests) == len(self.tracks)
+        reqs = (KbaTrackRequest * len(requests))()
+        keep, results = [], []
+        for i, r in enumerate(requests):
+            if r is None:
+                sel = Window(np.tile([1.0, 0, 0, 0, 0, 0, 0], (0, 1)), [], [[1.0, 0, 0]], [[1.0, 0, 0, 0, 0, 0, 0]], np.zeros((0, 3)), [],
+                             [0], [], [], [], [])
+                results.append(Result(sel, 1))
+                continue
+            r = dict(r)
+            kf, fx, lm, sel = Track._selection(r.pop("kf_slots"), r.pop("kf_fixed"), r.pop("lm_slots"), **r)
+            q = reqs[i]
+            q.n_kf, q.n_lm = len(kf), len(lm)
+            q.kf_slot, q.kf_fixed = kf.ctypes.data_as(c_int32_p), fx.ctypes.data_as(C.POINTER(C.c_uint8))
+            q.lm_slot, q.sel = lm.ctypes.data_as(c_int32_p), C.pointer(sel.c)
+            keep.append((kf, fx, lm, sel))
+            results.append(Result(sel, iterations_capacity))
+        rarr = (KbaResult * len(results))(*[r.c for r in results])
+        _check(lib().kba_track_group_solve(self._p, reqs, C.byref(opt or default_options()), rarr))
+        for r, c in zip(results, rarr):
+            r.c = c
+        return results
+
+    def transfer_bytes(self):
+        """(host->device bytes, device->host bytes) of the last group solve"""
+        a, b = C.c_int64(), C.c_int64()
+        _check(lib().kba_track_group_transfer_bytes(self._p, C.byref(a), C.byref(b)))
+        return a.value, b.value
+
+    def close(self):
+        if self._p:
+            lib().kba_track_group_destroy(self._p)
             self._p = C.c_void_p()
 
 

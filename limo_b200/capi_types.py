@@ -37,6 +37,11 @@ class KbaTrackCaps(C.Structure):
                 ("win_ground", C.c_int32)]
 
 
+class KbaTrackRequest(C.Structure):
+    _fields_ = [("n_kf", C.c_int32), ("kf_slot", c_int32_p), ("kf_fixed", c_uint8_p), ("n_lm", C.c_int32), ("lm_slot", c_int32_p),
+                ("sel", C.POINTER(KbaWindow))]
+
+
 class KbaOptions(C.Structure):
     _fields_ = [
         ("depth_thres", C.c_double), ("reprojection_thres", C.c_double),

@@ -6,6 +6,7 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <memory>
 #include <string>
 #include <thread>
 #include <vector>
@@ -190,6 +191,9 @@ struct kba_track {
     Staged<uint8_t> sel_fixed;
     Staged<double> p_dbl;                  // poses / landmark values on their way to the store
     Staged<int> p_slot;                    // ... and the slots they go to
+    Staged<TrackDev> tdev;                 // [1] the store and the selection of this solve, as the gather kernels read them
+    Staged<TrackSel> tsel;
+    std::vector<double> cam_intr, cam_pose;  // host copy of the cameras: capacity windows of kba_track_group_create
     int push_cap = 0, set_cap = 0;
     int64_t h2d_solve = 0, d2h_solve = 0, h2d_push = 0;
     template <typename T> int alloc(T** p, size_t n) {
@@ -201,6 +205,17 @@ struct kba_track {
         td.m_lm = arena_i[arena_cur][0]; td.m_cam = arena_i[arena_cur][1];
         td.m_u = arena_f[arena_cur][0]; td.m_v = arena_f[arena_cur][1]; td.m_d = arena_f[arena_cur][2];
     }
+};
+
+// several tracks solved as one batch (kba_track_group_*, at the end of this file)
+struct kba_track_group {
+    kba_handle* h = nullptr;
+    std::vector<kba_track*> tracks;
+    kba_batch* batch = nullptr;            // one capacity-shaped window per track
+    Staged<TrackDev> tdev;                 // [n_tracks] read at every solve: compaction re-points a track's arena
+    Staged<TrackSel> tsel;
+    Staged<int> lists;                     // every selection list of a solve (keyframe slots, landmark slots, fixation bytes), ONE copy
+    int64_t h2d_solve = 0, d2h_solve = 0;
 };
 
 static int validate_window(const kba_window* w, std::string& why) {
@@ -1276,7 +1291,119 @@ void kba_track_destroy(kba_track* t) {
     for (void* p : t->dev) cudaFree(p);
     t->p_lm.release(); t->p_cam.release(); t->sel_kf.release(); t->sel_lm.release(); t->lay.release();
     t->p_u.release(); t->p_v.release(); t->p_d.release(); t->sel_fixed.release(); t->p_dbl.release(); t->p_slot.release();
+    t->tdev.release(); t->tsel.release();
     delete t;
+}
+
+// A dummy window of a track's largest shape: the batch created from it has the capacity every later solve of the track fits in.
+// The observations are spread evenly over the landmarks and, within a landmark, over the keyframes in ascending order: the packing
+// kernels run once on this window (create = upload), and their per-landmark loops (insertion sort of a track, k_track_sort /
+// k_pack_obs) are written for tracks of a few dozen observations -- one landmark carrying all 2^18 of them kept a single GPU
+// thread busy for minutes.
+struct CapacityWindow {
+    std::vector<double> pose, plane, lmp, lmw, gw;
+    std::vector<uint8_t> fixed;
+    std::vector<int32_t> ptr, okf, gl, gk;
+    std::vector<float> u, v, d;
+    kba_window w{};
+    CapacityWindow(const kba_track_caps& c, int n_cam, const double* cam_intr, const double* cam_pose) {
+        const int K = c.win_keyframes, L = c.win_landmarks, O = c.win_observations, G = c.win_ground;
+        pose.assign(7 * (size_t)K, 0.0); plane.assign(4 * (size_t)K, 0.0); lmp.assign(3 * (size_t)L, 0.0); lmw.assign(L, 1.0);
+        gw.assign(std::max(G, 1), 1.0);
+        fixed.assign(K, 0);
+        ptr.assign(L + 1, O); okf.assign(O, 1); gl.assign(std::max(G, 1), 0); gk.assign(std::max(G, 1), 1);
+        u.assign(O, 0.f); v.assign(O, 0.f); d.assign(O, -1.f);
+        for (int k = 0; k < K; ++k) { pose[7 * k] = 1.0; plane[4 * k + 2] = 1.0; }
+        for (int j = 0; j < L; ++j) lmp[3 * j + 2] = 10.0;
+        for (int g = 0; g < G; ++g) gl[g] = g;
+        fixed[0] = 1;
+        for (int j = 0; j <= L; ++j) ptr[j] = (int32_t)(((long long)O * j) / L);
+        for (int j = 0; j < L; ++j) {
+            const int n = ptr[j + 1] - ptr[j];
+            for (int i = 0; i < n; ++i) okf[ptr[j] + i] = (n <= K) ? i : (int32_t)(((long long)i * K) / n);  // non-decreasing
+        }
+        w.n_kf = K; w.n_cam = n_cam; w.n_lm = L; w.n_obs = O; w.n_gp = G;
+        w.kf_pose = pose.data(); w.kf_fixed = fixed.data(); w.kf_plane = plane.data(); w.cam_intr = cam_intr; w.cam_pose = cam_pose;
+        w.lm_pos = lmp.data(); w.lm_weight = lmw.data(); w.lm_obs_ptr = ptr.data(); w.obs_kf = okf.data(); w.obs_u = u.data();
+        w.obs_v = v.data(); w.obs_d = d.data(); w.gp_lm = gl.data(); w.gp_kf = gk.data(); w.gp_weight = gw.data();
+        w.plane_reg_weight = G > 0 ? 10.0 : 0.0;
+    }
+};
+
+// what one solve of the stored window asks for (the arguments of kba_track_solve)
+struct TrackRequest {
+    int32_t n_kf = 0;
+    const int32_t* kf_slot = nullptr;
+    const uint8_t* kf_fixed = nullptr;
+    int32_t n_lm = 0;
+    const int32_t* lm_slot = nullptr;
+    const kba_window* sel = nullptr;
+    int max_meas = 0, n_free = 0;          // filled by track_check: largest keyframe measurement count, free keyframes
+};
+
+// every argument check of a track solve, before anything is uploaded or launched
+static int track_check(const kba_track* t, TrackRequest& q, std::string& why) {
+    if (!q.kf_slot || !q.kf_fixed || !q.lm_slot || !q.sel) { why = "null argument"; return KBA_ERR_BAD_ARG; }
+    const kba_track_caps& c = t->caps;
+    const kba_window* sel = q.sel;
+    if (q.n_kf < 3) { why = "fewer than 3 keyframes"; return KBA_ERR_NOT_ENOUGH_KF; }
+    if (q.n_kf > c.win_keyframes || q.n_lm > c.win_landmarks || q.n_lm < 0 || sel->n_gp < 0 || sel->n_gp > c.win_ground) {
+        why = "window larger than the capacities given to kba_track_create"; return KBA_ERR_CAPACITY;
+    }
+    long long n_meas = 0;
+    q.max_meas = 0; q.n_free = 0;
+    for (int k = 0; k < q.n_kf; ++k) {
+        const int slot = q.kf_slot[k];
+        if (slot < 0 || slot >= t->td.kf_cap || !t->kf_live[slot]) { why = "keyframe slot not pushed"; return KBA_ERR_BAD_ARG; }
+        n_meas += t->m_cnt[slot]; q.max_meas = std::max(q.max_meas, t->m_cnt[slot]);
+        q.n_free += q.kf_fixed[k] ? 0 : 1;
+    }
+    if (n_meas > c.win_observations) { why = "more observations than win_observations"; return KBA_ERR_CAPACITY; }
+    for (int j = 0; j < q.n_lm; ++j)
+        if (q.lm_slot[j] < 0 || q.lm_slot[j] >= t->td.lm_cap) { why = "landmark slot out of range"; return KBA_ERR_BAD_ARG; }
+    for (int g = 0; g < sel->n_gp; ++g)
+        if (!sel->gp_lm || !sel->gp_kf || !sel->gp_weight || sel->gp_lm[g] < 0 || sel->gp_lm[g] >= q.n_lm || sel->gp_kf[g] < 0 ||
+            sel->gp_kf[g] >= q.n_kf) {
+            why = "ground-plane index out of range"; return KBA_ERR_BAD_ARG;
+        }
+    const bool planes = sel->n_gp > 0 || sel->plane_reg_weight > 0;
+    if (planes && c.win_ground == 0) { why = "the track was created without ground-plane capacity"; return KBA_ERR_CAPACITY; }
+    if (sel->scale_weight != 0 && (sel->scale_kf0 < 0 || sel->scale_kf0 >= q.n_kf || sel->scale_kf1 < 0 || sel->scale_kf1 >= q.n_kf)) {
+        why = "scale regulariser keyframe out of range"; return KBA_ERR_BAD_ARG;
+    }
+    return KBA_OK;
+}
+
+// the window descriptor of a checked request (n_obs is written by the gather kernels); offsets and capacities stay as created
+static void track_desc(WinDesc& d, const kba_track* t, const TrackRequest& q) {
+    const kba_window* sel = q.sel;
+    d.n_kf = q.n_kf; d.n_lm = q.n_lm; d.n_obs = 0; d.n_gp = sel->n_gp;
+    d.n_chunks = (q.n_lm + 31) / 32; d.n_groups = (q.n_lm + 7) / 8;
+    d.scale_kf0 = sel->scale_kf0; d.scale_kf1 = sel->scale_kf1; d.scale_weight = sel->scale_weight; d.scale_value = sel->scale_value;
+    d.plane_reg_weight = sel->plane_reg_weight; d.plane_dist_fixed = sel->plane_dist_fixed; d.landmarks_fixed = 0;
+    d.speed_kf = 0; d.speed_weight = 0; d.speed_dt = 1;
+    d.max_rank = t->n_cam > 1 ? t->n_cam - 1 : 0;  // a rig may see a landmark from several cameras of one keyframe
+    d.idle = 0;
+}
+
+// fused Schur kernel instance a checked request needs (kba_batch_create's rule on its free keyframes)
+static int track_fused_slots(const TrackRequest& q) {
+    const bool planes = q.sel->n_gp > 0 || q.sel->plane_reg_weight > 0;
+    return ((planes ? 10 : 6) * q.n_free + 1 <= 176) ? 6 : 7;
+}
+
+// a track sitting a group solve out: nothing to gather, k_reset_state puts the window straight into PH_DONE
+static void idle_desc(WinDesc& d) {
+    d.n_kf = 0; d.n_lm = 0; d.n_obs = 0; d.n_gp = 0; d.n_chunks = 0; d.n_groups = 0;
+    d.scale_weight = 0; d.plane_reg_weight = 0; d.plane_dist_fixed = 0; d.landmarks_fixed = 0; d.speed_weight = 0; d.max_rank = 0;
+    d.idle = 1;
+}
+
+static TrackSel track_sel(const TrackRequest& q, const int* kf_slot_d, const uint8_t* kf_fixed_d, const int* lm_slot_d) {
+    TrackSel ts;
+    ts.kf_slot = kf_slot_d; ts.kf_fixed = kf_fixed_d; ts.lm_slot = lm_slot_d; ts.n_kf = q.n_kf; ts.n_lm = q.n_lm; ts.max_meas = q.max_meas;
+    ts.auto_scale = q.sel->scale_weight < 0 ? 1 : 0;
+    return ts;
 }
 
 int kba_track_create(kba_handle* h, const kba_track_caps* c, int32_t n_cam, const double* cam_intr, const double* cam_pose, kba_track** out) {
@@ -1290,32 +1417,11 @@ int kba_track_create(kba_handle* h, const kba_track_caps* c, int32_t n_cam, cons
     CU(cudaSetDevice(h->device));
     kba_track* t = new kba_track();
     t->h = h; t->caps = *c; t->n_cam = n_cam;
-    // capacity batch from a dummy window of the largest shape.  The observations are spread evenly over the landmarks and, within
-    // a landmark, over the keyframes in ascending order: the packing kernels run once on this window (create = upload), and their
-    // per-landmark loops (insertion sort of a track, k_track_sort / k_pack_obs) are written for tracks of a few dozen
-    // observations -- one landmark carrying all 2^18 of them kept a single GPU thread busy for minutes.
+    t->cam_intr.assign(cam_intr, cam_intr + 3 * (size_t)n_cam);
+    t->cam_pose.assign(cam_pose, cam_pose + 7 * (size_t)n_cam);
     {
-        const int K = c->win_keyframes, L = c->win_landmarks, O = c->win_observations, G = c->win_ground;
-        std::vector<double> pose(7 * (size_t)K, 0.0), plane(4 * (size_t)K, 0.0), lmp(3 * (size_t)L, 0.0), lmw(L, 1.0), gw(std::max(G, 1), 1.0);
-        std::vector<uint8_t> fixed(K, 0);
-        std::vector<int32_t> ptr(L + 1, O), okf(O, 1), gl(std::max(G, 1), 0), gk(std::max(G, 1), 1);
-        std::vector<float> u(O, 0.f), v(O, 0.f), d(O, -1.f);
-        for (int k = 0; k < K; ++k) { pose[7 * k] = 1.0; plane[4 * k + 2] = 1.0; }
-        for (int j = 0; j < L; ++j) lmp[3 * j + 2] = 10.0;
-        for (int g = 0; g < G; ++g) gl[g] = g;
-        fixed[0] = 1;
-        for (int j = 0; j <= L; ++j) ptr[j] = (int32_t)(((long long)O * j) / L);
-        for (int j = 0; j < L; ++j) {
-            const int n = ptr[j + 1] - ptr[j];
-            for (int i = 0; i < n; ++i) okf[ptr[j] + i] = (n <= K) ? i : (int32_t)(((long long)i * K) / n);  // non-decreasing
-        }
-        kba_window w{};
-        w.n_kf = K; w.n_cam = n_cam; w.n_lm = L; w.n_obs = O; w.n_gp = G;
-        w.kf_pose = pose.data(); w.kf_fixed = fixed.data(); w.kf_plane = plane.data(); w.cam_intr = cam_intr; w.cam_pose = cam_pose;
-        w.lm_pos = lmp.data(); w.lm_weight = lmw.data(); w.lm_obs_ptr = ptr.data(); w.obs_kf = okf.data(); w.obs_u = u.data();
-        w.obs_v = v.data(); w.obs_d = d.data(); w.gp_lm = gl.data(); w.gp_kf = gk.data(); w.gp_weight = gw.data();
-        w.plane_reg_weight = G > 0 ? 10.0 : 0.0;
-        const int rc = kba_batch_create(h, 1, &w, &t->batch);
+        const CapacityWindow cw(*c, n_cam, t->cam_intr.data(), t->cam_pose.data());
+        const int rc = kba_batch_create(h, 1, &cw.w, &t->batch);
         if (rc != KBA_OK) { delete t; return rc; }
         if (!t->batch->device_pack) { kba_track_destroy(t); return fail(KBA_ERR_CAPACITY, "kba_track_create: device packing is disabled (KBA_FUSED / KBA_DEVICE_PACK)"); }
     }
@@ -1337,6 +1443,7 @@ int kba_track_create(kba_handle* h, const kba_track_caps* c, int32_t n_cam, cons
     bad |= t->lay.alloc(2 * (size_t)td.kf_cap, true);
     t->set_cap = std::max(c->win_landmarks, 64);  // rows per staged scatter (landmarks or keyframes)
     bad |= t->p_dbl.alloc(7 * (size_t)t->set_cap, true); bad |= t->p_slot.alloc(t->set_cap, true);
+    bad |= t->tdev.alloc(1, true); bad |= t->tsel.alloc(1, true);
     if (bad) { kba_track_destroy(t); return fail(KBA_ERR_CUDA, "kba_track_create: out of memory"); }
     t->point_arena();
     t->m_off.assign(td.kf_cap, 0); t->m_cnt.assign(td.kf_cap, 0); t->kf_live.assign(td.kf_cap, 0);
@@ -1461,64 +1568,45 @@ int kba_track_set_landmarks(kba_track* t, int32_t n, const int32_t* slot, const 
 
 int kba_track_solve(kba_track* t, int32_t n_kf, const int32_t* kf_slot, const uint8_t* kf_fixed, int32_t n_lm, const int32_t* lm_slot,
                     const kba_window* sel, const kba_options* opt, kba_result* res) {
-    if (!t || !kf_slot || !kf_fixed || !lm_slot || !sel || !opt || !res) return fail(KBA_ERR_BAD_ARG, "null argument to kba_track_solve");
-    const kba_track_caps& c = t->caps;
-    if (n_kf < 3) return fail(KBA_ERR_NOT_ENOUGH_KF, "kba_track_solve: fewer than 3 keyframes");
-    if (n_kf > c.win_keyframes || n_lm > c.win_landmarks || n_lm < 0 || sel->n_gp < 0 || sel->n_gp > c.win_ground)
-        return fail(KBA_ERR_CAPACITY, "kba_track_solve: window larger than the capacities given to kba_track_create");
-    long long n_meas = 0;
-    int max_meas = 0, n_free = 0;
-    for (int k = 0; k < n_kf; ++k) {
-        if (kf_slot[k] < 0 || kf_slot[k] >= t->td.kf_cap || !t->kf_live[kf_slot[k]]) return fail(KBA_ERR_BAD_ARG, "kba_track_solve: keyframe slot not pushed");
-        n_meas += t->m_cnt[kf_slot[k]]; max_meas = std::max(max_meas, t->m_cnt[kf_slot[k]]);
-        n_free += kf_fixed[k] ? 0 : 1;
-    }
-    if (n_meas > c.win_observations) return fail(KBA_ERR_CAPACITY, "kba_track_solve: more observations than win_observations");
-    for (int j = 0; j < n_lm; ++j)
-        if (lm_slot[j] < 0 || lm_slot[j] >= t->td.lm_cap) return fail(KBA_ERR_BAD_ARG, "kba_track_solve: landmark slot out of range");
-    for (int g = 0; g < sel->n_gp; ++g)
-        if (!sel->gp_lm || !sel->gp_kf || !sel->gp_weight || sel->gp_lm[g] < 0 || sel->gp_lm[g] >= n_lm || sel->gp_kf[g] < 0 || sel->gp_kf[g] >= n_kf)
-            return fail(KBA_ERR_BAD_ARG, "kba_track_solve: ground-plane index out of range");
-    const bool planes = sel->n_gp > 0 || sel->plane_reg_weight > 0;
-    if (planes && c.win_ground == 0) return fail(KBA_ERR_CAPACITY, "kba_track_solve: the track was created without ground-plane capacity");
+    if (!t || !opt || !res) return fail(KBA_ERR_BAD_ARG, "null argument to kba_track_solve");
+    TrackRequest q;
+    q.n_kf = n_kf; q.kf_slot = kf_slot; q.kf_fixed = kf_fixed; q.n_lm = n_lm; q.lm_slot = lm_slot; q.sel = sel;
+    std::string why;
+    const int crc = track_check(t, q, why);
+    if (crc != KBA_OK) return fail(crc, "kba_track_solve: " + why);
     kba_batch* b = t->batch;
     CU(cudaSetDevice(t->h->device));
     cudaStream_t s = t->h->stream;
     // ---- the window descriptor of this solve (n_obs is written by the gather kernels)
     WinDesc& d = b->desc_h[0];
-    d.n_kf = n_kf; d.n_lm = n_lm; d.n_obs = 0; d.n_gp = sel->n_gp;
-    d.n_chunks = (n_lm + 31) / 32; d.n_groups = (n_lm + 7) / 8;
-    d.scale_kf0 = sel->scale_kf0; d.scale_kf1 = sel->scale_kf1; d.scale_weight = sel->scale_weight; d.scale_value = sel->scale_value;
-    d.plane_reg_weight = sel->plane_reg_weight; d.plane_dist_fixed = sel->plane_dist_fixed; d.landmarks_fixed = 0;
-    d.speed_kf = 0; d.speed_weight = 0; d.speed_dt = 1;
-    d.max_rank = t->n_cam > 1 ? t->n_cam - 1 : 0;  // a rig may see a landmark from several cameras of one keyframe
-    if (d.scale_weight != 0 && (d.scale_kf0 < 0 || d.scale_kf0 >= n_kf || d.scale_kf1 < 0 || d.scale_kf1 >= n_kf))
-        return fail(KBA_ERR_BAD_ARG, "kba_track_solve: scale regulariser keyframe out of range");
+    track_desc(d, t, q);
     b->desc.h[0] = d;
     b->lc.max_rank = d.max_rank;
-    b->lc.fused_slots = ((planes ? 10 : 6) * n_free + 1 <= 176) ? 6 : 7;
+    b->lc.fused_slots = track_fused_slots(q);
     memcpy(t->sel_kf.h, kf_slot, n_kf * sizeof(int)); memcpy(t->sel_fixed.h, kf_fixed, n_kf);
     memcpy(t->sel_lm.h, lm_slot, n_lm * sizeof(int));
     if (sel->n_gp) {
         memcpy(b->r_gp_lm.h, sel->gp_lm, sel->n_gp * sizeof(int)); memcpy(b->gp_kf.h, sel->gp_kf, sel->n_gp * sizeof(int));
         memcpy(b->gp_weight.h, sel->gp_weight, sel->n_gp * sizeof(double));
     }
+    t->tdev.h[0] = t->td;  // the arena pointers as they are now (compaction moves them)
+    t->tsel.h[0] = track_sel(q, t->sel_kf.d, t->sel_fixed.d, t->sel_lm.d);
     CU(b->desc.upload(s));
     CU(cudaMemcpyAsync(t->sel_kf.d, t->sel_kf.h, n_kf * sizeof(int), cudaMemcpyHostToDevice, s));
     CU(cudaMemcpyAsync(t->sel_fixed.d, t->sel_fixed.h, n_kf, cudaMemcpyHostToDevice, s));
     CU(cudaMemcpyAsync(t->sel_lm.d, t->sel_lm.h, n_lm * sizeof(int), cudaMemcpyHostToDevice, s));
+    CU(t->tdev.upload(s)); CU(t->tsel.upload(s));
     if (sel->n_gp) { CU(b->r_gp_lm.upload(s)); CU(b->gp_kf.upload(s)); CU(b->gp_weight.upload(s)); }
-    t->h2d_solve = (int64_t)sizeof(WinDesc) + n_kf * 5 + n_lm * 4 + sel->n_gp * 16;
+    t->h2d_solve = (int64_t)sizeof(WinDesc) + n_kf * 5 + n_lm * 4 + sel->n_gp * 16 + (int64_t)(sizeof(TrackDev) + sizeof(TrackSel));
     // ---- gather the CSR from the store, pack, solve, write back
-    TrackSel ts;
-    ts.kf_slot = t->sel_kf.d; ts.kf_fixed = t->sel_fixed.d; ts.lm_slot = t->sel_lm.d; ts.n_kf = n_kf; ts.n_lm = n_lm; ts.max_meas = max_meas;
-    ts.auto_scale = sel->scale_weight < 0 ? 1 : 0;
-    launch_track_gather(b->bd, b->raw, t->td, ts, s);
+    TrackGrid grid;
+    grid.max_kf = n_kf; grid.max_lm = n_lm; grid.max_meas = q.max_meas;
+    launch_track_gather(b->bd, b->raw, t->tdev.d, t->tsel.d, grid, s);
     launch_pack(b->bd, b->raw, s);
     CU(cudaGetLastError());
     int rc = kba_batch_solve(b, opt);
     if (rc != KBA_OK) return rc;
-    launch_track_writeback(b->bd, t->td, ts, s);
+    launch_track_writeback(b->bd, t->tdev.d, t->tsel.d, grid, s);
     rc = kba_batch_download(b, res);
     t->d2h_solve = (int64_t)b->d2h_bytes;
     return rc;
@@ -1529,6 +1617,142 @@ int kba_track_transfer_bytes(kba_track* t, int64_t* h2d, int64_t* d2h, int64_t* 
     if (h2d) *h2d = t->h2d_solve;
     if (d2h) *d2h = t->d2h_solve;
     if (push) *push = t->h2d_push;
+    return KBA_OK;
+}
+
+// ---------------------------------------------------------------------------------------------------------------------
+// several persistent windows solved in one batch (include/kba_b200.h, kba_track_group_*)
+// ---------------------------------------------------------------------------------------------------------------------
+void kba_track_group_destroy(kba_track_group* g) {
+    if (!g) return;
+    cudaStreamSynchronize(g->h->stream);
+    if (g->batch) kba_batch_destroy(g->batch);
+    g->tdev.release(); g->tsel.release(); g->lists.release();
+    delete g;
+}
+
+int kba_track_group_create(kba_handle* h, int32_t n_tracks, kba_track* const* tracks, kba_track_group** out) {
+    if (!h || !tracks || !out || n_tracks < 1) return fail(KBA_ERR_BAD_ARG, "kba_track_group_create: empty group or null argument");
+    for (int i = 0; i < n_tracks; ++i) {
+        if (!tracks[i]) return fail(KBA_ERR_BAD_ARG, "kba_track_group_create: track " + std::to_string(i) + " is null");
+        if (tracks[i]->h != h) return fail(KBA_ERR_BAD_ARG, "kba_track_group_create: track " + std::to_string(i) + " belongs to another handle");
+        for (int j = 0; j < i; ++j)
+            if (tracks[j] == tracks[i])
+                return fail(KBA_ERR_BAD_ARG, "kba_track_group_create: track " + std::to_string(i) + " is also track " + std::to_string(j));
+    }
+    CU(cudaSetDevice(h->device));
+    // one capacity window per track: the group batch has, window for window, the shapes of the tracks' own batches
+    std::vector<std::unique_ptr<CapacityWindow>> cws;
+    std::vector<kba_window> ws;
+    size_t list_ints = 0;
+    for (int i = 0; i < n_tracks; ++i) {
+        const kba_track* t = tracks[i];
+        cws.emplace_back(new CapacityWindow(t->caps, t->n_cam, t->cam_intr.data(), t->cam_pose.data()));
+        ws.push_back(cws.back()->w);
+        list_ints += (size_t)t->caps.win_keyframes + t->caps.win_landmarks + (t->caps.win_keyframes + 3) / 4;
+    }
+    kba_track_group* g = new kba_track_group();
+    g->h = h;
+    g->tracks.assign(tracks, tracks + n_tracks);
+    const int rc = kba_batch_create(h, n_tracks, ws.data(), &g->batch);
+    if (rc != KBA_OK) { delete g; return rc; }
+    if (!g->batch->device_pack) { kba_track_group_destroy(g); return fail(KBA_ERR_CAPACITY, "kba_track_group_create: device packing is disabled (KBA_FUSED / KBA_DEVICE_PACK)"); }
+    int bad = 0;
+    bad |= g->tdev.alloc(n_tracks, true); bad |= g->tsel.alloc(n_tracks, true); bad |= g->lists.alloc(list_ints, true);
+    if (bad) { kba_track_group_destroy(g); return fail(KBA_ERR_CUDA, "kba_track_group_create: out of memory"); }
+    *out = g;
+    return KBA_OK;
+}
+
+int kba_track_group_solve(kba_track_group* g, const kba_track_request* req, const kba_options* opt, kba_result* res) {
+    if (!g || !req || !opt || !res) return fail(KBA_ERR_BAD_ARG, "null argument to kba_track_group_solve");
+    const int n = (int)g->tracks.size();
+    // ---- every request is checked before anything is uploaded or launched
+    std::vector<TrackRequest> qs(n);
+    int active = 0;
+    for (int i = 0; i < n; ++i) {
+        const kba_track_request& r = req[i];
+        if (r.n_kf == 0) continue;  // sits this solve out
+        TrackRequest& q = qs[i];
+        q.n_kf = r.n_kf; q.kf_slot = r.kf_slot; q.kf_fixed = r.kf_fixed; q.n_lm = r.n_lm; q.lm_slot = r.lm_slot; q.sel = r.sel;
+        std::string why;
+        const int rc = track_check(g->tracks[i], q, why);
+        if (rc != KBA_OK) return fail(rc, "kba_track_group_solve: track " + std::to_string(i) + ": " + why);
+        ++active;
+    }
+    if (active == 0) {  // nothing to solve: no upload, no launch, every result idle
+        for (int i = 0; i < n; ++i) {
+            kba_result& r = res[i];
+            r.num_iteration_records = 0; r.num_solves = 0; r.status = KBA_OK;
+            r.initial_cost = 0.0; r.final_cost = 0.0; r.time_sec = 0.0;
+        }
+        g->h2d_solve = 0; g->d2h_solve = 0;
+        return KBA_OK;
+    }
+    kba_batch* b = g->batch;
+    CU(cudaSetDevice(g->h->device));
+    cudaStream_t s = g->h->stream;
+    // ---- descriptors, selection lists (one pinned buffer), track stores as they are now
+    int max_rank = 0, slots = 6;
+    bool any_gp = false;
+    TrackGrid grid;
+    size_t used = 0;
+    int64_t h2d = (int64_t)n * (int64_t)(sizeof(WinDesc) + sizeof(TrackDev) + sizeof(TrackSel));
+    for (int i = 0; i < n; ++i) {
+        const kba_track* t = g->tracks[i];
+        const TrackRequest& q = qs[i];
+        WinDesc& d = b->desc_h[i];
+        g->tdev.h[i] = t->td;  // compaction re-points a track's arena: read at every solve
+        if (!q.sel) {
+            idle_desc(d);
+            g->tsel.h[i] = TrackSel{};
+        } else {
+            track_desc(d, t, q);
+            max_rank = std::max(max_rank, d.max_rank);
+            slots = std::max(slots, track_fused_slots(q));
+            int* l = g->lists.h + used;
+            memcpy(l, q.kf_slot, q.n_kf * sizeof(int));
+            memcpy(l + q.n_kf, q.lm_slot, q.n_lm * sizeof(int));
+            memcpy(l + q.n_kf + q.n_lm, q.kf_fixed, q.n_kf);
+            const int* ld = g->lists.d + used;
+            g->tsel.h[i] = track_sel(q, ld, reinterpret_cast<const uint8_t*>(ld + q.n_kf + q.n_lm), ld + q.n_kf);
+            used += (size_t)q.n_kf + q.n_lm + (q.n_kf + 3) / 4;
+            const kba_window* sel = q.sel;
+            if (sel->n_gp) {
+                memcpy(b->r_gp_lm.h + d.gp_off, sel->gp_lm, sel->n_gp * sizeof(int)); memcpy(b->gp_kf.h + d.gp_off, sel->gp_kf, sel->n_gp * sizeof(int));
+                memcpy(b->gp_weight.h + d.gp_off, sel->gp_weight, sel->n_gp * sizeof(double));
+                any_gp = true;
+            }
+            grid.max_kf = std::max(grid.max_kf, q.n_kf); grid.max_lm = std::max(grid.max_lm, q.n_lm);
+            grid.max_meas = std::max(grid.max_meas, q.max_meas);
+            h2d += (int64_t)q.n_kf * 5 + (int64_t)q.n_lm * 4 + (int64_t)sel->n_gp * 16;
+        }
+        b->desc.h[i] = d;
+    }
+    // one launch configuration for the whole group, as kba_batch_solve has for any batch
+    b->lc.max_rank = max_rank;
+    b->lc.fused_slots = slots;
+    CU(b->desc.upload(s));
+    CU(cudaMemcpyAsync(g->lists.d, g->lists.h, used * sizeof(int), cudaMemcpyHostToDevice, s));
+    CU(g->tdev.upload(s)); CU(g->tsel.upload(s));
+    if (any_gp) { CU(b->r_gp_lm.upload(s)); CU(b->gp_kf.upload(s)); CU(b->gp_weight.upload(s)); }
+    g->h2d_solve = h2d;
+    // ---- gather every window from its store, pack, solve, write back
+    launch_track_gather(b->bd, b->raw, g->tdev.d, g->tsel.d, grid, s);
+    launch_pack(b->bd, b->raw, s);
+    CU(cudaGetLastError());
+    int rc = kba_batch_solve(b, opt);
+    if (rc != KBA_OK) return rc;
+    launch_track_writeback(b->bd, g->tdev.d, g->tsel.d, grid, s);
+    rc = kba_batch_download(b, res);
+    g->d2h_solve = (int64_t)b->d2h_bytes;
+    return rc;
+}
+
+int kba_track_group_transfer_bytes(kba_track_group* g, int64_t* h2d, int64_t* d2h) {
+    if (!g) return fail(KBA_ERR_BAD_ARG, "null track group");
+    if (h2d) *h2d = g->h2d_solve;
+    if (d2h) *d2h = g->d2h_solve;
     return KBA_OK;
 }
 

@@ -26,7 +26,9 @@ struct WinDesc {
     double scale_weight, scale_value;
     double plane_reg_weight;
     int plane_dist_fixed, landmarks_fixed;
-    int speed_kf, pad0;
+    int speed_kf;
+    int idle;                                       // 1: the window sits this solve out (k_reset_state: PH_DONE at once);
+                                                    //    set only by kba_track_group_solve
     double speed_weight, speed_dt;
     double speed_v_before[3];
     double speed_T_origin_before[7];

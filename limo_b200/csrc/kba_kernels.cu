@@ -2261,7 +2261,7 @@ __global__ void k_reset_state(BatchDev bd, int rounds_total_override, int min_la
     for (int i = threadIdx.x; i < wd.n_lm; i += blockDim.x) bd.lm_active[wd.lm_off + i] = 1;
     if (threadIdx.x == 0) {
         WinState& st = bd.state[w];
-        st.phase = PH_SOLVE_BEGIN;
+        st.phase = wd.idle ? PH_DONE : PH_SOLVE_BEGIN;  // an idle window (kba_track_group_solve) never iterates: no solve, no log
         st.cur = 0;
         st.solve_index = 0; st.round = 0; st.retried = 0; st.log_n = 0; st.n_solves = 0;
         int rounds = rounds_total_override;

@@ -88,15 +88,20 @@ struct TrackSel {
     const int* kf_slot = nullptr;    // [n_kf] ascending keyframe id
     const unsigned char* kf_fixed = nullptr;
     const int* lm_slot = nullptr;    // [n_lm] ascending landmark id
-    int n_kf = 0, n_lm = 0, max_meas = 0;
+    int n_kf = 0, n_lm = 0, max_meas = 0;  // n_kf = n_lm = 0: the window is idle (WinDesc::idle)
     int auto_scale = 0;              // 1: scale-regulariser weight by the reference rule (cpp:703-716) from the gathered window
 };
-// builds the window's raw CSR (PackRaw inputs of batch `bd`, window 0) from the track store; returns nothing: desc[0].n_obs
-// is written on the device
-void launch_track_gather(const BatchDev& bd, const PackRaw& raw_out, const TrackDev& td, const TrackSel& sel, cudaStream_t s);
+// grid sizes of the gather / write-back launches: maxima over the windows of the batch
+struct TrackGrid {
+    int max_kf = 0, max_lm = 0, max_meas = 0;
+};
+// builds the raw CSR of every window w of batch `bd` (its PackRaw inputs) from track store tds[w] and selection sels[w]
+// (device arrays of bd.n_win entries); desc[w].n_obs is written on the device
+void launch_track_gather(const BatchDev& bd, const PackRaw& raw_out, const TrackDev* tds, const TrackSel* sels, const TrackGrid& g,
+                         cudaStream_t s);
 void launch_scatter_rows(double* dst, const int* slot, const double* src, int n, int width, cudaStream_t s);
-// results of window 0 back into the track store
-void launch_track_writeback(const BatchDev& bd, const TrackDev& td, const TrackSel& sel, cudaStream_t s);
+// results of every window w back into track store tds[w]
+void launch_track_writeback(const BatchDev& bd, const TrackDev* tds, const TrackSel* sels, const TrackGrid& g, cudaStream_t s);
 
 cudaError_t configure_pack();
 int pack_max_landmarks();

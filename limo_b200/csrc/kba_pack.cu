@@ -211,21 +211,32 @@ __global__ void __launch_bounds__(256) k_unpack_landmarks(BatchDev bd, double* l
 // =====================================================================================================================
 // persistent window (kba_track_*): the window's raw CSR is gathered on the device from the measurement arena
 // =====================================================================================================================
-__global__ void __launch_bounds__(256) k_track_begin(BatchDev bd, PackRaw raw, TrackDev td, TrackSel sel, double* r_lm_pos,
+// Every kernel takes window w of the batch from its grid (blockIdx.y, or .z where .y is taken) and that window's track store
+// tds[w] and selection sels[w]: one window for kba_track_solve, one per track for kba_track_group_solve.  Writes go through
+// desc[w]'s offsets; the per-track scratch (sel_index, cursor, key, n_depth) is indexed window-locally -- a track is in a batch
+// at most once, so no two windows share it.  An idle window (a track sitting a group solve out) has empty selections.
+__global__ void __launch_bounds__(256) k_track_begin(BatchDev bd, const TrackDev* tds, const TrackSel* sels, double* r_lm_pos,
                                                      double* r_lm_weight, int* r_cnt) {
+    const int w = blockIdx.y;
+    const WinDesc& wd = bd.desc[w];
+    if (wd.idle) return;
+    const TrackDev& td = tds[w];
+    const TrackSel& sel = sels[w];
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i < sel.n_kf) {
         const int slot = sel.kf_slot[i];
-        for (int q = 0; q < 7; ++q) bd.pose0[7 * i + q] = td.kf_pose[7 * (size_t)slot + q];
-        for (int q = 0; q < 4; ++q) bd.plane0[4 * i + q] = td.kf_plane[4 * (size_t)slot + q];
-        bd.kf_fixed[i] = sel.kf_fixed[i];
+        const size_t k = (size_t)wd.kf_off + i;
+        for (int q = 0; q < 7; ++q) bd.pose0[7 * k + q] = td.kf_pose[7 * (size_t)slot + q];
+        for (int q = 0; q < 4; ++q) bd.plane0[4 * k + q] = td.kf_plane[4 * (size_t)slot + q];
+        bd.kf_fixed[k] = sel.kf_fixed[i];
     }
     if (i < sel.n_lm) {
         const int slot = sel.lm_slot[i];
+        const size_t L = (size_t)wd.lm_off + i;
         td.sel_index[slot] = i;
-        for (int q = 0; q < 3; ++q) r_lm_pos[3 * (size_t)i + q] = td.lm_pos[3 * (size_t)slot + q];
-        r_lm_weight[i] = td.lm_weight[slot];
-        r_cnt[i] = 0;
+        for (int q = 0; q < 3; ++q) r_lm_pos[3 * L + q] = td.lm_pos[3 * (size_t)slot + q];
+        r_lm_weight[L] = td.lm_weight[slot];
+        r_cnt[L] = 0;
         td.cursor[i] = 0;
     }
     if (i == 0) *td.n_depth = 0;
@@ -233,33 +244,47 @@ __global__ void __launch_bounds__(256) k_track_begin(BatchDev bd, PackRaw raw, T
 
 // pass 0: observations per selected landmark; pass 1: scatter behind the CSR pointers (order fixed afterwards by k_track_sort)
 template <int kPass>
-__global__ void __launch_bounds__(256) k_track_scatter(PackRaw raw, TrackDev td, TrackSel sel, int* r_cnt, int* r_kf, int* r_cam,
-                                                       float* r_u, float* r_v, float* r_d) {
-    const int k = blockIdx.y;
+__global__ void __launch_bounds__(256) k_track_scatter(BatchDev bd, PackRaw raw, const TrackDev* tds, const TrackSel* sels, int* r_cnt,
+                                                       int* r_kf, int* r_cam, float* r_u, float* r_v, float* r_d) {
+    const int w = blockIdx.z, k = blockIdx.y;
+    const TrackSel& sel = sels[w];
+    if (k >= sel.n_kf) return;
+    const TrackDev& td = tds[w];
+    const WinDesc& wd = bd.desc[w];
+    const int* lp = raw.lm_ptr + wd.lm_off + w;
+    int* cnt = r_cnt + wd.lm_off;
+    const size_t ob = (size_t)wd.obs_off;
     const int slot = sel.kf_slot[k];
     const int n = td.m_cnt[slot], m0 = td.m_off[slot];
     for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
         const int j = td.sel_index[td.m_lm[m0 + i]];
         if (j < 0) continue;
         if (kPass == 0) {
-            atomicAdd(&r_cnt[j], 1);
+            atomicAdd(&cnt[j], 1);
             if (td.m_d[m0 + i] > 0.0f) atomicAdd(td.n_depth, 1);
             continue;
         }
-        const int pos = raw.lm_ptr[j] + atomicAdd(&td.cursor[j], 1);
-        r_kf[pos] = k; r_cam[pos] = td.m_cam[m0 + i];
-        r_u[pos] = td.m_u[m0 + i]; r_v[pos] = td.m_v[m0 + i]; r_d[pos] = td.m_d[m0 + i];
+        const int pos = lp[j] + atomicAdd(&td.cursor[j], 1);
+        r_kf[ob + pos] = k; r_cam[ob + pos] = td.m_cam[m0 + i];
+        r_u[ob + pos] = td.m_u[m0 + i]; r_v[ob + pos] = td.m_v[m0 + i]; r_d[ob + pos] = td.m_d[m0 + i];
         td.key[pos] = ((long long)k << 32) | (long long)(m0 + i);
     }
 }
 
-__global__ void __launch_bounds__(1024) k_track_scan(BatchDev bd, TrackDev td, TrackSel sel, const int* r_cnt, int* r_lm_ptr) {
+// one CTA per window: CSR pointers of the gathered window, its observation count and, when asked, the scale-regulariser rule
+__global__ void __launch_bounds__(1024) k_track_scan(BatchDev bd, const TrackDev* tds, const TrackSel* sels, const int* r_cnt, int* r_lm_ptr) {
+    const int w = blockIdx.x;
+    WinDesc& d = bd.desc[w];
+    if (d.idle) return;
     __shared__ int s_scan[1024];
+    const TrackSel& sel = sels[w];
+    const int* cnt = r_cnt + d.lm_off;
+    int* lp = r_lm_ptr + d.lm_off + w;
     const int tid = threadIdx.x, nth = blockDim.x, n = sel.n_lm;
     int carry = 0;
     for (int c0 = 0; c0 < n; c0 += nth) {
         const int j = c0 + tid;
-        s_scan[tid] = j < n ? r_cnt[j] : 0;
+        s_scan[tid] = j < n ? cnt[j] : 0;
         __syncthreads();
         for (int off = 1; off < nth; off <<= 1) {
             const int v = tid >= off ? s_scan[tid - off] : 0;
@@ -267,17 +292,16 @@ __global__ void __launch_bounds__(1024) k_track_scan(BatchDev bd, TrackDev td, T
             s_scan[tid] += v;
             __syncthreads();
         }
-        if (j < n) r_lm_ptr[j + 1] = carry + s_scan[tid];
+        if (j < n) lp[j + 1] = carry + s_scan[tid];
         const int tot = s_scan[nth - 1];
         __syncthreads();
         carry += tot;
     }
     if (tid == 0) {
-        r_lm_ptr[0] = 0;
-        WinDesc& d = bd.desc[0];
+        lp[0] = 0;
         d.n_obs = carry;
         if (sel.auto_scale) {  // addScaleRegularization's weight (bundle_adjuster_keyframes.cpp:703-716) and the plane-distance rule (:722-728)
-            const int n_depth = *td.n_depth, n_gp = d.n_gp;
+            const int n_depth = *tds[w].n_depth, n_gp = d.n_gp;
             double wgt = 1000.0;
             if (n_depth > 10 || n_gp > 10) wgt = (n_gp < 30) ? 1000.0 / ((double)n_depth + (double)n_gp) : 0.0;
             d.scale_weight = wgt;
@@ -287,11 +311,18 @@ __global__ void __launch_bounds__(1024) k_track_scan(BatchDev bd, TrackDev td, T
 }
 
 // a landmark's observations in (keyframe, arena) order = (keyframe, camera id) order of the caller: insertion sort, <= a few dozen
-__global__ void __launch_bounds__(256) k_track_sort(TrackDev td, TrackSel sel, const int* r_lm_ptr, int* r_kf, int* r_cam, float* r_u,
-                                                    float* r_v, float* r_d) {
+__global__ void __launch_bounds__(256) k_track_sort(BatchDev bd, const TrackDev* tds, const TrackSel* sels, const int* r_lm_ptr, int* r_kf,
+                                                    int* r_cam, float* r_u, float* r_v, float* r_d) {
+    const int w = blockIdx.y;
+    const TrackSel& sel = sels[w];
     const int j = blockIdx.x * blockDim.x + threadIdx.x;
     if (j >= sel.n_lm) return;
-    const int o0 = r_lm_ptr[j], o1 = r_lm_ptr[j + 1];
+    const TrackDev& td = tds[w];
+    const WinDesc& wd = bd.desc[w];
+    const size_t ob = (size_t)wd.obs_off;
+    r_kf += ob; r_cam += ob; r_u += ob; r_v += ob; r_d += ob;
+    const int* lp = r_lm_ptr + wd.lm_off + w;
+    const int o0 = lp[j], o1 = lp[j + 1];
     for (int a = o0 + 1; a < o1; ++a) {
         const long long key = td.key[a];
         const int kf = r_kf[a], cam = r_cam[a];
@@ -307,17 +338,24 @@ __global__ void __launch_bounds__(256) k_track_sort(TrackDev td, TrackSel sel, c
     td.sel_index[sel.lm_slot[j]] = -1;  // restore the all -1 state for the next solve
 }
 
-__global__ void __launch_bounds__(256) k_track_writeback(BatchDev bd, TrackDev td, TrackSel sel) {
+__global__ void __launch_bounds__(256) k_track_writeback(BatchDev bd, const TrackDev* tds, const TrackSel* sels) {
+    const int w = blockIdx.y;
+    const TrackSel& sel = sels[w];
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    const int cur = bd.state[0].cur;
+    if (i >= sel.n_kf && i >= sel.n_lm) return;
+    const TrackDev& td = tds[w];
+    const WinDesc& wd = bd.desc[w];
+    const int cur = bd.state[w].cur;
     if (i < sel.n_kf) {
         const int slot = sel.kf_slot[i];
-        for (int q = 0; q < 7; ++q) td.kf_pose[7 * (size_t)slot + q] = bd.pose[cur][7 * i + q];
-        for (int q = 0; q < 4; ++q) td.kf_plane[4 * (size_t)slot + q] = bd.plane[cur][4 * i + q];
+        const size_t k = (size_t)wd.kf_off + i;
+        for (int q = 0; q < 7; ++q) td.kf_pose[7 * (size_t)slot + q] = bd.pose[cur][7 * k + q];
+        for (int q = 0; q < 4; ++q) td.kf_plane[4 * (size_t)slot + q] = bd.plane[cur][4 * k + q];
     }
     if (i < sel.n_lm) {  // i: sorted position
-        const int slot = sel.lm_slot[bd.lm_orig[i]];
-        for (int q = 0; q < 3; ++q) td.lm_pos[3 * (size_t)slot + q] = bd.lm[cur][3 * (size_t)i + q];
+        const size_t L = (size_t)wd.lm_off + i;
+        const int slot = sel.lm_slot[bd.lm_orig[L]];
+        for (int q = 0; q < 3; ++q) td.lm_pos[3 * (size_t)slot + q] = bd.lm[cur][3 * L + q];
     }
 }
 
@@ -333,25 +371,29 @@ void launch_scatter_rows(double* dst, const int* slot, const double* src, int n,
     LCHK("k_scatter_rows");
 }
 
-void launch_track_gather(const BatchDev& bd, const PackRaw& raw, const TrackDev& td, const TrackSel& sel, cudaStream_t s) {
+void launch_track_gather(const BatchDev& bd, const PackRaw& raw, const TrackDev* tds, const TrackSel* sels, const TrackGrid& g,
+                         cudaStream_t s) {
     // the PackRaw pointers are const views of buffers this batch owns: the gather is what fills them
     int* r_lm_ptr = const_cast<int*>(raw.lm_ptr);
     int* r_kf = const_cast<int*>(raw.obs_kf); int* r_cam = const_cast<int*>(raw.obs_cam);
     float* r_u = const_cast<float*>(raw.obs_u); float* r_v = const_cast<float*>(raw.obs_v); float* r_d = const_cast<float*>(raw.obs_d);
     double* r_pos = const_cast<double*>(raw.lm_pos); double* r_w = const_cast<double*>(raw.lm_weight);
     int* r_cnt = raw.lm_inv;  // scratch until the packing kernels overwrite it
-    const int n = sel.n_kf > sel.n_lm ? sel.n_kf : sel.n_lm;
-    k_track_begin<<<(n + 255) / 256, 256, 0, s>>>(bd, raw, td, sel, r_pos, r_w, r_cnt); LCHK("k_track_begin");
-    const dim3 gm((sel.max_meas + 255) / 256 > 0 ? (sel.max_meas + 255) / 256 : 1, sel.n_kf);
-    k_track_scatter<0><<<gm, 256, 0, s>>>(raw, td, sel, r_cnt, r_kf, r_cam, r_u, r_v, r_d); LCHK("k_track_scatter");
-    k_track_scan<<<1, 1024, 0, s>>>(bd, td, sel, r_cnt, r_lm_ptr); LCHK("k_track_scan");
-    k_track_scatter<1><<<gm, 256, 0, s>>>(raw, td, sel, r_cnt, r_kf, r_cam, r_u, r_v, r_d); LCHK("k_track_scatter");
-    k_track_sort<<<(sel.n_lm + 255) / 256, 256, 0, s>>>(td, sel, r_lm_ptr, r_kf, r_cam, r_u, r_v, r_d); LCHK("k_track_sort");
+    const int B = bd.n_win;
+    const int n = g.max_kf > g.max_lm ? g.max_kf : g.max_lm;
+    k_track_begin<<<dim3((n + 255) / 256 > 0 ? (n + 255) / 256 : 1, B), 256, 0, s>>>(bd, tds, sels, r_pos, r_w, r_cnt); LCHK("k_track_begin");
+    const dim3 gm((g.max_meas + 255) / 256 > 0 ? (g.max_meas + 255) / 256 : 1, g.max_kf > 0 ? g.max_kf : 1, B);
+    k_track_scatter<0><<<gm, 256, 0, s>>>(bd, raw, tds, sels, r_cnt, r_kf, r_cam, r_u, r_v, r_d); LCHK("k_track_scatter");
+    k_track_scan<<<B, 1024, 0, s>>>(bd, tds, sels, r_cnt, r_lm_ptr); LCHK("k_track_scan");
+    k_track_scatter<1><<<gm, 256, 0, s>>>(bd, raw, tds, sels, r_cnt, r_kf, r_cam, r_u, r_v, r_d); LCHK("k_track_scatter");
+    k_track_sort<<<dim3((g.max_lm + 255) / 256 > 0 ? (g.max_lm + 255) / 256 : 1, B), 256, 0, s>>>(bd, tds, sels, r_lm_ptr, r_kf, r_cam, r_u,
+                                                                                                r_v, r_d);
+    LCHK("k_track_sort");
 }
 
-void launch_track_writeback(const BatchDev& bd, const TrackDev& td, const TrackSel& sel, cudaStream_t s) {
-    const int n = sel.n_kf > sel.n_lm ? sel.n_kf : sel.n_lm;
-    k_track_writeback<<<(n + 255) / 256, 256, 0, s>>>(bd, td, sel); LCHK("k_track_writeback");
+void launch_track_writeback(const BatchDev& bd, const TrackDev* tds, const TrackSel* sels, const TrackGrid& g, cudaStream_t s) {
+    const int n = g.max_kf > g.max_lm ? g.max_kf : g.max_lm;
+    k_track_writeback<<<dim3((n + 255) / 256 > 0 ? (n + 255) / 256 : 1, bd.n_win), 256, 0, s>>>(bd, tds, sels); LCHK("k_track_writeback");
 }
 
 cudaError_t configure_pack() {
