@@ -343,6 +343,43 @@ int kba_track_group_solve(kba_track_group* g, const kba_track_request* req, cons
 /* upload / download of the last group solve, counted as kba_track_transfer_bytes counts them */
 int kba_track_group_transfer_bytes(kba_track_group* g, int64_t* h2d_last_solve, int64_t* d2h_last_solve);
 
+/* ---- adjustPoseOnly against the persistent store: one frame's pose per call, or one frame of each track of a group -------
+ * What limo calls on every frame (bundle_adjuster_keyframes.cpp:820-888): one free pose against constant landmarks, the optional
+ * SpeedRegularizationVector2 prior and the trimming rounds.  The result is that of kba_solve_window on the equivalent window: one
+ * keyframe (kf_fixed 0) at pose7, the frame's measurements as its observations in the caller's landmark order, landmark positions
+ * and weights read from the store by slot, landmarks_fixed = 1, no ground plane, no scale or plane regulariser.
+ *   - The frame is solved by ONE kernel (one CTA, the whole trimmed solve): a call makes one upload, one launch, one download
+ *     and one synchronisation, and allocates nothing after the first call of its track (group), which allocates the buffers for
+ *     the track's (group's) win_landmarks / win_observations.
+ *   - Validation, before anything is uploaded: null pointers, negative sizes, a slot or camera out of range, a slot that
+ *     reappears after its run has ended: KBA_ERR_BAD_ARG; more than win_observations measurements or more than win_landmarks
+ *     runs: KBA_ERR_CAPACITY; kba_options.precision != 0: KBA_ERR_BAD_ARG (FP64 only).  As for kba_solve_window: a speed prior
+ *     with speed_dt <= 0 is KBA_ERR_BAD_ARG, more than 6 trimming rounds (num_trim_rounds, or num_rounds_option when it is -1)
+ *     KBA_ERR_CAPACITY.  A group checks every frame first and
+ *     returns the failing frame's code, kba_last_error names its track index.
+ *   - Results: res->kf_pose [7], res->lm_rejected [number of runs, in run order], the summaries, the iteration log and
+ *     time_sec (the kernel's device time).  lm_pos and kf_plane are not written: the store is never modified, the frame is not
+ *     a keyframe.  kba_track_transfer_bytes (kba_track_group_transfer_bytes) then report this call's upload and download.
+ *   - Trimming: opt->num_trim_rounds as given; -1 = the reference rule on the frame's landmark count against
+ *     min_landmarks_for_trimming (30 for adjustPoseOnly, cpp:865).  solver_time_sec is applied per inner solve on the device.
+ *   - n_meas == 0: the frame sits the call out (res status KBA_OK, num_solves 0, nothing written). */
+typedef struct kba_track_frame {
+    int32_t n_meas;             /* 0: this frame sits the call out (res status KBA_OK, num_solves 0, nothing written) */
+    int32_t reserved_;
+    const double* pose7;        /* initial pose of the frame, 7-vector convention */
+    const int32_t* lm_slot;     /* [n_meas] store slots; one contiguous run per landmark, runs in the caller's landmark order
+                                   (ascending id, as selected_landmark_ids_ ∩ measurements_), cameras ascending inside a run */
+    const int32_t* cam;         /* [n_meas] or NULL (all camera 0) */
+    const float* u, *v, *d;     /* [n_meas] FeaturePoint; depth residual iff d > 0 */
+    double speed_weight;        /* SpeedRegularizationVector2 exactly as kba_window's speed_* fields; <= 0: none */
+    double speed_dt;
+    double speed_v_before[3];
+    double speed_T_origin_before[7];
+} kba_track_frame;
+int kba_track_adjust_pose(kba_track* t, const kba_track_frame* f, const kba_options* opt, kba_result* res);
+/* f[n_tracks], res[n_tracks]: frame i is tracked against track i's store, all frames in one launch */
+int kba_track_group_adjust_pose(kba_track_group* g, const kba_track_frame* f, const kba_options* opt, kba_result* res);
+
 /* ---- landmark initialisation of push() for a whole window (SURVEY 8(f) row 2) ------------------------------------------
  * Replaces, for all landmarks of `w` at once, what BundleAdjusterKeyframes::push() does per new landmark on the host:
  * the first observation with a lidar depth (d >= 0) is back-projected (bundle_adjuster_keyframes.cpp:332-355); without

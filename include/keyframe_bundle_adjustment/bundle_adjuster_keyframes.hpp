@@ -19,6 +19,7 @@
 
 struct kba_handle;
 struct kba_track;
+struct kba_window;
 
 namespace keyframe_bundle_adjustment {
 
@@ -74,6 +75,8 @@ public:
     // the lists of active keyframes / selected landmarks instead of re-packing and re-uploading the window (the reference
     // rebuilds its ceres::Problem per call, cpp:635-637).  On by default; windows the device-resident store cannot take (more than
     // 30 keyframes, ground-plane residuals, a camera that was not there at the first push) fall back to the rebuild path.
+    // adjustPoseOnly() then tracks the frame against the landmarks in that store (kba_track_adjust_pose) when the store has every
+    // landmark and camera of the frame, and otherwise rebuilds its one-keyframe window.
     void set_persistent_window(bool on) { persistent_window_ = on; }
     // host -> device bytes of the last solve() (either path) and of all push() calls so far (persistent path)
     long long lastSolveUploadBytes() const { return last_solve_h2d_; }
@@ -101,6 +104,9 @@ private:
     bool ensureHandle();
     bool trackPush(const Keyframe& kf);
     bool solveTracked(const std::vector<Keyframe*>& kfs, const std::vector<LandmarkId>& lm_ids, std::string& report);
+    bool adjustPoseTracked(Keyframe& kf, const std::vector<LandmarkId>& lm_ids, std::string& report);
+    bool flushLandmarks();  // new and dirty landmark state into the store, before any use of the track
+    void speedPrior(const Keyframe& speed_kf, kba_window& w) const;
     kba_track* track_{nullptr};
     bool persistent_window_{true}, track_failed_{false};
     std::map<KeyframeId, int> kf_slot_;
@@ -108,6 +114,7 @@ private:
     std::vector<int> free_kf_slots_;
     std::vector<std::array<double, 10>> track_cams_;  // camera values (f, pp, pose_camera_vehicle) the track was created with
     std::set<LandmarkId> new_landmarks_, dirty_weights_;
+    std::set<LandmarkId> dirty_positions_;  // positions the rebuild path wrote on the host only
     long long last_solve_h2d_{0}, push_h2d_{0};
 };
 

@@ -8,8 +8,8 @@ import os
 
 import numpy as np
 
-from .capi_types import (KbaCounters, KbaEvalOut, KbaLidarOptions, KbaOptions, KbaResult, KbaTrackCaps, KbaTrackRequest, KbaWindow,
-                         Result, Window, c_double_p, c_int32_p)
+from .capi_types import (KbaCounters, KbaEvalOut, KbaLidarOptions, KbaOptions, KbaResult, KbaTrackCaps, KbaTrackFrame, KbaTrackRequest,
+                         KbaWindow, Result, Window, c_double_p, c_int32_p)
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("KBA_LIB_PATH") or os.path.join(_HERE, "libkba_b200.so")  # KBA_LIB_PATH: instrumented builds
@@ -22,7 +22,8 @@ SYMBOLS = ["kba_version", "kba_last_error", "kba_default_options", "kba_create",
            "kba_shard_unique_id", "kba_shard_comm_create", "kba_shard_comm_destroy", "kba_batch_set_shard",
            "kba_init_landmarks", "kba_track_create", "kba_track_destroy", "kba_track_push_keyframe", "kba_track_drop_keyframe",
            "kba_track_set_landmarks", "kba_track_set_keyframe_pose", "kba_track_set_keyframe_poses", "kba_track_solve", "kba_track_transfer_bytes",
-           "kba_track_group_create", "kba_track_group_destroy", "kba_track_group_solve", "kba_track_group_transfer_bytes"]
+           "kba_track_group_create", "kba_track_group_destroy", "kba_track_group_solve", "kba_track_group_transfer_bytes",
+           "kba_track_adjust_pose", "kba_track_group_adjust_pose"]
 
 
 class KbaError(RuntimeError):
@@ -80,6 +81,8 @@ def lib():
         L.kba_track_group_destroy.restype = None
         L.kba_track_group_solve.argtypes = [vp, C.POINTER(KbaTrackRequest), C.POINTER(KbaOptions), C.POINTER(KbaResult)]
         L.kba_track_group_transfer_bytes.argtypes = [vp, C.POINTER(C.c_int64), C.POINTER(C.c_int64)]
+        L.kba_track_adjust_pose.argtypes = [vp, C.POINTER(KbaTrackFrame), C.POINTER(KbaOptions), C.POINTER(KbaResult)]
+        L.kba_track_group_adjust_pose.argtypes = [vp, C.POINTER(KbaTrackFrame), C.POINTER(KbaOptions), C.POINTER(KbaResult)]
         L.kba_lidar_default_options.argtypes = [C.POINTER(KbaLidarOptions)]
         L.kba_lidar_default_options.restype = None
         fp = C.POINTER(C.c_float)
@@ -226,6 +229,46 @@ class Track:
                                      lm.ctypes.data_as(c_int32_p), C.byref(sel.c), C.byref(opt or default_options()), C.byref(res.c)))
         return res
 
+    @staticmethod
+    def _frame(fr, pose7, lm_slot, u, v, d, cam=None, speed=None):
+        """fill KbaTrackFrame `fr`; returns the arrays it points into (keep them alive for the call) and the frame's run count.
+        speed: None or a dict weight, dt, v_before (3), T_origin_before (7) -- the speed_* fields of a window"""
+        f32 = lambda a: np.ascontiguousarray(a, dtype=np.float32)
+        pose = np.ascontiguousarray(pose7, dtype=np.float64).reshape(7)
+        lm, lmp = Track._i32(lm_slot)
+        uu, vv, dd = f32(u), f32(v), f32(d)
+        cm = None if cam is None else Track._i32(cam)[0]
+        fr.n_meas = len(lm)
+        fr.pose7 = pose.ctypes.data_as(c_double_p)
+        fr.lm_slot = lmp
+        fr.cam = C.cast(None, c_int32_p) if cm is None else cm.ctypes.data_as(c_int32_p)
+        fp = C.POINTER(C.c_float)
+        fr.u, fr.v, fr.d = uu.ctypes.data_as(fp), vv.ctypes.data_as(fp), dd.ctypes.data_as(fp)
+        if speed:
+            fr.speed_weight, fr.speed_dt = float(speed["weight"]), float(speed["dt"])
+            fr.speed_v_before = (C.c_double * 3)(*[float(x) for x in speed["v_before"]])
+            fr.speed_T_origin_before = (C.c_double * 7)(*[float(x) for x in speed["T_origin_before"]])
+        else:
+            fr.speed_weight, fr.speed_dt = 0.0, 1.0
+        n_runs = int(1 + np.count_nonzero(lm[1:] != lm[:-1])) if len(lm) else 0
+        return (pose, lm, uu, vv, dd, cm), n_runs
+
+    @staticmethod
+    def _frame_result(n_runs, iterations_capacity):
+        sel = Window(np.tile([1.0, 0, 0, 0, 0, 0, 0], (1, 1)), [0], [[1.0, 0, 0]], [[1.0, 0, 0, 0, 0, 0, 0]], np.zeros((n_runs, 3)),
+                     np.ones(n_runs), np.zeros(n_runs + 1, dtype=np.int32), [], [], [], [])
+        return Result(sel, iterations_capacity)
+
+    def adjust_pose(self, pose7, lm_slot, u, v, d, cam=None, speed=None, opt=None, iterations_capacity=256):
+        """adjustPoseOnly of one frame against this track's store (kba_track_adjust_pose): one free pose, landmarks read by slot
+        (lm_slot: one contiguous run per landmark, in the caller's landmark order).  Returns a Result: kf_pose [1, 7],
+        lm_rejected [runs], summaries and iterations; the store is not modified."""
+        fr = KbaTrackFrame()
+        keep, n_runs = self._frame(fr, pose7, lm_slot, u, v, d, cam, speed)
+        res = self._frame_result(n_runs, iterations_capacity)
+        _check(lib().kba_track_adjust_pose(self._p, C.byref(fr), C.byref(opt or default_options()), C.byref(res.c)))
+        return res
+
     def transfer_bytes(self):
         a, b, c = C.c_int64(), C.c_int64(), C.c_int64()
         _check(lib().kba_track_transfer_bytes(self._p, C.byref(a), C.byref(b), C.byref(c)))
@@ -268,6 +311,26 @@ class TrackGroup:
             results.append(Result(sel, iterations_capacity))
         rarr = (KbaResult * len(results))(*[r.c for r in results])
         _check(lib().kba_track_group_solve(self._p, reqs, C.byref(opt or default_options()), rarr))
+        for r, c in zip(results, rarr):
+            r.c = c
+        return results
+
+    def adjust_pose(self, frames, opt=None, iterations_capacity=256):
+        """one frame per track in one launch (kba_track_group_adjust_pose): each entry None (the track sits the call out) or a
+        dict with the arguments of Track.adjust_pose (pose7, lm_slot, u, v, d, cam, speed).  Returns one Result per track."""
+        assert len(frames) == len(self.tracks)
+        arr = (KbaTrackFrame * len(frames))()
+        keep, results = [], []
+        for i, fr in enumerate(frames):
+            if fr is None:
+                arr[i].n_meas = 0
+                results.append(Track._frame_result(0, 1))
+                continue
+            k, n_runs = Track._frame(arr[i], **fr)
+            keep.append(k)
+            results.append(Track._frame_result(n_runs, iterations_capacity))
+        rarr = (KbaResult * len(results))(*[r.c for r in results])
+        _check(lib().kba_track_group_adjust_pose(self._p, arr, C.byref(opt or default_options()), rarr))
         for r, c in zip(results, rarr):
             r.c = c
         return results

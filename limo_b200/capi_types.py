@@ -42,6 +42,12 @@ class KbaTrackRequest(C.Structure):
                 ("sel", C.POINTER(KbaWindow))]
 
 
+class KbaTrackFrame(C.Structure):
+    _fields_ = [("n_meas", C.c_int32), ("reserved_", C.c_int32), ("pose7", c_double_p), ("lm_slot", c_int32_p), ("cam", c_int32_p),
+                ("u", c_float_p), ("v", c_float_p), ("d", c_float_p), ("speed_weight", C.c_double), ("speed_dt", C.c_double),
+                ("speed_v_before", C.c_double * 3), ("speed_T_origin_before", C.c_double * 7)]
+
+
 class KbaOptions(C.Structure):
     _fields_ = [
         ("depth_thres", C.c_double), ("reprojection_thres", C.c_double),

@@ -185,6 +185,62 @@ void BundleAdjusterKeyframes::deactivateKeyframes(int min_num_connecting_landmar
     rest[1].second->fixation_status_ = Keyframe::FixationStatus::Scale;
 }
 
+namespace {
+// kba_options of solve() / adjustPoseOnly() (cpp:740-764, 864-869)
+kba_options solve_options(const BundleAdjusterKeyframes::OutlierRejectionOptions& o, double solver_time_sec, bool motion_only,
+                          size_t n_selected) {
+    kba_options opt;
+    kba_default_options(&opt);
+    opt.depth_thres = o.depth_thres;
+    opt.reprojection_thres = o.reprojection_thres;
+    opt.depth_quantile = o.depth_quantile;
+    opt.reprojection_quantile = o.reprojection_quantile;
+    opt.num_rounds_option = o.num_iterations;
+    opt.solver_time_sec = solver_time_sec;
+    if (motion_only) {  // cpp:864-869
+        opt.min_landmarks_for_trimming = 30;
+        opt.num_trim_rounds = n_selected > 30 ? o.num_iterations : 0;
+    }
+    return opt;
+}
+
+// stands in for robust_optimization::Summary::FullReport (robust_solving.hpp:54-59)
+std::string solve_report(const kba_result& r, const char* where) {
+    static const char* term[] = {"CONVERGENCE", "NO_CONVERGENCE", "FAILURE"};
+    std::stringstream ss;
+    ss << "Merged summaries:\n";
+    for (int i = 0; i < r.num_solves; ++i) {
+        const kba_solve_summary& s = r.solves[i];
+        ss << "--------------------------------------------------\nIteration No." << i << "\n"
+           << "Residual blocks " << s.num_residual_blocks << ", landmarks " << s.num_landmarks << "; initial cost "
+           << s.initial_cost << ", final cost " << s.final_cost << ", iterations " << s.num_iterations << " (successful "
+           << s.num_successful_steps << "), termination " << term[s.termination < 3 ? s.termination : 2] << "\n";
+    }
+    if (r.status != KBA_OK)  // like a Ceres failure, not surfaced as an exception (reference: only text in the report)
+        ss << "\nsolver did not finish (kba status " << r.status << "): the last accepted iterate was written back\n";
+    ss << "\nDuration solveTrimmed=" << r.time_sec << " sec" << where << "\n";
+    return ss.str();
+}
+}  // namespace
+
+// SpeedRegularizationVector2 of adjustPoseOnly (cpp:835-853) on keyframe 0 of w, when the reference adds it
+void BundleAdjusterKeyframes::speedPrior(const Keyframe& speed_kf, kba_window& w) const {
+    if (active_keyframe_ids_.size() <= 2) return;
+    auto sorted = getSortedActiveKeyframePtrs();
+    const Keyframe& b0 = *sorted[sorted.size() - 1];
+    const Keyframe& b1 = *sorted[sorted.size() - 2];
+    const double rot_diff = calcQuaternionDiff(b0.pose_, b1.pose_);
+    if (!(rot_diff < 0.03)) return;
+    const double dt_cur = convert(speed_kf.timestamp_) - convert(b0.timestamp_);
+    const double dt_before = convert(b0.timestamp_) - convert(b1.timestamp_);
+    if (dt_cur <= 0. || dt_before <= 0.) throw std::runtime_error("In PoseRegularizationSpeed: invalid timestamps");
+    const v3 v_before = (b0.getEigenPose() * b1.getEigenPose().inverse()).translation() / dt_before;
+    const Pose T_ob = convert(b0.getEigenPose().inverse());
+    w.speed_kf = 0; w.speed_weight = 1. * (1 - rot_diff / 0.03); w.speed_dt = dt_cur;
+    for (int i = 0; i < 3; ++i) w.speed_v_before[i] = v_before[i];
+    for (int i = 0; i < 7; ++i) w.speed_T_origin_before[i] = T_ob[i];
+}
+
 // Pack -> kba_solve_window -> scatter.  Replaces addActiveKeyframesToProblem / addKeyframeToProblem (cpp:498-627),
 // addGroundPlaneResiduals (:517-562), the scale / plane regulariser set-up (:703-728, 769-818, 890-904) and
 // robust_optimization::solveTrimmed (:765, :886).
@@ -257,21 +313,8 @@ std::string BundleAdjusterKeyframes::runWindow(const std::vector<Keyframe*>& kfs
         }
         if (n_gp > 0) w.plane_reg_weight = 10.;  // cpp:717-719
         w.plane_dist_fixed = n_depth < 10;       // cpp:722-728
-    } else if (speed_kf && active_keyframe_ids_.size() > 2) {  // cpp:835-853
-        auto sorted = getSortedActiveKeyframePtrs();
-        const Keyframe& b0 = *sorted[sorted.size() - 1];
-        const Keyframe& b1 = *sorted[sorted.size() - 2];
-        const double rot_diff = calcQuaternionDiff(b0.pose_, b1.pose_);
-        if (rot_diff < 0.03) {
-            const double dt_cur = convert(speed_kf->timestamp_) - convert(b0.timestamp_);
-            const double dt_before = convert(b0.timestamp_) - convert(b1.timestamp_);
-            if (dt_cur <= 0. || dt_before <= 0.) throw std::runtime_error("In PoseRegularizationSpeed: invalid timestamps");
-            const v3 v_before = (b0.getEigenPose() * b1.getEigenPose().inverse()).translation() / dt_before;
-            const Pose T_ob = convert(b0.getEigenPose().inverse());
-            w.speed_kf = 0; w.speed_weight = 1. * (1 - rot_diff / 0.03); w.speed_dt = dt_cur;
-            for (int i = 0; i < 3; ++i) w.speed_v_before[i] = v_before[i];
-            for (int i = 0; i < 7; ++i) w.speed_T_origin_before[i] = T_ob[i];
-        }
+    } else if (speed_kf) {
+        speedPrior(*speed_kf, w);
     }
     w.landmarks_fixed = motion_only;
     w.n_kf = int(kfs.size()); w.n_cam = int(cam_index.size()); w.n_lm = int(lm_ids.size()); w.n_obs = int(obs_kf.size());
@@ -282,18 +325,7 @@ std::string BundleAdjusterKeyframes::runWindow(const std::vector<Keyframe*>& kfs
     w.obs_kf = obs_kf.data(); w.obs_cam = obs_cam.data(); w.obs_u = obs_u.data(); w.obs_v = obs_v.data(); w.obs_d = obs_d.data();
     w.gp_lm = gp_lm.data(); w.gp_kf = gp_kf.data(); w.gp_weight = gp_weight.data();
 
-    kba_options opt;
-    kba_default_options(&opt);
-    opt.depth_thres = outlier_rejection_options_.depth_thres;
-    opt.reprojection_thres = outlier_rejection_options_.reprojection_thres;
-    opt.depth_quantile = outlier_rejection_options_.depth_quantile;
-    opt.reprojection_quantile = outlier_rejection_options_.reprojection_quantile;
-    opt.num_rounds_option = outlier_rejection_options_.num_iterations;
-    opt.solver_time_sec = solver_time_sec;
-    if (motion_only) {  // cpp:864-869
-        opt.min_landmarks_for_trimming = 30;
-        opt.num_trim_rounds = selected_landmark_ids_.size() > 30 ? outlier_rejection_options_.num_iterations : 0;
-    }
+    const kba_options opt = solve_options(outlier_rejection_options_, solver_time_sec, motion_only, selected_landmark_ids_.size());
     std::vector<double> out_pose(kf_pose.size()), out_plane(kf_plane.size()), out_lm(lm_pos.size() + 3);
     kba_result r{};
     r.kf_pose = out_pose.data(); r.kf_plane = out_plane.data(); r.lm_pos = out_lm.data();
@@ -310,22 +342,12 @@ std::string BundleAdjusterKeyframes::runWindow(const std::vector<Keyframe*>& kfs
         }
     }
     if (!motion_only)
-        for (size_t j = 0; j < lm_ids.size(); ++j) std::copy_n(out_lm.begin() + 3 * j, 3, landmarks_.at(lm_ids[j])->pos.begin());
+        for (size_t j = 0; j < lm_ids.size(); ++j) {
+            std::copy_n(out_lm.begin() + 3 * j, 3, landmarks_.at(lm_ids[j])->pos.begin());
+            if (track_) dirty_positions_.insert(lm_ids[j]);  // the store still holds the old position: flushLandmarks()
+        }
 
-    static const char* term[] = {"CONVERGENCE", "NO_CONVERGENCE", "FAILURE"};
-    std::stringstream ss;  // stands in for robust_optimization::Summary::FullReport (robust_solving.hpp:54-59)
-    ss << "Merged summaries:\n";
-    for (int i = 0; i < r.num_solves; ++i) {
-        const kba_solve_summary& s = r.solves[i];
-        ss << "--------------------------------------------------\nIteration No." << i << "\n"
-           << "Residual blocks " << s.num_residual_blocks << ", landmarks " << s.num_landmarks << "; initial cost "
-           << s.initial_cost << ", final cost " << s.final_cost << ", iterations " << s.num_iterations << " (successful "
-           << s.num_successful_steps << "), termination " << term[s.termination < 3 ? s.termination : 2] << "\n";
-    }
-    if (r.status != KBA_OK)  // like a Ceres failure, not surfaced as an exception (reference: only text in the report)
-        ss << "\nsolver did not finish (kba status " << r.status << "): the last accepted iterate was written back\n";
-    ss << "\nDuration solveTrimmed=" << r.time_sec << " sec\n";
-    return ss.str();
+    return solve_report(r, "");
 }
 
 std::string BundleAdjusterKeyframes::solve() {  // cpp:629-767
@@ -428,21 +450,7 @@ bool BundleAdjusterKeyframes::solveTracked(const std::vector<Keyframe*>& kfs, co
         planes.push_back(kf->local_ground_plane_.distance);
     }
     if (kba_track_set_keyframe_poses(track_, n_kf, kf_slots.data(), poses.data(), planes.data()) != KBA_OK) { track_failed_ = true; return false; }
-    {
-        std::vector<int32_t> slots; std::vector<double> pos, wgt;
-        for (const auto id : new_landmarks_) {
-            auto it = lm_slot_.find(id);
-            if (it == lm_slot_.end()) continue;  // created, but its keyframe has not reached the store yet
-            const Landmark& lm = *landmarks_.at(id);
-            slots.push_back(it->second); pos.insert(pos.end(), lm.pos.begin(), lm.pos.end()); wgt.push_back(lm.weight);
-        }
-        if (!slots.empty() && kba_track_set_landmarks(track_, int(slots.size()), slots.data(), pos.data(), wgt.data()) != KBA_OK) { track_failed_ = true; return false; }
-        for (const auto id : std::set<LandmarkId>(new_landmarks_)) if (lm_slot_.count(id)) new_landmarks_.erase(id);
-        slots.clear(); wgt.clear();
-        for (const auto id : dirty_weights_) { auto it = lm_slot_.find(id); if (it != lm_slot_.end()) { slots.push_back(it->second); wgt.push_back(landmarks_.at(id)->weight); } }
-        if (!slots.empty() && kba_track_set_landmarks(track_, int(slots.size()), slots.data(), nullptr, wgt.data()) != KBA_OK) { track_failed_ = true; return false; }
-        dirty_weights_.clear();
-    }
+    if (!flushLandmarks()) { track_failed_ = true; return false; }
     for (const auto id : lm_ids) {
         auto it = lm_slot_.find(id);
         if (it == lm_slot_.end()) return false;  // selected but never measured by a stored keyframe: let the rebuild path decide
@@ -453,14 +461,7 @@ bool BundleAdjusterKeyframes::solveTracked(const std::vector<Keyframe*>& kfs, co
     sel.scale_kf0 = 0; sel.scale_kf1 = 1;
     sel.scale_weight = -1.;  // the reference's rule (cpp:703-716), evaluated on the device from the gathered window
     sel.scale_value = n_kf > 1 ? (kfs[1]->getEigenPose() * kfs[0]->getEigenPose().inverse()).translation().norm() : 0.;
-    kba_options opt;
-    kba_default_options(&opt);
-    opt.depth_thres = outlier_rejection_options_.depth_thres;
-    opt.reprojection_thres = outlier_rejection_options_.reprojection_thres;
-    opt.depth_quantile = outlier_rejection_options_.depth_quantile;
-    opt.reprojection_quantile = outlier_rejection_options_.reprojection_quantile;
-    opt.num_rounds_option = outlier_rejection_options_.num_iterations;
-    opt.solver_time_sec = solver_time_sec;
+    const kba_options opt = solve_options(outlier_rejection_options_, solver_time_sec, false, lm_ids.size());
     std::vector<double> out_pose(7 * size_t(n_kf)), out_plane(4 * size_t(n_kf)), out_lm(3 * size_t(n_lm) + 3);
     kba_result r{};
     r.kf_pose = out_pose.data(); r.kf_plane = out_plane.data(); r.lm_pos = out_lm.data();
@@ -473,19 +474,82 @@ bool BundleAdjusterKeyframes::solveTracked(const std::vector<Keyframe*>& kfs, co
     last_solve_h2d_ = (long long)h2d + (long long)n_kf * (7 + 4) * 8;  // the selection lists + the active keyframes' poses
     for (int k = 0; k < n_kf; ++k) std::copy_n(out_pose.begin() + 7 * k, 7, kfs[k]->pose_.begin());  // in place, as the reference (cpp:554-557)
     for (int j = 0; j < n_lm; ++j) std::copy_n(out_lm.begin() + 3 * j, 3, landmarks_.at(lm_ids[j])->pos.begin());
-    static const char* term[] = {"CONVERGENCE", "NO_CONVERGENCE", "FAILURE"};
-    std::stringstream ss;
-    ss << "Merged summaries:\n";
-    for (int i = 0; i < r.num_solves; ++i) {
-        const kba_solve_summary& s = r.solves[i];
-        ss << "--------------------------------------------------\nIteration No." << i << "\n"
-           << "Residual blocks " << s.num_residual_blocks << ", landmarks " << s.num_landmarks << "; initial cost "
-           << s.initial_cost << ", final cost " << s.final_cost << ", iterations " << s.num_iterations << " (successful "
-           << s.num_successful_steps << "), termination " << term[s.termination < 3 ? s.termination : 2] << "\n";
+    report = solve_report(r, " (device-resident window)");
+    return true;
+}
+
+// Landmark state the host changed since the store last saw it: position and weight of new landmarks (push()), positions the
+// rebuild path wrote (runWindow), weights set by updateLabels().  A landmark without a slot is not in the store: a new one waits
+// for its keyframe; any other landmark gets its slot in trackPush() only while it is still new, so its value goes up then.
+// false: the store could not be written.
+bool BundleAdjusterKeyframes::flushLandmarks() {
+    std::vector<int32_t> slots;
+    std::vector<double> pos, wgt;
+    for (const auto id : new_landmarks_) {
+        auto it = lm_slot_.find(id);
+        if (it == lm_slot_.end()) continue;  // created, but its keyframe has not reached the store yet
+        const Landmark& lm = *landmarks_.at(id);
+        slots.push_back(it->second); pos.insert(pos.end(), lm.pos.begin(), lm.pos.end()); wgt.push_back(lm.weight);
     }
-    if (r.status != KBA_OK) ss << "\nsolver did not finish (kba status " << r.status << "): the last accepted iterate was written back\n";
-    ss << "\nDuration solveTrimmed=" << r.time_sec << " sec (device-resident window)\n";
-    report = ss.str();
+    if (!slots.empty() && kba_track_set_landmarks(track_, int(slots.size()), slots.data(), pos.data(), wgt.data()) != KBA_OK) return false;
+    for (const auto id : std::set<LandmarkId>(new_landmarks_)) if (lm_slot_.count(id)) new_landmarks_.erase(id);
+    slots.clear(); pos.clear();
+    for (const auto id : dirty_positions_) {
+        auto it = lm_slot_.find(id);
+        if (it == lm_slot_.end()) continue;
+        const Landmark& lm = *landmarks_.at(id);
+        slots.push_back(it->second); pos.insert(pos.end(), lm.pos.begin(), lm.pos.end());
+    }
+    if (!slots.empty() && kba_track_set_landmarks(track_, int(slots.size()), slots.data(), pos.data(), nullptr) != KBA_OK) return false;
+    dirty_positions_.clear();
+    slots.clear(); wgt.clear();
+    for (const auto id : dirty_weights_) { auto it = lm_slot_.find(id); if (it != lm_slot_.end()) { slots.push_back(it->second); wgt.push_back(landmarks_.at(id)->weight); } }
+    if (!slots.empty() && kba_track_set_landmarks(track_, int(slots.size()), slots.data(), nullptr, wgt.data()) != KBA_OK) return false;
+    dirty_weights_.clear();
+    return true;
+}
+
+// adjustPoseOnly() against the device-resident store: only the frame goes up.  false: not possible for this frame (caller rebuilds).
+bool BundleAdjusterKeyframes::adjustPoseTracked(Keyframe& kf, const std::vector<LandmarkId>& lm_ids, std::string& report) {
+    if (lm_ids.empty() || int(lm_ids.size()) > kTrackWinLandmarks) return false;
+    std::map<CameraId, int> cam_of;
+    for (const auto& c : kf.cameras_) {
+        const auto it = std::find(track_cams_.begin(), track_cams_.end(), camera_value(*c.second));
+        if (it == track_cams_.end()) return false;  // a camera the store does not know
+        cam_of[c.first] = int(it - track_cams_.begin());
+    }
+    std::vector<int32_t> lm, cam;
+    std::vector<float> u, v, d;
+    for (const auto id : lm_ids) {  // ascending landmark id, cameras in measurement order inside: runWindow's observation order
+        const auto it = lm_slot_.find(id);
+        if (it == lm_slot_.end()) return false;  // never measured by a stored keyframe
+        for (const auto& cm : kf.measurements_.at(id)) {
+            lm.push_back(it->second); cam.push_back(cam_of.at(cm.first));
+            u.push_back(cm.second.u); v.push_back(cm.second.v); d.push_back(cm.second.d);
+        }
+    }
+    if (int(lm.size()) > kTrackWinObservations) return false;
+    if (!flushLandmarks()) { track_failed_ = true; return false; }
+    kba_window w{};  // carries the speed prior
+    speedPrior(kf, w);
+    kba_track_frame f{};
+    f.n_meas = int(lm.size());
+    f.pose7 = kf.pose_.data(); f.lm_slot = lm.data(); f.cam = cam.data(); f.u = u.data(); f.v = v.data(); f.d = d.data();
+    f.speed_weight = w.speed_weight; f.speed_dt = w.speed_dt;
+    std::copy_n(w.speed_v_before, 3, f.speed_v_before);
+    std::copy_n(w.speed_T_origin_before, 7, f.speed_T_origin_before);
+    const kba_options opt = solve_options(outlier_rejection_options_, solver_time_sec, true, selected_landmark_ids_.size());
+    double out_pose[7];
+    kba_result r{};
+    r.kf_pose = out_pose;
+    const int rc = kba_track_adjust_pose(track_, &f, &opt, &r);
+    if (rc == KBA_ERR_CAPACITY) return false;
+    if (rc != KBA_OK) throw std::runtime_error(std::string("kba_b200: ") + kba_last_error());
+    int64_t h2d = 0;
+    kba_track_transfer_bytes(track_, &h2d, nullptr, nullptr);
+    last_solve_h2d_ = (long long)h2d;  // the frame upload
+    std::copy_n(out_pose, 7, kf.pose_.begin());  // in place, as the reference
+    report = solve_report(r, " (device-resident window)");
     return true;
 }
 
@@ -494,6 +558,8 @@ std::string BundleAdjusterKeyframes::adjustPoseOnly(Keyframe& kf) {  // cpp:820-
     std::vector<LandmarkId> lm_ids;
     for (const auto& m : kf.measurements_)
         if (selected_landmark_ids_.count(m.first)) lm_ids.push_back(m.first);  // landmarks_.at() would throw like the reference
+    std::string report;
+    if (persistent_window_ && track_ && !track_failed_ && adjustPoseTracked(kf, lm_ids, report)) return report;
     return runWindow({&kf}, lm_ids, true, &kf);
 }
 

@@ -173,6 +173,49 @@ struct kba_batch {
     }
 };
 
+// buffers of kba_track_adjust_pose / kba_track_group_adjust_pose (k_adjust_pose): allocated at the first call, for the capacities of
+// the track(s), then reused: a call makes one upload, one launch, one download and one synchronisation
+struct MotionBufs {
+    Staged<unsigned char> up;    // frame descriptors, run starts and measurements of one call (pinned + device)
+    Staged<unsigned char> out;   // FrameRes per frame, iteration records, rejections (device + pinned)
+    double* run_pw = nullptr, *trim_val = nullptr;
+    unsigned char* run_active = nullptr, *run_rej = nullptr;
+    IterRecord* log = nullptr;
+    cudaEvent_t ev0 = nullptr, ev1 = nullptr;
+    int frames_cap = 0, runs_cap = 0, meas_cap = 0;
+    std::vector<unsigned> seen;  // per landmark slot: the check that stamped it last (a slot must not reappear after its run)
+    unsigned stamp = 0;
+    static size_t al(size_t b) { return (b + 15) & ~(size_t)15; }
+    static size_t up_bytes(int frames, int runs, int meas) {
+        return al(sizeof(FrameDesc) * (size_t)frames) + al(4 * ((size_t)runs + frames)) + 5 * al(4 * (size_t)meas);
+    }
+    static size_t out_bytes(int frames, int log_cap, int runs) {
+        return al(sizeof(FrameRes) * (size_t)frames) + al(sizeof(IterRecord) * (size_t)frames * log_cap) + al((size_t)runs);
+    }
+    int alloc(int frames, int runs, int meas) {
+        frames_cap = frames; runs_cap = runs; meas_cap = meas;
+        int bad = up.alloc(up_bytes(frames, runs, meas), true) | out.alloc(out_bytes(frames, kIterLogCap, runs), true);
+        bad |= cudaMalloc(&run_pw, sizeof(double) * 4 * (size_t)std::max(runs, 1)) != cudaSuccess;
+        bad |= cudaMalloc(&trim_val, sizeof(double) * 2 * (size_t)std::max(runs, 1)) != cudaSuccess;
+        bad |= cudaMalloc(&run_active, (size_t)std::max(runs, 1)) != cudaSuccess;
+        bad |= cudaMalloc(&run_rej, (size_t)std::max(runs, 1)) != cudaSuccess;
+        bad |= cudaMalloc(&log, sizeof(IterRecord) * kIterLogCap * (size_t)frames) != cudaSuccess;
+        bad |= cudaEventCreate(&ev0) != cudaSuccess;
+        bad |= cudaEventCreate(&ev1) != cudaSuccess;
+        return bad;
+    }
+    ~MotionBufs() {
+        up.release(); out.release();
+        if (run_pw) cudaFree(run_pw);
+        if (trim_val) cudaFree(trim_val);
+        if (run_active) cudaFree(run_active);
+        if (run_rej) cudaFree(run_rej);
+        if (log) cudaFree(log);
+        if (ev0) cudaEventDestroy(ev0);
+        if (ev1) cudaEventDestroy(ev1);
+    }
+};
+
 // persistent, device-resident window (kba_track_*, at the end of this file)
 struct kba_track {
     kba_handle* h = nullptr;
@@ -196,6 +239,7 @@ struct kba_track {
     std::vector<double> cam_intr, cam_pose;  // host copy of the cameras: capacity windows of kba_track_group_create
     int push_cap = 0, set_cap = 0;
     int64_t h2d_solve = 0, d2h_solve = 0, h2d_push = 0;
+    std::unique_ptr<MotionBufs> motion;    // kba_track_adjust_pose, allocated at its first call
     template <typename T> int alloc(T** p, size_t n) {
         void* q = nullptr;
         if (cudaMalloc(&q, std::max<size_t>(n, 1) * sizeof(T)) != cudaSuccess) return 1;
@@ -216,6 +260,7 @@ struct kba_track_group {
     Staged<TrackSel> tsel;
     Staged<int> lists;                     // every selection list of a solve (keyframe slots, landmark slots, fixation bytes), ONE copy
     int64_t h2d_solve = 0, d2h_solve = 0;
+    std::unique_ptr<MotionBufs> motion;    // kba_track_group_adjust_pose, allocated at its first call
 };
 
 static int validate_window(const kba_window* w, std::string& why) {
@@ -1292,6 +1337,7 @@ void kba_track_destroy(kba_track* t) {
     t->p_lm.release(); t->p_cam.release(); t->sel_kf.release(); t->sel_lm.release(); t->lay.release();
     t->p_u.release(); t->p_v.release(); t->p_d.release(); t->sel_fixed.release(); t->p_dbl.release(); t->p_slot.release();
     t->tdev.release(); t->tsel.release();
+    t->motion.reset();
     delete t;
 }
 
@@ -1628,6 +1674,7 @@ void kba_track_group_destroy(kba_track_group* g) {
     cudaStreamSynchronize(g->h->stream);
     if (g->batch) kba_batch_destroy(g->batch);
     g->tdev.release(); g->tsel.release(); g->lists.release();
+    g->motion.reset();
     delete g;
 }
 
@@ -1756,5 +1803,215 @@ int kba_track_group_transfer_bytes(kba_track_group* g, int64_t* h2d, int64_t* d2
     return KBA_OK;
 }
 
+// ---------------------------------------------------------------------------------------------------------------------
+// motion-only frames against the persistent store (include/kba_b200.h, kba_track_adjust_pose / kba_track_group_adjust_pose)
+// ---------------------------------------------------------------------------------------------------------------------
+// every check of one frame, before anything is uploaded; n_runs = landmarks of the frame, rounds = trimming rounds it runs
+static int frame_check(const kba_track* t, const kba_track_frame* f, const kba_options* opt, MotionBufs& mb, int& n_runs, int& rounds,
+                       std::string& why) {
+    n_runs = 0;
+    if (f->n_meas < 0) { why = "negative n_meas"; return KBA_ERR_BAD_ARG; }
+    if (!f->pose7 || !f->lm_slot || !f->u || !f->v || !f->d) { why = "null pose or measurement array"; return KBA_ERR_BAD_ARG; }
+    if (f->speed_weight > 0 && !(f->speed_dt > 0)) { why = "speed prior: dt <= 0"; return KBA_ERR_BAD_ARG; }
+    if (f->n_meas > t->caps.win_observations) { why = "more measurements than win_observations"; return KBA_ERR_CAPACITY; }
+    if (++mb.stamp == 0) { std::fill(mb.seen.begin(), mb.seen.end(), 0u); mb.stamp = 1; }
+    for (int i = 0; i < f->n_meas; ++i) {
+        const int slot = f->lm_slot[i];
+        if (slot < 0 || slot >= t->td.lm_cap) { why = "landmark slot out of range"; return KBA_ERR_BAD_ARG; }
+        if (f->cam && (f->cam[i] < 0 || f->cam[i] >= t->n_cam)) { why = "camera index out of range"; return KBA_ERR_BAD_ARG; }
+        if (i > 0 && slot == f->lm_slot[i - 1]) continue;
+        if (mb.seen[slot] == mb.stamp) { why = "landmark slot " + std::to_string(slot) + " reappears after its run"; return KBA_ERR_BAD_ARG; }
+        mb.seen[slot] = mb.stamp;
+        ++n_runs;
+    }
+    if (n_runs > t->caps.win_landmarks) { why = "more landmarks than win_landmarks"; return KBA_ERR_CAPACITY; }
+    rounds = opt->num_trim_rounds;  // k_reset_state's rule on the frame's landmark count
+    if (rounds < 0) rounds = (n_runs > opt->min_landmarks_for_trimming) ? opt->num_rounds_option : 0;
+    if (rounds > 6) rounds = 6;
+    return KBA_OK;
+}
+
+static int options_check(const kba_options* opt, std::string& why) {
+    if (opt->precision != 0) { why = "a frame is solved in FP64 only (kba_options.precision must be 0)"; return KBA_ERR_BAD_ARG; }
+    if (opt->num_trim_rounds > 6 || (opt->num_trim_rounds < 0 && opt->num_rounds_option > 6)) {
+        why = "at most 6 trimming rounds (KBA_MAX_SOLVES = 8 inner solves incl. one retry and the final solve)"; return KBA_ERR_CAPACITY;
+    }
+    return KBA_OK;
+}
+
+static void idle_result(kba_result& r) {
+    r.num_iteration_records = 0; r.num_solves = 0; r.status = KBA_OK;
+    r.initial_cost = 0.0; r.final_cost = 0.0; r.time_sec = 0.0;
+}
+
+// frames f[i] of tracks ts[i] (already checked; runs[i] landmarks, rounds[i] trimming rounds; n_meas == 0: idle) as one launch
+static int adjust_pose_run(kba_handle* h, MotionBufs& mb, int n, kba_track* const* ts, const kba_track_frame* f, const int* runs,
+                           const int* rounds, const kba_options* opt, kba_result* res, int64_t& h2d, int64_t& d2h) {
+    std::vector<int> live;
+    int M = 0, Rn = 0, log_cap = 0;
+    bool any_cam = false;
+    for (int i = 0; i < n; ++i) {
+        if (f[i].n_meas == 0) { idle_result(res[i]); continue; }
+        live.push_back(i);
+        M += f[i].n_meas; Rn += runs[i];
+        any_cam |= f[i].cam != nullptr;
+        if (res[i].iterations) log_cap = std::max(log_cap, std::min(res[i].iterations_capacity, kIterLogCap));
+    }
+    h2d = 0; d2h = 0;
+    const int nf = (int)live.size();
+    if (nf == 0) return KBA_OK;
+    CU(cudaSetDevice(h->device));
+    cudaStream_t s = h->stream;
+    // ---- staged upload: descriptors | run starts | slots | cameras | u | v | d
+    unsigned char* base = mb.up.h;
+    FrameDesc* fd = reinterpret_cast<FrameDesc*>(base);
+    size_t off = MotionBufs::al(sizeof(FrameDesc) * (size_t)nf);
+    int* rs = reinterpret_cast<int*>(base + off); const size_t o_rs = off; off += MotionBufs::al(4 * ((size_t)Rn + nf));
+    const size_t o_lm = off; off += MotionBufs::al(4 * (size_t)M);
+    const size_t o_cam = off; if (any_cam) off += MotionBufs::al(4 * (size_t)M);
+    const size_t o_u = off; off += MotionBufs::al(4 * (size_t)M);
+    const size_t o_v = off; off += MotionBufs::al(4 * (size_t)M);
+    const size_t o_d = off; off += MotionBufs::al(4 * (size_t)M);
+    int mo = 0, ro = 0, rso = 0;
+    for (int q = 0; q < nf; ++q) {
+        const int i = live[q];
+        const kba_track_frame& F = f[i];
+        const kba_track* t = ts[i];
+        FrameDesc& d = fd[q];
+        d.n_meas = F.n_meas; d.n_runs = runs[i]; d.meas_off = mo; d.run_off = ro; d.rs_off = rso; d.rounds_total = rounds[i];
+        d.lm_pos = t->td.lm_pos; d.lm_weight = t->td.lm_weight;
+        d.cam16 = t->batch->bd.cam + (size_t)t->batch->desc_h[0].cam_off * kCamStride; d.n_cam = t->n_cam; d.pad = 0;
+        memcpy(d.pose7, F.pose7, sizeof(d.pose7));
+        d.speed_weight = F.speed_weight; d.speed_dt = F.speed_dt;
+        memcpy(d.speed_v_before, F.speed_v_before, sizeof(d.speed_v_before));
+        memcpy(d.speed_T_origin_before, F.speed_T_origin_before, sizeof(d.speed_T_origin_before));
+        int r = 0;
+        for (int k = 0; k < F.n_meas; ++k)
+            if (k == 0 || F.lm_slot[k] != F.lm_slot[k - 1]) rs[rso + r++] = k;
+        rs[rso + r] = F.n_meas;
+        memcpy(base + o_lm + 4 * (size_t)mo, F.lm_slot, 4 * (size_t)F.n_meas);
+        if (any_cam) {
+            if (F.cam) memcpy(base + o_cam + 4 * (size_t)mo, F.cam, 4 * (size_t)F.n_meas);
+            else memset(base + o_cam + 4 * (size_t)mo, 0, 4 * (size_t)F.n_meas);
+        }
+        memcpy(base + o_u + 4 * (size_t)mo, F.u, 4 * (size_t)F.n_meas);
+        memcpy(base + o_v + 4 * (size_t)mo, F.v, 4 * (size_t)F.n_meas);
+        memcpy(base + o_d + 4 * (size_t)mo, F.d, 4 * (size_t)F.n_meas);
+        mo += F.n_meas; ro += runs[i]; rso += runs[i] + 1;
+    }
+    unsigned char* dev = mb.up.d;
+    MotionArgs a;
+    a.fd = reinterpret_cast<const FrameDesc*>(dev);
+    a.run_start = reinterpret_cast<const int*>(dev + o_rs);
+    a.lm_slot = reinterpret_cast<const int*>(dev + o_lm);
+    a.cam = any_cam ? reinterpret_cast<const int*>(dev + o_cam) : nullptr;
+    a.u = reinterpret_cast<const float*>(dev + o_u);
+    a.v = reinterpret_cast<const float*>(dev + o_v);
+    a.d = reinterpret_cast<const float*>(dev + o_d);
+    a.run_pw = mb.run_pw; a.run_active = mb.run_active; a.run_rej = mb.run_rej; a.trim_val = mb.trim_val; a.log = mb.log;
+    a.total_runs = Rn; a.log_cap = log_cap;
+    const size_t o_log = MotionBufs::al(sizeof(FrameRes) * (size_t)nf);
+    const size_t o_rej = o_log + MotionBufs::al(sizeof(IterRecord) * (size_t)nf * log_cap);
+    const size_t n_out = o_rej + MotionBufs::al((size_t)Rn);
+    a.res = reinterpret_cast<FrameRes*>(mb.out.d);
+    a.res_log = reinterpret_cast<IterRecord*>(mb.out.d + o_log);
+    a.res_rej = mb.out.d + o_rej;
+    // ---- one upload, one launch, one download, one synchronisation
+    CU(cudaMemcpyAsync(mb.up.d, mb.up.h, off, cudaMemcpyHostToDevice, s));
+    CU(cudaEventRecord(mb.ev0, s));
+    launch_adjust_pose(a, nf, make_params(opt), s);
+    CU(cudaEventRecord(mb.ev1, s));
+    CU(cudaMemcpyAsync(mb.out.h, mb.out.d, n_out, cudaMemcpyDeviceToHost, s));
+    CU(wait_stream(h));
+    CU(cudaGetLastError());
+    float ms = 0.f;
+    CU(cudaEventElapsedTime(&ms, mb.ev0, mb.ev1));
+    h->counters.launches_total += 1;
+    h2d = (int64_t)off; d2h = (int64_t)n_out;
+    // ---- results
+    const FrameRes* fr = reinterpret_cast<const FrameRes*>(mb.out.h);
+    const IterRecord* lg = reinterpret_cast<const IterRecord*>(mb.out.h + o_log);
+    const unsigned char* rj = mb.out.h + o_rej;
+    for (int q = 0; q < nf; ++q) {
+        const int i = live[q];
+        const FrameRes& R = fr[q];
+        kba_result& r = res[i];
+        if (r.kf_pose) memcpy(r.kf_pose, R.pose, sizeof(R.pose));
+        if (r.lm_rejected) memcpy(r.lm_rejected, rj + fd[q].run_off, (size_t)runs[i]);
+        r.num_solves = R.n_solves;
+        for (int k = 0; k < R.n_solves && k < KBA_MAX_SOLVES; ++k) {
+            const SolveSummary& ss = R.solves[k];
+            kba_solve_summary& o = r.solves[k];
+            o.initial_cost = ss.initial_cost; o.final_cost = ss.final_cost; o.num_iterations = ss.num_iterations;
+            o.num_successful_steps = ss.num_successful_steps; o.termination = ss.termination;
+            o.num_landmarks = ss.num_landmarks; o.num_residual_blocks = ss.num_residual_blocks; o.reserved_ = 0;
+        }
+        r.initial_cost = R.n_solves > 0 ? R.solves[0].initial_cost : 0.0;
+        r.final_cost = R.n_solves > 0 ? R.solves[R.n_solves - 1].final_cost : 0.0;
+        r.status = R.done ? KBA_OK : KBA_ERR_TIMEOUT;
+        r.time_sec = 1e-3 * ms;
+        int k = 0;
+        if (r.iterations) {
+            for (; k < R.log_n && k < r.iterations_capacity && k < log_cap; ++k) {
+                const IterRecord& e = lg[(size_t)q * log_cap + k];
+                kba_iteration& o = r.iterations[k];
+                o.cost = e.cost; o.cost_change = e.cost_change; o.gradient_max_norm = e.gradient_max_norm;
+                o.step_norm = e.step_norm; o.relative_decrease = e.relative_decrease; o.trust_region_radius = e.radius;
+                o.iteration = e.iteration; o.solve_index = e.solve_index; o.step_is_valid = e.valid; o.step_is_successful = e.successful;
+            }
+        }
+        r.num_iteration_records = k;
+    }
+    return KBA_OK;
+}
+
+static int motion_alloc(std::unique_ptr<MotionBufs>& mb, int n, kba_track* const* ts) {
+    if (mb) return KBA_OK;
+    int runs = 0, meas = 0, lm_cap = 0;
+    for (int i = 0; i < n; ++i) {
+        runs += ts[i]->caps.win_landmarks; meas += ts[i]->caps.win_observations; lm_cap = std::max(lm_cap, ts[i]->td.lm_cap);
+    }
+    std::unique_ptr<MotionBufs> m(new MotionBufs());
+    if (m->alloc(n, runs, meas)) return fail(KBA_ERR_CUDA, "adjust_pose: out of memory");
+    m->seen.assign((size_t)lm_cap, 0u);
+    mb = std::move(m);
+    return KBA_OK;
+}
+
+int kba_track_adjust_pose(kba_track* t, const kba_track_frame* f, const kba_options* opt, kba_result* res) {
+    if (!t || !f || !opt || !res) return fail(KBA_ERR_BAD_ARG, "null argument to kba_track_adjust_pose");
+    std::string why;
+    int rc = options_check(opt, why);
+    if (rc != KBA_OK) return fail(rc, "kba_track_adjust_pose: " + why);
+    CU(cudaSetDevice(t->h->device));
+    rc = motion_alloc(t->motion, 1, &t);
+    if (rc != KBA_OK) return rc;
+    int runs = 0, rounds = 0;
+    if (f->n_meas != 0) {
+        rc = frame_check(t, f, opt, *t->motion, runs, rounds, why);
+        if (rc != KBA_OK) return fail(rc, "kba_track_adjust_pose: " + why);
+    }
+    return adjust_pose_run(t->h, *t->motion, 1, &t, f, &runs, &rounds, opt, res, t->h2d_solve, t->d2h_solve);
+}
+
+int kba_track_group_adjust_pose(kba_track_group* g, const kba_track_frame* f, const kba_options* opt, kba_result* res) {
+    if (!g || !f || !opt || !res) return fail(KBA_ERR_BAD_ARG, "null argument to kba_track_group_adjust_pose");
+    std::string why;
+    int rc = options_check(opt, why);
+    if (rc != KBA_OK) return fail(rc, "kba_track_group_adjust_pose: " + why);
+    const int n = (int)g->tracks.size();
+    CU(cudaSetDevice(g->h->device));
+    rc = motion_alloc(g->motion, n, g->tracks.data());
+    if (rc != KBA_OK) return rc;
+    std::vector<int> runs(n, 0), rounds(n, 0);
+    for (int i = 0; i < n; ++i) {  // every frame is checked before anything is uploaded or launched
+        if (f[i].n_meas == 0) continue;
+        rc = frame_check(g->tracks[i], &f[i], opt, *g->motion, runs[i], rounds[i], why);
+        if (rc != KBA_OK) return fail(rc, "kba_track_group_adjust_pose: track " + std::to_string(i) + ": " + why);
+    }
+    return adjust_pose_run(g->h, *g->motion, n, g->tracks.data(), f, runs.data(), rounds.data(), opt, res, g->h2d_solve, g->d2h_solve);
+}
+
 }  // extern "C"
+
 

@@ -103,6 +103,48 @@ void launch_scatter_rows(double* dst, const int* slot, const double* src, int n,
 // results of every window w back into track store tds[w]
 void launch_track_writeback(const BatchDev& bd, const TrackDev* tds, const TrackSel* sels, const TrackGrid& g, cudaStream_t s);
 
+// ---- motion-only frames against a track's store (kba_track_adjust_pose / kba_track_group_adjust_pose, kba_motion.cu) ----
+// One frame = one free pose against constant landmarks read from a store by slot: its measurements come in runs, one run per
+// landmark (the landmarks of the equivalent window, in the caller's order).
+struct FrameDesc {
+    int n_meas, n_runs;
+    int meas_off;               // first measurement of the frame in the call's staged arrays
+    int run_off;                // first run of the frame in the work / result arrays
+    int rs_off;                 // first entry of the frame's run_start list (n_runs + 1 entries, frame-local measurement indices)
+    int rounds_total;           // trimming rounds, resolved on the host (k_reset_state's rule)
+    const double* lm_pos;       // the track's store: positions [lm_cap*3] and weights by slot
+    const double* lm_weight;
+    const double* cam16;        // the track's staged cameras (kCamStride doubles each)
+    int n_cam, pad;
+    double pose7[7];
+    double speed_weight, speed_dt;
+    double speed_v_before[3];
+    double speed_T_origin_before[7];
+};
+// what one frame hands back (the frame's slot of the result block; its rejections and iteration records follow elsewhere in it)
+struct FrameRes {
+    double pose[7];
+    int n_solves, log_n, done, pad;
+    SolveSummary solves[8];
+};
+struct MotionArgs {
+    const FrameDesc* fd;        // [n_frames]
+    const int* lm_slot;         // [total measurements] staged per call
+    const int* cam;
+    const float* u, *v, *d;
+    const int* run_start;
+    double* run_pw;             // [4 * total runs] work: landmark position and weight of every run
+    unsigned char* run_active;  // [total runs] work
+    unsigned char* run_rej;     // [total runs] work
+    double* trim_val;           // [2 * total runs] work: per-run maximum raw residual (depth, reprojection)
+    IterRecord* log;            // [n_frames * kIterLogCap] work
+    FrameRes* res;              // [n_frames]
+    IterRecord* res_log;        // [n_frames * log_cap]
+    unsigned char* res_rej;     // [total runs]
+    int log_cap, total_runs;
+};
+void launch_adjust_pose(const MotionArgs& a, int n_frames, const SolveParams& sp, cudaStream_t s);
+
 cudaError_t configure_pack();
 int pack_max_landmarks();
 void launch_pack(const BatchDev& bd, const PackRaw& raw, cudaStream_t s);

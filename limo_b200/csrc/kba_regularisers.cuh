@@ -69,6 +69,27 @@ __device__ inline double plane_motion(const double* p0, const double* p1, const 
     return r;
 }
 
+// SpeedRegularizationVector2 (reference cost_functors_ceres.hpp:300-353): r = (R t_ob + t) / dt - v_before on one pose p;
+// T_ob = the frozen speed_T_origin_before (7-vector), J (3x6, may be NULL) = local Jacobian (rot | trans).
+__device__ inline void speed_regulariser(const double* p, const double* T_ob, const double* v_before, double dt, double r[3],
+                                         double* J) {
+    double R[9];
+    quat_to_rot<double>(p, R);
+    const double* tob = T_ob + 4;
+    double a[3];
+    for (int i = 0; i < 3; ++i) a[i] = R[3 * i] * tob[0] + R[3 * i + 1] * tob[1] + R[3 * i + 2] * tob[2];
+    const double idt = 1.0 / dt;
+    for (int i = 0; i < 3; ++i) r[i] = (a[i] + p[4 + i]) * idt - v_before[i];
+    if (!J) return;
+    // d/d(delta_rot) = -2 [a]x / dt, d/d(delta_t) = I / dt
+    const double X[9] = {0, -a[2], a[1], a[2], 0, -a[0], -a[1], a[0], 0};
+    for (int i = 0; i < 3; ++i)
+        for (int j = 0; j < 3; ++j) {
+            J[6 * i + j] = -2.0 * X[3 * i + j] * idt;
+            J[6 * i + 3 + j] = (i == j) ? idt : 0.0;
+        }
+}
+
 // Warp-cooperative J^T J / J^T r accumulation of one residual block (all 32 lanes pass identical arguments).
 // parts: column offsets (or -1 for constant blocks) and sizes; J row-major nres x (sum of sizes), already times sqrt(rho').
 template <typename Mat>
