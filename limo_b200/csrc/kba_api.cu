@@ -216,12 +216,29 @@ struct MotionBufs {
     }
 };
 
+// what solves and pose-only calls of stored windows run on: one per track (n = 1) and one per track group (one window per
+// track), created by track_solver_create
+struct TrackSolver {
+    kba_batch* batch = nullptr;            // one capacity-shaped window per track; its raw arrays are filled by the gather kernels
+    Staged<TrackDev> tdev;                 // [n] read at every solve: compaction re-points a track's arena
+    Staged<TrackSel> tsel;
+    Staged<int> lists;                     // every selection list of a solve (keyframe slots, landmark slots, fixation bytes), ONE copy
+    std::unique_ptr<MotionBufs> motion;    // pose-only calls, allocated at the first one
+    int64_t h2d = 0, d2h = 0;              // the last solve or pose-only call
+    void release() {
+        if (batch) kba_batch_destroy(batch);
+        batch = nullptr;
+        tdev.release(); tsel.release(); lists.release();
+        motion.reset();
+    }
+};
+
 // persistent, device-resident window (kba_track_*, at the end of this file)
 struct kba_track {
     kba_handle* h = nullptr;
     kba_track_caps caps{};
     int n_cam = 0;
-    kba_batch* batch = nullptr;            // one window of capacity shape; its raw arrays are filled by the gather kernels
+    TrackSolver solver;                    // window 0 of its batch is this track's window
     TrackDev td{};
     int* arena_i[2][2] = {{nullptr, nullptr}, {nullptr, nullptr}};      // [buffer][lm, cam]
     float* arena_f[2][3] = {{nullptr, nullptr, nullptr}, {nullptr, nullptr, nullptr}};  // [buffer][u, v, d]
@@ -229,17 +246,13 @@ struct kba_track {
     std::vector<int> m_off, m_cnt;         // host mirror of the arena layout
     std::vector<char> kf_live;
     std::vector<void*> dev;
-    Staged<int> p_lm, p_cam, sel_kf, sel_lm, lay;  // pinned staging: one push / one selection / arena layout
+    Staged<int> p_lm, p_cam, lay;          // pinned staging: one push / arena layout
     Staged<float> p_u, p_v, p_d;
-    Staged<uint8_t> sel_fixed;
     Staged<double> p_dbl;                  // poses / landmark values on their way to the store
     Staged<int> p_slot;                    // ... and the slots they go to
-    Staged<TrackDev> tdev;                 // [1] the store and the selection of this solve, as the gather kernels read them
-    Staged<TrackSel> tsel;
-    std::vector<double> cam_intr, cam_pose;  // host copy of the cameras: capacity windows of kba_track_group_create
+    std::vector<double> cam_intr, cam_pose;  // host copy of the cameras: capacity windows of the track and of its groups
     int push_cap = 0, set_cap = 0;
-    int64_t h2d_solve = 0, d2h_solve = 0, h2d_push = 0;
-    std::unique_ptr<MotionBufs> motion;    // kba_track_adjust_pose, allocated at its first call
+    int64_t h2d_push = 0;
     template <typename T> int alloc(T** p, size_t n) {
         void* q = nullptr;
         if (cudaMalloc(&q, std::max<size_t>(n, 1) * sizeof(T)) != cudaSuccess) return 1;
@@ -255,12 +268,7 @@ struct kba_track {
 struct kba_track_group {
     kba_handle* h = nullptr;
     std::vector<kba_track*> tracks;
-    kba_batch* batch = nullptr;            // one capacity-shaped window per track
-    Staged<TrackDev> tdev;                 // [n_tracks] read at every solve: compaction re-points a track's arena
-    Staged<TrackSel> tsel;
-    Staged<int> lists;                     // every selection list of a solve (keyframe slots, landmark slots, fixation bytes), ONE copy
-    int64_t h2d_solve = 0, d2h_solve = 0;
-    std::unique_ptr<MotionBufs> motion;    // kba_track_group_adjust_pose, allocated at its first call
+    TrackSolver solver;                    // window i of its batch is track i's
 };
 
 static int validate_window(const kba_window* w, std::string& why) {
@@ -1332,12 +1340,10 @@ int kba_eval(kba_handle* h, const kba_window* w, const kba_options* opt, kba_eva
 void kba_track_destroy(kba_track* t) {
     if (!t) return;
     cudaStreamSynchronize(t->h->stream);
-    if (t->batch) kba_batch_destroy(t->batch);
+    t->solver.release();
     for (void* p : t->dev) cudaFree(p);
-    t->p_lm.release(); t->p_cam.release(); t->sel_kf.release(); t->sel_lm.release(); t->lay.release();
-    t->p_u.release(); t->p_v.release(); t->p_d.release(); t->sel_fixed.release(); t->p_dbl.release(); t->p_slot.release();
-    t->tdev.release(); t->tsel.release();
-    t->motion.reset();
+    t->p_lm.release(); t->p_cam.release(); t->lay.release();
+    t->p_u.release(); t->p_v.release(); t->p_d.release(); t->p_dbl.release(); t->p_slot.release();
     delete t;
 }
 
@@ -1376,14 +1382,14 @@ struct CapacityWindow {
     }
 };
 
-// what one solve of the stored window asks for (the arguments of kba_track_solve)
+// what one solve of the stored window asks for (the arguments of kba_track_solve, one kba_track_request of a group)
 struct TrackRequest {
     int32_t n_kf = 0;
     const int32_t* kf_slot = nullptr;
     const uint8_t* kf_fixed = nullptr;
     int32_t n_lm = 0;
     const int32_t* lm_slot = nullptr;
-    const kba_window* sel = nullptr;
+    const kba_window* sel = nullptr;       // nullptr: the track sits a group solve out
     int max_meas = 0, n_free = 0;          // filled by track_check: largest keyframe measurement count, free keyframes
 };
 
@@ -1445,11 +1451,37 @@ static void idle_desc(WinDesc& d) {
     d.idle = 1;
 }
 
+static void idle_result(kba_result& r) {
+    r.num_iteration_records = 0; r.num_solves = 0; r.status = KBA_OK;
+    r.initial_cost = 0.0; r.final_cost = 0.0; r.time_sec = 0.0;
+}
+
 static TrackSel track_sel(const TrackRequest& q, const int* kf_slot_d, const uint8_t* kf_fixed_d, const int* lm_slot_d) {
     TrackSel ts;
     ts.kf_slot = kf_slot_d; ts.kf_fixed = kf_fixed_d; ts.lm_slot = lm_slot_d; ts.n_kf = q.n_kf; ts.n_lm = q.n_lm; ts.max_meas = q.max_meas;
     ts.auto_scale = q.sel->scale_weight < 0 ? 1 : 0;
     return ts;
+}
+
+// the solver of tracks ts[0..n): one capacity window per track, so its batch has room for every window a track's caps allow.
+// On failure everything it allocated is freed again.
+static int track_solver_create(kba_handle* h, int n, kba_track* const* ts, TrackSolver& sv, const std::string& who) {
+    std::vector<std::unique_ptr<CapacityWindow>> cws;
+    std::vector<kba_window> ws;
+    size_t list_ints = 0;
+    for (int i = 0; i < n; ++i) {
+        const kba_track* t = ts[i];
+        cws.emplace_back(new CapacityWindow(t->caps, t->n_cam, t->cam_intr.data(), t->cam_pose.data()));
+        ws.push_back(cws.back()->w);
+        list_ints += (size_t)t->caps.win_keyframes + t->caps.win_landmarks + (t->caps.win_keyframes + 3) / 4;
+    }
+    const int rc = kba_batch_create(h, n, ws.data(), &sv.batch);
+    if (rc != KBA_OK) return rc;
+    if (!sv.batch->device_pack) { sv.release(); return fail(KBA_ERR_CAPACITY, who + ": device packing is disabled (KBA_FUSED / KBA_DEVICE_PACK)"); }
+    int bad = 0;
+    bad |= sv.tdev.alloc(n, true); bad |= sv.tsel.alloc(n, true); bad |= sv.lists.alloc(list_ints, true);
+    if (bad) { sv.release(); return fail(KBA_ERR_CUDA, who + ": out of memory"); }
+    return KBA_OK;
 }
 
 int kba_track_create(kba_handle* h, const kba_track_caps* c, int32_t n_cam, const double* cam_intr, const double* cam_pose, kba_track** out) {
@@ -1465,12 +1497,8 @@ int kba_track_create(kba_handle* h, const kba_track_caps* c, int32_t n_cam, cons
     t->h = h; t->caps = *c; t->n_cam = n_cam;
     t->cam_intr.assign(cam_intr, cam_intr + 3 * (size_t)n_cam);
     t->cam_pose.assign(cam_pose, cam_pose + 7 * (size_t)n_cam);
-    {
-        const CapacityWindow cw(*c, n_cam, t->cam_intr.data(), t->cam_pose.data());
-        const int rc = kba_batch_create(h, 1, &cw.w, &t->batch);
-        if (rc != KBA_OK) { delete t; return rc; }
-        if (!t->batch->device_pack) { kba_track_destroy(t); return fail(KBA_ERR_CAPACITY, "kba_track_create: device packing is disabled (KBA_FUSED / KBA_DEVICE_PACK)"); }
-    }
+    const int rc = track_solver_create(h, 1, &t, t->solver, "kba_track_create");
+    if (rc != KBA_OK) { delete t; return rc; }
     int bad = 0;
     TrackDev& td = t->td;
     td.kf_cap = c->max_keyframes; td.lm_cap = c->max_landmarks; td.m_cap = c->max_measurements;
@@ -1485,11 +1513,9 @@ int kba_track_create(kba_handle* h, const kba_track_caps* c, int32_t n_cam, cons
     t->push_cap = std::min(c->max_measurements, 1 << 16);
     bad |= t->p_lm.alloc(t->push_cap, true); bad |= t->p_cam.alloc(t->push_cap, true); bad |= t->p_u.alloc(t->push_cap, true);
     bad |= t->p_v.alloc(t->push_cap, true); bad |= t->p_d.alloc(t->push_cap, true);
-    bad |= t->sel_kf.alloc(c->win_keyframes, true); bad |= t->sel_fixed.alloc(c->win_keyframes, true); bad |= t->sel_lm.alloc(c->win_landmarks, true);
     bad |= t->lay.alloc(2 * (size_t)td.kf_cap, true);
     t->set_cap = std::max(c->win_landmarks, 64);  // rows per staged scatter (landmarks or keyframes)
     bad |= t->p_dbl.alloc(7 * (size_t)t->set_cap, true); bad |= t->p_slot.alloc(t->set_cap, true);
-    bad |= t->tdev.alloc(1, true); bad |= t->tsel.alloc(1, true);
     if (bad) { kba_track_destroy(t); return fail(KBA_ERR_CUDA, "kba_track_create: out of memory"); }
     t->point_arena();
     t->m_off.assign(td.kf_cap, 0); t->m_cnt.assign(td.kf_cap, 0); t->kf_live.assign(td.kf_cap, 0);
@@ -1612,56 +1638,85 @@ int kba_track_set_landmarks(kba_track* t, int32_t n, const int32_t* slot, const 
     return rc;
 }
 
+// one solve of the stored windows of tracks ts[0..n) as one batch, window i = ts[i]'s; qs[i] is checked by track_check or sits
+// the solve out (sel == nullptr).  kba_track_solve (n = 1) and kba_track_group_solve.
+static int track_solve(kba_handle* h, TrackSolver& sv, int n, kba_track* const* ts, const TrackRequest* qs, const kba_options* opt,
+                       kba_result* res) {
+    kba_batch* b = sv.batch;
+    CU(cudaSetDevice(h->device));
+    cudaStream_t s = h->stream;
+    // ---- descriptors, selection lists (one pinned buffer), track stores as they are now
+    int max_rank = 0, slots = 6;
+    bool any_gp = false;
+    TrackGrid grid;
+    size_t used = 0;
+    int64_t h2d = (int64_t)n * (int64_t)(sizeof(WinDesc) + sizeof(TrackDev) + sizeof(TrackSel));
+    for (int i = 0; i < n; ++i) {
+        const kba_track* t = ts[i];
+        const TrackRequest& q = qs[i];
+        WinDesc& d = b->desc_h[i];
+        sv.tdev.h[i] = t->td;  // compaction re-points a track's arena: read at every solve
+        if (!q.sel) {
+            idle_desc(d);
+            sv.tsel.h[i] = TrackSel{};
+        } else {
+            track_desc(d, t, q);
+            max_rank = std::max(max_rank, d.max_rank);
+            slots = std::max(slots, track_fused_slots(q));
+            int* l = sv.lists.h + used;
+            memcpy(l, q.kf_slot, q.n_kf * sizeof(int));
+            memcpy(l + q.n_kf, q.lm_slot, q.n_lm * sizeof(int));
+            memcpy(l + q.n_kf + q.n_lm, q.kf_fixed, q.n_kf);
+            const int* ld = sv.lists.d + used;
+            sv.tsel.h[i] = track_sel(q, ld, reinterpret_cast<const uint8_t*>(ld + q.n_kf + q.n_lm), ld + q.n_kf);
+            used += (size_t)q.n_kf + q.n_lm + (q.n_kf + 3) / 4;
+            const kba_window* sel = q.sel;
+            if (sel->n_gp) {
+                memcpy(b->r_gp_lm.h + d.gp_off, sel->gp_lm, sel->n_gp * sizeof(int)); memcpy(b->gp_kf.h + d.gp_off, sel->gp_kf, sel->n_gp * sizeof(int));
+                memcpy(b->gp_weight.h + d.gp_off, sel->gp_weight, sel->n_gp * sizeof(double));
+                any_gp = true;
+            }
+            grid.max_kf = std::max(grid.max_kf, q.n_kf); grid.max_lm = std::max(grid.max_lm, q.n_lm);
+            grid.max_meas = std::max(grid.max_meas, q.max_meas);
+            h2d += (int64_t)q.n_kf * 5 + (int64_t)q.n_lm * 4 + (int64_t)sel->n_gp * 16;
+        }
+        b->desc.h[i] = d;
+    }
+    // one launch configuration for the whole batch, as kba_batch_solve has for any batch
+    b->lc.max_rank = max_rank;
+    b->lc.fused_slots = slots;
+    CU(b->desc.upload(s));
+    CU(cudaMemcpyAsync(sv.lists.d, sv.lists.h, used * sizeof(int), cudaMemcpyHostToDevice, s));
+    CU(sv.tdev.upload(s)); CU(sv.tsel.upload(s));
+    if (any_gp) { CU(b->r_gp_lm.upload(s)); CU(b->gp_kf.upload(s)); CU(b->gp_weight.upload(s)); }
+    sv.h2d = h2d;
+    // ---- gather every window from its store, pack, solve, write back
+    launch_track_gather(b->bd, b->raw, sv.tdev.d, sv.tsel.d, grid, s);
+    launch_pack(b->bd, b->raw, s);
+    CU(cudaGetLastError());
+    int rc = kba_batch_solve(b, opt);
+    if (rc != KBA_OK) return rc;
+    launch_track_writeback(b->bd, sv.tdev.d, sv.tsel.d, grid, s);
+    rc = kba_batch_download(b, res);
+    sv.d2h = (int64_t)b->d2h_bytes;
+    return rc;
+}
+
 int kba_track_solve(kba_track* t, int32_t n_kf, const int32_t* kf_slot, const uint8_t* kf_fixed, int32_t n_lm, const int32_t* lm_slot,
                     const kba_window* sel, const kba_options* opt, kba_result* res) {
     if (!t || !opt || !res) return fail(KBA_ERR_BAD_ARG, "null argument to kba_track_solve");
     TrackRequest q;
     q.n_kf = n_kf; q.kf_slot = kf_slot; q.kf_fixed = kf_fixed; q.n_lm = n_lm; q.lm_slot = lm_slot; q.sel = sel;
     std::string why;
-    const int crc = track_check(t, q, why);
-    if (crc != KBA_OK) return fail(crc, "kba_track_solve: " + why);
-    kba_batch* b = t->batch;
-    CU(cudaSetDevice(t->h->device));
-    cudaStream_t s = t->h->stream;
-    // ---- the window descriptor of this solve (n_obs is written by the gather kernels)
-    WinDesc& d = b->desc_h[0];
-    track_desc(d, t, q);
-    b->desc.h[0] = d;
-    b->lc.max_rank = d.max_rank;
-    b->lc.fused_slots = track_fused_slots(q);
-    memcpy(t->sel_kf.h, kf_slot, n_kf * sizeof(int)); memcpy(t->sel_fixed.h, kf_fixed, n_kf);
-    memcpy(t->sel_lm.h, lm_slot, n_lm * sizeof(int));
-    if (sel->n_gp) {
-        memcpy(b->r_gp_lm.h, sel->gp_lm, sel->n_gp * sizeof(int)); memcpy(b->gp_kf.h, sel->gp_kf, sel->n_gp * sizeof(int));
-        memcpy(b->gp_weight.h, sel->gp_weight, sel->n_gp * sizeof(double));
-    }
-    t->tdev.h[0] = t->td;  // the arena pointers as they are now (compaction moves them)
-    t->tsel.h[0] = track_sel(q, t->sel_kf.d, t->sel_fixed.d, t->sel_lm.d);
-    CU(b->desc.upload(s));
-    CU(cudaMemcpyAsync(t->sel_kf.d, t->sel_kf.h, n_kf * sizeof(int), cudaMemcpyHostToDevice, s));
-    CU(cudaMemcpyAsync(t->sel_fixed.d, t->sel_fixed.h, n_kf, cudaMemcpyHostToDevice, s));
-    CU(cudaMemcpyAsync(t->sel_lm.d, t->sel_lm.h, n_lm * sizeof(int), cudaMemcpyHostToDevice, s));
-    CU(t->tdev.upload(s)); CU(t->tsel.upload(s));
-    if (sel->n_gp) { CU(b->r_gp_lm.upload(s)); CU(b->gp_kf.upload(s)); CU(b->gp_weight.upload(s)); }
-    t->h2d_solve = (int64_t)sizeof(WinDesc) + n_kf * 5 + n_lm * 4 + sel->n_gp * 16 + (int64_t)(sizeof(TrackDev) + sizeof(TrackSel));
-    // ---- gather the CSR from the store, pack, solve, write back
-    TrackGrid grid;
-    grid.max_kf = n_kf; grid.max_lm = n_lm; grid.max_meas = q.max_meas;
-    launch_track_gather(b->bd, b->raw, t->tdev.d, t->tsel.d, grid, s);
-    launch_pack(b->bd, b->raw, s);
-    CU(cudaGetLastError());
-    int rc = kba_batch_solve(b, opt);
-    if (rc != KBA_OK) return rc;
-    launch_track_writeback(b->bd, t->tdev.d, t->tsel.d, grid, s);
-    rc = kba_batch_download(b, res);
-    t->d2h_solve = (int64_t)b->d2h_bytes;
-    return rc;
+    const int rc = track_check(t, q, why);
+    if (rc != KBA_OK) return fail(rc, "kba_track_solve: " + why);
+    return track_solve(t->h, t->solver, 1, &t, &q, opt, res);
 }
 
 int kba_track_transfer_bytes(kba_track* t, int64_t* h2d, int64_t* d2h, int64_t* push) {
     if (!t) return fail(KBA_ERR_BAD_ARG, "null track");
-    if (h2d) *h2d = t->h2d_solve;
-    if (d2h) *d2h = t->d2h_solve;
+    if (h2d) *h2d = t->solver.h2d;
+    if (d2h) *d2h = t->solver.d2h;
     if (push) *push = t->h2d_push;
     return KBA_OK;
 }
@@ -1672,9 +1727,7 @@ int kba_track_transfer_bytes(kba_track* t, int64_t* h2d, int64_t* d2h, int64_t* 
 void kba_track_group_destroy(kba_track_group* g) {
     if (!g) return;
     cudaStreamSynchronize(g->h->stream);
-    if (g->batch) kba_batch_destroy(g->batch);
-    g->tdev.release(); g->tsel.release(); g->lists.release();
-    g->motion.reset();
+    g->solver.release();
     delete g;
 }
 
@@ -1688,25 +1741,11 @@ int kba_track_group_create(kba_handle* h, int32_t n_tracks, kba_track* const* tr
                 return fail(KBA_ERR_BAD_ARG, "kba_track_group_create: track " + std::to_string(i) + " is also track " + std::to_string(j));
     }
     CU(cudaSetDevice(h->device));
-    // one capacity window per track: the group batch has, window for window, the shapes of the tracks' own batches
-    std::vector<std::unique_ptr<CapacityWindow>> cws;
-    std::vector<kba_window> ws;
-    size_t list_ints = 0;
-    for (int i = 0; i < n_tracks; ++i) {
-        const kba_track* t = tracks[i];
-        cws.emplace_back(new CapacityWindow(t->caps, t->n_cam, t->cam_intr.data(), t->cam_pose.data()));
-        ws.push_back(cws.back()->w);
-        list_ints += (size_t)t->caps.win_keyframes + t->caps.win_landmarks + (t->caps.win_keyframes + 3) / 4;
-    }
     kba_track_group* g = new kba_track_group();
     g->h = h;
     g->tracks.assign(tracks, tracks + n_tracks);
-    const int rc = kba_batch_create(h, n_tracks, ws.data(), &g->batch);
+    const int rc = track_solver_create(h, n_tracks, tracks, g->solver, "kba_track_group_create");
     if (rc != KBA_OK) { delete g; return rc; }
-    if (!g->batch->device_pack) { kba_track_group_destroy(g); return fail(KBA_ERR_CAPACITY, "kba_track_group_create: device packing is disabled (KBA_FUSED / KBA_DEVICE_PACK)"); }
-    int bad = 0;
-    bad |= g->tdev.alloc(n_tracks, true); bad |= g->tsel.alloc(n_tracks, true); bad |= g->lists.alloc(list_ints, true);
-    if (bad) { kba_track_group_destroy(g); return fail(KBA_ERR_CUDA, "kba_track_group_create: out of memory"); }
     *out = g;
     return KBA_OK;
 }
@@ -1728,78 +1767,17 @@ int kba_track_group_solve(kba_track_group* g, const kba_track_request* req, cons
         ++active;
     }
     if (active == 0) {  // nothing to solve: no upload, no launch, every result idle
-        for (int i = 0; i < n; ++i) {
-            kba_result& r = res[i];
-            r.num_iteration_records = 0; r.num_solves = 0; r.status = KBA_OK;
-            r.initial_cost = 0.0; r.final_cost = 0.0; r.time_sec = 0.0;
-        }
-        g->h2d_solve = 0; g->d2h_solve = 0;
+        for (int i = 0; i < n; ++i) idle_result(res[i]);
+        g->solver.h2d = 0; g->solver.d2h = 0;
         return KBA_OK;
     }
-    kba_batch* b = g->batch;
-    CU(cudaSetDevice(g->h->device));
-    cudaStream_t s = g->h->stream;
-    // ---- descriptors, selection lists (one pinned buffer), track stores as they are now
-    int max_rank = 0, slots = 6;
-    bool any_gp = false;
-    TrackGrid grid;
-    size_t used = 0;
-    int64_t h2d = (int64_t)n * (int64_t)(sizeof(WinDesc) + sizeof(TrackDev) + sizeof(TrackSel));
-    for (int i = 0; i < n; ++i) {
-        const kba_track* t = g->tracks[i];
-        const TrackRequest& q = qs[i];
-        WinDesc& d = b->desc_h[i];
-        g->tdev.h[i] = t->td;  // compaction re-points a track's arena: read at every solve
-        if (!q.sel) {
-            idle_desc(d);
-            g->tsel.h[i] = TrackSel{};
-        } else {
-            track_desc(d, t, q);
-            max_rank = std::max(max_rank, d.max_rank);
-            slots = std::max(slots, track_fused_slots(q));
-            int* l = g->lists.h + used;
-            memcpy(l, q.kf_slot, q.n_kf * sizeof(int));
-            memcpy(l + q.n_kf, q.lm_slot, q.n_lm * sizeof(int));
-            memcpy(l + q.n_kf + q.n_lm, q.kf_fixed, q.n_kf);
-            const int* ld = g->lists.d + used;
-            g->tsel.h[i] = track_sel(q, ld, reinterpret_cast<const uint8_t*>(ld + q.n_kf + q.n_lm), ld + q.n_kf);
-            used += (size_t)q.n_kf + q.n_lm + (q.n_kf + 3) / 4;
-            const kba_window* sel = q.sel;
-            if (sel->n_gp) {
-                memcpy(b->r_gp_lm.h + d.gp_off, sel->gp_lm, sel->n_gp * sizeof(int)); memcpy(b->gp_kf.h + d.gp_off, sel->gp_kf, sel->n_gp * sizeof(int));
-                memcpy(b->gp_weight.h + d.gp_off, sel->gp_weight, sel->n_gp * sizeof(double));
-                any_gp = true;
-            }
-            grid.max_kf = std::max(grid.max_kf, q.n_kf); grid.max_lm = std::max(grid.max_lm, q.n_lm);
-            grid.max_meas = std::max(grid.max_meas, q.max_meas);
-            h2d += (int64_t)q.n_kf * 5 + (int64_t)q.n_lm * 4 + (int64_t)sel->n_gp * 16;
-        }
-        b->desc.h[i] = d;
-    }
-    // one launch configuration for the whole group, as kba_batch_solve has for any batch
-    b->lc.max_rank = max_rank;
-    b->lc.fused_slots = slots;
-    CU(b->desc.upload(s));
-    CU(cudaMemcpyAsync(g->lists.d, g->lists.h, used * sizeof(int), cudaMemcpyHostToDevice, s));
-    CU(g->tdev.upload(s)); CU(g->tsel.upload(s));
-    if (any_gp) { CU(b->r_gp_lm.upload(s)); CU(b->gp_kf.upload(s)); CU(b->gp_weight.upload(s)); }
-    g->h2d_solve = h2d;
-    // ---- gather every window from its store, pack, solve, write back
-    launch_track_gather(b->bd, b->raw, g->tdev.d, g->tsel.d, grid, s);
-    launch_pack(b->bd, b->raw, s);
-    CU(cudaGetLastError());
-    int rc = kba_batch_solve(b, opt);
-    if (rc != KBA_OK) return rc;
-    launch_track_writeback(b->bd, g->tdev.d, g->tsel.d, grid, s);
-    rc = kba_batch_download(b, res);
-    g->d2h_solve = (int64_t)b->d2h_bytes;
-    return rc;
+    return track_solve(g->h, g->solver, n, g->tracks.data(), qs.data(), opt, res);
 }
 
 int kba_track_group_transfer_bytes(kba_track_group* g, int64_t* h2d, int64_t* d2h) {
     if (!g) return fail(KBA_ERR_BAD_ARG, "null track group");
-    if (h2d) *h2d = g->h2d_solve;
-    if (d2h) *d2h = g->d2h_solve;
+    if (h2d) *h2d = g->solver.h2d;
+    if (d2h) *d2h = g->solver.d2h;
     return KBA_OK;
 }
 
@@ -1839,11 +1817,6 @@ static int options_check(const kba_options* opt, std::string& why) {
     return KBA_OK;
 }
 
-static void idle_result(kba_result& r) {
-    r.num_iteration_records = 0; r.num_solves = 0; r.status = KBA_OK;
-    r.initial_cost = 0.0; r.final_cost = 0.0; r.time_sec = 0.0;
-}
-
 // frames f[i] of tracks ts[i] (already checked; runs[i] landmarks, rounds[i] trimming rounds; n_meas == 0: idle) as one launch
 static int adjust_pose_run(kba_handle* h, MotionBufs& mb, int n, kba_track* const* ts, const kba_track_frame* f, const int* runs,
                            const int* rounds, const kba_options* opt, kba_result* res, int64_t& h2d, int64_t& d2h) {
@@ -1880,7 +1853,7 @@ static int adjust_pose_run(kba_handle* h, MotionBufs& mb, int n, kba_track* cons
         FrameDesc& d = fd[q];
         d.n_meas = F.n_meas; d.n_runs = runs[i]; d.meas_off = mo; d.run_off = ro; d.rs_off = rso; d.rounds_total = rounds[i];
         d.lm_pos = t->td.lm_pos; d.lm_weight = t->td.lm_weight;
-        d.cam16 = t->batch->bd.cam + (size_t)t->batch->desc_h[0].cam_off * kCamStride; d.n_cam = t->n_cam; d.pad = 0;
+        d.cam16 = t->solver.batch->bd.cam + (size_t)t->solver.batch->desc_h[0].cam_off * kCamStride; d.n_cam = t->n_cam; d.pad = 0;
         memcpy(d.pose7, F.pose7, sizeof(d.pose7));
         d.speed_weight = F.speed_weight; d.speed_dt = F.speed_dt;
         memcpy(d.speed_v_before, F.speed_v_before, sizeof(d.speed_v_before));
@@ -1978,38 +1951,33 @@ static int motion_alloc(std::unique_ptr<MotionBufs>& mb, int n, kba_track* const
     return KBA_OK;
 }
 
-int kba_track_adjust_pose(kba_track* t, const kba_track_frame* f, const kba_options* opt, kba_result* res) {
-    if (!t || !f || !opt || !res) return fail(KBA_ERR_BAD_ARG, "null argument to kba_track_adjust_pose");
+// a pose-only call of a track (n = 1) or of a group: the options and every frame are checked before anything is uploaded or
+// launched.  Errors start with `who`; a group's name the failing track.
+static int track_adjust_pose(const std::string& who, bool group, kba_handle* h, TrackSolver& sv, int n, kba_track* const* ts,
+                             const kba_track_frame* f, const kba_options* opt, kba_result* res) {
     std::string why;
     int rc = options_check(opt, why);
-    if (rc != KBA_OK) return fail(rc, "kba_track_adjust_pose: " + why);
-    CU(cudaSetDevice(t->h->device));
-    rc = motion_alloc(t->motion, 1, &t);
+    if (rc != KBA_OK) return fail(rc, who + ": " + why);
+    CU(cudaSetDevice(h->device));
+    rc = motion_alloc(sv.motion, n, ts);
     if (rc != KBA_OK) return rc;
-    int runs = 0, rounds = 0;
-    if (f->n_meas != 0) {
-        rc = frame_check(t, f, opt, *t->motion, runs, rounds, why);
-        if (rc != KBA_OK) return fail(rc, "kba_track_adjust_pose: " + why);
+    std::vector<int> runs(n, 0), rounds(n, 0);
+    for (int i = 0; i < n; ++i) {
+        if (f[i].n_meas == 0) continue;
+        rc = frame_check(ts[i], &f[i], opt, *sv.motion, runs[i], rounds[i], why);
+        if (rc != KBA_OK) return fail(rc, who + ": " + (group ? "track " + std::to_string(i) + ": " : std::string()) + why);
     }
-    return adjust_pose_run(t->h, *t->motion, 1, &t, f, &runs, &rounds, opt, res, t->h2d_solve, t->d2h_solve);
+    return adjust_pose_run(h, *sv.motion, n, ts, f, runs.data(), rounds.data(), opt, res, sv.h2d, sv.d2h);
+}
+
+int kba_track_adjust_pose(kba_track* t, const kba_track_frame* f, const kba_options* opt, kba_result* res) {
+    if (!t || !f || !opt || !res) return fail(KBA_ERR_BAD_ARG, "null argument to kba_track_adjust_pose");
+    return track_adjust_pose("kba_track_adjust_pose", false, t->h, t->solver, 1, &t, f, opt, res);
 }
 
 int kba_track_group_adjust_pose(kba_track_group* g, const kba_track_frame* f, const kba_options* opt, kba_result* res) {
     if (!g || !f || !opt || !res) return fail(KBA_ERR_BAD_ARG, "null argument to kba_track_group_adjust_pose");
-    std::string why;
-    int rc = options_check(opt, why);
-    if (rc != KBA_OK) return fail(rc, "kba_track_group_adjust_pose: " + why);
-    const int n = (int)g->tracks.size();
-    CU(cudaSetDevice(g->h->device));
-    rc = motion_alloc(g->motion, n, g->tracks.data());
-    if (rc != KBA_OK) return rc;
-    std::vector<int> runs(n, 0), rounds(n, 0);
-    for (int i = 0; i < n; ++i) {  // every frame is checked before anything is uploaded or launched
-        if (f[i].n_meas == 0) continue;
-        rc = frame_check(g->tracks[i], &f[i], opt, *g->motion, runs[i], rounds[i], why);
-        if (rc != KBA_OK) return fail(rc, "kba_track_group_adjust_pose: track " + std::to_string(i) + ": " + why);
-    }
-    return adjust_pose_run(g->h, *g->motion, n, g->tracks.data(), f, runs.data(), rounds.data(), opt, res, g->h2d_solve, g->d2h_solve);
+    return track_adjust_pose("kba_track_group_adjust_pose", true, g->h, g->solver, (int)g->tracks.size(), g->tracks.data(), f, opt, res);
 }
 
 }  // extern "C"
