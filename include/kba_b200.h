@@ -277,10 +277,10 @@ typedef struct kba_track_caps {
     int32_t max_keyframes;     /* keyframe slots in the store (active or not)        */
     int32_t max_landmarks;     /* landmark slots                                      */
     int32_t max_measurements;  /* arena entries over all stored keyframes             */
-    int32_t win_keyframes;     /* largest window: keyframes (<= 30: fused path)       */
+    int32_t win_keyframes;     /* largest window: keyframes (<= 30: fused path; a solve with ground-plane blocks takes <= 18) */
     int32_t win_landmarks;     /*                 selected landmarks                  */
     int32_t win_observations;  /*                 observations                        */
-    int32_t win_ground;        /*                 ground-plane residuals              */
+    int32_t win_ground;        /*                 ground-plane residuals, or candidates of a device attachment (<= win_landmarks) */
 } kba_track_caps;
 int kba_track_create(kba_handle* h, const kba_track_caps* caps, int32_t n_cam, const double* cam_intr, const double* cam_pose,
                      kba_track** out);
@@ -299,7 +299,25 @@ int kba_track_set_keyframe_poses(kba_track* t, int32_t n, const int32_t* kf_slot
  * index into lm_slot), its keyframe / landmark / observation arrays are ignored; scale_weight < 0 asks for the reference's own rule
  * (cpp:703-716: 1000, or 1000 / (depth + ground-plane residuals) beyond ten of them; plane_dist_fixed by cpp:722-728), evaluated
  * on the device from the gathered window so that the host need not visit a single observation.  Results: res->kf_pose / kf_plane [n_kf],
- * res->lm_pos / lm_rejected [n_lm] in selection order. */
+ * res->lm_pos / lm_rejected [n_lm] in selection order.
+ * Ground-plane residuals come in one of two ways:
+ *   - host lists: gp_lm, gp_kf and gp_weight, attached and weighted by the caller as kba_window describes them;
+ *   - device attachment: n_gp > 0, gp_lm lists CANDIDATE ground landmarks (indices into lm_slot, strictly ascending) and gp_kf,
+ *     gp_weight are both NULL.  Each candidate is attached on the device exactly as addGroundPlaneResiduals (cpp:517-562) does it,
+ *     from the store's current poses, planes and landmark positions: keyframes in window order, a keyframe whose plane distance is
+ *     < -10 skipped, distance |R(q) p + t| (first strict minimum wins, a NaN is never a minimum), kept iff the distance is < 25
+ *     with weight 10 (1 - d / 25); kept residuals in candidate order.  The arithmetic is that of the reference's host code without
+ *     FMA contraction, so the lists equal those a host computes from the same state bit for bit.  The caller sends 4 B per
+ *     candidate instead of 16 B per residual, and need not keep landmark positions on the host.
+ * plane_reg_weight < 0 asks for the reference's rule (cpp:717-719): 10 iff at least one ground-plane residual is in the window
+ * (with either kind of lists).  Errors, all before anything is uploaded: only one of gp_kf / gp_weight NULL, candidates not
+ * strictly ascending or out of range: KBA_ERR_BAD_ARG; more residuals or candidates than win_ground: KBA_ERR_CAPACITY; a request
+ * that can carry plane blocks (ground-plane lists of either kind, or plane_reg_weight != 0) with 10 * n_kf + 1 > 184 (more than 18
+ * keyframes): KBA_ERR_CAPACITY -- the rule by which kba_batch_create keeps a window on the fused path, so that the track and
+ * kba_solve_window run the same solver.  solves[].num_residual_blocks counts the attached residuals; with nothing attached, kf_plane
+ * comes back bit-equal to the stored planes, so a caller may always copy planes back.  One exception to bit-equality with
+ * kba_solve_window: the Schur kernel variant is chosen before the attachment, counting plane rows whenever candidates are given,
+ * so an 18-free-keyframe window with nothing attached runs the seven-slot kernel where kba_solve_window runs the six-slot one. */
 int kba_track_solve(kba_track* t, int32_t n_kf, const int32_t* kf_slot, const uint8_t* kf_fixed, int32_t n_lm, const int32_t* lm_slot,
                     const kba_window* sel, const kba_options* opt, kba_result* res);
 int kba_track_transfer_bytes(kba_track* t, int64_t* h2d_last_solve, int64_t* d2h_last_solve, int64_t* h2d_pushes_total);
@@ -334,7 +352,8 @@ typedef struct kba_track_request {
     const uint8_t* kf_fixed;
     int32_t n_lm;
     const int32_t* lm_slot;
-    const kba_window* sel;      /* sizes, scalars and ground-plane lists, as for kba_track_solve */
+    const kba_window* sel;      /* sizes, scalars and ground-plane lists or candidates, as for kba_track_solve; a group may mix
+                                   device-attached, host-list and plane-free requests */
 } kba_track_request;
 int kba_track_group_create(kba_handle* h, int32_t n_tracks, kba_track* const* tracks, kba_track_group** out);
 void kba_track_group_destroy(kba_track_group* g);

@@ -222,7 +222,9 @@ class Track:
         return kf, fx, lm, sel
 
     def solve(self, kf_slots, kf_fixed, lm_slots, opt=None, **scalars):
-        """scalars: scale_kf0, scale_kf1, scale_weight, scale_value, plane_reg_weight, plane_dist_fixed, gp_lm, gp_kf, gp_weight"""
+        """scalars: scale_kf0, scale_kf1, scale_weight, scale_value, plane_reg_weight, plane_dist_fixed, gp_lm, gp_kf, gp_weight.
+        gp_lm without gp_kf / gp_weight: candidate ground landmarks (ascending indices into lm_slots), attached on the device
+        (kba_track_solve); plane_reg_weight < 0: 10 iff a ground-plane residual is in the window."""
         kf, fx, lm, sel = self._selection(kf_slots, kf_fixed, lm_slots, **scalars)
         res = Result(sel, 256)
         _check(lib().kba_track_solve(self._p, len(kf), kf.ctypes.data_as(c_int32_p), fx.ctypes.data_as(C.POINTER(C.c_uint8)), len(lm),

@@ -390,7 +390,9 @@ bool BundleAdjusterKeyframes::trackPush(const Keyframe& kf) {
             intr.insert(intr.end(), v.begin(), v.begin() + 3);
             pose.insert(pose.end(), v.begin() + 3, v.end());
         }
-        kba_track_caps caps{kTrackKeyframes, kTrackLandmarks, kTrackMeasurements, kTrackWinKeyframes, kTrackWinLandmarks, kTrackWinObservations, 0};
+        // ground capacity for every selected landmark: the candidate lists are 4 B per landmark
+        kba_track_caps caps{kTrackKeyframes, kTrackLandmarks, kTrackMeasurements, kTrackWinKeyframes, kTrackWinLandmarks, kTrackWinObservations,
+                            kTrackWinLandmarks};
         if (kba_track_create(handle_, &caps, int(track_cams_.size()), intr.data(), pose.data(), &track_) != KBA_OK) return false;
         for (int i = kTrackKeyframes - 1; i >= 0; --i) free_kf_slots_.push_back(i);
     }
@@ -433,8 +435,6 @@ bool BundleAdjusterKeyframes::trackPush(const Keyframe& kf) {
 // solve() on the device-resident window: only the selection goes up.  false: not possible for this window (caller rebuilds).
 bool BundleAdjusterKeyframes::solveTracked(const std::vector<Keyframe*>& kfs, const std::vector<LandmarkId>& lm_ids, std::string& report) {
     if (int(kfs.size()) > kTrackWinKeyframes || int(lm_ids.size()) > kTrackWinLandmarks) return false;
-    for (const auto lm_id : lm_ids)
-        if (landmarks_.at(lm_id)->is_ground_plane) return false;  // ground-plane residuals: plane blocks, rebuild path
     for (const Keyframe* kf : kfs)
         if (!kf_slot_.count(kf->timestamp_) && !trackPush(*kf)) { track_failed_ = true; return false; }
     // state the host may have changed since the last solve: poses / planes of the active keyframes, new landmarks, weights
@@ -456,8 +456,15 @@ bool BundleAdjusterKeyframes::solveTracked(const std::vector<Keyframe*>& kfs, co
         if (it == lm_slot_.end()) return false;  // selected but never measured by a stored keyframe: let the rebuild path decide
         lm_slots.push_back(it->second);
     }
+    // addGroundPlaneResiduals (cpp:517-562) on the device: the selected ground-plane landmarks go up as candidates, the store's
+    // poses, planes and positions decide which are attached to which keyframe
+    std::vector<int32_t> gp_cand;
+    for (int j = 0; j < n_lm; ++j)
+        if (landmarks_.at(lm_ids[j])->is_ground_plane) gp_cand.push_back(j);
     kba_window sel{};
     sel.n_kf = n_kf; sel.n_lm = n_lm;
+    sel.n_gp = int(gp_cand.size()); sel.gp_lm = gp_cand.data();
+    sel.plane_reg_weight = gp_cand.empty() ? 0. : -1.;  // -1: 10 iff a ground-plane residual is attached (cpp:717-719)
     sel.scale_kf0 = 0; sel.scale_kf1 = 1;
     sel.scale_weight = -1.;  // the reference's rule (cpp:703-716), evaluated on the device from the gathered window
     sel.scale_value = n_kf > 1 ? (kfs[1]->getEigenPose() * kfs[0]->getEigenPose().inverse()).translation().norm() : 0.;
@@ -466,13 +473,18 @@ bool BundleAdjusterKeyframes::solveTracked(const std::vector<Keyframe*>& kfs, co
     kba_result r{};
     r.kf_pose = out_pose.data(); r.kf_plane = out_plane.data(); r.lm_pos = out_lm.data();
     const int rc = kba_track_solve(track_, n_kf, kf_slots.data(), fixed.data(), n_lm, lm_slots.data(), &sel, &opt, &r);
-    if (rc == KBA_ERR_CAPACITY) return false;  // e.g. more observations than the store's window capacity: rebuild
+    // e.g. more observations than the store's window capacity, or more than 18 keyframes with ground-plane candidates: rebuild
+    if (rc == KBA_ERR_CAPACITY) return false;
     if (rc != KBA_OK) throw std::runtime_error(std::string("kba_b200: ") + kba_last_error());
     int64_t h2d = 0, d2h = 0, pushes = 0;
     kba_track_transfer_bytes(track_, &h2d, &d2h, &pushes);
     push_h2d_ = (long long)pushes;
     last_solve_h2d_ = (long long)h2d + (long long)n_kf * (7 + 4) * 8;  // the selection lists + the active keyframes' poses
-    for (int k = 0; k < n_kf; ++k) std::copy_n(out_pose.begin() + 7 * k, 7, kfs[k]->pose_.begin());  // in place, as the reference (cpp:554-557)
+    for (int k = 0; k < n_kf; ++k) {  // in place, as the reference (cpp:554-557); planes nothing was attached to come back unchanged
+        std::copy_n(out_pose.begin() + 7 * k, 7, kfs[k]->pose_.begin());
+        std::copy_n(out_plane.begin() + 4 * k, 3, kfs[k]->local_ground_plane_.direction.begin());
+        kfs[k]->local_ground_plane_.distance = out_plane[4 * k + 3];
+    }
     for (int j = 0; j < n_lm; ++j) std::copy_n(out_lm.begin() + 3 * j, 3, landmarks_.at(lm_ids[j])->pos.begin());
     report = solve_report(r, " (device-resident window)");
     return true;

@@ -675,7 +675,11 @@ int kba_enable_kernel_timing(kba_handle* h, int on) {
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
-int kba_batch_create(kba_handle* h, int32_t n_windows, const kba_window* w, kba_batch** out) {
+static int batch_upload(kba_batch* b, int32_t n_windows, const kba_window* w, const int* rows);
+
+// rows[i] (optional): reduced-system rows window i is sized for, instead of 6 per keyframe (10 with plane blocks) + 1.  A track's
+// capacity window uses it: it has room for all its keyframes without plane blocks, or for 18 of them with plane blocks.
+static int batch_create(kba_handle* h, int32_t n_windows, const kba_window* w, const int* rows_of, kba_batch** out) {
     if (!h || !w || !out || n_windows <= 0) return fail(KBA_ERR_BAD_ARG, "bad argument to kba_batch_create");
     CU(cudaSetDevice(h->device));
     std::string why;
@@ -705,7 +709,7 @@ int kba_batch_create(kba_handle* h, int32_t n_windows, const kba_window* w, kba_
         d.scale_kf0 = w[i].scale_kf0; d.scale_kf1 = w[i].scale_kf1;
         d.scale_weight = w[i].scale_weight; d.scale_value = w[i].scale_value;
         const bool planes = w[i].n_gp > 0 || w[i].plane_reg_weight > 0;
-        const int rows = (planes ? 10 : 6) * w[i].n_kf + 1;
+        const int rows = rows_of ? rows_of[i] : (planes ? 10 : 6) * w[i].n_kf + 1;
         max_rows = std::max(max_rows, rows);
         d.nr_cap = ((rows + 63) / 64) * 64;
         d.plane_reg_weight = w[i].plane_reg_weight; d.plane_dist_fixed = w[i].plane_dist_fixed;
@@ -867,12 +871,19 @@ int kba_batch_create(kba_handle* h, int32_t n_windows, const kba_window* w, kba_
         if (e != cudaSuccess) { b->release(); delete b; return fail(KBA_ERR_CUDA, cudaGetErrorString(e)); }
     }
     *out = b;
-    const int rc = kba_batch_upload(b, n_windows, w);
+    const int rc = batch_upload(b, n_windows, w, rows_of);
     if (rc != KBA_OK) { b->release(); delete b; *out = nullptr; }
     return rc;
 }
 
-int kba_batch_upload(kba_batch* b, int32_t n_windows, const kba_window* w) {
+int kba_batch_create(kba_handle* h, int32_t n_windows, const kba_window* w, kba_batch** out) {
+    return batch_create(h, n_windows, w, nullptr, out);
+}
+
+int kba_batch_upload(kba_batch* b, int32_t n_windows, const kba_window* w) { return batch_upload(b, n_windows, w, nullptr); }
+
+// rows: as for batch_create
+static int batch_upload(kba_batch* b, int32_t n_windows, const kba_window* w, const int* rows_of) {
     if (!b || !w || n_windows != b->bd.n_win) return fail(KBA_ERR_BAD_ARG, "bad argument to kba_batch_upload");
     CU(cudaSetDevice(b->h->device));  // callers may drive several handles from several host threads
     for (int i = 0; i < n_windows; ++i) {
@@ -885,7 +896,8 @@ int kba_batch_upload(kba_batch* b, int32_t n_windows, const kba_window* w) {
                                          "residuals) differ from kba_batch_create");
         // the reduced system was sized at create: 6 rows per keyframe, 10 with plane blocks
         const bool planes = w[i].n_gp > 0 || w[i].plane_reg_weight > 0;
-        if (((planes ? 10 : 6) * w[i].n_kf + 1 + 63) / 64 * 64 > d.nr_cap)
+        const int rows = rows_of ? rows_of[i] : (planes ? 10 : 6) * w[i].n_kf + 1;
+        if ((rows + 63) / 64 * 64 > d.nr_cap)
             return fail(KBA_ERR_BAD_ARG, "kba_batch_upload: window " + std::to_string(i) + " needs plane blocks the batch was not created with");
     }
     // packing (landmark sort, observation permutation, keyframe-major copy) is independent per window: host threads
@@ -1352,14 +1364,20 @@ void kba_track_destroy(kba_track* t) {
 // kernels run once on this window (create = upload), and their per-landmark loops (insertion sort of a track, k_track_sort /
 // k_pack_obs) are written for tracks of a few dozen observations -- one landmark carrying all 2^18 of them kept a single GPU
 // thread busy for minutes.
+// Its reduced system is sized for the larger of its windows without plane blocks (6 rows per keyframe) and with them (10 rows per
+// keyframe, for at most kTrackPlaneKf keyframes): 192 rows at 30 keyframes, the fused path.
+constexpr int kFusedMaxRows = 184;                         // small_syrk: every window of the batch within 184 reduced rows
+constexpr int kTrackPlaneKf = (kFusedMaxRows - 1) / 10;    // 18 keyframes with plane blocks
 struct CapacityWindow {
     std::vector<double> pose, plane, lmp, lmw, gw;
     std::vector<uint8_t> fixed;
     std::vector<int32_t> ptr, okf, gl, gk;
     std::vector<float> u, v, d;
     kba_window w{};
+    int rows = 0;
     CapacityWindow(const kba_track_caps& c, int n_cam, const double* cam_intr, const double* cam_pose) {
         const int K = c.win_keyframes, L = c.win_landmarks, O = c.win_observations, G = c.win_ground;
+        rows = std::max(6 * K + 1, G > 0 ? 10 * std::min(K, kTrackPlaneKf) + 1 : 0);
         pose.assign(7 * (size_t)K, 0.0); plane.assign(4 * (size_t)K, 0.0); lmp.assign(3 * (size_t)L, 0.0); lmw.assign(L, 1.0);
         gw.assign(std::max(G, 1), 1.0);
         fixed.assign(K, 0);
@@ -1391,7 +1409,17 @@ struct TrackRequest {
     const int32_t* lm_slot = nullptr;
     const kba_window* sel = nullptr;       // nullptr: the track sits a group solve out
     int max_meas = 0, n_free = 0;          // filled by track_check: largest keyframe measurement count, free keyframes
+    bool device_gp = false;                // filled by track_check: sel->gp_lm lists candidates, attached by k_track_ground
 };
+
+// ground points attached on the device: candidates in gp_lm, no keyframes or weights
+static bool device_attached(const kba_window* sel) { return sel->n_gp > 0 && sel->gp_lm && !sel->gp_kf && !sel->gp_weight; }
+
+// plane_reg_weight < 0: the reference's rule (cpp:717-719), 10 iff a ground-plane residual is in the window.  Host lists resolve
+// it here; with candidates k_track_ground resolves it from the residuals it keeps.
+static double plane_reg_weight(const kba_window* sel) {
+    return sel->plane_reg_weight < 0 ? (sel->n_gp > 0 ? 10.0 : 0.0) : sel->plane_reg_weight;
+}
 
 // every argument check of a track solve, before anything is uploaded or launched
 static int track_check(const kba_track* t, TrackRequest& q, std::string& why) {
@@ -1413,13 +1441,26 @@ static int track_check(const kba_track* t, TrackRequest& q, std::string& why) {
     if (n_meas > c.win_observations) { why = "more observations than win_observations"; return KBA_ERR_CAPACITY; }
     for (int j = 0; j < q.n_lm; ++j)
         if (q.lm_slot[j] < 0 || q.lm_slot[j] >= t->td.lm_cap) { why = "landmark slot out of range"; return KBA_ERR_BAD_ARG; }
-    for (int g = 0; g < sel->n_gp; ++g)
-        if (!sel->gp_lm || !sel->gp_kf || !sel->gp_weight || sel->gp_lm[g] < 0 || sel->gp_lm[g] >= q.n_lm || sel->gp_kf[g] < 0 ||
-            sel->gp_kf[g] >= q.n_kf) {
-            why = "ground-plane index out of range"; return KBA_ERR_BAD_ARG;
-        }
+    q.device_gp = device_attached(sel);
+    if (q.device_gp) {
+        for (int g = 0; g < sel->n_gp; ++g)
+            if (sel->gp_lm[g] < 0 || sel->gp_lm[g] >= q.n_lm || (g > 0 && sel->gp_lm[g] <= sel->gp_lm[g - 1])) {
+                why = "ground-plane candidates must be strictly ascending indices into lm_slot"; return KBA_ERR_BAD_ARG;
+            }
+    } else {
+        for (int g = 0; g < sel->n_gp; ++g)
+            if (!sel->gp_lm || !sel->gp_kf || !sel->gp_weight || sel->gp_lm[g] < 0 || sel->gp_lm[g] >= q.n_lm || sel->gp_kf[g] < 0 ||
+                sel->gp_kf[g] >= q.n_kf) {
+                why = "ground-plane index out of range (or only one of gp_kf / gp_weight given)"; return KBA_ERR_BAD_ARG;
+            }
+    }
     const bool planes = sel->n_gp > 0 || sel->plane_reg_weight > 0;
     if (planes && c.win_ground == 0) { why = "the track was created without ground-plane capacity"; return KBA_ERR_CAPACITY; }
+    // a request that can carry plane blocks stays on the fused path with all its keyframes (kba_batch_create's small_syrk rule)
+    if ((sel->n_gp > 0 || sel->plane_reg_weight != 0) && 10 * q.n_kf + 1 > kFusedMaxRows) {
+        why = "more than 18 keyframes with ground-plane blocks (184 reduced rows) -- such windows go through kba_solve_window";
+        return KBA_ERR_CAPACITY;
+    }
     if (sel->scale_weight != 0 && (sel->scale_kf0 < 0 || sel->scale_kf0 >= q.n_kf || sel->scale_kf1 < 0 || sel->scale_kf1 >= q.n_kf)) {
         why = "scale regulariser keyframe out of range"; return KBA_ERR_BAD_ARG;
     }
@@ -1429,18 +1470,22 @@ static int track_check(const kba_track* t, TrackRequest& q, std::string& why) {
 // the window descriptor of a checked request (n_obs is written by the gather kernels); offsets and capacities stay as created
 static void track_desc(WinDesc& d, const kba_track* t, const TrackRequest& q) {
     const kba_window* sel = q.sel;
-    d.n_kf = q.n_kf; d.n_lm = q.n_lm; d.n_obs = 0; d.n_gp = sel->n_gp;
+    d.n_kf = q.n_kf; d.n_lm = q.n_lm; d.n_obs = 0;
+    d.n_gp = q.device_gp ? 0 : sel->n_gp;  // candidates: k_track_ground writes the count it keeps
     d.n_chunks = (q.n_lm + 31) / 32; d.n_groups = (q.n_lm + 7) / 8;
     d.scale_kf0 = sel->scale_kf0; d.scale_kf1 = sel->scale_kf1; d.scale_weight = sel->scale_weight; d.scale_value = sel->scale_value;
-    d.plane_reg_weight = sel->plane_reg_weight; d.plane_dist_fixed = sel->plane_dist_fixed; d.landmarks_fixed = 0;
+    d.plane_reg_weight = q.device_gp ? sel->plane_reg_weight : plane_reg_weight(sel);
+    d.plane_dist_fixed = sel->plane_dist_fixed; d.landmarks_fixed = 0;
     d.speed_kf = 0; d.speed_weight = 0; d.speed_dt = 1;
     d.max_rank = t->n_cam > 1 ? t->n_cam - 1 : 0;  // a rig may see a landmark from several cameras of one keyframe
     d.idle = 0;
 }
 
-// fused Schur kernel instance a checked request needs (kba_batch_create's rule on its free keyframes)
+// fused Schur kernel instance a checked request needs (kba_batch_create's rule on its free keyframes).  The launch configuration is
+// fixed before the gather, so a request with candidates counts plane rows even if none of them is attached: an 18-free-keyframe
+// window with nothing attached runs the seven-slot kernel where kba_solve_window runs the six-slot one (and rounds differently).
 static int track_fused_slots(const TrackRequest& q) {
-    const bool planes = q.sel->n_gp > 0 || q.sel->plane_reg_weight > 0;
+    const bool planes = q.device_gp || q.sel->n_gp > 0 || plane_reg_weight(q.sel) > 0;
     return ((planes ? 10 : 6) * q.n_free + 1 <= 176) ? 6 : 7;
 }
 
@@ -1456,10 +1501,11 @@ static void idle_result(kba_result& r) {
     r.initial_cost = 0.0; r.final_cost = 0.0; r.time_sec = 0.0;
 }
 
-static TrackSel track_sel(const TrackRequest& q, const int* kf_slot_d, const uint8_t* kf_fixed_d, const int* lm_slot_d) {
+static TrackSel track_sel(const TrackRequest& q, const int* kf_slot_d, const uint8_t* kf_fixed_d, const int* lm_slot_d, const int* cand_d) {
     TrackSel ts;
     ts.kf_slot = kf_slot_d; ts.kf_fixed = kf_fixed_d; ts.lm_slot = lm_slot_d; ts.n_kf = q.n_kf; ts.n_lm = q.n_lm; ts.max_meas = q.max_meas;
     ts.auto_scale = q.sel->scale_weight < 0 ? 1 : 0;
+    if (q.device_gp) { ts.gp_cand = cand_d; ts.n_cand = q.sel->n_gp; }
     return ts;
 }
 
@@ -1468,14 +1514,16 @@ static TrackSel track_sel(const TrackRequest& q, const int* kf_slot_d, const uin
 static int track_solver_create(kba_handle* h, int n, kba_track* const* ts, TrackSolver& sv, const std::string& who) {
     std::vector<std::unique_ptr<CapacityWindow>> cws;
     std::vector<kba_window> ws;
+    std::vector<int> rows;
     size_t list_ints = 0;
     for (int i = 0; i < n; ++i) {
         const kba_track* t = ts[i];
         cws.emplace_back(new CapacityWindow(t->caps, t->n_cam, t->cam_intr.data(), t->cam_pose.data()));
         ws.push_back(cws.back()->w);
-        list_ints += (size_t)t->caps.win_keyframes + t->caps.win_landmarks + (t->caps.win_keyframes + 3) / 4;
+        rows.push_back(cws.back()->rows);
+        list_ints += (size_t)t->caps.win_keyframes + t->caps.win_landmarks + (t->caps.win_keyframes + 3) / 4 + t->caps.win_ground;
     }
-    const int rc = kba_batch_create(h, n, ws.data(), &sv.batch);
+    const int rc = batch_create(h, n, ws.data(), rows.data(), &sv.batch);
     if (rc != KBA_OK) return rc;
     if (!sv.batch->device_pack) { sv.release(); return fail(KBA_ERR_CAPACITY, who + ": device packing is disabled (KBA_FUSED / KBA_DEVICE_PACK)"); }
     int bad = 0;
@@ -1489,9 +1537,9 @@ int kba_track_create(kba_handle* h, const kba_track_caps* c, int32_t n_cam, cons
     if (c->max_keyframes < 3 || c->max_landmarks < 1 || c->max_measurements < 1 || c->win_keyframes < 3 || c->win_landmarks < 1 ||
         c->win_observations < 1 || c->win_ground < 0 || c->win_ground > c->win_landmarks)
         return fail(KBA_ERR_BAD_ARG, "kba_track_create: capacities");
-    if ((c->win_ground > 0 ? 10 : 6) * c->win_keyframes + 1 > 184 || c->win_keyframes > kFusedMaxKf || c->win_landmarks > pack_max_landmarks())
-        return fail(KBA_ERR_CAPACITY, "kba_track_create: the stored window must fit the fused path (<= 184 reduced rows: 30 keyframes, "
-                                      "18 with ground-plane blocks; <= 32768 landmarks) -- larger windows go through kba_solve_window");
+    if (6 * c->win_keyframes + 1 > kFusedMaxRows || c->win_keyframes > kFusedMaxKf || c->win_landmarks > pack_max_landmarks())
+        return fail(KBA_ERR_CAPACITY, "kba_track_create: the stored window must fit the fused path (<= 184 reduced rows: 30 keyframes; "
+                                      "<= 32768 landmarks) -- larger windows go through kba_solve_window");
     CU(cudaSetDevice(h->device));
     kba_track* t = new kba_track();
     t->h = h; t->caps = *c; t->n_cam = n_cam;
@@ -1663,22 +1711,26 @@ static int track_solve(kba_handle* h, TrackSolver& sv, int n, kba_track* const* 
             track_desc(d, t, q);
             max_rank = std::max(max_rank, d.max_rank);
             slots = std::max(slots, track_fused_slots(q));
+            // lists: keyframe slots | landmark slots | fixation bytes | ground-plane candidates
+            const kba_window* sel = q.sel;
+            const int n_cand = q.device_gp ? sel->n_gp : 0, fixed_ints = (q.n_kf + 3) / 4;
             int* l = sv.lists.h + used;
             memcpy(l, q.kf_slot, q.n_kf * sizeof(int));
             memcpy(l + q.n_kf, q.lm_slot, q.n_lm * sizeof(int));
             memcpy(l + q.n_kf + q.n_lm, q.kf_fixed, q.n_kf);
+            if (n_cand) memcpy(l + q.n_kf + q.n_lm + fixed_ints, sel->gp_lm, n_cand * sizeof(int));
             const int* ld = sv.lists.d + used;
-            sv.tsel.h[i] = track_sel(q, ld, reinterpret_cast<const uint8_t*>(ld + q.n_kf + q.n_lm), ld + q.n_kf);
-            used += (size_t)q.n_kf + q.n_lm + (q.n_kf + 3) / 4;
-            const kba_window* sel = q.sel;
-            if (sel->n_gp) {
+            sv.tsel.h[i] = track_sel(q, ld, reinterpret_cast<const uint8_t*>(ld + q.n_kf + q.n_lm), ld + q.n_kf, ld + q.n_kf + q.n_lm + fixed_ints);
+            used += (size_t)q.n_kf + q.n_lm + fixed_ints + n_cand;
+            if (sel->n_gp && !q.device_gp) {
                 memcpy(b->r_gp_lm.h + d.gp_off, sel->gp_lm, sel->n_gp * sizeof(int)); memcpy(b->gp_kf.h + d.gp_off, sel->gp_kf, sel->n_gp * sizeof(int));
                 memcpy(b->gp_weight.h + d.gp_off, sel->gp_weight, sel->n_gp * sizeof(double));
                 any_gp = true;
             }
             grid.max_kf = std::max(grid.max_kf, q.n_kf); grid.max_lm = std::max(grid.max_lm, q.n_lm);
             grid.max_meas = std::max(grid.max_meas, q.max_meas);
-            h2d += (int64_t)q.n_kf * 5 + (int64_t)q.n_lm * 4 + (int64_t)sel->n_gp * 16;
+            grid.any_cand |= n_cand > 0;
+            h2d += (int64_t)q.n_kf * 5 + (int64_t)q.n_lm * 4 + (q.device_gp ? (int64_t)n_cand * 4 : (int64_t)sel->n_gp * 16);
         }
         b->desc.h[i] = d;
     }

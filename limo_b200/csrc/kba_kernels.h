@@ -90,10 +90,13 @@ struct TrackSel {
     const int* lm_slot = nullptr;    // [n_lm] ascending landmark id
     int n_kf = 0, n_lm = 0, max_meas = 0;  // n_kf = n_lm = 0: the window is idle (WinDesc::idle)
     int auto_scale = 0;              // 1: scale-regulariser weight by the reference rule (cpp:703-716) from the gathered window
+    const int* gp_cand = nullptr;    // [n_cand] candidate ground points (index into lm_slot, ascending), attached by k_track_ground
+    int n_cand = 0;                  // 0: the window's ground-plane lists (if any) came from the host
 };
 // grid sizes of the gather / write-back launches: maxima over the windows of the batch
 struct TrackGrid {
     int max_kf = 0, max_lm = 0, max_meas = 0;
+    int any_cand = 0;                // some window attaches its ground points on the device
 };
 // builds the raw CSR of every window w of batch `bd` (its PackRaw inputs) from track store tds[w] and selection sels[w]
 // (device arrays of bd.n_win entries); desc[w].n_obs is written on the device

@@ -11,6 +11,7 @@
 //   k_pack_gp        : ground-plane residuals follow their landmark; shared-row flags
 //   k_pack_groups    : keyframe range of every 8-landmark group
 // Integer work only; every kernel is a streaming pass over 4-byte words (a config-2 window: 40k observations x ~50 B).
+#include <cfloat>
 #include <cstdint>
 
 #include <cuda_runtime.h>
@@ -242,6 +243,94 @@ __global__ void __launch_bounds__(256) k_track_begin(BatchDev bd, const TrackDev
     if (i == 0) *td.n_depth = 0;
 }
 
+// Ground points attached on the device: addGroundPlaneResiduals (reference bundle_adjuster_keyframes.cpp:517-562) on the gathered
+// window, for a window whose request lists candidate ground landmarks (TrackSel::gp_cand) instead of host-built lists.  One CTA per
+// window, after k_track_begin (poses, planes, positions gathered) and before k_track_scan (the scale rule reads n_gp).  A candidate
+// goes to the first keyframe, in window order, of strictly smallest distance |R(q) p + t| among those whose plane distance is not
+// below -10, and is kept iff that distance is under 25 m, with weight 10 (1 - d / 25).  The kept ones are compacted in candidate
+// order by an ordered block scan.  The arithmetic is the facade's host code operation for operation (mini_eigen.hpp: convert()
+// of the 7-vector, Eigen's un-normalised toRotationMatrix, R * p + t, the square root of the squared norm; g++ -O2 without FMA):
+// explicit round-to-nearest intrinsics, so that nothing is contracted and the lists equal the host's bit for bit.
+__device__ __forceinline__ double gp_mul(double a, double b) { return __dmul_rn(a, b); }
+__device__ __forceinline__ double gp_add(double a, double b) { return __dadd_rn(a, b); }
+__device__ __forceinline__ double gp_sub(double a, double b) { return __dsub_rn(a, b); }
+
+__global__ void __launch_bounds__(256) k_track_ground(BatchDev bd, const TrackSel* sels, const double* r_lm_pos, int* r_gp_lm) {
+    const int w = blockIdx.x;
+    const TrackSel& sel = sels[w];
+    if (sel.n_cand == 0) return;  // idle, plane-free or host lists: untouched
+    WinDesc& d = bd.desc[w];
+    __shared__ double s_T[kFusedMaxKf][12];  // R row-major, t
+    __shared__ int s_use[kFusedMaxKf];
+    __shared__ int s_warp[8];
+    __shared__ int s_base;
+    const int tid = threadIdx.x, lane = tid & 31, wp = tid >> 5, n_kf = sel.n_kf;
+    if (tid < n_kf) {
+        const double* q = bd.pose0 + 7 * ((size_t)d.kf_off + tid);
+        const double qw = q[0], qx = q[1], qy = q[2], qz = q[3];
+        const double tx = gp_mul(2.0, qx), ty = gp_mul(2.0, qy), tz = gp_mul(2.0, qz);
+        const double twx = gp_mul(tx, qw), twy = gp_mul(ty, qw), twz = gp_mul(tz, qw);
+        const double txx = gp_mul(tx, qx), txy = gp_mul(ty, qx), txz = gp_mul(tz, qx);
+        const double tyy = gp_mul(ty, qy), tyz = gp_mul(tz, qy), tzz = gp_mul(tz, qz);
+        const double Rq[9] = {gp_sub(1.0, gp_add(tyy, tzz)), gp_sub(txy, twz), gp_add(txz, twy),
+                              gp_add(txy, twz), gp_sub(1.0, gp_add(txx, tzz)), gp_sub(tyz, twx),
+                              gp_sub(txz, twy), gp_add(tyz, twx), gp_sub(1.0, gp_add(txx, tyy))};
+        // convert(): Identity().translate(t).rotate(q); the products with the identity are kept (they decide the inf / NaN cases)
+        double* T = s_T[tid];
+        for (int i = 0; i < 3; ++i) {
+            for (int j = 0; j < 3; ++j) {
+                double s = 0.0;
+                for (int k = 0; k < 3; ++k) s = gp_add(s, gp_mul(i == k ? 1.0 : 0.0, Rq[3 * k + j]));
+                T[3 * i + j] = s;
+            }
+            const double Iv = gp_add(gp_add(gp_mul(i == 0 ? 1.0 : 0.0, q[4]), gp_mul(i == 1 ? 1.0 : 0.0, q[5])), gp_mul(i == 2 ? 1.0 : 0.0, q[6]));
+            T[9 + i] = gp_add(0.0, Iv);
+        }
+        s_use[tid] = !(bd.plane0[4 * ((size_t)d.kf_off + tid) + 3] < -10.0);
+    }
+    if (tid == 0) s_base = 0;
+    __syncthreads();
+    const size_t go = (size_t)d.gp_off;
+    for (int c0 = 0; c0 < sel.n_cand; c0 += 256) {
+        const int c = c0 + tid;
+        int j = 0, best = 0;
+        double md = DBL_MAX;
+        if (c < sel.n_cand) {
+            j = sel.gp_cand[c];
+            const double* p = r_lm_pos + 3 * ((size_t)d.lm_off + j);
+            const double px = p[0], py = p[1], pz = p[2];
+            for (int k = 0; k < n_kf; ++k) {
+                if (!s_use[k]) continue;
+                const double* T = s_T[k];
+                const double x = gp_add(gp_add(gp_add(gp_mul(T[0], px), gp_mul(T[1], py)), gp_mul(T[2], pz)), T[9]);
+                const double y = gp_add(gp_add(gp_add(gp_mul(T[3], px), gp_mul(T[4], py)), gp_mul(T[5], pz)), T[10]);
+                const double z = gp_add(gp_add(gp_add(gp_mul(T[6], px), gp_mul(T[7], py)), gp_mul(T[8], pz)), T[11]);
+                const double dist = __dsqrt_rn(gp_add(gp_add(gp_mul(x, x), gp_mul(y, y)), gp_mul(z, z)));
+                if (dist < md) { md = dist; best = k; }  // first strict minimum; a NaN never is one
+            }
+        }
+        const bool keep = md < 25.0;  // false past the list and when no keyframe qualified
+        const unsigned m = __ballot_sync(0xffffffffu, keep);
+        if (lane == 0) s_warp[wp] = __popc(m);
+        __syncthreads();
+        int before = 0, total = 0;
+        for (int q = 0; q < 8; ++q) { const int n = s_warp[q]; if (q < wp) before += n; total += n; }
+        if (keep) {
+            const size_t G = go + s_base + before + __popc(m & ((1u << lane) - 1));
+            r_gp_lm[G] = j;
+            bd.gp_kf[G] = best;
+            bd.gp_weight[G] = gp_mul(10.0, gp_sub(1.0, __ddiv_rn(md, 25.0)));
+        }
+        __syncthreads();
+        if (tid == 0) s_base += total;
+        __syncthreads();
+    }
+    if (tid == 0) {
+        d.n_gp = s_base;
+        if (d.plane_reg_weight < 0) d.plane_reg_weight = s_base > 0 ? 10.0 : 0.0;  // cpp:717-719
+    }
+}
+
 // pass 0: observations per selected landmark; pass 1: scatter behind the CSR pointers (order fixed afterwards by k_track_sort)
 template <int kPass>
 __global__ void __launch_bounds__(256) k_track_scatter(BatchDev bd, PackRaw raw, const TrackDev* tds, const TrackSel* sels, int* r_cnt,
@@ -382,6 +471,7 @@ void launch_track_gather(const BatchDev& bd, const PackRaw& raw, const TrackDev*
     const int B = bd.n_win;
     const int n = g.max_kf > g.max_lm ? g.max_kf : g.max_lm;
     k_track_begin<<<dim3((n + 255) / 256 > 0 ? (n + 255) / 256 : 1, B), 256, 0, s>>>(bd, tds, sels, r_pos, r_w, r_cnt); LCHK("k_track_begin");
+    if (g.any_cand) { k_track_ground<<<B, 256, 0, s>>>(bd, sels, r_pos, const_cast<int*>(raw.gp_lm)); LCHK("k_track_ground"); }
     const dim3 gm((g.max_meas + 255) / 256 > 0 ? (g.max_meas + 255) / 256 : 1, g.max_kf > 0 ? g.max_kf : 1, B);
     k_track_scatter<0><<<gm, 256, 0, s>>>(bd, raw, tds, sels, r_cnt, r_kf, r_cam, r_u, r_v, r_d); LCHK("k_track_scatter");
     k_track_scan<<<B, 1024, 0, s>>>(bd, tds, sels, r_cnt, r_lm_ptr); LCHK("k_track_scan");
