@@ -8,10 +8,15 @@
 //                          landmark-column-major, and a track without gaps sits on consecutive rows, so a landmark's panel
 //                          column is ONE bulk copy (cp.async.bulk, 48 B per observation, complete_tx on the stage's "full"
 //                          mbarrier): 24 bulk copies + the z rows per group, nobody waits for data and the ring runs five
-//                          groups ahead.  Alternatives tried and dropped: zero segments as bulk copies too (no stores by the
-//                          SM at all, but a warp issues its bulk copies one lane after the other), 16-byte cp.async per lane
-//                          instead of bulk copies.  Landmarks whose rows are not one run fall back to nine 16-byte
-//                          cp.async per observation; windows with ground-plane rows or several cameras per keyframe (rows
+//                          groups ahead.  A stage is not zeroed whole: per stage and panel column a small table keeps the
+//                          rows that the group last assembled there may have left non-zero (its run and z row; every row of
+//                          its panel on the per-observation and synchronous paths), and the column's lane zeroes those rows
+//                          minus the ones its own bulk copy overwrites.  Alternatives tried and dropped: all 32 lanes
+//                          zeroing row-parallel around the runs (one shuffle per column for the run bounds, which queue
+//                          behind the consumers' shared-memory loads: slower than zeroing everything), zero segments as
+//                          bulk copies too (no stores by the SM at all, but a warp issues its bulk copies one lane after
+//                          the other), 16-byte cp.async per lane instead of bulk copies.  Landmarks whose rows are not one
+//                          run fall back to nine 16-byte cp.async per observation; windows with ground-plane rows or several cameras per keyframe (rows
 //                          that ADD onto others) take a synchronous variant of the same loop.
 //   consumers (12 warps) : Sred += V V^T on the FP64 tensor cores (mma.sync m16n8k8 / m16n8k4: on sm_90 they issue at twice
 //                          the FLOP rate of m8n8k4, scripts/dmma_rate.cu).  The whole lower triangle lives in the consumers'
@@ -76,7 +81,13 @@ __device__ __forceinline__ void reg_dec() { asm volatile("setmaxnreg.dec.sync.al
 template <int N>
 __device__ __forceinline__ void reg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
 
-constexpr size_t schur_fused_smem() { return (size_t)kFStages * kFStageDoubles * sizeof(double) + 24 * sizeof(uint64_t); }
+// stages, then 24 mbarrier slots, then the dirty-row table (one word per stage and panel column)
+constexpr size_t schur_fused_smem() {
+    return (size_t)kFStages * kFStageDoubles * sizeof(double) + 24 * sizeof(uint64_t) + kFStages * kGC * sizeof(unsigned);
+}
+// dirty-row table entry, in double2 rows of a panel column: rows [a, b) and row z (kNoRow: none) may be non-zero
+constexpr unsigned kNoRow = 0xff;
+__device__ __forceinline__ unsigned dirty_rows(int a, int b, unsigned z) { return (unsigned)a | (unsigned)b << 8 | z << 16; }
 
 // KBA_PROF build: cycles per role (lane 0 of every warp, summed over CTAs into BatchDev::prof) --
 //   consumers: [0] waiting for a full panel, [1] multiplying;  producers: [4] waiting for an empty stage, [5] zero fill +
@@ -170,6 +181,7 @@ __global__ void __launch_bounds__(512, 1) k_schur_fused(BatchDev bd) {
     double* stage = reinterpret_cast<double*>(fsm);
     uint64_t* full = reinterpret_cast<uint64_t*>(fsm + (size_t)kFStages * kFStageDoubles * sizeof(double));
     uint64_t* empty = full + kFStages;
+    unsigned* dirty = reinterpret_cast<unsigned*>(full + 24);
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int n_f = st.n_f, nt = (n_f + 8) >> 3, trhs = n_f >> 3;
     int per, used;
@@ -184,6 +196,8 @@ __global__ void __launch_bounds__(512, 1) k_schur_fused(BatchDev bd) {
         for (int i = 0; i < kFStages; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], kFConsumerWarps); }
         asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // the barriers are armed by bulk copies (async proxy) too
     }
+    // shared memory starts undefined: the first group of every stage zeroes whole columns
+    for (int i = tid; i < kFStages * kGC; i += blockDim.x) dirty[i] = dirty_rows(0, kFMaxRs / 2, kNoRow);
     __syncthreads();
     auto next_group = [&](int g) { while (g < g1 && grs[g] == 0) ++g; return g; };
 
@@ -238,14 +252,29 @@ __global__ void __launch_bounds__(512, 1) k_schur_fused(BatchDev bd) {
             if (gi >= kFStages) mbar_wait(&empty[slot], ((gi / kFStages) - 1) & 1);
             KBA_PROF_ACC(0);
             double* sb = stage + (size_t)slot * kFStageDoubles;
-            {   // rs = rows of this group's panel (multiple of 8); the column stride is the constant kFMaxRs
-                const int h = rs >> 1;
-                for (int c = 0; c < kGC; ++c)
-                    for (int r2 = lane; r2 < h; r2 += 32) reinterpret_cast<double2*>(sb + (size_t)c * kFMaxRs)[r2] = make_double2(0.0, 0.0);
-            }
             // does every landmark of the group have its rows in one run that starts on an even panel row?
             const bool no_run = lane < 24 && (run0.y < 0 || (run0.y > 0 && ((run0.z - 8 * t0) & 1)));
             const bool bulk = __ballot_sync(0xffffffffu, no_run) == 0u && !sync_path;
+            if (lane < kGC) {
+                // The column lane zeroes what the stage's previous group may have left in its column (double2 rows) except
+                // the rows [s, e) its own bulk copy overwrites, and records what this group may leave: the run and the z
+                // row on the bulk path, every row of the panel (rs rows, a multiple of 8) otherwise.  Each lane stores
+                // on its own, so the stores issue back to back.  The table word was written before the previous group's
+                // "full" arrival and is read after this stage's "empty" wait, the same hand-over as the panel itself.
+                unsigned* dl = dirty + slot * kGC + lane;
+                const unsigned d = *dl;
+                int s = 0, e = 0;
+                if (bulk && run0.y > 0) { s = (run0.z - 8 * t0) >> 1; e = s + 3 * run0.y; }
+                const int zl = (trhs >= t0 && trhs < t1) ? n_f - 8 * t0 : 8 * (t1 - t0) + (n_f - 8 * trhs);  // z row rl below
+                *dl = bulk ? dirty_rows(s, e, (unsigned)(zl >> 1)) : dirty_rows(0, rs >> 1, kNoRow);
+                const int a = d & 0xff, b = (d >> 8) & 0xff, z = d >> 16;
+                const bool zero_z = z != (int)kNoRow && (z < a || z >= b) && (z < s || z >= e);
+                const int m1 = min(b, s), m2 = max(a, e);
+                double2* col = reinterpret_cast<double2*>(sb + (size_t)lane * kFMaxRs);
+                if (zero_z) col[z] = make_double2(0.0, 0.0);
+                for (int r2 = a; r2 < m1; ++r2) col[r2] = make_double2(0.0, 0.0);
+                for (int r2 = m2; r2 < b; ++r2) col[r2] = make_double2(0.0, 0.0);
+            }
             asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // the zeros (generic proxy) before the bulk copies (async proxy)
             __syncwarp();
             KBA_PROF_ACC(1);
