@@ -29,7 +29,7 @@ extern "C" {
 #endif
 
 #define KBA_VERSION_MAJOR 0
-#define KBA_VERSION_MINOR 1
+#define KBA_VERSION_MINOR 2
 
 /* ---- status codes (reference: C++ exceptions / text report, bundle_adjuster_keyframes.cpp:630-632) ---- */
 enum {
@@ -277,10 +277,12 @@ typedef struct kba_track_caps {
     int32_t max_keyframes;     /* keyframe slots in the store (active or not)        */
     int32_t max_landmarks;     /* landmark slots                                      */
     int32_t max_measurements;  /* arena entries over all stored keyframes             */
-    int32_t win_keyframes;     /* largest window: keyframes (<= 30: fused path; a solve with ground-plane blocks takes <= 18) */
+    int32_t win_keyframes;     /* largest window: keyframes (win_rows = 0: <= 30, and a solve with ground-plane blocks takes <= 18) */
     int32_t win_landmarks;     /*                 selected landmarks                  */
     int32_t win_observations;  /*                 observations                        */
     int32_t win_ground;        /*                 ground-plane residuals, or candidates of a device attachment (<= win_landmarks) */
+    int32_t win_rows;          /*                 reduced-system rows: 6 per keyframe, 10 with plane blocks, plus one.  0: the fused
+                                                  path's limits above; else 6 * win_keyframes + 1 .. 640, see kba_track_solve */
 } kba_track_caps;
 int kba_track_create(kba_handle* h, const kba_track_caps* caps, int32_t n_cam, const double* cam_intr, const double* cam_pose,
                      kba_track** out);
@@ -311,13 +313,24 @@ int kba_track_set_keyframe_poses(kba_track* t, int32_t n, const int32_t* kf_slot
  *     candidate instead of 16 B per residual, and need not keep landmark positions on the host.
  * plane_reg_weight < 0 asks for the reference's rule (cpp:717-719): 10 iff at least one ground-plane residual is in the window
  * (with either kind of lists).  Errors, all before anything is uploaded: only one of gp_kf / gp_weight NULL, candidates not
- * strictly ascending or out of range: KBA_ERR_BAD_ARG; more residuals or candidates than win_ground: KBA_ERR_CAPACITY; a request
- * that can carry plane blocks (ground-plane lists of either kind, or plane_reg_weight != 0) with 10 * n_kf + 1 > 184 (more than 18
- * keyframes): KBA_ERR_CAPACITY -- the rule by which kba_batch_create keeps a window on the fused path, so that the track and
- * kba_solve_window run the same solver.  solves[].num_residual_blocks counts the attached residuals; with nothing attached, kf_plane
- * comes back bit-equal to the stored planes, so a caller may always copy planes back.  One exception to bit-equality with
- * kba_solve_window: the Schur kernel variant is chosen before the attachment, counting plane rows whenever candidates are given,
- * so an 18-free-keyframe window with nothing attached runs the seven-slot kernel where kba_solve_window runs the six-slot one. */
+ * strictly ascending or out of range: KBA_ERR_BAD_ARG; more residuals or candidates than win_ground: KBA_ERR_CAPACITY.
+ * Window size: a request has rows = (planes ? 10 : 6) * n_kf + 1 reduced rows, where planes = n_gp > 0 or plane_reg_weight > 0.
+ *   - caps.win_rows = 0: a request that can carry plane blocks (ground-plane lists of either kind, or plane_reg_weight != 0) with
+ *     10 * n_kf + 1 > 184 (more than 18 keyframes) is KBA_ERR_CAPACITY -- the rule by which kba_batch_create keeps a window on the
+ *     fused path, so that the track and kba_solve_window run the same solver.
+ *   - caps.win_rows > 0: a request with rows > win_rows is KBA_ERR_CAPACITY.  A track with win_rows > 184 owns a second solver,
+ *     sized for win_keyframes and win_rows, on the large-window path (k_schur_syrk and the row-major or split factorisation),
+ *     packed on the device like the fused one.  Each solve goes to the solver kba_batch_create would choose for the window: the
+ *     fused one iff rows <= 184 (so windows that fit the fused path keep its results bit for bit), the large one otherwise.  The
+ *     Schur split, the factorisation and each window's system size follow the solved window, as kba_batch_create derives them.
+ * solves[].num_residual_blocks counts the attached residuals; with nothing attached, kf_plane comes back bit-equal to the stored
+ * planes, so a caller may always copy planes back.  One exception to bit-equality with kba_solve_window: the solver path and the
+ * Schur kernel variant are chosen before the attachment, counting plane rows whenever candidates are given.  With nothing attached
+ *   - an 18-free-keyframe window runs the seven-slot fused kernel where kba_solve_window runs the six-slot one;
+ *   - a window of 19 to 30 keyframes runs the large-window path where kba_solve_window, seeing a plane-free window, runs the fused
+ *     one.
+ * Such results agree with kba_solve_window to the solver's tolerances (translations to 1e-6 m, the cost to 1e-8 relative), not
+ * bit for bit. */
 int kba_track_solve(kba_track* t, int32_t n_kf, const int32_t* kf_slot, const uint8_t* kf_fixed, int32_t n_lm, const int32_t* lm_slot,
                     const kba_window* sel, const kba_options* opt, kba_result* res);
 int kba_track_transfer_bytes(kba_track* t, int64_t* h2d_last_solve, int64_t* d2h_last_solve, int64_t* h2d_pushes_total);
@@ -341,7 +354,8 @@ int kba_track_transfer_bytes(kba_track* t, int64_t* h2d_last_solve, int64_t* d2h
  *     a window's budget includes the time its group's other windows take.
  *   - Launch configuration, decided per solve from the windows that are solved: the largest rig rank, the seven-slot Schur
  *     kernel if any window needs more than 176 reduced rows, and from these the fused-linearisation switch, as kba_batch_solve
- *     decides for any batch.  A window in a mixed group can therefore run a different kernel variant than alone (e.g. a
+ *     decides for any batch.  The whole group takes the large-window path when one of its requests has more than 184 rows
+ *     (kba_track_solve), so the group owns a second solver iff one of its tracks has win_rows > 184.  A window in a mixed group can therefore run a different kernel variant than alone (e.g. a
  *     multi-camera rig turns the fused linearisation off for every window) and round differently in the last bits.
  *   - Skipping: a request with n_kf == 0 sits the solve out: its store is untouched, res[i] gets status KBA_OK and
  *     num_solves 0, its output arrays are not written.  A call in which every track sits out returns at once. */

@@ -168,9 +168,12 @@ class Track:
     the lists of active keyframe slots and selected landmark slots."""
 
     def __init__(self, handle, cam_intr, cam_pose, max_keyframes, max_landmarks, max_measurements, win_keyframes,
-                 win_landmarks, win_observations, win_ground=0):
+                 win_landmarks, win_observations, win_ground=0, win_rows=0):
+        """win_rows: largest reduced system a solve may need (6 rows per keyframe, 10 with plane blocks, plus one); 0 keeps the
+        fused path's limits (30 keyframes, 18 with plane blocks), beyond 184 the track also owns a large-window solver"""
         self.handle = handle
-        caps = KbaTrackCaps(max_keyframes, max_landmarks, max_measurements, win_keyframes, win_landmarks, win_observations, win_ground)
+        caps = KbaTrackCaps(max_keyframes, max_landmarks, max_measurements, win_keyframes, win_landmarks, win_observations, win_ground,
+                            win_rows)
         intr = np.ascontiguousarray(cam_intr, dtype=np.float64).reshape(-1, 3)
         pose = np.ascontiguousarray(cam_pose, dtype=np.float64).reshape(-1, 7)
         self._p = C.c_void_p()

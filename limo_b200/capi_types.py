@@ -34,7 +34,7 @@ class KbaWindow(C.Structure):
 class KbaTrackCaps(C.Structure):
     _fields_ = [("max_keyframes", C.c_int32), ("max_landmarks", C.c_int32), ("max_measurements", C.c_int32),
                 ("win_keyframes", C.c_int32), ("win_landmarks", C.c_int32), ("win_observations", C.c_int32),
-                ("win_ground", C.c_int32)]
+                ("win_ground", C.c_int32), ("win_rows", C.c_int32)]
 
 
 class KbaTrackRequest(C.Structure):

@@ -390,9 +390,11 @@ bool BundleAdjusterKeyframes::trackPush(const Keyframe& kf) {
             intr.insert(intr.end(), v.begin(), v.begin() + 3);
             pose.insert(pose.end(), v.begin() + 3, v.end());
         }
-        // ground capacity for every selected landmark: the candidate lists are 4 B per landmark
+        // ground capacity for every selected landmark: the candidate lists are 4 B per landmark.  Reduced rows for every window
+        // up to kTrackWinKeyframes with plane blocks: windows beyond 184 rows (19-30 keyframes with ground points, limo's default of
+        // 20 among them) take the track's large-window solver instead of the rebuild path
         kba_track_caps caps{kTrackKeyframes, kTrackLandmarks, kTrackMeasurements, kTrackWinKeyframes, kTrackWinLandmarks, kTrackWinObservations,
-                            kTrackWinLandmarks};
+                            kTrackWinLandmarks, 10 * kTrackWinKeyframes + 1};
         if (kba_track_create(handle_, &caps, int(track_cams_.size()), intr.data(), pose.data(), &track_) != KBA_OK) return false;
         for (int i = kTrackKeyframes - 1; i >= 0; --i) free_kf_slots_.push_back(i);
     }
@@ -473,7 +475,7 @@ bool BundleAdjusterKeyframes::solveTracked(const std::vector<Keyframe*>& kfs, co
     kba_result r{};
     r.kf_pose = out_pose.data(); r.kf_plane = out_plane.data(); r.lm_pos = out_lm.data();
     const int rc = kba_track_solve(track_, n_kf, kf_slots.data(), fixed.data(), n_lm, lm_slots.data(), &sel, &opt, &r);
-    // e.g. more observations than the store's window capacity, or more than 18 keyframes with ground-plane candidates: rebuild
+    // e.g. more observations than the store's window capacity: rebuild
     if (rc == KBA_ERR_CAPACITY) return false;
     if (rc != KBA_OK) throw std::runtime_error(std::string("kba_b200: ") + kba_last_error());
     int64_t h2d = 0, d2h = 0, pushes = 0;

@@ -137,6 +137,7 @@ struct kba_batch {
     } sg;
     Staged<int> loop_pass;  // passes the WHILE node has run (device counter + pinned copy)
     long long solves_done = 0;
+    int p_split_cap = 0;    // a track's large-window solver: the largest Schur split sred has room for
 
     template <typename T>
     int dev_alloc(T** p, size_t count) {
@@ -238,7 +239,9 @@ struct kba_track {
     kba_handle* h = nullptr;
     kba_track_caps caps{};
     int n_cam = 0;
-    TrackSolver solver;                    // window 0 of its batch is this track's window
+    TrackSolver solver;                    // window 0 of its batch is this track's window (fused path)
+    TrackSolver large;                     // win_rows > 184: the same for windows of more than 184 reduced rows, else no batch
+    const TrackSolver* last = &solver;     // the solver of the last solve or pose-only call (transfer counts)
     TrackDev td{};
     int* arena_i[2][2] = {{nullptr, nullptr}, {nullptr, nullptr}};      // [buffer][lm, cam]
     float* arena_f[2][3] = {{nullptr, nullptr, nullptr}, {nullptr, nullptr, nullptr}};  // [buffer][u, v, d]
@@ -268,7 +271,9 @@ struct kba_track {
 struct kba_track_group {
     kba_handle* h = nullptr;
     std::vector<kba_track*> tracks;
-    TrackSolver solver;                    // window i of its batch is track i's
+    TrackSolver solver;                    // window i of its batch is track i's (fused path)
+    TrackSolver large;                     // some track has win_rows > 184: the whole group on the large-window path, else no batch
+    const TrackSolver* last = &solver;
 };
 
 static int validate_window(const kba_window* w, std::string& why) {
@@ -677,9 +682,29 @@ int kba_enable_kernel_timing(kba_handle* h, int on) {
 // ---------------------------------------------------------------------------------------------------------------------
 static int batch_upload(kba_batch* b, int32_t n_windows, const kba_window* w, const int* rows);
 
+// CTAs per window that k_schur_syrk deals a window's 32-landmark chunks to (large-window path): enough for the batch's block
+// pairs to fill the GPU, at most 16
+static int syrk_split(int nr_cap_max, int n_windows, int sm_count) {
+    const int nb = nr_cap_max / 64, pairs = nb * (nb + 1) / 2;
+    return std::min(16, (6 * sm_count + n_windows * pairs - 1) / (n_windows * pairs));
+}
+
+// how the reduced system is factored: tiled in one CTA up to 192 rows, else row-major -- spread over the GPU by k_chol_* when
+// the batch has few windows (KBA_SOLVE_ROW_MAJOR / KBA_SOLVE_SPLIT override)
+static void solve_layout(BatchDev& bd, int nr_cap_max, int n_windows, int sm_count) {
+    bd.solve_tiled = (nr_cap_max <= 192 && !bd.solve_row_major) ? 1 : 0;
+    // a single SM's FP64 rate bounds the one-CTA factorisation of a large system: with few windows spread it
+    const int split_dflt = (!bd.solve_tiled && n_windows <= 16) ? std::max(1, std::min(32, sm_count / n_windows)) : 0;
+    const char* e = std::getenv("KBA_SOLVE_SPLIT");
+    bd.solve_split = bd.solve_tiled ? 0 : (e ? std::atoi(e) : split_dflt);
+}
+
 // rows[i] (optional): reduced-system rows window i is sized for, instead of 6 per keyframe (10 with plane blocks) + 1.  A track's
-// capacity window uses it: it has room for all its keyframes without plane blocks, or for 18 of them with plane blocks.
-static int batch_create(kba_handle* h, int32_t n_windows, const kba_window* w, const int* rows_of, kba_batch** out) {
+// capacity window uses it: it has room for all its keyframes without plane blocks, or for 18 of them with plane blocks (fused
+// solver), or for win_rows rows (large-window solver).
+// track_large: a track's large-window solver -- packed on the device like a fused batch (kba_batch_create packs large windows on
+// the host)
+static int batch_create(kba_handle* h, int32_t n_windows, const kba_window* w, const int* rows_of, bool track_large, kba_batch** out) {
     if (!h || !w || !out || n_windows <= 0) return fail(KBA_ERR_BAD_ARG, "bad argument to kba_batch_create");
     CU(cudaSetDevice(h->device));
     std::string why;
@@ -733,10 +758,9 @@ static int batch_create(kba_handle* h, int32_t n_windows, const kba_window* w, c
     b->lc.sm_count = h->sm_count;
     // split the landmark chunks of each window over several CTAs when the batch alone cannot fill the GPU
     {
-        const int nb = nr_cap_max / 64, pairs = nb * (nb + 1) / 2;
         int max_chunks = 1;
         for (auto& d : b->desc_h) max_chunks = std::max(max_chunks, d.n_chunks);
-        int p = std::min(16, (6 * h->sm_count + n_windows * pairs - 1) / (n_windows * pairs));
+        int p = syrk_split(nr_cap_max, n_windows, h->sm_count);
         b->lc.small_syrk = (max_rows <= 184);
         if (b->lc.small_syrk) p = (h->sm_count + n_windows - 1) / n_windows;  // one CTA per SM, each owning all tiles
         bd.p_split = std::max(1, std::min(p, max_chunks));
@@ -764,15 +788,21 @@ static int batch_create(kba_handle* h, int32_t n_windows, const kba_window* w, c
         bd.eval_min_blocks = knob("KBA_EVAL_MIN_BLOCKS", 2);
         bd.eval_cs = knob("KBA_EVAL_CS", 0);
         bd.solve_row_major = knob("KBA_SOLVE_ROW_MAJOR", 0);
-        bd.solve_tiled = (nr_cap_max <= 192 && !bd.solve_row_major) ? 1 : 0;
-        // a single SM's FP64 rate bounds the one-CTA factorisation of a large system: with few windows spread it
-        const int split_dflt = (!bd.solve_tiled && n_windows <= 16) ? std::max(1, std::min(32, h->sm_count / n_windows)) : 0;
-        bd.solve_split = bd.solve_tiled ? 0 : knob("KBA_SOLVE_SPLIT", split_dflt);
+        solve_layout(bd, nr_cap_max, n_windows, h->sm_count);
     }
     bd.bs_parts = (bd.max_lm + 15) / 16;
-    {   // device-side packing: fused batches whose landmark keys fit the sort (KBA_DEVICE_PACK=0: host packing as in round 1)
+    {   // device-side packing: fused batches and a track's large-window solver, whose landmark keys fit the sort (KBA_DEVICE_PACK=0:
+        // host packing as in round 1)
         const char* pe = std::getenv("KBA_DEVICE_PACK");
-        b->device_pack = bd.fused && !g_force_host_pack && bd.max_lm <= pack_max_landmarks() && !(pe && std::atoi(pe) == 0);
+        b->device_pack = (bd.fused || track_large) && !g_force_host_pack && bd.max_lm <= pack_max_landmarks() && !(pe && std::atoi(pe) == 0);
+    }
+    if (track_large) {  // sred holds p_split partial systems: room for the largest split a solve of the track can select (track_solve)
+        int max_chunks = 1;
+        for (auto& d : b->desc_h) max_chunks = std::max(max_chunks, d.n_chunks);
+        int p = syrk_split(192, n_windows, h->sm_count);  // a window on this path has more than 184 rows: 192 at the least
+        if (const char* pe = std::getenv("KBA_P_SPLIT")) { if (std::atoi(pe) > 0) p = std::atoi(pe); }
+        bd.p_split = std::max(bd.p_split, std::max(1, std::min(p, max_chunks)));
+        b->p_split_cap = bd.p_split;
     }
     const bool hp = !b->device_pack;  // pinned host mirrors of the sorted layout are only needed when the host builds it
     int bad = 0;
@@ -867,6 +897,7 @@ static int batch_create(kba_handle* h, int32_t n_windows, const kba_window* w, c
         if (e == cudaSuccess) e = cudaEventCreateWithFlags(&b->ev_poll2, (h->blocking_sync ? cudaEventBlockingSync : 0) | cudaEventDisableTiming);
         if (e == cudaSuccess && b->loop_pass.alloc(1, true)) e = cudaErrorMemoryAllocation;
         if (e == cudaSuccess) e = configure_kernels(nr_cap_max);
+        if (e == cudaSuccess && track_large) e = configure_kernels(192);  // a solve of 185-192 rows takes the tiled factorisation
         if (e == cudaSuccess && b->device_pack) e = configure_pack();
         if (e != cudaSuccess) { b->release(); delete b; return fail(KBA_ERR_CUDA, cudaGetErrorString(e)); }
     }
@@ -877,7 +908,7 @@ static int batch_create(kba_handle* h, int32_t n_windows, const kba_window* w, c
 }
 
 int kba_batch_create(kba_handle* h, int32_t n_windows, const kba_window* w, kba_batch** out) {
-    return batch_create(h, n_windows, w, nullptr, out);
+    return batch_create(h, n_windows, w, nullptr, false, out);
 }
 
 int kba_batch_upload(kba_batch* b, int32_t n_windows, const kba_window* w) { return batch_upload(b, n_windows, w, nullptr); }
@@ -940,7 +971,9 @@ static int batch_upload(kba_batch* b, int32_t n_windows, const kba_window* w, co
             const int rows_per_kf = (w[i].n_gp > 0 || w[i].plane_reg_weight > 0) ? 10 : 6;
             long long tot = 0;
             for (int c = 0; c < d.n_chunks; ++c) {
-                const int nk = b->chunk_k1.h[d.chunk_off + c] - b->chunk_k0.h[d.chunk_off + c] + 1;
+                // device packing (a track's capacity window): the ranges are built on the device at every solve, so every chunk
+                // is sized for all the window's keyframes
+                const int nk = b->device_pack ? d.n_kf : b->chunk_k1.h[d.chunk_off + c] - b->chunk_k0.h[d.chunk_off + c] + 1;
                 if (nk <= 0) continue;
                 const int rows = 8 * ((rows_per_kf * nk + 14 + 7) / 8) + 8;
                 tot += 96LL * (((rows - 4 + 15) / 16) * 16 + 4);
@@ -1353,6 +1386,7 @@ void kba_track_destroy(kba_track* t) {
     if (!t) return;
     cudaStreamSynchronize(t->h->stream);
     t->solver.release();
+    t->large.release();
     for (void* p : t->dev) cudaFree(p);
     t->p_lm.release(); t->p_cam.release(); t->lay.release();
     t->p_u.release(); t->p_v.release(); t->p_d.release(); t->p_dbl.release(); t->p_slot.release();
@@ -1365,9 +1399,13 @@ void kba_track_destroy(kba_track* t) {
 // k_pack_obs) are written for tracks of a few dozen observations -- one landmark carrying all 2^18 of them kept a single GPU
 // thread busy for minutes.
 // Its reduced system is sized for the larger of its windows without plane blocks (6 rows per keyframe) and with them (10 rows per
-// keyframe, for at most kTrackPlaneKf keyframes): 192 rows at 30 keyframes, the fused path.
+// keyframe, for at most kTrackPlaneKf keyframes): 192 rows at 30 keyframes, the fused path.  The capacity window of the fused
+// solver of a track with win_rows > 184 is clipped to kTrackFusedKf keyframes; that of its large-window solver has all
+// win_keyframes and at least win_rows rows.
 constexpr int kFusedMaxRows = 184;                         // small_syrk: every window of the batch within 184 reduced rows
 constexpr int kTrackPlaneKf = (kFusedMaxRows - 1) / 10;    // 18 keyframes with plane blocks
+constexpr int kTrackFusedKf = (kFusedMaxRows - 1) / 6;     // 30 keyframes without
+static bool has_large(const kba_track_caps& c) { return c.win_rows > kFusedMaxRows; }
 struct CapacityWindow {
     std::vector<double> pose, plane, lmp, lmw, gw;
     std::vector<uint8_t> fixed;
@@ -1375,9 +1413,11 @@ struct CapacityWindow {
     std::vector<float> u, v, d;
     kba_window w{};
     int rows = 0;
-    CapacityWindow(const kba_track_caps& c, int n_cam, const double* cam_intr, const double* cam_pose) {
-        const int K = c.win_keyframes, L = c.win_landmarks, O = c.win_observations, G = c.win_ground;
+    CapacityWindow(const kba_track_caps& c, bool large, int n_cam, const double* cam_intr, const double* cam_pose) {
+        const int K = large ? c.win_keyframes : std::min(c.win_keyframes, kTrackFusedKf);
+        const int L = c.win_landmarks, O = c.win_observations, G = c.win_ground;
         rows = std::max(6 * K + 1, G > 0 ? 10 * std::min(K, kTrackPlaneKf) + 1 : 0);
+        if (large) rows = std::max(rows, c.win_rows);
         pose.assign(7 * (size_t)K, 0.0); plane.assign(4 * (size_t)K, 0.0); lmp.assign(3 * (size_t)L, 0.0); lmw.assign(L, 1.0);
         gw.assign(std::max(G, 1), 1.0);
         fixed.assign(K, 0);
@@ -1410,6 +1450,8 @@ struct TrackRequest {
     const kba_window* sel = nullptr;       // nullptr: the track sits a group solve out
     int max_meas = 0, n_free = 0;          // filled by track_check: largest keyframe measurement count, free keyframes
     bool device_gp = false;                // filled by track_check: sel->gp_lm lists candidates, attached by k_track_ground
+    int rows = 0;                          // filled by track_check: reduced rows kba_batch_create sizes the window for (6 or 10 per
+                                           // keyframe + 1, plane blocks counted whenever candidates are given)
 };
 
 // ground points attached on the device: candidates in gp_lm, no keyframes or weights
@@ -1456,9 +1498,16 @@ static int track_check(const kba_track* t, TrackRequest& q, std::string& why) {
     }
     const bool planes = sel->n_gp > 0 || sel->plane_reg_weight > 0;
     if (planes && c.win_ground == 0) { why = "the track was created without ground-plane capacity"; return KBA_ERR_CAPACITY; }
-    // a request that can carry plane blocks stays on the fused path with all its keyframes (kba_batch_create's small_syrk rule)
-    if ((sel->n_gp > 0 || sel->plane_reg_weight != 0) && 10 * q.n_kf + 1 > kFusedMaxRows) {
-        why = "more than 18 keyframes with ground-plane blocks (184 reduced rows) -- such windows go through kba_solve_window";
+    q.rows = (planes ? 10 : 6) * q.n_kf + 1;
+    if (c.win_rows == 0) {
+        // a request that can carry plane blocks stays on the fused path with all its keyframes (kba_batch_create's small_syrk rule)
+        if ((sel->n_gp > 0 || sel->plane_reg_weight != 0) && 10 * q.n_kf + 1 > kFusedMaxRows) {
+            why = "more than 18 keyframes with ground-plane blocks (184 reduced rows) -- such windows go through kba_solve_window";
+            return KBA_ERR_CAPACITY;
+        }
+    } else if (q.rows > c.win_rows) {
+        why = "a window of " + std::to_string(q.rows) + " reduced rows (6 per keyframe, 10 with ground-plane blocks, plus one) is larger "
+              "than win_rows = " + std::to_string(c.win_rows);
         return KBA_ERR_CAPACITY;
     }
     if (sel->scale_weight != 0 && (sel->scale_kf0 < 0 || sel->scale_kf0 >= q.n_kf || sel->scale_kf1 < 0 || sel->scale_kf1 >= q.n_kf)) {
@@ -1509,21 +1558,21 @@ static TrackSel track_sel(const TrackRequest& q, const int* kf_slot_d, const uin
     return ts;
 }
 
-// the solver of tracks ts[0..n): one capacity window per track, so its batch has room for every window a track's caps allow.
-// On failure everything it allocated is freed again.
-static int track_solver_create(kba_handle* h, int n, kba_track* const* ts, TrackSolver& sv, const std::string& who) {
+// the solver of tracks ts[0..n): one capacity window per track, so its batch has room for every window a track's caps allow on
+// the fused path (large = false) or on the large-window path.  On failure everything it allocated is freed again.
+static int track_solver_create(kba_handle* h, int n, kba_track* const* ts, bool large, TrackSolver& sv, const std::string& who) {
     std::vector<std::unique_ptr<CapacityWindow>> cws;
     std::vector<kba_window> ws;
     std::vector<int> rows;
     size_t list_ints = 0;
     for (int i = 0; i < n; ++i) {
         const kba_track* t = ts[i];
-        cws.emplace_back(new CapacityWindow(t->caps, t->n_cam, t->cam_intr.data(), t->cam_pose.data()));
+        cws.emplace_back(new CapacityWindow(t->caps, large, t->n_cam, t->cam_intr.data(), t->cam_pose.data()));
         ws.push_back(cws.back()->w);
         rows.push_back(cws.back()->rows);
         list_ints += (size_t)t->caps.win_keyframes + t->caps.win_landmarks + (t->caps.win_keyframes + 3) / 4 + t->caps.win_ground;
     }
-    const int rc = batch_create(h, n, ws.data(), rows.data(), &sv.batch);
+    const int rc = batch_create(h, n, ws.data(), rows.data(), large, &sv.batch);
     if (rc != KBA_OK) return rc;
     if (!sv.batch->device_pack) { sv.release(); return fail(KBA_ERR_CAPACITY, who + ": device packing is disabled (KBA_FUSED / KBA_DEVICE_PACK)"); }
     int bad = 0;
@@ -1537,16 +1586,23 @@ int kba_track_create(kba_handle* h, const kba_track_caps* c, int32_t n_cam, cons
     if (c->max_keyframes < 3 || c->max_landmarks < 1 || c->max_measurements < 1 || c->win_keyframes < 3 || c->win_landmarks < 1 ||
         c->win_observations < 1 || c->win_ground < 0 || c->win_ground > c->win_landmarks)
         return fail(KBA_ERR_BAD_ARG, "kba_track_create: capacities");
-    if (6 * c->win_keyframes + 1 > kFusedMaxRows || c->win_keyframes > kFusedMaxKf || c->win_landmarks > pack_max_landmarks())
+    if (c->win_rows < 0 || (c->win_rows > 0 && c->win_rows < 6 * c->win_keyframes + 1))
+        return fail(KBA_ERR_BAD_ARG, "kba_track_create: win_rows must be 0 or at least 6 * win_keyframes + 1");
+    if (c->win_rows > 640)
+        return fail(KBA_ERR_CAPACITY, "kba_track_create: win_rows larger than 640 (the largest reduced system kba_batch_create takes)");
+    if (c->win_rows == 0 && (6 * c->win_keyframes + 1 > kFusedMaxRows || c->win_keyframes > kFusedMaxKf))
         return fail(KBA_ERR_CAPACITY, "kba_track_create: the stored window must fit the fused path (<= 184 reduced rows: 30 keyframes; "
-                                      "<= 32768 landmarks) -- larger windows go through kba_solve_window");
+                                      "<= 32768 landmarks) -- give win_rows for larger windows");
+    if (c->win_landmarks > pack_max_landmarks())
+        return fail(KBA_ERR_CAPACITY, "kba_track_create: more than 32768 landmarks per window (the device sort)");
     CU(cudaSetDevice(h->device));
     kba_track* t = new kba_track();
     t->h = h; t->caps = *c; t->n_cam = n_cam;
     t->cam_intr.assign(cam_intr, cam_intr + 3 * (size_t)n_cam);
     t->cam_pose.assign(cam_pose, cam_pose + 7 * (size_t)n_cam);
-    const int rc = track_solver_create(h, 1, &t, t->solver, "kba_track_create");
-    if (rc != KBA_OK) { delete t; return rc; }
+    int rc = track_solver_create(h, 1, &t, false, t->solver, "kba_track_create");
+    if (rc == KBA_OK && has_large(*c)) rc = track_solver_create(h, 1, &t, true, t->large, "kba_track_create");
+    if (rc != KBA_OK) { t->solver.release(); delete t; return rc; }
     int bad = 0;
     TrackDev& td = t->td;
     td.kf_cap = c->max_keyframes; td.lm_cap = c->max_landmarks; td.m_cap = c->max_measurements;
@@ -1737,6 +1793,26 @@ static int track_solve(kba_handle* h, TrackSolver& sv, int n, kba_track* const* 
     // one launch configuration for the whole batch, as kba_batch_solve has for any batch
     b->lc.max_rank = max_rank;
     b->lc.fused_slots = slots;
+    if (!b->bd.fused) {
+        // large-window path: what kba_batch_create derives from the window shapes follows the solved windows, not the capacity
+        // windows -- each window's reduced-system size, the Schur split and the factorisation -- so that the solve rounds as
+        // kba_solve_window on the same windows does.  The buffers are sized for the largest values (batch_create, track_large).
+        int nr_cap_max = 64, max_chunks = 1;
+        for (int i = 0; i < n; ++i) {
+            WinDesc& d = b->desc_h[i];
+            d.nr_cap = qs[i].sel ? (qs[i].rows + 63) / 64 * 64 : 64;
+            nr_cap_max = std::max(nr_cap_max, d.nr_cap);
+            max_chunks = std::max(max_chunks, d.n_chunks);
+            b->desc.h[i].nr_cap = d.nr_cap;
+        }
+        BatchDev& bd = b->bd;
+        bd.nr_cap_max = nr_cap_max;
+        b->lc.nr_cap_max = nr_cap_max;
+        int p = syrk_split(nr_cap_max, n, h->sm_count);
+        if (const char* pe = std::getenv("KBA_P_SPLIT")) { if (std::atoi(pe) > 0) p = std::atoi(pe); }
+        bd.p_split = std::max(1, std::min(std::min(p, max_chunks), b->p_split_cap));
+        solve_layout(bd, nr_cap_max, n, h->sm_count);
+    }
     CU(b->desc.upload(s));
     CU(cudaMemcpyAsync(sv.lists.d, sv.lists.h, used * sizeof(int), cudaMemcpyHostToDevice, s));
     CU(sv.tdev.upload(s)); CU(sv.tsel.upload(s));
@@ -1762,13 +1838,16 @@ int kba_track_solve(kba_track* t, int32_t n_kf, const int32_t* kf_slot, const ui
     std::string why;
     const int rc = track_check(t, q, why);
     if (rc != KBA_OK) return fail(rc, "kba_track_solve: " + why);
-    return track_solve(t->h, t->solver, 1, &t, &q, opt, res);
+    // the solver kba_batch_create would choose for this window: fused iff at most 184 reduced rows (and so at most 30 keyframes)
+    TrackSolver& sv = q.rows > kFusedMaxRows ? t->large : t->solver;
+    t->last = &sv;
+    return track_solve(t->h, sv, 1, &t, &q, opt, res);
 }
 
 int kba_track_transfer_bytes(kba_track* t, int64_t* h2d, int64_t* d2h, int64_t* push) {
     if (!t) return fail(KBA_ERR_BAD_ARG, "null track");
-    if (h2d) *h2d = t->solver.h2d;
-    if (d2h) *d2h = t->solver.d2h;
+    if (h2d) *h2d = t->last->h2d;
+    if (d2h) *d2h = t->last->d2h;
     if (push) *push = t->h2d_push;
     return KBA_OK;
 }
@@ -1780,6 +1859,7 @@ void kba_track_group_destroy(kba_track_group* g) {
     if (!g) return;
     cudaStreamSynchronize(g->h->stream);
     g->solver.release();
+    g->large.release();
     delete g;
 }
 
@@ -1796,8 +1876,11 @@ int kba_track_group_create(kba_handle* h, int32_t n_tracks, kba_track* const* tr
     kba_track_group* g = new kba_track_group();
     g->h = h;
     g->tracks.assign(tracks, tracks + n_tracks);
-    const int rc = track_solver_create(h, n_tracks, tracks, g->solver, "kba_track_group_create");
-    if (rc != KBA_OK) { delete g; return rc; }
+    int rc = track_solver_create(h, n_tracks, tracks, false, g->solver, "kba_track_group_create");
+    bool large = false;
+    for (int i = 0; i < n_tracks; ++i) large |= has_large(tracks[i]->caps);
+    if (rc == KBA_OK && large) rc = track_solver_create(h, n_tracks, tracks, true, g->large, "kba_track_group_create");
+    if (rc != KBA_OK) { g->solver.release(); delete g; return rc; }
     *out = g;
     return KBA_OK;
 }
@@ -1808,6 +1891,7 @@ int kba_track_group_solve(kba_track_group* g, const kba_track_request* req, cons
     // ---- every request is checked before anything is uploaded or launched
     std::vector<TrackRequest> qs(n);
     int active = 0;
+    bool large = false;
     for (int i = 0; i < n; ++i) {
         const kba_track_request& r = req[i];
         if (r.n_kf == 0) continue;  // sits this solve out
@@ -1817,19 +1901,24 @@ int kba_track_group_solve(kba_track_group* g, const kba_track_request* req, cons
         const int rc = track_check(g->tracks[i], q, why);
         if (rc != KBA_OK) return fail(rc, "kba_track_group_solve: track " + std::to_string(i) + ": " + why);
         ++active;
+        large |= q.rows > kFusedMaxRows;
     }
     if (active == 0) {  // nothing to solve: no upload, no launch, every result idle
         for (int i = 0; i < n; ++i) idle_result(res[i]);
         g->solver.h2d = 0; g->solver.d2h = 0;
+        g->last = &g->solver;
         return KBA_OK;
     }
-    return track_solve(g->h, g->solver, n, g->tracks.data(), qs.data(), opt, res);
+    // kba_batch_create's rule for the whole batch: the large-window path as soon as one window needs it
+    TrackSolver& sv = large ? g->large : g->solver;
+    g->last = &sv;
+    return track_solve(g->h, sv, n, g->tracks.data(), qs.data(), opt, res);
 }
 
 int kba_track_group_transfer_bytes(kba_track_group* g, int64_t* h2d, int64_t* d2h) {
     if (!g) return fail(KBA_ERR_BAD_ARG, "null track group");
-    if (h2d) *h2d = g->solver.h2d;
-    if (d2h) *d2h = g->solver.d2h;
+    if (h2d) *h2d = g->last->h2d;
+    if (d2h) *d2h = g->last->d2h;
     return KBA_OK;
 }
 
@@ -2024,11 +2113,13 @@ static int track_adjust_pose(const std::string& who, bool group, kba_handle* h, 
 
 int kba_track_adjust_pose(kba_track* t, const kba_track_frame* f, const kba_options* opt, kba_result* res) {
     if (!t || !f || !opt || !res) return fail(KBA_ERR_BAD_ARG, "null argument to kba_track_adjust_pose");
+    t->last = &t->solver;
     return track_adjust_pose("kba_track_adjust_pose", false, t->h, t->solver, 1, &t, f, opt, res);
 }
 
 int kba_track_group_adjust_pose(kba_track_group* g, const kba_track_frame* f, const kba_options* opt, kba_result* res) {
     if (!g || !f || !opt || !res) return fail(KBA_ERR_BAD_ARG, "null argument to kba_track_group_adjust_pose");
+    g->last = &g->solver;
     return track_adjust_pose("kba_track_group_adjust_pose", true, g->h, g->solver, (int)g->tracks.size(), g->tracks.data(), f, opt, res);
 }
 

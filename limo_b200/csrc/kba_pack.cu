@@ -1,5 +1,5 @@
 // kba_pack.cu -- window packing on the device (SURVEY 8(f) row 3; replaces the host loops of fill_window in kba_api.cu for
-// batches on the fused small-window path).  The caller's window arrives as it is -- landmark-major CSR in the caller's landmark
+// batches on the fused small-window path and for the large-window solver of a track).  The caller's window arrives as it is -- landmark-major CSR in the caller's landmark
 // order (what addKeyframeToProblem enumerates, reference bundle_adjuster_keyframes.cpp:564-627) -- with ONE copy per array;
 // everything the solver derives from it is built here:
 //   k_pack_sort      : landmarks ordered by (first, last) observing keyframe (32-bit keys: 8 + 8 bits keyframes, 15 bits
@@ -9,7 +9,7 @@
 //   k_pack_kf_count / k_pack_kf_fill : the keyframe-major copy read by k_pose_hessian, in landmark-major order inside each
 //                      keyframe (deterministic reductions), by a block-wide ordered compaction per (keyframe, window)
 //   k_pack_gp        : ground-plane residuals follow their landmark; shared-row flags
-//   k_pack_groups    : keyframe range of every 8-landmark group
+//   k_pack_ranges    : keyframe range of every 8-landmark group (fused path) or 32-landmark chunk (large-window path)
 // Integer work only; every kernel is a streaming pass over 4-byte words (a config-2 window: 40k observations x ~50 B).
 #include <cfloat>
 #include <cstdint>
@@ -175,14 +175,17 @@ __global__ void __launch_bounds__(256) k_pack_gp(BatchDev bd, PackRaw raw) {
     bd.gp_shared[G] = shared;
 }
 
-// keyframe range [k0, k1] of every 8-landmark group (observations + the ground-plane keyframes of its landmarks)
-__global__ void __launch_bounds__(256) k_pack_groups(BatchDev bd) {
+// keyframe range [k0, k1] of every kWidth-landmark unit (observations + the ground-plane keyframes of its landmarks): the 8-landmark
+// groups of the fused Schur kernel, or the 32-landmark chunks of the large-window path (k_solve_begin, k_schur_syrk), which also get
+// their landmark range.  Runs after k_pack_gp (gp_of_lm).
+template <int kWidth>
+__global__ void __launch_bounds__(256) k_pack_ranges(BatchDev bd) {
     const int w = blockIdx.y;
     const WinDesc& wd = bd.desc[w];
     const int c = blockIdx.x * blockDim.x + threadIdx.x;
-    if (c >= wd.n_groups) return;
+    if (c >= (kWidth == 8 ? wd.n_groups : wd.n_chunks)) return;
     const int* lp = bd.lm_ptr + wd.lm_off + w;
-    const int j0 = c * 8, j1 = min(wd.n_lm, j0 + 8);
+    const int j0 = c * kWidth, j1 = min(wd.n_lm, j0 + kWidth);
     int k0 = wd.n_kf, k1 = -1;
     for (int o = lp[j0]; o < lp[j1]; ++o) {
         const int k = bd.obs_kf[(size_t)wd.obs_off + o];
@@ -193,8 +196,14 @@ __global__ void __launch_bounds__(256) k_pack_groups(BatchDev bd) {
             const int g = bd.gp_of_lm[wd.lm_off + j];
             if (g >= 0) { const int k = bd.gp_kf[wd.gp_off + g]; k0 = min(k0, k); k1 = max(k1, k); }
         }
-    bd.grp_k0[wd.grp_off + c] = k0;
-    bd.grp_k1[wd.grp_off + c] = k1;
+    if (kWidth == 8) {
+        bd.grp_k0[wd.grp_off + c] = k0;
+        bd.grp_k1[wd.grp_off + c] = k1;
+    } else {
+        const size_t C = (size_t)wd.chunk_off + c;
+        bd.chunk_lm0[C] = j0; bd.chunk_lm1[C] = j1;
+        bd.chunk_k0[C] = k0; bd.chunk_k1[C] = k1;
+    }
 }
 
 // landmark results back into the caller's order, so that the download is one plain copy per array
@@ -260,8 +269,8 @@ __global__ void __launch_bounds__(256) k_track_ground(BatchDev bd, const TrackSe
     const TrackSel& sel = sels[w];
     if (sel.n_cand == 0) return;  // idle, plane-free or host lists: untouched
     WinDesc& d = bd.desc[w];
-    __shared__ double s_T[kFusedMaxKf][12];  // R row-major, t
-    __shared__ int s_use[kFusedMaxKf];
+    __shared__ double s_T[kMaxKf][12];  // R row-major, t (a plane-carrying window on the large-window path has up to 63 keyframes)
+    __shared__ int s_use[kMaxKf];
     __shared__ int s_warp[8];
     __shared__ int s_base;
     const int tid = threadIdx.x, lane = tid & 31, wp = tid >> 5, n_kf = sel.n_kf;
@@ -502,7 +511,9 @@ void launch_pack(const BatchDev& bd, const PackRaw& raw, cudaStream_t s) {
     k_pack_kf_fill<<<dim3(bd.max_kf, B), 256, 0, s>>>(bd); LCHK("k_pack_kf_fill");
     if (bd.tot_gp > 0) k_pack_gp<<<dim3((bd.max_gp + 255) / 256, B), 256, 0, s>>>(bd, raw);
     LCHK("k_pack_gp");
-    k_pack_groups<<<dim3(((bd.max_lm + 7) / 8 + 255) / 256, B), 256, 0, s>>>(bd); LCHK("k_pack_groups");
+    if (bd.fused) k_pack_ranges<8><<<dim3(((bd.max_lm + 7) / 8 + 255) / 256, B), 256, 0, s>>>(bd);
+    else k_pack_ranges<32><<<dim3(((bd.max_lm + 31) / 32 + 255) / 256, B), 256, 0, s>>>(bd);
+    LCHK("k_pack_ranges");
 }
 
 void launch_unpack_landmarks(const BatchDev& bd, double* lm_user, unsigned char* rejected_user, cudaStream_t s) {
