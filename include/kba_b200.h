@@ -29,7 +29,7 @@ extern "C" {
 #endif
 
 #define KBA_VERSION_MAJOR 0
-#define KBA_VERSION_MINOR 2
+#define KBA_VERSION_MINOR 3
 
 /* ---- status codes (reference: C++ exceptions / text report, bundle_adjuster_keyframes.cpp:630-632) ---- */
 enum {
@@ -245,20 +245,35 @@ int kba_get_counters(kba_handle* h, kba_counters* out, int reset);
 int kba_enable_kernel_timing(kba_handle* h, int on);
 
 /* ---- ONE large window sharded over several GPUs by landmark blocks (BASELINE config 5) --------------------------------
- * Every rank (one process per GPU) holds ALL keyframes and a block of the landmarks with their observations
- * (limo_b200/parallel.py::shard_window shows the partition).  Per LM iteration the ranks exchange, with NCCL all-reduce
- * over NVLink, the reduced pose system [S | rhs] their landmarks contribute to, the per-keyframe J^T J blocks and the
- * cost / model-decrease scalars; the reduced solve and the LM controller then run replicated and bit-identically on
- * every rank (an NCCL all-reduce delivers the same bits everywhere).  Trimming quantiles are taken over all ranks'
- * landmarks.  There is no reference counterpart (the reference is single-process); north_star asks for it.
- * Restrictions: one window per batch, no ground-plane residuals (n_gp = 0), every free keyframe is in the program. */
+ * Every rank (one process per GPU) holds ALL keyframes and a block of the landmarks with their observations and ground-plane
+ * residuals (limo_b200/parallel.py::shard_window shows the partition: a ground-plane residual belongs to the rank owning its
+ * landmark).  Per linearisation the ranks exchange, in ONE sum all-reduce, the reduced system [S | rhs] their landmarks
+ * contribute to, the per-keyframe J^T J blocks, for a window with ground-plane residuals the per-keyframe 10 x 10
+ * (pose | normal | distance) blocks and the ground-plane cost, and the cost partials; per LM iteration the model-decrease,
+ * step and candidate-cost scalars.  The reduced solve and the LM controller then run replicated and bit-identically on every
+ * rank (the all-reduce delivers the same bits everywhere).  Trimming quantiles are taken over all ranks' landmarks.  There is
+ * no reference counterpart (the reference is single-process); north_star asks for it.
+ * Two kinds of communicator: NCCL (kba_shard_comm_create, one process per GPU) and in process (kba_shard_comm_create_local:
+ * W handles of one process on one device, each rank's kba_batch_solve called from its own host thread; its all-reduce adds the
+ * ranks' buffers in rank order).  Sharded solves on the in-process kind always run kernel by kernel on the stream (no graph). */
 typedef struct kba_shard_comm kba_shard_comm;
 #define KBA_SHARD_ID_BYTES 128
 int kba_shard_unique_id(void* id_out);  /* KBA_SHARD_ID_BYTES; rank 0 creates it, the host broadcasts it to all ranks */
 int kba_shard_comm_create(kba_handle* h, int32_t rank, int32_t world, const void* id, kba_shard_comm** out); /* collective */
+/* world communicators out[0..world-1] of one process, rank r driving handles[r]; 1 <= world <= 16, distinct handles on one
+ * device.  If one rank's kba_batch_set_shard or kba_batch_solve fails, the ranks waiting for it in an exchange return
+ * KBA_ERR_NCCL instead of blocking, and so does every later exchange of the group: create a new one.  Destroy each out[r]. */
+int kba_shard_comm_create_local(kba_handle* const* handles, int32_t world, kba_shard_comm** out);
 void kba_shard_comm_destroy(kba_shard_comm* c);
 /* b holds this rank's shard; lm_begin = index of its first landmark in the whole window, lm_total = landmarks of the
- * whole window.  Afterwards kba_batch_solve is a collective call: every rank must make it. */
+ * whole window.  Collective: every rank calls it, and afterwards kba_batch_solve is a collective call that every rank must make.
+ * Restrictions: one window per batch (KBA_ERR_BAD_ARG), every free keyframe is in the program, and every shard must size the
+ * same reduced system (KBA_ERR_BAD_ARG otherwise): with plane_reg_weight = 0 a shard has plane rows only if it holds
+ * ground-plane residuals, so then every shard must hold some, or none.  The window's scalars -- scale regulariser,
+ * plane_reg_weight, plane_dist_fixed, speed prior -- are given to every shard with the same values (shard_window copies them).
+ * Which keyframes' plane blocks are variable is decided for the whole window: kba_batch_solve first gathers the keyframe of
+ * every rank's ground-plane residuals (one all-reduce of lm_total doubles), and every rank applies the window-wide trimming
+ * decisions to that list, so a rank without ground-plane residuals takes the same layout as the plain solve of the window. */
 int kba_batch_set_shard(kba_batch* b, kba_shard_comm* comm, int32_t lm_begin, int32_t lm_total);
 
 /* ---- persistent, device-resident sliding window (SURVEY 8(f) row 3) ------------------------------------------------------------

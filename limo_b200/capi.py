@@ -19,7 +19,8 @@ SYMBOLS = ["kba_version", "kba_last_error", "kba_default_options", "kba_create",
            "kba_solve_window", "kba_solve_batch", "kba_eval", "kba_batch_create", "kba_batch_upload",
            "kba_batch_solve", "kba_batch_download", "kba_batch_transfer_bytes", "kba_batch_jacobian_pass", "kba_batch_destroy",
            "kba_get_counters", "kba_enable_kernel_timing", "kba_lidar_default_options", "kba_lidar_depth",
-           "kba_shard_unique_id", "kba_shard_comm_create", "kba_shard_comm_destroy", "kba_batch_set_shard",
+           "kba_shard_unique_id", "kba_shard_comm_create", "kba_shard_comm_create_local", "kba_shard_comm_destroy",
+           "kba_batch_set_shard",
            "kba_init_landmarks", "kba_track_create", "kba_track_destroy", "kba_track_push_keyframe", "kba_track_drop_keyframe",
            "kba_track_set_landmarks", "kba_track_set_keyframe_pose", "kba_track_set_keyframe_poses", "kba_track_solve", "kba_track_transfer_bytes",
            "kba_track_group_create", "kba_track_group_destroy", "kba_track_group_solve", "kba_track_group_transfer_bytes",
@@ -60,6 +61,7 @@ def lib():
         L.kba_enable_kernel_timing.argtypes = [vp, C.c_int]
         L.kba_shard_unique_id.argtypes = [C.c_char_p]
         L.kba_shard_comm_create.argtypes = [vp, C.c_int32, C.c_int32, C.c_char_p, C.POINTER(vp)]
+        L.kba_shard_comm_create_local.argtypes = [C.POINTER(vp), C.c_int32, C.POINTER(vp)]
         L.kba_shard_comm_destroy.argtypes = [vp]
         L.kba_shard_comm_destroy.restype = None
         L.kba_batch_set_shard.argtypes = [vp, vp, C.c_int32, C.c_int32]
@@ -363,13 +365,29 @@ def shard_unique_id():
 
 
 class ShardComm:
-    """NCCL communicator of the sharded window solve (kba_shard_comm_create is collective over all ranks)"""
+    """Communicator of the sharded window solve: NCCL, one process per GPU (kba_shard_comm_create is collective over all
+    ranks), or in process (ShardComm.local)"""
 
     def __init__(self, handle, rank, world, unique_id):
         assert len(unique_id) == SHARD_ID_BYTES
         self._p = C.c_void_p()
         self.rank, self.world = rank, world
         _check(lib().kba_shard_comm_create(handle._p, rank, world, C.c_char_p(unique_id), C.byref(self._p)))
+
+    @classmethod
+    def local(cls, handles):
+        """one communicator per handle, connecting W handles of this process on one device (kba_shard_comm_create_local):
+        rank r's batch is solved by handles[r] from its own thread (parallel.solve_sharded_local)"""
+        world = len(handles)
+        hs = (C.c_void_p * world)(*[h._p.value for h in handles])
+        out = (C.c_void_p * world)()
+        _check(lib().kba_shard_comm_create_local(hs, world, out))
+        comms = []
+        for r in range(world):
+            c = cls.__new__(cls)
+            c._p, c.rank, c.world = C.c_void_p(out[r]), r, world
+            comms.append(c)
+        return comms
 
     def close(self):
         if self._p:

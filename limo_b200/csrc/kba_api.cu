@@ -847,6 +847,7 @@ static int batch_create(kba_handle* h, int32_t n_windows, const kba_window* w, c
     bad |= b->plane_out[0].alloc(4 * kf, true); bad |= b->plane_out[1].alloc(4 * kf, true);
     bad |= b->gp_lm.alloc(gp, hp); bad |= b->gp_kf.alloc(gp, true); bad |= b->gp_weight.alloc(gp, true); bad |= b->gp_of_lm.alloc(lm, hp); bad |= b->gp_shared.alloc(gp, hp);
     bad |= b->dev_alloc(&bd.gp_lin, 14 * gp); bad |= b->dev_alloc(&bd.vgp, 30 * gp);
+    bad |= b->dev_alloc(&bd.gp_kfb, gp ? 65 * (size_t)kf : 0);
     bad |= b->dev_alloc(&bd.gp_cost_x, n_windows); bad |= b->dev_alloc(&bd.gp_cost_c, n_windows);
     bad |= b->dev_alloc(&bd.off_pose, kf); bad |= b->dev_alloc(&bd.off_dir, kf); bad |= b->dev_alloc(&bd.off_dist, kf);
     bad |= b->dev_alloc(&bd.bkf, 27 * kf);
@@ -1032,7 +1033,15 @@ static SolveParams make_params(const kba_options* o) {
     return sp;
 }
 
+static int batch_solve(kba_batch* b, const kba_options* opt);
 int kba_batch_solve(kba_batch* b, const kba_options* opt) {
+    const int rc = batch_solve(b, opt);
+    // a rank that fails leaves the collective solve: the in-process exchange releases the ranks waiting for it with an error
+    if (rc != KBA_OK && b && b->bd.sharded && b->lc.xchg.abort) b->lc.xchg.abort(b->lc.xchg.user);
+    return rc;
+}
+
+static int batch_solve(kba_batch* b, const kba_options* opt) {
     if (!b || !opt) return fail(KBA_ERR_BAD_ARG, "bad argument to kba_batch_solve");
     if (opt->precision != 0 && opt->precision != 1) return fail(KBA_ERR_BAD_ARG, "kba_options.precision must be 0 (FP64) or 1 (FP32 linearisation)");
     if (opt->num_trim_rounds > 6 || (opt->num_trim_rounds < 0 && opt->num_rounds_option > 6))
@@ -1060,6 +1069,7 @@ int kba_batch_solve(kba_batch* b, const kba_options* opt) {
     CU(cudaMemsetAsync(b->bd.cost_part_x, 0, sizeof(double) * (size_t)b->bd.n_win * b->bd.cost_parts, s));
     CU(cudaMemsetAsync(b->bd.cost_part_c, 0, sizeof(double) * (size_t)b->bd.n_win * b->bd.cost_parts, s));
     CU(cudaEventRecord(b->ev_a, s));
+    if (launch_shard_gather(b->bd, lc, s)) return KBA_ERR_NCCL;  // message set by the exchange
     launch_reset(b->bd, lc, s);
     // upper bound on passes: every solve needs (iterations + 2) passes, plus one pass per trimming step
     const int rounds_max = 7;
@@ -1072,9 +1082,10 @@ int kba_batch_solve(kba_batch* b, const kba_options* opt) {
     if (h->kernel_timing || launch_check_enabled() || s == nullptr || b->sg.unusable) gmode = 0;
     // Sharded solve: the NCCL all-reduces are captured with the kernels (flat graph, mode 1).  The first solve of a batch runs on
     // the stream so that NCCL sets its connections up outside a capture; the active-window count is read BEFORE the next graph is
-    // launched (no look-ahead): it is identical on all ranks, and every rank must launch the same number of graphs.
+    // launched (no look-ahead): it is identical on all ranks, and every rank must launch the same number of graphs.  The in-process
+    // exchange synchronises its ranks' host threads at enqueue time, which a graph cannot hold: always the stream path.
     const bool lockstep = b->bd.sharded != 0;
-    if (lockstep) gmode = (gmode && shard_graph_enabled() && b->solves_done > 0) ? 1 : 0;
+    if (lockstep) gmode = (gmode && lc.xchg.capturable && shard_graph_enabled() && b->solves_done > 0) ? 1 : 0;
     if (gmode) {
         std::vector<unsigned char> key;
         key.reserve(sizeof(BatchDev) + sizeof(SolveParams) + 64);
@@ -1181,23 +1192,41 @@ int kba_batch_solve(kba_batch* b, const kba_options* opt) {
     return KBA_OK;
 }
 
-int kba_batch_set_shard(kba_batch* b, kba_shard_comm* comm, int32_t lm_begin, int32_t lm_total) {
-    if (!b || !comm) return fail(KBA_ERR_BAD_ARG, "bad argument to kba_batch_set_shard");
+static int batch_set_shard(kba_batch* b, const kba::Exchange& xchg, int32_t lm_begin, int32_t lm_total) {
     BatchDev& bd = b->bd;
     if (bd.n_win != 1) return fail(KBA_ERR_BAD_ARG, "a sharded batch holds exactly one window (this rank's shard)");
-    if (bd.tot_gp > 0) return fail(KBA_ERR_CAPACITY, "sharded windows with ground-plane residuals are not supported");
     if (lm_begin < 0 || lm_total < lm_begin + (int)bd.tot_lm) return fail(KBA_ERR_BAD_ARG, "landmark block outside the window");
     if (bd.sharded) return fail(KBA_ERR_BAD_ARG, "kba_batch_set_shard called twice");
     const WinDesc& d = b->desc_h[0];
+    CU(cudaSetDevice(b->h->device));
+    cudaStream_t s = b->h->stream;
     int bad = 0;
-    const kba::Exchange xchg = kba_shard_exchange(comm);
-    const size_t n_x = (size_t)d.nr_cap * d.nr_cap + (size_t)d.n_kf * 27 + (size_t)bd.cost_parts + 2;
     bad |= b->dev_alloc(&bd.xs, 16 + (size_t)xchg.world);
+    if (bad) return fail(KBA_ERR_CUDA, "out of device memory (shard buffers)");
+    // what the ranks must agree on (max over the ranks): the size of the reduced system, whether any rank holds ground points, and
+    // the cost partial slots of the exchange (their count follows the rank's observations)
+    {
+        double v[4] = {(double)d.nr_cap, -(double)d.nr_cap, bd.tot_gp > 0 ? 1.0 : 0.0, (double)bd.cost_parts};
+        CU(cudaMemcpyAsync(bd.xs, v, sizeof v, cudaMemcpyHostToDevice, s));
+        if (xchg.allreduce(xchg.user, bd.xs, bd.xs, 4, 1, s)) return KBA_ERR_NCCL;
+        CU(cudaMemcpyAsync(v, bd.xs, sizeof v, cudaMemcpyDeviceToHost, s));
+        CU(cudaStreamSynchronize(s));
+        if (v[0] != -v[1])
+            return fail(KBA_ERR_BAD_ARG, "the shards size different reduced systems: with plane_reg_weight = 0, plane blocks exist on "
+                                         "the ranks holding ground-plane residuals only; give every shard the window's plane_reg_weight");
+        bd.shard_gp = v[2] > 0.0 ? 1 : 0;
+        bd.shard_cost_parts = (int)v[3];
+    }
+    const long long n_g = bd.shard_gp ? 65LL * d.n_kf + 1 : 0;  // kba_kernels.cu: shard_gp_doubles
+    const size_t n_x = (size_t)d.nr_cap * d.nr_cap + (size_t)d.n_kf * 27 + (size_t)n_g + (size_t)bd.shard_cost_parts + 2;
     bad |= b->dev_alloc(&bd.trim_send, 3 * (size_t)lm_total); bad |= b->dev_alloc(&bd.trim_glob, 3 * (size_t)lm_total);
     bad |= b->dev_alloc(&bd.reject_glob, (size_t)lm_total);
     bad |= b->dev_alloc(&bd.x_send, n_x); bad |= b->dev_alloc(&bd.x_recv, n_x);
+    if (bd.shard_gp) {
+        bad |= b->dev_alloc(&bd.gp_send, (size_t)lm_total); bad |= b->dev_alloc(&bd.gp_kf_glob, (size_t)lm_total);
+        bad |= b->dev_alloc(&bd.act_glob, (size_t)lm_total); bad |= b->dev_alloc(&bd.kf_gp_glob, (size_t)d.n_kf);
+    }
     if (bad) return fail(KBA_ERR_CUDA, "out of device memory (shard buffers)");
-    cudaStream_t s = b->h->stream;
     CU(cudaMemsetAsync(bd.xs, 0, (16 + (size_t)xchg.world) * sizeof(double), s));
     CU(cudaMemsetAsync(bd.trim_send, 0, 3 * (size_t)lm_total * sizeof(double), s));
     CU(cudaMemsetAsync(bd.x_send, 0, n_x * sizeof(double), s));
@@ -1207,6 +1236,14 @@ int kba_batch_set_shard(kba_batch* b, kba_shard_comm* comm, int32_t lm_begin, in
     b->lc.xchg = xchg;
     b->lc.shard_win.nr_cap = d.nr_cap; b->lc.shard_win.n_kf = d.n_kf;
     return KBA_OK;
+}
+
+int kba_batch_set_shard(kba_batch* b, kba_shard_comm* comm, int32_t lm_begin, int32_t lm_total) {
+    if (!b || !comm) return fail(KBA_ERR_BAD_ARG, "bad argument to kba_batch_set_shard");
+    const kba::Exchange xchg = kba_shard_exchange(comm);
+    const int rc = batch_set_shard(b, xchg, lm_begin, lm_total);
+    if (rc != KBA_OK && xchg.abort) xchg.abort(xchg.user);  // see kba_batch_solve
+    return rc;
 }
 
 int kba_batch_download(kba_batch* b, kba_result* res) {

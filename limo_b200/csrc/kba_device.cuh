@@ -147,12 +147,19 @@ struct BatchDev {
     int lm_begin, lm_total;   // first landmark of this rank's block / landmarks of the whole window (caller's order)
     int shard_rank, shard_world;
     double* xs;               // [16 + world] exchanged scalars (ONE sum all-reduce after the back substitution): 0 model, 1 step^2,
-                              //      2 |x|^2, 3 candidate cost, 4 eval-failed flag, 16 + r: gradient max-norm of rank r
-    double* x_send;           // [nr_cap^2 + 27 n_kf + cost_parts + 2] packed linearisation of this rank (k_shard_pack) and
-    double* x_recv;           //      its sum over the ranks (ONE all-reduce per linearisation)
+                              //      2 |x|^2, 3 candidate cost, 4 eval-failed flag, 5 ground-plane cost at the candidate,
+                              //      16 + r: gradient max-norm of rank r
+    double* x_send;           // [nr_cap^2 + 27 n_kf (+ 65 n_kf + 1) + shard_cost_parts + 2] packed linearisation of this rank
+    double* x_recv;           //      (k_shard_pack) and its sum over the ranks (ONE all-reduce per linearisation)
     double* trim_send;        // [3][lm_total] this rank's trimming values (+2, 0 where not owned), all-reduced into
     double* trim_glob;        // [3][lm_total]
     uint8_t* reject_glob;     // [lm_total]
+    int shard_cost_parts;     // cost partial slots in the exchange: the largest cost_parts of the ranks (zero padded)
+    int shard_gp;             // 1: some rank holds ground-plane residuals -- plane blocks, gp blocks and gp costs are window-wide
+    double* gp_send;          // [lm_total] keyframe + 1 of this rank's landmarks' ground-plane residuals (0: none), summed into
+    double* gp_kf_glob;       //      [lm_total] the same for the whole window (once per kba_batch_solve, k_shard_gp_gather)
+    uint8_t* act_glob;        // [lm_total] landmark not trimmed in the whole window (k_reset_state, k_trim_select)
+    uint8_t* kf_gp_glob;      // [n_kf] an active ground point of some rank is attached to the keyframe (k_shard_planes)
     int precision;            // 0: FP64; 1: residual / Jacobian blocks evaluated and stored in FP32 (res, jp, jl hold floats),
                               //    every accumulation (landmark blocks, Schur products, solve, cost) stays FP64
     int solve_row_major;      // debug knob: force the global-memory Cholesky even when the tiled one fits
@@ -214,6 +221,8 @@ struct BatchDev {
     int* gp_shared;           // [tot_gp] 1: the landmark is also observed from the gp keyframe (same pose rows)
     double* gp_lin;           // [14][tot_gp] robustified residual, J_f (pose 6, dir 3 local, dist 1), J_l (3)
     double* vgp;              // [30][tot_gp] V rows of the gp residual: (J_f^T J_l) L^-T, 10 x 3
+    double* gp_kfb;           // [tot_kf*65] per keyframe: its 10 x 10 (pose | normal | distance) Gauss-Newton block over the active
+                              //   gp residuals (55, lower-packed by rows) + the 10 gradient entries (k_gp_blocks)
     double* gp_cost_x;        // [n_win] robustified cost of the gp blocks at x / at the candidate (fixed-order sums)
     double* gp_cost_c;
 };

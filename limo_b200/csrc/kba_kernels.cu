@@ -31,6 +31,20 @@ namespace kba {
 // =====================================================================================================================
 // solve begin: program layout (which parameter blocks are in the reduced program) + LM state reset
 // =====================================================================================================================
+// sharded window with ground points, before k_solve_begin: a keyframe's plane blocks are variable when an active ground point of
+// ANY rank is attached to it (gp_kf_glob: k_shard_gp_gather; act_glob: the window-wide trimming decisions), so that every rank
+// takes the layout of the plain solve of the whole window
+__global__ void __launch_bounds__(256) k_shard_planes(BatchDev bd) {
+    if (bd.state[0].phase != PH_SOLVE_BEGIN) return;
+    const WinDesc& wd = bd.desc[0];
+    for (int k = threadIdx.x; k < wd.n_kf; k += blockDim.x) bd.kf_gp_glob[k] = 0;
+    __syncthreads();
+    for (int j = threadIdx.x; j < bd.lm_total; j += blockDim.x) {
+        const int kp = (int)bd.gp_kf_glob[j];
+        if (kp > 0 && bd.act_glob[j]) bd.kf_gp_glob[kp - 1] = 1;  // benign race: every writer stores 1
+    }
+}
+
 // 1024 threads: the layout tables of a solve's first pass are dependent-load chains per landmark / observation, and a trimmed
 // solve begins three to four times
 constexpr int kBeginThreads = 1024;
@@ -71,7 +85,10 @@ __global__ void __launch_bounds__(kBeginThreads) k_solve_begin(BatchDev bd, Solv
     atomicAdd(&s_cnt[0], n_lm_in);
     atomicAdd(&s_cnt[1], n_blocks);
     if (bd.sharded)  // another rank's landmarks may be the only ones seen from a keyframe: all free keyframes are variable
-        for (int k = threadIdx.x; k < wd.n_kf; k += blockDim.x) s_has[k] = 1;
+        for (int k = threadIdx.x; k < wd.n_kf; k += blockDim.x) {
+            s_has[k] = 1;
+            if (bd.shard_gp && bd.kf_gp_glob[k]) s_plane[k] = 1;  // ... and so may its ground points be (k_shard_planes)
+        }
     __syncthreads();
     if (threadIdx.x == 0) {
         if (wd.scale_weight > 0) { s_has[wd.scale_kf0] = 1; s_has[wd.scale_kf1] = 1; }
@@ -453,6 +470,44 @@ __global__ void __launch_bounds__(256) k_gp_eval(BatchDev bd, SolveParams sp) {
 }
 template __global__ void k_gp_eval<true>(BatchDev, SolveParams);
 template __global__ void k_gp_eval<false>(BatchDev, SolveParams);
+
+// per-keyframe ground-plane Gauss-Newton block after k_gp_eval<true>: the 55 lower-packed entries of the 10 x 10 (pose | normal |
+// distance) block and the 10 gradient entries, summed over the keyframe's active gp residuals in index order.  One warp per
+// keyframe, eight keyframes per CTA.  A separate array (not the reduced solve's own loop) so that a sharded window can exchange it.
+__global__ void __launch_bounds__(256) k_gp_blocks(BatchDev bd) {
+    const int w = blockIdx.y;
+    const WinState& st = bd.state[w];
+    if (st.phase != PH_ITERATE || !st.need_linearize) return;
+    const WinDesc& wd = bd.desc[w];
+    const int k = blockIdx.x * 8 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+    if (wd.n_gp == 0 || k >= wd.n_kf) return;
+    const size_t TG = (size_t)bd.tot_gp;
+    double acc[3] = {0.0, 0.0, 0.0};
+    int ea[3], eb[3];
+#pragma unroll
+    for (int s = 0; s < 3; ++s) {
+        const int e = lane + 32 * s;
+        int a = 0, b = 0;
+        if (e < 55) { while ((a + 1) * (a + 2) / 2 <= e) ++a; b = e - a * (a + 1) / 2; }
+        else if (e < 65) { a = e - 55; b = -1; }
+        else { a = -1; b = -1; }
+        ea[s] = a; eb[s] = b;
+    }
+    for (int gi = 0; gi < wd.n_gp; ++gi) {
+        const size_t G = (size_t)wd.gp_off + gi;
+        if (bd.gp_kf[G] != k || !bd.lm_active[wd.lm_off + bd.gp_lm[G]]) continue;
+#pragma unroll
+        for (int s = 0; s < 3; ++s) {
+            if (ea[s] < 0) continue;
+            const double va = bd.gp_lin[(1 + ea[s]) * TG + G];
+            const double vb = (eb[s] >= 0) ? bd.gp_lin[(1 + eb[s]) * TG + G] : bd.gp_lin[G];
+            acc[s] += va * vb;
+        }
+    }
+#pragma unroll
+    for (int s = 0; s < 3; ++s)
+        if (ea[s] >= 0) bd.gp_kfb[(size_t)(wd.kf_off + k) * 65 + lane + 32 * s] = acc[s];
+}
 
 // =====================================================================================================================
 // pose-side Gauss-Newton blocks: one CTA per (keyframe, window) walks the keyframe-major copy of the observations,
@@ -1099,44 +1154,22 @@ __global__ void __launch_bounds__(512, 1) k_reduced_solve(BatchDev bd, SolvePara
         }
     }
     __syncthreads();
-    // ---- + ground-plane blocks: per keyframe a 10 x 10 (pose | normal | distance) Gauss-Newton block, one warp per keyframe
-    if (wd.n_gp > 0) {
-        const int lane = tid & 31, nwarp = nth >> 5;
-        const size_t TG = (size_t)bd.tot_gp;
-        for (int k = tid >> 5; k < wd.n_kf; k += nwarp) {
-            double acc[3] = {0.0, 0.0, 0.0};
-            int ea[3], eb[3];
-#pragma unroll
-            for (int s = 0; s < 3; ++s) {
-                const int e = lane + 32 * s;
-                int a = 0, b = 0;
-                if (e < 55) { while ((a + 1) * (a + 2) / 2 <= e) ++a; b = e - a * (a + 1) / 2; }
-                else if (e < 65) { a = e - 55; b = -1; }
-                else { a = -1; b = -1; }
-                ea[s] = a; eb[s] = b;
-            }
-            for (int gi = 0; gi < wd.n_gp; ++gi) {
-                const size_t G = (size_t)wd.gp_off + gi;
-                if (bd.gp_kf[G] != k || !bd.lm_active[wd.lm_off + bd.gp_lm[G]]) continue;
-#pragma unroll
-                for (int s = 0; s < 3; ++s) {
-                    if (ea[s] < 0) continue;
-                    const double va = bd.gp_lin[(1 + ea[s]) * TG + G];
-                    const double vb = (eb[s] >= 0) ? bd.gp_lin[(1 + eb[s]) * TG + G] : bd.gp_lin[G];
-                    acc[s] += va * vb;
-                }
-            }
-#pragma unroll
-            for (int s = 0; s < 3; ++s) {
-                if (ea[s] < 0) continue;
-                const int ra = gp_row(bd, wd, k, ea[s]);
-                if (ra < 0) continue;
-                if (eb[s] < 0) { s_g[ra] += acc[s]; continue; }
-                const int rb = gp_row(bd, wd, k, eb[s]);
-                if (rb < 0) continue;
-                A(ra, rb) += acc[s];
-                if (ea[s] == eb[s]) s_fdiag[ra] += acc[s];
-            }
+    // ---- + ground-plane blocks: per keyframe the 10 x 10 (pose | normal | distance) Gauss-Newton block of k_gp_blocks (on a
+    //      sharded window: its sum over the ranks, so a rank without ground points adds the others' blocks) ----
+    if (wd.n_gp > 0 || bd.shard_gp) {
+        for (int idx = tid; idx < wd.n_kf * 65; idx += nth) {
+            const int k = idx / 65, e = idx - 65 * k;
+            int a, b;
+            if (e < 55) { a = 0; while ((a + 1) * (a + 2) / 2 <= e) ++a; b = e - a * (a + 1) / 2; }
+            else { a = e - 55; b = -1; }
+            const int ra = gp_row(bd, wd, k, a);
+            if (ra < 0) continue;
+            const double v = bd.gp_kfb[(size_t)(wd.kf_off + k) * 65 + e];
+            if (b < 0) { s_g[ra] += v; continue; }
+            const int rb = gp_row(bd, wd, k, b);
+            if (rb < 0) continue;
+            A(ra, rb) += v;
+            if (a == b) s_fdiag[ra] += v;
         }
         __syncthreads();
     }
@@ -1190,7 +1223,7 @@ __global__ void __launch_bounds__(512, 1) k_reduced_solve(BatchDev bd, SolvePara
         }
         if (lane == 0 && eval_cost) st.x_cost += plane_chain_cost(wd, P, PL);
     }
-    if (tid == 0 && wd.n_gp > 0 && eval_cost) st.x_cost += bd.gp_cost_x[w];
+    if (tid == 0 && (wd.n_gp > 0 || bd.shard_gp) && eval_cost) st.x_cost += bd.gp_cost_x[w];
     __syncthreads();
     // ---- regularisers (thread 0; a handful of residuals) ----
     if (tid == 0 && wd.scale_weight > 0) {
@@ -1804,53 +1837,58 @@ __global__ void __launch_bounds__(256) k_backsub_v(BatchDev bd, int n_units) {
 // restated in SURVEY.md A.6, and the solveTrimmed outer loop (reference robust_solving.cpp:140-248).
 // =====================================================================================================================
 // ---- sharded window: local partial sums -> the exchanged scalar block; flags out of / into the window state ----
-__global__ void __launch_bounds__(256) k_shard_scalars(BatchDev bd) {  // after k_backsub and k_eval_obs<false>
+__global__ void __launch_bounds__(32) k_shard_scalars(BatchDev bd) {  // after k_backsub and k_eval_obs<false>
+    // one warp, the partials summed in k_lm_update's order: with one rank the exchanged scalars are the plain solve's bits
     const WinState& st = bd.state[0];
     const WinDesc& wd = bd.desc[0];
-    __shared__ double s_red[8][5];
+    const int lane = threadIdx.x;
     double a = 0, b = 0, c = 0, cc = 0, g = 0;
     if (st.phase == PH_ITERATE) {
-        for (int q = threadIdx.x; q < (wd.n_lm + 15) / 16; q += blockDim.x) {
+        for (int q = lane; q < (wd.n_lm + 15) / 16; q += 32) {
             const double* p = bd.bs_part + (size_t)q * 4;
             a += p[0]; b += p[1]; c += p[2]; g = fmax(g, p[3]);
         }
-        for (int q = threadIdx.x; q < bd.cost_parts; q += blockDim.x) cc += bd.cost_part_c[q];
+        for (int q = lane; q < bd.cost_parts; q += 32) cc += bd.cost_part_c[q];
     }
-    a = warp_sum(a); b = warp_sum(b); c = warp_sum(c); cc = warp_sum(cc); g = warp_max(g);
-    if ((threadIdx.x & 31) == 0) {
-        double* r = s_red[threadIdx.x >> 5];
-        r[0] = a; r[1] = b; r[2] = c; r[3] = cc; r[4] = g;
-    }
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        double t[5] = {0, 0, 0, 0, 0};
-        for (int q = 0; q < 8; ++q) { for (int e = 0; e < 4; ++e) t[e] += s_red[q][e]; t[4] = fmax(t[4], s_red[q][4]); }
-        bd.xs[0] = t[0]; bd.xs[1] = t[1]; bd.xs[2] = t[2]; bd.xs[3] = t[3];
+    a = warp_sum(a); b = warp_sum(b); c = warp_sum(c); g = warp_max(g);
+    cc = warp_sum(cc);
+    if (lane == 0) {
+        bd.xs[0] = a; bd.xs[1] = b; bd.xs[2] = c; bd.xs[3] = cc;
         bd.xs[4] = (st.phase == PH_ITERATE && st.eval_failed) ? 1.0 : 0.0;
+        bd.xs[5] = (st.phase == PH_ITERATE && wd.n_gp > 0) ? bd.gp_cost_c[0] : 0.0;  // k_gp_eval<false>
         // the gradient max-norm rides in the same SUM all-reduce: one slot per rank, the others contribute zero
-        for (int r = 0; r < bd.shard_world; ++r) bd.xs[16 + r] = (r == bd.shard_rank) ? t[4] : 0.0;
+        for (int r = 0; r < bd.shard_world; ++r) bd.xs[16 + r] = (r == bd.shard_rank) ? g : 0.0;
     }
 }
-// The ONE exchange of a linearisation: [ reduced system (Schur sums + right-hand side) | pose blocks | cost partials at x |
-// evaluation-failed flag, landmark-block-not-PD flag ] packed into BatchDev::x_send, summed over the ranks into x_recv.
+// The ONE exchange of a linearisation: [ reduced system (Schur sums + right-hand side) | pose blocks | (window with ground points:
+// per-keyframe gp blocks, gp cost at x) | cost partials at x | evaluation-failed flag, landmark-block-not-PD flag ] packed into
+// BatchDev::x_send, summed over the ranks into x_recv.  A rank without ground points contributes zeros to the gp segment.
 // Out of place by construction: a pass that does not re-linearise (rejected step) packs the same local values again.
+__host__ __device__ inline long long shard_gp_doubles(int shard_gp, int n_kf) { return shard_gp ? 65LL * n_kf + 1 : 0; }
 __global__ void __launch_bounds__(256) k_shard_pack(BatchDev bd) {
     const WinState& st = bd.state[0];
     const WinDesc& wd = bd.desc[0];
-    const size_t n_s = (size_t)wd.nr_cap * wd.nr_cap, n_b = (size_t)wd.n_kf * 27, n_c = (size_t)bd.cost_parts;
+    const size_t n_s = (size_t)wd.nr_cap * wd.nr_cap, n_b = (size_t)wd.n_kf * 27, n_c = (size_t)bd.shard_cost_parts;
+    const size_t n_g = (size_t)shard_gp_doubles(bd.shard_gp, wd.n_kf), n_kb = (size_t)wd.n_kf * 65;
     const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-    const bool on = st.phase == PH_ITERATE;
+    const bool on = st.phase == PH_ITERATE, gp = on && wd.n_gp > 0;
     if (i < n_s) bd.x_send[i] = on ? bd.sred[i] : 0.0;
     else if (i < n_s + n_b) bd.x_send[i] = on ? bd.bkf[i - n_s] : 0.0;
-    else if (i < n_s + n_b + n_c) bd.x_send[i] = on ? bd.cost_part_x[i - n_s - n_b] : 0.0;
-    else if (i == n_s + n_b + n_c) bd.x_send[i] = (on && st.eval_failed) ? 1.0 : 0.0;
-    else if (i == n_s + n_b + n_c + 1) bd.x_send[i] = (on && st.solve_failed) ? 1.0 : 0.0;
+    else if (i < n_s + n_b + n_kb && n_g) bd.x_send[i] = gp ? bd.gp_kfb[i - n_s - n_b] : 0.0;
+    else if (i == n_s + n_b + n_kb && n_g) bd.x_send[i] = gp ? bd.gp_cost_x[0] : 0.0;
+    else if (i < n_s + n_b + n_g + n_c) {  // the ranks' slot counts differ: the segment has the largest, zero padded
+        const size_t q = i - n_s - n_b - n_g;
+        bd.x_send[i] = (on && q < (size_t)bd.cost_parts) ? bd.cost_part_x[q] : 0.0;
+    }
+    else if (i == n_s + n_b + n_g + n_c) bd.x_send[i] = (on && st.eval_failed) ? 1.0 : 0.0;
+    else if (i == n_s + n_b + n_g + n_c + 1) bd.x_send[i] = (on && st.solve_failed) ? 1.0 : 0.0;
 }
 __global__ void k_shard_flags(BatchDev bd) {  // after the exchange: a failure on any rank is a failure of the window
     WinState& st = bd.state[0];
     if (threadIdx.x != 0 || st.phase != PH_ITERATE) return;
     const WinDesc& wd = bd.desc[0];
-    const double* f = bd.x_recv + (size_t)wd.nr_cap * wd.nr_cap + (size_t)wd.n_kf * 27 + bd.cost_parts;
+    const double* f = bd.x_recv + (size_t)wd.nr_cap * wd.nr_cap + (size_t)wd.n_kf * 27 + shard_gp_doubles(bd.shard_gp, wd.n_kf) +
+                      bd.shard_cost_parts;
     if (f[0] > 0.0) st.eval_failed = 1;
     if (f[1] > 0.0 && !st.solve_failed) st.solve_failed = 1;
 }
@@ -1863,6 +1901,15 @@ __global__ void __launch_bounds__(256) k_shard_trim_scatter(BatchDev bd) {
     if (j >= wd.n_lm) return;
     const int gidx = bd.lm_begin + bd.lm_orig[j];
     for (int g = 0; g < 3; ++g) bd.trim_send[(size_t)g * bd.lm_total + gidx] = bd.trim_val[(size_t)g * bd.tot_lm + j] + 2.0;
+}
+// keyframe + 1 of this rank's ground points into their window-wide slots (gp_send is zero elsewhere); summed over the ranks
+// (launch_shard_gather), every rank knows which keyframe each ground point of the whole window is attached to
+__global__ void __launch_bounds__(256) k_shard_gp_gather(BatchDev bd) {
+    const WinDesc& wd = bd.desc[0];
+    const int g = blockIdx.x * blockDim.x + threadIdx.x;
+    if (g >= wd.n_gp) return;
+    const size_t G = (size_t)wd.gp_off + g;
+    bd.gp_send[bd.lm_begin + bd.lm_orig[wd.lm_off + bd.gp_lm[G]]] = (double)(bd.gp_kf[G] + 1);
 }
 
 __global__ void __launch_bounds__(128) k_lm_update(BatchDev bd, SolveParams sp) {
@@ -1891,9 +1938,10 @@ __global__ void __launch_bounds__(128) k_lm_update(BatchDev bd, SolveParams sp) 
     // the candidate's state (the controller flips st.cur only after it has asked for the candidate's cost)
     const double* P = bd.pose[1 - st.cur];
     const double* PL = bd.plane[1 - st.cur];
-    const double* gp_cost = bd.gp_cost_c + w;
+    const double* gp_cost = bd.sharded ? bd.xs + 5 : bd.gp_cost_c + w;
+    const bool has_gp = wd.n_gp > 0 || bd.shard_gp;
     lm_step(st, bd.log + (size_t)w * kIterLogCap, sp, !bd.sharded, bd.lin1 != 0, e_model, e_step, e_xn, e_g,
-            [&wd, cand_sum, P, PL, gp_cost]() {
+            [&wd, cand_sum, P, PL, gp_cost, has_gp]() {
         double cand = cand_sum;
         if (wd.scale_weight > 0) {
             double r;
@@ -1907,7 +1955,7 @@ __global__ void __launch_bounds__(128) k_lm_update(BatchDev bd, SolveParams sp) 
                               nullptr);
             cand += 0.5 * wd.speed_weight * (r[0] * r[0] + r[1] * r[1] + r[2] * r[2]);
         }
-        if (wd.n_gp > 0) cand += *gp_cost;
+        if (has_gp) cand += *gp_cost;
         if (wd.plane_reg_weight > 0 && wd.n_kf > 1) cand += plane_chain_cost(wd, P, PL);
         return cand;
     });
@@ -1996,6 +2044,9 @@ __global__ void __launch_bounds__(512) k_trim_select(BatchDev bd, SolveParams sp
     __syncthreads();
     for (int j = threadIdx.x; j < wd.n_lm; j += blockDim.x)
         if (rej[sh ? bd.lm_begin + orig[j] : j]) bd.lm_active[wd.lm_off + j] = 0;
+    if (sh && bd.shard_gp)  // the same decisions for the whole window: which ground points still hold plane blocks (k_solve_begin)
+        for (int j = threadIdx.x; j < bd.lm_total; j += blockDim.x)
+            if (rej[j]) bd.act_glob[j] = 0;
     __syncthreads();
     if (threadIdx.x == 0) trim_advance(st);
 }
@@ -2034,6 +2085,8 @@ __global__ void k_reset_state(BatchDev bd, int rounds_total_override, int min_la
         bd.lm[1][(size_t)wd.lm_off * 3 + i] = v;
     }
     for (int i = threadIdx.x; i < wd.n_lm; i += blockDim.x) bd.lm_active[wd.lm_off + i] = 1;
+    if (bd.sharded && bd.shard_gp)
+        for (int j = threadIdx.x; j < bd.lm_total; j += blockDim.x) bd.act_glob[j] = 1;
     if (threadIdx.x == 0) {
         WinState& st = bd.state[w];
         st.phase = wd.idle ? PH_DONE : PH_SOLVE_BEGIN;  // an idle window (kba_track_group_solve) never iterates: no solve, no log
@@ -2121,6 +2174,14 @@ static int strided_grid(int cfg, int n_units, int num, int den, int n_win, int s
     return ((long long)g * n_win >= (long long)waves * ctas_per_sm * sm_count && g >= 1) ? g : n_units;
 }
 
+int launch_shard_gather(const BatchDev& bd, const LaunchCfg& lc, cudaStream_t s) {
+    if (!bd.sharded || !bd.shard_gp) return 0;
+    cudaMemsetAsync(bd.gp_send, 0, sizeof(double) * (size_t)bd.lm_total, s);
+    if (bd.tot_gp > 0) k_shard_gp_gather<<<(unsigned)((bd.tot_gp + 255) / 256), 256, 0, s>>>(bd);
+    LCHK("k_shard_gp_gather");
+    return lc.xchg.allreduce(lc.xchg.user, bd.gp_send, bd.gp_kf_glob, bd.lm_total, 0, s);
+}
+
 void launch_reset(const BatchDev& bd, const LaunchCfg& lc, cudaStream_t s) {
     k_reset_state<<<bd.n_win, 256, 0, s>>>(bd, lc.rounds_override, lc.min_landmarks_for_trimming, lc.num_rounds_option); LCHK("k_reset_state");
 }
@@ -2131,12 +2192,17 @@ int launch_pass(const BatchDev& bd, const SolveParams& sp, const LaunchCfg& lc, 
     const dim3 g_lm((bd.max_lm + 63) / 64, B);
     if (!bd.fused) k_panel_zero<<<dim3(64, B), 256, 0, s>>>(bd);  // the fused path has no global V panels
     LCHK("k_panel_zero");
+    if (bd.sharded && bd.shard_gp) k_shard_planes<<<1, 256, 0, s>>>(bd);
+    LCHK("k_shard_planes");
     k_solve_begin<<<B, kBeginThreads, 0, s>>>(bd, sp); LCHK("k_solve_begin");
     const bool timed = lc.time_jacobian && lc.ev_pool && *lc.ev_used + 2 <= lc.ev_cap;
     // one-kernel linearisation (kba_linearize.cuh): fused path, FP64, at most one observation per (landmark, keyframe)
     const bool lin1 = bd.lin1 != 0;
     if (lin1) {
-        if (bd.tot_gp > 0) k_gp_eval<true><<<B, 256, 0, s>>>(bd, sp);
+        if (bd.tot_gp > 0) {
+            k_gp_eval<true><<<B, 256, 0, s>>>(bd, sp);
+            k_gp_blocks<<<dim3((bd.max_kf + 7) / 8, B), 256, 0, s>>>(bd);
+        }
         LCHK("k_gp_eval");
         if (timed) cudaEventRecord(lc.ev_pool[(*lc.ev_used)++], s);
         const int n_units = (lin_tile_bound(bd.max_obs, bd.max_lm) + kLinWarps - 1) / kLinWarps;
@@ -2150,7 +2216,10 @@ int launch_pass(const BatchDev& bd, const SolveParams& sp, const LaunchCfg& lc, 
         if (timed) cudaEventRecord(lc.ev_pool[(*lc.ev_used)++], s);
         launch_eval_obs<true>(bd, sp, s);
         if (timed) cudaEventRecord(lc.ev_pool[(*lc.ev_used)++], s);
-        if (bd.tot_gp > 0) k_gp_eval<true><<<B, 256, 0, s>>>(bd, sp);
+        if (bd.tot_gp > 0) {
+            k_gp_eval<true><<<B, 256, 0, s>>>(bd, sp);
+            k_gp_blocks<<<dim3((bd.max_kf + 7) / 8, B), 256, 0, s>>>(bd);
+        }
         LCHK("k_gp_eval");
         k_pose_hessian<<<dim3(bd.max_kf, B), 256, 0, s>>>(bd, sp); LCHK("k_pose_hessian");
     }
@@ -2180,15 +2249,19 @@ int launch_pass(const BatchDev& bd, const SolveParams& sp, const LaunchCfg& lc, 
     const dim3 g_red((lc.nr_cap_max * lc.nr_cap_max + 255) / 256, B);
     BatchDev bc = bd;  // consumer view of the reduced system
     if (bd.sharded) {
-        // the one exchange of the linearisation: reduced system (Schur sums + right-hand side), pose blocks, cost at x
+        // the one exchange of the linearisation: reduced system (Schur sums + right-hand side), pose blocks, ground-plane blocks and
+        // cost, cost at x
         if (bd.p_split > 1) k_sred_reduce<<<g_red, 256, 0, s>>>(bd, 1);
         LCHK("k_sred_reduce");
         const LaunchCfg::WinDescHost& wh = lc.shard_win;
-        const long long n_s = (long long)wh.nr_cap * wh.nr_cap, n_b = (long long)wh.n_kf * 27, n_x = n_s + n_b + bd.cost_parts + 2;
+        const long long n_s = (long long)wh.nr_cap * wh.nr_cap, n_b = (long long)wh.n_kf * 27, n_g = shard_gp_doubles(bd.shard_gp, wh.n_kf);
+        const long long n_x = n_s + n_b + n_g + bd.shard_cost_parts + 2;
         k_shard_pack<<<(unsigned)((n_x + 255) / 256), 256, 0, s>>>(bd); LCHK("k_shard_pack");
         if (int rc = lc.xchg.allreduce(lc.xchg.user, bd.x_send, bd.x_recv, n_x, 0, s)) return rc;
         k_shard_flags<<<1, 32, 0, s>>>(bd); LCHK("k_shard_flags");
-        bc.sred = bd.x_recv; bc.bkf = bd.x_recv + n_s; bc.cost_part_x = bd.x_recv + n_s + n_b;  // the solve reads the window-wide sums
+        // the solve reads the window-wide sums
+        bc.sred = bd.x_recv; bc.bkf = bd.x_recv + n_s; bc.cost_part_x = bd.x_recv + n_s + n_b + n_g; bc.cost_parts = bd.shard_cost_parts;
+        if (n_g) { bc.gp_kfb = bd.x_recv + n_s + n_b; bc.gp_cost_x = bd.x_recv + n_s + n_b + 65LL * wh.n_kf; }
         k_sred_reduce<<<g_red, 256, 0, s>>>(bc, 2); LCHK("k_sred_reduce");
     } else if (bd.p_split > 1) {
         k_sred_reduce<<<g_red, 256, 0, s>>>(bd, 0); LCHK("k_sred_reduce");
@@ -2219,7 +2292,7 @@ int launch_pass(const BatchDev& bd, const SolveParams& sp, const LaunchCfg& lc, 
     if (bd.tot_gp > 0) k_gp_eval<false><<<B, 256, 0, s>>>(bd, sp);
     LCHK("k_gp_eval");
     if (bd.sharded) {  // model decrease / step norm / candidate cost over all ranks
-        k_shard_scalars<<<1, 256, 0, s>>>(bd); LCHK("k_shard_scalars");
+        k_shard_scalars<<<1, 32, 0, s>>>(bd); LCHK("k_shard_scalars");
         // model decrease, step / state norms, candidate cost, failure flag (sums) and one gradient-max slot per rank
         if (int rc = lc.xchg.allreduce(lc.xchg.user, bd.xs, bd.xs, 16 + bd.shard_world, 0, s)) return rc;
     }
@@ -2233,6 +2306,8 @@ int launch_pass(const BatchDev& bd, const SolveParams& sp, const LaunchCfg& lc, 
     if (cnt) {
         const int gp = bd.tot_gp > 0 ? 1 : 0;
         const int prep = lin1 ? 1 : 2 + (bd.fused ? 1 : lc.max_rank + 1 + gp);  // pose blocks [, landmark blocks, V rows]
+        cnt->launches_total += gp; cnt->launches_prep += gp;                       // k_gp_blocks
+        if (bd.sharded && bd.shard_gp) cnt->launches_total += 1;                   // k_shard_planes
         const int split = (!bd.solve_tiled && bd.solve_split) ? 1 + 3 * ((lc.nr_cap_max + kNB - 1) / kNB) : 0;
         cnt->launches_total += (bd.fused ? 0 : 1) + 1 + 1 + gp + prep + 1 + (bd.p_split > 1 ? 1 : 0) + 1 + split + 1 + 1 + gp + 1 + 2;
         cnt->launches_jacobian += 1; cnt->launches_prep += prep + gp; cnt->launches_schur += 1; cnt->launches_solve += 2;

@@ -26,12 +26,15 @@ struct Counters {
     long long jacobian_obs = 0;
 };
 
-// cross-rank reduction hook of the sharded solve: out-of-place all-reduce of `count` doubles on stream s
-// (op 0 = sum, 1 = max); returns 0 on success.  Implemented over NCCL in kba_shard.cu.
+// cross-rank reduction hook of the sharded solve: all-reduce of `count` doubles on stream s (op 0 = sum, 1 = max; send == recv
+// allowed); returns 0 on success.  Implemented in kba_shard.cu over NCCL (one process per GPU) and in process (several handles
+// of one process on one device).
 struct Exchange {
     int (*allreduce)(void* user, const double* send, double* recv, long long count, int op, cudaStream_t s) = nullptr;
+    void (*abort)(void* user) = nullptr;  // this rank leaves the collective on an error: release the ranks waiting for it
     void* user = nullptr;
     int rank = 0, world = 1;
+    bool capturable = true;               // the all-reduce may be captured into a CUDA graph (no host step at enqueue time)
 };
 
 struct LaunchCfg {
@@ -155,6 +158,7 @@ void launch_unpack_landmarks(const BatchDev& bd, double* lm_user, unsigned char*
 
 cudaError_t configure_kernels(int nr_cap_max);
 void launch_reset(const BatchDev& bd, const LaunchCfg& lc, cudaStream_t s);
+int launch_shard_gather(const BatchDev& bd, const LaunchCfg& lc, cudaStream_t s);  // sharded window: attachment of all ground points
 int launch_pass(const BatchDev& bd, const SolveParams& sp, const LaunchCfg& lc, Counters* cnt, cudaStream_t s);
 void launch_count_active(const BatchDev& bd, cudaStream_t s);
 void launch_loop_cond(const BatchDev& bd, unsigned long long handle, int* pass, int max_passes, cudaStream_t s);  // WHILE-node condition

@@ -104,3 +104,58 @@ def shard_window(win, rank, world):
         landmarks_fixed=win.landmarks_fixed, speed_kf=win.speed_kf, speed_weight=win.speed_weight,
         speed_dt=win.speed_dt, speed_v_before=win.speed_v_before, speed_T_origin_before=win.speed_T_origin_before, **gp)
     return sub, j0, j1
+
+
+def solve_sharded_local(win, world, opt=None, handles=None, iterations_capacity=256, repeats=1):
+    """solve `win` sharded over `world` ranks of THIS process on one GPU (capi.ShardComm.local): rank r's shard is solved by its
+    own handle from its own thread, as each rank is its own process with NCCL.  The exchanged sums are those of a `world`-GPU
+    run; the time is not (the ranks share one device).  Returns [(result, j0, j1)] per rank; `repeats` > 1 solves again
+    (every solve of a batch starts from the uploaded state) and also returns the wall time of each solve in seconds."""
+    import threading
+    import time
+    from limo_b200 import capi
+    own = handles is None
+    handles = [capi.Handle(0) for _ in range(world)] if own else list(handles)
+    parts = [shard_window(win, r, world) for r in range(world)]
+    comms = capi.ShardComm.local(handles)
+    batches = [handles[r].batch([parts[r][0]]) for r in range(world)]
+    out, errors, times = [None] * world, [None] * world, [[] for _ in range(world)]
+
+    def run(r):
+        try:
+            batches[r].set_shard(comms[r], parts[r][1], win.n_lm)
+            for _ in range(repeats):
+                t0 = time.perf_counter()
+                batches[r].solve(opt or capi.default_options())
+                times[r].append(time.perf_counter() - t0)
+            out[r] = batches[r].download(iterations_capacity)[0]
+        except Exception as e:  # noqa: BLE001 -- re-raised below, after every thread has ended
+            errors[r] = e
+
+    threads = [threading.Thread(target=run, args=(r,)) for r in range(world)]
+    for t in threads:
+        t.start()
+    for t in threads:
+        t.join()
+    for b in batches:
+        b.close()
+    for c in comms:
+        c.close()
+    if own:
+        for h in handles:
+            h.close()
+    for e in errors:
+        if e is not None:
+            raise e
+    res = [(out[r], parts[r][1], parts[r][2]) for r in range(world)]
+    return (res, [max(ts) for ts in zip(*times)]) if repeats > 1 else res
+
+
+def merge_shards(results, n_lm):
+    """(kf_pose, kf_plane, lm_pos, lm_rejected) of the whole window from the ranks' results (poses / planes of rank 0)"""
+    lm_pos = np.zeros((n_lm, 3))
+    rej = np.zeros(n_lm, dtype=np.uint8)
+    for r, j0, j1 in results:
+        lm_pos[j0:j1] = r.lm_pos[:j1 - j0]
+        rej[j0:j1] = r.lm_rejected[:j1 - j0]
+    return results[0][0].kf_pose, results[0][0].kf_plane, lm_pos, rej
