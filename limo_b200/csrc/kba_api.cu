@@ -19,7 +19,6 @@
 using namespace kba;
 
 static thread_local std::string g_last_error;
-static thread_local bool g_force_host_pack = false;  // kba_eval: needs the host-side observation permutation
 static int fail(int code, const std::string& msg) {
     g_last_error = msg;
     return code;
@@ -95,8 +94,8 @@ struct kba_batch {
     Staged<uint8_t> kf_fixed;
     Staged<int> lm_ptr, obs_kf, obs_cam, obs_lm, kf_ptr, pm_lm, pm_cam, chunk_lm0, chunk_lm1, chunk_k0, chunk_k1, lm_orig, obs_orig;
     Staged<int> grp_k0, grp_k1;
-    // device-side packing (kba_pack.cu): the caller's arrays are uploaded as they are, the sorted layout is built by kernels
-    bool device_pack = false;
+    // device-side packing (kba_pack.cu, lc.plan.device_pack): the caller's arrays are uploaded as they are, the sorted layout is
+    // built by kernels
     Staged<int> r_lm_ptr, r_obs_kf, r_obs_cam, r_gp_lm;
     Staged<float> r_obs_u, r_obs_v, r_obs_d;
     Staged<double> r_lm_pos, r_lm_weight;
@@ -137,7 +136,6 @@ struct kba_batch {
     } sg;
     Staged<int> loop_pass;  // passes the WHILE node has run (device counter + pinned copy)
     long long solves_done = 0;
-    int p_split_cap = 0;    // a track's large-window solver: the largest Schur split sred has room for
 
     template <typename T>
     int dev_alloc(T** p, size_t count) {
@@ -240,7 +238,7 @@ struct kba_track {
     kba_track_caps caps{};
     int n_cam = 0;
     TrackSolver solver;                    // window 0 of its batch is this track's window (fused path)
-    TrackSolver large;                     // win_rows > 184: the same for windows of more than 184 reduced rows, else no batch
+    TrackSolver large;                     // win_rows > kFusedMaxRows: the same for windows of more rows, else no batch
     const TrackSolver* last = &solver;     // the solver of the last solve or pose-only call (transfer counts)
     TrackDev td{};
     int* arena_i[2][2] = {{nullptr, nullptr}, {nullptr, nullptr}};      // [buffer][lm, cam]
@@ -272,7 +270,7 @@ struct kba_track_group {
     kba_handle* h = nullptr;
     std::vector<kba_track*> tracks;
     TrackSolver solver;                    // window i of its batch is track i's (fused path)
-    TrackSolver large;                     // some track has win_rows > 184: the whole group on the large-window path, else no batch
+    TrackSolver large;                     // some track has win_rows > kFusedMaxRows: the whole group on the large-window path, else no batch
     const TrackSolver* last = &solver;
 };
 
@@ -469,10 +467,9 @@ static void fill_window_raw(kba_batch* b, int wi, const kba_window* w) {
 
 // reduced-system rows a window can have given its constant keyframes (k_solve_begin may leave out more)
 static int window_rows(const kba_window& w) {
-    const bool planes = w.n_gp > 0 || w.plane_reg_weight > 0;
     int n_free = 0;
     for (int k = 0; k < w.n_kf; ++k) n_free += w.kf_fixed[k] ? 0 : 1;
-    return (planes ? 10 : 6) * n_free + 1;
+    return reduced_rows(n_free, w.n_gp > 0 || w.plane_reg_weight > 0);
 }
 
 struct kba_shard_comm;
@@ -682,29 +679,17 @@ int kba_enable_kernel_timing(kba_handle* h, int on) {
 // ---------------------------------------------------------------------------------------------------------------------
 static int batch_upload(kba_batch* b, int32_t n_windows, const kba_window* w, const int* rows);
 
-// CTAs per window that k_schur_syrk deals a window's 32-landmark chunks to (large-window path): enough for the batch's block
-// pairs to fill the GPU, at most 16
-static int syrk_split(int nr_cap_max, int n_windows, int sm_count) {
-    const int nb = nr_cap_max / 64, pairs = nb * (nb + 1) / 2;
-    return std::min(16, (6 * sm_count + n_windows * pairs - 1) / (n_windows * pairs));
+// the fields of the batch's plan that the kernels read: the one place they are written
+static void apply_plan(kba_batch* b) {
+    const Plan& p = b->lc.plan;
+    b->bd.nr_cap_max = p.nr_cap_max; b->bd.fused = p.fused; b->bd.p_split = p.p_split;
+    b->bd.solve_tiled = p.solve_tiled; b->bd.solve_split = p.solve_split;
 }
 
-// how the reduced system is factored: tiled in one CTA up to 192 rows, else row-major -- spread over the GPU by k_chol_* when
-// the batch has few windows (KBA_SOLVE_ROW_MAJOR / KBA_SOLVE_SPLIT override)
-static void solve_layout(BatchDev& bd, int nr_cap_max, int n_windows, int sm_count) {
-    bd.solve_tiled = (nr_cap_max <= 192 && !bd.solve_row_major) ? 1 : 0;
-    // a single SM's FP64 rate bounds the one-CTA factorisation of a large system: with few windows spread it
-    const int split_dflt = (!bd.solve_tiled && n_windows <= 16) ? std::max(1, std::min(32, sm_count / n_windows)) : 0;
-    const char* e = std::getenv("KBA_SOLVE_SPLIT");
-    bd.solve_split = bd.solve_tiled ? 0 : (e ? std::atoi(e) : split_dflt);
-}
-
-// rows[i] (optional): reduced-system rows window i is sized for, instead of 6 per keyframe (10 with plane blocks) + 1.  A track's
+// rows_of[i] (optional): reduced-system rows window i is sized for, instead of reduced_rows on all its keyframes.  A track's
 // capacity window uses it: it has room for all its keyframes without plane blocks, or for 18 of them with plane blocks (fused
 // solver), or for win_rows rows (large-window solver).
-// track_large: a track's large-window solver -- packed on the device like a fused batch (kba_batch_create packs large windows on
-// the host)
-static int batch_create(kba_handle* h, int32_t n_windows, const kba_window* w, const int* rows_of, bool track_large, kba_batch** out) {
+static int batch_create(kba_handle* h, int32_t n_windows, const kba_window* w, const int* rows_of, Purpose purpose, kba_batch** out) {
     if (!h || !w || !out || n_windows <= 0) return fail(KBA_ERR_BAD_ARG, "bad argument to kba_batch_create");
     CU(cudaSetDevice(h->device));
     std::string why;
@@ -719,9 +704,8 @@ static int batch_create(kba_handle* h, int32_t n_windows, const kba_window* w, c
     BatchDev& bd = b->bd;
     bd.n_win = n_windows;
     b->desc_h.resize(n_windows);
+    std::vector<WinShape> shapes(n_windows);
     long long kf = 0, cam = 0, lm = 0, obs = 0, chunks = 0, soff = 0, gp = 0, groups = 0;
-    int max_rows = 0, max_rows_free = 0, max_groups = 1;
-    int nr_cap_max = 64;
     for (int i = 0; i < n_windows; ++i) {
         WinDesc& d = b->desc_h[i];
         memset(&d, 0, sizeof d);
@@ -729,82 +713,38 @@ static int batch_create(kba_handle* h, int32_t n_windows, const kba_window* w, c
         d.kf_off = (int)kf; d.cam_off = (int)cam; d.lm_off = (int)lm; d.obs_off = (int)obs; d.gp_off = (int)gp;
         d.chunk_off = (int)chunks; d.n_chunks = (w[i].n_lm + 31) / 32;
         d.grp_off = (int)groups; d.n_groups = (w[i].n_lm + 7) / 8;
-        groups += d.n_groups; max_groups = std::max(max_groups, d.n_groups);
-        max_rows_free = std::max(max_rows_free, window_rows(w[i]));
+        groups += d.n_groups;
         d.scale_kf0 = w[i].scale_kf0; d.scale_kf1 = w[i].scale_kf1;
         d.scale_weight = w[i].scale_weight; d.scale_value = w[i].scale_value;
-        const bool planes = w[i].n_gp > 0 || w[i].plane_reg_weight > 0;
-        const int rows = rows_of ? rows_of[i] : (planes ? 10 : 6) * w[i].n_kf + 1;
-        max_rows = std::max(max_rows, rows);
-        d.nr_cap = ((rows + 63) / 64) * 64;
+        WinShape& ws = shapes[i];
+        ws.rows = rows_of ? rows_of[i] : reduced_rows(w[i].n_kf, w[i].n_gp > 0 || w[i].plane_reg_weight > 0);
+        ws.free_rows = window_rows(w[i]);
+        ws.n_chunks = d.n_chunks; ws.n_groups = d.n_groups; ws.n_lm = w[i].n_lm;
+        d.nr_cap = nr_cap_of(ws.rows);
         d.plane_reg_weight = w[i].plane_reg_weight; d.plane_dist_fixed = w[i].plane_dist_fixed;
         d.s_off = soff;
         soff += (long long)d.nr_cap * d.nr_cap;
-        nr_cap_max = std::max(nr_cap_max, d.nr_cap);
         kf += w[i].n_kf; cam += w[i].n_cam; lm += w[i].n_lm; obs += w[i].n_obs; chunks += d.n_chunks; gp += w[i].n_gp;
         bd.max_obs = std::max(bd.max_obs, w[i].n_obs); bd.max_lm = std::max(bd.max_lm, w[i].n_lm);
         bd.max_kf = std::max(bd.max_kf, w[i].n_kf); bd.max_gp = std::max(bd.max_gp, w[i].n_gp);
     }
+    b->lc.knobs = read_knobs();
+    b->lc.plan = make_plan(shapes.data(), n_windows, h->sm_count, b->lc.knobs, purpose);
+    apply_plan(b);
+    const int nr_cap_max = b->lc.plan.nr_cap_max;
     if (obs > 2000000000LL) { b->release(); delete b; return fail(KBA_ERR_CAPACITY, "batch exceeds 2^31 observations"); }
-    if (nr_cap_max > 640) {  // shared-memory budget of the panel copies in k_reduced_solve / k_chol_trail (227 KB per CTA)
+    if (nr_cap_max > kMaxReducedRows) {
         b->release();
         delete b;
         return fail(KBA_ERR_CAPACITY, "reduced system larger than 640 rows (106 keyframes, or 63 with ground-plane blocks)");
     }
     bd.tot_kf = kf; bd.tot_cam = cam; bd.tot_lm = lm; bd.tot_obs = obs; bd.tot_chunks = (int)chunks; bd.tot_gp = gp;
     bd.tot_groups = (int)groups;
-    bd.nr_cap_max = nr_cap_max;
-    b->lc.nr_cap_max = nr_cap_max;
     b->lc.sm_count = h->sm_count;
-    // split the landmark chunks of each window over several CTAs when the batch alone cannot fill the GPU
-    {
-        int max_chunks = 1;
-        for (auto& d : b->desc_h) max_chunks = std::max(max_chunks, d.n_chunks);
-        int p = syrk_split(nr_cap_max, n_windows, h->sm_count);
-        b->lc.small_syrk = (max_rows <= 184);
-        if (b->lc.small_syrk) p = (h->sm_count + n_windows - 1) / n_windows;  // one CTA per SM, each owning all tiles
-        bd.p_split = std::max(1, std::min(p, max_chunks));
-        // fused small-window path (kba_schur_fused.cuh): no J_l, no global V panels; KBA_FUSED=0 keeps the round-1 kernels
-        const char* fe = std::getenv("KBA_FUSED");
-        bd.fused = (b->lc.small_syrk && bd.max_kf <= kFusedMaxKf && !(fe && std::atoi(fe) == 0)) ? 1 : 0;
-        // KBA_P_SPLIT pins the number of CTAs a window's landmark groups are split over.  The partial Schur sums are folded in
-        // a fixed order, so results are bit-reproducible for a given split; the default split follows the batch size.
-        if (const char* pe = std::getenv("KBA_P_SPLIT")) { if (std::atoi(pe) > 0) p = std::atoi(pe); }
-        // (a CTA of the fused Schur kernel takes at least 8 landmark groups of a window, see schur_split in kba_schur_fused.cuh: the
-        // partition of a window then does not depend on how many CTAs the batch was given)
-        if (bd.fused) bd.p_split = std::max(1, std::min(p, max_groups));
-        else if (std::getenv("KBA_P_SPLIT")) bd.p_split = std::max(1, std::min(p, max_chunks));
-        b->lc.fused_slots = (max_rows_free <= 176) ? 6 : 7;
-    }
     // cost partials: one per CTA of k_linearize (8 warp tiles each, kba_linearize.cuh: lin_tile_bound) or per 256-observation tile of k_eval_obs
     bd.cost_parts = std::max((bd.max_obs + 255) / 256, (bd.max_obs / 16 + bd.max_lm / 32 + 4 + 7) / 8);
-    { const char* le = std::getenv("KBA_LINEARIZE"); b->lc.lin_fused = !(le && std::atoi(le) == 0); }
-    { const char* le = std::getenv("KBA_LIN_GRID"); if (le) b->lc.lin_grid = std::max(-1, std::atoi(le)); }
-    { const char* le = std::getenv("KBA_BS_GRID"); if (le) b->lc.bs_grid = std::max(-1, std::atoi(le)); }
-    {  // tuning knobs of the residual/Jacobian kernel (see DESIGN.md)
-        auto knob = [](const char* name, int dflt) { const char* e = std::getenv(name); return e ? std::atoi(e) : dflt; };
-        bd.eval_tiles_jac = std::max(1, knob("KBA_EVAL_TILES_JAC", 8));
-        bd.eval_tiles_cost = std::max(1, knob("KBA_EVAL_TILES_COST", 8));
-        bd.eval_min_blocks = knob("KBA_EVAL_MIN_BLOCKS", 2);
-        bd.eval_cs = knob("KBA_EVAL_CS", 0);
-        bd.solve_row_major = knob("KBA_SOLVE_ROW_MAJOR", 0);
-        solve_layout(bd, nr_cap_max, n_windows, h->sm_count);
-    }
     bd.bs_parts = (bd.max_lm + 15) / 16;
-    {   // device-side packing: fused batches and a track's large-window solver, whose landmark keys fit the sort (KBA_DEVICE_PACK=0:
-        // host packing as in round 1)
-        const char* pe = std::getenv("KBA_DEVICE_PACK");
-        b->device_pack = (bd.fused || track_large) && !g_force_host_pack && bd.max_lm <= pack_max_landmarks() && !(pe && std::atoi(pe) == 0);
-    }
-    if (track_large) {  // sred holds p_split partial systems: room for the largest split a solve of the track can select (track_solve)
-        int max_chunks = 1;
-        for (auto& d : b->desc_h) max_chunks = std::max(max_chunks, d.n_chunks);
-        int p = syrk_split(192, n_windows, h->sm_count);  // a window on this path has more than 184 rows: 192 at the least
-        if (const char* pe = std::getenv("KBA_P_SPLIT")) { if (std::atoi(pe) > 0) p = std::atoi(pe); }
-        bd.p_split = std::max(bd.p_split, std::max(1, std::min(p, max_chunks)));
-        b->p_split_cap = bd.p_split;
-    }
-    const bool hp = !b->device_pack;  // pinned host mirrors of the sorted layout are only needed when the host builds it
+    const bool hp = !b->lc.plan.device_pack;  // pinned host mirrors of the sorted layout are only needed when the host builds it
     int bad = 0;
     bad |= b->desc.alloc(n_windows, true);
     bad |= b->pose0.alloc(7 * kf, true); bad |= b->plane0.alloc(4 * kf, true); bad |= b->kf_fixed.alloc(kf, true);
@@ -819,7 +759,7 @@ static int batch_create(kba_handle* h, int32_t n_windows, const kba_window* w, c
     bad |= b->lm_orig.alloc(lm, hp); bad |= b->obs_rank.alloc(obs, hp);
     if (hp) bad |= b->obs_orig.alloc(obs, true);
     bad |= b->grp_k0.alloc(groups, hp); bad |= b->grp_k1.alloc(groups, hp);
-    if (b->device_pack) {
+    if (b->lc.plan.device_pack) {
         bad |= b->r_lm_ptr.alloc(lm + n_windows, true); bad |= b->r_obs_kf.alloc(obs, true); bad |= b->r_obs_cam.alloc(obs, true);
         bad |= b->r_obs_u.alloc(obs, true); bad |= b->r_obs_v.alloc(obs, true); bad |= b->r_obs_d.alloc(obs, true);
         bad |= b->r_lm_pos.alloc(3 * lm, true); bad |= b->r_lm_weight.alloc(lm, true); bad |= b->r_gp_lm.alloc(gp, true);
@@ -884,7 +824,7 @@ static int batch_create(kba_handle* h, int32_t n_windows, const kba_window* w, c
     bd.gp_lm = b->gp_lm.d; bd.gp_kf = b->gp_kf.d; bd.gp_weight = b->gp_weight.d; bd.gp_of_lm = b->gp_of_lm.d; bd.gp_shared = b->gp_shared.d;
     bd.n_active = b->n_active.d;
     bd.jac_obs = b->jac_obs.d;
-    if (b->device_pack) {
+    if (b->lc.plan.device_pack) {
         PackRaw& r = b->raw;
         r.lm_ptr = b->r_lm_ptr.d; r.obs_kf = b->r_obs_kf.d; r.obs_cam = b->r_obs_cam.d;
         r.obs_u = b->r_obs_u.d; r.obs_v = b->r_obs_v.d; r.obs_d = b->r_obs_d.d;
@@ -898,8 +838,8 @@ static int batch_create(kba_handle* h, int32_t n_windows, const kba_window* w, c
         if (e == cudaSuccess) e = cudaEventCreateWithFlags(&b->ev_poll2, (h->blocking_sync ? cudaEventBlockingSync : 0) | cudaEventDisableTiming);
         if (e == cudaSuccess && b->loop_pass.alloc(1, true)) e = cudaErrorMemoryAllocation;
         if (e == cudaSuccess) e = configure_kernels(nr_cap_max);
-        if (e == cudaSuccess && track_large) e = configure_kernels(192);  // a solve of 185-192 rows takes the tiled factorisation
-        if (e == cudaSuccess && b->device_pack) e = configure_pack();
+        if (e == cudaSuccess && purpose == Purpose::TrackLarge) e = configure_kernels(kTiledMaxRows);  // re-planned solves factor tiled
+        if (e == cudaSuccess && b->lc.plan.device_pack) e = configure_pack();
         if (e != cudaSuccess) { b->release(); delete b; return fail(KBA_ERR_CUDA, cudaGetErrorString(e)); }
     }
     *out = b;
@@ -909,7 +849,7 @@ static int batch_create(kba_handle* h, int32_t n_windows, const kba_window* w, c
 }
 
 int kba_batch_create(kba_handle* h, int32_t n_windows, const kba_window* w, kba_batch** out) {
-    return batch_create(h, n_windows, w, nullptr, false, out);
+    return batch_create(h, n_windows, w, nullptr, Purpose::Batch, out);
 }
 
 int kba_batch_upload(kba_batch* b, int32_t n_windows, const kba_window* w) { return batch_upload(b, n_windows, w, nullptr); }
@@ -926,10 +866,9 @@ static int batch_upload(kba_batch* b, int32_t n_windows, const kba_window* w, co
         if (w[i].n_kf != d.n_kf || w[i].n_lm != d.n_lm || w[i].n_obs != d.n_obs || w[i].n_cam != d.n_cam || w[i].n_gp != d.n_gp)
             return fail(KBA_ERR_BAD_ARG, "kba_batch_upload: window shapes (keyframes, cameras, landmarks, observations, ground-plane "
                                          "residuals) differ from kba_batch_create");
-        // the reduced system was sized at create: 6 rows per keyframe, 10 with plane blocks
-        const bool planes = w[i].n_gp > 0 || w[i].plane_reg_weight > 0;
-        const int rows = rows_of ? rows_of[i] : (planes ? 10 : 6) * w[i].n_kf + 1;
-        if ((rows + 63) / 64 * 64 > d.nr_cap)
+        // the reduced system was sized at create
+        const int rows = rows_of ? rows_of[i] : reduced_rows(w[i].n_kf, w[i].n_gp > 0 || w[i].plane_reg_weight > 0);
+        if (nr_cap_of(rows) > d.nr_cap)
             return fail(KBA_ERR_BAD_ARG, "kba_batch_upload: window " + std::to_string(i) + " needs plane blocks the batch was not created with");
     }
     // packing (landmark sort, observation permutation, keyframe-major copy) is independent per window: host threads
@@ -942,7 +881,7 @@ static int batch_upload(kba_batch* b, int32_t n_windows, const kba_window* w, co
         memcpy(b->desc_h[i].speed_v_before, w[i].speed_v_before, sizeof(double) * 3);
         memcpy(b->desc_h[i].speed_T_origin_before, w[i].speed_T_origin_before, sizeof(double) * 7);
         b->desc.h[i] = b->desc_h[i];
-        if (b->device_pack) fill_window_raw(b, i, &w[i]);
+        if (b->lc.plan.device_pack) fill_window_raw(b, i, &w[i]);
         else fill_window(b, i, &w[i]);
     };
     {
@@ -960,10 +899,10 @@ static int batch_upload(kba_batch* b, int32_t n_windows, const kba_window* w, co
         }
     }
     for (int i = 0; i < n_windows; ++i) b->lc.max_rank = std::max(b->lc.max_rank, b->desc_h[i].max_rank);
-    if (b->bd.fused) {
+    if (b->lc.plan.fused) {  // the Schur kernel instance follows the keyframes the new contents fix
         int rows = 0;
         for (int i = 0; i < n_windows; ++i) rows = std::max(rows, window_rows(w[i]));
-        b->lc.fused_slots = (rows <= 176) ? 6 : 7;
+        b->lc.plan.fused_slots = fused_slots(rows);
     }
     if (!b->bd.fused) {   // V panel capacity: per chunk 96 columns x (rows of its keyframe range + right-hand-side tile), see k_solve_begin
         long long need = 0;
@@ -974,7 +913,7 @@ static int batch_upload(kba_batch* b, int32_t n_windows, const kba_window* w, co
             for (int c = 0; c < d.n_chunks; ++c) {
                 // device packing (a track's capacity window): the ranges are built on the device at every solve, so every chunk
                 // is sized for all the window's keyframes
-                const int nk = b->device_pack ? d.n_kf : b->chunk_k1.h[d.chunk_off + c] - b->chunk_k0.h[d.chunk_off + c] + 1;
+                const int nk = b->lc.plan.device_pack ? d.n_kf : b->chunk_k1.h[d.chunk_off + c] - b->chunk_k0.h[d.chunk_off + c] + 1;
                 if (nk <= 0) continue;
                 const int rows = 8 * ((rows_per_kf * nk + 14 + 7) / 8) + 8;
                 tot += 96LL * (((rows - 4 + 15) / 16) * 16 + 4);
@@ -989,7 +928,7 @@ static int batch_upload(kba_batch* b, int32_t n_windows, const kba_window* w, co
         for (int i = 0; i < n_windows; ++i) { b->desc_h[i].panel_off = (long long)i * b->bd.panel_cap; b->desc.h[i].panel_off = b->desc_h[i].panel_off; }
     }
     cudaStream_t s = b->h->stream;
-    if (b->device_pack) {  // the caller's arrays as they are (~33 B per observation), then the packing kernels
+    if (b->lc.plan.device_pack) {  // the caller's arrays as they are (~33 B per observation), then the packing kernels
         CU(b->desc.upload(s)); CU(b->pose0.upload(s)); CU(b->plane0.upload(s)); CU(b->kf_fixed.upload(s)); CU(b->cam.upload(s));
         CU(b->r_lm_pos.upload(s)); CU(b->r_lm_weight.upload(s)); CU(b->r_lm_ptr.upload(s));
         CU(b->r_obs_kf.upload(s)); CU(b->r_obs_cam.upload(s)); CU(b->r_obs_u.upload(s)); CU(b->r_obs_v.upload(s)); CU(b->r_obs_d.upload(s));
@@ -1047,7 +986,7 @@ static int batch_solve(kba_batch* b, const kba_options* opt) {
     if (opt->num_trim_rounds > 6 || (opt->num_trim_rounds < 0 && opt->num_rounds_option > 6))
         return fail(KBA_ERR_CAPACITY, "at most 6 trimming rounds (KBA_MAX_SOLVES = 8 inner solves incl. one retry and the final solve)");
     b->bd.precision = opt->precision;
-    b->bd.lin1 = (b->bd.fused && b->lc.lin_fused && opt->precision == 0 && b->lc.max_rank == 0) ? 1 : 0;
+    b->bd.lin1 = (b->lc.plan.fused && b->lc.knobs.lin_fused && opt->precision == 0 && b->lc.max_rank == 0) ? 1 : 0;
     kba_handle* h = b->h;
     CU(cudaSetDevice(h->device));
     cudaStream_t s = h->stream;
@@ -1090,9 +1029,8 @@ static int batch_solve(kba_batch* b, const kba_options* opt) {
         std::vector<unsigned char> key;
         key.reserve(sizeof(BatchDev) + sizeof(SolveParams) + 64);
         key_append(key, b->bd); key_append(key, sp); key_append(key, gmode); key_append(key, max_passes); key_append(key, s);
-        key_append(key, lc.nr_cap_max); key_append(key, lc.max_rank); key_append(key, (int)lc.small_syrk); key_append(key, (int)lc.lin_fused);
-        key_append(key, lc.fused_slots); key_append(key, lc.xchg.user);
-        key_append(key, lc.lin_grid); key_append(key, lc.bs_grid);
+        // the knobs are fixed at creation; the plan changes with uploads and track solves
+        key_append(key, lc.plan); key_append(key, lc.max_rank); key_append(key, lc.xchg.user);
         if (!(b->sg.exec && b->sg.key == key) && !build_solve_graph(b, sp, lc, gmode, max_passes, check_every, key)) gmode = 0;
     }
     if (gmode == 2) {
@@ -1253,7 +1191,7 @@ int kba_batch_download(kba_batch* b, kba_result* res) {
     CU(b->state.download(s)); CU(b->log.download(s));
     CU(b->pose_out[0].download(s)); CU(b->pose_out[1].download(s));
     const BatchDev& bd = b->bd;
-    if (b->device_pack) {  // landmarks come back in the caller's order: one kernel, one copy per array
+    if (b->lc.plan.device_pack) {  // landmarks come back in the caller's order: one kernel, one copy per array
         launch_unpack_landmarks(bd, b->lm_user.d, b->rej_user.d, s);
         CU(b->lm_user.download(s)); CU(b->rej_user.download(s));
     } else {
@@ -1261,7 +1199,7 @@ int kba_batch_download(kba_batch* b, kba_result* res) {
     }
     CU(b->plane_out[0].download(s)); CU(b->plane_out[1].download(s));
     CU(wait_stream(b->h));
-    b->d2h_bytes = sizeof(WinState) * bd.n_win + 2 * (7 + 4) * 8 * bd.tot_kf + (b->device_pack ? 1 : 2) * 3 * 8 * bd.tot_lm + bd.tot_lm;
+    b->d2h_bytes = sizeof(WinState) * bd.n_win + 2 * (7 + 4) * 8 * bd.tot_kf + (b->lc.plan.device_pack ? 1 : 2) * 3 * 8 * bd.tot_lm + bd.tot_lm;
     for (int i = 0; i < bd.n_win; ++i) {
         const WinDesc& d = b->desc_h[i];
         const WinState& st = b->state.h[i];
@@ -1269,7 +1207,7 @@ int kba_batch_download(kba_batch* b, kba_result* res) {
         const int cur = st.cur;
         if (r.kf_pose) memcpy(r.kf_pose, b->pose_out[cur].h + 7 * (size_t)d.kf_off, sizeof(double) * 7 * d.n_kf);
         if (r.kf_plane) memcpy(r.kf_plane, b->plane_out[cur].h + 4 * (size_t)d.kf_off, sizeof(double) * 4 * d.n_kf);
-        if (b->device_pack) {
+        if (b->lc.plan.device_pack) {
             if (r.lm_pos) memcpy(r.lm_pos, b->lm_user.h + 3 * (size_t)d.lm_off, 3 * sizeof(double) * d.n_lm);
             if (r.lm_rejected) memcpy(r.lm_rejected, b->rej_user.h + d.lm_off, d.n_lm);
         } else {
@@ -1369,9 +1307,7 @@ int kba_solve_window(kba_handle* h, const kba_window* w, const kba_options* opt,
 int kba_eval(kba_handle* h, const kba_window* w, const kba_options* opt, kba_eval_out* out) {
     if (!h || !w || !opt || !out) return fail(KBA_ERR_BAD_ARG, "null argument to kba_eval");
     kba_batch* b = nullptr;
-    g_force_host_pack = true;  // the inspection entry point maps observations back to the caller's order on the host
-    int rc = kba_batch_create(h, 1, w, &b);
-    g_force_host_pack = false;
+    int rc = batch_create(h, 1, w, nullptr, Purpose::HostPack, &b);
     if (rc != KBA_OK) return rc;
     float ms;
     rc = kba_batch_jacobian_pass(b, opt, 1, &ms);
@@ -1437,9 +1373,8 @@ void kba_track_destroy(kba_track* t) {
 // thread busy for minutes.
 // Its reduced system is sized for the larger of its windows without plane blocks (6 rows per keyframe) and with them (10 rows per
 // keyframe, for at most kTrackPlaneKf keyframes): 192 rows at 30 keyframes, the fused path.  The capacity window of the fused
-// solver of a track with win_rows > 184 is clipped to kTrackFusedKf keyframes; that of its large-window solver has all
+// solver of a track with win_rows > kFusedMaxRows is clipped to kTrackFusedKf keyframes; that of its large-window solver has all
 // win_keyframes and at least win_rows rows.
-constexpr int kFusedMaxRows = 184;                         // small_syrk: every window of the batch within 184 reduced rows
 constexpr int kTrackPlaneKf = (kFusedMaxRows - 1) / 10;    // 18 keyframes with plane blocks
 constexpr int kTrackFusedKf = (kFusedMaxRows - 1) / 6;     // 30 keyframes without
 static bool has_large(const kba_track_caps& c) { return c.win_rows > kFusedMaxRows; }
@@ -1453,7 +1388,7 @@ struct CapacityWindow {
     CapacityWindow(const kba_track_caps& c, bool large, int n_cam, const double* cam_intr, const double* cam_pose) {
         const int K = large ? c.win_keyframes : std::min(c.win_keyframes, kTrackFusedKf);
         const int L = c.win_landmarks, O = c.win_observations, G = c.win_ground;
-        rows = std::max(6 * K + 1, G > 0 ? 10 * std::min(K, kTrackPlaneKf) + 1 : 0);
+        rows = std::max(reduced_rows(K, false), G > 0 ? reduced_rows(std::min(K, kTrackPlaneKf), true) : 0);
         if (large) rows = std::max(rows, c.win_rows);
         pose.assign(7 * (size_t)K, 0.0); plane.assign(4 * (size_t)K, 0.0); lmp.assign(3 * (size_t)L, 0.0); lmw.assign(L, 1.0);
         gw.assign(std::max(G, 1), 1.0);
@@ -1487,8 +1422,8 @@ struct TrackRequest {
     const kba_window* sel = nullptr;       // nullptr: the track sits a group solve out
     int max_meas = 0, n_free = 0;          // filled by track_check: largest keyframe measurement count, free keyframes
     bool device_gp = false;                // filled by track_check: sel->gp_lm lists candidates, attached by k_track_ground
-    int rows = 0;                          // filled by track_check: reduced rows kba_batch_create sizes the window for (6 or 10 per
-                                           // keyframe + 1, plane blocks counted whenever candidates are given)
+    int rows = 0;                          // filled by track_check: reduced rows kba_batch_create sizes the window for (reduced_rows,
+                                           // plane blocks counted whenever candidates are given)
 };
 
 // ground points attached on the device: candidates in gp_lm, no keyframes or weights
@@ -1535,10 +1470,10 @@ static int track_check(const kba_track* t, TrackRequest& q, std::string& why) {
     }
     const bool planes = sel->n_gp > 0 || sel->plane_reg_weight > 0;
     if (planes && c.win_ground == 0) { why = "the track was created without ground-plane capacity"; return KBA_ERR_CAPACITY; }
-    q.rows = (planes ? 10 : 6) * q.n_kf + 1;
+    q.rows = reduced_rows(q.n_kf, planes);
     if (c.win_rows == 0) {
         // a request that can carry plane blocks stays on the fused path with all its keyframes (kba_batch_create's small_syrk rule)
-        if ((sel->n_gp > 0 || sel->plane_reg_weight != 0) && 10 * q.n_kf + 1 > kFusedMaxRows) {
+        if ((sel->n_gp > 0 || sel->plane_reg_weight != 0) && reduced_rows(q.n_kf, true) > kFusedMaxRows) {
             why = "more than 18 keyframes with ground-plane blocks (184 reduced rows) -- such windows go through kba_solve_window";
             return KBA_ERR_CAPACITY;
         }
@@ -1567,12 +1502,12 @@ static void track_desc(WinDesc& d, const kba_track* t, const TrackRequest& q) {
     d.idle = 0;
 }
 
-// fused Schur kernel instance a checked request needs (kba_batch_create's rule on its free keyframes).  The launch configuration is
-// fixed before the gather, so a request with candidates counts plane rows even if none of them is attached: an 18-free-keyframe
-// window with nothing attached runs the seven-slot kernel where kba_solve_window runs the six-slot one (and rounds differently).
-static int track_fused_slots(const TrackRequest& q) {
-    const bool planes = q.device_gp || q.sel->n_gp > 0 || plane_reg_weight(q.sel) > 0;
-    return ((planes ? 10 : 6) * q.n_free + 1 <= 176) ? 6 : 7;
+// reduced rows of the free keyframes of a checked request, which select the fused Schur kernel instance.  The launch
+// configuration is fixed before the gather, so a request with candidates counts plane rows even if none of them is attached: an
+// 18-free-keyframe window with nothing attached runs the seven-slot kernel where kba_solve_window runs the six-slot one (and
+// rounds differently).
+static int track_free_rows(const TrackRequest& q) {
+    return reduced_rows(q.n_free, q.device_gp || q.sel->n_gp > 0 || plane_reg_weight(q.sel) > 0);
 }
 
 // a track sitting a group solve out: nothing to gather, k_reset_state puts the window straight into PH_DONE
@@ -1609,9 +1544,9 @@ static int track_solver_create(kba_handle* h, int n, kba_track* const* ts, bool 
         rows.push_back(cws.back()->rows);
         list_ints += (size_t)t->caps.win_keyframes + t->caps.win_landmarks + (t->caps.win_keyframes + 3) / 4 + t->caps.win_ground;
     }
-    const int rc = batch_create(h, n, ws.data(), rows.data(), large, &sv.batch);
+    const int rc = batch_create(h, n, ws.data(), rows.data(), large ? Purpose::TrackLarge : Purpose::TrackFused, &sv.batch);
     if (rc != KBA_OK) return rc;
-    if (!sv.batch->device_pack) { sv.release(); return fail(KBA_ERR_CAPACITY, who + ": device packing is disabled (KBA_FUSED / KBA_DEVICE_PACK)"); }
+    if (!sv.batch->lc.plan.device_pack) { sv.release(); return fail(KBA_ERR_CAPACITY, who + ": device packing is disabled (KBA_FUSED / KBA_DEVICE_PACK)"); }
     int bad = 0;
     bad |= sv.tdev.alloc(n, true); bad |= sv.tsel.alloc(n, true); bad |= sv.lists.alloc(list_ints, true);
     if (bad) { sv.release(); return fail(KBA_ERR_CUDA, who + ": out of memory"); }
@@ -1623,14 +1558,14 @@ int kba_track_create(kba_handle* h, const kba_track_caps* c, int32_t n_cam, cons
     if (c->max_keyframes < 3 || c->max_landmarks < 1 || c->max_measurements < 1 || c->win_keyframes < 3 || c->win_landmarks < 1 ||
         c->win_observations < 1 || c->win_ground < 0 || c->win_ground > c->win_landmarks)
         return fail(KBA_ERR_BAD_ARG, "kba_track_create: capacities");
-    if (c->win_rows < 0 || (c->win_rows > 0 && c->win_rows < 6 * c->win_keyframes + 1))
+    if (c->win_rows < 0 || (c->win_rows > 0 && c->win_rows < reduced_rows(c->win_keyframes, false)))
         return fail(KBA_ERR_BAD_ARG, "kba_track_create: win_rows must be 0 or at least 6 * win_keyframes + 1");
-    if (c->win_rows > 640)
+    if (c->win_rows > kMaxReducedRows)
         return fail(KBA_ERR_CAPACITY, "kba_track_create: win_rows larger than 640 (the largest reduced system kba_batch_create takes)");
-    if (c->win_rows == 0 && (6 * c->win_keyframes + 1 > kFusedMaxRows || c->win_keyframes > kFusedMaxKf))
+    if (c->win_rows == 0 && reduced_rows(c->win_keyframes, false) > kFusedMaxRows)
         return fail(KBA_ERR_CAPACITY, "kba_track_create: the stored window must fit the fused path (<= 184 reduced rows: 30 keyframes; "
                                       "<= 32768 landmarks) -- give win_rows for larger windows");
-    if (c->win_landmarks > pack_max_landmarks())
+    if (c->win_landmarks > kPackMaxLandmarks)
         return fail(KBA_ERR_CAPACITY, "kba_track_create: more than 32768 landmarks per window (the device sort)");
     CU(cudaSetDevice(h->device));
     kba_track* t = new kba_track();
@@ -1787,7 +1722,8 @@ static int track_solve(kba_handle* h, TrackSolver& sv, int n, kba_track* const* 
     CU(cudaSetDevice(h->device));
     cudaStream_t s = h->stream;
     // ---- descriptors, selection lists (one pinned buffer), track stores as they are now
-    int max_rank = 0, slots = 6;
+    int max_rank = 0, max_free = 0;
+    std::vector<WinShape> solved(n);       // rows and chunks of the solved windows (large-window path)
     bool any_gp = false;
     TrackGrid grid;
     size_t used = 0;
@@ -1803,7 +1739,8 @@ static int track_solve(kba_handle* h, TrackSolver& sv, int n, kba_track* const* 
         } else {
             track_desc(d, t, q);
             max_rank = std::max(max_rank, d.max_rank);
-            slots = std::max(slots, track_fused_slots(q));
+            max_free = std::max(max_free, track_free_rows(q));
+            solved[i].rows = q.rows; solved[i].n_chunks = d.n_chunks;
             // lists: keyframe slots | landmark slots | fixation bytes | ground-plane candidates
             const kba_window* sel = q.sel;
             const int n_cand = q.device_gp ? sel->n_gp : 0, fixed_ints = (q.n_kf + 3) / 4;
@@ -1829,26 +1766,11 @@ static int track_solve(kba_handle* h, TrackSolver& sv, int n, kba_track* const* 
     }
     // one launch configuration for the whole batch, as kba_batch_solve has for any batch
     b->lc.max_rank = max_rank;
-    b->lc.fused_slots = slots;
-    if (!b->bd.fused) {
-        // large-window path: what kba_batch_create derives from the window shapes follows the solved windows, not the capacity
-        // windows -- each window's reduced-system size, the Schur split and the factorisation -- so that the solve rounds as
-        // kba_solve_window on the same windows does.  The buffers are sized for the largest values (batch_create, track_large).
-        int nr_cap_max = 64, max_chunks = 1;
-        for (int i = 0; i < n; ++i) {
-            WinDesc& d = b->desc_h[i];
-            d.nr_cap = qs[i].sel ? (qs[i].rows + 63) / 64 * 64 : 64;
-            nr_cap_max = std::max(nr_cap_max, d.nr_cap);
-            max_chunks = std::max(max_chunks, d.n_chunks);
-            b->desc.h[i].nr_cap = d.nr_cap;
-        }
-        BatchDev& bd = b->bd;
-        bd.nr_cap_max = nr_cap_max;
-        b->lc.nr_cap_max = nr_cap_max;
-        int p = syrk_split(nr_cap_max, n, h->sm_count);
-        if (const char* pe = std::getenv("KBA_P_SPLIT")) { if (std::atoi(pe) > 0) p = std::atoi(pe); }
-        bd.p_split = std::max(1, std::min(std::min(p, max_chunks), b->p_split_cap));
-        solve_layout(bd, nr_cap_max, n, h->sm_count);
+    b->lc.plan.fused_slots = fused_slots(max_free);
+    if (!b->lc.plan.fused) {  // the buffers are sized for the largest values (batch_create, Purpose::TrackLarge)
+        replan_large(b->lc.plan, solved.data(), n, h->sm_count, b->lc.knobs);
+        for (int i = 0; i < n; ++i) b->desc.h[i].nr_cap = b->desc_h[i].nr_cap = nr_cap_of(solved[i].rows);
+        apply_plan(b);
     }
     CU(b->desc.upload(s));
     CU(cudaMemcpyAsync(sv.lists.d, sv.lists.h, used * sizeof(int), cudaMemcpyHostToDevice, s));
@@ -1875,7 +1797,7 @@ int kba_track_solve(kba_track* t, int32_t n_kf, const int32_t* kf_slot, const ui
     std::string why;
     const int rc = track_check(t, q, why);
     if (rc != KBA_OK) return fail(rc, "kba_track_solve: " + why);
-    // the solver kba_batch_create would choose for this window: fused iff at most 184 reduced rows (and so at most 30 keyframes)
+    // the solver kba_batch_create would choose for this window: fused iff at most kFusedMaxRows reduced rows
     TrackSolver& sv = q.rows > kFusedMaxRows ? t->large : t->solver;
     t->last = &sv;
     return track_solve(t->h, sv, 1, &t, &q, opt, res);

@@ -7,6 +7,8 @@
 #include <cstdint>
 #include <cuda_runtime.h>
 
+#include "kba_plan.h"
+
 namespace kba {
 
 constexpr int kMaxKf = 128;         // keyframes per window the kernels stage in shared memory
@@ -14,7 +16,6 @@ constexpr int kMaxCam = 8;
 constexpr int kPoseStride = 12;     // staged pose: R (9, row-major) + t (3)
 constexpr int kCamStride = 16;      // staged camera: Rc (9) + tc (3) + f, cx, cy, pad
 constexpr int kIterLogCap = 160;    // iteration records kept per window
-constexpr int kFusedMaxKf = 32;     // keyframes of a window on the fused small-window path (<= 184 reduced rows)
 
 // ---- per-window descriptor (immutable after upload) --------------------------------------------------------------
 struct WinDesc {
@@ -162,13 +163,10 @@ struct BatchDev {
     uint8_t* kf_gp_glob;      // [n_kf] an active ground point of some rank is attached to the keyframe (k_shard_planes)
     int precision;            // 0: FP64; 1: residual / Jacobian blocks evaluated and stored in FP32 (res, jp, jl hold floats),
                               //    every accumulation (landmark blocks, Schur products, solve, cost) stays FP64
-    int solve_row_major;      // debug knob: force the global-memory Cholesky even when the tiled one fits
-    int solve_tiled;          // 1: k_reduced_solve<true> (<= 192 rows, shared-memory resident)
+    int solve_tiled;          // 1: k_reduced_solve<true> (<= kTiledMaxRows rows, shared-memory resident)
     int solve_split;          // > 0: large system of a small batch, factorisation spread over this many CTAs per window
     double* chol_w;           // [n_win][32*32] inverse of the current diagonal block's factor (split factorisation)
     double* chol_invd;        // [n_win][nr_cap_max] 1 / L_ii
-    int eval_tiles_jac, eval_tiles_cost, eval_min_blocks;  // 256-observation tiles per CTA / CTAs per SM of k_eval_obs
-    int eval_cs;              // 1: streaming (evict-first) stores of the residual / Jacobian blocks
     double* bs_part;          // [n_win][bs_parts][4]: model_e, step_sq, xnorm_sq, gmax_e
     int bs_parts;
     int nr_cap_max;           // largest nr_cap in the batch = stride of scale_f / lambda_f / grad_f / delta_f
@@ -192,7 +190,7 @@ struct BatchDev {
     // fused small-window path (k_schur_fused): J_l is not materialised (J_l = translation columns of J_p times R), the V
     // panels exist only in shared memory; per 8-landmark group the keyframe range (host, static) and, per solve, the
     // 8-row tile range of the reduced system it touches and the rows of its shared-memory panel
-    int fused;                // 1: every window of the batch has <= 184 reduced rows -> fused path, jl / vpanel unused
+    int fused;                // 1: every window of the batch has <= kFusedMaxRows reduced rows -> fused path, jl / vpanel unused
     int* grp_k0;              // [tot_groups]
     int* grp_k1;
     int* grp_t0;              // [tot_groups] tile range [t0, t1) aligned to 16-row blocks
@@ -372,13 +370,8 @@ __device__ inline bool eval_observation(const T* __restrict__ pose, const T* __r
 // Streaming form of eval_observation for the residual/Jacobian kernel: every Jacobian row is written to its SoA slot
 // as soon as it is formed, so at most one 3-vector m and the rotated point a stay live (64 registers -> 4 CTAs/SM).
 // res/jp/jl point at this observation's slot of component 0; `stride` is the component stride (total observations).
-// kJl: also store J_landmark (panel path); kCs: streaming (evict-first) stores -- the blocks are read back only after
-// hundreds of MB of other traffic, keeping them in L2 evicts what the next kernels would still hit
-template <typename T, bool kCs>
-__device__ __forceinline__ void lin_store(T* p, T v) {
-    if (kCs) __stcs(p, v); else *p = v;
-}
-template <typename T, bool kJl = true, bool kCs = false>
+// kJl: also store J_landmark (panel path)
+template <typename T, bool kJl = true>
 __device__ inline bool eval_observation_store(const T* __restrict__ pose, const T* __restrict__ cam, const T p[3], T u,
                                               T v, T d, T wt, T b_repr, T b_depth, T* __restrict__ res,
                                               T* __restrict__ jp, T* __restrict__ jl, size_t stride, bool write_jp,
@@ -404,9 +397,9 @@ __device__ inline bool eval_observation_store(const T* __restrict__ pose, const 
         cauchy<T>(b_depth, wt, rd * rd, hrd, sqd);
         half_rho_sum += hrd;
     }
-    lin_store<T, kCs>(res, sq * ru);
-    lin_store<T, kCs>(res + stride, sq * rv);
-    lin_store<T, kCs>(res + 2 * stride, sqd * rd);
+    res[0] = sq * ru;
+    res[stride] = sq * rv;
+    res[2 * stride] = sqd * rd;
     const T fz = f * iz * sq;
 #pragma unroll
     for (int i = 0; i < 3; ++i) {
@@ -416,18 +409,18 @@ __device__ inline bool eval_observation_store(const T* __restrict__ pose, const 
         else { m0 = sqd * cam[6]; m1 = sqd * cam[7]; m2 = sqd * cam[8]; }
         if (write_jp) {
             T* o = jp + (size_t)(6 * i) * stride;
-            lin_store<T, kCs>(o, T(-2) * (m1 * a2 - m2 * a1));
-            lin_store<T, kCs>(o + stride, T(-2) * (m2 * a0 - m0 * a2));
-            lin_store<T, kCs>(o + 2 * stride, T(-2) * (m0 * a1 - m1 * a0));
-            lin_store<T, kCs>(o + 3 * stride, m0);
-            lin_store<T, kCs>(o + 4 * stride, m1);
-            lin_store<T, kCs>(o + 5 * stride, m2);
+            o[0] = T(-2) * (m1 * a2 - m2 * a1);
+            o[stride] = T(-2) * (m2 * a0 - m0 * a2);
+            o[2 * stride] = T(-2) * (m0 * a1 - m1 * a0);
+            o[3 * stride] = m0;
+            o[4 * stride] = m1;
+            o[5 * stride] = m2;
         }
         if (kJl) {
             T* q = jl + (size_t)(3 * i) * stride;
-            lin_store<T, kCs>(q, m0 * pose[0] + m1 * pose[3] + m2 * pose[6]);
-            lin_store<T, kCs>(q + stride, m0 * pose[1] + m1 * pose[4] + m2 * pose[7]);
-            lin_store<T, kCs>(q + 2 * stride, m0 * pose[2] + m1 * pose[5] + m2 * pose[8]);
+            q[0] = m0 * pose[0] + m1 * pose[3] + m2 * pose[6];
+            q[stride] = m0 * pose[1] + m1 * pose[4] + m2 * pose[7];
+            q[2 * stride] = m0 * pose[2] + m1 * pose[5] + m2 * pose[8];
         }
     }
     return true;

@@ -1,5 +1,5 @@
 // kba_kernels.cu -- sm_90a kernels of the window solver.  One LM "pass" over a batch of windows is, for small windows
-// (every window <= 184 reduced rows and <= 32 keyframes: BASELINE configs 1-3),
+// (every window <= kFusedMaxRows reduced rows: BASELINE configs 1-3),
 //   k_solve_begin [-> k_gp_eval<true>] -> k_linearize (kba_linearize.cuh: evaluation + landmark blocks + V rows, Jacobian in registers)
 //   -> k_pose_hessian -> k_schur_fused (kba_schur_fused.cuh: warp-specialised FP64 tensor-core SYRK over bulk-copied V columns)
 //   [-> k_sred_reduce] -> k_reduced_solve<tiled> -> k_backsub_v -> k_eval_obs<false> (candidate cost) [-> k_gp_eval<false>]
@@ -241,7 +241,7 @@ __global__ void __launch_bounds__(256) k_panel_zero(BatchDev bd) {
 //   kJac = false: cost only, at the candidate point
 // Algorithmic HBM bytes per observation (FP64, with depth row): 20 read + 240 written (DESIGN.md).
 // =====================================================================================================================
-template <bool kJac, int kMinBlocks, typename TLin, bool kJl = true, bool kCs = false>
+template <bool kJac, int kMinBlocks, typename TLin, bool kJl = true>
 __global__ void __launch_bounds__(256, kMinBlocks) k_eval_obs(BatchDev bd, SolveParams sp, int tiles) {
     // A CTA walks `tiles` consecutive 256-observation tiles of one window with a two-deep software pipeline: while tile
     // t is evaluated, the measurement / landmark loads of tile t+1 and the landmark-index load of tile t+2 are in
@@ -328,13 +328,13 @@ __global__ void __launch_bounds__(256, kMinBlocks) k_eval_obs(BatchDev bd, Solve
                     float* resf = reinterpret_cast<float*>(bd.res) + o;
                     float* jpf = reinterpret_cast<float*>(bd.jp) + o;
                     float* jlf = reinterpret_cast<float*>(bd.jl) + o;
-                    eval_observation_store<float, kJl, kCs>(
+                    eval_observation_store<float, kJl>(
                         s_pose_f + kPoseStride * k, s_cam_f + kCamStride * c, pf, u, v, d, (float)wgt,
                         (float)(sp.reprojection_thres * sp.reprojection_thres), (float)(sp.depth_thres * sp.depth_thres),
                         resf, jpf, jlf, (size_t)bd.tot_obs, row >= 0 || !kJl, hrf);
                 }
             } else if (kJac) {  // rows are stored to their SoA slots as they are formed
-                ok = eval_observation_store<double, kJl, kCs>(
+                ok = eval_observation_store<double, kJl>(
                     s_pose + kPoseStride * k, s_cam + kCamStride * c, p, (double)u, (double)v, (double)d, wgt,
                     sp.reprojection_thres * sp.reprojection_thres, sp.depth_thres * sp.depth_thres, bd.res + o, bd.jp + o,
                     bd.jl + o, (size_t)bd.tot_obs, row >= 0 || !kJl, hr);
@@ -372,33 +372,21 @@ __global__ void __launch_bounds__(256, kMinBlocks) k_eval_obs(BatchDev bd, Solve
     }
 }
 
+// 8 tiles per CTA; two CTAs per SM for the linearisation, four for the cost.  The cost slots a CTA writes follow the tile count.
+constexpr int kEvalTiles = 8;
 template <bool kJac>
 static void launch_eval_obs(const BatchDev& bd, const SolveParams& sp, cudaStream_t s) {
-    const int tiles = kJac ? bd.eval_tiles_jac : bd.eval_tiles_cost;
-    const dim3 g((bd.max_obs + 256 * tiles - 1) / (256 * tiles), bd.n_win);
-    if (!kJac) { k_eval_obs<false, 4, double><<<g, 256, 0, s>>>(bd, sp, tiles); return; }
-    const int mb = bd.eval_min_blocks;
+    const dim3 g((bd.max_obs + 256 * kEvalTiles - 1) / (256 * kEvalTiles), bd.n_win);
+    if (!kJac) { k_eval_obs<false, 4, double><<<g, 256, 0, s>>>(bd, sp, kEvalTiles); return; }
     // fused path (kJl = false): J_l is not materialised, its consumers form it as (translation columns of J_p) R
     if (bd.precision == 1) {
-        if (bd.fused) k_eval_obs<true, 2, float, false><<<g, 256, 0, s>>>(bd, sp, tiles);
-        else k_eval_obs<true, 2, float, true><<<g, 256, 0, s>>>(bd, sp, tiles);
-        LCHK("k_eval_obs");
-    } else if (!bd.fused) {
-        if (mb == 2) k_eval_obs<true, 2, double, true><<<g, 256, 0, s>>>(bd, sp, tiles);
-        else if (mb == 3) k_eval_obs<true, 3, double, true><<<g, 256, 0, s>>>(bd, sp, tiles);
-        else k_eval_obs<true, 4, double, true><<<g, 256, 0, s>>>(bd, sp, tiles);
-        LCHK("k_eval_obs");
-    } else if (bd.eval_cs) {
-        if (mb == 2) k_eval_obs<true, 2, double, false, true><<<g, 256, 0, s>>>(bd, sp, tiles);
-        else if (mb == 3) k_eval_obs<true, 3, double, false, true><<<g, 256, 0, s>>>(bd, sp, tiles);
-        else k_eval_obs<true, 4, double, false, true><<<g, 256, 0, s>>>(bd, sp, tiles);
-        LCHK("k_eval_obs");
+        if (bd.fused) k_eval_obs<true, 2, float, false><<<g, 256, 0, s>>>(bd, sp, kEvalTiles);
+        else k_eval_obs<true, 2, float, true><<<g, 256, 0, s>>>(bd, sp, kEvalTiles);
     } else {
-        if (mb == 2) k_eval_obs<true, 2, double, false><<<g, 256, 0, s>>>(bd, sp, tiles);
-        else if (mb == 3) k_eval_obs<true, 3, double, false><<<g, 256, 0, s>>>(bd, sp, tiles);
-        else k_eval_obs<true, 4, double, false><<<g, 256, 0, s>>>(bd, sp, tiles);
-        LCHK("k_eval_obs");
+        if (bd.fused) k_eval_obs<true, 2, double, false><<<g, 256, 0, s>>>(bd, sp, kEvalTiles);
+        else k_eval_obs<true, 2, double, true><<<g, 256, 0, s>>>(bd, sp, kEvalTiles);
     }
+    LCHK("k_eval_obs");
 }
 
 // =====================================================================================================================
@@ -728,20 +716,20 @@ __global__ void __launch_bounds__(256, 2) k_schur_syrk(BatchDev bd) {
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
-// Register-resident, TMA-fed kernel for reduced systems of up to 184 rows (<= 30 free keyframes): ONE CTA owns the whole
+// Register-resident, TMA-fed kernel for reduced systems of up to kFusedMaxRows rows (<= 30 free keyframes): ONE CTA owns the whole
 // lower triangle of Sred as accumulator tiles spread over 16 warps.  k_landmark_reduce / k_obs_v have already laid V out
 // as dense column-major chunk panels in global memory (zeros included), so a panel half (48 columns x rs rows, <= 75 KB) arrives with ONE
 // cp.async.bulk into a 2-stage shared-memory ring while the tensor-core loop works on the other stage: no scatter, no
 // zero fill, no index loads in this kernel.  rs == 4 (mod 16) keeps the m8n8k4 fragment loads bank-conflict free.
 // ---------------------------------------------------------------------------------------------------------------------
-constexpr int kHalfCols = 48;
-constexpr int kStageDoubles = kHalfCols * 196;  // 184 rows -> rs = 196
-
 }  // namespace kba
 #include "kba_schur_fused.cuh"
 namespace kba {
 
-constexpr int kBlockSlots = 5;  // ceil(12*13/2 / 16) 16x16 blocks per warp for up to 184 reduced rows
+constexpr int kHalfCols = 48;
+constexpr int kStageDoubles = kHalfCols * kFMaxRs;
+
+constexpr int kBlockSlots = 5;  // ceil(12*13/2 / 16) 16x16 blocks per warp for up to kFusedMaxRows reduced rows
 // Which 16x16 blocks (linear index bi (bi + 1) / 2 + bj of the 12-row lower triangle) a warp owns.  The accumulators are
 // registers, so the map is static; a chunk only touches the blocks inside its keyframe row range (a sub-square of the
 // triangle plus the right-hand-side row), and with the plain cyclic map the busiest warp of such a chunk owns ~1.5x the
@@ -2143,7 +2131,7 @@ cudaError_t configure_kernels(int nr_cap_max) {
         if (e != cudaSuccess) return e;
         fixed_done[dev] = true;
     }
-    if (nr_cap_max <= 192 && nr_cap_max > hi_tiled[dev]) {
+    if (nr_cap_max <= kTiledMaxRows && nr_cap_max > hi_tiled[dev]) {
         e = cudaFuncSetAttribute(k_reduced_solve<true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                  (int)solve_tiled_smem(nr_cap_max));
         if (e != cudaSuccess) return e;
@@ -2206,7 +2194,7 @@ int launch_pass(const BatchDev& bd, const SolveParams& sp, const LaunchCfg& lc, 
         LCHK("k_gp_eval");
         if (timed) cudaEventRecord(lc.ev_pool[(*lc.ev_used)++], s);
         const int n_units = (lin_tile_bound(bd.max_obs, bd.max_lm) + kLinWarps - 1) / kLinWarps;
-        const dim3 g_lin(strided_grid(lc.lin_grid, n_units, 1, 8, B, lc.sm_count, kLinMinBlocks, 6), B);  // CTAs of a window stride over its units
+        const dim3 g_lin(strided_grid(lc.knobs.lin_grid, n_units, 1, 8, B, lc.sm_count, kLinMinBlocks, 6), B);  // CTAs of a window stride over its units
         if ((int)g_lin.x < n_units) k_linearize<true><<<g_lin, kLinThreads, 0, s>>>(bd, sp, n_units);
         else k_linearize<false><<<g_lin, kLinThreads, 0, s>>>(bd, sp, n_units);
         LCHK("k_linearize");
@@ -2229,7 +2217,7 @@ int launch_pass(const BatchDev& bd, const SolveParams& sp, const LaunchCfg& lc, 
             k_obs_v2<<<g_obs, 256, 0, s>>>(bd); LCHK("k_obs_v2");
         }
         const dim3 gf(bd.p_split, B);
-        if (lc.fused_slots == 7) k_schur_fused<7><<<gf, 512, schur_fused_smem(), s>>>(bd);
+        if (lc.plan.fused_slots == 7) k_schur_fused<7><<<gf, 512, schur_fused_smem(), s>>>(bd);
         else k_schur_fused<6><<<gf, 512, schur_fused_smem(), s>>>(bd);
         LCHK("k_schur_fused");
     } else {
@@ -2240,13 +2228,13 @@ int launch_pass(const BatchDev& bd, const SolveParams& sp, const LaunchCfg& lc, 
         LCHK("k_gp_panel");
     }
     if (bd.fused) {
-    } else if (lc.small_syrk) {
+    } else if (lc.plan.small_syrk) {
         k_schur_syrk_tma<<<dim3(bd.p_split, B), 512, schur_tma_smem(), s>>>(bd); LCHK("k_schur_syrk_tma");
     } else {
-        const int nb = lc.nr_cap_max / 64;
+        const int nb = lc.plan.nr_cap_max / 64;
         k_schur_syrk<<<dim3(nb * (nb + 1) / 2, bd.p_split, B), 256, schur_smem(), s>>>(bd); LCHK("k_schur_syrk");
     }
-    const dim3 g_red((lc.nr_cap_max * lc.nr_cap_max + 255) / 256, B);
+    const dim3 g_red((lc.plan.nr_cap_max * lc.plan.nr_cap_max + 255) / 256, B);
     BatchDev bc = bd;  // consumer view of the reduced system
     if (bd.sharded) {
         // the one exchange of the linearisation: reduced system (Schur sums + right-hand side), pose blocks, ground-plane blocks and
@@ -2267,22 +2255,22 @@ int launch_pass(const BatchDev& bd, const SolveParams& sp, const LaunchCfg& lc, 
         k_sred_reduce<<<g_red, 256, 0, s>>>(bd, 0); LCHK("k_sred_reduce");
     }
     if (bd.solve_tiled) {
-        k_reduced_solve<true><<<B, 512, solve_tiled_smem(lc.nr_cap_max), s>>>(bc, sp, 0); LCHK("k_reduced_solve");
+        k_reduced_solve<true><<<B, 512, solve_tiled_smem(lc.plan.nr_cap_max), s>>>(bc, sp, 0); LCHK("k_reduced_solve");
     } else if (!bd.solve_split) {
-        k_reduced_solve<false><<<B, 512, solve_smem(lc.nr_cap_max), s>>>(bc, sp, 0); LCHK("k_reduced_solve");
+        k_reduced_solve<false><<<B, 512, solve_smem(lc.plan.nr_cap_max), s>>>(bc, sp, 0); LCHK("k_reduced_solve");
     } else {  // few large windows: the factorisation is spread over the GPU, one 32-column block at a time
-        k_reduced_solve<false><<<B, 512, solve_smem(lc.nr_cap_max), s>>>(bc, sp, 1); LCHK("k_reduced_solve");
-        const int strips = (lc.nr_cap_max + 7) / 8;
-        for (int kb = 0; kb < lc.nr_cap_max; kb += kNB) {
+        k_reduced_solve<false><<<B, 512, solve_smem(lc.plan.nr_cap_max), s>>>(bc, sp, 1); LCHK("k_reduced_solve");
+        const int strips = (lc.plan.nr_cap_max + 7) / 8;
+        for (int kb = 0; kb < lc.plan.nr_cap_max; kb += kNB) {
             k_chol_diag<<<B, 32, 0, s>>>(bc, kb); LCHK("k_chol_diag");
             k_chol_panel<<<dim3((strips + 15) / 16, B), 512, 0, s>>>(bc, kb); LCHK("k_chol_panel");
-            k_chol_trail<<<dim3(bd.solve_split, B), 512, trail_smem(lc.nr_cap_max), s>>>(bc, kb); LCHK("k_chol_trail");
+            k_chol_trail<<<dim3(bd.solve_split, B), 512, trail_smem(lc.plan.nr_cap_max), s>>>(bc, kb); LCHK("k_chol_trail");
         }
-        k_reduced_solve<false><<<B, 512, solve_smem(lc.nr_cap_max), s>>>(bc, sp, 2); LCHK("k_reduced_solve");
+        k_reduced_solve<false><<<B, 512, solve_smem(lc.plan.nr_cap_max), s>>>(bc, sp, 2); LCHK("k_reduced_solve");
     }
     if (bd.fused) {
         const int n_units = (bd.max_lm + 15) / 16;
-        const int gx = strided_grid(lc.bs_grid, n_units, 1, 3, B, lc.sm_count, 2, 8);
+        const int gx = strided_grid(lc.knobs.bs_grid, n_units, 1, 3, B, lc.sm_count, 2, 8);
         if (gx < n_units) k_backsub_v<true><<<dim3(gx, B), 256, 0, s>>>(bd, n_units);
         else k_backsub_v<false><<<dim3(n_units, B), 256, 0, s>>>(bd, n_units);
     }
@@ -2308,7 +2296,7 @@ int launch_pass(const BatchDev& bd, const SolveParams& sp, const LaunchCfg& lc, 
         const int prep = lin1 ? 1 : 2 + (bd.fused ? 1 : lc.max_rank + 1 + gp);  // pose blocks [, landmark blocks, V rows]
         cnt->launches_total += gp; cnt->launches_prep += gp;                       // k_gp_blocks
         if (bd.sharded && bd.shard_gp) cnt->launches_total += 1;                   // k_shard_planes
-        const int split = (!bd.solve_tiled && bd.solve_split) ? 1 + 3 * ((lc.nr_cap_max + kNB - 1) / kNB) : 0;
+        const int split = (!bd.solve_tiled && bd.solve_split) ? 1 + 3 * ((lc.plan.nr_cap_max + kNB - 1) / kNB) : 0;
         cnt->launches_total += (bd.fused ? 0 : 1) + 1 + 1 + gp + prep + 1 + (bd.p_split > 1 ? 1 : 0) + 1 + split + 1 + 1 + gp + 1 + 2;
         cnt->launches_jacobian += 1; cnt->launches_prep += prep + gp; cnt->launches_schur += 1; cnt->launches_solve += 2;
         cnt->launches_backsub += 1; cnt->launches_cost += 1 + gp; cnt->launches_update += 1; cnt->launches_trim += 2;

@@ -38,14 +38,10 @@ struct Exchange {
 };
 
 struct LaunchCfg {
-    int nr_cap_max = 64;
+    Plan plan;                // what the batch runs (kba_plan.h); BatchDev holds the fields the kernels read
+    Knobs knobs;              // read when the batch was created
     int sm_count = 132;       // SMs of the device the batch runs on (strided_grid: waves of CTAs)
     int max_rank = 0;         // largest observation rank in the batch (multi-camera rigs)
-    bool small_syrk = false;  // every window has <= 184 reduced rows: register-resident Schur kernel
-    bool lin_fused = true;    // fused path: evaluation + landmark blocks + V rows in one kernel (k_linearize); KBA_LINEARIZE=0: three kernels
-    int lin_grid = -1;        // CTAs per window of k_linearize striding over its tile units (KBA_LIN_GRID; -1: by batch size, 0: one CTA per unit)
-    int bs_grid = -1;         // the same for k_backsub_v (KBA_BS_GRID; 0: one CTA per 16 landmarks)
-    int fused_slots = 6;      // fused Schur kernel instance: 6 accumulator blocks per warp (<= 176 rows) or 7 (<= 184)
     int rounds_override = -1, min_landmarks_for_trimming = 100, num_rounds_option = 1;
     bool time_jacobian = false;
     cudaEvent_t* ev_pool = nullptr;  // pairs of events bracketing each residual/Jacobian launch
@@ -152,7 +148,6 @@ struct MotionArgs {
 void launch_adjust_pose(const MotionArgs& a, int n_frames, const SolveParams& sp, cudaStream_t s);
 
 cudaError_t configure_pack();
-int pack_max_landmarks();
 void launch_pack(const BatchDev& bd, const PackRaw& raw, cudaStream_t s);
 void launch_unpack_landmarks(const BatchDev& bd, double* lm_user, unsigned char* rejected_user, cudaStream_t s);
 

@@ -21,8 +21,6 @@
 
 namespace kba {
 
-constexpr int kPackMaxLm = 32768;  // 15 index bits; 128 KB of keys in shared memory
-
 __global__ void __launch_bounds__(1024) k_pack_sort(BatchDev bd, PackRaw raw) {
     const int w = blockIdx.x;
     const WinDesc& wd = bd.desc[w];
@@ -496,10 +494,9 @@ void launch_track_writeback(const BatchDev& bd, const TrackDev* tds, const Track
 }
 
 cudaError_t configure_pack() {
-    return cudaFuncSetAttribute(k_pack_sort, cudaFuncAttributeMaxDynamicSharedMemorySize, kPackMaxLm * (int)sizeof(unsigned));
+    return cudaFuncSetAttribute(k_pack_sort, cudaFuncAttributeMaxDynamicSharedMemorySize, kPackMaxLandmarks * (int)sizeof(unsigned));
 }
 
-int pack_max_landmarks() { return kPackMaxLm; }
 
 void launch_pack(const BatchDev& bd, const PackRaw& raw, cudaStream_t s) {
     const int B = bd.n_win;

@@ -1,4 +1,4 @@
-// kba_schur_fused.cuh -- Schur complement of a small window (<= 184 reduced rows) in ONE warp-specialised kernel:
+// kba_schur_fused.cuh -- Schur complement of a small window (<= kFusedMaxRows reduced rows) in ONE warp-specialised kernel:
 //
 //   k_obs_v2 (kba_prep.cuh, one thread per observation, full occupancy) has written V_i = (J_p^T J_l) L^-T compactly:
 //   18 doubles per observation (3 columns x 6 rows), no padding.
@@ -37,14 +37,13 @@ namespace kba {
 constexpr int kLG = 8;                           // landmarks per group
 constexpr int kGC = 3 * kLG;                     // panel columns per group
 constexpr int kFStages = 6;                     // 6 x 37.6 KB: the async copies of up to five groups are in flight
-constexpr int kFMaxRs = 196;                     // 184 rows -> row stride 196 (== 4 mod 16)
+constexpr int kFMaxRs = (kFusedMaxRows + 11) / 16 * 16 + 4;  // row stride == 4 mod 16: 196
 constexpr int kFStageDoubles = kGC * kFMaxRs;
 constexpr int kFObs = 128;                       // observations staged per group = producer lanes
 constexpr int kFConsumerWarps = 12;
-constexpr int kFMaxKf = 32;
 
 // 16x16 block (16 bi + bj: block row bi, block column bj <= bi of the 12-row block triangle; 0xff: none) owned by each
-// consumer warp: slot 0 is the warp's block of row 11 (only systems of more than 176 rows have one), slots 1..6 blocks of
+// consumer warp: slot 0 is the warp's block of row 11 (only systems of more than kSixSlotMaxRows rows have one), slots 1..6 blocks of
 // rows <= 10.
 __constant__ unsigned char kSyrkMap12[12][7] = {
     {0xb6, 0x31, 0x61, 0x75, 0x80, 0x93, 0xaa}, {0xb1, 0x40, 0x42, 0x54, 0x84, 0x98, 0xff}, {0xb7, 0x10, 0x43, 0x52, 0x86, 0x95, 0xff},

@@ -35,7 +35,9 @@ CASES = {
     "config1": (lambda: synth.make_window(1), False, 1, None),                            # fused Schur kernel, small
     "config1_seed11": (lambda: synth.make_window(1, seed=11), False, 1, None),
     "config2_full": (lambda: synth.make_window(2), False, 8, None),                       # fused six-slot, the bench workload
-    "free_keyframes_30": (lambda: synth.make_window(2, n_kf=31, n_lm=700, n_obs=7000, seed=5), False, 1, None),  # seven-slot
+    # 187 rows over all 31 keyframes: the large-window path (k_schur_syrk, tiled k_reduced_solve at 192 rows), not the seven-slot
+    # kernel its 30 free keyframes would select on the fused path
+    "free_keyframes_30": (lambda: synth.make_window(2, n_kf=31, n_lm=700, n_obs=7000, seed=5), False, 1, None),
     "gap_over_fixed_keyframe": (lambda: _shapes("_gap_over_fixed_keyframe"), False, 1, None),   # per-observation copies
     "stereo_rig": (lambda: _shapes("_stereo_rig"), False, 1, None),                       # rank > 0: synchronous producer
     "ragged": (ew.CASES["ragged"], False, 1, None),                                       # empty CSR rows

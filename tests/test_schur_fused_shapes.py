@@ -66,7 +66,8 @@ def _window(case):
         return _gap_over_fixed_keyframe()
     if case == "stereo_rig":
         return _stereo_rig()
-    # 30 free keyframes: 180 pose rows + the right-hand side, a 12th block row (the kernel's seven-slot variant)
+    # 30 free keyframes, but 187 rows over all 31 keyframes: the large-window path (k_schur_syrk) with KBA_FUSED=1 as with
+    # KBA_FUSED=0, so this case compares that path with itself; the seven-slot variant needs 30 keyframes none of which is fixed
     return synth.make_window(2, n_kf=31, n_lm=700, n_obs=7000, seed=5)
 
 
