@@ -350,6 +350,48 @@ int kba_track_solve(kba_track* t, int32_t n_kf, const int32_t* kf_slot, const ui
                     const kba_window* sel, const kba_options* opt, kba_result* res);
 int kba_track_transfer_bytes(kba_track* t, int64_t* h2d_last_solve, int64_t* d2h_last_solve, int64_t* h2d_pushes_total);
 
+/* ---- landmark selection on the stored window (SURVEY row A17) ---------------------------------------------------------
+ * The per-landmark quantities of limo's selection chain (landmark_selector.hpp:118-253 with LandmarkRejectionSchemeCheirality and
+ * LandmarkSparsificationSchemeVoxel, as facade/landmark_selection.cpp states them), computed from what the store holds: keyframe
+ * poses, the measurement arena, landmark positions by slot, the cameras.  The host keeps the ranking that consumes them (the
+ * partial sorts, the std::rand shuffle of the middle bin, the bin caps), so a caller that ranks as LandmarkSelector::select does
+ * gets its selection bit for bit.  A request:
+ *   - kf_slot [n_kf]: the active keyframes in ascending timestamp (= id) order, every one pushed; the last one is the newest;
+ *   - lm_slot [n_cand]: the candidates, i.e. the active landmarks minus the outliers, in ascending id order (<= max_landmarks).
+ * Per candidate c:
+ *   - cheiral[c] = 1 iff z of cam * (kf * pos) is not below 0 for every arena entry of a listed keyframe that measures it;
+ *   - among the cheirality survivors (labelled in candidate order), the voxel scheme's steps 1-5: the position in the newest
+ *     keyframe's frame rounded to float, PassThrough z in [-20, 100], distance (double) to the path of the listed keyframes'
+ *     positions; far bin iff it is not below roi_far; the others on the float voxel grid of voxel_size (one point per voxel,
+ *     the centroid, labelled by the voxel's first candidate); middle bin iff the centroid's distance is not below roi_middle.
+ *     bin[c] = 0 near-bin voxel representative, 1 middle-bin representative, 2 far, -1 dropped (not cheiral, PassThrough,
+ *     not the first candidate of its voxel);
+ *   - near_order[0..*n_near): the near representatives' candidate indices in ascending voxel index (the scheme's ids_near);
+ *   - flow[c] (near representatives): calcFlow(use_mean = false), per camera index the sum of the pixel distances between
+ *     consecutive observations in keyframe order, the maximum over the cameras; NaN for a landmark no camera saw twice, and for
+ *     every other candidate.  Camera indices stand for the caller's camera ids: they must be in the same order;
+ *   - seen[c] (every candidate): how many listed keyframes measure it (chooseFarLmIds).
+ * Every float operation is the host code's, in its order, without contraction: the quantities equal the host's bit for bit.
+ * One upload (the lists), one launch sequence, one download; the first call allocates the buffers for the track's capacities,
+ * later calls allocate nothing.  kba_track_transfer_bytes then reports this call's upload and download.
+ * Errors, before anything is uploaded: a null pointer, n_kf < 1, a slot out of range or listed twice, a keyframe slot not pushed,
+ * a voxel size that is not finite and positive: KBA_ERR_BAD_ARG; more keyframes or candidates than the track has slots:
+ * KBA_ERR_CAPACITY. */
+typedef struct kba_select_params {
+    double voxel_size[3];      /* LandmarkSparsificationSchemeVoxel::Parameters::voxel_size_xyz                    */
+    double roi_far, roi_middle; /* roi_far_xyz[0], roi_middle_xyz[0]: distances to the keyframe path              */
+} kba_select_params;
+typedef struct kba_select_out {  /* caller-owned arrays of n_cand entries */
+    uint8_t* cheiral;
+    int8_t* bin;
+    int32_t* near_order;
+    int32_t* n_near;          /* one value */
+    double* flow;
+    int32_t* seen;
+} kba_select_out;
+int kba_track_select_landmarks(kba_track* t, int32_t n_kf, const int32_t* kf_slot, int32_t n_cand, const int32_t* lm_slot,
+                               const kba_select_params* p, kba_select_out* out);
+
 /* ---- many persistent windows in one launch: track groups -----------------------------------------------------------------
  * kba_track_solve solves one window per call, which leaves the GPU mostly idle.  A group solves one window of each of its tracks
  * as ONE batch (one kba_batch_solve: one CUDA graph launch), with the persistent store of every track: per solve only the

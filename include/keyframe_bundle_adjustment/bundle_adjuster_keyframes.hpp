@@ -78,6 +78,12 @@ public:
     // adjustPoseOnly() then tracks the frame against the landmarks in that store (kba_track_adjust_pose) when the store has every
     // landmark and camera of the frame, and otherwise rebuilds its one-keyframe window.
     void set_persistent_window(bool on) { persistent_window_ = on; }
+    // Not in the reference: with the persistent window on, solve() lets the store compute the per-landmark quantities of the
+    // landmark selector's chain (kba_track_select_landmarks) when the chain is cheirality + voxel (+ selection schemes, limo's
+    // mono-lidar configuration); the selector ranks them exactly as its host select() does, so the selection is the same.
+    // On by default; lastSelectionOnDevice() tells whether the last solve() selected that way.
+    void set_device_selection(bool on) { device_selection_ = on; }
+    bool lastSelectionOnDevice() const { return last_select_on_device_; }
     // host -> device bytes of the last solve() (either path) and of all push() calls so far (persistent path)
     long long lastSolveUploadBytes() const { return last_solve_h2d_; }
     long long pushUploadBytes() const { return push_h2d_; }
@@ -103,19 +109,21 @@ private:
     // persistent device-resident window
     bool ensureHandle();
     bool trackPush(const Keyframe& kf);
-    bool solveTracked(const std::vector<Keyframe*>& kfs, const std::vector<LandmarkId>& lm_ids, std::string& report);
+    bool trackSync(const std::vector<Keyframe*>& kfs);
+    bool selectOnDevice(const std::vector<Keyframe*>& kfs);
+    bool solveTracked(const std::vector<Keyframe*>& kfs, const std::vector<LandmarkId>& lm_ids, std::string& report, bool synced);
     bool adjustPoseTracked(Keyframe& kf, const std::vector<LandmarkId>& lm_ids, std::string& report);
     bool flushLandmarks();  // new and dirty landmark state into the store, before any use of the track
     void speedPrior(const Keyframe& speed_kf, kba_window& w) const;
     kba_track* track_{nullptr};
-    bool persistent_window_{true}, track_failed_{false};
+    bool persistent_window_{true}, track_failed_{false}, device_selection_{true}, last_select_on_device_{false};
     std::map<KeyframeId, int> kf_slot_;
     std::map<LandmarkId, int> lm_slot_;
     std::vector<int> free_kf_slots_;
     std::vector<std::array<double, 10>> track_cams_;  // camera values (f, pp, pose_camera_vehicle) the track was created with
     std::set<LandmarkId> new_landmarks_, dirty_weights_;
     std::set<LandmarkId> dirty_positions_;  // positions the rebuild path wrote on the host only
-    long long last_solve_h2d_{0}, push_h2d_{0};
+    long long last_solve_h2d_{0}, push_h2d_{0}, last_select_h2d_{0};
 };
 
 }  // namespace keyframe_bundle_adjustment

@@ -18,6 +18,9 @@ std::vector<LandmarkId> chooseMiddleLmIds(size_t max_num, const std::vector<Land
 // far bin: the ids observed from the most keyframes
 std::vector<LandmarkId> chooseFarLmIds(size_t max_num, const std::vector<LandmarkId>& ids_far,
                                        const std::map<KeyframeId, Keyframe::ConstPtr>& keyframes);
+// ... the same ranking from the number of keyframes observing each of them (from the device-resident store, say)
+std::vector<LandmarkId> chooseFarLmIds(size_t max_num, const std::vector<LandmarkId>& ids_far,
+                                       const std::map<LandmarkId, unsigned int>& seen);
 // per landmark and camera: pixel flow summed (use_mean: averaged) over consecutive keyframes that both see it; the
 // landmark's value is the maximum over the cameras.  Landmarks seen only once have no entry.
 std::map<LandmarkId, double> calcFlow(const std::vector<LandmarkId>& landmarks,

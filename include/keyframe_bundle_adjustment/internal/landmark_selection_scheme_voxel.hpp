@@ -32,6 +32,14 @@ public:
     std::set<LandmarkId> getSelection(const LandmarkMap& landmarks, const KeyframeMap& keyframes) const override;
     std::map<LandmarkId, LandmarkCategorizatonInterface::Category> getCategorizedSelection(
         const LandmarkMap& landmarks, const KeyframeMap& keyframes) const override;
+    // step 6 alone: the capped ranking of the bins from the per-landmark quantities of steps 1-5 (ids_near in ascending voxel
+    // index, ids_middle / ids_far ascending; flow of the near landmarks that have one, seen counts of the far ones).
+    // getCategorizedSelection ends in it; LandmarkSelector feeds it the quantities the device-resident store computed.
+    std::map<LandmarkId, LandmarkCategorizatonInterface::Category> rankBins(const std::vector<LandmarkId>& ids_near,
+                                                                            const std::map<LandmarkId, double>& flow,
+                                                                            const std::vector<LandmarkId>& ids_middle,
+                                                                            const std::vector<LandmarkId>& ids_far,
+                                                                            const std::map<LandmarkId, unsigned int>& seen) const;
     static ConstPtr createConst(Parameters p = Parameters()) { return ConstPtr(new LandmarkSparsificationSchemeVoxel(p)); }
     static Ptr create(Parameters p = Parameters()) { return Ptr(new LandmarkSparsificationSchemeVoxel(p)); }
     Parameters params_;

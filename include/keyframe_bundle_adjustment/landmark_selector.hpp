@@ -3,6 +3,7 @@
 // schemes name landmarks that are taken in any case, sparsification schemes thin out the rest; landmarks that were not
 // selected age in a counter that forgets after 10 s.
 #pragma once
+#include <cstdint>
 #include <map>
 #include <memory>
 #include <set>
@@ -28,6 +29,27 @@ public:
     std::set<LandmarkId> select(const std::map<LandmarkId, Landmark::ConstPtr>& landmarks,
                                 const std::map<KeyframeId, Keyframe::ConstPtr>& kfs);
 
+    // Not in the reference: the per-landmark quantities of the cheirality + voxel chain, computed outside the selector
+    // (kba_track_select_landmarks on the device-resident store, include/kba_b200.h).  candidates: the landmarks given to select()
+    // minus the outliers, ascending id; the other vectors by candidate, as kba_select_out describes them.
+    struct ChainQuantities {
+        std::vector<LandmarkId> candidates;
+        std::vector<uint8_t> cheiral;
+        std::vector<int8_t> bin;
+        std::vector<int32_t> near_order;  // the near bin, candidate indices in ascending voxel index
+        std::vector<double> flow;         // NaN: no flow value
+        std::vector<int32_t> seen;
+    };
+    // The voxel scheme of a chain such quantities stand for -- exactly one rejection scheme, the cheirality one, exactly one
+    // sparsification scheme, the voxel one, and any selection schemes (they run on the host over the cheirality survivors) --
+    // or nullptr for any other chain.
+    const LandmarkSparsificationSchemeVoxel* quantitiesChainVoxel() const;
+    // select() with q in place of the chain's own loops over keyframes and measurements: the ranking (std::rand included), the
+    // categories, the aging of unselected landmarks and the result are those of select(landmarks, kfs) on the same state.
+    // Throws std::invalid_argument if the chain is not one quantitiesChainVoxel() accepts or q.candidates are not the candidates.
+    std::set<LandmarkId> select(const std::map<LandmarkId, Landmark::ConstPtr>& landmarks,
+                                const std::map<KeyframeId, Keyframe::ConstPtr>& kfs, const ChainQuantities& q);
+
     void markUnselected(LandmarkId lm_id, TimestampNSec last_time_seen) {
         unselected_lms_[lm_id] += 1;
         last_time_seen_[lm_id] = last_time_seen;
@@ -48,6 +70,8 @@ public:
     std::set<LandmarkId> outlier_ids_;
 
 private:
+    std::set<LandmarkId> selectImpl(const std::map<LandmarkId, Landmark::ConstPtr>& landmarks,
+                                    const std::map<KeyframeId, Keyframe::ConstPtr>& kfs, const ChainQuantities* q);
     std::set<LandmarkId> runScheme(const LandmarkSchemeBase& scheme, const std::map<LandmarkId, Landmark::ConstPtr>& lms,
                                    const std::map<KeyframeId, Keyframe::ConstPtr>& kfs);
     std::map<LandmarkId, unsigned int> unselected_lms_;

@@ -8,8 +8,8 @@ import os
 
 import numpy as np
 
-from .capi_types import (KbaCounters, KbaEvalOut, KbaLidarOptions, KbaOptions, KbaResult, KbaTrackCaps, KbaTrackFrame, KbaTrackRequest,
-                         KbaWindow, Result, Window, c_double_p, c_int32_p)
+from .capi_types import (KbaCounters, KbaEvalOut, KbaLidarOptions, KbaOptions, KbaResult, KbaSelectOut, KbaSelectParams, KbaTrackCaps,
+                         KbaTrackFrame, KbaTrackRequest, KbaWindow, Result, Window, c_double_p, c_int32_p)
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("KBA_LIB_PATH") or os.path.join(_HERE, "libkba_b200.so")  # KBA_LIB_PATH: instrumented builds
@@ -24,7 +24,7 @@ SYMBOLS = ["kba_version", "kba_last_error", "kba_default_options", "kba_create",
            "kba_init_landmarks", "kba_track_create", "kba_track_destroy", "kba_track_push_keyframe", "kba_track_drop_keyframe",
            "kba_track_set_landmarks", "kba_track_set_keyframe_pose", "kba_track_set_keyframe_poses", "kba_track_solve", "kba_track_transfer_bytes",
            "kba_track_group_create", "kba_track_group_destroy", "kba_track_group_solve", "kba_track_group_transfer_bytes",
-           "kba_track_adjust_pose", "kba_track_group_adjust_pose"]
+           "kba_track_adjust_pose", "kba_track_group_adjust_pose", "kba_track_select_landmarks"]
 
 
 class KbaError(RuntimeError):
@@ -85,6 +85,7 @@ def lib():
         L.kba_track_group_transfer_bytes.argtypes = [vp, C.POINTER(C.c_int64), C.POINTER(C.c_int64)]
         L.kba_track_adjust_pose.argtypes = [vp, C.POINTER(KbaTrackFrame), C.POINTER(KbaOptions), C.POINTER(KbaResult)]
         L.kba_track_group_adjust_pose.argtypes = [vp, C.POINTER(KbaTrackFrame), C.POINTER(KbaOptions), C.POINTER(KbaResult)]
+        L.kba_track_select_landmarks.argtypes = [vp, C.c_int32, ip, C.c_int32, ip, C.POINTER(KbaSelectParams), C.POINTER(KbaSelectOut)]
         L.kba_lidar_default_options.argtypes = [C.POINTER(KbaLidarOptions)]
         L.kba_lidar_default_options.restype = None
         fp = C.POINTER(C.c_float)
@@ -275,6 +276,26 @@ class Track:
         res = self._frame_result(n_runs, iterations_capacity)
         _check(lib().kba_track_adjust_pose(self._p, C.byref(fr), C.byref(opt or default_options()), C.byref(res.c)))
         return res
+
+    def select_landmarks(self, kf_slots, lm_slots, voxel_size=(1.0, 1.0, 0.5), roi_far=50.0, roi_middle=25.0):
+        """per-landmark quantities of limo's selection chain on this track's store (kba_track_select_landmarks).
+        kf_slots: active keyframes in ascending timestamp order; lm_slots: candidates in ascending landmark id order.  The
+        defaults are LandmarkSparsificationSchemeVoxel::Parameters'.  Returns a dict of numpy arrays over the candidates:
+        cheiral (uint8), bin (int8: 0 near, 1 middle, 2 far, -1 dropped), near_order (int32 candidate indices in ascending voxel
+        index), flow (float64, NaN without a value), seen (int32)."""
+        kf, kfp = self._i32(kf_slots)
+        lm, lmp = self._i32(lm_slots)
+        n = len(lm)
+        out = dict(cheiral=np.zeros(n, np.uint8), bin=np.zeros(n, np.int8), near_order=np.zeros(n, np.int32),
+                   flow=np.zeros(n, np.float64), seen=np.zeros(n, np.int32))
+        n_near = np.zeros(1, np.int32)
+        o = KbaSelectOut(out["cheiral"].ctypes.data_as(C.POINTER(C.c_uint8)), out["bin"].ctypes.data_as(C.POINTER(C.c_int8)),
+                         out["near_order"].ctypes.data_as(c_int32_p), n_near.ctypes.data_as(c_int32_p),
+                         out["flow"].ctypes.data_as(c_double_p), out["seen"].ctypes.data_as(c_int32_p))
+        p = KbaSelectParams((C.c_double * 3)(*[float(x) for x in voxel_size]), float(roi_far), float(roi_middle))
+        _check(lib().kba_track_select_landmarks(self._p, len(kf), kfp, n, lmp, C.byref(p), C.byref(o)))
+        out["near_order"] = out["near_order"][:int(n_near[0])].copy()
+        return out
 
     def transfer_bytes(self):
         a, b, c = C.c_int64(), C.c_int64(), C.c_int64()

@@ -42,6 +42,15 @@ class KbaTrackRequest(C.Structure):
                 ("sel", C.POINTER(KbaWindow))]
 
 
+class KbaSelectParams(C.Structure):
+    _fields_ = [("voxel_size", C.c_double * 3), ("roi_far", C.c_double), ("roi_middle", C.c_double)]
+
+
+class KbaSelectOut(C.Structure):
+    _fields_ = [("cheiral", C.POINTER(C.c_uint8)), ("bin", C.POINTER(C.c_int8)), ("near_order", c_int32_p), ("n_near", c_int32_p),
+                ("flow", c_double_p), ("seen", c_int32_p)]
+
+
 class KbaTrackFrame(C.Structure):
     _fields_ = [("n_meas", C.c_int32), ("reserved_", C.c_int32), ("pose7", c_double_p), ("lm_slot", c_int32_p), ("cam", c_int32_p),
                 ("u", c_float_p), ("v", c_float_p), ("d", c_float_p), ("speed_weight", C.c_double), ("speed_dt", C.c_double),

@@ -350,15 +350,75 @@ std::string BundleAdjusterKeyframes::runWindow(const std::vector<Keyframe*>& kfs
     return solve_report(r, "");
 }
 
+namespace {
+std::array<double, 10> camera_value(const Camera& c);  // below, with the other helpers of the persistent window
+}  // namespace
+
 std::string BundleAdjusterKeyframes::solve() {  // cpp:629-767
     if (keyframes_.size() < 3) throw NotEnoughKeyframesException(keyframes_.size(), 3);
-    selected_landmark_ids_ = landmark_selector_->select(getActiveLandmarkConstPtrs(), getActiveKeyframeConstPtrs());
     std::vector<Keyframe*> kfs;
     for (const auto& id : active_keyframe_ids_) kfs.push_back(keyframes_.at(id).get());
+    last_select_h2d_ = 0;
+    const bool synced = selectOnDevice(kfs);
+    if (!synced) selected_landmark_ids_ = landmark_selector_->select(getActiveLandmarkConstPtrs(), getActiveKeyframeConstPtrs());
     std::vector<LandmarkId> lm_ids(selected_landmark_ids_.begin(), selected_landmark_ids_.end());
     std::string report;
-    if (persistent_window_ && !track_failed_ && solveTracked(kfs, lm_ids, report)) return report;
+    if (persistent_window_ && !track_failed_ && solveTracked(kfs, lm_ids, report, synced)) return report;
     return runWindow(kfs, lm_ids, false, nullptr);
+}
+
+// solve()'s landmark selection with the store computing the chain's per-landmark quantities (kba_track_select_landmarks) and the
+// selector ranking them: the same selection as the host select(), without a host pass over the window's measurements.  Only for
+// a chain the quantities stand for (LandmarkSelector::quantitiesChainVoxel), every active keyframe in the store, every candidate
+// with a slot, and camera ids that map onto the store's camera indices in the same order (flow is kept per camera).  true: the
+// selection is made and the store holds the active keyframes' current state; false: the caller selects on the host.
+bool BundleAdjusterKeyframes::selectOnDevice(const std::vector<Keyframe*>& kfs) {
+    last_select_on_device_ = false;
+    if (!device_selection_ || !persistent_window_ || track_failed_ || kfs.empty()) return false;
+    const LandmarkSparsificationSchemeVoxel* voxel = landmark_selector_->quantitiesChainVoxel();
+    if (!voxel) return false;
+    for (const Keyframe* kf : kfs)
+        if (!kf->is_active_) return false;  // the host's cheirality test skips inactive keyframes
+    if (!trackSync(kfs)) return false;
+    std::map<CameraId, int> cam_index;
+    for (const Keyframe* kf : kfs)
+        for (const auto& c : kf->cameras_) {
+            const int idx = int(std::find(track_cams_.begin(), track_cams_.end(), camera_value(*c.second)) - track_cams_.begin());
+            const auto ins = cam_index.emplace(c.first, idx);
+            if (!ins.second && ins.first->second != idx) return false;
+        }
+    int prev = -1;
+    for (const auto& el : cam_index) {
+        if (el.second <= prev) return false;
+        prev = el.second;
+    }
+    LandmarkSelector::ChainQuantities q;
+    std::vector<int32_t> kf_slots, lm_slots;
+    for (const Keyframe* kf : kfs) kf_slots.push_back(kf_slot_.at(kf->timestamp_));
+    const auto landmarks = getActiveLandmarkConstPtrs();
+    const auto& outliers = landmark_selector_->getOutliers();
+    for (const auto& el : landmarks) {
+        if (outliers.count(el.first)) continue;
+        const auto it = lm_slot_.find(el.first);
+        if (it == lm_slot_.end()) return false;
+        q.candidates.push_back(el.first);
+        lm_slots.push_back(it->second);
+    }
+    const size_t n = q.candidates.size();
+    q.cheiral.resize(n); q.bin.resize(n); q.near_order.resize(n); q.flow.resize(n); q.seen.resize(n);
+    int32_t n_near = 0;
+    const auto& vp = voxel->params_;
+    kba_select_params p{{vp.voxel_size_xyz[0], vp.voxel_size_xyz[1], vp.voxel_size_xyz[2]}, vp.roi_far_xyz[0], vp.roi_middle_xyz[0]};
+    kba_select_out o{q.cheiral.data(), q.bin.data(), q.near_order.data(), &n_near, q.flow.data(), q.seen.data()};
+    if (kba_track_select_landmarks(track_, int(kf_slots.size()), kf_slots.data(), int(n), lm_slots.data(), &p, &o) != KBA_OK)
+        throw std::runtime_error(std::string("kba_b200: ") + kba_last_error());
+    q.near_order.resize(size_t(n_near));
+    int64_t h2d = 0;
+    kba_track_transfer_bytes(track_, &h2d, nullptr, nullptr);
+    last_select_h2d_ = (long long)h2d;
+    selected_landmark_ids_ = landmark_selector_->select(landmarks, getActiveKeyframeConstPtrs(), q);
+    last_select_on_device_ = true;
+    return true;
 }
 
 // ---- persistent device-resident window ---------------------------------------------------------------------------------------
@@ -435,24 +495,37 @@ bool BundleAdjusterKeyframes::trackPush(const Keyframe& kf) {
 }
 
 // solve() on the device-resident window: only the selection goes up.  false: not possible for this window (caller rebuilds).
-bool BundleAdjusterKeyframes::solveTracked(const std::vector<Keyframe*>& kfs, const std::vector<LandmarkId>& lm_ids, std::string& report) {
-    if (int(kfs.size()) > kTrackWinKeyframes || int(lm_ids.size()) > kTrackWinLandmarks) return false;
+// The store brought to the host's state for the active keyframes kfs: every one pushed, their poses / planes, new landmarks,
+// positions and weights.  false: not possible (track_failed_ is set).
+bool BundleAdjusterKeyframes::trackSync(const std::vector<Keyframe*>& kfs) {
     for (const Keyframe* kf : kfs)
         if (!kf_slot_.count(kf->timestamp_) && !trackPush(*kf)) { track_failed_ = true; return false; }
-    // state the host may have changed since the last solve: poses / planes of the active keyframes, new landmarks, weights
-    const int n_kf = int(kfs.size()), n_lm = int(lm_ids.size());
-    std::vector<int32_t> kf_slots, lm_slots;
-    std::vector<uint8_t> fixed;
+    std::vector<int32_t> kf_slots;
     std::vector<double> poses, planes;
     for (const Keyframe* kf : kfs) {
         kf_slots.push_back(kf_slot_.at(kf->timestamp_));
-        fixed.push_back(kf->fixation_status_ == Keyframe::FixationStatus::Pose);
         poses.insert(poses.end(), kf->pose_.begin(), kf->pose_.end());
         planes.insert(planes.end(), kf->local_ground_plane_.direction.begin(), kf->local_ground_plane_.direction.end());
         planes.push_back(kf->local_ground_plane_.distance);
     }
-    if (kba_track_set_keyframe_poses(track_, n_kf, kf_slots.data(), poses.data(), planes.data()) != KBA_OK) { track_failed_ = true; return false; }
+    if (kba_track_set_keyframe_poses(track_, int(kfs.size()), kf_slots.data(), poses.data(), planes.data()) != KBA_OK) { track_failed_ = true; return false; }
     if (!flushLandmarks()) { track_failed_ = true; return false; }
+    return true;
+}
+
+// synced: trackSync(kfs) already ran for this solve (the device-side selection needed the same state)
+bool BundleAdjusterKeyframes::solveTracked(const std::vector<Keyframe*>& kfs, const std::vector<LandmarkId>& lm_ids, std::string& report,
+                                           bool synced) {
+    if (int(kfs.size()) > kTrackWinKeyframes || int(lm_ids.size()) > kTrackWinLandmarks) return false;
+    // state the host may have changed since the last solve: poses / planes of the active keyframes, new landmarks, weights
+    if (!synced && !trackSync(kfs)) return false;
+    const int n_kf = int(kfs.size()), n_lm = int(lm_ids.size());
+    std::vector<int32_t> kf_slots, lm_slots;
+    std::vector<uint8_t> fixed;
+    for (const Keyframe* kf : kfs) {
+        kf_slots.push_back(kf_slot_.at(kf->timestamp_));
+        fixed.push_back(kf->fixation_status_ == Keyframe::FixationStatus::Pose);
+    }
     for (const auto id : lm_ids) {
         auto it = lm_slot_.find(id);
         if (it == lm_slot_.end()) return false;  // selected but never measured by a stored keyframe: let the rebuild path decide
@@ -481,7 +554,8 @@ bool BundleAdjusterKeyframes::solveTracked(const std::vector<Keyframe*>& kfs, co
     int64_t h2d = 0, d2h = 0, pushes = 0;
     kba_track_transfer_bytes(track_, &h2d, &d2h, &pushes);
     push_h2d_ = (long long)pushes;
-    last_solve_h2d_ = (long long)h2d + (long long)n_kf * (7 + 4) * 8;  // the selection lists + the active keyframes' poses
+    // the selection lists + the active keyframes' poses, and the lists of a device-side landmark selection
+    last_solve_h2d_ = (long long)h2d + (long long)n_kf * (7 + 4) * 8 + last_select_h2d_;
     for (int k = 0; k < n_kf; ++k) {  // in place, as the reference (cpp:554-557); planes nothing was attached to come back unchanged
         std::copy_n(out_pose.begin() + 7 * k, 7, kfs[k]->pose_.begin());
         std::copy_n(out_plane.begin() + 4 * k, 3, kfs[k]->local_ground_plane_.direction.begin());

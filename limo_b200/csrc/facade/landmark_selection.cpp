@@ -6,6 +6,7 @@
 #include <cstdint>
 #include <cstdlib>
 #include <limits>
+#include <iterator>
 #include <stdexcept>
 
 #include "keyframe_bundle_adjustment/landmark_selector.hpp"
@@ -64,6 +65,11 @@ std::vector<LandmarkId> chooseFarLmIds(size_t max_num, const std::vector<Landmar
         for (const auto& kf : keyframes) n += kf.second->hasMeasurement(id) ? 1u : 0u;
         seen[id] = n;
     }
+    return chooseFarLmIds(max_num, ids_far, seen);
+}
+
+std::vector<LandmarkId> chooseFarLmIds(size_t max_num, const std::vector<LandmarkId>& ids_far,
+                                       const std::map<LandmarkId, unsigned int>& seen) {
     std::vector<LandmarkId> out(std::min(max_num, ids_far.size()));
     std::partial_sort_copy(ids_far.cbegin(), ids_far.cend(), out.begin(), out.end(),
                            [&](const LandmarkId& a, const LandmarkId& b) { return seen.at(a) > seen.at(b); });
@@ -232,10 +238,22 @@ std::map<LandmarkId, LandmarkCategorizatonInterface::Category> LandmarkSparsific
     for (const auto& p : near_pts) ids_near.push_back(lut.at(p.label));
     for (const auto& l : labels_middle) ids_middle.push_back(lut.at(l));
     for (const auto& l : labels_far) ids_far.push_back(lut.at(l));
-    const auto flow = landmark_helpers::calcFlow(ids_near, keyframes, false);
+    std::map<LandmarkId, unsigned int> seen;  // keyframes observing each far landmark (chooseFarLmIds)
+    for (const auto& id : ids_far) {
+        unsigned int n = 0;
+        for (const auto& kf : keyframes) n += kf.second->hasMeasurement(id) ? 1u : 0u;
+        seen[id] = n;
+    }
+    return rankBins(ids_near, landmark_helpers::calcFlow(ids_near, keyframes, false), ids_middle, ids_far, seen);
+}
+
+std::map<LandmarkId, LandmarkCategorizatonInterface::Category> LandmarkSparsificationSchemeVoxel::rankBins(
+    const std::vector<LandmarkId>& ids_near, const std::map<LandmarkId, double>& flow, const std::vector<LandmarkId>& ids_middle,
+    const std::vector<LandmarkId>& ids_far, const std::map<LandmarkId, unsigned int>& seen) const {
+    std::map<LandmarkId, Category> out;
     for (const auto& id : landmark_helpers::chooseNearLmIds(params_.max_num_landmarks_near, ids_near, flow)) out[id] = Category::NearField;
     for (const auto& id : landmark_helpers::chooseMiddleLmIds(params_.max_num_landmarks_middle, ids_middle)) out[id] = Category::MiddleField;
-    for (const auto& id : landmark_helpers::chooseFarLmIds(params_.max_num_landmarks_far, ids_far, keyframes)) out[id] = Category::FarField;
+    for (const auto& id : landmark_helpers::chooseFarLmIds(params_.max_num_landmarks_far, ids_far, seen)) out[id] = Category::FarField;
     return out;
 }
 
@@ -285,26 +303,75 @@ void LandmarkSelector::clean(TimestampNSec oldest_ts) {
     }
 }
 
+const LandmarkSparsificationSchemeVoxel* LandmarkSelector::quantitiesChainVoxel() const {
+    if (rejection_schemes_.size() != 1 || sparsification_schemes_.size() != 1) return nullptr;
+    if (!dynamic_cast<const LandmarkRejectionSchemeCheirality*>(rejection_schemes_[0].get())) return nullptr;
+    return dynamic_cast<const LandmarkSparsificationSchemeVoxel*>(sparsification_schemes_[0].get());
+}
+
 std::set<LandmarkId> LandmarkSelector::select(const std::map<LandmarkId, Landmark::ConstPtr>& landmarks,
                                               const std::map<KeyframeId, Keyframe::ConstPtr>& kfs) {
+    return selectImpl(landmarks, kfs, nullptr);
+}
+
+std::set<LandmarkId> LandmarkSelector::select(const std::map<LandmarkId, Landmark::ConstPtr>& landmarks,
+                                              const std::map<KeyframeId, Keyframe::ConstPtr>& kfs, const ChainQuantities& q) {
+    return selectImpl(landmarks, kfs, &q);
+}
+
+std::set<LandmarkId> LandmarkSelector::selectImpl(const std::map<LandmarkId, Landmark::ConstPtr>& landmarks,
+                                                  const std::map<KeyframeId, Keyframe::ConstPtr>& kfs, const ChainQuantities* q) {
     auto pick = [](const std::map<LandmarkId, Landmark::ConstPtr>& src, const std::set<LandmarkId>& ids,
                    std::map<LandmarkId, Landmark::ConstPtr>& dst) {  // addToMap: ids a scheme names but src lacks are skipped
         for (const auto& id : ids) { auto it = src.find(id); if (it != src.cend()) dst[id] = it->second; }
     };
     std::map<LandmarkId, Landmark::ConstPtr> non_rejected = landmarks;
     for (const auto& id : outlier_ids_) non_rejected.erase(id);
-    for (const auto& scheme : rejection_schemes_) {
-        const auto cur = runScheme(*scheme, non_rejected, kfs);
-        non_rejected.clear();
-        pick(landmarks, cur, non_rejected);
+    const LandmarkSparsificationSchemeVoxel* voxel = q ? quantitiesChainVoxel() : nullptr;
+    if (q) {  // the cheirality scheme's verdicts
+        if (!voxel) throw std::invalid_argument("LandmarkSelector::select: the chain is not cheirality + voxel (+ selection schemes)");
+        const size_t n = q->candidates.size();
+        if (n != non_rejected.size() || q->cheiral.size() != n || q->bin.size() != n || q->flow.size() != n || q->seen.size() != n ||
+            q->near_order.size() > n)
+            throw std::invalid_argument("LandmarkSelector::select: the quantities do not cover the candidates");
+        size_t c = 0;
+        for (auto it = non_rejected.begin(); it != non_rejected.end(); ++c) {
+            if (it->first != q->candidates[c]) throw std::invalid_argument("LandmarkSelector::select: candidates differ from the landmarks");
+            it = q->cheiral[c] ? std::next(it) : non_rejected.erase(it);
+        }
+    } else {
+        for (const auto& scheme : rejection_schemes_) {
+            const auto cur = runScheme(*scheme, non_rejected, kfs);
+            non_rejected.clear();
+            pick(landmarks, cur, non_rejected);
+        }
     }
     std::map<LandmarkId, Landmark::ConstPtr> selected;
     for (const auto& scheme : selection_schemes_) pick(non_rejected, runScheme(*scheme, non_rejected, kfs), selected);
     std::map<LandmarkId, Landmark::ConstPtr> sparsified = non_rejected;
-    for (const auto& scheme : sparsification_schemes_) {
-        const auto cur = runScheme(*scheme, sparsified, kfs);
+    if (q) {  // the voxel scheme's ranking over the bins the quantities describe (getCategorizedSelection's step 6)
+        std::vector<LandmarkId> ids_near, ids_middle, ids_far;
+        std::map<LandmarkId, double> flow;
+        std::map<LandmarkId, unsigned int> seen;
+        for (const int32_t c : q->near_order) {
+            ids_near.push_back(q->candidates.at(c));
+            if (!std::isnan(q->flow[c])) flow[q->candidates[c]] = q->flow[c];
+        }
+        for (size_t c = 0; c < q->candidates.size(); ++c) {
+            if (q->bin[c] == 1) ids_middle.push_back(q->candidates[c]);
+            if (q->bin[c] == 2) { ids_far.push_back(q->candidates[c]); seen[q->candidates[c]] = (unsigned int)q->seen[c]; }
+        }
+        landmark_categories_ = voxel->rankBins(ids_near, flow, ids_middle, ids_far, seen);
         sparsified.clear();
+        std::set<LandmarkId> cur;
+        for (const auto& el : landmark_categories_) cur.insert(el.first);
         pick(non_rejected, cur, sparsified);
+    } else {
+        for (const auto& scheme : sparsification_schemes_) {
+            const auto cur = runScheme(*scheme, sparsified, kfs);
+            sparsified.clear();
+            pick(non_rejected, cur, sparsified);
+        }
     }
     for (const auto& el : selected) sparsified[el.first] = el.second;
     std::set<LandmarkId> selection;

@@ -3,6 +3,7 @@
 #include <algorithm>
 #include <atomic>
 #include <chrono>
+#include <cmath>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -232,6 +233,27 @@ struct TrackSolver {
     }
 };
 
+// buffers of kba_track_select_landmarks (kba_select.cu): allocated at the first call for the track's capacities, then reused: a call
+// makes one upload (the lists), one launch sequence and one download (the outputs)
+struct SelectBufs {
+    Staged<int> up;                        // keyframe slots | candidate slots
+    Staged<unsigned char> out;             // flow | seen | near order | counters | cheirality | bins, laid out per call
+    SelectArgs a;                          // the scratch pointers; lists and outputs are set per call
+    std::vector<void*> dev;
+    std::vector<unsigned> kf_stamp, lm_stamp;  // duplicate checks: the call that named a slot last
+    unsigned stamp = 0;
+    TrackSolver counts;                    // only h2d / d2h: what kba_track_transfer_bytes reports after a selection
+    template <typename T> int alloc(T** p, size_t n) {
+        void* q = nullptr;
+        if (cudaMalloc(&q, std::max<size_t>(n, 1) * sizeof(T)) != cudaSuccess) return 1;
+        dev.push_back(q); *p = (T*)q; return 0;
+    }
+    ~SelectBufs() {
+        up.release(); out.release();
+        for (void* p : dev) cudaFree(p);
+    }
+};
+
 // persistent, device-resident window (kba_track_*, at the end of this file)
 struct kba_track {
     kba_handle* h = nullptr;
@@ -240,6 +262,7 @@ struct kba_track {
     TrackSolver solver;                    // window 0 of its batch is this track's window (fused path)
     TrackSolver large;                     // win_rows > kFusedMaxRows: the same for windows of more rows, else no batch
     const TrackSolver* last = &solver;     // the solver of the last solve or pose-only call (transfer counts)
+    std::unique_ptr<SelectBufs> select;    // kba_track_select_landmarks, allocated at its first call
     TrackDev td{};
     int* arena_i[2][2] = {{nullptr, nullptr}, {nullptr, nullptr}};      // [buffer][lm, cam]
     float* arena_f[2][3] = {{nullptr, nullptr, nullptr}, {nullptr, nullptr, nullptr}};  // [buffer][u, v, d]
@@ -1360,6 +1383,7 @@ void kba_track_destroy(kba_track* t) {
     cudaStreamSynchronize(t->h->stream);
     t->solver.release();
     t->large.release();
+    t->select.reset();
     for (void* p : t->dev) cudaFree(p);
     t->p_lm.release(); t->p_cam.release(); t->lay.release();
     t->p_u.release(); t->p_v.release(); t->p_d.release(); t->p_dbl.release(); t->p_slot.release();
@@ -1808,6 +1832,95 @@ int kba_track_transfer_bytes(kba_track* t, int64_t* h2d, int64_t* d2h, int64_t* 
     if (h2d) *h2d = t->last->h2d;
     if (d2h) *d2h = t->last->d2h;
     if (push) *push = t->h2d_push;
+    return KBA_OK;
+}
+
+// ---------------------------------------------------------------------------------------------------------------------
+// landmark selection on the stored window (include/kba_b200.h, kba_track_select_landmarks; kernels in kba_select.cu)
+// ---------------------------------------------------------------------------------------------------------------------
+static int select_alloc(kba_track* t) {
+    std::unique_ptr<SelectBufs> sb(new SelectBufs());
+    const TrackDev& td = t->td;
+    const size_t L = (size_t)td.lm_cap, K = (size_t)td.kf_cap;
+    SelectArgs& a = sb->a;
+    double* cams = nullptr;
+    int bad = 0;
+    bad |= sb->up.alloc(K + L, true);
+    bad |= sb->out.alloc(L * 18 + 64, true);
+    bad |= sb->alloc(&a.cand_of, L); bad |= sb->alloc(&a.kf_T, 12 * K); bad |= sb->alloc(&a.cam_T, 12 * (size_t)kMaxCam);
+    bad |= sb->alloc(&a.path, 3 * K); bad |= sb->alloc(&a.pt, 3 * L); bad |= sb->alloc(&a.cnt, L); bad |= sb->alloc(&a.cursor, L);
+    bad |= sb->alloc(&a.obs_off, L); bad |= sb->alloc(&a.in_list, L); bad |= sb->alloc(&a.vkey, L); bad |= sb->alloc(&a.sorted, L);
+    bad |= sb->alloc(&a.near_flag, L); bad |= sb->alloc(&a.okey, (size_t)td.m_cap); bad |= sb->alloc(&a.bounds, 6);
+    bad |= sb->alloc(&cams, 7 * (size_t)t->n_cam);
+    if (bad) return fail(KBA_ERR_CUDA, "kba_track_select_landmarks: out of memory");
+    cudaStream_t s = t->h->stream;
+    CU(cudaMemsetAsync(a.cand_of, 0xff, sizeof(int) * L, s));
+    CU(cudaMemcpyAsync(cams, t->cam_pose.data(), sizeof(double) * 7 * (size_t)t->n_cam, cudaMemcpyHostToDevice, s));
+    CU(cudaStreamSynchronize(s));
+    a.cam_pose7 = cams; a.n_cam = t->n_cam;
+    sb->kf_stamp.assign(K, 0); sb->lm_stamp.assign(L, 0);
+    t->select = std::move(sb);
+    return KBA_OK;
+}
+
+int kba_track_select_landmarks(kba_track* t, int32_t n_kf, const int32_t* kf_slot, int32_t n_cand, const int32_t* lm_slot,
+                               const kba_select_params* p, kba_select_out* o) {
+    static const char* who = "kba_track_select_landmarks: ";
+    if (!t || !kf_slot || !p || !o || (n_cand > 0 && !lm_slot) || !o->cheiral || !o->bin || !o->near_order || !o->n_near || !o->flow || !o->seen)
+        return fail(KBA_ERR_BAD_ARG, std::string(who) + "null argument");
+    if (n_kf < 1 || n_cand < 0) return fail(KBA_ERR_BAD_ARG, std::string(who) + "no keyframes or a negative size");
+    if (n_kf > t->td.kf_cap || n_cand > t->td.lm_cap) return fail(KBA_ERR_CAPACITY, std::string(who) + "more keyframes or candidates than the track's slots");
+    for (int q = 0; q < 3; ++q)
+        if (!(p->voxel_size[q] > 0.0) || !std::isfinite(p->voxel_size[q])) return fail(KBA_ERR_BAD_ARG, std::string(who) + "voxel sizes must be finite and positive");
+    CU(cudaSetDevice(t->h->device));
+    if (!t->select) { const int rc = select_alloc(t); if (rc != KBA_OK) return rc; }
+    SelectBufs& sb = *t->select;
+    if (++sb.stamp == 0) {  // the stamps wrapped: start over
+        std::fill(sb.kf_stamp.begin(), sb.kf_stamp.end(), 0u); std::fill(sb.lm_stamp.begin(), sb.lm_stamp.end(), 0u); sb.stamp = 1;
+    }
+    int max_meas = 0;
+    for (int k = 0; k < n_kf; ++k) {
+        const int s = kf_slot[k];
+        if (s < 0 || s >= t->td.kf_cap || !t->kf_live[s]) return fail(KBA_ERR_BAD_ARG, std::string(who) + "keyframe slot not pushed");
+        if (sb.kf_stamp[s] == sb.stamp) return fail(KBA_ERR_BAD_ARG, std::string(who) + "keyframe slot listed twice");
+        sb.kf_stamp[s] = sb.stamp;
+        max_meas = std::max(max_meas, t->m_cnt[s]);
+    }
+    for (int c = 0; c < n_cand; ++c) {
+        const int s = lm_slot[c];
+        if (s < 0 || s >= t->td.lm_cap) return fail(KBA_ERR_BAD_ARG, std::string(who) + "landmark slot out of range");
+        if (sb.lm_stamp[s] == sb.stamp) return fail(KBA_ERR_BAD_ARG, std::string(who) + "landmark slot listed twice");
+        sb.lm_stamp[s] = sb.stamp;
+    }
+    // ---- one upload: the lists
+    cudaStream_t s = t->h->stream;
+    memcpy(sb.up.h, kf_slot, sizeof(int) * (size_t)n_kf);
+    if (n_cand) memcpy(sb.up.h + n_kf, lm_slot, sizeof(int) * (size_t)n_cand);
+    CU(cudaMemcpyAsync(sb.up.d, sb.up.h, sizeof(int) * ((size_t)n_kf + n_cand), cudaMemcpyHostToDevice, s));
+    // ---- outputs laid out for this call: flow | seen | near order | counters | cheirality | bins
+    const size_t n = (size_t)n_cand;
+    const size_t o_seen = 8 * n, o_near = o_seen + 4 * n, o_cnt = o_near + 4 * n, o_ch = o_cnt + 16, o_bin = o_ch + n, bytes = o_bin + n;
+    SelectArgs a = sb.a;
+    a.td = t->td;
+    a.kf_slot = sb.up.d; a.lm_slot = sb.up.d + n_kf; a.n_kf = n_kf; a.n_cand = n_cand;
+    for (int q = 0; q < 3; ++q) a.leaf[q] = p->voxel_size[q];
+    a.roi_far = p->roi_far; a.roi_middle = p->roi_middle;
+    unsigned char* d = sb.out.d;
+    a.flow = reinterpret_cast<double*>(d); a.seen = reinterpret_cast<int*>(d + o_seen); a.near_order = reinterpret_cast<int*>(d + o_near);
+    a.counters = reinterpret_cast<int*>(d + o_cnt); a.n_near = a.counters + 1;
+    a.cheiral = d + o_ch; a.bin = reinterpret_cast<signed char*>(d + o_bin);
+    launch_select(a, max_meas, s);
+    CU(cudaGetLastError());
+    // ---- one download
+    CU(cudaMemcpyAsync(sb.out.h, sb.out.d, bytes, cudaMemcpyDeviceToHost, s));
+    CU(wait_stream(t->h));
+    const unsigned char* h = sb.out.h;
+    memcpy(o->flow, h, 8 * n); memcpy(o->seen, h + o_seen, 4 * n); memcpy(o->near_order, h + o_near, 4 * n);
+    memcpy(o->n_near, h + o_cnt + 4, 4);
+    memcpy(o->cheiral, h + o_ch, n); memcpy(o->bin, h + o_bin, n);
+    sb.counts.h2d = 4 * ((int64_t)n_kf + n_cand);
+    sb.counts.d2h = (int64_t)bytes;
+    t->last = &sb.counts;
     return KBA_OK;
 }
 

@@ -105,6 +105,42 @@ void launch_scatter_rows(double* dst, const int* slot, const double* src, int n,
 // results of every window w back into track store tds[w]
 void launch_track_writeback(const BatchDev& bd, const TrackDev* tds, const TrackSel* sels, const TrackGrid& g, cudaStream_t s);
 
+// ---- landmark selection on a track's store (kba_track_select_landmarks, kba_select.cu) ----
+// One request: active keyframe slots (ascending timestamp), candidate landmark slots (ascending id).  Scratch is sized for the
+// track's capacities at the first call; the outputs point into one device block that goes down in one copy.
+struct SelectArgs {
+    TrackDev td;
+    const int* kf_slot = nullptr;   // [n_kf]
+    const int* lm_slot = nullptr;   // [n_cand]
+    const double* cam_pose7 = nullptr;  // [n_cam * 7] the track's cameras
+    int n_kf = 0, n_cand = 0, n_cam = 0;
+    double leaf[3] = {0., 0., 0.}, roi_far = 0., roi_middle = 0.;
+    // scratch
+    int* cand_of = nullptr;         // [lm_cap] slot -> candidate, all -1 between calls
+    double* kf_T = nullptr;         // [kf_cap * 12] transforms of the listed keyframes
+    double* cam_T = nullptr;        // [kMaxCam * 12]
+    double* path = nullptr;         // [kf_cap * 3] keyframe positions seen from the newest keyframe
+    float* pt = nullptr;            // [lm_cap * 3] cloud points by candidate
+    int* cnt = nullptr;             // [lm_cap] arena entries per candidate
+    int* cursor = nullptr;          // [lm_cap]
+    int* obs_off = nullptr;         // [lm_cap] first key of a near candidate's observations
+    int* in_list = nullptr;         // [lm_cap] cloud points (candidate indices), in arrival order
+    long long* vkey = nullptr;      // [lm_cap] voxel index by cloud position
+    int* sorted = nullptr;          // [lm_cap] cloud positions in (voxel index, label) order
+    int* near_flag = nullptr;       // [lm_cap] by sorted position: a near voxel starts here
+    long long* okey = nullptr;      // [m_cap] (keyframe position, arena index) of the near candidates' observations
+    unsigned* bounds = nullptr;     // [6] order-preserving min xyz, max xyz of the cloud
+    int* counters = nullptr;        // [3] cloud points, near voxels, gathered observations
+    // outputs [n_cand]
+    unsigned char* cheiral = nullptr;
+    signed char* bin = nullptr;
+    int* near_order = nullptr;
+    int* n_near = nullptr;          // = counters + 1
+    double* flow = nullptr;
+    int* seen = nullptr;
+};
+void launch_select(const SelectArgs& a, int max_meas, cudaStream_t s);
+
 // ---- motion-only frames against a track's store (kba_track_adjust_pose / kba_track_group_adjust_pose, kba_motion.cu) ----
 // One frame = one free pose against constant landmarks read from a store by slot: its measurements come in runs, one run per
 // landmark (the landmarks of the equivalent window, in the caller's order).
