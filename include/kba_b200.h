@@ -373,7 +373,8 @@ int kba_track_transfer_bytes(kba_track* t, int64_t* h2d_last_solve, int64_t* d2h
  *   - seen[c] (every candidate): how many listed keyframes measure it (chooseFarLmIds).
  * Every float operation is the host code's, in its order, without contraction: the quantities equal the host's bit for bit.
  * One upload (the lists), one launch sequence, one download; the first call allocates the buffers for the track's capacities,
- * later calls allocate nothing.  kba_track_transfer_bytes then reports this call's upload and download.
+ * later calls allocate nothing.  kba_track_transfer_bytes then reports this call's upload and download: 4 * (n_kf + n_cand)
+ * and 18 * n_cand + 16 bytes.  kba_track_group_select_landmarks (below) selects for every track of a group at once.
  * Errors, before anything is uploaded: a null pointer, n_kf < 1, a slot out of range or listed twice, a keyframe slot not pushed,
  * a voxel size that is not finite and positive: KBA_ERR_BAD_ARG; more keyframes or candidates than the track has slots:
  * KBA_ERR_CAPACITY. */
@@ -430,8 +431,41 @@ int kba_track_group_create(kba_handle* h, int32_t n_tracks, kba_track* const* tr
 void kba_track_group_destroy(kba_track_group* g);
 /* req[n_tracks], res[n_tracks] */
 int kba_track_group_solve(kba_track_group* g, const kba_track_request* req, const kba_options* opt, kba_result* res);
-/* upload / download of the last group solve, counted as kba_track_transfer_bytes counts them */
+/* upload / download of the last group solve, pose-only call or selection, counted as kba_track_transfer_bytes counts them */
 int kba_track_group_transfer_bytes(kba_track_group* g, int64_t* h2d_last_solve, int64_t* d2h_last_solve);
+
+/* ---- landmark selection for every track of a group in one launch sequence -------------------------------------------------
+ * kba_track_select_landmarks for one request per track, each on its own track's store, as one window each of one launch sequence.
+ *   - Results: out[i] holds exactly what kba_track_select_landmarks(tracks[i], ...) writes for the same request, bit for bit:
+ *     cheiral, bin, near_order, *n_near, flow (NaN in the same places) and seen.  A single call is a one-request group call of
+ *     the same host code and kernels.
+ *   - Sitting out: a request with n_kf == 0 leaves out[i]'s arrays unwritten and sets *out[i].n_near = 0 (n_near must not be
+ *     NULL).  A call in which every request sits out returns at once: no upload, no launch.
+ *   - Validation: every other request is checked as kba_track_select_landmarks checks its arguments (n_kf < 0 is KBA_ERR_BAD_ARG)
+ *     before anything is uploaded.  If one fails, the call returns that request's code, kba_last_error names the track index,
+ *     and no out[i] is written.
+ *   - Transfers: one upload (every request's lists and the argument records of the windows), one launch sequence, one download
+ *     and one synchronisation per call.  Over the W requests that do not sit out, kba_track_group_transfer_bytes then reports
+ *         h2d = 4 * sum(n_kf + n_cand) + R * (W - 1)
+ *         d2h = 18 * sum(n_cand) + 16 * W
+ *     where R is the size of one window's argument record, a constant of the library build that the header does not fix
+ *     (the first window's record travels in the launch parameters).  With W = 1 these are kba_track_transfer_bytes' counts
+ *     after a single selection, and 0 / 0 when every request sits out.
+ *   - Memory: each member track's selection scratch (allocated at the first selection of that track by either entry point,
+ *     for the track's capacities) is used by both entry points, and the staging of kba_track_select_landmarks is allocated at
+ *     the track's first single call only; calls are serial on the handle's stream, so a track may
+ *     still be selected alone between group calls.  The group adds only its staging for the lists, the argument records and
+ *     the outputs (pinned and device, sized for its tracks' capacities), allocated at its first call in which some request
+ *     does not sit out. */
+typedef struct kba_select_request {
+    int32_t n_kf;                     /* 0: this track sits the call out; < 0: KBA_ERR_BAD_ARG                         */
+    int32_t n_cand;
+    const int32_t* kf_slot;           /* [n_kf]   as for kba_track_select_landmarks                                  */
+    const int32_t* lm_slot;           /* [n_cand] as for kba_track_select_landmarks                                  */
+    const kba_select_params* params;  /* per request, so that a sweep can vary the voxel size and ROIs per track       */
+} kba_select_request;
+/* req[n_tracks], out[n_tracks] */
+int kba_track_group_select_landmarks(kba_track_group* g, const kba_select_request* req, kba_select_out* out);
 
 /* ---- adjustPoseOnly against the persistent store: one frame's pose per call, or one frame of each track of a group -------
  * What limo calls on every frame (bundle_adjuster_keyframes.cpp:820-888): one free pose against constant landmarks, the optional

@@ -4,12 +4,13 @@ The product path: there is no CPU fallback.  Importing works without a GPU (symb
 computing call fails with KBA_ERR_CUDA when no sm_90 (H100) device is present.
 """
 import ctypes as C
+import functools
 import os
 
 import numpy as np
 
-from .capi_types import (KbaCounters, KbaEvalOut, KbaLidarOptions, KbaOptions, KbaResult, KbaSelectOut, KbaSelectParams, KbaTrackCaps,
-                         KbaTrackFrame, KbaTrackRequest, KbaWindow, Result, Window, c_double_p, c_int32_p)
+from .capi_types import (KbaCounters, KbaEvalOut, KbaLidarOptions, KbaOptions, KbaResult, KbaSelectOut, KbaSelectParams, KbaSelectRequest,
+                         KbaTrackCaps, KbaTrackFrame, KbaTrackRequest, KbaWindow, Result, Window, c_double_p, c_int32_p)
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("KBA_LIB_PATH") or os.path.join(_HERE, "libkba_b200.so")  # KBA_LIB_PATH: instrumented builds
@@ -24,11 +25,23 @@ SYMBOLS = ["kba_version", "kba_last_error", "kba_default_options", "kba_create",
            "kba_init_landmarks", "kba_track_create", "kba_track_destroy", "kba_track_push_keyframe", "kba_track_drop_keyframe",
            "kba_track_set_landmarks", "kba_track_set_keyframe_pose", "kba_track_set_keyframe_poses", "kba_track_solve", "kba_track_transfer_bytes",
            "kba_track_group_create", "kba_track_group_destroy", "kba_track_group_solve", "kba_track_group_transfer_bytes",
-           "kba_track_adjust_pose", "kba_track_group_adjust_pose", "kba_track_select_landmarks"]
+           "kba_track_adjust_pose", "kba_track_group_adjust_pose", "kba_track_select_landmarks", "kba_track_group_select_landmarks"]
 
 
 class KbaError(RuntimeError):
     pass
+
+
+# LandmarkSparsificationSchemeVoxel::Parameters' values: the defaults of a selection request
+SELECT_DEFAULTS = dict(voxel_size=(1.0, 1.0, 0.5), roi_far=50.0, roi_middle=25.0)
+
+
+@functools.lru_cache(maxsize=None)
+def _records(struct):
+    """numpy dtype with the layout of a ctypes mirror, pointers as addresses: arrays of structs filled by numpy"""
+    fmt = lambda t: np.uint64 if issubclass(t, (C._Pointer, C.c_void_p)) else np.dtype(t)  # noqa: E731
+    return np.dtype(dict(names=[f for f, _ in struct._fields_], formats=[fmt(t) for _, t in struct._fields_],
+                         offsets=[getattr(struct, f).offset for f, _ in struct._fields_], itemsize=C.sizeof(struct)))
 
 
 def lib():
@@ -86,6 +99,7 @@ def lib():
         L.kba_track_adjust_pose.argtypes = [vp, C.POINTER(KbaTrackFrame), C.POINTER(KbaOptions), C.POINTER(KbaResult)]
         L.kba_track_group_adjust_pose.argtypes = [vp, C.POINTER(KbaTrackFrame), C.POINTER(KbaOptions), C.POINTER(KbaResult)]
         L.kba_track_select_landmarks.argtypes = [vp, C.c_int32, ip, C.c_int32, ip, C.POINTER(KbaSelectParams), C.POINTER(KbaSelectOut)]
+        L.kba_track_group_select_landmarks.argtypes = [vp, C.POINTER(KbaSelectRequest), C.POINTER(KbaSelectOut)]
         L.kba_lidar_default_options.argtypes = [C.POINTER(KbaLidarOptions)]
         L.kba_lidar_default_options.restype = None
         fp = C.POINTER(C.c_float)
@@ -277,7 +291,8 @@ class Track:
         _check(lib().kba_track_adjust_pose(self._p, C.byref(fr), C.byref(opt or default_options()), C.byref(res.c)))
         return res
 
-    def select_landmarks(self, kf_slots, lm_slots, voxel_size=(1.0, 1.0, 0.5), roi_far=50.0, roi_middle=25.0):
+    def select_landmarks(self, kf_slots, lm_slots, voxel_size=SELECT_DEFAULTS["voxel_size"], roi_far=SELECT_DEFAULTS["roi_far"],
+                         roi_middle=SELECT_DEFAULTS["roi_middle"]):
         """per-landmark quantities of limo's selection chain on this track's store (kba_track_select_landmarks).
         kf_slots: active keyframes in ascending timestamp order; lm_slots: candidates in ascending landmark id order.  The
         defaults are LandmarkSparsificationSchemeVoxel::Parameters'.  Returns a dict of numpy arrays over the candidates:
@@ -363,8 +378,54 @@ class TrackGroup:
             r.c = c
         return results
 
+    def select_landmarks(self, requests):
+        """the selection quantities of every track in one launch sequence (kba_track_group_select_landmarks): each entry None
+        (the track sits the call out) or a dict with the arguments of Track.select_landmarks (kf_slots, lm_slots, voxel_size,
+        roi_far, roi_middle).  Returns one dict per track as Track.select_landmarks returns it (its arrays are views of buffers
+        shared by the call), None for a track that sat out."""
+        assert len(requests) == len(self.tracks)
+        n = len(requests)
+        act = [i for i, r in enumerate(requests) if r is not None]
+        prm = np.empty((len(act), 5), np.float64)  # kba_select_params of each request: voxel size xyz, roi_far, roi_middle
+        for q, i in enumerate(act):
+            r = requests[i]
+            extra = set(r) - {"kf_slots", "lm_slots", *SELECT_DEFAULTS}
+            if extra:
+                raise TypeError("select_landmarks: request %d has unexpected keys %s" % (i, sorted(extra)))
+            vs = np.asarray(r.get("voxel_size", SELECT_DEFAULTS["voxel_size"]), np.float64)
+            if vs.shape != (3,):
+                raise ValueError("select_landmarks: request %d: voxel_size must have 3 entries" % i)
+            prm[q] = (*vs, r.get("roi_far", SELECT_DEFAULTS["roi_far"]), r.get("roi_middle", SELECT_DEFAULTS["roi_middle"]))
+        # the request and output structs as numpy records, filled without a ctypes object per track
+        kfs = [np.ascontiguousarray(requests[i]["kf_slots"], dtype=np.int32).ravel() for i in act]
+        lms = [np.ascontiguousarray(requests[i]["lm_slots"], dtype=np.int32).ravel() for i in act]
+        for q, i in enumerate(act):
+            if len(kfs[q]) == 0:  # n_kf = 0 would sit the track out: a request without keyframes is an error, as for one track
+                raise KbaError("kba_track_group_select_landmarks: track %d: no keyframes or a negative size" % i)
+        nk, nc = np.array([len(a) for a in kfs], np.int64), np.array([len(a) for a in lms], np.int64)
+        lists = np.concatenate(kfs + lms + [np.zeros(1, np.int32)])
+        co = np.concatenate(([0], np.cumsum(nc)))
+        N = int(co[-1])
+        cheiral, bins, near = np.empty(N + 1, np.uint8), np.empty(N + 1, np.int8), np.empty(N + 1, np.int32)
+        flow, seen, n_near = np.empty(N + 1, np.float64), np.empty(N + 1, np.int32), np.zeros(n, np.int32)
+        req, out = np.zeros(n, _records(KbaSelectRequest)), np.zeros(n, _records(KbaSelectOut))
+        req["n_kf"][act], req["n_cand"][act] = nk, nc
+        req["kf_slot"][act] = lists.ctypes.data + 4 * np.concatenate(([0], np.cumsum(nk)[:-1]))
+        req["lm_slot"][act] = lists.ctypes.data + 4 * (nk.sum() + co[:-1])
+        req["params"][act] = prm.ctypes.data + C.sizeof(KbaSelectParams) * np.arange(len(act))
+        out["n_near"] = n_near.ctypes.data + 4 * np.arange(n)
+        for name, a in (("cheiral", cheiral), ("bin", bins), ("near_order", near), ("flow", flow), ("seen", seen)):
+            out[name][act] = a.ctypes.data + a.itemsize * co[:-1]
+        _check(lib().kba_track_group_select_landmarks(self._p, req.ctypes.data_as(C.POINTER(KbaSelectRequest)),
+                                                      out.ctypes.data_as(C.POINTER(KbaSelectOut))))
+        results = [None] * n
+        for q, i in enumerate(act):
+            a, b = int(co[q]), int(co[q + 1])
+            results[i] = dict(cheiral=cheiral[a:b], bin=bins[a:b], near_order=near[a:a + int(n_near[i])], flow=flow[a:b], seen=seen[a:b])
+        return results
+
     def transfer_bytes(self):
-        """(host->device bytes, device->host bytes) of the last group solve"""
+        """(host->device bytes, device->host bytes) of the last group solve, pose-only call or selection"""
         a, b = C.c_int64(), C.c_int64()
         _check(lib().kba_track_group_transfer_bytes(self._p, C.byref(a), C.byref(b)))
         return a.value, b.value

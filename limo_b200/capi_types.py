@@ -51,6 +51,11 @@ class KbaSelectOut(C.Structure):
                 ("flow", c_double_p), ("seen", c_int32_p)]
 
 
+class KbaSelectRequest(C.Structure):
+    _fields_ = [("n_kf", C.c_int32), ("n_cand", C.c_int32), ("kf_slot", c_int32_p), ("lm_slot", c_int32_p),
+                ("params", C.POINTER(KbaSelectParams))]
+
+
 class KbaTrackFrame(C.Structure):
     _fields_ = [("n_meas", C.c_int32), ("reserved_", C.c_int32), ("pose7", c_double_p), ("lm_slot", c_int32_p), ("cam", c_int32_p),
                 ("u", c_float_p), ("v", c_float_p), ("d", c_float_p), ("speed_weight", C.c_double), ("speed_dt", C.c_double),

@@ -233,23 +233,30 @@ struct TrackSolver {
     }
 };
 
-// buffers of kba_track_select_landmarks (kba_select.cu): allocated at the first call for the track's capacities, then reused: a call
-// makes one upload (the lists), one launch sequence and one download (the outputs)
+// staging of a selection call (select_run): one pinned upload, argument records of windows 1 .. W-1 | the windows' lists, and one
+// download, the windows' outputs: flow | seen | near order (all windows' candidates end to end) | counters [W] | cheirality | bins
+struct SelectStage {
+    Staged<unsigned char> up, out;
+    TrackSolver counts;                    // only h2d / d2h: what the transfer-bytes calls report after a selection
+    int alloc(size_t up_bytes, size_t out_bytes) { return up.alloc(up_bytes, true) | out.alloc(out_bytes, true); }
+    ~SelectStage() { up.release(); out.release(); }
+};
+
+// buffers of a track's selections (kba_select.cu): the scratch is allocated at its first selection, alone or in a group, for the
+// track's capacities, then reused by both entry points (calls are serial on the handle's stream).  The staging serves only
+// kba_track_select_landmarks and is allocated at its first call (a group stages its calls in its own)
 struct SelectBufs {
-    Staged<int> up;                        // keyframe slots | candidate slots
-    Staged<unsigned char> out;             // flow | seen | near order | counters | cheirality | bins, laid out per call
+    SelectStage stage;                     // kba_track_select_landmarks: keyframe slots | candidate slots, one window's outputs
     SelectArgs a;                          // the scratch pointers; lists and outputs are set per call
     std::vector<void*> dev;
     std::vector<unsigned> kf_stamp, lm_stamp;  // duplicate checks: the call that named a slot last
     unsigned stamp = 0;
-    TrackSolver counts;                    // only h2d / d2h: what kba_track_transfer_bytes reports after a selection
     template <typename T> int alloc(T** p, size_t n) {
         void* q = nullptr;
         if (cudaMalloc(&q, std::max<size_t>(n, 1) * sizeof(T)) != cudaSuccess) return 1;
         dev.push_back(q); *p = (T*)q; return 0;
     }
     ~SelectBufs() {
-        up.release(); out.release();
         for (void* p : dev) cudaFree(p);
     }
 };
@@ -294,6 +301,7 @@ struct kba_track_group {
     std::vector<kba_track*> tracks;
     TrackSolver solver;                    // window i of its batch is track i's (fused path)
     TrackSolver large;                     // some track has win_rows > kFusedMaxRows: the whole group on the large-window path, else no batch
+    std::unique_ptr<SelectStage> select;   // kba_track_group_select_landmarks, allocated at its first call
     const TrackSolver* last = &solver;
 };
 
@@ -1836,92 +1844,167 @@ int kba_track_transfer_bytes(kba_track* t, int64_t* h2d, int64_t* d2h, int64_t* 
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
-// landmark selection on the stored window (include/kba_b200.h, kba_track_select_landmarks; kernels in kba_select.cu)
+// landmark selection on the stored window (include/kba_b200.h, kba_track_select_landmarks / kba_track_group_select_landmarks;
+// kernels in kba_select.cu): a single call is a one-window call of select_run, as a group's requests are
 // ---------------------------------------------------------------------------------------------------------------------
-static int select_alloc(kba_track* t) {
+// download of a call: 18 bytes per candidate (flow, seen, near order, cheirality, bin) and 16 per window (its counters)
+static size_t select_out_bytes(size_t cands, size_t windows) { return 18 * cands + 16 * windows; }
+
+static int select_alloc(kba_track* t, std::string& why) {
     std::unique_ptr<SelectBufs> sb(new SelectBufs());
     const TrackDev& td = t->td;
     const size_t L = (size_t)td.lm_cap, K = (size_t)td.kf_cap;
     SelectArgs& a = sb->a;
     double* cams = nullptr;
     int bad = 0;
-    bad |= sb->up.alloc(K + L, true);
-    bad |= sb->out.alloc(L * 18 + 64, true);
     bad |= sb->alloc(&a.cand_of, L); bad |= sb->alloc(&a.kf_T, 12 * K); bad |= sb->alloc(&a.cam_T, 12 * (size_t)kMaxCam);
     bad |= sb->alloc(&a.path, 3 * K); bad |= sb->alloc(&a.pt, 3 * L); bad |= sb->alloc(&a.cnt, L); bad |= sb->alloc(&a.cursor, L);
     bad |= sb->alloc(&a.obs_off, L); bad |= sb->alloc(&a.in_list, L); bad |= sb->alloc(&a.vkey, L); bad |= sb->alloc(&a.sorted, L);
     bad |= sb->alloc(&a.near_flag, L); bad |= sb->alloc(&a.okey, (size_t)td.m_cap); bad |= sb->alloc(&a.bounds, 6);
     bad |= sb->alloc(&cams, 7 * (size_t)t->n_cam);
-    if (bad) return fail(KBA_ERR_CUDA, "kba_track_select_landmarks: out of memory");
+    if (bad) { why = "out of memory for the selection buffers"; return KBA_ERR_CUDA; }
     cudaStream_t s = t->h->stream;
-    CU(cudaMemsetAsync(a.cand_of, 0xff, sizeof(int) * L, s));
-    CU(cudaMemcpyAsync(cams, t->cam_pose.data(), sizeof(double) * 7 * (size_t)t->n_cam, cudaMemcpyHostToDevice, s));
-    CU(cudaStreamSynchronize(s));
+    cudaError_t e = cudaMemsetAsync(a.cand_of, 0xff, sizeof(int) * L, s);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(cams, t->cam_pose.data(), sizeof(double) * 7 * (size_t)t->n_cam, cudaMemcpyHostToDevice, s);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(s);
+    if (e != cudaSuccess) { why = std::string("selection buffers: ") + cudaGetErrorString(e); return KBA_ERR_CUDA; }
     a.cam_pose7 = cams; a.n_cam = t->n_cam;
     sb->kf_stamp.assign(K, 0); sb->lm_stamp.assign(L, 0);
     t->select = std::move(sb);
     return KBA_OK;
 }
 
-int kba_track_select_landmarks(kba_track* t, int32_t n_kf, const int32_t* kf_slot, int32_t n_cand, const int32_t* lm_slot,
-                               const kba_select_params* p, kba_select_out* o) {
-    static const char* who = "kba_track_select_landmarks: ";
-    if (!t || !kf_slot || !p || !o || (n_cand > 0 && !lm_slot) || !o->cheiral || !o->bin || !o->near_order || !o->n_near || !o->flow || !o->seen)
-        return fail(KBA_ERR_BAD_ARG, std::string(who) + "null argument");
-    if (n_kf < 1 || n_cand < 0) return fail(KBA_ERR_BAD_ARG, std::string(who) + "no keyframes or a negative size");
-    if (n_kf > t->td.kf_cap || n_cand > t->td.lm_cap) return fail(KBA_ERR_CAPACITY, std::string(who) + "more keyframes or candidates than the track's slots");
+// one selection request of track t (one window of select_run)
+struct SelectReq {
+    kba_track* t = nullptr;
+    int n_kf = 0, n_cand = 0;
+    const int* kf_slot = nullptr;
+    const int* lm_slot = nullptr;
+    const kba_select_params* p = nullptr;
+    const kba_select_out* o = nullptr;
+    int max_meas = 0;                      // set by select_check: arena entries of the largest listed keyframe
+};
+
+// every check of one request, before anything is uploaded; allocates the track's selection buffers at its first selection
+static int select_check(SelectReq& r, std::string& why) {
+    kba_track* t = r.t;
+    const kba_select_out* o = r.o;
+    if (!r.kf_slot || !r.p || !o || (r.n_cand > 0 && !r.lm_slot) || !o->cheiral || !o->bin || !o->near_order || !o->n_near || !o->flow || !o->seen) {
+        why = "null argument"; return KBA_ERR_BAD_ARG;
+    }
+    if (r.n_kf < 1 || r.n_cand < 0) { why = "no keyframes or a negative size"; return KBA_ERR_BAD_ARG; }
+    if (r.n_kf > t->td.kf_cap || r.n_cand > t->td.lm_cap) { why = "more keyframes or candidates than the track's slots"; return KBA_ERR_CAPACITY; }
     for (int q = 0; q < 3; ++q)
-        if (!(p->voxel_size[q] > 0.0) || !std::isfinite(p->voxel_size[q])) return fail(KBA_ERR_BAD_ARG, std::string(who) + "voxel sizes must be finite and positive");
-    CU(cudaSetDevice(t->h->device));
-    if (!t->select) { const int rc = select_alloc(t); if (rc != KBA_OK) return rc; }
+        if (!(r.p->voxel_size[q] > 0.0) || !std::isfinite(r.p->voxel_size[q])) { why = "voxel sizes must be finite and positive"; return KBA_ERR_BAD_ARG; }
+    const cudaError_t e = cudaSetDevice(t->h->device);
+    if (e != cudaSuccess) { why = std::string("cudaSetDevice: ") + cudaGetErrorString(e); return KBA_ERR_CUDA; }
+    if (!t->select) { const int rc = select_alloc(t, why); if (rc != KBA_OK) return rc; }
     SelectBufs& sb = *t->select;
     if (++sb.stamp == 0) {  // the stamps wrapped: start over
         std::fill(sb.kf_stamp.begin(), sb.kf_stamp.end(), 0u); std::fill(sb.lm_stamp.begin(), sb.lm_stamp.end(), 0u); sb.stamp = 1;
     }
-    int max_meas = 0;
-    for (int k = 0; k < n_kf; ++k) {
-        const int s = kf_slot[k];
-        if (s < 0 || s >= t->td.kf_cap || !t->kf_live[s]) return fail(KBA_ERR_BAD_ARG, std::string(who) + "keyframe slot not pushed");
-        if (sb.kf_stamp[s] == sb.stamp) return fail(KBA_ERR_BAD_ARG, std::string(who) + "keyframe slot listed twice");
+    r.max_meas = 0;
+    for (int k = 0; k < r.n_kf; ++k) {
+        const int s = r.kf_slot[k];
+        if (s < 0 || s >= t->td.kf_cap || !t->kf_live[s]) { why = "keyframe slot not pushed"; return KBA_ERR_BAD_ARG; }
+        if (sb.kf_stamp[s] == sb.stamp) { why = "keyframe slot listed twice"; return KBA_ERR_BAD_ARG; }
         sb.kf_stamp[s] = sb.stamp;
-        max_meas = std::max(max_meas, t->m_cnt[s]);
+        r.max_meas = std::max(r.max_meas, t->m_cnt[s]);
     }
-    for (int c = 0; c < n_cand; ++c) {
-        const int s = lm_slot[c];
-        if (s < 0 || s >= t->td.lm_cap) return fail(KBA_ERR_BAD_ARG, std::string(who) + "landmark slot out of range");
-        if (sb.lm_stamp[s] == sb.stamp) return fail(KBA_ERR_BAD_ARG, std::string(who) + "landmark slot listed twice");
+    for (int c = 0; c < r.n_cand; ++c) {
+        const int s = r.lm_slot[c];
+        if (s < 0 || s >= t->td.lm_cap) { why = "landmark slot out of range"; return KBA_ERR_BAD_ARG; }
+        if (sb.lm_stamp[s] == sb.stamp) { why = "landmark slot listed twice"; return KBA_ERR_BAD_ARG; }
         sb.lm_stamp[s] = sb.stamp;
     }
-    // ---- one upload: the lists
-    cudaStream_t s = t->h->stream;
-    memcpy(sb.up.h, kf_slot, sizeof(int) * (size_t)n_kf);
-    if (n_cand) memcpy(sb.up.h + n_kf, lm_slot, sizeof(int) * (size_t)n_cand);
-    CU(cudaMemcpyAsync(sb.up.d, sb.up.h, sizeof(int) * ((size_t)n_kf + n_cand), cudaMemcpyHostToDevice, s));
-    // ---- outputs laid out for this call: flow | seen | near order | counters | cheirality | bins
-    const size_t n = (size_t)n_cand;
-    const size_t o_seen = 8 * n, o_near = o_seen + 4 * n, o_cnt = o_near + 4 * n, o_ch = o_cnt + 16, o_bin = o_ch + n, bytes = o_bin + n;
-    SelectArgs a = sb.a;
-    a.td = t->td;
-    a.kf_slot = sb.up.d; a.lm_slot = sb.up.d + n_kf; a.n_kf = n_kf; a.n_cand = n_cand;
-    for (int q = 0; q < 3; ++q) a.leaf[q] = p->voxel_size[q];
-    a.roi_far = p->roi_far; a.roi_middle = p->roi_middle;
-    unsigned char* d = sb.out.d;
-    a.flow = reinterpret_cast<double*>(d); a.seen = reinterpret_cast<int*>(d + o_seen); a.near_order = reinterpret_cast<int*>(d + o_near);
-    a.counters = reinterpret_cast<int*>(d + o_cnt); a.n_near = a.counters + 1;
-    a.cheiral = d + o_ch; a.bin = reinterpret_cast<signed char*>(d + o_bin);
-    launch_select(a, max_meas, s);
-    CU(cudaGetLastError());
-    // ---- one download
-    CU(cudaMemcpyAsync(sb.out.h, sb.out.d, bytes, cudaMemcpyDeviceToHost, s));
-    CU(wait_stream(t->h));
-    const unsigned char* h = sb.out.h;
-    memcpy(o->flow, h, 8 * n); memcpy(o->seen, h + o_seen, 4 * n); memcpy(o->near_order, h + o_near, 4 * n);
-    memcpy(o->n_near, h + o_cnt + 4, 4);
-    memcpy(o->cheiral, h + o_ch, n); memcpy(o->bin, h + o_bin, n);
-    sb.counts.h2d = 4 * ((int64_t)n_kf + n_cand);
-    sb.counts.d2h = (int64_t)bytes;
-    t->last = &sb.counts;
     return KBA_OK;
+}
+
+// W checked requests of distinct tracks as the W windows of one launch sequence: one upload (the argument records of windows
+// 1 .. W-1, then every window's lists), one download (the outputs of all windows), one synchronisation, then the scatter into the
+// callers' arrays.  Window 0's record travels in the launch parameters (kba_select.cu).
+static int select_run(kba_handle* h, SelectStage& st, int W, const SelectReq* r) {
+    CU(cudaSetDevice(h->device));
+    cudaStream_t s = h->stream;
+    SelectGrid g;
+    size_t n_list = 0, N = 0;
+    for (int w = 0; w < W; ++w) {
+        const SelectReq& q = r[w];
+        n_list += (size_t)q.n_kf + q.n_cand; N += (size_t)q.n_cand;
+        g.max_kf = std::max(g.max_kf, q.n_kf); g.max_cand = std::max(g.max_cand, q.n_cand);
+        g.max_init = std::max(g.max_init, std::max(std::max(q.n_kf, q.n_cand), q.t->n_cam));
+        g.max_meas = std::max(g.max_meas, q.max_meas);
+    }
+    // ---- staging: records | lists up; flow | seen | near order (by candidate of all windows) | counters (by window) | cheirality | bins down
+    const size_t o_lists = sizeof(SelectArgs) * (size_t)(W - 1), up_bytes = o_lists + 4 * n_list;
+    const size_t o_seen = 8 * N, o_near = o_seen + 4 * N, o_cnt = o_near + 4 * N, o_ch = o_cnt + 16 * (size_t)W, o_bin = o_ch + N;
+    const size_t out_bytes = o_bin + N;
+    int* lists_h = reinterpret_cast<int*>(st.up.h + o_lists);
+    const int* lists_d = reinterpret_cast<const int*>(st.up.d + o_lists);
+    unsigned char* d = st.out.d;
+    SelectLaunch l;
+    l.rest = reinterpret_cast<const SelectArgs*>(st.up.d);
+    l.n_win = W;
+    size_t li = 0, c0 = 0;
+    for (int w = 0; w < W; ++w) {
+        const SelectReq& q = r[w];
+        memcpy(lists_h + li, q.kf_slot, 4 * (size_t)q.n_kf);
+        if (q.n_cand) memcpy(lists_h + li + q.n_kf, q.lm_slot, 4 * (size_t)q.n_cand);
+        SelectArgs a = q.t->select->a;
+        a.td = q.t->td;
+        a.kf_slot = lists_d + li; a.lm_slot = lists_d + li + q.n_kf; a.n_kf = q.n_kf; a.n_cand = q.n_cand;
+        for (int k = 0; k < 3; ++k) a.leaf[k] = q.p->voxel_size[k];
+        a.roi_far = q.p->roi_far; a.roi_middle = q.p->roi_middle;
+        a.flow = reinterpret_cast<double*>(d + 8 * c0); a.seen = reinterpret_cast<int*>(d + o_seen + 4 * c0);
+        a.near_order = reinterpret_cast<int*>(d + o_near + 4 * c0);
+        a.counters = reinterpret_cast<int*>(d + o_cnt + 16 * (size_t)w); a.n_near = a.counters + 1;
+        a.cheiral = d + o_ch + c0; a.bin = reinterpret_cast<signed char*>(d + o_bin + c0);
+        if (w == 0) l.w0 = a;
+        else memcpy(st.up.h + sizeof(SelectArgs) * (size_t)(w - 1), &a, sizeof(SelectArgs));
+        li += (size_t)q.n_kf + q.n_cand; c0 += (size_t)q.n_cand;
+    }
+    // ---- one upload, one launch sequence, one download, one synchronisation
+    CU(cudaMemcpyAsync(st.up.d, st.up.h, up_bytes, cudaMemcpyHostToDevice, s));
+    launch_select(l, g, s);
+    CU(cudaGetLastError());
+    CU(cudaMemcpyAsync(st.out.h, st.out.d, out_bytes, cudaMemcpyDeviceToHost, s));
+    CU(wait_stream(h));
+    // ---- scatter
+    const unsigned char* hb = st.out.h;
+    c0 = 0;
+    for (int w = 0; w < W; ++w) {
+        const kba_select_out* o = r[w].o;
+        const size_t n = (size_t)r[w].n_cand;
+        memcpy(o->flow, hb + 8 * c0, 8 * n); memcpy(o->seen, hb + o_seen + 4 * c0, 4 * n); memcpy(o->near_order, hb + o_near + 4 * c0, 4 * n);
+        memcpy(o->n_near, hb + o_cnt + 16 * (size_t)w + 4, 4);
+        memcpy(o->cheiral, hb + o_ch + c0, n); memcpy(o->bin, hb + o_bin + c0, n);
+        c0 += n;
+    }
+    st.counts.h2d = (int64_t)up_bytes;
+    st.counts.d2h = (int64_t)out_bytes;
+    return KBA_OK;
+}
+
+int kba_track_select_landmarks(kba_track* t, int32_t n_kf, const int32_t* kf_slot, int32_t n_cand, const int32_t* lm_slot,
+                               const kba_select_params* p, kba_select_out* o) {
+    static const std::string who = "kba_track_select_landmarks: ";
+    if (!t) return fail(KBA_ERR_BAD_ARG, who + "null argument");
+    SelectReq r;
+    r.t = t; r.n_kf = n_kf; r.n_cand = n_cand; r.kf_slot = kf_slot; r.lm_slot = lm_slot; r.p = p; r.o = o;
+    std::string why;
+    int rc = select_check(r, why);
+    if (rc != KBA_OK) return fail(rc, who + why);
+    SelectStage& st = t->select->stage;
+    if (!st.up.d) {  // the first single call of the track
+        const size_t K = (size_t)t->td.kf_cap, L = (size_t)t->td.lm_cap;
+        if (st.alloc(4 * (K + L), select_out_bytes(L, 1))) {
+            st.up.release(); st.out.release();
+            return fail(KBA_ERR_CUDA, who + "out of memory for the selection staging");
+        }
+    }
+    rc = select_run(t->h, st, 1, &r);
+    if (rc == KBA_OK) t->last = &t->select->stage.counts;
+    return rc;
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
@@ -1992,6 +2075,48 @@ int kba_track_group_transfer_bytes(kba_track_group* g, int64_t* h2d, int64_t* d2
     if (h2d) *h2d = g->last->h2d;
     if (d2h) *d2h = g->last->d2h;
     return KBA_OK;
+}
+
+int kba_track_group_select_landmarks(kba_track_group* g, const kba_select_request* req, kba_select_out* out) {
+    static const std::string who = "kba_track_group_select_landmarks: ";
+    if (!g || !req || !out) return fail(KBA_ERR_BAD_ARG, who + "null argument");
+    const int n = (int)g->tracks.size();
+    // ---- every request is checked before anything is uploaded or written
+    std::vector<SelectReq> rs;
+    for (int i = 0; i < n; ++i) {
+        const kba_select_request& q = req[i];
+        const std::string track = "track " + std::to_string(i) + ": ";
+        if (q.n_kf == 0) {  // sits the call out
+            if (!out[i].n_near) return fail(KBA_ERR_BAD_ARG, who + track + "null argument");
+            continue;
+        }
+        SelectReq r;
+        r.t = g->tracks[i]; r.n_kf = q.n_kf; r.n_cand = q.n_cand; r.kf_slot = q.kf_slot; r.lm_slot = q.lm_slot; r.p = q.params; r.o = &out[i];
+        std::string why;
+        const int rc = select_check(r, why);
+        if (rc != KBA_OK) return fail(rc, who + track + why);
+        rs.push_back(r);
+    }
+    int rc = KBA_OK;
+    if (rs.empty()) {  // every track sits out: no upload, no launch
+        g->solver.h2d = 0; g->solver.d2h = 0;
+        g->last = &g->solver;
+    } else {
+        if (!g->select) {  // staging for every track at its capacities, allocated once
+            size_t lists = 0, cands = 0;
+            for (const kba_track* t : g->tracks) { lists += (size_t)t->td.kf_cap + t->td.lm_cap; cands += (size_t)t->td.lm_cap; }
+            std::unique_ptr<SelectStage> st(new SelectStage());
+            if (st->alloc(sizeof(SelectArgs) * (size_t)(n - 1) + 4 * lists, select_out_bytes(cands, (size_t)n)))
+                return fail(KBA_ERR_CUDA, who + "out of memory for the selection staging");
+            g->select = std::move(st);
+        }
+        rc = select_run(g->h, *g->select, (int)rs.size(), rs.data());
+        if (rc != KBA_OK) return rc;
+        g->last = &g->select->counts;
+    }
+    for (int i = 0; i < n; ++i)
+        if (req[i].n_kf == 0) *out[i].n_near = 0;
+    return rc;
 }
 
 // ---------------------------------------------------------------------------------------------------------------------

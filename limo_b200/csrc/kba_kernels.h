@@ -105,9 +105,9 @@ void launch_scatter_rows(double* dst, const int* slot, const double* src, int n,
 // results of every window w back into track store tds[w]
 void launch_track_writeback(const BatchDev& bd, const TrackDev* tds, const TrackSel* sels, const TrackGrid& g, cudaStream_t s);
 
-// ---- landmark selection on a track's store (kba_track_select_landmarks, kba_select.cu) ----
-// One request: active keyframe slots (ascending timestamp), candidate landmark slots (ascending id).  Scratch is sized for the
-// track's capacities at the first call; the outputs point into one device block that goes down in one copy.
+// ---- landmark selection on a track's store (kba_track_select_landmarks / kba_track_group_select_landmarks, kba_select.cu) ----
+// One window = one request: active keyframe slots (ascending timestamp), candidate landmark slots (ascending id).  Scratch is the
+// track's, sized for its capacities at its first selection; the outputs point into one device block that goes down in one copy.
 struct SelectArgs {
     TrackDev td;
     const int* kf_slot = nullptr;   // [n_kf]
@@ -139,7 +139,20 @@ struct SelectArgs {
     double* flow = nullptr;
     int* seen = nullptr;
 };
-void launch_select(const SelectArgs& a, int max_meas, cudaStream_t s);
+// W windows in one launch sequence, window = grid z.  Window 0's arguments travel in the launch parameters, as a one-track
+// selection's always did, so that it uploads its lists and nothing else; windows 1 .. W-1 read theirs from a device array that
+// goes up in the same copy as the lists.
+struct SelectLaunch {
+    SelectArgs w0;
+    const SelectArgs* rest = nullptr;  // [n_win - 1]
+    int n_win = 0;
+};
+// grid sizes: maxima over the windows (threads beyond their own window's sizes exit)
+struct SelectGrid {
+    int max_kf = 0, max_cand = 0, max_init = 0;  // max_init: of max(n_cand, n_kf, n_cam)
+    int max_meas = 0;                            // arena entries of a listed keyframe
+};
+void launch_select(const SelectLaunch& l, const SelectGrid& g, cudaStream_t s);
 
 // ---- motion-only frames against a track's store (kba_track_adjust_pose / kba_track_group_adjust_pose, kba_motion.cu) ----
 // One frame = one free pose against constant landmarks read from a store by slot: its measurements come in runs, one run per

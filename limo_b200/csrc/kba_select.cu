@@ -7,6 +7,11 @@
 // (internal/mini_eigen.hpp, g++ -O2 without FMA), and the file is compiled with -fmad=false, so that each quantity equals the
 // host's bit for bit.  Only integer atomics; every order-dependent step (voxel centroids, the near order, flow sums) runs in
 // a fixed order.
+//
+// Windows: one launch sequence serves W requests (a track group's, kba_track_group_select_landmarks; a single call is W = 1),
+// window w = blockIdx.z.  Grids are sized from the maxima over the windows and threads beyond their own window's sizes exit.
+// A window's counters live in its output block and its bounds, slot map and the rest of its scratch in its track's buffers:
+// no two windows share a word (a group lists a track once).
 #include <cfloat>
 #include <cstdint>
 
@@ -95,10 +100,14 @@ __device__ Grid grid_of(const SelectArgs& a) {
     return g;
 }
 
+// the arguments of this block's window (the launch parameters are __grid_constant__, so window 0's are read in place)
+__device__ __forceinline__ const SelectArgs& win(const SelectLaunch& l) { return blockIdx.z == 0 ? l.w0 : l.rest[blockIdx.z - 1]; }
+
 }  // namespace
 
 // slot -> candidate map, output defaults, keyframe and camera transforms, the keyframe path seen from the newest keyframe
-__global__ void __launch_bounds__(256) k_sel_init(SelectArgs a) {
+__global__ void __launch_bounds__(256) k_sel_init(const __grid_constant__ SelectLaunch l) {
+    const SelectArgs& a = win(l);
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i < a.n_cand) {
         a.cand_of[a.lm_slot[i]] = i;
@@ -125,8 +134,10 @@ __global__ void __launch_bounds__(256) k_sel_init(SelectArgs a) {
 // Cheirality (landmark_selection.cpp:17-31): every arena entry of an active keyframe that measures a candidate, one thread per
 // entry: z of cam * (kf * pos) < 0 clears the flag.  Also the candidate's observation count (flow gather) and, on the first entry
 // of its run in the keyframe (entries come in landmark-id order), one more keyframe that measures it (chooseFarLmIds).
-__global__ void __launch_bounds__(256) k_sel_cheiral(SelectArgs a) {
+__global__ void __launch_bounds__(256) k_sel_cheiral(const __grid_constant__ SelectLaunch l) {
+    const SelectArgs& a = win(l);
     const int k = blockIdx.y;
+    if (k >= a.n_kf) return;
     const int slot = a.kf_slot[k];
     const int n = a.td.m_cnt[slot], m0 = a.td.m_off[slot];
     const double* T = a.kf_T + 12 * (size_t)k;
@@ -146,7 +157,9 @@ __global__ void __launch_bounds__(256) k_sel_cheiral(SelectArgs a) {
 // Voxel scheme steps 1-3 on the survivors: into the newest keyframe's frame (double, rounded to float), PassThrough z in
 // [-20, 100], far bin = not closer than roi_far to the path.  The rest joins the voxel cloud: its bounding box by integer
 // atomics on order-preserving bit patterns, its list in any order (the rank sort fixes the order).
-__global__ void __launch_bounds__(256) k_sel_points(SelectArgs a) {
+__global__ void __launch_bounds__(256) k_sel_points(const __grid_constant__ SelectLaunch l) {
+    const SelectArgs& a = win(l);
+    if ((int)(blockIdx.x * blockDim.x) >= a.n_cand) return;  // whole blocks only: every warp below takes part in the reductions
     const int c = blockIdx.x * blockDim.x + threadIdx.x;
     bool inside = false;
     float f[3] = {0.f, 0.f, 0.f};
@@ -174,7 +187,8 @@ __global__ void __launch_bounds__(256) k_sel_points(SelectArgs a) {
 }
 
 // voxel index of every cloud point, relative to the cloud's minimum (voxel_grid: float floor, truncation to int)
-__global__ void __launch_bounds__(256) k_sel_vkey(SelectArgs a) {
+__global__ void __launch_bounds__(256) k_sel_vkey(const __grid_constant__ SelectLaunch l) {
+    const SelectArgs& a = win(l);
     const int r = blockIdx.x * blockDim.x + threadIdx.x;
     if (r >= a.counters[0]) return;
     const Grid g = grid_of(a);
@@ -189,7 +203,8 @@ __global__ void __launch_bounds__(256) k_sel_vkey(SelectArgs a) {
 
 // std::sort of the (voxel index, label) pairs, as a rank: each point counts the points ordered before it (labels are unique and
 // ascend with the candidate index).  O(n^2) comparisons from shared-memory tiles -- a few dozen microseconds for 20k points.
-__global__ void __launch_bounds__(256) k_sel_rank(SelectArgs a) {
+__global__ void __launch_bounds__(256) k_sel_rank(const __grid_constant__ SelectLaunch l) {
+    const SelectArgs& a = win(l);
     __shared__ long long s_key[256];
     __shared__ int s_lab[256];
     const int n = a.counters[0];
@@ -215,7 +230,8 @@ __global__ void __launch_bounds__(256) k_sel_rank(SelectArgs a) {
 
 // one point per voxel (step 4): the first point of each run of equal voxel indices sums its run in sorted order (float), its
 // label is the run's smallest; step 5: middle bin = centroid not closer than roi_middle to the path, near bin = the others
-__global__ void __launch_bounds__(256) k_sel_voxels(SelectArgs a) {
+__global__ void __launch_bounds__(256) k_sel_voxels(const __grid_constant__ SelectLaunch l) {
+    const SelectArgs& a = win(l);
     const int r = blockIdx.x * blockDim.x + threadIdx.x;
     const int n = a.counters[0];
     if (r >= n) return;
@@ -240,8 +256,9 @@ __global__ void __launch_bounds__(256) k_sel_voxels(SelectArgs a) {
     }
 }
 
-// the near bin in ascending voxel index: an ordered compaction of the near flags, one CTA
-__global__ void __launch_bounds__(1024) k_sel_near_order(SelectArgs a) {
+// the near bin in ascending voxel index: an ordered compaction of the near flags, one CTA per window
+__global__ void __launch_bounds__(1024) k_sel_near_order(const __grid_constant__ SelectLaunch l) {
+    const SelectArgs& a = win(l);
     __shared__ int s_scan[1024];
     const int n = a.counters[0], tid = threadIdx.x;
     int carry = 0;
@@ -265,8 +282,10 @@ __global__ void __launch_bounds__(1024) k_sel_near_order(SelectArgs a) {
 }
 
 // the observations of every near landmark, (keyframe position, arena index) keys behind its offset
-__global__ void __launch_bounds__(256) k_sel_gather(SelectArgs a) {
+__global__ void __launch_bounds__(256) k_sel_gather(const __grid_constant__ SelectLaunch l) {
+    const SelectArgs& a = win(l);
     const int k = blockIdx.y;
+    if (k >= a.n_kf) return;
     const int slot = a.kf_slot[k];
     const int n = a.td.m_cnt[slot], m0 = a.td.m_off[slot];
     for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
@@ -279,7 +298,8 @@ __global__ void __launch_bounds__(256) k_sel_gather(SelectArgs a) {
 // calcFlow(use_mean = false) of a near landmark: its observations in time order (insertion sort of a few dozen keys), per camera
 // the sum of the double norms between consecutive observations, the maximum over the cameras in index order (max_element with
 // `<`); NaN when no camera saw it twice.  Then the slot -> candidate map goes back to all -1.
-__global__ void __launch_bounds__(256) k_sel_flow(SelectArgs a) {
+__global__ void __launch_bounds__(256) k_sel_flow(const __grid_constant__ SelectLaunch l) {
+    const SelectArgs& a = win(l);
     const int c = blockIdx.x * blockDim.x + threadIdx.x;
     if (c >= a.n_cand) return;
     if (a.bin[c] == 0) {
@@ -317,21 +337,20 @@ __global__ void __launch_bounds__(256) k_sel_flow(SelectArgs a) {
     a.cand_of[a.lm_slot[c]] = -1;
 }
 
-void launch_select(const SelectArgs& a, int max_meas, cudaStream_t s) {
-    const int nc = a.n_cand > 0 ? a.n_cand : 1;
-    int n0 = a.n_cand > a.n_kf ? a.n_cand : a.n_kf;
-    n0 = n0 > a.n_cam ? n0 : a.n_cam;
-    const int gc = (nc + 255) / 256;
-    const dim3 gm((max_meas + 255) / 256 > 0 ? (max_meas + 255) / 256 : 1, a.n_kf);
-    k_sel_init<<<(n0 + 255) / 256, 256, 0, s>>>(a); LCHK("k_sel_init");
-    k_sel_cheiral<<<gm, 256, 0, s>>>(a); LCHK("k_sel_cheiral");
-    k_sel_points<<<gc, 256, 0, s>>>(a); LCHK("k_sel_points");
-    k_sel_vkey<<<gc, 256, 0, s>>>(a); LCHK("k_sel_vkey");
-    k_sel_rank<<<gc, 256, 0, s>>>(a); LCHK("k_sel_rank");
-    k_sel_voxels<<<gc, 256, 0, s>>>(a); LCHK("k_sel_voxels");
-    k_sel_near_order<<<1, 1024, 0, s>>>(a); LCHK("k_sel_near_order");
-    k_sel_gather<<<gm, 256, 0, s>>>(a); LCHK("k_sel_gather");
-    k_sel_flow<<<gc, 256, 0, s>>>(a); LCHK("k_sel_flow");
+void launch_select(const SelectLaunch& l, const SelectGrid& g, cudaStream_t s) {
+    const unsigned W = (unsigned)l.n_win;
+    const dim3 gi((g.max_init + 255) / 256, 1, W);
+    const dim3 gc((g.max_cand > 0 ? g.max_cand + 255 : 256) / 256, 1, W);
+    const dim3 gm((g.max_meas + 255) / 256 > 0 ? (g.max_meas + 255) / 256 : 1, g.max_kf, W);
+    k_sel_init<<<gi, 256, 0, s>>>(l); LCHK("k_sel_init");
+    k_sel_cheiral<<<gm, 256, 0, s>>>(l); LCHK("k_sel_cheiral");
+    k_sel_points<<<gc, 256, 0, s>>>(l); LCHK("k_sel_points");
+    k_sel_vkey<<<gc, 256, 0, s>>>(l); LCHK("k_sel_vkey");
+    k_sel_rank<<<gc, 256, 0, s>>>(l); LCHK("k_sel_rank");
+    k_sel_voxels<<<gc, 256, 0, s>>>(l); LCHK("k_sel_voxels");
+    k_sel_near_order<<<dim3(1, 1, W), 1024, 0, s>>>(l); LCHK("k_sel_near_order");
+    k_sel_gather<<<gm, 256, 0, s>>>(l); LCHK("k_sel_gather");
+    k_sel_flow<<<gc, 256, 0, s>>>(l); LCHK("k_sel_flow");
 }
 
 }  // namespace kba
