@@ -197,7 +197,8 @@ typedef struct kba_result {
 typedef struct kba_eval_out {
     double* residual;  /* [3*n_obs] rows (u, v, depth), robustified (sqrt(rho') applied); row 2 = 0 if no depth */
     double* jac_pose;  /* [18*n_obs] 3x6 row-major, d r~ / d (delta_rot, delta_trans); zeros for fixed keyframes */
-    double* jac_lm;    /* [9*n_obs]  3x3 row-major, d r~ / d landmark */
+    double* jac_lm;    /* [9*n_obs]  3x3 row-major, d r~ / d landmark; precision 1 on the fused path: formed in FP64 from the
+                          FP32 jac_pose as the solver forms it (translation columns times the keyframe's rotation) */
     double* cost;      /* [1] 0.5 * sum rho over reprojection + depth blocks */
     int32_t* failed;   /* [1] 1 if any |z_cam| < 0.01 (evaluation failure, cost_functors_ceres.hpp:78-83) */
 } kba_eval_out;

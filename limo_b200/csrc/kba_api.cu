@@ -1369,13 +1369,14 @@ int kba_eval(kba_handle* h, const kba_window* w, const kba_options* opt, kba_eva
     for (size_t e = 0; e < n; ++e) {  // e: internal (sorted) observation slot, o: the caller's observation index
         const size_t o = (size_t)b->obs_orig.h[e];
         const bool fixed = offp[w->obs_kf[o]] < 0;
-        // precision 1: the streams hold floats (same component-major layout)
-        auto at = [&](const std::vector<double>& v, size_t idx) {
-            return opt->precision ? (double)reinterpret_cast<const float*>(v.data())[idx] : v[idx];
+        // precision 1: the streams hold floats (same component-major layout); J_l expanded on the fused path is FP64 either way
+        auto at = [&](const std::vector<double>& v, size_t idx, bool f32) {
+            return f32 ? (double)reinterpret_cast<const float*>(v.data())[idx] : v[idx];
         };
-        if (out->residual) for (int q = 0; q < 3; ++q) out->residual[3 * o + q] = at(res_h, q * n + e);
-        if (out->jac_pose) for (int q = 0; q < 18; ++q) out->jac_pose[18 * o + q] = fixed ? 0.0 : at(jp_h, q * n + e);
-        if (out->jac_lm) for (int q = 0; q < 9; ++q) out->jac_lm[9 * o + q] = at(jl_h, q * n + e);
+        const bool f32 = opt->precision != 0;
+        if (out->residual) for (int q = 0; q < 3; ++q) out->residual[3 * o + q] = at(res_h, q * n + e, f32);
+        if (out->jac_pose) for (int q = 0; q < 18; ++q) out->jac_pose[18 * o + q] = fixed ? 0.0 : at(jp_h, q * n + e, f32);
+        if (out->jac_lm) for (int q = 0; q < 9; ++q) out->jac_lm[9 * o + q] = at(jl_h, q * n + e, f32 && !bd.fused);
     }
     if (out->cost) { double c = 0; for (int q = 0; q < bd.cost_parts; ++q) c += cost_h[q]; out->cost[0] = c; }
     if (out->failed) out->failed[0] = st.eval_failed;

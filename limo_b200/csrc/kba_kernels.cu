@@ -2339,9 +2339,10 @@ void launch_jacobian_only(const BatchDev& bd, const SolveParams& sp, cudaStream_
     launch_eval_obs<true>(bd, sp, s);
 }
 // inspection entry point (kba_eval) on the fused path: J_l of every observation, formed exactly as the consumers of the
-// linearisation form it -- translation columns of the materialised J_p times the staged rotation of the keyframe
+// linearisation form it -- translation columns of the materialised J_p times the staged rotation of the keyframe, in FP64
+// whatever precision J_p is stored in (precision 1: FP32 J_p, widened, times the FP64 rotation; the product is not rounded)
 template <typename TLin>
-__global__ void k_expand_jl(BatchDev bd, TLin* out) {
+__global__ void k_expand_jl(BatchDev bd, double* out) {
     const WinDesc& wd = bd.desc[0];
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= wd.n_obs) return;
@@ -2350,12 +2351,12 @@ __global__ void k_expand_jl(BatchDev bd, TLin* out) {
     const TLin* jp = reinterpret_cast<const TLin*>(bd.jp);
     for (int r = 0; r < 3; ++r) {
         const double m0 = (double)jp[(6 * r + 3) * T + o], m1 = (double)jp[(6 * r + 4) * T + o], m2 = (double)jp[(6 * r + 5) * T + o];
-        for (int c = 0; c < 3; ++c) out[(size_t)(3 * r + c) * T + o] = (TLin)(m0 * R[c] + m1 * R[3 + c] + m2 * R[6 + c]);
+        for (int c = 0; c < 3; ++c) out[(size_t)(3 * r + c) * T + o] = m0 * R[c] + m1 * R[3 + c] + m2 * R[6 + c];
     }
 }
 void launch_expand_jl(const BatchDev& bd, double* out, cudaStream_t s) {
     const int n = (int)bd.tot_obs;
-    if (bd.precision) k_expand_jl<float><<<(n + 255) / 256, 256, 0, s>>>(bd, reinterpret_cast<float*>(out));
+    if (bd.precision) k_expand_jl<float><<<(n + 255) / 256, 256, 0, s>>>(bd, out);
     else k_expand_jl<double><<<(n + 255) / 256, 256, 0, s>>>(bd, out);
     LCHK("k_expand_jl");
 }

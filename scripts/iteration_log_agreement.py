@@ -1,10 +1,11 @@
 """How closely the CUDA path reproduces the oracle's iteration log: the worst deviation per log field on every window of
 tests/test_iteration_log.py -- whole log, head of the log, and beside them the oracle against itself with its sums split over
 another number of threads -- on the kernel variants and the FP32 linearisation mode, and the deviation of the first LM step
-from the dense extended-precision step of tests/test_first_step_dense.py.  The tolerances of tests/iter_log.py and the figures
-in DESIGN.md section 2 come from this table; the card's name and power limit are printed with it.  Needs an H100.
+from the dense extended-precision step of tests/test_first_step_dense.py (oracle and CUDA path, every window there).  The
+tolerances of tests/iter_log.py and tests/test_first_step_dense.py and the figures in DESIGN.md section 2 come from this table;
+the card's name and power limit are printed with it.  Needs an H100.
 
-    python scripts/iteration_log_agreement.py [output file]
+    python scripts/iteration_log_agreement.py [output file] [--dense-only]
 """
 import os
 import subprocess
@@ -18,7 +19,9 @@ from tests import iter_log as il
 from tests import test_first_step_dense as fs
 from tests import test_iteration_log as tl
 
-out = open(sys.argv[1], "w") if len(sys.argv) > 1 else None
+args = [a for a in sys.argv[1:] if a != "--dense-only"]
+dense_only = "--dense-only" in sys.argv[1:]   # only the dense first step: the iteration logs take most of the run
+out = open(args[0], "w") if args else None
 
 
 def say(*a):
@@ -41,7 +44,7 @@ def row(label, gpu, cpu, prefix, solves=None, head=False):
 
 say(subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True).stdout.strip())
 h = capi.Handle(0)
-for name in tl.CASES:
+for name in [] if dense_only else tl.CASES:
     win, opt, prefix, threads = tl.build_case(name)
     rc = orc.solve_window(win, opt, num_threads=threads, iterations_capacity=tl.LOG_CAPACITY)
     rg = row(name + (" (prefix rule)" if prefix else ""), h.solve_window(win, opt, iterations_capacity=tl.LOG_CAPACITY), rc, prefix)
@@ -54,20 +57,31 @@ for name in tl.CASES:
             il.check_log_invariants(res, opt, name)
         except AssertionError as e:
             say("    invariants (%s) FAIL %s" % (who, e))
-for name in ("config2_slice", "config3_kf8"):
+for name in [] if dense_only else ("config2_slice", "config3_kf8"):
     win, opt, prefix, threads = tl.build_case(name)
     rc = orc.solve_window(win, opt, num_threads=threads, iterations_capacity=tl.LOG_CAPACITY)
     for variant in ("KBA_LINEARIZE", "KBA_FUSED"):
         os.environ[variant] = "0"
         row("%s %s=0" % (name, variant), h.solve_window(win, opt, iterations_capacity=tl.LOG_CAPACITY), rc, prefix)
         del os.environ[variant]
-win, opt, prefix, threads = tl.build_case("config2_full")
-rc = orc.solve_window(win, opt, num_threads=threads, iterations_capacity=tl.LOG_CAPACITY)
-opt.precision = 1
-row("config2_full precision=1, solve 0", h.solve_window(win, opt, iterations_capacity=tl.LOG_CAPACITY), rc, False, solves=(0,))
-for name, make in fs.WINDOWS.items():
-    win, opt = make(), capi.default_options()
-    ref = fs.dense_first_step(win, opt, h.evaluate(win), h.evaluate, orc)
-    dev = fs._check_first_step(h.solve_window(win, opt), ref, float("inf"), name)
-    say("%-36s " % ("dense step: " + name) + "  ".join("%s %.1e" % kv for kv in dev.items()))
+if not dense_only:
+    win, opt, prefix, threads = tl.build_case("config2_full")
+    rc = orc.solve_window(win, opt, num_threads=threads, iterations_capacity=tl.LOG_CAPACITY)
+    opt.precision = 1
+    row("config2_full precision=1, solve 0", h.solve_window(win, opt, iterations_capacity=tl.LOG_CAPACITY), rc, False, solves=(0,))
+
+
+def dense_row(label, devs):
+    """the worst deviation of each record field over `devs` (one dict per window of a batch)"""
+    say("%-44s " % label + "  ".join("%s %.1e" % (k, max(d[k] for d in devs)) for k in devs[0]))
+
+
+for name in fs.WINDOWS:   # the oracle against the dense step (needs no GPU; the CPU suite holds it)
+    win, opt = fs.build(name)
+    ref = fs.dense_first_step(win, opt, orc.evaluate(win, opt), lambda w: orc.evaluate(w, opt), orc)
+    dense_row("dense step, oracle: %s (%s)" % (name, fs.WINDOWS[name][1]),
+              [fs._check_first_step(orc.solve_window(win, opt), ref, float("inf"), name)])
+for name in fs.CUDA_CASES:
+    ref, results, tol = fs.cuda_first_step(h, orc, name)
+    dense_row("dense step, cuda: %s (%s)" % (name, tol), [fs._check_first_step(r, ref, float("inf"), name) for r in results])
 h.close()

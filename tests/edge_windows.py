@@ -1,13 +1,26 @@
 """Edge-case windows shared by the CPU (oracle only) and GPU (CUDA vs oracle) tests: ragged CSR rows, fully constant
 keyframes, an evaluation failure at the first iterate, and a window too small for trimming."""
+import inspect
+
 import numpy as np
 
 from limo_b200 import synth
 from limo_b200.capi_types import Window
 
+WINDOW_FIELDS = tuple(inspect.signature(Window.__init__).parameters)[1:]
+
+
+def copy_window(win, **over):
+    """copy of `win` with every field of Window (ground points, plane blocks, scale, plane-chain and speed regularisers
+    included) and some of them overridden"""
+    args = {k: getattr(win, k) for k in WINDOW_FIELDS}
+    args.update(over)
+    return Window(**args)
+
 
 def _rebuild(win, keep_obs=None, **over):
-    """copy of `win` with some observations dropped (keep_obs: boolean mask over observations) and fields overridden"""
+    """copy of `win` with some observations dropped (keep_obs: boolean mask over observations) and fields overridden;
+    ground points, plane blocks and the regularisers are not carried over (copy_window keeps them)"""
     ptr = np.asarray(win.lm_obs_ptr)
     keep = np.ones(win.n_obs, dtype=bool) if keep_obs is None else keep_obs
     counts = np.array([keep[ptr[j]:ptr[j + 1]].sum() for j in range(win.n_lm)])

@@ -2,14 +2,22 @@
 
 tests/test_iteration_log.py holds the CUDA log to the oracle's, and so trusts the oracle's Schur elimination, Jacobi scaling,
 damping, back substitution and controller arithmetic.  This file pins the first step of both to a reference that shares none
-of that code: the damped normal equations of the WHOLE problem (poses and landmarks, no elimination), assembled and solved in
-numpy.longdouble -- on the x86 hosts this suite runs on that is the 80-bit extended type (64-bit significand), which is what
-the host provides; the test is skipped where longdouble is no wider than double.
+of that code: the damped normal equations of the WHOLE program (poses, plane directions and distances, landmarks; no
+elimination), assembled and solved in numpy.longdouble -- on the x86 hosts this suite runs on that is the 80-bit extended type
+(64-bit significand), which is what the host provides; the test is skipped where longdouble is no wider than double.
 
-From the implementation under test it takes the robustified blocks (r, J_pose, J_landmark, cost) of evaluate(), which
-tests/test_gpu_parity.py::test_eval_matches_oracle and tests/test_oracle_jacobians.py pin on their own, and from the oracle
-the two operators pose_plus and scale_reg, which tests/test_oracle_jacobians.py checks by finite differences.  Plane-free
-windows only: the plane blocks and the regulariser chain of ground-plane windows have no dense reference here.
+From the implementation under test it takes the robustified observation blocks (r, J_pose, J_landmark, cost) of evaluate(),
+which tests/test_gpu_parity.py::test_eval_matches_oracle and tests/test_oracle_jacobians.py pin on their own.  From the oracle
+it takes the single-residual functions pose_plus, dir_plus, gp_height, gp_motion, scale_reg and speed_reg, which
+tests/test_oracle_jacobians.py checks by finite differences.  Everything else -- which parameter blocks are in the program, the
+Huber corrector of the ground rows, the weights of the plane chain, the FixScaleVectorPlus Jacobian of the direction-difference
+rows, the step and the controller -- is restated here.
+
+The windows between them select every solver path of limo_b200/csrc/kba_plan.h (asserted on each, through the plan driver of
+tests/test_launch_plan.py): the fused path with and without plane rows, the seven-slot k_schur_fused<7> (windows with no fixed
+keyframe: a free gauge makes their later iterates drift along flat directions, but the first damped step is well defined), the
+large-window path with the tiled, the split (k_chol_*) and the one-CTA row-major factorisation, the 6x6 motion-only system with
+its speed prior, and FP32 observation blocks.
 """
 from types import SimpleNamespace
 
@@ -20,15 +28,33 @@ import scipy.linalg
 from limo_b200 import synth
 from tests import edge_windows as ew
 from tests import iter_log as il
+from tests.test_launch_plan import driver  # noqa: F401  (the plan driver fixture)
 
 LD = np.longdouble
 pytestmark = pytest.mark.skipif(np.finfo(LD).eps >= np.finfo(np.float64).eps, reason="numpy.longdouble is not an extended type here")
 
-# Records 0 and 1 against the dense step, relative (cost_change in units of the cost).  Worst observed over the five windows,
-# oracle: step_norm 2.4e-12 (ragged: landmarks seen once, held by the damping alone), cost 4.1e-13, cost_change 1.7e-13,
-# relative_decrease 2.9e-13; CUDA path on an NVIDIA H100 80GB HBM3 (700 W): step_norm 1.2e-12, cost 4.2e-13, cost_change
-# 1.7e-13, relative_decrease 3.0e-13 (scripts/iteration_log_agreement.py).  About 100 times the worst of them:
+# Records 0 and 1 against the dense step, relative (cost_change in units of the cost).  Worst observed, oracle and CUDA path on an
+# NVIDIA H100 80GB HBM3 (power limit 700 W), by scripts/iteration_log_agreement.py:
+#   plane-free windows (config1 .. config5_kf40_lm700, motion_only_speed_prior, the batch of 17):
+#     oracle: step_norm 2.4e-12 (ragged: landmarks seen once, held by the damping alone), cost 5.7e-13, relative_decrease 2.9e-13
+#     CUDA:   step_norm 1.2e-12 (stereo_rig), cost 4.2e-13, cost_change 1.7e-13, relative_decrease 3.0e-13 (config2_slice)
+#   ground-plane windows (config3_kf8, config3_kf14, planes_kf18_none_fixed, config3_kf30_lm600):
+#     oracle: step_norm 8.0e-13 (config3_kf14), cost 7.5e-13, relative_decrease 4.0e-13 (planes_kf18_none_fixed)
+#     CUDA:   step_norm 2.8e-13 (config3_kf14), cost 3.1e-14, relative_decrease 1.7e-14
+# STEP_TOL is about 100 times the worst plane-free deviation.  A ground window has few ground rows: one of them, or one row of
+# the plane chain, wrong by 1e-6 moves the records by 9e-11 .. 1.8e-10 (test_dense_step_notices_a_wrong_ground_row), so
+# GROUND_TOL sits between that and the worst ground deviation (12 times the oracle's, 36 times the CUDA path's).
+#
+# FP32 blocks (kba_options.precision = 1, config2_slice): cost 1 2.8e-05, step_norm 1.1e-05, relative_decrease 3.6e-05, and
+# gradient_max_norm 1.3e-06 already in record 0.  That is not rounding of the FP64 chain: the solve does not form the normal
+# equations of the blocks kba_eval reports.  The landmark blocks and the pose-landmark coupling come from the FP32 J_p and r,
+# but k_pose_hessian re-evaluates each observation's pose rows in FP64 for the pose blocks and the pose gradient.  No single
+# Jacobian gives that system, so the reference, built from the FP32 blocks alone, differs from it by what FP32 rounding does to
+# the pose rows.  FP32_TOL is about 100 times the measured deviation and tells a working FP32 mode from a broken one.
 STEP_TOL = 1e-10
+GROUND_TOL = 1e-11
+FP32_TOL = 4e-3
+TOL = {"plane_free": STEP_TOL, "ground": GROUND_TOL, "fp32": FP32_TOL}
 
 
 def _shapes(name):
@@ -36,13 +62,86 @@ def _shapes(name):
     return getattr(sf, name)()
 
 
+def _motion_only(with_prior):
+    from tests import test_iteration_log as tl
+    return tl._motion_only(with_prior)
+
+
+def _no_fixed_keyframe(win):
+    return ew.copy_window(win, kf_fixed=np.zeros(win.n_kf, dtype=np.uint8))
+
+
+# name -> (window builder, tolerance class, columns of the dense system, launch plan fields the window selects as a batch of one).
+# Names follow tests/test_iteration_log.CASES where the window is there; landmark counts are cut so that every dense system
+# stays below 2 500 columns.
 WINDOWS = {
-    "config1": lambda: synth.make_window(1),
-    "config2_slice": lambda: synth.make_window(2, n_kf=12, n_lm=400, n_obs=3000),
-    "stereo_rig": lambda: _shapes("_stereo_rig"),
-    "gap_over_fixed_keyframe": lambda: _shapes("_gap_over_fixed_keyframe"),
-    "ragged": ew.CASES["ragged"],
+    "config1": (lambda: synth.make_window(1), "plane_free", 624, dict(fused=1, fused_slots=6)),
+    "config2_slice": (lambda: synth.make_window(2, n_kf=12, n_lm=400, n_obs=3000), "plane_free", 1266,
+                      dict(fused=1, fused_slots=6)),
+    "stereo_rig": (lambda: _shapes("_stereo_rig"), "plane_free", 942, dict(fused=1, fused_slots=6)),
+    "gap_over_fixed_keyframe": (lambda: _shapes("_gap_over_fixed_keyframe"), "plane_free", 2148, dict(fused=1, fused_slots=6)),
+    "ragged": (ew.CASES["ragged"], "plane_free", 612, dict(fused=1, fused_slots=6)),
+    # plane rows, Huber ground rows and the plane chain on the fused path
+    "config3_kf8": (lambda: synth.make_window(3, seed=41, n_kf=8, n_lm=300, n_obs=1800, gp_frac=0.2), "ground", 970,
+                    dict(fused=1, fused_slots=6)),
+    "config3_kf14": (lambda: synth.make_window(3, seed=41, n_kf=14, n_lm=500, n_obs=4500), "ground", 1630,
+                     dict(fused=1, fused_slots=6)),
+    # 181 rows over 18 keyframes with plane blocks, none of them fixed: k_schur_fused<7> with plane blocks
+    "planes_kf18_none_fixed": (lambda: _no_fixed_keyframe(synth.make_window(3, seed=43, n_kf=18, n_lm=500, n_obs=4500)),
+                               "ground", 1680, dict(fused=1, fused_slots=7)),
+    # 181 rows over 30 plane-free keyframes, none of them fixed: k_schur_fused<7>
+    "free_kf30_none_fixed": (lambda: _no_fixed_keyframe(synth.make_window(2, n_kf=30, n_lm=700, n_obs=7000, seed=5)),
+                             "plane_free", 2280, dict(fused=1, fused_slots=7)),
+    # 187 rows over 31 keyframes: the large-window path, k_reduced_solve tiled at 192 rows
+    "free_keyframes_30": (lambda: synth.make_window(2, n_kf=31, n_lm=700, n_obs=7000, seed=5), "plane_free", 2280,
+                          dict(fused=0, small_syrk=0, nr_cap_max=192, solve_tiled=1, solve_split=0)),
+    # 301 rows with plane blocks: k_eval_obs<true>, k_schur_syrk, row-major factorisation split over 32 CTAs (k_chol_*)
+    "config3_kf30_lm600": (lambda: synth.make_window(3, seed=41, n_lm=600, n_obs=6000), "ground", 2090,
+                           dict(fused=0, small_syrk=0, nr_cap_max=320, solve_tiled=0, solve_split=32)),
+    # 241 rows, plane-free: row-major, k_chol_* split
+    "config5_kf40_lm700": (lambda: synth.make_window(5, n_kf=40, n_lm=700, n_obs=8000), "plane_free", 2334,
+                           dict(fused=0, small_syrk=0, nr_cap_max=256, solve_tiled=0, solve_split=32)),
+    # adjustPoseOnly: landmarks constant, one pose and the speed prior
+    "motion_only_speed_prior": (lambda: _motion_only(True), "plane_free", 6, dict(fused=1, fused_slots=6)),
 }
+
+
+def _motion_options(opt):
+    opt.min_landmarks_for_trimming = 30
+
+
+OPTION_HOOKS = {"motion_only_speed_prior": _motion_options}
+
+# CUDA runs: name -> (window of WINDOWS, kba_options.precision, copies in one kba_solve_batch, plan fields beyond the window's)
+CUDA_CASES = dict({name: (name, 0, 1, {}) for name in WINDOWS},
+                  # 17 windows: more than the split factorisation takes, so k_reduced_solve factorises each in one CTA
+                  config5_kf40_lm700_batch17=("config5_kf40_lm700", 0, 17, dict(solve_tiled=0, solve_split=0)),
+                  # FP32 observation blocks (k_eval_obs<float>), everything after them in FP64
+                  config2_slice_fp32=("config2_slice", 1, 1, {}))
+
+
+def build(name):
+    """(window, options) of a window of WINDOWS"""
+    from oracle import oracle as orc
+    opt = orc.default_options()
+    if name in OPTION_HOOKS:
+        OPTION_HOOKS[name](opt)
+    return WINDOWS[name][0](), opt
+
+
+def plan_shape(win):
+    """(rows, free rows, 32-landmark chunks, 8-landmark groups, landmarks) of a window as kba_batch_create sizes it"""
+    planes = win.n_gp > 0 or win.plane_reg_weight > 0
+    per = 10 if planes else 6
+    free = int((np.asarray(win.kf_fixed) == 0).sum())
+    return per * win.n_kf + 1, per * free + 1, -(-win.n_lm // 32), -(-win.n_lm // 8), win.n_lm
+
+
+def assert_path(driver, windows, want):  # noqa: F811
+    """the launch plan of kba_solve_batch on `windows` (default knobs, an H100's SMs) has the fields of `want`"""
+    from tests.test_launch_plan import FIELDS, _query
+    got = dict(zip(FIELDS, map(int, driver(_query("plan", [plan_shape(w) for w in windows], "batch", 1, 0, 1))[0].split())))
+    assert {k: got[k] for k in want} == want, (got, want)
 
 
 def _solve_spd(A, b):
@@ -61,57 +160,141 @@ def _solve_spd(A, b):
     raise AssertionError("iterative refinement did not converge")
 
 
-def dense_first_step(win, opt, blocks, evaluate, orc):
+def program_columns(win):
+    """The parameter blocks of the window's first solve and their columns, by the rules of the oracle's program_layout
+    (kba_oracle.c): a pose for each keyframe that is observed, anchors a ground point, is a scale keyframe or carries the speed
+    prior -- every keyframe under the plane-chain regularisation (weight > 0, at least two keyframes); a direction (3) and a
+    distance (1) for each keyframe with a ground point, or every keyframe under the regularisation, no distance when
+    plane_dist_fixed; nothing for a fixed keyframe; a landmark for each landmark with an observation or a ground point, none when
+    landmarks_fixed.  Columns run keyframe by keyframe (pose, direction, distance), then the landmarks."""
+    K = win.n_kf
+    gp_lm = np.zeros(0, dtype=int) if win.n_gp == 0 else np.asarray(win.gp_lm)
+    gp_kf = np.zeros(0, dtype=int) if win.n_gp == 0 else np.asarray(win.gp_kf)
+    pose_in, plane_in = np.zeros(K, dtype=bool), np.zeros(K, dtype=bool)
+    pose_in[np.asarray(win.obs_kf)] = True
+    pose_in[gp_kf] = plane_in[gp_kf] = True
+    if win.scale_weight > 0:
+        pose_in[[win.scale_kf0, win.scale_kf1]] = True
+    if win.plane_reg_weight > 0 and K > 1:
+        pose_in[:] = plane_in[:] = True
+    if win.speed_weight > 0:
+        pose_in[win.speed_kf] = True
+    L = SimpleNamespace(pose={}, dir={}, dist={})
+    n = 0
+    for k in range(K):
+        if win.kf_fixed[k]:
+            continue
+        if pose_in[k]:
+            L.pose[k] = n; n += 6
+        if plane_in[k]:
+            L.dir[k] = n; n += 3
+            if not win.plane_dist_fixed:
+                L.dist[k] = n; n += 1
+    L.n_f = n
+    lm_in = np.diff(np.asarray(win.lm_obs_ptr)) > 0
+    lm_in[gp_lm] = True
+    if win.landmarks_fixed:
+        lm_in[:] = False
+    L.lm_in = np.flatnonzero(lm_in)
+    L.lm = np.full(win.n_lm, -1)
+    L.lm[L.lm_in] = n + 3 * np.arange(len(L.lm_in))
+    L.n = n + 3 * len(L.lm_in)
+    return L
+
+
+def _dir_plus_jacobian(n):
+    """FixScaleVectorPlus at delta = 0, local_parameterizations.hpp:146-162: (I - n n^T / |n|^2) / |n|"""
+    n = np.asarray(n, dtype=LD)
+    nn = n @ n
+    return (np.eye(3, dtype=LD) - np.outer(n, n) / nn) / np.sqrt(nn)
+
+
+def _row(kind, parts, r, sqrt_rho1):
+    """one residual block: (column or None (constant block), Jacobian) parts and the residual, each times sqrt(rho') -- Ceres'
+    corrector for rho'' <= 0, which holds for every loss here"""
+    parts = [(c, sqrt_rho1 * np.atleast_2d(np.asarray(J, dtype=LD))) for c, J in parts if c is not None and c >= 0]
+    return SimpleNamespace(kind=kind, parts=parts, r=sqrt_rho1 * np.atleast_1d(np.asarray(r, dtype=LD)))
+
+
+def other_rows(win, opt, orc, L, poses, planes, lms):
+    """The residual blocks besides the observations, and their cost, at (poses, planes, lms):
+      ground points: gp_height with ScaledLoss(Huber(gp_huber), weight) (cpp:517-562);
+      scale: scale_reg with ScaledLoss(Trivial, weight) (cpp:890-904);
+      plane chain (cpp:769-818), for each pair of consecutive keyframes: dir1 - dir0 (weight 3w), dist1 - dist0 (w),
+      gp_motion (2w); for each keyframe (0, 0, 1) - dir (w);
+      speed prior: speed_reg with weight speed_weight (cpp:835-853)."""
+    rows, cost = [], LD(0)
+
+    def trivial(kind, parts, r, weight):
+        nonlocal cost
+        r = np.atleast_1d(np.asarray(r, dtype=LD))
+        cost += LD(weight) * (r @ r) / 2
+        rows.append(_row(kind, parts, r, np.sqrt(LD(weight))))
+
+    a = LD(opt.gp_huber)
+    for g in range(win.n_gp):
+        j, k = int(win.gp_lm[g]), int(win.gp_kf[g])
+        res, jp, jd, jdist, jl = orc.gp_height(poses[k], planes[k, :3], planes[k, 3], lms[j])
+        s, w = LD(res[0]) ** 2, LD(win.gp_weight[g])
+        rho0, rho1 = (2 * a * np.sqrt(s) - a * a, a / np.sqrt(s)) if s > a * a else (s, LD(1))
+        cost += w * rho0 / 2
+        rows.append(_row("ground", [(L.pose.get(k), jp), (L.dir.get(k), jd), (L.dist.get(k), jdist), (L.lm[j], jl)], res,
+                         np.sqrt(w * rho1)))
+    if win.scale_weight > 0:
+        res, j1, j0 = orc.scale_reg(poses[win.scale_kf1], poses[win.scale_kf0], win.scale_value)
+        trivial("scale", [(L.pose.get(win.scale_kf1), j1), (L.pose.get(win.scale_kf0), j0)], res, win.scale_weight)
+    if win.plane_reg_weight > 0 and win.n_kf > 1:
+        w = win.plane_reg_weight
+        for k0 in range(win.n_kf - 1):
+            k1 = k0 + 1
+            n0, n1 = planes[k0, :3], planes[k1, :3]
+            trivial("plane_dir", [(L.dir.get(k1), _dir_plus_jacobian(n1)), (L.dir.get(k0), -_dir_plus_jacobian(n0))],
+                    np.asarray(n1, dtype=LD) - np.asarray(n0, dtype=LD), 3 * w)
+            trivial("plane_dist", [(L.dist.get(k1), [[1.0]]), (L.dist.get(k0), [[-1.0]])], LD(planes[k1, 3]) - LD(planes[k0, 3]), w)
+            res, j0, j1, jd = orc.gp_motion(poses[k0], poses[k1], n0)
+            trivial("plane_motion", [(L.pose.get(k0), j0), (L.pose.get(k1), j1), (L.dir.get(k0), jd)], res, 2 * w)
+        for k in range(win.n_kf):
+            trivial("plane_up", [(L.dir.get(k), -_dir_plus_jacobian(planes[k, :3]))],
+                    np.array([0, 0, 1], dtype=LD) - np.asarray(planes[k, :3], dtype=LD), w)
+    if win.speed_weight > 0:
+        res, jp = orc.speed_reg(poses[win.speed_kf], win.speed_T_origin_before, win.speed_dt, win.speed_v_before)
+        trivial("speed", [(L.pose.get(win.speed_kf), jp)], res, win.speed_weight)
+    return rows, cost
+
+
+def _planes(win):
+    """the plane state (direction, distance) of every keyframe: the window's, or the oracle's default (0, 0, 1, 0)"""
+    return np.tile([0.0, 0.0, 1.0, 0.0], (win.n_kf, 1)) if win.kf_plane is None else win.kf_plane.copy()
+
+
+def dense_first_step(win, opt, blocks, evaluate, orc, tamper=None):
     """Records 0 and 1 of the first inner solve as a dense reference gives them.
 
-    blocks: (r [n_obs, 3], jac_pose [n_obs, 3, 6], jac_lm [n_obs, 3, 3], cost) at the window's state; evaluate(window) returns
-    the same tuple (the candidate's cost is taken from it); orc: the oracle binding (pose_plus, scale_reg).
-    Unknowns: 6 columns per keyframe that is not constant, then 3 per landmark with an observation.  The Jacobian is never
-    stored densely (18 000 x 2 100 longdoubles); J^T J and J^T r are summed from its blocks, which is the same matrix."""
+    blocks: (r [n_obs, 3], jac_pose [n_obs, 3, 6], jac_lm [n_obs, 3, 3], cost) of the observations at the window's state;
+    evaluate(window) returns the same tuple (the candidate's observation cost is taken from it); orc: the oracle binding (its
+    single-residual functions).  tamper(rows), if given, may change the residual blocks at the window's state before the system
+    is formed (the negative controls).  The Jacobian is never stored densely (18 000 x 2 300 longdoubles); J^T J and J^T r are
+    summed from its blocks, which is the same matrix."""
     r, jp, jl = (np.asarray(a, dtype=LD) for a in blocks[:3])
-    cost_x = LD(blocks[3])
-    ptr = np.asarray(win.lm_obs_ptr)
-    lm_of_obs = np.repeat(np.arange(win.n_lm), np.diff(ptr))
+    L = program_columns(win)
+    n = L.n
+    lm_of_obs = np.repeat(np.arange(win.n_lm), np.diff(np.asarray(win.lm_obs_ptr)))
     kf_of_obs = np.asarray(win.obs_kf)
-    has_scale = win.scale_weight > 0
-    free_kf = [k for k in range(win.n_kf) if not win.kf_fixed[k] and
-               ((kf_of_obs == k).any() or (has_scale and k in (win.scale_kf0, win.scale_kf1)))]
-    col_kf = {k: 6 * i for i, k in enumerate(free_kf)}
-    in_lm = np.flatnonzero(np.diff(ptr) > 0)
-    n_p = 6 * len(free_kf)
-    col_lm = np.full(win.n_lm, -1)
-    col_lm[in_lm] = n_p + 3 * np.arange(len(in_lm))
-    n = n_p + 3 * len(in_lm)
+    planes0 = _planes(win)
 
-    # rows of the Jacobian as (columns, values, residual): observations, then the scale regulariser
-    rows_c, rows_v, rows_r = [], [], []
-    for o in range(win.n_obs):
-        k, j = int(kf_of_obs[o]), int(lm_of_obs[o])
-        cols = np.arange(col_lm[j], col_lm[j] + 3)
-        vals = jl[o]
-        if k in col_kf:
-            cols = np.concatenate([np.arange(col_kf[k], col_kf[k] + 6), cols])
-            vals = np.concatenate([jp[o], jl[o]], axis=1)
-        rows_c.append(cols); rows_v.append(vals); rows_r.append(r[o])
-
-    def scale_row(poses):
-        """sqrt(weight) * (residual, Jacobian) of the scale regulariser |t(pose1 relative to pose0)| - scale_value: Ceres'
-        ScaledLoss(TrivialLoss, weight) corrects a block by sqrt(rho') = sqrt(weight); its cost is weight * r^2 / 2"""
-        res, j1, j0 = orc.scale_reg(poses[win.scale_kf1], poses[win.scale_kf0], win.scale_value)
-        sw = np.sqrt(LD(win.scale_weight))
-        cols, vals = [], []
-        for k, jk in ((win.scale_kf1, j1), (win.scale_kf0, j0)):
-            if k in col_kf:
-                cols.append(np.arange(col_kf[k], col_kf[k] + 6)); vals.append(sw * jk.astype(LD))
-        return np.concatenate(cols), np.concatenate(vals, axis=1), sw * res.astype(LD), LD(win.scale_weight) * LD(res[0]) ** 2 / 2
-
-    reg_cost = LD(0)
-    if has_scale:
-        cols, vals, res, reg_cost = scale_row(win.kf_pose)
-        rows_c.append(cols); rows_v.append(vals); rows_r.append(res)
+    rows = [SimpleNamespace(kind="observation", r=r[o], parts=[(c, J) for c, J in ((L.pose.get(int(kf_of_obs[o])), jp[o]),
+                                                                                    (L.lm[lm_of_obs[o]], jl[o]))
+                                                                if c is not None and c >= 0])
+            for o in range(win.n_obs)]
+    more, other_cost = other_rows(win, opt, orc, L, win.kf_pose, planes0, win.lm_pos)
+    rows += more
+    if tamper:
+        tamper(rows)
+    rows = [(np.concatenate([np.arange(c, c + J.shape[1]) for c, J in rw.parts]), np.concatenate([J for _, J in rw.parts], axis=1),
+             rw.r) for rw in rows if rw.parts]
 
     H, g = np.zeros((n, n), dtype=LD), np.zeros(n, dtype=LD)
-    for cols, vals, res in zip(rows_c, rows_v, rows_r):
+    for cols, vals, res in rows:
         H[np.ix_(cols, cols)] += vals.T @ vals
         g[cols] += vals.T @ res
     c = np.diag(H).copy()                                   # squared column norms
@@ -122,33 +305,43 @@ def dense_first_step(win, opt, blocks, evaluate, orc):
     A[np.diag_indices(n)] += D
     delta = s * _solve_spd(A, -s * g)
     model = LD(0)                                           # -(J delta)^T (r + J delta / 2)
-    for cols, vals, res in zip(rows_c, rows_v, rows_r):
+    for cols, vals, res in rows:
         jd = vals @ delta[cols]
         model -= jd @ (res + jd / 2)
 
-    def plus(step):
-        """x + step: pose_plus on the keyframes, addition on the landmarks; and the norms of the ambient difference"""
-        step = step.astype(np.float64)
-        poses, lms = win.kf_pose.copy(), win.lm_pos.copy()
-        for k, c0 in col_kf.items():
-            poses[k] = orc.pose_plus(win.kf_pose[k], step[c0:c0 + 6])
-        lms[in_lm] += step[n_p:].reshape(-1, 3)
-        diff = np.concatenate([(poses - win.kf_pose)[free_kf].ravel(), (lms - win.lm_pos)[in_lm].ravel()]).astype(LD)
-        return poses, lms, np.sqrt(diff @ diff), np.abs(diff).max()
+    def blocks_of(poses, planes, lms):
+        """the variable blocks of a state in ambient coordinates, one vector"""
+        return np.concatenate([poses[list(L.pose)].ravel(), planes[list(L.dir)][:, :3].ravel(), planes[list(L.dist)][:, 3],
+                               lms[L.lm_in].ravel()]).astype(LD)
 
-    out = SimpleNamespace(cost0=cost_x + reg_cost, radius0=radius, n_columns=n)
-    out.gradient_max_norm0 = plus(-g)[3]
-    poses, lms, out.step_norm, _ = plus(delta)
-    cand = ew._rebuild(win, kf_pose=poses, lm_pos=lms)
+    def plus(step):
+        """x + step: pose_plus on the poses, dir_plus on the directions, addition on distances and landmarks; and the norms of
+        the ambient difference"""
+        step = step.astype(np.float64)
+        poses, planes, lms = win.kf_pose.copy(), planes0.copy(), win.lm_pos.copy()
+        for k, c0 in L.pose.items():
+            poses[k] = orc.pose_plus(win.kf_pose[k], step[c0:c0 + 6])
+        for k, c0 in L.dir.items():
+            planes[k, :3] = orc.dir_plus(planes0[k, :3], step[c0:c0 + 3])
+        for k, c0 in L.dist.items():
+            planes[k, 3] = planes0[k, 3] + step[c0]
+        lms[L.lm_in] += step[L.n_f:].reshape(-1, 3)
+        diff = blocks_of(poses, planes, lms) - blocks_of(win.kf_pose, planes0, win.lm_pos)
+        return poses, planes, lms, np.sqrt(diff @ diff), np.abs(diff).max()
+
+    out = SimpleNamespace(cost0=LD(blocks[3]) + other_cost, radius0=radius, n_columns=n)
+    out.gradient_max_norm0 = plus(-g)[4]
+    poses, planes, lms, out.step_norm, _ = plus(delta)
+    cand = ew.copy_window(win, kf_pose=poses, kf_plane=None if win.kf_plane is None else planes, lm_pos=lms)
     cand_blocks = evaluate(cand)
     assert cand_blocks[4] == 0
-    cand_cost = LD(cand_blocks[3]) + (scale_row(poses)[3] if has_scale else 0)
+    cand_cost = LD(cand_blocks[3]) + other_rows(win, opt, orc, L, poses, planes, lms)[1]
     out.cost_change = out.cost0 - cand_cost
     out.relative_decrease = out.cost_change / model
     out.successful = bool(out.relative_decrease > opt.min_relative_decrease)
     # neither tolerance test fires on the first step of these windows (the record would be written differently)
-    x = np.concatenate([win.kf_pose[free_kf].ravel(), win.lm_pos[in_lm].ravel()])
-    assert out.step_norm > opt.parameter_tolerance * (np.linalg.norm(x) + opt.parameter_tolerance)
+    x = blocks_of(win.kf_pose, planes0, win.lm_pos)
+    assert out.step_norm > opt.parameter_tolerance * (np.sqrt(x @ x) + opt.parameter_tolerance)
     assert abs(out.cost_change) > opt.function_tolerance * out.cost0
     out.cost1 = cand_cost                                   # the accepted iterate's cost, or the rejected candidate's
     rho = out.relative_decrease
@@ -179,25 +372,60 @@ def _check_first_step(res, ref, tol, label):
 
 
 @pytest.mark.parametrize("name", list(WINDOWS))
-def test_oracle_first_step_matches_dense_step(oracle, name):
-    """the oracle's elimination, scaling, damping, back substitution and controller arithmetic, without a GPU"""
-    win = WINDOWS[name]()
-    opt = oracle.default_options()
-    ref = dense_first_step(win, opt, oracle.evaluate(win), oracle.evaluate, oracle)
-    assert ref.successful and ref.n_columns > 3 * 190
-    _check_first_step(oracle.solve_window(win, opt), ref, STEP_TOL, name)
+def test_oracle_first_step_matches_dense_step(oracle, driver, name):  # noqa: F811
+    """the oracle's elimination, scaling, damping, back substitution and controller arithmetic, without a GPU; and the solver
+    path the window selects on the CUDA side"""
+    _, tol, columns, path = WINDOWS[name]
+    win, opt = build(name)
+    assert_path(driver, [win], path)
+    ref = dense_first_step(win, opt, oracle.evaluate(win, opt), lambda w: oracle.evaluate(w, opt), oracle)
+    assert ref.successful and ref.n_columns == columns
+    _check_first_step(oracle.solve_window(win, opt), ref, TOL[tol], name)
 
 
 def test_dense_step_notices_a_wrong_block(oracle):
     """the reference can fail: the landmark Jacobian of ONE observation of 1000 off by 1e-6 moves the candidate cost by 1.4e-9"""
-    win = WINDOWS["config1"]()
-    opt = oracle.default_options()
+    win, opt = build("config1")
     r, jp, jl, cost, failed = oracle.evaluate(win)
     jl = jl.copy()
     jl[5] *= 1 + 1e-6
     ref = dense_first_step(win, opt, (r, jp, jl, cost, failed), oracle.evaluate, oracle)
     with pytest.raises(AssertionError):
         _check_first_step(oracle.solve_window(win, opt), ref, STEP_TOL, "perturbed")
+
+
+def _scale_part(kind, which, part, factor):
+    """tamper(): the `part`-th Jacobian part of the `which`-th residual block of `kind` times `factor`"""
+    def tamper(rows):
+        rw = [x for x in rows if x.kind == kind][which]
+        c, J = rw.parts[part]
+        rw.parts[part] = (c, J * LD(factor))
+    return tamper
+
+
+@pytest.mark.parametrize("kind, which, part", [("ground", 0, 1),          # a ground point's direction Jacobian
+                                               ("plane_motion", 2, 0)])   # a plane-chain row: gp_motion, pose of keyframe 2
+def test_dense_step_notices_a_wrong_ground_row(oracle, kind, which, part):
+    """the reference can fail on a ground window at the tolerance ground windows are held to: one ground row or one plane-chain
+    row of config3_kf8 off by 1e-6"""
+    win, opt = build("config3_kf8")
+    blocks = oracle.evaluate(win, opt)
+    res = oracle.solve_window(win, opt)
+    _check_first_step(res, dense_first_step(win, opt, blocks, oracle.evaluate, oracle), GROUND_TOL, "as it is")
+    ref = dense_first_step(win, opt, blocks, oracle.evaluate, oracle, tamper=_scale_part(kind, which, part, 1 + 1e-6))
+    with pytest.raises(AssertionError):
+        _check_first_step(res, ref, GROUND_TOL, "perturbed")
+
+
+def test_window_copy_keeps_every_field():
+    """copy_window carries the ground points, plane blocks and regularisers that the no-fixed-keyframe windows need"""
+    ground, speed = build("config3_kf8")[0], build("motion_only_speed_prior")[0]
+    assert ground.n_gp > 0 and ground.plane_reg_weight > 0 and speed.speed_weight > 0 and speed.landmarks_fixed
+    for win in (ground, speed):
+        cp = ew.copy_window(win)
+        for f in ew.WINDOW_FIELDS:
+            a, b = getattr(win, f), getattr(cp, f)
+            assert (a is None and b is None) or np.array_equal(np.asarray(a), np.asarray(b)), f
 
 
 @pytest.fixture(scope="module")
@@ -208,12 +436,25 @@ def handle():
     h.close()
 
 
+def cuda_first_step(handle, oracle, name):
+    """(the dense step of a CUDA case from kba_eval's blocks, the kba_solve_batch results of its copies, tolerance class)"""
+    window, precision, copies, _ = CUDA_CASES[name]
+    win, opt = build(window)
+    opt.precision = precision
+    ref = dense_first_step(win, opt, handle.evaluate(win, opt), lambda w: handle.evaluate(w, opt), oracle)
+    results = handle.solve_batch([win] * copies, opt, iterations_capacity=256)
+    return ref, results, "fp32" if precision else WINDOWS[window][1]
+
+
 @pytest.mark.gpu
-@pytest.mark.parametrize("name", list(WINDOWS))
-def test_cuda_first_step_matches_dense_step(handle, oracle, name):
+@pytest.mark.parametrize("name", list(CUDA_CASES))
+def test_cuda_first_step_matches_dense_step(handle, oracle, driver, name):  # noqa: F811
     """the CUDA pass chain of one LM iteration without the oracle's solver: blocks from kba_eval, the step from the dense
-    reference, records 0 and 1 of kba_solve_window"""
-    win = WINDOWS[name]()
-    opt = handle.default_options()
-    ref = dense_first_step(win, opt, handle.evaluate(win), handle.evaluate, oracle)
-    _check_first_step(handle.solve_window(win, opt), ref, STEP_TOL, name)
+    reference, records 0 and 1 of kba_solve_batch -- of every window of a batch of copies -- on the solver path the window
+    selects (asserted here, in the same run)"""
+    window, _, copies, path = CUDA_CASES[name]
+    assert_path(driver, [build(window)[0]] * copies, dict(WINDOWS[window][3], **path))
+    ref, results, tol = cuda_first_step(handle, oracle, name)
+    for i, res in enumerate(results):
+        assert res.c.status == 0
+        _check_first_step(res, ref, TOL[tol], "%s, window %d" % (name, i))

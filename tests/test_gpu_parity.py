@@ -384,6 +384,23 @@ def test_fp32_linearisation_mode(handle, oracle):
         assert (rg.lm_rejected[:win.n_lm] != rc.lm_rejected[:win.n_lm]).mean() <= 0.005
 
 
+@pytest.mark.parametrize("precision", [0, 1])
+def test_eval_landmark_jacobian_is_the_one_the_fused_solve_forms(handle, precision):
+    """On the fused path J_l is not stored: the solve forms it in FP64 as (translation columns of J_p) R(keyframe), from the
+    FP32 J_p under precision 1.  kba_eval must report that matrix, not a copy rounded to FP32: tests/test_first_step_dense.py
+    builds the solve's normal equations from what kba_eval reports."""
+    from limo_b200 import capi
+    opt = capi.default_options()
+    opt.precision = precision
+    win = synth.make_window(2, n_kf=12, n_lm=400, n_obs=3000)
+    _, jp, jl, _, failed = handle.evaluate(win, opt)
+    R = np.stack([g.pose_to_iso(p)[:3, :3] for p in win.kf_pose])[win.obs_kf]
+    want = jp[:, :, 3:6] @ R
+    free = win.kf_fixed[win.obs_kf] == 0                    # a constant keyframe's J_p is reported as zeros
+    assert failed == 0 and free.sum() > 0.8 * win.n_obs
+    assert np.abs(jl[free] - want[free]).max() <= 1e-13 * np.abs(want).max()
+
+
 @pytest.mark.parametrize("case", ["ragged", "all_keyframes_fixed", "evaluation_failure", "tiny"])
 def test_edge_case_windows_match_oracle(handle, oracle, case):
     """ragged CSR rows (landmarks with zero / one observation), a window whose keyframes are all constant (no reduced

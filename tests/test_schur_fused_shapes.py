@@ -68,6 +68,7 @@ def _window(case):
         return _stereo_rig()
     # 30 free keyframes, but 187 rows over all 31 keyframes: the large-window path (k_schur_syrk) with KBA_FUSED=1 as with
     # KBA_FUSED=0, so this case compares that path with itself; the seven-slot variant needs 30 keyframes none of which is fixed
+    # (tests/test_first_step_dense.py holds its first step to the dense reference)
     return synth.make_window(2, n_kf=31, n_lm=700, n_obs=7000, seed=5)
 
 
