@@ -432,7 +432,7 @@ int kba_track_group_create(kba_handle* h, int32_t n_tracks, kba_track* const* tr
 void kba_track_group_destroy(kba_track_group* g);
 /* req[n_tracks], res[n_tracks] */
 int kba_track_group_solve(kba_track_group* g, const kba_track_request* req, const kba_options* opt, kba_result* res);
-/* upload / download of the last group solve, pose-only call or selection, counted as kba_track_transfer_bytes counts them */
+/* upload / download of the last group solve, pose-only call, selection or creation, counted as kba_track_transfer_bytes counts them */
 int kba_track_group_transfer_bytes(kba_track_group* g, int64_t* h2d_last_solve, int64_t* d2h_last_solve);
 
 /* ---- landmark selection for every track of a group in one launch sequence -------------------------------------------------
@@ -467,6 +467,61 @@ typedef struct kba_select_request {
 } kba_select_request;
 /* req[n_tracks], out[n_tracks] */
 int kba_track_group_select_landmarks(kba_track_group* g, const kba_select_request* req, kba_select_out* out);
+
+/* ---- landmark creation of push() on the stored window (SURVEY row A18) ------------------------------------------------
+ * What BundleAdjusterKeyframes::push() does for every landmark a pushed keyframe measures for the first time
+ * (bundle_adjuster_keyframes.cpp:289-382, facade/bundle_adjuster_keyframes.cpp), computed from what the store holds: keyframe
+ * poses, the measurement arena, the cameras.  The caller pushes the keyframe (kba_track_push_keyframe), then asks for its new
+ * landmarks here instead of keeping a host copy of the window to triangulate from.  A request:
+ *   - kf_slot [n_kf]: the active keyframes in ascending timestamp (= id) order, every one pushed, the new keyframe among them;
+ *   - kf_new: the index in kf_slot of the keyframe just pushed;
+ *   - lm_slot [n_new]: the landmarks it measures that do not exist yet (the caller keeps LandmarkId -> slot).
+ * Per requested landmark c, in request order:
+ *   - has depth (flags bit 1) iff an arena entry of kf_new for it has d >= 0 (containsDepth; a NaN depth is no depth).  Then the
+ *     first entry of kf_new for it in arena order that calculateLandmark(kf, id) does not skip (it skips d < 0 only, so a NaN
+ *     depth before the valid one is taken and the position is NaN, as on the host) is back-projected: x = (u - cx) z / f,
+ *     y = (v - cy) z / f, z = d, and pos = (cam * kf).inverse() * (x, y, z);
+ *   - else its rays, over the listed keyframes in list order and a keyframe's entries for it in arena order: each is
+ *     normalized(intrin_inv * (u, v, 1)) with pose (cam * kf).inverse(), intrin_inv the cofactor inverse of K.  With fewer than
+ *     two rays it is not created; else pos = triangulate_rays of the facade: sum (I - r r^T) inverted, times sum (I - r r^T) t.
+ *     Arena order within a keyframe must be the caller's camera-id order (Keyframe::cameras_), as for the select call's flow;
+ *   - created (flags bit 0): pos goes into the store's slot with weight 1 (Landmark::weight's default) and to out.pos[3c..3c+3);
+ *     a landmark that is not created leaves its store slot untouched and gets NaN in out.pos.
+ * Every double operation is the facade's host code's, in its order, without contraction: the positions equal the host push()'s
+ * bit for bit, and a degenerate triangulation (parallel rays) gives the host's inf or NaN.
+ * One upload (the lists), one launch sequence, one download; the first call allocates the buffers for the track's capacities,
+ * later calls allocate nothing.  kba_track_transfer_bytes then reports this call's upload and download: 4 * (n_kf + n_new) and
+ * 25 * n_new bytes.
+ * Errors, before anything is uploaded or written: a null pointer, n_kf < 1, n_new < 0, kf_new outside [0, n_kf), a slot out of
+ * range or listed twice, a keyframe slot not pushed: KBA_ERR_BAD_ARG; more keyframes or landmarks than the track has slots:
+ * KBA_ERR_CAPACITY.
+ * kba_track_group_create_landmarks does this for one request per track of a group in one launch sequence (window = request):
+ *   - out[i] and track i's store get exactly what kba_track_create_landmarks(tracks[i], &req[i], &out[i]) writes, bit for bit;
+ *   - a request with n_kf == 0 sits the call out: out[i] is not written, its store is untouched; a call in which every request
+ *     sits out returns at once (no upload, no launch);
+ *   - every other request is checked as the single call checks it before anything is uploaded; if one fails, the call returns
+ *     its code, kba_last_error names the track index, and no output or store is written;
+ *   - over the W requests that do not sit out, kba_track_group_transfer_bytes then reports
+ *         h2d = 4 * sum(n_kf + n_new) + R * (W - 1),   d2h = 25 * sum(n_new)
+ *     where R is the size of one window's argument record, a constant of the library build (the first window's record travels
+ *     in the launch parameters);
+ *   - memory: each track's creation scratch is shared by both entry points; the group adds its own staging, sized for its
+ *     tracks' capacities and allocated at its first call in which some request does not sit out. */
+typedef struct kba_create_request {
+    int32_t n_kf;               /* 0 (group call): this track sits the call out                                        */
+    int32_t kf_new;             /* index into kf_slot of the keyframe just pushed                                      */
+    int32_t n_new;
+    int32_t reserved_;
+    const int32_t* kf_slot;     /* [n_kf]  the active keyframes in ascending id order, every one pushed                */
+    const int32_t* lm_slot;     /* [n_new] the landmarks kf_new measures that do not exist yet                         */
+} kba_create_request;
+typedef struct kba_create_out {  /* caller-owned arrays */
+    double* pos;                /* [3 * n_new] created positions, NaN where not created                                */
+    uint8_t* flags;             /* [n_new] bit 0 created, bit 1 has depth                                              */
+} kba_create_out;
+int kba_track_create_landmarks(kba_track* t, const kba_create_request* req, kba_create_out* out);
+/* req[n_tracks], out[n_tracks] */
+int kba_track_group_create_landmarks(kba_track_group* g, const kba_create_request* req, kba_create_out* out);
 
 /* ---- adjustPoseOnly against the persistent store: one frame's pose per call, or one frame of each track of a group -------
  * What limo calls on every frame (bundle_adjuster_keyframes.cpp:820-888): one free pose against constant landmarks, the optional

@@ -9,7 +9,7 @@ import os
 
 import numpy as np
 
-from .capi_types import (KbaCounters, KbaEvalOut, KbaLidarOptions, KbaOptions, KbaResult, KbaSelectOut, KbaSelectParams, KbaSelectRequest,
+from .capi_types import (KbaCounters, KbaCreateOut, KbaCreateRequest, KbaEvalOut, KbaLidarOptions, KbaOptions, KbaResult, KbaSelectOut, KbaSelectParams, KbaSelectRequest,
                          KbaTrackCaps, KbaTrackFrame, KbaTrackRequest, KbaWindow, Result, Window, c_double_p, c_int32_p)
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
@@ -25,7 +25,8 @@ SYMBOLS = ["kba_version", "kba_last_error", "kba_default_options", "kba_create",
            "kba_init_landmarks", "kba_track_create", "kba_track_destroy", "kba_track_push_keyframe", "kba_track_drop_keyframe",
            "kba_track_set_landmarks", "kba_track_set_keyframe_pose", "kba_track_set_keyframe_poses", "kba_track_solve", "kba_track_transfer_bytes",
            "kba_track_group_create", "kba_track_group_destroy", "kba_track_group_solve", "kba_track_group_transfer_bytes",
-           "kba_track_adjust_pose", "kba_track_group_adjust_pose", "kba_track_select_landmarks", "kba_track_group_select_landmarks"]
+           "kba_track_adjust_pose", "kba_track_group_adjust_pose", "kba_track_select_landmarks", "kba_track_group_select_landmarks",
+           "kba_track_create_landmarks", "kba_track_group_create_landmarks"]
 
 
 class KbaError(RuntimeError):
@@ -100,6 +101,8 @@ def lib():
         L.kba_track_group_adjust_pose.argtypes = [vp, C.POINTER(KbaTrackFrame), C.POINTER(KbaOptions), C.POINTER(KbaResult)]
         L.kba_track_select_landmarks.argtypes = [vp, C.c_int32, ip, C.c_int32, ip, C.POINTER(KbaSelectParams), C.POINTER(KbaSelectOut)]
         L.kba_track_group_select_landmarks.argtypes = [vp, C.POINTER(KbaSelectRequest), C.POINTER(KbaSelectOut)]
+        L.kba_track_create_landmarks.argtypes = [vp, C.POINTER(KbaCreateRequest), C.POINTER(KbaCreateOut)]
+        L.kba_track_group_create_landmarks.argtypes = [vp, C.POINTER(KbaCreateRequest), C.POINTER(KbaCreateOut)]
         L.kba_lidar_default_options.argtypes = [C.POINTER(KbaLidarOptions)]
         L.kba_lidar_default_options.restype = None
         fp = C.POINTER(C.c_float)
@@ -312,6 +315,20 @@ class Track:
         out["near_order"] = out["near_order"][:int(n_near[0])].copy()
         return out
 
+    def create_landmarks(self, kf_slots, kf_new, lm_slots):
+        """push()'s landmark creation on this track's store (kba_track_create_landmarks): kf_slots the active keyframes in
+        ascending id order, kf_new the index in kf_slots of the keyframe just pushed, lm_slots the landmarks it measures that do
+        not exist yet.  Returns (pos [n, 3] float64, NaN where not created; flags [n] uint8: bit 0 created, bit 1 has depth);
+        created landmarks are written into the store with weight 1."""
+        kf, kfp = self._i32(kf_slots)
+        lm, lmp = self._i32(lm_slots)
+        n = len(lm)
+        pos, flags = np.zeros((n, 3), np.float64), np.zeros(n, np.uint8)
+        q = KbaCreateRequest(n_kf=len(kf), kf_new=int(kf_new), n_new=n, kf_slot=kfp, lm_slot=lmp)
+        o = KbaCreateOut(pos.ctypes.data_as(c_double_p), flags.ctypes.data_as(C.POINTER(C.c_uint8)))
+        _check(lib().kba_track_create_landmarks(self._p, C.byref(q), C.byref(o)))
+        return pos, flags
+
     def transfer_bytes(self):
         a, b, c = C.c_int64(), C.c_int64(), C.c_int64()
         _check(lib().kba_track_transfer_bytes(self._p, C.byref(a), C.byref(b), C.byref(c)))
@@ -424,8 +441,34 @@ class TrackGroup:
             results[i] = dict(cheiral=cheiral[a:b], bin=bins[a:b], near_order=near[a:a + int(n_near[i])], flow=flow[a:b], seen=seen[a:b])
         return results
 
+    def create_landmarks(self, requests):
+        """push()'s landmark creation for every track in one launch sequence (kba_track_group_create_landmarks): each entry None
+        (the track sits the call out) or a dict with the arguments of Track.create_landmarks (kf_slots, kf_new, lm_slots).
+        Returns one (pos, flags) per track as Track.create_landmarks returns it, None for a track that sat out."""
+        assert len(requests) == len(self.tracks)
+        n = len(requests)
+        reqs, outs = (KbaCreateRequest * n)(), (KbaCreateOut * n)()
+        keep, results = [], [None] * n
+        for i, r in enumerate(requests):
+            if r is None:
+                continue
+            extra = set(r) - {"kf_slots", "kf_new", "lm_slots"}
+            if extra:
+                raise TypeError("create_landmarks: request %d has unexpected keys %s" % (i, sorted(extra)))
+            kf, kfp = Track._i32(r["kf_slots"])
+            lm, lmp = Track._i32(r["lm_slots"])
+            if len(kf) == 0:  # n_kf = 0 would sit the track out: a request without keyframes is an error, as for one track
+                raise KbaError("kba_track_group_create_landmarks: track %d: no keyframes or a negative size" % i)
+            pos, flags = np.zeros((len(lm), 3), np.float64), np.zeros(len(lm), np.uint8)
+            reqs[i] = KbaCreateRequest(n_kf=len(kf), kf_new=int(r["kf_new"]), n_new=len(lm), kf_slot=kfp, lm_slot=lmp)
+            outs[i] = KbaCreateOut(pos.ctypes.data_as(c_double_p), flags.ctypes.data_as(C.POINTER(C.c_uint8)))
+            keep.append((kf, lm))
+            results[i] = (pos, flags)
+        _check(lib().kba_track_group_create_landmarks(self._p, reqs, outs))
+        return results
+
     def transfer_bytes(self):
-        """(host->device bytes, device->host bytes) of the last group solve, pose-only call or selection"""
+        """(host->device bytes, device->host bytes) of the last group solve, pose-only call, selection or creation"""
         a, b = C.c_int64(), C.c_int64()
         _check(lib().kba_track_group_transfer_bytes(self._p, C.byref(a), C.byref(b)))
         return a.value, b.value

@@ -56,6 +56,15 @@ class KbaSelectRequest(C.Structure):
                 ("params", C.POINTER(KbaSelectParams))]
 
 
+class KbaCreateRequest(C.Structure):
+    _fields_ = [("n_kf", C.c_int32), ("kf_new", C.c_int32), ("n_new", C.c_int32), ("reserved_", C.c_int32), ("kf_slot", c_int32_p),
+                ("lm_slot", c_int32_p)]
+
+
+class KbaCreateOut(C.Structure):
+    _fields_ = [("pos", c_double_p), ("flags", C.POINTER(C.c_uint8))]
+
+
 class KbaTrackFrame(C.Structure):
     _fields_ = [("n_meas", C.c_int32), ("reserved_", C.c_int32), ("pose7", c_double_p), ("lm_slot", c_int32_p), ("cam", c_int32_p),
                 ("u", c_float_p), ("v", c_float_p), ("d", c_float_p), ("speed_weight", C.c_double), ("speed_dt", C.c_double),

@@ -233,8 +233,9 @@ struct TrackSolver {
     }
 };
 
-// staging of a selection call (select_run): one pinned upload, argument records of windows 1 .. W-1 | the windows' lists, and one
-// download, the windows' outputs: flow | seen | near order (all windows' candidates end to end) | counters [W] | cheirality | bins
+// staging of a selection or creation call (select_run, create_run): one pinned upload, argument records of windows 1 .. W-1 | the
+// windows' lists, and one download of the windows' outputs (for a selection: flow | seen | near order (all windows' candidates end
+// to end) | counters [W] | cheirality | bins; for a creation: positions | flags)
 struct SelectStage {
     Staged<unsigned char> up, out;
     TrackSolver counts;                    // only h2d / d2h: what the transfer-bytes calls report after a selection
@@ -261,6 +262,24 @@ struct SelectBufs {
     }
 };
 
+// buffers of a track's landmark creations (kba_create.cu), kept like SelectBufs: scratch and the track's cameras on the device at
+// its first creation, alone or in a group; the staging at its first single call
+struct CreateBufs {
+    SelectStage stage;                     // kba_track_create_landmarks: keyframe slots | landmark slots, one window's outputs
+    CreateArgs a;                          // the scratch pointers; lists and outputs are set per call
+    std::vector<void*> dev;
+    std::vector<unsigned> kf_stamp, lm_stamp;  // duplicate checks: the call that named a slot last
+    unsigned stamp = 0;
+    template <typename T> int alloc(T** p, size_t n) {
+        void* q = nullptr;
+        if (cudaMalloc(&q, std::max<size_t>(n, 1) * sizeof(T)) != cudaSuccess) return 1;
+        dev.push_back(q); *p = (T*)q; return 0;
+    }
+    ~CreateBufs() {
+        for (void* p : dev) cudaFree(p);
+    }
+};
+
 // persistent, device-resident window (kba_track_*, at the end of this file)
 struct kba_track {
     kba_handle* h = nullptr;
@@ -270,6 +289,7 @@ struct kba_track {
     TrackSolver large;                     // win_rows > kFusedMaxRows: the same for windows of more rows, else no batch
     const TrackSolver* last = &solver;     // the solver of the last solve or pose-only call (transfer counts)
     std::unique_ptr<SelectBufs> select;    // kba_track_select_landmarks, allocated at its first call
+    std::unique_ptr<CreateBufs> create;    // kba_track_create_landmarks, allocated at its first call
     TrackDev td{};
     int* arena_i[2][2] = {{nullptr, nullptr}, {nullptr, nullptr}};      // [buffer][lm, cam]
     float* arena_f[2][3] = {{nullptr, nullptr, nullptr}, {nullptr, nullptr, nullptr}};  // [buffer][u, v, d]
@@ -302,6 +322,7 @@ struct kba_track_group {
     TrackSolver solver;                    // window i of its batch is track i's (fused path)
     TrackSolver large;                     // some track has win_rows > kFusedMaxRows: the whole group on the large-window path, else no batch
     std::unique_ptr<SelectStage> select;   // kba_track_group_select_landmarks, allocated at its first call
+    std::unique_ptr<SelectStage> create;   // kba_track_group_create_landmarks, allocated at its first call
     const TrackSolver* last = &solver;
 };
 
@@ -1393,6 +1414,7 @@ void kba_track_destroy(kba_track* t) {
     t->solver.release();
     t->large.release();
     t->select.reset();
+    t->create.reset();
     for (void* p : t->dev) cudaFree(p);
     t->p_lm.release(); t->p_cam.release(); t->lay.release();
     t->p_u.release(); t->p_v.release(); t->p_d.release(); t->p_dbl.release(); t->p_slot.release();
@@ -2118,6 +2140,190 @@ int kba_track_group_select_landmarks(kba_track_group* g, const kba_select_reques
     for (int i = 0; i < n; ++i)
         if (req[i].n_kf == 0) *out[i].n_near = 0;
     return rc;
+}
+
+// ---------------------------------------------------------------------------------------------------------------------
+// landmark creation of push() on the stored window (include/kba_b200.h, kba_track_create_landmarks /
+// kba_track_group_create_landmarks; kernels in kba_create.cu): a single call is a one-window call of create_run
+// ---------------------------------------------------------------------------------------------------------------------
+static int create_alloc(kba_track* t, std::string& why) {
+    std::unique_ptr<CreateBufs> cb(new CreateBufs());
+    const TrackDev& td = t->td;
+    const size_t L = (size_t)td.lm_cap, K = (size_t)td.kf_cap, NC = (size_t)t->n_cam;
+    CreateArgs& a = cb->a;
+    double* intr = nullptr, *pose = nullptr;
+    int bad = 0;
+    bad |= cb->alloc(&a.req_of, L); bad |= cb->alloc(&a.ray_T, 12 * K * NC); bad |= cb->alloc(&a.intr_inv, 9 * NC);
+    bad |= cb->alloc(&a.cnt, L); bad |= cb->alloc(&a.cursor, L); bad |= cb->alloc(&a.off, L); bad |= cb->alloc(&a.key, (size_t)td.m_cap);
+    bad |= cb->alloc(&a.total, 1); bad |= cb->alloc(&intr, 3 * NC); bad |= cb->alloc(&pose, 7 * NC);
+    if (bad) { why = "out of memory for the creation buffers"; return KBA_ERR_CUDA; }
+    cudaStream_t s = t->h->stream;
+    cudaError_t e = cudaMemsetAsync(a.req_of, 0xff, sizeof(int) * L, s);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(intr, t->cam_intr.data(), sizeof(double) * 3 * NC, cudaMemcpyHostToDevice, s);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(pose, t->cam_pose.data(), sizeof(double) * 7 * NC, cudaMemcpyHostToDevice, s);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(s);
+    if (e != cudaSuccess) { why = std::string("creation buffers: ") + cudaGetErrorString(e); return KBA_ERR_CUDA; }
+    a.cam_intr = intr; a.cam_pose7 = pose; a.n_cam = t->n_cam;
+    cb->kf_stamp.assign(K, 0); cb->lm_stamp.assign(L, 0);
+    t->create = std::move(cb);
+    return KBA_OK;
+}
+
+// one creation request of track t (one window of create_run)
+struct CreateReq {
+    kba_track* t = nullptr;
+    const kba_create_request* q = nullptr;
+    const kba_create_out* o = nullptr;
+    int max_meas = 0;                      // set by create_check: arena entries of the largest listed keyframe
+};
+
+// every check of one request, before anything is uploaded; allocates the track's creation buffers at its first creation
+static int create_check(CreateReq& r, std::string& why) {
+    kba_track* t = r.t;
+    const kba_create_request& q = *r.q;
+    if (!q.kf_slot || (q.n_new > 0 && (!q.lm_slot || !r.o->pos || !r.o->flags))) { why = "null argument"; return KBA_ERR_BAD_ARG; }
+    if (q.n_kf < 1 || q.n_new < 0) { why = "no keyframes or a negative size"; return KBA_ERR_BAD_ARG; }
+    if (q.n_kf > t->td.kf_cap || q.n_new > t->td.lm_cap) { why = "more keyframes or landmarks than the track's slots"; return KBA_ERR_CAPACITY; }
+    if (q.kf_new < 0 || q.kf_new >= q.n_kf) { why = "kf_new outside [0, n_kf)"; return KBA_ERR_BAD_ARG; }
+    const cudaError_t e = cudaSetDevice(t->h->device);
+    if (e != cudaSuccess) { why = std::string("cudaSetDevice: ") + cudaGetErrorString(e); return KBA_ERR_CUDA; }
+    if (!t->create) { const int rc = create_alloc(t, why); if (rc != KBA_OK) return rc; }
+    CreateBufs& cb = *t->create;
+    if (++cb.stamp == 0) {  // the stamps wrapped: start over
+        std::fill(cb.kf_stamp.begin(), cb.kf_stamp.end(), 0u); std::fill(cb.lm_stamp.begin(), cb.lm_stamp.end(), 0u); cb.stamp = 1;
+    }
+    r.max_meas = 0;
+    for (int k = 0; k < q.n_kf; ++k) {
+        const int s = q.kf_slot[k];
+        if (s < 0 || s >= t->td.kf_cap || !t->kf_live[s]) { why = "keyframe slot not pushed"; return KBA_ERR_BAD_ARG; }
+        if (cb.kf_stamp[s] == cb.stamp) { why = "keyframe slot listed twice"; return KBA_ERR_BAD_ARG; }
+        cb.kf_stamp[s] = cb.stamp;
+        r.max_meas = std::max(r.max_meas, t->m_cnt[s]);
+    }
+    for (int c = 0; c < q.n_new; ++c) {
+        const int s = q.lm_slot[c];
+        if (s < 0 || s >= t->td.lm_cap) { why = "landmark slot out of range"; return KBA_ERR_BAD_ARG; }
+        if (cb.lm_stamp[s] == cb.stamp) { why = "landmark slot listed twice"; return KBA_ERR_BAD_ARG; }
+        cb.lm_stamp[s] = cb.stamp;
+    }
+    return KBA_OK;
+}
+
+// W checked requests of distinct tracks as the W windows of one launch sequence: one upload (the argument records of windows
+// 1 .. W-1, then every window's lists), one download (positions of all windows | their flags), one synchronisation, then the
+// scatter into the callers' arrays.  Window 0's record travels in the launch parameters (kba_create.cu).
+static int create_run(kba_handle* h, SelectStage& st, int W, const CreateReq* r) {
+    CU(cudaSetDevice(h->device));
+    cudaStream_t s = h->stream;
+    CreateGrid g;
+    size_t n_list = 0, N = 0;
+    for (int w = 0; w < W; ++w) {
+        const kba_create_request& q = *r[w].q;
+        n_list += (size_t)q.n_kf + q.n_new; N += (size_t)q.n_new;
+        g.max_kf = std::max(g.max_kf, q.n_kf); g.max_new = std::max(g.max_new, q.n_new);
+        g.max_init = std::max(g.max_init, std::max(q.n_new, q.n_kf * r[w].t->n_cam));
+        g.max_meas = std::max(g.max_meas, r[w].max_meas);
+    }
+    const size_t o_lists = sizeof(CreateArgs) * (size_t)(W - 1), up_bytes = o_lists + 4 * n_list;
+    const size_t o_flags = 24 * N, out_bytes = o_flags + N;
+    int* lists_h = reinterpret_cast<int*>(st.up.h + o_lists);
+    const int* lists_d = reinterpret_cast<const int*>(st.up.d + o_lists);
+    unsigned char* d = st.out.d;
+    CreateLaunch l;
+    l.rest = reinterpret_cast<const CreateArgs*>(st.up.d);
+    l.n_win = W;
+    size_t li = 0, c0 = 0;
+    for (int w = 0; w < W; ++w) {
+        const kba_create_request& q = *r[w].q;
+        memcpy(lists_h + li, q.kf_slot, 4 * (size_t)q.n_kf);
+        if (q.n_new) memcpy(lists_h + li + q.n_kf, q.lm_slot, 4 * (size_t)q.n_new);
+        CreateArgs a = r[w].t->create->a;
+        a.td = r[w].t->td;
+        a.kf_slot = lists_d + li; a.lm_slot = lists_d + li + q.n_kf;
+        a.n_kf = q.n_kf; a.kf_new = q.kf_new; a.n_new = q.n_new;
+        a.pos = reinterpret_cast<double*>(d + 24 * c0); a.flags = d + o_flags + c0;
+        if (w == 0) l.w0 = a;
+        else memcpy(st.up.h + sizeof(CreateArgs) * (size_t)(w - 1), &a, sizeof(CreateArgs));
+        li += (size_t)q.n_kf + q.n_new; c0 += (size_t)q.n_new;
+    }
+    CU(cudaMemcpyAsync(st.up.d, st.up.h, up_bytes, cudaMemcpyHostToDevice, s));
+    launch_create(l, g, s);
+    cudaError_t e = cudaGetLastError();
+    if (e == cudaSuccess) e = cudaMemcpyAsync(st.out.h, st.out.d, out_bytes, cudaMemcpyDeviceToHost, s);
+    if (e == cudaSuccess) e = wait_stream(h);
+    if (e != cudaSuccess) {
+        // k_cr_init fills each window's slot -> request map and only k_cr_land clears it: after a failed launch sequence the maps
+        // are cleared here, so that no later call reads this call's request indices (a sticky error leaves the context unusable
+        // anyway, and these calls then fail as well)
+        for (int w = 0; w < W; ++w) cudaMemsetAsync(r[w].t->create->a.req_of, 0xff, sizeof(int) * (size_t)r[w].t->td.lm_cap, s);
+        cudaStreamSynchronize(s);
+        return fail(KBA_ERR_CUDA, std::string("landmark creation: ") + cudaGetErrorString(e));
+    }
+    const unsigned char* hb = st.out.h;
+    c0 = 0;
+    for (int w = 0; w < W; ++w) {
+        const size_t n = (size_t)r[w].q->n_new;
+        if (n) { memcpy(r[w].o->pos, hb + 24 * c0, 24 * n); memcpy(r[w].o->flags, hb + o_flags + c0, n); }
+        c0 += n;
+    }
+    st.counts.h2d = (int64_t)up_bytes;
+    st.counts.d2h = (int64_t)out_bytes;
+    return KBA_OK;
+}
+
+int kba_track_create_landmarks(kba_track* t, const kba_create_request* req, kba_create_out* out) {
+    static const std::string who = "kba_track_create_landmarks: ";
+    if (!t || !req || !out) return fail(KBA_ERR_BAD_ARG, who + "null argument");
+    CreateReq r;
+    r.t = t; r.q = req; r.o = out;
+    std::string why;
+    int rc = create_check(r, why);
+    if (rc != KBA_OK) return fail(rc, who + why);
+    SelectStage& st = t->create->stage;
+    if (!st.up.d) {  // the first single call of the track
+        const size_t K = (size_t)t->td.kf_cap, L = (size_t)t->td.lm_cap;
+        if (st.alloc(4 * (K + L), 25 * L)) {
+            st.up.release(); st.out.release();
+            return fail(KBA_ERR_CUDA, who + "out of memory for the creation staging");
+        }
+    }
+    rc = create_run(t->h, st, 1, &r);
+    if (rc == KBA_OK) t->last = &t->create->stage.counts;
+    return rc;
+}
+
+int kba_track_group_create_landmarks(kba_track_group* g, const kba_create_request* req, kba_create_out* out) {
+    static const std::string who = "kba_track_group_create_landmarks: ";
+    if (!g || !req || !out) return fail(KBA_ERR_BAD_ARG, who + "null argument");
+    const int n = (int)g->tracks.size();
+    // ---- every request is checked before anything is uploaded or written
+    std::vector<CreateReq> rs;
+    for (int i = 0; i < n; ++i) {
+        if (req[i].n_kf == 0) continue;  // sits the call out
+        CreateReq r;
+        r.t = g->tracks[i]; r.q = &req[i]; r.o = &out[i];
+        std::string why;
+        const int rc = create_check(r, why);
+        if (rc != KBA_OK) return fail(rc, who + "track " + std::to_string(i) + ": " + why);
+        rs.push_back(r);
+    }
+    if (rs.empty()) {  // every track sits out: no upload, no launch
+        g->solver.h2d = 0; g->solver.d2h = 0;
+        g->last = &g->solver;
+        return KBA_OK;
+    }
+    if (!g->create) {  // staging for every track at its capacities, allocated once
+        size_t lists = 0, lms = 0;
+        for (const kba_track* t : g->tracks) { lists += (size_t)t->td.kf_cap + t->td.lm_cap; lms += (size_t)t->td.lm_cap; }
+        std::unique_ptr<SelectStage> st(new SelectStage());
+        if (st->alloc(sizeof(CreateArgs) * (size_t)(n - 1) + 4 * lists, 25 * lms))
+            return fail(KBA_ERR_CUDA, who + "out of memory for the creation staging");
+        g->create = std::move(st);
+    }
+    const int rc = create_run(g->h, *g->create, (int)rs.size(), rs.data());
+    if (rc != KBA_OK) return rc;
+    g->last = &g->create->counts;
+    return KBA_OK;
 }
 
 // ---------------------------------------------------------------------------------------------------------------------

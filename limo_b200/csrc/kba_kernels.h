@@ -154,6 +154,41 @@ struct SelectGrid {
 };
 void launch_select(const SelectLaunch& l, const SelectGrid& g, cudaStream_t s);
 
+// ---- landmark creation of push() on a track's store (kba_track_create_landmarks / kba_track_group_create_landmarks, kba_create.cu) ----
+// One window = one request: the active keyframe slots (ascending id, kf_new the one just pushed) and the slots of the landmarks to
+// create.  Scratch is the track's, sized for its capacities at its first creation; the outputs point into one device block.
+struct CreateArgs {
+    TrackDev td;
+    const int* kf_slot = nullptr;     // [n_kf]
+    const int* lm_slot = nullptr;     // [n_new]
+    const double* cam_intr = nullptr; // [n_cam * 3] the track's cameras: f, cx, cy
+    const double* cam_pose7 = nullptr;// [n_cam * 7]
+    int n_kf = 0, kf_new = 0, n_new = 0, n_cam = 0;
+    // scratch
+    int* req_of = nullptr;            // [lm_cap] slot -> request index, all -1 between calls
+    double* ray_T = nullptr;          // [kf_cap * n_cam * 12] (cam * kf).inverse() of every listed keyframe and camera
+    double* intr_inv = nullptr;       // [n_cam * 9] Camera::intrin_inv
+    int* cnt = nullptr;               // [lm_cap] arena entries per request
+    int* cursor = nullptr;            // [lm_cap]
+    int* off = nullptr;               // [lm_cap] first key of a request's entries
+    long long* key = nullptr;         // [m_cap] (keyframe position, arena index) of every gathered entry
+    int* total = nullptr;             // [1] gathered entries
+    // outputs [n_new]
+    double* pos = nullptr;            // [3 * n_new]
+    unsigned char* flags = nullptr;
+};
+// W windows in one launch sequence, window = grid z; window 0's arguments travel in the launch parameters (as SelectLaunch)
+struct CreateLaunch {
+    CreateArgs w0;
+    const CreateArgs* rest = nullptr;  // [n_win - 1]
+    int n_win = 0;
+};
+struct CreateGrid {
+    int max_kf = 0, max_new = 0, max_init = 0;  // max_init: of max(n_new, n_kf * n_cam)
+    int max_meas = 0;                           // arena entries of a listed keyframe
+};
+void launch_create(const CreateLaunch& l, const CreateGrid& g, cudaStream_t s);
+
 // ---- motion-only frames against a track's store (kba_track_adjust_pose / kba_track_group_adjust_pose, kba_motion.cu) ----
 // One frame = one free pose against constant landmarks read from a store by slot: its measurements come in runs, one run per
 // landmark (the landmarks of the equivalent window, in the caller's order).
