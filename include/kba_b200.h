@@ -432,7 +432,7 @@ int kba_track_group_create(kba_handle* h, int32_t n_tracks, kba_track* const* tr
 void kba_track_group_destroy(kba_track_group* g);
 /* req[n_tracks], res[n_tracks] */
 int kba_track_group_solve(kba_track_group* g, const kba_track_request* req, const kba_options* opt, kba_result* res);
-/* upload / download of the last group solve, pose-only call, selection or creation, counted as kba_track_transfer_bytes counts them */
+/* upload / download of the last group solve, pose-only call, selection, creation or upkeep call, counted as kba_track_transfer_bytes counts them */
 int kba_track_group_transfer_bytes(kba_track_group* g, int64_t* h2d_last_solve, int64_t* d2h_last_solve);
 
 /* ---- landmark selection for every track of a group in one launch sequence -------------------------------------------------
@@ -522,6 +522,81 @@ typedef struct kba_create_out {  /* caller-owned arrays */
 int kba_track_create_landmarks(kba_track* t, const kba_create_request* req, kba_create_out* out);
 /* req[n_tracks], out[n_tracks] */
 int kba_track_group_create_landmarks(kba_track_group* g, const kba_create_request* req, kba_create_out* out);
+
+/* ---- window upkeep on the stored window: deactivateKeyframes and the AddDepth scheme's costs ------------------------------
+ * The two steps of limo's keyframe step that read every active keyframe's measurements, computed from what the store holds, so
+ * that a track (group) user keeps no host copy of the window's measurements.  Both take the slot contract of the select and
+ * create calls: a keyframe's arena entries come in landmark-id order (one run per landmark), so the distinct landmarks of a
+ * keyframe are the first entries of its runs; the caller keeps LandmarkId -> slot.  Everything else is as for the create call:
+ *   - one upload (the lists), one launch sequence, one download, one synchronisation per call; the first call of a track by
+ *     either entry point allocates its upkeep scratch, its first single call its staging, later calls allocate nothing;
+ *   - every request is checked before anything is uploaded or written; null pointers, n_kf < 1, a negative size, a keyframe
+ *     slot not pushed or listed twice, a landmark slot out of range or listed twice: KBA_ERR_BAD_ARG; more keyframes or
+ *     landmarks than the track has slots: KBA_ERR_CAPACITY;
+ *   - the group forms serve one request per track in one launch sequence (window = request): out[i] is bit for bit what the
+ *     single call writes for req[i]; a request with n_kf == 0 sits the call out (out[i] not written; a call in which every
+ *     request sits out returns at once); a failing request returns its code, kba_last_error names its track, nothing is written;
+ *   - memory: a track's upkeep scratch is shared by both entry points; a group adds its own staging, sized for its tracks'
+ *     capacities and allocated at its first call in which some request does not sit out.
+ *
+ * kba_track_deactivate_keyframes: BundleAdjusterKeyframes::deactivateKeyframes(min_connecting, min_window, max_window)
+ * (bundle_adjuster_keyframes.cpp:907-987).  A request:
+ *   - kf_slot [n_kf]: the active keyframes in ascending id order, every one pushed; the last one is the newest;
+ *   - lm_slot [n_lm]: the active landmarks (active_landmark_ids_; a slot never created is allowed), any order.
+ * Outputs, all integer arithmetic, so exactly the facade's:
+ *   - kf_common[k]: the number of distinct landmark slots of keyframe k's arena entries that the newest keyframe's entries
+ *     also name (getCommonLandmarkIds: all of its measurements, not only active landmarks), for every k;
+ *   - kf_active[k] with n = n_kf - 1 - k: 0 if n > max_window - 1, else 1 if n < min_window - 1, else kf_common[k] > min_connecting;
+ *   - lm_active[j]: 1 iff landmark j is measured by some keyframe with kf_active = 1 (the new active_landmark_ids_).
+ * The caller still fixes the two oldest survivors.  Transfers (kba_track_transfer_bytes; over the W requests that do not sit out
+ * for kba_track_group_transfer_bytes, R the size of one window's argument record, a constant of the library build):
+ *         h2d = 4 * sum(n_kf + n_lm) + R * (W - 1),   d2h = sum(5 * n_kf + n_lm)
+ *
+ * kba_track_depth_costs: the quantities of LandmarkSelectionSchemeAddDepth::getSelection (landmark_selection_scheme_add_depth.cpp:
+ * 16-75) with limo's sorter (mono_lidar.cpp:418-429: float(local.norm())).  A request:
+ *   - kf_slot [n_kf]: the active keyframes in ascending id order (the scheme's FrameIndex i is kf_slot[i], 0 the oldest);
+ *   - lm_slot [n_elig]: the eligible landmarks in ascending id order (non_rejected ∩ comparator; for limo is_ground_plane);
+ *   - cap: the capacity of out.cand / out.cost; below B = sum over k of min(n_elig, arena entries of kf_slot[k]): KBA_ERR_CAPACITY.
+ * Outputs: for every keyframe k, the pairs (cand, cost) of the eligible landmarks k measures at off[k] .. off[k + 1), in arena
+ * order (ascending id: the order of the host's cost vector); cand is the index into lm_slot, cost the host's value bit for bit:
+ * worst = -DBL_MAX folded by std::max(worst, double(float(|kf * pos|))) over the keyframe's entries of that landmark -- a NaN
+ * norm (a landmark created from a NaN depth has a NaN position) leaves -DBL_MAX.  The caller then runs the facade's
+ * std::partial_sort over each off[ind] .. off[ind + 1) for its (ind, wanted) entries and gets the scheme's selection bit for
+ * bit, ties and -DBL_MAX included.  Transfers (as above, B_w the bound of request w):
+ *         h2d = 4 * sum(n_kf + n_elig) + R * (W - 1),   d2h = sum(4 * n_kf + 12 * B_w) */
+typedef struct kba_deactivate_request {
+    int32_t n_kf;               /* 0 (group call): this track sits the call out                                        */
+    int32_t n_lm;
+    int32_t min_connecting, min_window, max_window;
+    int32_t reserved_;
+    const int32_t* kf_slot;     /* [n_kf] the active keyframes in ascending id order; the last one is the newest         */
+    const int32_t* lm_slot;     /* [n_lm] the active landmarks                                                          */
+} kba_deactivate_request;
+typedef struct kba_deactivate_out {  /* caller-owned arrays */
+    uint8_t* kf_active;         /* [n_kf] */
+    int32_t* kf_common;         /* [n_kf] */
+    uint8_t* lm_active;         /* [n_lm] */
+} kba_deactivate_out;
+int kba_track_deactivate_keyframes(kba_track* t, const kba_deactivate_request* req, kba_deactivate_out* out);
+/* req[n_tracks], out[n_tracks] */
+int kba_track_group_deactivate_keyframes(kba_track_group* g, const kba_deactivate_request* req, kba_deactivate_out* out);
+
+typedef struct kba_depth_request {
+    int32_t n_kf;               /* 0 (group call): this track sits the call out                                        */
+    int32_t n_elig;
+    int32_t cap;                /* entries of out.cand / out.cost                                                        */
+    int32_t reserved_;
+    const int32_t* kf_slot;     /* [n_kf] the active keyframes in ascending id order                                    */
+    const int32_t* lm_slot;     /* [n_elig] the eligible landmarks in ascending id order                                */
+} kba_depth_request;
+typedef struct kba_depth_out {  /* caller-owned arrays */
+    int32_t* off;               /* [n_kf + 1] keyframe k's pairs are off[k] .. off[k + 1)                                */
+    int32_t* cand;              /* [cap] index into lm_slot                                                             */
+    double* cost;               /* [cap] */
+} kba_depth_out;
+int kba_track_depth_costs(kba_track* t, const kba_depth_request* req, kba_depth_out* out);
+/* req[n_tracks], out[n_tracks] */
+int kba_track_group_depth_costs(kba_track_group* g, const kba_depth_request* req, kba_depth_out* out);
 
 /* ---- adjustPoseOnly against the persistent store: one frame's pose per call, or one frame of each track of a group -------
  * What limo calls on every frame (bundle_adjuster_keyframes.cpp:820-888): one free pose against constant landmarks, the optional

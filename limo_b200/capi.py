@@ -9,7 +9,7 @@ import os
 
 import numpy as np
 
-from .capi_types import (KbaCounters, KbaCreateOut, KbaCreateRequest, KbaEvalOut, KbaLidarOptions, KbaOptions, KbaResult, KbaSelectOut, KbaSelectParams, KbaSelectRequest,
+from .capi_types import (KbaCounters, KbaCreateOut, KbaCreateRequest, KbaDeactivateOut, KbaDeactivateRequest, KbaDepthOut, KbaDepthRequest, KbaEvalOut, KbaLidarOptions, KbaOptions, KbaResult, KbaSelectOut, KbaSelectParams, KbaSelectRequest,
                          KbaTrackCaps, KbaTrackFrame, KbaTrackRequest, KbaWindow, Result, Window, c_double_p, c_int32_p)
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
@@ -26,7 +26,8 @@ SYMBOLS = ["kba_version", "kba_last_error", "kba_default_options", "kba_create",
            "kba_track_set_landmarks", "kba_track_set_keyframe_pose", "kba_track_set_keyframe_poses", "kba_track_solve", "kba_track_transfer_bytes",
            "kba_track_group_create", "kba_track_group_destroy", "kba_track_group_solve", "kba_track_group_transfer_bytes",
            "kba_track_adjust_pose", "kba_track_group_adjust_pose", "kba_track_select_landmarks", "kba_track_group_select_landmarks",
-           "kba_track_create_landmarks", "kba_track_group_create_landmarks"]
+           "kba_track_create_landmarks", "kba_track_group_create_landmarks", "kba_track_deactivate_keyframes",
+           "kba_track_group_deactivate_keyframes", "kba_track_depth_costs", "kba_track_group_depth_costs"]
 
 
 class KbaError(RuntimeError):
@@ -103,6 +104,10 @@ def lib():
         L.kba_track_group_select_landmarks.argtypes = [vp, C.POINTER(KbaSelectRequest), C.POINTER(KbaSelectOut)]
         L.kba_track_create_landmarks.argtypes = [vp, C.POINTER(KbaCreateRequest), C.POINTER(KbaCreateOut)]
         L.kba_track_group_create_landmarks.argtypes = [vp, C.POINTER(KbaCreateRequest), C.POINTER(KbaCreateOut)]
+        L.kba_track_deactivate_keyframes.argtypes = [vp, C.POINTER(KbaDeactivateRequest), C.POINTER(KbaDeactivateOut)]
+        L.kba_track_group_deactivate_keyframes.argtypes = [vp, C.POINTER(KbaDeactivateRequest), C.POINTER(KbaDeactivateOut)]
+        L.kba_track_depth_costs.argtypes = [vp, C.POINTER(KbaDepthRequest), C.POINTER(KbaDepthOut)]
+        L.kba_track_group_depth_costs.argtypes = [vp, C.POINTER(KbaDepthRequest), C.POINTER(KbaDepthOut)]
         L.kba_lidar_default_options.argtypes = [C.POINTER(KbaLidarOptions)]
         L.kba_lidar_default_options.restype = None
         fp = C.POINTER(C.c_float)
@@ -329,6 +334,44 @@ class Track:
         _check(lib().kba_track_create_landmarks(self._p, C.byref(q), C.byref(o)))
         return pos, flags
 
+    @staticmethod
+    def _deactivate_args(kf_slots, lm_slots, min_connecting=3, min_window=4, max_window=20):
+        kf, kfp = Track._i32(kf_slots)
+        lm, lmp = Track._i32(lm_slots)
+        res = (np.zeros(len(kf), np.uint8), np.zeros(len(kf), np.int32), np.zeros(len(lm), np.uint8))
+        q = KbaDeactivateRequest(n_kf=len(kf), n_lm=len(lm), min_connecting=int(min_connecting), min_window=int(min_window),
+                                 max_window=int(max_window), kf_slot=kfp, lm_slot=lmp)
+        o = KbaDeactivateOut(res[0].ctypes.data_as(C.POINTER(C.c_uint8)), res[1].ctypes.data_as(C.POINTER(C.c_int32)),
+                             res[2].ctypes.data_as(C.POINTER(C.c_uint8)))
+        return q, o, res, (kf, lm)
+
+    def deactivate_keyframes(self, kf_slots, lm_slots, min_connecting=3, min_window=4, max_window=20):
+        """deactivateKeyframes() on this track's store (kba_track_deactivate_keyframes): kf_slots the active keyframes in ascending
+        id order (the last one the newest), lm_slots the active landmarks.  Returns (kf_active [n_kf] uint8, kf_common [n_kf] int32:
+        distinct landmarks shared with the newest keyframe, lm_active [n_lm] uint8: measured by a keyframe that stays active)."""
+        q, o, res, _keep = self._deactivate_args(kf_slots, lm_slots, min_connecting, min_window, max_window)
+        _check(lib().kba_track_deactivate_keyframes(self._p, C.byref(q), C.byref(o)))
+        return res
+
+    @staticmethod
+    def _depth_args(kf_slots, lm_slots, cap=None):
+        kf, kfp = Track._i32(kf_slots)
+        lm, lmp = Track._i32(lm_slots)
+        cap = min(len(kf) * len(lm), 2**31 - 1) if cap is None else int(cap)  # len(kf) * len(lm) bounds the pairs
+        off, cand, cost = np.zeros(len(kf) + 1, np.int32), np.zeros(max(cap, 0), np.int32), np.zeros(max(cap, 0), np.float64)
+        q = KbaDepthRequest(n_kf=len(kf), n_elig=len(lm), cap=cap, kf_slot=kfp, lm_slot=lmp)
+        o = KbaDepthOut(off.ctypes.data_as(C.POINTER(C.c_int32)), cand.ctypes.data_as(C.POINTER(C.c_int32)), cost.ctypes.data_as(c_double_p))
+        return q, o, (off, cand, cost), (kf, lm)
+
+    def depth_costs(self, kf_slots, lm_slots, cap=None):
+        """The AddDepth scheme's costs on this track's store (kba_track_depth_costs) for limo's sorter: kf_slots the active keyframes
+        in ascending id order (FrameIndex i = kf_slots[i]), lm_slots the eligible landmarks in ascending id order.  Returns (off
+        [n_kf + 1], cand, cost): keyframe k's eligible landmarks (indices into lm_slots, arena order) and costs at off[k] ..
+        off[k + 1).  cap: output capacity (default n_kf * n_elig)."""
+        q, o, (off, cand, cost), _keep = self._depth_args(kf_slots, lm_slots, cap)
+        _check(lib().kba_track_depth_costs(self._p, C.byref(q), C.byref(o)))
+        return off, cand[:off[-1]].copy(), cost[:off[-1]].copy()
+
     def transfer_bytes(self):
         a, b, c = C.c_int64(), C.c_int64(), C.c_int64()
         _check(lib().kba_track_transfer_bytes(self._p, C.byref(a), C.byref(b), C.byref(c)))
@@ -467,8 +510,42 @@ class TrackGroup:
         _check(lib().kba_track_group_create_landmarks(self._p, reqs, outs))
         return results
 
+    def _upkeep(self, requests, keys, args, Req, Out, fn):
+        assert len(requests) == len(self.tracks)
+        n = len(requests)
+        reqs, outs = (Req * n)(), (Out * n)()
+        keep, results = [], [None] * n
+        for i, r in enumerate(requests):
+            if r is None:
+                continue
+            extra = set(r) - keys
+            if extra:
+                raise TypeError("request %d has unexpected keys %s" % (i, sorted(extra)))
+            q, o, res, lists = args(**r)
+            if q.n_kf == 0:  # n_kf = 0 would sit the track out: a request without keyframes is an error, as for one track
+                raise KbaError("%s: track %d: no keyframes or a negative size" % (fn, i))
+            reqs[i], outs[i] = q, o
+            keep.append(lists)
+            results[i] = res
+        _check(getattr(lib(), fn)(self._p, reqs, outs))
+        return results
+
+    def deactivate_keyframes(self, requests):
+        """deactivateKeyframes() for every track in one launch sequence (kba_track_group_deactivate_keyframes): each entry None (the
+        track sits the call out) or a dict with the arguments of Track.deactivate_keyframes.  Returns one (kf_active, kf_common,
+        lm_active) per track, None for a track that sat out."""
+        return self._upkeep(requests, {"kf_slots", "lm_slots", "min_connecting", "min_window", "max_window"}, Track._deactivate_args,
+                            KbaDeactivateRequest, KbaDeactivateOut, "kba_track_group_deactivate_keyframes")
+
+    def depth_costs(self, requests):
+        """The AddDepth costs for every track in one launch sequence (kba_track_group_depth_costs): each entry None or a dict with
+        the arguments of Track.depth_costs.  Returns one (off, cand, cost) per track, None for a track that sat out."""
+        res = self._upkeep(requests, {"kf_slots", "lm_slots", "cap"}, Track._depth_args, KbaDepthRequest, KbaDepthOut,
+                           "kba_track_group_depth_costs")
+        return [None if r is None else (r[0], r[1][:r[0][-1]].copy(), r[2][:r[0][-1]].copy()) for r in res]
+
     def transfer_bytes(self):
-        """(host->device bytes, device->host bytes) of the last group solve, pose-only call, selection or creation"""
+        """(host->device bytes, device->host bytes) of the last group solve, pose-only call, selection, creation or upkeep call"""
         a, b = C.c_int64(), C.c_int64()
         _check(lib().kba_track_group_transfer_bytes(self._p, C.byref(a), C.byref(b)))
         return a.value, b.value

@@ -65,6 +65,24 @@ class KbaCreateOut(C.Structure):
     _fields_ = [("pos", c_double_p), ("flags", C.POINTER(C.c_uint8))]
 
 
+class KbaDeactivateRequest(C.Structure):
+    _fields_ = [("n_kf", C.c_int32), ("n_lm", C.c_int32), ("min_connecting", C.c_int32), ("min_window", C.c_int32),
+                ("max_window", C.c_int32), ("reserved_", C.c_int32), ("kf_slot", c_int32_p), ("lm_slot", c_int32_p)]
+
+
+class KbaDeactivateOut(C.Structure):
+    _fields_ = [("kf_active", C.POINTER(C.c_uint8)), ("kf_common", c_int32_p), ("lm_active", C.POINTER(C.c_uint8))]
+
+
+class KbaDepthRequest(C.Structure):
+    _fields_ = [("n_kf", C.c_int32), ("n_elig", C.c_int32), ("cap", C.c_int32), ("reserved_", C.c_int32), ("kf_slot", c_int32_p),
+                ("lm_slot", c_int32_p)]
+
+
+class KbaDepthOut(C.Structure):
+    _fields_ = [("off", c_int32_p), ("cand", c_int32_p), ("cost", c_double_p)]
+
+
 class KbaTrackFrame(C.Structure):
     _fields_ = [("n_meas", C.c_int32), ("reserved_", C.c_int32), ("pose7", c_double_p), ("lm_slot", c_int32_p), ("cam", c_int32_p),
                 ("u", c_float_p), ("v", c_float_p), ("d", c_float_p), ("speed_weight", C.c_double), ("speed_dt", C.c_double),

@@ -280,6 +280,19 @@ struct CreateBufs {
     }
 };
 
+// buffers of a track's upkeep calls (kba_upkeep.cu), kept like CreateBufs: the stamped slot map at its first upkeep call, alone or
+// in a group; the staging at its first single call
+struct UpkeepBufs {
+    SelectStage stage;                     // the single calls: keyframe slots | landmark slots, one window's outputs
+    unsigned long long* map = nullptr;     // [lm_cap] (stamp << 32) | payload by slot, all 0 (stamp 0: never a call's) at first
+    unsigned stamp = 0;                    // the last stamp a call used
+    std::vector<unsigned> kf_stamp, lm_stamp;  // duplicate checks: the check that named a slot last
+    unsigned check = 0;
+    ~UpkeepBufs() {
+        if (map) cudaFree(map);
+    }
+};
+
 // persistent, device-resident window (kba_track_*, at the end of this file)
 struct kba_track {
     kba_handle* h = nullptr;
@@ -290,6 +303,7 @@ struct kba_track {
     const TrackSolver* last = &solver;     // the solver of the last solve or pose-only call (transfer counts)
     std::unique_ptr<SelectBufs> select;    // kba_track_select_landmarks, allocated at its first call
     std::unique_ptr<CreateBufs> create;    // kba_track_create_landmarks, allocated at its first call
+    std::unique_ptr<UpkeepBufs> upkeep;    // kba_track_deactivate_keyframes / kba_track_depth_costs, allocated at the first of them
     TrackDev td{};
     int* arena_i[2][2] = {{nullptr, nullptr}, {nullptr, nullptr}};      // [buffer][lm, cam]
     float* arena_f[2][3] = {{nullptr, nullptr, nullptr}, {nullptr, nullptr, nullptr}};  // [buffer][u, v, d]
@@ -323,6 +337,7 @@ struct kba_track_group {
     TrackSolver large;                     // some track has win_rows > kFusedMaxRows: the whole group on the large-window path, else no batch
     std::unique_ptr<SelectStage> select;   // kba_track_group_select_landmarks, allocated at its first call
     std::unique_ptr<SelectStage> create;   // kba_track_group_create_landmarks, allocated at its first call
+    std::unique_ptr<SelectStage> upkeep;   // kba_track_group_deactivate_keyframes / _depth_costs, allocated at the first of them
     const TrackSolver* last = &solver;
 };
 
@@ -1415,6 +1430,7 @@ void kba_track_destroy(kba_track* t) {
     t->large.release();
     t->select.reset();
     t->create.reset();
+    t->upkeep.reset();
     for (void* p : t->dev) cudaFree(p);
     t->p_lm.release(); t->p_cam.release(); t->lay.release();
     t->p_u.release(); t->p_v.release(); t->p_d.release(); t->p_dbl.release(); t->p_slot.release();
@@ -2324,6 +2340,262 @@ int kba_track_group_create_landmarks(kba_track_group* g, const kba_create_reques
     if (rc != KBA_OK) return rc;
     g->last = &g->create->counts;
     return KBA_OK;
+}
+
+// ---------------------------------------------------------------------------------------------------------------------
+// window upkeep on the stored window (include/kba_b200.h, kba_track_deactivate_keyframes / kba_track_depth_costs and their group
+// forms; kernels in kba_upkeep.cu): a single call is a one-window call of upkeep_run
+// ---------------------------------------------------------------------------------------------------------------------
+// the largest download of one window of track t: deactivation 5 * n_kf + n_lm, depth costs 4 * n_kf + 12 * B with B <= m_cap
+static size_t upkeep_out_cap(const kba_track* t) {
+    const size_t K = (size_t)t->td.kf_cap, L = (size_t)t->td.lm_cap, M = (size_t)t->td.m_cap;
+    return std::max(5 * K + L, 4 * K + 12 * M);
+}
+
+// one upkeep request of track t (one window of upkeep_run), either kind
+struct UpkeepReq {
+    kba_track* t = nullptr;
+    int n_kf = 0, n_lm = 0;
+    const int32_t* kf_slot = nullptr, *lm_slot = nullptr;
+    const kba_deactivate_request* dq = nullptr;  // deactivation
+    const kba_deactivate_out* dout = nullptr;
+    const kba_depth_out* cout = nullptr;          // depth costs
+    int cap = 0;
+    int bound = 0, max_meas = 0;                  // set by upkeep_check: the depth costs' B, arena entries of the largest keyframe
+};
+
+// every check of one request, before anything is uploaded; allocates the track's slot map at its first upkeep call
+static int upkeep_check(UpkeepReq& r, std::string& why) {
+    kba_track* t = r.t;
+    const bool depth = r.cout != nullptr;
+    if (!r.kf_slot || (r.n_lm > 0 && !r.lm_slot)) { why = "null argument"; return KBA_ERR_BAD_ARG; }
+    if (depth ? (!r.cout->off || (r.cap > 0 && (!r.cout->cand || !r.cout->cost)))
+              : (!r.dout->kf_active || !r.dout->kf_common || (r.n_lm > 0 && !r.dout->lm_active))) {
+        why = "null argument"; return KBA_ERR_BAD_ARG;
+    }
+    if (r.n_kf < 1 || r.n_lm < 0 || r.cap < 0) { why = "no keyframes or a negative size"; return KBA_ERR_BAD_ARG; }
+    if (r.n_kf > t->td.kf_cap || r.n_lm > t->td.lm_cap) { why = "more keyframes or landmarks than the track's slots"; return KBA_ERR_CAPACITY; }
+    const cudaError_t e = cudaSetDevice(t->h->device);
+    if (e != cudaSuccess) { why = std::string("cudaSetDevice: ") + cudaGetErrorString(e); return KBA_ERR_CUDA; }
+    if (!t->upkeep) {
+        std::unique_ptr<UpkeepBufs> ub(new UpkeepBufs());
+        const size_t L = (size_t)t->td.lm_cap;
+        if (cudaMalloc(&ub->map, sizeof(unsigned long long) * std::max<size_t>(L, 1)) != cudaSuccess) {
+            why = "out of memory for the upkeep buffers"; return KBA_ERR_CUDA;
+        }
+        cudaError_t me = cudaMemsetAsync(ub->map, 0, sizeof(unsigned long long) * L, t->h->stream);
+        if (me == cudaSuccess) me = cudaStreamSynchronize(t->h->stream);
+        if (me != cudaSuccess) { why = std::string("upkeep buffers: ") + cudaGetErrorString(me); return KBA_ERR_CUDA; }
+        ub->kf_stamp.assign((size_t)t->td.kf_cap, 0); ub->lm_stamp.assign(L, 0);
+        t->upkeep = std::move(ub);
+    }
+    UpkeepBufs& ub = *t->upkeep;
+    if (++ub.check == 0) {  // the check stamps wrapped: start over
+        std::fill(ub.kf_stamp.begin(), ub.kf_stamp.end(), 0u); std::fill(ub.lm_stamp.begin(), ub.lm_stamp.end(), 0u); ub.check = 1;
+    }
+    r.max_meas = 0;
+    int64_t bound = 0;
+    for (int k = 0; k < r.n_kf; ++k) {
+        const int s = r.kf_slot[k];
+        if (s < 0 || s >= t->td.kf_cap || !t->kf_live[s]) { why = "keyframe slot not pushed"; return KBA_ERR_BAD_ARG; }
+        if (ub.kf_stamp[s] == ub.check) { why = "keyframe slot listed twice"; return KBA_ERR_BAD_ARG; }
+        ub.kf_stamp[s] = ub.check;
+        r.max_meas = std::max(r.max_meas, t->m_cnt[s]);
+        bound += std::min(r.n_lm, t->m_cnt[s]);
+    }
+    for (int j = 0; j < r.n_lm; ++j) {
+        const int s = r.lm_slot[j];
+        if (s < 0 || s >= t->td.lm_cap) { why = "landmark slot out of range"; return KBA_ERR_BAD_ARG; }
+        if (ub.lm_stamp[s] == ub.check) { why = "landmark slot listed twice"; return KBA_ERR_BAD_ARG; }
+        ub.lm_stamp[s] = ub.check;
+    }
+    r.bound = (int)bound;  // <= the arena entries of distinct keyframes <= m_cap
+    if (depth && r.cap < r.bound) { why = "cap below the sum over keyframes of min(n_elig, arena entries)"; return KBA_ERR_CAPACITY; }
+    return KBA_OK;
+}
+
+// W checked requests of distinct tracks, all of one kind, as the W windows of one launch sequence: one upload (the argument
+// records of windows 1 .. W-1, then every window's lists), one download, one synchronisation, then the scatter into the callers'
+// arrays.  Downloads: deactivation kf_common of all windows | kf_active | lm_active; depth costs cost | cnt | cand, each window's
+// pairs at its keyframes' bounds.  Window 0's record travels in the launch parameters (kba_upkeep.cu).
+static int upkeep_run(kba_handle* h, SelectStage& st, int W, const UpkeepReq* r, bool depth) {
+    CU(cudaSetDevice(h->device));
+    cudaStream_t s = h->stream;
+    UpkeepGrid g;
+    size_t n_list = 0, SK = 0, SL = 0, SB = 0;
+    for (int w = 0; w < W; ++w) {
+        n_list += (size_t)r[w].n_kf + r[w].n_lm; SK += (size_t)r[w].n_kf; SL += (size_t)r[w].n_lm; SB += (size_t)r[w].bound;
+        g.max_kf = std::max(g.max_kf, r[w].n_kf); g.max_lm = std::max(g.max_lm, r[w].n_lm);
+        g.max_meas = std::max(g.max_meas, r[w].max_meas);
+    }
+    const size_t o_lists = sizeof(UpkeepArgs) * (size_t)(W - 1), up_bytes = o_lists + 4 * n_list;
+    // deactivation: common | active | lm_active; depth: cost | cnt | cand
+    const size_t o2 = depth ? 8 * SB : 4 * SK, o3 = depth ? o2 + 4 * SK : o2 + SK;
+    const size_t out_bytes = depth ? o3 + 4 * SB : o3 + SL;
+    int* lists_h = reinterpret_cast<int*>(st.up.h + o_lists);
+    const int* lists_d = reinterpret_cast<const int*>(st.up.d + o_lists);
+    unsigned char* d = st.out.d;
+    UpkeepLaunch l;
+    l.rest = reinterpret_cast<const UpkeepArgs*>(st.up.d);
+    l.n_win = W;
+    size_t li = 0, cK = 0, cL = 0, cB = 0;
+    for (int w = 0; w < W; ++w) {
+        const UpkeepReq& q = r[w];
+        UpkeepBufs& ub = *q.t->upkeep;
+        if (ub.stamp >= 0xfffffff0u) {  // the stamps wrap: the map starts over from all 0
+            CU(cudaMemsetAsync(ub.map, 0, sizeof(unsigned long long) * (size_t)q.t->td.lm_cap, s));
+            ub.stamp = 0;
+        }
+        memcpy(lists_h + li, q.kf_slot, 4 * (size_t)q.n_kf);
+        if (q.n_lm) memcpy(lists_h + li + q.n_kf, q.lm_slot, 4 * (size_t)q.n_lm);
+        UpkeepArgs a;
+        a.td = q.t->td;
+        a.kf_slot = lists_d + li; a.lm_slot = lists_d + li + q.n_kf;
+        a.n_kf = q.n_kf; a.n_lm = q.n_lm;
+        a.stamp = ub.stamp + 1; ub.stamp += 2;
+        a.map = ub.map;
+        if (depth) {
+            a.cost = reinterpret_cast<double*>(d + 8 * cB); a.cnt = reinterpret_cast<int*>(d + o2 + 4 * cK);
+            a.cand = reinterpret_cast<int*>(d + o3 + 4 * cB);
+        } else {
+            a.min_connecting = q.dq->min_connecting; a.min_window = q.dq->min_window; a.max_window = q.dq->max_window;
+            a.kf_common = reinterpret_cast<int*>(d + 4 * cK); a.kf_active = d + o2 + cK; a.lm_active = d + o3 + cL;
+        }
+        if (w == 0) l.w0 = a;
+        else memcpy(st.up.h + sizeof(UpkeepArgs) * (size_t)(w - 1), &a, sizeof(UpkeepArgs));
+        li += (size_t)q.n_kf + q.n_lm; cK += (size_t)q.n_kf; cL += (size_t)q.n_lm; cB += (size_t)q.bound;
+    }
+    CU(cudaMemcpyAsync(st.up.d, st.up.h, up_bytes, cudaMemcpyHostToDevice, s));
+    if (depth) launch_depth_costs(l, g, s);
+    else launch_deactivate(l, g, s);
+    cudaError_t e = cudaGetLastError();
+    if (e == cudaSuccess) e = cudaMemcpyAsync(st.out.h, st.out.d, out_bytes, cudaMemcpyDeviceToHost, s);
+    if (e == cudaSuccess) e = wait_stream(h);
+    if (e != cudaSuccess) {
+        // a failed sequence may have left any of this call's stamps in the maps: they go back to all 0 here, so that the map's
+        // state does not depend on how far the sequence got (a sticky error leaves the context unusable anyway, and these calls
+        // then fail as well)
+        for (int w = 0; w < W; ++w) cudaMemsetAsync(r[w].t->upkeep->map, 0, sizeof(unsigned long long) * (size_t)r[w].t->td.lm_cap, s);
+        cudaStreamSynchronize(s);
+        return fail(KBA_ERR_CUDA, std::string(depth ? "depth costs: " : "keyframe deactivation: ") + cudaGetErrorString(e));
+    }
+    const unsigned char* hb = st.out.h;
+    cK = cL = cB = 0;
+    for (int w = 0; w < W; ++w) {
+        const UpkeepReq& q = r[w];
+        const size_t K = (size_t)q.n_kf, L = (size_t)q.n_lm;
+        if (depth) {
+            const int* cnt = reinterpret_cast<const int*>(hb + o2 + 4 * cK);
+            int32_t* off = q.cout->off;
+            size_t base = cB;  // keyframe k's pairs in the download start at the sum of the earlier keyframes' bounds
+            off[0] = 0;
+            for (size_t k = 0; k < K; ++k) {
+                const int n = cnt[k];
+                if (n) {
+                    memcpy(q.cout->cand + off[k], hb + o3 + 4 * base, 4 * (size_t)n);
+                    memcpy(q.cout->cost + off[k], hb + 8 * base, 8 * (size_t)n);
+                }
+                off[k + 1] = off[k] + n;
+                base += (size_t)std::min(q.n_lm, q.t->m_cnt[q.kf_slot[k]]);
+            }
+        } else {
+            memcpy(q.dout->kf_common, hb + 4 * cK, 4 * K);
+            memcpy(q.dout->kf_active, hb + o2 + cK, K);
+            if (L) memcpy(q.dout->lm_active, hb + o3 + cL, L);
+        }
+        cK += K; cL += L; cB += (size_t)q.bound;
+    }
+    st.counts.h2d = (int64_t)up_bytes;
+    st.counts.d2h = (int64_t)out_bytes;
+    return KBA_OK;
+}
+
+static int upkeep_single(kba_track* t, UpkeepReq& r, bool depth, const std::string& who) {
+    std::string why;
+    int rc = upkeep_check(r, why);
+    if (rc != KBA_OK) return fail(rc, who + why);
+    SelectStage& st = t->upkeep->stage;
+    if (!st.up.d) {  // the first single call of the track
+        const size_t K = (size_t)t->td.kf_cap, L = (size_t)t->td.lm_cap;
+        if (st.alloc(4 * (K + L), upkeep_out_cap(t))) {
+            st.up.release(); st.out.release();
+            return fail(KBA_ERR_CUDA, who + "out of memory for the upkeep staging");
+        }
+    }
+    rc = upkeep_run(t->h, st, 1, &r, depth);
+    if (rc == KBA_OK) t->last = &t->upkeep->stage.counts;
+    return rc;
+}
+
+// every request of a group checked, then one upkeep_run over those that do not sit out
+static int upkeep_group(kba_track_group* g, std::vector<UpkeepReq>& all, bool depth, const std::string& who) {
+    const int n = (int)g->tracks.size();
+    std::vector<UpkeepReq> rs;
+    for (int i = 0; i < n; ++i) {
+        if (all[i].n_kf == 0) continue;  // sits the call out
+        std::string why;
+        const int rc = upkeep_check(all[i], why);
+        if (rc != KBA_OK) return fail(rc, who + "track " + std::to_string(i) + ": " + why);
+        rs.push_back(all[i]);
+    }
+    if (rs.empty()) {  // every track sits out: no upload, no launch
+        g->solver.h2d = 0; g->solver.d2h = 0;
+        g->last = &g->solver;
+        return KBA_OK;
+    }
+    if (!g->upkeep) {  // staging for every track at its capacities, allocated once
+        size_t lists = 0, outs = 0;
+        for (const kba_track* t : g->tracks) { lists += (size_t)t->td.kf_cap + t->td.lm_cap; outs += upkeep_out_cap(t); }
+        std::unique_ptr<SelectStage> st(new SelectStage());
+        if (st->alloc(sizeof(UpkeepArgs) * (size_t)(n - 1) + 4 * lists, outs)) return fail(KBA_ERR_CUDA, who + "out of memory for the upkeep staging");
+        g->upkeep = std::move(st);
+    }
+    const int rc = upkeep_run(g->h, *g->upkeep, (int)rs.size(), rs.data(), depth);
+    if (rc != KBA_OK) return rc;
+    g->last = &g->upkeep->counts;
+    return KBA_OK;
+}
+
+static UpkeepReq deactivate_req(kba_track* t, const kba_deactivate_request* q, const kba_deactivate_out* o) {
+    UpkeepReq r;
+    r.t = t; r.n_kf = q->n_kf; r.n_lm = q->n_lm; r.kf_slot = q->kf_slot; r.lm_slot = q->lm_slot; r.dq = q; r.dout = o;
+    return r;
+}
+
+static UpkeepReq depth_req(kba_track* t, const kba_depth_request* q, const kba_depth_out* o) {
+    UpkeepReq r;
+    r.t = t; r.n_kf = q->n_kf; r.n_lm = q->n_elig; r.kf_slot = q->kf_slot; r.lm_slot = q->lm_slot; r.cout = o; r.cap = q->cap;
+    return r;
+}
+
+int kba_track_deactivate_keyframes(kba_track* t, const kba_deactivate_request* req, kba_deactivate_out* out) {
+    static const std::string who = "kba_track_deactivate_keyframes: ";
+    if (!t || !req || !out) return fail(KBA_ERR_BAD_ARG, who + "null argument");
+    UpkeepReq r = deactivate_req(t, req, out);
+    return upkeep_single(t, r, false, who);
+}
+
+int kba_track_depth_costs(kba_track* t, const kba_depth_request* req, kba_depth_out* out) {
+    static const std::string who = "kba_track_depth_costs: ";
+    if (!t || !req || !out) return fail(KBA_ERR_BAD_ARG, who + "null argument");
+    UpkeepReq r = depth_req(t, req, out);
+    return upkeep_single(t, r, true, who);
+}
+
+int kba_track_group_deactivate_keyframes(kba_track_group* g, const kba_deactivate_request* req, kba_deactivate_out* out) {
+    static const std::string who = "kba_track_group_deactivate_keyframes: ";
+    if (!g || !req || !out) return fail(KBA_ERR_BAD_ARG, who + "null argument");
+    std::vector<UpkeepReq> all;
+    for (size_t i = 0; i < g->tracks.size(); ++i) all.push_back(deactivate_req(g->tracks[i], &req[i], &out[i]));
+    return upkeep_group(g, all, false, who);
+}
+
+int kba_track_group_depth_costs(kba_track_group* g, const kba_depth_request* req, kba_depth_out* out) {
+    static const std::string who = "kba_track_group_depth_costs: ";
+    if (!g || !req || !out) return fail(KBA_ERR_BAD_ARG, who + "null argument");
+    std::vector<UpkeepReq> all;
+    for (size_t i = 0; i < g->tracks.size(); ++i) all.push_back(depth_req(g->tracks[i], &req[i], &out[i]));
+    return upkeep_group(g, all, true, who);
 }
 
 // ---------------------------------------------------------------------------------------------------------------------

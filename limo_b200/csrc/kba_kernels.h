@@ -189,6 +189,41 @@ struct CreateGrid {
 };
 void launch_create(const CreateLaunch& l, const CreateGrid& g, cudaStream_t s);
 
+// ---- window upkeep on a track's store (kba_track_deactivate_keyframes / kba_track_depth_costs and their group forms,
+// kba_upkeep.cu) ----
+// One window = one request: the active keyframe slots (ascending id) and a landmark list (deactivation: the active landmarks;
+// depth costs: the eligible ones, ascending id).  The slot map is the track's; an entry is (stamp << 32) | payload and counts only
+// when its stamp is this call's, so the map needs no clearing between calls.
+struct UpkeepArgs {
+    TrackDev td;
+    const int* kf_slot = nullptr;          // [n_kf]
+    const int* lm_slot = nullptr;          // [n_lm]
+    int n_kf = 0, n_lm = 0;
+    int min_connecting = 0, min_window = 0, max_window = 0;
+    unsigned stamp = 0;                    // deactivation uses stamp (newest keyframe) and stamp + 1 (surviving keyframes)
+    unsigned long long* map = nullptr;     // [lm_cap] scratch, by slot
+    // deactivation outputs
+    int* kf_common = nullptr;              // [n_kf]
+    unsigned char* kf_active = nullptr;    // [n_kf]
+    unsigned char* lm_active = nullptr;    // [n_lm]
+    // depth-cost outputs: keyframe k's pairs at base_k = sum over k' < k of min(n_lm, arena entries of k')
+    int* cnt = nullptr;                    // [n_kf] pairs of keyframe k
+    int* cand = nullptr;                   // [B]
+    double* cost = nullptr;                // [B]
+};
+// W windows in one launch sequence, window = grid z; window 0's arguments travel in the launch parameters (as SelectLaunch)
+struct UpkeepLaunch {
+    UpkeepArgs w0;
+    const UpkeepArgs* rest = nullptr;      // [n_win - 1]
+    int n_win = 0;
+};
+struct UpkeepGrid {
+    int max_kf = 0, max_lm = 0;
+    int max_meas = 0;                      // arena entries of a listed keyframe
+};
+void launch_deactivate(const UpkeepLaunch& l, const UpkeepGrid& g, cudaStream_t s);
+void launch_depth_costs(const UpkeepLaunch& l, const UpkeepGrid& g, cudaStream_t s);
+
 // ---- motion-only frames against a track's store (kba_track_adjust_pose / kba_track_group_adjust_pose, kba_motion.cu) ----
 // One frame = one free pose against constant landmarks read from a store by slot: its measurements come in runs, one run per
 // landmark (the landmarks of the equivalent window, in the caller's order).
