@@ -432,7 +432,7 @@ int kba_track_group_create(kba_handle* h, int32_t n_tracks, kba_track* const* tr
 void kba_track_group_destroy(kba_track_group* g);
 /* req[n_tracks], res[n_tracks] */
 int kba_track_group_solve(kba_track_group* g, const kba_track_request* req, const kba_options* opt, kba_result* res);
-/* upload / download of the last group solve, pose-only call, selection, creation or upkeep call, counted as kba_track_transfer_bytes counts them */
+/* upload / download of the last group solve, pose-only call, selection, creation, upkeep or flow call, counted as kba_track_transfer_bytes counts them */
 int kba_track_group_transfer_bytes(kba_track_group* g, int64_t* h2d_last_solve, int64_t* d2h_last_solve);
 
 /* ---- landmark selection for every track of a group in one launch sequence -------------------------------------------------
@@ -597,6 +597,63 @@ typedef struct kba_depth_out {  /* caller-owned arrays */
 int kba_track_depth_costs(kba_track* t, const kba_depth_request* req, kba_depth_out* out);
 /* req[n_tracks], out[n_tracks] */
 int kba_track_group_depth_costs(kba_track_group* g, const kba_depth_request* req, kba_depth_out* out);
+
+/* ---- keyframe selection on the stored window: the flow scheme's quantity ------------------------------------------------
+ * KeyframeRejectionSchemeFlow::isUsable (keyframe_rejection_scheme_flow.cpp:17-74), the one scheme of limo's KeyframeSelector
+ * (mono_lidar.cpp:447-453, mono_standalone.cpp:327-333) that reads stored measurements: the new frame's pixel positions against
+ * those of the newest active keyframe, which the store already holds.  The rotation angle of KeyframeSelectionSchemePose, the
+ * time rule of KeyframeSparsificationSchemeTime and the composition of the verdicts (KeyframeSelector::select) stay with the
+ * caller.  A request:
+ *   - kf_last: the slot of the newest active keyframe (the one with the largest time stamp among the caller's last_frames);
+ *     it must be pushed.  In a group call kf_last < 0 sits the track out; in the single call it is KBA_ERR_BAD_ARG;
+ *   - lm_slot, cam (or NULL: camera 0), u, v [n_meas]: the new frame's measurements whose landmark has a slot, in
+ *     Keyframe::measurements_ order: one run per landmark, runs in ascending landmark id, cameras ascending inside a run (the run
+ *     contract of kba_track_frame).  A measurement whose landmark has no slot cannot match (every landmark a pushed keyframe
+ *     measures has one): the caller leaves it out.  n_meas == 0 is a valid request with no match;
+ *   - min_median_flow: the scheme's parameter.
+ * Outputs, every double operation the facade's, in its order, without FMA contraction, so bit for bit its flow scheme, NaN
+ * included:
+ *   - n_matched: the (landmark, camera) pairs of the frame that the newest keyframe also measures (hasMeasurement(lm, cam));
+ *   - flow_sum: the sum, in request order, of sqrt(dx * dx + dy * dy) over the matched pairs, dx = double(u) - double(u_last),
+ *     dy likewise;
+ *   - mean_flow_sq: s = flow_sum; s /= n_matched; s * s (0 / 0 = NaN without a match);
+ *   - usable: mean_flow_sq > min_median_flow * min_median_flow (0 for NaN): isUsable for a non-empty last_frames and a frame
+ *     with measurements.  The two early returns stay with the caller: an empty last_frames is usable, a frame without
+ *     measurements is not;
+ *   - match [n_meas] (optional, NULL: not written): the index, among kf_last's measurements as pushed, of the matched entry, or -1.
+ * As for the upkeep calls:
+ *   - one upload, one launch sequence, one download, one synchronisation per call; the first call of a track by either entry
+ *     point allocates the upkeep scratch (shared with the upkeep calls) if it is not there yet, its first single call its flow
+ *     staging (sized for win_observations), later calls allocate nothing;
+ *   - every request is checked before anything is uploaded or written: null pointers, n_meas < 0, kf_last not pushed, a slot or
+ *     camera out of range, a slot that reappears after its run has ended, a camera not ascending inside a run: KBA_ERR_BAD_ARG;
+ *     n_meas > win_observations: KBA_ERR_CAPACITY;
+ *   - the group form serves one request per track in one launch sequence (window = request): out[i] is bit for bit what the
+ *     single call writes for req[i]; a request with kf_last < 0 sits the call out (out[i] not written; a call in which every
+ *     request sits out returns at once); a failing request returns its code, kba_last_error names its track, nothing is written.
+ * Transfers (kba_track_transfer_bytes; over the W requests that do not sit out for kba_track_group_transfer_bytes, R the size of
+ * one window's argument record, a constant of the library build; the cameras are uploaded also when cam is NULL, the match
+ * indices downloaded also when match is NULL):
+ *         h2d = 16 * sum(n_meas) + R * (W - 1),   d2h = sum(4 * n_meas + 24) */
+typedef struct kba_flow_request {
+    int32_t kf_last;            /* slot of the newest active keyframe; < 0 (group call): this track sits the call out          */
+    int32_t n_meas;
+    const int32_t* lm_slot;     /* [n_meas] runs as kba_track_frame's                                                          */
+    const int32_t* cam;         /* [n_meas] or NULL (all camera 0)                                                              */
+    const float* u, *v;         /* [n_meas] */
+    double min_median_flow;
+} kba_flow_request;
+typedef struct kba_flow_out {   /* caller-owned */
+    int32_t n_matched;
+    uint8_t usable;
+    uint8_t reserved_[3];
+    double flow_sum;
+    double mean_flow_sq;
+    int32_t* match;             /* [n_meas] or NULL */
+} kba_flow_out;
+int kba_track_frame_flow(kba_track* t, const kba_flow_request* req, kba_flow_out* out);
+/* req[n_tracks], out[n_tracks] */
+int kba_track_group_frame_flow(kba_track_group* g, const kba_flow_request* req, kba_flow_out* out);
 
 /* ---- adjustPoseOnly against the persistent store: one frame's pose per call, or one frame of each track of a group -------
  * What limo calls on every frame (bundle_adjuster_keyframes.cpp:820-888): one free pose against constant landmarks, the optional

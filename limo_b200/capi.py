@@ -9,7 +9,7 @@ import os
 
 import numpy as np
 
-from .capi_types import (KbaCounters, KbaCreateOut, KbaCreateRequest, KbaDeactivateOut, KbaDeactivateRequest, KbaDepthOut, KbaDepthRequest, KbaEvalOut, KbaLidarOptions, KbaOptions, KbaResult, KbaSelectOut, KbaSelectParams, KbaSelectRequest,
+from .capi_types import (KbaCounters, KbaCreateOut, KbaCreateRequest, KbaDeactivateOut, KbaDeactivateRequest, KbaDepthOut, KbaDepthRequest, KbaEvalOut, KbaFlowOut, KbaFlowRequest, KbaLidarOptions, KbaOptions, KbaResult, KbaSelectOut, KbaSelectParams, KbaSelectRequest,
                          KbaTrackCaps, KbaTrackFrame, KbaTrackRequest, KbaWindow, Result, Window, c_double_p, c_int32_p)
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
@@ -27,7 +27,8 @@ SYMBOLS = ["kba_version", "kba_last_error", "kba_default_options", "kba_create",
            "kba_track_group_create", "kba_track_group_destroy", "kba_track_group_solve", "kba_track_group_transfer_bytes",
            "kba_track_adjust_pose", "kba_track_group_adjust_pose", "kba_track_select_landmarks", "kba_track_group_select_landmarks",
            "kba_track_create_landmarks", "kba_track_group_create_landmarks", "kba_track_deactivate_keyframes",
-           "kba_track_group_deactivate_keyframes", "kba_track_depth_costs", "kba_track_group_depth_costs"]
+           "kba_track_group_deactivate_keyframes", "kba_track_depth_costs", "kba_track_group_depth_costs", "kba_track_frame_flow",
+           "kba_track_group_frame_flow"]
 
 
 class KbaError(RuntimeError):
@@ -108,6 +109,8 @@ def lib():
         L.kba_track_group_deactivate_keyframes.argtypes = [vp, C.POINTER(KbaDeactivateRequest), C.POINTER(KbaDeactivateOut)]
         L.kba_track_depth_costs.argtypes = [vp, C.POINTER(KbaDepthRequest), C.POINTER(KbaDepthOut)]
         L.kba_track_group_depth_costs.argtypes = [vp, C.POINTER(KbaDepthRequest), C.POINTER(KbaDepthOut)]
+        L.kba_track_frame_flow.argtypes = [vp, C.POINTER(KbaFlowRequest), C.POINTER(KbaFlowOut)]
+        L.kba_track_group_frame_flow.argtypes = [vp, C.POINTER(KbaFlowRequest), C.POINTER(KbaFlowOut)]
         L.kba_lidar_default_options.argtypes = [C.POINTER(KbaLidarOptions)]
         L.kba_lidar_default_options.restype = None
         fp = C.POINTER(C.c_float)
@@ -372,6 +375,32 @@ class Track:
         _check(lib().kba_track_depth_costs(self._p, C.byref(q), C.byref(o)))
         return off, cand[:off[-1]].copy(), cost[:off[-1]].copy()
 
+    @staticmethod
+    def _flow_args(kf_last, lm_slot, u, v, cam=None, min_median_flow=5.0):
+        lm, lmp = Track._i32(lm_slot)
+        cm, cmp_ = (None, C.cast(None, c_int32_p)) if cam is None else Track._i32(cam)
+        fp = C.POINTER(C.c_float)
+        uu, vv = (np.ascontiguousarray(x, dtype=np.float32) for x in (u, v))
+        match = np.zeros(len(lm), np.int32)
+        q = KbaFlowRequest(kf_last=int(kf_last), n_meas=len(lm), lm_slot=lmp, cam=cmp_, u=uu.ctypes.data_as(fp), v=vv.ctypes.data_as(fp),
+                           min_median_flow=float(min_median_flow))
+        o = KbaFlowOut(match=match.ctypes.data_as(c_int32_p))
+        return q, o, match, (lm, cm, uu, vv)
+
+    @staticmethod
+    def _flow_result(o, match):
+        return dict(n_matched=o.n_matched, flow_sum=o.flow_sum, mean_flow_sq=o.mean_flow_sq, usable=bool(o.usable), match=match)
+
+    def frame_flow(self, kf_last, lm_slot, u, v, cam=None, min_median_flow=5.0):
+        """KeyframeRejectionSchemeFlow's quantity of a new frame against the stored keyframe kf_last, the newest active one
+        (kba_track_frame_flow): the frame's measurements whose landmark has a slot, in Keyframe::measurements_ order (runs by
+        landmark, ascending id, cameras ascending inside a run).  Returns a dict: n_matched, flow_sum, mean_flow_sq (NaN without a
+        match), usable (mean_flow_sq > min_median_flow ** 2) and match [n_meas] (index into kf_last's measurements, -1: none).
+        min_median_flow defaults to limo's launch files' 5 px."""
+        q, o, match, _keep = self._flow_args(kf_last, lm_slot, u, v, cam, min_median_flow)
+        _check(lib().kba_track_frame_flow(self._p, C.byref(q), C.byref(o)))
+        return self._flow_result(o, match)
+
     def transfer_bytes(self):
         a, b, c = C.c_int64(), C.c_int64(), C.c_int64()
         _check(lib().kba_track_transfer_bytes(self._p, C.byref(a), C.byref(b), C.byref(c)))
@@ -544,8 +573,30 @@ class TrackGroup:
                            "kba_track_group_depth_costs")
         return [None if r is None else (r[0], r[1][:r[0][-1]].copy(), r[2][:r[0][-1]].copy()) for r in res]
 
+    def frame_flow(self, requests):
+        """The flow scheme's quantity for one frame of every track in one launch sequence (kba_track_group_frame_flow): each entry
+        None (the track sits the call out) or a dict with the arguments of Track.frame_flow.  Returns one result dict per track,
+        None for a track that sat out."""
+        assert len(requests) == len(self.tracks)
+        n = len(requests)
+        reqs, outs = (KbaFlowRequest * n)(), (KbaFlowOut * n)()
+        for i in range(n):
+            reqs[i].kf_last = -1
+        keep, matches = [], [None] * n
+        for i, r in enumerate(requests):
+            if r is None:
+                continue
+            q, o, match, lists = Track._flow_args(**r)
+            if q.kf_last < 0:  # kf_last < 0 would sit the track out: an error here, as for one track
+                raise KbaError("kba_track_group_frame_flow: track %d: kf_last not pushed" % i)
+            reqs[i], outs[i] = q, o
+            keep.append(lists)
+            matches[i] = match
+        _check(lib().kba_track_group_frame_flow(self._p, reqs, outs))
+        return [None if m is None else Track._flow_result(outs[i], m) for i, m in enumerate(matches)]
+
     def transfer_bytes(self):
-        """(host->device bytes, device->host bytes) of the last group solve, pose-only call, selection, creation or upkeep call"""
+        """(host->device bytes, device->host bytes) of the last group solve, pose-only call, selection, creation, upkeep or flow call"""
         a, b = C.c_int64(), C.c_int64()
         _check(lib().kba_track_group_transfer_bytes(self._p, C.byref(a), C.byref(b)))
         return a.value, b.value

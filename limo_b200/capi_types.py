@@ -83,6 +83,16 @@ class KbaDepthOut(C.Structure):
     _fields_ = [("off", c_int32_p), ("cand", c_int32_p), ("cost", c_double_p)]
 
 
+class KbaFlowRequest(C.Structure):
+    _fields_ = [("kf_last", C.c_int32), ("n_meas", C.c_int32), ("lm_slot", c_int32_p), ("cam", c_int32_p), ("u", c_float_p), ("v", c_float_p),
+                ("min_median_flow", C.c_double)]
+
+
+class KbaFlowOut(C.Structure):
+    _fields_ = [("n_matched", C.c_int32), ("usable", C.c_uint8), ("reserved_", C.c_uint8 * 3), ("flow_sum", C.c_double),
+                ("mean_flow_sq", C.c_double), ("match", c_int32_p)]
+
+
 class KbaTrackFrame(C.Structure):
     _fields_ = [("n_meas", C.c_int32), ("reserved_", C.c_int32), ("pose7", c_double_p), ("lm_slot", c_int32_p), ("cam", c_int32_p),
                 ("u", c_float_p), ("v", c_float_p), ("d", c_float_p), ("speed_weight", C.c_double), ("speed_dt", C.c_double),

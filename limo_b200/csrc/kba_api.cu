@@ -284,6 +284,7 @@ struct CreateBufs {
 // in a group; the staging at its first single call
 struct UpkeepBufs {
     SelectStage stage;                     // the single calls: keyframe slots | landmark slots, one window's outputs
+    SelectStage flow;                      // kba_track_frame_flow: one frame's lists and outputs, at its first call
     unsigned long long* map = nullptr;     // [lm_cap] (stamp << 32) | payload by slot, all 0 (stamp 0: never a call's) at first
     unsigned stamp = 0;                    // the last stamp a call used
     std::vector<unsigned> kf_stamp, lm_stamp;  // duplicate checks: the check that named a slot last
@@ -338,6 +339,7 @@ struct kba_track_group {
     std::unique_ptr<SelectStage> select;   // kba_track_group_select_landmarks, allocated at its first call
     std::unique_ptr<SelectStage> create;   // kba_track_group_create_landmarks, allocated at its first call
     std::unique_ptr<SelectStage> upkeep;   // kba_track_group_deactivate_keyframes / _depth_costs, allocated at the first of them
+    std::unique_ptr<SelectStage> flow;     // kba_track_group_frame_flow, allocated at its first call
     const TrackSolver* last = &solver;
 };
 
@@ -2364,17 +2366,8 @@ struct UpkeepReq {
     int bound = 0, max_meas = 0;                  // set by upkeep_check: the depth costs' B, arena entries of the largest keyframe
 };
 
-// every check of one request, before anything is uploaded; allocates the track's slot map at its first upkeep call
-static int upkeep_check(UpkeepReq& r, std::string& why) {
-    kba_track* t = r.t;
-    const bool depth = r.cout != nullptr;
-    if (!r.kf_slot || (r.n_lm > 0 && !r.lm_slot)) { why = "null argument"; return KBA_ERR_BAD_ARG; }
-    if (depth ? (!r.cout->off || (r.cap > 0 && (!r.cout->cand || !r.cout->cost)))
-              : (!r.dout->kf_active || !r.dout->kf_common || (r.n_lm > 0 && !r.dout->lm_active))) {
-        why = "null argument"; return KBA_ERR_BAD_ARG;
-    }
-    if (r.n_kf < 1 || r.n_lm < 0 || r.cap < 0) { why = "no keyframes or a negative size"; return KBA_ERR_BAD_ARG; }
-    if (r.n_kf > t->td.kf_cap || r.n_lm > t->td.lm_cap) { why = "more keyframes or landmarks than the track's slots"; return KBA_ERR_CAPACITY; }
+// the track's upkeep scratch (slot map, duplicate-check stamps), allocated at its first upkeep or flow call, and a fresh check stamp
+static int upkeep_bufs(kba_track* t, std::string& why) {
     const cudaError_t e = cudaSetDevice(t->h->device);
     if (e != cudaSuccess) { why = std::string("cudaSetDevice: ") + cudaGetErrorString(e); return KBA_ERR_CUDA; }
     if (!t->upkeep) {
@@ -2393,6 +2386,23 @@ static int upkeep_check(UpkeepReq& r, std::string& why) {
     if (++ub.check == 0) {  // the check stamps wrapped: start over
         std::fill(ub.kf_stamp.begin(), ub.kf_stamp.end(), 0u); std::fill(ub.lm_stamp.begin(), ub.lm_stamp.end(), 0u); ub.check = 1;
     }
+    return KBA_OK;
+}
+
+// every check of one request, before anything is uploaded; allocates the track's slot map at its first upkeep call
+static int upkeep_check(UpkeepReq& r, std::string& why) {
+    kba_track* t = r.t;
+    const bool depth = r.cout != nullptr;
+    if (!r.kf_slot || (r.n_lm > 0 && !r.lm_slot)) { why = "null argument"; return KBA_ERR_BAD_ARG; }
+    if (depth ? (!r.cout->off || (r.cap > 0 && (!r.cout->cand || !r.cout->cost)))
+              : (!r.dout->kf_active || !r.dout->kf_common || (r.n_lm > 0 && !r.dout->lm_active))) {
+        why = "null argument"; return KBA_ERR_BAD_ARG;
+    }
+    if (r.n_kf < 1 || r.n_lm < 0 || r.cap < 0) { why = "no keyframes or a negative size"; return KBA_ERR_BAD_ARG; }
+    if (r.n_kf > t->td.kf_cap || r.n_lm > t->td.lm_cap) { why = "more keyframes or landmarks than the track's slots"; return KBA_ERR_CAPACITY; }
+    const int rb = upkeep_bufs(t, why);
+    if (rb != KBA_OK) return rb;
+    UpkeepBufs& ub = *t->upkeep;
     r.max_meas = 0;
     int64_t bound = 0;
     for (int k = 0; k < r.n_kf; ++k) {
@@ -2596,6 +2606,174 @@ int kba_track_group_depth_costs(kba_track_group* g, const kba_depth_request* req
     std::vector<UpkeepReq> all;
     for (size_t i = 0; i < g->tracks.size(); ++i) all.push_back(depth_req(g->tracks[i], &req[i], &out[i]));
     return upkeep_group(g, all, true, who);
+}
+
+// ---------------------------------------------------------------------------------------------------------------------
+// the flow scheme of keyframe selection on the stored window (include/kba_b200.h, kba_track_frame_flow /
+// kba_track_group_frame_flow; kernels in kba_keyframe.cu): a single call is a one-window call of flow_run
+// ---------------------------------------------------------------------------------------------------------------------
+// every check of one request, before anything is uploaded; allocates the track's upkeep scratch at its first upkeep or flow call
+static int flow_check(kba_track* t, const kba_flow_request* q, std::string& why) {
+    const int n = q->n_meas;
+    if (n < 0) { why = "negative size"; return KBA_ERR_BAD_ARG; }
+    if (n > 0 && (!q->lm_slot || !q->u || !q->v)) { why = "null argument"; return KBA_ERR_BAD_ARG; }
+    if (q->kf_last < 0 || q->kf_last >= t->td.kf_cap || !t->kf_live[q->kf_last]) { why = "kf_last not pushed"; return KBA_ERR_BAD_ARG; }
+    if (n > t->caps.win_observations) { why = "more measurements than win_observations"; return KBA_ERR_CAPACITY; }
+    const int rb = upkeep_bufs(t, why);
+    if (rb != KBA_OK) return rb;
+    UpkeepBufs& ub = *t->upkeep;
+    for (int i = 0; i < n; ++i) {
+        const int s = q->lm_slot[i], c = q->cam ? q->cam[i] : 0;
+        if (s < 0 || s >= t->td.lm_cap) { why = "landmark slot out of range"; return KBA_ERR_BAD_ARG; }
+        if (c < 0 || c >= t->n_cam) { why = "camera out of range"; return KBA_ERR_BAD_ARG; }
+        if (i > 0 && s == q->lm_slot[i - 1]) {
+            if (c <= (q->cam ? q->cam[i - 1] : 0)) { why = "camera not ascending inside a run"; return KBA_ERR_BAD_ARG; }
+            continue;
+        }
+        if (ub.lm_stamp[s] == ub.check) { why = "landmark slot reappears after its run"; return KBA_ERR_BAD_ARG; }
+        ub.lm_stamp[s] = ub.check;
+    }
+    return KBA_OK;
+}
+
+// W checked requests of distinct tracks as the W windows of one launch sequence: one upload (the argument records of windows
+// 1 .. W-1, then every window's lm | cam | u | v), one download (the FlowRes records of all windows, then their match indices),
+// one synchronisation, then the scatter into the callers' outputs.  Window 0's record travels in the launch parameters.
+static int flow_run(kba_handle* h, SelectStage& st, int W, kba_track* const* ts, const kba_flow_request* const* qs,
+                    kba_flow_out* const* os) {
+    CU(cudaSetDevice(h->device));
+    cudaStream_t s = h->stream;
+    FlowGrid g;
+    size_t SN = 0;
+    for (int w = 0; w < W; ++w) {
+        SN += (size_t)qs[w]->n_meas;
+        g.max_last = std::max(g.max_last, ts[w]->m_cnt[qs[w]->kf_last]);
+    }
+    const size_t o_lists = sizeof(FlowArgs) * (size_t)(W - 1), up_bytes = o_lists + 16 * SN;
+    const size_t o_match = sizeof(FlowRes) * (size_t)W, out_bytes = o_match + 4 * SN;
+    unsigned char* up_h = st.up.h + o_lists;
+    const unsigned char* up_d = st.up.d + o_lists;
+    FlowLaunch l;
+    l.rest = reinterpret_cast<const FlowArgs*>(st.up.d);
+    l.n_win = W;
+    size_t li = 0, mi = 0;
+    for (int w = 0; w < W; ++w) {
+        const kba_flow_request& q = *qs[w];
+        const size_t n = (size_t)q.n_meas;
+        UpkeepBufs& ub = *ts[w]->upkeep;
+        if (ub.stamp >= 0xfffffff0u) {  // the stamps wrap: the map starts over from all 0
+            CU(cudaMemsetAsync(ub.map, 0, sizeof(unsigned long long) * (size_t)ts[w]->td.lm_cap, s));
+            ub.stamp = 0;
+        }
+        int32_t* lm = reinterpret_cast<int32_t*>(up_h + li);
+        int32_t* cam = lm + n;
+        if (n) {
+            memcpy(lm, q.lm_slot, 4 * n);
+            if (q.cam) memcpy(cam, q.cam, 4 * n);
+            else memset(cam, 0, 4 * n);
+            memcpy(cam + n, q.u, 4 * n);
+            memcpy(cam + 2 * n, q.v, 4 * n);
+        }
+        FlowArgs a;
+        a.td = ts[w]->td;
+        a.kf_last = q.kf_last; a.n_meas = q.n_meas;
+        a.lm_slot = reinterpret_cast<const int*>(up_d + li); a.cam = a.lm_slot + n;
+        a.u = reinterpret_cast<const float*>(a.cam + n); a.v = a.u + n;
+        a.min_median_flow = q.min_median_flow;
+        a.stamp = ++ub.stamp;
+        a.map = ub.map;
+        a.res = reinterpret_cast<FlowRes*>(st.out.d) + w;
+        a.match = reinterpret_cast<int*>(st.out.d + o_match) + mi;
+        if (w == 0) l.w0 = a;
+        else memcpy(st.up.h + sizeof(FlowArgs) * (size_t)(w - 1), &a, sizeof(FlowArgs));
+        li += 16 * n; mi += n;
+    }
+    CU(cudaMemcpyAsync(st.up.d, st.up.h, up_bytes, cudaMemcpyHostToDevice, s));
+    launch_frame_flow(l, g, s);
+    cudaError_t e = cudaGetLastError();
+    if (e == cudaSuccess) e = cudaMemcpyAsync(st.out.h, st.out.d, out_bytes, cudaMemcpyDeviceToHost, s);
+    if (e == cudaSuccess) e = wait_stream(h);
+    if (e != cudaSuccess) {
+        // as upkeep_run: the maps go back to all 0, whatever stamps the failed sequence left in them
+        for (int w = 0; w < W; ++w) cudaMemsetAsync(ts[w]->upkeep->map, 0, sizeof(unsigned long long) * (size_t)ts[w]->td.lm_cap, s);
+        cudaStreamSynchronize(s);
+        return fail(KBA_ERR_CUDA, std::string("frame flow: ") + cudaGetErrorString(e));
+    }
+    const FlowRes* res = reinterpret_cast<const FlowRes*>(st.out.h);
+    const int32_t* match = reinterpret_cast<const int32_t*>(st.out.h + o_match);
+    mi = 0;
+    for (int w = 0; w < W; ++w) {
+        kba_flow_out& o = *os[w];
+        const size_t n = (size_t)qs[w]->n_meas;
+        o.n_matched = res[w].n_matched;
+        o.usable = (uint8_t)res[w].usable;
+        o.flow_sum = res[w].flow_sum;
+        o.mean_flow_sq = res[w].mean_flow_sq;
+        if (res[w].n_matched == 0) {
+            // 0 / 0: the NaN's bits are the host CPU's default NaN in the facade (x86-64: sign bit set), which the device's
+            // canonical NaN is not, so the library forms this one quotient with the host's own arithmetic
+            volatile double zero = 0.;
+            const double q0 = o.flow_sum / zero;
+            o.mean_flow_sq = q0 * q0;
+        }
+        if (o.match && n) memcpy(o.match, match + mi, 4 * n);
+        mi += n;
+    }
+    st.counts.h2d = (int64_t)up_bytes;
+    st.counts.d2h = (int64_t)out_bytes;
+    return KBA_OK;
+}
+
+int kba_track_frame_flow(kba_track* t, const kba_flow_request* req, kba_flow_out* out) {
+    static const std::string who = "kba_track_frame_flow: ";
+    if (!t || !req || !out) return fail(KBA_ERR_BAD_ARG, who + "null argument");
+    std::string why;
+    int rc = flow_check(t, req, why);
+    if (rc != KBA_OK) return fail(rc, who + why);
+    SelectStage& st = t->upkeep->flow;
+    if (!st.up.d) {  // the first single call of the track: staging for win_observations measurements
+        const size_t O = (size_t)t->caps.win_observations;
+        if (st.alloc(16 * O, sizeof(FlowRes) + 4 * O)) {
+            st.up.release(); st.out.release();
+            return fail(KBA_ERR_CUDA, who + "out of memory for the flow staging");
+        }
+    }
+    rc = flow_run(t->h, st, 1, &t, &req, &out);
+    if (rc == KBA_OK) t->last = &st.counts;
+    return rc;
+}
+
+int kba_track_group_frame_flow(kba_track_group* g, const kba_flow_request* req, kba_flow_out* out) {
+    static const std::string who = "kba_track_group_frame_flow: ";
+    if (!g || !req || !out) return fail(KBA_ERR_BAD_ARG, who + "null argument");
+    const int n = (int)g->tracks.size();
+    std::vector<kba_track*> ts;
+    std::vector<const kba_flow_request*> qs;
+    std::vector<kba_flow_out*> os;
+    for (int i = 0; i < n; ++i) {
+        if (req[i].kf_last < 0) continue;  // sits the call out
+        std::string why;
+        const int rc = flow_check(g->tracks[i], &req[i], why);
+        if (rc != KBA_OK) return fail(rc, who + "track " + std::to_string(i) + ": " + why);
+        ts.push_back(g->tracks[i]); qs.push_back(&req[i]); os.push_back(&out[i]);
+    }
+    if (ts.empty()) {  // every track sits out: no upload, no launch
+        g->solver.h2d = 0; g->solver.d2h = 0;
+        g->last = &g->solver;
+        return KBA_OK;
+    }
+    if (!g->flow) {  // staging for every track at its win_observations, allocated once
+        size_t obs = 0;
+        for (const kba_track* t : g->tracks) obs += (size_t)t->caps.win_observations;
+        std::unique_ptr<SelectStage> st(new SelectStage());
+        if (st->alloc(sizeof(FlowArgs) * (size_t)(n - 1) + 16 * obs, sizeof(FlowRes) * (size_t)n + 4 * obs))
+            return fail(KBA_ERR_CUDA, who + "out of memory for the flow staging");
+        g->flow = std::move(st);
+    }
+    const int rc = flow_run(g->h, *g->flow, (int)ts.size(), ts.data(), qs.data(), os.data());
+    if (rc != KBA_OK) return rc;
+    g->last = &g->flow->counts;
+    return KBA_OK;
 }
 
 // ---------------------------------------------------------------------------------------------------------------------

@@ -224,6 +224,37 @@ struct UpkeepGrid {
 void launch_deactivate(const UpkeepLaunch& l, const UpkeepGrid& g, cudaStream_t s);
 void launch_depth_costs(const UpkeepLaunch& l, const UpkeepGrid& g, cudaStream_t s);
 
+// ---- the flow scheme of keyframe selection on a track's store (kba_track_frame_flow / kba_track_group_frame_flow,
+// kba_keyframe.cu) ----
+// One window = one request: the new frame's measurements (runs by landmark slot, cameras ascending inside a run) against the
+// stored keyframe kf_last.  The slot map is the track's upkeep map (UpkeepArgs): kf_last's runs are marked with the call's stamp
+// and their first entry, so the map needs no clearing between calls.
+struct FlowRes {                           // one window's download record, 24 bytes
+    double flow_sum, mean_flow_sq;
+    int n_matched, usable;
+};
+struct FlowArgs {
+    TrackDev td;
+    int kf_last = 0, n_meas = 0;
+    const int* lm_slot = nullptr;          // [n_meas]
+    const int* cam = nullptr;              // [n_meas]
+    const float* u = nullptr, *v = nullptr;  // [n_meas]
+    double min_median_flow = 0;
+    unsigned stamp = 0;
+    unsigned long long* map = nullptr;     // [lm_cap] scratch, by slot
+    FlowRes* res = nullptr;
+    int* match = nullptr;                  // [n_meas] index into kf_last's entries, -1: no match
+};
+struct FlowLaunch {
+    FlowArgs w0;
+    const FlowArgs* rest = nullptr;        // [n_win - 1]
+    int n_win = 0;
+};
+struct FlowGrid {
+    int max_last = 0;                      // arena entries of the largest kf_last
+};
+void launch_frame_flow(const FlowLaunch& l, const FlowGrid& g, cudaStream_t s);
+
 // ---- motion-only frames against a track's store (kba_track_adjust_pose / kba_track_group_adjust_pose, kba_motion.cu) ----
 // One frame = one free pose against constant landmarks read from a store by slot: its measurements come in runs, one run per
 // landmark (the landmarks of the equivalent window, in the caller's order).
