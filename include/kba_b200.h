@@ -432,7 +432,7 @@ int kba_track_group_create(kba_handle* h, int32_t n_tracks, kba_track* const* tr
 void kba_track_group_destroy(kba_track_group* g);
 /* req[n_tracks], res[n_tracks] */
 int kba_track_group_solve(kba_track_group* g, const kba_track_request* req, const kba_options* opt, kba_result* res);
-/* upload / download of the last group solve, pose-only call, selection, creation, upkeep or flow call, counted as kba_track_transfer_bytes counts them */
+/* upload / download of the last group solve, pose-only call, selection, creation, upkeep, flow or reclaim call, counted as kba_track_transfer_bytes counts them */
 int kba_track_group_transfer_bytes(kba_track_group* g, int64_t* h2d_last_solve, int64_t* d2h_last_solve);
 
 /* ---- landmark selection for every track of a group in one launch sequence -------------------------------------------------
@@ -654,6 +654,46 @@ typedef struct kba_flow_out {   /* caller-owned */
 int kba_track_frame_flow(kba_track* t, const kba_flow_request* req, kba_flow_out* out);
 /* req[n_tracks], out[n_tracks] */
 int kba_track_group_frame_flow(kba_track_group* g, const kba_flow_request* req, kba_flow_out* out);
+
+/* ---- free landmark slots of the stored window: recycle slots as keyframe slots are recycled --------------------------------
+ * A keyframe slot is free again after kba_track_drop_keyframe; a landmark slot is free once no live keyframe (pushed and not
+ * dropped) measures it, which only the store can tell a caller that keeps no host copy of the measurements.  A request names a
+ * slot range [lo, hi), 0 <= lo <= hi <= max_landmarks (a caller with dense slots from 0 asks for [0, slots handed out)).
+ * Outputs:
+ *   - n_free and free_slot [0 .. n_free): the slots of the range that no arena entry of a live keyframe names, ascending;
+ *   - pos [3 * n_free] and weight [n_free], each optional (NULL: not written): the store's current values of those slots, bit
+ *     for bit.  A caller that evicts a landmark keeps them, and restores the landmark with kba_track_set_landmarks when its id is
+ *     measured again (push() never re-creates a landmark that exists).
+ * The caller allocates free_slot (and pos, weight) for the whole range, hi - lo entries.  Liveness is the caller's: the live
+ * keyframe slots go up with the request (a dropped keyframe's entries stay in the arena until the next compaction).  The call
+ * does not write the store: a slot handed out again must be written (kba_track_create_landmarks or kba_track_set_landmarks)
+ * before any call reads it.  Integer work only, so the result is deterministic.  As for the upkeep calls:
+ *   - one upload, one launch sequence, one download, one synchronisation per call; the first call of a track by either entry
+ *     point allocates its upkeep scratch (shared with the upkeep and flow calls) if it is not there yet, its first single call
+ *     its reclaim staging (sized for every keyframe slot and a range of max_landmarks), later calls allocate nothing.  An empty
+ *     range (hi == lo) in the single call gives n_free = 0 without an upload or a launch;
+ *   - every request is checked before anything is uploaded or written: a null pointer (free_slot may be NULL only for an empty
+ *     range), a range outside [0, max_landmarks] or with hi < lo: KBA_ERR_BAD_ARG;
+ *   - the group form serves one request per track in one launch sequence (window = request): out[i] is bit for bit what the
+ *     single call writes for req[i]; a request with hi == lo sits the call out (out[i] not written; a call in which every
+ *     request sits out returns at once); a failing request returns its code, kba_last_error names its track, nothing is written.
+ * Transfers (kba_track_transfer_bytes; over the W requests that do not sit out for kba_track_group_transfer_bytes, R the size of
+ * one window's argument record, a constant of the library build; n_w = hi - lo, L_w the live keyframes of request w's track;
+ * the slots are downloaded for the whole range):
+ *         h2d = 4 * sum(L_w) + R * (W - 1),   d2h = sum(4 + 4 * n_w + (pos ? 24 * n_w : 0) + (weight ? 8 * n_w : 0)) */
+typedef struct kba_reclaim_request {
+    int32_t lo, hi;             /* slot range [lo, hi); hi == lo (group call): this track sits the call out                  */
+} kba_reclaim_request;
+typedef struct kba_reclaim_out {  /* caller-owned */
+    int32_t n_free;
+    int32_t reserved_;
+    int32_t* free_slot;         /* [hi - lo]; the first n_free are written                                                   */
+    double* pos;                /* [3 * (hi - lo)] or NULL                                                                   */
+    double* weight;             /* [hi - lo] or NULL                                                                         */
+} kba_reclaim_out;
+int kba_track_reclaim_landmarks(kba_track* t, const kba_reclaim_request* req, kba_reclaim_out* out);
+/* req[n_tracks], out[n_tracks] */
+int kba_track_group_reclaim_landmarks(kba_track_group* g, const kba_reclaim_request* req, kba_reclaim_out* out);
 
 /* ---- adjustPoseOnly against the persistent store: one frame's pose per call, or one frame of each track of a group -------
  * What limo calls on every frame (bundle_adjuster_keyframes.cpp:820-888): one free pose against constant landmarks, the optional

@@ -78,6 +78,11 @@ public:
     // adjustPoseOnly() then tracks the frame against the landmarks in that store (kba_track_adjust_pose) when the store has every
     // landmark and camera of the frame, and otherwise rebuilds its one-keyframe window.
     void set_persistent_window(bool on) { persistent_window_ = on; }
+    // Not in the reference: the capacities of that store (defaults 256 keyframes, 131072 landmarks, 2^21 measurements).  Landmark
+    // slots that no stored keyframe measures any more are reclaimed when the store runs out (kba_track_reclaim_landmarks), so the
+    // landmark capacity bounds the landmarks of the stored keyframes, not those of the whole run.  Only before the store exists
+    // (the first solve()); afterwards it throws std::logic_error.
+    void set_track_capacity(int max_keyframes, int max_landmarks, int max_measurements);
     // Not in the reference: with the persistent window on, solve() lets the store compute the per-landmark quantities of the
     // landmark selector's chain (kba_track_select_landmarks) when the chain is cheirality + voxel (+ selection schemes, limo's
     // mono-lidar configuration); the selector ranks them exactly as its host select() does, so the selection is the same.
@@ -114,14 +119,19 @@ private:
     bool solveTracked(const std::vector<Keyframe*>& kfs, const std::vector<LandmarkId>& lm_ids, std::string& report, bool synced);
     bool adjustPoseTracked(Keyframe& kf, const std::vector<LandmarkId>& lm_ids, std::string& report);
     bool flushLandmarks();  // new and dirty landmark state into the store, before any use of the track
+    void dropInactiveKeyframes(size_t max_free_kf_slots);
+    bool reclaimLandmarkSlots(const Keyframe& kf);
     void speedPrior(const Keyframe& speed_kf, kba_window& w) const;
     kba_track* track_{nullptr};
     bool persistent_window_{true}, track_failed_{false}, device_selection_{true}, last_select_on_device_{false};
+    int track_keyframes_{256}, track_landmarks_{1 << 17}, track_measurements_{1 << 21};
     std::map<KeyframeId, int> kf_slot_;
     std::map<LandmarkId, int> lm_slot_;
-    std::vector<int> free_kf_slots_;
+    std::vector<LandmarkId> slot_lm_;  // the landmark a slot was handed to (slot -> id), for every slot handed out so far
+    std::vector<int> free_kf_slots_, free_lm_slots_;
     std::vector<std::array<double, 10>> track_cams_;  // camera values (f, pp, pose_camera_vehicle) the track was created with
     std::set<LandmarkId> new_landmarks_, dirty_weights_;
+    std::set<LandmarkId> restore_landmarks_;  // existing landmarks that got a slot again: position and weight go up at the flush
     std::set<LandmarkId> dirty_positions_;  // positions the rebuild path wrote on the host only
     long long last_solve_h2d_{0}, push_h2d_{0}, last_select_h2d_{0};
 };

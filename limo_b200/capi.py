@@ -9,7 +9,7 @@ import os
 
 import numpy as np
 
-from .capi_types import (KbaCounters, KbaCreateOut, KbaCreateRequest, KbaDeactivateOut, KbaDeactivateRequest, KbaDepthOut, KbaDepthRequest, KbaEvalOut, KbaFlowOut, KbaFlowRequest, KbaLidarOptions, KbaOptions, KbaResult, KbaSelectOut, KbaSelectParams, KbaSelectRequest,
+from .capi_types import (KbaCounters, KbaCreateOut, KbaCreateRequest, KbaDeactivateOut, KbaDeactivateRequest, KbaDepthOut, KbaDepthRequest, KbaEvalOut, KbaFlowOut, KbaFlowRequest, KbaLidarOptions, KbaOptions, KbaReclaimOut, KbaReclaimRequest, KbaResult, KbaSelectOut, KbaSelectParams, KbaSelectRequest,
                          KbaTrackCaps, KbaTrackFrame, KbaTrackRequest, KbaWindow, Result, Window, c_double_p, c_int32_p)
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
@@ -28,7 +28,7 @@ SYMBOLS = ["kba_version", "kba_last_error", "kba_default_options", "kba_create",
            "kba_track_adjust_pose", "kba_track_group_adjust_pose", "kba_track_select_landmarks", "kba_track_group_select_landmarks",
            "kba_track_create_landmarks", "kba_track_group_create_landmarks", "kba_track_deactivate_keyframes",
            "kba_track_group_deactivate_keyframes", "kba_track_depth_costs", "kba_track_group_depth_costs", "kba_track_frame_flow",
-           "kba_track_group_frame_flow"]
+           "kba_track_group_frame_flow", "kba_track_reclaim_landmarks", "kba_track_group_reclaim_landmarks"]
 
 
 class KbaError(RuntimeError):
@@ -111,6 +111,8 @@ def lib():
         L.kba_track_group_depth_costs.argtypes = [vp, C.POINTER(KbaDepthRequest), C.POINTER(KbaDepthOut)]
         L.kba_track_frame_flow.argtypes = [vp, C.POINTER(KbaFlowRequest), C.POINTER(KbaFlowOut)]
         L.kba_track_group_frame_flow.argtypes = [vp, C.POINTER(KbaFlowRequest), C.POINTER(KbaFlowOut)]
+        L.kba_track_reclaim_landmarks.argtypes = [vp, C.POINTER(KbaReclaimRequest), C.POINTER(KbaReclaimOut)]
+        L.kba_track_group_reclaim_landmarks.argtypes = [vp, C.POINTER(KbaReclaimRequest), C.POINTER(KbaReclaimOut)]
         L.kba_lidar_default_options.argtypes = [C.POINTER(KbaLidarOptions)]
         L.kba_lidar_default_options.restype = None
         fp = C.POINTER(C.c_float)
@@ -401,6 +403,32 @@ class Track:
         _check(lib().kba_track_frame_flow(self._p, C.byref(q), C.byref(o)))
         return self._flow_result(o, match)
 
+    @staticmethod
+    def _reclaim_args(lo, hi, evict=False):
+        n = max(int(hi) - int(lo), 0)
+        slot = np.zeros(n, np.int32)
+        pos, weight = (np.zeros((n, 3), np.float64), np.zeros(n, np.float64)) if evict else (None, None)
+        q = KbaReclaimRequest(lo=int(lo), hi=int(hi))
+        o = KbaReclaimOut(free_slot=slot.ctypes.data_as(c_int32_p))
+        if evict:
+            o.pos, o.weight = pos.ctypes.data_as(c_double_p), weight.ctypes.data_as(c_double_p)
+        return q, o, (slot, pos, weight)
+
+    @staticmethod
+    def _reclaim_result(o, res, evict):
+        n = o.n_free
+        slot, pos, weight = res
+        return (slot[:n].copy(), pos[:n].copy(), weight[:n].copy()) if evict else slot[:n].copy()
+
+    def reclaim_landmarks(self, lo, hi, evict=False):
+        """The landmark slots in [lo, hi) that no live keyframe (pushed and not dropped) measures, ascending
+        (kba_track_reclaim_landmarks).  Returns the slots, or with evict=True (slots, pos [n, 3], weight [n]): the store's current
+        values of those slots, for a caller that restores an evicted landmark later with set_landmarks.  The store is not written:
+        a slot handed out again must be written (create_landmarks or set_landmarks) before a call reads it."""
+        q, o, res = self._reclaim_args(lo, hi, evict)
+        _check(lib().kba_track_reclaim_landmarks(self._p, C.byref(q), C.byref(o)))
+        return self._reclaim_result(o, res, evict)
+
     def transfer_bytes(self):
         a, b, c = C.c_int64(), C.c_int64(), C.c_int64()
         _check(lib().kba_track_transfer_bytes(self._p, C.byref(a), C.byref(b), C.byref(c)))
@@ -594,6 +622,37 @@ class TrackGroup:
             matches[i] = match
         _check(lib().kba_track_group_frame_flow(self._p, reqs, outs))
         return [None if m is None else Track._flow_result(outs[i], m) for i, m in enumerate(matches)]
+
+    def reclaim_landmarks(self, requests):
+        """The free landmark slots of every track in one launch sequence (kba_track_group_reclaim_landmarks): each entry None (the
+        track sits the call out) or a dict with the arguments of Track.reclaim_landmarks (lo, hi, evict).  Returns one result per
+        track as Track.reclaim_landmarks returns it, None for a track that sat out."""
+        assert len(requests) == len(self.tracks)
+        n = len(requests)
+        reqs, outs = (KbaReclaimRequest * n)(), (KbaReclaimOut * n)()
+        keep = [None] * n
+        for i, r in enumerate(requests):
+            if r is None:
+                continue
+            extra = set(r) - {"lo", "hi", "evict"}
+            if extra:
+                raise TypeError("reclaim_landmarks: request %d has unexpected keys %s" % (i, sorted(extra)))
+            q, o, res = Track._reclaim_args(r["lo"], r["hi"], r.get("evict", False))
+            if q.hi == q.lo:  # an empty range would sit the track out: here it is an empty result, as for one track
+                keep[i] = None
+                continue
+            reqs[i], outs[i] = q, o
+            keep[i] = (res, bool(r.get("evict", False)))
+        _check(lib().kba_track_group_reclaim_landmarks(self._p, reqs, outs))
+        results = [None] * n
+        for i, r in enumerate(requests):
+            if r is None:
+                continue
+            if keep[i] is None:
+                results[i] = Track._reclaim_result(KbaReclaimOut(), Track._reclaim_args(0, 0, r.get("evict", False))[2], r.get("evict", False))
+            else:
+                results[i] = Track._reclaim_result(outs[i], *keep[i])
+        return results
 
     def transfer_bytes(self):
         """(host->device bytes, device->host bytes) of the last group solve, pose-only call, selection, creation, upkeep or flow call"""

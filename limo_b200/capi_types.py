@@ -93,6 +93,14 @@ class KbaFlowOut(C.Structure):
                 ("mean_flow_sq", C.c_double), ("match", c_int32_p)]
 
 
+class KbaReclaimRequest(C.Structure):
+    _fields_ = [("lo", C.c_int32), ("hi", C.c_int32)]
+
+
+class KbaReclaimOut(C.Structure):
+    _fields_ = [("n_free", C.c_int32), ("reserved_", C.c_int32), ("free_slot", c_int32_p), ("pos", c_double_p), ("weight", c_double_p)]
+
+
 class KbaTrackFrame(C.Structure):
     _fields_ = [("n_meas", C.c_int32), ("reserved_", C.c_int32), ("pose7", c_double_p), ("lm_slot", c_int32_p), ("cam", c_int32_p),
                 ("u", c_float_p), ("v", c_float_p), ("d", c_float_p), ("speed_weight", C.c_double), ("speed_dt", C.c_double),

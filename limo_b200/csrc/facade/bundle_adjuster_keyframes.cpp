@@ -433,7 +433,6 @@ std::array<double, 10> camera_value(const Camera& c) {
     std::copy(c.pose_camera_vehicle.begin(), c.pose_camera_vehicle.end(), k.begin() + 3);
     return k;
 }
-constexpr int kTrackKeyframes = 256, kTrackLandmarks = 1 << 17, kTrackMeasurements = 1 << 21;
 constexpr int kTrackWinKeyframes = 30, kTrackWinLandmarks = 16384, kTrackWinObservations = 1 << 18;
 }  // namespace
 
@@ -453,10 +452,10 @@ bool BundleAdjusterKeyframes::trackPush(const Keyframe& kf) {
         // ground capacity for every selected landmark: the candidate lists are 4 B per landmark.  Reduced rows for every window
         // up to kTrackWinKeyframes with plane blocks: windows beyond 184 rows (19-30 keyframes with ground points, limo's default of
         // 20 among them) take the track's large-window solver instead of the rebuild path
-        kba_track_caps caps{kTrackKeyframes, kTrackLandmarks, kTrackMeasurements, kTrackWinKeyframes, kTrackWinLandmarks, kTrackWinObservations,
+        kba_track_caps caps{track_keyframes_, track_landmarks_, track_measurements_, kTrackWinKeyframes, kTrackWinLandmarks, kTrackWinObservations,
                             kTrackWinLandmarks, 10 * kTrackWinKeyframes + 1};
         if (kba_track_create(handle_, &caps, int(track_cams_.size()), intr.data(), pose.data(), &track_) != KBA_OK) return false;
-        for (int i = kTrackKeyframes - 1; i >= 0; --i) free_kf_slots_.push_back(i);
+        for (int i = track_keyframes_ - 1; i >= 0; --i) free_kf_slots_.push_back(i);
     }
     std::map<CameraId, int> cam_of;
     for (const auto& c : kf.cameras_) {
@@ -465,21 +464,28 @@ bool BundleAdjusterKeyframes::trackPush(const Keyframe& kf) {
         cam_of[c.first] = int(it - track_cams_.begin());
     }
     if (free_kf_slots_.empty()) {  // reclaim the slots of the oldest keyframes that are no longer active
-        for (auto it = kf_slot_.begin(); it != kf_slot_.end() && free_kf_slots_.size() < 32;) {
-            if (active_keyframe_ids_.count(it->first)) { ++it; continue; }
-            kba_track_drop_keyframe(track_, it->second);
-            free_kf_slots_.push_back(it->second);
-            it = kf_slot_.erase(it);
-        }
+        dropInactiveKeyframes(32);
         if (free_kf_slots_.empty()) return false;
     }
+    // before any slot is handed to kf: kf is not in the arena yet, so a slot given to it here would count as free
+    if (!reclaimLandmarkSlots(kf)) return false;
     std::vector<int32_t> lm, cam;
     std::vector<float> u, v, d;
     for (const auto& m : kf.measurements_) {
         auto it = lm_slot_.find(m.first);
         if (it == lm_slot_.end()) {
-            if (int(lm_slot_.size()) >= kTrackLandmarks) return false;
-            it = lm_slot_.emplace(m.first, int(lm_slot_.size())).first;
+            int s = int(slot_lm_.size());  // dense from 0 until the first reclaim, then from the free list first
+            if (!free_lm_slots_.empty()) {
+                s = free_lm_slots_.back();
+                free_lm_slots_.pop_back();
+                slot_lm_[size_t(s)] = m.first;
+            } else {
+                if (s >= track_landmarks_) return false;
+                slot_lm_.push_back(m.first);
+            }
+            it = lm_slot_.emplace(m.first, s).first;
+            // a landmark measured again after its slot was reclaimed: its host state goes up at the flush
+            if (landmarks_.count(m.first) && !new_landmarks_.count(m.first)) restore_landmarks_.insert(m.first);
         }
         for (const auto& cm : m.second) {
             lm.push_back(it->second); cam.push_back(cam_of.at(cm.first));
@@ -492,6 +498,51 @@ bool BundleAdjusterKeyframes::trackPush(const Keyframe& kf) {
     free_kf_slots_.pop_back();
     kf_slot_[kf.timestamp_] = slot;
     return true;
+}
+
+void BundleAdjusterKeyframes::set_track_capacity(int max_keyframes, int max_landmarks, int max_measurements) {
+    if (track_) throw std::logic_error("set_track_capacity: the device-resident store exists already");
+    track_keyframes_ = max_keyframes; track_landmarks_ = max_landmarks; track_measurements_ = max_measurements;
+}
+
+// the stored keyframes that are no longer active leave the store, oldest first, until max_free_kf_slots keyframe slots are free
+void BundleAdjusterKeyframes::dropInactiveKeyframes(size_t max_free_kf_slots) {
+    for (auto it = kf_slot_.begin(); it != kf_slot_.end() && free_kf_slots_.size() < max_free_kf_slots;) {
+        if (active_keyframe_ids_.count(it->first)) { ++it; continue; }
+        kba_track_drop_keyframe(track_, it->second);
+        free_kf_slots_.push_back(it->second);
+        it = kf_slot_.erase(it);
+    }
+}
+
+// Landmark slots for the landmarks of kf that have none.  When the free list and the unused capacity cannot cover them, the
+// slots no stored keyframe measures (kba_track_reclaim_landmarks) go on the free list: first as the store stands, then after the
+// stored keyframes that are no longer active have left it.  A landmark whose slot is reclaimed keeps its host state in landmarks_
+// and gets a slot again when a keyframe that measures it is pushed (restore_landmarks_).  false: still too few slots.
+bool BundleAdjusterKeyframes::reclaimLandmarkSlots(const Keyframe& kf) {
+    size_t need = 0;
+    for (const auto& m : kf.measurements_) need += lm_slot_.count(m.first) == 0;
+    auto room = [&] { return free_lm_slots_.size() + size_t(track_landmarks_) - slot_lm_.size(); };
+    for (int pass = 0; pass < 2 && need > room(); ++pass) {
+        if (pass == 1) dropInactiveKeyframes(size_t(track_keyframes_));
+        const int hi = int(slot_lm_.size());
+        std::vector<int32_t> free_slot(size_t(hi) + 1);
+        kba_reclaim_request q{0, hi};
+        kba_reclaim_out o{};
+        o.free_slot = free_slot.data();
+        if (kba_track_reclaim_landmarks(track_, &q, &o) != KBA_OK) return false;
+        for (int i = o.n_free - 1; i >= 0; --i) {  // descending onto the free list: the lowest slot is handed out first
+            const int s = free_slot[size_t(i)];
+            const LandmarkId id = slot_lm_[size_t(s)];
+            const auto it = lm_slot_.find(id);
+            if (it == lm_slot_.end() || it->second != s) continue;  // on the free list already
+            if (kf.measurements_.count(id)) continue;               // kf measures it: it keeps its slot
+            lm_slot_.erase(it);
+            restore_landmarks_.erase(id);
+            free_lm_slots_.push_back(s);
+        }
+    }
+    return need <= room();
 }
 
 // solve() on the device-resident window: only the selection goes up.  false: not possible for this window (caller rebuilds).
@@ -566,13 +617,22 @@ bool BundleAdjusterKeyframes::solveTracked(const std::vector<Keyframe*>& kfs, co
     return true;
 }
 
-// Landmark state the host changed since the store last saw it: position and weight of new landmarks (push()), positions the
-// rebuild path wrote (runWindow), weights set by updateLabels().  A landmark without a slot is not in the store: a new one waits
-// for its keyframe; any other landmark gets its slot in trackPush() only while it is still new, so its value goes up then.
-// false: the store could not be written.
+// Landmark state the host changed since the store last saw it: position and weight of new landmarks (push()) and of landmarks
+// that got a slot again after theirs was reclaimed, positions the rebuild path wrote (runWindow), weights set by updateLabels().
+// A landmark without a slot is not in the store: its value goes up when it gets one (a new one with its keyframe, a reclaimed
+// one through restore_landmarks_).  false: the store could not be written.
 bool BundleAdjusterKeyframes::flushLandmarks() {
     std::vector<int32_t> slots;
     std::vector<double> pos, wgt;
+    for (const auto id : restore_landmarks_) {
+        auto it = lm_slot_.find(id);
+        if (it == lm_slot_.end()) continue;
+        const Landmark& lm = *landmarks_.at(id);
+        slots.push_back(it->second); pos.insert(pos.end(), lm.pos.begin(), lm.pos.end()); wgt.push_back(lm.weight);
+    }
+    if (!slots.empty() && kba_track_set_landmarks(track_, int(slots.size()), slots.data(), pos.data(), wgt.data()) != KBA_OK) return false;
+    restore_landmarks_.clear();
+    slots.clear(); pos.clear(); wgt.clear();
     for (const auto id : new_landmarks_) {
         auto it = lm_slot_.find(id);
         if (it == lm_slot_.end()) continue;  // created, but its keyframe has not reached the store yet
@@ -609,8 +669,17 @@ bool BundleAdjusterKeyframes::adjustPoseTracked(Keyframe& kf, const std::vector<
     std::vector<int32_t> lm, cam;
     std::vector<float> u, v, d;
     for (const auto id : lm_ids) {  // ascending landmark id, cameras in measurement order inside: runWindow's observation order
-        const auto it = lm_slot_.find(id);
-        if (it == lm_slot_.end()) return false;  // never measured by a stored keyframe
+        auto it = lm_slot_.find(id);
+        if (it == lm_slot_.end()) {
+            // no stored keyframe measures it (any more): a slot from the free list, which is only filled once slots were
+            // reclaimed, with its host state (flushLandmarks below); without a free slot the frame goes the rebuild path
+            if (free_lm_slots_.empty()) return false;
+            const int s = free_lm_slots_.back();
+            free_lm_slots_.pop_back();
+            slot_lm_[size_t(s)] = id;
+            it = lm_slot_.emplace(id, s).first;
+            restore_landmarks_.insert(id);
+        }
         for (const auto& cm : kf.measurements_.at(id)) {
             lm.push_back(it->second); cam.push_back(cam_of.at(cm.first));
             u.push_back(cm.second.u); v.push_back(cm.second.v); d.push_back(cm.second.d);

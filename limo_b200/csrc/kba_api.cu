@@ -285,12 +285,15 @@ struct CreateBufs {
 struct UpkeepBufs {
     SelectStage stage;                     // the single calls: keyframe slots | landmark slots, one window's outputs
     SelectStage flow;                      // kba_track_frame_flow: one frame's lists and outputs, at its first call
+    SelectStage reclaim;                   // kba_track_reclaim_landmarks: the live keyframe slots and one range's outputs, at its first call
     unsigned long long* map = nullptr;     // [lm_cap] (stamp << 32) | payload by slot, all 0 (stamp 0: never a call's) at first
+    int* blk = nullptr;                    // [ceil(lm_cap / kReclaimChunk)] free slots per chunk of a reclaimed range
     unsigned stamp = 0;                    // the last stamp a call used
     std::vector<unsigned> kf_stamp, lm_stamp;  // duplicate checks: the check that named a slot last
     unsigned check = 0;
     ~UpkeepBufs() {
         if (map) cudaFree(map);
+        if (blk) cudaFree(blk);
     }
 };
 
@@ -340,6 +343,7 @@ struct kba_track_group {
     std::unique_ptr<SelectStage> create;   // kba_track_group_create_landmarks, allocated at its first call
     std::unique_ptr<SelectStage> upkeep;   // kba_track_group_deactivate_keyframes / _depth_costs, allocated at the first of them
     std::unique_ptr<SelectStage> flow;     // kba_track_group_frame_flow, allocated at its first call
+    std::unique_ptr<SelectStage> reclaim;  // kba_track_group_reclaim_landmarks, allocated at its first call
     const TrackSolver* last = &solver;
 };
 
@@ -2372,8 +2376,9 @@ static int upkeep_bufs(kba_track* t, std::string& why) {
     if (e != cudaSuccess) { why = std::string("cudaSetDevice: ") + cudaGetErrorString(e); return KBA_ERR_CUDA; }
     if (!t->upkeep) {
         std::unique_ptr<UpkeepBufs> ub(new UpkeepBufs());
-        const size_t L = (size_t)t->td.lm_cap;
-        if (cudaMalloc(&ub->map, sizeof(unsigned long long) * std::max<size_t>(L, 1)) != cudaSuccess) {
+        const size_t L = (size_t)t->td.lm_cap, C = (L + kReclaimChunk - 1) / kReclaimChunk;
+        if (cudaMalloc(&ub->map, sizeof(unsigned long long) * std::max<size_t>(L, 1)) != cudaSuccess ||
+            cudaMalloc(&ub->blk, sizeof(int) * std::max<size_t>(C, 1)) != cudaSuccess) {
             why = "out of memory for the upkeep buffers"; return KBA_ERR_CUDA;
         }
         cudaError_t me = cudaMemsetAsync(ub->map, 0, sizeof(unsigned long long) * L, t->h->stream);
@@ -2773,6 +2778,158 @@ int kba_track_group_frame_flow(kba_track_group* g, const kba_flow_request* req, 
     const int rc = flow_run(g->h, *g->flow, (int)ts.size(), ts.data(), qs.data(), os.data());
     if (rc != KBA_OK) return rc;
     g->last = &g->flow->counts;
+    return KBA_OK;
+}
+
+// ---------------------------------------------------------------------------------------------------------------------
+// free landmark slots of the stored window (include/kba_b200.h, kba_track_reclaim_landmarks / kba_track_group_reclaim_landmarks;
+// kernels in kba_reclaim.cu): a single call is a one-window call of reclaim_run
+// ---------------------------------------------------------------------------------------------------------------------
+// the largest download of one window of track t: positions, weights and slots of a range of lm_cap slots, and n_free
+static size_t reclaim_out_cap(const kba_track* t) { return 36 * (size_t)t->td.lm_cap + 4; }
+
+// every check of one request, before anything is uploaded; allocates the track's upkeep scratch at its first upkeep, flow or
+// reclaim call
+static int reclaim_check(kba_track* t, const kba_reclaim_request* q, const kba_reclaim_out* o, std::string& why) {
+    if (q->lo < 0 || q->hi < q->lo || q->hi > t->td.lm_cap) { why = "slot range not within [0, max_landmarks]"; return KBA_ERR_BAD_ARG; }
+    if (q->hi > q->lo && !o->free_slot) { why = "null argument"; return KBA_ERR_BAD_ARG; }
+    return upkeep_bufs(t, why);
+}
+
+// W checked requests of distinct tracks, none of them an empty range, as the W windows of one launch sequence: one upload (the
+// argument records of windows 1 .. W-1, then every window's live keyframe slots), one download (the positions of the windows that
+// ask for them | their weights | every window's slots | n_free of every window, each window's part sized for its whole range),
+// one synchronisation, then the scatter into the callers' outputs.  Window 0's record travels in the launch parameters.
+static int reclaim_run(kba_handle* h, SelectStage& st, int W, kba_track* const* ts, const kba_reclaim_request* const* qs,
+                       kba_reclaim_out* const* os) {
+    CU(cudaSetDevice(h->device));
+    cudaStream_t s = h->stream;
+    ReclaimGrid g;
+    size_t SP = 0, SW = 0, SN = 0;
+    for (int w = 0; w < W; ++w) {
+        const size_t n = (size_t)(qs[w]->hi - qs[w]->lo);
+        SN += n; SP += os[w]->pos ? n : 0; SW += os[w]->weight ? n : 0;
+        g.max_range = std::max(g.max_range, qs[w]->hi - qs[w]->lo);
+    }
+    const size_t o_lists = sizeof(ReclaimArgs) * (size_t)(W - 1);
+    const size_t o_w = 24 * SP, o_s = o_w + 8 * SW, o_n = o_s + 4 * SN, out_bytes = o_n + 4 * (size_t)W;
+    int* lists_h = reinterpret_cast<int*>(st.up.h + o_lists);
+    const int* lists_d = reinterpret_cast<const int*>(st.up.d + o_lists);
+    unsigned char* d = st.out.d;
+    ReclaimLaunch l;
+    l.rest = reinterpret_cast<const ReclaimArgs*>(st.up.d);
+    l.n_win = W;
+    size_t li = 0, cP = 0, cW = 0, cN = 0;
+    for (int w = 0; w < W; ++w) {
+        kba_track* t = ts[w];
+        UpkeepBufs& ub = *t->upkeep;
+        if (ub.stamp >= 0xfffffff0u) {  // the stamps wrap: the map starts over from all 0
+            CU(cudaMemsetAsync(ub.map, 0, sizeof(unsigned long long) * (size_t)t->td.lm_cap, s));
+            ub.stamp = 0;
+        }
+        ReclaimArgs a;
+        a.td = t->td;
+        a.kf_live = lists_d + li;
+        for (int k = 0; k < t->td.kf_cap; ++k) {
+            if (!t->kf_live[k]) continue;
+            lists_h[li + (size_t)a.n_live++] = k;
+            g.max_meas = std::max(g.max_meas, t->m_cnt[k]);
+        }
+        g.max_live = std::max(g.max_live, a.n_live);
+        const size_t n = (size_t)(qs[w]->hi - qs[w]->lo);
+        a.lo = qs[w]->lo; a.hi = qs[w]->hi;
+        a.stamp = ++ub.stamp;
+        a.map = ub.map; a.blk = ub.blk;
+        a.n_free = reinterpret_cast<int*>(d + o_n) + w;
+        a.free_slot = reinterpret_cast<int*>(d + o_s) + cN;
+        if (os[w]->pos) { a.pos = reinterpret_cast<double*>(d) + 3 * cP; cP += n; }
+        if (os[w]->weight) { a.weight = reinterpret_cast<double*>(d + o_w) + cW; cW += n; }
+        if (w == 0) l.w0 = a;
+        else memcpy(st.up.h + sizeof(ReclaimArgs) * (size_t)(w - 1), &a, sizeof(ReclaimArgs));
+        li += (size_t)a.n_live; cN += n;
+    }
+    const size_t up_bytes = o_lists + 4 * li;
+    CU(cudaMemcpyAsync(st.up.d, st.up.h, up_bytes, cudaMemcpyHostToDevice, s));
+    launch_reclaim(l, g, s);
+    cudaError_t e = cudaGetLastError();
+    if (e == cudaSuccess) e = cudaMemcpyAsync(st.out.h, st.out.d, out_bytes, cudaMemcpyDeviceToHost, s);
+    if (e == cudaSuccess) e = wait_stream(h);
+    if (e != cudaSuccess) {
+        // as upkeep_run: the maps go back to all 0, whatever stamps the failed sequence left in them
+        for (int w = 0; w < W; ++w) cudaMemsetAsync(ts[w]->upkeep->map, 0, sizeof(unsigned long long) * (size_t)ts[w]->td.lm_cap, s);
+        cudaStreamSynchronize(s);
+        return fail(KBA_ERR_CUDA, std::string("landmark reclaim: ") + cudaGetErrorString(e));
+    }
+    const unsigned char* hb = st.out.h;
+    const int32_t* n_free = reinterpret_cast<const int32_t*>(hb + o_n);
+    cP = cW = cN = 0;
+    for (int w = 0; w < W; ++w) {
+        kba_reclaim_out& o = *os[w];
+        const size_t n = (size_t)(qs[w]->hi - qs[w]->lo), nf = (size_t)n_free[w];
+        o.n_free = n_free[w];
+        if (nf) memcpy(o.free_slot, hb + o_s + 4 * cN, 4 * nf);
+        if (o.pos) { if (nf) memcpy(o.pos, hb + 24 * cP, 24 * nf); cP += n; }
+        if (o.weight) { if (nf) memcpy(o.weight, hb + o_w + 8 * cW, 8 * nf); cW += n; }
+        cN += n;
+    }
+    st.counts.h2d = (int64_t)up_bytes;
+    st.counts.d2h = (int64_t)out_bytes;
+    return KBA_OK;
+}
+
+int kba_track_reclaim_landmarks(kba_track* t, const kba_reclaim_request* req, kba_reclaim_out* out) {
+    static const std::string who = "kba_track_reclaim_landmarks: ";
+    if (!t || !req || !out) return fail(KBA_ERR_BAD_ARG, who + "null argument");
+    std::string why;
+    int rc = reclaim_check(t, req, out, why);
+    if (rc != KBA_OK) return fail(rc, who + why);
+    SelectStage& st = t->upkeep->reclaim;
+    if (req->hi == req->lo) {  // an empty range: nothing is free, no upload, no launch
+        out->n_free = 0;
+        st.counts.h2d = 0; st.counts.d2h = 0;
+        t->last = &st.counts;
+        return KBA_OK;
+    }
+    if (!st.up.d) {  // the first single call of the track: staging for every keyframe slot and a range of max_landmarks
+        if (st.alloc(4 * (size_t)t->td.kf_cap, reclaim_out_cap(t))) {
+            st.up.release(); st.out.release();
+            return fail(KBA_ERR_CUDA, who + "out of memory for the reclaim staging");
+        }
+    }
+    rc = reclaim_run(t->h, st, 1, &t, &req, &out);
+    if (rc == KBA_OK) t->last = &st.counts;
+    return rc;
+}
+
+int kba_track_group_reclaim_landmarks(kba_track_group* g, const kba_reclaim_request* req, kba_reclaim_out* out) {
+    static const std::string who = "kba_track_group_reclaim_landmarks: ";
+    if (!g || !req || !out) return fail(KBA_ERR_BAD_ARG, who + "null argument");
+    const int n = (int)g->tracks.size();
+    std::vector<kba_track*> ts;
+    std::vector<const kba_reclaim_request*> qs;
+    std::vector<kba_reclaim_out*> os;
+    for (int i = 0; i < n; ++i) {
+        if (req[i].hi == req[i].lo) continue;  // sits the call out
+        std::string why;
+        const int rc = reclaim_check(g->tracks[i], &req[i], &out[i], why);
+        if (rc != KBA_OK) return fail(rc, who + "track " + std::to_string(i) + ": " + why);
+        ts.push_back(g->tracks[i]); qs.push_back(&req[i]); os.push_back(&out[i]);
+    }
+    if (ts.empty()) {  // every track sits out: no upload, no launch
+        g->solver.h2d = 0; g->solver.d2h = 0;
+        g->last = &g->solver;
+        return KBA_OK;
+    }
+    if (!g->reclaim) {  // staging for every track at its capacities, allocated once
+        size_t kfs = 0, outs = 0;
+        for (const kba_track* t : g->tracks) { kfs += (size_t)t->td.kf_cap; outs += reclaim_out_cap(t); }
+        std::unique_ptr<SelectStage> st(new SelectStage());
+        if (st->alloc(sizeof(ReclaimArgs) * (size_t)(n - 1) + 4 * kfs, outs)) return fail(KBA_ERR_CUDA, who + "out of memory for the reclaim staging");
+        g->reclaim = std::move(st);
+    }
+    const int rc = reclaim_run(g->h, *g->reclaim, (int)ts.size(), ts.data(), qs.data(), os.data());
+    if (rc != KBA_OK) return rc;
+    g->last = &g->reclaim->counts;
     return KBA_OK;
 }
 

@@ -255,6 +255,34 @@ struct FlowGrid {
 };
 void launch_frame_flow(const FlowLaunch& l, const FlowGrid& g, cudaStream_t s);
 
+// ---- free landmark slots of a track's store (kba_track_reclaim_landmarks / kba_track_group_reclaim_landmarks, kba_reclaim.cu) ----
+// One window = one request: the slot range [lo, hi) and the track's live keyframe slots.  The slot map is the track's upkeep map:
+// every arena entry of a live keyframe is marked with the call's stamp, the unmarked slots of the range are the free ones.
+constexpr int kReclaimChunk = 1024;        // slots of the range per block of k_rc_count / k_rc_write (256 threads, 4 slots each)
+struct ReclaimArgs {
+    TrackDev td;
+    const int* kf_live = nullptr;          // [n_live] live keyframe slots
+    int n_live = 0, lo = 0, hi = 0;
+    unsigned stamp = 0;
+    unsigned long long* map = nullptr;     // [lm_cap] scratch, by slot
+    int* blk = nullptr;                    // [ceil(lm_cap / kReclaimChunk)] scratch: free slots per chunk of the range
+    // outputs
+    int* n_free = nullptr;                 // [1]
+    int* free_slot = nullptr;              // [hi - lo]
+    double* pos = nullptr;                 // [3 * (hi - lo)] or null
+    double* weight = nullptr;              // [hi - lo] or null
+};
+struct ReclaimLaunch {
+    ReclaimArgs w0;
+    const ReclaimArgs* rest = nullptr;     // [n_win - 1]
+    int n_win = 0;
+};
+struct ReclaimGrid {
+    int max_live = 0, max_meas = 0;        // live keyframes of a window, arena entries of a live keyframe
+    int max_range = 0;                     // hi - lo
+};
+void launch_reclaim(const ReclaimLaunch& l, const ReclaimGrid& g, cudaStream_t s);
+
 // ---- motion-only frames against a track's store (kba_track_adjust_pose / kba_track_group_adjust_pose, kba_motion.cu) ----
 // One frame = one free pose against constant landmarks read from a store by slot: its measurements come in runs, one run per
 // landmark (the landmarks of the equivalent window, in the caller's order).
