@@ -354,9 +354,9 @@ int kba_track_transfer_bytes(kba_track* t, int64_t* h2d_last_solve, int64_t* d2h
 /* ---- landmark selection on the stored window (SURVEY row A17) ---------------------------------------------------------
  * The per-landmark quantities of limo's selection chain (landmark_selector.hpp:118-253 with LandmarkRejectionSchemeCheirality and
  * LandmarkSparsificationSchemeVoxel, as facade/landmark_selection.cpp states them), computed from what the store holds: keyframe
- * poses, the measurement arena, landmark positions by slot, the cameras.  The host keeps the ranking that consumes them (the
- * partial sorts, the std::rand shuffle of the middle bin, the bin caps), so a caller that ranks as LandmarkSelector::select does
- * gets its selection bit for bit.  A request:
+ * poses, the measurement arena, landmark positions by slot, the cameras.  A caller that ranks them as LandmarkSelector::select
+ * does (the partial sorts, the std::rand shuffle of the middle bin, the bin caps) gets its selection bit for bit;
+ * kba_track_rank_landmarks (below) does that ranking on the device instead.  A request:
  *   - kf_slot [n_kf]: the active keyframes in ascending timestamp (= id) order, every one pushed; the last one is the newest;
  *   - lm_slot [n_cand]: the candidates, i.e. the active landmarks minus the outliers, in ascending id order (<= max_landmarks).
  * Per candidate c:
@@ -694,6 +694,103 @@ typedef struct kba_reclaim_out {  /* caller-owned */
 int kba_track_reclaim_landmarks(kba_track* t, const kba_reclaim_request* req, kba_reclaim_out* out);
 /* req[n_tracks], out[n_tracks] */
 int kba_track_group_reclaim_landmarks(kba_track_group* g, const kba_reclaim_request* req, kba_reclaim_out* out);
+
+/* ---- ranked landmark selection on the stored window, and the solve of that ranking (SURVEY row A17) ------------------------
+ * kba_track_select_landmarks leaves the ranking of its quantities to the host; kba_track_rank_landmarks ranks them on the
+ * device as LandmarkSelector::select (facade/landmark_selection.cpp) does for limo's chain -- cheirality, voxel, AddDepth with
+ * limo's sorter -- and keeps the ranked selection on the track, where kba_track_solve_ranked reads it.  A request:
+ *   - kf_slot [n_kf], lm_slot [n_cand], params: exactly as for kba_track_select_landmarks (n_cand <= 57344);
+ *   - elig [n_cand] or NULL (none): the AddDepth comparator's verdict per candidate (limo: is_ground_plane);
+ *   - max_near, max_middle, max_far: the voxel scheme's caps (max_num_landmarks_{near,middle,far});
+ *   - depth [n_depth] (n_depth <= 1024): the AddDepth scheme's (FrameIndex, NumberLandmarks) entries; an entry with
+ *     ind >= n_kf is skipped, as the scheme skips it;
+ *   - draw, draw_ctx: the random source of the middle bin's shuffle (below).
+ * The ranking, bit for bit the facade's from the same store state, ties included:
+ *   - near: the near representatives with a flow, in near order, std::partial_sort_copy by flow descending, capped;
+ *   - middle: the middle representatives in candidate order, libstdc++'s random_shuffle (for i = 1 .. n - 1: j = draw % (i + 1),
+ *     swap), the first max_middle kept;
+ *   - far: the far candidates in candidate order, std::partial_sort_copy by seen descending, capped;
+ *   - AddDepth, per entry (ind, wanted): the cheirality survivors with elig set that keyframe kf_slot[ind] measures, in its arena
+ *     order, with kba_track_depth_costs' cost; std::partial_sort ascending, the first min(wanted, n) kept.
+ * Each partial sort replays libstdc++'s heap (make_heap, __adjust_heap), so the tied elements it keeps are the host's.
+ * The selection is the union of the bins and the AddDepth picks in ascending candidate order.  Outputs:
+ *   - n_sel, and cand [n_sel] (candidate indices, ascending) with category [n_sel]: 0 near, 1 middle, 2 far, 3 AddDepth only;
+ *     the caller allocates both for n_cand entries;
+ *   - n_ground: the selected candidates with elig set, which kba_track_solve_ranked can attach on the device;
+ *   - n_draws: the draws the shuffle used, max(n_middle - 1, 0).
+ * Draws: the shuffle needs exactly max(n_middle - 1, 0) of them, which is known on the device only.  The call therefore
+ * synchronises once in its middle: after the chain's quantities it downloads 4 bytes per window (the middle bin's size), calls
+ * draw(draw_ctx, n, out) once for a request that needs n > 0 draws (requests in order, before any ranking kernel runs) and
+ * uploads the draws.  A draw function returning nonzero, or a NULL one where draws are needed, fails the call with
+ * KBA_ERR_BAD_ARG after that synchronisation: no output is written and the track keeps no ranking.  A caller whose draw function
+ * fills out[] with std::rand() gets the facade's selection and leaves std::rand's sequence where the facade's select() leaves it.
+ * The track keeps the ranked slots, the ground candidates and the keyframe list until its next ranking.  The ranking goes stale
+ * at any call that changes the store: push, drop, set_landmarks, set_keyframe_pose(s), create_landmarks, reclaim_landmarks and
+ * every solve (alone or in a group, ranked or not).
+ * Transfers (kba_track_transfer_bytes; over the W requests that do not sit out for kba_track_group_transfer_bytes, R the size of
+ * one window's argument records, a constant of the library build; D_w = max(n_middle_w - 1, 0) the draws of request w;
+ * B_w = min(n_cand, min(max_near, n_cand) + min(max_middle, n_middle) + min(max_far, n_cand) + sum of min(wanted, n_cand)),
+ * the bound of its selection; elig bytes travel also when elig is NULL):
+ *         h2d = sum(4 * (n_kf + n_cand) + n_cand + 8 * n_depth) + R * (W - 1) + 8 * W + 4 * sum(D_w)
+ *         d2h = 4 * W + sum(8 + 5 * B_w)
+ * Two uploads (the lists; then the output offsets and the draws), one launch sequence in two parts, two downloads (the middle
+ * bin's sizes; then the outputs), two synchronisations.  The first call of a track by either entry point allocates its ranking
+ * buffers (and its selection scratch, if no selection allocated it), the first single call its staging; later calls allocate
+ * nothing.
+ * Errors, before anything is uploaded or written: those of kba_track_select_landmarks, a null out.cand / out.category with
+ * n_cand > 0, a negative cap, n_depth < 0, depth NULL with n_depth > 0, an entry with ind < 0 or wanted < 0: KBA_ERR_BAD_ARG;
+ * n_cand > 57344, n_depth > 1024, or an entry with min(wanted, arena entries of kf_slot[ind]) > 57344: KBA_ERR_CAPACITY.
+ * kba_track_group_rank_landmarks ranks one request per track of a group in one launch sequence (window = request): out[i] and
+ * track i's ranking are bit for bit what kba_track_rank_landmarks(tracks[i], &req[i], &out[i]) gives, draws included (each
+ * request's draw function is called with its own count); a request with n_kf == 0 sits the call out (out[i] not written, its
+ * ranking kept); every other request is checked before anything is uploaded; a failing one returns its code and
+ * kba_last_error names its track. */
+typedef struct kba_depth_entry {
+    int32_t ind;                /* FrameIndex: kf_slot[ind] (0 the oldest listed keyframe)                                    */
+    int32_t wanted;             /* NumberLandmarks                                                                            */
+} kba_depth_entry;
+typedef struct kba_rank_request {
+    int32_t n_kf;               /* 0 (group call): this track sits the call out                                              */
+    int32_t n_cand;
+    const int32_t* kf_slot;     /* [n_kf]   as for kba_track_select_landmarks                                               */
+    const int32_t* lm_slot;     /* [n_cand] as for kba_track_select_landmarks                                               */
+    const uint8_t* elig;        /* [n_cand] or NULL (no candidate is eligible)                                               */
+    const kba_select_params* params;
+    int32_t max_near, max_middle, max_far;
+    int32_t n_depth;
+    const kba_depth_entry* depth;  /* [n_depth] */
+    int32_t (*draw)(void* ctx, int32_t n, int32_t* out);  /* fills out[0 .. n); 0 = success */
+    void* draw_ctx;
+} kba_rank_request;
+typedef struct kba_rank_out {   /* caller-owned */
+    int32_t n_sel;
+    int32_t n_ground;
+    int32_t n_draws;
+    int32_t reserved_;
+    int32_t* cand;              /* [n_cand]; the first n_sel are written                                                     */
+    int8_t* category;           /* [n_cand]; the first n_sel are written                                                     */
+} kba_rank_out;
+int kba_track_rank_landmarks(kba_track* t, const kba_rank_request* req, kba_rank_out* out);
+/* req[n_tracks], out[n_tracks] */
+int kba_track_group_rank_landmarks(kba_track_group* g, const kba_rank_request* req, kba_rank_out* out);
+/* kba_track_solve on the track's last ranking: lm_slot is the ranked selection (n_lm = n_sel), in ranked order, and the results'
+ * landmark arrays follow it.  sel as for kba_track_solve, except that gp_lm, gp_kf and gp_weight all NULL with n_gp > 0 attach
+ * the ranking's ground candidates on the device (none: no ground-plane residuals, as kba_track_solve with n_gp = 0); host lists
+ * and caller candidates index the ranked selection.  Nothing about the selection is uploaded.  Errors, before anything is
+ * uploaded: no ranking, a stale one, or kf_slot different from the ranking's keyframe list: KBA_ERR_BAD_ARG; then those of
+ * kba_track_solve.  The results equal kba_track_solve's on the same lists bit for bit, and the solve makes the ranking stale. */
+int kba_track_solve_ranked(kba_track* t, int32_t n_kf, const int32_t* kf_slot, const uint8_t* kf_fixed, const kba_window* sel,
+                           const kba_options* opt, kba_result* res);
+typedef struct kba_ranked_request {
+    int32_t n_kf;               /* 0: this track sits this solve out (as for kba_track_group_solve)                           */
+    int32_t reserved_;
+    const int32_t* kf_slot;
+    const uint8_t* kf_fixed;
+    const kba_window* sel;
+} kba_ranked_request;
+/* kba_track_group_solve on every track's last ranking; each request is checked as kba_track_solve_ranked checks it.
+ * req[n_tracks], res[n_tracks] */
+int kba_track_group_solve_ranked(kba_track_group* g, const kba_ranked_request* req, const kba_options* opt, kba_result* res);
 
 /* ---- adjustPoseOnly against the persistent store: one frame's pose per call, or one frame of each track of a group -------
  * What limo calls on every frame (bundle_adjuster_keyframes.cpp:820-888): one free pose against constant landmarks, the optional

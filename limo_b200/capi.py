@@ -9,7 +9,7 @@ import os
 
 import numpy as np
 
-from .capi_types import (KbaCounters, KbaCreateOut, KbaCreateRequest, KbaDeactivateOut, KbaDeactivateRequest, KbaDepthOut, KbaDepthRequest, KbaEvalOut, KbaFlowOut, KbaFlowRequest, KbaLidarOptions, KbaOptions, KbaReclaimOut, KbaReclaimRequest, KbaResult, KbaSelectOut, KbaSelectParams, KbaSelectRequest,
+from .capi_types import (KbaCounters, KbaCreateOut, KbaCreateRequest, KbaDeactivateOut, KbaDeactivateRequest, KbaDepthEntry, KbaDepthOut, KbaDepthRequest, KbaDrawFn, KbaEvalOut, KbaFlowOut, KbaFlowRequest, KbaLidarOptions, KbaOptions, KbaRankedRequest, KbaRankOut, KbaRankRequest, KbaReclaimOut, KbaReclaimRequest, KbaResult, KbaSelectOut, KbaSelectParams, KbaSelectRequest,
                          KbaTrackCaps, KbaTrackFrame, KbaTrackRequest, KbaWindow, Result, Window, c_double_p, c_int32_p)
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
@@ -28,11 +28,43 @@ SYMBOLS = ["kba_version", "kba_last_error", "kba_default_options", "kba_create",
            "kba_track_adjust_pose", "kba_track_group_adjust_pose", "kba_track_select_landmarks", "kba_track_group_select_landmarks",
            "kba_track_create_landmarks", "kba_track_group_create_landmarks", "kba_track_deactivate_keyframes",
            "kba_track_group_deactivate_keyframes", "kba_track_depth_costs", "kba_track_group_depth_costs", "kba_track_frame_flow",
-           "kba_track_group_frame_flow", "kba_track_reclaim_landmarks", "kba_track_group_reclaim_landmarks"]
+           "kba_track_group_frame_flow", "kba_track_reclaim_landmarks", "kba_track_group_reclaim_landmarks",
+           "kba_track_rank_landmarks", "kba_track_group_rank_landmarks", "kba_track_solve_ranked", "kba_track_group_solve_ranked"]
 
 
 class KbaError(RuntimeError):
     pass
+
+
+# LandmarkSparsificationSchemeVoxel::Parameters' bin caps: the defaults of a ranking request
+RANK_DEFAULTS = dict(max_near=300, max_middle=300, max_far=300)
+
+
+def _draw_source(draws):
+    """the kba_rank_request draw function of `draws`: a callable n -> n ints, an array consumed from its start, or None (no
+    function: a request that needs draws fails)"""
+    if draws is None:
+        return KbaDrawFn()
+    if callable(draws):
+        take = draws
+    else:
+        src = np.ascontiguousarray(draws, dtype=np.int64).ravel()
+
+        def take(n):
+            if n > len(src):
+                raise ValueError("%d draws asked, %d given" % (n, len(src)))
+            return src[:n]
+
+    def fn(_ctx, n, out):
+        try:
+            v = np.ascontiguousarray(np.asarray(take(int(n)), dtype=np.int64).ravel().astype(np.int32))  # alive until the copy
+            if len(v) != n:
+                return 1
+            C.memmove(out, v.ctypes.data, 4 * int(n))
+            return 0
+        except Exception:  # a failing source fails the call (KBA_ERR_BAD_ARG), it must not unwind through C
+            return 1
+    return KbaDrawFn(fn)
 
 
 # LandmarkSparsificationSchemeVoxel::Parameters' values: the defaults of a selection request
@@ -113,6 +145,10 @@ def lib():
         L.kba_track_group_frame_flow.argtypes = [vp, C.POINTER(KbaFlowRequest), C.POINTER(KbaFlowOut)]
         L.kba_track_reclaim_landmarks.argtypes = [vp, C.POINTER(KbaReclaimRequest), C.POINTER(KbaReclaimOut)]
         L.kba_track_group_reclaim_landmarks.argtypes = [vp, C.POINTER(KbaReclaimRequest), C.POINTER(KbaReclaimOut)]
+        L.kba_track_rank_landmarks.argtypes = [vp, C.POINTER(KbaRankRequest), C.POINTER(KbaRankOut)]
+        L.kba_track_group_rank_landmarks.argtypes = [vp, C.POINTER(KbaRankRequest), C.POINTER(KbaRankOut)]
+        L.kba_track_solve_ranked.argtypes = [vp, C.c_int32, ip, u8p, C.POINTER(KbaWindow), C.POINTER(KbaOptions), C.POINTER(KbaResult)]
+        L.kba_track_group_solve_ranked.argtypes = [vp, C.POINTER(KbaRankedRequest), C.POINTER(KbaOptions), C.POINTER(KbaResult)]
         L.kba_lidar_default_options.argtypes = [C.POINTER(KbaLidarOptions)]
         L.kba_lidar_default_options.restype = None
         fp = C.POINTER(C.c_float)
@@ -202,6 +238,7 @@ class Track:
         """win_rows: largest reduced system a solve may need (6 rows per keyframe, 10 with plane blocks, plus one); 0 keeps the
         fused path's limits (30 keyframes, 18 with plane blocks), beyond 184 the track also owns a large-window solver"""
         self.handle = handle
+        self._n_sel = None  # size of the track's last ranking (rank_landmarks, alone or in a group): what solve_ranked returns
         caps = KbaTrackCaps(max_keyframes, max_landmarks, max_measurements, win_keyframes, win_landmarks, win_observations, win_ground,
                             win_rows)
         intr = np.ascontiguousarray(cam_intr, dtype=np.float64).reshape(-1, 3)
@@ -429,6 +466,62 @@ class Track:
         _check(lib().kba_track_reclaim_landmarks(self._p, C.byref(q), C.byref(o)))
         return self._reclaim_result(o, res, evict)
 
+    @staticmethod
+    def _rank_args(kf_slots, lm_slots, elig=None, voxel_size=SELECT_DEFAULTS["voxel_size"], roi_far=SELECT_DEFAULTS["roi_far"],
+                   roi_middle=SELECT_DEFAULTS["roi_middle"], max_near=RANK_DEFAULTS["max_near"], max_middle=RANK_DEFAULTS["max_middle"],
+                   max_far=RANK_DEFAULTS["max_far"], depth=(), draws=None):
+        """fill a kba_rank_request; returns (request, out, result arrays, what must stay alive during the call)"""
+        kf, kfp = Track._i32(kf_slots)
+        lm, lmp = Track._i32(lm_slots)
+        n = len(lm)
+        el = None if elig is None else np.ascontiguousarray(elig, dtype=np.uint8).reshape(n)
+        dp = np.ascontiguousarray(np.asarray(depth, dtype=np.int32).reshape(-1, 2))
+        p = KbaSelectParams((C.c_double * 3)(*[float(x) for x in voxel_size]), float(roi_far), float(roi_middle))
+        cand, cat = np.zeros(n, np.int32), np.zeros(n, np.int8)
+        fn = _draw_source(draws)
+        q = KbaRankRequest(n_kf=len(kf), n_cand=n, kf_slot=kfp, lm_slot=lmp,
+                           elig=C.cast(None, C.POINTER(C.c_uint8)) if el is None else el.ctypes.data_as(C.POINTER(C.c_uint8)),
+                           params=C.cast(C.pointer(p), C.c_void_p), max_near=int(max_near), max_middle=int(max_middle), max_far=int(max_far),
+                           n_depth=len(dp), depth=dp.ctypes.data_as(C.POINTER(KbaDepthEntry)), draw=fn)
+        o = KbaRankOut(cand=cand.ctypes.data_as(c_int32_p), category=cat.ctypes.data_as(C.POINTER(C.c_int8)))
+        return q, o, (cand, cat), (kf, lm, el, dp, p, fn)
+
+    @staticmethod
+    def _rank_result(o, res):
+        cand, cat = res
+        return dict(cand=cand[:o.n_sel].copy(), category=cat[:o.n_sel].copy(), n_ground=o.n_ground, n_draws=o.n_draws)
+
+    def rank_landmarks(self, kf_slots, lm_slots, elig=None, draws=None, **kw):
+        """The ranked selection of limo's chain on this track's store (kba_track_rank_landmarks): the arguments of select_landmarks,
+        elig [n_cand] (the AddDepth comparator per candidate, None: none), the caps max_near / max_middle / max_far, depth: the
+        AddDepth (FrameIndex, NumberLandmarks) entries, draws: the middle bin's random source -- a callable n -> n ints, or an
+        array whose first n entries are taken (too short: the call fails), or None when no draw can be needed.  Returns a dict:
+        cand (ascending candidate indices), category (0 near, 1 middle, 2 far, 3 AddDepth only), n_ground, n_draws.  The track
+        keeps the ranking for solve_ranked."""
+        q, o, res, _keep = self._rank_args(kf_slots, lm_slots, elig=elig, draws=draws, **kw)
+        _check(lib().kba_track_rank_landmarks(self._p, C.byref(q), C.byref(o)))
+        self._n_sel = o.n_sel
+        return self._rank_result(o, res)
+
+    def _ranked_selection(self, kf_slots, kf_fixed, ground=False, **scalars):
+        """the arrays of a solve of this track's last ranking, its results sized for that ranking"""
+        if self._n_sel is None:
+            raise KbaError("solve_ranked: the track has no ranking to solve (rank_landmarks)")
+        kf, fx, _lm, sel = Track._selection(kf_slots, kf_fixed, np.zeros(self._n_sel, np.int32), **scalars)
+        if ground:  # the ranking's ground candidates, attached on the device: n_gp > 0 with no lists
+            sel.c.n_gp = 1
+        return kf, fx, sel
+
+    def solve_ranked(self, kf_slots, kf_fixed, opt=None, ground=False, **scalars):
+        """solve() on this track's last ranking (kba_track_solve_ranked), made by rank_landmarks of this track or of a TrackGroup:
+        ground=True attaches its ground candidates on the device; the other scalars as for solve (gp_* lists index the ranking).
+        Results come in ranked order, sized for the ranking."""
+        kf, fx, sel = self._ranked_selection(kf_slots, kf_fixed, ground, **scalars)
+        res = Result(sel, 256)
+        _check(lib().kba_track_solve_ranked(self._p, len(kf), kf.ctypes.data_as(c_int32_p), fx.ctypes.data_as(C.POINTER(C.c_uint8)),
+                                            C.byref(sel.c), C.byref(opt or default_options()), C.byref(res.c)))
+        return res
+
     def transfer_bytes(self):
         a, b, c = C.c_int64(), C.c_int64(), C.c_int64()
         _check(lib().kba_track_transfer_bytes(self._p, C.byref(a), C.byref(b), C.byref(c)))
@@ -652,6 +745,56 @@ class TrackGroup:
                 results[i] = Track._reclaim_result(KbaReclaimOut(), Track._reclaim_args(0, 0, r.get("evict", False))[2], r.get("evict", False))
             else:
                 results[i] = Track._reclaim_result(outs[i], *keep[i])
+        return results
+
+    def rank_landmarks(self, requests):
+        """The ranked selection of every track in one launch sequence (kba_track_group_rank_landmarks): each entry None (the track
+        sits the call out, its ranking kept) or a dict with the arguments of Track.rank_landmarks.  Returns one result dict per
+        track, None for a track that sat out."""
+        assert len(requests) == len(self.tracks)
+        n = len(requests)
+        reqs, outs = (KbaRankRequest * n)(), (KbaRankOut * n)()
+        keep, results = [], [None] * n
+        for i, r in enumerate(requests):
+            if r is None:
+                continue
+            q, o, res, lists = Track._rank_args(**r)
+            if q.n_kf == 0:  # n_kf = 0 would sit the track out: a request without keyframes is an error, as for one track
+                raise KbaError("kba_track_group_rank_landmarks: track %d: no keyframes or a negative size" % i)
+            reqs[i], outs[i] = q, o
+            keep.append(lists)
+            results[i] = res
+        _check(lib().kba_track_group_rank_landmarks(self._p, reqs, outs))
+        for i, r in enumerate(results):
+            if r is not None:
+                self.tracks[i]._n_sel = outs[i].n_sel
+        return [None if r is None else Track._rank_result(outs[i], r) for i, r in enumerate(results)]
+
+    def solve_ranked(self, requests, opt=None, iterations_capacity=256):
+        """solve_ranked for every track as one batch (kba_track_group_solve_ranked): each entry None (the track sits this solve out)
+        or a dict with the arguments of Track.solve_ranked (kf_slots, kf_fixed, ground and the scalar keywords).  Returns one
+        Result per track, sized for its ranking."""
+        assert len(requests) == len(self.tracks)
+        reqs = (KbaRankedRequest * len(requests))()
+        keep, results = [], []
+        for i, r in enumerate(requests):
+            if r is None:
+                sel = Window(np.tile([1.0, 0, 0, 0, 0, 0, 0], (0, 1)), [], [[1.0, 0, 0]], [[1.0, 0, 0, 0, 0, 0, 0]], np.zeros((0, 3)), [],
+                             [0], [], [], [], [])
+                results.append(Result(sel, 1))
+                continue
+            r = dict(r)
+            kf, fx, sel = self.tracks[i]._ranked_selection(r.pop("kf_slots"), r.pop("kf_fixed"), r.pop("ground", False), **r)
+            q = reqs[i]
+            q.n_kf = len(kf)
+            q.kf_slot, q.kf_fixed = kf.ctypes.data_as(c_int32_p), fx.ctypes.data_as(C.POINTER(C.c_uint8))
+            q.sel = C.cast(C.pointer(sel.c), C.c_void_p)
+            keep.append((kf, fx, sel))
+            results.append(Result(sel, iterations_capacity))
+        rarr = (KbaResult * len(results))(*[r.c for r in results])
+        _check(lib().kba_track_group_solve_ranked(self._p, reqs, C.byref(opt or default_options()), rarr))
+        for r, c in zip(results, rarr):
+            r.c = c
         return results
 
     def transfer_bytes(self):

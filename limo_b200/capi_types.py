@@ -101,6 +101,29 @@ class KbaReclaimOut(C.Structure):
     _fields_ = [("n_free", C.c_int32), ("reserved_", C.c_int32), ("free_slot", c_int32_p), ("pos", c_double_p), ("weight", c_double_p)]
 
 
+class KbaDepthEntry(C.Structure):
+    _fields_ = [("ind", C.c_int32), ("wanted", C.c_int32)]
+
+
+# int32_t (*draw)(void* ctx, int32_t n, int32_t* out) of kba_rank_request
+KbaDrawFn = C.CFUNCTYPE(C.c_int32, C.c_void_p, C.c_int32, c_int32_p)
+
+
+class KbaRankRequest(C.Structure):
+    _fields_ = [("n_kf", C.c_int32), ("n_cand", C.c_int32), ("kf_slot", c_int32_p), ("lm_slot", c_int32_p), ("elig", c_uint8_p),
+                ("params", C.c_void_p), ("max_near", C.c_int32), ("max_middle", C.c_int32), ("max_far", C.c_int32), ("n_depth", C.c_int32),
+                ("depth", C.POINTER(KbaDepthEntry)), ("draw", KbaDrawFn), ("draw_ctx", C.c_void_p)]
+
+
+class KbaRankOut(C.Structure):
+    _fields_ = [("n_sel", C.c_int32), ("n_ground", C.c_int32), ("n_draws", C.c_int32), ("reserved_", C.c_int32), ("cand", c_int32_p),
+                ("category", C.POINTER(C.c_int8))]
+
+
+class KbaRankedRequest(C.Structure):
+    _fields_ = [("n_kf", C.c_int32), ("reserved_", C.c_int32), ("kf_slot", c_int32_p), ("kf_fixed", c_uint8_p), ("sel", C.c_void_p)]
+
+
 class KbaTrackFrame(C.Structure):
     _fields_ = [("n_meas", C.c_int32), ("reserved_", C.c_int32), ("pose7", c_double_p), ("lm_slot", c_int32_p), ("cam", c_int32_p),
                 ("u", c_float_p), ("v", c_float_p), ("d", c_float_p), ("speed_weight", C.c_double), ("speed_dt", C.c_double),

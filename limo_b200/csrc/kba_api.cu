@@ -297,6 +297,33 @@ struct UpkeepBufs {
     }
 };
 
+// buffers of a track's ranked selections (kba_rank.cu), kept like SelectBufs: the quantities, the scratch and the ranking at its first
+// ranking, alone or in a group; the staging at its first single call.  The ranking is what kba_track_solve_ranked reads.
+struct RankBufs {
+    SelectStage stage;                     // kba_track_rank_landmarks: one window's lists, draws and outputs
+    unsigned char* qty = nullptr;          // the chain's quantities, as select_run lays out one window's: flow | seen | near order |
+                                           // counters | cheirality | bins, for lm_cap candidates
+    int* mark = nullptr;                   // [lm_cap]
+    int* dcand = nullptr;                  // [m_cap]
+    double* dcost = nullptr;               // [m_cap]
+    int* dcnt = nullptr;                   // [kf_cap]
+    int* sel_slot = nullptr;               // [lm_cap] the ranked slots
+    int* gp = nullptr;                     // [lm_cap] the ranked ground candidates
+    std::vector<int> kf;                   // the ranking's keyframe list
+    int n_sel = 0, n_ground = 0;
+    uint64_t gen = 0;                      // kba_track::gen when it was ranked
+    bool valid = false;
+    std::vector<void*> dev;
+    template <typename T> int alloc(T** p, size_t n) {
+        void* q = nullptr;
+        if (cudaMalloc(&q, std::max<size_t>(n, 1) * sizeof(T)) != cudaSuccess) return 1;
+        dev.push_back(q); *p = (T*)q; return 0;
+    }
+    ~RankBufs() {
+        for (void* p : dev) cudaFree(p);
+    }
+};
+
 // persistent, device-resident window (kba_track_*, at the end of this file)
 struct kba_track {
     kba_handle* h = nullptr;
@@ -308,6 +335,8 @@ struct kba_track {
     std::unique_ptr<SelectBufs> select;    // kba_track_select_landmarks, allocated at its first call
     std::unique_ptr<CreateBufs> create;    // kba_track_create_landmarks, allocated at its first call
     std::unique_ptr<UpkeepBufs> upkeep;    // kba_track_deactivate_keyframes / kba_track_depth_costs, allocated at the first of them
+    std::unique_ptr<RankBufs> rank;        // kba_track_rank_landmarks, allocated at its first call
+    uint64_t gen = 0;                      // counts the calls that changed the store: a ranking of an older generation is stale
     TrackDev td{};
     int* arena_i[2][2] = {{nullptr, nullptr}, {nullptr, nullptr}};      // [buffer][lm, cam]
     float* arena_f[2][3] = {{nullptr, nullptr, nullptr}, {nullptr, nullptr, nullptr}};  // [buffer][u, v, d]
@@ -344,6 +373,7 @@ struct kba_track_group {
     std::unique_ptr<SelectStage> upkeep;   // kba_track_group_deactivate_keyframes / _depth_costs, allocated at the first of them
     std::unique_ptr<SelectStage> flow;     // kba_track_group_frame_flow, allocated at its first call
     std::unique_ptr<SelectStage> reclaim;  // kba_track_group_reclaim_landmarks, allocated at its first call
+    std::unique_ptr<SelectStage> rank;     // kba_track_group_rank_landmarks, allocated at its first call
     const TrackSolver* last = &solver;
 };
 
@@ -1437,6 +1467,7 @@ void kba_track_destroy(kba_track* t) {
     t->select.reset();
     t->create.reset();
     t->upkeep.reset();
+    t->rank.reset();
     for (void* p : t->dev) cudaFree(p);
     t->p_lm.release(); t->p_cam.release(); t->lay.release();
     t->p_u.release(); t->p_v.release(); t->p_d.release(); t->p_dbl.release(); t->p_slot.release();
@@ -1501,6 +1532,8 @@ struct TrackRequest {
     bool device_gp = false;                // filled by track_check: sel->gp_lm lists candidates, attached by k_track_ground
     int rows = 0;                          // filled by track_check: reduced rows kba_batch_create sizes the window for (reduced_rows,
                                            // plane blocks counted whenever candidates are given)
+    bool ranked = false;                   // the landmarks are the track's ranking (kba_track_solve_ranked): lm_slot is not read
+    bool rank_gp = false;                  // ... and so are the ground-plane candidates (sel->n_gp of them)
 };
 
 // ground points attached on the device: candidates in gp_lm, no keyframes or weights
@@ -1514,7 +1547,7 @@ static double plane_reg_weight(const kba_window* sel) {
 
 // every argument check of a track solve, before anything is uploaded or launched
 static int track_check(const kba_track* t, TrackRequest& q, std::string& why) {
-    if (!q.kf_slot || !q.kf_fixed || !q.lm_slot || !q.sel) { why = "null argument"; return KBA_ERR_BAD_ARG; }
+    if (!q.kf_slot || !q.kf_fixed || (!q.lm_slot && !q.ranked) || !q.sel) { why = "null argument"; return KBA_ERR_BAD_ARG; }
     const kba_track_caps& c = t->caps;
     const kba_window* sel = q.sel;
     if (q.n_kf < 3) { why = "fewer than 3 keyframes"; return KBA_ERR_NOT_ENOUGH_KF; }
@@ -1530,10 +1563,12 @@ static int track_check(const kba_track* t, TrackRequest& q, std::string& why) {
         q.n_free += q.kf_fixed[k] ? 0 : 1;
     }
     if (n_meas > c.win_observations) { why = "more observations than win_observations"; return KBA_ERR_CAPACITY; }
-    for (int j = 0; j < q.n_lm; ++j)
+    for (int j = 0; j < q.n_lm && !q.ranked; ++j)
         if (q.lm_slot[j] < 0 || q.lm_slot[j] >= t->td.lm_cap) { why = "landmark slot out of range"; return KBA_ERR_BAD_ARG; }
-    q.device_gp = device_attached(sel);
-    if (q.device_gp) {
+    q.device_gp = q.rank_gp || device_attached(sel);
+    if (q.rank_gp) {
+        // the ranking's ground candidates: ascending indices into its selection by construction
+    } else if (q.device_gp) {
         for (int g = 0; g < sel->n_gp; ++g)
             if (sel->gp_lm[g] < 0 || sel->gp_lm[g] >= q.n_lm || (g > 0 && sel->gp_lm[g] <= sel->gp_lm[g - 1])) {
                 why = "ground-plane candidates must be strictly ascending indices into lm_slot"; return KBA_ERR_BAD_ARG;
@@ -1738,6 +1773,7 @@ int kba_track_push_keyframe(kba_track* t, int32_t slot, const double* pose7, con
         CU(cudaStreamSynchronize(s));
     }
     t->m_off[slot] = t->arena_used; t->m_cnt[slot] = n; t->kf_live[slot] = 1;
+    t->gen++;
     t->arena_used += n;
     t->h2d_push += (int64_t)n * 20 + 11 * 8;
     const int rc = track_upload_layout(t);
@@ -1748,6 +1784,7 @@ int kba_track_push_keyframe(kba_track* t, int32_t slot, const double* pose7, con
 int kba_track_drop_keyframe(kba_track* t, int32_t slot) {
     if (!t || slot < 0 || slot >= t->td.kf_cap) return fail(KBA_ERR_BAD_ARG, "bad argument to kba_track_drop_keyframe");
     t->kf_live[slot] = 0;  // the arena space is reclaimed by the next compaction
+    t->gen++;
     return KBA_OK;
 }
 
@@ -1771,6 +1808,7 @@ static int track_scatter(kba_track* t, double* dst, int cap_slots, int n, const 
 int kba_track_set_keyframe_poses(kba_track* t, int32_t n, const int32_t* slot, const double* pose7s, const double* plane4s) {
     if (!t || n < 0 || (n > 0 && (!slot || !pose7s))) return fail(KBA_ERR_BAD_ARG, "bad argument to kba_track_set_keyframe_poses");
     CU(cudaSetDevice(t->h->device));
+    t->gen++;
     int rc = track_scatter(t, t->td.kf_pose, t->td.kf_cap, n, slot, pose7s, 7);
     if (rc == KBA_OK && plane4s) rc = track_scatter(t, t->td.kf_plane, t->td.kf_cap, n, slot, plane4s, 4);
     return rc;
@@ -1784,6 +1822,7 @@ int kba_track_set_keyframe_pose(kba_track* t, int32_t slot, const double* pose7,
 int kba_track_set_landmarks(kba_track* t, int32_t n, const int32_t* slot, const double* pos3, const double* weight) {
     if (!t || n < 0 || (n > 0 && !slot)) return fail(KBA_ERR_BAD_ARG, "bad argument to kba_track_set_landmarks");
     CU(cudaSetDevice(t->h->device));
+    t->gen++;
     int rc = KBA_OK;
     if (pos3) rc = track_scatter(t, t->td.lm_pos, t->td.lm_cap, n, slot, pos3, 3);
     if (rc == KBA_OK && weight) rc = track_scatter(t, t->td.lm_weight, t->td.lm_cap, n, slot, weight, 1);
@@ -1819,16 +1858,23 @@ static int track_solve(kba_handle* h, TrackSolver& sv, int n, kba_track* const* 
             max_free = std::max(max_free, track_free_rows(q));
             solved[i].rows = q.rows; solved[i].n_chunks = d.n_chunks;
             // lists: keyframe slots | landmark slots | fixation bytes | ground-plane candidates
+            // (a ranked request's landmarks and ground candidates are the track's ranking, already on the device)
             const kba_window* sel = q.sel;
             const int n_cand = q.device_gp ? sel->n_gp : 0, fixed_ints = (q.n_kf + 3) / 4;
             int* l = sv.lists.h + used;
-            memcpy(l, q.kf_slot, q.n_kf * sizeof(int));
-            memcpy(l + q.n_kf, q.lm_slot, q.n_lm * sizeof(int));
-            memcpy(l + q.n_kf + q.n_lm, q.kf_fixed, q.n_kf);
-            if (n_cand) memcpy(l + q.n_kf + q.n_lm + fixed_ints, sel->gp_lm, n_cand * sizeof(int));
             const int* ld = sv.lists.d + used;
-            sv.tsel.h[i] = track_sel(q, ld, reinterpret_cast<const uint8_t*>(ld + q.n_kf + q.n_lm), ld + q.n_kf, ld + q.n_kf + q.n_lm + fixed_ints);
-            used += (size_t)q.n_kf + q.n_lm + fixed_ints + n_cand;
+            size_t at = (size_t)q.n_kf;
+            memcpy(l, q.kf_slot, q.n_kf * sizeof(int));
+            const int* lm_d = q.ranked ? ts[i]->rank->sel_slot : ld + at;
+            if (!q.ranked) { memcpy(l + at, q.lm_slot, q.n_lm * sizeof(int)); at += (size_t)q.n_lm; }
+            memcpy(l + at, q.kf_fixed, q.n_kf);
+            const uint8_t* fx_d = reinterpret_cast<const uint8_t*>(ld + at);
+            at += (size_t)fixed_ints;
+            const int* cand_d = q.rank_gp ? ts[i]->rank->gp : ld + at;
+            if (n_cand && !q.rank_gp) { memcpy(l + at, sel->gp_lm, n_cand * sizeof(int)); at += (size_t)n_cand; }
+            sv.tsel.h[i] = track_sel(q, ld, fx_d, lm_d, cand_d);
+            used += at;
+            ts[i]->gen++;  // the solve writes the store back
             if (sel->n_gp && !q.device_gp) {
                 memcpy(b->r_gp_lm.h + d.gp_off, sel->gp_lm, sel->n_gp * sizeof(int)); memcpy(b->gp_kf.h + d.gp_off, sel->gp_kf, sel->n_gp * sizeof(int));
                 memcpy(b->gp_weight.h + d.gp_off, sel->gp_weight, sel->n_gp * sizeof(double));
@@ -1837,7 +1883,8 @@ static int track_solve(kba_handle* h, TrackSolver& sv, int n, kba_track* const* 
             grid.max_kf = std::max(grid.max_kf, q.n_kf); grid.max_lm = std::max(grid.max_lm, q.n_lm);
             grid.max_meas = std::max(grid.max_meas, q.max_meas);
             grid.any_cand |= n_cand > 0;
-            h2d += (int64_t)q.n_kf * 5 + (int64_t)q.n_lm * 4 + (q.device_gp ? (int64_t)n_cand * 4 : (int64_t)sel->n_gp * 16);
+            h2d += (int64_t)q.n_kf * 5 + (q.ranked ? 0 : (int64_t)q.n_lm * 4) +
+                   (q.device_gp ? (q.rank_gp ? 0 : (int64_t)n_cand * 4) : (int64_t)sel->n_gp * 16);
         }
         b->desc.h[i] = d;
     }
@@ -1928,13 +1975,15 @@ struct SelectReq {
     const kba_select_params* p = nullptr;
     const kba_select_out* o = nullptr;
     int max_meas = 0;                      // set by select_check: arena entries of the largest listed keyframe
+    bool quantities_only = false;          // a ranking's selection: the quantities stay on the device, `o` is not used
 };
 
 // every check of one request, before anything is uploaded; allocates the track's selection buffers at its first selection
 static int select_check(SelectReq& r, std::string& why) {
     kba_track* t = r.t;
     const kba_select_out* o = r.o;
-    if (!r.kf_slot || !r.p || !o || (r.n_cand > 0 && !r.lm_slot) || !o->cheiral || !o->bin || !o->near_order || !o->n_near || !o->flow || !o->seen) {
+    if (!r.kf_slot || !r.p || (r.n_cand > 0 && !r.lm_slot) ||
+        (!r.quantities_only && (!o || !o->cheiral || !o->bin || !o->near_order || !o->n_near || !o->flow || !o->seen))) {
         why = "null argument"; return KBA_ERR_BAD_ARG;
     }
     if (r.n_kf < 1 || r.n_cand < 0) { why = "no keyframes or a negative size"; return KBA_ERR_BAD_ARG; }
@@ -2236,6 +2285,7 @@ static int create_check(CreateReq& r, std::string& why) {
 // scatter into the callers' arrays.  Window 0's record travels in the launch parameters (kba_create.cu).
 static int create_run(kba_handle* h, SelectStage& st, int W, const CreateReq* r) {
     CU(cudaSetDevice(h->device));
+    for (int w = 0; w < W; ++w) r[w].t->gen++;
     cudaStream_t s = h->stream;
     CreateGrid g;
     size_t n_list = 0, N = 0;
@@ -2803,6 +2853,7 @@ static int reclaim_check(kba_track* t, const kba_reclaim_request* q, const kba_r
 static int reclaim_run(kba_handle* h, SelectStage& st, int W, kba_track* const* ts, const kba_reclaim_request* const* qs,
                        kba_reclaim_out* const* os) {
     CU(cudaSetDevice(h->device));
+    for (int w = 0; w < W; ++w) ts[w]->gen++;
     cudaStream_t s = h->stream;
     ReclaimGrid g;
     size_t SP = 0, SW = 0, SN = 0;
@@ -3134,6 +3185,315 @@ int kba_track_group_adjust_pose(kba_track_group* g, const kba_track_frame* f, co
     return track_adjust_pose("kba_track_group_adjust_pose", true, g->h, g->solver, (int)g->tracks.size(), g->tracks.data(), f, opt, res);
 }
 
+// ---------------------------------------------------------------------------------------------------------------------
+// ranked landmark selection on the stored window, and solves of the ranking (include/kba_b200.h, kba_track_rank_landmarks /
+// kba_track_solve_ranked and their group forms; kernels in kba_select.cu and kba_rank.cu)
+// ---------------------------------------------------------------------------------------------------------------------
+static int rank_alloc(kba_track* t, std::string& why) {
+    std::unique_ptr<RankBufs> rb(new RankBufs());
+    const size_t L = (size_t)t->td.lm_cap, K = (size_t)t->td.kf_cap, M = (size_t)t->td.m_cap;
+    int bad = 0;
+    bad |= rb->alloc(&rb->qty, select_out_bytes(L, 1)); bad |= rb->alloc(&rb->mark, L); bad |= rb->alloc(&rb->dcand, M);
+    bad |= rb->alloc(&rb->dcost, M); bad |= rb->alloc(&rb->dcnt, K); bad |= rb->alloc(&rb->sel_slot, L); bad |= rb->alloc(&rb->gp, L);
+    if (bad) { why = "out of memory for the ranking buffers"; return KBA_ERR_CUDA; }
+    t->rank = std::move(rb);
+    return KBA_OK;
+}
+
+// upload and download capacities of a staging that serves tracks ts[0..n) (one window each)
+static size_t rank_up_cap(int n, kba_track* const* ts) {
+    size_t b = (sizeof(SelectArgs) + sizeof(RankArgs)) * (size_t)(n - 1) + 8 * (size_t)kRankMaxDepth * n + 8 * (size_t)n + 8;
+    for (int i = 0; i < n; ++i) b += 4 * (size_t)ts[i]->td.kf_cap + 9 * (size_t)ts[i]->td.lm_cap;  // lists, flags, draws
+    return b;
+}
+static size_t rank_out_cap(int n, kba_track* const* ts) {
+    size_t b = 16 * (size_t)n + 8;
+    for (int i = 0; i < n; ++i) b += 5 * (size_t)ts[i]->td.lm_cap;
+    return b;
+}
+
+struct RankReq {
+    kba_track* t = nullptr;
+    const kba_rank_request* q = nullptr;
+    kba_rank_out* o = nullptr;
+    SelectReq s;                           // the selection chain of the same lists
+};
+
+// every check of one request, before anything is uploaded; allocates the track's selection and ranking buffers at its first call
+static int rank_check(RankReq& r, std::string& why) {
+    const kba_rank_request* q = r.q;
+    if (!r.o || (q->n_cand > 0 && (!r.o->cand || !r.o->category)) || (q->n_depth > 0 && !q->depth)) {
+        why = "null argument"; return KBA_ERR_BAD_ARG;
+    }
+    if (q->max_near < 0 || q->max_middle < 0 || q->max_far < 0 || q->n_depth < 0) { why = "a negative cap or size"; return KBA_ERR_BAD_ARG; }
+    for (int e = 0; e < q->n_depth; ++e)
+        if (q->depth[e].ind < 0 || q->depth[e].wanted < 0) { why = "an AddDepth entry with a negative index or count"; return KBA_ERR_BAD_ARG; }
+    if (q->n_cand > kRankMaxCand) { why = "more than 57344 candidates"; return KBA_ERR_CAPACITY; }
+    if (q->n_depth > kRankMaxDepth) { why = "more than 1024 AddDepth entries"; return KBA_ERR_CAPACITY; }
+    SelectReq& s = r.s;
+    s.t = r.t; s.n_kf = q->n_kf; s.n_cand = q->n_cand; s.kf_slot = q->kf_slot; s.lm_slot = q->lm_slot; s.p = q->params;
+    s.quantities_only = true;
+    int rc = select_check(s, why);
+    if (rc != KBA_OK) return rc;
+    for (int e = 0; e < q->n_depth; ++e)  // the AddDepth heap of an entry lives in shared memory
+        if (q->depth[e].ind < q->n_kf && std::min(q->depth[e].wanted, r.t->m_cnt[q->kf_slot[q->depth[e].ind]]) > kRankMaxCand) {
+            why = "an AddDepth entry keeps more than 57344 landmarks"; return KBA_ERR_CAPACITY;
+        }
+    if (!r.t->rank) rc = rank_alloc(r.t, why);
+    return rc;
+}
+
+// W checked requests of distinct tracks as the W windows of one launch sequence in two parts (include/kba_b200.h): the lists go
+// up, the chain and the AddDepth costs run, the middle bins' sizes come down; the draw functions fill the draws, which go up with
+// each window's output offsets; the heaps, the shuffle and the union run, the outputs come down.
+static int rank_run(kba_handle* h, SelectStage& st, int W, RankReq* r) {
+    CU(cudaSetDevice(h->device));
+    cudaStream_t s = h->stream;
+    SelectGrid sg;
+    RankGrid rg;
+    size_t n_list = 0, N = 0, ND = 0;
+    for (int w = 0; w < W; ++w) {
+        const kba_rank_request& q = *r[w].q;
+        n_list += (size_t)q.n_kf + q.n_cand; N += (size_t)q.n_cand; ND += (size_t)q.n_depth;
+        sg.max_kf = std::max(sg.max_kf, q.n_kf); sg.max_cand = std::max(sg.max_cand, q.n_cand);
+        sg.max_init = std::max(sg.max_init, std::max(std::max(q.n_kf, q.n_cand), r[w].t->n_cam));
+        sg.max_meas = std::max(sg.max_meas, r[w].s.max_meas);
+        rg.max_depth = std::max(rg.max_depth, q.n_depth);
+    }
+    rg.max_kf = sg.max_kf; rg.max_cand = sg.max_cand;
+    // ---- staging up: select records | rank records | AddDepth entries | lists | flags, then (first draw, first output) per window |
+    // draws; down: middle-bin sizes, then (n_sel, n_ground) per window | candidates | categories
+    static_assert(sizeof(SelectArgs) % 8 == 0 && sizeof(RankArgs) % 8 == 0, "records keep the entries 8-byte aligned");
+    const size_t o_rrec = sizeof(SelectArgs) * (size_t)(W - 1), o_depth = o_rrec + sizeof(RankArgs) * (size_t)(W - 1);
+    const size_t o_lists = o_depth + 8 * ND, o_elig = o_lists + 4 * n_list, up_bytes = o_elig + N, o_p2 = (up_bytes + 7) & ~(size_t)7;
+    const size_t o_res = (4 * (size_t)W + 7) & ~(size_t)7;
+    unsigned char* uh = st.up.h;
+    const unsigned char* ud = st.up.d;
+    SelectLaunch sl;
+    sl.rest = reinterpret_cast<const SelectArgs*>(ud);
+    sl.n_win = W;
+    RankLaunch rl;
+    rl.rest = reinterpret_cast<const RankArgs*>(ud + o_rrec);
+    rl.n_win = W;
+    rl.n_mid = reinterpret_cast<int*>(st.out.d);
+    rl.p2 = reinterpret_cast<const int*>(ud + o_p2);
+    rl.res = reinterpret_cast<int*>(st.out.d + o_res);
+    size_t li = 0, c0 = 0, d0 = 0;
+    for (int w = 0; w < W; ++w) {
+        const kba_rank_request& q = *r[w].q;
+        kba_track* t = r[w].t;
+        RankBufs& rb = *t->rank;
+        int* lists_h = reinterpret_cast<int*>(uh + o_lists) + li;
+        const int* lists_d = reinterpret_cast<const int*>(ud + o_lists) + li;
+        memcpy(lists_h, q.kf_slot, 4 * (size_t)q.n_kf);
+        if (q.n_cand) memcpy(lists_h + q.n_kf, q.lm_slot, 4 * (size_t)q.n_cand);
+        if (q.elig) memcpy(uh + o_elig + c0, q.elig, (size_t)q.n_cand); else memset(uh + o_elig + c0, 0, (size_t)q.n_cand);
+        for (int e = 0; e < q.n_depth; ++e) {
+            int* de = reinterpret_cast<int*>(uh + o_depth) + 2 * (d0 + e);
+            de[0] = q.depth[e].ind; de[1] = q.depth[e].wanted;
+        }
+        // the chain: its quantities go to the ranking's device block instead of the download
+        const size_t L = (size_t)t->td.lm_cap;
+        unsigned char* qd = rb.qty;
+        SelectArgs a = t->select->a;
+        a.td = t->td;
+        a.kf_slot = lists_d; a.lm_slot = lists_d + q.n_kf; a.n_kf = q.n_kf; a.n_cand = q.n_cand;
+        for (int k = 0; k < 3; ++k) a.leaf[k] = q.params->voxel_size[k];
+        a.roi_far = q.params->roi_far; a.roi_middle = q.params->roi_middle;
+        a.flow = reinterpret_cast<double*>(qd); a.seen = reinterpret_cast<int*>(qd + 8 * L); a.near_order = reinterpret_cast<int*>(qd + 12 * L);
+        a.counters = reinterpret_cast<int*>(qd + 16 * L); a.n_near = a.counters + 1;
+        a.cheiral = qd + 16 * L + 16; a.bin = reinterpret_cast<signed char*>(qd + 17 * L + 16);
+        RankArgs ra;
+        ra.td = t->td;
+        ra.kf_slot = a.kf_slot; ra.lm_slot = a.lm_slot; ra.elig = ud + o_elig + c0;
+        ra.depth = reinterpret_cast<const int*>(ud + o_depth) + 2 * d0;
+        ra.n_kf = q.n_kf; ra.n_cand = q.n_cand; ra.n_depth = q.n_depth;
+        ra.max_near = q.max_near; ra.max_middle = q.max_middle; ra.max_far = q.max_far;
+        ra.cheiral = a.cheiral; ra.bin = a.bin; ra.near_order = a.near_order; ra.n_near = a.n_near; ra.flow = a.flow; ra.seen = a.seen;
+        ra.cand_of = a.cand_of; ra.mark = rb.mark; ra.dcand = rb.dcand; ra.dcost = rb.dcost; ra.dcnt = rb.dcnt;
+        ra.sel_slot = rb.sel_slot; ra.gp = rb.gp;
+        if (w == 0) { sl.w0 = a; rl.w0 = ra; }
+        else {
+            memcpy(uh + sizeof(SelectArgs) * (size_t)(w - 1), &a, sizeof(SelectArgs));
+            memcpy(uh + o_rrec + sizeof(RankArgs) * (size_t)(w - 1), &ra, sizeof(RankArgs));
+        }
+        li += (size_t)q.n_kf + q.n_cand; c0 += (size_t)q.n_cand; d0 += (size_t)q.n_depth;
+    }
+    // ---- part one: the chain's quantities, the middle bins' sizes and the AddDepth costs
+    CU(cudaMemcpyAsync(st.up.d, st.up.h, up_bytes, cudaMemcpyHostToDevice, s));
+    CU(cudaMemsetAsync(rl.n_mid, 0, 4 * (size_t)W, s));
+    launch_select(sl, sg, s);
+    launch_rank_prepare(rl, rg, s);
+    CU(cudaGetLastError());
+    CU(cudaMemcpyAsync(st.out.h, st.out.d, 4 * (size_t)W, cudaMemcpyDeviceToHost, s));
+    CU(wait_stream(h));
+    // ---- the draws, each window's output offset and the heaps' shared memory
+    const int* n_mid = reinterpret_cast<const int*>(st.out.h);
+    int* p2 = reinterpret_cast<int*>(uh + o_p2);
+    int* draws = p2 + 2 * W;
+    size_t n_draws = 0, n_out = 0;
+    std::vector<int> bound(W);
+    for (int w = 0; w < W; ++w) {
+        const kba_rank_request& q = *r[w].q;
+        const int nm = n_mid[w], D = std::max(nm - 1, 0), n = q.n_cand;
+        long long b = std::min(q.max_near, n) + (long long)std::min(q.max_middle, nm) + std::min(q.max_far, n);
+        // an AddDepth heap holds at most min(wanted, arena entries of its keyframe) elements, whatever the runs of the keyframe
+        int heap = std::max(std::min(q.max_near, n), std::min(q.max_far, n));
+        for (int e = 0; e < q.n_depth; ++e) {
+            b += std::min(q.depth[e].wanted, n);
+            if (q.depth[e].ind < q.n_kf) heap = std::max(heap, std::min(q.depth[e].wanted, r[w].t->m_cnt[q.kf_slot[q.depth[e].ind]]));
+        }
+        bound[w] = (int)std::min<long long>(b, n);
+        rg.heap_ints = std::max(rg.heap_ints, heap);
+        rg.mid_ints = std::max(rg.mid_ints, nm);
+        p2[2 * w] = (int)n_draws; p2[2 * w + 1] = (int)n_out;
+        n_out += (size_t)bound[w];
+        if (D == 0) continue;
+        std::string why;
+        if (!q.draw) why = "the middle bin needs " + std::to_string(D) + " draws and there is no draw function";
+        else if (q.draw(q.draw_ctx, D, draws + n_draws) != 0) why = "the draw function failed";
+        if (!why.empty()) {  // nothing is written; the slot maps go back to all -1 and no track keeps a ranking
+            for (int v = 0; v < W; ++v) {
+                r[v].t->rank->valid = false;
+                cudaMemsetAsync(r[v].t->select->a.cand_of, 0xff, sizeof(int) * (size_t)r[v].t->td.lm_cap, s);
+            }
+            cudaStreamSynchronize(s);
+            return fail(KBA_ERR_BAD_ARG, std::string(W > 1 ? "track " + std::to_string(w) + ": " : "") + why);
+        }
+        n_draws += (size_t)D;
+    }
+    // ---- part two: heaps, shuffle, union
+    const size_t p2_bytes = 8 * (size_t)W + 4 * n_draws;
+    CU(cudaMemcpyAsync(st.up.d + o_p2, uh + o_p2, p2_bytes, cudaMemcpyHostToDevice, s));
+    rl.out_cand = reinterpret_cast<int*>(st.out.d + o_res + 8 * (size_t)W);
+    rl.out_cat = reinterpret_cast<signed char*>(st.out.d + o_res + 8 * (size_t)W + 4 * n_out);
+    launch_rank(rl, rg, s);
+    CU(cudaGetLastError());
+    const size_t out_bytes = 8 * (size_t)W + 5 * n_out;
+    CU(cudaMemcpyAsync(st.out.h + o_res, st.out.d + o_res, out_bytes, cudaMemcpyDeviceToHost, s));
+    CU(wait_stream(h));
+    // ---- scatter
+    const int* res = reinterpret_cast<const int*>(st.out.h + o_res);
+    const unsigned char* hc = st.out.h + o_res + 8 * (size_t)W;
+    for (int w = 0; w < W; ++w) {
+        kba_rank_out& o = *r[w].o;
+        RankBufs& rb = *r[w].t->rank;
+        const int n_sel = res[2 * w], off = p2[2 * w + 1];
+        o.n_sel = n_sel; o.n_ground = res[2 * w + 1]; o.n_draws = std::max(n_mid[w] - 1, 0);
+        if (n_sel) { memcpy(o.cand, hc + 4 * (size_t)off, 4 * (size_t)n_sel); memcpy(o.category, hc + 4 * n_out + off, (size_t)n_sel); }
+        rb.kf.assign(r[w].q->kf_slot, r[w].q->kf_slot + r[w].q->n_kf);
+        rb.n_sel = n_sel; rb.n_ground = o.n_ground; rb.gen = r[w].t->gen; rb.valid = true;
+    }
+    st.counts.h2d = (int64_t)(up_bytes + p2_bytes);
+    st.counts.d2h = (int64_t)(4 * (size_t)W + out_bytes);
+    return KBA_OK;
+}
+
+int kba_track_rank_landmarks(kba_track* t, const kba_rank_request* req, kba_rank_out* out) {
+    static const std::string who = "kba_track_rank_landmarks: ";
+    if (!t || !req) return fail(KBA_ERR_BAD_ARG, who + "null argument");
+    RankReq r;
+    r.t = t; r.q = req; r.o = out;
+    std::string why;
+    int rc = rank_check(r, why);
+    if (rc != KBA_OK) return fail(rc, who + why);
+    SelectStage& st = t->rank->stage;
+    if (!st.up.d && st.alloc(rank_up_cap(1, &t), rank_out_cap(1, &t))) {  // the first single call of the track
+        st.up.release(); st.out.release();
+        return fail(KBA_ERR_CUDA, who + "out of memory for the ranking staging");
+    }
+    rc = rank_run(t->h, st, 1, &r);
+    if (rc == KBA_OK) t->last = &st.counts;
+    return rc;
+}
+
+int kba_track_group_rank_landmarks(kba_track_group* g, const kba_rank_request* req, kba_rank_out* out) {
+    static const std::string who = "kba_track_group_rank_landmarks: ";
+    if (!g || !req || !out) return fail(KBA_ERR_BAD_ARG, who + "null argument");
+    const int n = (int)g->tracks.size();
+    // ---- every request is checked before anything is uploaded or written
+    std::vector<RankReq> rs;
+    for (int i = 0; i < n; ++i) {
+        if (req[i].n_kf == 0) continue;  // sits the call out
+        RankReq r;
+        r.t = g->tracks[i]; r.q = &req[i]; r.o = &out[i];
+        std::string why;
+        const int rc = rank_check(r, why);
+        if (rc != KBA_OK) return fail(rc, who + "track " + std::to_string(i) + ": " + why);
+        rs.push_back(r);
+    }
+    if (rs.empty()) {  // every track sits out: no upload, no launch
+        g->solver.h2d = 0; g->solver.d2h = 0;
+        g->last = &g->solver;
+        return KBA_OK;
+    }
+    if (!g->rank) {  // staging for every track at its capacities, allocated once
+        std::unique_ptr<SelectStage> st(new SelectStage());
+        if (st->alloc(rank_up_cap(n, g->tracks.data()), rank_out_cap(n, g->tracks.data())))
+            return fail(KBA_ERR_CUDA, who + "out of memory for the ranking staging");
+        g->rank = std::move(st);
+    }
+    const int rc = rank_run(g->h, *g->rank, (int)rs.size(), rs.data());
+    if (rc != KBA_OK) return rc;
+    g->last = &g->rank->counts;
+    return KBA_OK;
+}
+
+// the checks of a solve of track t's ranking; sel2 receives the caller's window with the ranking's ground-candidate count
+static int ranked_check(kba_track* t, int32_t n_kf, const int32_t* kf_slot, const uint8_t* kf_fixed, const kba_window* sel,
+                        TrackRequest& q, kba_window& sel2, std::string& why) {
+    if (!kf_slot || !kf_fixed || !sel) { why = "null argument"; return KBA_ERR_BAD_ARG; }
+    const RankBufs* rb = t->rank.get();
+    if (!rb || !rb->valid) { why = "the track has no ranking to solve (kba_track_rank_landmarks)"; return KBA_ERR_BAD_ARG; }
+    if (rb->gen != t->gen) { why = "the ranking is stale: the store changed after it was ranked"; return KBA_ERR_BAD_ARG; }
+    if (n_kf != (int)rb->kf.size() || !std::equal(rb->kf.begin(), rb->kf.end(), kf_slot)) {
+        why = "the keyframes differ from the ranking's"; return KBA_ERR_BAD_ARG;
+    }
+    sel2 = *sel;
+    const bool from_ranking = sel->n_gp > 0 && !sel->gp_lm && !sel->gp_kf && !sel->gp_weight;
+    if (from_ranking) sel2.n_gp = rb->n_ground;
+    q.n_kf = n_kf; q.kf_slot = kf_slot; q.kf_fixed = kf_fixed; q.n_lm = rb->n_sel; q.lm_slot = nullptr; q.sel = &sel2;
+    q.ranked = true; q.rank_gp = from_ranking && rb->n_ground > 0;
+    return track_check(t, q, why);
+}
+
+int kba_track_solve_ranked(kba_track* t, int32_t n_kf, const int32_t* kf_slot, const uint8_t* kf_fixed, const kba_window* sel,
+                           const kba_options* opt, kba_result* res) {
+    if (!t || !opt || !res) return fail(KBA_ERR_BAD_ARG, "null argument to kba_track_solve_ranked");
+    TrackRequest q;
+    kba_window sel2;
+    std::string why;
+    const int rc = ranked_check(t, n_kf, kf_slot, kf_fixed, sel, q, sel2, why);
+    if (rc != KBA_OK) return fail(rc, "kba_track_solve_ranked: " + why);
+    TrackSolver& sv = q.rows > kFusedMaxRows ? t->large : t->solver;
+    t->last = &sv;
+    return track_solve(t->h, sv, 1, &t, &q, opt, res);
+}
+
+int kba_track_group_solve_ranked(kba_track_group* g, const kba_ranked_request* req, const kba_options* opt, kba_result* res) {
+    if (!g || !req || !opt || !res) return fail(KBA_ERR_BAD_ARG, "null argument to kba_track_group_solve_ranked");
+    const int n = (int)g->tracks.size();
+    std::vector<TrackRequest> qs(n);
+    std::vector<kba_window> sels(n);
+    int active = 0;
+    bool large = false;
+    for (int i = 0; i < n; ++i) {
+        if (req[i].n_kf == 0) continue;  // sits this solve out
+        std::string why;
+        const int rc = ranked_check(g->tracks[i], req[i].n_kf, req[i].kf_slot, req[i].kf_fixed, req[i].sel, qs[i], sels[i], why);
+        if (rc != KBA_OK) return fail(rc, "kba_track_group_solve_ranked: track " + std::to_string(i) + ": " + why);
+        ++active;
+        large |= qs[i].rows > kFusedMaxRows;
+    }
+    if (active == 0) {
+        for (int i = 0; i < n; ++i) idle_result(res[i]);
+        g->solver.h2d = 0; g->solver.d2h = 0;
+        g->last = &g->solver;
+        return KBA_OK;
+    }
+    TrackSolver& sv = large ? g->large : g->solver;
+    g->last = &sv;
+    return track_solve(g->h, sv, n, g->tracks.data(), qs.data(), opt, res);
+}
+
 }  // extern "C"
-
-

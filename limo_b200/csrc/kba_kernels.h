@@ -283,6 +283,57 @@ struct ReclaimGrid {
 };
 void launch_reclaim(const ReclaimLaunch& l, const ReclaimGrid& g, cudaStream_t s);
 
+// ---- the ranked selection on a track's store (kba_track_rank_landmarks / kba_track_group_rank_landmarks, kba_rank.cu) ----
+// One window = one request, run after launch_select on the same lists.  The first part (launch_rank_prepare) counts the middle
+// bin and computes the AddDepth costs; the host then downloads the counts and uploads the draws; the second part (launch_rank)
+// replays the partial sorts, shuffles the middle bin and compacts the union into the track's ranked list.
+constexpr int kRankMaxCand = 57344;        // candidates of a request: the middle bin and every heap live in shared memory, 4 B each
+constexpr int kRankMaxDepth = 1024;        // AddDepth entries of a request: one block each
+struct RankArgs {
+    TrackDev td;
+    const int* kf_slot = nullptr;          // [n_kf]
+    const int* lm_slot = nullptr;          // [n_cand]
+    const unsigned char* elig = nullptr;   // [n_cand]
+    const int* depth = nullptr;            // [2 * n_depth] (ind, wanted)
+    int n_kf = 0, n_cand = 0, n_depth = 0;
+    int max_near = 0, max_middle = 0, max_far = 0;
+    // the selection chain's quantities (the SelectArgs outputs of the same window), on the device only
+    const unsigned char* cheiral = nullptr;
+    const signed char* bin = nullptr;
+    const int* near_order = nullptr;
+    const int* n_near = nullptr;
+    const double* flow = nullptr;
+    const int* seen = nullptr;
+    // scratch
+    int* cand_of = nullptr;                // SelectArgs::cand_of: slot -> candidate for the call, all -1 again at its end
+    int* mark = nullptr;                   // [lm_cap] by candidate: bit 0 near, 1 middle, 2 far, 3 AddDepth
+    int* dcand = nullptr;                  // [m_cap] listed keyframe k's i-th eligible landmark (candidate) at m_off[kf_slot[k]] + i
+    double* dcost = nullptr;               // [m_cap] ... and its cost
+    int* dcnt = nullptr;                   // [kf_cap] eligible landmarks of listed keyframe k
+    // the track's ranking
+    int* sel_slot = nullptr;               // [lm_cap] ranked landmark slots
+    int* gp = nullptr;                     // [lm_cap] ranked ground candidates, indices into sel_slot
+};
+// W windows in one launch sequence, window = grid z; window 0's arguments travel in the launch parameters (as SelectLaunch).
+// n_mid, p2 and the outputs are shared by the windows, indexed by window.
+struct RankLaunch {
+    RankArgs w0;
+    const RankArgs* rest = nullptr;        // [n_win - 1]
+    int n_win = 0;
+    int* n_mid = nullptr;                  // [n_win] middle-bin sizes (zeroed before launch_rank_prepare)
+    const int* p2 = nullptr;               // [2 * n_win] (first draw, first output) of each window, then the draws end to end
+    int* res = nullptr;                    // [2 * n_win] n_sel, n_ground of each window
+    int* out_cand = nullptr;               // outputs of window w from its first output on
+    signed char* out_cat = nullptr;
+};
+struct RankGrid {
+    int max_kf = 0, max_cand = 0, max_depth = 0;
+    int mid_ints = 1;                      // dynamic shared memory of k_rk_heap, in ints: the largest middle bin
+    int heap_ints = 1;                     // ... and the largest near, far or AddDepth heap
+};
+void launch_rank_prepare(const RankLaunch& l, const RankGrid& g, cudaStream_t s);
+void launch_rank(const RankLaunch& l, const RankGrid& g, cudaStream_t s);
+
 // ---- motion-only frames against a track's store (kba_track_adjust_pose / kba_track_group_adjust_pose, kba_motion.cu) ----
 // One frame = one free pose against constant landmarks read from a store by slot: its measurements come in runs, one run per
 // landmark (the landmarks of the equivalent window, in the caller's order).

@@ -6,14 +6,15 @@
 // are the first entries of its runs.  The track's slot map holds (stamp << 32) | payload; an entry counts only when its stamp is
 // the call's, so the map is never cleared between calls.
 //
-// Exactness: deactivation is integer arithmetic.  The cost is float(|kf * pos|) as limo's sorter computes it, with explicit
-// round-to-nearest intrinsics in mini_eigen's order for Isometry3d * Vector3d and norm(); the file is compiled with -fmad=false.
+// Exactness: deactivation is integer arithmetic.  The cost is float(|kf * pos|) as limo's sorter computes it (depth_cost,
+// kba_depth_cost.cuh, shared with the ranked selection); the file is compiled with -fmad=false.
 //
 // Windows: one launch sequence serves W requests (a track group's; a single call is W = 1), window w = blockIdx.z, as in
 // kba_select.cu: grids from the maxima over the windows, blocks beyond their window's sizes exit.
 #include <cfloat>
 #include <cstdint>
 
+#include "kba_depth_cost.cuh"
 #include "kba_exact.cuh"
 #include "kba_kernels.h"
 
@@ -130,11 +131,8 @@ __global__ void __launch_bounds__(256) k_up_depth(const __grid_constant__ Upkeep
         __syncthreads();
         if (j >= 0) {
             const int at = base + done + warp_off[warp] + __popc(hit & ((1u << lane) - 1u));
-            const double* p = a.td.lm_pos + 3 * (size_t)a.td.m_lm[m0 + i];
-            const double x = iso_row(T, 0, p[0], p[1], p[2]), y = iso_row(T, 1, p[0], p[1], p[2]), z = iso_row(T, 2, p[0], p[1], p[2]);
-            const double v = (double)__double2float_rn(__dsqrt_rn(da(da(dm(x, x), dm(y, y)), dm(z, z))));
             a.cand[at] = j;
-            a.cost[at] = -DBL_MAX < v ? v : -DBL_MAX;  // std::max(-DBL_MAX, v): a NaN leaves -DBL_MAX
+            a.cost[at] = depth_cost(T, a.td.lm_pos + 3 * (size_t)a.td.m_lm[m0 + i]);
         }
         done += chunk;
         __syncthreads();
