@@ -18,6 +18,15 @@ tests/test_launch_plan.py): the fused path with and without plane rows, the seve
 keyframe: a free gauge makes their later iterates drift along flat directions, but the first damped step is well defined), the
 large-window path with the tiled, the split (k_chol_*) and the one-CTA row-major factorisation, the 6x6 motion-only system with
 its speed prior, and FP32 observation blocks.
+
+The Schur split (p_split: the CTAs a window's Schur sum is spread over) follows the batch size, and each case asserts it.  A
+window solved alone splits its sum over 25 .. 88 CTAs on the fused path and over 16 on the large-window path, the batch of 17
+over 5: k_sred_reduce folds the partial sums and k_reduced_solve takes A from it.  The batches of 264 (config2_slice in FP64
+and FP32, config2_kf30_lm700 with the headline's 30 keyframes), 132 (free_keyframes_30, config3_kf30_lm600) and 80
+(config5_kf40_lm700) windows run at p_split = 1, the shapes bench.py times: one CTA owns all of a window's landmark groups in
+k_schur_fused, k_schur_syrk runs at a grid depth of 1, k_sred_reduce is not launched, and k_reduced_solve gathers A from the
+single sum itself, tiled or row-major.  The split factorisation at p_split = 1 (KBA_P_SPLIT=1) is in
+tests/test_bench_shapes.py.
 """
 from types import SimpleNamespace
 
@@ -41,14 +50,20 @@ pytestmark = pytest.mark.skipif(np.finfo(LD).eps >= np.finfo(np.float64).eps, re
 #   ground-plane windows (config3_kf8, config3_kf14, planes_kf18_none_fixed, config3_kf30_lm600):
 #     oracle: step_norm 8.0e-13 (config3_kf14), cost 7.5e-13, relative_decrease 4.0e-13 (planes_kf18_none_fixed)
 #     CUDA:   step_norm 2.8e-13 (config3_kf14), cost 3.1e-14, relative_decrease 1.7e-14
+#   config2_kf30_lm700: oracle cost 7.7e-13, step_norm 2.7e-13, relative_decrease 3.9e-13; CUDA cost 6.1e-14, step_norm 1.8e-13
+#   the batches at p_split = 1, worst window of each batch:
+#     plane-free (config2_slice and config2_kf30_lm700 x 264, free_keyframes_30 x 132, config5_kf40_lm700 x 80):
+#             cost 4.1e-13, cost_change 1.7e-13, step_norm 6.5e-13, relative_decrease 3.0e-13 (config2_slice x 264)
+#     ground (config3_kf30_lm600 x 132): cost 3.0e-14, cost_change 9.2e-15, step_norm 1.8e-13, relative_decrease 1.2e-14
+#     config3_kf30_lm600 alone with KBA_P_SPLIT=1, factorised by k_chol_* (tests/test_bench_shapes.py): the same figures
 # STEP_TOL is about 100 times the worst plane-free deviation.  A ground window has few ground rows: one of them, or one row of
 # the plane chain, wrong by 1e-6 moves the records by 9e-11 .. 1.8e-10 (test_dense_step_notices_a_wrong_ground_row), so
 # GROUND_TOL sits between that and the worst ground deviation (12 times the oracle's, 36 times the CUDA path's).
 #
-# FP32 blocks (kba_options.precision = 1, config2_slice): cost 1 2.8e-05, step_norm 1.1e-05, relative_decrease 3.6e-05, and
-# gradient_max_norm 1.3e-06 already in record 0.  That is not rounding of the FP64 chain: the solve does not form the normal
-# equations of the blocks kba_eval reports.  The landmark blocks and the pose-landmark coupling come from the FP32 J_p and r,
-# but k_pose_hessian re-evaluates each observation's pose rows in FP64 for the pose blocks and the pose gradient.  No single
+# FP32 blocks (kba_options.precision = 1, config2_slice, alone and x 264): cost 1 2.8e-05, step_norm 1.1e-05,
+# relative_decrease 3.6e-05, and gradient_max_norm 1.3e-06 already in record 0.  That is not rounding of the FP64 chain: the
+# solve does not form the normal equations of the blocks kba_eval reports.  The landmark blocks and the pose-landmark coupling
+# come from the FP32 J_p and r, but k_pose_hessian re-evaluates each observation's pose rows in FP64 for the pose blocks and the pose gradient.  No single
 # Jacobian gives that system, so the reference, built from the FP32 blocks alone, differs from it by what FP32 rounding does to
 # the pose rows.  FP32_TOL is about 100 times the measured deviation and tells a working FP32 mode from a broken one.
 STEP_TOL = 1e-10
@@ -89,6 +104,9 @@ WINDOWS = {
     # 181 rows over 18 keyframes with plane blocks, none of them fixed: k_schur_fused<7> with plane blocks
     "planes_kf18_none_fixed": (lambda: _no_fixed_keyframe(synth.make_window(3, seed=43, n_kf=18, n_lm=500, n_obs=4500)),
                                "ground", 1680, dict(fused=1, fused_slots=7)),
+    # 181 rows over 30 keyframes, 175 of them free: k_schur_fused<6> at the headline's 30 keyframes (config2_slice has 67 rows)
+    "config2_kf30_lm700": (lambda: synth.make_window(2, n_kf=30, n_lm=700, n_obs=7000, seed=5), "plane_free", 2274,
+                           dict(fused=1, fused_slots=6)),
     # 181 rows over 30 plane-free keyframes, none of them fixed: k_schur_fused<7>
     "free_kf30_none_fixed": (lambda: _no_fixed_keyframe(synth.make_window(2, n_kf=30, n_lm=700, n_obs=7000, seed=5)),
                              "plane_free", 2280, dict(fused=1, fused_slots=7)),
@@ -115,9 +133,21 @@ OPTION_HOOKS = {"motion_only_speed_prior": _motion_options}
 # CUDA runs: name -> (window of WINDOWS, kba_options.precision, copies in one kba_solve_batch, plan fields beyond the window's)
 CUDA_CASES = dict({name: (name, 0, 1, {}) for name in WINDOWS},
                   # 17 windows: more than the split factorisation takes, so k_reduced_solve factorises each in one CTA
-                  config5_kf40_lm700_batch17=("config5_kf40_lm700", 0, 17, dict(solve_tiled=0, solve_split=0)),
+                  config5_kf40_lm700_batch17=("config5_kf40_lm700", 0, 17, dict(p_split=5, solve_tiled=0, solve_split=0)),
                   # FP32 observation blocks (k_eval_obs<float>), everything after them in FP64
-                  config2_slice_fp32=("config2_slice", 1, 1, {}))
+                  config2_slice_fp32=("config2_slice", 1, 1, {}),
+                  # The batch sizes bench.py times put each window's Schur sum on one CTA (p_split = 1): k_sred_reduce is not
+                  # launched and k_reduced_solve gathers A from the sums itself.  264 windows: bench.py's headline batch, the
+                  # fused six-slot kernel with one CTA owning all of a window's landmark groups, then the tiled solve
+                  config2_slice_batch264=("config2_slice", 0, 264, dict(p_split=1, solve_tiled=1)),
+                  config2_slice_fp32_batch264=("config2_slice", 1, 264, dict(p_split=1, solve_tiled=1)),
+                  config2_kf30_lm700_batch264=("config2_kf30_lm700", 0, 264, dict(p_split=1, solve_tiled=1)),
+                  # 132 windows: k_schur_syrk at a grid depth of 1, tiled k_reduced_solve<true>
+                  free_keyframes_30_batch132=("free_keyframes_30", 0, 132, dict(p_split=1, solve_tiled=1, solve_split=0)),
+                  # 132 windows: config 3's sub-record shape, the row-major k_reduced_solve<false> in one CTA per window
+                  config3_kf30_lm600_batch132=("config3_kf30_lm600", 0, 132, dict(p_split=1, solve_tiled=0, solve_split=0)),
+                  # the same plane-free; 80 is the smallest batch for which syrk_split(256, n, 132) == 1
+                  config5_kf40_lm700_batch80=("config5_kf40_lm700", 0, 80, dict(p_split=1, solve_tiled=0, solve_split=0)))
 
 
 def build(name):
@@ -426,6 +456,14 @@ def test_window_copy_keeps_every_field():
         for f in ew.WINDOW_FIELDS:
             a, b = getattr(win, f), getattr(cp, f)
             assert (a is None and b is None) or np.array_equal(np.asarray(a), np.asarray(b)), f
+
+
+@pytest.mark.parametrize("name", list(CUDA_CASES))
+def test_cuda_case_selects_its_path(driver, name):  # noqa: F811
+    """the launch plan each CUDA case runs on, held without a GPU: a change to the rules that moves a case off its path fails
+    here, before the GPU run compares the wrong path"""
+    window, _, copies, path = CUDA_CASES[name]
+    assert_path(driver, [build(window)[0]] * copies, dict(WINDOWS[window][3], **path))
 
 
 @pytest.fixture(scope="module")
