@@ -183,8 +183,6 @@ struct MotionBufs {
     IterRecord* log = nullptr;
     cudaEvent_t ev0 = nullptr, ev1 = nullptr;
     int frames_cap = 0, runs_cap = 0, meas_cap = 0;
-    std::vector<unsigned> seen;  // per landmark slot: the check that stamped it last (a slot must not reappear after its run)
-    unsigned stamp = 0;
     static size_t al(size_t b) { return (b + 15) & ~(size_t)15; }
     static size_t up_bytes(int frames, int runs, int meas) {
         return al(sizeof(FrameDesc) * (size_t)frames) + al(4 * ((size_t)runs + frames)) + 5 * al(4 * (size_t)meas);
@@ -216,6 +214,12 @@ struct MotionBufs {
     }
 };
 
+// bytes one call moved each way: what the transfer-bytes calls report for the last call
+struct Transfer {
+    int64_t h2d = 0, d2h = 0;
+};
+static const Transfer kNoTransfer{};       // a call in which nothing ran
+
 // what solves and pose-only calls of stored windows run on: one per track (n = 1) and one per track group (one window per
 // track), created by track_solver_create
 struct TrackSolver {
@@ -224,7 +228,7 @@ struct TrackSolver {
     Staged<TrackSel> tsel;
     Staged<int> lists;                     // every selection list of a solve (keyframe slots, landmark slots, fixation bytes), ONE copy
     std::unique_ptr<MotionBufs> motion;    // pose-only calls, allocated at the first one
-    int64_t h2d = 0, d2h = 0;              // the last solve or pose-only call
+    Transfer counts;                       // the last solve or pose-only call
     void release() {
         if (batch) kba_batch_destroy(batch);
         batch = nullptr;
@@ -233,74 +237,55 @@ struct TrackSolver {
     }
 };
 
-// staging of a selection or creation call (select_run, create_run): one pinned upload, argument records of windows 1 .. W-1 | the
-// windows' lists, and one download of the windows' outputs (for a selection: flow | seen | near order (all windows' candidates end
-// to end) | counters [W] | cheirality | bins; for a creation: positions | flags)
-struct SelectStage {
+// staging of a store call (select_run .. rank_run): one pinned upload, argument records of windows 1 .. W-1 | the windows' lists,
+// and one download of the windows' outputs (for a selection: flow | seen | near order (all windows' candidates end to end) |
+// counters [W] | cheirality | bins; for a creation: positions | flags)
+struct StoreStage {
     Staged<unsigned char> up, out;
-    TrackSolver counts;                    // only h2d / d2h: what the transfer-bytes calls report after a selection
+    Transfer counts;                       // the last run's
     int alloc(size_t up_bytes, size_t out_bytes) { return up.alloc(up_bytes, true) | out.alloc(out_bytes, true); }
-    ~SelectStage() { up.release(); out.release(); }
+    ~StoreStage() { up.release(); out.release(); }
 };
 
-// buffers of a track's selections (kba_select.cu): the scratch is allocated at its first selection, alone or in a group, for the
-// track's capacities, then reused by both entry points (calls are serial on the handle's stream).  The staging serves only
-// kba_track_select_landmarks and is allocated at its first call (a group stages its calls in its own)
+// device allocations freed with their owner
+struct DevAllocs {
+    std::vector<void*> ptrs;
+    template <typename T> int alloc(T** p, size_t n) {
+        void* q = nullptr;
+        if (cudaMalloc(&q, std::max<size_t>(n, 1) * sizeof(T)) != cudaSuccess) return 1;
+        ptrs.push_back(q); *p = (T*)q; return 0;
+    }
+    ~DevAllocs() {
+        for (void* p : ptrs) cudaFree(p);
+    }
+};
+
+// scratch of a track's selections (kba_select.cu): allocated at its first selection or ranking, alone or in a group, for the
+// track's capacities, then reused by every entry point (calls are serial on the handle's stream)
 struct SelectBufs {
-    SelectStage stage;                     // kba_track_select_landmarks: keyframe slots | candidate slots, one window's outputs
     SelectArgs a;                          // the scratch pointers; lists and outputs are set per call
-    std::vector<void*> dev;
-    std::vector<unsigned> kf_stamp, lm_stamp;  // duplicate checks: the call that named a slot last
-    unsigned stamp = 0;
-    template <typename T> int alloc(T** p, size_t n) {
-        void* q = nullptr;
-        if (cudaMalloc(&q, std::max<size_t>(n, 1) * sizeof(T)) != cudaSuccess) return 1;
-        dev.push_back(q); *p = (T*)q; return 0;
-    }
-    ~SelectBufs() {
-        for (void* p : dev) cudaFree(p);
-    }
+    DevAllocs dev;
 };
 
-// buffers of a track's landmark creations (kba_create.cu), kept like SelectBufs: scratch and the track's cameras on the device at
-// its first creation, alone or in a group; the staging at its first single call
+// scratch of a track's landmark creations (kba_create.cu), kept like SelectBufs: scratch and the track's cameras on the device at
+// its first creation, alone or in a group
 struct CreateBufs {
-    SelectStage stage;                     // kba_track_create_landmarks: keyframe slots | landmark slots, one window's outputs
     CreateArgs a;                          // the scratch pointers; lists and outputs are set per call
-    std::vector<void*> dev;
-    std::vector<unsigned> kf_stamp, lm_stamp;  // duplicate checks: the call that named a slot last
-    unsigned stamp = 0;
-    template <typename T> int alloc(T** p, size_t n) {
-        void* q = nullptr;
-        if (cudaMalloc(&q, std::max<size_t>(n, 1) * sizeof(T)) != cudaSuccess) return 1;
-        dev.push_back(q); *p = (T*)q; return 0;
-    }
-    ~CreateBufs() {
-        for (void* p : dev) cudaFree(p);
-    }
+    DevAllocs dev;
 };
 
-// buffers of a track's upkeep calls (kba_upkeep.cu), kept like CreateBufs: the stamped slot map at its first upkeep call, alone or
-// in a group; the staging at its first single call
+// scratch of a track's upkeep, flow and reclaim calls (kba_upkeep.cu, kba_keyframe.cu, kba_reclaim.cu), kept like CreateBufs: the
+// stamped slot map at the first of them, alone or in a group
 struct UpkeepBufs {
-    SelectStage stage;                     // the single calls: keyframe slots | landmark slots, one window's outputs
-    SelectStage flow;                      // kba_track_frame_flow: one frame's lists and outputs, at its first call
-    SelectStage reclaim;                   // kba_track_reclaim_landmarks: the live keyframe slots and one range's outputs, at its first call
     unsigned long long* map = nullptr;     // [lm_cap] (stamp << 32) | payload by slot, all 0 (stamp 0: never a call's) at first
     int* blk = nullptr;                    // [ceil(lm_cap / kReclaimChunk)] free slots per chunk of a reclaimed range
     unsigned stamp = 0;                    // the last stamp a call used
-    std::vector<unsigned> kf_stamp, lm_stamp;  // duplicate checks: the check that named a slot last
-    unsigned check = 0;
-    ~UpkeepBufs() {
-        if (map) cudaFree(map);
-        if (blk) cudaFree(blk);
-    }
+    DevAllocs dev;
 };
 
 // buffers of a track's ranked selections (kba_rank.cu), kept like SelectBufs: the quantities, the scratch and the ranking at its first
-// ranking, alone or in a group; the staging at its first single call.  The ranking is what kba_track_solve_ranked reads.
+// ranking, alone or in a group.  The ranking is what kba_track_solve_ranked reads.
 struct RankBufs {
-    SelectStage stage;                     // kba_track_rank_landmarks: one window's lists, draws and outputs
     unsigned char* qty = nullptr;          // the chain's quantities, as select_run lays out one window's: flow | seen | near order |
                                            // counters | cheirality | bins, for lm_cap candidates
     int* mark = nullptr;                   // [lm_cap]
@@ -313,29 +298,43 @@ struct RankBufs {
     int n_sel = 0, n_ground = 0;
     uint64_t gen = 0;                      // kba_track::gen when it was ranked
     bool valid = false;
-    std::vector<void*> dev;
-    template <typename T> int alloc(T** p, size_t n) {
-        void* q = nullptr;
-        if (cudaMalloc(&q, std::max<size_t>(n, 1) * sizeof(T)) != cudaSuccess) return 1;
-        dev.push_back(q); *p = (T*)q; return 0;
+    DevAllocs dev;
+};
+
+// the duplicate checks of a track's slot lists (check_slot_lists, flow_check, frame_check): the check that named a slot last
+struct SlotStamps {
+    std::vector<unsigned> kf, lm;          // [kf_cap], [lm_cap]
+    unsigned cur = 0;
+    void next() {  // a fresh stamp; when the stamps wrap, start over
+        if (++cur == 0) { std::fill(kf.begin(), kf.end(), 0u); std::fill(lm.begin(), lm.end(), 0u); cur = 1; }
     }
-    ~RankBufs() {
-        for (void* p : dev) cudaFree(p);
-    }
+};
+
+// the store calls that stage their requests, one staging each; deactivation and depth costs share the upkeep one
+enum StoreCall { kSelectCall, kCreateCall, kUpkeepCall, kFlowCall, kReclaimCall, kRankCall, kStoreCalls };
+
+// what a track and a track group own alike.  A track's set is {the track}: its calls run the host code of a group's, with one
+// window.
+struct TrackSet {
+    kba_handle* h = nullptr;
+    std::vector<kba_track*> tracks;
+    TrackSolver solver;                    // window i of its batch is tracks[i]'s (fused path)
+    TrackSolver large;                     // some track has win_rows > kFusedMaxRows: the whole set on the large-window path, else no batch
+    std::unique_ptr<StoreStage> stage[kStoreCalls];  // each at its call's first run, for every track's capacities
+    const Transfer* last = &kNoTransfer;   // the transfer counts of the last call
+    ~TrackSet() { solver.release(); large.release(); }
 };
 
 // persistent, device-resident window (kba_track_*, at the end of this file)
 struct kba_track {
-    kba_handle* h = nullptr;
+    TrackSet set;                          // {this}
     kba_track_caps caps{};
     int n_cam = 0;
-    TrackSolver solver;                    // window 0 of its batch is this track's window (fused path)
-    TrackSolver large;                     // win_rows > kFusedMaxRows: the same for windows of more rows, else no batch
-    const TrackSolver* last = &solver;     // the solver of the last solve or pose-only call (transfer counts)
-    std::unique_ptr<SelectBufs> select;    // kba_track_select_landmarks, allocated at its first call
-    std::unique_ptr<CreateBufs> create;    // kba_track_create_landmarks, allocated at its first call
-    std::unique_ptr<UpkeepBufs> upkeep;    // kba_track_deactivate_keyframes / kba_track_depth_costs, allocated at the first of them
-    std::unique_ptr<RankBufs> rank;        // kba_track_rank_landmarks, allocated at its first call
+    std::unique_ptr<SelectBufs> select;    // selections and rankings, allocated at the first of them
+    std::unique_ptr<CreateBufs> create;    // landmark creations, allocated at the first one
+    std::unique_ptr<UpkeepBufs> upkeep;    // upkeep, flow and reclaim calls, allocated at the first of them
+    std::unique_ptr<RankBufs> rank;        // rankings, allocated at the first one
+    SlotStamps stamps;
     uint64_t gen = 0;                      // counts the calls that changed the store: a ranking of an older generation is stale
     TrackDev td{};
     int* arena_i[2][2] = {{nullptr, nullptr}, {nullptr, nullptr}};      // [buffer][lm, cam]
@@ -343,7 +342,7 @@ struct kba_track {
     int arena_cur = 0, arena_used = 0;
     std::vector<int> m_off, m_cnt;         // host mirror of the arena layout
     std::vector<char> kf_live;
-    std::vector<void*> dev;
+    DevAllocs dev;
     Staged<int> p_lm, p_cam, lay;          // pinned staging: one push / arena layout
     Staged<float> p_u, p_v, p_d;
     Staged<double> p_dbl;                  // poses / landmark values on their way to the store
@@ -351,11 +350,6 @@ struct kba_track {
     std::vector<double> cam_intr, cam_pose;  // host copy of the cameras: capacity windows of the track and of its groups
     int push_cap = 0, set_cap = 0;
     int64_t h2d_push = 0;
-    template <typename T> int alloc(T** p, size_t n) {
-        void* q = nullptr;
-        if (cudaMalloc(&q, std::max<size_t>(n, 1) * sizeof(T)) != cudaSuccess) return 1;
-        dev.push_back(q); *p = (T*)q; return 0;
-    }
     void point_arena() {
         td.m_lm = arena_i[arena_cur][0]; td.m_cam = arena_i[arena_cur][1];
         td.m_u = arena_f[arena_cur][0]; td.m_v = arena_f[arena_cur][1]; td.m_d = arena_f[arena_cur][2];
@@ -364,17 +358,7 @@ struct kba_track {
 
 // several tracks solved as one batch (kba_track_group_*, at the end of this file)
 struct kba_track_group {
-    kba_handle* h = nullptr;
-    std::vector<kba_track*> tracks;
-    TrackSolver solver;                    // window i of its batch is track i's (fused path)
-    TrackSolver large;                     // some track has win_rows > kFusedMaxRows: the whole group on the large-window path, else no batch
-    std::unique_ptr<SelectStage> select;   // kba_track_group_select_landmarks, allocated at its first call
-    std::unique_ptr<SelectStage> create;   // kba_track_group_create_landmarks, allocated at its first call
-    std::unique_ptr<SelectStage> upkeep;   // kba_track_group_deactivate_keyframes / _depth_costs, allocated at the first of them
-    std::unique_ptr<SelectStage> flow;     // kba_track_group_frame_flow, allocated at its first call
-    std::unique_ptr<SelectStage> reclaim;  // kba_track_group_reclaim_landmarks, allocated at its first call
-    std::unique_ptr<SelectStage> rank;     // kba_track_group_rank_landmarks, allocated at its first call
-    const TrackSolver* last = &solver;
+    TrackSet set;
 };
 
 static int validate_window(const kba_window* w, std::string& why) {
@@ -1461,14 +1445,7 @@ int kba_eval(kba_handle* h, const kba_window* w, const kba_options* opt, kba_eva
 // ---------------------------------------------------------------------------------------------------------------------
 void kba_track_destroy(kba_track* t) {
     if (!t) return;
-    cudaStreamSynchronize(t->h->stream);
-    t->solver.release();
-    t->large.release();
-    t->select.reset();
-    t->create.reset();
-    t->upkeep.reset();
-    t->rank.reset();
-    for (void* p : t->dev) cudaFree(p);
+    cudaStreamSynchronize(t->set.h->stream);
     t->p_lm.release(); t->p_cam.release(); t->lay.release();
     t->p_u.release(); t->p_v.release(); t->p_d.release(); t->p_dbl.release(); t->p_slot.release();
     delete t;
@@ -1534,6 +1511,7 @@ struct TrackRequest {
                                            // plane blocks counted whenever candidates are given)
     bool ranked = false;                   // the landmarks are the track's ranking (kba_track_solve_ranked): lm_slot is not read
     bool rank_gp = false;                  // ... and so are the ground-plane candidates (sel->n_gp of them)
+    kba_window ranked_sel{};               // a ranked request's window (ranked_check): sel points here
 };
 
 // ground points attached on the device: candidates in gp_lm, no keyframes or weights
@@ -1681,23 +1659,24 @@ int kba_track_create(kba_handle* h, const kba_track_caps* c, int32_t n_cam, cons
         return fail(KBA_ERR_CAPACITY, "kba_track_create: more than 32768 landmarks per window (the device sort)");
     CU(cudaSetDevice(h->device));
     kba_track* t = new kba_track();
-    t->h = h; t->caps = *c; t->n_cam = n_cam;
+    t->set.h = h; t->set.tracks = {t}; t->caps = *c; t->n_cam = n_cam;
     t->cam_intr.assign(cam_intr, cam_intr + 3 * (size_t)n_cam);
     t->cam_pose.assign(cam_pose, cam_pose + 7 * (size_t)n_cam);
-    int rc = track_solver_create(h, 1, &t, false, t->solver, "kba_track_create");
-    if (rc == KBA_OK && has_large(*c)) rc = track_solver_create(h, 1, &t, true, t->large, "kba_track_create");
-    if (rc != KBA_OK) { t->solver.release(); delete t; return rc; }
+    int rc = track_solver_create(h, 1, &t, false, t->set.solver, "kba_track_create");
+    if (rc == KBA_OK && has_large(*c)) rc = track_solver_create(h, 1, &t, true, t->set.large, "kba_track_create");
+    if (rc != KBA_OK) { delete t; return rc; }
     int bad = 0;
     TrackDev& td = t->td;
+    DevAllocs& dev = t->dev;
     td.kf_cap = c->max_keyframes; td.lm_cap = c->max_landmarks; td.m_cap = c->max_measurements;
-    bad |= t->alloc(&td.kf_pose, 7 * (size_t)td.kf_cap); bad |= t->alloc(&td.kf_plane, 4 * (size_t)td.kf_cap);
-    bad |= t->alloc(&td.m_off, td.kf_cap); bad |= t->alloc(&td.m_cnt, td.kf_cap);
+    bad |= dev.alloc(&td.kf_pose, 7 * (size_t)td.kf_cap); bad |= dev.alloc(&td.kf_plane, 4 * (size_t)td.kf_cap);
+    bad |= dev.alloc(&td.m_off, td.kf_cap); bad |= dev.alloc(&td.m_cnt, td.kf_cap);
     for (int b2 = 0; b2 < 2; ++b2) {
-        for (int q = 0; q < 2; ++q) bad |= t->alloc(&t->arena_i[b2][q], td.m_cap);
-        for (int q = 0; q < 3; ++q) bad |= t->alloc(&t->arena_f[b2][q], td.m_cap);
+        for (int q = 0; q < 2; ++q) bad |= dev.alloc(&t->arena_i[b2][q], td.m_cap);
+        for (int q = 0; q < 3; ++q) bad |= dev.alloc(&t->arena_f[b2][q], td.m_cap);
     }
-    bad |= t->alloc(&td.lm_pos, 3 * (size_t)td.lm_cap); bad |= t->alloc(&td.lm_weight, td.lm_cap); bad |= t->alloc(&td.sel_index, td.lm_cap);
-    bad |= t->alloc(&td.cursor, c->win_landmarks); bad |= t->alloc(&td.key, c->win_observations); bad |= t->alloc(&td.n_depth, 1);
+    bad |= dev.alloc(&td.lm_pos, 3 * (size_t)td.lm_cap); bad |= dev.alloc(&td.lm_weight, td.lm_cap); bad |= dev.alloc(&td.sel_index, td.lm_cap);
+    bad |= dev.alloc(&td.cursor, c->win_landmarks); bad |= dev.alloc(&td.key, c->win_observations); bad |= dev.alloc(&td.n_depth, 1);
     t->push_cap = std::min(c->max_measurements, 1 << 16);
     bad |= t->p_lm.alloc(t->push_cap, true); bad |= t->p_cam.alloc(t->push_cap, true); bad |= t->p_u.alloc(t->push_cap, true);
     bad |= t->p_v.alloc(t->push_cap, true); bad |= t->p_d.alloc(t->push_cap, true);
@@ -1707,6 +1686,7 @@ int kba_track_create(kba_handle* h, const kba_track_caps* c, int32_t n_cam, cons
     if (bad) { kba_track_destroy(t); return fail(KBA_ERR_CUDA, "kba_track_create: out of memory"); }
     t->point_arena();
     t->m_off.assign(td.kf_cap, 0); t->m_cnt.assign(td.kf_cap, 0); t->kf_live.assign(td.kf_cap, 0);
+    t->stamps.kf.assign(td.kf_cap, 0u); t->stamps.lm.assign(td.lm_cap, 0u);
     cudaStream_t s = h->stream;
     CU(cudaMemsetAsync(td.sel_index, 0xff, sizeof(int) * (size_t)td.lm_cap, s));
     CU(cudaMemsetAsync(td.m_cnt, 0, sizeof(int) * (size_t)td.kf_cap, s));
@@ -1720,7 +1700,7 @@ static int track_upload_layout(kba_track* t) {  // arena offsets / counts of eve
     const int K = t->td.kf_cap;
     memcpy(t->lay.h, t->m_off.data(), K * sizeof(int));
     memcpy(t->lay.h + K, t->m_cnt.data(), K * sizeof(int));
-    cudaStream_t s = t->h->stream;
+    cudaStream_t s = t->set.h->stream;
     CU(cudaMemcpyAsync(t->td.m_off, t->lay.h, K * sizeof(int), cudaMemcpyHostToDevice, s));
     CU(cudaMemcpyAsync(t->td.m_cnt, t->lay.h + K, K * sizeof(int), cudaMemcpyHostToDevice, s));
     CU(cudaStreamSynchronize(s));  // the pinned layout buffer is reused by the next call
@@ -1730,7 +1710,7 @@ static int track_upload_layout(kba_track* t) {  // arena offsets / counts of eve
 
 static int track_compact(kba_track* t) {  // live keyframes copied, in slot order, into the other arena
     const int other = 1 - t->arena_cur;
-    cudaStream_t s = t->h->stream;
+    cudaStream_t s = t->set.h->stream;
     int used = 0;
     for (int k = 0; k < t->td.kf_cap; ++k) {
         if (!t->kf_live[k] || t->m_cnt[k] == 0) { if (!t->kf_live[k]) t->m_cnt[k] = 0; continue; }
@@ -1752,13 +1732,13 @@ int kba_track_push_keyframe(kba_track* t, int32_t slot, const double* pose7, con
     if (t->kf_live[slot]) return fail(KBA_ERR_BAD_ARG, "kba_track_push_keyframe: slot in use (drop it first)");
     for (int i = 0; i < n; ++i)
         if (lm[i] < 0 || lm[i] >= t->td.lm_cap || (cam && (cam[i] < 0 || cam[i] >= t->n_cam))) return fail(KBA_ERR_BAD_ARG, "kba_track_push_keyframe: landmark slot / camera out of range");
-    CU(cudaSetDevice(t->h->device));
+    CU(cudaSetDevice(t->set.h->device));
     if (t->arena_used + n > t->td.m_cap) {
         const int rc = track_compact(t);
         if (rc != KBA_OK) return rc;
         if (t->arena_used + n > t->td.m_cap) return fail(KBA_ERR_CAPACITY, "kba_track_push_keyframe: measurement arena full");
     }
-    cudaStream_t s = t->h->stream;
+    cudaStream_t s = t->set.h->stream;
     for (int i0 = 0; i0 < n; i0 += t->push_cap) {  // staged through pinned memory in chunks
         const int m = std::min(t->push_cap, n - i0);
         memcpy(t->p_lm.h, lm + i0, m * sizeof(int));
@@ -1790,7 +1770,7 @@ int kba_track_drop_keyframe(kba_track* t, int32_t slot) {
 
 // rows of `width` doubles into their store slots: staged through pinned memory, one copy + one scatter kernel per chunk
 static int track_scatter(kba_track* t, double* dst, int cap_slots, int n, const int32_t* slot, const double* src, int width) {
-    cudaStream_t s = t->h->stream;
+    cudaStream_t s = t->set.h->stream;
     for (int i0 = 0; i0 < n; i0 += t->set_cap) {
         const int m = std::min(t->set_cap, n - i0);
         for (int i = 0; i < m; ++i)
@@ -1807,7 +1787,7 @@ static int track_scatter(kba_track* t, double* dst, int cap_slots, int n, const 
 
 int kba_track_set_keyframe_poses(kba_track* t, int32_t n, const int32_t* slot, const double* pose7s, const double* plane4s) {
     if (!t || n < 0 || (n > 0 && (!slot || !pose7s))) return fail(KBA_ERR_BAD_ARG, "bad argument to kba_track_set_keyframe_poses");
-    CU(cudaSetDevice(t->h->device));
+    CU(cudaSetDevice(t->set.h->device));
     t->gen++;
     int rc = track_scatter(t, t->td.kf_pose, t->td.kf_cap, n, slot, pose7s, 7);
     if (rc == KBA_OK && plane4s) rc = track_scatter(t, t->td.kf_plane, t->td.kf_cap, n, slot, plane4s, 4);
@@ -1821,7 +1801,7 @@ int kba_track_set_keyframe_pose(kba_track* t, int32_t slot, const double* pose7,
 
 int kba_track_set_landmarks(kba_track* t, int32_t n, const int32_t* slot, const double* pos3, const double* weight) {
     if (!t || n < 0 || (n > 0 && !slot)) return fail(KBA_ERR_BAD_ARG, "bad argument to kba_track_set_landmarks");
-    CU(cudaSetDevice(t->h->device));
+    CU(cudaSetDevice(t->set.h->device));
     t->gen++;
     int rc = KBA_OK;
     if (pos3) rc = track_scatter(t, t->td.lm_pos, t->td.lm_cap, n, slot, pos3, 3);
@@ -1900,7 +1880,7 @@ static int track_solve(kba_handle* h, TrackSolver& sv, int n, kba_track* const* 
     CU(cudaMemcpyAsync(sv.lists.d, sv.lists.h, used * sizeof(int), cudaMemcpyHostToDevice, s));
     CU(sv.tdev.upload(s)); CU(sv.tsel.upload(s));
     if (any_gp) { CU(b->r_gp_lm.upload(s)); CU(b->gp_kf.upload(s)); CU(b->gp_weight.upload(s)); }
-    sv.h2d = h2d;
+    sv.counts.h2d = h2d;
     // ---- gather every window from its store, pack, solve, write back
     launch_track_gather(b->bd, b->raw, sv.tdev.d, sv.tsel.d, grid, s);
     launch_pack(b->bd, b->raw, s);
@@ -1909,31 +1889,206 @@ static int track_solve(kba_handle* h, TrackSolver& sv, int n, kba_track* const* 
     if (rc != KBA_OK) return rc;
     launch_track_writeback(b->bd, sv.tdev.d, sv.tsel.d, grid, s);
     rc = kba_batch_download(b, res);
-    sv.d2h = (int64_t)b->d2h_bytes;
+    sv.counts.d2h = (int64_t)b->d2h_bytes;
     return rc;
+}
+
+// the checks of a solve of track t's ranking: q holds the caller's keyframe lists and window; it is pointed at the ranking and at
+// q.ranked_sel, the caller's window with the ranking's ground-candidate count
+static int ranked_check(kba_track* t, TrackRequest& q, std::string& why) {
+    if (!q.kf_slot || !q.kf_fixed || !q.sel) { why = "null argument"; return KBA_ERR_BAD_ARG; }
+    const RankBufs* rb = t->rank.get();
+    if (!rb || !rb->valid) { why = "the track has no ranking to solve (kba_track_rank_landmarks)"; return KBA_ERR_BAD_ARG; }
+    if (rb->gen != t->gen) { why = "the ranking is stale: the store changed after it was ranked"; return KBA_ERR_BAD_ARG; }
+    if (q.n_kf != (int)rb->kf.size() || !std::equal(rb->kf.begin(), rb->kf.end(), q.kf_slot)) {
+        why = "the keyframes differ from the ranking's"; return KBA_ERR_BAD_ARG;
+    }
+    const kba_window* sel = q.sel;
+    q.ranked_sel = *sel;
+    const bool from_ranking = sel->n_gp > 0 && !sel->gp_lm && !sel->gp_kf && !sel->gp_weight;
+    if (from_ranking) q.ranked_sel.n_gp = rb->n_ground;
+    q.n_lm = rb->n_sel; q.lm_slot = nullptr; q.sel = &q.ranked_sel;
+    q.rank_gp = from_ranking && rb->n_ground > 0;
+    return track_check(t, q, why);
+}
+
+static std::string track_prefix(bool group, int i) { return group ? "track " + std::to_string(i) + ": " : std::string(); }
+
+// one solve of the windows of a track (group = false) or of a group, qs[i] track i's request.  Every request is checked in track
+// order before anything is uploaded or launched; in a group, one with n_kf == 0 sits the solve out.  The solver is the one
+// kba_batch_create would choose for the whole batch: the large-window path as soon as one window needs more than kFusedMaxRows
+// reduced rows.
+static int set_solve(TrackSet& s, bool group, const std::string& who, TrackRequest* qs, const kba_options* opt, kba_result* res) {
+    const int n = (int)s.tracks.size();
+    bool any = false, large = false;
+    for (int i = 0; i < n; ++i) {
+        TrackRequest& q = qs[i];
+        if (group && q.n_kf == 0) { q.sel = nullptr; continue; }  // sits this solve out
+        std::string why;
+        const int rc = q.ranked ? ranked_check(s.tracks[i], q, why) : track_check(s.tracks[i], q, why);
+        if (rc != KBA_OK) return fail(rc, who + track_prefix(group, i) + why);
+        any = true;
+        large |= q.rows > kFusedMaxRows;
+    }
+    if (!any) {  // nothing to solve: no upload, no launch, every result idle
+        for (int i = 0; i < n; ++i) idle_result(res[i]);
+        s.last = &kNoTransfer;
+        return KBA_OK;
+    }
+    TrackSolver& sv = large ? s.large : s.solver;
+    s.last = &sv.counts;
+    return track_solve(s.h, sv, n, s.tracks.data(), qs, opt, res);
+}
+
+static TrackRequest track_request(int32_t n_kf, const int32_t* kf_slot, const uint8_t* kf_fixed, int32_t n_lm, const int32_t* lm_slot,
+                                  const kba_window* sel, bool ranked) {
+    TrackRequest q;
+    q.n_kf = n_kf; q.kf_slot = kf_slot; q.kf_fixed = kf_fixed; q.n_lm = n_lm; q.lm_slot = lm_slot; q.sel = sel; q.ranked = ranked;
+    return q;
 }
 
 int kba_track_solve(kba_track* t, int32_t n_kf, const int32_t* kf_slot, const uint8_t* kf_fixed, int32_t n_lm, const int32_t* lm_slot,
                     const kba_window* sel, const kba_options* opt, kba_result* res) {
     if (!t || !opt || !res) return fail(KBA_ERR_BAD_ARG, "null argument to kba_track_solve");
-    TrackRequest q;
-    q.n_kf = n_kf; q.kf_slot = kf_slot; q.kf_fixed = kf_fixed; q.n_lm = n_lm; q.lm_slot = lm_slot; q.sel = sel;
-    std::string why;
-    const int rc = track_check(t, q, why);
-    if (rc != KBA_OK) return fail(rc, "kba_track_solve: " + why);
-    // the solver kba_batch_create would choose for this window: fused iff at most kFusedMaxRows reduced rows
-    TrackSolver& sv = q.rows > kFusedMaxRows ? t->large : t->solver;
-    t->last = &sv;
-    return track_solve(t->h, sv, 1, &t, &q, opt, res);
+    TrackRequest q = track_request(n_kf, kf_slot, kf_fixed, n_lm, lm_slot, sel, false);
+    return set_solve(t->set, false, "kba_track_solve: ", &q, opt, res);
 }
 
 int kba_track_transfer_bytes(kba_track* t, int64_t* h2d, int64_t* d2h, int64_t* push) {
     if (!t) return fail(KBA_ERR_BAD_ARG, "null track");
-    if (h2d) *h2d = t->last->h2d;
-    if (d2h) *d2h = t->last->d2h;
+    if (h2d) *h2d = t->set.last->h2d;
+    if (d2h) *d2h = t->set.last->d2h;
     if (push) *push = t->h2d_push;
     return KBA_OK;
 }
+
+// ---------------------------------------------------------------------------------------------------------------------
+// several persistent windows solved in one batch (include/kba_b200.h, kba_track_group_*)
+// ---------------------------------------------------------------------------------------------------------------------
+void kba_track_group_destroy(kba_track_group* g) {
+    if (!g) return;
+    cudaStreamSynchronize(g->set.h->stream);
+    delete g;
+}
+
+int kba_track_group_create(kba_handle* h, int32_t n_tracks, kba_track* const* tracks, kba_track_group** out) {
+    if (!h || !tracks || !out || n_tracks < 1) return fail(KBA_ERR_BAD_ARG, "kba_track_group_create: empty group or null argument");
+    for (int i = 0; i < n_tracks; ++i) {
+        if (!tracks[i]) return fail(KBA_ERR_BAD_ARG, "kba_track_group_create: track " + std::to_string(i) + " is null");
+        if (tracks[i]->set.h != h) return fail(KBA_ERR_BAD_ARG, "kba_track_group_create: track " + std::to_string(i) + " belongs to another handle");
+        for (int j = 0; j < i; ++j)
+            if (tracks[j] == tracks[i])
+                return fail(KBA_ERR_BAD_ARG, "kba_track_group_create: track " + std::to_string(i) + " is also track " + std::to_string(j));
+    }
+    CU(cudaSetDevice(h->device));
+    kba_track_group* g = new kba_track_group();
+    g->set.h = h;
+    g->set.tracks.assign(tracks, tracks + n_tracks);
+    int rc = track_solver_create(h, n_tracks, tracks, false, g->set.solver, "kba_track_group_create");
+    bool large = false;
+    for (int i = 0; i < n_tracks; ++i) large |= has_large(tracks[i]->caps);
+    if (rc == KBA_OK && large) rc = track_solver_create(h, n_tracks, tracks, true, g->set.large, "kba_track_group_create");
+    if (rc != KBA_OK) { delete g; return rc; }
+    *out = g;
+    return KBA_OK;
+}
+
+int kba_track_group_solve(kba_track_group* g, const kba_track_request* req, const kba_options* opt, kba_result* res) {
+    if (!g || !req || !opt || !res) return fail(KBA_ERR_BAD_ARG, "null argument to kba_track_group_solve");
+    std::vector<TrackRequest> qs;
+    for (size_t i = 0; i < g->set.tracks.size(); ++i)
+        qs.push_back(track_request(req[i].n_kf, req[i].kf_slot, req[i].kf_fixed, req[i].n_lm, req[i].lm_slot, req[i].sel, false));
+    return set_solve(g->set, true, "kba_track_group_solve: ", qs.data(), opt, res);
+}
+
+int kba_track_group_transfer_bytes(kba_track_group* g, int64_t* h2d, int64_t* d2h) {
+    if (!g) return fail(KBA_ERR_BAD_ARG, "null track group");
+    if (h2d) *h2d = g->set.last->h2d;
+    if (d2h) *d2h = g->set.last->d2h;
+    return KBA_OK;
+}
+
+// ---------------------------------------------------------------------------------------------------------------------
+// store calls of a track and of a group (landmark selection, creation, upkeep, frame flow, reclaim, ranking): one driver, which a
+// single call runs with the track's one-track set
+// ---------------------------------------------------------------------------------------------------------------------
+// the slot lists of one request of track t, checked with a fresh stamp of its duplicate checks: keyframes pushed, landmarks in
+// range, no slot listed twice.  max_meas: arena entries of the largest listed keyframe.
+static int check_slot_lists(kba_track* t, int n_kf, const int32_t* kf_slot, int n_lm, const int32_t* lm_slot, int& max_meas,
+                            std::string& why) {
+    SlotStamps& st = t->stamps;
+    st.next();
+    max_meas = 0;
+    for (int k = 0; k < n_kf; ++k) {
+        const int s = kf_slot[k];
+        if (s < 0 || s >= t->td.kf_cap || !t->kf_live[s]) { why = "keyframe slot not pushed"; return KBA_ERR_BAD_ARG; }
+        if (st.kf[s] == st.cur) { why = "keyframe slot listed twice"; return KBA_ERR_BAD_ARG; }
+        st.kf[s] = st.cur;
+        max_meas = std::max(max_meas, t->m_cnt[s]);
+    }
+    for (int j = 0; j < n_lm; ++j) {
+        const int s = lm_slot[j];
+        if (s < 0 || s >= t->td.lm_cap) { why = "landmark slot out of range"; return KBA_ERR_BAD_ARG; }
+        if (st.lm[s] == st.cur) { why = "landmark slot listed twice"; return KBA_ERR_BAD_ARG; }
+        st.lm[s] = st.cur;
+    }
+    return KBA_OK;
+}
+
+// One store call of the tracks of s (group = false: a single call), req[i] / out[i] track i's.  C describes the call:
+//   Request, Out         its public request and output types; Req the checked request of one window
+//   slot, staging        its staging in s.stage and the staging's name in errors
+//   sits_out(q)          a group's request that sits the call out: not checked, except what sit_out_check reads; a single
+//                        request is checked, and then does not run (a reclaim of an empty range: the other checks refuse it)
+//   sat_out(o, group)    what a request that sat out writes once the call succeeded
+//   make, check          the request of one window, and every check of it before anything is uploaded
+//   capacity(n, ts, ..)  the staging's upload and download bytes for tracks ts[0..n) at their capacities (n = 1: a single call's)
+//   run                  the requests that do not sit out as the windows of one launch sequence; a failure of request w it
+//                        reports as (bad = w, why)
+// Requests are checked in track order, and the first failure, named after its track in a group, returns before anything is
+// uploaded or written.  A call in which nothing runs reports no transfers.
+extern "C++" {  // templates have C++ linkage
+template <class C>
+static int store_call(TrackSet& s, bool group, const std::string& who, const typename C::Request* req, typename C::Out* out) {
+    const int n = (int)s.tracks.size();
+    std::vector<typename C::Req> rs;
+    std::vector<int> track_of;             // rs[w] is the request of track track_of[w]
+    for (int i = 0; i < n; ++i) {
+        const bool sits_out = C::sits_out(req[i]);
+        std::string why;
+        int rc;
+        typename C::Req r;
+        if (group && sits_out) {
+            rc = C::sit_out_check(out[i], why);
+        } else {
+            r = C::make(s.tracks[i], req[i], out + i);
+            rc = C::check(r, why);
+        }
+        if (rc != KBA_OK) return fail(rc, who + track_prefix(group, i) + why);
+        if (!sits_out) { rs.push_back(r); track_of.push_back(i); }
+    }
+    if (rs.empty()) {  // no upload, no launch
+        s.last = &kNoTransfer;
+    } else {
+        std::unique_ptr<StoreStage>& st = s.stage[C::slot];
+        if (!st) {
+            size_t up = 0, down = 0;
+            C::capacity(n, s.tracks.data(), up, down);
+            std::unique_ptr<StoreStage> fresh(new StoreStage());
+            if (fresh->alloc(up, down)) return fail(KBA_ERR_CUDA, who + "out of memory for the " + C::staging + " staging");
+            st = std::move(fresh);
+        }
+        int bad = -1;
+        std::string why;
+        const int rc = C::run(s.h, *st, (int)rs.size(), rs.data(), bad, why);
+        if (rc != KBA_OK) return bad < 0 ? rc : fail(rc, who + track_prefix(group, track_of[bad]) + why);
+        s.last = &st->counts;
+    }
+    for (int i = 0; i < n; ++i)
+        if (C::sits_out(req[i])) C::sat_out(out + i, group);
+    return KBA_OK;
+}
+}  // extern "C++"
 
 // ---------------------------------------------------------------------------------------------------------------------
 // landmark selection on the stored window (include/kba_b200.h, kba_track_select_landmarks / kba_track_group_select_landmarks;
@@ -1949,19 +2104,19 @@ static int select_alloc(kba_track* t, std::string& why) {
     SelectArgs& a = sb->a;
     double* cams = nullptr;
     int bad = 0;
-    bad |= sb->alloc(&a.cand_of, L); bad |= sb->alloc(&a.kf_T, 12 * K); bad |= sb->alloc(&a.cam_T, 12 * (size_t)kMaxCam);
-    bad |= sb->alloc(&a.path, 3 * K); bad |= sb->alloc(&a.pt, 3 * L); bad |= sb->alloc(&a.cnt, L); bad |= sb->alloc(&a.cursor, L);
-    bad |= sb->alloc(&a.obs_off, L); bad |= sb->alloc(&a.in_list, L); bad |= sb->alloc(&a.vkey, L); bad |= sb->alloc(&a.sorted, L);
-    bad |= sb->alloc(&a.near_flag, L); bad |= sb->alloc(&a.okey, (size_t)td.m_cap); bad |= sb->alloc(&a.bounds, 6);
-    bad |= sb->alloc(&cams, 7 * (size_t)t->n_cam);
+    DevAllocs& dev = sb->dev;
+    bad |= dev.alloc(&a.cand_of, L); bad |= dev.alloc(&a.kf_T, 12 * K); bad |= dev.alloc(&a.cam_T, 12 * (size_t)kMaxCam);
+    bad |= dev.alloc(&a.path, 3 * K); bad |= dev.alloc(&a.pt, 3 * L); bad |= dev.alloc(&a.cnt, L); bad |= dev.alloc(&a.cursor, L);
+    bad |= dev.alloc(&a.obs_off, L); bad |= dev.alloc(&a.in_list, L); bad |= dev.alloc(&a.vkey, L); bad |= dev.alloc(&a.sorted, L);
+    bad |= dev.alloc(&a.near_flag, L); bad |= dev.alloc(&a.okey, (size_t)td.m_cap); bad |= dev.alloc(&a.bounds, 6);
+    bad |= dev.alloc(&cams, 7 * (size_t)t->n_cam);
     if (bad) { why = "out of memory for the selection buffers"; return KBA_ERR_CUDA; }
-    cudaStream_t s = t->h->stream;
+    cudaStream_t s = t->set.h->stream;
     cudaError_t e = cudaMemsetAsync(a.cand_of, 0xff, sizeof(int) * L, s);
     if (e == cudaSuccess) e = cudaMemcpyAsync(cams, t->cam_pose.data(), sizeof(double) * 7 * (size_t)t->n_cam, cudaMemcpyHostToDevice, s);
     if (e == cudaSuccess) e = cudaStreamSynchronize(s);
     if (e != cudaSuccess) { why = std::string("selection buffers: ") + cudaGetErrorString(e); return KBA_ERR_CUDA; }
     a.cam_pose7 = cams; a.n_cam = t->n_cam;
-    sb->kf_stamp.assign(K, 0); sb->lm_stamp.assign(L, 0);
     t->select = std::move(sb);
     return KBA_OK;
 }
@@ -1990,34 +2145,16 @@ static int select_check(SelectReq& r, std::string& why) {
     if (r.n_kf > t->td.kf_cap || r.n_cand > t->td.lm_cap) { why = "more keyframes or candidates than the track's slots"; return KBA_ERR_CAPACITY; }
     for (int q = 0; q < 3; ++q)
         if (!(r.p->voxel_size[q] > 0.0) || !std::isfinite(r.p->voxel_size[q])) { why = "voxel sizes must be finite and positive"; return KBA_ERR_BAD_ARG; }
-    const cudaError_t e = cudaSetDevice(t->h->device);
+    const cudaError_t e = cudaSetDevice(t->set.h->device);
     if (e != cudaSuccess) { why = std::string("cudaSetDevice: ") + cudaGetErrorString(e); return KBA_ERR_CUDA; }
     if (!t->select) { const int rc = select_alloc(t, why); if (rc != KBA_OK) return rc; }
-    SelectBufs& sb = *t->select;
-    if (++sb.stamp == 0) {  // the stamps wrapped: start over
-        std::fill(sb.kf_stamp.begin(), sb.kf_stamp.end(), 0u); std::fill(sb.lm_stamp.begin(), sb.lm_stamp.end(), 0u); sb.stamp = 1;
-    }
-    r.max_meas = 0;
-    for (int k = 0; k < r.n_kf; ++k) {
-        const int s = r.kf_slot[k];
-        if (s < 0 || s >= t->td.kf_cap || !t->kf_live[s]) { why = "keyframe slot not pushed"; return KBA_ERR_BAD_ARG; }
-        if (sb.kf_stamp[s] == sb.stamp) { why = "keyframe slot listed twice"; return KBA_ERR_BAD_ARG; }
-        sb.kf_stamp[s] = sb.stamp;
-        r.max_meas = std::max(r.max_meas, t->m_cnt[s]);
-    }
-    for (int c = 0; c < r.n_cand; ++c) {
-        const int s = r.lm_slot[c];
-        if (s < 0 || s >= t->td.lm_cap) { why = "landmark slot out of range"; return KBA_ERR_BAD_ARG; }
-        if (sb.lm_stamp[s] == sb.stamp) { why = "landmark slot listed twice"; return KBA_ERR_BAD_ARG; }
-        sb.lm_stamp[s] = sb.stamp;
-    }
-    return KBA_OK;
+    return check_slot_lists(t, r.n_kf, r.kf_slot, r.n_cand, r.lm_slot, r.max_meas, why);
 }
 
 // W checked requests of distinct tracks as the W windows of one launch sequence: one upload (the argument records of windows
 // 1 .. W-1, then every window's lists), one download (the outputs of all windows), one synchronisation, then the scatter into the
 // callers' arrays.  Window 0's record travels in the launch parameters (kba_select.cu).
-static int select_run(kba_handle* h, SelectStage& st, int W, const SelectReq* r) {
+static int select_run(kba_handle* h, StoreStage& st, int W, const SelectReq* r) {
     CU(cudaSetDevice(h->device));
     cudaStream_t s = h->stream;
     SelectGrid g;
@@ -2079,138 +2216,45 @@ static int select_run(kba_handle* h, SelectStage& st, int W, const SelectReq* r)
     return KBA_OK;
 }
 
+struct Select {
+    using Request = kba_select_request;
+    using Out = kba_select_out;
+    using Req = SelectReq;
+    static constexpr StoreCall slot = kSelectCall;
+    static constexpr const char* staging = "selection";
+    static bool sits_out(const Request& q) { return q.n_kf == 0; }
+    static int sit_out_check(const Out& o, std::string& why) {  // the request's n_near is written
+        if (o.n_near) return KBA_OK;
+        why = "null argument"; return KBA_ERR_BAD_ARG;
+    }
+    static void sat_out(Out* o, bool) { *o->n_near = 0; }
+    static Req make(kba_track* t, const Request& q, Out* o) {
+        Req r;
+        r.t = t; r.n_kf = q.n_kf; r.n_cand = q.n_cand; r.kf_slot = q.kf_slot; r.lm_slot = q.lm_slot; r.p = q.params; r.o = o;
+        return r;
+    }
+    static int check(Req& r, std::string& why) { return select_check(r, why); }
+    static void capacity(int n, kba_track* const* ts, size_t& up, size_t& down) {
+        size_t lists = 0, cands = 0;
+        for (int i = 0; i < n; ++i) { lists += (size_t)ts[i]->td.kf_cap + ts[i]->td.lm_cap; cands += (size_t)ts[i]->td.lm_cap; }
+        up = sizeof(SelectArgs) * (size_t)(n - 1) + 4 * lists;
+        down = select_out_bytes(cands, (size_t)n);
+    }
+    static int run(kba_handle* h, StoreStage& st, int W, Req* r, int&, std::string&) { return select_run(h, st, W, r); }
+};
+
 int kba_track_select_landmarks(kba_track* t, int32_t n_kf, const int32_t* kf_slot, int32_t n_cand, const int32_t* lm_slot,
                                const kba_select_params* p, kba_select_out* o) {
     static const std::string who = "kba_track_select_landmarks: ";
     if (!t) return fail(KBA_ERR_BAD_ARG, who + "null argument");
-    SelectReq r;
-    r.t = t; r.n_kf = n_kf; r.n_cand = n_cand; r.kf_slot = kf_slot; r.lm_slot = lm_slot; r.p = p; r.o = o;
-    std::string why;
-    int rc = select_check(r, why);
-    if (rc != KBA_OK) return fail(rc, who + why);
-    SelectStage& st = t->select->stage;
-    if (!st.up.d) {  // the first single call of the track
-        const size_t K = (size_t)t->td.kf_cap, L = (size_t)t->td.lm_cap;
-        if (st.alloc(4 * (K + L), select_out_bytes(L, 1))) {
-            st.up.release(); st.out.release();
-            return fail(KBA_ERR_CUDA, who + "out of memory for the selection staging");
-        }
-    }
-    rc = select_run(t->h, st, 1, &r);
-    if (rc == KBA_OK) t->last = &t->select->stage.counts;
-    return rc;
-}
-
-// ---------------------------------------------------------------------------------------------------------------------
-// several persistent windows solved in one batch (include/kba_b200.h, kba_track_group_*)
-// ---------------------------------------------------------------------------------------------------------------------
-void kba_track_group_destroy(kba_track_group* g) {
-    if (!g) return;
-    cudaStreamSynchronize(g->h->stream);
-    g->solver.release();
-    g->large.release();
-    delete g;
-}
-
-int kba_track_group_create(kba_handle* h, int32_t n_tracks, kba_track* const* tracks, kba_track_group** out) {
-    if (!h || !tracks || !out || n_tracks < 1) return fail(KBA_ERR_BAD_ARG, "kba_track_group_create: empty group or null argument");
-    for (int i = 0; i < n_tracks; ++i) {
-        if (!tracks[i]) return fail(KBA_ERR_BAD_ARG, "kba_track_group_create: track " + std::to_string(i) + " is null");
-        if (tracks[i]->h != h) return fail(KBA_ERR_BAD_ARG, "kba_track_group_create: track " + std::to_string(i) + " belongs to another handle");
-        for (int j = 0; j < i; ++j)
-            if (tracks[j] == tracks[i])
-                return fail(KBA_ERR_BAD_ARG, "kba_track_group_create: track " + std::to_string(i) + " is also track " + std::to_string(j));
-    }
-    CU(cudaSetDevice(h->device));
-    kba_track_group* g = new kba_track_group();
-    g->h = h;
-    g->tracks.assign(tracks, tracks + n_tracks);
-    int rc = track_solver_create(h, n_tracks, tracks, false, g->solver, "kba_track_group_create");
-    bool large = false;
-    for (int i = 0; i < n_tracks; ++i) large |= has_large(tracks[i]->caps);
-    if (rc == KBA_OK && large) rc = track_solver_create(h, n_tracks, tracks, true, g->large, "kba_track_group_create");
-    if (rc != KBA_OK) { g->solver.release(); delete g; return rc; }
-    *out = g;
-    return KBA_OK;
-}
-
-int kba_track_group_solve(kba_track_group* g, const kba_track_request* req, const kba_options* opt, kba_result* res) {
-    if (!g || !req || !opt || !res) return fail(KBA_ERR_BAD_ARG, "null argument to kba_track_group_solve");
-    const int n = (int)g->tracks.size();
-    // ---- every request is checked before anything is uploaded or launched
-    std::vector<TrackRequest> qs(n);
-    int active = 0;
-    bool large = false;
-    for (int i = 0; i < n; ++i) {
-        const kba_track_request& r = req[i];
-        if (r.n_kf == 0) continue;  // sits this solve out
-        TrackRequest& q = qs[i];
-        q.n_kf = r.n_kf; q.kf_slot = r.kf_slot; q.kf_fixed = r.kf_fixed; q.n_lm = r.n_lm; q.lm_slot = r.lm_slot; q.sel = r.sel;
-        std::string why;
-        const int rc = track_check(g->tracks[i], q, why);
-        if (rc != KBA_OK) return fail(rc, "kba_track_group_solve: track " + std::to_string(i) + ": " + why);
-        ++active;
-        large |= q.rows > kFusedMaxRows;
-    }
-    if (active == 0) {  // nothing to solve: no upload, no launch, every result idle
-        for (int i = 0; i < n; ++i) idle_result(res[i]);
-        g->solver.h2d = 0; g->solver.d2h = 0;
-        g->last = &g->solver;
-        return KBA_OK;
-    }
-    // kba_batch_create's rule for the whole batch: the large-window path as soon as one window needs it
-    TrackSolver& sv = large ? g->large : g->solver;
-    g->last = &sv;
-    return track_solve(g->h, sv, n, g->tracks.data(), qs.data(), opt, res);
-}
-
-int kba_track_group_transfer_bytes(kba_track_group* g, int64_t* h2d, int64_t* d2h) {
-    if (!g) return fail(KBA_ERR_BAD_ARG, "null track group");
-    if (h2d) *h2d = g->last->h2d;
-    if (d2h) *d2h = g->last->d2h;
-    return KBA_OK;
+    const kba_select_request q = {n_kf, n_cand, kf_slot, lm_slot, p};
+    return store_call<Select>(t->set, false, who, &q, o);
 }
 
 int kba_track_group_select_landmarks(kba_track_group* g, const kba_select_request* req, kba_select_out* out) {
     static const std::string who = "kba_track_group_select_landmarks: ";
     if (!g || !req || !out) return fail(KBA_ERR_BAD_ARG, who + "null argument");
-    const int n = (int)g->tracks.size();
-    // ---- every request is checked before anything is uploaded or written
-    std::vector<SelectReq> rs;
-    for (int i = 0; i < n; ++i) {
-        const kba_select_request& q = req[i];
-        const std::string track = "track " + std::to_string(i) + ": ";
-        if (q.n_kf == 0) {  // sits the call out
-            if (!out[i].n_near) return fail(KBA_ERR_BAD_ARG, who + track + "null argument");
-            continue;
-        }
-        SelectReq r;
-        r.t = g->tracks[i]; r.n_kf = q.n_kf; r.n_cand = q.n_cand; r.kf_slot = q.kf_slot; r.lm_slot = q.lm_slot; r.p = q.params; r.o = &out[i];
-        std::string why;
-        const int rc = select_check(r, why);
-        if (rc != KBA_OK) return fail(rc, who + track + why);
-        rs.push_back(r);
-    }
-    int rc = KBA_OK;
-    if (rs.empty()) {  // every track sits out: no upload, no launch
-        g->solver.h2d = 0; g->solver.d2h = 0;
-        g->last = &g->solver;
-    } else {
-        if (!g->select) {  // staging for every track at its capacities, allocated once
-            size_t lists = 0, cands = 0;
-            for (const kba_track* t : g->tracks) { lists += (size_t)t->td.kf_cap + t->td.lm_cap; cands += (size_t)t->td.lm_cap; }
-            std::unique_ptr<SelectStage> st(new SelectStage());
-            if (st->alloc(sizeof(SelectArgs) * (size_t)(n - 1) + 4 * lists, select_out_bytes(cands, (size_t)n)))
-                return fail(KBA_ERR_CUDA, who + "out of memory for the selection staging");
-            g->select = std::move(st);
-        }
-        rc = select_run(g->h, *g->select, (int)rs.size(), rs.data());
-        if (rc != KBA_OK) return rc;
-        g->last = &g->select->counts;
-    }
-    for (int i = 0; i < n; ++i)
-        if (req[i].n_kf == 0) *out[i].n_near = 0;
-    return rc;
+    return store_call<Select>(g->set, true, who, req, out);
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
@@ -2224,18 +2268,18 @@ static int create_alloc(kba_track* t, std::string& why) {
     CreateArgs& a = cb->a;
     double* intr = nullptr, *pose = nullptr;
     int bad = 0;
-    bad |= cb->alloc(&a.req_of, L); bad |= cb->alloc(&a.ray_T, 12 * K * NC); bad |= cb->alloc(&a.intr_inv, 9 * NC);
-    bad |= cb->alloc(&a.cnt, L); bad |= cb->alloc(&a.cursor, L); bad |= cb->alloc(&a.off, L); bad |= cb->alloc(&a.key, (size_t)td.m_cap);
-    bad |= cb->alloc(&a.total, 1); bad |= cb->alloc(&intr, 3 * NC); bad |= cb->alloc(&pose, 7 * NC);
+    DevAllocs& dev = cb->dev;
+    bad |= dev.alloc(&a.req_of, L); bad |= dev.alloc(&a.ray_T, 12 * K * NC); bad |= dev.alloc(&a.intr_inv, 9 * NC);
+    bad |= dev.alloc(&a.cnt, L); bad |= dev.alloc(&a.cursor, L); bad |= dev.alloc(&a.off, L); bad |= dev.alloc(&a.key, (size_t)td.m_cap);
+    bad |= dev.alloc(&a.total, 1); bad |= dev.alloc(&intr, 3 * NC); bad |= dev.alloc(&pose, 7 * NC);
     if (bad) { why = "out of memory for the creation buffers"; return KBA_ERR_CUDA; }
-    cudaStream_t s = t->h->stream;
+    cudaStream_t s = t->set.h->stream;
     cudaError_t e = cudaMemsetAsync(a.req_of, 0xff, sizeof(int) * L, s);
     if (e == cudaSuccess) e = cudaMemcpyAsync(intr, t->cam_intr.data(), sizeof(double) * 3 * NC, cudaMemcpyHostToDevice, s);
     if (e == cudaSuccess) e = cudaMemcpyAsync(pose, t->cam_pose.data(), sizeof(double) * 7 * NC, cudaMemcpyHostToDevice, s);
     if (e == cudaSuccess) e = cudaStreamSynchronize(s);
     if (e != cudaSuccess) { why = std::string("creation buffers: ") + cudaGetErrorString(e); return KBA_ERR_CUDA; }
     a.cam_intr = intr; a.cam_pose7 = pose; a.n_cam = t->n_cam;
-    cb->kf_stamp.assign(K, 0); cb->lm_stamp.assign(L, 0);
     t->create = std::move(cb);
     return KBA_OK;
 }
@@ -2244,7 +2288,7 @@ static int create_alloc(kba_track* t, std::string& why) {
 struct CreateReq {
     kba_track* t = nullptr;
     const kba_create_request* q = nullptr;
-    const kba_create_out* o = nullptr;
+    kba_create_out* o = nullptr;
     int max_meas = 0;                      // set by create_check: arena entries of the largest listed keyframe
 };
 
@@ -2256,34 +2300,16 @@ static int create_check(CreateReq& r, std::string& why) {
     if (q.n_kf < 1 || q.n_new < 0) { why = "no keyframes or a negative size"; return KBA_ERR_BAD_ARG; }
     if (q.n_kf > t->td.kf_cap || q.n_new > t->td.lm_cap) { why = "more keyframes or landmarks than the track's slots"; return KBA_ERR_CAPACITY; }
     if (q.kf_new < 0 || q.kf_new >= q.n_kf) { why = "kf_new outside [0, n_kf)"; return KBA_ERR_BAD_ARG; }
-    const cudaError_t e = cudaSetDevice(t->h->device);
+    const cudaError_t e = cudaSetDevice(t->set.h->device);
     if (e != cudaSuccess) { why = std::string("cudaSetDevice: ") + cudaGetErrorString(e); return KBA_ERR_CUDA; }
     if (!t->create) { const int rc = create_alloc(t, why); if (rc != KBA_OK) return rc; }
-    CreateBufs& cb = *t->create;
-    if (++cb.stamp == 0) {  // the stamps wrapped: start over
-        std::fill(cb.kf_stamp.begin(), cb.kf_stamp.end(), 0u); std::fill(cb.lm_stamp.begin(), cb.lm_stamp.end(), 0u); cb.stamp = 1;
-    }
-    r.max_meas = 0;
-    for (int k = 0; k < q.n_kf; ++k) {
-        const int s = q.kf_slot[k];
-        if (s < 0 || s >= t->td.kf_cap || !t->kf_live[s]) { why = "keyframe slot not pushed"; return KBA_ERR_BAD_ARG; }
-        if (cb.kf_stamp[s] == cb.stamp) { why = "keyframe slot listed twice"; return KBA_ERR_BAD_ARG; }
-        cb.kf_stamp[s] = cb.stamp;
-        r.max_meas = std::max(r.max_meas, t->m_cnt[s]);
-    }
-    for (int c = 0; c < q.n_new; ++c) {
-        const int s = q.lm_slot[c];
-        if (s < 0 || s >= t->td.lm_cap) { why = "landmark slot out of range"; return KBA_ERR_BAD_ARG; }
-        if (cb.lm_stamp[s] == cb.stamp) { why = "landmark slot listed twice"; return KBA_ERR_BAD_ARG; }
-        cb.lm_stamp[s] = cb.stamp;
-    }
-    return KBA_OK;
+    return check_slot_lists(t, q.n_kf, q.kf_slot, q.n_new, q.lm_slot, r.max_meas, why);
 }
 
 // W checked requests of distinct tracks as the W windows of one launch sequence: one upload (the argument records of windows
 // 1 .. W-1, then every window's lists), one download (positions of all windows | their flags), one synchronisation, then the
 // scatter into the callers' arrays.  Window 0's record travels in the launch parameters (kba_create.cu).
-static int create_run(kba_handle* h, SelectStage& st, int W, const CreateReq* r) {
+static int create_run(kba_handle* h, StoreStage& st, int W, const CreateReq* r) {
     CU(cudaSetDevice(h->device));
     for (int w = 0; w < W; ++w) r[w].t->gen++;
     cudaStream_t s = h->stream;
@@ -2343,59 +2369,40 @@ static int create_run(kba_handle* h, SelectStage& st, int W, const CreateReq* r)
     return KBA_OK;
 }
 
+struct Create {
+    using Request = kba_create_request;
+    using Out = kba_create_out;
+    using Req = CreateReq;
+    static constexpr StoreCall slot = kCreateCall;
+    static constexpr const char* staging = "creation";
+    static bool sits_out(const Request& q) { return q.n_kf == 0; }
+    static int sit_out_check(const Out&, std::string&) { return KBA_OK; }
+    static void sat_out(Out*, bool) {}
+    static Req make(kba_track* t, const Request& q, Out* o) {
+        Req r;
+        r.t = t; r.q = &q; r.o = o;
+        return r;
+    }
+    static int check(Req& r, std::string& why) { return create_check(r, why); }
+    static void capacity(int n, kba_track* const* ts, size_t& up, size_t& down) {
+        size_t lists = 0, lms = 0;
+        for (int i = 0; i < n; ++i) { lists += (size_t)ts[i]->td.kf_cap + ts[i]->td.lm_cap; lms += (size_t)ts[i]->td.lm_cap; }
+        up = sizeof(CreateArgs) * (size_t)(n - 1) + 4 * lists;
+        down = 25 * lms;
+    }
+    static int run(kba_handle* h, StoreStage& st, int W, Req* r, int&, std::string&) { return create_run(h, st, W, r); }
+};
+
 int kba_track_create_landmarks(kba_track* t, const kba_create_request* req, kba_create_out* out) {
     static const std::string who = "kba_track_create_landmarks: ";
     if (!t || !req || !out) return fail(KBA_ERR_BAD_ARG, who + "null argument");
-    CreateReq r;
-    r.t = t; r.q = req; r.o = out;
-    std::string why;
-    int rc = create_check(r, why);
-    if (rc != KBA_OK) return fail(rc, who + why);
-    SelectStage& st = t->create->stage;
-    if (!st.up.d) {  // the first single call of the track
-        const size_t K = (size_t)t->td.kf_cap, L = (size_t)t->td.lm_cap;
-        if (st.alloc(4 * (K + L), 25 * L)) {
-            st.up.release(); st.out.release();
-            return fail(KBA_ERR_CUDA, who + "out of memory for the creation staging");
-        }
-    }
-    rc = create_run(t->h, st, 1, &r);
-    if (rc == KBA_OK) t->last = &t->create->stage.counts;
-    return rc;
+    return store_call<Create>(t->set, false, who, req, out);
 }
 
 int kba_track_group_create_landmarks(kba_track_group* g, const kba_create_request* req, kba_create_out* out) {
     static const std::string who = "kba_track_group_create_landmarks: ";
     if (!g || !req || !out) return fail(KBA_ERR_BAD_ARG, who + "null argument");
-    const int n = (int)g->tracks.size();
-    // ---- every request is checked before anything is uploaded or written
-    std::vector<CreateReq> rs;
-    for (int i = 0; i < n; ++i) {
-        if (req[i].n_kf == 0) continue;  // sits the call out
-        CreateReq r;
-        r.t = g->tracks[i]; r.q = &req[i]; r.o = &out[i];
-        std::string why;
-        const int rc = create_check(r, why);
-        if (rc != KBA_OK) return fail(rc, who + "track " + std::to_string(i) + ": " + why);
-        rs.push_back(r);
-    }
-    if (rs.empty()) {  // every track sits out: no upload, no launch
-        g->solver.h2d = 0; g->solver.d2h = 0;
-        g->last = &g->solver;
-        return KBA_OK;
-    }
-    if (!g->create) {  // staging for every track at its capacities, allocated once
-        size_t lists = 0, lms = 0;
-        for (const kba_track* t : g->tracks) { lists += (size_t)t->td.kf_cap + t->td.lm_cap; lms += (size_t)t->td.lm_cap; }
-        std::unique_ptr<SelectStage> st(new SelectStage());
-        if (st->alloc(sizeof(CreateArgs) * (size_t)(n - 1) + 4 * lists, 25 * lms))
-            return fail(KBA_ERR_CUDA, who + "out of memory for the creation staging");
-        g->create = std::move(st);
-    }
-    const int rc = create_run(g->h, *g->create, (int)rs.size(), rs.data());
-    if (rc != KBA_OK) return rc;
-    g->last = &g->create->counts;
-    return KBA_OK;
+    return store_call<Create>(g->set, true, who, req, out);
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
@@ -2414,32 +2421,24 @@ struct UpkeepReq {
     int n_kf = 0, n_lm = 0;
     const int32_t* kf_slot = nullptr, *lm_slot = nullptr;
     const kba_deactivate_request* dq = nullptr;  // deactivation
-    const kba_deactivate_out* dout = nullptr;
-    const kba_depth_out* cout = nullptr;          // depth costs
+    kba_deactivate_out* dout = nullptr;
+    kba_depth_out* cout = nullptr;                // depth costs
     int cap = 0;
     int bound = 0, max_meas = 0;                  // set by upkeep_check: the depth costs' B, arena entries of the largest keyframe
 };
 
-// the track's upkeep scratch (slot map, duplicate-check stamps), allocated at its first upkeep or flow call, and a fresh check stamp
+// the track's upkeep scratch (the slot map), allocated at its first upkeep, flow or reclaim call
 static int upkeep_bufs(kba_track* t, std::string& why) {
-    const cudaError_t e = cudaSetDevice(t->h->device);
+    const cudaError_t e = cudaSetDevice(t->set.h->device);
     if (e != cudaSuccess) { why = std::string("cudaSetDevice: ") + cudaGetErrorString(e); return KBA_ERR_CUDA; }
     if (!t->upkeep) {
         std::unique_ptr<UpkeepBufs> ub(new UpkeepBufs());
         const size_t L = (size_t)t->td.lm_cap, C = (L + kReclaimChunk - 1) / kReclaimChunk;
-        if (cudaMalloc(&ub->map, sizeof(unsigned long long) * std::max<size_t>(L, 1)) != cudaSuccess ||
-            cudaMalloc(&ub->blk, sizeof(int) * std::max<size_t>(C, 1)) != cudaSuccess) {
-            why = "out of memory for the upkeep buffers"; return KBA_ERR_CUDA;
-        }
-        cudaError_t me = cudaMemsetAsync(ub->map, 0, sizeof(unsigned long long) * L, t->h->stream);
-        if (me == cudaSuccess) me = cudaStreamSynchronize(t->h->stream);
+        if (ub->dev.alloc(&ub->map, L) | ub->dev.alloc(&ub->blk, C)) { why = "out of memory for the upkeep buffers"; return KBA_ERR_CUDA; }
+        cudaError_t me = cudaMemsetAsync(ub->map, 0, sizeof(unsigned long long) * L, t->set.h->stream);
+        if (me == cudaSuccess) me = cudaStreamSynchronize(t->set.h->stream);
         if (me != cudaSuccess) { why = std::string("upkeep buffers: ") + cudaGetErrorString(me); return KBA_ERR_CUDA; }
-        ub->kf_stamp.assign((size_t)t->td.kf_cap, 0); ub->lm_stamp.assign(L, 0);
         t->upkeep = std::move(ub);
-    }
-    UpkeepBufs& ub = *t->upkeep;
-    if (++ub.check == 0) {  // the check stamps wrapped: start over
-        std::fill(ub.kf_stamp.begin(), ub.kf_stamp.end(), 0u); std::fill(ub.lm_stamp.begin(), ub.lm_stamp.end(), 0u); ub.check = 1;
     }
     return KBA_OK;
 }
@@ -2455,25 +2454,11 @@ static int upkeep_check(UpkeepReq& r, std::string& why) {
     }
     if (r.n_kf < 1 || r.n_lm < 0 || r.cap < 0) { why = "no keyframes or a negative size"; return KBA_ERR_BAD_ARG; }
     if (r.n_kf > t->td.kf_cap || r.n_lm > t->td.lm_cap) { why = "more keyframes or landmarks than the track's slots"; return KBA_ERR_CAPACITY; }
-    const int rb = upkeep_bufs(t, why);
-    if (rb != KBA_OK) return rb;
-    UpkeepBufs& ub = *t->upkeep;
-    r.max_meas = 0;
+    int rc = upkeep_bufs(t, why);
+    if (rc == KBA_OK) rc = check_slot_lists(t, r.n_kf, r.kf_slot, r.n_lm, r.lm_slot, r.max_meas, why);
+    if (rc != KBA_OK) return rc;
     int64_t bound = 0;
-    for (int k = 0; k < r.n_kf; ++k) {
-        const int s = r.kf_slot[k];
-        if (s < 0 || s >= t->td.kf_cap || !t->kf_live[s]) { why = "keyframe slot not pushed"; return KBA_ERR_BAD_ARG; }
-        if (ub.kf_stamp[s] == ub.check) { why = "keyframe slot listed twice"; return KBA_ERR_BAD_ARG; }
-        ub.kf_stamp[s] = ub.check;
-        r.max_meas = std::max(r.max_meas, t->m_cnt[s]);
-        bound += std::min(r.n_lm, t->m_cnt[s]);
-    }
-    for (int j = 0; j < r.n_lm; ++j) {
-        const int s = r.lm_slot[j];
-        if (s < 0 || s >= t->td.lm_cap) { why = "landmark slot out of range"; return KBA_ERR_BAD_ARG; }
-        if (ub.lm_stamp[s] == ub.check) { why = "landmark slot listed twice"; return KBA_ERR_BAD_ARG; }
-        ub.lm_stamp[s] = ub.check;
-    }
+    for (int k = 0; k < r.n_kf; ++k) bound += std::min(r.n_lm, t->m_cnt[r.kf_slot[k]]);
     r.bound = (int)bound;  // <= the arena entries of distinct keyframes <= m_cap
     if (depth && r.cap < r.bound) { why = "cap below the sum over keyframes of min(n_elig, arena entries)"; return KBA_ERR_CAPACITY; }
     return KBA_OK;
@@ -2483,7 +2468,7 @@ static int upkeep_check(UpkeepReq& r, std::string& why) {
 // records of windows 1 .. W-1, then every window's lists), one download, one synchronisation, then the scatter into the callers'
 // arrays.  Downloads: deactivation kf_common of all windows | kf_active | lm_active; depth costs cost | cnt | cand, each window's
 // pairs at its keyframes' bounds.  Window 0's record travels in the launch parameters (kba_upkeep.cu).
-static int upkeep_run(kba_handle* h, SelectStage& st, int W, const UpkeepReq* r, bool depth) {
+static int upkeep_run(kba_handle* h, StoreStage& st, int W, const UpkeepReq* r, bool depth) {
     CU(cudaSetDevice(h->device));
     cudaStream_t s = h->stream;
     UpkeepGrid g;
@@ -2575,98 +2560,79 @@ static int upkeep_run(kba_handle* h, SelectStage& st, int W, const UpkeepReq* r,
     return KBA_OK;
 }
 
-static int upkeep_single(kba_track* t, UpkeepReq& r, bool depth, const std::string& who) {
-    std::string why;
-    int rc = upkeep_check(r, why);
-    if (rc != KBA_OK) return fail(rc, who + why);
-    SelectStage& st = t->upkeep->stage;
-    if (!st.up.d) {  // the first single call of the track
-        const size_t K = (size_t)t->td.kf_cap, L = (size_t)t->td.lm_cap;
-        if (st.alloc(4 * (K + L), upkeep_out_cap(t))) {
-            st.up.release(); st.out.release();
-            return fail(KBA_ERR_CUDA, who + "out of memory for the upkeep staging");
-        }
-    }
-    rc = upkeep_run(t->h, st, 1, &r, depth);
-    if (rc == KBA_OK) t->last = &t->upkeep->stage.counts;
-    return rc;
-}
-
-// every request of a group checked, then one upkeep_run over those that do not sit out
-static int upkeep_group(kba_track_group* g, std::vector<UpkeepReq>& all, bool depth, const std::string& who) {
-    const int n = (int)g->tracks.size();
-    std::vector<UpkeepReq> rs;
-    for (int i = 0; i < n; ++i) {
-        if (all[i].n_kf == 0) continue;  // sits the call out
-        std::string why;
-        const int rc = upkeep_check(all[i], why);
-        if (rc != KBA_OK) return fail(rc, who + "track " + std::to_string(i) + ": " + why);
-        rs.push_back(all[i]);
-    }
-    if (rs.empty()) {  // every track sits out: no upload, no launch
-        g->solver.h2d = 0; g->solver.d2h = 0;
-        g->last = &g->solver;
-        return KBA_OK;
-    }
-    if (!g->upkeep) {  // staging for every track at its capacities, allocated once
-        size_t lists = 0, outs = 0;
-        for (const kba_track* t : g->tracks) { lists += (size_t)t->td.kf_cap + t->td.lm_cap; outs += upkeep_out_cap(t); }
-        std::unique_ptr<SelectStage> st(new SelectStage());
-        if (st->alloc(sizeof(UpkeepArgs) * (size_t)(n - 1) + 4 * lists, outs)) return fail(KBA_ERR_CUDA, who + "out of memory for the upkeep staging");
-        g->upkeep = std::move(st);
-    }
-    const int rc = upkeep_run(g->h, *g->upkeep, (int)rs.size(), rs.data(), depth);
-    if (rc != KBA_OK) return rc;
-    g->last = &g->upkeep->counts;
-    return KBA_OK;
-}
-
-static UpkeepReq deactivate_req(kba_track* t, const kba_deactivate_request* q, const kba_deactivate_out* o) {
+extern "C++" {  // overloads and templates have C++ linkage
+static UpkeepReq upkeep_req(kba_track* t, const kba_deactivate_request& q, kba_deactivate_out* o) {
     UpkeepReq r;
-    r.t = t; r.n_kf = q->n_kf; r.n_lm = q->n_lm; r.kf_slot = q->kf_slot; r.lm_slot = q->lm_slot; r.dq = q; r.dout = o;
+    r.t = t; r.n_kf = q.n_kf; r.n_lm = q.n_lm; r.kf_slot = q.kf_slot; r.lm_slot = q.lm_slot; r.dq = &q; r.dout = o;
     return r;
 }
 
-static UpkeepReq depth_req(kba_track* t, const kba_depth_request* q, const kba_depth_out* o) {
+static UpkeepReq upkeep_req(kba_track* t, const kba_depth_request& q, kba_depth_out* o) {
     UpkeepReq r;
-    r.t = t; r.n_kf = q->n_kf; r.n_lm = q->n_elig; r.kf_slot = q->kf_slot; r.lm_slot = q->lm_slot; r.cout = o; r.cap = q->cap;
+    r.t = t; r.n_kf = q.n_kf; r.n_lm = q.n_elig; r.kf_slot = q.kf_slot; r.lm_slot = q.lm_slot; r.cout = o; r.cap = q.cap;
     return r;
 }
+
+// deactivation (Depth = false) and depth costs (Depth = true): one staging, one check, one run
+template <class Q, class O, bool Depth>
+struct Upkeep {
+    using Request = Q;
+    using Out = O;
+    using Req = UpkeepReq;
+    static constexpr StoreCall slot = kUpkeepCall;
+    static constexpr const char* staging = "upkeep";
+    static bool sits_out(const Request& q) { return q.n_kf == 0; }
+    static int sit_out_check(const Out&, std::string&) { return KBA_OK; }
+    static void sat_out(Out*, bool) {}
+    static Req make(kba_track* t, const Request& q, Out* o) { return upkeep_req(t, q, o); }
+    static int check(Req& r, std::string& why) { return upkeep_check(r, why); }
+    static void capacity(int n, kba_track* const* ts, size_t& up, size_t& down) {
+        size_t lists = 0;
+        down = 0;
+        for (int i = 0; i < n; ++i) { lists += (size_t)ts[i]->td.kf_cap + ts[i]->td.lm_cap; down += upkeep_out_cap(ts[i]); }
+        up = sizeof(UpkeepArgs) * (size_t)(n - 1) + 4 * lists;
+    }
+    static int run(kba_handle* h, StoreStage& st, int W, Req* r, int&, std::string&) { return upkeep_run(h, st, W, r, Depth); }
+};
+}  // extern "C++"
+using Deactivate = Upkeep<kba_deactivate_request, kba_deactivate_out, false>;
+using DepthCosts = Upkeep<kba_depth_request, kba_depth_out, true>;
 
 int kba_track_deactivate_keyframes(kba_track* t, const kba_deactivate_request* req, kba_deactivate_out* out) {
     static const std::string who = "kba_track_deactivate_keyframes: ";
     if (!t || !req || !out) return fail(KBA_ERR_BAD_ARG, who + "null argument");
-    UpkeepReq r = deactivate_req(t, req, out);
-    return upkeep_single(t, r, false, who);
+    return store_call<Deactivate>(t->set, false, who, req, out);
 }
 
 int kba_track_depth_costs(kba_track* t, const kba_depth_request* req, kba_depth_out* out) {
     static const std::string who = "kba_track_depth_costs: ";
     if (!t || !req || !out) return fail(KBA_ERR_BAD_ARG, who + "null argument");
-    UpkeepReq r = depth_req(t, req, out);
-    return upkeep_single(t, r, true, who);
+    return store_call<DepthCosts>(t->set, false, who, req, out);
 }
 
 int kba_track_group_deactivate_keyframes(kba_track_group* g, const kba_deactivate_request* req, kba_deactivate_out* out) {
     static const std::string who = "kba_track_group_deactivate_keyframes: ";
     if (!g || !req || !out) return fail(KBA_ERR_BAD_ARG, who + "null argument");
-    std::vector<UpkeepReq> all;
-    for (size_t i = 0; i < g->tracks.size(); ++i) all.push_back(deactivate_req(g->tracks[i], &req[i], &out[i]));
-    return upkeep_group(g, all, false, who);
+    return store_call<Deactivate>(g->set, true, who, req, out);
 }
 
 int kba_track_group_depth_costs(kba_track_group* g, const kba_depth_request* req, kba_depth_out* out) {
     static const std::string who = "kba_track_group_depth_costs: ";
     if (!g || !req || !out) return fail(KBA_ERR_BAD_ARG, who + "null argument");
-    std::vector<UpkeepReq> all;
-    for (size_t i = 0; i < g->tracks.size(); ++i) all.push_back(depth_req(g->tracks[i], &req[i], &out[i]));
-    return upkeep_group(g, all, true, who);
+    return store_call<DepthCosts>(g->set, true, who, req, out);
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
 // the flow scheme of keyframe selection on the stored window (include/kba_b200.h, kba_track_frame_flow /
 // kba_track_group_frame_flow; kernels in kba_keyframe.cu): a single call is a one-window call of flow_run
 // ---------------------------------------------------------------------------------------------------------------------
+// one frame-flow request of track t (one window of flow_run)
+struct FlowReq {
+    kba_track* t = nullptr;
+    const kba_flow_request* q = nullptr;
+    kba_flow_out* o = nullptr;
+};
+
 // every check of one request, before anything is uploaded; allocates the track's upkeep scratch at its first upkeep or flow call
 static int flow_check(kba_track* t, const kba_flow_request* q, std::string& why) {
     const int n = q->n_meas;
@@ -2676,7 +2642,8 @@ static int flow_check(kba_track* t, const kba_flow_request* q, std::string& why)
     if (n > t->caps.win_observations) { why = "more measurements than win_observations"; return KBA_ERR_CAPACITY; }
     const int rb = upkeep_bufs(t, why);
     if (rb != KBA_OK) return rb;
-    UpkeepBufs& ub = *t->upkeep;
+    SlotStamps& st = t->stamps;
+    st.next();
     for (int i = 0; i < n; ++i) {
         const int s = q->lm_slot[i], c = q->cam ? q->cam[i] : 0;
         if (s < 0 || s >= t->td.lm_cap) { why = "landmark slot out of range"; return KBA_ERR_BAD_ARG; }
@@ -2685,8 +2652,8 @@ static int flow_check(kba_track* t, const kba_flow_request* q, std::string& why)
             if (c <= (q->cam ? q->cam[i - 1] : 0)) { why = "camera not ascending inside a run"; return KBA_ERR_BAD_ARG; }
             continue;
         }
-        if (ub.lm_stamp[s] == ub.check) { why = "landmark slot reappears after its run"; return KBA_ERR_BAD_ARG; }
-        ub.lm_stamp[s] = ub.check;
+        if (st.lm[s] == st.cur) { why = "landmark slot reappears after its run"; return KBA_ERR_BAD_ARG; }
+        st.lm[s] = st.cur;
     }
     return KBA_OK;
 }
@@ -2694,15 +2661,14 @@ static int flow_check(kba_track* t, const kba_flow_request* q, std::string& why)
 // W checked requests of distinct tracks as the W windows of one launch sequence: one upload (the argument records of windows
 // 1 .. W-1, then every window's lm | cam | u | v), one download (the FlowRes records of all windows, then their match indices),
 // one synchronisation, then the scatter into the callers' outputs.  Window 0's record travels in the launch parameters.
-static int flow_run(kba_handle* h, SelectStage& st, int W, kba_track* const* ts, const kba_flow_request* const* qs,
-                    kba_flow_out* const* os) {
+static int flow_run(kba_handle* h, StoreStage& st, int W, const FlowReq* r) {
     CU(cudaSetDevice(h->device));
     cudaStream_t s = h->stream;
     FlowGrid g;
     size_t SN = 0;
     for (int w = 0; w < W; ++w) {
-        SN += (size_t)qs[w]->n_meas;
-        g.max_last = std::max(g.max_last, ts[w]->m_cnt[qs[w]->kf_last]);
+        SN += (size_t)r[w].q->n_meas;
+        g.max_last = std::max(g.max_last, r[w].t->m_cnt[r[w].q->kf_last]);
     }
     const size_t o_lists = sizeof(FlowArgs) * (size_t)(W - 1), up_bytes = o_lists + 16 * SN;
     const size_t o_match = sizeof(FlowRes) * (size_t)W, out_bytes = o_match + 4 * SN;
@@ -2713,11 +2679,11 @@ static int flow_run(kba_handle* h, SelectStage& st, int W, kba_track* const* ts,
     l.n_win = W;
     size_t li = 0, mi = 0;
     for (int w = 0; w < W; ++w) {
-        const kba_flow_request& q = *qs[w];
+        const kba_flow_request& q = *r[w].q;
         const size_t n = (size_t)q.n_meas;
-        UpkeepBufs& ub = *ts[w]->upkeep;
+        UpkeepBufs& ub = *r[w].t->upkeep;
         if (ub.stamp >= 0xfffffff0u) {  // the stamps wrap: the map starts over from all 0
-            CU(cudaMemsetAsync(ub.map, 0, sizeof(unsigned long long) * (size_t)ts[w]->td.lm_cap, s));
+            CU(cudaMemsetAsync(ub.map, 0, sizeof(unsigned long long) * (size_t)r[w].t->td.lm_cap, s));
             ub.stamp = 0;
         }
         int32_t* lm = reinterpret_cast<int32_t*>(up_h + li);
@@ -2730,7 +2696,7 @@ static int flow_run(kba_handle* h, SelectStage& st, int W, kba_track* const* ts,
             memcpy(cam + 2 * n, q.v, 4 * n);
         }
         FlowArgs a;
-        a.td = ts[w]->td;
+        a.td = r[w].t->td;
         a.kf_last = q.kf_last; a.n_meas = q.n_meas;
         a.lm_slot = reinterpret_cast<const int*>(up_d + li); a.cam = a.lm_slot + n;
         a.u = reinterpret_cast<const float*>(a.cam + n); a.v = a.u + n;
@@ -2750,7 +2716,7 @@ static int flow_run(kba_handle* h, SelectStage& st, int W, kba_track* const* ts,
     if (e == cudaSuccess) e = wait_stream(h);
     if (e != cudaSuccess) {
         // as upkeep_run: the maps go back to all 0, whatever stamps the failed sequence left in them
-        for (int w = 0; w < W; ++w) cudaMemsetAsync(ts[w]->upkeep->map, 0, sizeof(unsigned long long) * (size_t)ts[w]->td.lm_cap, s);
+        for (int w = 0; w < W; ++w) cudaMemsetAsync(r[w].t->upkeep->map, 0, sizeof(unsigned long long) * (size_t)r[w].t->td.lm_cap, s);
         cudaStreamSynchronize(s);
         return fail(KBA_ERR_CUDA, std::string("frame flow: ") + cudaGetErrorString(e));
     }
@@ -2758,8 +2724,8 @@ static int flow_run(kba_handle* h, SelectStage& st, int W, kba_track* const* ts,
     const int32_t* match = reinterpret_cast<const int32_t*>(st.out.h + o_match);
     mi = 0;
     for (int w = 0; w < W; ++w) {
-        kba_flow_out& o = *os[w];
-        const size_t n = (size_t)qs[w]->n_meas;
+        kba_flow_out& o = *r[w].o;
+        const size_t n = (size_t)r[w].q->n_meas;
         o.n_matched = res[w].n_matched;
         o.usable = (uint8_t)res[w].usable;
         o.flow_sum = res[w].flow_sum;
@@ -2779,56 +2745,40 @@ static int flow_run(kba_handle* h, SelectStage& st, int W, kba_track* const* ts,
     return KBA_OK;
 }
 
+struct Flow {
+    using Request = kba_flow_request;
+    using Out = kba_flow_out;
+    using Req = FlowReq;
+    static constexpr StoreCall slot = kFlowCall;
+    static constexpr const char* staging = "flow";
+    static bool sits_out(const Request& q) { return q.kf_last < 0; }
+    static int sit_out_check(const Out&, std::string&) { return KBA_OK; }
+    static void sat_out(Out*, bool) {}
+    static Req make(kba_track* t, const Request& q, Out* o) {
+        Req r;
+        r.t = t; r.q = &q; r.o = o;
+        return r;
+    }
+    static int check(Req& r, std::string& why) { return flow_check(r.t, r.q, why); }
+    static void capacity(int n, kba_track* const* ts, size_t& up, size_t& down) {  // win_observations measurements per track
+        size_t obs = 0;
+        for (int i = 0; i < n; ++i) obs += (size_t)ts[i]->caps.win_observations;
+        up = sizeof(FlowArgs) * (size_t)(n - 1) + 16 * obs;
+        down = sizeof(FlowRes) * (size_t)n + 4 * obs;
+    }
+    static int run(kba_handle* h, StoreStage& st, int W, Req* r, int&, std::string&) { return flow_run(h, st, W, r); }
+};
+
 int kba_track_frame_flow(kba_track* t, const kba_flow_request* req, kba_flow_out* out) {
     static const std::string who = "kba_track_frame_flow: ";
     if (!t || !req || !out) return fail(KBA_ERR_BAD_ARG, who + "null argument");
-    std::string why;
-    int rc = flow_check(t, req, why);
-    if (rc != KBA_OK) return fail(rc, who + why);
-    SelectStage& st = t->upkeep->flow;
-    if (!st.up.d) {  // the first single call of the track: staging for win_observations measurements
-        const size_t O = (size_t)t->caps.win_observations;
-        if (st.alloc(16 * O, sizeof(FlowRes) + 4 * O)) {
-            st.up.release(); st.out.release();
-            return fail(KBA_ERR_CUDA, who + "out of memory for the flow staging");
-        }
-    }
-    rc = flow_run(t->h, st, 1, &t, &req, &out);
-    if (rc == KBA_OK) t->last = &st.counts;
-    return rc;
+    return store_call<Flow>(t->set, false, who, req, out);
 }
 
 int kba_track_group_frame_flow(kba_track_group* g, const kba_flow_request* req, kba_flow_out* out) {
     static const std::string who = "kba_track_group_frame_flow: ";
     if (!g || !req || !out) return fail(KBA_ERR_BAD_ARG, who + "null argument");
-    const int n = (int)g->tracks.size();
-    std::vector<kba_track*> ts;
-    std::vector<const kba_flow_request*> qs;
-    std::vector<kba_flow_out*> os;
-    for (int i = 0; i < n; ++i) {
-        if (req[i].kf_last < 0) continue;  // sits the call out
-        std::string why;
-        const int rc = flow_check(g->tracks[i], &req[i], why);
-        if (rc != KBA_OK) return fail(rc, who + "track " + std::to_string(i) + ": " + why);
-        ts.push_back(g->tracks[i]); qs.push_back(&req[i]); os.push_back(&out[i]);
-    }
-    if (ts.empty()) {  // every track sits out: no upload, no launch
-        g->solver.h2d = 0; g->solver.d2h = 0;
-        g->last = &g->solver;
-        return KBA_OK;
-    }
-    if (!g->flow) {  // staging for every track at its win_observations, allocated once
-        size_t obs = 0;
-        for (const kba_track* t : g->tracks) obs += (size_t)t->caps.win_observations;
-        std::unique_ptr<SelectStage> st(new SelectStage());
-        if (st->alloc(sizeof(FlowArgs) * (size_t)(n - 1) + 16 * obs, sizeof(FlowRes) * (size_t)n + 4 * obs))
-            return fail(KBA_ERR_CUDA, who + "out of memory for the flow staging");
-        g->flow = std::move(st);
-    }
-    const int rc = flow_run(g->h, *g->flow, (int)ts.size(), ts.data(), qs.data(), os.data());
-    if (rc != KBA_OK) return rc;
-    g->last = &g->flow->counts;
-    return KBA_OK;
+    return store_call<Flow>(g->set, true, who, req, out);
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
@@ -2837,6 +2787,13 @@ int kba_track_group_frame_flow(kba_track_group* g, const kba_flow_request* req, 
 // ---------------------------------------------------------------------------------------------------------------------
 // the largest download of one window of track t: positions, weights and slots of a range of lm_cap slots, and n_free
 static size_t reclaim_out_cap(const kba_track* t) { return 36 * (size_t)t->td.lm_cap + 4; }
+
+// one reclaim request of track t (one window of reclaim_run)
+struct ReclaimReq {
+    kba_track* t = nullptr;
+    const kba_reclaim_request* q = nullptr;
+    kba_reclaim_out* o = nullptr;
+};
 
 // every check of one request, before anything is uploaded; allocates the track's upkeep scratch at its first upkeep, flow or
 // reclaim call
@@ -2850,17 +2807,16 @@ static int reclaim_check(kba_track* t, const kba_reclaim_request* q, const kba_r
 // argument records of windows 1 .. W-1, then every window's live keyframe slots), one download (the positions of the windows that
 // ask for them | their weights | every window's slots | n_free of every window, each window's part sized for its whole range),
 // one synchronisation, then the scatter into the callers' outputs.  Window 0's record travels in the launch parameters.
-static int reclaim_run(kba_handle* h, SelectStage& st, int W, kba_track* const* ts, const kba_reclaim_request* const* qs,
-                       kba_reclaim_out* const* os) {
+static int reclaim_run(kba_handle* h, StoreStage& st, int W, const ReclaimReq* r) {
     CU(cudaSetDevice(h->device));
-    for (int w = 0; w < W; ++w) ts[w]->gen++;
+    for (int w = 0; w < W; ++w) r[w].t->gen++;
     cudaStream_t s = h->stream;
     ReclaimGrid g;
     size_t SP = 0, SW = 0, SN = 0;
     for (int w = 0; w < W; ++w) {
-        const size_t n = (size_t)(qs[w]->hi - qs[w]->lo);
-        SN += n; SP += os[w]->pos ? n : 0; SW += os[w]->weight ? n : 0;
-        g.max_range = std::max(g.max_range, qs[w]->hi - qs[w]->lo);
+        const size_t n = (size_t)(r[w].q->hi - r[w].q->lo);
+        SN += n; SP += r[w].o->pos ? n : 0; SW += r[w].o->weight ? n : 0;
+        g.max_range = std::max(g.max_range, r[w].q->hi - r[w].q->lo);
     }
     const size_t o_lists = sizeof(ReclaimArgs) * (size_t)(W - 1);
     const size_t o_w = 24 * SP, o_s = o_w + 8 * SW, o_n = o_s + 4 * SN, out_bytes = o_n + 4 * (size_t)W;
@@ -2872,7 +2828,7 @@ static int reclaim_run(kba_handle* h, SelectStage& st, int W, kba_track* const* 
     l.n_win = W;
     size_t li = 0, cP = 0, cW = 0, cN = 0;
     for (int w = 0; w < W; ++w) {
-        kba_track* t = ts[w];
+        kba_track* t = r[w].t;
         UpkeepBufs& ub = *t->upkeep;
         if (ub.stamp >= 0xfffffff0u) {  // the stamps wrap: the map starts over from all 0
             CU(cudaMemsetAsync(ub.map, 0, sizeof(unsigned long long) * (size_t)t->td.lm_cap, s));
@@ -2887,14 +2843,14 @@ static int reclaim_run(kba_handle* h, SelectStage& st, int W, kba_track* const* 
             g.max_meas = std::max(g.max_meas, t->m_cnt[k]);
         }
         g.max_live = std::max(g.max_live, a.n_live);
-        const size_t n = (size_t)(qs[w]->hi - qs[w]->lo);
-        a.lo = qs[w]->lo; a.hi = qs[w]->hi;
+        const size_t n = (size_t)(r[w].q->hi - r[w].q->lo);
+        a.lo = r[w].q->lo; a.hi = r[w].q->hi;
         a.stamp = ++ub.stamp;
         a.map = ub.map; a.blk = ub.blk;
         a.n_free = reinterpret_cast<int*>(d + o_n) + w;
         a.free_slot = reinterpret_cast<int*>(d + o_s) + cN;
-        if (os[w]->pos) { a.pos = reinterpret_cast<double*>(d) + 3 * cP; cP += n; }
-        if (os[w]->weight) { a.weight = reinterpret_cast<double*>(d + o_w) + cW; cW += n; }
+        if (r[w].o->pos) { a.pos = reinterpret_cast<double*>(d) + 3 * cP; cP += n; }
+        if (r[w].o->weight) { a.weight = reinterpret_cast<double*>(d + o_w) + cW; cW += n; }
         if (w == 0) l.w0 = a;
         else memcpy(st.up.h + sizeof(ReclaimArgs) * (size_t)(w - 1), &a, sizeof(ReclaimArgs));
         li += (size_t)a.n_live; cN += n;
@@ -2907,7 +2863,7 @@ static int reclaim_run(kba_handle* h, SelectStage& st, int W, kba_track* const* 
     if (e == cudaSuccess) e = wait_stream(h);
     if (e != cudaSuccess) {
         // as upkeep_run: the maps go back to all 0, whatever stamps the failed sequence left in them
-        for (int w = 0; w < W; ++w) cudaMemsetAsync(ts[w]->upkeep->map, 0, sizeof(unsigned long long) * (size_t)ts[w]->td.lm_cap, s);
+        for (int w = 0; w < W; ++w) cudaMemsetAsync(r[w].t->upkeep->map, 0, sizeof(unsigned long long) * (size_t)r[w].t->td.lm_cap, s);
         cudaStreamSynchronize(s);
         return fail(KBA_ERR_CUDA, std::string("landmark reclaim: ") + cudaGetErrorString(e));
     }
@@ -2915,8 +2871,8 @@ static int reclaim_run(kba_handle* h, SelectStage& st, int W, kba_track* const* 
     const int32_t* n_free = reinterpret_cast<const int32_t*>(hb + o_n);
     cP = cW = cN = 0;
     for (int w = 0; w < W; ++w) {
-        kba_reclaim_out& o = *os[w];
-        const size_t n = (size_t)(qs[w]->hi - qs[w]->lo), nf = (size_t)n_free[w];
+        kba_reclaim_out& o = *r[w].o;
+        const size_t n = (size_t)(r[w].q->hi - r[w].q->lo), nf = (size_t)n_free[w];
         o.n_free = n_free[w];
         if (nf) memcpy(o.free_slot, hb + o_s + 4 * cN, 4 * nf);
         if (o.pos) { if (nf) memcpy(o.pos, hb + 24 * cP, 24 * nf); cP += n; }
@@ -2928,81 +2884,63 @@ static int reclaim_run(kba_handle* h, SelectStage& st, int W, kba_track* const* 
     return KBA_OK;
 }
 
+struct Reclaim {
+    using Request = kba_reclaim_request;
+    using Out = kba_reclaim_out;
+    using Req = ReclaimReq;
+    static constexpr StoreCall slot = kReclaimCall;
+    static constexpr const char* staging = "reclaim";
+    static bool sits_out(const Request& q) { return q.hi == q.lo; }
+    static int sit_out_check(const Out&, std::string&) { return KBA_OK; }
+    static void sat_out(Out* o, bool group) {  // a single call's empty range has no free slot; a group's leaves out[i] as it is
+        if (!group) o->n_free = 0;
+    }
+    static Req make(kba_track* t, const Request& q, Out* o) {
+        Req r;
+        r.t = t; r.q = &q; r.o = o;
+        return r;
+    }
+    static int check(Req& r, std::string& why) { return reclaim_check(r.t, r.q, r.o, why); }
+    static void capacity(int n, kba_track* const* ts, size_t& up, size_t& down) {  // every keyframe slot, a range of max_landmarks
+        size_t kfs = 0;
+        down = 0;
+        for (int i = 0; i < n; ++i) { kfs += (size_t)ts[i]->td.kf_cap; down += reclaim_out_cap(ts[i]); }
+        up = sizeof(ReclaimArgs) * (size_t)(n - 1) + 4 * kfs;
+    }
+    static int run(kba_handle* h, StoreStage& st, int W, Req* r, int&, std::string&) { return reclaim_run(h, st, W, r); }
+};
+
 int kba_track_reclaim_landmarks(kba_track* t, const kba_reclaim_request* req, kba_reclaim_out* out) {
     static const std::string who = "kba_track_reclaim_landmarks: ";
     if (!t || !req || !out) return fail(KBA_ERR_BAD_ARG, who + "null argument");
-    std::string why;
-    int rc = reclaim_check(t, req, out, why);
-    if (rc != KBA_OK) return fail(rc, who + why);
-    SelectStage& st = t->upkeep->reclaim;
-    if (req->hi == req->lo) {  // an empty range: nothing is free, no upload, no launch
-        out->n_free = 0;
-        st.counts.h2d = 0; st.counts.d2h = 0;
-        t->last = &st.counts;
-        return KBA_OK;
-    }
-    if (!st.up.d) {  // the first single call of the track: staging for every keyframe slot and a range of max_landmarks
-        if (st.alloc(4 * (size_t)t->td.kf_cap, reclaim_out_cap(t))) {
-            st.up.release(); st.out.release();
-            return fail(KBA_ERR_CUDA, who + "out of memory for the reclaim staging");
-        }
-    }
-    rc = reclaim_run(t->h, st, 1, &t, &req, &out);
-    if (rc == KBA_OK) t->last = &st.counts;
-    return rc;
+    return store_call<Reclaim>(t->set, false, who, req, out);
 }
 
 int kba_track_group_reclaim_landmarks(kba_track_group* g, const kba_reclaim_request* req, kba_reclaim_out* out) {
     static const std::string who = "kba_track_group_reclaim_landmarks: ";
     if (!g || !req || !out) return fail(KBA_ERR_BAD_ARG, who + "null argument");
-    const int n = (int)g->tracks.size();
-    std::vector<kba_track*> ts;
-    std::vector<const kba_reclaim_request*> qs;
-    std::vector<kba_reclaim_out*> os;
-    for (int i = 0; i < n; ++i) {
-        if (req[i].hi == req[i].lo) continue;  // sits the call out
-        std::string why;
-        const int rc = reclaim_check(g->tracks[i], &req[i], &out[i], why);
-        if (rc != KBA_OK) return fail(rc, who + "track " + std::to_string(i) + ": " + why);
-        ts.push_back(g->tracks[i]); qs.push_back(&req[i]); os.push_back(&out[i]);
-    }
-    if (ts.empty()) {  // every track sits out: no upload, no launch
-        g->solver.h2d = 0; g->solver.d2h = 0;
-        g->last = &g->solver;
-        return KBA_OK;
-    }
-    if (!g->reclaim) {  // staging for every track at its capacities, allocated once
-        size_t kfs = 0, outs = 0;
-        for (const kba_track* t : g->tracks) { kfs += (size_t)t->td.kf_cap; outs += reclaim_out_cap(t); }
-        std::unique_ptr<SelectStage> st(new SelectStage());
-        if (st->alloc(sizeof(ReclaimArgs) * (size_t)(n - 1) + 4 * kfs, outs)) return fail(KBA_ERR_CUDA, who + "out of memory for the reclaim staging");
-        g->reclaim = std::move(st);
-    }
-    const int rc = reclaim_run(g->h, *g->reclaim, (int)ts.size(), ts.data(), qs.data(), os.data());
-    if (rc != KBA_OK) return rc;
-    g->last = &g->reclaim->counts;
-    return KBA_OK;
+    return store_call<Reclaim>(g->set, true, who, req, out);
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
 // motion-only frames against the persistent store (include/kba_b200.h, kba_track_adjust_pose / kba_track_group_adjust_pose)
 // ---------------------------------------------------------------------------------------------------------------------
 // every check of one frame, before anything is uploaded; n_runs = landmarks of the frame, rounds = trimming rounds it runs
-static int frame_check(const kba_track* t, const kba_track_frame* f, const kba_options* opt, MotionBufs& mb, int& n_runs, int& rounds,
-                       std::string& why) {
+static int frame_check(kba_track* t, const kba_track_frame* f, const kba_options* opt, int& n_runs, int& rounds, std::string& why) {
     n_runs = 0;
     if (f->n_meas < 0) { why = "negative n_meas"; return KBA_ERR_BAD_ARG; }
     if (!f->pose7 || !f->lm_slot || !f->u || !f->v || !f->d) { why = "null pose or measurement array"; return KBA_ERR_BAD_ARG; }
     if (f->speed_weight > 0 && !(f->speed_dt > 0)) { why = "speed prior: dt <= 0"; return KBA_ERR_BAD_ARG; }
     if (f->n_meas > t->caps.win_observations) { why = "more measurements than win_observations"; return KBA_ERR_CAPACITY; }
-    if (++mb.stamp == 0) { std::fill(mb.seen.begin(), mb.seen.end(), 0u); mb.stamp = 1; }
+    SlotStamps& st = t->stamps;
+    st.next();
     for (int i = 0; i < f->n_meas; ++i) {
         const int slot = f->lm_slot[i];
         if (slot < 0 || slot >= t->td.lm_cap) { why = "landmark slot out of range"; return KBA_ERR_BAD_ARG; }
         if (f->cam && (f->cam[i] < 0 || f->cam[i] >= t->n_cam)) { why = "camera index out of range"; return KBA_ERR_BAD_ARG; }
         if (i > 0 && slot == f->lm_slot[i - 1]) continue;
-        if (mb.seen[slot] == mb.stamp) { why = "landmark slot " + std::to_string(slot) + " reappears after its run"; return KBA_ERR_BAD_ARG; }
-        mb.seen[slot] = mb.stamp;
+        if (st.lm[slot] == st.cur) { why = "landmark slot " + std::to_string(slot) + " reappears after its run"; return KBA_ERR_BAD_ARG; }
+        st.lm[slot] = st.cur;
         ++n_runs;
     }
     if (n_runs > t->caps.win_landmarks) { why = "more landmarks than win_landmarks"; return KBA_ERR_CAPACITY; }
@@ -3022,7 +2960,7 @@ static int options_check(const kba_options* opt, std::string& why) {
 
 // frames f[i] of tracks ts[i] (already checked; runs[i] landmarks, rounds[i] trimming rounds; n_meas == 0: idle) as one launch
 static int adjust_pose_run(kba_handle* h, MotionBufs& mb, int n, kba_track* const* ts, const kba_track_frame* f, const int* runs,
-                           const int* rounds, const kba_options* opt, kba_result* res, int64_t& h2d, int64_t& d2h) {
+                           const int* rounds, const kba_options* opt, kba_result* res, Transfer& tr) {
     std::vector<int> live;
     int M = 0, Rn = 0, log_cap = 0;
     bool any_cam = false;
@@ -3033,7 +2971,7 @@ static int adjust_pose_run(kba_handle* h, MotionBufs& mb, int n, kba_track* cons
         any_cam |= f[i].cam != nullptr;
         if (res[i].iterations) log_cap = std::max(log_cap, std::min(res[i].iterations_capacity, kIterLogCap));
     }
-    h2d = 0; d2h = 0;
+    tr = Transfer{};
     const int nf = (int)live.size();
     if (nf == 0) return KBA_OK;
     CU(cudaSetDevice(h->device));
@@ -3056,7 +2994,7 @@ static int adjust_pose_run(kba_handle* h, MotionBufs& mb, int n, kba_track* cons
         FrameDesc& d = fd[q];
         d.n_meas = F.n_meas; d.n_runs = runs[i]; d.meas_off = mo; d.run_off = ro; d.rs_off = rso; d.rounds_total = rounds[i];
         d.lm_pos = t->td.lm_pos; d.lm_weight = t->td.lm_weight;
-        d.cam16 = t->solver.batch->bd.cam + (size_t)t->solver.batch->desc_h[0].cam_off * kCamStride; d.n_cam = t->n_cam; d.pad = 0;
+        d.cam16 = t->set.solver.batch->bd.cam + (size_t)t->set.solver.batch->desc_h[0].cam_off * kCamStride; d.n_cam = t->n_cam; d.pad = 0;
         memcpy(d.pose7, F.pose7, sizeof(d.pose7));
         d.speed_weight = F.speed_weight; d.speed_dt = F.speed_dt;
         memcpy(d.speed_v_before, F.speed_v_before, sizeof(d.speed_v_before));
@@ -3103,7 +3041,7 @@ static int adjust_pose_run(kba_handle* h, MotionBufs& mb, int n, kba_track* cons
     float ms = 0.f;
     CU(cudaEventElapsedTime(&ms, mb.ev0, mb.ev1));
     h->counters.launches_total += 1;
-    h2d = (int64_t)off; d2h = (int64_t)n_out;
+    tr.h2d = (int64_t)off; tr.d2h = (int64_t)n_out;
     // ---- results
     const FrameRes* fr = reinterpret_cast<const FrameRes*>(mb.out.h);
     const IterRecord* lg = reinterpret_cast<const IterRecord*>(mb.out.h + o_log);
@@ -3143,46 +3081,44 @@ static int adjust_pose_run(kba_handle* h, MotionBufs& mb, int n, kba_track* cons
 
 static int motion_alloc(std::unique_ptr<MotionBufs>& mb, int n, kba_track* const* ts) {
     if (mb) return KBA_OK;
-    int runs = 0, meas = 0, lm_cap = 0;
-    for (int i = 0; i < n; ++i) {
-        runs += ts[i]->caps.win_landmarks; meas += ts[i]->caps.win_observations; lm_cap = std::max(lm_cap, ts[i]->td.lm_cap);
-    }
+    int runs = 0, meas = 0;
+    for (int i = 0; i < n; ++i) { runs += ts[i]->caps.win_landmarks; meas += ts[i]->caps.win_observations; }
     std::unique_ptr<MotionBufs> m(new MotionBufs());
     if (m->alloc(n, runs, meas)) return fail(KBA_ERR_CUDA, "adjust_pose: out of memory");
-    m->seen.assign((size_t)lm_cap, 0u);
     mb = std::move(m);
     return KBA_OK;
 }
 
-// a pose-only call of a track (n = 1) or of a group: the options and every frame are checked before anything is uploaded or
-// launched.  Errors start with `who`; a group's name the failing track.
-static int track_adjust_pose(const std::string& who, bool group, kba_handle* h, TrackSolver& sv, int n, kba_track* const* ts,
-                             const kba_track_frame* f, const kba_options* opt, kba_result* res) {
+// a pose-only call of a track (group = false) or of a group: the options and every frame are checked before anything is uploaded
+// or launched.  Errors start with `who`; a group's name the failing track.
+static int track_adjust_pose(TrackSet& s, bool group, const std::string& who, const kba_track_frame* f, const kba_options* opt,
+                             kba_result* res) {
+    TrackSolver& sv = s.solver;
+    s.last = &sv.counts;
     std::string why;
     int rc = options_check(opt, why);
-    if (rc != KBA_OK) return fail(rc, who + ": " + why);
-    CU(cudaSetDevice(h->device));
-    rc = motion_alloc(sv.motion, n, ts);
+    if (rc != KBA_OK) return fail(rc, who + why);
+    CU(cudaSetDevice(s.h->device));
+    const int n = (int)s.tracks.size();
+    rc = motion_alloc(sv.motion, n, s.tracks.data());
     if (rc != KBA_OK) return rc;
     std::vector<int> runs(n, 0), rounds(n, 0);
     for (int i = 0; i < n; ++i) {
         if (f[i].n_meas == 0) continue;
-        rc = frame_check(ts[i], &f[i], opt, *sv.motion, runs[i], rounds[i], why);
-        if (rc != KBA_OK) return fail(rc, who + ": " + (group ? "track " + std::to_string(i) + ": " : std::string()) + why);
+        rc = frame_check(s.tracks[i], &f[i], opt, runs[i], rounds[i], why);
+        if (rc != KBA_OK) return fail(rc, who + track_prefix(group, i) + why);
     }
-    return adjust_pose_run(h, *sv.motion, n, ts, f, runs.data(), rounds.data(), opt, res, sv.h2d, sv.d2h);
+    return adjust_pose_run(s.h, *sv.motion, n, s.tracks.data(), f, runs.data(), rounds.data(), opt, res, sv.counts);
 }
 
 int kba_track_adjust_pose(kba_track* t, const kba_track_frame* f, const kba_options* opt, kba_result* res) {
     if (!t || !f || !opt || !res) return fail(KBA_ERR_BAD_ARG, "null argument to kba_track_adjust_pose");
-    t->last = &t->solver;
-    return track_adjust_pose("kba_track_adjust_pose", false, t->h, t->solver, 1, &t, f, opt, res);
+    return track_adjust_pose(t->set, false, "kba_track_adjust_pose: ", f, opt, res);
 }
 
 int kba_track_group_adjust_pose(kba_track_group* g, const kba_track_frame* f, const kba_options* opt, kba_result* res) {
     if (!g || !f || !opt || !res) return fail(KBA_ERR_BAD_ARG, "null argument to kba_track_group_adjust_pose");
-    g->last = &g->solver;
-    return track_adjust_pose("kba_track_group_adjust_pose", true, g->h, g->solver, (int)g->tracks.size(), g->tracks.data(), f, opt, res);
+    return track_adjust_pose(g->set, true, "kba_track_group_adjust_pose: ", f, opt, res);
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
@@ -3193,23 +3129,12 @@ static int rank_alloc(kba_track* t, std::string& why) {
     std::unique_ptr<RankBufs> rb(new RankBufs());
     const size_t L = (size_t)t->td.lm_cap, K = (size_t)t->td.kf_cap, M = (size_t)t->td.m_cap;
     int bad = 0;
-    bad |= rb->alloc(&rb->qty, select_out_bytes(L, 1)); bad |= rb->alloc(&rb->mark, L); bad |= rb->alloc(&rb->dcand, M);
-    bad |= rb->alloc(&rb->dcost, M); bad |= rb->alloc(&rb->dcnt, K); bad |= rb->alloc(&rb->sel_slot, L); bad |= rb->alloc(&rb->gp, L);
+    DevAllocs& dev = rb->dev;
+    bad |= dev.alloc(&rb->qty, select_out_bytes(L, 1)); bad |= dev.alloc(&rb->mark, L); bad |= dev.alloc(&rb->dcand, M);
+    bad |= dev.alloc(&rb->dcost, M); bad |= dev.alloc(&rb->dcnt, K); bad |= dev.alloc(&rb->sel_slot, L); bad |= dev.alloc(&rb->gp, L);
     if (bad) { why = "out of memory for the ranking buffers"; return KBA_ERR_CUDA; }
     t->rank = std::move(rb);
     return KBA_OK;
-}
-
-// upload and download capacities of a staging that serves tracks ts[0..n) (one window each)
-static size_t rank_up_cap(int n, kba_track* const* ts) {
-    size_t b = (sizeof(SelectArgs) + sizeof(RankArgs)) * (size_t)(n - 1) + 8 * (size_t)kRankMaxDepth * n + 8 * (size_t)n + 8;
-    for (int i = 0; i < n; ++i) b += 4 * (size_t)ts[i]->td.kf_cap + 9 * (size_t)ts[i]->td.lm_cap;  // lists, flags, draws
-    return b;
-}
-static size_t rank_out_cap(int n, kba_track* const* ts) {
-    size_t b = 16 * (size_t)n + 8;
-    for (int i = 0; i < n; ++i) b += 5 * (size_t)ts[i]->td.lm_cap;
-    return b;
 }
 
 struct RankReq {
@@ -3245,8 +3170,9 @@ static int rank_check(RankReq& r, std::string& why) {
 
 // W checked requests of distinct tracks as the W windows of one launch sequence in two parts (include/kba_b200.h): the lists go
 // up, the chain and the AddDepth costs run, the middle bins' sizes come down; the draw functions fill the draws, which go up with
-// each window's output offsets; the heaps, the shuffle and the union run, the outputs come down.
-static int rank_run(kba_handle* h, SelectStage& st, int W, RankReq* r) {
+// each window's output offsets; the heaps, the shuffle and the union run, the outputs come down.  A draw function that fails
+// or is missing fails the call as request `bad`, for `why`.
+static int rank_run(kba_handle* h, StoreStage& st, int W, RankReq* r, int& bad, std::string& why) {
     CU(cudaSetDevice(h->device));
     cudaStream_t s = h->stream;
     SelectGrid sg;
@@ -3349,7 +3275,6 @@ static int rank_run(kba_handle* h, SelectStage& st, int W, RankReq* r) {
         p2[2 * w] = (int)n_draws; p2[2 * w + 1] = (int)n_out;
         n_out += (size_t)bound[w];
         if (D == 0) continue;
-        std::string why;
         if (!q.draw) why = "the middle bin needs " + std::to_string(D) + " draws and there is no draw function";
         else if (q.draw(q.draw_ctx, D, draws + n_draws) != 0) why = "the draw function failed";
         if (!why.empty()) {  // nothing is written; the slot maps go back to all -1 and no track keeps a ranking
@@ -3358,7 +3283,8 @@ static int rank_run(kba_handle* h, SelectStage& st, int W, RankReq* r) {
                 cudaMemsetAsync(r[v].t->select->a.cand_of, 0xff, sizeof(int) * (size_t)r[v].t->td.lm_cap, s);
             }
             cudaStreamSynchronize(s);
-            return fail(KBA_ERR_BAD_ARG, std::string(W > 1 ? "track " + std::to_string(w) + ": " : "") + why);
+            bad = w;
+            return KBA_ERR_BAD_ARG;
         }
         n_draws += (size_t)D;
     }
@@ -3389,111 +3315,57 @@ static int rank_run(kba_handle* h, SelectStage& st, int W, RankReq* r) {
     return KBA_OK;
 }
 
+struct Rank {
+    using Request = kba_rank_request;
+    using Out = kba_rank_out;
+    using Req = RankReq;
+    static constexpr StoreCall slot = kRankCall;
+    static constexpr const char* staging = "ranking";
+    static bool sits_out(const Request& q) { return q.n_kf == 0; }
+    static int sit_out_check(const Out&, std::string&) { return KBA_OK; }
+    static void sat_out(Out*, bool) {}
+    static Req make(kba_track* t, const Request& q, Out* o) {
+        Req r;
+        r.t = t; r.q = &q; r.o = o;
+        return r;
+    }
+    static int check(Req& r, std::string& why) { return rank_check(r, why); }
+    static void capacity(int n, kba_track* const* ts, size_t& up, size_t& down) {
+        up = (sizeof(SelectArgs) + sizeof(RankArgs)) * (size_t)(n - 1) + 8 * (size_t)kRankMaxDepth * n + 8 * (size_t)n + 8;
+        down = 16 * (size_t)n + 8;
+        for (int i = 0; i < n; ++i) {
+            up += 4 * (size_t)ts[i]->td.kf_cap + 9 * (size_t)ts[i]->td.lm_cap;  // lists, flags, draws
+            down += 5 * (size_t)ts[i]->td.lm_cap;
+        }
+    }
+    static int run(kba_handle* h, StoreStage& st, int W, Req* r, int& bad, std::string& why) { return rank_run(h, st, W, r, bad, why); }
+};
+
 int kba_track_rank_landmarks(kba_track* t, const kba_rank_request* req, kba_rank_out* out) {
     static const std::string who = "kba_track_rank_landmarks: ";
     if (!t || !req) return fail(KBA_ERR_BAD_ARG, who + "null argument");
-    RankReq r;
-    r.t = t; r.q = req; r.o = out;
-    std::string why;
-    int rc = rank_check(r, why);
-    if (rc != KBA_OK) return fail(rc, who + why);
-    SelectStage& st = t->rank->stage;
-    if (!st.up.d && st.alloc(rank_up_cap(1, &t), rank_out_cap(1, &t))) {  // the first single call of the track
-        st.up.release(); st.out.release();
-        return fail(KBA_ERR_CUDA, who + "out of memory for the ranking staging");
-    }
-    rc = rank_run(t->h, st, 1, &r);
-    if (rc == KBA_OK) t->last = &st.counts;
-    return rc;
+    return store_call<Rank>(t->set, false, who, req, out);  // a null out fails in rank_check
 }
 
 int kba_track_group_rank_landmarks(kba_track_group* g, const kba_rank_request* req, kba_rank_out* out) {
     static const std::string who = "kba_track_group_rank_landmarks: ";
     if (!g || !req || !out) return fail(KBA_ERR_BAD_ARG, who + "null argument");
-    const int n = (int)g->tracks.size();
-    // ---- every request is checked before anything is uploaded or written
-    std::vector<RankReq> rs;
-    for (int i = 0; i < n; ++i) {
-        if (req[i].n_kf == 0) continue;  // sits the call out
-        RankReq r;
-        r.t = g->tracks[i]; r.q = &req[i]; r.o = &out[i];
-        std::string why;
-        const int rc = rank_check(r, why);
-        if (rc != KBA_OK) return fail(rc, who + "track " + std::to_string(i) + ": " + why);
-        rs.push_back(r);
-    }
-    if (rs.empty()) {  // every track sits out: no upload, no launch
-        g->solver.h2d = 0; g->solver.d2h = 0;
-        g->last = &g->solver;
-        return KBA_OK;
-    }
-    if (!g->rank) {  // staging for every track at its capacities, allocated once
-        std::unique_ptr<SelectStage> st(new SelectStage());
-        if (st->alloc(rank_up_cap(n, g->tracks.data()), rank_out_cap(n, g->tracks.data())))
-            return fail(KBA_ERR_CUDA, who + "out of memory for the ranking staging");
-        g->rank = std::move(st);
-    }
-    const int rc = rank_run(g->h, *g->rank, (int)rs.size(), rs.data());
-    if (rc != KBA_OK) return rc;
-    g->last = &g->rank->counts;
-    return KBA_OK;
-}
-
-// the checks of a solve of track t's ranking; sel2 receives the caller's window with the ranking's ground-candidate count
-static int ranked_check(kba_track* t, int32_t n_kf, const int32_t* kf_slot, const uint8_t* kf_fixed, const kba_window* sel,
-                        TrackRequest& q, kba_window& sel2, std::string& why) {
-    if (!kf_slot || !kf_fixed || !sel) { why = "null argument"; return KBA_ERR_BAD_ARG; }
-    const RankBufs* rb = t->rank.get();
-    if (!rb || !rb->valid) { why = "the track has no ranking to solve (kba_track_rank_landmarks)"; return KBA_ERR_BAD_ARG; }
-    if (rb->gen != t->gen) { why = "the ranking is stale: the store changed after it was ranked"; return KBA_ERR_BAD_ARG; }
-    if (n_kf != (int)rb->kf.size() || !std::equal(rb->kf.begin(), rb->kf.end(), kf_slot)) {
-        why = "the keyframes differ from the ranking's"; return KBA_ERR_BAD_ARG;
-    }
-    sel2 = *sel;
-    const bool from_ranking = sel->n_gp > 0 && !sel->gp_lm && !sel->gp_kf && !sel->gp_weight;
-    if (from_ranking) sel2.n_gp = rb->n_ground;
-    q.n_kf = n_kf; q.kf_slot = kf_slot; q.kf_fixed = kf_fixed; q.n_lm = rb->n_sel; q.lm_slot = nullptr; q.sel = &sel2;
-    q.ranked = true; q.rank_gp = from_ranking && rb->n_ground > 0;
-    return track_check(t, q, why);
+    return store_call<Rank>(g->set, true, who, req, out);
 }
 
 int kba_track_solve_ranked(kba_track* t, int32_t n_kf, const int32_t* kf_slot, const uint8_t* kf_fixed, const kba_window* sel,
                            const kba_options* opt, kba_result* res) {
     if (!t || !opt || !res) return fail(KBA_ERR_BAD_ARG, "null argument to kba_track_solve_ranked");
-    TrackRequest q;
-    kba_window sel2;
-    std::string why;
-    const int rc = ranked_check(t, n_kf, kf_slot, kf_fixed, sel, q, sel2, why);
-    if (rc != KBA_OK) return fail(rc, "kba_track_solve_ranked: " + why);
-    TrackSolver& sv = q.rows > kFusedMaxRows ? t->large : t->solver;
-    t->last = &sv;
-    return track_solve(t->h, sv, 1, &t, &q, opt, res);
+    TrackRequest q = track_request(n_kf, kf_slot, kf_fixed, 0, nullptr, sel, true);
+    return set_solve(t->set, false, "kba_track_solve_ranked: ", &q, opt, res);
 }
 
 int kba_track_group_solve_ranked(kba_track_group* g, const kba_ranked_request* req, const kba_options* opt, kba_result* res) {
     if (!g || !req || !opt || !res) return fail(KBA_ERR_BAD_ARG, "null argument to kba_track_group_solve_ranked");
-    const int n = (int)g->tracks.size();
-    std::vector<TrackRequest> qs(n);
-    std::vector<kba_window> sels(n);
-    int active = 0;
-    bool large = false;
-    for (int i = 0; i < n; ++i) {
-        if (req[i].n_kf == 0) continue;  // sits this solve out
-        std::string why;
-        const int rc = ranked_check(g->tracks[i], req[i].n_kf, req[i].kf_slot, req[i].kf_fixed, req[i].sel, qs[i], sels[i], why);
-        if (rc != KBA_OK) return fail(rc, "kba_track_group_solve_ranked: track " + std::to_string(i) + ": " + why);
-        ++active;
-        large |= qs[i].rows > kFusedMaxRows;
-    }
-    if (active == 0) {
-        for (int i = 0; i < n; ++i) idle_result(res[i]);
-        g->solver.h2d = 0; g->solver.d2h = 0;
-        g->last = &g->solver;
-        return KBA_OK;
-    }
-    TrackSolver& sv = large ? g->large : g->solver;
-    g->last = &sv;
-    return track_solve(g->h, sv, n, g->tracks.data(), qs.data(), opt, res);
+    std::vector<TrackRequest> qs;
+    for (size_t i = 0; i < g->set.tracks.size(); ++i)
+        qs.push_back(track_request(req[i].n_kf, req[i].kf_slot, req[i].kf_fixed, 0, nullptr, req[i].sel, true));
+    return set_solve(g->set, true, "kba_track_group_solve_ranked: ", qs.data(), opt, res);
 }
 
 }  // extern "C"

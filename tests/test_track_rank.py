@@ -370,6 +370,46 @@ def test_rank_rejects_bad_requests_and_writes_nothing():
     t.close(); h.close()
 
 
+@pytest.mark.gpu
+def test_group_rank_draw_failure_names_its_track():
+    """a group of three whose track 0 sits out and whose track 2's draws are too short: the error names track 2 (not its index
+    among the requests that run), nothing is written, and neither running track keeps a ranking"""
+    from limo_b200 import capi
+    h = capi.Handle(0)
+    scs = [Scene(41, n_kf=12, n_lm=900, rig=False), Scene(42, n_kf=12, n_lm=1000, rig=True), Scene(21, n_kf=12, n_lm=1200, rig=True)]
+    ts = [_track(h, sc) for sc in scs]
+    g = capi.TrackGroup(h, ts)
+    kf_list = list(range(1, 12))
+    cands = [scs[i].slot[_candidates(scs[i], kf_list)] for i in range(3)]
+    q2 = host_select(scs[2], kf_list, _candidates(scs[2], kf_list), VOX["voxel_size"], VOX["roi_far"], VOX["roi_middle"])
+    assert (q2["bin"] == 1).sum() > 1  # track 2 needs draws
+    rng = np.random.default_rng(11)
+    ts[1].rank_landmarks(kf_list, cands[1], draws=rng.integers(0, 2**31 - 1, len(cands[1])), **CAPS, **VOX)  # a ranking to lose
+    reqs, outs = (capi.KbaRankRequest * 3)(), (capi.KbaRankOut * 3)()
+    keep = []
+    for i, draws in ((1, rng.integers(0, 2**31 - 1, len(cands[1]))), (2, np.zeros(0, np.int64))):
+        q, o, (c, k), lists = capi.Track._rank_args(kf_list, cands[i], draws=draws, **CAPS, **VOX)
+        c[:] = -7
+        k[:] = -7
+        o.n_sel = o.n_ground = o.n_draws = -7
+        reqs[i], outs[i] = q, o
+        keep.append((i, c, k, lists))
+    outs[0].n_sel = outs[0].n_ground = outs[0].n_draws = -7
+    assert capi.lib().kba_track_group_rank_landmarks(g._p, reqs, outs) == 1  # KBA_ERR_BAD_ARG
+    msg = capi.lib().kba_last_error().decode()
+    assert "kba_track_group_rank_landmarks" in msg and "track 2: " in msg, msg
+    for i in range(3):
+        assert (outs[i].n_sel, outs[i].n_ground, outs[i].n_draws) == (-7, -7, -7), i
+    for i, c, k, _ in keep:
+        assert (c == -7).all() and (k == -7).all(), i
+        with pytest.raises(capi.KbaError, match="no ranking"):
+            ts[i].solve_ranked(kf_list, np.r_[[1], np.zeros(10, np.uint8)])
+    g.close()
+    for t in ts:
+        t.close()
+    h.close()
+
+
 def _same_result(a, b):
     for key in ("kf_pose", "kf_plane", "lm_pos"):
         assert np.array_equal(getattr(a, key).view(np.int64), getattr(b, key).view(np.int64)), key
