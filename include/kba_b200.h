@@ -219,6 +219,11 @@ int kba_set_stream(kba_handle* h, void* cuda_stream);    /* cudaStream_t; NULL =
 int kba_solve_window(kba_handle* h, const kba_window* w, const kba_options* opt, kba_result* res);
 /* many independent windows in one call ("BA windows/s") */
 int kba_solve_batch(kba_handle* h, int32_t n_windows, const kba_window* w, const kba_options* opt, kba_result* res);
+/* kba_solve_batch with opts[n_windows]: window i is solved with opts[i] exactly as kba_solve_batch solves it with that one set
+ * (a parameter sweep over one recording in one launch).  Checked before anything is uploaded: an entry that kba_batch_solve
+ * refuses, or entries whose precision differs (it selects the kernel variants of the whole batch), fail the call with its code,
+ * and kba_last_error names the window index. */
+int kba_solve_batch_opts(kba_handle* h, int32_t n_windows, const kba_window* w, const kba_options* opts, kba_result* res);
 /* residuals + Jacobian blocks of the reprojection / depth residuals at the input state
  * (what ceres::Problem::Evaluate would return for those blocks, cf. robust_solving.cpp:44) */
 int kba_eval(kba_handle* h, const kba_window* w, const kba_options* opt, kba_eval_out* out);
@@ -231,6 +236,14 @@ int kba_batch_upload(kba_batch* b, int32_t n_windows, const kba_window* w); /* r
  * handle runs on the legacy default stream, which cannot be captured: give the handle a stream of its own (kba_create does,
  * kba_set_stream with a created stream keeps it).  INTEGRATION.md lists the switches (KBA_GRAPH, ...). */
 int kba_batch_solve(kba_batch* b, const kba_options* opt);
+/* kba_batch_solve with one kba_options per window, opts[n_windows]: window i runs with opts[i] (thresholds, quantiles, trimming,
+ * iteration counts, tolerances, time limit) and its results equal those of kba_batch_solve(b, &opts[i]) for that window bit for
+ * bit.  precision must be the same in every entry (KBA_ERR_BAD_ARG otherwise); each entry is checked as kba_batch_solve checks
+ * its one, before anything is uploaded, and kba_last_error names the window index.  The pass cap follows the largest iteration
+ * counts; the host safety cap the largest solver_time_sec (none if some window has none).  The options live on the device and go
+ * up only when they differ from the last solve's of the batch: a resident re-solve with the same options copies nothing more,
+ * and changing only the options does not rebuild the solve's CUDA graph. */
+int kba_batch_solve_opts(kba_batch* b, const kba_options* opts);
 int kba_batch_download(kba_batch* b, kba_result* res);
 int kba_batch_transfer_bytes(kba_batch* b, int64_t* h2d_bytes, int64_t* d2h_bytes); /* of the last upload / download */
 int kba_batch_jacobian_pass(kba_batch* b, const kba_options* opt, int32_t repeats, float* ms_out); /* residual/Jacobian kernel only */
@@ -408,8 +421,10 @@ int kba_track_select_landmarks(kba_track* t, int32_t n_kf, const int32_t* kf_slo
  *     call returns that request's code before anything is uploaded or launched, kba_last_error names the track index, and no
  *     store changes.
  *   - Results: window i is the window kba_track_solve would build for track i; its results go to res[i] and into track i's
- *     store exactly as for a single solve.  One kba_options applies to the whole group; solver_time_sec is checked on the
- *     group's shared passes: each window's inner solves are timed on the device while the passes of the whole group run, so
+ *     store exactly as for a single solve.  One kba_options applies to the whole group, or one per track with the _opts
+ *     forms (kba_track_group_solve_opts, kba_track_group_solve_ranked_opts, kba_track_group_adjust_pose_opts: a parameter
+ *     sweep over one recording, each track a grid point).  precision is the same for every track.  solver_time_sec is checked
+ *     on the group's shared passes: each window's inner solves are timed on the device while the passes of the whole group run, so
  *     a window's budget includes the time its group's other windows take.
  *   - Launch configuration, decided per solve from the windows that are solved: the largest rig rank, the seven-slot Schur
  *     kernel if any window needs more than 176 reduced rows, and from these the fused-linearisation switch, as kba_batch_solve
@@ -432,6 +447,11 @@ int kba_track_group_create(kba_handle* h, int32_t n_tracks, kba_track* const* tr
 void kba_track_group_destroy(kba_track_group* g);
 /* req[n_tracks], res[n_tracks] */
 int kba_track_group_solve(kba_track_group* g, const kba_track_request* req, const kba_options* opt, kba_result* res);
+/* kba_track_group_solve with opts[n_tracks]: track i's window runs with opts[i], and its results and store equal those of
+ * kba_track_solve with opts[i] bit for bit.  The entries of the tracks that solve are checked as kba_batch_solve_opts checks
+ * them, before anything is uploaded, and kba_last_error names the track index; a track that sits the solve out (n_kf == 0) does
+ * not read its entry.  The options travel in the lists' copy, and only when they differ from the group's last solve's. */
+int kba_track_group_solve_opts(kba_track_group* g, const kba_track_request* req, const kba_options* opts, kba_result* res);
 /* upload / download of the last group solve, pose-only call, selection, creation, upkeep, flow or reclaim call, counted as kba_track_transfer_bytes counts them */
 int kba_track_group_transfer_bytes(kba_track_group* g, int64_t* h2d_last_solve, int64_t* d2h_last_solve);
 
@@ -791,6 +811,8 @@ typedef struct kba_ranked_request {
 /* kba_track_group_solve on every track's last ranking; each request is checked as kba_track_solve_ranked checks it.
  * req[n_tracks], res[n_tracks] */
 int kba_track_group_solve_ranked(kba_track_group* g, const kba_ranked_request* req, const kba_options* opt, kba_result* res);
+/* kba_track_group_solve_ranked with opts[n_tracks], one per track, as kba_track_group_solve_opts takes them */
+int kba_track_group_solve_ranked_opts(kba_track_group* g, const kba_ranked_request* req, const kba_options* opts, kba_result* res);
 
 /* ---- adjustPoseOnly against the persistent store: one frame's pose per call, or one frame of each track of a group -------
  * What limo calls on every frame (bundle_adjuster_keyframes.cpp:820-888): one free pose against constant landmarks, the optional
@@ -828,6 +850,10 @@ typedef struct kba_track_frame {
 int kba_track_adjust_pose(kba_track* t, const kba_track_frame* f, const kba_options* opt, kba_result* res);
 /* f[n_tracks], res[n_tracks]: frame i is tracked against track i's store, all frames in one launch */
 int kba_track_group_adjust_pose(kba_track_group* g, const kba_track_frame* f, const kba_options* opt, kba_result* res);
+/* kba_track_group_adjust_pose with opts[n_tracks]: frame i is tracked with opts[i], exactly as kba_track_adjust_pose with opts[i].
+ * The entries of the frames that are tracked are checked before anything is uploaded (kba_last_error names the track index); a
+ * frame with n_meas == 0 does not read its entry. */
+int kba_track_group_adjust_pose_opts(kba_track_group* g, const kba_track_frame* f, const kba_options* opts, kba_result* res);
 
 /* ---- landmark initialisation of push() for a whole window (SURVEY 8(f) row 2) ------------------------------------------
  * Replaces, for all landmarks of `w` at once, what BundleAdjusterKeyframes::push() does per new landmark on the host:

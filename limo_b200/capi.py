@@ -29,7 +29,9 @@ SYMBOLS = ["kba_version", "kba_last_error", "kba_default_options", "kba_create",
            "kba_track_create_landmarks", "kba_track_group_create_landmarks", "kba_track_deactivate_keyframes",
            "kba_track_group_deactivate_keyframes", "kba_track_depth_costs", "kba_track_group_depth_costs", "kba_track_frame_flow",
            "kba_track_group_frame_flow", "kba_track_reclaim_landmarks", "kba_track_group_reclaim_landmarks",
-           "kba_track_rank_landmarks", "kba_track_group_rank_landmarks", "kba_track_solve_ranked", "kba_track_group_solve_ranked"]
+           "kba_track_rank_landmarks", "kba_track_group_rank_landmarks", "kba_track_solve_ranked", "kba_track_group_solve_ranked",
+           "kba_solve_batch_opts", "kba_batch_solve_opts", "kba_track_group_solve_opts", "kba_track_group_solve_ranked_opts",
+           "kba_track_group_adjust_pose_opts"]
 
 
 class KbaError(RuntimeError):
@@ -149,6 +151,11 @@ def lib():
         L.kba_track_group_rank_landmarks.argtypes = [vp, C.POINTER(KbaRankRequest), C.POINTER(KbaRankOut)]
         L.kba_track_solve_ranked.argtypes = [vp, C.c_int32, ip, u8p, C.POINTER(KbaWindow), C.POINTER(KbaOptions), C.POINTER(KbaResult)]
         L.kba_track_group_solve_ranked.argtypes = [vp, C.POINTER(KbaRankedRequest), C.POINTER(KbaOptions), C.POINTER(KbaResult)]
+        L.kba_solve_batch_opts.argtypes = [vp, C.c_int32, C.POINTER(KbaWindow), C.POINTER(KbaOptions), C.POINTER(KbaResult)]
+        L.kba_batch_solve_opts.argtypes = [vp, C.POINTER(KbaOptions)]
+        L.kba_track_group_solve_opts.argtypes = [vp, C.POINTER(KbaTrackRequest), C.POINTER(KbaOptions), C.POINTER(KbaResult)]
+        L.kba_track_group_solve_ranked_opts.argtypes = [vp, C.POINTER(KbaRankedRequest), C.POINTER(KbaOptions), C.POINTER(KbaResult)]
+        L.kba_track_group_adjust_pose_opts.argtypes = [vp, C.POINTER(KbaTrackFrame), C.POINTER(KbaOptions), C.POINTER(KbaResult)]
         L.kba_lidar_default_options.argtypes = [C.POINTER(KbaLidarOptions)]
         L.kba_lidar_default_options.restype = None
         fp = C.POINTER(C.c_float)
@@ -167,6 +174,18 @@ def default_options():
     o = KbaOptions()
     lib().kba_default_options(C.byref(o))
     return o
+
+
+def _options(opt, n, single, per_unit):
+    """(C function, options argument) of a call over n windows, tracks or frames: opt None or one KbaOptions -> the single-options
+    function; a sequence with one KbaOptions (or None: the defaults) per unit -> its per-unit form.  A wrong length raises before
+    any C call."""
+    if opt is None or isinstance(opt, KbaOptions):
+        return single, C.byref(opt or default_options())
+    opts = list(opt)
+    if len(opts) != n:
+        raise ValueError("%d option sets for %d windows / tracks" % (len(opts), n))
+    return per_unit, (KbaOptions * n)(*[o or default_options() for o in opts])
 
 
 def lidar_default_options():
@@ -188,7 +207,9 @@ class Batch:
         _check(lib().kba_batch_upload(self._p, len(self.windows), self._arr))
 
     def solve(self, opt=None):
-        _check(lib().kba_batch_solve(self._p, C.byref(opt or default_options())))
+        """opt: one KbaOptions for every window, or a sequence of one per window (kba_batch_solve_opts)"""
+        fn, o = _options(opt, len(self.windows), lib().kba_batch_solve, lib().kba_batch_solve_opts)
+        _check(fn(self._p, o))
 
     def download(self, iterations_capacity=0, results=None):
         """results: reuse the buffers of an earlier download (avoids re-allocating numpy arrays every step)"""
@@ -544,8 +565,10 @@ class TrackGroup:
 
     def solve(self, requests, opt=None, iterations_capacity=256):
         """requests: one per track, None (the track sits this solve out) or a dict with the arguments of Track.solve
-        (kf_slots, kf_fixed, lm_slots and the scalar keywords).  Returns one Result per track."""
+        (kf_slots, kf_fixed, lm_slots and the scalar keywords).  opt: one KbaOptions, or one per track
+        (kba_track_group_solve_opts).  Returns one Result per track."""
         assert len(requests) == len(self.tracks)
+        fn, o = _options(opt, len(self.tracks), lib().kba_track_group_solve, lib().kba_track_group_solve_opts)
         reqs = (KbaTrackRequest * len(requests))()
         keep, results = [], []
         for i, r in enumerate(requests):
@@ -563,15 +586,17 @@ class TrackGroup:
             keep.append((kf, fx, lm, sel))
             results.append(Result(sel, iterations_capacity))
         rarr = (KbaResult * len(results))(*[r.c for r in results])
-        _check(lib().kba_track_group_solve(self._p, reqs, C.byref(opt or default_options()), rarr))
+        _check(fn(self._p, reqs, o, rarr))
         for r, c in zip(results, rarr):
             r.c = c
         return results
 
     def adjust_pose(self, frames, opt=None, iterations_capacity=256):
         """one frame per track in one launch (kba_track_group_adjust_pose): each entry None (the track sits the call out) or a
-        dict with the arguments of Track.adjust_pose (pose7, lm_slot, u, v, d, cam, speed).  Returns one Result per track."""
+        dict with the arguments of Track.adjust_pose (pose7, lm_slot, u, v, d, cam, speed).  opt: one KbaOptions, or one per
+        track (kba_track_group_adjust_pose_opts).  Returns one Result per track."""
         assert len(frames) == len(self.tracks)
+        fn, o = _options(opt, len(self.tracks), lib().kba_track_group_adjust_pose, lib().kba_track_group_adjust_pose_opts)
         arr = (KbaTrackFrame * len(frames))()
         keep, results = [], []
         for i, fr in enumerate(frames):
@@ -583,7 +608,7 @@ class TrackGroup:
             keep.append(k)
             results.append(Track._frame_result(n_runs, iterations_capacity))
         rarr = (KbaResult * len(results))(*[r.c for r in results])
-        _check(lib().kba_track_group_adjust_pose(self._p, arr, C.byref(opt or default_options()), rarr))
+        _check(fn(self._p, arr, o, rarr))
         for r, c in zip(results, rarr):
             r.c = c
         return results
@@ -773,8 +798,9 @@ class TrackGroup:
     def solve_ranked(self, requests, opt=None, iterations_capacity=256):
         """solve_ranked for every track as one batch (kba_track_group_solve_ranked): each entry None (the track sits this solve out)
         or a dict with the arguments of Track.solve_ranked (kf_slots, kf_fixed, ground and the scalar keywords).  Returns one
-        Result per track, sized for its ranking."""
+        Result per track, sized for its ranking.  opt: one KbaOptions, or one per track (kba_track_group_solve_ranked_opts)."""
         assert len(requests) == len(self.tracks)
+        fn, o = _options(opt, len(self.tracks), lib().kba_track_group_solve_ranked, lib().kba_track_group_solve_ranked_opts)
         reqs = (KbaRankedRequest * len(requests))()
         keep, results = [], []
         for i, r in enumerate(requests):
@@ -792,7 +818,7 @@ class TrackGroup:
             keep.append((kf, fx, sel))
             results.append(Result(sel, iterations_capacity))
         rarr = (KbaResult * len(results))(*[r.c for r in results])
-        _check(lib().kba_track_group_solve_ranked(self._p, reqs, C.byref(opt or default_options()), rarr))
+        _check(fn(self._p, reqs, o, rarr))
         for r, c in zip(results, rarr):
             r.c = c
         return results
@@ -868,10 +894,12 @@ class Handle:
         return res
 
     def solve_batch(self, windows, opt=None, iterations_capacity=1):
+        """opt: one KbaOptions for every window, or a sequence of one per window (kba_solve_batch_opts)"""
+        fn, o = _options(opt, len(windows), lib().kba_solve_batch, lib().kba_solve_batch_opts)
         results = [Result(w, iterations_capacity) for w in windows]
         warr = (KbaWindow * len(windows))(*[w.c for w in windows])
         rarr = (KbaResult * len(windows))(*[r.c for r in results])
-        _check(lib().kba_solve_batch(self._p, len(windows), warr, C.byref(opt or default_options()), rarr))
+        _check(fn(self._p, len(windows), warr, o, rarr))
         for r, c in zip(results, rarr):
             r.c = c
         self._keep = rarr

@@ -7,6 +7,7 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <functional>
 #include <memory>
 #include <string>
 #include <thread>
@@ -121,7 +122,8 @@ struct kba_batch {
     cudaEvent_t ev_a = nullptr, ev_b = nullptr, ev_poll = nullptr, ev_poll2 = nullptr;
     // The pass sequence as a CUDA graph (kba_batch_solve): mode 2 = ONE launch per solve, the passes are the body of a conditional
     // WHILE node whose condition the device sets (k_loop_cond); mode 1 = a graph of `check_every` passes launched until the
-    // downloaded active-window count is zero.  Rebuilt when anything a kernel receives by value changes (`key`).
+    // downloaded active-window count is zero.  Rebuilt when anything a kernel receives by value changes (`key`); the solver options
+    // are read from device memory (BatchDev::wsp), so a solve with other options launches the same graph.
     struct SolveGraph {
         cudaGraph_t graph = nullptr;
         cudaGraphExec_t exec = nullptr;
@@ -137,6 +139,10 @@ struct kba_batch {
     } sg;
     Staged<int> loop_pass;  // passes the WHILE node has run (device counter + pinned copy)
     long long solves_done = 0;
+    // the solver options of every window (BatchDev::wsp): staged here, or at the front of a track solver's list upload
+    // (track_solver_create re-points bd.wsp), and uploaded only when they differ from wsp_dev, what the device holds
+    Staged<SolveParams> wsp;
+    std::vector<SolveParams> wsp_dev;
 
     template <typename T>
     int dev_alloc(T** p, size_t count) {
@@ -170,13 +176,14 @@ struct kba_batch {
         if (ev_poll2) cudaEventDestroy(ev_poll2);
         sg.destroy();
         loop_pass.release();
+        wsp.release();
     }
 };
 
 // buffers of kba_track_adjust_pose / kba_track_group_adjust_pose (k_adjust_pose): allocated at the first call, for the capacities of
 // the track(s), then reused: a call makes one upload, one launch, one download and one synchronisation
 struct MotionBufs {
-    Staged<unsigned char> up;    // frame descriptors, run starts and measurements of one call (pinned + device)
+    Staged<unsigned char> up;    // frame descriptors, solver options, run starts and measurements of one call (pinned + device)
     Staged<unsigned char> out;   // FrameRes per frame, iteration records, rejections (device + pinned)
     double* run_pw = nullptr, *trim_val = nullptr;
     unsigned char* run_active = nullptr, *run_rej = nullptr;
@@ -185,7 +192,8 @@ struct MotionBufs {
     int frames_cap = 0, runs_cap = 0, meas_cap = 0;
     static size_t al(size_t b) { return (b + 15) & ~(size_t)15; }
     static size_t up_bytes(int frames, int runs, int meas) {
-        return al(sizeof(FrameDesc) * (size_t)frames) + al(4 * ((size_t)runs + frames)) + 5 * al(4 * (size_t)meas);
+        return al(sizeof(FrameDesc) * (size_t)frames) + al(sizeof(SolveParams) * (size_t)frames) + al(4 * ((size_t)runs + frames)) +
+               5 * al(4 * (size_t)meas);
     }
     static size_t out_bytes(int frames, int log_cap, int runs) {
         return al(sizeof(FrameRes) * (size_t)frames) + al(sizeof(IterRecord) * (size_t)frames * log_cap) + al((size_t)runs);
@@ -226,7 +234,9 @@ struct TrackSolver {
     kba_batch* batch = nullptr;            // one capacity-shaped window per track; its raw arrays are filled by the gather kernels
     Staged<TrackDev> tdev;                 // [n] read at every solve: compaction re-points a track's arena
     Staged<TrackSel> tsel;
-    Staged<int> lists;                     // every selection list of a solve (keyframe slots, landmark slots, fixation bytes), ONE copy
+    Staged<int> lists;                     // the windows' solver options (BatchDev::wsp), then every selection list of a solve (keyframe
+                                           // slots, landmark slots, fixation bytes): ONE copy, from the lists on when the options are
+                                           // those the device holds
     std::unique_ptr<MotionBufs> motion;    // pose-only calls, allocated at the first one
     Transfer counts;                       // the last solve or pose-only call
     void release() {
@@ -591,7 +601,7 @@ static void key_append(std::vector<unsigned char>& k, const T& v) {
 }
 
 // (re)builds b->sg for the given kernel arguments; false = not possible here (b->sg.unusable is set, the caller takes the stream path)
-static bool build_solve_graph(kba_batch* b, const SolveParams& sp, const LaunchCfg& lc, int mode, int max_passes, int check_every,
+static bool build_solve_graph(kba_batch* b, const LaunchCfg& lc, int mode, int max_passes, int check_every,
                               const std::vector<unsigned char>& key) {
     kba_batch::SolveGraph& g = b->sg;
     g.destroy();
@@ -616,7 +626,7 @@ static bool build_solve_graph(kba_batch* b, const SolveParams& sp, const LaunchC
         if (e == cudaSuccess) e = cudaStreamBeginCaptureToGraph(s, np.conditional.phGraph_out[0], nullptr, nullptr, 0, cudaStreamCaptureModeThreadLocal);
         if (e == cudaSuccess) {
             capturing = true;
-            rc_pass = launch_pass(b->bd, sp, lc, &per, s);
+            rc_pass = launch_pass(b->bd, lc, &per, s);
             launch_loop_cond(b->bd, (unsigned long long)handle, b->loop_pass.d, max_passes, s);
             cudaGraph_t body = nullptr;
             e = cudaStreamEndCapture(s, &body);
@@ -627,7 +637,7 @@ static bool build_solve_graph(kba_batch* b, const SolveParams& sp, const LaunchC
         e = cudaStreamBeginCapture(s, cudaStreamCaptureModeThreadLocal);
         if (e == cudaSuccess) {
             capturing = true;
-            for (int i = 0; i < check_every && !rc_pass; ++i) rc_pass = launch_pass(b->bd, sp, lc, i == 0 ? &per : nullptr, s);
+            for (int i = 0; i < check_every && !rc_pass; ++i) rc_pass = launch_pass(b->bd, lc, i == 0 ? &per : nullptr, s);
             launch_count_active(b->bd, s);
             b->n_active.download(s);
             e = cudaStreamEndCapture(s, &g.graph);
@@ -867,7 +877,7 @@ static int batch_create(kba_handle* h, int32_t n_windows, const kba_window* w, c
         bad |= b->dev_alloc(&bd.chunk_poff, chunks); bad |= b->dev_alloc(&bd.chunk_rs, chunks);
     }
     bad |= b->dev_alloc(&bd.chunk_t0, chunks); bad |= b->dev_alloc(&bd.chunk_t1, chunks); bad |= b->dev_alloc(&bd.obs_row, obs);
-    bad |= b->state.alloc(n_windows, true); bad |= b->log.alloc((size_t)n_windows * kIterLogCap, true);
+    bad |= b->state.alloc(n_windows, true); bad |= b->log.alloc((size_t)n_windows * kIterLogCap, true); bad |= b->wsp.alloc(n_windows, true);
     for (int q = 0; q < 2; ++q) { bad |= b->pose_out[q].alloc(7 * kf, true); bad |= b->lm_out[q].alloc(3 * lm, hp); }
     bad |= b->lm_active.alloc(lm, hp); bad |= b->n_active.alloc(1, true); bad |= b->jac_obs.alloc(1, true);
     // device-only scratch
@@ -895,7 +905,7 @@ static int batch_create(kba_handle* h, int32_t n_windows, const kba_window* w, c
         b->release(); delete b;
         return fail(KBA_ERR_CUDA, msg);
     }
-    bd.desc = b->desc.d; bd.state = b->state.d; bd.log = b->log.d;
+    bd.desc = b->desc.d; bd.state = b->state.d; bd.log = b->log.d; bd.wsp = b->wsp.d;
     bd.pose0 = b->pose0.d; bd.plane0 = b->plane0.d; bd.pose[0] = b->pose_out[0].d; bd.pose[1] = b->pose_out[1].d;
     bd.kf_fixed = b->kf_fixed.d; bd.cam = b->cam.d;
     bd.lm0 = b->lm0.d; bd.lm[0] = b->lm_out[0].d; bd.lm[1] = b->lm_out[1].d; bd.lm_weight = b->lm_weight.d;
@@ -1045,6 +1055,7 @@ static int batch_upload(kba_batch* b, int32_t n_windows, const kba_window* w, co
 
 static SolveParams make_params(const kba_options* o) {
     SolveParams sp;
+    memset(&sp, 0, sizeof sp);
     sp.gp_huber = o->gp_huber; sp.gp_quantile = o->gp_quantile;
     sp.depth_thres = o->depth_thres; sp.reprojection_thres = o->reprojection_thres;
     sp.depth_quantile = o->depth_quantile; sp.reprojection_quantile = o->reprojection_quantile;
@@ -1056,32 +1067,99 @@ static SolveParams make_params(const kba_options* o) {
     sp.final_solver_iterations = o->final_solver_iterations; sp.min_residual_groups = o->min_residual_groups;
     sp.max_consecutive_invalid_steps = o->max_consecutive_invalid_steps;
     sp.max_solver_time = o->solver_time_sec;
+    sp.rounds_override = o->num_trim_rounds; sp.min_landmarks_for_trimming = o->min_landmarks_for_trimming;
+    sp.num_rounds_option = o->num_rounds_option;
     return sp;
 }
 
-static int batch_solve(kba_batch* b, const kba_options* opt);
-int kba_batch_solve(kba_batch* b, const kba_options* opt) {
-    const int rc = batch_solve(b, opt);
-    // a rank that fails leaves the collective solve: the in-process exchange releases the ranks waiting for it with an error
+// what the host derives from the options of a solve's windows
+struct SolveTotals {
+    int precision = 0;      // batch-wide: it selects the kernel variants
+    int max_passes = 0;     // pass cap of the solve, from the largest iteration counts
+    double time_cap = 0;    // host safety cap (seconds per inner solve), <= 0: none -- some window has no time limit
+};
+
+// Every check of a solve's options, before anything is uploaded.  opts[i] is unit i's (per_unit, n entries) or opts[0] every
+// unit's; live(i) false: unit i sits the solve out and its entry is not read.  Errors name the unit ("window 3: ...") when the
+// options are per unit.
+static int solve_options_check(int n, const kba_options* opts, bool per_unit, const char* unit, const std::function<bool(int)>& live,
+                               SolveTotals& tot, std::string& why) {
+    int first = -1, max_trim = 0, max_final = 0;
+    bool no_cap = false;
+    for (int i = 0; i < (per_unit ? n : 1); ++i) {
+        if (per_unit && !live(i)) continue;
+        const kba_options* o = &opts[i];
+        const std::string at = per_unit ? std::string(unit) + std::to_string(i) + ": " : std::string();
+        if (o->precision != 0 && o->precision != 1) { why = at + "kba_options.precision must be 0 (FP64) or 1 (FP32 linearisation)"; return KBA_ERR_BAD_ARG; }
+        if (first >= 0 && o->precision != opts[first].precision) {
+            why = at + "kba_options.precision differs from " + unit + std::to_string(first) + "'s: the precision is the same for the whole batch";
+            return KBA_ERR_BAD_ARG;
+        }
+        if (o->num_trim_rounds > 6 || (o->num_trim_rounds < 0 && o->num_rounds_option > 6)) {
+            why = at + "at most 6 trimming rounds (KBA_MAX_SOLVES = 8 inner solves incl. one retry and the final solve)";
+            return KBA_ERR_CAPACITY;
+        }
+        if (first < 0) { first = i; tot.precision = o->precision; tot.time_cap = o->solver_time_sec; }
+        max_trim = std::max(max_trim, o->trim_solver_iterations); max_final = std::max(max_final, o->final_solver_iterations);
+        no_cap |= !(o->solver_time_sec > 0);
+        tot.time_cap = std::max(tot.time_cap, o->solver_time_sec);
+    }
+    // upper bound on passes: every solve needs (iterations + 2) passes, plus one pass per trimming step
+    const int rounds_max = 7;
+    tot.max_passes = rounds_max * (3 * max_trim + 4) + max_final + 8;
+    if (no_cap) tot.time_cap = 0;
+    return KBA_OK;
+}
+
+// The device options of every window of b into sp[0 .. n_win): opts[i] (per_window) or opts[0]; a window that sits the solve out
+// keeps what the device holds (its entry is not read).  True when they differ from what the device holds, which b->wsp_dev then
+// records: the caller uploads them.
+static bool stage_params(kba_batch* b, bool per_window, const kba_options* opts, SolveParams* sp) {
+    const int n = b->bd.n_win;
+    const bool known = (int)b->wsp_dev.size() == n;
+    const SolveParams one = make_params(opts);
+    for (int i = 0; i < n; ++i) {
+        if (b->desc_h[i].idle) {
+            if (known) sp[i] = b->wsp_dev[i];
+            else memset(&sp[i], 0, sizeof(SolveParams));
+        } else {
+            sp[i] = per_window ? make_params(&opts[i]) : one;
+        }
+    }
+    if (known && memcmp(sp, b->wsp_dev.data(), sizeof(SolveParams) * n) == 0) return false;
+    b->wsp_dev.assign(sp, sp + n);
+    return true;
+}
+
+static int batch_run(kba_batch* b, const SolveTotals& tot);
+static int batch_solve(kba_batch* b, bool per_window, const kba_options* opts) {
+    if (!b || !opts) return fail(KBA_ERR_BAD_ARG, "bad argument to kba_batch_solve");
+    SolveTotals tot;
+    std::string why;
+    const int rc = solve_options_check(b->bd.n_win, opts, per_window, "window ", [b](int i) { return !b->desc_h[i].idle; }, tot, why);
+    if (rc != KBA_OK) return fail(rc, why);
+    CU(cudaSetDevice(b->h->device));
+    if (stage_params(b, per_window, opts, b->wsp.h)) CU(b->wsp.upload(b->h->stream));
+    return batch_run(b, tot);
+}
+
+// a rank that fails leaves the collective solve: the in-process exchange releases the ranks waiting for it with an error
+static int batch_solve_collective(kba_batch* b, bool per_window, const kba_options* opts) {
+    const int rc = batch_solve(b, per_window, opts);
     if (rc != KBA_OK && b && b->bd.sharded && b->lc.xchg.abort) b->lc.xchg.abort(b->lc.xchg.user);
     return rc;
 }
+int kba_batch_solve(kba_batch* b, const kba_options* opt) { return batch_solve_collective(b, false, opt); }
+int kba_batch_solve_opts(kba_batch* b, const kba_options* opts) { return batch_solve_collective(b, true, opts); }
 
-static int batch_solve(kba_batch* b, const kba_options* opt) {
-    if (!b || !opt) return fail(KBA_ERR_BAD_ARG, "bad argument to kba_batch_solve");
-    if (opt->precision != 0 && opt->precision != 1) return fail(KBA_ERR_BAD_ARG, "kba_options.precision must be 0 (FP64) or 1 (FP32 linearisation)");
-    if (opt->num_trim_rounds > 6 || (opt->num_trim_rounds < 0 && opt->num_rounds_option > 6))
-        return fail(KBA_ERR_CAPACITY, "at most 6 trimming rounds (KBA_MAX_SOLVES = 8 inner solves incl. one retry and the final solve)");
-    b->bd.precision = opt->precision;
-    b->bd.lin1 = (b->lc.plan.fused && b->lc.knobs.lin_fused && opt->precision == 0 && b->lc.max_rank == 0) ? 1 : 0;
+// the solve of batch b with its options on the device (BatchDev::wsp), checked and derived into tot
+static int batch_run(kba_batch* b, const SolveTotals& tot) {
+    b->bd.precision = tot.precision;
+    b->bd.lin1 = (b->lc.plan.fused && b->lc.knobs.lin_fused && tot.precision == 0 && b->lc.max_rank == 0) ? 1 : 0;
     kba_handle* h = b->h;
     CU(cudaSetDevice(h->device));
     cudaStream_t s = h->stream;
-    const SolveParams sp = make_params(opt);
     LaunchCfg lc = b->lc;
-    lc.rounds_override = opt->num_trim_rounds;
-    lc.min_landmarks_for_trimming = opt->min_landmarks_for_trimming;
-    lc.num_rounds_option = opt->num_rounds_option;
     lc.time_jacobian = h->kernel_timing;
     if (h->kernel_timing && h->ev_pool.empty()) {
         h->ev_pool.resize(1024);
@@ -1097,9 +1175,7 @@ static int batch_solve(kba_batch* b, const kba_options* opt) {
     CU(cudaEventRecord(b->ev_a, s));
     if (launch_shard_gather(b->bd, lc, s)) return KBA_ERR_NCCL;  // message set by the exchange
     launch_reset(b->bd, lc, s);
-    // upper bound on passes: every solve needs (iterations + 2) passes, plus one pass per trimming step
-    const int rounds_max = 7;
-    const int max_passes = rounds_max * (3 * opt->trim_solver_iterations + 4) + opt->final_solver_iterations + 8;
+    const int max_passes = tot.max_passes;
     const auto t0 = std::chrono::steady_clock::now();
     int check_every = 4;
     bool timed_out = false, poll_pending = false;
@@ -1114,11 +1190,11 @@ static int batch_solve(kba_batch* b, const kba_options* opt) {
     if (lockstep) gmode = (gmode && lc.xchg.capturable && shard_graph_enabled() && b->solves_done > 0) ? 1 : 0;
     if (gmode) {
         std::vector<unsigned char> key;
-        key.reserve(sizeof(BatchDev) + sizeof(SolveParams) + 64);
-        key_append(key, b->bd); key_append(key, sp); key_append(key, gmode); key_append(key, max_passes); key_append(key, s);
+        key.reserve(sizeof(BatchDev) + 64);
+        key_append(key, b->bd); key_append(key, gmode); key_append(key, max_passes); key_append(key, s);
         // the knobs are fixed at creation; the plan changes with uploads and track solves
         key_append(key, lc.plan); key_append(key, lc.max_rank); key_append(key, lc.xchg.user);
-        if (!(b->sg.exec && b->sg.key == key) && !build_solve_graph(b, sp, lc, gmode, max_passes, check_every, key)) gmode = 0;
+        if (!(b->sg.exec && b->sg.key == key) && !build_solve_graph(b, lc, gmode, max_passes, check_every, key)) gmode = 0;
     }
     if (gmode == 2) {
         CU(cudaMemsetAsync(b->loop_pass.d, 0, sizeof(int), s));
@@ -1149,9 +1225,9 @@ static int batch_solve(kba_batch* b, const kba_options* opt) {
             } else if (g >= 1) {  // the count of the previous launch is read while this one runs (the device never waits for the host)
                 CU(wait_event(h, evs[(g - 1) & 1]));
                 if (b->n_active.h[0] == 0) break;
-                if (opt->solver_time_sec > 0) {
+                if (tot.time_cap > 0) {
                     const double el = std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
-                    if (el > KBA_MAX_SOLVES * opt->solver_time_sec + 2.0) { timed_out = true; break; }
+                    if (el > KBA_MAX_SOLVES * tot.time_cap + 2.0) { timed_out = true; break; }
                 }
             }
         }
@@ -1168,7 +1244,7 @@ static int batch_solve(kba_batch* b, const kba_options* opt) {
         return KBA_OK;
     }
     for (int pass = 0; pass < max_passes; ++pass) {
-        if (launch_pass(b->bd, sp, lc, &h->counters, s)) {  // message set by the exchange
+        if (launch_pass(b->bd, lc, &h->counters, s)) {  // message set by the exchange
             cudaEventRecord(b->ev_b, s);
             return KBA_ERR_NCCL;
         }
@@ -1186,9 +1262,9 @@ static int batch_solve(kba_batch* b, const kba_options* opt) {
                 CU(wait_event(h, b->ev_poll));
                 poll_pending = false;
                 if (b->n_active.h[0] == 0) break;
-                if (opt->solver_time_sec > 0 && !b->bd.sharded) {  // host safety cap, see below
+                if (tot.time_cap > 0 && !b->bd.sharded) {  // host safety cap, see below
                     const double el = std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
-                    if (el > KBA_MAX_SOLVES * opt->solver_time_sec + 2.0) { timed_out = true; break; }
+                    if (el > KBA_MAX_SOLVES * tot.time_cap + 2.0) { timed_out = true; break; }
                 }
             }
             launch_count_active(b->bd, s);
@@ -1356,13 +1432,13 @@ int kba_batch_jacobian_pass(kba_batch* b, const kba_options* opt, int32_t repeat
     if (!b || !opt || repeats < 1) return fail(KBA_ERR_BAD_ARG, "bad argument to kba_batch_jacobian_pass");
     kba_handle* h = b->h;
     cudaStream_t s = h->stream;
-    const SolveParams sp = make_params(opt);
     if (opt->precision != 0 && opt->precision != 1) return fail(KBA_ERR_BAD_ARG, "kba_options.precision must be 0 or 1");
     b->bd.precision = opt->precision;
+    if (stage_params(b, false, opt, b->wsp.h)) CU(b->wsp.upload(s));
     launch_reset(b->bd, b->lc, s);
     launch_force_linearize(b->bd, s);
     CU(cudaEventRecord(b->ev_a, s));
-    for (int i = 0; i < repeats; ++i) launch_jacobian_only(b->bd, sp, s);
+    for (int i = 0; i < repeats; ++i) launch_jacobian_only(b->bd, s);
     CU(cudaEventRecord(b->ev_b, s));
     CU(cudaStreamSynchronize(s));
     CU(cudaGetLastError());
@@ -1376,15 +1452,26 @@ int kba_batch_jacobian_pass(kba_batch* b, const kba_options* opt, int32_t repeat
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
-int kba_solve_batch(kba_handle* h, int32_t n_windows, const kba_window* w, const kba_options* opt, kba_result* res) {
-    if (!h || !w || !opt || !res) return fail(KBA_ERR_BAD_ARG, "null argument to kba_solve_batch");
+static int solve_batch(kba_handle* h, int32_t n_windows, const kba_window* w, bool per_window, const kba_options* opts, kba_result* res) {
+    if (!h || !w || !opts || !res) return fail(KBA_ERR_BAD_ARG, "null argument to kba_solve_batch");
+    SolveTotals tot;
+    std::string why;
+    int rc = solve_options_check(n_windows, opts, per_window, "window ", [](int) { return true; }, tot, why);
+    if (rc != KBA_OK) return fail(rc, why);
     kba_batch* b = nullptr;
-    int rc = kba_batch_create(h, n_windows, w, &b);
+    rc = kba_batch_create(h, n_windows, w, &b);
     if (rc != KBA_OK) return rc;
-    rc = kba_batch_solve(b, opt);
+    rc = batch_solve(b, per_window, opts);
     if (rc == KBA_OK) rc = kba_batch_download(b, res);
     kba_batch_destroy(b);
     return rc;
+}
+
+int kba_solve_batch(kba_handle* h, int32_t n_windows, const kba_window* w, const kba_options* opt, kba_result* res) {
+    return solve_batch(h, n_windows, w, false, opt, res);
+}
+int kba_solve_batch_opts(kba_handle* h, int32_t n_windows, const kba_window* w, const kba_options* opts, kba_result* res) {
+    return solve_batch(h, n_windows, w, true, opts, res);
 }
 
 int kba_solve_window(kba_handle* h, const kba_window* w, const kba_options* opt, kba_result* res) {
@@ -1620,13 +1707,19 @@ static TrackSel track_sel(const TrackRequest& q, const int* kf_slot_d, const uin
     return ts;
 }
 
+// ints at the front of TrackSolver::lists that hold the options of n windows
+static size_t params_ints(int n) {
+    static_assert(sizeof(SolveParams) % 8 == 0, "the lists after the options stay 8-byte aligned");
+    return (size_t)n * sizeof(SolveParams) / sizeof(int);
+}
+
 // the solver of tracks ts[0..n): one capacity window per track, so its batch has room for every window a track's caps allow on
 // the fused path (large = false) or on the large-window path.  On failure everything it allocated is freed again.
 static int track_solver_create(kba_handle* h, int n, kba_track* const* ts, bool large, TrackSolver& sv, const std::string& who) {
     std::vector<std::unique_ptr<CapacityWindow>> cws;
     std::vector<kba_window> ws;
     std::vector<int> rows;
-    size_t list_ints = 0;
+    size_t list_ints = params_ints(n);
     for (int i = 0; i < n; ++i) {
         const kba_track* t = ts[i];
         cws.emplace_back(new CapacityWindow(t->caps, large, t->n_cam, t->cam_intr.data(), t->cam_pose.data()));
@@ -1640,6 +1733,7 @@ static int track_solver_create(kba_handle* h, int n, kba_track* const* ts, bool 
     int bad = 0;
     bad |= sv.tdev.alloc(n, true); bad |= sv.tsel.alloc(n, true); bad |= sv.lists.alloc(list_ints, true);
     if (bad) { sv.release(); return fail(KBA_ERR_CUDA, who + ": out of memory"); }
+    sv.batch->bd.wsp = reinterpret_cast<const SolveParams*>(sv.lists.d);  // the options travel with the lists
     return KBA_OK;
 }
 
@@ -1812,8 +1906,8 @@ int kba_track_set_landmarks(kba_track* t, int32_t n, const int32_t* slot, const 
 
 // one solve of the stored windows of tracks ts[0..n) as one batch, window i = ts[i]'s; qs[i] is checked by track_check or sits
 // the solve out (sel == nullptr).  kba_track_solve (n = 1) and kba_track_group_solve.
-static int track_solve(kba_handle* h, TrackSolver& sv, int n, kba_track* const* ts, const TrackRequest* qs, const kba_options* opt,
-                       kba_result* res) {
+static int track_solve(kba_handle* h, TrackSolver& sv, int n, kba_track* const* ts, const TrackRequest* qs, bool per_track,
+                       const kba_options* opts, const SolveTotals& tot, kba_result* res) {
     kba_batch* b = sv.batch;
     CU(cudaSetDevice(h->device));
     cudaStream_t s = h->stream;
@@ -1822,7 +1916,8 @@ static int track_solve(kba_handle* h, TrackSolver& sv, int n, kba_track* const* 
     std::vector<WinShape> solved(n);       // rows and chunks of the solved windows (large-window path)
     bool any_gp = false;
     TrackGrid grid;
-    size_t used = 0;
+    const size_t p_ints = params_ints(n);
+    size_t used = p_ints;
     int64_t h2d = (int64_t)n * (int64_t)(sizeof(WinDesc) + sizeof(TrackDev) + sizeof(TrackSel));
     for (int i = 0; i < n; ++i) {
         const kba_track* t = ts[i];
@@ -1876,8 +1971,11 @@ static int track_solve(kba_handle* h, TrackSolver& sv, int n, kba_track* const* 
         for (int i = 0; i < n; ++i) b->desc.h[i].nr_cap = b->desc_h[i].nr_cap = nr_cap_of(solved[i].rows);
         apply_plan(b);
     }
+    // the options go up in the lists' copy when they differ from what the device holds (a re-solve with the same ones: none)
+    const size_t from = stage_params(b, per_track, opts, reinterpret_cast<SolveParams*>(sv.lists.h)) ? 0 : p_ints;
+    h2d += (int64_t)((p_ints - from) * sizeof(int));
     CU(b->desc.upload(s));
-    CU(cudaMemcpyAsync(sv.lists.d, sv.lists.h, used * sizeof(int), cudaMemcpyHostToDevice, s));
+    CU(cudaMemcpyAsync(sv.lists.d + from, sv.lists.h + from, (used - from) * sizeof(int), cudaMemcpyHostToDevice, s));
     CU(sv.tdev.upload(s)); CU(sv.tsel.upload(s));
     if (any_gp) { CU(b->r_gp_lm.upload(s)); CU(b->gp_kf.upload(s)); CU(b->gp_weight.upload(s)); }
     sv.counts.h2d = h2d;
@@ -1885,7 +1983,7 @@ static int track_solve(kba_handle* h, TrackSolver& sv, int n, kba_track* const* 
     launch_track_gather(b->bd, b->raw, sv.tdev.d, sv.tsel.d, grid, s);
     launch_pack(b->bd, b->raw, s);
     CU(cudaGetLastError());
-    int rc = kba_batch_solve(b, opt);
+    int rc = batch_run(b, tot);
     if (rc != KBA_OK) return rc;
     launch_track_writeback(b->bd, sv.tdev.d, sv.tsel.d, grid, s);
     rc = kba_batch_download(b, res);
@@ -1918,9 +2016,14 @@ static std::string track_prefix(bool group, int i) { return group ? "track " + s
 // order before anything is uploaded or launched; in a group, one with n_kf == 0 sits the solve out.  The solver is the one
 // kba_batch_create would choose for the whole batch: the large-window path as soon as one window needs more than kFusedMaxRows
 // reduced rows.
-static int set_solve(TrackSet& s, bool group, const std::string& who, TrackRequest* qs, const kba_options* opt, kba_result* res) {
+static int set_solve(TrackSet& s, bool group, const std::string& who, TrackRequest* qs, bool per_track, const kba_options* opts,
+                     kba_result* res) {
     const int n = (int)s.tracks.size();
     bool any = false, large = false;
+    SolveTotals tot;
+    std::string owhy;
+    const int orc = solve_options_check(n, opts, per_track, "track ", [&](int i) { return !(group && qs[i].n_kf == 0); }, tot, owhy);
+    if (orc != KBA_OK) return fail(orc, who + owhy);
     for (int i = 0; i < n; ++i) {
         TrackRequest& q = qs[i];
         if (group && q.n_kf == 0) { q.sel = nullptr; continue; }  // sits this solve out
@@ -1937,7 +2040,7 @@ static int set_solve(TrackSet& s, bool group, const std::string& who, TrackReque
     }
     TrackSolver& sv = large ? s.large : s.solver;
     s.last = &sv.counts;
-    return track_solve(s.h, sv, n, s.tracks.data(), qs, opt, res);
+    return track_solve(s.h, sv, n, s.tracks.data(), qs, per_track, opts, tot, res);
 }
 
 static TrackRequest track_request(int32_t n_kf, const int32_t* kf_slot, const uint8_t* kf_fixed, int32_t n_lm, const int32_t* lm_slot,
@@ -1951,7 +2054,7 @@ int kba_track_solve(kba_track* t, int32_t n_kf, const int32_t* kf_slot, const ui
                     const kba_window* sel, const kba_options* opt, kba_result* res) {
     if (!t || !opt || !res) return fail(KBA_ERR_BAD_ARG, "null argument to kba_track_solve");
     TrackRequest q = track_request(n_kf, kf_slot, kf_fixed, n_lm, lm_slot, sel, false);
-    return set_solve(t->set, false, "kba_track_solve: ", &q, opt, res);
+    return set_solve(t->set, false, "kba_track_solve: ", &q, false, opt, res);
 }
 
 int kba_track_transfer_bytes(kba_track* t, int64_t* h2d, int64_t* d2h, int64_t* push) {
@@ -1993,12 +2096,19 @@ int kba_track_group_create(kba_handle* h, int32_t n_tracks, kba_track* const* tr
     return KBA_OK;
 }
 
-int kba_track_group_solve(kba_track_group* g, const kba_track_request* req, const kba_options* opt, kba_result* res) {
-    if (!g || !req || !opt || !res) return fail(KBA_ERR_BAD_ARG, "null argument to kba_track_group_solve");
+static int group_solve(kba_track_group* g, const kba_track_request* req, bool per_track, const kba_options* opts, kba_result* res,
+                       const std::string& who) {
+    if (!g || !req || !opts || !res) return fail(KBA_ERR_BAD_ARG, "null argument to " + who.substr(0, who.size() - 2));
     std::vector<TrackRequest> qs;
     for (size_t i = 0; i < g->set.tracks.size(); ++i)
         qs.push_back(track_request(req[i].n_kf, req[i].kf_slot, req[i].kf_fixed, req[i].n_lm, req[i].lm_slot, req[i].sel, false));
-    return set_solve(g->set, true, "kba_track_group_solve: ", qs.data(), opt, res);
+    return set_solve(g->set, true, who, qs.data(), per_track, opts, res);
+}
+int kba_track_group_solve(kba_track_group* g, const kba_track_request* req, const kba_options* opt, kba_result* res) {
+    return group_solve(g, req, false, opt, res, "kba_track_group_solve: ");
+}
+int kba_track_group_solve_opts(kba_track_group* g, const kba_track_request* req, const kba_options* opts, kba_result* res) {
+    return group_solve(g, req, true, opts, res, "kba_track_group_solve_opts: ");
 }
 
 int kba_track_group_transfer_bytes(kba_track_group* g, int64_t* h2d, int64_t* d2h) {
@@ -2958,9 +3068,10 @@ static int options_check(const kba_options* opt, std::string& why) {
     return KBA_OK;
 }
 
-// frames f[i] of tracks ts[i] (already checked; runs[i] landmarks, rounds[i] trimming rounds; n_meas == 0: idle) as one launch
+// frames f[i] of tracks ts[i] (already checked; runs[i] landmarks, rounds[i] trimming rounds; n_meas == 0: idle) as one launch;
+// opts[i] (per_frame) or opts[0] are their options
 static int adjust_pose_run(kba_handle* h, MotionBufs& mb, int n, kba_track* const* ts, const kba_track_frame* f, const int* runs,
-                           const int* rounds, const kba_options* opt, kba_result* res, Transfer& tr) {
+                           const int* rounds, bool per_frame, const kba_options* opts, kba_result* res, Transfer& tr) {
     std::vector<int> live;
     int M = 0, Rn = 0, log_cap = 0;
     bool any_cam = false;
@@ -2976,10 +3087,11 @@ static int adjust_pose_run(kba_handle* h, MotionBufs& mb, int n, kba_track* cons
     if (nf == 0) return KBA_OK;
     CU(cudaSetDevice(h->device));
     cudaStream_t s = h->stream;
-    // ---- staged upload: descriptors | run starts | slots | cameras | u | v | d
+    // ---- staged upload: descriptors | options | run starts | slots | cameras | u | v | d
     unsigned char* base = mb.up.h;
     FrameDesc* fd = reinterpret_cast<FrameDesc*>(base);
     size_t off = MotionBufs::al(sizeof(FrameDesc) * (size_t)nf);
+    SolveParams* sp = reinterpret_cast<SolveParams*>(base + off); const size_t o_sp = off; off += MotionBufs::al(sizeof(SolveParams) * (size_t)nf);
     int* rs = reinterpret_cast<int*>(base + off); const size_t o_rs = off; off += MotionBufs::al(4 * ((size_t)Rn + nf));
     const size_t o_lm = off; off += MotionBufs::al(4 * (size_t)M);
     const size_t o_cam = off; if (any_cam) off += MotionBufs::al(4 * (size_t)M);
@@ -2993,6 +3105,7 @@ static int adjust_pose_run(kba_handle* h, MotionBufs& mb, int n, kba_track* cons
         const kba_track* t = ts[i];
         FrameDesc& d = fd[q];
         d.n_meas = F.n_meas; d.n_runs = runs[i]; d.meas_off = mo; d.run_off = ro; d.rs_off = rso; d.rounds_total = rounds[i];
+        sp[q] = make_params(&opts[per_frame ? i : 0]);
         d.lm_pos = t->td.lm_pos; d.lm_weight = t->td.lm_weight;
         d.cam16 = t->set.solver.batch->bd.cam + (size_t)t->set.solver.batch->desc_h[0].cam_off * kCamStride; d.n_cam = t->n_cam; d.pad = 0;
         memcpy(d.pose7, F.pose7, sizeof(d.pose7));
@@ -3016,6 +3129,7 @@ static int adjust_pose_run(kba_handle* h, MotionBufs& mb, int n, kba_track* cons
     unsigned char* dev = mb.up.d;
     MotionArgs a;
     a.fd = reinterpret_cast<const FrameDesc*>(dev);
+    a.sp = reinterpret_cast<const SolveParams*>(dev + o_sp);
     a.run_start = reinterpret_cast<const int*>(dev + o_rs);
     a.lm_slot = reinterpret_cast<const int*>(dev + o_lm);
     a.cam = any_cam ? reinterpret_cast<const int*>(dev + o_cam) : nullptr;
@@ -3033,7 +3147,7 @@ static int adjust_pose_run(kba_handle* h, MotionBufs& mb, int n, kba_track* cons
     // ---- one upload, one launch, one download, one synchronisation
     CU(cudaMemcpyAsync(mb.up.d, mb.up.h, off, cudaMemcpyHostToDevice, s));
     CU(cudaEventRecord(mb.ev0, s));
-    launch_adjust_pose(a, nf, make_params(opt), s);
+    launch_adjust_pose(a, nf, s);
     CU(cudaEventRecord(mb.ev1, s));
     CU(cudaMemcpyAsync(mb.out.h, mb.out.d, n_out, cudaMemcpyDeviceToHost, s));
     CU(wait_stream(h));
@@ -3091,34 +3205,43 @@ static int motion_alloc(std::unique_ptr<MotionBufs>& mb, int n, kba_track* const
 
 // a pose-only call of a track (group = false) or of a group: the options and every frame are checked before anything is uploaded
 // or launched.  Errors start with `who`; a group's name the failing track.
-static int track_adjust_pose(TrackSet& s, bool group, const std::string& who, const kba_track_frame* f, const kba_options* opt,
-                             kba_result* res) {
+static int track_adjust_pose(TrackSet& s, bool group, const std::string& who, const kba_track_frame* f, bool per_frame,
+                             const kba_options* opts, kba_result* res) {
     TrackSolver& sv = s.solver;
     s.last = &sv.counts;
     std::string why;
-    int rc = options_check(opt, why);
-    if (rc != KBA_OK) return fail(rc, who + why);
-    CU(cudaSetDevice(s.h->device));
     const int n = (int)s.tracks.size();
+    int rc = KBA_OK;
+    for (int i = 0; i < (per_frame ? n : 1); ++i) {
+        if (per_frame && f[i].n_meas == 0) continue;  // a frame that sits the call out: its entry is not read
+        rc = options_check(&opts[i], why);
+        if (rc != KBA_OK) return fail(rc, who + (per_frame ? track_prefix(true, i) : std::string()) + why);
+    }
+    CU(cudaSetDevice(s.h->device));
     rc = motion_alloc(sv.motion, n, s.tracks.data());
     if (rc != KBA_OK) return rc;
     std::vector<int> runs(n, 0), rounds(n, 0);
     for (int i = 0; i < n; ++i) {
         if (f[i].n_meas == 0) continue;
-        rc = frame_check(s.tracks[i], &f[i], opt, runs[i], rounds[i], why);
+        rc = frame_check(s.tracks[i], &f[i], &opts[per_frame ? i : 0], runs[i], rounds[i], why);
         if (rc != KBA_OK) return fail(rc, who + track_prefix(group, i) + why);
     }
-    return adjust_pose_run(s.h, *sv.motion, n, s.tracks.data(), f, runs.data(), rounds.data(), opt, res, sv.counts);
+    return adjust_pose_run(s.h, *sv.motion, n, s.tracks.data(), f, runs.data(), rounds.data(), per_frame, opts, res, sv.counts);
 }
 
 int kba_track_adjust_pose(kba_track* t, const kba_track_frame* f, const kba_options* opt, kba_result* res) {
     if (!t || !f || !opt || !res) return fail(KBA_ERR_BAD_ARG, "null argument to kba_track_adjust_pose");
-    return track_adjust_pose(t->set, false, "kba_track_adjust_pose: ", f, opt, res);
+    return track_adjust_pose(t->set, false, "kba_track_adjust_pose: ", f, false, opt, res);
 }
 
 int kba_track_group_adjust_pose(kba_track_group* g, const kba_track_frame* f, const kba_options* opt, kba_result* res) {
     if (!g || !f || !opt || !res) return fail(KBA_ERR_BAD_ARG, "null argument to kba_track_group_adjust_pose");
-    return track_adjust_pose(g->set, true, "kba_track_group_adjust_pose: ", f, opt, res);
+    return track_adjust_pose(g->set, true, "kba_track_group_adjust_pose: ", f, false, opt, res);
+}
+
+int kba_track_group_adjust_pose_opts(kba_track_group* g, const kba_track_frame* f, const kba_options* opts, kba_result* res) {
+    if (!g || !f || !opts || !res) return fail(KBA_ERR_BAD_ARG, "null argument to kba_track_group_adjust_pose_opts");
+    return track_adjust_pose(g->set, true, "kba_track_group_adjust_pose_opts: ", f, true, opts, res);
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
@@ -3357,15 +3480,22 @@ int kba_track_solve_ranked(kba_track* t, int32_t n_kf, const int32_t* kf_slot, c
                            const kba_options* opt, kba_result* res) {
     if (!t || !opt || !res) return fail(KBA_ERR_BAD_ARG, "null argument to kba_track_solve_ranked");
     TrackRequest q = track_request(n_kf, kf_slot, kf_fixed, 0, nullptr, sel, true);
-    return set_solve(t->set, false, "kba_track_solve_ranked: ", &q, opt, res);
+    return set_solve(t->set, false, "kba_track_solve_ranked: ", &q, false, opt, res);
 }
 
-int kba_track_group_solve_ranked(kba_track_group* g, const kba_ranked_request* req, const kba_options* opt, kba_result* res) {
-    if (!g || !req || !opt || !res) return fail(KBA_ERR_BAD_ARG, "null argument to kba_track_group_solve_ranked");
+static int group_solve_ranked(kba_track_group* g, const kba_ranked_request* req, bool per_track, const kba_options* opts,
+                              kba_result* res, const std::string& who) {
+    if (!g || !req || !opts || !res) return fail(KBA_ERR_BAD_ARG, "null argument to " + who.substr(0, who.size() - 2));
     std::vector<TrackRequest> qs;
     for (size_t i = 0; i < g->set.tracks.size(); ++i)
         qs.push_back(track_request(req[i].n_kf, req[i].kf_slot, req[i].kf_fixed, 0, nullptr, req[i].sel, true));
-    return set_solve(g->set, true, "kba_track_group_solve_ranked: ", qs.data(), opt, res);
+    return set_solve(g->set, true, who, qs.data(), per_track, opts, res);
+}
+int kba_track_group_solve_ranked(kba_track_group* g, const kba_ranked_request* req, const kba_options* opt, kba_result* res) {
+    return group_solve_ranked(g, req, false, opt, res, "kba_track_group_solve_ranked: ");
+}
+int kba_track_group_solve_ranked_opts(kba_track_group* g, const kba_ranked_request* req, const kba_options* opts, kba_result* res) {
+    return group_solve_ranked(g, req, true, opts, res, "kba_track_group_solve_ranked_opts: ");
 }
 
 }  // extern "C"

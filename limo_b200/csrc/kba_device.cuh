@@ -82,6 +82,7 @@ struct WinState {
 };
 
 // ---- batch-flat device arrays --------------------------------------------------------------------------------------------
+struct SolveParams;
 struct BatchDev {
     int n_win;
     int max_obs, max_lm, max_kf, max_gp;   // maxima over the batch (grid sizing)
@@ -223,15 +224,21 @@ struct BatchDev {
                               //   gp residuals (55, lower-packed by rows) + the 10 gradient entries (k_gp_blocks)
     double* gp_cost_x;        // [n_win] robustified cost of the gp blocks at x / at the candidate (fixed-order sums)
     double* gp_cost_c;
+    const SolveParams* wsp;   // [n_win] solver options of each window (every pass kernel reads its window's entry)
 };
 
-struct SolveParams {  // kba_options subset used on the device
+// kba_options subset used on the device, one per window (BatchDev::wsp) or per frame (MotionArgs::sp).  The host compares the
+// bytes with what the device holds, so every byte is a field (no padding).
+struct SolveParams {
     double gp_huber, gp_quantile;
     double depth_thres, reprojection_thres, depth_quantile, reprojection_quantile;
     double function_tolerance, gradient_tolerance, parameter_tolerance;
     double initial_radius, max_radius, min_radius, min_relative_decrease, min_lm_diagonal, max_lm_diagonal;
     int trim_solver_iterations, final_solver_iterations, min_residual_groups, max_consecutive_invalid_steps;
     double max_solver_time;  // seconds per inner solve (ceres max_solver_time_in_seconds), <= 0: none
+    // trimming rounds (k_reset_state): num_trim_rounds, or -1 = num_rounds_option iff the window has more than
+    // min_landmarks_for_trimming landmarks
+    int rounds_override, min_landmarks_for_trimming, num_rounds_option, pad_;
 };
 
 __device__ __forceinline__ unsigned long long global_timer_ns() {

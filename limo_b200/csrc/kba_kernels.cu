@@ -48,8 +48,9 @@ __global__ void __launch_bounds__(256) k_shard_planes(BatchDev bd) {
 // 1024 threads: the layout tables of a solve's first pass are dependent-load chains per landmark / observation, and a trimmed
 // solve begins three to four times
 constexpr int kBeginThreads = 1024;
-__global__ void __launch_bounds__(kBeginThreads) k_solve_begin(BatchDev bd, SolveParams sp) {
+__global__ void __launch_bounds__(kBeginThreads) k_solve_begin(BatchDev bd) {
     const int w = blockIdx.x;
+    const SolveParams& sp = bd.wsp[w];
     WinState& st = bd.state[w];
     if (st.phase != PH_SOLVE_BEGIN) return;
     const WinDesc wd = bd.desc[w];
@@ -242,7 +243,7 @@ __global__ void __launch_bounds__(256) k_panel_zero(BatchDev bd) {
 // Algorithmic HBM bytes per observation (FP64, with depth row): 20 read + 240 written (DESIGN.md).
 // =====================================================================================================================
 template <bool kJac, int kMinBlocks, typename TLin, bool kJl = true>
-__global__ void __launch_bounds__(256, kMinBlocks) k_eval_obs(BatchDev bd, SolveParams sp, int tiles) {
+__global__ void __launch_bounds__(256, kMinBlocks) k_eval_obs(BatchDev bd, int tiles) {
     // A CTA walks `tiles` consecutive 256-observation tiles of one window with a two-deep software pipeline: while tile
     // t is evaluated, the measurement / landmark loads of tile t+1 and the landmark-index load of tile t+2 are in
     // flight, so the dependent chain index -> landmark is hidden; the keyframe poses are staged once per CTA.
@@ -258,6 +259,7 @@ __global__ void __launch_bounds__(256, kMinBlocks) k_eval_obs(BatchDev bd, Solve
     __shared__ __align__(8) uint64_t s_bar;
     __shared__ double s_red[8];
     __shared__ int s_cnt[8];
+    __shared__ double s_b[2];  // the window's squared Cauchy scales (reprojection, depth), published by the staging barrier
     constexpr bool kF32 = sizeof(TLin) == 4;  // FP32 evaluation + storage of the linearisation (precision 1)
     __shared__ float s_pose_f[kF32 ? kMaxKf * kPoseStride : 1];
     __shared__ float s_cam_f[kF32 ? kMaxCam * kCamStride : 1];
@@ -280,6 +282,10 @@ __global__ void __launch_bounds__(256, kMinBlocks) k_eval_obs(BatchDev bd, Solve
         p0 = lm_buf[3 * (size_t)L]; p1 = lm_buf[3 * (size_t)L + 1]; p2 = lm_buf[3 * (size_t)L + 2];
         wgt = bd.lm_weight[L];
         act = bd.lm_active[L];
+    }
+    if (threadIdx.x == 0) {
+        const SolveParams& sp = bd.wsp[w];
+        s_b[0] = sp.reprojection_thres * sp.reprojection_thres; s_b[1] = sp.depth_thres * sp.depth_thres;
     }
     stage_window_bulk(wd, bd.rt[buf], bd.cam, s_pose, s_cam, &s_bar);  // poses (R | t) and cameras: two bulk copies
     if (kF32) {
@@ -320,8 +326,7 @@ __global__ void __launch_bounds__(256, kMinBlocks) k_eval_obs(BatchDev bd, Solve
                 double r[3], raw[2];
                 ok = eval_observation<double, false>(
                     s_pose + kPoseStride * k, s_cam + kCamStride * c, p, (double)u, (double)v, (double)d, wgt,
-                    sp.reprojection_thres * sp.reprojection_thres, sp.depth_thres * sp.depth_thres, r, nullptr, nullptr, hr,
-                    raw);
+                    s_b[0], s_b[1], r, nullptr, nullptr, hr, raw);
                 if (ok) {
                     const float pf[3] = {(float)p0, (float)p1, (float)p2};
                     float hrf;
@@ -330,20 +335,19 @@ __global__ void __launch_bounds__(256, kMinBlocks) k_eval_obs(BatchDev bd, Solve
                     float* jlf = reinterpret_cast<float*>(bd.jl) + o;
                     eval_observation_store<float, kJl>(
                         s_pose_f + kPoseStride * k, s_cam_f + kCamStride * c, pf, u, v, d, (float)wgt,
-                        (float)(sp.reprojection_thres * sp.reprojection_thres), (float)(sp.depth_thres * sp.depth_thres),
+                        (float)s_b[0], (float)s_b[1],
                         resf, jpf, jlf, (size_t)bd.tot_obs, row >= 0 || !kJl, hrf);
                 }
             } else if (kJac) {  // rows are stored to their SoA slots as they are formed
                 ok = eval_observation_store<double, kJl>(
                     s_pose + kPoseStride * k, s_cam + kCamStride * c, p, (double)u, (double)v, (double)d, wgt,
-                    sp.reprojection_thres * sp.reprojection_thres, sp.depth_thres * sp.depth_thres, bd.res + o, bd.jp + o,
+                    s_b[0], s_b[1], bd.res + o, bd.jp + o,
                     bd.jl + o, (size_t)bd.tot_obs, row >= 0 || !kJl, hr);
             } else {
                 double r[3], raw[2];
                 ok = eval_observation<double, false>(
                     s_pose + kPoseStride * k, s_cam + kCamStride * c, p, (double)u, (double)v, (double)d, wgt,
-                    sp.reprojection_thres * sp.reprojection_thres, sp.depth_thres * sp.depth_thres, r, nullptr, nullptr,
-                    hr, raw);
+                    s_b[0], s_b[1], r, nullptr, nullptr, hr, raw);
             }
             if (!ok) {
                 st.eval_failed = 1;  // benign race
@@ -375,16 +379,16 @@ __global__ void __launch_bounds__(256, kMinBlocks) k_eval_obs(BatchDev bd, Solve
 // 8 tiles per CTA; two CTAs per SM for the linearisation, four for the cost.  The cost slots a CTA writes follow the tile count.
 constexpr int kEvalTiles = 8;
 template <bool kJac>
-static void launch_eval_obs(const BatchDev& bd, const SolveParams& sp, cudaStream_t s) {
+static void launch_eval_obs(const BatchDev& bd, cudaStream_t s) {
     const dim3 g((bd.max_obs + 256 * kEvalTiles - 1) / (256 * kEvalTiles), bd.n_win);
-    if (!kJac) { k_eval_obs<false, 4, double><<<g, 256, 0, s>>>(bd, sp, kEvalTiles); return; }
+    if (!kJac) { k_eval_obs<false, 4, double><<<g, 256, 0, s>>>(bd, kEvalTiles); return; }
     // fused path (kJl = false): J_l is not materialised, its consumers form it as (translation columns of J_p) R
     if (bd.precision == 1) {
-        if (bd.fused) k_eval_obs<true, 2, float, false><<<g, 256, 0, s>>>(bd, sp, kEvalTiles);
-        else k_eval_obs<true, 2, float, true><<<g, 256, 0, s>>>(bd, sp, kEvalTiles);
+        if (bd.fused) k_eval_obs<true, 2, float, false><<<g, 256, 0, s>>>(bd, kEvalTiles);
+        else k_eval_obs<true, 2, float, true><<<g, 256, 0, s>>>(bd, kEvalTiles);
     } else {
-        if (bd.fused) k_eval_obs<true, 2, double, false><<<g, 256, 0, s>>>(bd, sp, kEvalTiles);
-        else k_eval_obs<true, 2, double, true><<<g, 256, 0, s>>>(bd, sp, kEvalTiles);
+        if (bd.fused) k_eval_obs<true, 2, double, false><<<g, 256, 0, s>>>(bd, kEvalTiles);
+        else k_eval_obs<true, 2, double, true><<<g, 256, 0, s>>>(bd, kEvalTiles);
     }
     LCHK("k_eval_obs");
 }
@@ -396,7 +400,7 @@ static void launch_eval_obs(const BatchDev& bd, const SolveParams& sp, cudaStrea
 //   else: cost at the candidate
 // =====================================================================================================================
 template <bool kJac>
-__global__ void __launch_bounds__(256) k_gp_eval(BatchDev bd, SolveParams sp) {
+__global__ void __launch_bounds__(256) k_gp_eval(BatchDev bd) {
     const int w = blockIdx.x;
     const WinState& st = bd.state[w];
     if (st.phase != PH_ITERATE) return;
@@ -423,7 +427,7 @@ __global__ void __launch_bounds__(256) k_gp_eval(BatchDev bd, SolveParams sp) {
         const double px[3] = {a[0] + ps[4], a[1] + ps[5], a[2] + ps[6]};
         const double n[3] = {pl[0], pl[1], pl[2]};
         const double r = n[0] * px[0] + n[1] * px[1] + n[2] * px[2] + pl[3];
-        const double s = r * r, ah = sp.gp_huber, wt = bd.gp_weight[G];
+        const double s = r * r, ah = bd.wsp[w].gp_huber, wt = bd.gp_weight[G];
         double rho, rho1;
         if (s > ah * ah) { const double q = sqrt(s); rho = 2.0 * ah * q - ah * ah; rho1 = fmax(DBL_MIN, ah / q); }
         else { rho = s; rho1 = 1.0; }
@@ -456,8 +460,8 @@ __global__ void __launch_bounds__(256) k_gp_eval(BatchDev bd, SolveParams sp) {
         (kJac ? bd.gp_cost_x : bd.gp_cost_c)[w] = s;
     }
 }
-template __global__ void k_gp_eval<true>(BatchDev, SolveParams);
-template __global__ void k_gp_eval<false>(BatchDev, SolveParams);
+template __global__ void k_gp_eval<true>(BatchDev);
+template __global__ void k_gp_eval<false>(BatchDev);
 
 // per-keyframe ground-plane Gauss-Newton block after k_gp_eval<true>: the 55 lower-packed entries of the 10 x 10 (pose | normal |
 // distance) block and the 10 gradient entries, summed over the keyframe's active gp residuals in index order.  One warp per
@@ -502,7 +506,7 @@ __global__ void __launch_bounds__(256) k_gp_blocks(BatchDev bd) {
 // re-evaluates the Jacobian rows (cheaper than gathering the materialised J_pose across sectors) and reduces
 // B_k = sum J_p^T J_p (21 unique) and g_k = sum J_p^T r (6) with a fixed-shape tree -> deterministic, no atomics.
 // =====================================================================================================================
-__global__ void __launch_bounds__(256, 2) k_pose_hessian(BatchDev bd, SolveParams sp) {
+__global__ void __launch_bounds__(256, 2) k_pose_hessian(BatchDev bd) {
     const int w = blockIdx.y, k = blockIdx.x;
     const WinState& st = bd.state[w];
     if (st.phase != PH_ITERATE || !st.need_linearize) return;
@@ -516,8 +520,11 @@ __global__ void __launch_bounds__(256, 2) k_pose_hessian(BatchDev bd, SolveParam
     __shared__ double s_acc[9][256];
     __shared__ long long s_ob;                              // the window's first observation, its landmark offset, the end of
     __shared__ int s_lm_off, s_e1;                          // this keyframe's observations: re-read in every iteration (below)
+    __shared__ double s_b[2];                               // the window's squared Cauchy scales (reprojection, depth), likewise
     if (threadIdx.x == 0) {
         s_ob = wd.obs_off; s_lm_off = wd.lm_off; s_e1 = bd.kf_ptr[wd.kf_off + w + k + 1];
+        const SolveParams& sp = bd.wsp[w];
+        s_b[0] = sp.reprojection_thres * sp.reprojection_thres; s_b[1] = sp.depth_thres * sp.depth_thres;
         const double* p = bd.pose[st.cur] + 7 * (size_t)(wd.kf_off + k);
         double R[9];
         quat_to_rot<double>(p, R);
@@ -574,8 +581,7 @@ __global__ void __launch_bounds__(256, 2) k_pose_hessian(BatchDev bd, SolveParam
             const double p[3] = {p0, p1, p2};
             double r[3], m[9], a[3], raw[2], hr;
             if (eval_factored<double, true, false>(s_pose, s_cam + kCamStride * cam, p, (double)u, (double)v, (double)d,
-                                                   wgt, sp.reprojection_thres * sp.reprojection_thres,
-                                                   sp.depth_thres * sp.depth_thres, r, m, a, hr, raw)) {
+                                                   wgt, s_b[0], s_b[1], r, m, a, hr, raw)) {
                 // J_p = m [K | I] with K = -2 [a]x (kba_device.cuh: eval_factored), so with M = m^T m and h = m^T r
                 //   J_p^T J_p = [K^T M K, K^T M; M K, M],  J_p^T r = [K^T h; h],  K^T v = 2 a x v,  (row_i(P) K) = 2 a x row_i(P)
                 double mm[6], h[3];
@@ -1027,8 +1033,9 @@ __global__ void __launch_bounds__(256) k_sred_reduce(BatchDev bd, int mode) {
 // the factorisation over many SMs (one SM's FP64 throughput bounds the n^3/3 trailing flops of a 594-row system);
 // stage 2 = back substitution and candidate state only.
 template <bool kTiled>
-__global__ void __launch_bounds__(512, 1) k_reduced_solve(BatchDev bd, SolveParams sp, int stage) {
+__global__ void __launch_bounds__(512, 1) k_reduced_solve(BatchDev bd, int stage) {
     const int w = blockIdx.x;
+    const SolveParams& sp = bd.wsp[w];
     WinState& st = bd.state[w];
     if (st.phase != PH_ITERATE) return;
     const WinDesc& wd = bd.desc[w];
@@ -1900,7 +1907,7 @@ __global__ void __launch_bounds__(256) k_shard_gp_gather(BatchDev bd) {
     bd.gp_send[bd.lm_begin + bd.lm_orig[wd.lm_off + bd.gp_lm[G]]] = (double)(bd.gp_kf[G] + 1);
 }
 
-__global__ void __launch_bounds__(128) k_lm_update(BatchDev bd, SolveParams sp) {
+__global__ void __launch_bounds__(128) k_lm_update(BatchDev bd) {
     // one warp per window: the lanes reduce the partial sums (fixed shape: strided partials, then a butterfly), lane 0
     // then runs the controller
     const int w = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
@@ -1928,7 +1935,7 @@ __global__ void __launch_bounds__(128) k_lm_update(BatchDev bd, SolveParams sp) 
     const double* PL = bd.plane[1 - st.cur];
     const double* gp_cost = bd.sharded ? bd.xs + 5 : bd.gp_cost_c + w;
     const bool has_gp = wd.n_gp > 0 || bd.shard_gp;
-    lm_step(st, bd.log + (size_t)w * kIterLogCap, sp, !bd.sharded, bd.lin1 != 0, e_model, e_step, e_xn, e_g,
+    lm_step(st, bd.log + (size_t)w * kIterLogCap, bd.wsp[w], !bd.sharded, bd.lin1 != 0, e_model, e_step, e_xn, e_g,
             [&wd, cand_sum, P, PL, gp_cost, has_gp]() {
         double cand = cand_sum;
         if (wd.scale_weight > 0) {
@@ -1953,11 +1960,12 @@ __global__ void __launch_bounds__(128) k_lm_update(BatchDev bd, SolveParams sp) 
 // trimming (reference robust_solving.cpp:67-125, trimmer_quantile.hpp:40-63)
 // =====================================================================================================================
 // per-landmark maximum of the un-robustified block norms, per residual group (0 depth, 1 reprojection, 2 ground plane)
-__global__ void __launch_bounds__(256) k_trim_eval(BatchDev bd, SolveParams sp) {
+__global__ void __launch_bounds__(256) k_trim_eval(BatchDev bd) {
     const int w = blockIdx.y;
     const WinState& st = bd.state[w];
     if (st.phase != PH_TRIM) return;
     const WinDesc& wd = bd.desc[w];
+    const SolveParams& sp = bd.wsp[w];
     __shared__ double s_pose[kMaxKf * kPoseStride];
     __shared__ double s_cam[kMaxCam * kCamStride];
     stage_window(wd, bd.pose[st.cur], bd.cam, s_pose, s_cam);
@@ -2008,8 +2016,9 @@ __global__ void __launch_bounds__(256) k_trim_eval(BatchDev bd, SolveParams sp) 
 }
 
 // quantile rejection per group by exact rank (ties broken by landmark index, trim_select_group), then start the next solve
-__global__ void __launch_bounds__(512) k_trim_select(BatchDev bd, SolveParams sp) {
+__global__ void __launch_bounds__(512) k_trim_select(BatchDev bd) {
     const int w = blockIdx.x;
+    const SolveParams& sp = bd.wsp[w];
     WinState& st = bd.state[w];
     if (st.phase != PH_TRIM) return;
     const WinDesc& wd = bd.desc[w];
@@ -2046,7 +2055,7 @@ __global__ void k_count_active(BatchDev bd) {
 }
 
 // reset of the solver state from the uploaded values
-__global__ void k_reset_state(BatchDev bd, int rounds_total_override, int min_landmarks_for_trimming, int num_rounds_option) {
+__global__ void k_reset_state(BatchDev bd) {
     const int w = blockIdx.x;
     const WinDesc& wd = bd.desc[w];
     for (int i = threadIdx.x; i < wd.n_kf * 7; i += blockDim.x) {
@@ -2080,8 +2089,9 @@ __global__ void k_reset_state(BatchDev bd, int rounds_total_override, int min_la
         st.phase = wd.idle ? PH_DONE : PH_SOLVE_BEGIN;  // an idle window (kba_track_group_solve) never iterates: no solve, no log
         st.cur = 0;
         st.solve_index = 0; st.round = 0; st.retried = 0; st.log_n = 0; st.n_solves = 0;
-        int rounds = rounds_total_override;
-        if (rounds < 0) rounds = ((bd.sharded ? bd.lm_total : wd.n_lm) > min_landmarks_for_trimming) ? num_rounds_option : 0;
+        const SolveParams& sp = bd.wsp[w];
+        int rounds = sp.rounds_override;
+        if (rounds < 0) rounds = ((bd.sharded ? bd.lm_total : wd.n_lm) > sp.min_landmarks_for_trimming) ? sp.num_rounds_option : 0;
         if (rounds > 6) rounds = 6;
         st.rounds_total = rounds;
         st.is_final = (rounds == 0);
@@ -2171,10 +2181,10 @@ int launch_shard_gather(const BatchDev& bd, const LaunchCfg& lc, cudaStream_t s)
 }
 
 void launch_reset(const BatchDev& bd, const LaunchCfg& lc, cudaStream_t s) {
-    k_reset_state<<<bd.n_win, 256, 0, s>>>(bd, lc.rounds_override, lc.min_landmarks_for_trimming, lc.num_rounds_option); LCHK("k_reset_state");
+    k_reset_state<<<bd.n_win, 256, 0, s>>>(bd); LCHK("k_reset_state");
 }
 
-int launch_pass(const BatchDev& bd, const SolveParams& sp, const LaunchCfg& lc, Counters* cnt, cudaStream_t s) {
+int launch_pass(const BatchDev& bd, const LaunchCfg& lc, Counters* cnt, cudaStream_t s) {
     const int B = bd.n_win;
     const dim3 g_obs((bd.max_obs + 255) / 256, B);
     const dim3 g_lm((bd.max_lm + 63) / 64, B);
@@ -2182,38 +2192,38 @@ int launch_pass(const BatchDev& bd, const SolveParams& sp, const LaunchCfg& lc, 
     LCHK("k_panel_zero");
     if (bd.sharded && bd.shard_gp) k_shard_planes<<<1, 256, 0, s>>>(bd);
     LCHK("k_shard_planes");
-    k_solve_begin<<<B, kBeginThreads, 0, s>>>(bd, sp); LCHK("k_solve_begin");
+    k_solve_begin<<<B, kBeginThreads, 0, s>>>(bd); LCHK("k_solve_begin");
     const bool timed = lc.time_jacobian && lc.ev_pool && *lc.ev_used + 2 <= lc.ev_cap;
     // one-kernel linearisation (kba_linearize.cuh): fused path, FP64, at most one observation per (landmark, keyframe)
     const bool lin1 = bd.lin1 != 0;
     if (lin1) {
         if (bd.tot_gp > 0) {
-            k_gp_eval<true><<<B, 256, 0, s>>>(bd, sp);
+            k_gp_eval<true><<<B, 256, 0, s>>>(bd);
             k_gp_blocks<<<dim3((bd.max_kf + 7) / 8, B), 256, 0, s>>>(bd);
         }
         LCHK("k_gp_eval");
         if (timed) cudaEventRecord(lc.ev_pool[(*lc.ev_used)++], s);
         const int n_units = (lin_tile_bound(bd.max_obs, bd.max_lm) + kLinWarps - 1) / kLinWarps;
         const dim3 g_lin(strided_grid(lc.knobs.lin_grid, n_units, 1, 8, B, lc.sm_count, kLinMinBlocks, 6), B);  // CTAs of a window stride over its units
-        if ((int)g_lin.x < n_units) k_linearize<true><<<g_lin, kLinThreads, 0, s>>>(bd, sp, n_units);
-        else k_linearize<false><<<g_lin, kLinThreads, 0, s>>>(bd, sp, n_units);
+        if ((int)g_lin.x < n_units) k_linearize<true><<<g_lin, kLinThreads, 0, s>>>(bd, n_units);
+        else k_linearize<false><<<g_lin, kLinThreads, 0, s>>>(bd, n_units);
         LCHK("k_linearize");
         if (timed) cudaEventRecord(lc.ev_pool[(*lc.ev_used)++], s);
-        k_pose_hessian<<<dim3(bd.max_kf, B), 256, 0, s>>>(bd, sp); LCHK("k_pose_hessian");
+        k_pose_hessian<<<dim3(bd.max_kf, B), 256, 0, s>>>(bd); LCHK("k_pose_hessian");
     } else {
         if (timed) cudaEventRecord(lc.ev_pool[(*lc.ev_used)++], s);
-        launch_eval_obs<true>(bd, sp, s);
+        launch_eval_obs<true>(bd, s);
         if (timed) cudaEventRecord(lc.ev_pool[(*lc.ev_used)++], s);
         if (bd.tot_gp > 0) {
-            k_gp_eval<true><<<B, 256, 0, s>>>(bd, sp);
+            k_gp_eval<true><<<B, 256, 0, s>>>(bd);
             k_gp_blocks<<<dim3((bd.max_kf + 7) / 8, B), 256, 0, s>>>(bd);
         }
         LCHK("k_gp_eval");
-        k_pose_hessian<<<dim3(bd.max_kf, B), 256, 0, s>>>(bd, sp); LCHK("k_pose_hessian");
+        k_pose_hessian<<<dim3(bd.max_kf, B), 256, 0, s>>>(bd); LCHK("k_pose_hessian");
     }
     if (bd.fused) {
         if (!lin1) {
-            k_landmark_reduce<true><<<dim3((bd.max_lm + 15) / 16, B), 256, 0, s>>>(bd, sp); LCHK("k_landmark_reduce");
+            k_landmark_reduce<true><<<dim3((bd.max_lm + 15) / 16, B), 256, 0, s>>>(bd); LCHK("k_landmark_reduce");
             k_obs_v2<<<g_obs, 256, 0, s>>>(bd); LCHK("k_obs_v2");
         }
         const dim3 gf(bd.p_split, B);
@@ -2221,7 +2231,7 @@ int launch_pass(const BatchDev& bd, const SolveParams& sp, const LaunchCfg& lc, 
         else k_schur_fused<6><<<gf, 512, schur_fused_smem(), s>>>(bd);
         LCHK("k_schur_fused");
     } else {
-        k_landmark_reduce<false><<<dim3((bd.max_lm + 15) / 16, B), 256, 0, s>>>(bd, sp); LCHK("k_landmark_reduce");
+        k_landmark_reduce<false><<<dim3((bd.max_lm + 15) / 16, B), 256, 0, s>>>(bd); LCHK("k_landmark_reduce");
         for (int round = 0; round <= lc.max_rank; ++round) k_obs_v<<<g_obs, 256, 0, s>>>(bd, round);
         LCHK("k_obs_v");
         if (bd.tot_gp > 0) k_gp_panel<<<dim3((bd.max_gp * 10 + 255) / 256, B), 256, 0, s>>>(bd);
@@ -2255,18 +2265,18 @@ int launch_pass(const BatchDev& bd, const SolveParams& sp, const LaunchCfg& lc, 
         k_sred_reduce<<<g_red, 256, 0, s>>>(bd, 0); LCHK("k_sred_reduce");
     }
     if (bd.solve_tiled) {
-        k_reduced_solve<true><<<B, 512, solve_tiled_smem(lc.plan.nr_cap_max), s>>>(bc, sp, 0); LCHK("k_reduced_solve");
+        k_reduced_solve<true><<<B, 512, solve_tiled_smem(lc.plan.nr_cap_max), s>>>(bc, 0); LCHK("k_reduced_solve");
     } else if (!bd.solve_split) {
-        k_reduced_solve<false><<<B, 512, solve_smem(lc.plan.nr_cap_max), s>>>(bc, sp, 0); LCHK("k_reduced_solve");
+        k_reduced_solve<false><<<B, 512, solve_smem(lc.plan.nr_cap_max), s>>>(bc, 0); LCHK("k_reduced_solve");
     } else {  // few large windows: the factorisation is spread over the GPU, one 32-column block at a time
-        k_reduced_solve<false><<<B, 512, solve_smem(lc.plan.nr_cap_max), s>>>(bc, sp, 1); LCHK("k_reduced_solve");
+        k_reduced_solve<false><<<B, 512, solve_smem(lc.plan.nr_cap_max), s>>>(bc, 1); LCHK("k_reduced_solve");
         const int strips = (lc.plan.nr_cap_max + 7) / 8;
         for (int kb = 0; kb < lc.plan.nr_cap_max; kb += kNB) {
             k_chol_diag<<<B, 32, 0, s>>>(bc, kb); LCHK("k_chol_diag");
             k_chol_panel<<<dim3((strips + 15) / 16, B), 512, 0, s>>>(bc, kb); LCHK("k_chol_panel");
             k_chol_trail<<<dim3(bd.solve_split, B), 512, trail_smem(lc.plan.nr_cap_max), s>>>(bc, kb); LCHK("k_chol_trail");
         }
-        k_reduced_solve<false><<<B, 512, solve_smem(lc.plan.nr_cap_max), s>>>(bc, sp, 2); LCHK("k_reduced_solve");
+        k_reduced_solve<false><<<B, 512, solve_smem(lc.plan.nr_cap_max), s>>>(bc, 2); LCHK("k_reduced_solve");
     }
     if (bd.fused) {
         const int n_units = (bd.max_lm + 15) / 16;
@@ -2276,21 +2286,21 @@ int launch_pass(const BatchDev& bd, const SolveParams& sp, const LaunchCfg& lc, 
     }
     else k_backsub<<<dim3((bd.max_lm + 15) / 16, B), 256, 0, s>>>(bd);
     LCHK("k_backsub");
-    launch_eval_obs<false>(bd, sp, s);
-    if (bd.tot_gp > 0) k_gp_eval<false><<<B, 256, 0, s>>>(bd, sp);
+    launch_eval_obs<false>(bd, s);
+    if (bd.tot_gp > 0) k_gp_eval<false><<<B, 256, 0, s>>>(bd);
     LCHK("k_gp_eval");
     if (bd.sharded) {  // model decrease / step norm / candidate cost over all ranks
         k_shard_scalars<<<1, 32, 0, s>>>(bd); LCHK("k_shard_scalars");
         // model decrease, step / state norms, candidate cost, failure flag (sums) and one gradient-max slot per rank
         if (int rc = lc.xchg.allreduce(lc.xchg.user, bd.xs, bd.xs, 16 + bd.shard_world, 0, s)) return rc;
     }
-    k_lm_update<<<(B * 32 + 127) / 128, 128, 0, s>>>(bd, sp); LCHK("k_lm_update");
-    k_trim_eval<<<g_lm, 256, 0, s>>>(bd, sp); LCHK("k_trim_eval");
+    k_lm_update<<<(B * 32 + 127) / 128, 128, 0, s>>>(bd); LCHK("k_lm_update");
+    k_trim_eval<<<g_lm, 256, 0, s>>>(bd); LCHK("k_trim_eval");
     if (bd.sharded) {  // quantiles are taken over the landmarks of all ranks
         k_shard_trim_scatter<<<(bd.max_lm + 255) / 256, 256, 0, s>>>(bd); LCHK("k_shard_trim_scatter");
         if (int rc = lc.xchg.allreduce(lc.xchg.user, bd.trim_send, bd.trim_glob, 3LL * bd.lm_total, 0, s)) return rc;
     }
-    k_trim_select<<<B, 512, 0, s>>>(bd, sp); LCHK("k_trim_select");
+    k_trim_select<<<B, 512, 0, s>>>(bd); LCHK("k_trim_select");
     if (cnt) {
         const int gp = bd.tot_gp > 0 ? 1 : 0;
         const int prep = lin1 ? 1 : 2 + (bd.fused ? 1 : lc.max_rank + 1 + gp);  // pose blocks [, landmark blocks, V rows]
@@ -2334,9 +2344,8 @@ __global__ void k_force_linearize(BatchDev bd) {
     WinState& st = bd.state[w];
     st.phase = PH_ITERATE; st.need_linearize = 1; st.iter0 = 1; st.cur = 0; st.eval_failed = 0; st.solve_failed = 0;
 }
-void launch_jacobian_only(const BatchDev& bd, const SolveParams& sp, cudaStream_t s) {
-    const dim3 g_obs((bd.max_obs + 255) / 256, bd.n_win);
-    launch_eval_obs<true>(bd, sp, s);
+void launch_jacobian_only(const BatchDev& bd, cudaStream_t s) {
+    launch_eval_obs<true>(bd, s);
 }
 // inspection entry point (kba_eval) on the fused path: J_l of every observation, formed exactly as the consumers of the
 // linearisation form it -- translation columns of the materialised J_p times the staged rotation of the keyframe, in FP64
@@ -2361,7 +2370,7 @@ void launch_expand_jl(const BatchDev& bd, double* out, cudaStream_t s) {
     LCHK("k_expand_jl");
 }
 void launch_force_linearize(const BatchDev& bd, cudaStream_t s) {
-    k_solve_begin<<<bd.n_win, kBeginThreads, 0, s>>>(bd, SolveParams{}); LCHK("k_solve_begin");  // layout (off_pose) for the eval entry point
+    k_solve_begin<<<bd.n_win, kBeginThreads, 0, s>>>(bd); LCHK("k_solve_begin");  // layout (off_pose) for the eval entry point
     k_force_linearize<<<(bd.n_win + 127) / 128, 128, 0, s>>>(bd); LCHK("k_force_linearize");
 }
 

@@ -42,7 +42,6 @@ struct LaunchCfg {
     Knobs knobs;              // read when the batch was created
     int sm_count = 132;       // SMs of the device the batch runs on (strided_grid: waves of CTAs)
     int max_rank = 0;         // largest observation rank in the batch (multi-camera rigs)
-    int rounds_override = -1, min_landmarks_for_trimming = 100, num_rounds_option = 1;
     bool time_jacobian = false;
     cudaEvent_t* ev_pool = nullptr;  // pairs of events bracketing each residual/Jacobian launch
     int ev_cap = 0;
@@ -342,7 +341,7 @@ struct FrameDesc {
     int meas_off;               // first measurement of the frame in the call's staged arrays
     int run_off;                // first run of the frame in the work / result arrays
     int rs_off;                 // first entry of the frame's run_start list (n_runs + 1 entries, frame-local measurement indices)
-    int rounds_total;           // trimming rounds, resolved on the host (k_reset_state's rule)
+    int rounds_total;           // trimming rounds, resolved on the host (k_reset_state's rule on MotionArgs::sp of the frame)
     const double* lm_pos;       // the track's store: positions [lm_cap*3] and weights by slot
     const double* lm_weight;
     const double* cam16;        // the track's staged cameras (kCamStride doubles each)
@@ -360,6 +359,7 @@ struct FrameRes {
 };
 struct MotionArgs {
     const FrameDesc* fd;        // [n_frames]
+    const SolveParams* sp;      // [n_frames] solver options of each frame
     const int* lm_slot;         // [total measurements] staged per call
     const int* cam;
     const float* u, *v, *d;
@@ -374,7 +374,7 @@ struct MotionArgs {
     unsigned char* res_rej;     // [total runs]
     int log_cap, total_runs;
 };
-void launch_adjust_pose(const MotionArgs& a, int n_frames, const SolveParams& sp, cudaStream_t s);
+void launch_adjust_pose(const MotionArgs& a, int n_frames, cudaStream_t s);
 
 cudaError_t configure_pack();
 void launch_pack(const BatchDev& bd, const PackRaw& raw, cudaStream_t s);
@@ -383,11 +383,11 @@ void launch_unpack_landmarks(const BatchDev& bd, double* lm_user, unsigned char*
 cudaError_t configure_kernels(int nr_cap_max);
 void launch_reset(const BatchDev& bd, const LaunchCfg& lc, cudaStream_t s);
 int launch_shard_gather(const BatchDev& bd, const LaunchCfg& lc, cudaStream_t s);  // sharded window: attachment of all ground points
-int launch_pass(const BatchDev& bd, const SolveParams& sp, const LaunchCfg& lc, Counters* cnt, cudaStream_t s);
+int launch_pass(const BatchDev& bd, const LaunchCfg& lc, Counters* cnt, cudaStream_t s);
 void launch_count_active(const BatchDev& bd, cudaStream_t s);
 void launch_loop_cond(const BatchDev& bd, unsigned long long handle, int* pass, int max_passes, cudaStream_t s);  // WHILE-node condition
 void launch_force_linearize(const BatchDev& bd, cudaStream_t s);
-void launch_jacobian_only(const BatchDev& bd, const SolveParams& sp, cudaStream_t s);
+void launch_jacobian_only(const BatchDev& bd, cudaStream_t s);
 void launch_expand_jl(const BatchDev& bd, double* out, cudaStream_t s);  // fused path: J_l as its consumers form it
 
 }  // namespace kba

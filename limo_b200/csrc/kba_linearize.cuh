@@ -96,11 +96,11 @@ constexpr int kLinMinBlocks = 3;
 // k_linearize's static shared memory (the arrays declared in the kernel, below): it has to stay within the 48 KB a kernel may
 // declare statically; a larger kFusedMaxKf or kMaxCam means dynamic shared memory (or thinner per-lane strips)
 constexpr size_t kLinStaticSmem = sizeof(double) * (kFusedMaxKf * kPoseStride + kMaxCam * kCamStride + kLinWarps * 9 * 33 +
-                                                    kLinWarps * 32 * 9 + kLinWarps) +
+                                                    kLinWarps * 32 * 9 + kLinWarps + 4) +
                                   sizeof(int) * (kLinWarps * 6 * 32 + kLinWarps) + sizeof(uint64_t);
 static_assert(kLinStaticSmem <= 48 * 1024, "k_linearize: static shared memory over 48 KB");
 template <bool kLoop>
-__global__ void __launch_bounds__(kLinThreads, kLinMinBlocks) k_linearize(BatchDev bd, SolveParams sp, int n_units) {
+__global__ void __launch_bounds__(kLinThreads, kLinMinBlocks) k_linearize(BatchDev bd, int n_units) {
     const int w = blockIdx.y;
     WinState& st = bd.state[w];
     if (st.phase != PH_ITERATE) return;
@@ -132,6 +132,9 @@ __global__ void __launch_bounds__(kLinThreads, kLinMinBlocks) k_linearize(BatchD
                                                         // division calls would spill them
     __shared__ double s_red[kLinWarps];
     __shared__ int s_cnt[kLinWarps];
+    __shared__ double s_prm[4];                         // the window's options (BatchDev::wsp): squared Cauchy scales of the
+                                                        // reprojection and depth rows, LM diagonal bounds -- staged with the
+                                                        // poses, read where they are used (no register is live for them)
     for (int unit = blockIdx.x; unit < n_units; unit += gridDim.x) {
     asm volatile("" ::: "memory");  // the window's values are re-read per unit: hoisted out of the loop, they would be spilled
     if (unit * kLinWarps >= n_tiles()) {                  // no tile in this unit: its cost slot still has to read zero
@@ -165,7 +168,14 @@ __global__ void __launch_bounds__(kLinThreads, kLinMinBlocks) k_linearize(BatchD
     int (*six)[32] = s_ix[warp];
     // once, in the CTA's first unit (the poses do not change within a pass): units are taken in increasing order, so when the
     // first one holds no tile, none does
-    if (unit == (int)blockIdx.x) stage_window_bulk(wd, bd.rt[st.cur], bd.cam, s_pose, s_cam, &s_bar);
+    if (unit == (int)blockIdx.x) {
+        if (tid == 0) {
+            const SolveParams& sp = bd.wsp[w];
+            s_prm[0] = sp.reprojection_thres * sp.reprojection_thres; s_prm[1] = sp.depth_thres * sp.depth_thres;
+            s_prm[2] = sp.min_lm_diagonal; s_prm[3] = sp.max_lm_diagonal;
+        }
+        stage_window_bulk(wd, bd.rt[st.cur], bd.cam, s_pose, s_cam, &s_bar);  // its barrier publishes s_prm
+    }
     six[0][lane] = kf; six[1][lane] = row0; six[2][lane] = wd.obs_off + p0; six[3][lane] = p1 - p0; six[4][lane] = wd.lm_off + j;
     six[5][lane] = have ? 1 | (act ? 2 : 0) | ((p0 - tile.x) << 2) : 0;
     // ---- evaluate my observation; contributions to its landmark block
@@ -178,7 +188,7 @@ __global__ void __launch_bounds__(kLinThreads, kLinMinBlocks) k_linearize(BatchD
         // them, m and r would be live across the join and spilled
         const auto evaluate = [&](auto with_cost) {
             double r[3], m[9], raw[2];
-            const double br = sp.reprojection_thres * sp.reprojection_thres, bdp = sp.depth_thres * sp.depth_thres;
+            const double br = s_prm[0], bdp = s_prm[1];
             ok = eval_factored<double, true, decltype(with_cost)::value>(s_pose + kPoseStride * kf, s_cam + kCamStride * cam, p,
                                                                           (double)mu, (double)mv, (double)md, wgt, br, bdp, r, m,
                                                                           sma + 6, hr, raw);
@@ -276,7 +286,7 @@ __global__ void __launch_bounds__(kLinThreads, kLinMinBlocks) k_linearize(BatchD
             for (int e = 0; e < 3; ++e) {
                 tt[e] = st.iter0 ? 1.0 + sqrt(cd[e]) : tt_ld[e];
                 const double t2 = tt[e] * tt[e];
-                lam[e] = fmin(fmax(cd[e], sp.min_lm_diagonal * t2), sp.max_lm_diagonal * t2) * inv_radius;
+                lam[e] = fmin(fmax(cd[e], s_prm[2] * t2), s_prm[3] * t2) * inv_radius;
             }
             // Cholesky of C + diag(lam) through the reciprocal square roots of the pivots: L^-1 is what every consumer wants
             // (V = E L^-T, z = L^-1 g, the back substitution), L itself is never needed

@@ -56,8 +56,9 @@ __device__ __forceinline__ void stage_rt(const double* p7, double* rt) {
 }
 
 // One CTA per SM: at two (128 registers) the kernel spills; at one it takes 235 registers and none.
-__global__ void __launch_bounds__(kMotionThreads, 1) k_adjust_pose(MotionArgs A, SolveParams sp) {
+__global__ void __launch_bounds__(kMotionThreads, 1) k_adjust_pose(MotionArgs A) {
     const FrameDesc& F = A.fd[blockIdx.x];
+    const SolveParams& sp = A.sp[blockIdx.x];
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     __shared__ WinState s_st;
     __shared__ double s_pose[2][7];             // x / candidate (ping-pong by s_st.cur, as BatchDev::pose)
@@ -380,9 +381,9 @@ __global__ void __launch_bounds__(kMotionThreads, 1) k_adjust_pose(MotionArgs A,
     for (int r = tid; r < n_runs; r += kMotionThreads) A.res_rej[F.run_off + r] = act[r] ? 0 : 1;
 }
 
-void launch_adjust_pose(const MotionArgs& a, int n_frames, const SolveParams& sp, cudaStream_t s) {
+void launch_adjust_pose(const MotionArgs& a, int n_frames, cudaStream_t s) {
     if (n_frames <= 0) return;
-    k_adjust_pose<<<n_frames, kMotionThreads, 0, s>>>(a, sp);
+    k_adjust_pose<<<n_frames, kMotionThreads, 0, s>>>(a);
     LCHK("k_adjust_pose");
 }
 

@@ -14,8 +14,9 @@ __device__ __forceinline__ int gp_row(const BatchDev& bd, const WinDesc& wd, int
 // kFused: J_l is not materialised; it is formed here as (translation columns of J_p) R(keyframe), the rotations staged by
 // one bulk copy, and the z row goes to global memory only (lm_z) -- the fused Schur kernel builds its panels itself.
 template <bool kFused>
-__global__ void __launch_bounds__(256, 4) k_landmark_reduce(BatchDev bd, SolveParams sp) {
+__global__ void __launch_bounds__(256, 4) k_landmark_reduce(BatchDev bd) {
     const int w = blockIdx.y;
+    const SolveParams& sp = bd.wsp[w];
     WinState& st = bd.state[w];
     if (st.phase != PH_ITERATE) return;
     const WinDesc& wd = bd.desc[w];
