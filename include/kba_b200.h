@@ -452,7 +452,8 @@ int kba_track_group_solve(kba_track_group* g, const kba_track_request* req, cons
  * them, before anything is uploaded, and kba_last_error names the track index; a track that sits the solve out (n_kf == 0) does
  * not read its entry.  The options travel in the lists' copy, and only when they differ from the group's last solve's. */
 int kba_track_group_solve_opts(kba_track_group* g, const kba_track_request* req, const kba_options* opts, kba_result* res);
-/* upload / download of the last group solve, pose-only call, selection, creation, upkeep, flow or reclaim call, counted as kba_track_transfer_bytes counts them */
+/* upload / download of the last group solve, pose-only call, selection, creation, upkeep, flow or reclaim call or store write,
+ * counted as kba_track_transfer_bytes counts them */
 int kba_track_group_transfer_bytes(kba_track_group* g, int64_t* h2d_last_solve, int64_t* d2h_last_solve);
 
 /* ---- landmark selection for every track of a group in one launch sequence -------------------------------------------------
@@ -714,6 +715,61 @@ typedef struct kba_reclaim_out {  /* caller-owned */
 int kba_track_reclaim_landmarks(kba_track* t, const kba_reclaim_request* req, kba_reclaim_out* out);
 /* req[n_tracks], out[n_tracks] */
 int kba_track_group_reclaim_landmarks(kba_track_group* g, const kba_reclaim_request* req, kba_reclaim_out* out);
+
+/* ---- store writes for every track of a group: push, drop, landmark values and keyframe poses in one call each -----------------
+ * The group forms of kba_track_push_keyframe, kba_track_drop_keyframe, kba_track_set_landmarks and kba_track_set_keyframe_poses,
+ * one request per track (req[n_tracks]); each single call is the one-track form of the same host code and kernels.
+ *   - Sitting out: a push or drop with kf_slot < 0, a landmark or pose write with n == 0.  A call in which every request sits out
+ *     returns at once.
+ *   - Validation: every other request gets the checks of its single call, with the same error codes, before anything is uploaded:
+ *     a null array, a negative size, a slot or camera out of range, a push into a slot in use: KBA_ERR_BAD_ARG; a push whose
+ *     measurements do not fit max_measurements next to the track's live (pushed, not dropped) keyframes' measurements:
+ *     KBA_ERR_CAPACITY, decided from the host's mirror of the arena, so nothing is compacted.  If one request fails, the call returns
+ *     its code, kba_last_error names the track index, and no store changes.
+ *   - Results: each track's store afterwards equals, bit for bit, what the single calls in track order leave: arena contents at the
+ *     same offsets, poses, planes, positions and weights.  A slot listed twice in one write is written in an unspecified order.
+ *   - A push appends the keyframe's measurements to the track's arena.  A track whose arena has no room left at its end first
+ *     compacts: its live keyframes, in slot order, are copied into the track's second arena (k_arena_compact), then the keyframe is
+ *     appended there (k_store_append, which also writes the keyframe's arena offset, count, pose and plane).  plane4 NULL stores
+ *     (0, 0, 1, 0); cam NULL stores camera 0 for every measurement.
+ *   - Transfers: one upload (the rows of every request and a fixed record per track, plus a record per live keyframe of a track
+ *     that compacts), one launch sequence and one synchronisation per call; more only when the rows exceed the staging, which holds
+ *     min(max_measurements, 65536) pushed rows or max(win_landmarks, 64) landmark / pose rows per track, allocated for the set's
+ *     capacities at the first call of each kind (a drop shares the push's).  A drop moves nothing.
+ *     kba_track_group_transfer_bytes (kba_track_transfer_bytes for a single call) reports the call's upload and 0 bytes down.
+ *     Each track's h2d_pushes_total counts its own rows: 20 bytes per pushed measurement plus 88 per keyframe, and 4 + 24 (pos)
+ *     + 8 (weight) bytes per landmark row.
+ *   - Each track that a request changed (every request that does not sit out) makes its ranking stale; the others keep theirs. */
+typedef struct kba_push_request {  /* one keyframe into track i's store */
+    int32_t kf_slot;            /* < 0: this track sits the call out                                                           */
+    int32_t n_meas;             /* >= 0                                                                                        */
+    const double* pose7;
+    const double* plane4;       /* NULL: (0, 0, 1, 0)                                                                          */
+    const int32_t* lm_slot;     /* [n_meas] */
+    const int32_t* cam;         /* [n_meas] or NULL (every measurement camera 0)                                               */
+    const float* u;             /* [n_meas] */
+    const float* v;
+    const float* d;
+} kba_push_request;
+int kba_track_group_push_keyframes(kba_track_group* g, const kba_push_request* req);
+/* kf_slot[n_tracks]; < 0 sits out */
+int kba_track_group_drop_keyframes(kba_track_group* g, const int32_t* kf_slot);
+typedef struct kba_landmark_write {
+    int32_t n;                  /* 0: this track sits the call out                                                             */
+    int32_t reserved_;
+    const int32_t* lm_slot;     /* [n] */
+    const double* pos3;         /* [3 * n] or NULL */
+    const double* weight;       /* [n] or NULL */
+} kba_landmark_write;
+int kba_track_group_set_landmarks(kba_track_group* g, const kba_landmark_write* req);
+typedef struct kba_pose_write {
+    int32_t n;                  /* 0: this track sits the call out                                                             */
+    int32_t reserved_;
+    const int32_t* kf_slot;     /* [n] */
+    const double* pose7s;       /* [7 * n] */
+    const double* plane4s;      /* [4 * n] or NULL (planes unchanged) */
+} kba_pose_write;
+int kba_track_group_set_keyframe_poses(kba_track_group* g, const kba_pose_write* req);
 
 /* ---- ranked landmark selection on the stored window, and the solve of that ranking (SURVEY row A17) ------------------------
  * kba_track_select_landmarks leaves the ranking of its quantities to the host; kba_track_rank_landmarks ranks them on the

@@ -9,7 +9,7 @@ import os
 
 import numpy as np
 
-from .capi_types import (KbaCounters, KbaCreateOut, KbaCreateRequest, KbaDeactivateOut, KbaDeactivateRequest, KbaDepthEntry, KbaDepthOut, KbaDepthRequest, KbaDrawFn, KbaEvalOut, KbaFlowOut, KbaFlowRequest, KbaLidarOptions, KbaOptions, KbaRankedRequest, KbaRankOut, KbaRankRequest, KbaReclaimOut, KbaReclaimRequest, KbaResult, KbaSelectOut, KbaSelectParams, KbaSelectRequest,
+from .capi_types import (KbaCounters, KbaCreateOut, KbaCreateRequest, KbaDeactivateOut, KbaDeactivateRequest, KbaDepthEntry, KbaDepthOut, KbaDepthRequest, KbaDrawFn, KbaEvalOut, KbaFlowOut, KbaFlowRequest, KbaLandmarkWrite, KbaLidarOptions, KbaOptions, KbaPoseWrite, KbaPushRequest, KbaRankedRequest, KbaRankOut, KbaRankRequest, KbaReclaimOut, KbaReclaimRequest, KbaResult, KbaSelectOut, KbaSelectParams, KbaSelectRequest,
                          KbaTrackCaps, KbaTrackFrame, KbaTrackRequest, KbaWindow, Result, Window, c_double_p, c_int32_p)
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
@@ -31,7 +31,8 @@ SYMBOLS = ["kba_version", "kba_last_error", "kba_default_options", "kba_create",
            "kba_track_group_frame_flow", "kba_track_reclaim_landmarks", "kba_track_group_reclaim_landmarks",
            "kba_track_rank_landmarks", "kba_track_group_rank_landmarks", "kba_track_solve_ranked", "kba_track_group_solve_ranked",
            "kba_solve_batch_opts", "kba_batch_solve_opts", "kba_track_group_solve_opts", "kba_track_group_solve_ranked_opts",
-           "kba_track_group_adjust_pose_opts"]
+           "kba_track_group_adjust_pose_opts", "kba_track_group_push_keyframes", "kba_track_group_drop_keyframes",
+           "kba_track_group_set_landmarks", "kba_track_group_set_keyframe_poses"]
 
 
 class KbaError(RuntimeError):
@@ -156,6 +157,10 @@ def lib():
         L.kba_track_group_solve_opts.argtypes = [vp, C.POINTER(KbaTrackRequest), C.POINTER(KbaOptions), C.POINTER(KbaResult)]
         L.kba_track_group_solve_ranked_opts.argtypes = [vp, C.POINTER(KbaRankedRequest), C.POINTER(KbaOptions), C.POINTER(KbaResult)]
         L.kba_track_group_adjust_pose_opts.argtypes = [vp, C.POINTER(KbaTrackFrame), C.POINTER(KbaOptions), C.POINTER(KbaResult)]
+        L.kba_track_group_push_keyframes.argtypes = [vp, C.POINTER(KbaPushRequest)]
+        L.kba_track_group_drop_keyframes.argtypes = [vp, ip]
+        L.kba_track_group_set_landmarks.argtypes = [vp, C.POINTER(KbaLandmarkWrite)]
+        L.kba_track_group_set_keyframe_poses.argtypes = [vp, C.POINTER(KbaPoseWrite)]
         L.kba_lidar_default_options.argtypes = [C.POINTER(KbaLidarOptions)]
         L.kba_lidar_default_options.restype = None
         fp = C.POINTER(C.c_float)
@@ -823,8 +828,89 @@ class TrackGroup:
             r.c = c
         return results
 
+    def push_keyframes(self, requests):
+        """one keyframe into every track's store in one call (kba_track_group_push_keyframes): each entry None (the track sits the
+        call out) or a dict with the arguments of Track.push_keyframe (slot, pose7, lm_slot, u, v, d and optionally cam, plane4)"""
+        assert len(requests) == len(self.tracks)
+        reqs = (KbaPushRequest * len(requests))()
+        keep = []
+        fp = C.POINTER(C.c_float)
+        for i, r in enumerate(requests):
+            if r is None:
+                reqs[i].kf_slot = -1
+                continue
+            extra = set(r) - {"slot", "pose7", "lm_slot", "u", "v", "d", "cam", "plane4"}
+            if extra:
+                raise TypeError("push_keyframes: request %d has unexpected keys %s" % (i, sorted(extra)))
+            if int(r["slot"]) < 0:  # a negative slot would sit the track out: an error here, as for one track
+                raise KbaError("kba_track_group_push_keyframes: track %d: keyframe slot out of range" % i)
+            pose = np.ascontiguousarray(r["pose7"], dtype=np.float64)
+            pl = None if r.get("plane4") is None else np.ascontiguousarray(r["plane4"], dtype=np.float64)
+            lm = np.ascontiguousarray(r["lm_slot"], dtype=np.int32)
+            cm = None if r.get("cam") is None else np.ascontiguousarray(r["cam"], dtype=np.int32)
+            uu, vv, dd = (np.ascontiguousarray(r[k], dtype=np.float32) for k in ("u", "v", "d"))
+            q = reqs[i]
+            q.kf_slot, q.n_meas = int(r["slot"]), len(lm)
+            q.pose7 = pose.ctypes.data_as(c_double_p)
+            q.plane4 = C.cast(None, c_double_p) if pl is None else pl.ctypes.data_as(c_double_p)
+            q.lm_slot = lm.ctypes.data_as(c_int32_p)
+            q.cam = C.cast(None, c_int32_p) if cm is None else cm.ctypes.data_as(c_int32_p)
+            q.u, q.v, q.d = uu.ctypes.data_as(fp), vv.ctypes.data_as(fp), dd.ctypes.data_as(fp)
+            keep.append((pose, pl, lm, cm, uu, vv, dd))
+        _check(lib().kba_track_group_push_keyframes(self._p, reqs))
+
+    def drop_keyframes(self, slots):
+        """one keyframe slot per track out of its window (kba_track_group_drop_keyframes): None or a negative slot sits out"""
+        assert len(slots) == len(self.tracks)
+        arr = np.array([-1 if s is None else int(s) for s in slots], dtype=np.int32)
+        _check(lib().kba_track_group_drop_keyframes(self._p, arr.ctypes.data_as(c_int32_p)))
+
+    def set_landmarks(self, requests):
+        """landmark positions and weights of every track in one call (kba_track_group_set_landmarks): each entry None (the track
+        sits the call out) or a dict with the arguments of Track.set_landmarks (lm_slot, and optionally pos, weight)"""
+        assert len(requests) == len(self.tracks)
+        reqs = (KbaLandmarkWrite * len(requests))()
+        keep = []
+        for i, r in enumerate(requests):
+            if r is None:
+                continue
+            extra = set(r) - {"lm_slot", "pos", "weight"}
+            if extra:
+                raise TypeError("set_landmarks: request %d has unexpected keys %s" % (i, sorted(extra)))
+            lm = np.ascontiguousarray(r["lm_slot"], dtype=np.int32).ravel()
+            p = None if r.get("pos") is None else np.ascontiguousarray(r["pos"], dtype=np.float64).reshape(-1, 3)
+            w = None if r.get("weight") is None else np.ascontiguousarray(r["weight"], dtype=np.float64)
+            q = reqs[i]
+            q.n, q.lm_slot = len(lm), lm.ctypes.data_as(c_int32_p)
+            q.pos3 = C.cast(None, c_double_p) if p is None else p.ctypes.data_as(c_double_p)
+            q.weight = C.cast(None, c_double_p) if w is None else w.ctypes.data_as(c_double_p)
+            keep.append((lm, p, w))
+        _check(lib().kba_track_group_set_landmarks(self._p, reqs))
+
+    def set_keyframe_poses(self, requests):
+        """keyframe poses (and planes) of every track in one call (kba_track_group_set_keyframe_poses): each entry None (the track
+        sits the call out) or a dict with the arguments of Track.set_keyframe_poses (kf_slots, pose7s, and optionally plane4s)"""
+        assert len(requests) == len(self.tracks)
+        reqs = (KbaPoseWrite * len(requests))()
+        keep = []
+        for i, r in enumerate(requests):
+            if r is None:
+                continue
+            extra = set(r) - {"kf_slots", "pose7s", "plane4s"}
+            if extra:
+                raise TypeError("set_keyframe_poses: request %d has unexpected keys %s" % (i, sorted(extra)))
+            kf = np.ascontiguousarray(r["kf_slots"], dtype=np.int32).ravel()
+            p = np.ascontiguousarray(r["pose7s"], dtype=np.float64).reshape(-1, 7)
+            pl = None if r.get("plane4s") is None else np.ascontiguousarray(r["plane4s"], dtype=np.float64).reshape(-1, 4)
+            q = reqs[i]
+            q.n, q.kf_slot, q.pose7s = len(kf), kf.ctypes.data_as(c_int32_p), p.ctypes.data_as(c_double_p)
+            q.plane4s = C.cast(None, c_double_p) if pl is None else pl.ctypes.data_as(c_double_p)
+            keep.append((kf, p, pl))
+        _check(lib().kba_track_group_set_keyframe_poses(self._p, reqs))
+
     def transfer_bytes(self):
-        """(host->device bytes, device->host bytes) of the last group solve, pose-only call, selection, creation, upkeep or flow call"""
+        """(host->device bytes, device->host bytes) of the last group solve, pose-only call, selection, creation, upkeep, flow
+        call or store write"""
         a, b = C.c_int64(), C.c_int64()
         _check(lib().kba_track_group_transfer_bytes(self._p, C.byref(a), C.byref(b)))
         return a.value, b.value

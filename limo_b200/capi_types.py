@@ -101,6 +101,19 @@ class KbaReclaimOut(C.Structure):
     _fields_ = [("n_free", C.c_int32), ("reserved_", C.c_int32), ("free_slot", c_int32_p), ("pos", c_double_p), ("weight", c_double_p)]
 
 
+class KbaPushRequest(C.Structure):
+    _fields_ = [("kf_slot", C.c_int32), ("n_meas", C.c_int32), ("pose7", c_double_p), ("plane4", c_double_p), ("lm_slot", c_int32_p),
+                ("cam", c_int32_p), ("u", c_float_p), ("v", c_float_p), ("d", c_float_p)]
+
+
+class KbaLandmarkWrite(C.Structure):
+    _fields_ = [("n", C.c_int32), ("reserved_", C.c_int32), ("lm_slot", c_int32_p), ("pos3", c_double_p), ("weight", c_double_p)]
+
+
+class KbaPoseWrite(C.Structure):
+    _fields_ = [("n", C.c_int32), ("reserved_", C.c_int32), ("kf_slot", c_int32_p), ("pose7s", c_double_p), ("plane4s", c_double_p)]
+
+
 class KbaDepthEntry(C.Structure):
     _fields_ = [("ind", C.c_int32), ("wanted", C.c_int32)]
 

@@ -320,8 +320,10 @@ struct SlotStamps {
     }
 };
 
-// the store calls that stage their requests, one staging each; deactivation and depth costs share the upkeep one
-enum StoreCall { kSelectCall, kCreateCall, kUpkeepCall, kFlowCall, kReclaimCall, kRankCall, kStoreCalls };
+// the store calls that stage their requests, one staging each; deactivation and depth costs share the upkeep one, a drop shares
+// the push's
+enum StoreCall { kSelectCall, kCreateCall, kUpkeepCall, kFlowCall, kReclaimCall, kRankCall, kPushCall, kLandmarkWriteCall, kPoseWriteCall,
+                 kStoreCalls };
 
 // what a track and a track group own alike.  A track's set is {the track}: its calls run the host code of a group's, with one
 // window.
@@ -353,13 +355,8 @@ struct kba_track {
     std::vector<int> m_off, m_cnt;         // host mirror of the arena layout
     std::vector<char> kf_live;
     DevAllocs dev;
-    Staged<int> p_lm, p_cam, lay;          // pinned staging: one push / arena layout
-    Staged<float> p_u, p_v, p_d;
-    Staged<double> p_dbl;                  // poses / landmark values on their way to the store
-    Staged<int> p_slot;                    // ... and the slots they go to
     std::vector<double> cam_intr, cam_pose;  // host copy of the cameras: capacity windows of the track and of its groups
-    int push_cap = 0, set_cap = 0;
-    int64_t h2d_push = 0;
+    int64_t h2d_push = 0;                  // rows the store writes sent: pushes and landmark values
     void point_arena() {
         td.m_lm = arena_i[arena_cur][0]; td.m_cam = arena_i[arena_cur][1];
         td.m_u = arena_f[arena_cur][0]; td.m_v = arena_f[arena_cur][1]; td.m_d = arena_f[arena_cur][2];
@@ -1533,8 +1530,6 @@ int kba_eval(kba_handle* h, const kba_window* w, const kba_options* opt, kba_eva
 void kba_track_destroy(kba_track* t) {
     if (!t) return;
     cudaStreamSynchronize(t->set.h->stream);
-    t->p_lm.release(); t->p_cam.release(); t->lay.release();
-    t->p_u.release(); t->p_v.release(); t->p_d.release(); t->p_dbl.release(); t->p_slot.release();
     delete t;
 }
 
@@ -1771,12 +1766,6 @@ int kba_track_create(kba_handle* h, const kba_track_caps* c, int32_t n_cam, cons
     }
     bad |= dev.alloc(&td.lm_pos, 3 * (size_t)td.lm_cap); bad |= dev.alloc(&td.lm_weight, td.lm_cap); bad |= dev.alloc(&td.sel_index, td.lm_cap);
     bad |= dev.alloc(&td.cursor, c->win_landmarks); bad |= dev.alloc(&td.key, c->win_observations); bad |= dev.alloc(&td.n_depth, 1);
-    t->push_cap = std::min(c->max_measurements, 1 << 16);
-    bad |= t->p_lm.alloc(t->push_cap, true); bad |= t->p_cam.alloc(t->push_cap, true); bad |= t->p_u.alloc(t->push_cap, true);
-    bad |= t->p_v.alloc(t->push_cap, true); bad |= t->p_d.alloc(t->push_cap, true);
-    bad |= t->lay.alloc(2 * (size_t)td.kf_cap, true);
-    t->set_cap = std::max(c->win_landmarks, 64);  // rows per staged scatter (landmarks or keyframes)
-    bad |= t->p_dbl.alloc(7 * (size_t)t->set_cap, true); bad |= t->p_slot.alloc(t->set_cap, true);
     if (bad) { kba_track_destroy(t); return fail(KBA_ERR_CUDA, "kba_track_create: out of memory"); }
     t->point_arena();
     t->m_off.assign(td.kf_cap, 0); t->m_cnt.assign(td.kf_cap, 0); t->kf_live.assign(td.kf_cap, 0);
@@ -1788,120 +1777,6 @@ int kba_track_create(kba_handle* h, const kba_track_caps* c, int32_t n_cam, cons
     CU(cudaStreamSynchronize(s));
     *out = t;
     return KBA_OK;
-}
-
-static int track_upload_layout(kba_track* t) {  // arena offsets / counts of every keyframe slot
-    const int K = t->td.kf_cap;
-    memcpy(t->lay.h, t->m_off.data(), K * sizeof(int));
-    memcpy(t->lay.h + K, t->m_cnt.data(), K * sizeof(int));
-    cudaStream_t s = t->set.h->stream;
-    CU(cudaMemcpyAsync(t->td.m_off, t->lay.h, K * sizeof(int), cudaMemcpyHostToDevice, s));
-    CU(cudaMemcpyAsync(t->td.m_cnt, t->lay.h + K, K * sizeof(int), cudaMemcpyHostToDevice, s));
-    CU(cudaStreamSynchronize(s));  // the pinned layout buffer is reused by the next call
-    t->h2d_push += 2 * K * (int64_t)sizeof(int);
-    return KBA_OK;
-}
-
-static int track_compact(kba_track* t) {  // live keyframes copied, in slot order, into the other arena
-    const int other = 1 - t->arena_cur;
-    cudaStream_t s = t->set.h->stream;
-    int used = 0;
-    for (int k = 0; k < t->td.kf_cap; ++k) {
-        if (!t->kf_live[k] || t->m_cnt[k] == 0) { if (!t->kf_live[k]) t->m_cnt[k] = 0; continue; }
-        const size_t n = (size_t)t->m_cnt[k], o = (size_t)t->m_off[k];
-        for (int q = 0; q < 2; ++q) CU(cudaMemcpyAsync(t->arena_i[other][q] + used, t->arena_i[t->arena_cur][q] + o, n * sizeof(int), cudaMemcpyDeviceToDevice, s));
-        for (int q = 0; q < 3; ++q) CU(cudaMemcpyAsync(t->arena_f[other][q] + used, t->arena_f[t->arena_cur][q] + o, n * sizeof(float), cudaMemcpyDeviceToDevice, s));
-        t->m_off[k] = used;
-        used += (int)n;
-    }
-    t->arena_cur = other; t->arena_used = used;
-    t->point_arena();
-    return KBA_OK;
-}
-
-int kba_track_push_keyframe(kba_track* t, int32_t slot, const double* pose7, const double* plane4, int32_t n, const int32_t* lm,
-                            const int32_t* cam, const float* u, const float* v, const float* d) {
-    if (!t || !pose7 || n < 0 || slot < 0 || slot >= t->td.kf_cap || (n > 0 && (!lm || !u || !v || !d)))
-        return fail(KBA_ERR_BAD_ARG, "bad argument to kba_track_push_keyframe");
-    if (t->kf_live[slot]) return fail(KBA_ERR_BAD_ARG, "kba_track_push_keyframe: slot in use (drop it first)");
-    for (int i = 0; i < n; ++i)
-        if (lm[i] < 0 || lm[i] >= t->td.lm_cap || (cam && (cam[i] < 0 || cam[i] >= t->n_cam))) return fail(KBA_ERR_BAD_ARG, "kba_track_push_keyframe: landmark slot / camera out of range");
-    CU(cudaSetDevice(t->set.h->device));
-    if (t->arena_used + n > t->td.m_cap) {
-        const int rc = track_compact(t);
-        if (rc != KBA_OK) return rc;
-        if (t->arena_used + n > t->td.m_cap) return fail(KBA_ERR_CAPACITY, "kba_track_push_keyframe: measurement arena full");
-    }
-    cudaStream_t s = t->set.h->stream;
-    for (int i0 = 0; i0 < n; i0 += t->push_cap) {  // staged through pinned memory in chunks
-        const int m = std::min(t->push_cap, n - i0);
-        memcpy(t->p_lm.h, lm + i0, m * sizeof(int));
-        if (cam) memcpy(t->p_cam.h, cam + i0, m * sizeof(int)); else memset(t->p_cam.h, 0, m * sizeof(int));
-        memcpy(t->p_u.h, u + i0, m * sizeof(float)); memcpy(t->p_v.h, v + i0, m * sizeof(float)); memcpy(t->p_d.h, d + i0, m * sizeof(float));
-        const size_t o = (size_t)t->arena_used + i0;
-        CU(cudaMemcpyAsync(t->td.m_lm + o, t->p_lm.h, m * sizeof(int), cudaMemcpyHostToDevice, s));
-        CU(cudaMemcpyAsync(t->td.m_cam + o, t->p_cam.h, m * sizeof(int), cudaMemcpyHostToDevice, s));
-        CU(cudaMemcpyAsync(t->td.m_u + o, t->p_u.h, m * sizeof(float), cudaMemcpyHostToDevice, s));
-        CU(cudaMemcpyAsync(t->td.m_v + o, t->p_v.h, m * sizeof(float), cudaMemcpyHostToDevice, s));
-        CU(cudaMemcpyAsync(t->td.m_d + o, t->p_d.h, m * sizeof(float), cudaMemcpyHostToDevice, s));
-        CU(cudaStreamSynchronize(s));
-    }
-    t->m_off[slot] = t->arena_used; t->m_cnt[slot] = n; t->kf_live[slot] = 1;
-    t->gen++;
-    t->arena_used += n;
-    t->h2d_push += (int64_t)n * 20 + 11 * 8;
-    const int rc = track_upload_layout(t);
-    if (rc != KBA_OK) return rc;
-    return kba_track_set_keyframe_pose(t, slot, pose7, plane4);
-}
-
-int kba_track_drop_keyframe(kba_track* t, int32_t slot) {
-    if (!t || slot < 0 || slot >= t->td.kf_cap) return fail(KBA_ERR_BAD_ARG, "bad argument to kba_track_drop_keyframe");
-    t->kf_live[slot] = 0;  // the arena space is reclaimed by the next compaction
-    t->gen++;
-    return KBA_OK;
-}
-
-// rows of `width` doubles into their store slots: staged through pinned memory, one copy + one scatter kernel per chunk
-static int track_scatter(kba_track* t, double* dst, int cap_slots, int n, const int32_t* slot, const double* src, int width) {
-    cudaStream_t s = t->set.h->stream;
-    for (int i0 = 0; i0 < n; i0 += t->set_cap) {
-        const int m = std::min(t->set_cap, n - i0);
-        for (int i = 0; i < m; ++i)
-            if (slot[i0 + i] < 0 || slot[i0 + i] >= cap_slots) return fail(KBA_ERR_BAD_ARG, "kba_track: slot out of range");
-        memcpy(t->p_slot.h, slot + i0, m * sizeof(int));
-        memcpy(t->p_dbl.h, src + (size_t)width * i0, (size_t)width * m * sizeof(double));
-        CU(cudaMemcpyAsync(t->p_slot.d, t->p_slot.h, m * sizeof(int), cudaMemcpyHostToDevice, s));
-        CU(cudaMemcpyAsync(t->p_dbl.d, t->p_dbl.h, (size_t)width * m * sizeof(double), cudaMemcpyHostToDevice, s));
-        launch_scatter_rows(dst, t->p_slot.d, t->p_dbl.d, m, width, s);
-        CU(cudaStreamSynchronize(s));  // the staging buffers are reused
-    }
-    return KBA_OK;
-}
-
-int kba_track_set_keyframe_poses(kba_track* t, int32_t n, const int32_t* slot, const double* pose7s, const double* plane4s) {
-    if (!t || n < 0 || (n > 0 && (!slot || !pose7s))) return fail(KBA_ERR_BAD_ARG, "bad argument to kba_track_set_keyframe_poses");
-    CU(cudaSetDevice(t->set.h->device));
-    t->gen++;
-    int rc = track_scatter(t, t->td.kf_pose, t->td.kf_cap, n, slot, pose7s, 7);
-    if (rc == KBA_OK && plane4s) rc = track_scatter(t, t->td.kf_plane, t->td.kf_cap, n, slot, plane4s, 4);
-    return rc;
-}
-
-int kba_track_set_keyframe_pose(kba_track* t, int32_t slot, const double* pose7, const double* plane4) {
-    static const double kNoPlane[4] = {0., 0., 1., 0.};
-    return kba_track_set_keyframe_poses(t, 1, &slot, pose7, plane4 ? plane4 : kNoPlane);
-}
-
-int kba_track_set_landmarks(kba_track* t, int32_t n, const int32_t* slot, const double* pos3, const double* weight) {
-    if (!t || n < 0 || (n > 0 && !slot)) return fail(KBA_ERR_BAD_ARG, "bad argument to kba_track_set_landmarks");
-    CU(cudaSetDevice(t->set.h->device));
-    t->gen++;
-    int rc = KBA_OK;
-    if (pos3) rc = track_scatter(t, t->td.lm_pos, t->td.lm_cap, n, slot, pos3, 3);
-    if (rc == KBA_OK && weight) rc = track_scatter(t, t->td.lm_weight, t->td.lm_cap, n, slot, weight, 1);
-    t->h2d_push += (int64_t)n * ((pos3 ? 24 : 0) + (weight ? 8 : 0) + 4);
-    return rc;
 }
 
 // one solve of the stored windows of tracks ts[0..n) as one batch, window i = ts[i]'s; qs[i] is checked by track_check or sits
@@ -2151,6 +2026,7 @@ static int check_slot_lists(kba_track* t, int n_kf, const int32_t* kf_slot, int 
 //   sits_out(q)          a group's request that sits the call out: not checked, except what sit_out_check reads; a single
 //                        request is checked, and then does not run (a reclaim of an empty range: the other checks refuse it)
 //   sat_out(o, group)    what a request that sat out writes once the call succeeded
+//                        (the store writes have no outputs: out is null, and neither is called)
 //   make, check          the request of one window, and every check of it before anything is uploaded
 //   capacity(n, ts, ..)  the staging's upload and download bytes for tracks ts[0..n) at their capacities (n = 1: a single call's)
 //   run                  the requests that do not sit out as the windows of one launch sequence; a failure of request w it
@@ -2169,9 +2045,9 @@ static int store_call(TrackSet& s, bool group, const std::string& who, const typ
         int rc;
         typename C::Req r;
         if (group && sits_out) {
-            rc = C::sit_out_check(out[i], why);
+            rc = out ? C::sit_out_check(out[i], why) : KBA_OK;
         } else {
-            r = C::make(s.tracks[i], req[i], out + i);
+            r = C::make(s.tracks[i], req[i], out ? out + i : nullptr);
             rc = C::check(r, why);
         }
         if (rc != KBA_OK) return fail(rc, who + track_prefix(group, i) + why);
@@ -2194,7 +2070,7 @@ static int store_call(TrackSet& s, bool group, const std::string& who, const typ
         if (rc != KBA_OK) return bad < 0 ? rc : fail(rc, who + track_prefix(group, track_of[bad]) + why);
         s.last = &st->counts;
     }
-    for (int i = 0; i < n; ++i)
+    for (int i = 0; i < n && out; ++i)
         if (C::sits_out(req[i])) C::sat_out(out + i, group);
     return KBA_OK;
 }
@@ -3496,6 +3372,380 @@ int kba_track_group_solve_ranked(kba_track_group* g, const kba_ranked_request* r
 }
 int kba_track_group_solve_ranked_opts(kba_track_group* g, const kba_ranked_request* req, const kba_options* opts, kba_result* res) {
     return group_solve_ranked(g, req, true, opts, res, "kba_track_group_solve_ranked_opts: ");
+}
+
+// ---------------------------------------------------------------------------------------------------------------------
+// store writes of a track and of a group (include/kba_b200.h, kba_track_push_keyframe / kba_track_group_push_keyframes, the drops,
+// landmark values and keyframe poses; kernels in kba_store.cu and kba_pack.cu): a single call is a one-track call of store_call.
+// A call checks every request, then makes one upload, one launch sequence and one synchronisation; more only when its rows
+// exceed the staging, which holds the tracks' rows of one push (up to 65536 each) or one window's landmarks (win_landmarks).
+// ---------------------------------------------------------------------------------------------------------------------
+static size_t align16(size_t b) { return (b + 15) & ~(size_t)15; }
+
+// the writes have no outputs
+struct NoOut {};
+struct WriteCall {
+    using Out = NoOut;
+    static int sit_out_check(const Out&, std::string&) { return KBA_OK; }
+    static void sat_out(Out*, bool) {}
+};
+
+struct PushReq {
+    kba_track* t = nullptr;
+    const kba_push_request* q = nullptr;
+};
+
+// every check of kba_track_push_keyframe, the arena's capacity decided from the host mirror: nothing is compacted for a push that
+// cannot fit
+static int push_check(const PushReq& r, std::string& why) {
+    const kba_track* t = r.t;
+    const kba_push_request& q = *r.q;
+    if (!q.pose7 || q.n_meas < 0 || q.kf_slot < 0 || q.kf_slot >= t->td.kf_cap || (q.n_meas > 0 && (!q.lm_slot || !q.u || !q.v || !q.d))) {
+        why = "null argument, negative size or keyframe slot out of range"; return KBA_ERR_BAD_ARG;
+    }
+    if (t->kf_live[q.kf_slot]) { why = "slot in use (drop it first)"; return KBA_ERR_BAD_ARG; }
+    for (int i = 0; i < q.n_meas; ++i)
+        if (q.lm_slot[i] < 0 || q.lm_slot[i] >= t->td.lm_cap || (q.cam && (q.cam[i] < 0 || q.cam[i] >= t->n_cam))) {
+            why = "landmark slot / camera out of range"; return KBA_ERR_BAD_ARG;
+        }
+    long long live = 0;
+    for (int k = 0; k < t->td.kf_cap; ++k) live += t->kf_live[k] ? t->m_cnt[k] : 0;
+    if (live + q.n_meas > t->td.m_cap) { why = "measurement arena full"; return KBA_ERR_CAPACITY; }
+    return KBA_OK;
+}
+
+// rows of one push staged per track: larger pushes go up in several flushes
+constexpr int kPushStageRows = 1 << 16;
+
+// W checked pushes of distinct tracks.  The host mirror decides every offset first: a track whose arena has no room left compacts
+// (its live keyframes in slot order into the other arena, as runs of k_arena_compact), and each keyframe goes to the end of its
+// track's arena (segments of k_store_append, which also write its layout, pose and plane).  The staging, flushed when its rows are
+// full: compaction records | runs | segments | the five columns (lm, cam, u, v, d) of `stride` words; a segment's rows start at a
+// column offset congruent to their arena offset modulo 4, so that the copies run on 16-byte vectors.
+static int push_run(kba_handle* h, StoreStage& st, int W, const PushReq* r) {
+    static const double kNoPlane[4] = {0., 0., 1., 0.};
+    CU(cudaSetDevice(h->device));
+    cudaStream_t s = h->stream;
+    std::vector<CompactTrack> ct;
+    std::vector<CompactRun> runs;
+    std::vector<StoreAppend> app(W);
+    int max_run = 0;
+    for (int w = 0; w < W; ++w) {
+        kba_track* t = r[w].t;
+        const kba_push_request& q = *r[w].q;
+        if (t->arena_used + q.n_meas > t->td.m_cap) {
+            const int cur = t->arena_cur, other = 1 - cur;
+            CompactTrack c;
+            for (int j = 0; j < 2; ++j) { c.src[j] = (const unsigned*)t->arena_i[cur][j]; c.dst[j] = (unsigned*)t->arena_i[other][j]; }
+            for (int j = 0; j < 3; ++j) { c.src[2 + j] = (const unsigned*)t->arena_f[cur][j]; c.dst[2 + j] = (unsigned*)t->arena_f[other][j]; }
+            c.m_off = t->td.m_off; c.m_cnt = t->td.m_cnt;
+            int used = 0;
+            for (int k = 0; k < t->td.kf_cap; ++k) {
+                const int n = t->m_cnt[k];
+                if (!t->kf_live[k]) {  // a dropped keyframe's count is cleared
+                    if (n) { runs.push_back(CompactRun{(int)ct.size(), k, 0, t->m_off[k], 0, 0}); t->m_cnt[k] = 0; }
+                    continue;
+                }
+                if (n == 0) continue;
+                runs.push_back(CompactRun{(int)ct.size(), k, t->m_off[k], used, n, 0});
+                max_run = std::max(max_run, n);
+                t->m_off[k] = used;
+                used += n;
+            }
+            ct.push_back(c);
+            t->arena_cur = other; t->arena_used = used;
+            t->point_arena();
+        }
+        StoreAppend& a = app[w];
+        a.col[0] = (unsigned*)t->td.m_lm; a.col[1] = (unsigned*)t->td.m_cam;
+        a.col[2] = (unsigned*)t->td.m_u; a.col[3] = (unsigned*)t->td.m_v; a.col[4] = (unsigned*)t->td.m_d;
+        a.m_off = t->td.m_off; a.m_cnt = t->td.m_cnt; a.kf_pose = t->td.kf_pose; a.kf_plane = t->td.kf_plane;
+        memcpy(a.pose, q.pose7, sizeof(a.pose));
+        memcpy(a.plane, q.plane4 ? q.plane4 : kNoPlane, sizeof(a.plane));
+        a.slot = q.kf_slot; a.off = t->arena_used; a.cnt = q.n_meas; a.cam_zero = q.cam ? 0 : 1;
+        t->m_off[q.kf_slot] = t->arena_used; t->m_cnt[q.kf_slot] = q.n_meas; t->kf_live[q.kf_slot] = 1;
+        t->arena_used += q.n_meas;
+        t->gen++;
+        t->h2d_push += (int64_t)q.n_meas * 20 + 11 * 8;
+    }
+    // ---- segments, flushed when the staging's rows are full (the first flush carries the compactions)
+    const size_t rec = align16(sizeof(CompactTrack) * ct.size()) + align16(sizeof(CompactRun) * runs.size()) +
+                       align16(sizeof(StoreAppend) * (size_t)W);
+    const int cap = (int)(((st.up.n - rec) / 20) & ~(size_t)3);
+    std::vector<StoreAppend> segs;
+    std::vector<int> seg_w;
+    int used = 0, max_rows = 0;
+    bool first = true;
+    int64_t up = 0;
+    auto flush = [&]() -> int {
+        const size_t nct = first ? ct.size() : 0, nrun = first ? runs.size() : 0;
+        const size_t o_run = align16(sizeof(CompactTrack) * nct), o_app = o_run + align16(sizeof(CompactRun) * nrun);
+        const size_t o_col = o_app + align16(sizeof(StoreAppend) * segs.size());
+        const int stride = (used + 3) & ~3;
+        unsigned char* hb = st.up.h;
+        if (nct) memcpy(hb, ct.data(), sizeof(CompactTrack) * nct);
+        if (nrun) memcpy(hb + o_run, runs.data(), sizeof(CompactRun) * nrun);
+        memcpy(hb + o_app, segs.data(), sizeof(StoreAppend) * segs.size());
+        unsigned* col = reinterpret_cast<unsigned*>(hb + o_col);
+        for (size_t i = 0; i < segs.size(); ++i) {
+            const StoreAppend& a = segs[i];
+            const kba_push_request& q = *r[seg_w[i]].q;
+            if (a.n == 0) continue;
+            const size_t b = 4 * (size_t)a.n;
+            memcpy(col + a.src, q.lm_slot + a.seg, b);
+            if (q.cam) memcpy(col + stride + a.src, q.cam + a.seg, b);
+            memcpy(col + 2 * (size_t)stride + a.src, q.u + a.seg, b);
+            memcpy(col + 3 * (size_t)stride + a.src, q.v + a.seg, b);
+            memcpy(col + 4 * (size_t)stride + a.src, q.d + a.seg, b);
+        }
+        const size_t bytes = o_col + 20 * (size_t)stride;
+        CU(cudaMemcpyAsync(st.up.d, hb, bytes, cudaMemcpyHostToDevice, s));
+        const unsigned char* db = st.up.d;
+        launch_store_push(reinterpret_cast<const CompactTrack*>(db), reinterpret_cast<const CompactRun*>(db + o_run), (int)nrun, max_run,
+                          reinterpret_cast<const StoreAppend*>(db + o_app), (int)segs.size(), max_rows,
+                          reinterpret_cast<const unsigned*>(db + o_col), stride, s);
+        CU(cudaGetLastError());
+        CU(wait_stream(h));  // the staging is reused by the next flush
+        up += (int64_t)bytes;
+        first = false; segs.clear(); seg_w.clear(); used = 0; max_rows = 0;
+        return KBA_OK;
+    };
+    for (int w = 0; w < W; ++w) {
+        const int n = app[w].cnt;
+        for (int done = 0;;) {  // one segment per flush; a keyframe without measurements is one empty segment
+            const int dst = app[w].off + done, src = used + ((dst - used) & 3);
+            const int m = std::min(n - done, cap - src);
+            if (m < 0 || (m == 0 && done < n)) {
+                const int rc = flush();
+                if (rc != KBA_OK) return rc;
+                continue;
+            }
+            StoreAppend a = app[w];
+            a.seg = done; a.n = m; a.src = src;
+            segs.push_back(a); seg_w.push_back(w);
+            used = src + m; max_rows = std::max(max_rows, m); done += m;
+            if (done >= n) break;
+        }
+    }
+    const int rc = flush();
+    if (rc != KBA_OK) return rc;
+    st.counts.h2d = up;
+    st.counts.d2h = 0;
+    return KBA_OK;
+}
+
+struct Push : WriteCall {
+    using Request = kba_push_request;
+    using Req = PushReq;
+    static constexpr StoreCall slot = kPushCall;
+    static constexpr const char* staging = "keyframe";
+    static bool sits_out(const Request& q) { return q.kf_slot < 0; }
+    static Req make(kba_track* t, const Request& q, Out*) { return PushReq{t, &q}; }
+    static int check(Req& r, std::string& why) { return push_check(r, why); }
+    static void capacity(int n, kba_track* const* ts, size_t& up, size_t& down) {  // every track pushing and compacting
+        size_t kfs = 0, rows = 4 * (size_t)n + 8;
+        for (int i = 0; i < n; ++i) { kfs += (size_t)ts[i]->td.kf_cap; rows += (size_t)std::min(ts[i]->td.m_cap, kPushStageRows); }
+        up = align16(sizeof(CompactTrack) * n) + align16(sizeof(CompactRun) * kfs) + align16(sizeof(StoreAppend) * n) + 20 * rows;
+        down = 0;
+    }
+    static int run(kba_handle* h, StoreStage& st, int W, Req* r, int&, std::string&) { return push_run(h, st, W, r); }
+};
+
+// a drop moves nothing: the arena space of the keyframe is reclaimed by the next compaction
+struct DropReq {
+    kba_track* t = nullptr;
+    int32_t slot = -1;
+};
+struct Drop : WriteCall {
+    using Request = int32_t;
+    using Req = DropReq;
+    static constexpr StoreCall slot = kPushCall;
+    static constexpr const char* staging = "keyframe";
+    static bool sits_out(const Request& q) { return q < 0; }
+    static Req make(kba_track* t, const Request& q, Out*) { return DropReq{t, q}; }
+    static int check(Req& r, std::string& why) {
+        if (r.slot >= 0 && r.slot < r.t->td.kf_cap) return KBA_OK;
+        why = "keyframe slot out of range"; return KBA_ERR_BAD_ARG;
+    }
+    static void capacity(int n, kba_track* const* ts, size_t& up, size_t& down) { Push::capacity(n, ts, up, down); }
+    static int run(kba_handle*, StoreStage& st, int W, Req* r, int&, std::string&) {
+        for (int w = 0; w < W; ++w) { r[w].t->kf_live[r[w].slot] = 0; r[w].t->gen++; }
+        st.counts = Transfer{};
+        return KBA_OK;
+    }
+};
+
+// one landmark or keyframe write of track t: n rows of two arrays of widths wa, wb (either may be NULL) into dst_a, dst_b by slot
+struct ScatterReq {
+    kba_track* t = nullptr;
+    int n = 0;
+    const int32_t* slot = nullptr;
+    const double* a = nullptr;
+    const double* b = nullptr;
+};
+
+// rows per track of a scatter's staging: one window's landmarks
+static size_t scatter_rows(const kba_track* t) { return (size_t)std::max(t->caps.win_landmarks, 64); }
+static size_t scatter_records(int W) { return 2 * align16(sizeof(ScatterWin) * (size_t)W) + 16; }
+
+// W checked writes of distinct tracks: the slots | rows of array a | rows of array b, with a window record per track and array;
+// one k_scatter_rows launch per array, flushed when the staging's rows are full
+static int scatter_run(kba_handle* h, StoreStage& st, int W, const ScatterReq* r, int wa, int wb, bool landmarks) {
+    CU(cudaSetDevice(h->device));
+    cudaStream_t s = h->stream;
+    for (int w = 0; w < W; ++w) r[w].t->gen++;
+    st.counts = Transfer{};
+    bool any = false;
+    for (int w = 0; w < W; ++w) any |= r[w].a || r[w].b;
+    if (!any) return KBA_OK;
+    struct Seg { int w, done, m; };
+    std::vector<Seg> segs;
+    const int cap = (int)((st.up.n - scatter_records(W)) / (4 + 8 * (size_t)(wa + wb)));
+    int rows = 0;
+    auto flush = [&]() -> int {
+        std::vector<ScatterWin> win_a, win_b;
+        int ra = 0, rb = 0, max_a = 0, max_b = 0;
+        int r0 = 0;
+        for (const Seg& g : segs) {
+            const ScatterReq& q = r[g.w];
+            const TrackDev& td = q.t->td;
+            if (q.a) { ScatterWin x; x.dst = landmarks ? td.lm_pos : td.kf_pose; x.slot0 = r0; x.val0 = ra; x.n = g.m; win_a.push_back(x); ra += g.m; max_a = std::max(max_a, g.m); }
+            if (q.b) { ScatterWin x; x.dst = landmarks ? td.lm_weight : td.kf_plane; x.slot0 = r0; x.val0 = rb; x.n = g.m; win_b.push_back(x); rb += g.m; max_b = std::max(max_b, g.m); }
+            r0 += g.m;
+        }
+        const size_t o_b = align16(sizeof(ScatterWin) * win_a.size()), o_slot = o_b + align16(sizeof(ScatterWin) * win_b.size());
+        const size_t o_va = o_slot + align16(4 * (size_t)r0), o_vb = o_va + 8 * (size_t)wa * ra, bytes = o_vb + 8 * (size_t)wb * rb;
+        unsigned char* hb = st.up.h;
+        memcpy(hb, win_a.data(), sizeof(ScatterWin) * win_a.size());
+        memcpy(hb + o_b, win_b.data(), sizeof(ScatterWin) * win_b.size());
+        int* slot_h = reinterpret_cast<int*>(hb + o_slot);
+        double* va = reinterpret_cast<double*>(hb + o_va), *vb = reinterpret_cast<double*>(hb + o_vb);
+        for (const Seg& g : segs) {
+            const ScatterReq& q = r[g.w];
+            memcpy(slot_h, q.slot + g.done, 4 * (size_t)g.m);
+            slot_h += g.m;
+            if (q.a) { memcpy(va, q.a + (size_t)wa * g.done, 8 * (size_t)wa * g.m); va += (size_t)wa * g.m; }
+            if (q.b) { memcpy(vb, q.b + (size_t)wb * g.done, 8 * (size_t)wb * g.m); vb += (size_t)wb * g.m; }
+        }
+        CU(cudaMemcpyAsync(st.up.d, hb, bytes, cudaMemcpyHostToDevice, s));
+        const unsigned char* db = st.up.d;
+        const int* slot_d = reinterpret_cast<const int*>(db + o_slot);
+        launch_scatter_rows(reinterpret_cast<const ScatterWin*>(db), (int)win_a.size(), max_a, slot_d,
+                            reinterpret_cast<const double*>(db + o_va), wa, s);
+        launch_scatter_rows(reinterpret_cast<const ScatterWin*>(db + o_b), (int)win_b.size(), max_b, slot_d,
+                            reinterpret_cast<const double*>(db + o_vb), wb, s);
+        CU(cudaGetLastError());
+        CU(wait_stream(h));  // the staging is reused by the next flush
+        st.counts.h2d += (int64_t)bytes;
+        segs.clear(); rows = 0;
+        return KBA_OK;
+    };
+    for (int w = 0; w < W; ++w) {
+        if (!r[w].a && !r[w].b) continue;
+        for (int done = 0; done < r[w].n;) {
+            if (rows == cap) { const int rc = flush(); if (rc != KBA_OK) return rc; }
+            const int m = std::min(r[w].n - done, cap - rows);
+            segs.push_back(Seg{w, done, m});
+            rows += m; done += m;
+        }
+    }
+    return segs.empty() ? KBA_OK : flush();
+}
+
+// every check of kba_track_set_landmarks / kba_track_set_keyframe_poses: slots in range (a slot listed twice is written in an
+// unspecified order, as it always was)
+static int scatter_check(const ScatterReq& r, bool need_a, int cap_slots, const char* what, std::string& why) {
+    if (r.n < 0 || (r.n > 0 && (!r.slot || (need_a && !r.a)))) { why = "null argument or negative size"; return KBA_ERR_BAD_ARG; }
+    for (int i = 0; i < r.n; ++i)
+        if (r.slot[i] < 0 || r.slot[i] >= cap_slots) { why = std::string(what) + " slot out of range"; return KBA_ERR_BAD_ARG; }
+    return KBA_OK;
+}
+
+extern "C++" {  // templates have C++ linkage
+template <class Q, bool Landmarks>
+struct Scatter : WriteCall {
+    using Request = Q;
+    using Req = ScatterReq;
+    static constexpr int wa = Landmarks ? 3 : 7, wb = Landmarks ? 1 : 4;
+    static constexpr StoreCall slot = Landmarks ? kLandmarkWriteCall : kPoseWriteCall;
+    static constexpr const char* staging = Landmarks ? "landmark" : "keyframe pose";
+    static bool sits_out(const Request& q) { return q.n == 0; }
+    static Req make(kba_track* t, const kba_landmark_write& q, Out*) { return ScatterReq{t, q.n, q.lm_slot, q.pos3, q.weight}; }
+    static Req make(kba_track* t, const kba_pose_write& q, Out*) { return ScatterReq{t, q.n, q.kf_slot, q.pose7s, q.plane4s}; }
+    static int check(Req& r, std::string& why) {
+        return Landmarks ? scatter_check(r, false, r.t->td.lm_cap, "landmark", why) : scatter_check(r, true, r.t->td.kf_cap, "keyframe", why);
+    }
+    static void capacity(int n, kba_track* const* ts, size_t& up, size_t& down) {
+        size_t rows = 0;
+        for (int i = 0; i < n; ++i) rows += scatter_rows(ts[i]);
+        up = scatter_records(n) + (4 + 8 * (size_t)(wa + wb)) * rows;
+        down = 0;
+    }
+    static int run(kba_handle* h, StoreStage& st, int W, Req* r, int&, std::string&) {
+        if (Landmarks)
+            for (int w = 0; w < W; ++w) r[w].t->h2d_push += (int64_t)r[w].n * ((r[w].a ? 24 : 0) + (r[w].b ? 8 : 0) + 4);
+        return scatter_run(h, st, W, r, wa, wb, Landmarks);
+    }
+};
+}  // extern "C++"
+using LandmarkWrite = Scatter<kba_landmark_write, true>;
+using PoseWrite = Scatter<kba_pose_write, false>;
+
+int kba_track_push_keyframe(kba_track* t, int32_t slot, const double* pose7, const double* plane4, int32_t n, const int32_t* lm,
+                            const int32_t* cam, const float* u, const float* v, const float* d) {
+    static const std::string who = "kba_track_push_keyframe: ";
+    if (!t) return fail(KBA_ERR_BAD_ARG, who + "null argument");
+    const kba_push_request q = {slot, n, pose7, plane4, lm, cam, u, v, d};
+    return store_call<Push>(t->set, false, who, &q, nullptr);
+}
+
+int kba_track_group_push_keyframes(kba_track_group* g, const kba_push_request* req) {
+    static const std::string who = "kba_track_group_push_keyframes: ";
+    if (!g || !req) return fail(KBA_ERR_BAD_ARG, who + "null argument");
+    return store_call<Push>(g->set, true, who, req, nullptr);
+}
+
+int kba_track_drop_keyframe(kba_track* t, int32_t slot) {
+    static const std::string who = "kba_track_drop_keyframe: ";
+    if (!t) return fail(KBA_ERR_BAD_ARG, who + "null argument");
+    return store_call<Drop>(t->set, false, who, &slot, nullptr);
+}
+
+int kba_track_group_drop_keyframes(kba_track_group* g, const int32_t* kf_slot) {
+    static const std::string who = "kba_track_group_drop_keyframes: ";
+    if (!g || !kf_slot) return fail(KBA_ERR_BAD_ARG, who + "null argument");
+    return store_call<Drop>(g->set, true, who, kf_slot, nullptr);
+}
+
+int kba_track_set_landmarks(kba_track* t, int32_t n, const int32_t* slot, const double* pos3, const double* weight) {
+    static const std::string who = "kba_track_set_landmarks: ";
+    if (!t) return fail(KBA_ERR_BAD_ARG, who + "null argument");
+    const kba_landmark_write q = {n, 0, slot, pos3, weight};
+    return store_call<LandmarkWrite>(t->set, false, who, &q, nullptr);
+}
+
+int kba_track_group_set_landmarks(kba_track_group* g, const kba_landmark_write* req) {
+    static const std::string who = "kba_track_group_set_landmarks: ";
+    if (!g || !req) return fail(KBA_ERR_BAD_ARG, who + "null argument");
+    return store_call<LandmarkWrite>(g->set, true, who, req, nullptr);
+}
+
+int kba_track_set_keyframe_poses(kba_track* t, int32_t n, const int32_t* slot, const double* pose7s, const double* plane4s) {
+    static const std::string who = "kba_track_set_keyframe_poses: ";
+    if (!t) return fail(KBA_ERR_BAD_ARG, who + "null argument");
+    const kba_pose_write q = {n, 0, slot, pose7s, plane4s};
+    return store_call<PoseWrite>(t->set, false, who, &q, nullptr);
+}
+
+int kba_track_set_keyframe_pose(kba_track* t, int32_t slot, const double* pose7, const double* plane4) {
+    static const double kNoPlane[4] = {0., 0., 1., 0.};
+    return kba_track_set_keyframe_poses(t, 1, &slot, pose7, plane4 ? plane4 : kNoPlane);
+}
+
+int kba_track_group_set_keyframe_poses(kba_track_group* g, const kba_pose_write* req) {
+    static const std::string who = "kba_track_group_set_keyframe_poses: ";
+    if (!g || !req) return fail(KBA_ERR_BAD_ARG, who + "null argument");
+    return store_call<PoseWrite>(g->set, true, who, req, nullptr);
 }
 
 }  // extern "C"

@@ -100,7 +100,44 @@ struct TrackGrid {
 // (device arrays of bd.n_win entries); desc[w].n_obs is written on the device
 void launch_track_gather(const BatchDev& bd, const PackRaw& raw_out, const TrackDev* tds, const TrackSel* sels, const TrackGrid& g,
                          cudaStream_t s);
-void launch_scatter_rows(double* dst, const int* slot, const double* src, int n, int width, cudaStream_t s);
+// rows of `width` doubles into store slots, for n windows (tracks) in one launch: row r of window w is row val0 + r of `val`, its
+// slot slot[slot0 + r], written to dst[slot * width ..]
+struct ScatterWin {
+    double* dst = nullptr;
+    int slot0 = 0, val0 = 0, n = 0, pad = 0;
+};
+void launch_scatter_rows(const ScatterWin* wins, int n_win, int max_rows, const int* slot, const double* val, int width, cudaStream_t s);
+
+// ---- store writes of a track group (kba_track_group_push_keyframes, kba_store.cu) ---------------------------------------
+// One staged segment of a pushed keyframe: rows src .. src + n of the staged columns (lm, cam, u, v, d, 4 bytes each) go to arena
+// entries off + seg .. of the track's current arena; the keyframe's layout (m_off = off, m_cnt = cnt), pose and plane are written
+// with it.  cam_zero: no camera column, every measurement is camera 0.
+struct StoreAppend {
+    unsigned* col[5] = {nullptr, nullptr, nullptr, nullptr, nullptr};  // the current arena: lm, cam, u, v, d
+    int* m_off = nullptr;
+    int* m_cnt = nullptr;
+    double* kf_pose = nullptr;
+    double* kf_plane = nullptr;
+    double pose[7] = {0, 0, 0, 0, 0, 0, 0};
+    double plane[4] = {0, 0, 0, 0};
+    int slot = 0, off = 0, cnt = 0, seg = 0, n = 0, src = 0, cam_zero = 0, pad = 0;
+};
+// one track's compaction: its live keyframes' runs copied from one arena into the other
+struct CompactTrack {
+    const unsigned* src[5] = {nullptr, nullptr, nullptr, nullptr, nullptr};
+    unsigned* dst[5] = {nullptr, nullptr, nullptr, nullptr, nullptr};
+    int* m_off = nullptr;
+    int* m_cnt = nullptr;
+};
+// one keyframe slot of a compaction: n entries from src to dst, then m_off[slot] = dst, m_cnt[slot] = n (n = 0: a dropped slot's
+// count cleared, dst its unchanged offset)
+struct CompactRun {
+    int track = 0, slot = 0, src = 0, dst = 0, n = 0, pad = 0;
+};
+// the compaction runs (if any), then the appends, on stream s: cols = the staged columns, 5 x stride entries
+void launch_store_push(const CompactTrack* ct, const CompactRun* runs, int n_runs, int max_run, const StoreAppend* app, int n_app,
+                       int max_rows, const unsigned* cols, int stride, cudaStream_t s);
+
 // results of every window w back into track store tds[w]
 void launch_track_writeback(const BatchDev& bd, const TrackDev* tds, const TrackSel* sels, const TrackGrid& g, cudaStream_t s);
 

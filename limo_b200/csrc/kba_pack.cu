@@ -456,14 +456,16 @@ __global__ void __launch_bounds__(256) k_track_writeback(BatchDev bd, const Trac
 }
 
 // dst[slot[i]][0..width) = src[i][0..width): host-staged rows into their store slots (poses, planes, landmark values)
-__global__ void __launch_bounds__(256) k_scatter_rows(double* dst, const int* slot, const double* src, int n, int width) {
+// window blockIdx.y's rows
+__global__ void __launch_bounds__(256) k_scatter_rows(const ScatterWin* wins, const int* slot, const double* val, int width) {
+    const ScatterWin w = wins[blockIdx.y];
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n * width) return;
+    if (i >= w.n * width) return;
     const int r = i / width, c = i - r * width;
-    dst[(size_t)slot[r] * width + c] = src[i];
+    w.dst[(size_t)slot[w.slot0 + r] * width + c] = val[(size_t)w.val0 * width + i];
 }
-void launch_scatter_rows(double* dst, const int* slot, const double* src, int n, int width, cudaStream_t s) {
-    if (n > 0) k_scatter_rows<<<(n * width + 255) / 256, 256, 0, s>>>(dst, slot, src, n, width);
+void launch_scatter_rows(const ScatterWin* wins, int n_win, int max_rows, const int* slot, const double* val, int width, cudaStream_t s) {
+    if (n_win > 0 && max_rows > 0) k_scatter_rows<<<dim3((max_rows * width + 255) / 256, n_win), 256, 0, s>>>(wins, slot, val, width);
     LCHK("k_scatter_rows");
 }
 
