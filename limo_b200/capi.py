@@ -5,12 +5,14 @@ computing call fails with KBA_ERR_CUDA when no sm_90 (H100) device is present.
 """
 import ctypes as C
 import functools
+import itertools
 import os
 
 import numpy as np
 
 from .capi_types import (KbaCounters, KbaCreateOut, KbaCreateRequest, KbaDeactivateOut, KbaDeactivateRequest, KbaDepthEntry, KbaDepthOut, KbaDepthRequest, KbaDrawFn, KbaEvalOut, KbaFlowOut, KbaFlowRequest, KbaLandmarkWrite, KbaLidarOptions, KbaOptions, KbaPoseWrite, KbaPushRequest, KbaRankedRequest, KbaRankOut, KbaRankRequest, KbaReclaimOut, KbaReclaimRequest, KbaResult, KbaSelectOut, KbaSelectParams, KbaSelectRequest,
-                         KbaTrackCaps, KbaTrackFrame, KbaTrackRequest, KbaWindow, Result, Window, c_double_p, c_int32_p)
+                         KbaTrackCaps, KbaTrackFrame, KbaTrackRequest, KbaWindow, Result, Window, c_double_p, c_float_p, c_int32_p,
+                         c_uint8_p)
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("KBA_LIB_PATH") or os.path.join(_HERE, "libkba_b200.so")  # KBA_LIB_PATH: instrumented builds
@@ -255,9 +257,83 @@ class Batch:
             pass
 
 
+def _arr(a, dtype, *shape):
+    """a as a contiguous array of dtype (reshaped to shape, if given); None stays None (a NULL pointer to the C call)"""
+    if a is None:
+        return None
+    a = np.ascontiguousarray(a, dtype=dtype)
+    return a.reshape(shape) if shape else a
+
+
+_c_int8_p, _depth_p = C.POINTER(C.c_int8), C.POINTER(KbaDepthEntry)
+
+
+def _p(a, ptype):
+    """a's data as the pointer type ptype, for a struct field or an argument; None stays None (NULL)"""
+    return None if a is None else a.ctypes.data_as(ptype)
+
+
+_I7 = [1.0, 0, 0, 0, 0, 0, 0]
+
+
+def _sel_window(n_kf, n_lm, kf_fixed=None, **scalars):
+    """the `sel` window of a solve of the store: it carries the sizes, the scalars and the ground-plane lists, and sizes the
+    solve's Result"""
+    return Window(np.tile(_I7, (n_kf, 1)), np.zeros(n_kf, np.uint8) if kf_fixed is None else kf_fixed, [[1.0, 0, 0]], [_I7],
+                  np.zeros((n_lm, 3)), np.ones(n_lm), np.zeros(n_lm + 1, dtype=np.int32), [], [], [], [], **scalars)
+
+
+def _filled(res):
+    """the result function of a solve into Result res: c is the KbaResult the call filled (res.c, or a group's array entry)"""
+    def done(c):
+        res.c = c
+        return res
+    return done
+
+
+def _idle(Req, n_kf):
+    """the entry of a track that sits a group solve (n_kf = 0) or pose-only call (n_kf = 1: its one pose) out: a zeroed request
+    and an idle Result"""
+    res = Result(_sel_window(n_kf, 0), 1)
+    return Req(), res.c, (), _filled(res)
+
+
+def _select_args(kf_slots, lm_slots, voxel_size=SELECT_DEFAULTS["voxel_size"], roi_far=SELECT_DEFAULTS["roi_far"],
+                 roi_middle=SELECT_DEFAULTS["roi_middle"]):
+    """a selection's lists and its kba_select_params as 5 doubles (voxel size xyz, roi_far, roi_middle), the struct's layout"""
+    vs = np.asarray(voxel_size, np.float64)
+    if vs.shape != (3,):
+        raise ValueError("voxel_size must have 3 entries")
+    prm = np.empty(5, np.float64)
+    prm[:3], prm[3], prm[4] = vs, roi_far, roi_middle
+    return _arr(kf_slots, np.int32, -1), _arr(lm_slots, np.int32, -1), prm
+
+
+def _select_outputs(n_cand):
+    """the output buffers of a selection over requests of n_cand[i] candidates, shared by the call (a call that succeeds writes
+    every entry), each request's offset co[i] in them and its n_near entry, and result(i) -> request i's dict of views"""
+    co = [0, *itertools.accumulate(n_cand)]
+    N = co[-1]
+    bufs = dict(cheiral=np.empty(N + 1, np.uint8), bin=np.empty(N + 1, np.int8), near_order=np.empty(N + 1, np.int32),
+                flow=np.empty(N + 1, np.float64), seen=np.empty(N + 1, np.int32))
+    n_near = np.zeros(len(n_cand), np.int32)
+
+    def result(i):
+        a, b = co[i], co[i + 1]
+        return dict(cheiral=bufs["cheiral"][a:b], bin=bufs["bin"][a:b], near_order=bufs["near_order"][a:a + int(n_near[i])],
+                    flow=bufs["flow"][a:b], seen=bufs["seen"][a:b])
+    return bufs, co, n_near, result
+
+
 class Track:
     """Persistent, device-resident sliding window (kba_track_*): keyframes are uploaded once when pushed, a solve sends only
-    the lists of active keyframe slots and selected landmark slots."""
+    the lists of active keyframe slots and selected landmark slots.
+
+    Each store call turns its keywords into C structs in one builder (Track._push_request, ._landmark_write, ._solve_request,
+    ...), which TrackGroup also calls, with a group request's keywords.  A builder returns (the request in the group ABI's
+    struct, the output struct or None, the arrays both point into -- outputs first -- which must stay alive during the call,
+    the function of the filled output struct that gives the call's result, or None).  The selection shares _select_args and
+    _select_outputs instead: its group call fills numpy records."""
 
     def __init__(self, handle, cam_intr, cam_pose, max_keyframes, max_landmarks, max_measurements, win_keyframes,
                  win_landmarks, win_observations, win_ground=0, win_rows=0):
@@ -273,99 +349,77 @@ class Track:
         _check(lib().kba_track_create(handle._p, C.byref(caps), len(intr), intr.ctypes.data_as(c_double_p),
                                       pose.ctypes.data_as(c_double_p), C.byref(self._p)))
 
-    @staticmethod
-    def _i32(a):
-        a = np.ascontiguousarray(a, dtype=np.int32)
-        return a, a.ctypes.data_as(C.POINTER(C.c_int32))
+    def _push_request(self, slot, pose7, lm_slot, u, v, d, cam=None, plane4=None):
+        pose, pl, lm, cm = _arr(pose7, np.float64), _arr(plane4, np.float64), _arr(lm_slot, np.int32, -1), _arr(cam, np.int32, -1)
+        uu, vv, dd = (_arr(x, np.float32) for x in (u, v, d))
+        q = KbaPushRequest(int(slot), len(lm), _p(pose, c_double_p), _p(pl, c_double_p), _p(lm, c_int32_p), _p(cm, c_int32_p),
+                           _p(uu, c_float_p), _p(vv, c_float_p), _p(dd, c_float_p))
+        return q, None, (pose, pl, lm, cm, uu, vv, dd), None
 
     def push_keyframe(self, slot, pose7, lm_slot, u, v, d, cam=None, plane4=None):
-        fp = C.POINTER(C.c_float)
-        pose = np.ascontiguousarray(pose7, dtype=np.float64)
-        pl = None if plane4 is None else np.ascontiguousarray(plane4, dtype=np.float64)
-        lm, lmp = self._i32(lm_slot)
-        cm, cmp_ = (None, C.cast(None, C.POINTER(C.c_int32))) if cam is None else self._i32(cam)
-        uu, vv, dd = (np.ascontiguousarray(x, dtype=np.float32) for x in (u, v, d))
-        _check(lib().kba_track_push_keyframe(self._p, int(slot), pose.ctypes.data_as(c_double_p),
-                                             C.cast(None, c_double_p) if pl is None else pl.ctypes.data_as(c_double_p), len(lm), lmp, cmp_,
-                                             uu.ctypes.data_as(fp), vv.ctypes.data_as(fp), dd.ctypes.data_as(fp)))
+        q, _, _keep, _ = self._push_request(slot, pose7, lm_slot, u, v, d, cam, plane4)
+        _check(lib().kba_track_push_keyframe(self._p, q.kf_slot, q.pose7, q.plane4, q.n_meas, q.lm_slot, q.cam, q.u, q.v, q.d))
 
     def drop_keyframe(self, slot):
         _check(lib().kba_track_drop_keyframe(self._p, int(slot)))
 
+    def _landmark_write(self, lm_slot, pos=None, weight=None):
+        lm, p, w = _arr(lm_slot, np.int32, -1), _arr(pos, np.float64, -1, 3), _arr(weight, np.float64)
+        q = KbaLandmarkWrite(n=len(lm), lm_slot=_p(lm, c_int32_p), pos3=_p(p, c_double_p), weight=_p(w, c_double_p))
+        return q, None, (lm, p, w), None
+
     def set_landmarks(self, lm_slot, pos=None, weight=None):
-        lm, lmp = self._i32(lm_slot)
-        p = None if pos is None else np.ascontiguousarray(pos, dtype=np.float64).reshape(-1, 3)
-        w = None if weight is None else np.ascontiguousarray(weight, dtype=np.float64)
-        _check(lib().kba_track_set_landmarks(self._p, len(lm), lmp, C.cast(None, c_double_p) if p is None else p.ctypes.data_as(c_double_p),
-                                             C.cast(None, c_double_p) if w is None else w.ctypes.data_as(c_double_p)))
+        q, _, _keep, _ = self._landmark_write(lm_slot, pos, weight)
+        _check(lib().kba_track_set_landmarks(self._p, q.n, q.lm_slot, q.pos3, q.weight))
+
+    def _pose_write(self, kf_slots, pose7s, plane4s=None):
+        kf, p, pl = _arr(kf_slots, np.int32, -1), _arr(pose7s, np.float64, -1, 7), _arr(plane4s, np.float64, -1, 4)
+        q = KbaPoseWrite(n=len(kf), kf_slot=_p(kf, c_int32_p), pose7s=_p(p, c_double_p), plane4s=_p(pl, c_double_p))
+        return q, None, (kf, p, pl), None
 
     def set_keyframe_poses(self, kf_slots, pose7s, plane4s=None):
-        kf, kfp = self._i32(kf_slots)
-        p = np.ascontiguousarray(pose7s, dtype=np.float64).reshape(-1, 7)
-        pl = None if plane4s is None else np.ascontiguousarray(plane4s, dtype=np.float64).reshape(-1, 4)
-        _check(lib().kba_track_set_keyframe_poses(self._p, len(kf), kfp, p.ctypes.data_as(c_double_p),
-                                                  C.cast(None, c_double_p) if pl is None else pl.ctypes.data_as(c_double_p)))
+        q, _, _keep, _ = self._pose_write(kf_slots, pose7s, plane4s)
+        _check(lib().kba_track_set_keyframe_poses(self._p, q.n, q.kf_slot, q.pose7s, q.plane4s))
 
-    @staticmethod
-    def _selection(kf_slots, kf_fixed, lm_slots, **scalars):
-        """the arrays of one solve and the `sel` window that carries its sizes, scalars and ground-plane lists"""
-        kf, _ = Track._i32(kf_slots)
-        lm, _ = Track._i32(lm_slots)
-        fx = np.ascontiguousarray(kf_fixed, dtype=np.uint8)
-        n_kf, n_lm = len(kf), len(lm)
-        sel = Window(np.tile([1.0, 0, 0, 0, 0, 0, 0], (n_kf, 1)), fx, [[1.0, 0, 0]], [[1.0, 0, 0, 0, 0, 0, 0]], np.zeros((n_lm, 3)),
-                     np.ones(n_lm), np.zeros(n_lm + 1, dtype=np.int32), [], [], [], [], **scalars)
-        return kf, fx, lm, sel
+    def _solve_request(self, capacity, kf_slots, kf_fixed, lm_slots, **scalars):
+        """capacity: the Result's iteration records"""
+        kf, fx, lm = _arr(kf_slots, np.int32, -1), _arr(kf_fixed, np.uint8), _arr(lm_slots, np.int32, -1)
+        sel = _sel_window(len(kf), len(lm), fx, **scalars)
+        res = Result(sel, capacity)
+        q = KbaTrackRequest(len(kf), _p(kf, c_int32_p), _p(fx, c_uint8_p), len(lm), _p(lm, c_int32_p), C.pointer(sel.c))
+        return q, res.c, (kf, fx, lm, sel), _filled(res)
 
     def solve(self, kf_slots, kf_fixed, lm_slots, opt=None, **scalars):
         """scalars: scale_kf0, scale_kf1, scale_weight, scale_value, plane_reg_weight, plane_dist_fixed, gp_lm, gp_kf, gp_weight.
         gp_lm without gp_kf / gp_weight: candidate ground landmarks (ascending indices into lm_slots), attached on the device
         (kba_track_solve); plane_reg_weight < 0: 10 iff a ground-plane residual is in the window."""
-        kf, fx, lm, sel = self._selection(kf_slots, kf_fixed, lm_slots, **scalars)
-        res = Result(sel, 256)
-        _check(lib().kba_track_solve(self._p, len(kf), kf.ctypes.data_as(c_int32_p), fx.ctypes.data_as(C.POINTER(C.c_uint8)), len(lm),
-                                     lm.ctypes.data_as(c_int32_p), C.byref(sel.c), C.byref(opt or default_options()), C.byref(res.c)))
-        return res
+        q, o, _keep, done = self._solve_request(256, kf_slots, kf_fixed, lm_slots, **scalars)
+        _check(lib().kba_track_solve(self._p, q.n_kf, q.kf_slot, q.kf_fixed, q.n_lm, q.lm_slot, q.sel, C.byref(opt or default_options()),
+                                     C.byref(o)))
+        return done(o)
 
-    @staticmethod
-    def _frame(fr, pose7, lm_slot, u, v, d, cam=None, speed=None):
-        """fill KbaTrackFrame `fr`; returns the arrays it points into (keep them alive for the call) and the frame's run count.
-        speed: None or a dict weight, dt, v_before (3), T_origin_before (7) -- the speed_* fields of a window"""
-        f32 = lambda a: np.ascontiguousarray(a, dtype=np.float32)
-        pose = np.ascontiguousarray(pose7, dtype=np.float64).reshape(7)
-        lm, lmp = Track._i32(lm_slot)
-        uu, vv, dd = f32(u), f32(v), f32(d)
-        cm = None if cam is None else Track._i32(cam)[0]
-        fr.n_meas = len(lm)
-        fr.pose7 = pose.ctypes.data_as(c_double_p)
-        fr.lm_slot = lmp
-        fr.cam = C.cast(None, c_int32_p) if cm is None else cm.ctypes.data_as(c_int32_p)
-        fp = C.POINTER(C.c_float)
-        fr.u, fr.v, fr.d = uu.ctypes.data_as(fp), vv.ctypes.data_as(fp), dd.ctypes.data_as(fp)
+    def _frame_request(self, capacity, pose7, lm_slot, u, v, d, cam=None, speed=None):
+        """speed: None or a dict weight, dt, v_before (3), T_origin_before (7) -- the speed_* fields of a window.  The Result
+        (capacity iteration records) has one landmark per run of lm_slot."""
+        pose, lm, cm = _arr(pose7, np.float64, 7), _arr(lm_slot, np.int32, -1), _arr(cam, np.int32, -1)
+        uu, vv, dd = (_arr(x, np.float32) for x in (u, v, d))
+        fr = KbaTrackFrame(n_meas=len(lm), pose7=_p(pose, c_double_p), lm_slot=_p(lm, c_int32_p), cam=_p(cm, c_int32_p),
+                           u=_p(uu, c_float_p), v=_p(vv, c_float_p), d=_p(dd, c_float_p), speed_weight=0.0, speed_dt=1.0)
         if speed:
             fr.speed_weight, fr.speed_dt = float(speed["weight"]), float(speed["dt"])
             fr.speed_v_before = (C.c_double * 3)(*[float(x) for x in speed["v_before"]])
             fr.speed_T_origin_before = (C.c_double * 7)(*[float(x) for x in speed["T_origin_before"]])
-        else:
-            fr.speed_weight, fr.speed_dt = 0.0, 1.0
         n_runs = int(1 + np.count_nonzero(lm[1:] != lm[:-1])) if len(lm) else 0
-        return (pose, lm, uu, vv, dd, cm), n_runs
-
-    @staticmethod
-    def _frame_result(n_runs, iterations_capacity):
-        sel = Window(np.tile([1.0, 0, 0, 0, 0, 0, 0], (1, 1)), [0], [[1.0, 0, 0]], [[1.0, 0, 0, 0, 0, 0, 0]], np.zeros((n_runs, 3)),
-                     np.ones(n_runs), np.zeros(n_runs + 1, dtype=np.int32), [], [], [], [])
-        return Result(sel, iterations_capacity)
+        res = Result(_sel_window(1, n_runs), capacity)
+        return fr, res.c, (pose, lm, uu, vv, dd, cm), _filled(res)
 
     def adjust_pose(self, pose7, lm_slot, u, v, d, cam=None, speed=None, opt=None, iterations_capacity=256):
         """adjustPoseOnly of one frame against this track's store (kba_track_adjust_pose): one free pose, landmarks read by slot
         (lm_slot: one contiguous run per landmark, in the caller's landmark order).  Returns a Result: kf_pose [1, 7],
         lm_rejected [runs], summaries and iterations; the store is not modified."""
-        fr = KbaTrackFrame()
-        keep, n_runs = self._frame(fr, pose7, lm_slot, u, v, d, cam, speed)
-        res = self._frame_result(n_runs, iterations_capacity)
-        _check(lib().kba_track_adjust_pose(self._p, C.byref(fr), C.byref(opt or default_options()), C.byref(res.c)))
-        return res
+        q, o, _keep, done = self._frame_request(iterations_capacity, pose7, lm_slot, u, v, d, cam, speed)
+        _check(lib().kba_track_adjust_pose(self._p, C.byref(q), C.byref(opt or default_options()), C.byref(o)))
+        return done(o)
 
     def select_landmarks(self, kf_slots, lm_slots, voxel_size=SELECT_DEFAULTS["voxel_size"], roi_far=SELECT_DEFAULTS["roi_far"],
                          roi_middle=SELECT_DEFAULTS["roi_middle"]):
@@ -374,87 +428,73 @@ class Track:
         defaults are LandmarkSparsificationSchemeVoxel::Parameters'.  Returns a dict of numpy arrays over the candidates:
         cheiral (uint8), bin (int8: 0 near, 1 middle, 2 far, -1 dropped), near_order (int32 candidate indices in ascending voxel
         index), flow (float64, NaN without a value), seen (int32)."""
-        kf, kfp = self._i32(kf_slots)
-        lm, lmp = self._i32(lm_slots)
-        n = len(lm)
-        out = dict(cheiral=np.zeros(n, np.uint8), bin=np.zeros(n, np.int8), near_order=np.zeros(n, np.int32),
-                   flow=np.zeros(n, np.float64), seen=np.zeros(n, np.int32))
-        n_near = np.zeros(1, np.int32)
-        o = KbaSelectOut(out["cheiral"].ctypes.data_as(C.POINTER(C.c_uint8)), out["bin"].ctypes.data_as(C.POINTER(C.c_int8)),
-                         out["near_order"].ctypes.data_as(c_int32_p), n_near.ctypes.data_as(c_int32_p),
-                         out["flow"].ctypes.data_as(c_double_p), out["seen"].ctypes.data_as(c_int32_p))
-        p = KbaSelectParams((C.c_double * 3)(*[float(x) for x in voxel_size]), float(roi_far), float(roi_middle))
-        _check(lib().kba_track_select_landmarks(self._p, len(kf), kfp, n, lmp, C.byref(p), C.byref(o)))
-        out["near_order"] = out["near_order"][:int(n_near[0])].copy()
-        return out
+        kf, lm, prm = _select_args(kf_slots, lm_slots, voxel_size, roi_far, roi_middle)
+        b, _co, n_near, result = _select_outputs([len(lm)])
+        o = KbaSelectOut(_p(b["cheiral"], c_uint8_p), _p(b["bin"], _c_int8_p), _p(b["near_order"], c_int32_p), _p(n_near, c_int32_p),
+                         _p(b["flow"], c_double_p), _p(b["seen"], c_int32_p))
+        _check(lib().kba_track_select_landmarks(self._p, len(kf), _p(kf, c_int32_p), len(lm), _p(lm, c_int32_p),
+                                                prm.ctypes.data_as(C.POINTER(KbaSelectParams)), C.byref(o)))
+        res = result(0)
+        res["near_order"] = res["near_order"].copy()
+        return res
+
+    def _create_request(self, kf_slots, kf_new, lm_slots):
+        kf, lm = _arr(kf_slots, np.int32, -1), _arr(lm_slots, np.int32, -1)
+        pos, flags = np.zeros((len(lm), 3), np.float64), np.zeros(len(lm), np.uint8)
+        q = KbaCreateRequest(n_kf=len(kf), kf_new=int(kf_new), n_new=len(lm), kf_slot=_p(kf, c_int32_p), lm_slot=_p(lm, c_int32_p))
+        return q, KbaCreateOut(_p(pos, c_double_p), _p(flags, c_uint8_p)), (pos, flags, kf, lm), lambda o: (pos, flags)
 
     def create_landmarks(self, kf_slots, kf_new, lm_slots):
         """push()'s landmark creation on this track's store (kba_track_create_landmarks): kf_slots the active keyframes in
         ascending id order, kf_new the index in kf_slots of the keyframe just pushed, lm_slots the landmarks it measures that do
         not exist yet.  Returns (pos [n, 3] float64, NaN where not created; flags [n] uint8: bit 0 created, bit 1 has depth);
         created landmarks are written into the store with weight 1."""
-        kf, kfp = self._i32(kf_slots)
-        lm, lmp = self._i32(lm_slots)
-        n = len(lm)
-        pos, flags = np.zeros((n, 3), np.float64), np.zeros(n, np.uint8)
-        q = KbaCreateRequest(n_kf=len(kf), kf_new=int(kf_new), n_new=n, kf_slot=kfp, lm_slot=lmp)
-        o = KbaCreateOut(pos.ctypes.data_as(c_double_p), flags.ctypes.data_as(C.POINTER(C.c_uint8)))
+        q, o, _keep, done = self._create_request(kf_slots, kf_new, lm_slots)
         _check(lib().kba_track_create_landmarks(self._p, C.byref(q), C.byref(o)))
-        return pos, flags
+        return done(o)
 
-    @staticmethod
-    def _deactivate_args(kf_slots, lm_slots, min_connecting=3, min_window=4, max_window=20):
-        kf, kfp = Track._i32(kf_slots)
-        lm, lmp = Track._i32(lm_slots)
+    def _deactivate_request(self, kf_slots, lm_slots, min_connecting=3, min_window=4, max_window=20):
+        kf, lm = _arr(kf_slots, np.int32, -1), _arr(lm_slots, np.int32, -1)
         res = (np.zeros(len(kf), np.uint8), np.zeros(len(kf), np.int32), np.zeros(len(lm), np.uint8))
         q = KbaDeactivateRequest(n_kf=len(kf), n_lm=len(lm), min_connecting=int(min_connecting), min_window=int(min_window),
-                                 max_window=int(max_window), kf_slot=kfp, lm_slot=lmp)
-        o = KbaDeactivateOut(res[0].ctypes.data_as(C.POINTER(C.c_uint8)), res[1].ctypes.data_as(C.POINTER(C.c_int32)),
-                             res[2].ctypes.data_as(C.POINTER(C.c_uint8)))
-        return q, o, res, (kf, lm)
+                                 max_window=int(max_window), kf_slot=_p(kf, c_int32_p), lm_slot=_p(lm, c_int32_p))
+        o = KbaDeactivateOut(_p(res[0], c_uint8_p), _p(res[1], c_int32_p), _p(res[2], c_uint8_p))
+        return q, o, (*res, kf, lm), lambda o: res
 
     def deactivate_keyframes(self, kf_slots, lm_slots, min_connecting=3, min_window=4, max_window=20):
         """deactivateKeyframes() on this track's store (kba_track_deactivate_keyframes): kf_slots the active keyframes in ascending
         id order (the last one the newest), lm_slots the active landmarks.  Returns (kf_active [n_kf] uint8, kf_common [n_kf] int32:
         distinct landmarks shared with the newest keyframe, lm_active [n_lm] uint8: measured by a keyframe that stays active)."""
-        q, o, res, _keep = self._deactivate_args(kf_slots, lm_slots, min_connecting, min_window, max_window)
+        q, o, _keep, done = self._deactivate_request(kf_slots, lm_slots, min_connecting, min_window, max_window)
         _check(lib().kba_track_deactivate_keyframes(self._p, C.byref(q), C.byref(o)))
-        return res
+        return done(o)
 
-    @staticmethod
-    def _depth_args(kf_slots, lm_slots, cap=None):
-        kf, kfp = Track._i32(kf_slots)
-        lm, lmp = Track._i32(lm_slots)
+    def _depth_request(self, kf_slots, lm_slots, cap=None):
+        kf, lm = _arr(kf_slots, np.int32, -1), _arr(lm_slots, np.int32, -1)
         cap = min(len(kf) * len(lm), 2**31 - 1) if cap is None else int(cap)  # len(kf) * len(lm) bounds the pairs
         off, cand, cost = np.zeros(len(kf) + 1, np.int32), np.zeros(max(cap, 0), np.int32), np.zeros(max(cap, 0), np.float64)
-        q = KbaDepthRequest(n_kf=len(kf), n_elig=len(lm), cap=cap, kf_slot=kfp, lm_slot=lmp)
-        o = KbaDepthOut(off.ctypes.data_as(C.POINTER(C.c_int32)), cand.ctypes.data_as(C.POINTER(C.c_int32)), cost.ctypes.data_as(c_double_p))
-        return q, o, (off, cand, cost), (kf, lm)
+        q = KbaDepthRequest(n_kf=len(kf), n_elig=len(lm), cap=cap, kf_slot=_p(kf, c_int32_p), lm_slot=_p(lm, c_int32_p))
+        o = KbaDepthOut(_p(off, c_int32_p), _p(cand, c_int32_p), _p(cost, c_double_p))
+        return q, o, (off, cand, cost, kf, lm), lambda o: (off, cand[:off[-1]].copy(), cost[:off[-1]].copy())
 
     def depth_costs(self, kf_slots, lm_slots, cap=None):
         """The AddDepth scheme's costs on this track's store (kba_track_depth_costs) for limo's sorter: kf_slots the active keyframes
         in ascending id order (FrameIndex i = kf_slots[i]), lm_slots the eligible landmarks in ascending id order.  Returns (off
         [n_kf + 1], cand, cost): keyframe k's eligible landmarks (indices into lm_slots, arena order) and costs at off[k] ..
         off[k + 1).  cap: output capacity (default n_kf * n_elig)."""
-        q, o, (off, cand, cost), _keep = self._depth_args(kf_slots, lm_slots, cap)
+        q, o, _keep, done = self._depth_request(kf_slots, lm_slots, cap)
         _check(lib().kba_track_depth_costs(self._p, C.byref(q), C.byref(o)))
-        return off, cand[:off[-1]].copy(), cost[:off[-1]].copy()
+        return done(o)
 
-    @staticmethod
-    def _flow_args(kf_last, lm_slot, u, v, cam=None, min_median_flow=5.0):
-        lm, lmp = Track._i32(lm_slot)
-        cm, cmp_ = (None, C.cast(None, c_int32_p)) if cam is None else Track._i32(cam)
-        fp = C.POINTER(C.c_float)
-        uu, vv = (np.ascontiguousarray(x, dtype=np.float32) for x in (u, v))
+    def _flow_request(self, kf_last, lm_slot, u, v, cam=None, min_median_flow=5.0):
+        lm, cm, uu, vv = _arr(lm_slot, np.int32, -1), _arr(cam, np.int32, -1), _arr(u, np.float32), _arr(v, np.float32)
         match = np.zeros(len(lm), np.int32)
-        q = KbaFlowRequest(kf_last=int(kf_last), n_meas=len(lm), lm_slot=lmp, cam=cmp_, u=uu.ctypes.data_as(fp), v=vv.ctypes.data_as(fp),
-                           min_median_flow=float(min_median_flow))
-        o = KbaFlowOut(match=match.ctypes.data_as(c_int32_p))
-        return q, o, match, (lm, cm, uu, vv)
+        q = KbaFlowRequest(kf_last=int(kf_last), n_meas=len(lm), lm_slot=_p(lm, c_int32_p), cam=_p(cm, c_int32_p),
+                           u=_p(uu, c_float_p), v=_p(vv, c_float_p), min_median_flow=float(min_median_flow))
 
-    @staticmethod
-    def _flow_result(o, match):
-        return dict(n_matched=o.n_matched, flow_sum=o.flow_sum, mean_flow_sq=o.mean_flow_sq, usable=bool(o.usable), match=match)
+        def done(o):
+            return dict(n_matched=o.n_matched, flow_sum=o.flow_sum, mean_flow_sq=o.mean_flow_sq, usable=bool(o.usable), match=match)
+        return q, KbaFlowOut(match=_p(match, c_int32_p)), (match, lm, cm, uu, vv), done
 
     def frame_flow(self, kf_last, lm_slot, u, v, cam=None, min_median_flow=5.0):
         """KeyframeRejectionSchemeFlow's quantity of a new frame against the stored keyframe kf_last, the newest active one
@@ -462,60 +502,48 @@ class Track:
         landmark, ascending id, cameras ascending inside a run).  Returns a dict: n_matched, flow_sum, mean_flow_sq (NaN without a
         match), usable (mean_flow_sq > min_median_flow ** 2) and match [n_meas] (index into kf_last's measurements, -1: none).
         min_median_flow defaults to limo's launch files' 5 px."""
-        q, o, match, _keep = self._flow_args(kf_last, lm_slot, u, v, cam, min_median_flow)
+        q, o, _keep, done = self._flow_request(kf_last, lm_slot, u, v, cam, min_median_flow)
         _check(lib().kba_track_frame_flow(self._p, C.byref(q), C.byref(o)))
-        return self._flow_result(o, match)
+        return done(o)
 
-    @staticmethod
-    def _reclaim_args(lo, hi, evict=False):
+    def _reclaim_request(self, lo, hi, evict=False):
         n = max(int(hi) - int(lo), 0)
         slot = np.zeros(n, np.int32)
         pos, weight = (np.zeros((n, 3), np.float64), np.zeros(n, np.float64)) if evict else (None, None)
-        q = KbaReclaimRequest(lo=int(lo), hi=int(hi))
-        o = KbaReclaimOut(free_slot=slot.ctypes.data_as(c_int32_p))
-        if evict:
-            o.pos, o.weight = pos.ctypes.data_as(c_double_p), weight.ctypes.data_as(c_double_p)
-        return q, o, (slot, pos, weight)
+        o = KbaReclaimOut(free_slot=_p(slot, c_int32_p), pos=_p(pos, c_double_p), weight=_p(weight, c_double_p))
 
-    @staticmethod
-    def _reclaim_result(o, res, evict):
-        n = o.n_free
-        slot, pos, weight = res
-        return (slot[:n].copy(), pos[:n].copy(), weight[:n].copy()) if evict else slot[:n].copy()
+        def done(o):
+            k = o.n_free
+            return (slot[:k].copy(), pos[:k].copy(), weight[:k].copy()) if evict else slot[:k].copy()
+        return KbaReclaimRequest(lo=int(lo), hi=int(hi)), o, (slot, pos, weight), done
 
     def reclaim_landmarks(self, lo, hi, evict=False):
         """The landmark slots in [lo, hi) that no live keyframe (pushed and not dropped) measures, ascending
         (kba_track_reclaim_landmarks).  Returns the slots, or with evict=True (slots, pos [n, 3], weight [n]): the store's current
         values of those slots, for a caller that restores an evicted landmark later with set_landmarks.  The store is not written:
         a slot handed out again must be written (create_landmarks or set_landmarks) before a call reads it."""
-        q, o, res = self._reclaim_args(lo, hi, evict)
+        q, o, _keep, done = self._reclaim_request(lo, hi, evict)
         _check(lib().kba_track_reclaim_landmarks(self._p, C.byref(q), C.byref(o)))
-        return self._reclaim_result(o, res, evict)
+        return done(o)
 
-    @staticmethod
-    def _rank_args(kf_slots, lm_slots, elig=None, voxel_size=SELECT_DEFAULTS["voxel_size"], roi_far=SELECT_DEFAULTS["roi_far"],
-                   roi_middle=SELECT_DEFAULTS["roi_middle"], max_near=RANK_DEFAULTS["max_near"], max_middle=RANK_DEFAULTS["max_middle"],
-                   max_far=RANK_DEFAULTS["max_far"], depth=(), draws=None):
-        """fill a kba_rank_request; returns (request, out, result arrays, what must stay alive during the call)"""
-        kf, kfp = Track._i32(kf_slots)
-        lm, lmp = Track._i32(lm_slots)
+    def _rank_request(self, kf_slots, lm_slots, elig=None, voxel_size=SELECT_DEFAULTS["voxel_size"], roi_far=SELECT_DEFAULTS["roi_far"],
+                      roi_middle=SELECT_DEFAULTS["roi_middle"], max_near=RANK_DEFAULTS["max_near"], max_middle=RANK_DEFAULTS["max_middle"],
+                      max_far=RANK_DEFAULTS["max_far"], depth=(), draws=None):
+        """its result function keeps the size of the ranking for solve_ranked"""
+        kf, lm, prm = _select_args(kf_slots, lm_slots, voxel_size, roi_far, roi_middle)
         n = len(lm)
-        el = None if elig is None else np.ascontiguousarray(elig, dtype=np.uint8).reshape(n)
+        el = _arr(elig, np.uint8, n)
         dp = np.ascontiguousarray(np.asarray(depth, dtype=np.int32).reshape(-1, 2))
-        p = KbaSelectParams((C.c_double * 3)(*[float(x) for x in voxel_size]), float(roi_far), float(roi_middle))
         cand, cat = np.zeros(n, np.int32), np.zeros(n, np.int8)
         fn = _draw_source(draws)
-        q = KbaRankRequest(n_kf=len(kf), n_cand=n, kf_slot=kfp, lm_slot=lmp,
-                           elig=C.cast(None, C.POINTER(C.c_uint8)) if el is None else el.ctypes.data_as(C.POINTER(C.c_uint8)),
-                           params=C.cast(C.pointer(p), C.c_void_p), max_near=int(max_near), max_middle=int(max_middle), max_far=int(max_far),
-                           n_depth=len(dp), depth=dp.ctypes.data_as(C.POINTER(KbaDepthEntry)), draw=fn)
-        o = KbaRankOut(cand=cand.ctypes.data_as(c_int32_p), category=cat.ctypes.data_as(C.POINTER(C.c_int8)))
-        return q, o, (cand, cat), (kf, lm, el, dp, p, fn)
+        q = KbaRankRequest(n_kf=len(kf), n_cand=n, kf_slot=_p(kf, c_int32_p), lm_slot=_p(lm, c_int32_p), elig=_p(el, c_uint8_p),
+                           params=prm.ctypes.data, max_near=int(max_near), max_middle=int(max_middle), max_far=int(max_far),
+                           n_depth=len(dp), depth=_p(dp, _depth_p), draw=fn)
 
-    @staticmethod
-    def _rank_result(o, res):
-        cand, cat = res
-        return dict(cand=cand[:o.n_sel].copy(), category=cat[:o.n_sel].copy(), n_ground=o.n_ground, n_draws=o.n_draws)
+        def done(o):
+            self._n_sel = o.n_sel
+            return dict(cand=cand[:o.n_sel].copy(), category=cat[:o.n_sel].copy(), n_ground=o.n_ground, n_draws=o.n_draws)
+        return q, KbaRankOut(cand=_p(cand, c_int32_p), category=_p(cat, _c_int8_p)), (cand, cat, kf, lm, el, dp, prm, fn), done
 
     def rank_landmarks(self, kf_slots, lm_slots, elig=None, draws=None, **kw):
         """The ranked selection of limo's chain on this track's store (kba_track_rank_landmarks): the arguments of select_landmarks,
@@ -524,29 +552,30 @@ class Track:
         array whose first n entries are taken (too short: the call fails), or None when no draw can be needed.  Returns a dict:
         cand (ascending candidate indices), category (0 near, 1 middle, 2 far, 3 AddDepth only), n_ground, n_draws.  The track
         keeps the ranking for solve_ranked."""
-        q, o, res, _keep = self._rank_args(kf_slots, lm_slots, elig=elig, draws=draws, **kw)
+        q, o, _keep, done = self._rank_request(kf_slots, lm_slots, elig=elig, draws=draws, **kw)
         _check(lib().kba_track_rank_landmarks(self._p, C.byref(q), C.byref(o)))
-        self._n_sel = o.n_sel
-        return self._rank_result(o, res)
+        return done(o)
 
-    def _ranked_selection(self, kf_slots, kf_fixed, ground=False, **scalars):
-        """the arrays of a solve of this track's last ranking, its results sized for that ranking"""
+    def _ranked_request(self, capacity, kf_slots, kf_fixed, ground=False, **scalars):
+        """a solve of this track's last ranking, its Result (capacity iteration records) sized for that ranking"""
         if self._n_sel is None:
             raise KbaError("solve_ranked: the track has no ranking to solve (rank_landmarks)")
-        kf, fx, _lm, sel = Track._selection(kf_slots, kf_fixed, np.zeros(self._n_sel, np.int32), **scalars)
+        kf, fx = _arr(kf_slots, np.int32, -1), _arr(kf_fixed, np.uint8)
+        sel = _sel_window(len(kf), self._n_sel, fx, **scalars)
         if ground:  # the ranking's ground candidates, attached on the device: n_gp > 0 with no lists
             sel.c.n_gp = 1
-        return kf, fx, sel
+        res = Result(sel, capacity)
+        q = KbaRankedRequest(n_kf=len(kf), kf_slot=_p(kf, c_int32_p), kf_fixed=_p(fx, c_uint8_p), sel=C.addressof(sel.c))
+        return q, res.c, (kf, fx, sel), _filled(res)
 
     def solve_ranked(self, kf_slots, kf_fixed, opt=None, ground=False, **scalars):
         """solve() on this track's last ranking (kba_track_solve_ranked), made by rank_landmarks of this track or of a TrackGroup:
         ground=True attaches its ground candidates on the device; the other scalars as for solve (gp_* lists index the ranking).
         Results come in ranked order, sized for the ranking."""
-        kf, fx, sel = self._ranked_selection(kf_slots, kf_fixed, ground, **scalars)
-        res = Result(sel, 256)
-        _check(lib().kba_track_solve_ranked(self._p, len(kf), kf.ctypes.data_as(c_int32_p), fx.ctypes.data_as(C.POINTER(C.c_uint8)),
-                                            C.byref(sel.c), C.byref(opt or default_options()), C.byref(res.c)))
-        return res
+        q, o, _keep, done = self._ranked_request(256, kf_slots, kf_fixed, ground, **scalars)
+        _check(lib().kba_track_solve_ranked(self._p, q.n_kf, q.kf_slot, q.kf_fixed, C.cast(q.sel, C.POINTER(KbaWindow)),
+                                            C.byref(opt or default_options()), C.byref(o)))
+        return done(o)
 
     def transfer_bytes(self):
         a, b, c = C.c_int64(), C.c_int64(), C.c_int64()
@@ -559,6 +588,19 @@ class Track:
             self._p = C.c_void_p()
 
 
+def _built(fn, i, r, build, *args):
+    """build(*args, **r): the structs of request r, the i-th of the group call fn.  A key the single call does not take, or a
+    malformed argument, raises naming the request."""
+    try:
+        return build(*args, **r)
+    except (TypeError, ValueError) as e:
+        raise type(e)("%s: request %d: %s" % (fn.__name__, i, e)) from None
+
+
+def _no_keyframes(q):  # n_kf = 0 would sit the track out: a request without keyframes is an error, as for one track
+    return q.n_kf == 0
+
+
 class TrackGroup:
     """Several persistent windows solved as one batch (kba_track_group_*): one launch for a window of every track."""
 
@@ -568,296 +610,149 @@ class TrackGroup:
         self._p = C.c_void_p()
         _check(lib().kba_track_group_create(handle._p, len(self.tracks), arr, C.byref(self._p)))
 
+    def _call(self, fn, requests, build, Req, Out=None, idle=None, sits_out=None, why=None, opt=()):
+        """The group call fn(group, requests, *opt, outputs) with one entry per track, and its results (None for a track that
+        sat out).  requests[i] None sits track i out: idle() gives its entry, else it is a zeroed request.  Otherwise requests[i]
+        holds the keywords of the single call, and build (a Track builder) makes its entry.  A request that the group call would
+        read as a sit-out (sits_out(request)) fails with why, as the single call fails, or without why its result is the one of
+        an untouched output, as the single call answers it."""
+        assert len(requests) == len(self.tracks)
+        n = len(requests)
+        reqs, outs = (Req * n)(), (Out * n)() if Out else None
+        keep, results, done = [], [None] * n, []  # keep: the arrays the entries point into, alive until the call returns
+        for i, r in enumerate(requests):
+            if r is None:
+                if idle is None:
+                    continue
+                q, o, k, d = idle()
+            else:
+                q, o, k, d = _built(fn, i, r, build, self.tracks[i])
+                if sits_out is not None and sits_out(q):
+                    if why:
+                        raise KbaError("%s: track %d: %s" % (fn.__name__, i, why))
+                    results[i] = d(Out())
+                    continue
+            reqs[i] = q
+            if Out:
+                outs[i] = o
+            keep.append(k)
+            if d:
+                done.append((i, d))
+        _check(fn(self._p, reqs, *opt, *([outs] if Out else [])))
+        for i, d in done:
+            results[i] = d(outs[i])
+        return results
+
     def solve(self, requests, opt=None, iterations_capacity=256):
         """requests: one per track, None (the track sits this solve out) or a dict with the arguments of Track.solve
         (kf_slots, kf_fixed, lm_slots and the scalar keywords).  opt: one KbaOptions, or one per track
         (kba_track_group_solve_opts).  Returns one Result per track."""
-        assert len(requests) == len(self.tracks)
         fn, o = _options(opt, len(self.tracks), lib().kba_track_group_solve, lib().kba_track_group_solve_opts)
-        reqs = (KbaTrackRequest * len(requests))()
-        keep, results = [], []
-        for i, r in enumerate(requests):
-            if r is None:
-                sel = Window(np.tile([1.0, 0, 0, 0, 0, 0, 0], (0, 1)), [], [[1.0, 0, 0]], [[1.0, 0, 0, 0, 0, 0, 0]], np.zeros((0, 3)), [],
-                             [0], [], [], [], [])
-                results.append(Result(sel, 1))
-                continue
-            r = dict(r)
-            kf, fx, lm, sel = Track._selection(r.pop("kf_slots"), r.pop("kf_fixed"), r.pop("lm_slots"), **r)
-            q = reqs[i]
-            q.n_kf, q.n_lm = len(kf), len(lm)
-            q.kf_slot, q.kf_fixed = kf.ctypes.data_as(c_int32_p), fx.ctypes.data_as(C.POINTER(C.c_uint8))
-            q.lm_slot, q.sel = lm.ctypes.data_as(c_int32_p), C.pointer(sel.c)
-            keep.append((kf, fx, lm, sel))
-            results.append(Result(sel, iterations_capacity))
-        rarr = (KbaResult * len(results))(*[r.c for r in results])
-        _check(fn(self._p, reqs, o, rarr))
-        for r, c in zip(results, rarr):
-            r.c = c
-        return results
+        return self._call(fn, requests, lambda t, **r: t._solve_request(iterations_capacity, **r), KbaTrackRequest, KbaResult,
+                          idle=lambda: _idle(KbaTrackRequest, 0), opt=(o,))
 
     def adjust_pose(self, frames, opt=None, iterations_capacity=256):
         """one frame per track in one launch (kba_track_group_adjust_pose): each entry None (the track sits the call out) or a
         dict with the arguments of Track.adjust_pose (pose7, lm_slot, u, v, d, cam, speed).  opt: one KbaOptions, or one per
         track (kba_track_group_adjust_pose_opts).  Returns one Result per track."""
-        assert len(frames) == len(self.tracks)
         fn, o = _options(opt, len(self.tracks), lib().kba_track_group_adjust_pose, lib().kba_track_group_adjust_pose_opts)
-        arr = (KbaTrackFrame * len(frames))()
-        keep, results = [], []
-        for i, fr in enumerate(frames):
-            if fr is None:
-                arr[i].n_meas = 0
-                results.append(Track._frame_result(0, 1))
-                continue
-            k, n_runs = Track._frame(arr[i], **fr)
-            keep.append(k)
-            results.append(Track._frame_result(n_runs, iterations_capacity))
-        rarr = (KbaResult * len(results))(*[r.c for r in results])
-        _check(fn(self._p, arr, o, rarr))
-        for r, c in zip(results, rarr):
-            r.c = c
-        return results
+        return self._call(fn, frames, lambda t, **r: t._frame_request(iterations_capacity, **r), KbaTrackFrame, KbaResult,
+                          idle=lambda: _idle(KbaTrackFrame, 1), opt=(o,))
 
     def select_landmarks(self, requests):
         """the selection quantities of every track in one launch sequence (kba_track_group_select_landmarks): each entry None
         (the track sits the call out) or a dict with the arguments of Track.select_landmarks (kf_slots, lm_slots, voxel_size,
         roi_far, roi_middle).  Returns one dict per track as Track.select_landmarks returns it (its arrays are views of buffers
         shared by the call), None for a track that sat out."""
+        # Not _call: the outputs share buffers sized by every request, and the request and output structs are numpy records,
+        # filled without a ctypes object per track.  With one KbaSelectRequest and KbaSelectOut per track instead, a group
+        # call of 132 tracks took 7.4-8.4 ms against 2.0-2.6 ms at 12 keyframes / 1.1k landmarks, and 14.3-14.7 ms against
+        # 19.3-26.3 ms at 20 keyframes / 8k landmarks, a difference not broken down yet (scripts/group_select_bench.py,
+        # medians of 30 calls over several runs, NVIDIA H100 80GB HBM3 at a 700 W power limit).
         assert len(requests) == len(self.tracks)
-        n = len(requests)
+        fn = lib().kba_track_group_select_landmarks
         act = [i for i, r in enumerate(requests) if r is not None]
-        prm = np.empty((len(act), 5), np.float64)  # kba_select_params of each request: voxel size xyz, roi_far, roi_middle
-        for q, i in enumerate(act):
-            r = requests[i]
-            extra = set(r) - {"kf_slots", "lm_slots", *SELECT_DEFAULTS}
-            if extra:
-                raise TypeError("select_landmarks: request %d has unexpected keys %s" % (i, sorted(extra)))
-            vs = np.asarray(r.get("voxel_size", SELECT_DEFAULTS["voxel_size"]), np.float64)
-            if vs.shape != (3,):
-                raise ValueError("select_landmarks: request %d: voxel_size must have 3 entries" % i)
-            prm[q] = (*vs, r.get("roi_far", SELECT_DEFAULTS["roi_far"]), r.get("roi_middle", SELECT_DEFAULTS["roi_middle"]))
-        # the request and output structs as numpy records, filled without a ctypes object per track
-        kfs = [np.ascontiguousarray(requests[i]["kf_slots"], dtype=np.int32).ravel() for i in act]
-        lms = [np.ascontiguousarray(requests[i]["lm_slots"], dtype=np.int32).ravel() for i in act]
-        for q, i in enumerate(act):
-            if len(kfs[q]) == 0:  # n_kf = 0 would sit the track out: a request without keyframes is an error, as for one track
-                raise KbaError("kba_track_group_select_landmarks: track %d: no keyframes or a negative size" % i)
-        nk, nc = np.array([len(a) for a in kfs], np.int64), np.array([len(a) for a in lms], np.int64)
-        lists = np.concatenate(kfs + lms + [np.zeros(1, np.int32)])
-        co = np.concatenate(([0], np.cumsum(nc)))
-        N = int(co[-1])
-        cheiral, bins, near = np.empty(N + 1, np.uint8), np.empty(N + 1, np.int8), np.empty(N + 1, np.int32)
-        flow, seen, n_near = np.empty(N + 1, np.float64), np.empty(N + 1, np.int32), np.zeros(n, np.int32)
-        req, out = np.zeros(n, _records(KbaSelectRequest)), np.zeros(n, _records(KbaSelectOut))
-        req["n_kf"][act], req["n_cand"][act] = nk, nc
+        args = [_built(fn, i, requests[i], _select_args) for i in act]
+        for i, (kf, _lm, _prm) in zip(act, args):
+            if len(kf) == 0:  # n_kf = 0 would sit the track out: a request without keyframes is an error, as for one track
+                raise KbaError("%s: track %d: no keyframes or a negative size" % (fn.__name__, i))
+        n_cand = [0] * len(requests)
+        for i, (_kf, lm, _prm) in zip(act, args):
+            n_cand[i] = len(lm)
+        bufs, co, n_near, result = _select_outputs(n_cand)
+        co = np.array(co[:-1], np.int64)[act]  # the candidate offset of each request that runs
+        out = np.zeros(len(requests), _records(KbaSelectOut))
+        out["n_near"] = n_near.ctypes.data + 4 * np.arange(len(requests))
+        for name, a in bufs.items():
+            out[name][act] = a.ctypes.data + a.itemsize * co
+        nk = np.array([len(kf) for kf, _lm, _prm in args], np.int64)
+        lists = np.concatenate([a[0] for a in args] + [a[1] for a in args] + [np.zeros(1, np.int32)])
+        prm = np.concatenate([a[2] for a in args] + [np.zeros(0)])
+        req = np.zeros(len(requests), _records(KbaSelectRequest))
+        req["n_kf"][act], req["n_cand"][act] = nk, [len(lm) for _kf, lm, _prm in args]
         req["kf_slot"][act] = lists.ctypes.data + 4 * np.concatenate(([0], np.cumsum(nk)[:-1]))
-        req["lm_slot"][act] = lists.ctypes.data + 4 * (nk.sum() + co[:-1])
+        req["lm_slot"][act] = lists.ctypes.data + 4 * (nk.sum() + co)
         req["params"][act] = prm.ctypes.data + C.sizeof(KbaSelectParams) * np.arange(len(act))
-        out["n_near"] = n_near.ctypes.data + 4 * np.arange(n)
-        for name, a in (("cheiral", cheiral), ("bin", bins), ("near_order", near), ("flow", flow), ("seen", seen)):
-            out[name][act] = a.ctypes.data + a.itemsize * co[:-1]
-        _check(lib().kba_track_group_select_landmarks(self._p, req.ctypes.data_as(C.POINTER(KbaSelectRequest)),
-                                                      out.ctypes.data_as(C.POINTER(KbaSelectOut))))
-        results = [None] * n
-        for q, i in enumerate(act):
-            a, b = int(co[q]), int(co[q + 1])
-            results[i] = dict(cheiral=cheiral[a:b], bin=bins[a:b], near_order=near[a:a + int(n_near[i])], flow=flow[a:b], seen=seen[a:b])
-        return results
+        _check(fn(self._p, req.ctypes.data_as(C.POINTER(KbaSelectRequest)), out.ctypes.data_as(C.POINTER(KbaSelectOut))))
+        return [None if r is None else result(i) for i, r in enumerate(requests)]
 
     def create_landmarks(self, requests):
         """push()'s landmark creation for every track in one launch sequence (kba_track_group_create_landmarks): each entry None
         (the track sits the call out) or a dict with the arguments of Track.create_landmarks (kf_slots, kf_new, lm_slots).
         Returns one (pos, flags) per track as Track.create_landmarks returns it, None for a track that sat out."""
-        assert len(requests) == len(self.tracks)
-        n = len(requests)
-        reqs, outs = (KbaCreateRequest * n)(), (KbaCreateOut * n)()
-        keep, results = [], [None] * n
-        for i, r in enumerate(requests):
-            if r is None:
-                continue
-            extra = set(r) - {"kf_slots", "kf_new", "lm_slots"}
-            if extra:
-                raise TypeError("create_landmarks: request %d has unexpected keys %s" % (i, sorted(extra)))
-            kf, kfp = Track._i32(r["kf_slots"])
-            lm, lmp = Track._i32(r["lm_slots"])
-            if len(kf) == 0:  # n_kf = 0 would sit the track out: a request without keyframes is an error, as for one track
-                raise KbaError("kba_track_group_create_landmarks: track %d: no keyframes or a negative size" % i)
-            pos, flags = np.zeros((len(lm), 3), np.float64), np.zeros(len(lm), np.uint8)
-            reqs[i] = KbaCreateRequest(n_kf=len(kf), kf_new=int(r["kf_new"]), n_new=len(lm), kf_slot=kfp, lm_slot=lmp)
-            outs[i] = KbaCreateOut(pos.ctypes.data_as(c_double_p), flags.ctypes.data_as(C.POINTER(C.c_uint8)))
-            keep.append((kf, lm))
-            results[i] = (pos, flags)
-        _check(lib().kba_track_group_create_landmarks(self._p, reqs, outs))
-        return results
-
-    def _upkeep(self, requests, keys, args, Req, Out, fn):
-        assert len(requests) == len(self.tracks)
-        n = len(requests)
-        reqs, outs = (Req * n)(), (Out * n)()
-        keep, results = [], [None] * n
-        for i, r in enumerate(requests):
-            if r is None:
-                continue
-            extra = set(r) - keys
-            if extra:
-                raise TypeError("request %d has unexpected keys %s" % (i, sorted(extra)))
-            q, o, res, lists = args(**r)
-            if q.n_kf == 0:  # n_kf = 0 would sit the track out: a request without keyframes is an error, as for one track
-                raise KbaError("%s: track %d: no keyframes or a negative size" % (fn, i))
-            reqs[i], outs[i] = q, o
-            keep.append(lists)
-            results[i] = res
-        _check(getattr(lib(), fn)(self._p, reqs, outs))
-        return results
+        return self._call(lib().kba_track_group_create_landmarks, requests, Track._create_request, KbaCreateRequest, KbaCreateOut,
+                          sits_out=_no_keyframes, why="no keyframes or a negative size")
 
     def deactivate_keyframes(self, requests):
         """deactivateKeyframes() for every track in one launch sequence (kba_track_group_deactivate_keyframes): each entry None (the
         track sits the call out) or a dict with the arguments of Track.deactivate_keyframes.  Returns one (kf_active, kf_common,
         lm_active) per track, None for a track that sat out."""
-        return self._upkeep(requests, {"kf_slots", "lm_slots", "min_connecting", "min_window", "max_window"}, Track._deactivate_args,
-                            KbaDeactivateRequest, KbaDeactivateOut, "kba_track_group_deactivate_keyframes")
+        return self._call(lib().kba_track_group_deactivate_keyframes, requests, Track._deactivate_request, KbaDeactivateRequest,
+                          KbaDeactivateOut, sits_out=_no_keyframes, why="no keyframes or a negative size")
 
     def depth_costs(self, requests):
         """The AddDepth costs for every track in one launch sequence (kba_track_group_depth_costs): each entry None or a dict with
         the arguments of Track.depth_costs.  Returns one (off, cand, cost) per track, None for a track that sat out."""
-        res = self._upkeep(requests, {"kf_slots", "lm_slots", "cap"}, Track._depth_args, KbaDepthRequest, KbaDepthOut,
-                           "kba_track_group_depth_costs")
-        return [None if r is None else (r[0], r[1][:r[0][-1]].copy(), r[2][:r[0][-1]].copy()) for r in res]
+        return self._call(lib().kba_track_group_depth_costs, requests, Track._depth_request, KbaDepthRequest, KbaDepthOut,
+                          sits_out=_no_keyframes, why="no keyframes or a negative size")
 
     def frame_flow(self, requests):
         """The flow scheme's quantity for one frame of every track in one launch sequence (kba_track_group_frame_flow): each entry
         None (the track sits the call out) or a dict with the arguments of Track.frame_flow.  Returns one result dict per track,
         None for a track that sat out."""
-        assert len(requests) == len(self.tracks)
-        n = len(requests)
-        reqs, outs = (KbaFlowRequest * n)(), (KbaFlowOut * n)()
-        for i in range(n):
-            reqs[i].kf_last = -1
-        keep, matches = [], [None] * n
-        for i, r in enumerate(requests):
-            if r is None:
-                continue
-            q, o, match, lists = Track._flow_args(**r)
-            if q.kf_last < 0:  # kf_last < 0 would sit the track out: an error here, as for one track
-                raise KbaError("kba_track_group_frame_flow: track %d: kf_last not pushed" % i)
-            reqs[i], outs[i] = q, o
-            keep.append(lists)
-            matches[i] = match
-        _check(lib().kba_track_group_frame_flow(self._p, reqs, outs))
-        return [None if m is None else Track._flow_result(outs[i], m) for i, m in enumerate(matches)]
+        return self._call(lib().kba_track_group_frame_flow, requests, Track._flow_request, KbaFlowRequest, KbaFlowOut,
+                          idle=lambda: (KbaFlowRequest(kf_last=-1), KbaFlowOut(), (), None), sits_out=lambda q: q.kf_last < 0,
+                          why="kf_last not pushed")
 
     def reclaim_landmarks(self, requests):
         """The free landmark slots of every track in one launch sequence (kba_track_group_reclaim_landmarks): each entry None (the
         track sits the call out) or a dict with the arguments of Track.reclaim_landmarks (lo, hi, evict).  Returns one result per
         track as Track.reclaim_landmarks returns it, None for a track that sat out."""
-        assert len(requests) == len(self.tracks)
-        n = len(requests)
-        reqs, outs = (KbaReclaimRequest * n)(), (KbaReclaimOut * n)()
-        keep = [None] * n
-        for i, r in enumerate(requests):
-            if r is None:
-                continue
-            extra = set(r) - {"lo", "hi", "evict"}
-            if extra:
-                raise TypeError("reclaim_landmarks: request %d has unexpected keys %s" % (i, sorted(extra)))
-            q, o, res = Track._reclaim_args(r["lo"], r["hi"], r.get("evict", False))
-            if q.hi == q.lo:  # an empty range would sit the track out: here it is an empty result, as for one track
-                keep[i] = None
-                continue
-            reqs[i], outs[i] = q, o
-            keep[i] = (res, bool(r.get("evict", False)))
-        _check(lib().kba_track_group_reclaim_landmarks(self._p, reqs, outs))
-        results = [None] * n
-        for i, r in enumerate(requests):
-            if r is None:
-                continue
-            if keep[i] is None:
-                results[i] = Track._reclaim_result(KbaReclaimOut(), Track._reclaim_args(0, 0, r.get("evict", False))[2], r.get("evict", False))
-            else:
-                results[i] = Track._reclaim_result(outs[i], *keep[i])
-        return results
+        # an empty range would sit the track out: its result is the empty one of a single call
+        return self._call(lib().kba_track_group_reclaim_landmarks, requests, Track._reclaim_request, KbaReclaimRequest, KbaReclaimOut,
+                          sits_out=lambda q: q.hi == q.lo)
 
     def rank_landmarks(self, requests):
         """The ranked selection of every track in one launch sequence (kba_track_group_rank_landmarks): each entry None (the track
         sits the call out, its ranking kept) or a dict with the arguments of Track.rank_landmarks.  Returns one result dict per
         track, None for a track that sat out."""
-        assert len(requests) == len(self.tracks)
-        n = len(requests)
-        reqs, outs = (KbaRankRequest * n)(), (KbaRankOut * n)()
-        keep, results = [], [None] * n
-        for i, r in enumerate(requests):
-            if r is None:
-                continue
-            q, o, res, lists = Track._rank_args(**r)
-            if q.n_kf == 0:  # n_kf = 0 would sit the track out: a request without keyframes is an error, as for one track
-                raise KbaError("kba_track_group_rank_landmarks: track %d: no keyframes or a negative size" % i)
-            reqs[i], outs[i] = q, o
-            keep.append(lists)
-            results[i] = res
-        _check(lib().kba_track_group_rank_landmarks(self._p, reqs, outs))
-        for i, r in enumerate(results):
-            if r is not None:
-                self.tracks[i]._n_sel = outs[i].n_sel
-        return [None if r is None else Track._rank_result(outs[i], r) for i, r in enumerate(results)]
+        return self._call(lib().kba_track_group_rank_landmarks, requests, Track._rank_request, KbaRankRequest, KbaRankOut,
+                          sits_out=_no_keyframes, why="no keyframes or a negative size")
 
     def solve_ranked(self, requests, opt=None, iterations_capacity=256):
         """solve_ranked for every track as one batch (kba_track_group_solve_ranked): each entry None (the track sits this solve out)
         or a dict with the arguments of Track.solve_ranked (kf_slots, kf_fixed, ground and the scalar keywords).  Returns one
         Result per track, sized for its ranking.  opt: one KbaOptions, or one per track (kba_track_group_solve_ranked_opts)."""
-        assert len(requests) == len(self.tracks)
         fn, o = _options(opt, len(self.tracks), lib().kba_track_group_solve_ranked, lib().kba_track_group_solve_ranked_opts)
-        reqs = (KbaRankedRequest * len(requests))()
-        keep, results = [], []
-        for i, r in enumerate(requests):
-            if r is None:
-                sel = Window(np.tile([1.0, 0, 0, 0, 0, 0, 0], (0, 1)), [], [[1.0, 0, 0]], [[1.0, 0, 0, 0, 0, 0, 0]], np.zeros((0, 3)), [],
-                             [0], [], [], [], [])
-                results.append(Result(sel, 1))
-                continue
-            r = dict(r)
-            kf, fx, sel = self.tracks[i]._ranked_selection(r.pop("kf_slots"), r.pop("kf_fixed"), r.pop("ground", False), **r)
-            q = reqs[i]
-            q.n_kf = len(kf)
-            q.kf_slot, q.kf_fixed = kf.ctypes.data_as(c_int32_p), fx.ctypes.data_as(C.POINTER(C.c_uint8))
-            q.sel = C.cast(C.pointer(sel.c), C.c_void_p)
-            keep.append((kf, fx, sel))
-            results.append(Result(sel, iterations_capacity))
-        rarr = (KbaResult * len(results))(*[r.c for r in results])
-        _check(fn(self._p, reqs, o, rarr))
-        for r, c in zip(results, rarr):
-            r.c = c
-        return results
+        return self._call(fn, requests, lambda t, **r: t._ranked_request(iterations_capacity, **r), KbaRankedRequest, KbaResult,
+                          idle=lambda: _idle(KbaRankedRequest, 0), opt=(o,))
 
     def push_keyframes(self, requests):
         """one keyframe into every track's store in one call (kba_track_group_push_keyframes): each entry None (the track sits the
         call out) or a dict with the arguments of Track.push_keyframe (slot, pose7, lm_slot, u, v, d and optionally cam, plane4)"""
-        assert len(requests) == len(self.tracks)
-        reqs = (KbaPushRequest * len(requests))()
-        keep = []
-        fp = C.POINTER(C.c_float)
-        for i, r in enumerate(requests):
-            if r is None:
-                reqs[i].kf_slot = -1
-                continue
-            extra = set(r) - {"slot", "pose7", "lm_slot", "u", "v", "d", "cam", "plane4"}
-            if extra:
-                raise TypeError("push_keyframes: request %d has unexpected keys %s" % (i, sorted(extra)))
-            if int(r["slot"]) < 0:  # a negative slot would sit the track out: an error here, as for one track
-                raise KbaError("kba_track_group_push_keyframes: track %d: keyframe slot out of range" % i)
-            pose = np.ascontiguousarray(r["pose7"], dtype=np.float64)
-            pl = None if r.get("plane4") is None else np.ascontiguousarray(r["plane4"], dtype=np.float64)
-            lm = np.ascontiguousarray(r["lm_slot"], dtype=np.int32)
-            cm = None if r.get("cam") is None else np.ascontiguousarray(r["cam"], dtype=np.int32)
-            uu, vv, dd = (np.ascontiguousarray(r[k], dtype=np.float32) for k in ("u", "v", "d"))
-            q = reqs[i]
-            q.kf_slot, q.n_meas = int(r["slot"]), len(lm)
-            q.pose7 = pose.ctypes.data_as(c_double_p)
-            q.plane4 = C.cast(None, c_double_p) if pl is None else pl.ctypes.data_as(c_double_p)
-            q.lm_slot = lm.ctypes.data_as(c_int32_p)
-            q.cam = C.cast(None, c_int32_p) if cm is None else cm.ctypes.data_as(c_int32_p)
-            q.u, q.v, q.d = uu.ctypes.data_as(fp), vv.ctypes.data_as(fp), dd.ctypes.data_as(fp)
-            keep.append((pose, pl, lm, cm, uu, vv, dd))
-        _check(lib().kba_track_group_push_keyframes(self._p, reqs))
+        self._call(lib().kba_track_group_push_keyframes, requests, Track._push_request, KbaPushRequest,
+                   idle=lambda: (KbaPushRequest(kf_slot=-1), None, (), None), sits_out=lambda q: q.kf_slot < 0,
+                   why="keyframe slot out of range")
 
     def drop_keyframes(self, slots):
         """one keyframe slot per track out of its window (kba_track_group_drop_keyframes): None or a negative slot sits out"""
@@ -868,45 +763,12 @@ class TrackGroup:
     def set_landmarks(self, requests):
         """landmark positions and weights of every track in one call (kba_track_group_set_landmarks): each entry None (the track
         sits the call out) or a dict with the arguments of Track.set_landmarks (lm_slot, and optionally pos, weight)"""
-        assert len(requests) == len(self.tracks)
-        reqs = (KbaLandmarkWrite * len(requests))()
-        keep = []
-        for i, r in enumerate(requests):
-            if r is None:
-                continue
-            extra = set(r) - {"lm_slot", "pos", "weight"}
-            if extra:
-                raise TypeError("set_landmarks: request %d has unexpected keys %s" % (i, sorted(extra)))
-            lm = np.ascontiguousarray(r["lm_slot"], dtype=np.int32).ravel()
-            p = None if r.get("pos") is None else np.ascontiguousarray(r["pos"], dtype=np.float64).reshape(-1, 3)
-            w = None if r.get("weight") is None else np.ascontiguousarray(r["weight"], dtype=np.float64)
-            q = reqs[i]
-            q.n, q.lm_slot = len(lm), lm.ctypes.data_as(c_int32_p)
-            q.pos3 = C.cast(None, c_double_p) if p is None else p.ctypes.data_as(c_double_p)
-            q.weight = C.cast(None, c_double_p) if w is None else w.ctypes.data_as(c_double_p)
-            keep.append((lm, p, w))
-        _check(lib().kba_track_group_set_landmarks(self._p, reqs))
+        self._call(lib().kba_track_group_set_landmarks, requests, Track._landmark_write, KbaLandmarkWrite)
 
     def set_keyframe_poses(self, requests):
         """keyframe poses (and planes) of every track in one call (kba_track_group_set_keyframe_poses): each entry None (the track
         sits the call out) or a dict with the arguments of Track.set_keyframe_poses (kf_slots, pose7s, and optionally plane4s)"""
-        assert len(requests) == len(self.tracks)
-        reqs = (KbaPoseWrite * len(requests))()
-        keep = []
-        for i, r in enumerate(requests):
-            if r is None:
-                continue
-            extra = set(r) - {"kf_slots", "pose7s", "plane4s"}
-            if extra:
-                raise TypeError("set_keyframe_poses: request %d has unexpected keys %s" % (i, sorted(extra)))
-            kf = np.ascontiguousarray(r["kf_slots"], dtype=np.int32).ravel()
-            p = np.ascontiguousarray(r["pose7s"], dtype=np.float64).reshape(-1, 7)
-            pl = None if r.get("plane4s") is None else np.ascontiguousarray(r["plane4s"], dtype=np.float64).reshape(-1, 4)
-            q = reqs[i]
-            q.n, q.kf_slot, q.pose7s = len(kf), kf.ctypes.data_as(c_int32_p), p.ctypes.data_as(c_double_p)
-            q.plane4s = C.cast(None, c_double_p) if pl is None else pl.ctypes.data_as(c_double_p)
-            keep.append((kf, p, pl))
-        _check(lib().kba_track_group_set_keyframe_poses(self._p, reqs))
+        self._call(lib().kba_track_group_set_keyframe_poses, requests, Track._pose_write, KbaPoseWrite)
 
     def transfer_bytes(self):
         """(host->device bytes, device->host bytes) of the last group solve, pose-only call, selection, creation, upkeep, flow

@@ -275,7 +275,6 @@ def test_flow_errors_write_nothing():
     """every invalid request fails with its code before anything is written: the outputs of the single call and of every request
     of a group stay as they were; a valid call afterwards equals the statement"""
     from limo_b200 import capi
-    from limo_b200.capi import Track
     dr = KeyframeDrive(41, n_frames=16, window=4, rig=True, n_feat=80)
     steps = list(replay(dr))
     h = capi.Handle(0)
@@ -308,8 +307,8 @@ def test_flow_errors_write_nothing():
     L = capi.lib()
 
     def call(fn, p, reqs):
-        qs = [Track._flow_args(**r) for r in reqs]
-        for q, o, match, _keep in qs:
+        qs = [t._flow_request(**r) for r in reqs]
+        for q, o, (match, *_keep), _done in qs:
             match[:] = -7
             o.n_matched, o.usable, o.flow_sum, o.mean_flow_sq = 99, 7, 1.5, 2.5
         if len(qs) == 1:
@@ -324,14 +323,14 @@ def test_flow_errors_write_nothing():
         assert msg in L.kba_last_error().decode()
         rc, qs2 = call(L.kba_track_group_frame_flow, g._p, [good, r])
         assert rc == code and re.search("track 1: .*" + msg, L.kba_last_error().decode()), msg
-        for _q, o, match, _keep in qs + qs2:  # nothing written
+        for _q, o, (match, *_keep), _done in qs + qs2:  # nothing written
             assert (o.n_matched, o.usable, o.flow_sum, o.mean_flow_sq) == (99, 7, 1.5, 2.5) and (match == -7).all()
-    q, o, match, _keep = Track._flow_args(**dict(good, kf_last=-1))
+    q, o, _keep, _done = t._flow_request(**dict(good, kf_last=-1))
     assert L.kba_track_frame_flow(t._p, C.byref(q), C.byref(o)) == 1  # kf_last < 0 sits out only in a group call
-    q, o, match, _keep = Track._flow_args(**good)
+    q, o, _keep, _done = t._flow_request(**good)
     q.lm_slot = C.cast(None, C.POINTER(C.c_int32))
     assert L.kba_track_frame_flow(t._p, C.byref(q), C.byref(o)) == 1 and "null argument" in L.kba_last_error().decode()
-    q, o, match, _keep = Track._flow_args(**good)
+    q, o, _keep, _done = t._flow_request(**good)
     q.n_meas = -1
     assert L.kba_track_frame_flow(t._p, C.byref(q), C.byref(o)) == 1 and "negative size" in L.kba_last_error().decode()
     for x in (t, other):

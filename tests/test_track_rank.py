@@ -357,7 +357,7 @@ def test_rank_rejects_bad_requests_and_writes_nothing():
                     (dict(kf_slots=kf_list, lm_slots=cand, depth=[(0, 1)] * 1025), "1024"),
                     (dict(kf_slots=kf_list, lm_slots=cand, draws=None), "draw"),
                     (dict(kf_slots=kf_list, lm_slots=cand, draws=np.zeros(1, np.int64)), "draw function failed")):
-        q, o, (c, k), keep = capi.Track._rank_args(**kw)
+        q, o, (c, k, *keep), _done = t._rank_request(**kw)
         c[:] = -7
         k[:] = -7
         o.n_sel = o.n_ground = o.n_draws = -7
@@ -388,7 +388,7 @@ def test_group_rank_draw_failure_names_its_track():
     reqs, outs = (capi.KbaRankRequest * 3)(), (capi.KbaRankOut * 3)()
     keep = []
     for i, draws in ((1, rng.integers(0, 2**31 - 1, len(cands[1]))), (2, np.zeros(0, np.int64))):
-        q, o, (c, k), lists = capi.Track._rank_args(kf_list, cands[i], draws=draws, **CAPS, **VOX)
+        q, o, (c, k, *lists), _done = ts[i]._rank_request(kf_list, cands[i], draws=draws, **CAPS, **VOX)
         c[:] = -7
         k[:] = -7
         o.n_sel = o.n_ground = o.n_draws = -7

@@ -318,7 +318,6 @@ def test_upkeep_errors_write_nothing():
     """every invalid request fails with its code before anything is written: sentinel outputs of the single call and of every
     request of a group stay as they were; the valid call afterwards equals the restatement"""
     from limo_b200 import capi
-    from limo_b200.capi import Track
     dr = UpkeepDrive(41, n_push=6, window=4, rig=True, new_per_push=30)
     steps = _steps(dr)
     h = capi.Handle(0)
@@ -351,28 +350,28 @@ def test_upkeep_errors_write_nothing():
         return [a.copy() for a in res]
 
     for rd, rc_, code, msg in bad:
-        for r, args, fn, gfn, Req, Out, good in ((rd, Track._deactivate_args, L.kba_track_deactivate_keyframes,
+        for r, args, fn, gfn, Req, Out, good in ((rd, t._deactivate_request, L.kba_track_deactivate_keyframes,
                                                    L.kba_track_group_deactivate_keyframes, capi.KbaDeactivateRequest, capi.KbaDeactivateOut,
                                                    good_d),
-                                                  (rc_, Track._depth_args, L.kba_track_depth_costs, L.kba_track_group_depth_costs,
+                                                  (rc_, t._depth_request, L.kba_track_depth_costs, L.kba_track_group_depth_costs,
                                                    capi.KbaDepthRequest, capi.KbaDepthOut, good_c)):
             if r is None:
                 continue
-            q, o, res, _keep = args(**r)
+            q, o, (*res, _kf, _lm), _done = args(**r)
             before = sentinel(res)
             assert fn(t._p, C.byref(q), C.byref(o)) == code
             assert msg in L.kba_last_error().decode()
             assert all(np.array_equal(a, b) for a, b in zip(res, before))
             if not r["kf_slots"]:
                 continue  # n_kf = 0 sits a group call out
-            q0, o0, res0, _keep0 = args(**good)
+            q0, o0, (*res0, _kf0, _lm0), _done0 = args(**good)
             before0 = sentinel(res0)
             reqs, outs = (Req * 2)(q0, q), (Out * 2)(o0, o)
             assert gfn(g._p, reqs, outs) == code
             assert re.search("track 1: .*" + msg, L.kba_last_error().decode())
             assert all(np.array_equal(a, b) for a, b in zip(res + res0, before + before0))
-    for fn, args, good in ((L.kba_track_deactivate_keyframes, Track._deactivate_args, good_d), (L.kba_track_depth_costs, Track._depth_args, good_c)):
-        q, o, res, _keep = args(**good)
+    for fn, args, good in ((L.kba_track_deactivate_keyframes, t._deactivate_request, good_d), (L.kba_track_depth_costs, t._depth_request, good_c)):
+        q, o, _keep, _done = args(**good)
         o2 = type(o)()  # null output arrays
         assert fn(t._p, C.byref(q), C.byref(o2)) == 1
     for x in (t, other):
