@@ -947,6 +947,45 @@ int kba_lidar_depth(kba_handle* h, const float* cloud, int32_t n_points, int32_t
                     const double* intr, const float* features_uv, int32_t n_features, const kba_lidar_options* opt,
                     float* depth_out, float* device_ms);
 
+/* ---- lidar depth for many clouds and cameras in one call -------------------------------------------------------------
+ * The per-frame DepthEstimator call for many frames, and for the cameras of a rig, at once.  A view is one camera looking at
+ * one cloud with one feature list; kba_lidar_depth is the batch of one view of one cloud.
+ *   - Results: views[i].depth_out equals, bit for bit, kba_lidar_depth on clouds[views[i].cloud] with that view's pose,
+ *     intrinsics, features and options.
+ *   - Shared clouds: several views may name the same cloud; it is uploaded once per call.
+ *   - Sitting out: a view with n_features == 0 is skipped and none of its other fields is read (depth_out may be NULL).  A
+ *     cloud that no remaining view names is neither read, uploaded nor projected.  A call in which every view sits out returns
+ *     KBA_OK at once with *device_ms = 0.
+ *   - Validation, before anything is uploaded: a null pointer where data is needed (clouds or views with a positive count,
+ *     the options when a view works, a working view's T_cam_lidar, intr, features_uv or depth_out, a named cloud's points
+ *     when n_points > 0), a negative count, stride < 3 or a cloud index out of range: KBA_ERR_BAD_ARG.  More than INT32_MAX
+ *     (view, point) pairs, cells (sum over views of ceil(w/16) * ceil(h/16) + 1) or 2 * features: KBA_ERR_CAPACITY.
+ *     kba_last_error names the failing cloud or view index, and no depth_out is written.  Options are not checked.
+ *   - Cost of a call: one launch sequence (memset, count, scan, fill, feature kernels) whatever the number of views; one
+ *     copy per used cloud from the caller's memory; one packed upload of the features and per-view parameters; one download
+ *     of all depths; one synchronisation.  The handle's grow-only device workspace takes 24 B of sorted point record per
+ *     (view, point) pair, plus the used clouds, 12 B per cell, and 12 B per feature: no allocation once it is large enough.
+ *   - device_ms: the kernels of the whole call, between events as in kba_lidar_depth. */
+typedef struct kba_lidar_cloud {
+    const float* points;        /* n_points x stride floats, xyz first (as kba_lidar_depth's cloud) */
+    int32_t n_points;
+    int32_t stride;             /* >= 3 */
+} kba_lidar_cloud;
+typedef struct kba_lidar_view {
+    int32_t cloud;              /* index into clouds[] */
+    int32_t n_features;         /* 0: the view sits out, depth_out is not written (may be NULL) */
+    const double* T_cam_lidar;  /* 7-vector, camera <- lidar */
+    const double* intr;         /* f, cx, cy */
+    const float* features_uv;   /* n_features x 2 */
+    float* depth_out;           /* n_features, -1 = no depth */
+} kba_lidar_view;
+int kba_lidar_depth_batch(kba_handle* h, int32_t n_clouds, const kba_lidar_cloud* clouds, int32_t n_views,
+                          const kba_lidar_view* views, const kba_lidar_options* opt, float* device_ms);
+/* opts[n_views]: view i runs with opts[i] (a rig whose cameras differ in image size, or a parameter sweep); a view that sits
+ * out does not read its entry */
+int kba_lidar_depth_batch_opts(kba_handle* h, int32_t n_clouds, const kba_lidar_cloud* clouds, int32_t n_views,
+                               const kba_lidar_view* views, const kba_lidar_options* opts, float* device_ms);
+
 #ifdef __cplusplus
 }
 #endif

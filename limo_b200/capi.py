@@ -10,7 +10,7 @@ import os
 
 import numpy as np
 
-from .capi_types import (KbaCounters, KbaCreateOut, KbaCreateRequest, KbaDeactivateOut, KbaDeactivateRequest, KbaDepthEntry, KbaDepthOut, KbaDepthRequest, KbaDrawFn, KbaEvalOut, KbaFlowOut, KbaFlowRequest, KbaLandmarkWrite, KbaLidarOptions, KbaOptions, KbaPoseWrite, KbaPushRequest, KbaRankedRequest, KbaRankOut, KbaRankRequest, KbaReclaimOut, KbaReclaimRequest, KbaResult, KbaSelectOut, KbaSelectParams, KbaSelectRequest,
+from .capi_types import (KbaCounters, KbaCreateOut, KbaCreateRequest, KbaDeactivateOut, KbaDeactivateRequest, KbaDepthEntry, KbaDepthOut, KbaDepthRequest, KbaDrawFn, KbaEvalOut, KbaFlowOut, KbaFlowRequest, KbaLandmarkWrite, KbaLidarCloud, KbaLidarOptions, KbaLidarView, KbaOptions, KbaPoseWrite, KbaPushRequest, KbaRankedRequest, KbaRankOut, KbaRankRequest, KbaReclaimOut, KbaReclaimRequest, KbaResult, KbaSelectOut, KbaSelectParams, KbaSelectRequest,
                          KbaTrackCaps, KbaTrackFrame, KbaTrackRequest, KbaWindow, Result, Window, c_double_p, c_float_p, c_int32_p,
                          c_uint8_p)
 
@@ -34,7 +34,8 @@ SYMBOLS = ["kba_version", "kba_last_error", "kba_default_options", "kba_create",
            "kba_track_rank_landmarks", "kba_track_group_rank_landmarks", "kba_track_solve_ranked", "kba_track_group_solve_ranked",
            "kba_solve_batch_opts", "kba_batch_solve_opts", "kba_track_group_solve_opts", "kba_track_group_solve_ranked_opts",
            "kba_track_group_adjust_pose_opts", "kba_track_group_push_keyframes", "kba_track_group_drop_keyframes",
-           "kba_track_group_set_landmarks", "kba_track_group_set_keyframe_poses"]
+           "kba_track_group_set_landmarks", "kba_track_group_set_keyframe_poses", "kba_lidar_depth_batch",
+           "kba_lidar_depth_batch_opts"]
 
 
 class KbaError(RuntimeError):
@@ -168,6 +169,8 @@ def lib():
         fp = C.POINTER(C.c_float)
         L.kba_lidar_depth.argtypes = [vp, fp, C.c_int32, C.c_int32, c_double_p, c_double_p, fp, C.c_int32,
                                       C.POINTER(KbaLidarOptions), fp, fp]
+        for f in (L.kba_lidar_depth_batch, L.kba_lidar_depth_batch_opts):
+            f.argtypes = [vp, C.c_int32, C.POINTER(KbaLidarCloud), C.c_int32, C.POINTER(KbaLidarView), C.POINTER(KbaLidarOptions), fp]
         _lib = L
     return _lib
 
@@ -199,6 +202,43 @@ def lidar_default_options():
     o = KbaLidarOptions()
     lib().kba_lidar_default_options(C.byref(o))
     return o
+
+
+def _lidar_batch_request(clouds, views, opt):
+    """the arguments of kba_lidar_depth_batch(_opts) for Handle.lidar_depth_batch: (C function, clouds array, views array,
+    options argument, one depth array per view, the arrays the structs point into).  opt None or one KbaLidarOptions -> the
+    single-options function; a sequence with one KbaLidarOptions (or None: the defaults) per view -> the _opts form.  A view
+    naming a missing cloud, or an opt sequence of the wrong length, raises before any C call."""
+    cl = [np.ascontiguousarray(c, dtype=np.float32) for c in clouds]
+    for i, c in enumerate(cl):
+        if c.ndim != 2:
+            raise ValueError("cloud %d: an [n, stride] array expected, got shape %s" % (i, c.shape))
+    carr = (KbaLidarCloud * len(cl))()
+    for c, a in zip(carr, cl):
+        c.points, c.n_points, c.stride = a.ctypes.data_as(c_float_p), a.shape[0], a.shape[1]
+    views = list(views)
+    varr = (KbaLidarView * len(views))()
+    keep, outs = list(cl), []
+    for i, (v, (ci, T, K, uv)) in enumerate(zip(varr, views)):
+        if not 0 <= int(ci) < len(cl):
+            raise IndexError("view %d names cloud %d, there are %d clouds" % (i, int(ci), len(cl)))
+        T = np.ascontiguousarray(T, dtype=np.float64).ravel(); K = np.ascontiguousarray(K, dtype=np.float64).ravel()
+        uv = np.ascontiguousarray(uv, dtype=np.float32).reshape(-1, 2)
+        if T.size != 7 or K.size != 3:
+            raise ValueError("view %d: T_cam_lidar has 7 entries and intr 3, got %d and %d" % (i, T.size, K.size))
+        out = np.full(len(uv), -1.0, dtype=np.float32)
+        keep += [T, K, uv]
+        outs.append(out)
+        v.cloud, v.n_features = int(ci), len(uv)
+        v.T_cam_lidar, v.intr, v.features_uv = T.ctypes.data_as(c_double_p), K.ctypes.data_as(c_double_p), uv.ctypes.data_as(c_float_p)
+        v.depth_out = out.ctypes.data_as(c_float_p) if len(uv) else None  # a view without features sits out
+    if opt is None or isinstance(opt, KbaLidarOptions):
+        return lib().kba_lidar_depth_batch, carr, varr, C.byref(opt or lidar_default_options()), outs, keep
+    opts = list(opt)
+    if len(opts) != len(views):
+        raise ValueError("%d option sets for %d views" % (len(opts), len(views)))
+    return (lib().kba_lidar_depth_batch_opts, carr, varr,
+            (KbaLidarOptions * len(opts))(*[o or lidar_default_options() for o in opts]), outs, keep)
 
 
 class Batch:
@@ -890,6 +930,15 @@ class Handle:
                                      len(feats), C.byref(opt or lidar_default_options()), out.ctypes.data_as(fp),
                                      C.byref(ms)))
         return out[:len(feats)], ms.value
+
+    def lidar_depth_batch(self, clouds, views, opt=None):
+        """depths of many views in one call (kba_lidar_depth_batch).  clouds: float32 [n, stride>=3] arrays; views:
+        (cloud index, T_cam_lidar, intr, features_uv [m, 2]) each; opt: None, one KbaLidarOptions, or one per view.  ->
+        (one float32 depth array [m] per view (-1 = none), device ms)"""
+        fn, carr, varr, o, outs, _keep = _lidar_batch_request(clouds, views, opt)
+        ms = C.c_float()
+        _check(fn(self._p, len(carr), carr, len(varr), varr, o, C.byref(ms)))
+        return outs, ms.value
 
     def counters(self, reset=False):
         c = KbaCounters()

@@ -214,6 +214,17 @@ class KbaLidarOptions(C.Structure):
     ]
 
 
+class KbaLidarCloud(C.Structure):
+    _fields_ = [("points", c_float_p), ("n_points", C.c_int32), ("stride", C.c_int32)]
+
+
+class KbaLidarView(C.Structure):
+    _fields_ = [
+        ("cloud", C.c_int32), ("n_features", C.c_int32), ("T_cam_lidar", c_double_p), ("intr", c_double_p),
+        ("features_uv", c_float_p), ("depth_out", c_float_p),
+    ]
+
+
 def _ptr(a, ctype):
     if a is None:
         return C.cast(None, C.POINTER(ctype))

@@ -1,13 +1,22 @@
-// kba_lidar.cu -- lidar depth extraction on sm_90a (BASELINE config 4; C ABI: kba_lidar_depth in kba_b200.h).
-//   k_lidar_bin<false>: project the cloud (coalesced float loads), count points per 16x16-pixel image cell
-//   k_lidar_scan      : exclusive scan of the cell counts (one CTA)
-//   k_lidar_bin<true> : project again and scatter (u, v, x, y, z, index) into cell-sorted order
-//   k_lidar_feature   : one warp per feature: gather the pixel rectangle from the overlapping cells, depth histogram,
-//                       largest triangle, plane / view-ray intersection, depth gates
+// kba_lidar.cu -- lidar depth extraction on sm_90a (BASELINE config 4; C ABI: kba_lidar_depth_batch and kba_lidar_depth, its
+// one-view case, in kba_b200.h).  A call works on "views": a cloud seen by one camera with one feature list.  Per-view
+// parameters live in a device array; each view's cell counts, starts and cursors sit at its own offset of one concatenated
+// array, and its sorted point records in a segment of its cloud's n_points.
+//   k_lidar_bin<false>: all (view, point) pairs: project the cloud (coalesced float loads), count points per 16x16-pixel cell
+//   k_lidar_scan      : one CTA per view: exclusive scan of its cell counts
+//   k_lidar_bin<true> : project again and scatter (u, v, x, y, z, index) into each view's cell-sorted order
+//   k_lidar_feature   : one warp per feature of all views: gather the pixel rectangle from the overlapping cells, depth
+//                       histogram, largest triangle, plane / view-ray intersection, depth gates
+// The bin passes map a block to its view by a per-view block-offset prefix (binary search), the feature pass a warp by the
+// feature-offset prefix: no CTA idles on a view smaller than the largest.
 // Compiled with -fmad=false: the arithmetic is single precision with the operation order of the specification so that the
 // discrete decisions (rectangle membership, histogram bin, arg-max triangle) do not depend on FMA contraction.
+#include <algorithm>
+#include <climits>
 #include <cstdint>
+#include <cstring>
 #include <string>
+#include <vector>
 
 #include <cuda_runtime.h>
 
@@ -26,9 +35,25 @@ struct LidarParams {
     int hist_min_count, min_points;
     float depth_min, depth_max, local_tol, crossnorm_min, viewray_min;
     int local_enabled;
+    // where the view's data sits in the call's concatenated device arrays
+    long long cloud_off;       // floats, into the clouds
+    int n_points, stride;
+    int cell_off;              // cells_x * cells_y + 1 entries of counts, cursors and starts
+    int sort_off;              // n_points sorted point records
 };
 
 struct ProjPt { float u, v, x, y, z; int idx; };
+
+// the segment of x in a prefix off[0] = 0 <= ... <= off[n] with x < off[n]: the largest s < n with off[s] <= x (empty
+// segments are skipped)
+__device__ __forceinline__ int segment_of(const int* __restrict__ off, int n, int x) {
+    int lo = 0, hi = n - 1;
+    while (lo < hi) {
+        const int mid = (lo + hi + 1) >> 1;
+        if (off[mid] <= x) lo = mid; else hi = mid - 1;
+    }
+    return lo;
+}
 
 __device__ __forceinline__ bool project(const LidarParams& P, const float* __restrict__ p, ProjPt& o) {
     const float x = P.R[0] * p[0] + P.R[1] * p[1] + P.R[2] * p[2] + P.t[0];
@@ -41,25 +66,35 @@ __device__ __forceinline__ bool project(const LidarParams& P, const float* __res
     return true;
 }
 
+// blk_off[n_views + 1]: blocks of 256 points per view
 template <bool kFill>
-__global__ void __launch_bounds__(256) k_lidar_bin(LidarParams P, const float* __restrict__ cloud, int n, int stride,
-                                                   int* __restrict__ cell_count, const int* __restrict__ cell_start,
-                                                   int* __restrict__ cell_cursor, ProjPt* __restrict__ sorted) {
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
+__global__ void __launch_bounds__(256) k_lidar_bin(const LidarParams* __restrict__ par, const int* __restrict__ blk_off, int n_views,
+                                                   const float* __restrict__ clouds, int* __restrict__ cell_count,
+                                                   const int* __restrict__ cell_start, int* __restrict__ cell_cursor,
+                                                   ProjPt* __restrict__ sorted) {
+    const int view = segment_of(blk_off, n_views, blockIdx.x);
+    const LidarParams& P = par[view];
+    const int i = (blockIdx.x - blk_off[view]) * blockDim.x + threadIdx.x;
+    if (i >= P.n_points) return;
     ProjPt q;
-    if (!project(P, cloud + (size_t)i * stride, q)) return;
-    const int cell = ((int)q.v / kCell) * P.cells_x + ((int)q.u / kCell);
+    if (!project(P, clouds + P.cloud_off + (size_t)i * P.stride, q)) return;
+    const int cell = P.cell_off + ((int)q.v / kCell) * P.cells_x + ((int)q.u / kCell);
     if (!kFill) {
         atomicAdd(&cell_count[cell], 1);
     } else {
         q.idx = i;
-        sorted[cell_start[cell] + atomicAdd(&cell_cursor[cell], 1)] = q;
+        sorted[P.sort_off + cell_start[cell] + atomicAdd(&cell_cursor[cell], 1)] = q;
     }
 }
 
-__global__ void __launch_bounds__(1024) k_lidar_scan(const int* __restrict__ cnt, int* __restrict__ start, int ncell) {
+// one CTA per view; a view's starts are relative to its sorted segment
+__global__ void __launch_bounds__(1024) k_lidar_scan(const LidarParams* __restrict__ par, const int* __restrict__ cell_count,
+                                                     int* __restrict__ cell_start) {
     __shared__ int s_part[1024];
+    const LidarParams& P = par[blockIdx.x];
+    const int* cnt = cell_count + P.cell_off;
+    int* start = cell_start + P.cell_off;
+    const int ncell = P.cells_x * P.cells_y;
     const int per = (ncell + 1023) / 1024, b0 = threadIdx.x * per;
     int s = 0;
     for (int c = b0; c < min(ncell, b0 + per); ++c) s += cnt[c];
@@ -80,17 +115,25 @@ __device__ __forceinline__ int bin_of(float z, float zmin, float bw) {
     return b > kBins - 1 ? kBins - 1 : b;
 }
 
-__global__ void __launch_bounds__(128) k_lidar_feature(LidarParams P, const ProjPt* __restrict__ sorted,
-                                                       const int* __restrict__ cell_start, const float* __restrict__ feats,
+// feat_off[n_views + 1]: the views' features concatenated, n_feats in all.  The result does not depend on the order in which
+// the fill pass's atomics placed the points inside a cell: the histogram counts and the nearest depth are order-free, the
+// largest triangle is chosen by area and then by the points' original indices, and a rectangle with more than kMaxNb points
+// gives -1 whatever was gathered.  That is what makes the depths bit-identical to the sequential specification.
+__global__ void __launch_bounds__(128) k_lidar_feature(const LidarParams* __restrict__ par, const int* __restrict__ feat_off,
+                                                       int n_views, const ProjPt* __restrict__ sorted_all,
+                                                       const int* __restrict__ cell_start_all, const float* __restrict__ feats,
                                                        int n_feats, float* __restrict__ out) {
     __shared__ ProjPt s_nb[4][kMaxNb];
     __shared__ int s_cnt[4][kBins];
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int k = blockIdx.x * 4 + warp;
     if (k >= n_feats) return;
+    const LidarParams P = par[segment_of(feat_off, n_views, k)];  // a copy: read through a reference it spills (ptxas -v)
+    const ProjPt* sorted = sorted_all + P.sort_off;
+    const int* cell_start = cell_start_all + P.cell_off;
     ProjPt* nb = s_nb[warp];
     int* cnt = s_cnt[warp];
-    const float fu = feats[2 * k], fv = feats[2 * k + 1];
+    const float fu = feats[2 * (size_t)k], fv = feats[2 * (size_t)k + 1];
     const float cu = fu + P.offx, cv = fv + P.offy;
     // ---- gather the rectangle ----
     const int cx0 = max(0, (int)floorf((cu - P.hw) / kCell)), cx1 = min(P.cells_x - 1, (int)floorf((cu + P.hw) / kCell));
@@ -207,6 +250,25 @@ void quat_R(const double* q, float* R) {
     for (int i = 0; i < 9; ++i) R[i] = (float)M[i];
 }
 
+// a view's pose, intrinsics and options in the kernels' single precision; a negative image size has no cells
+void view_params(const kba_lidar_view& v, const kba_lidar_options* o, LidarParams& P) {
+    const double* T = v.T_cam_lidar;
+    const double* intr = v.intr;
+    quat_R(T, P.R);
+    P.t[0] = (float)T[4]; P.t[1] = (float)T[5]; P.t[2] = (float)T[6];
+    P.f = (float)intr[0]; P.cx = (float)intr[1]; P.cy = (float)intr[2];
+    P.width = o->image_width; P.height = o->image_height;
+    P.cells_x = std::max(0, (P.width + kCell - 1) / kCell); P.cells_y = std::max(0, (P.height + kCell - 1) / kCell);
+    P.hw = 0.5f * (float)o->rect_width; P.hh = 0.5f * (float)o->rect_height;
+    P.offx = (float)o->rect_offset_x; P.offy = (float)o->rect_offset_y; P.bw = (float)o->hist_bin_width;
+    P.hist_min_count = o->hist_min_count; P.min_points = o->min_points;
+    P.depth_min = (float)o->depth_min; P.depth_max = (float)o->depth_max;
+    P.local_enabled = o->local_rel_tolerance >= 0; P.local_tol = (float)o->local_rel_tolerance;
+    P.crossnorm_min = (float)o->triangle_crossnorm_min; P.viewray_min = (float)o->viewray_plane_min;
+}
+
+size_t al(size_t b) { return (b + 255) & ~(size_t)255; }
+
 }  // namespace
 
 extern "C" void kba_lidar_default_options(kba_lidar_options* o) {
@@ -224,60 +286,121 @@ extern "C" int kba_internal_stream(kba_handle* h, cudaStream_t* s, int* device);
 extern "C" int kba_internal_fail(int code, const char* msg);
 extern "C" int kba_internal_workspace(kba_handle* h, size_t bytes, void** out);
 
-extern "C" int kba_lidar_depth(kba_handle* h, const float* cloud, int32_t n_points, int32_t stride, const double* T,
-                               const double* intr, const float* feats, int32_t n_feats, const kba_lidar_options* o,
-                               float* depth_out, float* device_ms) {
-    if (!h || !cloud || !T || !intr || !feats || !o || !depth_out || stride < 3 || n_points < 0 || n_feats < 0)
-        return kba_internal_fail(KBA_ERR_BAD_ARG, "bad argument to kba_lidar_depth");
+namespace {
+
+int fail_at(int code, const char* fn, const char* what, long long i, const char* msg) {
+    const std::string m = std::string(fn) + ": " + what + " " + std::to_string(i) + ": " + msg;
+    return kba_internal_fail(code, m.c_str());
+}
+
+// the host code of every lidar call: opts[0] for every view, or opts[i] for view i (per_view)
+int lidar_batch(kba_handle* h, int32_t n_clouds, const kba_lidar_cloud* clouds, int32_t n_views, const kba_lidar_view* views,
+                const kba_lidar_options* opts, bool per_view, float* device_ms, const char* fn) {
+    const std::string name(fn);
+    if (!h) return kba_internal_fail(KBA_ERR_BAD_ARG, (name + ": null handle").c_str());
+    if (n_clouds < 0 || n_views < 0) return kba_internal_fail(KBA_ERR_BAD_ARG, (name + ": negative cloud or view count").c_str());
+    if ((n_clouds > 0 && !clouds) || (n_views > 0 && !views)) return kba_internal_fail(KBA_ERR_BAD_ARG, (name + ": null clouds or views").c_str());
+    // ---- validation: views, then the clouds the working views name, then the 32-bit totals ----
+    std::vector<int> work;
+    for (int i = 0; i < n_views; ++i) {
+        const kba_lidar_view& v = views[i];
+        if (v.n_features < 0) return fail_at(KBA_ERR_BAD_ARG, fn, "view", i, "negative n_features");
+        if (v.n_features == 0) continue;
+        if (v.cloud < 0 || v.cloud >= n_clouds) return fail_at(KBA_ERR_BAD_ARG, fn, "view", i, "cloud index out of range");
+        if (!v.T_cam_lidar || !v.intr || !v.features_uv || !v.depth_out) return fail_at(KBA_ERR_BAD_ARG, fn, "view", i, "null pointer");
+        work.push_back(i);
+    }
+    if (work.empty()) {
+        if (device_ms) *device_ms = 0.0f;
+        return KBA_OK;
+    }
+    if (!opts) return kba_internal_fail(KBA_ERR_BAD_ARG, (name + ": null options").c_str());
+    std::vector<long long> cloud_off(n_clouds, -1);  // floats into the device clouds; -1: no working view names it
+    size_t b_clouds = 0;
+    for (int i : work) {
+        const int c = views[i].cloud;
+        if (cloud_off[c] >= 0) continue;
+        const kba_lidar_cloud& cl = clouds[c];
+        if (cl.n_points < 0) return fail_at(KBA_ERR_BAD_ARG, fn, "cloud", c, "negative n_points");
+        if (cl.stride < 3) return fail_at(KBA_ERR_BAD_ARG, fn, "cloud", c, "stride < 3");
+        if (cl.n_points > 0 && !cl.points) return fail_at(KBA_ERR_BAD_ARG, fn, "cloud", c, "null points");
+        cloud_off[c] = (long long)(b_clouds / sizeof(float));
+        b_clouds += al(sizeof(float) * (size_t)cl.n_points * cl.stride);
+    }
+    const int nw = (int)work.size();
+    std::vector<LidarParams> par(nw);
+    std::vector<int> blk_off(nw + 1, 0), feat_off(nw + 1, 0);
+    long long cells = 0, pairs = 0, blocks = 0, feats = 0;
+    for (int w = 0; w < nw; ++w) {
+        const int i = work[w];
+        const kba_lidar_view& v = views[i];
+        const kba_lidar_cloud& cl = clouds[v.cloud];
+        LidarParams& P = par[w];
+        view_params(v, per_view ? &opts[i] : opts, P);
+        P.cloud_off = cloud_off[v.cloud]; P.n_points = cl.n_points; P.stride = cl.stride;
+        P.cell_off = (int)std::min<long long>(cells, INT_MAX); P.sort_off = (int)std::min<long long>(pairs, INT_MAX);
+        cells += (long long)P.cells_x * P.cells_y + 1;
+        pairs += cl.n_points;
+        blocks += (cl.n_points + 255) / 256;
+        feats += v.n_features;
+        if (cells > INT_MAX || pairs > INT_MAX || 2 * feats > INT_MAX)
+            return fail_at(KBA_ERR_CAPACITY, fn, "view", i, "the call's cells, (view, point) pairs or features exceed 32-bit indexing");
+        blk_off[w + 1] = (int)blocks; feat_off[w + 1] = (int)feats;
+    }
     cudaStream_t s;
     int device;
     if (kba_internal_stream(h, &s, &device) != KBA_OK) return KBA_ERR_BAD_ARG;
-    LidarParams P;
-    quat_R(T, P.R);
-    P.t[0] = (float)T[4]; P.t[1] = (float)T[5]; P.t[2] = (float)T[6];
-    P.f = (float)intr[0]; P.cx = (float)intr[1]; P.cy = (float)intr[2];
-    P.width = o->image_width; P.height = o->image_height;
-    P.cells_x = (P.width + kCell - 1) / kCell; P.cells_y = (P.height + kCell - 1) / kCell;
-    P.hw = 0.5f * (float)o->rect_width; P.hh = 0.5f * (float)o->rect_height;
-    P.offx = (float)o->rect_offset_x; P.offy = (float)o->rect_offset_y; P.bw = (float)o->hist_bin_width;
-    P.hist_min_count = o->hist_min_count; P.min_points = o->min_points;
-    P.depth_min = (float)o->depth_min; P.depth_max = (float)o->depth_max;
-    P.local_enabled = o->local_rel_tolerance >= 0; P.local_tol = (float)o->local_rel_tolerance;
-    P.crossnorm_min = (float)o->triangle_crossnorm_min; P.viewray_min = (float)o->viewray_plane_min;
-    const int ncell = P.cells_x * P.cells_y;
-    // one device workspace owned by the handle (grow-only): cloud | features | depths | cell counts, starts, cursors | sorted points
-    auto al = [](size_t b) { return (b + 255) & ~(size_t)255; };
-    const size_t b_cloud = al(sizeof(float) * (size_t)std::max(n_points, 1) * stride), b_feat = al(sizeof(float) * 2 * (size_t)std::max(n_feats, 1)),
-                 b_out = al(sizeof(float) * (size_t)std::max(n_feats, 1)), b_cell = al(sizeof(int) * (size_t)(ncell + 1)),
-                 b_sorted = al(sizeof(ProjPt) * (size_t)std::max(n_points, 1));
+    // one device workspace owned by the handle (grow-only):
+    //   clouds | packed upload (features | view parameters | block and feature prefixes) | depths | cell counts, cursors | cell
+    //   starts | sorted point records
+    const size_t b_feat = al(sizeof(float) * 2 * (size_t)feats), b_par = al(sizeof(LidarParams) * nw), b_pre = al(sizeof(int) * (nw + 1)),
+                 b_pack = b_feat + b_par + 2 * b_pre, b_out = al(sizeof(float) * (size_t)feats), b_cell = al(sizeof(int) * (size_t)cells),
+                 b_sorted = al(sizeof(ProjPt) * (size_t)std::max(pairs, 1LL));
     void* ws = nullptr;
-    if (kba_internal_workspace(h, b_cloud + b_feat + b_out + 3 * b_cell + b_sorted, &ws) != KBA_OK) return KBA_ERR_CUDA;
+    if (kba_internal_workspace(h, b_clouds + b_pack + b_out + 3 * b_cell + b_sorted, &ws) != KBA_OK) return KBA_ERR_CUDA;
     char* wp = (char*)ws;
-    float* d_cloud = (float*)wp; wp += b_cloud;
-    float* d_feats = (float*)wp; wp += b_feat;
+    float* d_clouds = (float*)wp; wp += b_clouds;
+    char* d_pack = wp; wp += b_pack;
+    const float* d_feats = (const float*)d_pack;
+    const LidarParams* d_par = (const LidarParams*)(d_pack + b_feat);
+    const int* d_blk = (const int*)(d_pack + b_feat + b_par);
+    const int* d_fo = (const int*)(d_pack + b_feat + b_par + b_pre);
     float* d_out = (float*)wp; wp += b_out;
     int* d_cnt = (int*)wp; wp += b_cell;
+    int* d_cur = (int*)wp; wp += b_cell;  // right after the counts: one memset clears both
     int* d_start = (int*)wp; wp += b_cell;
-    int* d_cur = (int*)wp; wp += b_cell;
     ProjPt* d_sorted = (ProjPt*)wp;
+    // host staging of the packed upload and of the depths, grow-only per host thread
+    static thread_local std::vector<char> pack;
+    static thread_local std::vector<float> depths;
+    if (pack.size() < b_pack) pack.resize(b_pack);
+    if (depths.size() < (size_t)feats) depths.resize((size_t)feats);
+    for (int w = 0; w < nw; ++w) {
+        const kba_lidar_view& v = views[work[w]];
+        memcpy(pack.data() + sizeof(float) * 2 * (size_t)feat_off[w], v.features_uv, sizeof(float) * 2 * (size_t)v.n_features);
+    }
+    memcpy(pack.data() + b_feat, par.data(), sizeof(LidarParams) * nw);
+    memcpy(pack.data() + b_feat + b_par, blk_off.data(), sizeof(int) * (nw + 1));
+    memcpy(pack.data() + b_feat + b_par + b_pre, feat_off.data(), sizeof(int) * (nw + 1));
     cudaEvent_t e0 = nullptr, e1 = nullptr;
     cudaError_t err = cudaSuccess;
     auto chk = [&](cudaError_t e) { if (err == cudaSuccess && e != cudaSuccess) err = e; };
     chk(cudaSetDevice(device));
     if (device_ms) { chk(cudaEventCreate(&e0)); chk(cudaEventCreate(&e1)); }
     if (err == cudaSuccess) {
-        chk(cudaMemcpyAsync(d_cloud, cloud, sizeof(float) * (size_t)n_points * stride, cudaMemcpyHostToDevice, s));
-        chk(cudaMemcpyAsync(d_feats, feats, sizeof(float) * 2 * (size_t)n_feats, cudaMemcpyHostToDevice, s));
+        for (int c = 0; c < n_clouds; ++c)
+            if (cloud_off[c] >= 0 && clouds[c].n_points > 0)
+                chk(cudaMemcpyAsync(d_clouds + cloud_off[c], clouds[c].points, sizeof(float) * (size_t)clouds[c].n_points * clouds[c].stride,
+                                    cudaMemcpyHostToDevice, s));
+        chk(cudaMemcpyAsync(d_pack, pack.data(), b_pack, cudaMemcpyHostToDevice, s));
         if (e0) chk(cudaEventRecord(e0, s));
-        chk(cudaMemsetAsync(d_cnt, 0, sizeof(int) * ncell, s));
-        chk(cudaMemsetAsync(d_cur, 0, sizeof(int) * ncell, s));
-        const int gp = (n_points + 255) / 256;
-        if (n_points > 0) k_lidar_bin<false><<<gp, 256, 0, s>>>(P, d_cloud, n_points, stride, d_cnt, nullptr, nullptr, nullptr);
-        k_lidar_scan<<<1, 1024, 0, s>>>(d_cnt, d_start, ncell);
-        if (n_points > 0) k_lidar_bin<true><<<gp, 256, 0, s>>>(P, d_cloud, n_points, stride, d_cnt, d_start, d_cur, d_sorted);
-        if (n_feats > 0) k_lidar_feature<<<(n_feats + 3) / 4, 128, 0, s>>>(P, d_sorted, d_start, d_feats, n_feats, d_out);
+        chk(cudaMemsetAsync(d_cnt, 0, 2 * b_cell, s));
+        if (blocks > 0) k_lidar_bin<false><<<(unsigned)blocks, 256, 0, s>>>(d_par, d_blk, nw, d_clouds, d_cnt, nullptr, nullptr, nullptr);
+        k_lidar_scan<<<nw, 1024, 0, s>>>(d_par, d_cnt, d_start);
+        if (blocks > 0) k_lidar_bin<true><<<(unsigned)blocks, 256, 0, s>>>(d_par, d_blk, nw, d_clouds, d_cnt, d_start, d_cur, d_sorted);
+        k_lidar_feature<<<(unsigned)((feats + 3) / 4), 128, 0, s>>>(d_par, d_fo, nw, d_sorted, d_start, d_feats, (int)feats, d_out);
         if (e1) chk(cudaEventRecord(e1, s));
-        chk(cudaMemcpyAsync(depth_out, d_out, sizeof(float) * (size_t)n_feats, cudaMemcpyDeviceToHost, s));
+        chk(cudaMemcpyAsync(depths.data(), d_out, sizeof(float) * (size_t)feats, cudaMemcpyDeviceToHost, s));
         chk(cudaStreamSynchronize(s));
         chk(cudaGetLastError());
         if (err == cudaSuccess && device_ms) chk(cudaEventElapsedTime(device_ms, e0, e1));
@@ -285,5 +408,32 @@ extern "C" int kba_lidar_depth(kba_handle* h, const float* cloud, int32_t n_poin
     if (e0) cudaEventDestroy(e0);
     if (e1) cudaEventDestroy(e1);
     if (err != cudaSuccess) return kba_internal_fail(KBA_ERR_CUDA, cudaGetErrorString(err));
+    for (int w = 0; w < nw; ++w) {
+        const kba_lidar_view& v = views[work[w]];
+        memcpy(v.depth_out, depths.data() + feat_off[w], sizeof(float) * (size_t)v.n_features);
+    }
     return KBA_OK;
+}
+
+}  // namespace
+
+extern "C" int kba_lidar_depth_batch(kba_handle* h, int32_t n_clouds, const kba_lidar_cloud* clouds, int32_t n_views,
+                                     const kba_lidar_view* views, const kba_lidar_options* opt, float* device_ms) {
+    return lidar_batch(h, n_clouds, clouds, n_views, views, opt, false, device_ms, "kba_lidar_depth_batch");
+}
+
+extern "C" int kba_lidar_depth_batch_opts(kba_handle* h, int32_t n_clouds, const kba_lidar_cloud* clouds, int32_t n_views,
+                                          const kba_lidar_view* views, const kba_lidar_options* opts, float* device_ms) {
+    return lidar_batch(h, n_clouds, clouds, n_views, views, opts, true, device_ms, "kba_lidar_depth_batch_opts");
+}
+
+// the one-view, one-cloud batch
+extern "C" int kba_lidar_depth(kba_handle* h, const float* cloud, int32_t n_points, int32_t stride, const double* T,
+                               const double* intr, const float* feats, int32_t n_feats, const kba_lidar_options* o,
+                               float* depth_out, float* device_ms) {
+    if (!h || !cloud || !T || !intr || !feats || !o || !depth_out || stride < 3 || n_points < 0 || n_feats < 0)
+        return kba_internal_fail(KBA_ERR_BAD_ARG, "bad argument to kba_lidar_depth");
+    const kba_lidar_cloud c{cloud, n_points, stride};
+    const kba_lidar_view v{0, n_feats, T, intr, feats, depth_out};
+    return lidar_batch(h, 1, &c, 1, &v, o, false, device_ms, "kba_lidar_depth");
 }
