@@ -215,7 +215,8 @@ void kba_destroy(kba_handle* h);
 int kba_set_stream(kba_handle* h, void* cuda_stream);    /* cudaStream_t; NULL = default stream */
 
 /* --- host-buffer entry points (the reference-facing calls) --- */
-/* replaces robust_optimization::solveTrimmed(...) as called from solve() (cpp:765) */
+/* replaces robust_optimization::solveTrimmed(...) as called from solve() (cpp:765); up to 128 keyframes per window, ground-plane
+ * blocks included (kba_batch_create's limits) */
 int kba_solve_window(kba_handle* h, const kba_window* w, const kba_options* opt, kba_result* res);
 /* many independent windows in one call ("BA windows/s") */
 int kba_solve_batch(kba_handle* h, int32_t n_windows, const kba_window* w, const kba_options* opt, kba_result* res);
@@ -229,6 +230,9 @@ int kba_solve_batch_opts(kba_handle* h, int32_t n_windows, const kba_window* w, 
 int kba_eval(kba_handle* h, const kba_window* w, const kba_options* opt, kba_eval_out* out);
 
 /* --- device-resident batch (inputs stay in HBM between solves) --- */
+/* A window has at most 128 keyframes (KBA_ERR_CAPACITY): a reduced system of up to 1281 rows with ground-plane blocks, allocated
+ * as 1344 (about 14.5 MB per window for A plus as much per CTA its Schur sum is split over).  Above 640 rows the factorisation
+ * is always spread over the GPU.  The same limits hold for kba_solve_window / kba_solve_batch, which create such a batch. */
 int kba_batch_create(kba_handle* h, int32_t n_windows, const kba_window* w, kba_batch** out);
 int kba_batch_upload(kba_batch* b, int32_t n_windows, const kba_window* w); /* re-upload state, same shapes */
 /* resets to the uploaded state and solves; returns when every window is done.  Issued as ONE CUDA graph launch (the
@@ -281,7 +285,8 @@ int kba_shard_comm_create_local(kba_handle* const* handles, int32_t world, kba_s
 void kba_shard_comm_destroy(kba_shard_comm* c);
 /* b holds this rank's shard; lm_begin = index of its first landmark in the whole window, lm_total = landmarks of the
  * whole window.  Collective: every rank calls it, and afterwards kba_batch_solve is a collective call that every rank must make.
- * Restrictions: one window per batch (KBA_ERR_BAD_ARG), every free keyframe is in the program, and every shard must size the
+ * Restrictions: one window per batch (KBA_ERR_BAD_ARG; up to 128 keyframes, as kba_batch_create takes), every free keyframe is
+ * in the program, and every shard must size the
  * same reduced system (KBA_ERR_BAD_ARG otherwise): with plane_reg_weight = 0 a shard has plane rows only if it holds
  * ground-plane residuals, so then every shard must hold some, or none.  The window's scalars -- scale regulariser,
  * plane_reg_weight, plane_dist_fixed, speed prior -- are given to every shard with the same values (shard_window copies them).
@@ -311,7 +316,8 @@ typedef struct kba_track_caps {
     int32_t win_observations;  /*                 observations                        */
     int32_t win_ground;        /*                 ground-plane residuals, or candidates of a device attachment (<= win_landmarks) */
     int32_t win_rows;          /*                 reduced-system rows: 6 per keyframe, 10 with plane blocks, plus one.  0: the fused
-                                                  path's limits above; else 6 * win_keyframes + 1 .. 640, see kba_track_solve */
+                                                  path's limits above; else 6 * win_keyframes + 1 .. 640 (the track's own
+                                                  limit; kba_batch_create takes more), see kba_track_solve */
 } kba_track_caps;
 int kba_track_create(kba_handle* h, const kba_track_caps* caps, int32_t n_cam, const double* cam_intr, const double* cam_pose,
                      kba_track** out);

@@ -777,7 +777,7 @@ static int batch_upload(kba_batch* b, int32_t n_windows, const kba_window* w, co
 static void apply_plan(kba_batch* b) {
     const Plan& p = b->lc.plan;
     b->bd.nr_cap_max = p.nr_cap_max; b->bd.fused = p.fused; b->bd.p_split = p.p_split;
-    b->bd.solve_tiled = p.solve_tiled; b->bd.solve_split = p.solve_split;
+    b->bd.solve_tiled = p.solve_tiled; b->bd.solve_split = p.solve_split; b->bd.solve_banded = p.solve_banded;
 }
 
 // rows_of[i] (optional): reduced-system rows window i is sized for, instead of reduced_rows on all its keyframes.  A track's
@@ -830,7 +830,7 @@ static int batch_create(kba_handle* h, int32_t n_windows, const kba_window* w, c
     if (nr_cap_max > kMaxReducedRows) {
         b->release();
         delete b;
-        return fail(KBA_ERR_CAPACITY, "reduced system larger than 640 rows (106 keyframes, or 63 with ground-plane blocks)");
+        return fail(KBA_ERR_CAPACITY, "reduced system larger than 1344 rows (128 keyframes with ground-plane blocks)");
     }
     bd.tot_kf = kf; bd.tot_cam = cam; bd.tot_lm = lm; bd.tot_obs = obs; bd.tot_chunks = (int)chunks; bd.tot_gp = gp;
     bd.tot_groups = (int)groups;
@@ -1739,8 +1739,8 @@ int kba_track_create(kba_handle* h, const kba_track_caps* c, int32_t n_cam, cons
         return fail(KBA_ERR_BAD_ARG, "kba_track_create: capacities");
     if (c->win_rows < 0 || (c->win_rows > 0 && c->win_rows < reduced_rows(c->win_keyframes, false)))
         return fail(KBA_ERR_BAD_ARG, "kba_track_create: win_rows must be 0 or at least 6 * win_keyframes + 1");
-    if (c->win_rows > kMaxReducedRows)
-        return fail(KBA_ERR_CAPACITY, "kba_track_create: win_rows larger than 640 (the largest reduced system kba_batch_create takes)");
+    if (c->win_rows > kTrackMaxRows)
+        return fail(KBA_ERR_CAPACITY, "kba_track_create: win_rows larger than 640 (the largest window a track's solver is sized for)");
     if (c->win_rows == 0 && reduced_rows(c->win_keyframes, false) > kFusedMaxRows)
         return fail(KBA_ERR_CAPACITY, "kba_track_create: the stored window must fit the fused path (<= 184 reduced rows: 30 keyframes; "
                                       "<= 32768 landmarks) -- give win_rows for larger windows");

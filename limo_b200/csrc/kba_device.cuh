@@ -11,7 +11,6 @@
 
 namespace kba {
 
-constexpr int kMaxKf = 128;         // keyframes per window the kernels stage in shared memory
 constexpr int kMaxCam = 8;
 constexpr int kPoseStride = 12;     // staged pose: R (9, row-major) + t (3)
 constexpr int kCamStride = 16;      // staged camera: Rc (9) + tc (3) + f, cx, cy, pad
@@ -166,6 +165,7 @@ struct BatchDev {
                               //    every accumulation (landmark blocks, Schur products, solve, cost) stays FP64
     int solve_tiled;          // 1: k_reduced_solve<true> (<= kTiledMaxRows rows, shared-memory resident)
     int solve_split;          // > 0: large system of a small batch, factorisation spread over this many CTAs per window
+    int solve_banded;         // 1: above kPanelMaxRows rows: k_sred_reduce writes A, k_chol_trail_band updates the trailing matrix
     double* chol_w;           // [n_win][32*32] inverse of the current diagonal block's factor (split factorisation)
     double* chol_invd;        // [n_win][nr_cap_max] 1 / L_ii
     double* bs_part;          // [n_win][bs_parts][4]: model_e, step_sq, xnorm_sq, gmax_e

@@ -1093,7 +1093,7 @@ __global__ void __launch_bounds__(512, 1) k_reduced_solve(BatchDev bd, int stage
         const size_t pstride = (size_t)ld * ld;
         const int np = 1;  // with p_split > 1, k_sred_reduce has folded the partials into slot 0
         const int rows = kTiled ? ((n + 8) & ~7) : n + 1;  // tiled: whole tile rows, zero padded
-        bool done_by_reduce = !kTiled && (bd.p_split > 1 || bd.sharded) && !wd.landmarks_fixed;  // see k_sred_reduce
+        bool done_by_reduce = !kTiled && (bd.p_split > 1 || bd.sharded || bd.solve_banded) && !wd.landmarks_fixed;  // see k_sred_reduce
         if (kTiled && bd.p_split > 1 && !bd.sharded && !wd.landmarks_fixed) {
             // k_sred_reduce left A tile-packed and padded in global memory (L2): a linear copy, 16 bytes per thread and load
             const int ntr = rows >> 3;
@@ -1643,6 +1643,82 @@ __global__ void __launch_bounds__(512, 1) k_chol_trail(BatchDev bd, int kb) {
     }
 }
 
+// trailing update above kPanelMaxRows rows, where no CTA holds the whole panel: the result is cut into 64x64 blocks (I >= J)
+// and every CTA takes every gridDim.x-th block, staging only the 64 panel rows of its row band and the 64 of its column band
+// (36 KB whatever n).  Warp w computes the 16x8 tiles (w & 3, 4 (w >> 2) .. 4 (w >> 2) + 3) of the block on m16n8k8 DMMA: one
+// accumulator per tile, the 32 panel columns summed in column order from zero, then subtracted from the element -- the same
+// operations for an element whichever CTA owns its block, so any solve_split gives the same bits.
+constexpr int kBandRows = 64;
+__global__ void __launch_bounds__(256, 2) k_chol_trail_band(BatchDev bd, int kb) {
+    const int w = blockIdx.y;
+    const WinState& st = bd.state[w];
+    if (st.phase != PH_ITERATE || st.solve_failed || kb + kNB >= st.n_f) return;  // nothing below a last, partial block
+    const WinDesc& wd = bd.desc[w];
+    const int n = st.n_f, ld = wd.nr_cap;
+    const int r0 = kb + kNB, m = n + 1 - r0, nbk = (m + kBandRows - 1) / kBandRows, npair = nbk * (nbk + 1) / 2;
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, fr = lane >> 2, fc = lane & 3;
+    __shared__ double s_X[2][kBandRows * kPanelStride];  // panel rows of the row band, of the column band
+    double* A = bd.amat + wd.s_off;
+    const int ta = warp & 3, tb0 = 4 * (warp >> 2);  // 16-row strip, first of the warp's four 8-column tiles
+    for (int p = blockIdx.x; p < npair; p += gridDim.x) {
+        int I = (int)((sqrtf(8.0f * (float)p + 1.0f) - 1.0f) * 0.5f);
+        while ((I + 1) * (I + 2) / 2 <= p) ++I;
+        while (I * (I + 1) / 2 > p) --I;
+        const int J = p - I * (I + 1) / 2;
+        for (int idx = tid; idx < 2 * kBandRows * kNB; idx += blockDim.x) {
+            const int h = idx / (kBandRows * kNB), i = (idx >> 5) & (kBandRows - 1), c = idx & 31;
+            const int row = kBandRows * (h ? J : I) + i;
+            s_X[h][i * kPanelStride + c] = row < m ? A[(size_t)(r0 + row) * ld + kb + c] : 0.0;
+        }
+        // the result elements this lane updates, requested before the tensor-core work: rows gr, gr + 8, columns gc, gc + 1
+        const int gr = r0 + kBandRows * I + 16 * ta + fr;
+        double2 cv[4][2];
+#pragma unroll
+        for (int t = 0; t < 4; ++t) {
+            const int gc = r0 + kBandRows * J + 8 * (tb0 + t) + 2 * fc;
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                const int r = gr + 8 * h;
+                cv[t][h] = make_double2(0.0, 0.0);
+                if (r <= n && gc + 1 <= r) cv[t][h] = *reinterpret_cast<const double2*>(A + (size_t)r * ld + gc);
+                else if (r <= n && gc <= r) cv[t][h].x = A[(size_t)r * ld + gc];
+            }
+        }
+        __syncthreads();
+        // a 16x8 tile that lies above the diagonal of a diagonal block, or below the last row, is not computed
+        const bool rows_live = kBandRows * I + 16 * ta < m;
+        double c[4][4];
+#pragma unroll
+        for (int t = 0; t < 4; ++t) c[t][0] = c[t][1] = c[t][2] = c[t][3] = 0.0;
+        if (rows_live) {
+            const double* pa = s_X[0] + (16 * ta + fr) * kPanelStride + fc;
+            const double* pb = s_X[1] + (8 * tb0 + fr) * kPanelStride + fc;
+#pragma unroll
+            for (int k = 0; k < kNB; k += 8) {
+                const double a0 = pa[k], a1 = pa[8 * kPanelStride + k], a2 = pa[k + 4], a3 = pa[8 * kPanelStride + k + 4];
+#pragma unroll
+                for (int t = 0; t < 4; ++t)
+                    if (I > J || 8 * (tb0 + t) <= 16 * ta + 15)
+                        dmma16k8(c[t], a0, a1, a2, a3, pb[8 * t * kPanelStride + k], pb[8 * t * kPanelStride + k + 4]);
+            }
+        }
+#pragma unroll
+        for (int t = 0; t < 4; ++t) {
+            const int gc = r0 + kBandRows * J + 8 * (tb0 + t) + 2 * fc;
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                const int r = gr + 8 * h;
+                double2 v = cv[t][h];
+                v.x -= c[t][2 * h];
+                v.y -= c[t][2 * h + 1];
+                if (r <= n && gc + 1 <= r) *reinterpret_cast<double2*>(A + (size_t)r * ld + gc) = v;
+                else if (r <= n && gc <= r) A[(size_t)r * ld + gc] = v.x;
+            }
+        }
+        __syncthreads();  // the next block's panel rows overwrite s_X
+    }
+}
+
 // =====================================================================================================================
 // back-substitution: delta_p_j = -L^-T (z_j + sum_i V_i^T delta_f,i); candidate landmarks; deterministic partial sums
 // =====================================================================================================================
@@ -2115,6 +2191,8 @@ static inline size_t schur_smem() { return (size_t)2 * kKC * kGS * sizeof(double
 static inline size_t schur_tma_smem() { return (size_t)2 * kStageDoubles * sizeof(double); }
 static inline size_t solve_smem(int ld) { return ((size_t)5 * ld + kNB + kNB * (kNB + 1) + (size_t)(ld + 8) * kPanelStride) * sizeof(double); }
 static inline size_t trail_smem(int ld) { return (size_t)(ld + 8) * kPanelStride * sizeof(double); }
+// stages 1 and 2 of k_reduced_solve<false> never touch the panel copy: all that grows with the rows above kPanelMaxRows
+static inline size_t solve_stage_smem(int ld) { return ((size_t)5 * ld + kNB + kNB * (kNB + 1)) * sizeof(double); }
 static inline size_t solve_tiled_smem(int ld) {
     const int nt = ld / 8;
     return ((size_t)5 * ld + kNB + kNB * (kNB + 1) + (size_t)nt * (nt + 1) / 2 * 64) * sizeof(double);
@@ -2125,6 +2203,7 @@ static inline size_t solve_tiled_smem(int ld) {
 // solves did exactly that: "invalid argument" at the next launch) -- so the sizes only ever grow, per device.
 cudaError_t configure_kernels(int nr_cap_max) {
     static int hi_tiled[64] = {0}, hi_rows[64] = {0};
+    static size_t hi_solve[64] = {0};
     static bool fixed_done[64] = {false};
     int dev = 0;
     cudaError_t e = cudaGetDevice(&dev);
@@ -2147,12 +2226,17 @@ cudaError_t configure_kernels(int nr_cap_max) {
         if (e != cudaSuccess) return e;
         hi_tiled[dev] = nr_cap_max;
     }
-    if (nr_cap_max > hi_rows[dev]) {
+    // above kPanelMaxRows: k_chol_trail is not launched, and k_reduced_solve<false> runs stages 1 and 2 only
+    if (nr_cap_max <= kPanelMaxRows && nr_cap_max > hi_rows[dev]) {
         e = cudaFuncSetAttribute(k_chol_trail, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)trail_smem(nr_cap_max));
         if (e != cudaSuccess) return e;
-        e = cudaFuncSetAttribute(k_reduced_solve<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)solve_smem(nr_cap_max));
-        if (e != cudaSuccess) return e;
         hi_rows[dev] = nr_cap_max;
+    }
+    const size_t solve = nr_cap_max <= kPanelMaxRows ? solve_smem(nr_cap_max) : solve_stage_smem(nr_cap_max);
+    if (solve > hi_solve[dev]) {
+        e = cudaFuncSetAttribute(k_reduced_solve<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)solve);
+        if (e != cudaSuccess) return e;
+        hi_solve[dev] = solve;
     }
     return cudaSuccess;
 }
@@ -2261,22 +2345,26 @@ int launch_pass(const BatchDev& bd, const LaunchCfg& lc, Counters* cnt, cudaStre
         bc.sred = bd.x_recv; bc.bkf = bd.x_recv + n_s; bc.cost_part_x = bd.x_recv + n_s + n_b + n_g; bc.cost_parts = bd.shard_cost_parts;
         if (n_g) { bc.gp_kfb = bd.x_recv + n_s + n_b; bc.gp_cost_x = bd.x_recv + n_s + n_b + 65LL * wh.n_kf; }
         k_sred_reduce<<<g_red, 256, 0, s>>>(bc, 2); LCHK("k_sred_reduce");
-    } else if (bd.p_split > 1) {
+    } else if (bd.p_split > 1 || bd.solve_banded) {  // banded: A = -Sred by the whole GPU, not by stage 1's one CTA
         k_sred_reduce<<<g_red, 256, 0, s>>>(bd, 0); LCHK("k_sred_reduce");
     }
     if (bd.solve_tiled) {
         k_reduced_solve<true><<<B, 512, solve_tiled_smem(lc.plan.nr_cap_max), s>>>(bc, 0); LCHK("k_reduced_solve");
     } else if (!bd.solve_split) {
         k_reduced_solve<false><<<B, 512, solve_smem(lc.plan.nr_cap_max), s>>>(bc, 0); LCHK("k_reduced_solve");
-    } else {  // few large windows: the factorisation is spread over the GPU, one 32-column block at a time
-        k_reduced_solve<false><<<B, 512, solve_smem(lc.plan.nr_cap_max), s>>>(bc, 1); LCHK("k_reduced_solve");
+    } else {  // few large windows, or any above kPanelMaxRows: the factorisation is spread over the GPU, one 32-column block at a time
+        const bool banded = bd.solve_banded != 0;
+        const size_t stage_smem = banded ? solve_stage_smem(lc.plan.nr_cap_max) : solve_smem(lc.plan.nr_cap_max);
+        k_reduced_solve<false><<<B, 512, stage_smem, s>>>(bc, 1); LCHK("k_reduced_solve");
         const int strips = (lc.plan.nr_cap_max + 7) / 8;
         for (int kb = 0; kb < lc.plan.nr_cap_max; kb += kNB) {
             k_chol_diag<<<B, 32, 0, s>>>(bc, kb); LCHK("k_chol_diag");
             k_chol_panel<<<dim3((strips + 15) / 16, B), 512, 0, s>>>(bc, kb); LCHK("k_chol_panel");
-            k_chol_trail<<<dim3(bd.solve_split, B), 512, trail_smem(lc.plan.nr_cap_max), s>>>(bc, kb); LCHK("k_chol_trail");
+            if (banded) k_chol_trail_band<<<dim3(bd.solve_split, B), 256, 0, s>>>(bc, kb);
+            else k_chol_trail<<<dim3(bd.solve_split, B), 512, trail_smem(lc.plan.nr_cap_max), s>>>(bc, kb);
+            LCHK("k_chol_trail");
         }
-        k_reduced_solve<false><<<B, 512, solve_smem(lc.plan.nr_cap_max), s>>>(bc, 2); LCHK("k_reduced_solve");
+        k_reduced_solve<false><<<B, 512, stage_smem, s>>>(bc, 2); LCHK("k_reduced_solve");
     }
     if (bd.fused) {
         const int n_units = (bd.max_lm + 15) / 16;
@@ -2307,7 +2395,7 @@ int launch_pass(const BatchDev& bd, const LaunchCfg& lc, Counters* cnt, cudaStre
         cnt->launches_total += gp; cnt->launches_prep += gp;                       // k_gp_blocks
         if (bd.sharded && bd.shard_gp) cnt->launches_total += 1;                   // k_shard_planes
         const int split = (!bd.solve_tiled && bd.solve_split) ? 1 + 3 * ((lc.plan.nr_cap_max + kNB - 1) / kNB) : 0;
-        cnt->launches_total += (bd.fused ? 0 : 1) + 1 + 1 + gp + prep + 1 + (bd.p_split > 1 ? 1 : 0) + 1 + split + 1 + 1 + gp + 1 + 2;
+        cnt->launches_total += (bd.fused ? 0 : 1) + 1 + 1 + gp + prep + 1 + (bd.p_split > 1 || bd.solve_banded ? 1 : 0) + 1 + split + 1 + 1 + gp + 1 + 2;
         cnt->launches_jacobian += 1; cnt->launches_prep += prep + gp; cnt->launches_schur += 1; cnt->launches_solve += 2;
         cnt->launches_backsub += 1; cnt->launches_cost += 1 + gp; cnt->launches_update += 1; cnt->launches_trim += 2;
     }

@@ -267,7 +267,7 @@ __global__ void __launch_bounds__(256) k_track_ground(BatchDev bd, const TrackSe
     const TrackSel& sel = sels[w];
     if (sel.n_cand == 0) return;  // idle, plane-free or host lists: untouched
     WinDesc& d = bd.desc[w];
-    __shared__ double s_T[kMaxKf][12];  // R row-major, t (a plane-carrying window on the large-window path has up to 63 keyframes)
+    __shared__ double s_T[kMaxKf][12];  // R row-major, t (every keyframe a window may have; a track's ground window has at most 63)
     __shared__ int s_use[kMaxKf];
     __shared__ int s_warp[8];
     __shared__ int s_base;

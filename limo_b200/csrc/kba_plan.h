@@ -9,12 +9,14 @@ namespace kba {
 constexpr int kFusedMaxRows = 184;          // every window within this many reduced rows: the fused path (k_schur_fused)
 constexpr int kSixSlotMaxRows = 176;        // k_schur_fused<6>: 11 16-row block rows; <7> has a 12th for up to kFusedMaxRows
 constexpr int kTiledMaxRows = 192;          // k_reduced_solve<true>: the reduced system factorised in one CTA's shared memory
-constexpr int kMaxReducedRows = 640;        // shared-memory panel copies of k_reduced_solve / k_chol_trail (227 KB per CTA)
+constexpr int kPanelMaxRows = 640;          // shared-memory panel copies of stage 0 of k_reduced_solve / k_chol_trail (227 KB per CTA)
+constexpr int kTrackMaxRows = 640;          // a track's large-window solver (kba_track_caps.win_rows); limo's windows are far smaller
 constexpr int kSyrkMaxSplit = 16;           // most CTAs k_schur_syrk deals a window's 32-landmark chunks to
 constexpr int kSplitSolveMaxWindows = 16;   // batches of at most this many windows spread a large factorisation (k_chol_*) ...
 constexpr int kSplitSolveMaxCtas = 32;      // ... over at most this many CTAs per window
 constexpr int kFusedMaxKf = 32;             // keyframes the fused-path kernels stage in shared memory
 constexpr int kPackMaxLandmarks = 32768;    // device packing: 15 index bits, 128 KB of sort keys in shared memory
+constexpr int kMaxKf = 128;                 // keyframes per window the kernels stage in shared memory
 static_assert((kFusedMaxRows - 1) / 6 <= kFusedMaxKf, "a window has at least 6 reduced rows per keyframe");
 
 // reduced-system rows of n_kf keyframes: 6 per pose, 4 more with plane blocks, and the right-hand side
@@ -23,6 +25,9 @@ constexpr int reduced_rows(int n_kf, bool planes) { return (planes ? 10 : 6) * n
 constexpr int nr_cap_of(int rows) { return std::max(64, (rows + 63) / 64 * 64); }
 // k_schur_fused instance for the largest reduced rows of the free keyframes of a batch
 constexpr int fused_slots(int free_rows) { return free_rows <= kSixSlotMaxRows ? 6 : 7; }
+// largest reduced system kba_batch_create takes: kMaxKf keyframes with plane blocks (1281 rows, allocated as 1344)
+constexpr int kMaxReducedRows = nr_cap_of(reduced_rows(kMaxKf, true));
+static_assert(nr_cap_of(kPanelMaxRows) == kPanelMaxRows, "the panel bound is a whole number of 64-row blocks");
 
 // what the environment selects, read once per kba_batch_create (a track's solvers keep those of their creation)
 struct Knobs {
@@ -66,6 +71,7 @@ struct Plan {
     int p_split_cap = 1;  // the largest p_split sred has room for
     int solve_tiled = 0;  // k_reduced_solve<true>, else the row-major factorisation
     int solve_split = 0;  // > 0: the row-major factorisation spread over this many CTAs per window (k_chol_*)
+    int solve_banded = 0; // nr_cap_max > kPanelMaxRows: k_sred_reduce forms A, k_chol_trail_band updates, no panel copy anywhere
     int device_pack = 0;  // packing kernels (kba_pack.cu) instead of the host
 };
 
@@ -76,11 +82,15 @@ inline int syrk_split(int nr_cap_max, int n_windows, int sm_count) {
 }
 
 // the factorisation: tiled in one CTA when it fits, else row-major, spread over the GPU when the batch has few windows (a single
-// SM's FP64 rate bounds the one-CTA factorisation of a large system)
+// SM's FP64 rate bounds the one-CTA factorisation of a large system).  Above kPanelMaxRows the one-CTA factorisation (stage 0)
+// has no room for its panel copy: such a batch is always split, over at least one CTA per window, whatever its size.
 inline void plan_solve(Plan& p, int n_windows, int sm_count, const Knobs& k) {
     p.solve_tiled = p.nr_cap_max <= kTiledMaxRows;
-    const int split = n_windows <= kSplitSolveMaxWindows ? std::max(1, std::min(kSplitSolveMaxCtas, sm_count / n_windows)) : 0;
+    p.solve_banded = p.nr_cap_max > kPanelMaxRows;
+    const int spread = std::max(1, std::min(kSplitSolveMaxCtas, sm_count / n_windows));
+    const int split = (n_windows <= kSplitSolveMaxWindows || p.solve_banded) ? spread : 0;
     p.solve_split = p.solve_tiled ? 0 : (k.solve_split >= 0 ? k.solve_split : split);
+    if (p.solve_banded) p.solve_split = std::max(1, p.solve_split);
 }
 
 // The plan of a batch of n windows.  The path is decided on the rows of all keyframes, the Schur kernel instance on the free
