@@ -29,7 +29,7 @@ extern "C" {
 #endif
 
 #define KBA_VERSION_MAJOR 0
-#define KBA_VERSION_MINOR 3
+#define KBA_VERSION_MINOR 4
 
 /* ---- status codes (reference: C++ exceptions / text report, bundle_adjuster_keyframes.cpp:630-632) ---- */
 enum {
@@ -776,6 +776,72 @@ typedef struct kba_pose_write {
     const double* plane4s;      /* [4 * n] or NULL (planes unchanged) */
 } kba_pose_write;
 int kba_track_group_set_keyframe_poses(kba_track_group* g, const kba_pose_write* req);
+
+/* ---- snapshots of the stored window: save, load and clone a track, save every track of a group -------------------------------
+ * A track's store is the only copy of its state (landmarks created on the device, poses and positions written back by solves).
+ * A snapshot is that state as a little-endian byte buffer, to move a track to another handle or device, to resume after the
+ * process ended, to fork a track, or to read the whole map (limo's dumpMap).  Format (version KBA_SNAPSHOT_VERSION):
+ *   - a kba_snapshot_header at offset 0, then four sections, each at an 8-byte aligned offset, each a list of arrays in
+ *     structure-of-arrays form, every array starting 8-byte aligned (4-byte arrays padded with zero bytes to a multiple of 8):
+ *       cameras       cam_intr double [3 * n_cam], cam_pose double [7 * n_cam]
+ *       keyframes     the live keyframes (pushed, not dropped) in ascending slot order: slot int32 [K], count int32 [K] (arena
+ *                     entries), pose7 double [7 * K], plane4 double [4 * K]
+ *       measurements  the live keyframes' arena runs concatenated in that order: lm int32 [M], cam int32 [M], u, v, d float [M]
+ *       landmarks     pos double [3 * lm_cap], weight double [lm_cap], every slot
+ *     K = n_keyframes, M = n_entries = sum(count), lm_cap = caps.max_landmarks; the sections follow each other in this order
+ *     from offset sizeof(kba_snapshot_header) without gaps, so every offset and size follows from n_cam, K, M and lm_cap.
+ *   - Canonical: stores with the same cameras, caps, live keyframes (slots, poses, planes, measurements) and landmark values give
+ *     the same bytes, whatever their arena history (which arena is current, compactions, dropped keyframes' entries still in
+ *     the arena).  Nothing else of the track is saved: not its rankings, generation, solvers, staging or cached options.  A slot
+ *     never written holds 0 (kba_track_create zero-fills positions and weights).
+ * kba_track_save writes the snapshot of t into buf (bytes = its capacity; kba_track_snapshot_size gives the size): a smaller
+ *   buffer is KBA_ERR_CAPACITY and nothing is written.  One upload of the keyframe lists, one launch sequence, one download,
+ *   one synchronisation.  The store does not change: a ranking made before a save can be solved after it.
+ * kba_track_load creates a track on h (any device) whose store gives the same snapshot back, byte for byte.  caps NULL takes the
+ *   saved caps; other caps get kba_track_create's checks and must hold the content: max_keyframes above every live slot,
+ *   max_landmarks >= lm_cap, max_measurements >= n_entries, else KBA_ERR_CAPACITY (larger window caps grow a track).  Slots
+ *   beyond the saved lm_cap hold 0.  The buffer comes from outside the program, so before anything is allocated every
+ *   structural field is checked: magic, format version, reserved_ 0, counts, every offset and size against the counts and
+ *   bytes, slots strictly ascending in [0, caps.max_keyframes), counts >= 0 summing to n_entries, every entry's landmark slot in
+ *   [0, lm_cap) and camera in [0, n_cam); a failure is KBA_ERR_BAD_ARG, and kba_last_error names the field.  Floating-point
+ *   values are taken as they are.  The loaded arena is compact from offset 0, the track starts without a ranking.  One
+ *   upload, one launch sequence, one synchronisation.
+ * kba_track_clone gives the store kba_track_load(h, save(src), caps) gives.  On src's device the copy goes from store to store
+ *   without a host round trip; on another device it is a save and a load.  The copy reads src after src's earlier calls on
+ *   its handle's stream (an event orders h's stream after it).
+ * kba_track_group_save saves every track whose bufs[i] is not NULL (bytes[i] its capacity); a NULL buffer sits the call out.
+ *   Buffer i gets exactly what kba_track_save writes for track i.  Every request is checked first: a failure returns its code,
+ *   kba_last_error names the track, and no buffer is written.  One launch sequence, one download and one synchronisation for
+ *   the whole group.  To load a group, load each track and call kba_track_group_create.
+ * Staging: the first save of a track or group allocates a device image and a pinned host copy of it for the snapshots of its
+ * tracks at their capacities (every keyframe slot live, a full arena), a loaded or cloned track its own at creation.
+ * kba_track_transfer_bytes / kba_track_group_transfer_bytes then report the last save's upload and download (d2h = the
+ * snapshots' bytes), a load's upload. */
+#define KBA_SNAPSHOT_MAGIC 0x504E534Bu   /* the bytes "KSNP" */
+#define KBA_SNAPSHOT_VERSION 1
+typedef struct kba_snapshot_header {
+    uint32_t magic;             /* KBA_SNAPSHOT_MAGIC                                                                          */
+    uint32_t format_version;    /* KBA_SNAPSHOT_VERSION                                                                        */
+    int32_t writer_version;     /* kba_version() of the library that wrote it                                                  */
+    int32_t n_cam;
+    kba_track_caps caps;        /* the track's                                                                                 */
+    int32_t n_keyframes;        /* live keyframes                                                                              */
+    int32_t n_entries;          /* their arena entries                                                                         */
+    int32_t lm_cap;             /* landmark slots saved: caps.max_landmarks                                                    */
+    int32_t reserved_;          /* 0                                                                                           */
+    int64_t cam_offset, cam_bytes;       /* sections: byte offset from the start of the buffer, and size                       */
+    int64_t kf_offset, kf_bytes;
+    int64_t meas_offset, meas_bytes;
+    int64_t lm_offset, lm_bytes;         /* lm_offset + lm_bytes: the snapshot's size                                          */
+} kba_snapshot_header;
+int kba_track_snapshot_size(const kba_track* t, int64_t* bytes);
+int kba_track_save(kba_track* t, void* buf, int64_t bytes);
+int kba_track_load(kba_handle* h, const void* buf, int64_t bytes, const kba_track_caps* caps, kba_track** out);
+int kba_track_clone(kba_track* src, kba_handle* h, const kba_track_caps* caps, kba_track** out);
+/* bytes[n_tracks]: each track's kba_track_snapshot_size */
+int kba_track_group_snapshot_sizes(kba_track_group* g, int64_t* bytes);
+/* bufs[n_tracks] (NULL: the track sits out), bytes[n_tracks] */
+int kba_track_group_save(kba_track_group* g, void* const* bufs, const int64_t* bytes);
 
 /* ---- ranked landmark selection on the stored window, and the solve of that ranking (SURVEY row A17) ------------------------
  * kba_track_select_landmarks leaves the ranking of its quantities to the host; kba_track_rank_landmarks ranks them on the

@@ -11,7 +11,7 @@ import os
 import numpy as np
 
 from .capi_types import (KbaCounters, KbaCreateOut, KbaCreateRequest, KbaDeactivateOut, KbaDeactivateRequest, KbaDepthEntry, KbaDepthOut, KbaDepthRequest, KbaDrawFn, KbaEvalOut, KbaFlowOut, KbaFlowRequest, KbaLandmarkWrite, KbaLidarCloud, KbaLidarOptions, KbaLidarView, KbaOptions, KbaPoseWrite, KbaPushRequest, KbaRankedRequest, KbaRankOut, KbaRankRequest, KbaReclaimOut, KbaReclaimRequest, KbaResult, KbaSelectOut, KbaSelectParams, KbaSelectRequest,
-                         KbaTrackCaps, KbaTrackFrame, KbaTrackRequest, KbaWindow, Result, Window, c_double_p, c_float_p, c_int32_p,
+                         KbaSnapshotHeader, KbaTrackCaps, KbaTrackFrame, KbaTrackRequest, KbaWindow, Result, Window, c_double_p, c_float_p, c_int32_p,
                          c_uint8_p)
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
@@ -35,7 +35,8 @@ SYMBOLS = ["kba_version", "kba_last_error", "kba_default_options", "kba_create",
            "kba_solve_batch_opts", "kba_batch_solve_opts", "kba_track_group_solve_opts", "kba_track_group_solve_ranked_opts",
            "kba_track_group_adjust_pose_opts", "kba_track_group_push_keyframes", "kba_track_group_drop_keyframes",
            "kba_track_group_set_landmarks", "kba_track_group_set_keyframe_poses", "kba_lidar_depth_batch",
-           "kba_lidar_depth_batch_opts"]
+           "kba_lidar_depth_batch_opts", "kba_track_snapshot_size", "kba_track_save", "kba_track_load", "kba_track_clone",
+           "kba_track_group_snapshot_sizes", "kba_track_group_save"]
 
 
 class KbaError(RuntimeError):
@@ -164,6 +165,13 @@ def lib():
         L.kba_track_group_drop_keyframes.argtypes = [vp, ip]
         L.kba_track_group_set_landmarks.argtypes = [vp, C.POINTER(KbaLandmarkWrite)]
         L.kba_track_group_set_keyframe_poses.argtypes = [vp, C.POINTER(KbaPoseWrite)]
+        i64p = C.POINTER(C.c_int64)
+        L.kba_track_snapshot_size.argtypes = [vp, i64p]
+        L.kba_track_save.argtypes = [vp, vp, C.c_int64]
+        L.kba_track_load.argtypes = [vp, vp, C.c_int64, C.POINTER(KbaTrackCaps), C.POINTER(vp)]
+        L.kba_track_clone.argtypes = [vp, vp, C.POINTER(KbaTrackCaps), C.POINTER(vp)]
+        L.kba_track_group_snapshot_sizes.argtypes = [vp, i64p]
+        L.kba_track_group_save.argtypes = [vp, C.POINTER(vp), i64p]
         L.kba_lidar_default_options.argtypes = [C.POINTER(KbaLidarOptions)]
         L.kba_lidar_default_options.restype = None
         fp = C.POINTER(C.c_float)
@@ -381,8 +389,8 @@ class Track:
         fused path's limits (30 keyframes, 18 with plane blocks), beyond 184 the track also owns a large-window solver"""
         self.handle = handle
         self._n_sel = None  # size of the track's last ranking (rank_landmarks, alone or in a group): what solve_ranked returns
-        caps = KbaTrackCaps(max_keyframes, max_landmarks, max_measurements, win_keyframes, win_landmarks, win_observations, win_ground,
-                            win_rows)
+        self.caps = caps = KbaTrackCaps(max_keyframes, max_landmarks, max_measurements, win_keyframes, win_landmarks, win_observations,
+                                        win_ground, win_rows)
         intr = np.ascontiguousarray(cam_intr, dtype=np.float64).reshape(-1, 3)
         pose = np.ascontiguousarray(cam_pose, dtype=np.float64).reshape(-1, 7)
         self._p = C.c_void_p()
@@ -622,6 +630,53 @@ class Track:
         _check(lib().kba_track_transfer_bytes(self._p, C.byref(a), C.byref(b), C.byref(c)))
         return a.value, b.value, c.value
 
+    def snapshot(self):
+        """the store as a snapshot (kba_track_save): a numpy uint8 array, read by capi_types.parse_snapshot and Track.load"""
+        n = C.c_int64()
+        _check(lib().kba_track_snapshot_size(self._p, C.byref(n)))
+        buf = np.empty(n.value, np.uint8)
+        _check(lib().kba_track_save(self._p, buf.ctypes.data, n.value))
+        return buf
+
+    @staticmethod
+    def _caps(saved, kw):
+        """saved caps (a KbaTrackCaps) with the keyword caps kw changed, or None (the saved caps) without keywords"""
+        if not kw:
+            return None
+        c = KbaTrackCaps.from_buffer_copy(saved)
+        for k, v in kw.items():
+            if not hasattr(c, k):
+                raise TypeError("unknown track cap %r" % k)
+            setattr(c, k, int(v))
+        return c
+
+    @classmethod
+    def _adopt(cls, handle, p, caps):
+        t = cls.__new__(cls)
+        t.handle, t._n_sel, t._p, t.caps = handle, None, p, caps
+        return t
+
+    @classmethod
+    def load(cls, handle, data, caps=None):
+        """A track on handle whose store is the snapshot data (kba_track_load).  caps: None (the saved caps) or a dict of keyword
+        caps (max_keyframes, ..., win_rows) that replace the saved ones, e.g. dict(win_keyframes=20) to grow the window."""
+        buf = np.ascontiguousarray(np.frombuffer(data, np.uint8) if not isinstance(data, np.ndarray) else data.view(np.uint8).ravel())
+        saved = KbaSnapshotHeader.from_buffer_copy(buf[:C.sizeof(KbaSnapshotHeader)].tobytes()).caps \
+            if len(buf) >= C.sizeof(KbaSnapshotHeader) else KbaTrackCaps()
+        c = cls._caps(saved, caps or {})
+        p = C.c_void_p()
+        _check(lib().kba_track_load(handle._p, buf.ctypes.data, len(buf), C.byref(c) if c else None, C.byref(p)))
+        return cls._adopt(handle, p, c or KbaTrackCaps.from_buffer_copy(saved))
+
+    def clone(self, handle=None, **caps):
+        """a copy of this track on handle (default: this track's handle) with the keyword caps changed (kba_track_clone); on the
+        same device the store is copied without a host round trip"""
+        h = handle or self.handle
+        c = self._caps(self.caps, caps)
+        p = C.c_void_p()
+        _check(lib().kba_track_clone(self._p, h._p, C.byref(c) if c else None, C.byref(p)))
+        return self._adopt(h, p, c or KbaTrackCaps.from_buffer_copy(self.caps))
+
     def close(self):
         if self._p:
             lib().kba_track_destroy(self._p)
@@ -809,6 +864,18 @@ class TrackGroup:
         """keyframe poses (and planes) of every track in one call (kba_track_group_set_keyframe_poses): each entry None (the track
         sits the call out) or a dict with the arguments of Track.set_keyframe_poses (kf_slots, pose7s, and optionally plane4s)"""
         self._call(lib().kba_track_group_set_keyframe_poses, requests, Track._pose_write, KbaPoseWrite)
+
+    def snapshot(self, which=None):
+        """the snapshots of the tracks in `which` (indices; None: every track) in one call (kba_track_group_save): a list with one
+        numpy uint8 array per track, None for a track that sat out"""
+        n = len(self.tracks)
+        sizes = np.zeros(n, np.int64)
+        _check(lib().kba_track_group_snapshot_sizes(self._p, sizes.ctypes.data_as(C.POINTER(C.c_int64))))
+        take = set(range(n)) if which is None else {int(i) for i in which}
+        out = [np.empty(sizes[i], np.uint8) if i in take else None for i in range(n)]
+        bufs = (C.c_void_p * n)(*[None if b is None else b.ctypes.data for b in out])
+        _check(lib().kba_track_group_save(self._p, bufs, sizes.ctypes.data_as(C.POINTER(C.c_int64))))
+        return out
 
     def transfer_bytes(self):
         """(host->device bytes, device->host bytes) of the last group solve, pose-only call, selection, creation, upkeep, flow

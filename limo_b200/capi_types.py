@@ -114,6 +114,85 @@ class KbaPoseWrite(C.Structure):
     _fields_ = [("n", C.c_int32), ("reserved_", C.c_int32), ("kf_slot", c_int32_p), ("pose7s", c_double_p), ("plane4s", c_double_p)]
 
 
+# ---- snapshots of a track's store (kba_track_save, include/kba_b200.h) ----------------------------------------------------------
+SNAPSHOT_MAGIC = 0x504E534B    # the bytes "KSNP"
+SNAPSHOT_VERSION = 1
+
+
+class KbaSnapshotHeader(C.Structure):
+    _fields_ = [("magic", C.c_uint32), ("format_version", C.c_uint32), ("writer_version", C.c_int32), ("n_cam", C.c_int32),
+                ("caps", KbaTrackCaps), ("n_keyframes", C.c_int32), ("n_entries", C.c_int32), ("lm_cap", C.c_int32),
+                ("reserved_", C.c_int32), ("cam_offset", C.c_int64), ("cam_bytes", C.c_int64), ("kf_offset", C.c_int64),
+                ("kf_bytes", C.c_int64), ("meas_offset", C.c_int64), ("meas_bytes", C.c_int64), ("lm_offset", C.c_int64),
+                ("lm_bytes", C.c_int64)]
+
+
+def _align8(b):
+    return (b + 7) & ~7
+
+
+def _snapshot_layout(n_cam, K, M, L):
+    """byte offset of every array of a snapshot with these counts, and its end (the layout of include/kba_b200.h)"""
+    o = dict(cam_intr=C.sizeof(KbaSnapshotHeader))
+    o["cam_pose"] = o["cam_intr"] + 24 * n_cam
+    o["slot"] = o["cam_pose"] + 56 * n_cam
+    o["count"] = o["slot"] + _align8(4 * K)
+    o["pose"] = o["count"] + _align8(4 * K)
+    o["plane"] = o["pose"] + 56 * K
+    col = _align8(4 * M)
+    for i, name in enumerate(("lm", "cam", "u", "v", "d")):
+        o[name] = o["plane"] + 32 * K + i * col
+    o["pos"] = o["lm"] + 5 * col
+    o["weight"] = o["pos"] + 24 * L
+    o["end"] = o["weight"] + 8 * L
+    return o
+
+
+def parse_snapshot(data):
+    """The contents of a track snapshot (kba_track_save, Track.snapshot) as numpy views of `data`, after the checks kba_track_load
+    makes.  Returns a dict: header (the KbaSnapshotHeader), cam_intr [n_cam, 3], cam_pose [n_cam, 7]; the live keyframes in ascending
+    slot order: slot, count, pose [K, 7], plane [K, 4]; their measurements in that order: lm, cam, u, v, d [M]; the landmark values
+    of every slot: pos [lm_cap, 3], weight [lm_cap].  A malformed snapshot raises ValueError naming the field.  Needs no GPU."""
+    buf = np.frombuffer(data, dtype=np.uint8) if not isinstance(data, np.ndarray) else data.view(np.uint8).ravel()
+    if len(buf) < C.sizeof(KbaSnapshotHeader):
+        raise ValueError("truncated snapshot: shorter than the header")
+    hd = KbaSnapshotHeader.from_buffer_copy(buf[:C.sizeof(KbaSnapshotHeader)].tobytes())
+    checks = [("magic", hd.magic == SNAPSHOT_MAGIC), ("format_version", hd.format_version == SNAPSHOT_VERSION),
+              ("reserved_", hd.reserved_ == 0), ("n_cam", 1 <= hd.n_cam <= len(buf) // 80),
+              ("lm_cap", 1 <= hd.lm_cap == hd.caps.max_landmarks), ("n_keyframes", 0 <= hd.n_keyframes <= hd.caps.max_keyframes),
+              ("n_entries", 0 <= hd.n_entries <= hd.caps.max_measurements)]
+    for name, ok in checks:
+        if not ok:
+            raise ValueError("snapshot header: %s" % name)
+    K, M, L = hd.n_keyframes, hd.n_entries, hd.lm_cap
+    o = _snapshot_layout(hd.n_cam, K, M, L)
+    want = dict(cam_offset=o["cam_intr"], cam_bytes=o["slot"] - o["cam_intr"], kf_offset=o["slot"], kf_bytes=o["lm"] - o["slot"],
+                meas_offset=o["lm"], meas_bytes=o["pos"] - o["lm"], lm_offset=o["pos"], lm_bytes=o["end"] - o["pos"])
+    for name, v in want.items():
+        if getattr(hd, name) != v:
+            raise ValueError("snapshot header: %s %d, the counts give %d" % (name, getattr(hd, name), v))
+    if o["end"] > len(buf):
+        raise ValueError("truncated snapshot: %d bytes, the sections end at %d" % (len(buf), o["end"]))
+
+    def arr(name, dtype, n, *shape):
+        a = buf[o[name]:o[name] + n * np.dtype(dtype).itemsize].view(dtype)
+        return a.reshape(shape) if shape else a
+    out = dict(header=hd, cam_intr=arr("cam_intr", np.float64, 3 * hd.n_cam, -1, 3), cam_pose=arr("cam_pose", np.float64, 7 * hd.n_cam, -1, 7),
+               slot=arr("slot", np.int32, K), count=arr("count", np.int32, K), pose=arr("pose", np.float64, 7 * K, -1, 7),
+               plane=arr("plane", np.float64, 4 * K, -1, 4), lm=arr("lm", np.int32, M), cam=arr("cam", np.int32, M), u=arr("u", np.float32, M),
+               v=arr("v", np.float32, M), d=arr("d", np.float32, M), pos=arr("pos", np.float64, 3 * L, -1, 3), weight=arr("weight", np.float64, L))
+    s = out["slot"]
+    if K and (s.min() < 0 or s.max() >= hd.caps.max_keyframes or np.any(np.diff(s) <= 0)):
+        raise ValueError("keyframe slots: not ascending in [0, caps.max_keyframes)")
+    if np.any(out["count"] < 0) or int(out["count"].astype(np.int64).sum()) != M:
+        raise ValueError("keyframe counts: negative, or their sum is not n_entries = %d" % M)
+    if M and (out["lm"].min() < 0 or out["lm"].max() >= L):
+        raise ValueError("measurement landmark slot out of [0, lm_cap)")
+    if M and (out["cam"].min() < 0 or out["cam"].max() >= hd.n_cam):
+        raise ValueError("measurement camera out of [0, n_cam)")
+    return out
+
+
 class KbaDepthEntry(C.Structure):
     _fields_ = [("ind", C.c_int32), ("wanted", C.c_int32)]
 

@@ -323,7 +323,7 @@ struct SlotStamps {
 // the store calls that stage their requests, one staging each; deactivation and depth costs share the upkeep one, a drop shares
 // the push's
 enum StoreCall { kSelectCall, kCreateCall, kUpkeepCall, kFlowCall, kReclaimCall, kRankCall, kPushCall, kLandmarkWriteCall, kPoseWriteCall,
-                 kStoreCalls };
+                 kSnapshotCall, kStoreCalls };
 
 // what a track and a track group own alike.  A track's set is {the track}: its calls run the host code of a group's, with one
 // window.
@@ -1773,6 +1773,7 @@ int kba_track_create(kba_handle* h, const kba_track_caps* c, int32_t n_cam, cons
     cudaStream_t s = h->stream;
     CU(cudaMemsetAsync(td.sel_index, 0xff, sizeof(int) * (size_t)td.lm_cap, s));
     CU(cudaMemsetAsync(td.m_cnt, 0, sizeof(int) * (size_t)td.kf_cap, s));
+    CU(cudaMemsetAsync(td.lm_pos, 0, sizeof(double) * 3 * (size_t)td.lm_cap, s));  // a slot never written saves as 0
     CU(cudaMemsetAsync(td.lm_weight, 0, sizeof(double) * (size_t)td.lm_cap, s));
     CU(cudaStreamSynchronize(s));
     *out = t;
@@ -3746,6 +3747,416 @@ int kba_track_group_set_keyframe_poses(kba_track_group* g, const kba_pose_write*
     static const std::string who = "kba_track_group_set_keyframe_poses: ";
     if (!g || !req) return fail(KBA_ERR_BAD_ARG, who + "null argument");
     return store_call<PoseWrite>(g->set, true, who, req, nullptr);
+}
+
+
+// ---------------------------------------------------------------------------------------------------------------------
+// snapshots of the stored window (include/kba_b200.h, kba_track_save / kba_track_load / kba_track_clone / kba_track_group_save;
+// kernels in kba_store.cu).  A snapshot is assembled as an image in device memory: the host uploads each image's head (header,
+// cameras, keyframe lists), k_copy_spans copies the heads, poses, planes and landmark values into the images, k_arena_compact the
+// live keyframes' runs.  A load goes the other way from an image: k_store_append writes the runs and the keyframe layout,
+// k_copy_spans the poses, planes and landmark values.  A single save is a one-track call of store_call.
+// ---------------------------------------------------------------------------------------------------------------------
+static int64_t align8(int64_t b) { return (b + 7) & ~(int64_t)7; }
+
+// byte offsets of a snapshot's arrays, from its counts (n_cam, K live keyframes, M entries, L landmark slots); col is the bytes of
+// one measurement column
+struct SnapLayout {
+    int64_t cam_intr = 0, cam_pose = 0, kf_slot = 0, kf_count = 0, kf_pose = 0, kf_plane = 0, meas = 0, col = 0, lm_pos = 0,
+            lm_weight = 0, end = 0;
+    SnapLayout() = default;
+    SnapLayout(int64_t n_cam, int64_t K, int64_t M, int64_t L) {
+        cam_intr = sizeof(kba_snapshot_header); cam_pose = cam_intr + 24 * n_cam;
+        kf_slot = cam_pose + 56 * n_cam; kf_count = kf_slot + align8(4 * K); kf_pose = kf_count + align8(4 * K);
+        kf_plane = kf_pose + 56 * K; meas = kf_plane + 32 * K; col = align8(4 * M);
+        lm_pos = meas + 5 * col; lm_weight = lm_pos + 24 * L; end = lm_weight + 8 * L;
+    }
+    void sections(kba_snapshot_header& hd) const {
+        hd.cam_offset = cam_intr; hd.cam_bytes = kf_slot - cam_intr; hd.kf_offset = kf_slot; hd.kf_bytes = meas - kf_slot;
+        hd.meas_offset = meas; hd.meas_bytes = lm_pos - meas; hd.lm_offset = lm_pos; hd.lm_bytes = end - lm_pos;
+    }
+};
+
+// what a snapshot of t holds: its live keyframe slots (ascending), their counts, and the layout
+struct SnapContent {
+    std::vector<int> slot, cnt;
+    int M = 0, L = 0;
+    SnapLayout lay;
+};
+static SnapContent snap_content(const kba_track* t) {
+    SnapContent c;
+    for (int k = 0; k < t->td.kf_cap; ++k)
+        if (t->kf_live[k]) { c.slot.push_back(k); c.cnt.push_back(t->m_cnt[k]); c.M += t->m_cnt[k]; }
+    c.L = t->td.lm_cap;
+    c.lay = SnapLayout(t->n_cam, (int64_t)c.slot.size(), c.M, c.L);
+    return c;
+}
+
+static kba_snapshot_header snap_header(const kba_track* t, const SnapContent& c) {
+    kba_snapshot_header hd;
+    memset(&hd, 0, sizeof(hd));
+    hd.magic = KBA_SNAPSHOT_MAGIC; hd.format_version = KBA_SNAPSHOT_VERSION; hd.writer_version = KBA_VERSION_MAJOR * 100 + KBA_VERSION_MINOR;
+    hd.n_cam = t->n_cam; hd.caps = t->caps; hd.n_keyframes = (int32_t)c.slot.size(); hd.n_entries = c.M; hd.lm_cap = c.L;
+    c.lay.sections(hd);
+    return hd;
+}
+
+// the staging of a track's snapshots at its capacities: every keyframe slot live, a full arena
+static SnapLayout snap_capacity(const kba_track* t) { return SnapLayout(t->n_cam, t->td.kf_cap, t->td.m_cap, t->td.lm_cap); }
+static size_t snap_spans(int64_t K) { return 8 + 2 * (size_t)K; }  // head, 5 column pads, positions, weights; pose and plane per keyframe
+static size_t save_records(int W, size_t kfs, size_t spans) {
+    return align16(sizeof(CompactTrack) * W) + align16(sizeof(CompactRun) * kfs) + align16(sizeof(CopySpan) * spans) + 16;
+}
+static size_t load_records(int64_t K) { return align16(sizeof(StoreAppend) * (size_t)K) + align16(sizeof(CopySpan) * snap_spans(K)); }
+
+static const unsigned* words(const void* p) { return reinterpret_cast<const unsigned*>(p); }
+
+struct SaveReq {
+    kba_track* t = nullptr;
+    void* buf = nullptr;
+    int64_t bytes = 0;
+    SnapContent c;
+};
+
+// the images of W saves in st.out.d, image w at img[w]: one upload of the records and heads, k_copy_spans, k_arena_compact (no
+// synchronisation).  The upload: CompactTrack [W] | runs | spans | 16 zero bytes (the columns' padding) | the heads.
+static int snap_gather(kba_handle* h, StoreStage& st, int W, const SaveReq* r, std::vector<int64_t>& img, int64_t& up) {
+    CU(cudaSetDevice(h->device));
+    cudaStream_t s = h->stream;
+    size_t n_run = 0, n_span = 0;
+    int64_t heads = 0;
+    img.assign(W, 0);
+    for (int w = 0; w < W; ++w) {
+        for (int n : r[w].c.cnt) n_run += n > 0;
+        n_span += snap_spans((int64_t)r[w].c.slot.size());
+        heads += r[w].c.lay.kf_pose;
+        if (w > 0) img[w] = img[w - 1] + r[w - 1].c.lay.end;  // every size is a multiple of 8
+    }
+    const size_t o_run = align16(sizeof(CompactTrack) * W), o_span = o_run + align16(sizeof(CompactRun) * n_run);
+    const size_t o_zero = o_span + align16(sizeof(CopySpan) * n_span), o_head = o_zero + 16;
+    unsigned char* hb = st.up.h;
+    const unsigned char* ub = st.up.d;
+    unsigned char* ob = st.out.d;
+    memset(hb + o_zero, 0, 16 + (size_t)heads);
+    CompactTrack* ct = reinterpret_cast<CompactTrack*>(hb);
+    CompactRun* runs = reinterpret_cast<CompactRun*>(hb + o_run);
+    CopySpan* spans = reinterpret_cast<CopySpan*>(hb + o_span);
+    size_t nr = 0, ns = 0;
+    int max_run = 0;
+    long long max_words = 0;
+    auto span = [&](const void* src, void* dst, long long n) {
+        spans[ns].src = words(src); spans[ns].dst = reinterpret_cast<unsigned*>(dst); spans[ns].n = n; ++ns;
+        max_words = std::max(max_words, n);
+    };
+    int64_t o_h = (int64_t)o_head;
+    for (int w = 0; w < W; ++w) {
+        const kba_track* t = r[w].t;
+        const SnapContent& c = r[w].c;
+        const SnapLayout& L = c.lay;
+        const int K = (int)c.slot.size();
+        unsigned char* hd = hb + o_h;  // the head: header | cameras | slots | counts (padding zero)
+        const kba_snapshot_header head = snap_header(t, c);
+        memcpy(hd, &head, sizeof(head));
+        memcpy(hd + L.cam_intr, t->cam_intr.data(), 24 * (size_t)t->n_cam);
+        memcpy(hd + L.cam_pose, t->cam_pose.data(), 56 * (size_t)t->n_cam);
+        memcpy(hd + L.kf_slot, c.slot.data(), 4 * (size_t)K);
+        memcpy(hd + L.kf_count, c.cnt.data(), 4 * (size_t)K);
+        unsigned char* im = ob + img[w];
+        span(ub + o_h, im, L.kf_pose / 4);
+        for (int i = 0; i < K; ++i) {
+            span(t->td.kf_pose + 7 * (size_t)c.slot[i], im + L.kf_pose + 56 * (int64_t)i, 14);
+            span(t->td.kf_plane + 4 * (size_t)c.slot[i], im + L.kf_plane + 32 * (int64_t)i, 8);
+        }
+        for (int q = 0; q < 5; ++q)  // an odd column ends in a word of padding
+            span(ub + o_zero, im + L.meas + q * L.col + 4 * (int64_t)c.M, (L.col - 4 * (int64_t)c.M) / 4);
+        span(t->td.lm_pos, im + L.lm_pos, 6 * (long long)c.L);
+        span(t->td.lm_weight, im + L.lm_weight, 2 * (long long)c.L);
+        CompactTrack& x = ct[w];
+        x = CompactTrack{};
+        for (int j = 0; j < 2; ++j) x.src[j] = words(t->arena_i[t->arena_cur][j]);
+        for (int j = 0; j < 3; ++j) x.src[2 + j] = words(t->arena_f[t->arena_cur][j]);
+        for (int q = 0; q < 5; ++q) x.dst[q] = reinterpret_cast<unsigned*>(im + L.meas + q * L.col);
+        for (int i = 0, dst = 0; i < K; dst += c.cnt[i], ++i) {
+            if (c.cnt[i] == 0) continue;
+            runs[nr++] = CompactRun{w, c.slot[i], t->m_off[c.slot[i]], dst, c.cnt[i], 0};
+            max_run = std::max(max_run, c.cnt[i]);
+        }
+        o_h += L.kf_pose;
+    }
+    up = o_h;
+    CU(cudaMemcpyAsync(st.up.d, hb, (size_t)up, cudaMemcpyHostToDevice, s));
+    launch_copy_spans(reinterpret_cast<const CopySpan*>(ub + o_span), (int)ns, max_words, s);
+    launch_store_push(reinterpret_cast<const CompactTrack*>(ub), reinterpret_cast<const CompactRun*>(ub + o_run), (int)nr, max_run,
+                      nullptr, 0, 0, nullptr, 0, s);
+    CU(cudaGetLastError());
+    return KBA_OK;
+}
+
+// W checked saves: the images, one download, one synchronisation, each image into its caller's buffer
+static int save_run(kba_handle* h, StoreStage& st, int W, const SaveReq* r) {
+    std::vector<int64_t> img;
+    int64_t up = 0;
+    int rc = snap_gather(h, st, W, r, img, up);
+    if (rc != KBA_OK) return rc;
+    const int64_t total = img[W - 1] + r[W - 1].c.lay.end;
+    CU(cudaMemcpyAsync(st.out.h, st.out.d, (size_t)total, cudaMemcpyDeviceToHost, h->stream));
+    CU(wait_stream(h));
+    for (int w = 0; w < W; ++w) memcpy(r[w].buf, st.out.h + img[w], (size_t)r[w].c.lay.end);
+    st.counts.h2d = up;
+    st.counts.d2h = total;
+    return KBA_OK;
+}
+
+// the staging of the snapshot call for tracks ts[0..n) at their capacities; a single track's also holds a load's records and image
+static void snap_stage_bytes(int n, kba_track* const* ts, size_t& up, size_t& down) {
+    size_t kfs = 0, spans = 0, heads = 0, images = 0;
+    for (int i = 0; i < n; ++i) {
+        const SnapLayout c = snap_capacity(ts[i]);
+        kfs += (size_t)ts[i]->td.kf_cap; spans += snap_spans(ts[i]->td.kf_cap); heads += (size_t)c.kf_pose; images += (size_t)c.end;
+    }
+    up = save_records(n, kfs, spans) + heads;
+    if (n == 1) up = std::max(up, load_records(ts[0]->td.kf_cap) + images);
+    down = images;
+}
+
+static int snap_stage(TrackSet& s, const std::string& who, StoreStage*& st) {
+    std::unique_ptr<StoreStage>& p = s.stage[kSnapshotCall];
+    if (!p) {
+        size_t up = 0, down = 0;
+        snap_stage_bytes((int)s.tracks.size(), s.tracks.data(), up, down);
+        std::unique_ptr<StoreStage> fresh(new StoreStage());
+        if (fresh->alloc(up, down)) return fail(KBA_ERR_CUDA, who + "out of memory for the snapshot staging");
+        p = std::move(fresh);
+    }
+    st = p.get();
+    return KBA_OK;
+}
+
+struct SnapshotWrite {
+    void* buf;
+    int64_t bytes;
+};
+struct Save : WriteCall {
+    using Request = SnapshotWrite;
+    using Req = SaveReq;
+    static constexpr StoreCall slot = kSnapshotCall;
+    static constexpr const char* staging = "snapshot";
+    static bool sits_out(const Request& q) { return q.buf == nullptr; }
+    static Req make(kba_track* t, const Request& q, Out*) {
+        SaveReq r;
+        r.t = t; r.buf = q.buf; r.bytes = q.bytes; r.c = snap_content(t);
+        return r;
+    }
+    static int check(Req& r, std::string& why) {
+        if (!r.buf) { why = "null buffer"; return KBA_ERR_BAD_ARG; }
+        if (r.bytes < r.c.lay.end) {
+            why = "a buffer of " + std::to_string(r.bytes) + " bytes, the snapshot has " + std::to_string(r.c.lay.end);
+            return KBA_ERR_CAPACITY;
+        }
+        return KBA_OK;
+    }
+    static void capacity(int n, kba_track* const* ts, size_t& up, size_t& down) { snap_stage_bytes(n, ts, up, down); }
+    static int run(kba_handle* h, StoreStage& st, int W, Req* r, int&, std::string&) { return save_run(h, st, W, r); }
+};
+
+// every structural field of a snapshot from outside the program, before anything is allocated: hd, the slots, the counts
+static int snap_check(const unsigned char* b, int64_t bytes, kba_snapshot_header& hd, std::vector<int>& slot, std::vector<int>& cnt,
+                      std::string& why) {
+    why = "";
+    if (bytes < (int64_t)sizeof(hd)) { why = "truncated buffer: shorter than the header"; return KBA_ERR_BAD_ARG; }
+    memcpy(&hd, b, sizeof(hd));
+    if (hd.magic != KBA_SNAPSHOT_MAGIC) why = "magic";
+    else if (hd.format_version != KBA_SNAPSHOT_VERSION) why = "format_version " + std::to_string(hd.format_version) + " (this library reads 1)";
+    else if (hd.reserved_ != 0) why = "reserved_";
+    else if (hd.n_cam < 1 || (int64_t)hd.n_cam > bytes / 80) why = "n_cam";
+    else if (hd.lm_cap < 1 || hd.lm_cap != hd.caps.max_landmarks) why = "lm_cap (caps.max_landmarks)";
+    else if (hd.n_keyframes < 0 || hd.n_keyframes > hd.caps.max_keyframes) why = "n_keyframes";
+    else if (hd.n_entries < 0 || hd.n_entries > hd.caps.max_measurements) why = "n_entries";
+    if (!why.empty()) { why = "snapshot header: " + why; return KBA_ERR_BAD_ARG; }
+    const SnapLayout L(hd.n_cam, hd.n_keyframes, hd.n_entries, hd.lm_cap);
+    kba_snapshot_header want = hd;
+    L.sections(want);
+    const char* names[] = {"cam_offset", "cam_bytes", "kf_offset", "kf_bytes", "meas_offset", "meas_bytes", "lm_offset", "lm_bytes"};
+    const int64_t got[] = {hd.cam_offset, hd.cam_bytes, hd.kf_offset, hd.kf_bytes, hd.meas_offset, hd.meas_bytes, hd.lm_offset, hd.lm_bytes};
+    const int64_t exp[] = {want.cam_offset, want.cam_bytes, want.kf_offset, want.kf_bytes, want.meas_offset, want.meas_bytes,
+                           want.lm_offset, want.lm_bytes};
+    for (int i = 0; i < 8; ++i)
+        if (got[i] != exp[i]) {
+            why = std::string("snapshot header: ") + names[i] + " " + std::to_string(got[i]) + ", the counts give " + std::to_string(exp[i]);
+            return KBA_ERR_BAD_ARG;
+        }
+    if (L.end > bytes) {
+        why = "truncated buffer: " + std::to_string(bytes) + " bytes, the sections end at " + std::to_string(L.end);
+        return KBA_ERR_BAD_ARG;
+    }
+    const int K = hd.n_keyframes, M = hd.n_entries;
+    slot.resize(K); cnt.resize(K);
+    memcpy(slot.data(), b + L.kf_slot, 4 * (size_t)K);
+    memcpy(cnt.data(), b + L.kf_count, 4 * (size_t)K);
+    int64_t sum = 0;
+    for (int i = 0; i < K; ++i) {
+        if (slot[i] < 0 || slot[i] >= hd.caps.max_keyframes || (i > 0 && slot[i] <= slot[i - 1])) {
+            why = "keyframe slot " + std::to_string(i) + ": not ascending in [0, caps.max_keyframes)"; return KBA_ERR_BAD_ARG;
+        }
+        if (cnt[i] < 0) { why = "keyframe count " + std::to_string(i) + " negative"; return KBA_ERR_BAD_ARG; }
+        sum += cnt[i];
+    }
+    if (sum != M) { why = "keyframe counts sum to " + std::to_string(sum) + ", n_entries is " + std::to_string(M); return KBA_ERR_BAD_ARG; }
+    std::vector<int32_t> col(M);
+    memcpy(col.data(), b + L.meas, 4 * (size_t)M);
+    for (int i = 0; i < M; ++i)
+        if (col[i] < 0 || col[i] >= hd.lm_cap) { why = "measurement " + std::to_string(i) + ": landmark slot out of [0, lm_cap)"; return KBA_ERR_BAD_ARG; }
+    memcpy(col.data(), b + L.meas + L.col, 4 * (size_t)M);
+    for (int i = 0; i < M; ++i)
+        if (col[i] < 0 || col[i] >= hd.n_cam) { why = "measurement " + std::to_string(i) + ": camera out of [0, n_cam)"; return KBA_ERR_BAD_ARG; }
+    return KBA_OK;
+}
+
+// caps given at a load or clone must hold the snapshot's content
+static int snap_caps_check(const kba_track_caps* caps, const std::vector<int>& slot, int M, int L, std::string& why) {
+    if (!caps) return KBA_OK;
+    if (!slot.empty() && caps->max_keyframes <= slot.back()) why = "caps.max_keyframes does not hold keyframe slot " + std::to_string(slot.back());
+    else if (caps->max_landmarks < L) why = "caps.max_landmarks below the snapshot's " + std::to_string(L) + " landmark slots";
+    else if (caps->max_measurements < M) why = "caps.max_measurements below the snapshot's " + std::to_string(M) + " arena entries";
+    return why.empty() ? KBA_OK : KBA_ERR_CAPACITY;
+}
+
+// a new track on h with caps and cameras, its store written from a snapshot image: host_img (uploaded with the records) or, when
+// null, dev_img in device memory of h's device, which h's stream may read.  slot, cnt: the image's live keyframes; L its slots.
+static int snap_create(kba_handle* h, const kba_track_caps& caps, int n_cam, const double* intr, const double* pose, const std::vector<int>& slot,
+                       const std::vector<int>& cnt, int L, const unsigned char* host_img, const unsigned char* dev_img, const std::string& who,
+                       kba_track** out) {
+    const int K = (int)slot.size();
+    int M = 0;
+    for (int n : cnt) M += n;
+    const SnapLayout lay(n_cam, K, M, L);
+    kba_track* t = nullptr;
+    int rc = kba_track_create(h, &caps, n_cam, intr, pose, &t);
+    if (rc != KBA_OK) return rc;
+    std::unique_ptr<kba_track, void (*)(kba_track*)> guard(t, kba_track_destroy);
+    StoreStage* st = nullptr;
+    rc = snap_stage(t->set, who, st);
+    if (rc != KBA_OK) return rc;
+    cudaStream_t s = h->stream;
+    const size_t o_span = align16(sizeof(StoreAppend) * (size_t)K), o_img = load_records(K);
+    unsigned char* hb = st->up.h;
+    const unsigned char* ub = st->up.d;
+    if (host_img) { memcpy(hb + o_img, host_img, (size_t)lay.end); dev_img = ub + o_img; }
+    StoreAppend* app = reinterpret_cast<StoreAppend*>(hb);
+    CopySpan* spans = reinterpret_cast<CopySpan*>(hb + o_span);
+    TrackDev& td = t->td;
+    int ns = 0, max_rows = 0;
+    long long max_words = 0;
+    auto span = [&](const void* src, void* dst, long long n) {
+        spans[ns].src = words(src); spans[ns].dst = reinterpret_cast<unsigned*>(dst); spans[ns].n = n; ++ns;
+        max_words = std::max(max_words, n);
+    };
+    for (int i = 0, off = 0; i < K; off += cnt[i], ++i) {
+        StoreAppend a;  // the record's pose and plane are 0: the spans below write the snapshot's after it
+        a.col[0] = (unsigned*)td.m_lm; a.col[1] = (unsigned*)td.m_cam; a.col[2] = (unsigned*)td.m_u; a.col[3] = (unsigned*)td.m_v;
+        a.col[4] = (unsigned*)td.m_d;
+        a.m_off = td.m_off; a.m_cnt = td.m_cnt; a.kf_pose = td.kf_pose; a.kf_plane = td.kf_plane;
+        a.slot = slot[i]; a.off = off; a.cnt = cnt[i]; a.seg = 0; a.n = cnt[i]; a.src = off; a.cam_zero = 0;
+        app[i] = a;
+        max_rows = std::max(max_rows, cnt[i]);
+        span(dev_img + lay.kf_pose + 56 * (int64_t)i, td.kf_pose + 7 * (size_t)slot[i], 14);
+        span(dev_img + lay.kf_plane + 32 * (int64_t)i, td.kf_plane + 4 * (size_t)slot[i], 8);
+        t->m_off[slot[i]] = off; t->m_cnt[slot[i]] = cnt[i]; t->kf_live[slot[i]] = 1;
+    }
+    span(dev_img + lay.lm_pos, td.lm_pos, 6 * (long long)L);
+    span(dev_img + lay.lm_weight, td.lm_weight, 2 * (long long)L);
+    const size_t up = host_img ? o_img + (size_t)lay.end : o_img;
+    CU(cudaMemcpyAsync(st->up.d, hb, up, cudaMemcpyHostToDevice, s));
+    launch_store_push(nullptr, nullptr, 0, 0, reinterpret_cast<const StoreAppend*>(ub), K, max_rows, words(dev_img + lay.meas),
+                      (int)(lay.col / 4), s);
+    launch_copy_spans(reinterpret_cast<const CopySpan*>(ub + o_span), ns, max_words, s);
+    CU(cudaGetLastError());
+    CU(wait_stream(h));
+    t->arena_used = M;
+    st->counts.h2d = (int64_t)up; st->counts.d2h = 0;
+    t->set.last = &st->counts;
+    *out = guard.release();
+    return KBA_OK;
+}
+
+int kba_track_snapshot_size(const kba_track* t, int64_t* bytes) {
+    if (!t || !bytes) return fail(KBA_ERR_BAD_ARG, "kba_track_snapshot_size: null argument");
+    *bytes = snap_content(t).lay.end;
+    return KBA_OK;
+}
+
+int kba_track_group_snapshot_sizes(kba_track_group* g, int64_t* bytes) {
+    if (!g || !bytes) return fail(KBA_ERR_BAD_ARG, "kba_track_group_snapshot_sizes: null argument");
+    for (size_t i = 0; i < g->set.tracks.size(); ++i) bytes[i] = snap_content(g->set.tracks[i]).lay.end;
+    return KBA_OK;
+}
+
+int kba_track_save(kba_track* t, void* buf, int64_t bytes) {
+    static const std::string who = "kba_track_save: ";
+    if (!t) return fail(KBA_ERR_BAD_ARG, who + "null argument");
+    const SnapshotWrite q = {buf, bytes};
+    return store_call<Save>(t->set, false, who, &q, nullptr);
+}
+
+int kba_track_group_save(kba_track_group* g, void* const* bufs, const int64_t* bytes) {
+    static const std::string who = "kba_track_group_save: ";
+    if (!g || !bufs || !bytes) return fail(KBA_ERR_BAD_ARG, who + "null argument");
+    std::vector<SnapshotWrite> q(g->set.tracks.size());
+    for (size_t i = 0; i < q.size(); ++i) q[i] = SnapshotWrite{bufs[i], bytes[i]};
+    return store_call<Save>(g->set, true, who, q.data(), nullptr);
+}
+
+int kba_track_load(kba_handle* h, const void* buf, int64_t bytes, const kba_track_caps* caps, kba_track** out) {
+    static const std::string who = "kba_track_load: ";
+    if (!h || !buf || !out) return fail(KBA_ERR_BAD_ARG, who + "null argument");
+    const unsigned char* b = static_cast<const unsigned char*>(buf);
+    kba_snapshot_header hd;
+    std::vector<int> slot, cnt;
+    std::string why;
+    int rc = snap_check(b, bytes, hd, slot, cnt, why);
+    if (rc == KBA_OK) rc = snap_caps_check(caps, slot, hd.n_entries, hd.lm_cap, why);
+    if (rc != KBA_OK) return fail(rc, who + why);
+    const SnapLayout L(hd.n_cam, hd.n_keyframes, hd.n_entries, hd.lm_cap);
+    std::vector<double> intr(3 * (size_t)hd.n_cam), pose(7 * (size_t)hd.n_cam);
+    memcpy(intr.data(), b + L.cam_intr, 8 * intr.size());
+    memcpy(pose.data(), b + L.cam_pose, 8 * pose.size());
+    return snap_create(h, caps ? *caps : hd.caps, hd.n_cam, intr.data(), pose.data(), slot, cnt, hd.lm_cap, b, nullptr, who, out);
+}
+
+int kba_track_clone(kba_track* src, kba_handle* h, const kba_track_caps* caps, kba_track** out) {
+    static const std::string who = "kba_track_clone: ";
+    if (!src || !h || !out) return fail(KBA_ERR_BAD_ARG, who + "null argument");
+    SaveReq r;
+    r.t = src; r.c = snap_content(src);
+    std::string why;
+    const int rc = snap_caps_check(caps, r.c.slot, r.c.M, r.c.L, why);
+    if (rc != KBA_OK) return fail(rc, who + why);
+    kba_handle* hs = src->set.h;
+    if (hs->device != h->device) {  // across devices: a save and a load
+        std::vector<unsigned char> buf((size_t)r.c.lay.end);
+        const int rs = kba_track_save(src, buf.data(), (int64_t)buf.size());
+        if (rs != KBA_OK) return rs;
+        return kba_track_load(h, buf.data(), (int64_t)buf.size(), caps, out);
+    }
+    StoreStage* st = nullptr;
+    int rs = snap_stage(src->set, who, st);
+    if (rs != KBA_OK) return rs;
+    std::vector<int64_t> img;
+    int64_t up = 0;
+    rs = snap_gather(hs, *st, 1, &r, img, up);
+    if (rs != KBA_OK) return rs;
+    st->counts.h2d = up; st->counts.d2h = 0;
+    src->set.last = &st->counts;
+    if (hs->stream != h->stream) {  // h's stream reads the image after src's stream wrote it
+        cudaEvent_t ev = nullptr;
+        CU(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
+        cudaError_t e = cudaEventRecord(ev, hs->stream);
+        if (e == cudaSuccess) e = cudaStreamWaitEvent(h->stream, ev, 0);
+        cudaEventDestroy(ev);
+        if (e != cudaSuccess) return fail(KBA_ERR_CUDA, who + cudaGetErrorString(e));
+    }
+    return snap_create(h, caps ? *caps : src->caps, src->n_cam, src->cam_intr.data(), src->cam_pose.data(), r.c.slot, r.c.cnt, r.c.L,
+                       nullptr, st->out.d, who, out);
 }
 
 }  // extern "C"

@@ -122,7 +122,8 @@ struct StoreAppend {
     double plane[4] = {0, 0, 0, 0};
     int slot = 0, off = 0, cnt = 0, seg = 0, n = 0, src = 0, cam_zero = 0, pad = 0;
 };
-// one track's compaction: its live keyframes' runs copied from one arena into the other
+// one track's compaction: its live keyframes' runs copied from one arena into the other.  m_off null: the runs are copied out
+// of the store (into a snapshot) and no layout is written.
 struct CompactTrack {
     const unsigned* src[5] = {nullptr, nullptr, nullptr, nullptr, nullptr};
     unsigned* dst[5] = {nullptr, nullptr, nullptr, nullptr, nullptr};
@@ -137,6 +138,14 @@ struct CompactRun {
 // the compaction runs (if any), then the appends, on stream s: cols = the staged columns, 5 x stride entries
 void launch_store_push(const CompactTrack* ct, const CompactRun* runs, int n_runs, int max_run, const StoreAppend* app, int n_app,
                        int max_rows, const unsigned* cols, int stride, cudaStream_t s);
+// n words from src to dst: the parts of a snapshot that are not arena runs (header and keyframe lists, poses, planes, landmark
+// values), between a store and a snapshot image in device memory, for many tracks in one launch (k_copy_spans, kba_store.cu)
+struct CopySpan {
+    const unsigned* src = nullptr;
+    unsigned* dst = nullptr;
+    long long n = 0;
+};
+void launch_copy_spans(const CopySpan* spans, int n_spans, long long max_words, cudaStream_t s);
 
 // results of every window w back into track store tds[w]
 void launch_track_writeback(const BatchDev& bd, const TrackDev* tds, const TrackSel* sels, const TrackGrid& g, cudaStream_t s);

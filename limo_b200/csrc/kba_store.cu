@@ -1,5 +1,7 @@
 // kba_store.cu -- store writes of the device-resident window (include/kba_b200.h, kba_track_group_push_keyframes): the arena
-// compaction and the append of pushed keyframes, for every track of a call in one launch each.
+// compaction and the append of pushed keyframes, for every track of a call in one launch each; and the copies of a snapshot
+// (kba_track_save / kba_track_load / kba_track_clone), which move the live keyframes' runs with the same two kernels and
+// everything else as spans of words (k_copy_spans).
 //
 // The host decides every offset from its mirror of the arena layout (kba_api.cu, push_run): a compaction copies each live
 // keyframe's run, in slot order, from the current arena into the other one; an append copies a keyframe's staged rows into the
@@ -39,9 +41,16 @@ __global__ void __launch_bounds__(256) k_arena_compact(const CompactTrack* ct, c
     const CompactRun r = runs[blockIdx.x];
     const CompactTrack& t = ct[r.track];
     const int q = blockIdx.y, i0 = blockIdx.z * kSlice;
-    if (q == 0 && i0 == 0 && threadIdx.x == 0) { t.m_off[r.slot] = r.dst; t.m_cnt[r.slot] = r.n; }
+    if (t.m_off && q == 0 && i0 == 0 && threadIdx.x == 0) { t.m_off[r.slot] = r.dst; t.m_cnt[r.slot] = r.n; }
     if (i0 >= r.n) return;
     copy_words(t.dst[q] + r.dst + i0, t.src[q] + r.src + i0, min(kSlice, r.n - i0));
+}
+
+// span blockIdx.x, its slices blockIdx.y, blockIdx.y + gridDim.y, ..
+__global__ void __launch_bounds__(256) k_copy_spans(const CopySpan* spans) {
+    const CopySpan sp = spans[blockIdx.x];
+    for (long long i0 = (long long)blockIdx.y * kSlice; i0 < sp.n; i0 += (long long)gridDim.y * kSlice)
+        copy_words(sp.dst + i0, sp.src + i0, (int)min((long long)kSlice, sp.n - i0));
 }
 
 // segment blockIdx.x, column blockIdx.y, slice blockIdx.z of it; block (x, 0, 0) also writes the keyframe's layout, pose and plane
@@ -73,6 +82,13 @@ void launch_store_push(const CompactTrack* ct, const CompactRun* runs, int n_run
         k_store_append<<<dim3(n_app, 5, (std::max(max_rows, 1) + kSlice - 1) / kSlice), 256, 0, s>>>(app, cols, stride);
         LCHK("k_store_append");
     }
+}
+
+void launch_copy_spans(const CopySpan* spans, int n_spans, long long max_words, cudaStream_t s) {
+    if (n_spans <= 0 || max_words <= 0) return;
+    const long long slices = std::min<long long>((max_words + kSlice - 1) / kSlice, 65535);
+    k_copy_spans<<<dim3(n_spans, (unsigned)slices), 256, 0, s>>>(spans);
+    LCHK("k_copy_spans");
 }
 
 }  // namespace kba
