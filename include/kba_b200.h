@@ -29,7 +29,7 @@ extern "C" {
 #endif
 
 #define KBA_VERSION_MAJOR 0
-#define KBA_VERSION_MINOR 4
+#define KBA_VERSION_MINOR 5
 
 /* ---- status codes (reference: C++ exceptions / text report, bundle_adjuster_keyframes.cpp:630-632) ---- */
 enum {
@@ -461,6 +461,67 @@ int kba_track_group_solve_opts(kba_track_group* g, const kba_track_request* req,
 /* upload / download of the last group solve, pose-only call, selection, creation, upkeep, flow or reclaim call or store write,
  * counted as kba_track_transfer_bytes counts them */
 int kba_track_group_transfer_bytes(kba_track_group* g, int64_t* h2d_last_solve, int64_t* d2h_last_solve);
+
+/* ---- evaluation of the stored window: residuals, costs and trimming decisions at the store's state --------------------------
+ * How well the stored window fits its measurements, without solving it: for threshold tuning, outlier labelling, checking a
+ * track after kba_track_load or monitoring a long drive.  A request is a kba_track_request exactly as for kba_track_solve (host
+ * ground-plane lists or device-attached candidates, scale_weight < 0 and plane_reg_weight < 0 resolved by the same rules), and the
+ * window evaluated is the one kba_track_solve would build for it, array for array, at the store's current poses, planes and
+ * landmark positions.  Every value comes from the solver's own device code, so the total cost equals the initial_cost of
+ * solves[0] of kba_track_solve on the same request to the last bits of its summation order.
+ * The observation order is the window's own: landmarks in lm_slot order, then keyframes in kf_slot order, then cameras ascending.
+ *   - n_obs: the window's observation count, always written;
+ *   - obs_lm, obs_kf, obs_cam [n_obs]: index into lm_slot, index into kf_slot, the store's camera;
+ *   - residual [3 n_obs]: the rows (u, v, depth) of the observation's residual before any loss or weight: projection minus
+ *     measurement in pixels, z_cam - d in metres (0 without a depth, d <= 0);
+ *   - rho [2 n_obs]: the scaled Cauchy loss w b log(1 + s / b) of the reprojection block (s = u^2 + v^2, b = reprojection_thres^2)
+ *     and of the depth block (s = depth^2, b = depth_thres^2; 0 without a depth), w the landmark's weight; the cost is half
+ *     their sum.  An observation with |z_cam| < 0.01 gets NaN rows and losses and sets `failed`;
+ *   - trim_repr, trim_depth [n_lm]: the trimming values of solveTrimmed at this state: per landmark the largest raw block norm
+ *     (|(u, v)|, |depth|) over its observations, -1 without one;
+ *   - rejected_repr, rejected_depth [n_lm]: 1 where TrimmerQuantile at opt's reprojection / depth quantile over those values
+ *     rejects the landmark (min_residual_groups applies; ties broken by landmark index), the selection code of the solver;
+ *   - n_gp, gp_lm, gp_kf, gp_weight, gp_residual [n_gp]: the attached ground-plane residuals (the request's host lists, or what the
+ *     device attachment kept, as kba_track_solve attaches them) with their height residual n . (R p + t) + dist; the caller
+ *     allocates win_ground entries;
+ *   - cost[6]: reprojection, depth, ground plane (HuberLoss(gp_huber) scaled by the weights), scale regulariser, plane chain and
+ *     their total, each 1/2 sum rho as ceres counts it;
+ *   - failed: 1 if some observation has |z_cam| < 0.01.
+ * Any output array may be NULL.  Per-observation arrays hold obs_capacity entries: if the window has more observations, the call
+ * returns KBA_ERR_CAPACITY after writing n_obs (and nothing else), and the caller retries with larger arrays.
+ * Errors, before anything is uploaded: those of kba_track_solve, and opt->precision != 0 (FP64 only): KBA_ERR_BAD_ARG.
+ * The store is never modified: a later solve gives the results it would give without the evaluation, bit for bit, and a ranking
+ * stays valid.  One upload (the lists, and a record per window), one launch sequence (the gather of kba_track_solve and two
+ * kernels), one download and one synchronisation; the first call allocates the track's (group's) output staging for its
+ * capacities.  kba_track_transfer_bytes (kba_track_group_transfer_bytes) then report this call's upload and download.
+ * The group forms evaluate one request per track in one launch sequence: out[i] is bit for bit what kba_track_evaluate gives
+ * track i for req[i]; a request with n_kf == 0 sits the call out (out[i] is not written); every request is checked first and a
+ * failing one returns its code with kba_last_error naming its track; the _opts form takes one kba_options per track. */
+typedef struct kba_evaluate_out {  /* caller-owned arrays, any of them may be NULL */
+    int32_t obs_capacity;       /* entries of obs_lm, obs_kf, obs_cam (residual: 3 per entry, rho: 2 per entry)             */
+    int32_t n_obs;              /* written by the library                                                                   */
+    int32_t n_gp;
+    int32_t failed;
+    double cost[6];             /* reprojection, depth, ground plane, scale regulariser, plane chain, total                 */
+    int32_t* obs_lm;            /* [n_obs] */
+    int32_t* obs_kf;
+    int32_t* obs_cam;
+    double* residual;           /* [3 n_obs] */
+    double* rho;                /* [2 n_obs] */
+    double* trim_repr;          /* [n_lm] */
+    double* trim_depth;
+    uint8_t* rejected_repr;     /* [n_lm] */
+    uint8_t* rejected_depth;
+    int32_t* gp_lm;             /* [win_ground] */
+    int32_t* gp_kf;
+    double* gp_weight;
+    double* gp_residual;
+} kba_evaluate_out;
+int kba_track_evaluate(kba_track* t, const kba_track_request* req, const kba_options* opt, kba_evaluate_out* out);
+/* req[n_tracks], out[n_tracks] */
+int kba_track_group_evaluate(kba_track_group* g, const kba_track_request* req, const kba_options* opt, kba_evaluate_out* out);
+/* opts[n_tracks]: track i is evaluated with opts[i] (its thresholds and quantiles); a track that sits out does not read its entry */
+int kba_track_group_evaluate_opts(kba_track_group* g, const kba_track_request* req, const kba_options* opts, kba_evaluate_out* out);
 
 /* ---- landmark selection for every track of a group in one launch sequence -------------------------------------------------
  * kba_track_select_landmarks for one request per track, each on its own track's store, as one window each of one launch sequence.

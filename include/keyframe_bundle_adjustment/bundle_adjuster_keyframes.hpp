@@ -11,6 +11,7 @@
 #include <memory>
 #include <set>
 #include <string>
+#include <tuple>
 #include <vector>
 
 #include "internal/triangulator.hpp"
@@ -20,6 +21,7 @@
 struct kba_handle;
 struct kba_track;
 struct kba_window;
+struct kba_evaluate_out;
 
 namespace keyframe_bundle_adjustment {
 
@@ -94,6 +96,32 @@ public:
     long long pushUploadBytes() const { return push_h2d_; }
     void updateLabels(const Tracklets& t, double shrubbery_weight = 1.);
 
+    // What evaluateResiduals() finds (not in the reference, whose evaluateResiduals() only writes into its ceres::Problem).
+    struct Evaluation {
+        struct Residual {                  // one observation: rows before any loss or weight, and the scaled Cauchy losses
+            double u{0.}, v{0.}, depth{0.};  // projection - measurement (px), z_cam - d (m; 0 without a depth); NaN if it failed
+            double rho_reprojection{0.}, rho_depth{0.};
+        };
+        struct Trim {                      // one landmark: solveTrimmed's trimming values and TrimmerQuantile's decisions
+            double reprojection{-1.}, depth{-1.};  // largest raw block norm over its observations, -1 without one
+            bool rejected_reprojection{false}, rejected_depth{false};
+        };
+        using ObservationKey = std::tuple<LandmarkId, KeyframeId, CameraId>;  // (landmark id, keyframe timestamp, camera id)
+        std::map<ObservationKey, Residual> residuals;
+        std::map<LandmarkId, Trim> landmarks;
+        std::map<LandmarkId, double> ground_plane;  // height residual of every attached ground-plane landmark
+        // reprojection, depth, ground plane, scale regulariser, plane chain, total: 1/2 sum rho, as ceres counts the cost
+        double cost_reprojection{0.}, cost_depth{0.}, cost_ground_plane{0.}, cost_scale{0.}, cost_plane_chain{0.}, cost_total{0.};
+        bool failed{false};                // some observation has |z_cam| < 0.01
+    };
+    // The reference's evaluateResiduals() (bundle_adjuster_keyframes.hpp:171-175): the last solve()'s window (the active keyframes,
+    // selected_landmark_ids_) evaluated at the current state with outlier_rejection_options_, on the device-resident store
+    // (kba_track_evaluate), into last_evaluation_.  It changes no selection, outlier set, pose or landmark.  Throws
+    // std::runtime_error naming the reason when the persistent window is off or failed, before the first solve(), or when the
+    // window does not fit the store; there is no host fallback.
+    void evaluateResiduals();
+    Evaluation last_evaluation_;
+
     std::map<KeyframeId, Keyframe::Ptr> keyframes_;
     std::map<LandmarkId, Landmark::Ptr> landmarks_;
     std::set<KeyframeId> active_keyframe_ids_;
@@ -117,6 +145,8 @@ private:
     bool trackSync(const std::vector<Keyframe*>& kfs);
     bool selectOnDevice(const std::vector<Keyframe*>& kfs);
     bool solveTracked(const std::vector<Keyframe*>& kfs, const std::vector<LandmarkId>& lm_ids, std::string& report, bool synced);
+    struct TrackRequest;  // a track solve's or evaluation's lists (trackRequest)
+    bool trackRequest(const std::vector<Keyframe*>& kfs, const std::vector<LandmarkId>& lm_ids, TrackRequest& q) const;
     bool adjustPoseTracked(Keyframe& kf, const std::vector<LandmarkId>& lm_ids, std::string& report);
     bool flushLandmarks();  // new and dirty landmark state into the store, before any use of the track
     void dropInactiveKeyframes(size_t max_free_kf_slots);
@@ -135,5 +165,12 @@ private:
     std::set<LandmarkId> dirty_positions_;  // positions the rebuild path wrote on the host only
     long long last_solve_h2d_{0}, push_h2d_{0}, last_select_h2d_{0};
 };
+
+// the outputs of kba_track_evaluate for the window of keyframes kfs (ascending id) and landmarks lm_ids (ascending id), keyed as
+// BundleAdjusterKeyframes::Evaluation keys them; track_cams are the store's cameras (focal length, principal point,
+// pose_camera_vehicle) in index order.  The window's observations come landmark by landmark, keyframe by keyframe and, inside a
+// keyframe, in Keyframe::measurements_ order; an output that does not follow that order throws std::runtime_error.
+BundleAdjusterKeyframes::Evaluation keyEvaluation(const std::vector<const Keyframe*>& kfs, const std::vector<LandmarkId>& lm_ids,
+                                                  const std::vector<std::array<double, 10>>& track_cams, const kba_evaluate_out& out);
 
 }  // namespace keyframe_bundle_adjustment

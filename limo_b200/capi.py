@@ -10,7 +10,7 @@ import os
 
 import numpy as np
 
-from .capi_types import (KbaCounters, KbaCreateOut, KbaCreateRequest, KbaDeactivateOut, KbaDeactivateRequest, KbaDepthEntry, KbaDepthOut, KbaDepthRequest, KbaDrawFn, KbaEvalOut, KbaFlowOut, KbaFlowRequest, KbaLandmarkWrite, KbaLidarCloud, KbaLidarOptions, KbaLidarView, KbaOptions, KbaPoseWrite, KbaPushRequest, KbaRankedRequest, KbaRankOut, KbaRankRequest, KbaReclaimOut, KbaReclaimRequest, KbaResult, KbaSelectOut, KbaSelectParams, KbaSelectRequest,
+from .capi_types import (KbaCounters, KbaCreateOut, KbaCreateRequest, KbaDeactivateOut, KbaDeactivateRequest, KbaDepthEntry, KbaDepthOut, KbaDepthRequest, KbaDrawFn, KbaEvalOut, KbaEvaluateOut, KbaFlowOut, KbaFlowRequest, KbaLandmarkWrite, KbaLidarCloud, KbaLidarOptions, KbaLidarView, KbaOptions, KbaPoseWrite, KbaPushRequest, KbaRankedRequest, KbaRankOut, KbaRankRequest, KbaReclaimOut, KbaReclaimRequest, KbaResult, KbaSelectOut, KbaSelectParams, KbaSelectRequest,
                          KbaSnapshotHeader, KbaTrackCaps, KbaTrackFrame, KbaTrackRequest, KbaWindow, Result, Window, c_double_p, c_float_p, c_int32_p,
                          c_uint8_p)
 
@@ -36,7 +36,8 @@ SYMBOLS = ["kba_version", "kba_last_error", "kba_default_options", "kba_create",
            "kba_track_group_adjust_pose_opts", "kba_track_group_push_keyframes", "kba_track_group_drop_keyframes",
            "kba_track_group_set_landmarks", "kba_track_group_set_keyframe_poses", "kba_lidar_depth_batch",
            "kba_lidar_depth_batch_opts", "kba_track_snapshot_size", "kba_track_save", "kba_track_load", "kba_track_clone",
-           "kba_track_group_snapshot_sizes", "kba_track_group_save"]
+           "kba_track_group_snapshot_sizes", "kba_track_group_save", "kba_track_evaluate", "kba_track_group_evaluate",
+           "kba_track_group_evaluate_opts"]
 
 
 class KbaError(RuntimeError):
@@ -172,6 +173,9 @@ def lib():
         L.kba_track_clone.argtypes = [vp, vp, C.POINTER(KbaTrackCaps), C.POINTER(vp)]
         L.kba_track_group_snapshot_sizes.argtypes = [vp, i64p]
         L.kba_track_group_save.argtypes = [vp, C.POINTER(vp), i64p]
+        L.kba_track_evaluate.argtypes = [vp, C.POINTER(KbaTrackRequest), C.POINTER(KbaOptions), C.POINTER(KbaEvaluateOut)]
+        for f in (L.kba_track_group_evaluate, L.kba_track_group_evaluate_opts):
+            f.argtypes = [vp, C.POINTER(KbaTrackRequest), C.POINTER(KbaOptions), C.POINTER(KbaEvaluateOut)]
         L.kba_lidar_default_options.argtypes = [C.POINTER(KbaLidarOptions)]
         L.kba_lidar_default_options.restype = None
         fp = C.POINTER(C.c_float)
@@ -373,6 +377,31 @@ def _select_outputs(n_cand):
     return bufs, co, n_near, result
 
 
+COST_PARTS = ("reprojection", "depth", "ground_plane", "scale", "plane_chain", "total")
+
+
+def _evaluate_outputs(n_lm, obs_cap, gp_cap):
+    """the output struct of an evaluation of n_lm landmarks with room for obs_cap observations and gp_cap ground-plane residuals,
+    its arrays, and the function of the filled struct that gives the evaluation's dict of numpy arrays"""
+    b = dict(obs_lm=np.empty(obs_cap, np.int32), obs_kf=np.empty(obs_cap, np.int32), obs_cam=np.empty(obs_cap, np.int32),
+             residual=np.empty((obs_cap, 3)), rho=np.empty((obs_cap, 2)), trim_repr=np.empty(n_lm), trim_depth=np.empty(n_lm),
+             rejected_repr=np.empty(n_lm, np.uint8), rejected_depth=np.empty(n_lm, np.uint8), gp_lm=np.empty(gp_cap, np.int32),
+             gp_kf=np.empty(gp_cap, np.int32), gp_weight=np.empty(gp_cap), gp_residual=np.empty(gp_cap))
+    o = KbaEvaluateOut(obs_capacity=obs_cap)
+    ptr = dict(KbaEvaluateOut._fields_)
+    for k, a in b.items():
+        setattr(o, k, a.ctypes.data_as(ptr[k]))
+
+    def done(c):
+        n, g = c.n_obs, c.n_gp
+        r = {k: (a[:n] if k.startswith("obs_") or k in ("residual", "rho") else a[:g] if k.startswith("gp_") else a)
+             for k, a in b.items()}
+        r.update(n_obs=n, n_gp=g, failed=bool(c.failed), cost=np.array(c.cost[:]))
+        r.update(rejected_repr=r["rejected_repr"].astype(bool), rejected_depth=r["rejected_depth"].astype(bool))
+        return r
+    return o, tuple(b.values()), done
+
+
 class Track:
     """Persistent, device-resident sliding window (kba_track_*): keyframes are uploaded once when pushed, a solve sends only
     the lists of active keyframe slots and selected landmark slots.
@@ -444,6 +473,23 @@ class Track:
         q, o, _keep, done = self._solve_request(256, kf_slots, kf_fixed, lm_slots, **scalars)
         _check(lib().kba_track_solve(self._p, q.n_kf, q.kf_slot, q.kf_fixed, q.n_lm, q.lm_slot, q.sel, C.byref(opt or default_options()),
                                      C.byref(o)))
+        return done(o)
+
+    def _evaluate_request(self, kf_slots, kf_fixed, lm_slots, obs_capacity=None, **scalars):
+        """the solve's request (_solve_request) and the outputs of an evaluation of it: obs_capacity observations (default: the
+        track's win_observations, which holds any window), win_ground ground-plane residuals"""
+        q, _, keep, _ = self._solve_request(1, kf_slots, kf_fixed, lm_slots, **scalars)
+        cap = self.caps.win_observations if obs_capacity is None else int(obs_capacity)
+        o, bufs, done = _evaluate_outputs(q.n_lm, cap, self.caps.win_ground)
+        return q, o, (*bufs, *keep), done
+
+    def evaluate(self, kf_slots, kf_fixed, lm_slots, opt=None, obs_capacity=None, **scalars):
+        """residuals, losses, trimming values and decisions and the cost parts of the window Track.solve would build for these
+        arguments, at the store's state, without changing it (kba_track_evaluate).  Returns a dict: n_obs, obs_lm, obs_kf, obs_cam,
+        residual [n_obs, 3] (u, v, depth before any loss), rho [n_obs, 2] (scaled Cauchy losses), trim_repr, trim_depth,
+        rejected_repr, rejected_depth [n_lm], n_gp, gp_lm, gp_kf, gp_weight, gp_residual [n_gp], cost [6] (COST_PARTS), failed."""
+        q, o, _keep, done = self._evaluate_request(kf_slots, kf_fixed, lm_slots, obs_capacity, **scalars)
+        _check(lib().kba_track_evaluate(self._p, C.byref(q), C.byref(opt or default_options()), C.byref(o)))
         return done(o)
 
     def _frame_request(self, capacity, pose7, lm_slot, u, v, d, cam=None, speed=None):
@@ -745,6 +791,14 @@ class TrackGroup:
         fn, o = _options(opt, len(self.tracks), lib().kba_track_group_solve, lib().kba_track_group_solve_opts)
         return self._call(fn, requests, lambda t, **r: t._solve_request(iterations_capacity, **r), KbaTrackRequest, KbaResult,
                           idle=lambda: _idle(KbaTrackRequest, 0), opt=(o,))
+
+    def evaluate(self, requests, opt=None):
+        """one evaluation per track in one launch sequence (kba_track_group_evaluate): requests as for TrackGroup.solve, with the
+        keywords of Track.evaluate; opt: one KbaOptions, or one per track (kba_track_group_evaluate_opts).  Returns one dict per
+        track (Track.evaluate's), None for a track that sat out."""
+        fn, o = _options(opt, len(self.tracks), lib().kba_track_group_evaluate, lib().kba_track_group_evaluate_opts)
+        return self._call(fn, requests, lambda t, **r: t._evaluate_request(**r), KbaTrackRequest, KbaEvaluateOut,
+                          sits_out=_no_keyframes, why="fewer than 3 keyframes (kba_track_evaluate refuses it with error 3)", opt=(o,))
 
     def adjust_pose(self, frames, opt=None, iterations_capacity=256):
         """one frame per track in one launch (kba_track_group_adjust_pose): each entry None (the track sits the call out) or a

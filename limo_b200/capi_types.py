@@ -42,6 +42,13 @@ class KbaTrackRequest(C.Structure):
                 ("sel", C.POINTER(KbaWindow))]
 
 
+class KbaEvaluateOut(C.Structure):
+    _fields_ = [("obs_capacity", C.c_int32), ("n_obs", C.c_int32), ("n_gp", C.c_int32), ("failed", C.c_int32), ("cost", C.c_double * 6),
+                ("obs_lm", c_int32_p), ("obs_kf", c_int32_p), ("obs_cam", c_int32_p), ("residual", c_double_p), ("rho", c_double_p),
+                ("trim_repr", c_double_p), ("trim_depth", c_double_p), ("rejected_repr", c_uint8_p), ("rejected_depth", c_uint8_p),
+                ("gp_lm", c_int32_p), ("gp_kf", c_int32_p), ("gp_weight", c_double_p), ("gp_residual", c_double_p)]
+
+
 class KbaSelectParams(C.Structure):
     _fields_ = [("voxel_size", C.c_double * 3), ("roi_far", C.c_double), ("roi_middle", C.c_double)]
 

@@ -564,6 +564,39 @@ bool BundleAdjusterKeyframes::trackSync(const std::vector<Keyframe*>& kfs) {
     return true;
 }
 
+// the lists of a solve or evaluation of the window kfs / lm_ids on the track (sel points into q's candidate list)
+struct BundleAdjusterKeyframes::TrackRequest {
+    std::vector<int32_t> kf_slots, lm_slots, gp_cand;
+    std::vector<uint8_t> fixed;
+    kba_window sel{};
+};
+
+// false: a selected landmark was never measured by a stored keyframe (no slot)
+bool BundleAdjusterKeyframes::trackRequest(const std::vector<Keyframe*>& kfs, const std::vector<LandmarkId>& lm_ids, TrackRequest& q) const {
+    const int n_kf = int(kfs.size()), n_lm = int(lm_ids.size());
+    for (const Keyframe* kf : kfs) {
+        q.kf_slots.push_back(kf_slot_.at(kf->timestamp_));
+        q.fixed.push_back(kf->fixation_status_ == Keyframe::FixationStatus::Pose);
+    }
+    for (const auto id : lm_ids) {
+        auto it = lm_slot_.find(id);
+        if (it == lm_slot_.end()) return false;
+        q.lm_slots.push_back(it->second);
+    }
+    // addGroundPlaneResiduals (cpp:517-562) on the device: the selected ground-plane landmarks go up as candidates, the store's
+    // poses, planes and positions decide which are attached to which keyframe
+    for (int j = 0; j < n_lm; ++j)
+        if (landmarks_.at(lm_ids[j])->is_ground_plane) q.gp_cand.push_back(j);
+    kba_window& sel = q.sel;
+    sel.n_kf = n_kf; sel.n_lm = n_lm;
+    sel.n_gp = int(q.gp_cand.size()); sel.gp_lm = q.gp_cand.data();
+    sel.plane_reg_weight = q.gp_cand.empty() ? 0. : -1.;  // -1: 10 iff a ground-plane residual is attached (cpp:717-719)
+    sel.scale_kf0 = 0; sel.scale_kf1 = 1;
+    sel.scale_weight = -1.;  // the reference's rule (cpp:703-716), evaluated on the device from the gathered window
+    sel.scale_value = n_kf > 1 ? (kfs[1]->getEigenPose() * kfs[0]->getEigenPose().inverse()).translation().norm() : 0.;
+    return true;
+}
+
 // synced: trackSync(kfs) already ran for this solve (the device-side selection needed the same state)
 bool BundleAdjusterKeyframes::solveTracked(const std::vector<Keyframe*>& kfs, const std::vector<LandmarkId>& lm_ids, std::string& report,
                                            bool synced) {
@@ -571,29 +604,11 @@ bool BundleAdjusterKeyframes::solveTracked(const std::vector<Keyframe*>& kfs, co
     // state the host may have changed since the last solve: poses / planes of the active keyframes, new landmarks, weights
     if (!synced && !trackSync(kfs)) return false;
     const int n_kf = int(kfs.size()), n_lm = int(lm_ids.size());
-    std::vector<int32_t> kf_slots, lm_slots;
-    std::vector<uint8_t> fixed;
-    for (const Keyframe* kf : kfs) {
-        kf_slots.push_back(kf_slot_.at(kf->timestamp_));
-        fixed.push_back(kf->fixation_status_ == Keyframe::FixationStatus::Pose);
-    }
-    for (const auto id : lm_ids) {
-        auto it = lm_slot_.find(id);
-        if (it == lm_slot_.end()) return false;  // selected but never measured by a stored keyframe: let the rebuild path decide
-        lm_slots.push_back(it->second);
-    }
-    // addGroundPlaneResiduals (cpp:517-562) on the device: the selected ground-plane landmarks go up as candidates, the store's
-    // poses, planes and positions decide which are attached to which keyframe
-    std::vector<int32_t> gp_cand;
-    for (int j = 0; j < n_lm; ++j)
-        if (landmarks_.at(lm_ids[j])->is_ground_plane) gp_cand.push_back(j);
-    kba_window sel{};
-    sel.n_kf = n_kf; sel.n_lm = n_lm;
-    sel.n_gp = int(gp_cand.size()); sel.gp_lm = gp_cand.data();
-    sel.plane_reg_weight = gp_cand.empty() ? 0. : -1.;  // -1: 10 iff a ground-plane residual is attached (cpp:717-719)
-    sel.scale_kf0 = 0; sel.scale_kf1 = 1;
-    sel.scale_weight = -1.;  // the reference's rule (cpp:703-716), evaluated on the device from the gathered window
-    sel.scale_value = n_kf > 1 ? (kfs[1]->getEigenPose() * kfs[0]->getEigenPose().inverse()).translation().norm() : 0.;
+    TrackRequest q;
+    if (!trackRequest(kfs, lm_ids, q)) return false;  // selected but never measured by a stored keyframe: let the rebuild path decide
+    const std::vector<int32_t>& kf_slots = q.kf_slots, &lm_slots = q.lm_slots;
+    const std::vector<uint8_t>& fixed = q.fixed;
+    const kba_window& sel = q.sel;
     const kba_options opt = solve_options(outlier_rejection_options_, solver_time_sec, false, lm_ids.size());
     std::vector<double> out_pose(7 * size_t(n_kf)), out_plane(4 * size_t(n_kf)), out_lm(3 * size_t(n_lm) + 3);
     kba_result r{};
@@ -615,6 +630,69 @@ bool BundleAdjusterKeyframes::solveTracked(const std::vector<Keyframe*>& kfs, co
     for (int j = 0; j < n_lm; ++j) std::copy_n(out_lm.begin() + 3 * j, 3, landmarks_.at(lm_ids[j])->pos.begin());
     report = solve_report(r, " (device-resident window)");
     return true;
+}
+
+void BundleAdjusterKeyframes::evaluateResiduals() {
+    const char* who = "evaluateResiduals: ";
+    if (!persistent_window_) throw std::runtime_error(std::string(who) + "the persistent window is off (set_persistent_window(false)); there is no host evaluation");
+    if (track_failed_) throw std::runtime_error(std::string(who) + "the device-resident store failed (a keyframe or landmark it could not take)");
+    if (!track_) throw std::runtime_error(std::string(who) + "no device-resident window yet: call solve() first");
+    std::vector<Keyframe*> kfs;
+    for (const auto& id : active_keyframe_ids_) kfs.push_back(keyframes_.at(id).get());
+    std::vector<LandmarkId> lm_ids(selected_landmark_ids_.begin(), selected_landmark_ids_.end());
+    if (kfs.size() < 3) throw std::runtime_error(std::string(who) + "fewer than 3 active keyframes");
+    if (int(kfs.size()) > kTrackWinKeyframes || int(lm_ids.size()) > kTrackWinLandmarks)
+        throw std::runtime_error(std::string(who) + "the window is larger than the device-resident store's window capacity");
+    if (!trackSync(kfs)) throw std::runtime_error(std::string(who) + "the device-resident store failed while taking the current state");
+    TrackRequest q;
+    if (!trackRequest(kfs, lm_ids, q)) throw std::runtime_error(std::string(who) + "a selected landmark is not in the device-resident store");
+    const kba_options opt = solve_options(outlier_rejection_options_, solver_time_sec, false, lm_ids.size());
+    const size_t n_lm = lm_ids.size(), cap = size_t(kTrackWinObservations), n_gp = q.gp_cand.size();
+    std::vector<int32_t> obs_lm(cap), obs_kf(cap), obs_cam(cap), gp_lm(n_gp + 1), gp_kf(n_gp + 1);
+    std::vector<double> res(3 * cap), rho(2 * cap), trim_r(n_lm + 1), trim_d(n_lm + 1), gp_w(n_gp + 1), gp_r(n_gp + 1);
+    std::vector<uint8_t> rej_r(n_lm + 1), rej_d(n_lm + 1);
+    kba_evaluate_out out{};
+    out.obs_capacity = int32_t(cap);
+    out.obs_lm = obs_lm.data(); out.obs_kf = obs_kf.data(); out.obs_cam = obs_cam.data(); out.residual = res.data(); out.rho = rho.data();
+    out.trim_repr = trim_r.data(); out.trim_depth = trim_d.data(); out.rejected_repr = rej_r.data(); out.rejected_depth = rej_d.data();
+    out.gp_lm = gp_lm.data(); out.gp_kf = gp_kf.data(); out.gp_weight = gp_w.data(); out.gp_residual = gp_r.data();
+    kba_track_request req{int32_t(kfs.size()), q.kf_slots.data(), q.fixed.data(), int32_t(n_lm), q.lm_slots.data(), &q.sel};
+    if (kba_track_evaluate(track_, &req, &opt, &out) != KBA_OK) throw std::runtime_error(std::string(who) + "kba_b200: " + kba_last_error());
+    last_evaluation_ = keyEvaluation(std::vector<const Keyframe*>(kfs.begin(), kfs.end()), lm_ids, track_cams_, out);
+}
+
+BundleAdjusterKeyframes::Evaluation keyEvaluation(const std::vector<const Keyframe*>& kfs, const std::vector<LandmarkId>& lm_ids,
+                                                  const std::vector<std::array<double, 10>>& track_cams, const kba_evaluate_out& out) {
+    BundleAdjusterKeyframes::Evaluation e;
+    auto bad = [](const std::string& why) { throw std::runtime_error("evaluateResiduals: " + why); };
+    int o = 0;
+    for (size_t j = 0; j < lm_ids.size(); ++j) {
+        for (size_t k = 0; k < kfs.size(); ++k) {
+            const auto it = kfs[k]->measurements_.find(lm_ids[j]);
+            if (it == kfs[k]->measurements_.end()) continue;
+            for (const auto& cm : it->second) {
+                if (o >= out.n_obs) bad("fewer observations in the window than the keyframes measure");
+                const int cam = int(std::find(track_cams.begin(), track_cams.end(), camera_value(*kfs[k]->cameras_.at(cm.first))) - track_cams.begin());
+                if (out.obs_lm[o] != int(j) || out.obs_kf[o] != int(k) || out.obs_cam[o] != cam)
+                    bad("observation " + std::to_string(o) + " is not the one the host enumerates");
+                BundleAdjusterKeyframes::Evaluation::Residual r;
+                r.u = out.residual[3 * o]; r.v = out.residual[3 * o + 1]; r.depth = out.residual[3 * o + 2];
+                r.rho_reprojection = out.rho[2 * o]; r.rho_depth = out.rho[2 * o + 1];
+                e.residuals[std::make_tuple(lm_ids[j], KeyframeId(kfs[k]->timestamp_), cm.first)] = r;
+                ++o;
+            }
+        }
+        BundleAdjusterKeyframes::Evaluation::Trim t;
+        t.reprojection = out.trim_repr[j]; t.depth = out.trim_depth[j];
+        t.rejected_reprojection = out.rejected_repr[j] != 0; t.rejected_depth = out.rejected_depth[j] != 0;
+        e.landmarks[lm_ids[j]] = t;
+    }
+    if (o != out.n_obs) bad("more observations in the window than the keyframes measure");
+    for (int g = 0; g < out.n_gp; ++g) e.ground_plane[lm_ids.at(size_t(out.gp_lm[g]))] = out.gp_residual[g];
+    e.cost_reprojection = out.cost[0]; e.cost_depth = out.cost[1]; e.cost_ground_plane = out.cost[2];
+    e.cost_scale = out.cost[3]; e.cost_plane_chain = out.cost[4]; e.cost_total = out.cost[5];
+    e.failed = out.failed != 0;
+    return e;
 }
 
 // Landmark state the host changed since the store last saw it: position and weight of new landmarks (push()) and of landmarks

@@ -325,6 +325,8 @@ struct SlotStamps {
 enum StoreCall { kSelectCall, kCreateCall, kUpkeepCall, kFlowCall, kReclaimCall, kRankCall, kPushCall, kLandmarkWriteCall, kPoseWriteCall,
                  kSnapshotCall, kStoreCalls };
 
+struct EvalStage;
+
 // what a track and a track group own alike.  A track's set is {the track}: its calls run the host code of a group's, with one
 // window.
 struct TrackSet {
@@ -334,8 +336,22 @@ struct TrackSet {
     TrackSolver large;                     // some track has win_rows > kFusedMaxRows: the whole set on the large-window path, else no batch
     std::unique_ptr<StoreStage> stage[kStoreCalls];  // each at its call's first run, for every track's capacities
     const Transfer* last = &kNoTransfer;   // the transfer counts of the last call
-    ~TrackSet() { solver.release(); large.release(); }
+    std::unique_ptr<EvalStage> eval;       // evaluations, at the first one
+    ~TrackSet();
 };
+
+// staging of the evaluations of a track or group (kba_evaluate.cu): the output block (device + pinned), laid out per call so that
+// one copy brings down exactly the call's outputs, the windows' regions in it, and the cost partials (device only).  Allocated at
+// the first evaluation for the capacities of the set's tracks.
+struct EvalStage {
+    Staged<unsigned char> out;
+    Staged<EvalWin> wins;
+    double* part = nullptr;
+    DevAllocs dev;
+    Transfer counts;                       // the last evaluation's
+    ~EvalStage() { out.release(); wins.release(); }
+};
+TrackSet::~TrackSet() { solver.release(); large.release(); }
 
 // persistent, device-resident window (kba_track_*, at the end of this file)
 struct kba_track {
@@ -1588,6 +1604,7 @@ struct TrackRequest {
     const int32_t* lm_slot = nullptr;
     const kba_window* sel = nullptr;       // nullptr: the track sits a group solve out
     int max_meas = 0, n_free = 0;          // filled by track_check: largest keyframe measurement count, free keyframes
+    int n_meas = 0;                        // filled by track_check: measurements of the listed keyframes, a bound on the observations
     bool device_gp = false;                // filled by track_check: sel->gp_lm lists candidates, attached by k_track_ground
     int rows = 0;                          // filled by track_check: reduced rows kba_batch_create sizes the window for (reduced_rows,
                                            // plane blocks counted whenever candidates are given)
@@ -1623,6 +1640,7 @@ static int track_check(const kba_track* t, TrackRequest& q, std::string& why) {
         q.n_free += q.kf_fixed[k] ? 0 : 1;
     }
     if (n_meas > c.win_observations) { why = "more observations than win_observations"; return KBA_ERR_CAPACITY; }
+    q.n_meas = (int)n_meas;
     for (int j = 0; j < q.n_lm && !q.ranked; ++j)
         if (q.lm_slot[j] < 0 || q.lm_slot[j] >= t->td.lm_cap) { why = "landmark slot out of range"; return KBA_ERR_BAD_ARG; }
     q.device_gp = q.rank_gp || device_attached(sel);
@@ -1780,21 +1798,23 @@ int kba_track_create(kba_handle* h, const kba_track_caps* c, int32_t n_cam, cons
     return KBA_OK;
 }
 
-// one solve of the stored windows of tracks ts[0..n) as one batch, window i = ts[i]'s; qs[i] is checked by track_check or sits
-// the solve out (sel == nullptr).  kba_track_solve (n = 1) and kba_track_group_solve.
-static int track_solve(kba_handle* h, TrackSolver& sv, int n, kba_track* const* ts, const TrackRequest* qs, bool per_track,
-                       const kba_options* opts, const SolveTotals& tot, kba_result* res) {
-    kba_batch* b = sv.batch;
-    CU(cudaSetDevice(h->device));
-    cudaStream_t s = h->stream;
-    // ---- descriptors, selection lists (one pinned buffer), track stores as they are now
-    int max_rank = 0, max_free = 0;
-    std::vector<WinShape> solved(n);       // rows and chunks of the solved windows (large-window path)
-    bool any_gp = false;
+// the host side of the gather of tracks ts[0..n) into sv's batch, window i = ts[i]'s: what staging the requests leaves for the launch
+struct StagedLists {
     TrackGrid grid;
-    const size_t p_ints = params_ints(n);
-    size_t used = p_ints;
-    int64_t h2d = (int64_t)n * (int64_t)(sizeof(WinDesc) + sizeof(TrackDev) + sizeof(TrackSel));
+    size_t used = 0;                       // ints of sv.lists in use (the options' included)
+    int64_t h2d = 0;                       // bytes the upload moves, the options' excluded
+    int max_rank = 0, max_free = 0;        // of the windows that do not sit out: rig rank, free reduced rows (track_free_rows)
+    std::vector<WinShape> solved;          // rows and chunks of those windows (large-window path)
+    bool any_gp = false;                   // some window has host ground-plane lists
+};
+
+// descriptors, selection lists (one pinned buffer) and track stores as they are now of requests qs[0..n), each checked by
+// track_check or sitting out (sel == nullptr), into sv's staging
+static void stage_requests(TrackSolver& sv, int n, kba_track* const* ts, const TrackRequest* qs, StagedLists& sl) {
+    kba_batch* b = sv.batch;
+    sl.solved.assign(n, WinShape{});
+    sl.used = params_ints(n);
+    sl.h2d = (int64_t)n * (int64_t)(sizeof(WinDesc) + sizeof(TrackDev) + sizeof(TrackSel));
     for (int i = 0; i < n; ++i) {
         const kba_track* t = ts[i];
         const TrackRequest& q = qs[i];
@@ -1805,15 +1825,15 @@ static int track_solve(kba_handle* h, TrackSolver& sv, int n, kba_track* const* 
             sv.tsel.h[i] = TrackSel{};
         } else {
             track_desc(d, t, q);
-            max_rank = std::max(max_rank, d.max_rank);
-            max_free = std::max(max_free, track_free_rows(q));
-            solved[i].rows = q.rows; solved[i].n_chunks = d.n_chunks;
+            sl.max_rank = std::max(sl.max_rank, d.max_rank);
+            sl.max_free = std::max(sl.max_free, track_free_rows(q));
+            sl.solved[i].rows = q.rows; sl.solved[i].n_chunks = d.n_chunks;
             // lists: keyframe slots | landmark slots | fixation bytes | ground-plane candidates
             // (a ranked request's landmarks and ground candidates are the track's ranking, already on the device)
             const kba_window* sel = q.sel;
             const int n_cand = q.device_gp ? sel->n_gp : 0, fixed_ints = (q.n_kf + 3) / 4;
-            int* l = sv.lists.h + used;
-            const int* ld = sv.lists.d + used;
+            int* l = sv.lists.h + sl.used;
+            const int* ld = sv.lists.d + sl.used;
             size_t at = (size_t)q.n_kf;
             memcpy(l, q.kf_slot, q.n_kf * sizeof(int));
             const int* lm_d = q.ranked ? ts[i]->rank->sel_slot : ld + at;
@@ -1824,44 +1844,66 @@ static int track_solve(kba_handle* h, TrackSolver& sv, int n, kba_track* const* 
             const int* cand_d = q.rank_gp ? ts[i]->rank->gp : ld + at;
             if (n_cand && !q.rank_gp) { memcpy(l + at, sel->gp_lm, n_cand * sizeof(int)); at += (size_t)n_cand; }
             sv.tsel.h[i] = track_sel(q, ld, fx_d, lm_d, cand_d);
-            used += at;
-            ts[i]->gen++;  // the solve writes the store back
+            sl.used += at;
             if (sel->n_gp && !q.device_gp) {
                 memcpy(b->r_gp_lm.h + d.gp_off, sel->gp_lm, sel->n_gp * sizeof(int)); memcpy(b->gp_kf.h + d.gp_off, sel->gp_kf, sel->n_gp * sizeof(int));
                 memcpy(b->gp_weight.h + d.gp_off, sel->gp_weight, sel->n_gp * sizeof(double));
-                any_gp = true;
+                sl.any_gp = true;
             }
-            grid.max_kf = std::max(grid.max_kf, q.n_kf); grid.max_lm = std::max(grid.max_lm, q.n_lm);
-            grid.max_meas = std::max(grid.max_meas, q.max_meas);
-            grid.any_cand |= n_cand > 0;
-            h2d += (int64_t)q.n_kf * 5 + (q.ranked ? 0 : (int64_t)q.n_lm * 4) +
-                   (q.device_gp ? (q.rank_gp ? 0 : (int64_t)n_cand * 4) : (int64_t)sel->n_gp * 16);
+            sl.grid.max_kf = std::max(sl.grid.max_kf, q.n_kf); sl.grid.max_lm = std::max(sl.grid.max_lm, q.n_lm);
+            sl.grid.max_meas = std::max(sl.grid.max_meas, q.max_meas);
+            sl.grid.any_cand |= n_cand > 0;
+            sl.h2d += (int64_t)q.n_kf * 5 + (q.ranked ? 0 : (int64_t)q.n_lm * 4) +
+                      (q.device_gp ? (q.rank_gp ? 0 : (int64_t)n_cand * 4) : (int64_t)sel->n_gp * 16);
         }
         b->desc.h[i] = d;
     }
+}
+
+// the staged requests up, then the gather of every window from its store.  The options go up in the lists' copy when they differ
+// from what the device holds (a re-solve with the same ones: none).
+static int upload_and_gather(kba_handle* h, TrackSolver& sv, bool per_track, const kba_options* opts, StagedLists& sl) {
+    kba_batch* b = sv.batch;
+    cudaStream_t s = h->stream;
+    const size_t p_ints = params_ints(b->bd.n_win);
+    const size_t from = stage_params(b, per_track, opts, reinterpret_cast<SolveParams*>(sv.lists.h)) ? 0 : p_ints;
+    sl.h2d += (int64_t)((p_ints - from) * sizeof(int));
+    CU(b->desc.upload(s));
+    CU(cudaMemcpyAsync(sv.lists.d + from, sv.lists.h + from, (sl.used - from) * sizeof(int), cudaMemcpyHostToDevice, s));
+    CU(sv.tdev.upload(s)); CU(sv.tsel.upload(s));
+    if (sl.any_gp) { CU(b->r_gp_lm.upload(s)); CU(b->gp_kf.upload(s)); CU(b->gp_weight.upload(s)); }
+    launch_track_gather(b->bd, b->raw, sv.tdev.d, sv.tsel.d, sl.grid, s);
+    return KBA_OK;
+}
+
+// one solve of the stored windows of tracks ts[0..n) as one batch, window i = ts[i]'s; qs[i] is checked by track_check or sits
+// the solve out (sel == nullptr).  kba_track_solve (n = 1) and kba_track_group_solve.
+static int track_solve(kba_handle* h, TrackSolver& sv, int n, kba_track* const* ts, const TrackRequest* qs, bool per_track,
+                       const kba_options* opts, const SolveTotals& tot, kba_result* res) {
+    kba_batch* b = sv.batch;
+    CU(cudaSetDevice(h->device));
+    cudaStream_t s = h->stream;
+    StagedLists sl;
+    stage_requests(sv, n, ts, qs, sl);
+    for (int i = 0; i < n; ++i)
+        if (qs[i].sel) ts[i]->gen++;  // the solve writes the store back
     // one launch configuration for the whole batch, as kba_batch_solve has for any batch
-    b->lc.max_rank = max_rank;
-    b->lc.plan.fused_slots = fused_slots(max_free);
+    b->lc.max_rank = sl.max_rank;
+    b->lc.plan.fused_slots = fused_slots(sl.max_free);
     if (!b->lc.plan.fused) {  // the buffers are sized for the largest values (batch_create, Purpose::TrackLarge)
-        replan_large(b->lc.plan, solved.data(), n, h->sm_count, b->lc.knobs);
-        for (int i = 0; i < n; ++i) b->desc.h[i].nr_cap = b->desc_h[i].nr_cap = nr_cap_of(solved[i].rows);
+        replan_large(b->lc.plan, sl.solved.data(), n, h->sm_count, b->lc.knobs);
+        for (int i = 0; i < n; ++i) b->desc.h[i].nr_cap = b->desc_h[i].nr_cap = nr_cap_of(sl.solved[i].rows);
         apply_plan(b);
     }
-    // the options go up in the lists' copy when they differ from what the device holds (a re-solve with the same ones: none)
-    const size_t from = stage_params(b, per_track, opts, reinterpret_cast<SolveParams*>(sv.lists.h)) ? 0 : p_ints;
-    h2d += (int64_t)((p_ints - from) * sizeof(int));
-    CU(b->desc.upload(s));
-    CU(cudaMemcpyAsync(sv.lists.d + from, sv.lists.h + from, (used - from) * sizeof(int), cudaMemcpyHostToDevice, s));
-    CU(sv.tdev.upload(s)); CU(sv.tsel.upload(s));
-    if (any_gp) { CU(b->r_gp_lm.upload(s)); CU(b->gp_kf.upload(s)); CU(b->gp_weight.upload(s)); }
-    sv.counts.h2d = h2d;
-    // ---- gather every window from its store, pack, solve, write back
-    launch_track_gather(b->bd, b->raw, sv.tdev.d, sv.tsel.d, grid, s);
+    int rc = upload_and_gather(h, sv, per_track, opts, sl);
+    if (rc != KBA_OK) return rc;
+    sv.counts.h2d = sl.h2d;
+    // ---- pack, solve, write back
     launch_pack(b->bd, b->raw, s);
     CU(cudaGetLastError());
-    int rc = batch_run(b, tot);
+    rc = batch_run(b, tot);
     if (rc != KBA_OK) return rc;
-    launch_track_writeback(b->bd, sv.tdev.d, sv.tsel.d, grid, s);
+    launch_track_writeback(b->bd, sv.tdev.d, sv.tsel.d, sl.grid, s);
     rc = kba_batch_download(b, res);
     sv.counts.d2h = (int64_t)b->d2h_bytes;
     return rc;
@@ -1992,6 +2034,175 @@ int kba_track_group_transfer_bytes(kba_track_group* g, int64_t* h2d, int64_t* d2
     if (h2d) *h2d = g->set.last->h2d;
     if (d2h) *d2h = g->set.last->d2h;
     return KBA_OK;
+}
+
+// ---------------------------------------------------------------------------------------------------------------------
+// evaluation of the stored windows at the store's state (include/kba_b200.h, kba_track_evaluate / kba_track_group_evaluate)
+// ---------------------------------------------------------------------------------------------------------------------
+static size_t al8(size_t b) { return (b + 7) & ~(size_t)7; }
+
+// one call's output block: the windows' records, then each array for the call's totals (observation bounds TO, landmarks TL,
+// ground-plane lists TG), back to back, 8-byte aligned
+extern "C++" {  // templates have C++ linkage
+struct EvalLayout {
+    size_t head = 0, res = 0, rho = 0, trim = 0, gp_w = 0, gp_r = 0, obs_lm = 0, obs_kf = 0, obs_cam = 0, gp_lm = 0, gp_kf = 0, rej = 0, bytes = 0;
+    EvalLayout(size_t W, size_t TO, size_t TL, size_t TG) {
+        size_t at = 0;
+        auto put = [&at](size_t& off, size_t b) { off = at; at += al8(b); };
+        put(head, sizeof(EvalHead) * W);
+        put(res, 24 * TO); put(rho, 16 * TO); put(trim, 16 * TL); put(gp_w, 8 * TG); put(gp_r, 8 * TG);
+        put(obs_lm, 4 * TO); put(obs_kf, 4 * TO); put(obs_cam, 4 * TO); put(gp_lm, 4 * TG); put(gp_kf, 4 * TG); put(rej, 2 * TL);
+        bytes = at;
+    }
+    template <typename T> T* at(unsigned char* base, size_t off) const { return reinterpret_cast<T*>(base + off); }
+    EvalOut view(unsigned char* b, double* part) const {
+        EvalOut o;
+        o.head = at<EvalHead>(b, head); o.res = at<double>(b, res); o.rho = at<double>(b, rho); o.trim = at<double>(b, trim);
+        o.gp_w = at<double>(b, gp_w); o.gp_r = at<double>(b, gp_r); o.obs_lm = at<int>(b, obs_lm); o.obs_kf = at<int>(b, obs_kf);
+        o.obs_cam = at<int>(b, obs_cam); o.gp_lm = at<int>(b, gp_lm); o.gp_kf = at<int>(b, gp_kf); o.rej = at<unsigned char>(b, rej);
+        o.part = part;
+        return o;
+    }
+};
+}  // extern "C++"
+
+static int eval_stage(TrackSet& s, const std::string& who) {
+    if (s.eval) return KBA_OK;
+    size_t TO = 0, TL = 0, TG = 0, parts = 0;
+    for (const kba_track* t : s.tracks) {
+        TO += (size_t)t->caps.win_observations; TL += (size_t)t->caps.win_landmarks; TG += (size_t)t->caps.win_ground;
+        parts += (size_t)(t->caps.win_landmarks + 63) / 64;
+    }
+    std::unique_ptr<EvalStage> e(new EvalStage());
+    const size_t n = s.tracks.size();
+    int bad = e->out.alloc(EvalLayout(n, TO, TL, TG).bytes, true) | e->wins.alloc(n, true);
+    bad |= e->dev.alloc(&e->part, 3 * std::max<size_t>(parts, 1));
+    if (bad) return fail(KBA_ERR_CUDA, who + "out of memory (evaluation staging)");
+    s.eval = std::move(e);
+    return KBA_OK;
+}
+
+static bool obs_arrays(const kba_evaluate_out& o) { return o.obs_lm || o.obs_kf || o.obs_cam || o.residual || o.rho; }
+
+// one evaluation of the windows of a track (group = false) or of a group, qs[i] track i's request; the checks are a solve's (and
+// FP64 only), in track order before anything is uploaded; in a group a request with n_kf == 0 sits the call out
+static int set_evaluate(TrackSet& s, bool group, const std::string& who, TrackRequest* qs, bool per_track, const kba_options* opts,
+                        kba_evaluate_out* out) {
+    const int n = (int)s.tracks.size();
+    auto live = [&](int i) { return !(group && qs[i].n_kf == 0); };
+    SolveTotals tot;
+    std::string owhy;
+    const int orc = solve_options_check(n, opts, per_track, "track ", live, tot, owhy);
+    if (orc != KBA_OK) return fail(orc, who + owhy);
+    // FP64 only: per track, the entries of the tracks that are evaluated; one set, whenever some track is evaluated
+    for (int i = 0; i < n; ++i) {
+        if (!live(i)) continue;
+        const int o = per_track ? i : 0;
+        if (opts[o].precision != 0)
+            return fail(KBA_ERR_BAD_ARG, who + (per_track ? track_prefix(true, i) : std::string()) + "kba_options.precision must be 0: evaluation is FP64 only");
+        if (!per_track) break;
+    }
+    bool any = false, large = false;
+    for (int i = 0; i < n; ++i) {
+        TrackRequest& q = qs[i];
+        if (!live(i)) { q.sel = nullptr; continue; }
+        std::string why;
+        int rc = track_check(s.tracks[i], q, why);
+        if (rc == KBA_OK && obs_arrays(out[i]) && out[i].obs_capacity < 0) { why = "negative obs_capacity"; rc = KBA_ERR_BAD_ARG; }
+        if (rc != KBA_OK) return fail(rc, who + track_prefix(group, i) + why);
+        any = true;
+        large |= q.rows > kFusedMaxRows;
+    }
+    if (!any) { s.last = &kNoTransfer; return KBA_OK; }
+    kba_handle* h = s.h;
+    CU(cudaSetDevice(h->device));
+    int rc = eval_stage(s, who);
+    if (rc != KBA_OK) return rc;
+    EvalStage& e = *s.eval;
+    TrackSolver& sv = large ? s.large : s.solver;
+    cudaStream_t st = h->stream;
+    // the windows' regions: observations bounded by the listed keyframes' measurements, the ground-plane lists by their request
+    size_t TO = 0, TL = 0, TG = 0, parts = 0;
+    int max_lm = 0;
+    for (int i = 0; i < n; ++i) {
+        const TrackRequest& q = qs[i];
+        EvalWin& ew = e.wins.h[i];
+        ew = EvalWin{};
+        ew.obs0 = (int)TO; ew.lm0 = (int)TL; ew.gp0 = (int)TG; ew.part0 = (int)parts;
+        if (!q.sel) continue;
+        ew.n_part = (q.n_lm + 63) / 64;
+        TO += (size_t)q.n_meas; TL += (size_t)q.n_lm; TG += (size_t)q.sel->n_gp; parts += (size_t)ew.n_part;
+        max_lm = std::max(max_lm, q.n_lm);
+    }
+    for (int i = 0; i < n; ++i) e.wins.h[i].n_lm_total = (int)TL;
+    const EvalLayout lay(n, TO, TL, TG);
+    StagedLists sl;
+    stage_requests(sv, n, s.tracks.data(), qs, sl);
+    rc = upload_and_gather(h, sv, per_track, opts, sl);
+    if (rc != KBA_OK) return rc;
+    CU(e.wins.upload(st));
+    launch_evaluate(sv.batch->bd, sv.batch->raw, e.wins.d, lay.view(e.out.d, e.part), max_lm, st);
+    CU(cudaGetLastError());
+    CU(cudaMemcpyAsync(e.out.h, e.out.d, lay.bytes, cudaMemcpyDeviceToHost, st));
+    CU(wait_stream(h));
+    e.counts.h2d = sl.h2d + (int64_t)(sizeof(EvalWin) * n);
+    e.counts.d2h = (int64_t)lay.bytes;
+    s.last = &e.counts;
+    // the results: a short observation capacity fails the call after every n_obs is written
+    const EvalOut o = lay.view(e.out.h, nullptr);
+    int short_at = -1;
+    for (int i = 0; i < n; ++i) {
+        if (!qs[i].sel) continue;
+        out[i].n_obs = o.head[i].n_obs;
+        if (short_at < 0 && obs_arrays(out[i]) && o.head[i].n_obs > out[i].obs_capacity) short_at = i;
+    }
+    if (short_at >= 0)
+        return fail(KBA_ERR_CAPACITY, who + track_prefix(group, short_at) + "the window has " + std::to_string(o.head[short_at].n_obs) +
+                                          " observations, more than obs_capacity = " + std::to_string(out[short_at].obs_capacity));
+    for (int i = 0; i < n; ++i) {
+        if (!qs[i].sel) continue;
+        const EvalWin& ew = e.wins.h[i];
+        const EvalHead& hd = o.head[i];
+        kba_evaluate_out& r = out[i];
+        const size_t no = (size_t)hd.n_obs, nl = (size_t)qs[i].n_lm, ng = (size_t)hd.n_gp;
+        r.n_gp = hd.n_gp; r.failed = hd.failed;
+        memcpy(r.cost, hd.cost, sizeof r.cost);
+        if (r.obs_lm) memcpy(r.obs_lm, o.obs_lm + ew.obs0, 4 * no);
+        if (r.obs_kf) memcpy(r.obs_kf, o.obs_kf + ew.obs0, 4 * no);
+        if (r.obs_cam) memcpy(r.obs_cam, o.obs_cam + ew.obs0, 4 * no);
+        if (r.residual) memcpy(r.residual, o.res + 3 * (size_t)ew.obs0, 24 * no);
+        if (r.rho) memcpy(r.rho, o.rho + 2 * (size_t)ew.obs0, 16 * no);
+        if (r.trim_repr) memcpy(r.trim_repr, o.trim + ew.lm0, 8 * nl);
+        if (r.trim_depth) memcpy(r.trim_depth, o.trim + TL + ew.lm0, 8 * nl);
+        if (r.rejected_repr) memcpy(r.rejected_repr, o.rej + ew.lm0, nl);
+        if (r.rejected_depth) memcpy(r.rejected_depth, o.rej + TL + ew.lm0, nl);
+        if (r.gp_lm) memcpy(r.gp_lm, o.gp_lm + ew.gp0, 4 * ng);
+        if (r.gp_kf) memcpy(r.gp_kf, o.gp_kf + ew.gp0, 4 * ng);
+        if (r.gp_weight) memcpy(r.gp_weight, o.gp_w + ew.gp0, 8 * ng);
+        if (r.gp_residual) memcpy(r.gp_residual, o.gp_r + ew.gp0, 8 * ng);
+    }
+    return KBA_OK;
+}
+
+int kba_track_evaluate(kba_track* t, const kba_track_request* req, const kba_options* opt, kba_evaluate_out* out) {
+    if (!t || !req || !opt || !out) return fail(KBA_ERR_BAD_ARG, "null argument to kba_track_evaluate");
+    TrackRequest q = track_request(req->n_kf, req->kf_slot, req->kf_fixed, req->n_lm, req->lm_slot, req->sel, false);
+    return set_evaluate(t->set, false, "kba_track_evaluate: ", &q, false, opt, out);
+}
+
+static int group_evaluate(kba_track_group* g, const kba_track_request* req, bool per_track, const kba_options* opts, kba_evaluate_out* out,
+                          const std::string& who) {
+    if (!g || !req || !opts || !out) return fail(KBA_ERR_BAD_ARG, "null argument to " + who.substr(0, who.size() - 2));
+    std::vector<TrackRequest> qs;
+    for (size_t i = 0; i < g->set.tracks.size(); ++i)
+        qs.push_back(track_request(req[i].n_kf, req[i].kf_slot, req[i].kf_fixed, req[i].n_lm, req[i].lm_slot, req[i].sel, false));
+    return set_evaluate(g->set, true, who, qs.data(), per_track, opts, out);
+}
+int kba_track_group_evaluate(kba_track_group* g, const kba_track_request* req, const kba_options* opt, kba_evaluate_out* out) {
+    return group_evaluate(g, req, false, opt, out, "kba_track_group_evaluate: ");
+}
+int kba_track_group_evaluate_opts(kba_track_group* g, const kba_track_request* req, const kba_options* opts, kba_evaluate_out* out) {
+    return group_evaluate(g, req, true, opts, out, "kba_track_group_evaluate_opts: ");
 }
 
 // ---------------------------------------------------------------------------------------------------------------------

@@ -420,17 +420,12 @@ __global__ void __launch_bounds__(256) k_gp_eval(BatchDev bd) {
         const double* ps = bd.pose[buf] + 7 * (size_t)(wd.kf_off + k);
         const double* pl = bd.plane[buf] + 4 * (size_t)(wd.kf_off + k);
         const double* p = bd.lm[buf] + 3 * (size_t)L;
-        double R[9];
-        quat_to_rot<double>(ps, R);
-        const double a[3] = {R[0] * p[0] + R[1] * p[1] + R[2] * p[2], R[3] * p[0] + R[4] * p[1] + R[5] * p[2],
-                             R[6] * p[0] + R[7] * p[1] + R[8] * p[2]};
-        const double px[3] = {a[0] + ps[4], a[1] + ps[5], a[2] + ps[6]};
+        double R[9], a[3], px[3];
+        const double r = gp_height(ps, pl, p, R, a, px);
         const double n[3] = {pl[0], pl[1], pl[2]};
-        const double r = n[0] * px[0] + n[1] * px[1] + n[2] * px[2] + pl[3];
-        const double s = r * r, ah = bd.wsp[w].gp_huber, wt = bd.gp_weight[G];
+        const double wt = bd.gp_weight[G];
         double rho, rho1;
-        if (s > ah * ah) { const double q = sqrt(s); rho = 2.0 * ah * q - ah * ah; rho1 = fmax(DBL_MIN, ah / q); }
-        else { rho = s; rho1 = 1.0; }
+        gp_huber(r * r, bd.wsp[w].gp_huber, rho, rho1);
         cost += 0.5 * wt * rho;
         if (kJac) {
             const double sq = sqrt(wt * rho1);
@@ -884,36 +879,6 @@ __global__ void __launch_bounds__(512, 1) k_schur_syrk_tma(BatchDev bd) {
 // =====================================================================================================================
 constexpr int kNB = 32;           // Cholesky block size
 constexpr int kPanelStride = 36;  // row stride of the shared-memory panel copy (row-major path)
-
-// PoseRegularization residual |(T1 T0^-1).t| - s0 with local Jacobians (reference cost_functors_ceres.hpp:224-250).
-__device__ void scale_regulariser(const double* p1, const double* p0, double s0, double& r, double* j1, double* j0) {
-    double R1[9], R0[9];
-    quat_to_rot<double>(p1, R1);
-    quat_to_rot<double>(p0, R0);
-    const double* t1 = p1 + 4, *t0 = p0 + 4;
-    double c[3], rc[3], d[3];
-    for (int i = 0; i < 3; ++i) c[i] = R0[i] * t0[0] + R0[3 + i] * t0[1] + R0[6 + i] * t0[2];          // R0^T t0
-    for (int i = 0; i < 3; ++i) rc[i] = R1[3 * i] * c[0] + R1[3 * i + 1] * c[1] + R1[3 * i + 2] * c[2];  // R1 c
-    for (int i = 0; i < 3; ++i) d[i] = t1[i] - rc[i];
-    const double nrm = sqrt(d[0] * d[0] + d[1] * d[1] + d[2] * d[2]);
-    r = nrm - s0;
-    if (!j1) return;
-    const double u[3] = {d[0] / nrm, d[1] / nrm, d[2] / nrm};
-    // dd/d(dr1) = 2 [R1 c]x -> u^T 2 [rc]x = 2 (u x rc)^T ... (u^T [a]x = (u x a)^T)
-    j1[0] = 2.0 * (u[1] * rc[2] - u[2] * rc[1]);
-    j1[1] = 2.0 * (u[2] * rc[0] - u[0] * rc[2]);
-    j1[2] = 2.0 * (u[0] * rc[1] - u[1] * rc[0]);
-    j1[3] = u[0]; j1[4] = u[1]; j1[5] = u[2];
-    // dd/d(dt0) = -R1 R0^T ;  dd/d(dr0) = -2 R1 R0^T [t0]x
-    double ur[3];  // u^T R1 R0^T  = (R0 R1^T u)^T
-    double tmp[3];
-    for (int i = 0; i < 3; ++i) tmp[i] = R1[i] * u[0] + R1[3 + i] * u[1] + R1[6 + i] * u[2];               // R1^T u
-    for (int i = 0; i < 3; ++i) ur[i] = R0[3 * i] * tmp[0] + R0[3 * i + 1] * tmp[1] + R0[3 * i + 2] * tmp[2];  // R0 R1^T u
-    j0[3] = -ur[0]; j0[4] = -ur[1]; j0[5] = -ur[2];
-    j0[0] = -2.0 * (ur[1] * t0[2] - ur[2] * t0[1]);
-    j0[1] = -2.0 * (ur[2] * t0[0] - ur[0] * t0[2]);
-    j0[2] = -2.0 * (ur[0] * t0[1] - ur[1] * t0[0]);
-}
 
 // Views of the reduced system: row-major in global memory (any size), or the lower triangle packed as 8x8 tiles in
 // shared memory (<= 192 rows).  Inside a tile the two 8x4 halves are stored one after the other, which is exactly the

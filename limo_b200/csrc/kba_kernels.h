@@ -379,6 +379,29 @@ struct RankGrid {
 void launch_rank_prepare(const RankLaunch& l, const RankGrid& g, cudaStream_t s);
 void launch_rank(const RankLaunch& l, const RankGrid& g, cudaStream_t s);
 
+// ---- evaluation of stored windows at the store's state (kba_track_evaluate / kba_track_group_evaluate, kba_evaluate.cu) ----
+// Run after launch_track_gather on the same batch, in place of the packing and the solve: the outputs of window w go to its
+// regions of one output block (EvalOut), in the window's own order, so that one copy brings every window's outputs down.
+struct EvalWin {                           // window w's regions, in entries of each array
+    int obs0;                              // observations: obs_*, res (3 per entry), rho (2 per entry)
+    int lm0;                               // landmarks: trim and rej, group g at g * n_lm_total + lm0
+    int gp0;                               // ground-plane residuals
+    int part0, n_part;                     // cost partials of k_ev_obs: one per 64 landmarks
+    int n_lm_total;                        // landmark entries of the whole block
+};
+struct EvalHead {                          // one window's record of the block, 64 bytes
+    int n_obs, n_gp, failed, pad;
+    double cost[6];                        // reprojection, depth, ground plane, scale regulariser, plane chain, total
+};
+struct EvalOut {
+    EvalHead* head;                        // [n_win]
+    double* res, *rho, *trim, *gp_w, *gp_r;
+    int* obs_lm, *obs_kf, *obs_cam, *gp_lm, *gp_kf;
+    unsigned char* rej;
+    double* part;                          // [3 * partials] scratch (not downloaded)
+};
+void launch_evaluate(const BatchDev& bd, const PackRaw& raw, const EvalWin* wins, const EvalOut& o, int max_lm, cudaStream_t s);
+
 // ---- motion-only frames against a track's store (kba_track_adjust_pose / kba_track_group_adjust_pose, kba_motion.cu) ----
 // One frame = one free pose against constant landmarks read from a store by slot: its measurements come in runs, one run per
 // landmark (the landmarks of the equivalent window, in the caller's order).

@@ -2,6 +2,8 @@
 // regularisation chain (reference bundle_adjuster_keyframes.cpp:769-818, cost_functors_ceres.hpp:394-438,507-555) and the
 // warp-cooperative accumulation of a small residual block into the reduced normal equations.
 #pragma once
+#include <cfloat>
+
 #include "kba_device.cuh"
 
 namespace kba {
@@ -67,6 +69,53 @@ __device__ inline double plane_motion(const double* p0, const double* p1, const 
         for (int j = 0; j < 3; ++j) jd[j] = u[0] * P[j] + u[1] * P[3 + j] + u[2] * P[6 + j];
     }
     return r;
+}
+
+// PoseRegularization residual |(T1 T0^-1).t| - s0 with local Jacobians (reference cost_functors_ceres.hpp:224-250).
+__device__ inline void scale_regulariser(const double* p1, const double* p0, double s0, double& r, double* j1, double* j0) {
+    double R1[9], R0[9];
+    quat_to_rot<double>(p1, R1);
+    quat_to_rot<double>(p0, R0);
+    const double* t1 = p1 + 4, *t0 = p0 + 4;
+    double c[3], rc[3], d[3];
+    for (int i = 0; i < 3; ++i) c[i] = R0[i] * t0[0] + R0[3 + i] * t0[1] + R0[6 + i] * t0[2];          // R0^T t0
+    for (int i = 0; i < 3; ++i) rc[i] = R1[3 * i] * c[0] + R1[3 * i + 1] * c[1] + R1[3 * i + 2] * c[2];  // R1 c
+    for (int i = 0; i < 3; ++i) d[i] = t1[i] - rc[i];
+    const double nrm = sqrt(d[0] * d[0] + d[1] * d[1] + d[2] * d[2]);
+    r = nrm - s0;
+    if (!j1) return;
+    const double u[3] = {d[0] / nrm, d[1] / nrm, d[2] / nrm};
+    // dd/d(dr1) = 2 [R1 c]x -> u^T 2 [rc]x = 2 (u x rc)^T ... (u^T [a]x = (u x a)^T)
+    j1[0] = 2.0 * (u[1] * rc[2] - u[2] * rc[1]);
+    j1[1] = 2.0 * (u[2] * rc[0] - u[0] * rc[2]);
+    j1[2] = 2.0 * (u[0] * rc[1] - u[1] * rc[0]);
+    j1[3] = u[0]; j1[4] = u[1]; j1[5] = u[2];
+    // dd/d(dt0) = -R1 R0^T ;  dd/d(dr0) = -2 R1 R0^T [t0]x
+    double ur[3];  // u^T R1 R0^T  = (R0 R1^T u)^T
+    double tmp[3];
+    for (int i = 0; i < 3; ++i) tmp[i] = R1[i] * u[0] + R1[3 + i] * u[1] + R1[6 + i] * u[2];               // R1^T u
+    for (int i = 0; i < 3; ++i) ur[i] = R0[3 * i] * tmp[0] + R0[3 * i + 1] * tmp[1] + R0[3 * i + 2] * tmp[2];  // R0 R1^T u
+    j0[3] = -ur[0]; j0[4] = -ur[1]; j0[5] = -ur[2];
+    j0[0] = -2.0 * (ur[1] * t0[2] - ur[2] * t0[1]);
+    j0[1] = -2.0 * (ur[2] * t0[0] - ur[0] * t0[2]);
+    j0[2] = -2.0 * (ur[0] * t0[1] - ur[1] * t0[0]);
+}
+
+// Ground-plane height residual r = n . (R(q) p + t) + dist of landmark p against keyframe pose ps (7-vector) and plane pl
+// (reference cost_functors_ceres.hpp:355-392); R, a = R p and px = a + t are kept for the Jacobian.
+__device__ inline double gp_height(const double* ps, const double* pl, const double* p, double R[9], double a[3], double px[3]) {
+    quat_to_rot<double>(ps, R);
+    a[0] = R[0] * p[0] + R[1] * p[1] + R[2] * p[2];
+    a[1] = R[3] * p[0] + R[4] * p[1] + R[5] * p[2];
+    a[2] = R[6] * p[0] + R[7] * p[1] + R[8] * p[2];
+    px[0] = a[0] + ps[4]; px[1] = a[1] + ps[5]; px[2] = a[2] + ps[6];
+    return pl[0] * px[0] + pl[1] * px[1] + pl[2] * px[2] + pl[3];
+}
+
+// HuberLoss(ah) of a squared residual s (bundle_adjuster_keyframes.cpp:549): rho and rho'
+__device__ inline void gp_huber(double s, double ah, double& rho, double& rho1) {
+    if (s > ah * ah) { const double q = sqrt(s); rho = 2.0 * ah * q - ah * ah; rho1 = fmax(DBL_MIN, ah / q); }
+    else { rho = s; rho1 = 1.0; }
 }
 
 // SpeedRegularizationVector2 (reference cost_functors_ceres.hpp:300-353): r = (R t_ob + t) / dt - v_before on one pose p;
