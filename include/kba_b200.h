@@ -1003,6 +1003,114 @@ int kba_track_group_solve_ranked(kba_track_group* g, const kba_ranked_request* r
 /* kba_track_group_solve_ranked with opts[n_tracks], one per track, as kba_track_group_solve_opts takes them */
 int kba_track_group_solve_ranked_opts(kba_track_group* g, const kba_ranked_request* req, const kba_options* opts, kba_result* res);
 
+/* ---- limo's solve block as one call: deactivateKeyframes, updateLabels and the ranked solve ---------------------------------
+ * What limo runs once it decides to solve (mono_lidar.cpp:249-255, mono_standalone.cpp:171-183):
+ *     deactivateKeyframes(min_connecting, min_window, max_window); updateLabels(tracklets, shrubbery_weight); solve();
+ * on the stored window, with its results equal, bit for bit, to those of the chain of store calls a caller runs today:
+ *   1. kba_track_deactivate_keyframes on kf_slot / lm_slot (the request's first six fields mean what kba_deactivate_request's do);
+ *   2. the post-deactivation lists: the keyframes with kf_active = 1 and the landmarks with lm_active = 1, order kept; the oldest
+ *      kept keyframe gets FixationStatus::Pose (bundle_adjuster_keyframes.cpp:980; Scale has no effect on the solve, cpp:736),
+ *      every other one is free;
+ *   3. updateLabels (cpp:388-431, facade/bundle_adjuster_keyframes.cpp) over the tracklets, each (landmark slot, label,
+ *      is_outlier), slot -1 for an id without one, and the class table (label, classes) of labels_ (an unlisted label has none):
+ *        - the new outlier set: the caller's outliers (outlier_slot) that are still active, plus every tracklet with is_outlier
+ *          set or a label of class KBA_LABEL_OUTLIER;
+ *        - a tracklet whose landmark is still active: a shrubbery label writes shrubbery_weight into the store's weight of its
+ *          slot; its ground flag becomes (label of class KBA_LABEL_GROUND), the last tracklet of a slot deciding.  The other
+ *          listed landmarks keep the flag the caller gives in lm_ground (NULL: none is ground);
+ *   4. kba_track_rank_landmarks on the post-deactivation keyframes and the candidates -- the still-active landmarks that are not
+ *      in the new outlier set, in lm_slot order -- with elig = the candidates' ground flags (limo's AddDepth comparator,
+ *      is_ground_plane), and params, the caps, the AddDepth entries and the draw function as kba_rank_request takes them;
+ *   5. kba_track_solve_ranked on the post-deactivation keyframes and their fixation with `sel` (its scalars and ground mode, as
+ *      that call takes them; scale_kf0 / scale_kf1 index the post-deactivation keyframes; n_kf / n_lm are not read).
+ * Outputs (caller-owned; cand / category and the result's landmark arrays sized for n_lm, its keyframe arrays for n_kf):
+ *   - kf_active, kf_common [n_kf], lm_active [n_lm]: as the deactivation writes them;
+ *   - lm_outlier [n_lm], trk_outlier [n_trk]: the new outlier set over the listed landmarks and over the tracklets (a tracklet is
+ *     flagged iff its landmark is in the set); lm_ground [n_lm]: the listed landmarks' ground flags after the labels;
+ *   - rank: n_sel, cand (indices into the candidates of step 4), category, n_ground, n_draws, as the ranking writes them;
+ *   - res: the ranked solve's kba_result (keyframe arrays in post-deactivation order, landmark arrays in ranked order).
+ * With these a caller keeps its bookkeeping (active_keyframe_ids_, the outlier set, selected_landmark_ids_) as after the chain.
+ * On the device: one upload (the lists, the tracklets' classes, the AddDepth entries and every window's argument records) and ONE
+ * launch sequence run the deactivation (k_up_*), updateLabels and the post-deactivation lists (k_kfs_labels, which also writes
+ * the ranking records' sizes) and the ranking's first part (k_sel_*, k_rk_prep, k_rk_depth), then one download brings back the
+ * deactivation's and the labels' outputs, the kept keyframes and the middle bins' sizes.  The host then checks the ranking and
+ * the solve on the kept keyframes, calls the draw functions, uploads the draws and runs the ranking's second part (k_rk_heap,
+ * k_rk_union; one download), and launches k_kfs_weights (the shrubbery weights) ahead of the ranked solve.
+ * Checks: every check that needs only the request runs before anything is uploaded: those of the deactivation, the tracklets'
+ * slots in [-1, max_landmarks), the outlier slots in range, the ranking's parameters, caps and AddDepth entries, n_lm <= 57344
+ * (the ranking's candidate bound: the candidates are a subset of the listed landmarks), the options.  The checks on the kept
+ * keyframes (none kept: KBA_ERR_BAD_ARG; those of kba_track_solve; an AddDepth heap over 57344) and a failing or missing draw
+ * function refuse the call after the first download, the ranked solve's checks after the second, all with the codes and
+ * messages of the underlying calls and before the store is written: a refused call writes no output and leaves every store's
+ * content (its snapshot) as it was.  Its rankings do not survive it: a call refused before the ranking's second part leaves the
+ * tracks it ran for without a ranking (kba_track_solve_ranked refuses to solve), one refused by the ranked solve's checks
+ * leaves them this call's ranking.  The shrubbery weights go into the store after the ranking (which does not read weights, so
+ * it stays valid) and before the solve.
+ * Transfers (kba_track_transfer_bytes / kba_track_group_transfer_bytes), over the W requests that do not sit out, R the size of
+ * one window's argument records (a constant of the library build), D_w the draws and B_w the selection bound of request w as
+ * kba_track_rank_landmarks states them, each request's arrays padded to 8-byte boundaries:
+ *         h2d = R * W + sum(8 n_depth + 4 (n_kf + n_lm + n_outlier + n_trk) + n_lm + n_trk) + 8 W + 4 sum(D_w) + the solve's
+ *         d2h = 4 W + sum(8 + 9 n_kf + 3 n_lm + n_trk) + 8 W + 5 sum(B_w) + the solve's
+ * where the solve's are kba_track_solve_ranked's (kba_track_group_solve_ranked's).  Allocations: each track's label scratch
+ * (8 bytes per landmark slot) and the scratch of the selection, ranking and upkeep calls at their first use by any entry point;
+ * the call's staging grows to its largest call: a call no larger than an earlier one allocates nothing on the device.
+ * The group forms serve one request per track (req[n_tracks], out[n_tracks], res[n_tracks]), each step for all tracks at once as
+ * the step's group call does it: a request with n_kf == 0 sits the call out (its outputs are not written, res[i] is idle as for
+ * kba_track_group_solve); a failing request returns its code and kba_last_error names its track; _opts takes one kba_options per
+ * track.  A single call is the group call's one-track case. */
+#define KBA_LABEL_OUTLIER 1
+#define KBA_LABEL_SHRUBBERY 2
+#define KBA_LABEL_GROUND 4
+typedef struct kba_label_class {
+    int32_t label;
+    int32_t classes;            /* KBA_LABEL_* bits                                                                           */
+} kba_label_class;
+typedef struct kba_tracklet {
+    int32_t lm_slot;            /* -1: the landmark id has no slot                                                             */
+    int32_t label;
+    uint8_t is_outlier;
+    uint8_t reserved_[3];
+} kba_tracklet;
+typedef struct kba_kfsolve_request {
+    int32_t n_kf;               /* 0 (group call): this track sits the call out                                               */
+    int32_t n_lm;
+    int32_t min_connecting, min_window, max_window;
+    int32_t n_trk;
+    const int32_t* kf_slot;     /* [n_kf] the active keyframes in ascending id order; the last one is the newest             */
+    const int32_t* lm_slot;     /* [n_lm] the active landmarks in ascending id order                                          */
+    const uint8_t* lm_ground;   /* [n_lm] is_ground_plane of the listed landmarks before the call, or NULL (none)             */
+    const kba_tracklet* trk;    /* [n_trk] the current frame's tracklets                                                      */
+    const kba_label_class* classes;  /* [n_class] */
+    int32_t n_class;
+    int32_t n_outlier;
+    const int32_t* outlier_slot;     /* [n_outlier] the caller's current outlier set (landmark_selector_->getOutliers())       */
+    double shrubbery_weight;
+    const kba_select_params* params; /* the ranking, as kba_rank_request                                                       */
+    int32_t max_near, max_middle, max_far;
+    int32_t n_depth;
+    const kba_depth_entry* depth;
+    int32_t (*draw)(void* ctx, int32_t n, int32_t* out);
+    void* draw_ctx;
+    const kba_window* sel;      /* the solve's scalars and ground mode, as kba_track_solve_ranked takes them                    */
+} kba_kfsolve_request;
+typedef struct kba_kfsolve_out {  /* caller-owned */
+    uint8_t* kf_active;         /* [n_kf] */
+    int32_t* kf_common;         /* [n_kf] */
+    uint8_t* lm_active;         /* [n_lm] */
+    uint8_t* lm_outlier;        /* [n_lm] */
+    uint8_t* lm_ground;         /* [n_lm] */
+    uint8_t* trk_outlier;       /* [n_trk] */
+    kba_rank_out rank;          /* cand, category: [n_lm] */
+} kba_kfsolve_out;
+int kba_track_keyframe_solve(kba_track* t, const kba_kfsolve_request* req, const kba_options* opt, kba_kfsolve_out* out,
+                             kba_result* res);
+/* req[n_tracks], out[n_tracks], res[n_tracks] */
+int kba_track_group_keyframe_solve(kba_track_group* g, const kba_kfsolve_request* req, const kba_options* opt, kba_kfsolve_out* out,
+                                   kba_result* res);
+/* opts[n_tracks]: track i's solve runs with opts[i]; a track that sits out does not read its entry */
+int kba_track_group_keyframe_solve_opts(kba_track_group* g, const kba_kfsolve_request* req, const kba_options* opts,
+                                        kba_kfsolve_out* out, kba_result* res);
+
 /* ---- adjustPoseOnly against the persistent store: one frame's pose per call, or one frame of each track of a group -------
  * What limo calls on every frame (bundle_adjuster_keyframes.cpp:820-888): one free pose against constant landmarks, the optional
  * SpeedRegularizationVector2 prior and the trimming rounds.  The result is that of kba_solve_window on the equivalent window: one

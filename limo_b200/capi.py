@@ -10,7 +10,7 @@ import os
 
 import numpy as np
 
-from .capi_types import (KbaCounters, KbaCreateOut, KbaCreateRequest, KbaDeactivateOut, KbaDeactivateRequest, KbaDepthEntry, KbaDepthOut, KbaDepthRequest, KbaDrawFn, KbaEvalOut, KbaEvaluateOut, KbaFlowOut, KbaFlowRequest, KbaLandmarkWrite, KbaLidarCloud, KbaLidarOptions, KbaLidarView, KbaOptions, KbaPoseWrite, KbaPushRequest, KbaRankedRequest, KbaRankOut, KbaRankRequest, KbaReclaimOut, KbaReclaimRequest, KbaResult, KbaSelectOut, KbaSelectParams, KbaSelectRequest,
+from .capi_types import (KbaCounters, KbaCreateOut, KbaCreateRequest, KbaDeactivateOut, KbaDeactivateRequest, KbaDepthEntry, KbaDepthOut, KbaDepthRequest, KbaDrawFn, KbaEvalOut, KbaEvaluateOut, KbaFlowOut, KbaFlowRequest, KbaKfsolveOut, KbaKfsolveRequest, KbaLabelClass, KbaLandmarkWrite, KbaLidarCloud, KbaLidarOptions, KbaLidarView, KbaOptions, KbaPoseWrite, KbaPushRequest, KbaRankedRequest, KbaRankOut, KbaRankRequest, KbaReclaimOut, KbaReclaimRequest, KbaResult, KbaSelectOut, KbaSelectParams, KbaSelectRequest, KbaTracklet,
                          KbaSnapshotHeader, KbaTrackCaps, KbaTrackFrame, KbaTrackRequest, KbaWindow, Result, Window, c_double_p, c_float_p, c_int32_p,
                          c_uint8_p)
 
@@ -37,7 +37,8 @@ SYMBOLS = ["kba_version", "kba_last_error", "kba_default_options", "kba_create",
            "kba_track_group_set_landmarks", "kba_track_group_set_keyframe_poses", "kba_lidar_depth_batch",
            "kba_lidar_depth_batch_opts", "kba_track_snapshot_size", "kba_track_save", "kba_track_load", "kba_track_clone",
            "kba_track_group_snapshot_sizes", "kba_track_group_save", "kba_track_evaluate", "kba_track_group_evaluate",
-           "kba_track_group_evaluate_opts"]
+           "kba_track_group_evaluate_opts", "kba_track_keyframe_solve", "kba_track_group_keyframe_solve",
+           "kba_track_group_keyframe_solve_opts"]
 
 
 class KbaError(RuntimeError):
@@ -176,6 +177,8 @@ def lib():
         L.kba_track_evaluate.argtypes = [vp, C.POINTER(KbaTrackRequest), C.POINTER(KbaOptions), C.POINTER(KbaEvaluateOut)]
         for f in (L.kba_track_group_evaluate, L.kba_track_group_evaluate_opts):
             f.argtypes = [vp, C.POINTER(KbaTrackRequest), C.POINTER(KbaOptions), C.POINTER(KbaEvaluateOut)]
+        for f in (L.kba_track_keyframe_solve, L.kba_track_group_keyframe_solve, L.kba_track_group_keyframe_solve_opts):
+            f.argtypes = [vp, C.POINTER(KbaKfsolveRequest), C.POINTER(KbaOptions), C.POINTER(KbaKfsolveOut), C.POINTER(KbaResult)]
         L.kba_lidar_default_options.argtypes = [C.POINTER(KbaLidarOptions)]
         L.kba_lidar_default_options.restype = None
         fp = C.POINTER(C.c_float)
@@ -671,6 +674,70 @@ class Track:
                                             C.byref(opt or default_options()), C.byref(o)))
         return done(o)
 
+    def _keyframe_solve_request(self, capacity, kf_slots, lm_slots, min_connecting=3, min_window=4, max_window=20, lm_ground=None,
+                                tracklets=(), label_classes=None, outliers=(), shrubbery_weight=1.0, voxel_size=SELECT_DEFAULTS["voxel_size"],
+                                roi_far=SELECT_DEFAULTS["roi_far"], roi_middle=SELECT_DEFAULTS["roi_middle"], max_near=RANK_DEFAULTS["max_near"],
+                                max_middle=RANK_DEFAULTS["max_middle"], max_far=RANK_DEFAULTS["max_far"], depth=(), draws=None, ground=False,
+                                **scalars):
+        """the deactivation's lists, updateLabels' inputs, the ranking's and the solve's keywords.  Returns a builder's four values
+        and the KbaResult the call fills (the call has two outputs); the result function takes a group call's filled KbaResult as
+        its second argument and keeps the size of the ranking for solve_ranked."""
+        kf, lm, prm = _select_args(kf_slots, lm_slots, voxel_size, roi_far, roi_middle)
+        K, L = len(kf), len(lm)
+        gr = _arr(lm_ground, np.uint8, L)
+        # a kba_tracklet is three little-endian int32 words: slot, label, is_outlier (the byte) with its three zero bytes
+        trk = np.ascontiguousarray(np.asarray(tracklets, dtype=np.int64).reshape(-1, 3).astype(np.int32))
+        if trk.size and (trk[:, 2].min() < 0 or trk[:, 2].max() > 1):
+            raise ValueError("tracklet is_outlier must be 0 or 1")
+        cls = np.ascontiguousarray(np.array(sorted((label_classes or {}).items()), dtype=np.int32).reshape(-1, 2))
+        out_slots = _arr(outliers, np.int32, -1)
+        dp = np.ascontiguousarray(np.asarray(depth, dtype=np.int32).reshape(-1, 2))
+        fn = _draw_source(draws)
+        sel = _sel_window(K, L, **scalars)
+        if ground:  # the ranking's ground candidates, attached on the device: n_gp > 0 with no lists
+            sel.c.n_gp = 1
+        res = Result(sel, capacity)
+        bufs = dict(kf_active=np.zeros(K, np.uint8), kf_common=np.zeros(K, np.int32), lm_active=np.zeros(L, np.uint8),
+                    lm_outlier=np.zeros(L, np.uint8), lm_ground=np.zeros(L, np.uint8), trk_outlier=np.zeros(len(trk), np.uint8),
+                    cand=np.zeros(L, np.int32), category=np.zeros(L, np.int8))
+        q = KbaKfsolveRequest(n_kf=K, n_lm=L, min_connecting=int(min_connecting), min_window=int(min_window), max_window=int(max_window),
+                              n_trk=len(trk), kf_slot=_p(kf, c_int32_p), lm_slot=_p(lm, c_int32_p), lm_ground=_p(gr, c_uint8_p),
+                              trk=_p(trk, C.POINTER(KbaTracklet)), classes=_p(cls, C.POINTER(KbaLabelClass)), n_class=len(cls),
+                              n_outlier=len(out_slots), outlier_slot=_p(out_slots, c_int32_p), shrubbery_weight=float(shrubbery_weight),
+                              params=prm.ctypes.data, max_near=int(max_near), max_middle=int(max_middle), max_far=int(max_far),
+                              n_depth=len(dp), depth=_p(dp, _depth_p), draw=fn, sel=C.addressof(sel.c))
+        o = KbaKfsolveOut(kf_active=_p(bufs["kf_active"], c_uint8_p), kf_common=_p(bufs["kf_common"], c_int32_p),
+                          lm_active=_p(bufs["lm_active"], c_uint8_p), lm_outlier=_p(bufs["lm_outlier"], c_uint8_p),
+                          lm_ground=_p(bufs["lm_ground"], c_uint8_p), trk_outlier=_p(bufs["trk_outlier"], c_uint8_p),
+                          rank=KbaRankOut(cand=_p(bufs["cand"], c_int32_p), category=_p(bufs["category"], _c_int8_p)))
+
+        def done(o, c=None):  # c: the KbaResult a group call filled (a single call fills res.c itself)
+            r = o.rank
+            self._n_sel = r.n_sel
+            if c is not None:
+                res.c = c
+            n_kept = int(bufs["kf_active"].sum())
+            res.kf_pose, res.kf_plane = res.kf_pose[:n_kept], res.kf_plane[:n_kept]
+            res.lm_pos, res.lm_rejected, res.n_lm = res.lm_pos[:max(r.n_sel, 1)], res.lm_rejected[:max(r.n_sel, 1)], r.n_sel
+            out = {k: bufs[k] for k in ("kf_active", "kf_common", "lm_active", "lm_outlier", "lm_ground", "trk_outlier")}
+            out.update(cand=bufs["cand"][:r.n_sel].copy(), category=bufs["category"][:r.n_sel].copy(), n_ground=r.n_ground,
+                       n_draws=r.n_draws, result=res)
+            return out
+        return q, o, (*bufs.values(), kf, lm, gr, trk, cls, out_slots, dp, prm, fn, sel, res), done, res.c
+
+    def keyframe_solve(self, kf_slots, lm_slots, opt=None, iterations_capacity=256, **kw):
+        """limo's solve block -- deactivateKeyframes, updateLabels and solve() -- as one call (kba_track_keyframe_solve): kf_slots /
+        lm_slots the active keyframes and landmarks in ascending id order with the keywords of deactivate_keyframes; lm_ground
+        [n_lm] the landmarks' ground flags before the call (None: none); tracklets [(slot or -1, label, is_outlier)];
+        label_classes {label: LABEL_* bits}; outliers: the current outlier set's slots; shrubbery_weight; the ranking's keywords
+        of rank_landmarks (without lists or elig); ground and the scalar keywords of solve_ranked.  Returns one dict: the
+        deactivation's kf_active, kf_common, lm_active; lm_outlier, lm_ground, trk_outlier after the labels; the ranking's cand
+        (indices into the still-active, non-outlier landmarks in list order), category, n_ground, n_draws; and result, the ranked
+        solve's Result (keyframe arrays for the kept keyframes, landmark arrays in ranked order)."""
+        q, o, _keep, done, rc = self._keyframe_solve_request(iterations_capacity, kf_slots, lm_slots, **kw)
+        _check(lib().kba_track_keyframe_solve(self._p, C.byref(q), C.byref(opt or default_options()), C.byref(o), C.byref(rc)))
+        return done(o)
+
     def transfer_bytes(self):
         a, b, c = C.c_int64(), C.c_int64(), C.c_int64()
         _check(lib().kba_track_transfer_bytes(self._p, C.byref(a), C.byref(b), C.byref(c)))
@@ -895,6 +962,32 @@ class TrackGroup:
         fn, o = _options(opt, len(self.tracks), lib().kba_track_group_solve_ranked, lib().kba_track_group_solve_ranked_opts)
         return self._call(fn, requests, lambda t, **r: t._ranked_request(iterations_capacity, **r), KbaRankedRequest, KbaResult,
                           idle=lambda: _idle(KbaRankedRequest, 0), opt=(o,))
+
+    def keyframe_solve(self, requests, opt=None, iterations_capacity=256):
+        """limo's solve block for every track (kba_track_group_keyframe_solve): each entry None (the track sits the call out) or
+        a dict with the arguments of Track.keyframe_solve.  opt: one KbaOptions, or one per track
+        (kba_track_group_keyframe_solve_opts).  Returns one result dict per track (Track.keyframe_solve's), None for a track that
+        sat out."""
+        # Not _call: the call has two output arrays, the dicts and the solve results
+        n = len(self.tracks)
+        assert len(requests) == n
+        fn, o = _options(opt, n, lib().kba_track_group_keyframe_solve, lib().kba_track_group_keyframe_solve_opts)
+        reqs, outs, ress = (KbaKfsolveRequest * n)(), (KbaKfsolveOut * n)(), (KbaResult * n)()
+        keep, done = [], []
+        for i, r in enumerate(requests):
+            if r is None:
+                continue
+            q, ob, k, d, rc = _built(fn, i, r, lambda t, **kw: t._keyframe_solve_request(iterations_capacity, **kw), self.tracks[i])
+            if _no_keyframes(q):
+                raise KbaError("%s: track %d: no keyframes or a negative size" % (fn.__name__, i))
+            reqs[i], outs[i], ress[i] = q, ob, rc
+            keep.append(k)
+            done.append((i, d))
+        _check(fn(self._p, reqs, o, outs, ress))
+        results = [None] * n
+        for i, d in done:
+            results[i] = d(outs[i], ress[i])
+        return results
 
     def push_keyframes(self, requests):
         """one keyframe into every track's store in one call (kba_track_group_push_keyframes): each entry None (the track sits the

@@ -223,6 +223,32 @@ class KbaRankedRequest(C.Structure):
     _fields_ = [("n_kf", C.c_int32), ("reserved_", C.c_int32), ("kf_slot", c_int32_p), ("kf_fixed", c_uint8_p), ("sel", C.c_void_p)]
 
 
+# kba_label_class.classes bits
+LABEL_OUTLIER, LABEL_SHRUBBERY, LABEL_GROUND = 1, 2, 4
+
+
+class KbaLabelClass(C.Structure):
+    _fields_ = [("label", C.c_int32), ("classes", C.c_int32)]
+
+
+class KbaTracklet(C.Structure):
+    _fields_ = [("lm_slot", C.c_int32), ("label", C.c_int32), ("is_outlier", C.c_uint8), ("reserved_", C.c_uint8 * 3)]
+
+
+class KbaKfsolveRequest(C.Structure):
+    _fields_ = [("n_kf", C.c_int32), ("n_lm", C.c_int32), ("min_connecting", C.c_int32), ("min_window", C.c_int32),
+                ("max_window", C.c_int32), ("n_trk", C.c_int32), ("kf_slot", c_int32_p), ("lm_slot", c_int32_p), ("lm_ground", c_uint8_p),
+                ("trk", C.POINTER(KbaTracklet)), ("classes", C.POINTER(KbaLabelClass)), ("n_class", C.c_int32), ("n_outlier", C.c_int32),
+                ("outlier_slot", c_int32_p), ("shrubbery_weight", C.c_double), ("params", C.c_void_p), ("max_near", C.c_int32),
+                ("max_middle", C.c_int32), ("max_far", C.c_int32), ("n_depth", C.c_int32), ("depth", C.POINTER(KbaDepthEntry)),
+                ("draw", KbaDrawFn), ("draw_ctx", C.c_void_p), ("sel", C.c_void_p)]
+
+
+class KbaKfsolveOut(C.Structure):
+    _fields_ = [("kf_active", c_uint8_p), ("kf_common", c_int32_p), ("lm_active", c_uint8_p), ("lm_outlier", c_uint8_p),
+                ("lm_ground", c_uint8_p), ("trk_outlier", c_uint8_p), ("rank", KbaRankOut)]
+
+
 class KbaTrackFrame(C.Structure):
     _fields_ = [("n_meas", C.c_int32), ("reserved_", C.c_int32), ("pose7", c_double_p), ("lm_slot", c_int32_p), ("cam", c_int32_p),
                 ("u", c_float_p), ("v", c_float_p), ("d", c_float_p), ("speed_weight", C.c_double), ("speed_dt", C.c_double),

@@ -311,6 +311,13 @@ struct RankBufs {
     DevAllocs dev;
 };
 
+// a track's label scratch (k_kfs_labels), allocated at its first keyframe solve, alone or in a group
+struct KfsBufs {
+    int* lm_at = nullptr;                  // [lm_cap] -1 between calls
+    int* last = nullptr;                   // [lm_cap]
+    DevAllocs dev;
+};
+
 // the duplicate checks of a track's slot lists (check_slot_lists, flow_check, frame_check): the check that named a slot last
 struct SlotStamps {
     std::vector<unsigned> kf, lm;          // [kf_cap], [lm_cap]
@@ -323,7 +330,7 @@ struct SlotStamps {
 // the store calls that stage their requests, one staging each; deactivation and depth costs share the upkeep one, a drop shares
 // the push's
 enum StoreCall { kSelectCall, kCreateCall, kUpkeepCall, kFlowCall, kReclaimCall, kRankCall, kPushCall, kLandmarkWriteCall, kPoseWriteCall,
-                 kSnapshotCall, kStoreCalls };
+                 kSnapshotCall, kKfSolveCall, kStoreCalls };
 
 struct EvalStage;
 
@@ -362,6 +369,7 @@ struct kba_track {
     std::unique_ptr<CreateBufs> create;    // landmark creations, allocated at the first one
     std::unique_ptr<UpkeepBufs> upkeep;    // upkeep, flow and reclaim calls, allocated at the first of them
     std::unique_ptr<RankBufs> rank;        // rankings, allocated at the first one
+    std::unique_ptr<KfsBufs> kfs;          // keyframe solves' label scratch, allocated at the first one
     SlotStamps stamps;
     uint64_t gen = 0;                      // counts the calls that changed the store: a ranking of an older generation is stale
     TrackDev td{};
@@ -3355,17 +3363,24 @@ struct RankReq {
     SelectReq s;                           // the selection chain of the same lists
 };
 
+// the checks of a ranking's caps, candidate count and AddDepth entries
+static int rank_entries_check(int n_cand, int max_near, int max_middle, int max_far, int n_depth, const kba_depth_entry* depth,
+                              std::string& why) {
+    if (n_depth > 0 && !depth) { why = "null argument"; return KBA_ERR_BAD_ARG; }
+    if (max_near < 0 || max_middle < 0 || max_far < 0 || n_depth < 0) { why = "a negative cap or size"; return KBA_ERR_BAD_ARG; }
+    for (int e = 0; e < n_depth; ++e)
+        if (depth[e].ind < 0 || depth[e].wanted < 0) { why = "an AddDepth entry with a negative index or count"; return KBA_ERR_BAD_ARG; }
+    if (n_cand > kRankMaxCand) { why = "more than 57344 candidates"; return KBA_ERR_CAPACITY; }
+    if (n_depth > kRankMaxDepth) { why = "more than 1024 AddDepth entries"; return KBA_ERR_CAPACITY; }
+    return KBA_OK;
+}
+
 // every check of one request, before anything is uploaded; allocates the track's selection and ranking buffers at its first call
 static int rank_check(RankReq& r, std::string& why) {
     const kba_rank_request* q = r.q;
-    if (!r.o || (q->n_cand > 0 && (!r.o->cand || !r.o->category)) || (q->n_depth > 0 && !q->depth)) {
-        why = "null argument"; return KBA_ERR_BAD_ARG;
-    }
-    if (q->max_near < 0 || q->max_middle < 0 || q->max_far < 0 || q->n_depth < 0) { why = "a negative cap or size"; return KBA_ERR_BAD_ARG; }
-    for (int e = 0; e < q->n_depth; ++e)
-        if (q->depth[e].ind < 0 || q->depth[e].wanted < 0) { why = "an AddDepth entry with a negative index or count"; return KBA_ERR_BAD_ARG; }
-    if (q->n_cand > kRankMaxCand) { why = "more than 57344 candidates"; return KBA_ERR_CAPACITY; }
-    if (q->n_depth > kRankMaxDepth) { why = "more than 1024 AddDepth entries"; return KBA_ERR_CAPACITY; }
+    if (!r.o || (q->n_cand > 0 && (!r.o->cand || !r.o->category))) { why = "null argument"; return KBA_ERR_BAD_ARG; }
+    const int ec = rank_entries_check(q->n_cand, q->max_near, q->max_middle, q->max_far, q->n_depth, q->depth, why);
+    if (ec != KBA_OK) return ec;
     SelectReq& s = r.s;
     s.t = r.t; s.n_kf = q->n_kf; s.n_cand = q->n_cand; s.kf_slot = q->kf_slot; s.lm_slot = q->lm_slot; s.p = q->params;
     s.quantities_only = true;
@@ -3960,6 +3975,396 @@ int kba_track_group_set_keyframe_poses(kba_track_group* g, const kba_pose_write*
     return store_call<PoseWrite>(g->set, true, who, req, nullptr);
 }
 
+// ---------------------------------------------------------------------------------------------------------------------
+// limo's solve block as one call (include/kba_b200.h, kba_track_keyframe_solve and its group forms; kernels in kba_upkeep.cu,
+// kba_kfsolve.cu, kba_select.cu, kba_rank.cu).  One upload and one launch sequence run the deactivation, updateLabels and the
+// post-deactivation lists (k_kfs_labels) and the ranking's first part for every window; one download brings back what the host
+// needs next: the draws' counts, the kept keyframes, and the outputs.  Then the draws, the ranking's second part, the shrubbery
+// weights (k_kfs_weights) and the ranked solve.  Every output is staged here and written when the call succeeds.
+// ---------------------------------------------------------------------------------------------------------------------
+// the KBA_LABEL_* classes of a label in the request's class table
+static int label_classes(const kba_kfsolve_request& q, int32_t label) {
+    int c = 0;
+    for (int i = 0; i < q.n_class; ++i)
+        if (q.classes[i].label == label) c |= q.classes[i].classes;
+    return c;
+}
+
+// the checks that need only the request and are not the deactivation's (upkeep_check)
+static int kfsolve_check(const kba_track* t, const kba_kfsolve_request& q, const kba_kfsolve_out* o, std::string& why) {
+    if (!o || !q.sel || !q.params || !o->kf_active || !o->kf_common || (q.n_trk > 0 && (!q.trk || !o->trk_outlier)) ||
+        (q.n_class > 0 && !q.classes) || (q.n_outlier > 0 && !q.outlier_slot) ||
+        (q.n_lm > 0 && (!o->lm_active || !o->lm_outlier || !o->lm_ground || !o->rank.cand || !o->rank.category))) {
+        why = "null argument"; return KBA_ERR_BAD_ARG;
+    }
+    if (q.n_trk < 0 || q.n_class < 0 || q.n_outlier < 0) { why = "a negative size"; return KBA_ERR_BAD_ARG; }
+    for (int i = 0; i < q.n_trk; ++i)
+        if (q.trk[i].lm_slot < -1 || q.trk[i].lm_slot >= t->td.lm_cap) { why = "tracklet landmark slot out of range"; return KBA_ERR_BAD_ARG; }
+    for (int i = 0; i < q.n_outlier; ++i)
+        if (q.outlier_slot[i] < 0 || q.outlier_slot[i] >= t->td.lm_cap) { why = "outlier landmark slot out of range"; return KBA_ERR_BAD_ARG; }
+    for (int k = 0; k < 3; ++k)
+        if (!(q.params->voxel_size[k] > 0.0) || !std::isfinite(q.params->voxel_size[k])) {
+            why = "voxel sizes must be finite and positive"; return KBA_ERR_BAD_ARG;
+        }
+    // the candidates are a subset of the listed landmarks: their bound is checked before anything runs
+    return rank_entries_check(q.n_lm, q.max_near, q.max_middle, q.max_far, q.n_depth, q.depth, why);
+}
+
+static int kfs_bufs(kba_track* t, std::string& why) {
+    if (t->kfs) return KBA_OK;
+    std::unique_ptr<KfsBufs> kb(new KfsBufs());
+    const size_t L = (size_t)t->td.lm_cap;
+    if (kb->dev.alloc(&kb->lm_at, L) | kb->dev.alloc(&kb->last, L)) { why = "out of memory for the label buffers"; return KBA_ERR_CUDA; }
+    cudaError_t e = cudaMemsetAsync(kb->lm_at, 0xff, sizeof(int) * L, t->set.h->stream);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(t->set.h->stream);
+    if (e != cudaSuccess) { why = std::string("label buffers: ") + cudaGetErrorString(e); return KBA_ERR_CUDA; }
+    t->kfs = std::move(kb);
+    return KBA_OK;
+}
+
+// offsets in a staging block, each aligned
+struct Bump {
+    size_t at = 0;
+    size_t take(size_t bytes, size_t align = 8) { at = (at + align - 1) & ~(align - 1); const size_t o = at; at += bytes; return o; }
+};
+
+// one live request's place in the call's staging (byte offsets; `d_*` in the download block, `x_*` in its device-only part)
+struct KfsWin {
+    kba_track* t = nullptr;
+    int i = 0;                             // track index in the set
+    int max_meas = 0;
+    size_t u_kf, u_lm, u_out, u_trk, u_gin, u_cls, u_depth;
+    size_t d_cnt, d_common, d_post, d_kfa, d_lma, d_lmo, d_gr, d_tro;
+    size_t x_fixed, x_cand, x_elig, x_shrub;
+    int K = 0, N = 0, bound = 0, p_out = 0;
+    std::vector<int> kf, fixed;
+};
+
+// the refused call's cleanup after the ranking's first part ran: the slot maps back to all -1, no track keeps a ranking
+static void kfs_abandon(cudaStream_t s, const std::vector<KfsWin>& ws) {
+    for (const KfsWin& w : ws) {
+        w.t->rank->valid = false;
+        cudaMemsetAsync(w.t->select->a.cand_of, 0xff, sizeof(int) * (size_t)w.t->td.lm_cap, s);
+    }
+    cudaStreamSynchronize(s);
+}
+
+// one keyframe solve of the tracks of s (group = false: a single call), req[i] / out[i] / res[i] track i's
+static int set_keyframe_solve(TrackSet& s, bool group, const std::string& who, const kba_kfsolve_request* req, bool per_track,
+                              const kba_options* opts, kba_kfsolve_out* out, kba_result* res) {
+    const int n = (int)s.tracks.size();
+    auto sits_out = [&](int i) { return group && req[i].n_kf == 0; };
+    SolveTotals tot;
+    std::string owhy;
+    const int orc = solve_options_check(n, opts, per_track, "track ", [&](int i) { return !sits_out(i); }, tot, owhy);
+    if (orc != KBA_OK) return fail(orc, who + owhy);
+    // ---- every check that needs only the request; the scratch of each step at its first use
+    std::vector<KfsWin> ws;
+    for (int i = 0; i < n; ++i) {
+        if (sits_out(i)) continue;
+        kba_track* t = s.tracks[i];
+        const kba_kfsolve_request& q = req[i];
+        std::string why;
+        int rc = kfsolve_check(t, q, out + i, why);
+        if (rc == KBA_OK) {
+            const kba_deactivate_request dq{q.n_kf, q.n_lm, q.min_connecting, q.min_window, q.max_window, 0, q.kf_slot, q.lm_slot};
+            kba_deactivate_out dout{out[i].kf_active, out[i].kf_common, out[i].lm_active};
+            UpkeepReq ur = upkeep_req(t, dq, &dout);
+            rc = upkeep_check(ur, why);
+            if (rc == KBA_OK && !t->select) rc = select_alloc(t, why);
+            if (rc == KBA_OK && !t->rank) rc = rank_alloc(t, why);
+            if (rc == KBA_OK) rc = kfs_bufs(t, why);
+            KfsWin w;
+            w.t = t; w.i = i; w.max_meas = ur.max_meas;
+            ws.push_back(w);
+        }
+        if (rc != KBA_OK) return fail(rc, who + track_prefix(group, i) + why);
+    }
+    if (ws.empty()) {  // no upload, no launch
+        for (int i = 0; i < n; ++i) idle_result(res[i]);
+        s.last = &kNoTransfer;
+        return KBA_OK;
+    }
+    kba_handle* h = s.h;
+    CU(cudaSetDevice(h->device));
+    cudaStream_t st_s = h->stream;
+    const int W = (int)ws.size();
+    // ---- layout: up = records | AddDepth entries | int lists | byte lists, then the draws' block; out = the first download |
+    // device-only lists | the ranking's outputs
+    Bump up, dn, dx;
+    const size_t o_up_rec = up.take(sizeof(UpkeepArgs) * (size_t)(W - 1)), o_kfs = up.take(sizeof(KfsArgs) * (size_t)W);
+    const size_t o_sel = up.take(sizeof(SelectArgs) * (size_t)W), o_rank = up.take(sizeof(RankArgs) * (size_t)W);
+    const size_t o_mid = dn.take(4 * (size_t)W);
+    size_t sum_lm = 0, sum_trk = 0, max_draws = 0;
+    UpkeepGrid ug;
+    SelectGrid sg;
+    RankGrid rg;
+    int max_trk = 0;
+    for (KfsWin& w : ws) {
+        const kba_kfsolve_request& q = req[w.i];
+        const size_t K = (size_t)q.n_kf, L = (size_t)q.n_lm, O = (size_t)q.n_outlier, T = (size_t)q.n_trk;
+        w.u_depth = up.take(8 * (size_t)q.n_depth);
+        w.u_kf = up.take(4 * K, 4); w.u_lm = up.take(4 * L, 4); w.u_out = up.take(4 * O, 4); w.u_trk = up.take(4 * T, 4);
+        w.d_cnt = dn.take(8); w.d_common = dn.take(4 * K, 4); w.d_post = dn.take(4 * K, 4);
+        w.x_cand = dx.take(4 * L);
+        sum_lm += L; sum_trk += T; max_draws += L > 0 ? L - 1 : 0;
+        ug.max_kf = std::max(ug.max_kf, q.n_kf); ug.max_lm = std::max(ug.max_lm, q.n_lm); ug.max_meas = std::max(ug.max_meas, w.max_meas);
+        sg.max_init = std::max(sg.max_init, std::max(std::max(q.n_kf, q.n_lm), w.t->n_cam));
+        rg.max_depth = std::max(rg.max_depth, q.n_depth);
+        max_trk = std::max(max_trk, q.n_trk);
+    }
+    for (KfsWin& w : ws) {  // the byte lists after every window's ints
+        const kba_kfsolve_request& q = req[w.i];
+        const size_t K = (size_t)q.n_kf, L = (size_t)q.n_lm, T = (size_t)q.n_trk;
+        w.u_gin = up.take(L, 1); w.u_cls = up.take(T, 1);
+        w.d_kfa = dn.take(K, 1); w.d_lma = dn.take(L, 1); w.d_lmo = dn.take(L, 1); w.d_gr = dn.take(L, 1); w.d_tro = dn.take(T, 1);
+        w.x_fixed = dx.take(K, 1); w.x_elig = dx.take(L, 1); w.x_shrub = dx.take(T, 1);
+    }
+    sg.max_kf = ug.max_kf; sg.max_cand = ug.max_lm; sg.max_meas = ug.max_meas;
+    rg.max_kf = sg.max_kf; rg.max_cand = sg.max_cand;
+    const size_t up1 = up.at, o_p2 = up.take(8 * (size_t)W + 4 * max_draws), down1 = dn.at;
+    const size_t o_x = (down1 + 7) & ~(size_t)7, o_res = o_x + ((dx.at + 7) & ~(size_t)7);
+    const size_t out_need = o_res + 8 * (size_t)W + 5 * sum_lm;
+    std::unique_ptr<StoreStage>& stage = s.stage[kKfSolveCall];
+    if (!stage || stage->up.n < up.at || stage->out.n < out_need) {  // grow-only: a call no larger than an earlier one allocates nothing
+        std::unique_ptr<StoreStage> fresh(new StoreStage());
+        if (fresh->alloc(std::max(up.at, stage ? stage->up.n : 0), std::max(out_need, stage ? stage->out.n : 0)))
+            return fail(KBA_ERR_CUDA, who + "out of memory for the keyframe solve staging");
+        stage = std::move(fresh);
+    }
+    StoreStage& st = *stage;
+    unsigned char* uh = st.up.h, *od = st.out.d;
+    const unsigned char* ud = st.up.d;
+    // ---- records and lists
+    UpkeepLaunch ul;
+    ul.rest = reinterpret_cast<const UpkeepArgs*>(ud + o_up_rec);
+    ul.n_win = W;
+    KfsArgs* kfs_h = reinterpret_cast<KfsArgs*>(uh + o_kfs);
+    SelectArgs* sel_h = reinterpret_cast<SelectArgs*>(uh + o_sel);
+    RankArgs* rank_h = reinterpret_cast<RankArgs*>(uh + o_rank);
+    for (int v = 0; v < W; ++v) {
+        KfsWin& w = ws[v];
+        kba_track* t = w.t;
+        const kba_kfsolve_request& q = req[w.i];
+        memcpy(uh + w.u_kf, q.kf_slot, 4 * (size_t)q.n_kf);
+        if (q.n_lm) memcpy(uh + w.u_lm, q.lm_slot, 4 * (size_t)q.n_lm);
+        if (q.n_outlier) memcpy(uh + w.u_out, q.outlier_slot, 4 * (size_t)q.n_outlier);
+        if (q.lm_ground) memcpy(uh + w.u_gin, q.lm_ground, (size_t)q.n_lm); else memset(uh + w.u_gin, 0, (size_t)q.n_lm);
+        int* ts = reinterpret_cast<int*>(uh + w.u_trk);
+        for (int i = 0; i < q.n_trk; ++i) {
+            const int c = label_classes(q, q.trk[i].label);
+            ts[i] = q.trk[i].lm_slot;
+            uh[w.u_cls + i] = (unsigned char)(((q.trk[i].is_outlier || (c & KBA_LABEL_OUTLIER)) ? kKfsMarked : 0) |
+                                              ((c & KBA_LABEL_SHRUBBERY) ? kKfsShrub : 0) | ((c & KBA_LABEL_GROUND) ? kKfsGround : 0));
+        }
+        int* de = reinterpret_cast<int*>(uh + w.u_depth);
+        for (int e = 0; e < q.n_depth; ++e) { de[2 * e] = q.depth[e].ind; de[2 * e + 1] = q.depth[e].wanted; }
+        // the deactivation
+        UpkeepBufs& ub = *t->upkeep;
+        if (ub.stamp >= 0xfffffff0u) {  // the stamps wrap: the map starts over from all 0
+            CU(cudaMemsetAsync(ub.map, 0, sizeof(unsigned long long) * (size_t)t->td.lm_cap, st_s));
+            ub.stamp = 0;
+        }
+        UpkeepArgs a;
+        a.td = t->td;
+        a.kf_slot = reinterpret_cast<const int*>(ud + w.u_kf); a.lm_slot = reinterpret_cast<const int*>(ud + w.u_lm);
+        a.n_kf = q.n_kf; a.n_lm = q.n_lm;
+        a.stamp = ub.stamp + 1; ub.stamp += 2;
+        a.map = ub.map;
+        a.min_connecting = q.min_connecting; a.min_window = q.min_window; a.max_window = q.max_window;
+        a.kf_common = reinterpret_cast<int*>(od + w.d_common); a.kf_active = od + w.d_kfa; a.lm_active = od + w.d_lma;
+        if (v == 0) ul.w0 = a;
+        else memcpy(uh + o_up_rec + sizeof(UpkeepArgs) * (size_t)(v - 1), &a, sizeof(UpkeepArgs));
+        // the labels and the post-deactivation lists
+        KfsArgs k;
+        k.kf_slot = a.kf_slot; k.lm_slot = a.lm_slot; k.kf_active = a.kf_active; k.lm_active = a.lm_active;
+        k.ground_in = ud + w.u_gin; k.out_slot = reinterpret_cast<const int*>(ud + w.u_out);
+        k.trk_slot = reinterpret_cast<const int*>(ud + w.u_trk); k.trk_cls = ud + w.u_cls;
+        k.n_kf = q.n_kf; k.n_lm = q.n_lm; k.n_out = q.n_outlier; k.n_trk = q.n_trk;
+        k.lm_at = t->kfs->lm_at; k.last = t->kfs->last;
+        k.lm_out = od + w.d_lmo; k.ground = od + w.d_gr; k.trk_out = od + w.d_tro; k.shrub = od + o_x + w.x_shrub;
+        k.kf_post = reinterpret_cast<int*>(od + w.d_post); k.fixed = od + o_x + w.x_fixed;
+        k.cand = reinterpret_cast<int*>(od + o_x + w.x_cand); k.elig = od + o_x + w.x_elig;
+        k.counts = reinterpret_cast<int*>(od + w.d_cnt);
+        k.sel = reinterpret_cast<SelectArgs*>(st.up.d + o_sel) + v; k.rank = reinterpret_cast<RankArgs*>(st.up.d + o_rank) + v;
+        k.lm_weight = t->td.lm_weight; k.shrub_weight = q.shrubbery_weight;
+        kfs_h[v] = k;
+        // the ranking's chain on the device-built lists; k_kfs_labels writes its n_kf and n_cand
+        const size_t L = (size_t)t->td.lm_cap;
+        unsigned char* qd = t->rank->qty;
+        SelectArgs sa = t->select->a;
+        sa.td = t->td;
+        sa.kf_slot = k.kf_post; sa.lm_slot = k.cand; sa.n_kf = 0; sa.n_cand = 0;
+        for (int c = 0; c < 3; ++c) sa.leaf[c] = q.params->voxel_size[c];
+        sa.roi_far = q.params->roi_far; sa.roi_middle = q.params->roi_middle;
+        sa.flow = reinterpret_cast<double*>(qd); sa.seen = reinterpret_cast<int*>(qd + 8 * L); sa.near_order = reinterpret_cast<int*>(qd + 12 * L);
+        sa.counters = reinterpret_cast<int*>(qd + 16 * L); sa.n_near = sa.counters + 1;
+        sa.cheiral = qd + 16 * L + 16; sa.bin = reinterpret_cast<signed char*>(qd + 17 * L + 16);
+        sel_h[v] = sa;
+        RankArgs ra;
+        ra.td = t->td;
+        ra.kf_slot = sa.kf_slot; ra.lm_slot = sa.lm_slot; ra.elig = k.elig;
+        ra.depth = reinterpret_cast<const int*>(ud + w.u_depth);
+        ra.n_kf = 0; ra.n_cand = 0; ra.n_depth = q.n_depth;
+        ra.max_near = q.max_near; ra.max_middle = q.max_middle; ra.max_far = q.max_far;
+        ra.cheiral = sa.cheiral; ra.bin = sa.bin; ra.near_order = sa.near_order; ra.n_near = sa.n_near; ra.flow = sa.flow; ra.seen = sa.seen;
+        RankBufs& rb = *t->rank;
+        ra.cand_of = sa.cand_of; ra.mark = rb.mark; ra.dcand = rb.dcand; ra.dcost = rb.dcost; ra.dcnt = rb.dcnt;
+        ra.sel_slot = rb.sel_slot; ra.gp = rb.gp;
+        rank_h[v] = ra;
+        t->rank->valid = false;  // replaced by this call's, or none if it is refused
+    }
+    // ---- one upload, one launch sequence (deactivation, labels and lists, the ranking's first part), one download
+    const KfsArgs* kfs_d = reinterpret_cast<const KfsArgs*>(ud + o_kfs);
+    SelectLaunch sl;
+    sl.all = reinterpret_cast<const SelectArgs*>(ud + o_sel); sl.n_win = W;
+    RankLaunch rl;
+    rl.all = reinterpret_cast<const RankArgs*>(ud + o_rank); rl.n_win = W;
+    rl.n_mid = reinterpret_cast<int*>(od + o_mid);
+    CU(cudaMemcpyAsync(st.up.d, st.up.h, up1, cudaMemcpyHostToDevice, st_s));
+    CU(cudaMemsetAsync(rl.n_mid, 0, 4 * (size_t)W, st_s));
+    launch_deactivate(ul, ug, st_s);
+    launch_kfs_labels(kfs_d, W, st_s);
+    launch_select(sl, sg, st_s);
+    launch_rank_prepare(rl, rg, st_s);
+    CU(cudaGetLastError());
+    CU(cudaMemcpyAsync(st.out.h, st.out.d, down1, cudaMemcpyDeviceToHost, st_s));
+    CU(wait_stream(h));
+    Transfer sum;
+    sum.h2d = (int64_t)up1; sum.d2h = (int64_t)down1;
+    const unsigned char* oh = st.out.h;
+    // ---- the checks of the ranking and of the solve on the post-deactivation lists, then the draws
+    const int* n_mid = reinterpret_cast<const int*>(oh + o_mid);
+    int* p2 = reinterpret_cast<int*>(uh + o_p2);
+    int* draws = p2 + 2 * W;
+    size_t n_draws = 0, n_out = 0;
+    std::vector<TrackRequest> qs(n);
+    for (int v = 0; v < W; ++v) {
+        KfsWin& w = ws[v];
+        const kba_kfsolve_request& q = req[w.i];
+        const int* cnt = reinterpret_cast<const int*>(oh + w.d_cnt);
+        w.K = cnt[0]; w.N = cnt[1];
+        std::string why;
+        int rc = KBA_OK;
+        if (w.K == 0) { why = "no keyframes or a negative size"; rc = KBA_ERR_BAD_ARG; }
+        if (rc == KBA_OK) {
+            const int* post = reinterpret_cast<const int*>(oh + w.d_post);
+            w.kf.assign(post, post + w.K);
+            w.fixed.assign(w.K, 0);
+            w.fixed[0] = 1;
+            for (int e = 0; e < q.n_depth && rc == KBA_OK; ++e)  // the AddDepth heap of an entry lives in shared memory
+                if (q.depth[e].ind < w.K && std::min(q.depth[e].wanted, w.t->m_cnt[w.kf[q.depth[e].ind]]) > kRankMaxCand) {
+                    why = "an AddDepth entry keeps more than 57344 landmarks"; rc = KBA_ERR_CAPACITY;
+                }
+        }
+        if (rc == KBA_OK) {
+            // the solve's keyframe checks; the ranking's ground candidates are not known yet: on a window without any
+            kba_window sel0 = *q.sel;
+            sel0.n_gp = 0;
+            std::vector<uint8_t> f8(w.fixed.begin(), w.fixed.end());
+            TrackRequest q0 = track_request(w.K, w.kf.data(), f8.data(), 0, nullptr, &sel0, true);
+            rc = track_check(w.t, q0, why);
+        }
+        if (rc == KBA_OK) {
+            const int nm = n_mid[v], D = std::max(nm - 1, 0), N = w.N;
+            long long b = std::min(q.max_near, N) + (long long)std::min(q.max_middle, nm) + std::min(q.max_far, N);
+            int heap = std::max(std::min(q.max_near, N), std::min(q.max_far, N));
+            for (int e = 0; e < q.n_depth; ++e) {
+                b += std::min(q.depth[e].wanted, N);
+                if (q.depth[e].ind < w.K) heap = std::max(heap, std::min(q.depth[e].wanted, w.t->m_cnt[w.kf[q.depth[e].ind]]));
+            }
+            w.bound = (int)std::min<long long>(b, N);
+            rg.heap_ints = std::max(rg.heap_ints, heap);
+            rg.mid_ints = std::max(rg.mid_ints, nm);
+            p2[2 * v] = (int)n_draws; p2[2 * v + 1] = (int)n_out;
+            w.p_out = (int)n_out;
+            n_out += (size_t)w.bound;
+            if (D > 0) {
+                if (!q.draw) { why = "the middle bin needs " + std::to_string(D) + " draws and there is no draw function"; rc = KBA_ERR_BAD_ARG; }
+                else if (q.draw(q.draw_ctx, D, draws + n_draws) != 0) { why = "the draw function failed"; rc = KBA_ERR_BAD_ARG; }
+                n_draws += (size_t)D;
+            }
+        }
+        if (rc != KBA_OK) {
+            kfs_abandon(st_s, ws);
+            return fail(rc, who + track_prefix(group, w.i) + why);
+        }
+    }
+    // ---- the ranking's second part
+    const size_t p2_bytes = 8 * (size_t)W + 4 * n_draws;
+    CU(cudaMemcpyAsync(st.up.d + o_p2, uh + o_p2, p2_bytes, cudaMemcpyHostToDevice, st_s));
+    rl.p2 = reinterpret_cast<const int*>(ud + o_p2);
+    rl.res = reinterpret_cast<int*>(od + o_res);
+    rl.out_cand = reinterpret_cast<int*>(od + o_res + 8 * (size_t)W);
+    rl.out_cat = reinterpret_cast<signed char*>(od + o_res + 8 * (size_t)W + 4 * n_out);
+    launch_rank(rl, rg, st_s);
+    CU(cudaGetLastError());
+    const size_t down2 = 8 * (size_t)W + 5 * n_out;
+    CU(cudaMemcpyAsync(st.out.h + o_res, st.out.d + o_res, down2, cudaMemcpyDeviceToHost, st_s));
+    CU(wait_stream(h));
+    sum.h2d += (int64_t)p2_bytes; sum.d2h += (int64_t)down2;
+    const int* rres = reinterpret_cast<const int*>(oh + o_res);
+    for (int v = 0; v < W; ++v) {
+        KfsWin& w = ws[v];
+        RankBufs& rb = *w.t->rank;
+        rb.kf = w.kf; rb.n_sel = rres[2 * v]; rb.n_ground = rres[2 * v + 1]; rb.gen = w.t->gen; rb.valid = true;
+    }
+    // ---- the ranked solve's checks, the shrubbery weights, the solve
+    std::vector<std::vector<uint8_t>> fixed8(n);
+    for (const KfsWin& w : ws) {
+        fixed8[w.i].assign(w.fixed.begin(), w.fixed.end());
+        qs[w.i] = track_request(w.K, w.kf.data(), fixed8[w.i].data(), 0, nullptr, req[w.i].sel, true);
+        TrackRequest q = qs[w.i];
+        std::string why;
+        const int rc = ranked_check(w.t, q, why);
+        if (rc != KBA_OK) return fail(rc, who + track_prefix(group, w.i) + why);
+    }
+    launch_kfs_weights(kfs_d, W, max_trk, st_s);
+    CU(cudaGetLastError());
+    for (const KfsWin& w : ws) { w.t->gen++; w.t->rank->gen = w.t->gen; }  // the weights do not enter the ranking
+    int rc = set_solve(s, group, who, qs.data(), per_track, opts, res);
+    if (rc != KBA_OK) return rc;
+    sum.h2d += s.last->h2d; sum.d2h += s.last->d2h;
+    // ---- the outputs
+    const unsigned char* hc = oh + o_res + 8 * (size_t)W;
+    for (int v = 0; v < W; ++v) {
+        const KfsWin& w = ws[v];
+        const kba_kfsolve_request& q = req[w.i];
+        kba_kfsolve_out& o = out[w.i];
+        memcpy(o.kf_active, oh + w.d_kfa, (size_t)q.n_kf); memcpy(o.kf_common, oh + w.d_common, 4 * (size_t)q.n_kf);
+        if (q.n_lm) {
+            memcpy(o.lm_active, oh + w.d_lma, (size_t)q.n_lm); memcpy(o.lm_outlier, oh + w.d_lmo, (size_t)q.n_lm);
+            memcpy(o.lm_ground, oh + w.d_gr, (size_t)q.n_lm);
+        }
+        if (q.n_trk) memcpy(o.trk_outlier, oh + w.d_tro, (size_t)q.n_trk);
+        const int n_sel = rres[2 * v];
+        o.rank.n_sel = n_sel; o.rank.n_ground = rres[2 * v + 1]; o.rank.n_draws = std::max(n_mid[v] - 1, 0);
+        if (n_sel) { memcpy(o.rank.cand, hc + 4 * (size_t)w.p_out, 4 * (size_t)n_sel); memcpy(o.rank.category, hc + 4 * n_out + w.p_out, (size_t)n_sel); }
+    }
+    st.counts = sum;
+    s.last = &st.counts;
+    return KBA_OK;
+}
+
+int kba_track_keyframe_solve(kba_track* t, const kba_kfsolve_request* req, const kba_options* opt, kba_kfsolve_out* out, kba_result* res) {
+    static const std::string who = "kba_track_keyframe_solve: ";
+    if (!t || !req || !opt || !out || !res) return fail(KBA_ERR_BAD_ARG, who + "null argument");
+    return set_keyframe_solve(t->set, false, who, req, false, opt, out, res);
+}
+
+static int group_keyframe_solve(kba_track_group* g, const kba_kfsolve_request* req, bool per_track, const kba_options* opts,
+                                kba_kfsolve_out* out, kba_result* res, const std::string& who) {
+    if (!g || !req || !opts || !out || !res) return fail(KBA_ERR_BAD_ARG, who + "null argument");
+    return set_keyframe_solve(g->set, true, who, req, per_track, opts, out, res);
+}
+int kba_track_group_keyframe_solve(kba_track_group* g, const kba_kfsolve_request* req, const kba_options* opt, kba_kfsolve_out* out,
+                                   kba_result* res) {
+    return group_keyframe_solve(g, req, false, opt, out, res, "kba_track_group_keyframe_solve: ");
+}
+int kba_track_group_keyframe_solve_opts(kba_track_group* g, const kba_kfsolve_request* req, const kba_options* opts,
+                                        kba_kfsolve_out* out, kba_result* res) {
+    return group_keyframe_solve(g, req, true, opts, out, res, "kba_track_group_keyframe_solve_opts: ");
+}
 
 // ---------------------------------------------------------------------------------------------------------------------
 // snapshots of the stored window (include/kba_b200.h, kba_track_save / kba_track_load / kba_track_clone / kba_track_group_save;

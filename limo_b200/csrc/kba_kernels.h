@@ -190,6 +190,8 @@ struct SelectArgs {
 struct SelectLaunch {
     SelectArgs w0;
     const SelectArgs* rest = nullptr;  // [n_win - 1]
+    const SelectArgs* all = nullptr;   // [n_win] or null: every window's record in device memory (w0, rest unused), for records that
+                                       // an earlier kernel of the same sequence completes (k_kfs_labels)
     int n_win = 0;
 };
 // grid sizes: maxima over the windows (threads beyond their own window's sizes exit)
@@ -364,6 +366,7 @@ struct RankArgs {
 struct RankLaunch {
     RankArgs w0;
     const RankArgs* rest = nullptr;        // [n_win - 1]
+    const RankArgs* all = nullptr;         // [n_win] or null: as SelectLaunch::all
     int n_win = 0;
     int* n_mid = nullptr;                  // [n_win] middle-bin sizes (zeroed before launch_rank_prepare)
     const int* p2 = nullptr;               // [2 * n_win] (first draw, first output) of each window, then the draws end to end
@@ -378,6 +381,41 @@ struct RankGrid {
 };
 void launch_rank_prepare(const RankLaunch& l, const RankGrid& g, cudaStream_t s);
 void launch_rank(const RankLaunch& l, const RankGrid& g, cudaStream_t s);
+
+// ---- limo's solve block on a track's store (kba_track_keyframe_solve and its group forms, kba_kfsolve.cu) ----
+// One window = one request, one CTA.  k_kfs_labels runs between launch_deactivate and launch_select of the same sequence: updateLabels
+// over the deactivation's outputs, the post-deactivation keyframe list and the ranking's candidates, whose counts it writes into the
+// window's SelectArgs / RankArgs records (launched with `all`).  k_kfs_weights writes the shrubbery weights once the call's checks
+// have passed.
+constexpr unsigned char kKfsMarked = 1, kKfsShrub = 2, kKfsGround = 4;  // trk_cls: outlier (is_outlier or label), shrubbery, ground
+struct KfsArgs {
+    const int* kf_slot = nullptr;          // [n_kf] the request's keyframes
+    const int* lm_slot = nullptr;          // [n_lm] the request's landmarks
+    const unsigned char* kf_active = nullptr;  // [n_kf] the deactivation's outputs
+    const unsigned char* lm_active = nullptr;  // [n_lm]
+    const unsigned char* ground_in = nullptr;  // [n_lm] or null
+    const int* out_slot = nullptr;         // [n_out] the caller's outlier set
+    const int* trk_slot = nullptr;         // [n_trk] slot or -1
+    const unsigned char* trk_cls = nullptr;    // [n_trk] kKfs* bits
+    int n_kf = 0, n_lm = 0, n_out = 0, n_trk = 0;
+    int* lm_at = nullptr;                  // [lm_cap] scratch, -1 between calls
+    int* last = nullptr;                   // [lm_cap] scratch
+    unsigned char* lm_out = nullptr;       // [n_lm] outputs
+    unsigned char* ground = nullptr;       // [n_lm]
+    unsigned char* trk_out = nullptr;      // [n_trk]
+    unsigned char* shrub = nullptr;        // [n_trk]
+    int* kf_post = nullptr;                // [n_kf] the kept keyframes, then their fixation
+    unsigned char* fixed = nullptr;        // [n_kf]
+    int* cand = nullptr;                   // [n_lm] the candidates' slots and AddDepth eligibility
+    unsigned char* elig = nullptr;         // [n_lm]
+    int* counts = nullptr;                 // [2] kept keyframes, candidates
+    SelectArgs* sel = nullptr;             // the window's records: n_kf, n_cand written
+    RankArgs* rank = nullptr;
+    double* lm_weight = nullptr;           // the store's weights
+    double shrub_weight = 0.;
+};
+void launch_kfs_labels(const KfsArgs* args, int n_win, cudaStream_t s);
+void launch_kfs_weights(const KfsArgs* args, int n_win, int max_trk, cudaStream_t s);
 
 // ---- evaluation of stored windows at the store's state (kba_track_evaluate / kba_track_group_evaluate, kba_evaluate.cu) ----
 // Run after launch_track_gather on the same batch, in place of the packing and the solve: the outputs of window w go to its

@@ -24,7 +24,9 @@ namespace {
 
 using namespace exact;
 
-__device__ __forceinline__ const RankArgs& win(const RankLaunch& l) { return blockIdx.z == 0 ? l.w0 : l.rest[blockIdx.z - 1]; }
+__device__ __forceinline__ const RankArgs& win(const RankLaunch& l) {
+    return l.all ? l.all[blockIdx.z] : (blockIdx.z == 0 ? l.w0 : l.rest[blockIdx.z - 1]);
+}
 
 // ---- libstdc++'s heap on element ids, `less` the partial sort's comparator (the heap's top is its greatest element) ----------
 template <class Less>

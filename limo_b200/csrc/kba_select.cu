@@ -73,7 +73,9 @@ __device__ Grid grid_of(const SelectArgs& a) {
 }
 
 // the arguments of this block's window (the launch parameters are __grid_constant__, so window 0's are read in place)
-__device__ __forceinline__ const SelectArgs& win(const SelectLaunch& l) { return blockIdx.z == 0 ? l.w0 : l.rest[blockIdx.z - 1]; }
+__device__ __forceinline__ const SelectArgs& win(const SelectLaunch& l) {
+    return l.all ? l.all[blockIdx.z] : (blockIdx.z == 0 ? l.w0 : l.rest[blockIdx.z - 1]);
+}
 
 }  // namespace
 
