@@ -1152,6 +1152,105 @@ int kba_track_group_adjust_pose(kba_track_group* g, const kba_track_frame* f, co
  * frame with n_meas == 0 does not read its entry. */
 int kba_track_group_adjust_pose_opts(kba_track_group* g, const kba_track_frame* f, const kba_options* opts, kba_result* res);
 
+/* ---- limo's frame step as one call: adjustPoseOnly, keyframe selection and the push with its new landmarks ----------------------
+ * What limo runs on every camera frame (mono_lidar.cpp:200-232, mono_standalone.cpp:134-168):
+ *     adjustPoseOnly(*cur_frame); kfs = keyframe_selector_.select({cur_frame}, active keyframes); if (!kfs.empty()) push(*kf);
+ * on the stored window, with its results equal, bit for bit, to those of the chain of store calls a caller runs today:
+ *   1. kba_track_adjust_pose on the measurements of the runs with run_sel set (landmark_selector_->getLastSelection(),
+ *      bundle_adjuster_keyframes.cpp:828), in request order, with pose7 and the speed_* fields (those of kba_track_frame).  With
+ *      adjust == 0 (mono_lidar's external prior, mono_lidar.cpp:200) or no run selected, no solve runs and the frame's pose is
+ *      pose7; res is then idle (status KBA_OK, num_solves 0, nothing written), as kba_track_adjust_pose leaves a frame without
+ *      measurements;
+ *   2. kba_track_frame_flow over all measurements against kf_last = kf_slot[n_kf - 1] with min_median_flow;
+ *   3. the verdict of KeyframeSelector::select({frame}, active keyframes) with limo's three schemes, composed on the host (one
+ *      frame, a non-empty buffer: flow and (pose or time)):
+ *        - flow: n_meas > 0 and mean_flow_sq > min_median_flow^2 (the flow call's usable);
+ *        - pose: angle > critical_quaternion_diff, angle = calcQuaternionDiff(frame pose, kf_last's stored pose) in the facade's
+ *          operation order (limo_b200/keyframe_selector.py; it goes through atan2, which stays on the host);
+ *        - time: (stamp - stamp_last) mod 2^64 > time_difference_ns;
+ *   4. if selected, kba_track_push_keyframe(kf_new, frame pose, plane4, the frame's measurements) -- compacting the arena first
+ *      when its end has no room, exactly as the push does;
+ *   5. if selected, kba_track_create_landmarks over kf_slot followed by kf_new (kf_new last) for the landmarks new_slot names.
+ * The request's measurements follow the run contract of kba_track_frame and kba_flow_request: one run per landmark, runs in
+ * ascending landmark id, cameras ascending inside a run.  Every run's landmark has a slot: a landmark the frame measures for the
+ * first time carries the slot the caller assigns it, and new_slot lists those to create.  A frame that is not selected leaves
+ * the store untouched (its ranking stays valid); a selected one writes it, and its ranking is stale.
+ * Outputs: the flow call's (n_matched, flow_sum, mean_flow_sq, match), angle, the three scheme verdicts and selected, always;
+ * pos and flags (kba_create_out's) only when the frame is selected.  res is the adjustment's kba_result as kba_track_adjust_pose
+ * writes it (kf_pose [7], lm_rejected [selected runs, in run order]).
+ * On the device: ONE upload (the frame's five columns, 20 bytes per measurement, the run flags, the keyframe and new-landmark
+ * lists and every window's argument records) and one launch sequence run k_fs_gather (the selected runs gathered into the
+ * pose-only kernel's input by a block-wide ballot scan, kf_last's stored pose copied out), k_adjust_pose and the flow kernels,
+ * which read the staged columns in place; ONE download brings back the adjustment's results, the flow's and kf_last's pose.
+ * The host composes the verdicts.  Only if some frame is selected: one upload of the push's and the creation's argument
+ * records, k_arena_compact (tracks that compact), k_store_append -- which copies the staged columns and takes the adjusted pose
+ * from the adjustment's output in device memory -- and the creation's kernels, then one download of the creations' outputs.
+ * Two synchronisations per call, one when no frame is selected.
+ * Checks: every check runs before anything is uploaded: null pointers, n_kf < 1 (single call), negative sizes; the keyframe
+ * list as the create call checks it (pushed, listed once, n_kf + 1 keyframe slots); kf_new out of range or in use
+ * (KBA_ERR_BAD_ARG); the run contract, landmark slots and cameras in range (KBA_ERR_BAD_ARG); new_slot in range and listed once
+ * (KBA_ERR_BAD_ARG); n_meas > win_observations, more selected runs than win_landmarks, and measurements that would not fit
+ * max_measurements next to the live keyframes' were the frame selected (from the host's mirror of the arena): KBA_ERR_CAPACITY;
+ * with adjust set, the options as kba_track_adjust_pose checks them (precision != 0: KBA_ERR_BAD_ARG) and a speed prior with
+ * speed_dt <= 0.  A refused call writes no output and changes no store; nothing refuses after the first download.
+ * Transfers (kba_track_transfer_bytes / kba_track_group_transfer_bytes), over the W requests that do not sit out, A of them
+ * adjusted (adjust set and a run selected), S selected, C of those compacting with P keyframe slots holding measurements in
+ * all, R_1, R_a, R_2, R_c and R_p sizes of argument records (constants of the library build), L the iteration records the
+ * results take (min(iterations_capacity, 160) of the adjusted frames' largest, 0 without iterations arrays):
+ *         h2d = R_1 W + R_a A + sum(20 n_meas + 4 (n_kf + 1 + n_new) + n_runs) + (S ? R_2 S + R_c C + R_p P : 0)
+ *         d2h = R_f A + R_i A L + sum over adjusted frames of their selected runs + sum(4 n_meas + 80) + 25 sum over selected of n_new
+ * with R_f, R_i the sizes of a frame's result and iteration records; each term of h2d and of d2h is one region of the staging.
+ * Allocations: the call uses each track's motion (pose-only), upkeep, flow and creation scratch, allocated at their first use
+ * by any entry point; its staging grows to its largest call: a call no larger than an earlier one allocates nothing.
+ * The group forms serve one request per track (req[n_tracks], out[n_tracks], res[n_tracks]), each phase one launch sequence
+ * over every track that takes part: a request with n_kf == 0 sits the call out (out[i] not written, res[i] idle); a failing
+ * request returns its code and kba_last_error names its track; _opts takes one kba_options per track (a track that sits out
+ * or is not adjusted does not read its entry).  If no track is selected the call ends after the first download.  A single
+ * call is the group call's one-track case. */
+typedef struct kba_frame_step_request {
+    int32_t n_kf;               /* 0 (group call): this track sits the call out                                              */
+    int32_t n_meas;
+    const int32_t* kf_slot;     /* [n_kf] the active keyframes in ascending id order; the last one is the newest (kf_last)   */
+    const int32_t* lm_slot;     /* [n_meas] every measurement of the frame, runs as kba_track_frame's                         */
+    const int32_t* cam;         /* [n_meas] or NULL (all camera 0)                                                            */
+    const float* u, *v, *d;     /* [n_meas] FeaturePoint; d < 0: no depth                                                     */
+    const uint8_t* run_sel;     /* [runs of lm_slot] 1: the run's landmark is in the last selection (adjustPoseOnly's)        */
+    int32_t n_new;
+    int32_t kf_new;             /* the slot the frame is pushed into if selected: free when the call starts                  */
+    const int32_t* new_slot;    /* [n_new] the landmarks to create if selected (kba_create_request's lm_slot)                 */
+    const double* pose7;        /* the frame's initial pose (the prior)                                                        */
+    const double* plane4;       /* the pushed keyframe's plane; NULL: (0, 0, 1, 0)                                             */
+    double speed_weight;        /* the speed prior, as kba_track_frame's speed_* fields; <= 0: none                           */
+    double speed_dt;
+    double speed_v_before[3];
+    double speed_T_origin_before[7];
+    double min_median_flow;     /* KeyframeRejectionSchemeFlow                                                                */
+    double critical_quaternion_diff;  /* KeyframeSelectionSchemePose, radians                                                 */
+    uint64_t time_difference_ns;      /* KeyframeSparsificationSchemeTime::time_difference_nano_sec_                          */
+    uint64_t stamp;             /* the frame's time stamp, ns                                                                 */
+    uint64_t stamp_last;        /* kf_last's time stamp, ns                                                                   */
+    uint8_t adjust;             /* 0: the pose is taken as given, no solve runs                                               */
+    uint8_t reserved_[7];
+} kba_frame_step_request;
+typedef struct kba_frame_step_out {  /* caller-owned */
+    int32_t n_matched;          /* the flow call's outputs                                                                    */
+    uint8_t usable_flow, usable_pose, usable_time, selected;  /* the three schemes' verdicts and the selector's                */
+    double flow_sum;
+    double mean_flow_sq;
+    double angle;               /* calcQuaternionDiff(frame pose, kf_last's stored pose)                                      */
+    int32_t* match;             /* [n_meas] or NULL                                                                           */
+    double* pos;                /* [3 * n_new] written only when selected; NaN where not created                              */
+    uint8_t* flags;             /* [n_new] written only when selected: bit 0 created, bit 1 has depth                         */
+} kba_frame_step_out;
+int kba_track_frame_step(kba_track* t, const kba_frame_step_request* req, const kba_options* opt, kba_frame_step_out* out,
+                         kba_result* res);
+/* req[n_tracks], out[n_tracks], res[n_tracks] */
+int kba_track_group_frame_step(kba_track_group* g, const kba_frame_step_request* req, const kba_options* opt,
+                               kba_frame_step_out* out, kba_result* res);
+/* opts[n_tracks]: track i's adjustment runs with opts[i] */
+int kba_track_group_frame_step_opts(kba_track_group* g, const kba_frame_step_request* req, const kba_options* opts,
+                                    kba_frame_step_out* out, kba_result* res);
+
 /* ---- landmark initialisation of push() for a whole window (SURVEY 8(f) row 2) ------------------------------------------
  * Replaces, for all landmarks of `w` at once, what BundleAdjusterKeyframes::push() does per new landmark on the host:
  * the first observation with a lidar depth (d >= 0) is back-projected (bundle_adjuster_keyframes.cpp:332-355); without

@@ -10,7 +10,7 @@ import os
 
 import numpy as np
 
-from .capi_types import (KbaCounters, KbaCreateOut, KbaCreateRequest, KbaDeactivateOut, KbaDeactivateRequest, KbaDepthEntry, KbaDepthOut, KbaDepthRequest, KbaDrawFn, KbaEvalOut, KbaEvaluateOut, KbaFlowOut, KbaFlowRequest, KbaKfsolveOut, KbaKfsolveRequest, KbaLabelClass, KbaLandmarkWrite, KbaLidarCloud, KbaLidarOptions, KbaLidarView, KbaOptions, KbaPoseWrite, KbaPushRequest, KbaRankedRequest, KbaRankOut, KbaRankRequest, KbaReclaimOut, KbaReclaimRequest, KbaResult, KbaSelectOut, KbaSelectParams, KbaSelectRequest, KbaTracklet,
+from .capi_types import (KbaCounters, KbaCreateOut, KbaCreateRequest, KbaDeactivateOut, KbaDeactivateRequest, KbaDepthEntry, KbaDepthOut, KbaDepthRequest, KbaDrawFn, KbaEvalOut, KbaEvaluateOut, KbaFlowOut, KbaFlowRequest, KbaFrameStepOut, KbaFrameStepRequest, KbaKfsolveOut, KbaKfsolveRequest, KbaLabelClass, KbaLandmarkWrite, KbaLidarCloud, KbaLidarOptions, KbaLidarView, KbaOptions, KbaPoseWrite, KbaPushRequest, KbaRankedRequest, KbaRankOut, KbaRankRequest, KbaReclaimOut, KbaReclaimRequest, KbaResult, KbaSelectOut, KbaSelectParams, KbaSelectRequest, KbaTracklet,
                          KbaSnapshotHeader, KbaTrackCaps, KbaTrackFrame, KbaTrackRequest, KbaWindow, Result, Window, c_double_p, c_float_p, c_int32_p,
                          c_uint8_p)
 
@@ -38,7 +38,7 @@ SYMBOLS = ["kba_version", "kba_last_error", "kba_default_options", "kba_create",
            "kba_lidar_depth_batch_opts", "kba_track_snapshot_size", "kba_track_save", "kba_track_load", "kba_track_clone",
            "kba_track_group_snapshot_sizes", "kba_track_group_save", "kba_track_evaluate", "kba_track_group_evaluate",
            "kba_track_group_evaluate_opts", "kba_track_keyframe_solve", "kba_track_group_keyframe_solve",
-           "kba_track_group_keyframe_solve_opts"]
+           "kba_track_group_keyframe_solve_opts", "kba_track_frame_step", "kba_track_group_frame_step", "kba_track_group_frame_step_opts"]
 
 
 class KbaError(RuntimeError):
@@ -179,6 +179,8 @@ def lib():
             f.argtypes = [vp, C.POINTER(KbaTrackRequest), C.POINTER(KbaOptions), C.POINTER(KbaEvaluateOut)]
         for f in (L.kba_track_keyframe_solve, L.kba_track_group_keyframe_solve, L.kba_track_group_keyframe_solve_opts):
             f.argtypes = [vp, C.POINTER(KbaKfsolveRequest), C.POINTER(KbaOptions), C.POINTER(KbaKfsolveOut), C.POINTER(KbaResult)]
+        for f in (L.kba_track_frame_step, L.kba_track_group_frame_step, L.kba_track_group_frame_step_opts):
+            f.argtypes = [vp, C.POINTER(KbaFrameStepRequest), C.POINTER(KbaOptions), C.POINTER(KbaFrameStepOut), C.POINTER(KbaResult)]
         L.kba_lidar_default_options.argtypes = [C.POINTER(KbaLidarOptions)]
         L.kba_lidar_default_options.restype = None
         fp = C.POINTER(C.c_float)
@@ -403,6 +405,91 @@ def _evaluate_outputs(n_lm, obs_cap, gp_cap):
         r.update(rejected_repr=r["rejected_repr"].astype(bool), rejected_depth=r["rejected_depth"].astype(bool))
         return r
     return o, tuple(b.values()), done
+
+
+def _frame_step_args(kf_slots, lm_slot, u, v, d, run_sel, kf_new, pose7, stamp, stamp_last, critical_quaternion_diff,
+                     time_difference_ns, cam=None, new_slots=(), plane4=None, adjust=True, speed=None, min_median_flow=5.0):
+    """one frame step request's arrays and scalars, checked where the C call would read past an array"""
+    kf, lm, cm, new = _arr(kf_slots, np.int32, -1), _arr(lm_slot, np.int32, -1), _arr(cam, np.int32, -1), _arr(new_slots, np.int32, -1)
+    uu, vv, dd = (_arr(x, np.float32, -1) for x in (u, v, d))
+    rs = np.ascontiguousarray(np.asarray(run_sel, dtype=bool).ravel().astype(np.uint8))
+    n_runs = int(1 + np.count_nonzero(lm[1:] != lm[:-1])) if len(lm) else 0
+    if len(rs) != n_runs:
+        raise ValueError("run_sel has %d flags for %d runs" % (len(rs), n_runs))
+    if any(a is not None and len(a) != len(lm) for a in (cm, uu, vv, dd)):
+        raise ValueError("cam, u, v, d must have one entry per measurement")
+    pose, pl = _arr(pose7, np.float64, 7), _arr(plane4, np.float64, 4)
+    sp = dict(speed_weight=0.0, speed_dt=1.0, speed_v_before=np.zeros(3), speed_T_origin_before=np.zeros(7))
+    if speed:
+        sp.update(speed_weight=float(speed["weight"]), speed_dt=float(speed["dt"]), speed_v_before=np.asarray(speed["v_before"], np.float64),
+                  speed_T_origin_before=np.asarray(speed["T_origin_before"], np.float64))
+    return dict(kf=kf, lm=lm, cam=cm, new=new, u=uu, v=vv, d=dd, run_sel=rs, pose=pose, plane=pl, kf_new=int(kf_new),
+                n_sel_runs=int(rs.sum()), adjust=int(bool(adjust)), min_median_flow=float(min_median_flow),
+                critical_quaternion_diff=float(critical_quaternion_diff), time_difference_ns=int(time_difference_ns), stamp=int(stamp),
+                stamp_last=int(stamp_last), **sp)
+
+
+def _frame_step_records(fn, requests, capacity):
+    """the request and output arrays of a frame step over requests (None: the track sits out) as numpy records, the KbaResult
+    array, the buffers they point into, and result(i, filled KbaResult array) -> request i's dict.  No ctypes object per track
+    but its Result."""
+    n = len(requests)
+    act = [i for i, r in enumerate(requests) if r is not None]
+    args = [_built(fn, i, requests[i], _frame_step_args) for i in act]
+    for i, a in zip(act, args):
+        if len(a["kf"]) == 0:  # n_kf = 0 would sit the track out: a request without keyframes is an error, as for one track
+            raise KbaError("%s: track %d: no keyframes or a negative size" % (fn.__name__, i))
+    req, out = np.zeros(n, _records(KbaFrameStepRequest)), np.zeros(n, _records(KbaFrameStepOut))
+    nk, nm, nn = (np.array([len(a[k]) for a in args], np.int64) for k in ("kf", "lm", "new"))
+    has_cam = np.array([a["cam"] is not None for a in args], bool)
+    ints = np.concatenate([a["kf"] for a in args] + [a["lm"] for a in args] + [a["cam"] for a in args if a["cam"] is not None] +
+                          [a["new"] for a in args] + [np.zeros(1, np.int32)])
+    flts = np.concatenate([a[k] for k in ("u", "v", "d") for a in args] + [np.zeros(1, np.float32)])
+    flags = np.concatenate([a["run_sel"] for a in args] + [np.zeros(1, np.uint8)])
+    poses = np.concatenate([a["pose"] for a in args] + [np.zeros(0)])
+    planes = np.concatenate([a["plane"] for a in args if a["plane"] is not None] + [np.zeros(0)])
+    ex = lambda c: np.concatenate(([0], np.cumsum(c)[:-1])).astype(np.int64)  # noqa: E731  exclusive sums
+    M, K = int(nm.sum()), int(nk.sum())
+    cam_off = K + M + ex(np.where(has_cam, nm, 0))
+    req["n_kf"][act], req["n_meas"][act], req["n_new"][act] = nk, nm, nn
+    req["kf_slot"][act] = ints.ctypes.data + 4 * ex(nk)
+    req["lm_slot"][act] = ints.ctypes.data + 4 * (K + ex(nm))
+    req["cam"][act] = np.where(has_cam, ints.ctypes.data + 4 * cam_off, 0)
+    req["new_slot"][act] = ints.ctypes.data + 4 * (K + M + int(nm[has_cam].sum()) + ex(nn))
+    for j, k in enumerate(("u", "v", "d")):
+        req[k][act] = flts.ctypes.data + 4 * (j * M + ex(nm))
+    req["run_sel"][act] = flags.ctypes.data + ex([len(a["run_sel"]) for a in args])
+    req["pose7"][act] = poses.ctypes.data + 56 * np.arange(len(act))
+    has_plane = np.array([a["plane"] is not None for a in args], bool)
+    req["plane4"][act] = np.where(has_plane, planes.ctypes.data + 32 * ex(has_plane), 0)
+    for k in ("kf_new", "adjust", "min_median_flow", "critical_quaternion_diff", "time_difference_ns", "stamp", "stamp_last",
+              "speed_weight", "speed_dt", "speed_v_before", "speed_T_origin_before"):
+        req[k][act] = [a[k] for a in args]
+    match = np.zeros(M + 1, np.int32)
+    pos, cflags = np.full((int(nn.sum()) + 1, 3), np.nan), np.zeros(int(nn.sum()) + 1, np.uint8)
+    out["match"][act] = match.ctypes.data + 4 * ex(nm)
+    out["pos"][act] = pos.ctypes.data + 24 * ex(nn)
+    out["flags"][act] = cflags.ctypes.data + ex(nn)
+    ress = (KbaResult * n)()
+    results = {}
+    for j, i in enumerate(act):
+        results[i] = Result(_sel_window(1, args[j]["n_sel_runs"]), capacity)
+        ress[i] = results[i].c
+    row = dict(zip(act, range(len(act))))
+    mo, no = dict(zip(act, ex(nm))), dict(zip(act, ex(nn)))
+
+    def result(i, filled):
+        o, j = out[i], row[i]
+        res = results[i]
+        res.c = filled[i]
+        m0, n0 = int(mo[i]), int(no[i])
+        picked = bool(o["selected"])
+        return dict(n_matched=int(o["n_matched"]), flow_sum=float(o["flow_sum"]), mean_flow_sq=float(o["mean_flow_sq"]),
+                    match=match[m0:m0 + nm[j]].copy(), angle=float(o["angle"]), usable_flow=bool(o["usable_flow"]),
+                    usable_pose=bool(o["usable_pose"]), usable_time=bool(o["usable_time"]), selected=picked,
+                    pos=pos[n0:n0 + nn[j]].copy() if picked else None, flags=cflags[n0:n0 + nn[j]].copy() if picked else None,
+                    result=res)
+    return req, out, ress, (ints, flts, flags, poses, planes, match, pos, cflags, results), result
 
 
 class Track:
@@ -738,6 +825,21 @@ class Track:
         _check(lib().kba_track_keyframe_solve(self._p, C.byref(q), C.byref(opt or default_options()), C.byref(o), C.byref(rc)))
         return done(o)
 
+    def frame_step(self, opt=None, iterations_capacity=256, **kw):
+        """limo's frame step -- adjustPoseOnly, KeyframeSelector::select and push() with its new landmarks -- as one call
+        (kba_track_frame_step).  Keywords: kf_slots (the active keyframes in ascending id order, the newest last), the frame's
+        measurements lm_slot, u, v, d and cam (every run's landmark with a slot; runs as for adjust_pose), run_sel (one flag per
+        run: the landmark is in the last selection), kf_new (the free slot the frame is pushed into if selected), new_slots (the
+        landmarks to create then), pose7, plane4, adjust (False: the pose is taken as given), speed (as for adjust_pose),
+        min_median_flow, critical_quaternion_diff (radians), time_difference_ns, stamp and stamp_last (ns).  Returns a dict: the
+        flow's n_matched, flow_sum, mean_flow_sq, match; angle; usable_flow, usable_pose, usable_time, selected; pos, flags (the
+        creation's, None when not selected); result, the adjustment's Result."""
+        fn = lib().kba_track_frame_step
+        req, out, ress, _keep, result = _frame_step_records(fn, [kw], iterations_capacity)
+        _check(fn(self._p, req.ctypes.data_as(C.POINTER(KbaFrameStepRequest)), C.byref(opt or default_options()),
+                  out.ctypes.data_as(C.POINTER(KbaFrameStepOut)), ress))
+        return result(0, ress)
+
     def transfer_bytes(self):
         a, b, c = C.c_int64(), C.c_int64(), C.c_int64()
         _check(lib().kba_track_transfer_bytes(self._p, C.byref(a), C.byref(b), C.byref(c)))
@@ -988,6 +1090,17 @@ class TrackGroup:
         for i, d in done:
             results[i] = d(outs[i], ress[i])
         return results
+
+    def frame_step(self, requests, opt=None, iterations_capacity=256):
+        """limo's frame step for every track (kba_track_group_frame_step): each entry None (the track sits the call out) or a dict
+        with the keywords of Track.frame_step.  opt: one KbaOptions, or one per track (kba_track_group_frame_step_opts).  Returns
+        one result dict per track (Track.frame_step's), None for a track that sat out."""
+        # Not _call: the request and output structs are numpy records, filled without a ctypes object per track
+        assert len(requests) == len(self.tracks)
+        fn, o = _options(opt, len(self.tracks), lib().kba_track_group_frame_step, lib().kba_track_group_frame_step_opts)
+        req, out, ress, _keep, result = _frame_step_records(fn, requests, iterations_capacity)
+        _check(fn(self._p, req.ctypes.data_as(C.POINTER(KbaFrameStepRequest)), o, out.ctypes.data_as(C.POINTER(KbaFrameStepOut)), ress))
+        return [None if r is None else result(i, ress) for i, r in enumerate(requests)]
 
     def push_keyframes(self, requests):
         """one keyframe into every track's store in one call (kba_track_group_push_keyframes): each entry None (the track sits the

@@ -255,6 +255,21 @@ class KbaTrackFrame(C.Structure):
                 ("speed_v_before", C.c_double * 3), ("speed_T_origin_before", C.c_double * 7)]
 
 
+class KbaFrameStepRequest(C.Structure):
+    _fields_ = [("n_kf", C.c_int32), ("n_meas", C.c_int32), ("kf_slot", c_int32_p), ("lm_slot", c_int32_p), ("cam", c_int32_p),
+                ("u", c_float_p), ("v", c_float_p), ("d", c_float_p), ("run_sel", c_uint8_p), ("n_new", C.c_int32), ("kf_new", C.c_int32),
+                ("new_slot", c_int32_p), ("pose7", c_double_p), ("plane4", c_double_p), ("speed_weight", C.c_double),
+                ("speed_dt", C.c_double), ("speed_v_before", C.c_double * 3), ("speed_T_origin_before", C.c_double * 7),
+                ("min_median_flow", C.c_double), ("critical_quaternion_diff", C.c_double), ("time_difference_ns", C.c_uint64),
+                ("stamp", C.c_uint64), ("stamp_last", C.c_uint64), ("adjust", C.c_uint8), ("reserved_", C.c_uint8 * 7)]
+
+
+class KbaFrameStepOut(C.Structure):
+    _fields_ = [("n_matched", C.c_int32), ("usable_flow", C.c_uint8), ("usable_pose", C.c_uint8), ("usable_time", C.c_uint8),
+                ("selected", C.c_uint8), ("flow_sum", C.c_double), ("mean_flow_sq", C.c_double), ("angle", C.c_double),
+                ("match", c_int32_p), ("pos", c_double_p), ("flags", c_uint8_p)]
+
+
 class KbaOptions(C.Structure):
     _fields_ = [
         ("depth_thres", C.c_double), ("reprojection_thres", C.c_double),

@@ -330,7 +330,7 @@ struct SlotStamps {
 // the store calls that stage their requests, one staging each; deactivation and depth costs share the upkeep one, a drop shares
 // the push's
 enum StoreCall { kSelectCall, kCreateCall, kUpkeepCall, kFlowCall, kReclaimCall, kRankCall, kPushCall, kLandmarkWriteCall, kPoseWriteCall,
-                 kSnapshotCall, kKfSolveCall, kStoreCalls };
+                 kSnapshotCall, kKfSolveCall, kFrameStepCall, kStoreCalls };
 
 struct EvalStage;
 
@@ -2864,6 +2864,15 @@ static int flow_check(kba_track* t, const kba_flow_request* q, std::string& why)
     return KBA_OK;
 }
 
+// a flow record's mean_flow_sq.  Without a match it is 0 / 0: the NaN's bits are the host CPU's default NaN in the facade (x86-64:
+// sign bit set), which the device's canonical NaN is not, so the library forms this one quotient with the host's own arithmetic.
+static double mean_flow_sq(const FlowRes& r) {
+    if (r.n_matched != 0) return r.mean_flow_sq;
+    volatile double zero = 0.;
+    const double q0 = r.flow_sum / zero;
+    return q0 * q0;
+}
+
 // W checked requests of distinct tracks as the W windows of one launch sequence: one upload (the argument records of windows
 // 1 .. W-1, then every window's lm | cam | u | v), one download (the FlowRes records of all windows, then their match indices),
 // one synchronisation, then the scatter into the callers' outputs.  Window 0's record travels in the launch parameters.
@@ -2935,14 +2944,7 @@ static int flow_run(kba_handle* h, StoreStage& st, int W, const FlowReq* r) {
         o.n_matched = res[w].n_matched;
         o.usable = (uint8_t)res[w].usable;
         o.flow_sum = res[w].flow_sum;
-        o.mean_flow_sq = res[w].mean_flow_sq;
-        if (res[w].n_matched == 0) {
-            // 0 / 0: the NaN's bits are the host CPU's default NaN in the facade (x86-64: sign bit set), which the device's
-            // canonical NaN is not, so the library forms this one quotient with the host's own arithmetic
-            volatile double zero = 0.;
-            const double q0 = o.flow_sum / zero;
-            o.mean_flow_sq = q0 * q0;
-        }
+        o.mean_flow_sq = mean_flow_sq(res[w]);
         if (o.match && n) memcpy(o.match, match + mi, 4 * n);
         mi += n;
     }
@@ -3164,6 +3166,35 @@ static int options_check(const kba_options* opt, std::string& why) {
     return KBA_OK;
 }
 
+// one frame's results of k_adjust_pose (its FrameRes, log_cap iteration records, `runs` rejection flags) into r; ms the kernel's time
+static void frame_result(const FrameRes& R, const IterRecord* lg, int log_cap, const unsigned char* rej, int runs, float ms, kba_result& r) {
+    if (r.kf_pose) memcpy(r.kf_pose, R.pose, sizeof(R.pose));
+    if (r.lm_rejected) memcpy(r.lm_rejected, rej, (size_t)runs);
+    r.num_solves = R.n_solves;
+    for (int k = 0; k < R.n_solves && k < KBA_MAX_SOLVES; ++k) {
+        const SolveSummary& ss = R.solves[k];
+        kba_solve_summary& o = r.solves[k];
+        o.initial_cost = ss.initial_cost; o.final_cost = ss.final_cost; o.num_iterations = ss.num_iterations;
+        o.num_successful_steps = ss.num_successful_steps; o.termination = ss.termination;
+        o.num_landmarks = ss.num_landmarks; o.num_residual_blocks = ss.num_residual_blocks; o.reserved_ = 0;
+    }
+    r.initial_cost = R.n_solves > 0 ? R.solves[0].initial_cost : 0.0;
+    r.final_cost = R.n_solves > 0 ? R.solves[R.n_solves - 1].final_cost : 0.0;
+    r.status = R.done ? KBA_OK : KBA_ERR_TIMEOUT;
+    r.time_sec = 1e-3 * ms;
+    int k = 0;
+    if (r.iterations) {
+        for (; k < R.log_n && k < r.iterations_capacity && k < log_cap; ++k) {
+            const IterRecord& e = lg[k];
+            kba_iteration& o = r.iterations[k];
+            o.cost = e.cost; o.cost_change = e.cost_change; o.gradient_max_norm = e.gradient_max_norm;
+            o.step_norm = e.step_norm; o.relative_decrease = e.relative_decrease; o.trust_region_radius = e.radius;
+            o.iteration = e.iteration; o.solve_index = e.solve_index; o.step_is_valid = e.valid; o.step_is_successful = e.successful;
+        }
+    }
+    r.num_iteration_records = k;
+}
+
 // frames f[i] of tracks ts[i] (already checked; runs[i] landmarks, rounds[i] trimming rounds; n_meas == 0: idle) as one launch;
 // opts[i] (per_frame) or opts[0] are their options
 static int adjust_pose_run(kba_handle* h, MotionBufs& mb, int n, kba_track* const* ts, const kba_track_frame* f, const int* runs,
@@ -3256,36 +3287,8 @@ static int adjust_pose_run(kba_handle* h, MotionBufs& mb, int n, kba_track* cons
     const FrameRes* fr = reinterpret_cast<const FrameRes*>(mb.out.h);
     const IterRecord* lg = reinterpret_cast<const IterRecord*>(mb.out.h + o_log);
     const unsigned char* rj = mb.out.h + o_rej;
-    for (int q = 0; q < nf; ++q) {
-        const int i = live[q];
-        const FrameRes& R = fr[q];
-        kba_result& r = res[i];
-        if (r.kf_pose) memcpy(r.kf_pose, R.pose, sizeof(R.pose));
-        if (r.lm_rejected) memcpy(r.lm_rejected, rj + fd[q].run_off, (size_t)runs[i]);
-        r.num_solves = R.n_solves;
-        for (int k = 0; k < R.n_solves && k < KBA_MAX_SOLVES; ++k) {
-            const SolveSummary& ss = R.solves[k];
-            kba_solve_summary& o = r.solves[k];
-            o.initial_cost = ss.initial_cost; o.final_cost = ss.final_cost; o.num_iterations = ss.num_iterations;
-            o.num_successful_steps = ss.num_successful_steps; o.termination = ss.termination;
-            o.num_landmarks = ss.num_landmarks; o.num_residual_blocks = ss.num_residual_blocks; o.reserved_ = 0;
-        }
-        r.initial_cost = R.n_solves > 0 ? R.solves[0].initial_cost : 0.0;
-        r.final_cost = R.n_solves > 0 ? R.solves[R.n_solves - 1].final_cost : 0.0;
-        r.status = R.done ? KBA_OK : KBA_ERR_TIMEOUT;
-        r.time_sec = 1e-3 * ms;
-        int k = 0;
-        if (r.iterations) {
-            for (; k < R.log_n && k < r.iterations_capacity && k < log_cap; ++k) {
-                const IterRecord& e = lg[(size_t)q * log_cap + k];
-                kba_iteration& o = r.iterations[k];
-                o.cost = e.cost; o.cost_change = e.cost_change; o.gradient_max_norm = e.gradient_max_norm;
-                o.step_norm = e.step_norm; o.relative_decrease = e.relative_decrease; o.trust_region_radius = e.radius;
-                o.iteration = e.iteration; o.solve_index = e.solve_index; o.step_is_valid = e.valid; o.step_is_successful = e.successful;
-            }
-        }
-        r.num_iteration_records = k;
-    }
+    for (int q = 0; q < nf; ++q)
+        frame_result(fr[q], lg + (size_t)q * log_cap, log_cap, rj + fd[q].run_off, runs[live[q]], ms, res[live[q]]);
     return KBA_OK;
 }
 
@@ -3644,13 +3647,55 @@ static int push_check(const PushReq& r, std::string& why) {
 // rows of one push staged per track: larger pushes go up in several flushes
 constexpr int kPushStageRows = 1 << 16;
 
+// the host mirror's part of one push of n_meas measurements into keyframe slot `slot` of track t: a track whose arena has no room
+// left at its end compacts (its live keyframes in slot order into the other arena: a CompactTrack and its runs, appended to ct and
+// runs), then the keyframe goes to the end of the arena.  Returns its append record (seg, n, src still to be set).
+static StoreAppend append_plan(kba_track* t, int32_t slot, int32_t n_meas, const double* pose7, const double* plane4, bool cam_zero,
+                               std::vector<CompactTrack>& ct, std::vector<CompactRun>& runs, int& max_run) {
+    static const double kNoPlane[4] = {0., 0., 1., 0.};
+    if (t->arena_used + n_meas > t->td.m_cap) {
+        const int cur = t->arena_cur, other = 1 - cur;
+        CompactTrack c;
+        for (int j = 0; j < 2; ++j) { c.src[j] = (const unsigned*)t->arena_i[cur][j]; c.dst[j] = (unsigned*)t->arena_i[other][j]; }
+        for (int j = 0; j < 3; ++j) { c.src[2 + j] = (const unsigned*)t->arena_f[cur][j]; c.dst[2 + j] = (unsigned*)t->arena_f[other][j]; }
+        c.m_off = t->td.m_off; c.m_cnt = t->td.m_cnt;
+        int used = 0;
+        for (int k = 0; k < t->td.kf_cap; ++k) {
+            const int n = t->m_cnt[k];
+            if (!t->kf_live[k]) {  // a dropped keyframe's count is cleared
+                if (n) { runs.push_back(CompactRun{(int)ct.size(), k, 0, t->m_off[k], 0, 0}); t->m_cnt[k] = 0; }
+                continue;
+            }
+            if (n == 0) continue;
+            runs.push_back(CompactRun{(int)ct.size(), k, t->m_off[k], used, n, 0});
+            max_run = std::max(max_run, n);
+            t->m_off[k] = used;
+            used += n;
+        }
+        ct.push_back(c);
+        t->arena_cur = other; t->arena_used = used;
+        t->point_arena();
+    }
+    StoreAppend a;
+    a.col[0] = (unsigned*)t->td.m_lm; a.col[1] = (unsigned*)t->td.m_cam;
+    a.col[2] = (unsigned*)t->td.m_u; a.col[3] = (unsigned*)t->td.m_v; a.col[4] = (unsigned*)t->td.m_d;
+    a.m_off = t->td.m_off; a.m_cnt = t->td.m_cnt; a.kf_pose = t->td.kf_pose; a.kf_plane = t->td.kf_plane;
+    memcpy(a.pose, pose7, sizeof(a.pose));
+    memcpy(a.plane, plane4 ? plane4 : kNoPlane, sizeof(a.plane));
+    a.slot = slot; a.off = t->arena_used; a.cnt = n_meas; a.cam_zero = cam_zero ? 1 : 0;
+    t->m_off[slot] = t->arena_used; t->m_cnt[slot] = n_meas; t->kf_live[slot] = 1;
+    t->arena_used += n_meas;
+    t->gen++;
+    t->h2d_push += (int64_t)n_meas * 20 + 11 * 8;
+    return a;
+}
+
 // W checked pushes of distinct tracks.  The host mirror decides every offset first: a track whose arena has no room left compacts
 // (its live keyframes in slot order into the other arena, as runs of k_arena_compact), and each keyframe goes to the end of its
 // track's arena (segments of k_store_append, which also write its layout, pose and plane).  The staging, flushed when its rows are
 // full: compaction records | runs | segments | the five columns (lm, cam, u, v, d) of `stride` words; a segment's rows start at a
 // column offset congruent to their arena offset modulo 4, so that the copies run on 16-byte vectors.
 static int push_run(kba_handle* h, StoreStage& st, int W, const PushReq* r) {
-    static const double kNoPlane[4] = {0., 0., 1., 0.};
     CU(cudaSetDevice(h->device));
     cudaStream_t s = h->stream;
     std::vector<CompactTrack> ct;
@@ -3658,42 +3703,8 @@ static int push_run(kba_handle* h, StoreStage& st, int W, const PushReq* r) {
     std::vector<StoreAppend> app(W);
     int max_run = 0;
     for (int w = 0; w < W; ++w) {
-        kba_track* t = r[w].t;
         const kba_push_request& q = *r[w].q;
-        if (t->arena_used + q.n_meas > t->td.m_cap) {
-            const int cur = t->arena_cur, other = 1 - cur;
-            CompactTrack c;
-            for (int j = 0; j < 2; ++j) { c.src[j] = (const unsigned*)t->arena_i[cur][j]; c.dst[j] = (unsigned*)t->arena_i[other][j]; }
-            for (int j = 0; j < 3; ++j) { c.src[2 + j] = (const unsigned*)t->arena_f[cur][j]; c.dst[2 + j] = (unsigned*)t->arena_f[other][j]; }
-            c.m_off = t->td.m_off; c.m_cnt = t->td.m_cnt;
-            int used = 0;
-            for (int k = 0; k < t->td.kf_cap; ++k) {
-                const int n = t->m_cnt[k];
-                if (!t->kf_live[k]) {  // a dropped keyframe's count is cleared
-                    if (n) { runs.push_back(CompactRun{(int)ct.size(), k, 0, t->m_off[k], 0, 0}); t->m_cnt[k] = 0; }
-                    continue;
-                }
-                if (n == 0) continue;
-                runs.push_back(CompactRun{(int)ct.size(), k, t->m_off[k], used, n, 0});
-                max_run = std::max(max_run, n);
-                t->m_off[k] = used;
-                used += n;
-            }
-            ct.push_back(c);
-            t->arena_cur = other; t->arena_used = used;
-            t->point_arena();
-        }
-        StoreAppend& a = app[w];
-        a.col[0] = (unsigned*)t->td.m_lm; a.col[1] = (unsigned*)t->td.m_cam;
-        a.col[2] = (unsigned*)t->td.m_u; a.col[3] = (unsigned*)t->td.m_v; a.col[4] = (unsigned*)t->td.m_d;
-        a.m_off = t->td.m_off; a.m_cnt = t->td.m_cnt; a.kf_pose = t->td.kf_pose; a.kf_plane = t->td.kf_plane;
-        memcpy(a.pose, q.pose7, sizeof(a.pose));
-        memcpy(a.plane, q.plane4 ? q.plane4 : kNoPlane, sizeof(a.plane));
-        a.slot = q.kf_slot; a.off = t->arena_used; a.cnt = q.n_meas; a.cam_zero = q.cam ? 0 : 1;
-        t->m_off[q.kf_slot] = t->arena_used; t->m_cnt[q.kf_slot] = q.n_meas; t->kf_live[q.kf_slot] = 1;
-        t->arena_used += q.n_meas;
-        t->gen++;
-        t->h2d_push += (int64_t)q.n_meas * 20 + 11 * 8;
+        app[w] = append_plan(r[w].t, q.kf_slot, q.n_meas, q.pose7, q.plane4, q.cam == nullptr, ct, runs, max_run);
     }
     // ---- segments, flushed when the staging's rows are full (the first flush carries the compactions)
     const size_t rec = align16(sizeof(CompactTrack) * ct.size()) + align16(sizeof(CompactRun) * runs.size()) +
@@ -4364,6 +4375,412 @@ int kba_track_group_keyframe_solve(kba_track_group* g, const kba_kfsolve_request
 int kba_track_group_keyframe_solve_opts(kba_track_group* g, const kba_kfsolve_request* req, const kba_options* opts,
                                         kba_kfsolve_out* out, kba_result* res) {
     return group_keyframe_solve(g, req, true, opts, out, res, "kba_track_group_keyframe_solve_opts: ");
+}
+
+// ---------------------------------------------------------------------------------------------------------------------
+// limo's frame step as one store call (include/kba_b200.h, kba_track_frame_step and its group forms; kernels in kba_framestep.cu,
+// kba_motion.cu, kba_keyframe.cu, kba_store.cu, kba_create.cu).  One upload stages every window's frame once; one launch
+// sequence gathers the adjusted frames' selected runs (k_fs_gather), adjusts their poses and computes the flow from the staged
+// columns; one download brings back what the host's verdict needs.  The selected windows then append the staged columns (the
+// adjusted pose read from device memory) and create their landmarks: one more upload of records and one more download.
+// ---------------------------------------------------------------------------------------------------------------------
+// KeyframeSelectionSchemePose's angle: calcQuaternionDiff of the facade (mini_eigen.hpp), the angle of AngleAxisd(q1.inverse() *
+// q0), in its operation order (limo_b200/keyframe_selector.py states the same), on the host: atan2 has no bit-exact device twin
+static double quaternion_diff(const double* p0, const double* p1) {
+    const double w0 = p0[0], x0 = p0[1], y0 = p0[2], z0 = p0[3];
+    const double w1 = p1[0], x1 = p1[1], y1 = p1[2], z1 = p1[3];
+    const double n = w1 * w1 + x1 * x1 + y1 * y1 + z1 * z1;
+    const double aw = w1 / n, ax = -x1 / n, ay = -y1 / n, az = -z1 / n;
+    const double qw = aw * w0 - ax * x0 - ay * y0 - az * z0;
+    const double qx = aw * x0 + ax * w0 + ay * z0 - az * y0;
+    const double qy = aw * y0 - ax * z0 + ay * w0 + az * x0;
+    const double qz = aw * z0 + ax * y0 - ay * x0 + az * w0;
+    const double sn = std::sqrt(qx * qx + qy * qy + qz * qz);
+    return sn != 0.0 ? 2.0 * std::atan2(sn, std::fabs(qw)) : 0.0;
+}
+
+// one live request's place in the call (byte offsets into the staging)
+struct StepWin {
+    kba_track* t = nullptr;
+    int i = 0;                             // track index in the set
+    const kba_frame_step_request* q = nullptr;
+    int n_runs = 0, sel_runs = 0, sel_meas = 0, rounds = 0, max_meas = 0;
+    bool adjusted = false;                 // a pose-only frame of the launch: adjust set and a run selected
+    int a = -1;                            // its index among the adjusted frames
+    int src = 0, flag0 = 0;                // its rows of the staged columns, its first run flag
+    size_t u_list = 0;                     // kf_slot | kf_new | new_slot
+    size_t d_pose = 0, d_flow = 0, d_match = 0, d_create = 0;
+    bool selected = false;
+    double angle = 0.;
+    unsigned char verdict[3] = {0, 0, 0};
+};
+
+// every check of one request that needs only the request; allocates the track's upkeep and creation scratch at their first use
+static int step_check(kba_track* t, const kba_frame_step_request& q, const kba_frame_step_out* o, const kba_options* opt,
+                      StepWin& w, std::string& why) {
+    if (!o || !q.kf_slot || !q.pose7 || (q.n_meas > 0 && (!q.lm_slot || !q.u || !q.v || !q.d || !q.run_sel)) ||
+        (q.n_new > 0 && (!q.new_slot || !o->pos || !o->flags))) {
+        why = "null argument"; return KBA_ERR_BAD_ARG;
+    }
+    if (q.n_kf < 1 || q.n_meas < 0 || q.n_new < 0) { why = "no keyframes or a negative size"; return KBA_ERR_BAD_ARG; }
+    if (q.n_kf + 1 > t->td.kf_cap || q.n_new > t->td.lm_cap) { why = "more keyframes or landmarks than the track's slots"; return KBA_ERR_CAPACITY; }
+    if (q.kf_new < 0 || q.kf_new >= t->td.kf_cap) { why = "kf_new out of range"; return KBA_ERR_BAD_ARG; }
+    if (t->kf_live[q.kf_new]) { why = "kf_new in use (drop it first)"; return KBA_ERR_BAD_ARG; }
+    if (q.n_meas > t->caps.win_observations) { why = "more measurements than win_observations"; return KBA_ERR_CAPACITY; }
+    if (q.adjust) {
+        const int rc = options_check(opt, why);
+        if (rc != KBA_OK) return rc;
+        if (q.speed_weight > 0 && !(q.speed_dt > 0)) { why = "speed prior: dt <= 0"; return KBA_ERR_BAD_ARG; }
+    }
+    const cudaError_t e = cudaSetDevice(t->set.h->device);
+    if (e != cudaSuccess) { why = std::string("cudaSetDevice: ") + cudaGetErrorString(e); return KBA_ERR_CUDA; }
+    int rc = upkeep_bufs(t, why);
+    if (rc == KBA_OK && !t->create) rc = create_alloc(t, why);
+    if (rc == KBA_OK) rc = check_slot_lists(t, q.n_kf, q.kf_slot, q.n_new, q.new_slot, w.max_meas, why);
+    if (rc != KBA_OK) return rc;
+    // the run contract, as the flow and pose-only calls check it
+    SlotStamps& st = t->stamps;
+    st.next();
+    w.n_runs = w.sel_runs = w.sel_meas = 0;
+    for (int i = 0; i < q.n_meas; ++i) {
+        const int sl = q.lm_slot[i], c = q.cam ? q.cam[i] : 0;
+        if (sl < 0 || sl >= t->td.lm_cap) { why = "landmark slot out of range"; return KBA_ERR_BAD_ARG; }
+        if (c < 0 || c >= t->n_cam) { why = "camera out of range"; return KBA_ERR_BAD_ARG; }
+        if (i > 0 && sl == q.lm_slot[i - 1]) {
+            if (c <= (q.cam ? q.cam[i - 1] : 0)) { why = "camera not ascending inside a run"; return KBA_ERR_BAD_ARG; }
+        } else {
+            if (st.lm[sl] == st.cur) { why = "landmark slot reappears after its run"; return KBA_ERR_BAD_ARG; }
+            st.lm[sl] = st.cur;
+            w.sel_runs += q.run_sel[w.n_runs] ? 1 : 0;
+            ++w.n_runs;
+        }
+        w.sel_meas += q.run_sel[w.n_runs - 1] ? 1 : 0;
+    }
+    w.adjusted = q.adjust && w.sel_runs > 0;
+    if (w.adjusted && w.sel_runs > t->caps.win_landmarks) { why = "more selected landmarks than win_landmarks"; return KBA_ERR_CAPACITY; }
+    long long live = 0;
+    for (int k = 0; k < t->td.kf_cap; ++k) live += t->kf_live[k] ? t->m_cnt[k] : 0;
+    if (live + q.n_meas > t->td.m_cap) { why = "measurement arena full"; return KBA_ERR_CAPACITY; }
+    w.rounds = opt->num_trim_rounds;  // k_reset_state's rule on the frame's landmark count, as frame_check
+    if (w.rounds < 0) w.rounds = (w.sel_runs > opt->min_landmarks_for_trimming) ? opt->num_rounds_option : 0;
+    if (w.rounds > 6) w.rounds = 6;
+    w.max_meas = std::max(w.max_meas, q.n_meas);  // the creation lists the new keyframe too
+    return KBA_OK;
+}
+
+// one frame step of the tracks of s (group = false: a single call), req[i] / out[i] / res[i] track i's
+static int set_frame_step(TrackSet& s, bool group, const std::string& who, const kba_frame_step_request* req, bool per_track,
+                          const kba_options* opts, kba_frame_step_out* out, kba_result* res) {
+    const int n = (int)s.tracks.size();
+    std::vector<StepWin> ws;
+    for (int i = 0; i < n; ++i) {
+        if (group && req[i].n_kf == 0) continue;
+        StepWin w;
+        w.t = s.tracks[i]; w.i = i; w.q = &req[i];
+        std::string why;
+        const int rc = step_check(w.t, req[i], out + i, &opts[per_track ? i : 0], w, why);
+        if (rc != KBA_OK) return fail(rc, who + track_prefix(group, i) + why);
+        ws.push_back(w);
+    }
+    for (int i = 0; i < n; ++i) idle_result(res[i]);  // written below for the adjusted frames
+    if (ws.empty()) {  // no upload, no launch
+        s.last = &kNoTransfer;
+        return KBA_OK;
+    }
+    kba_handle* h = s.h;
+    CU(cudaSetDevice(h->device));
+    cudaStream_t cs = h->stream;
+    TrackSolver& sv = s.solver;
+    if (motion_alloc(sv.motion, n, s.tracks.data()) != KBA_OK) return fail(KBA_ERR_CUDA, who + "out of memory for the pose-only buffers");
+    MotionBufs& mb = *sv.motion;
+    const int W = (int)ws.size();
+    // ---- layout.  up: step records | flow records | frame descriptors | solver options | columns lm, cam, u, v, d | lists | run
+    // flags, then the second phase's records; down: frame results | iteration records | flow records | kf_last poses | match
+    // indices | rejections, then the creations' positions | flags
+    int A = 0, N = 0, Rn = 0, log_cap = 0, R_all = 0;
+    size_t n_lists = 0, n_new = 0, kf_caps = 0;
+    FlowGrid fg;
+    for (StepWin& w : ws) {
+        const kba_frame_step_request& q = *w.q;
+        w.src = N; w.flag0 = R_all;
+        N += q.n_meas; R_all += w.n_runs;
+        n_lists += (size_t)q.n_kf + 1 + q.n_new; n_new += (size_t)q.n_new; kf_caps += (size_t)w.t->td.kf_cap;
+        fg.max_last = std::max(fg.max_last, w.t->m_cnt[q.kf_slot[q.n_kf - 1]]);
+        if (w.adjusted) {
+            w.a = A++; Rn += w.sel_runs;
+            const kba_result& r = res[w.i];
+            if (r.iterations) log_cap = std::max(log_cap, std::min(r.iterations_capacity, kIterLogCap));
+        }
+    }
+    Bump up, dn;
+    const size_t o_step = up.take(sizeof(StepArgs) * (size_t)W), o_flow = up.take(sizeof(FlowArgs) * (size_t)W);
+    const size_t o_fd = up.take(sizeof(FrameDesc) * (size_t)A), o_sp = up.take(sizeof(SolveParams) * (size_t)A);
+    const size_t o_cols = up.take(20 * (size_t)N, 4);
+    for (StepWin& w : ws) w.u_list = up.take(4 * ((size_t)w.q->n_kf + 1 + w.q->n_new), 4);
+    const size_t o_flags = up.take((size_t)R_all, 1), up1 = up.at;
+    const size_t o_fr = dn.take(sizeof(FrameRes) * (size_t)A), o_log = dn.take(sizeof(IterRecord) * (size_t)A * log_cap);
+    const size_t o_fres = dn.take(sizeof(FlowRes) * (size_t)W), o_pose = dn.take(56 * (size_t)W);
+    const size_t o_match = dn.take(4 * (size_t)N, 4), o_rej = dn.take((size_t)Rn, 1), down1 = dn.at;
+    // the second phase at its largest: every window selected and compacting
+    Bump up2 = up, dn2 = dn;
+    up2.take(0);
+    const size_t up2_0 = up2.at;
+    up2.take((sizeof(StoreAppend) + sizeof(CreateArgs) + sizeof(CompactTrack)) * (size_t)W + sizeof(CompactRun) * kf_caps);
+    dn2.take(0);
+    const size_t dn2_0 = dn2.at;
+    dn2.take(25 * n_new);
+    std::unique_ptr<StoreStage>& stage = s.stage[kFrameStepCall];
+    if (!stage || stage->up.n < up2.at || stage->out.n < dn2.at) {  // grow-only: a call no larger than an earlier one allocates nothing
+        std::unique_ptr<StoreStage> fresh(new StoreStage());
+        if (fresh->alloc(std::max(up2.at, stage ? stage->up.n : 0), std::max(dn2.at, stage ? stage->out.n : 0)))
+            return fail(KBA_ERR_CUDA, who + "out of memory for the frame step staging");
+        stage = std::move(fresh);
+    }
+    StoreStage& st = *stage;
+    unsigned char* uh = st.up.h, *od = st.out.d;
+    const unsigned char* ud = st.up.d;
+    // ---- staging: the columns, lists and flags once; the records of the gather, the adjustment and the flow
+    unsigned* cols_h = reinterpret_cast<unsigned*>(uh + o_cols);
+    const unsigned* cols_d = reinterpret_cast<const unsigned*>(ud + o_cols);
+    StepArgs* step_h = reinterpret_cast<StepArgs*>(uh + o_step);
+    FlowArgs* flow_h = reinterpret_cast<FlowArgs*>(uh + o_flow);
+    FrameDesc* fd = reinterpret_cast<FrameDesc*>(uh + o_fd);
+    SolveParams* sp = reinterpret_cast<SolveParams*>(uh + o_sp);
+    const size_t m_cols = MotionBufs::al(sizeof(FrameDesc) * (size_t)mb.frames_cap) + MotionBufs::al(sizeof(SolveParams) * (size_t)mb.frames_cap);
+    const size_t m_lm = m_cols + MotionBufs::al(4 * ((size_t)Rn + A)), m_stride = MotionBufs::al(4 * (size_t)std::max(N, 1));
+    int mo = 0, ro = 0, rso = 0;
+    for (int v = 0; v < W; ++v) {
+        StepWin& w = ws[v];
+        kba_track* t = w.t;
+        const kba_frame_step_request& q = *w.q;
+        const size_t m = (size_t)q.n_meas, b = 4 * m;
+        if (m) {
+            memcpy(cols_h + w.src, q.lm_slot, b);
+            if (q.cam) memcpy(cols_h + N + w.src, q.cam, b); else memset(cols_h + N + w.src, 0, b);
+            memcpy(cols_h + 2 * (size_t)N + w.src, q.u, b);
+            memcpy(cols_h + 3 * (size_t)N + w.src, q.v, b);
+            memcpy(cols_h + 4 * (size_t)N + w.src, q.d, b);
+            memcpy(uh + o_flags + w.flag0, q.run_sel, (size_t)w.n_runs);
+        }
+        int* lh = reinterpret_cast<int*>(uh + w.u_list);
+        memcpy(lh, q.kf_slot, 4 * (size_t)q.n_kf);
+        lh[q.n_kf] = q.kf_new;
+        if (q.n_new) memcpy(lh + q.n_kf + 1, q.new_slot, 4 * (size_t)q.n_new);
+        w.d_pose = o_pose + 56 * (size_t)v; w.d_flow = o_fres + sizeof(FlowRes) * (size_t)v; w.d_match = o_match + 4 * (size_t)w.src;
+        const int kf_last = q.kf_slot[q.n_kf - 1];
+        StepArgs sa;
+        sa.src = w.src; sa.n_meas = q.n_meas; sa.flag0 = w.flag0; sa.adjust = w.adjusted ? 1 : 0;
+        sa.kf_pose = t->td.kf_pose + 7 * (size_t)kf_last; sa.last_pose = reinterpret_cast<double*>(od + w.d_pose);
+        if (w.adjusted) {
+            sa.meas_off = mo; sa.rs_off = rso;
+            FrameDesc& d = fd[w.a];
+            d.n_meas = w.sel_meas; d.n_runs = w.sel_runs; d.meas_off = mo; d.run_off = ro; d.rs_off = rso; d.rounds_total = w.rounds;
+            sp[w.a] = make_params(&opts[per_track ? w.i : 0]);
+            d.lm_pos = t->td.lm_pos; d.lm_weight = t->td.lm_weight;
+            d.cam16 = t->set.solver.batch->bd.cam + (size_t)t->set.solver.batch->desc_h[0].cam_off * kCamStride; d.n_cam = t->n_cam; d.pad = 0;
+            memcpy(d.pose7, q.pose7, sizeof(d.pose7));
+            d.speed_weight = q.speed_weight; d.speed_dt = q.speed_dt;
+            memcpy(d.speed_v_before, q.speed_v_before, sizeof(d.speed_v_before));
+            memcpy(d.speed_T_origin_before, q.speed_T_origin_before, sizeof(d.speed_T_origin_before));
+            mo += w.sel_meas; ro += w.sel_runs; rso += w.sel_runs + 1;
+        }
+        step_h[v] = sa;
+        UpkeepBufs& ub = *t->upkeep;
+        if (ub.stamp >= 0xfffffff0u) {  // the stamps wrap: the map starts over from all 0
+            CU(cudaMemsetAsync(ub.map, 0, sizeof(unsigned long long) * (size_t)t->td.lm_cap, cs));
+            ub.stamp = 0;
+        }
+        FlowArgs fa;
+        fa.td = t->td;
+        fa.kf_last = kf_last; fa.n_meas = q.n_meas;
+        fa.lm_slot = reinterpret_cast<const int*>(cols_d + w.src); fa.cam = reinterpret_cast<const int*>(cols_d + N + w.src);
+        fa.u = reinterpret_cast<const float*>(cols_d + 2 * (size_t)N + w.src); fa.v = reinterpret_cast<const float*>(cols_d + 3 * (size_t)N + w.src);
+        fa.min_median_flow = q.min_median_flow;
+        fa.stamp = ++ub.stamp;
+        fa.map = ub.map;
+        fa.res = reinterpret_cast<FlowRes*>(od + w.d_flow);
+        fa.match = reinterpret_cast<int*>(od + w.d_match);
+        flow_h[v] = fa;
+    }
+    StepLaunch gl;
+    gl.win = reinterpret_cast<const StepArgs*>(ud + o_step);
+    gl.cols = cols_d; gl.stride = N; gl.run_sel = ud + o_flags; gl.n_win = W;
+    unsigned char* md = mb.up.d;
+    for (int c = 0; c < 5; ++c) gl.dst[c] = reinterpret_cast<unsigned*>(md + m_lm + (size_t)c * m_stride);
+    gl.run_start = reinterpret_cast<int*>(md + m_cols);
+    MotionArgs ma;
+    ma.fd = reinterpret_cast<const FrameDesc*>(ud + o_fd);
+    ma.sp = reinterpret_cast<const SolveParams*>(ud + o_sp);
+    ma.run_start = gl.run_start;
+    ma.lm_slot = reinterpret_cast<const int*>(gl.dst[0]); ma.cam = reinterpret_cast<const int*>(gl.dst[1]);
+    ma.u = reinterpret_cast<const float*>(gl.dst[2]); ma.v = reinterpret_cast<const float*>(gl.dst[3]); ma.d = reinterpret_cast<const float*>(gl.dst[4]);
+    ma.run_pw = mb.run_pw; ma.run_active = mb.run_active; ma.run_rej = mb.run_rej; ma.trim_val = mb.trim_val; ma.log = mb.log;
+    ma.total_runs = Rn; ma.log_cap = log_cap;
+    ma.res = reinterpret_cast<FrameRes*>(od + o_fr);
+    ma.res_log = reinterpret_cast<IterRecord*>(od + o_log);
+    ma.res_rej = od + o_rej;
+    FlowLaunch fl;
+    fl.w0 = flow_h[0];
+    fl.rest = reinterpret_cast<const FlowArgs*>(ud + o_flow) + 1;
+    fl.n_win = W;
+    // ---- one upload, one launch sequence, one download, one synchronisation
+    auto reset_maps = [&]() {  // as flow_run: after a failed sequence the maps go back to all 0
+        for (const StepWin& w : ws) cudaMemsetAsync(w.t->upkeep->map, 0, sizeof(unsigned long long) * (size_t)w.t->td.lm_cap, cs);
+        cudaStreamSynchronize(cs);
+    };
+    cudaError_t e = cudaMemcpyAsync(st.up.d, uh, up1, cudaMemcpyHostToDevice, cs);
+    if (e == cudaSuccess) {
+        launch_frame_step_gather(gl, cs);
+        e = cudaEventRecord(mb.ev0, cs);
+    }
+    if (e == cudaSuccess) {
+        if (A > 0) launch_adjust_pose(ma, A, cs);
+        e = cudaEventRecord(mb.ev1, cs);
+    }
+    if (e == cudaSuccess) {
+        launch_frame_flow(fl, fg, cs);
+        e = cudaGetLastError();
+    }
+    if (e == cudaSuccess) e = cudaMemcpyAsync(st.out.h, od, down1, cudaMemcpyDeviceToHost, cs);
+    if (e == cudaSuccess) e = wait_stream(h);
+    if (e != cudaSuccess) {
+        reset_maps();
+        return fail(KBA_ERR_CUDA, who + "frame step: " + cudaGetErrorString(e));
+    }
+    float ms = 0.f;
+    if (A > 0) {
+        h->counters.launches_total += 1;
+        CU(cudaEventElapsedTime(&ms, mb.ev0, mb.ev1));
+    }
+    // ---- the verdicts (KeyframeSelector::select({frame}, active keyframes): flow and (pose or time))
+    const unsigned char* oh = st.out.h;
+    const FrameRes* fr = reinterpret_cast<const FrameRes*>(oh + o_fr);
+    std::vector<int> sel;
+    for (int v = 0; v < W; ++v) {
+        StepWin& w = ws[v];
+        const kba_frame_step_request& q = *w.q;
+        const FlowRes& f = *reinterpret_cast<const FlowRes*>(oh + w.d_flow);
+        const double* pose = w.adjusted ? fr[w.a].pose : q.pose7;
+        w.angle = quaternion_diff(pose, reinterpret_cast<const double*>(oh + w.d_pose));
+        w.verdict[0] = q.n_meas > 0 && f.usable;
+        w.verdict[1] = w.angle > q.critical_quaternion_diff;
+        w.verdict[2] = q.stamp - q.stamp_last > q.time_difference_ns;
+        w.selected = w.verdict[0] && (w.verdict[1] || w.verdict[2]);
+        if (w.selected) sel.push_back(v);
+    }
+    int64_t up_bytes = (int64_t)up1, down_bytes = (int64_t)down1;
+    // ---- the push and the creation of the selected windows: one upload of records, one launch sequence, one download
+    if (!sel.empty()) {
+        const int S = (int)sel.size();
+        std::vector<CompactTrack> ct;
+        std::vector<CompactRun> runs;
+        std::vector<StoreAppend> app(S);
+        std::vector<CreateArgs> cr(S);
+        int max_run = 0, max_rows = 0;
+        CreateGrid cg;
+        Bump dc;
+        dc.at = dn2_0;
+        for (int j = 0; j < S; ++j) {
+            StepWin& w = ws[sel[j]];
+            kba_track* t = w.t;
+            const kba_frame_step_request& q = *w.q;
+            StoreAppend& a = app[j];
+            a = append_plan(t, q.kf_new, q.n_meas, q.pose7, q.plane4, false, ct, runs, max_run);
+            a.seg = 0; a.n = q.n_meas; a.src = w.src;
+            if (w.adjusted) a.pose_src = reinterpret_cast<const double*>(od + o_fr) + (size_t)w.a * (sizeof(FrameRes) / sizeof(double));
+            max_rows = std::max(max_rows, q.n_meas);
+            CreateArgs c = t->create->a;
+            c.td = t->td;
+            c.kf_slot = reinterpret_cast<const int*>(ud + w.u_list); c.lm_slot = c.kf_slot + q.n_kf + 1;
+            c.n_kf = q.n_kf + 1; c.kf_new = q.n_kf; c.n_new = q.n_new;
+            w.d_create = dc.take(24 * (size_t)q.n_new);
+            c.pos = reinterpret_cast<double*>(od + w.d_create);
+            cr[j] = c;
+            t->gen++;
+            cg.max_kf = std::max(cg.max_kf, c.n_kf); cg.max_new = std::max(cg.max_new, q.n_new);
+            cg.max_init = std::max(cg.max_init, std::max(q.n_new, c.n_kf * t->n_cam));
+            cg.max_meas = std::max(cg.max_meas, w.max_meas);
+        }
+        for (int j = 0; j < S; ++j) cr[j].flags = od + dc.take((size_t)ws[sel[j]].q->n_new, 1);
+        Bump u2;
+        u2.at = up2_0;
+        const size_t o_app = u2.take(sizeof(StoreAppend) * (size_t)S), o_cr = u2.take(sizeof(CreateArgs) * (size_t)S);
+        const size_t o_ct = u2.take(sizeof(CompactTrack) * ct.size()), o_run = u2.take(sizeof(CompactRun) * runs.size());
+        memcpy(uh + o_app, app.data(), sizeof(StoreAppend) * (size_t)S);
+        memcpy(uh + o_cr, cr.data(), sizeof(CreateArgs) * (size_t)S);
+        if (!ct.empty()) memcpy(uh + o_ct, ct.data(), sizeof(CompactTrack) * ct.size());
+        if (!runs.empty()) memcpy(uh + o_run, runs.data(), sizeof(CompactRun) * runs.size());
+        CreateLaunch cl;
+        cl.w0 = cr[0];
+        cl.rest = reinterpret_cast<const CreateArgs*>(ud + o_cr) + 1;
+        cl.n_win = S;
+        e = cudaMemcpyAsync(st.up.d + up2_0, uh + up2_0, u2.at - up2_0, cudaMemcpyHostToDevice, cs);
+        if (e == cudaSuccess) {
+            launch_store_push(reinterpret_cast<const CompactTrack*>(ud + o_ct), reinterpret_cast<const CompactRun*>(ud + o_run), (int)runs.size(),
+                              max_run, reinterpret_cast<const StoreAppend*>(ud + o_app), S, max_rows, cols_d, N, cs);
+            launch_create(cl, cg, cs);
+            e = cudaGetLastError();
+        }
+        if (e == cudaSuccess) e = cudaMemcpyAsync(st.out.h + dn2_0, od + dn2_0, dc.at - dn2_0, cudaMemcpyDeviceToHost, cs);
+        if (e == cudaSuccess) e = wait_stream(h);
+        if (e != cudaSuccess) {
+            // as create_run: the slot -> request maps go back to all -1
+            for (int j = 0; j < S; ++j)
+                cudaMemsetAsync(ws[sel[j]].t->create->a.req_of, 0xff, sizeof(int) * (size_t)ws[sel[j]].t->td.lm_cap, cs);
+            cudaStreamSynchronize(cs);
+            return fail(KBA_ERR_CUDA, who + "frame step push: " + cudaGetErrorString(e));
+        }
+        up_bytes += (int64_t)(u2.at - up2_0);
+        down_bytes += (int64_t)(dc.at - dn2_0);
+        for (int j = 0; j < S; ++j) {
+            const StepWin& w = ws[sel[j]];
+            const size_t m = (size_t)w.q->n_new;
+            if (m) {
+                memcpy(out[w.i].pos, st.out.h + w.d_create, 24 * m);
+                memcpy(out[w.i].flags, st.out.h + (reinterpret_cast<const unsigned char*>(cr[j].flags) - od), m);
+            }
+        }
+    }
+    // ---- outputs
+    const IterRecord* lg = reinterpret_cast<const IterRecord*>(oh + o_log);
+    const unsigned char* rj = oh + o_rej;
+    for (const StepWin& w : ws) {
+        kba_frame_step_out& o = out[w.i];
+        const FlowRes& f = *reinterpret_cast<const FlowRes*>(oh + w.d_flow);
+        o.n_matched = f.n_matched;
+        o.flow_sum = f.flow_sum;
+        o.mean_flow_sq = mean_flow_sq(f);
+        if (o.match && w.q->n_meas) memcpy(o.match, oh + w.d_match, 4 * (size_t)w.q->n_meas);
+        o.angle = w.angle;
+        o.usable_flow = w.verdict[0]; o.usable_pose = w.verdict[1]; o.usable_time = w.verdict[2];
+        o.selected = w.selected ? 1 : 0;
+        if (w.adjusted)
+            frame_result(fr[w.a], lg + (size_t)w.a * log_cap, log_cap, rj + fd[w.a].run_off, w.sel_runs, ms, res[w.i]);
+    }
+    st.counts.h2d = up_bytes;
+    st.counts.d2h = down_bytes;
+    s.last = &st.counts;
+    return KBA_OK;
+}
+
+int kba_track_frame_step(kba_track* t, const kba_frame_step_request* req, const kba_options* opt, kba_frame_step_out* out, kba_result* res) {
+    static const std::string who = "kba_track_frame_step: ";
+    if (!t || !req || !opt || !out || !res) return fail(KBA_ERR_BAD_ARG, who + "null argument");
+    return set_frame_step(t->set, false, who, req, false, opt, out, res);
+}
+
+static int group_frame_step(kba_track_group* g, const kba_frame_step_request* req, bool per_track, const kba_options* opts,
+                            kba_frame_step_out* out, kba_result* res, const std::string& who) {
+    if (!g || !req || !opts || !out || !res) return fail(KBA_ERR_BAD_ARG, who + "null argument");
+    return set_frame_step(g->set, true, who, req, per_track, opts, out, res);
+}
+int kba_track_group_frame_step(kba_track_group* g, const kba_frame_step_request* req, const kba_options* opt, kba_frame_step_out* out,
+                               kba_result* res) {
+    return group_frame_step(g, req, false, opt, out, res, "kba_track_group_frame_step: ");
+}
+int kba_track_group_frame_step_opts(kba_track_group* g, const kba_frame_step_request* req, const kba_options* opts,
+                                    kba_frame_step_out* out, kba_result* res) {
+    return group_frame_step(g, req, true, opts, out, res, "kba_track_group_frame_step_opts: ");
 }
 
 // ---------------------------------------------------------------------------------------------------------------------

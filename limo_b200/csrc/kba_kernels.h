@@ -120,6 +120,7 @@ struct StoreAppend {
     double* kf_plane = nullptr;
     double pose[7] = {0, 0, 0, 0, 0, 0, 0};
     double plane[4] = {0, 0, 0, 0};
+    const double* pose_src = nullptr;  // [7] or null: the pose is read from device memory (a frame step's adjusted pose), not `pose`
     int slot = 0, off = 0, cnt = 0, seg = 0, n = 0, src = 0, cam_zero = 0, pad = 0;
 };
 // one track's compaction: its live keyframes' runs copied from one arena into the other.  m_off null: the runs are copied out
@@ -482,6 +483,30 @@ struct MotionArgs {
     int log_cap, total_runs;
 };
 void launch_adjust_pose(const MotionArgs& a, int n_frames, cudaStream_t s);
+
+// ---- limo's frame step on a track's store (kba_track_frame_step and its group forms, kba_framestep.cu) ----
+// One window = one request, one CTA of k_fs_gather, which runs ahead of k_adjust_pose and the flow kernels in the same sequence:
+// it copies kf_last's stored pose into the download and, for a frame that is adjusted, gathers the measurements of its selected
+// runs from the staged columns into the pose-only kernel's input (MotionArgs' lm_slot .. d and run_start at meas_off / rs_off),
+// keeping their order with a block-wide ballot scan.  The host knows the gathered sizes from its checks and writes the FrameDesc.
+struct StepArgs {
+    int src = 0, n_meas = 0;               // the window's rows of the staged columns
+    int flag0 = 0;                         // its first run flag
+    int adjust = 0;                        // 1: gather the selected runs
+    int meas_off = 0, rs_off = 0;          // where they go: MotionArgs' columns, run_start
+    const double* kf_pose = nullptr;       // [7] kf_last's stored pose
+    double* last_pose = nullptr;           // [7] its copy in the download
+};
+struct StepLaunch {
+    const StepArgs* win = nullptr;         // [n_win]
+    const unsigned* cols = nullptr;        // the staged columns lm, cam, u, v, d, `stride` words each
+    int stride = 0;
+    const unsigned char* run_sel = nullptr;  // every window's run flags, end to end
+    unsigned* dst[5] = {nullptr, nullptr, nullptr, nullptr, nullptr};  // MotionArgs' lm_slot, cam, u, v, d
+    int* run_start = nullptr;              // MotionArgs' run_start
+    int n_win = 0;
+};
+void launch_frame_step_gather(const StepLaunch& l, cudaStream_t s);
 
 cudaError_t configure_pack();
 void launch_pack(const BatchDev& bd, const PackRaw& raw, cudaStream_t s);

@@ -58,7 +58,7 @@ __global__ void __launch_bounds__(256) k_store_append(const StoreAppend* app, co
     const StoreAppend& a = app[blockIdx.x];
     const int q = blockIdx.y, i0 = blockIdx.z * kSlice;
     if (q == 0 && i0 == 0) {
-        if (threadIdx.x < 7) a.kf_pose[7 * (size_t)a.slot + threadIdx.x] = a.pose[threadIdx.x];
+        if (threadIdx.x < 7) a.kf_pose[7 * (size_t)a.slot + threadIdx.x] = a.pose_src ? a.pose_src[threadIdx.x] : a.pose[threadIdx.x];
         else if (threadIdx.x < 11) a.kf_plane[4 * (size_t)a.slot + threadIdx.x - 7] = a.plane[threadIdx.x - 7];
         else if (threadIdx.x == 32) { a.m_off[a.slot] = a.off; a.m_cnt[a.slot] = a.cnt; }
     }
