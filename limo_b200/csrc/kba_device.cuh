@@ -378,15 +378,19 @@ __device__ inline bool eval_observation(const T* __restrict__ pose, const T* __r
 // as soon as it is formed, so at most one 3-vector m and the rotated point a stay live (64 registers -> 4 CTAs/SM).
 // res/jp/jl point at this observation's slot of component 0; `stride` is the component stride (total observations).
 // kJl: also store J_landmark (panel path)
-template <typename T, bool kJl = true>
+// kArm: p and the translation of `pose` are taken relative to an anchor c (p - c and t + R c), so that x = R (p - c) + (t + R c)
+// is formed from window-sized terms; arm = R c restores the rotation columns' lever arm a = R p = R (p - c) + R c, since the
+// parametrisation rotates about the origin, not about c
+template <typename T, bool kJl = true, bool kArm = false>
 __device__ inline bool eval_observation_store(const T* __restrict__ pose, const T* __restrict__ cam, const T p[3], T u,
                                               T v, T d, T wt, T b_repr, T b_depth, T* __restrict__ res,
                                               T* __restrict__ jp, T* __restrict__ jl, size_t stride, bool write_jp,
-                                              T& half_rho_sum) {
-    const T a0 = pose[0] * p[0] + pose[1] * p[1] + pose[2] * p[2];
-    const T a1 = pose[3] * p[0] + pose[4] * p[1] + pose[5] * p[2];
-    const T a2 = pose[6] * p[0] + pose[7] * p[1] + pose[8] * p[2];
-    const T x0 = a0 + pose[9], x1 = a1 + pose[10], x2 = a2 + pose[11];
+                                              T& half_rho_sum, const T* __restrict__ arm = nullptr) {
+    const T b0 = pose[0] * p[0] + pose[1] * p[1] + pose[2] * p[2];
+    const T b1 = pose[3] * p[0] + pose[4] * p[1] + pose[5] * p[2];
+    const T b2 = pose[6] * p[0] + pose[7] * p[1] + pose[8] * p[2];
+    const T x0 = b0 + pose[9], x1 = b1 + pose[10], x2 = b2 + pose[11];
+    const T a0 = kArm ? b0 + arm[0] : b0, a1 = kArm ? b1 + arm[1] : b1, a2 = kArm ? b2 + arm[2] : b2;
     const T c0 = cam[0] * x0 + cam[1] * x1 + cam[2] * x2 + cam[9];
     const T c1 = cam[3] * x0 + cam[4] * x1 + cam[5] * x2 + cam[10];
     const T c2 = cam[6] * x0 + cam[7] * x1 + cam[8] * x2 + cam[11];

@@ -263,6 +263,8 @@ __global__ void __launch_bounds__(256, kMinBlocks) k_eval_obs(BatchDev bd, int t
     constexpr bool kF32 = sizeof(TLin) == 4;  // FP32 evaluation + storage of the linearisation (precision 1)
     __shared__ float s_pose_f[kF32 ? kMaxKf * kPoseStride : 1];
     __shared__ float s_cam_f[kF32 ? kMaxCam * kCamStride : 1];
+    __shared__ float s_arm_f[kF32 ? kMaxKf * 3 : 1];  // R_k c: the rotation columns' lever arm at the anchor c
+    double anc[3] = {0.0, 0.0, 0.0};
     const int buf = kJac ? st.cur : 1 - st.cur;
     const double* __restrict__ lm_buf = bd.lm[buf];
     const int i0 = blockIdx.x * tiles * 256 + threadIdx.x;
@@ -289,7 +291,26 @@ __global__ void __launch_bounds__(256, kMinBlocks) k_eval_obs(BatchDev bd, int t
     }
     stage_window_bulk(wd, bd.rt[buf], bd.cam, s_pose, s_cam, &s_bar);  // poses (R | t) and cameras: two bulk copies
     if (kF32) {
-        for (int i = threadIdx.x; i < wd.n_kf * kPoseStride; i += blockDim.x) s_pose_f[i] = (float)s_pose[i];
+        // FP32 blocks are formed relative to an anchor c, keyframe 0's centre -R_0^T t_0 (FP64) on a 64 m grid: a window
+        // kilometres from the origin would otherwise round R p and t, each of the size of that distance, before they cancel
+        // to a camera-frame point of a few metres.  p - c and t_k + R_k c are formed in FP64, so x = R p + t is unchanged in
+        // exact arithmetic.  On the grid, a window whose keyframe 0 is within 32 m of the origin has c = 0 and the blocks it
+        // had without the anchor, bit for bit; any other is evaluated as if it were that close.
+        constexpr double kGrid = 64.0;
+#pragma unroll
+        for (int j = 0; j < 3; ++j)
+            anc[j] = kGrid * rint(-(s_pose[j] * s_pose[9] + s_pose[3 + j] * s_pose[10] + s_pose[6 + j] * s_pose[11]) / kGrid);
+        for (int i = threadIdx.x; i < wd.n_kf * kPoseStride; i += blockDim.x) {
+            const int k = i / kPoseStride, e = i - k * kPoseStride;
+            if (e < 9) {
+                s_pose_f[i] = (float)s_pose[i];
+            } else {
+                const double* P = s_pose + kPoseStride * k + 3 * (e - 9);
+                const double rc = P[0] * anc[0] + P[1] * anc[1] + P[2] * anc[2];
+                s_pose_f[i] = (float)(s_pose[i] + rc);
+                s_arm_f[3 * k + e - 9] = (float)rc;
+            }
+        }
         for (int i = threadIdx.x; i < wd.n_cam * kCamStride; i += blockDim.x) s_cam_f[i] = (float)s_cam[i];
         __syncthreads();
     }
@@ -328,15 +349,15 @@ __global__ void __launch_bounds__(256, kMinBlocks) k_eval_obs(BatchDev bd, int t
                     s_pose + kPoseStride * k, s_cam + kCamStride * c, p, (double)u, (double)v, (double)d, wgt,
                     s_b[0], s_b[1], r, nullptr, nullptr, hr, raw);
                 if (ok) {
-                    const float pf[3] = {(float)p0, (float)p1, (float)p2};
+                    const float pf[3] = {(float)(p0 - anc[0]), (float)(p1 - anc[1]), (float)(p2 - anc[2])};
                     float hrf;
                     float* resf = reinterpret_cast<float*>(bd.res) + o;
                     float* jpf = reinterpret_cast<float*>(bd.jp) + o;
                     float* jlf = reinterpret_cast<float*>(bd.jl) + o;
-                    eval_observation_store<float, kJl>(
+                    eval_observation_store<float, kJl, true>(
                         s_pose_f + kPoseStride * k, s_cam_f + kCamStride * c, pf, u, v, d, (float)wgt,
                         (float)s_b[0], (float)s_b[1],
-                        resf, jpf, jlf, (size_t)bd.tot_obs, row >= 0 || !kJl, hrf);
+                        resf, jpf, jlf, (size_t)bd.tot_obs, row >= 0 || !kJl, hrf, s_arm_f + 3 * k);
                 }
             } else if (kJac) {  // rows are stored to their SoA slots as they are formed
                 ok = eval_observation_store<double, kJl>(
