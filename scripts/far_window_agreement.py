@@ -32,7 +32,7 @@ def first_step(name, dist):
     win, opt, _ = tf.far_case(window, dist)
     opt.precision = precision
     h = _h()
-    ref = fs.dense_first_step(win, opt, h.evaluate(win, opt), lambda w: h.evaluate(w, opt), orc)
+    ref = fs.cuda_reference(h, orc, win, opt)
     worst = {}
     for res in h.solve_batch([win] * copies, opt, iterations_capacity=256):
         for k, v in fs._check_first_step(res, ref, 1.0, name).items():

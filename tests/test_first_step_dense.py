@@ -17,14 +17,16 @@ The windows between them select every solver path of limo_b200/csrc/kba_plan.h (
 tests/test_launch_plan.py): the fused path with and without plane rows, the seven-slot k_schur_fused<7> (windows with no fixed
 keyframe: a free gauge makes their later iterates drift along flat directions, but the first damped step is well defined), the
 large-window path with the tiled, the split (k_chol_*) and the one-CTA row-major factorisation, the 6x6 motion-only system with
-its speed prior, and FP32 observation blocks.
+its speed prior.  FP32 observation blocks (kba_options.precision = 1) run on the fused six- and seven-slot paths, the split
+factorisation with and without plane blocks, config 3's batch of 132 and (tests/test_large_reduced_rows.py) the 651-row
+k_chol_trail_band path, each held at its FP64 class against the mixed system the FP32 solve forms (dense_first_step).
 
 The Schur split (p_split: the CTAs a window's Schur sum is spread over) follows the batch size, and each case asserts it.  A
 window solved alone splits its sum over 25 .. 88 CTAs on the fused path and over 16 on the large-window path, the batch of 17
 over 5: k_sred_reduce folds the partial sums and k_reduced_solve takes A from it.  The batches of 264 (config2_slice in FP64
-and FP32, config2_kf30_lm700 with the headline's 30 keyframes), 132 (free_keyframes_30, config3_kf30_lm600) and 80
-(config5_kf40_lm700) windows run at p_split = 1, the shapes bench.py times: one CTA owns all of a window's landmark groups in
-k_schur_fused, k_schur_syrk runs at a grid depth of 1, k_sred_reduce is not launched, and k_reduced_solve gathers A from the
+and FP32, config2_kf30_lm700 with the headline's 30 keyframes), 132 (free_keyframes_30, config3_kf30_lm600 in FP64 and FP32)
+and 80 (config5_kf40_lm700) windows run at p_split = 1, the shapes bench.py times: one CTA owns all of a window's landmark
+groups in k_schur_fused, k_schur_syrk runs at a grid depth of 1, k_sred_reduce is not launched, and k_reduced_solve gathers A from the
 single sum itself, tiled or row-major.  The split factorisation at p_split = 1 (KBA_P_SPLIT=1) is in
 tests/test_bench_shapes.py.
 """
@@ -60,16 +62,21 @@ pytestmark = pytest.mark.skipif(np.finfo(LD).eps >= np.finfo(np.float64).eps, re
 # the plane chain, wrong by 1e-6 moves the records by 9e-11 .. 1.8e-10 (test_dense_step_notices_a_wrong_ground_row), so
 # GROUND_TOL sits between that and the worst ground deviation (12 times the oracle's, 36 times the CUDA path's).
 #
-# FP32 blocks (kba_options.precision = 1, config2_slice, alone and x 264): cost 1 2.8e-05, step_norm 1.1e-05,
-# relative_decrease 3.6e-05, and gradient_max_norm 1.3e-06 already in record 0.  That is not rounding of the FP64 chain: the
-# solve does not form the normal equations of the blocks kba_eval reports.  The landmark blocks and the pose-landmark coupling
-# come from the FP32 J_p and r, but k_pose_hessian re-evaluates each observation's pose rows in FP64 for the pose blocks and the pose gradient.  No single
-# Jacobian gives that system, so the reference, built from the FP32 blocks alone, differs from it by what FP32 rounding does to
-# the pose rows.  FP32_TOL is about 100 times the measured deviation and tells a working FP32 mode from a broken one.
+# FP32 blocks (kba_options.precision = 1).  The FP32 solve does not form the normal equations of the blocks kba_eval reports:
+# k_pose_hessian re-evaluates each observation's pose rows in FP64 for the pose blocks and the pose gradient, while the landmark
+# blocks, the landmark gradient and the pose-landmark coupling come from the FP32 J_p, J_l and r.  dense_first_step forms that
+# mixed system when given the FP64 blocks beside the FP32 ones (cuda_reference), and every FP32 case is held at its FP64 class.
+# Worst deviation, every window of each batch, at the origin and at 1, 5 and 10 km (tests/test_far_windows.py), measured on an
+# NVIDIA H100 80GB HBM3 (power limit 700 W) by scripts/fp32_agreement.py:
+#   plane-free (config2_slice alone and x 264, free_kf30_none_fixed, config5_kf40_lm700): 9.6e-13 (config5_kf40_lm700, 1 km;
+#     1.5e-13 at the origin)
+#   ground (config3_kf30_lm600 alone and x 132): 2.5e-13 (5 km; 1.5e-13 at the origin); the 651-row window 8.4e-14
+# The reference built from the FP32 blocks alone (the pose rows from FP32 as well) is off by 2.4e-06 .. 2.3e-04 on the same
+# cases, and one FP32 landmark Jacobian row or one FP32 residual off by 1e-6 moves the mixed reference by 7.2e-10 .. 1.5e-09
+# (config2_slice, config3_kf30_lm600): both fail the classes (test_cuda_fp32_step_is_the_mixed_system).
 STEP_TOL = 1e-10
 GROUND_TOL = 1e-11
-FP32_TOL = 4e-3
-TOL = {"plane_free": STEP_TOL, "ground": GROUND_TOL, "fp32": FP32_TOL}
+TOL = {"plane_free": STEP_TOL, "ground": GROUND_TOL}
 
 
 def _shapes(name):
@@ -134,8 +141,13 @@ OPTION_HOOKS = {"motion_only_speed_prior": _motion_options}
 CUDA_CASES = dict({name: (name, 0, 1, {}) for name in WINDOWS},
                   # 17 windows: more than the split factorisation takes, so k_reduced_solve factorises each in one CTA
                   config5_kf40_lm700_batch17=("config5_kf40_lm700", 0, 17, dict(p_split=5, solve_tiled=0, solve_split=0)),
-                  # FP32 observation blocks (k_eval_obs<float>), everything after them in FP64
+                  # FP32 observation blocks (k_eval_obs<float>), everything after them in FP64, on every path they take: the
+                  # fused six- and seven-slot kernels, the split (k_chol_*) factorisation with and without plane blocks, and
+                  # config 3's sub-record shape below
                   config2_slice_fp32=("config2_slice", 1, 1, {}),
+                  free_kf30_none_fixed_fp32=("free_kf30_none_fixed", 1, 1, {}),
+                  config3_kf30_lm600_fp32=("config3_kf30_lm600", 1, 1, {}),
+                  config5_kf40_lm700_fp32=("config5_kf40_lm700", 1, 1, {}),
                   # The batch sizes bench.py times put each window's Schur sum on one CTA (p_split = 1): k_sred_reduce is not
                   # launched and k_reduced_solve gathers A from the sums itself.  264 windows: bench.py's headline batch, the
                   # fused six-slot kernel with one CTA owning all of a window's landmark groups, then the tiled solve
@@ -146,6 +158,7 @@ CUDA_CASES = dict({name: (name, 0, 1, {}) for name in WINDOWS},
                   free_keyframes_30_batch132=("free_keyframes_30", 0, 132, dict(p_split=1, solve_tiled=1, solve_split=0)),
                   # 132 windows: config 3's sub-record shape, the row-major k_reduced_solve<false> in one CTA per window
                   config3_kf30_lm600_batch132=("config3_kf30_lm600", 0, 132, dict(p_split=1, solve_tiled=0, solve_split=0)),
+                  config3_kf30_lm600_fp32_batch132=("config3_kf30_lm600", 1, 132, dict(p_split=1, solve_tiled=0, solve_split=0)),
                   # the same plane-free; 80 is the smallest batch for which syrk_split(256, n, 132) == 1
                   config5_kf40_lm700_batch80=("config5_kf40_lm700", 0, 80, dict(p_split=1, solve_tiled=0, solve_split=0)))
 
@@ -297,36 +310,63 @@ def _planes(win):
     return np.tile([0.0, 0.0, 1.0, 0.0], (win.n_kf, 1)) if win.kf_plane is None else win.kf_plane.copy()
 
 
-def dense_first_step(win, opt, blocks, evaluate, orc, tamper=None):
+def dense_first_step(win, opt, blocks, evaluate, orc, tamper=None, fp64_blocks=None):
     """Records 0 and 1 of the first inner solve as a dense reference gives them.
 
     blocks: (r [n_obs, 3], jac_pose [n_obs, 3, 6], jac_lm [n_obs, 3, 3], cost) of the observations at the window's state;
     evaluate(window) returns the same tuple (the candidate's observation cost is taken from it); orc: the oracle binding (its
     single-residual functions).  tamper(rows), if given, may change the residual blocks at the window's state before the system
     is formed (the negative controls).  The Jacobian is never stored densely (18 000 x 2 300 longdoubles); J^T J and J^T r are
-    summed from its blocks, which is the same matrix."""
+    summed from its blocks, which is the same matrix.
+
+    fp64_blocks: the FP64 blocks of the same observations (kba_eval at precision 0), given with the FP32 `blocks` of
+    kba_options.precision = 1.  The FP32 solve does not form the normal equations of one Jacobian but a mixed system, and with
+    both sets given the reference forms that system:
+      - k_pose_hessian re-evaluates every observation's pose rows in FP64: the pose-pose blocks B_k = sum J_p^T J_p, the pose
+        gradient g_k = sum J_p^T r and so the pose columns' Jacobi norms (the diagonal of B_k, k_reduced_solve) come from the
+        rows of `fp64_blocks`;
+      - k_landmark_reduce sums C_j = sum J_l^T J_l and g_j = sum J_l^T r (and the landmark columns' Jacobi norms) from the FP32
+        J_l and r, and k_obs_v / k_obs_v2 the coupling J_p^T J_l from the FP32 J_p and J_l, each widened to FP64 (lin_load).  The
+        J_l is the stored FP32 one on the large-window path (k_eval_obs<float, true>) and the FP32 translation columns times R
+        formed in FP64 on the fused path (k_eval_obs<float, false>); kba_eval reports whichever the window's path consumes;
+      - ground rows, the plane chain and the regularisers are FP64 either way (k_gp_eval, k_reduced_solve).
+    Then the model decrease is the one k_reduced_solve and k_backsub form from that g, the step and the damping,
+    (-g^T delta + delta^T Lambda delta) / 2 with Lambda the damping in unscaled columns, summed to k_lm_update's model_change: the
+    row form -(J delta)^T (r + J delta / 2) equals it only for a consistent Jacobian.  gradient_max_norm is taken from the same
+    g."""
     r, jp, jl = (np.asarray(a, dtype=LD) for a in blocks[:3])
     L = program_columns(win)
     n = L.n
     lm_of_obs = np.repeat(np.arange(win.n_lm), np.diff(np.asarray(win.lm_obs_ptr)))
     kf_of_obs = np.asarray(win.obs_kf)
     planes0 = _planes(win)
+    mixed = fp64_blocks is not None
+    if mixed:
+        r64, jp64 = (np.asarray(a, dtype=LD) for a in fp64_blocks[:2])
 
-    rows = [SimpleNamespace(kind="observation", r=r[o], parts=[(c, J) for c, J in ((L.pose.get(int(kf_of_obs[o])), jp[o]),
-                                                                                    (L.lm[lm_of_obs[o]], jl[o]))
+    rows = []
+    for o in range(win.n_obs):
+        pc = L.pose.get(int(kf_of_obs[o]))
+        rw = SimpleNamespace(kind="observation", r=r[o], parts=[(c, J) for c, J in ((pc, jp[o]), (L.lm[lm_of_obs[o]], jl[o]))
                                                                 if c is not None and c >= 0])
-            for o in range(win.n_obs)]
+        # the pose part, when there is one, is the row's first: its J^T J and J^T r come from the FP64 row
+        rw.pose64 = (jp64[o], r64[o]) if mixed and pc is not None else None
+        rows.append(rw)
     more, other_cost = other_rows(win, opt, orc, L, win.kf_pose, planes0, win.lm_pos)
     rows += more
     if tamper:
         tamper(rows)
     rows = [(np.concatenate([np.arange(c, c + J.shape[1]) for c, J in rw.parts]), np.concatenate([J for _, J in rw.parts], axis=1),
-             rw.r) for rw in rows if rw.parts]
+             rw.r, getattr(rw, "pose64", None)) for rw in rows if rw.parts]
 
     H, g = np.zeros((n, n), dtype=LD), np.zeros(n, dtype=LD)
-    for cols, vals, res in rows:
-        H[np.ix_(cols, cols)] += vals.T @ vals
-        g[cols] += vals.T @ res
+    for cols, vals, res, pose64 in rows:
+        M, v = vals.T @ vals, vals.T @ res
+        if pose64 is not None:
+            M[:6, :6] = pose64[0].T @ pose64[0]
+            v[:6] = pose64[0].T @ pose64[1]
+        H[np.ix_(cols, cols)] += M
+        g[cols] += v
     c = np.diag(H).copy()                                   # squared column norms
     s = 1 / (1 + np.sqrt(c))                                # Jacobi scaling, taken once at the first iterate
     radius = LD(opt.initial_trust_region_radius)
@@ -334,10 +374,13 @@ def dense_first_step(win, opt, blocks, evaluate, orc, tamper=None):
     A = H * s[:, None] * s[None, :]
     A[np.diag_indices(n)] += D
     delta = s * _solve_spd(A, -s * g)
-    model = LD(0)                                           # -(J delta)^T (r + J delta / 2)
-    for cols, vals, res in rows:
-        jd = vals @ delta[cols]
-        model -= jd @ (res + jd / 2)
+    if mixed:                                               # (-g^T delta + delta^T Lambda delta) / 2, Lambda = D / s^2
+        model = (-(g @ delta) + (D / (s * s)) @ (delta * delta)) / 2
+    else:                                                   # -(J delta)^T (r + J delta / 2)
+        model = LD(0)
+        for cols, vals, res, _ in rows:
+            jd = vals @ delta[cols]
+            model -= jd @ (res + jd / 2)
 
     def blocks_of(poses, planes, lms):
         """the variable blocks of a state in ambient coordinates, one vector"""
@@ -424,6 +467,51 @@ def test_dense_step_notices_a_wrong_block(oracle):
         _check_first_step(oracle.solve_window(win, opt), ref, STEP_TOL, "perturbed")
 
 
+# The mixed system of the FP32 mode with both block sets the same is the system of one Jacobian: worst deviation from the row
+# form over the windows below 3.8e-18 (CPU, x86 80-bit longdouble); MIXED_SELF_TOL is 26 times it.  One landmark Jacobian row
+# or one residual of the observation with the largest residual, off by 1e-6, moves the records by 7.2e-10 .. 5.8e-09.
+MIXED_SELF_TOL = 1e-16
+RECORD_FIELDS = ("cost0", "gradient_max_norm0", "step_norm", "cost_change", "relative_decrease", "cost1", "radius1")
+
+
+def record_deviation(a, b):
+    """largest relative difference between the records of two dense steps (cost_change in units of the cost)"""
+    scale = dict(cost_change=b.cost0)
+    return max(abs(getattr(a, f) - getattr(b, f)) / abs(scale.get(f, getattr(b, f))) for f in RECORD_FIELDS)
+
+
+def tampered(blocks, what, factor=1 + 1e-6):
+    """a copy of observation blocks with the residual (what="r") or the first landmark Jacobian row (what="jl") of the
+    observation with the largest residual times `factor`"""
+    r, jp, jl = (np.array(a, copy=True) for a in blocks[:3])
+    o = int(np.argmax(np.linalg.norm(r, axis=1)))
+    if what == "r":
+        r[o] *= factor
+    else:
+        jl[o, 0] *= factor
+    return (r, jp, jl) + tuple(blocks[3:])
+
+
+@pytest.mark.parametrize("name", ["config2_slice", "free_kf30_none_fixed", "config3_kf30_lm600", "config5_kf40_lm700"])
+def test_mixed_system_of_equal_blocks_is_the_dense_step(oracle, name):
+    """dense_first_step's mixed system (FP64 pose rows beside the FP32 blocks) given the oracle's FP64 blocks twice is the
+    system of one Jacobian: its records are the row form's to MIXED_SELF_TOL, and the oracle's step still meets its class.  And
+    it can fail: one landmark Jacobian row or one residual of the second set, off by 1e-6, moves it out of the class"""
+    win, opt = build(name)
+    tol = TOL[WINDOWS[name][1]]
+    blocks = oracle.evaluate(win, opt)
+    ev = lambda w: oracle.evaluate(w, opt)  # noqa: E731
+    ref = dense_first_step(win, opt, blocks, ev, oracle)
+    mixed = dense_first_step(win, opt, blocks, ev, oracle, fp64_blocks=blocks)
+    assert record_deviation(mixed, ref) <= MIXED_SELF_TOL
+    res = oracle.solve_window(win, opt)
+    _check_first_step(res, mixed, tol, name)
+    for what in ("jl", "r"):
+        bad = dense_first_step(win, opt, tampered(blocks, what), ev, oracle, fp64_blocks=blocks)
+        with pytest.raises(AssertionError):
+            _check_first_step(res, bad, tol, "%s, %s perturbed" % (name, what))
+
+
 def _scale_part(kind, which, part, factor):
     """tamper(): the `part`-th Jacobian part of the `which`-th residual block of `kind` times `factor`"""
     def tamper(rows):
@@ -474,14 +562,27 @@ def handle():
     h.close()
 
 
+def cuda_reference(handle, oracle, win, opt, fp32_pose_rows=False, **kw):
+    """the dense step of a window from the blocks kba_eval reports under `opt`.  Under precision 1 it is the mixed system the
+    FP32 solve forms (dense_first_step): the FP64 blocks, for the pose rows, are evaluated beside the FP32 ones.
+    fp32_pose_rows: take the pose rows from the FP32 blocks as well (one Jacobian for the whole system; a negative control)."""
+    blocks = handle.evaluate(win, opt)
+    fp64 = None
+    if opt.precision and not fp32_pose_rows:
+        opt.precision = 0
+        fp64 = handle.evaluate(win, opt)
+        opt.precision = 1
+    return dense_first_step(win, opt, blocks, lambda w: handle.evaluate(w, opt), oracle, fp64_blocks=fp64, **kw)
+
+
 def cuda_first_step(handle, oracle, name):
     """(the dense step of a CUDA case from kba_eval's blocks, the kba_solve_batch results of its copies, tolerance class)"""
     window, precision, copies, _ = CUDA_CASES[name]
     win, opt = build(window)
     opt.precision = precision
-    ref = dense_first_step(win, opt, handle.evaluate(win, opt), lambda w: handle.evaluate(w, opt), oracle)
+    ref = cuda_reference(handle, oracle, win, opt)
     results = handle.solve_batch([win] * copies, opt, iterations_capacity=256)
-    return ref, results, "fp32" if precision else WINDOWS[window][1]
+    return ref, results, WINDOWS[window][1]
 
 
 @pytest.mark.gpu
@@ -496,3 +597,27 @@ def test_cuda_first_step_matches_dense_step(handle, oracle, driver, name):  # no
     for i, res in enumerate(results):
         assert res.c.status == 0
         _check_first_step(res, ref, TOL[tol], "%s, window %d" % (name, i))
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("name", ["config2_slice", "config3_kf30_lm600"])
+def test_cuda_fp32_step_is_the_mixed_system(handle, oracle, name):
+    """the tight classes tell the FP32 solve's system from a near one, on the fused and on the large-window path: the mixed
+    reference holds, and each of these fails -- the reference of one Jacobian, its pose rows from the FP32 blocks too; the
+    mixed reference with one FP32 landmark Jacobian row, or one FP32 residual, off by 1e-6"""
+    win, opt = build(name)
+    opt.precision = 1
+    tol = TOL[WINDOWS[name][1]]
+    [res] = handle.solve_batch([win], opt, iterations_capacity=256)
+    assert res.c.status == 0
+    _check_first_step(res, cuda_reference(handle, oracle, win, opt), tol, name)
+    with pytest.raises(AssertionError):
+        _check_first_step(res, cuda_reference(handle, oracle, win, opt, fp32_pose_rows=True), tol, name + ", FP32 pose rows")
+    b32 = handle.evaluate(win, opt)
+    opt.precision = 0
+    b64 = handle.evaluate(win, opt)
+    opt.precision = 1
+    for what in ("jl", "r"):
+        ref = dense_first_step(win, opt, tampered(b32, what), lambda w: handle.evaluate(w, opt), oracle, fp64_blocks=b64)
+        with pytest.raises(AssertionError):
+            _check_first_step(res, ref, tol, "%s, %s perturbed" % (name, what))

@@ -362,9 +362,10 @@ def test_sharded_solve_with_one_rank_equals_plain_solve(handle):
 def test_fp32_linearisation_mode(handle, oracle):
     """kba_options.precision = 1 (BASELINE config 3's FP32 setting): residual / Jacobian blocks are evaluated and stored
     in single precision, every accumulation and the cost stay FP64.  Tolerances are single-precision ones, set from
-    the measured deviations (scripts/fp32_check.py: blocks 1e-5 of the largest entry, final cost 4e-7 relative, poses
+    the measured deviations (scripts/fp32_check.py and scripts/fp32_agreement.py for the blocks; final cost 4e-7 relative, poses
     1.7 mm -- the flat directions of the problem amplify the gradient noise): north_star's 1e-6 m is an FP64 statement."""
     from limo_b200 import capi
+    from tests.test_far_windows import check_fp32_blocks
     opt = capi.default_options()
     opt.precision = 1
     win = synth.make_window(2, n_kf=12, n_lm=400, n_obs=3000)
@@ -373,7 +374,8 @@ def test_fp32_linearisation_mode(handle, oracle):
     assert failed == 0 and cost == pytest.approx(cost0, rel=1e-12)  # the cost is evaluated in FP64
     assert np.abs(r - r0).max() <= 2e-3                             # pixels, values up to ~1e3 before the loss
     assert np.abs(jp - jp0).max() <= 3e-5 * np.abs(jp0).max() and np.abs(jl - jl0).max() <= 3e-5 * np.abs(jl0).max()
-    assert np.abs(jp - jp0).max() > 0.0                             # ... and it really is the single-precision path
+    # and every column family against kba_eval's FP64 blocks at the bounds tests/test_far_windows.py holds far from the origin
+    check_fp32_blocks(win, (r, jp, jl), handle.evaluate(win, capi.default_options()), "config2_slice")
     for cfg, kw in ((2, dict()), (3, dict(seed=41))):
         win = synth.make_window(cfg, **kw)
         rg = handle.solve_window(win, opt)

@@ -180,6 +180,20 @@ def test_cuda_first_step_651_rows_matches_dense_step(handle, oracle, driver):  #
 
 
 @pytest.mark.gpu
+def test_cuda_fp32_first_step_651_rows_matches_dense_step(handle, oracle, driver):  # noqa: F811
+    """the same in FP32 (k_eval_obs<float, true>, the split factorisation with k_chol_trail_band): the mixed system of the FP32
+    solve (tests/test_first_step_dense.dense_first_step), at the ground windows' tolerance"""
+    w = _ground_651()
+    opt = oracle.default_options()
+    opt.precision = 1
+    fs.assert_path(driver, [w], PATH_651)
+    ref = fs.cuda_reference(handle, oracle, w, opt)
+    [res] = handle.solve_batch([w], opt, iterations_capacity=256)
+    assert res.c.status == 0
+    fs._check_first_step(res, ref, fs.GROUND_TOL, "ground_651, FP32")
+
+
+@pytest.mark.gpu
 def test_solve_split_is_bit_identical(handle, monkeypatch):
     """KBA_SOLVE_SPLIT = 1, 8 and 32 on the 1001-row window: each result element of the trailing update sums in the same order
     whichever CTA owns its block"""
