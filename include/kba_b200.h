@@ -1326,6 +1326,50 @@ int kba_lidar_depth_batch(kba_handle* h, int32_t n_clouds, const kba_lidar_cloud
 int kba_lidar_depth_batch_opts(kba_handle* h, int32_t n_clouds, const kba_lidar_cloud* clouds, int32_t n_views,
                                const kba_lidar_view* views, const kba_lidar_options* opts, float* device_ms);
 
+/* ---- limo's mono-lidar frame step as one store call: the frame's depths from its lidar cloud ---------------------------
+ * kba_track_frame_step with the DepthEstimator call of the front end folded in: the frame's measurements get their depths
+ * from the frame's cloud on the device, and the frame step runs on those depths without a round trip through the host.
+ *   - Contract: a request's d column is not read (it may be NULL).  Measurement m of camera c gets, bit for bit, the depth
+ *     kba_lidar_depth_batch_opts gives it for the view with lid's cloud, pose T_cam_lidar + 7 c, the track's camera c
+ *     intrinsics as created, options opt[c] and camera c's measurements (u, v) in request order as its features; a camera
+ *     with no measurements is no view.  Everything after that -- res, every field of out, the store afterwards -- is exactly
+ *     kba_track_frame_step on those depths.  depth_out, when set, receives the depth each measurement got (-1: none).
+ *   - Checks, all before anything is uploaded, and a refused call writes no output and changes no store: the frame step's own
+ *     (except for d); a null lid, T_cam_lidar or opt; a null points with n_points > 0; n_points < 0 or stride < 3
+ *     (KBA_ERR_BAD_ARG); the lidar batch's 32-bit totals over the call's views (KBA_ERR_CAPACITY).  kba_last_error names
+ *     the track.  Options are not checked.
+ *   - Cost: the frame step's shape.  One copy of each cloud a view reads, from the caller's memory into the handle's lidar
+ *     workspace (as kba_lidar_depth_batch copies it); one upload of the staging, in which the lidar views' parameters and one
+ *     feature index per measurement replace the d column; one launch sequence: the lidar kernels (memset, count, scan, fill,
+ *     feature), whose feature pass writes the staged d column, then k_fs_gather, k_adjust_pose and the flow kernels; one
+ *     download; two synchronisations, one when no frame is selected.  The push's k_store_append and the creation read the
+ *     extracted depths from the staged d column.
+ *   - Transfers (kba_track_transfer_bytes / kba_track_group_transfer_bytes), with the terms of kba_track_frame_step's formulas,
+ *     V the views (cameras with measurements over the W requests), R_v the size of a view's parameter record (a constant of
+ *     the library build), R the run flags sum(n_runs), the clouds summed over the requests with n_meas > 0:
+ *         h2d = R_1 W + R_a A + R_v V + 8 (V + 1) + sum(20 n_meas + 4 (n_kf + 1 + n_new)) + 4 ceil(R / 4)
+ *               + sum(4 n_points stride) + (S ? R_2 S + R_c C + R_p P : 0)
+ *         d2h = kba_track_frame_step's d2h + 4 sum over requests with depth_out of n_meas
+ *     (20 bytes per measurement: the columns lm, cam, u, v and the feature index; no d column goes up).
+ *   - Allocations: the frame step's, plus the handle's lidar workspace (grow-only, shared with kba_lidar_depth_batch).
+ * The group forms take lid[n_tracks] next to req[n_tracks]: each request brings its own cloud; a request that sits out
+ * (n_kf == 0) does not read its entry.  _opts takes one kba_options per track, as kba_track_group_frame_step_opts. */
+typedef struct kba_frame_lidar {
+    const float* points;                 /* the frame's cloud, n_points x stride floats, xyz first (as kba_lidar_cloud)      */
+    int32_t n_points, stride;            /* n_points may be 0: every depth is -1                                               */
+    const double* T_cam_lidar;           /* [7 * n_cam]: camera c <- lidar, for every camera of the track                      */
+    const kba_lidar_options* opt;        /* [n_cam]: camera c's extraction options (rigs whose cameras differ in image size)   */
+    float* depth_out;                    /* [n_meas] or NULL: the depth each measurement got, -1 = none                        */
+} kba_frame_lidar;
+int kba_track_frame_step_lidar(kba_track* t, const kba_frame_step_request* req, const kba_frame_lidar* lid, const kba_options* opt,
+                               kba_frame_step_out* out, kba_result* res);
+/* req[n_tracks], lid[n_tracks], out[n_tracks], res[n_tracks] */
+int kba_track_group_frame_step_lidar(kba_track_group* g, const kba_frame_step_request* req, const kba_frame_lidar* lid,
+                                     const kba_options* opt, kba_frame_step_out* out, kba_result* res);
+/* opts[n_tracks]: track i's adjustment runs with opts[i] */
+int kba_track_group_frame_step_lidar_opts(kba_track_group* g, const kba_frame_step_request* req, const kba_frame_lidar* lid,
+                                          const kba_options* opts, kba_frame_step_out* out, kba_result* res);
+
 #ifdef __cplusplus
 }
 #endif

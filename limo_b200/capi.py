@@ -10,7 +10,7 @@ import os
 
 import numpy as np
 
-from .capi_types import (KbaCounters, KbaCreateOut, KbaCreateRequest, KbaDeactivateOut, KbaDeactivateRequest, KbaDepthEntry, KbaDepthOut, KbaDepthRequest, KbaDrawFn, KbaEvalOut, KbaEvaluateOut, KbaFlowOut, KbaFlowRequest, KbaFrameStepOut, KbaFrameStepRequest, KbaKfsolveOut, KbaKfsolveRequest, KbaLabelClass, KbaLandmarkWrite, KbaLidarCloud, KbaLidarOptions, KbaLidarView, KbaOptions, KbaPoseWrite, KbaPushRequest, KbaRankedRequest, KbaRankOut, KbaRankRequest, KbaReclaimOut, KbaReclaimRequest, KbaResult, KbaSelectOut, KbaSelectParams, KbaSelectRequest, KbaTracklet,
+from .capi_types import (KbaCounters, KbaCreateOut, KbaCreateRequest, KbaDeactivateOut, KbaDeactivateRequest, KbaDepthEntry, KbaDepthOut, KbaDepthRequest, KbaDrawFn, KbaEvalOut, KbaEvaluateOut, KbaFlowOut, KbaFlowRequest, KbaFrameLidar, KbaFrameStepOut, KbaFrameStepRequest, KbaKfsolveOut, KbaKfsolveRequest, KbaLabelClass, KbaLandmarkWrite, KbaLidarCloud, KbaLidarOptions, KbaLidarView, KbaOptions, KbaPoseWrite, KbaPushRequest, KbaRankedRequest, KbaRankOut, KbaRankRequest, KbaReclaimOut, KbaReclaimRequest, KbaResult, KbaSelectOut, KbaSelectParams, KbaSelectRequest, KbaTracklet,
                          KbaSnapshotHeader, KbaTrackCaps, KbaTrackFrame, KbaTrackRequest, KbaWindow, Result, Window, c_double_p, c_float_p, c_int32_p,
                          c_uint8_p)
 
@@ -38,7 +38,8 @@ SYMBOLS = ["kba_version", "kba_last_error", "kba_default_options", "kba_create",
            "kba_lidar_depth_batch_opts", "kba_track_snapshot_size", "kba_track_save", "kba_track_load", "kba_track_clone",
            "kba_track_group_snapshot_sizes", "kba_track_group_save", "kba_track_evaluate", "kba_track_group_evaluate",
            "kba_track_group_evaluate_opts", "kba_track_keyframe_solve", "kba_track_group_keyframe_solve",
-           "kba_track_group_keyframe_solve_opts", "kba_track_frame_step", "kba_track_group_frame_step", "kba_track_group_frame_step_opts"]
+           "kba_track_group_keyframe_solve_opts", "kba_track_frame_step", "kba_track_group_frame_step", "kba_track_group_frame_step_opts",
+           "kba_track_frame_step_lidar", "kba_track_group_frame_step_lidar", "kba_track_group_frame_step_lidar_opts"]
 
 
 class KbaError(RuntimeError):
@@ -181,6 +182,9 @@ def lib():
             f.argtypes = [vp, C.POINTER(KbaKfsolveRequest), C.POINTER(KbaOptions), C.POINTER(KbaKfsolveOut), C.POINTER(KbaResult)]
         for f in (L.kba_track_frame_step, L.kba_track_group_frame_step, L.kba_track_group_frame_step_opts):
             f.argtypes = [vp, C.POINTER(KbaFrameStepRequest), C.POINTER(KbaOptions), C.POINTER(KbaFrameStepOut), C.POINTER(KbaResult)]
+        for f in (L.kba_track_frame_step_lidar, L.kba_track_group_frame_step_lidar, L.kba_track_group_frame_step_lidar_opts):
+            f.argtypes = [vp, C.POINTER(KbaFrameStepRequest), C.POINTER(KbaFrameLidar), C.POINTER(KbaOptions), C.POINTER(KbaFrameStepOut),
+                          C.POINTER(KbaResult)]
         L.kba_lidar_default_options.argtypes = [C.POINTER(KbaLidarOptions)]
         L.kba_lidar_default_options.restype = None
         fp = C.POINTER(C.c_float)
@@ -407,10 +411,36 @@ def _evaluate_outputs(n_lm, obs_cap, gp_cap):
     return o, tuple(b.values()), done
 
 
-def _frame_step_args(kf_slots, lm_slot, u, v, d, run_sel, kf_new, pose7, stamp, stamp_last, critical_quaternion_diff,
-                     time_difference_ns, cam=None, new_slots=(), plane4=None, adjust=True, speed=None, min_median_flow=5.0):
-    """one frame step request's arrays and scalars, checked where the C call would read past an array"""
+def _frame_lidar_args(cloud, T_cam_lidar, lidar_opt, depths):
+    """the lidar part of a frame step request: its cloud, one pose per camera and one KbaLidarOptions per camera (lidar_opt None
+    or one KbaLidarOptions: the same for every camera; a sequence: one per camera, None entries the defaults)"""
+    cl = np.ascontiguousarray(cloud, dtype=np.float32)
+    if cl.ndim != 2 or cl.shape[1] < 3:
+        raise ValueError("cloud: an [n, stride >= 3] array expected, got shape %s" % (cl.shape,))
+    if T_cam_lidar is None:
+        raise ValueError("a cloud needs T_cam_lidar, one 7-vector per camera")
+    T = np.ascontiguousarray(T_cam_lidar, dtype=np.float64)
+    if T.size == 0 or T.size % 7:
+        raise ValueError("T_cam_lidar: one 7-vector per camera, got %d entries" % T.size)
+    T = T.reshape(-1, 7)
+    if lidar_opt is None or isinstance(lidar_opt, KbaLidarOptions):
+        opts = [lidar_opt] * len(T)
+    else:
+        opts = list(lidar_opt)
+        if len(opts) != len(T):
+            raise ValueError("%d lidar option sets for %d cameras" % (len(opts), len(T)))
+    return dict(cloud=cl, T=T, opts=(KbaLidarOptions * len(T))(*[o or lidar_default_options() for o in opts]), depths=bool(depths))
+
+
+def _frame_step_args(kf_slots, lm_slot, u, v, run_sel, kf_new, pose7, stamp, stamp_last, critical_quaternion_diff,
+                     time_difference_ns, d=None, cam=None, new_slots=(), plane4=None, adjust=True, speed=None, min_median_flow=5.0,
+                     cloud=None, T_cam_lidar=None, lidar_opt=None, depths=False):
+    """one frame step request's arrays and scalars, checked where the C call would read past an array.  With a cloud the depths
+    come from it (the lidar form) and d is not taken."""
     kf, lm, cm, new = _arr(kf_slots, np.int32, -1), _arr(lm_slot, np.int32, -1), _arr(cam, np.int32, -1), _arr(new_slots, np.int32, -1)
+    if (d is None) == (cloud is None):
+        raise ValueError("a request takes d (the depths) or a lidar cloud, not both")
+    lid = None if cloud is None else _frame_lidar_args(cloud, T_cam_lidar, lidar_opt, depths)
     uu, vv, dd = (_arr(x, np.float32, -1) for x in (u, v, d))
     rs = np.ascontiguousarray(np.asarray(run_sel, dtype=bool).ravel().astype(np.uint8))
     n_runs = int(1 + np.count_nonzero(lm[1:] != lm[:-1])) if len(lm) else 0
@@ -423,28 +453,34 @@ def _frame_step_args(kf_slots, lm_slot, u, v, d, run_sel, kf_new, pose7, stamp, 
     if speed:
         sp.update(speed_weight=float(speed["weight"]), speed_dt=float(speed["dt"]), speed_v_before=np.asarray(speed["v_before"], np.float64),
                   speed_T_origin_before=np.asarray(speed["T_origin_before"], np.float64))
-    return dict(kf=kf, lm=lm, cam=cm, new=new, u=uu, v=vv, d=dd, run_sel=rs, pose=pose, plane=pl, kf_new=int(kf_new),
+    return dict(kf=kf, lm=lm, cam=cm, new=new, u=uu, v=vv, d=dd, lidar=lid, run_sel=rs, pose=pose, plane=pl, kf_new=int(kf_new),
                 n_sel_runs=int(rs.sum()), adjust=int(bool(adjust)), min_median_flow=float(min_median_flow),
                 critical_quaternion_diff=float(critical_quaternion_diff), time_difference_ns=int(time_difference_ns), stamp=int(stamp),
                 stamp_last=int(stamp_last), **sp)
 
 
-def _frame_step_records(fn, requests, capacity):
+def _frame_step_records(fn, requests, capacity, lidar=False, n_cam=None):
     """the request and output arrays of a frame step over requests (None: the track sits out) as numpy records, the KbaResult
     array, the buffers they point into, and result(i, filled KbaResult array) -> request i's dict.  No ctypes object per track
-    but its Result."""
+    but its Result.  lidar: every request carries a cloud (the _lidar forms): the kba_frame_lidar records are returned sixth.
+    n_cam: the tracks' camera counts, which each request's T_cam_lidar must match (None: not checked)."""
     n = len(requests)
     act = [i for i, r in enumerate(requests) if r is not None]
     args = [_built(fn, i, requests[i], _frame_step_args) for i in act]
     for i, a in zip(act, args):
         if len(a["kf"]) == 0:  # n_kf = 0 would sit the track out: a request without keyframes is an error, as for one track
             raise KbaError("%s: track %d: no keyframes or a negative size" % (fn.__name__, i))
+        if (a["lidar"] is not None) != lidar:
+            raise ValueError("%s: request %d: %s" % (fn.__name__, i, "no cloud in a lidar call" if lidar else "a cloud in a call without lidar"))
+        if lidar and n_cam is not None and len(a["lidar"]["T"]) != n_cam[i]:
+            raise ValueError("%s: request %d: T_cam_lidar has %d poses for %d cameras" % (fn.__name__, i, len(a["lidar"]["T"]), n_cam[i]))
     req, out = np.zeros(n, _records(KbaFrameStepRequest)), np.zeros(n, _records(KbaFrameStepOut))
     nk, nm, nn = (np.array([len(a[k]) for a in args], np.int64) for k in ("kf", "lm", "new"))
     has_cam = np.array([a["cam"] is not None for a in args], bool)
     ints = np.concatenate([a["kf"] for a in args] + [a["lm"] for a in args] + [a["cam"] for a in args if a["cam"] is not None] +
                           [a["new"] for a in args] + [np.zeros(1, np.int32)])
-    flts = np.concatenate([a[k] for k in ("u", "v", "d") for a in args] + [np.zeros(1, np.float32)])
+    cols = ("u", "v") if lidar else ("u", "v", "d")  # the lidar form reads no d column
+    flts = np.concatenate([a[k] for k in cols for a in args] + [np.zeros(1, np.float32)])
     flags = np.concatenate([a["run_sel"] for a in args] + [np.zeros(1, np.uint8)])
     poses = np.concatenate([a["pose"] for a in args] + [np.zeros(0)])
     planes = np.concatenate([a["plane"] for a in args if a["plane"] is not None] + [np.zeros(0)])
@@ -456,7 +492,7 @@ def _frame_step_records(fn, requests, capacity):
     req["lm_slot"][act] = ints.ctypes.data + 4 * (K + ex(nm))
     req["cam"][act] = np.where(has_cam, ints.ctypes.data + 4 * cam_off, 0)
     req["new_slot"][act] = ints.ctypes.data + 4 * (K + M + int(nm[has_cam].sum()) + ex(nn))
-    for j, k in enumerate(("u", "v", "d")):
+    for j, k in enumerate(cols):
         req[k][act] = flts.ctypes.data + 4 * (j * M + ex(nm))
     req["run_sel"][act] = flags.ctypes.data + ex([len(a["run_sel"]) for a in args])
     req["pose7"][act] = poses.ctypes.data + 56 * np.arange(len(act))
@@ -470,6 +506,18 @@ def _frame_step_records(fn, requests, capacity):
     out["match"][act] = match.ctypes.data + 4 * ex(nm)
     out["pos"][act] = pos.ctypes.data + 24 * ex(nn)
     out["flags"][act] = cflags.ctypes.data + ex(nn)
+    depth = np.full(M + 1, -1.0, np.float32)
+    lid, lkeep = None, ()
+    if lidar:
+        lid = np.zeros(n, _records(KbaFrameLidar))
+        la = [a["lidar"] for a in args]
+        lid["points"][act] = [x["cloud"].ctypes.data for x in la]
+        lid["n_points"][act] = [x["cloud"].shape[0] for x in la]
+        lid["stride"][act] = [x["cloud"].shape[1] for x in la]
+        lid["T_cam_lidar"][act] = [x["T"].ctypes.data for x in la]
+        lid["opt"][act] = [C.addressof(x["opts"]) for x in la]
+        lid["depth_out"][act] = np.where([x["depths"] for x in la], depth.ctypes.data + 4 * ex(nm), 0)
+        lkeep = (depth, la)
     ress = (KbaResult * n)()
     results = {}
     for j, i in enumerate(act):
@@ -488,8 +536,9 @@ def _frame_step_records(fn, requests, capacity):
                     match=match[m0:m0 + nm[j]].copy(), angle=float(o["angle"]), usable_flow=bool(o["usable_flow"]),
                     usable_pose=bool(o["usable_pose"]), usable_time=bool(o["usable_time"]), selected=picked,
                     pos=pos[n0:n0 + nn[j]].copy() if picked else None, flags=cflags[n0:n0 + nn[j]].copy() if picked else None,
-                    result=res)
-    return req, out, ress, (ints, flts, flags, poses, planes, match, pos, cflags, results), result
+                    depth=depth[m0:m0 + nm[j]].copy() if lidar and args[j]["lidar"]["depths"] else None, result=res)
+    keep = (ints, flts, flags, poses, planes, match, pos, cflags, lkeep, results)
+    return (req, out, ress, keep, result, lid) if lidar else (req, out, ress, keep, result)
 
 
 class Track:
@@ -512,6 +561,7 @@ class Track:
                                         win_ground, win_rows)
         intr = np.ascontiguousarray(cam_intr, dtype=np.float64).reshape(-1, 3)
         pose = np.ascontiguousarray(cam_pose, dtype=np.float64).reshape(-1, 7)
+        self.n_cam = len(intr)
         self._p = C.c_void_p()
         _check(lib().kba_track_create(handle._p, C.byref(caps), len(intr), intr.ctypes.data_as(c_double_p),
                                       pose.ctypes.data_as(c_double_p), C.byref(self._p)))
@@ -831,14 +881,15 @@ class Track:
         measurements lm_slot, u, v, d and cam (every run's landmark with a slot; runs as for adjust_pose), run_sel (one flag per
         run: the landmark is in the last selection), kf_new (the free slot the frame is pushed into if selected), new_slots (the
         landmarks to create then), pose7, plane4, adjust (False: the pose is taken as given), speed (as for adjust_pose),
-        min_median_flow, critical_quaternion_diff (radians), time_difference_ns, stamp and stamp_last (ns).  Returns a dict: the
+        min_median_flow, critical_quaternion_diff (radians), time_difference_ns, stamp and stamp_last (ns).
+        mono-lidar (kba_track_frame_step_lidar): cloud ([n, stride >= 3] float32, xyz first) instead of d, with T_cam_lidar (one
+        7-vector per camera, camera <- lidar), lidar_opt (None, one KbaLidarOptions, or one per camera) and depths (True: return
+        the depth each measurement got): the measurements' depths come from the cloud on the device.  Returns a dict: the
         flow's n_matched, flow_sum, mean_flow_sq, match; angle; usable_flow, usable_pose, usable_time, selected; pos, flags (the
-        creation's, None when not selected); result, the adjustment's Result."""
-        fn = lib().kba_track_frame_step
-        req, out, ress, _keep, result = _frame_step_records(fn, [kw], iterations_capacity)
-        _check(fn(self._p, req.ctypes.data_as(C.POINTER(KbaFrameStepRequest)), C.byref(opt or default_options()),
-                  out.ctypes.data_as(C.POINTER(KbaFrameStepOut)), ress))
-        return result(0, ress)
+        creation's, None when not selected); depth (the lidar depths when asked for, else None); result, the adjustment's
+        Result."""
+        return _frame_step_call(self._p, lib().kba_track_frame_step, lib().kba_track_frame_step_lidar, [kw],
+                                C.byref(opt or default_options()), iterations_capacity, [self.n_cam])[0]
 
     def transfer_bytes(self):
         a, b, c = C.c_int64(), C.c_int64(), C.c_int64()
@@ -866,9 +917,9 @@ class Track:
         return c
 
     @classmethod
-    def _adopt(cls, handle, p, caps):
+    def _adopt(cls, handle, p, caps, n_cam):
         t = cls.__new__(cls)
-        t.handle, t._n_sel, t._p, t.caps = handle, None, p, caps
+        t.handle, t._n_sel, t._p, t.caps, t.n_cam = handle, None, p, caps, n_cam
         return t
 
     @classmethod
@@ -876,12 +927,13 @@ class Track:
         """A track on handle whose store is the snapshot data (kba_track_load).  caps: None (the saved caps) or a dict of keyword
         caps (max_keyframes, ..., win_rows) that replace the saved ones, e.g. dict(win_keyframes=20) to grow the window."""
         buf = np.ascontiguousarray(np.frombuffer(data, np.uint8) if not isinstance(data, np.ndarray) else data.view(np.uint8).ravel())
-        saved = KbaSnapshotHeader.from_buffer_copy(buf[:C.sizeof(KbaSnapshotHeader)].tobytes()).caps \
-            if len(buf) >= C.sizeof(KbaSnapshotHeader) else KbaTrackCaps()
+        hd = KbaSnapshotHeader.from_buffer_copy(buf[:C.sizeof(KbaSnapshotHeader)].tobytes()) \
+            if len(buf) >= C.sizeof(KbaSnapshotHeader) else None
+        saved = hd.caps if hd is not None else KbaTrackCaps()
         c = cls._caps(saved, caps or {})
         p = C.c_void_p()
         _check(lib().kba_track_load(handle._p, buf.ctypes.data, len(buf), C.byref(c) if c else None, C.byref(p)))
-        return cls._adopt(handle, p, c or KbaTrackCaps.from_buffer_copy(saved))
+        return cls._adopt(handle, p, c or KbaTrackCaps.from_buffer_copy(saved), hd.n_cam)  # a snapshot that loads has a header
 
     def clone(self, handle=None, **caps):
         """a copy of this track on handle (default: this track's handle) with the keyword caps changed (kba_track_clone); on the
@@ -890,7 +942,7 @@ class Track:
         c = self._caps(self.caps, caps)
         p = C.c_void_p()
         _check(lib().kba_track_clone(self._p, h._p, C.byref(c) if c else None, C.byref(p)))
-        return self._adopt(h, p, c or KbaTrackCaps.from_buffer_copy(self.caps))
+        return self._adopt(h, p, c or KbaTrackCaps.from_buffer_copy(self.caps), self.n_cam)
 
     def close(self):
         if self._p:
@@ -905,6 +957,17 @@ def _built(fn, i, r, build, *args):
         return build(*args, **r)
     except (TypeError, ValueError) as e:
         raise type(e)("%s: request %d: %s" % (fn.__name__, i, e)) from None
+
+
+def _frame_step_call(p, fn, fn_lidar, requests, o, capacity, n_cam):
+    """a frame step of the track or group p through fn, or through fn_lidar when the requests carry clouds: one result dict per
+    request, None for a track that sits out"""
+    lidar = any(r is not None and "cloud" in r for r in requests)
+    f = fn_lidar if lidar else fn
+    req, out, ress, _keep, result, *lid = _frame_step_records(f, requests, capacity, lidar, n_cam)
+    args = [req.ctypes.data_as(C.POINTER(KbaFrameStepRequest))] + [x.ctypes.data_as(C.POINTER(KbaFrameLidar)) for x in lid]
+    _check(f(p, *args, o, out.ctypes.data_as(C.POINTER(KbaFrameStepOut)), ress))
+    return [None if r is None else result(i, ress) for i, r in enumerate(requests)]
 
 
 def _no_keyframes(q):  # n_kf = 0 would sit the track out: a request without keyframes is an error, as for one track
@@ -1097,10 +1160,10 @@ class TrackGroup:
         one result dict per track (Track.frame_step's), None for a track that sat out."""
         # Not _call: the request and output structs are numpy records, filled without a ctypes object per track
         assert len(requests) == len(self.tracks)
-        fn, o = _options(opt, len(self.tracks), lib().kba_track_group_frame_step, lib().kba_track_group_frame_step_opts)
-        req, out, ress, _keep, result = _frame_step_records(fn, requests, iterations_capacity)
-        _check(fn(self._p, req.ctypes.data_as(C.POINTER(KbaFrameStepRequest)), o, out.ctypes.data_as(C.POINTER(KbaFrameStepOut)), ress))
-        return [None if r is None else result(i, ress) for i, r in enumerate(requests)]
+        L = lib()
+        fn, o = _options(opt, len(self.tracks), L.kba_track_group_frame_step, L.kba_track_group_frame_step_opts)
+        fn_lidar, _ = _options(opt, len(self.tracks), L.kba_track_group_frame_step_lidar, L.kba_track_group_frame_step_lidar_opts)
+        return _frame_step_call(self._p, fn, fn_lidar, requests, o, iterations_capacity, [t.n_cam for t in self.tracks])
 
     def push_keyframes(self, requests):
         """one keyframe into every track's store in one call (kba_track_group_push_keyframes): each entry None (the track sits the

@@ -352,6 +352,13 @@ class KbaLidarView(C.Structure):
     ]
 
 
+class KbaFrameLidar(C.Structure):
+    _fields_ = [
+        ("points", c_float_p), ("n_points", C.c_int32), ("stride", C.c_int32), ("T_cam_lidar", c_double_p),
+        ("opt", C.POINTER(KbaLidarOptions)), ("depth_out", c_float_p),
+    ]
+
+
 def _ptr(a, ctype):
     if a is None:
         return C.cast(None, C.POINTER(ctype))

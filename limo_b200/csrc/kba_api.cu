@@ -4413,12 +4413,14 @@ struct StepWin {
     bool selected = false;
     double angle = 0.;
     unsigned char verdict[3] = {0, 0, 0};
+    // the lidar form: the rows of each camera's measurements (a view each), in request order, camera by camera
+    std::vector<int> cam_rows, cam_off;    // cam_off[n_cam + 1]: camera c's rows are cam_rows[cam_off[c] .. cam_off[c + 1])
 };
 
 // every check of one request that needs only the request; allocates the track's upkeep and creation scratch at their first use
 static int step_check(kba_track* t, const kba_frame_step_request& q, const kba_frame_step_out* o, const kba_options* opt,
-                      StepWin& w, std::string& why) {
-    if (!o || !q.kf_slot || !q.pose7 || (q.n_meas > 0 && (!q.lm_slot || !q.u || !q.v || !q.d || !q.run_sel)) ||
+                      const kba_frame_lidar* lid, StepWin& w, std::string& why) {
+    if (!o || !q.kf_slot || !q.pose7 || (q.n_meas > 0 && (!q.lm_slot || !q.u || !q.v || (!q.d && !lid) || !q.run_sel)) ||
         (q.n_new > 0 && (!q.new_slot || !o->pos || !o->flags))) {
         why = "null argument"; return KBA_ERR_BAD_ARG;
     }
@@ -4465,12 +4467,24 @@ static int step_check(kba_track* t, const kba_frame_step_request& q, const kba_f
     if (w.rounds < 0) w.rounds = (w.sel_runs > opt->min_landmarks_for_trimming) ? opt->num_rounds_option : 0;
     if (w.rounds > 6) w.rounds = 6;
     w.max_meas = std::max(w.max_meas, q.n_meas);  // the creation lists the new keyframe too
+    if (!lid) return KBA_OK;
+    // the lidar form: the frame's cloud, and one view per camera that measures something
+    if (!lid->T_cam_lidar || !lid->opt) { why = "null T_cam_lidar or lidar options"; return KBA_ERR_BAD_ARG; }
+    if (lid->n_points < 0 || lid->stride < 3) { why = "cloud: negative n_points or stride < 3"; return KBA_ERR_BAD_ARG; }
+    if (lid->n_points > 0 && !lid->points) { why = "cloud: null points"; return KBA_ERR_BAD_ARG; }
+    w.cam_off.assign(t->n_cam + 1, 0);
+    for (int i = 0; i < q.n_meas; ++i) ++w.cam_off[(q.cam ? q.cam[i] : 0) + 1];
+    for (int c = 0; c < t->n_cam; ++c) w.cam_off[c + 1] += w.cam_off[c];
+    w.cam_rows.resize((size_t)q.n_meas);
+    std::vector<int> at(w.cam_off.begin(), w.cam_off.end() - 1);
+    for (int i = 0; i < q.n_meas; ++i) w.cam_rows[at[q.cam ? q.cam[i] : 0]++] = i;
     return KBA_OK;
 }
 
-// one frame step of the tracks of s (group = false: a single call), req[i] / out[i] / res[i] track i's
+// one frame step of the tracks of s (group = false: a single call), req[i] / out[i] / res[i] / lid[i] track i's; lid null: the
+// requests' d columns are the depths, else the lidar kernels extract them from lid[i]'s cloud into the staged d column
 static int set_frame_step(TrackSet& s, bool group, const std::string& who, const kba_frame_step_request* req, bool per_track,
-                          const kba_options* opts, kba_frame_step_out* out, kba_result* res) {
+                          const kba_options* opts, kba_frame_step_out* out, kba_result* res, const kba_frame_lidar* lid) {
     const int n = (int)s.tracks.size();
     std::vector<StepWin> ws;
     for (int i = 0; i < n; ++i) {
@@ -4478,9 +4492,33 @@ static int set_frame_step(TrackSet& s, bool group, const std::string& who, const
         StepWin w;
         w.t = s.tracks[i]; w.i = i; w.q = &req[i];
         std::string why;
-        const int rc = step_check(w.t, req[i], out + i, &opts[per_track ? i : 0], w, why);
+        const int rc = step_check(w.t, req[i], out + i, &opts[per_track ? i : 0], lid ? lid + i : nullptr, w, why);
         if (rc != KBA_OK) return fail(rc, who + track_prefix(group, i) + why);
-        ws.push_back(w);
+        ws.push_back(std::move(w));
+    }
+    // the lidar views (cloud v is ws[v]'s), those of the frames whose depths are downloaded first: their features lead the
+    // feature order, so the download is the first n_copy depths in that order
+    LidarPlan plan((int)ws.size());
+    std::vector<int> lid_order;
+    int n_copy = 0;
+    int64_t cloud_bytes = 0;
+    if (lid) {
+        for (int pass = 0; pass < 2; ++pass)
+            for (int v = 0; v < (int)ws.size(); ++v)
+                if ((lid[ws[v].i].depth_out != nullptr) == (pass == 0) && ws[v].q->n_meas > 0) lid_order.push_back(v);
+        for (int v : lid_order) {
+            const StepWin& w = ws[v];
+            const kba_frame_lidar& l = lid[w.i];
+            const kba_lidar_cloud cl{l.points, l.n_points, l.stride};
+            if (l.depth_out) n_copy += w.q->n_meas;
+            cloud_bytes += 4 * (int64_t)l.n_points * l.stride;
+            for (int c = 0; c < w.t->n_cam; ++c) {
+                const int m = w.cam_off[c + 1] - w.cam_off[c];
+                if (m > 0 && plan.add(v, cl, l.T_cam_lidar + 7 * c, w.t->cam_intr.data() + 3 * c, l.opt + c, m) != KBA_OK)
+                    return fail(KBA_ERR_CAPACITY, who + track_prefix(group, w.i) +
+                                                      "the call's lidar cells, (view, point) pairs or features exceed 32-bit indexing");
+            }
+        }
     }
     for (int i = 0; i < n; ++i) idle_result(res[i]);  // written below for the adjusted frames
     if (ws.empty()) {  // no upload, no launch
@@ -4515,12 +4553,19 @@ static int set_frame_step(TrackSet& s, bool group, const std::string& who, const
     Bump up, dn;
     const size_t o_step = up.take(sizeof(StepArgs) * (size_t)W), o_flow = up.take(sizeof(FlowArgs) * (size_t)W);
     const size_t o_fd = up.take(sizeof(FrameDesc) * (size_t)A), o_sp = up.take(sizeof(SolveParams) * (size_t)A);
-    const size_t o_cols = up.take(20 * (size_t)N, 4);
+    // the lidar form replaces the d column's upload by the lidar views' parameters and one feature index per measurement; the
+    // columns then come last, so that the d column, which the lidar kernels write, is the first region past the upload
+    size_t o_cols = lid ? 0 : up.take(20 * (size_t)N, 4), o_lpack = 0, o_idx = 0, o_dep = 0;
+    if (lid) { o_lpack = up.take(plan.pack_bytes()); o_idx = up.take(4 * (size_t)N, 4); }
     for (StepWin& w : ws) w.u_list = up.take(4 * ((size_t)w.q->n_kf + 1 + w.q->n_new), 4);
-    const size_t o_flags = up.take((size_t)R_all, 1), up1 = up.at;
+    const size_t o_flags = up.take((size_t)R_all, 1);
+    if (lid) o_cols = up.take(20 * (size_t)N, 4);
+    const size_t up1 = lid ? o_cols + 16 * (size_t)N : up.at;
     const size_t o_fr = dn.take(sizeof(FrameRes) * (size_t)A), o_log = dn.take(sizeof(IterRecord) * (size_t)A * log_cap);
     const size_t o_fres = dn.take(sizeof(FlowRes) * (size_t)W), o_pose = dn.take(56 * (size_t)W);
-    const size_t o_match = dn.take(4 * (size_t)N, 4), o_rej = dn.take((size_t)Rn, 1), down1 = dn.at;
+    const size_t o_match = dn.take(4 * (size_t)N, 4);
+    if (lid) o_dep = dn.take(4 * (size_t)n_copy, 4);
+    const size_t o_rej = dn.take((size_t)Rn, 1), down1 = dn.at;
     // the second phase at its largest: every window selected and compacting
     Bump up2 = up, dn2 = dn;
     up2.take(0);
@@ -4539,6 +4584,8 @@ static int set_frame_step(TrackSet& s, bool group, const std::string& who, const
     StoreStage& st = *stage;
     unsigned char* uh = st.up.h, *od = st.out.d;
     const unsigned char* ud = st.up.d;
+    LidarWs lws;
+    if (!plan.par.empty() && lidar_workspace(h, plan, 0, lws) != KBA_OK) return fail(KBA_ERR_CUDA, who + "out of memory for the lidar workspace");
     // ---- staging: the columns, lists and flags once; the records of the gather, the adjustment and the flow
     unsigned* cols_h = reinterpret_cast<unsigned*>(uh + o_cols);
     const unsigned* cols_d = reinterpret_cast<const unsigned*>(ud + o_cols);
@@ -4559,7 +4606,7 @@ static int set_frame_step(TrackSet& s, bool group, const std::string& who, const
             if (q.cam) memcpy(cols_h + N + w.src, q.cam, b); else memset(cols_h + N + w.src, 0, b);
             memcpy(cols_h + 2 * (size_t)N + w.src, q.u, b);
             memcpy(cols_h + 3 * (size_t)N + w.src, q.v, b);
-            memcpy(cols_h + 4 * (size_t)N + w.src, q.d, b);
+            if (!lid) memcpy(cols_h + 4 * (size_t)N + w.src, q.d, b);
             memcpy(uh + o_flags + w.flag0, q.run_sel, (size_t)w.n_runs);
         }
         int* lh = reinterpret_cast<int*>(uh + w.u_list);
@@ -4602,6 +4649,21 @@ static int set_frame_step(TrackSet& s, bool group, const std::string& who, const
         fa.match = reinterpret_cast<int*>(od + w.d_match);
         flow_h[v] = fa;
     }
+    std::vector<kba_lidar_cloud> clouds;
+    LidarStaged lf;
+    if (lid) {
+        plan.pack(uh + o_lpack);
+        int* idx = reinterpret_cast<int*>(uh + o_idx);
+        for (int v : lid_order) {
+            const StepWin& w = ws[v];
+            for (int r : w.cam_rows) *idx++ = w.src + r;
+        }
+        for (const StepWin& w : ws) clouds.push_back(kba_lidar_cloud{lid[w.i].points, lid[w.i].n_points, lid[w.i].stride});
+        lf.u = reinterpret_cast<const float*>(cols_d + 2 * (size_t)N); lf.v = reinterpret_cast<const float*>(cols_d + 3 * (size_t)N);
+        lf.idx = reinterpret_cast<const int*>(ud + o_idx);
+        lf.d = reinterpret_cast<float*>(st.up.d + o_cols + 16 * (size_t)N);
+        lf.n_copy = n_copy; lf.copy = reinterpret_cast<float*>(od + o_dep);
+    }
     StepLaunch gl;
     gl.win = reinterpret_cast<const StepArgs*>(ud + o_step);
     gl.cols = cols_d; gl.stride = N; gl.run_sel = ud + o_flags; gl.n_win = W;
@@ -4628,7 +4690,9 @@ static int set_frame_step(TrackSet& s, bool group, const std::string& who, const
         for (const StepWin& w : ws) cudaMemsetAsync(w.t->upkeep->map, 0, sizeof(unsigned long long) * (size_t)w.t->td.lm_cap, cs);
         cudaStreamSynchronize(cs);
     };
-    cudaError_t e = cudaMemcpyAsync(st.up.d, uh, up1, cudaMemcpyHostToDevice, cs);
+    cudaError_t e = plan.par.empty() ? cudaSuccess : lidar_copy_clouds(plan, clouds.data(), lws, cs);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(st.up.d, uh, up1, cudaMemcpyHostToDevice, cs);
+    if (e == cudaSuccess && !plan.par.empty()) e = launch_lidar_staged(plan, lws, ud + o_lpack, lf, cs);  // the d column
     if (e == cudaSuccess) {
         launch_frame_step_gather(gl, cs);
         e = cudaEventRecord(mb.ev0, cs);
@@ -4668,7 +4732,7 @@ static int set_frame_step(TrackSet& s, bool group, const std::string& who, const
         w.selected = w.verdict[0] && (w.verdict[1] || w.verdict[2]);
         if (w.selected) sel.push_back(v);
     }
-    int64_t up_bytes = (int64_t)up1, down_bytes = (int64_t)down1;
+    int64_t up_bytes = (int64_t)up1 + cloud_bytes, down_bytes = (int64_t)down1;
     // ---- the push and the creation of the selected windows: one upload of records, one launch sequence, one download
     if (!sel.empty()) {
         const int S = (int)sel.size();
@@ -4742,6 +4806,15 @@ static int set_frame_step(TrackSet& s, bool group, const std::string& who, const
         }
     }
     // ---- outputs
+    if (n_copy) {
+        const float* dep = reinterpret_cast<const float*>(oh + o_dep);
+        for (int v : lid_order) {
+            const StepWin& w = ws[v];
+            float* d = lid[w.i].depth_out;
+            if (!d) break;  // the downloaded frames come first
+            for (int r : w.cam_rows) d[r] = *dep++;
+        }
+    }
     const IterRecord* lg = reinterpret_cast<const IterRecord*>(oh + o_log);
     const unsigned char* rj = oh + o_rej;
     for (const StepWin& w : ws) {
@@ -4766,21 +4839,36 @@ static int set_frame_step(TrackSet& s, bool group, const std::string& who, const
 int kba_track_frame_step(kba_track* t, const kba_frame_step_request* req, const kba_options* opt, kba_frame_step_out* out, kba_result* res) {
     static const std::string who = "kba_track_frame_step: ";
     if (!t || !req || !opt || !out || !res) return fail(KBA_ERR_BAD_ARG, who + "null argument");
-    return set_frame_step(t->set, false, who, req, false, opt, out, res);
+    return set_frame_step(t->set, false, who, req, false, opt, out, res, nullptr);
+}
+int kba_track_frame_step_lidar(kba_track* t, const kba_frame_step_request* req, const kba_frame_lidar* lid, const kba_options* opt,
+                               kba_frame_step_out* out, kba_result* res) {
+    static const std::string who = "kba_track_frame_step_lidar: ";
+    if (!t || !req || !lid || !opt || !out || !res) return fail(KBA_ERR_BAD_ARG, who + "null argument");
+    return set_frame_step(t->set, false, who, req, false, opt, out, res, lid);
 }
 
+// lidar: a _lidar form, which needs lid
 static int group_frame_step(kba_track_group* g, const kba_frame_step_request* req, bool per_track, const kba_options* opts,
-                            kba_frame_step_out* out, kba_result* res, const std::string& who) {
-    if (!g || !req || !opts || !out || !res) return fail(KBA_ERR_BAD_ARG, who + "null argument");
-    return set_frame_step(g->set, true, who, req, per_track, opts, out, res);
+                            kba_frame_step_out* out, kba_result* res, const std::string& who, bool lidar, const kba_frame_lidar* lid) {
+    if (!g || !req || !opts || !out || !res || (lidar && !lid)) return fail(KBA_ERR_BAD_ARG, who + "null argument");
+    return set_frame_step(g->set, true, who, req, per_track, opts, out, res, lid);
 }
 int kba_track_group_frame_step(kba_track_group* g, const kba_frame_step_request* req, const kba_options* opt, kba_frame_step_out* out,
                                kba_result* res) {
-    return group_frame_step(g, req, false, opt, out, res, "kba_track_group_frame_step: ");
+    return group_frame_step(g, req, false, opt, out, res, "kba_track_group_frame_step: ", false, nullptr);
 }
 int kba_track_group_frame_step_opts(kba_track_group* g, const kba_frame_step_request* req, const kba_options* opts,
                                     kba_frame_step_out* out, kba_result* res) {
-    return group_frame_step(g, req, true, opts, out, res, "kba_track_group_frame_step_opts: ");
+    return group_frame_step(g, req, true, opts, out, res, "kba_track_group_frame_step_opts: ", false, nullptr);
+}
+int kba_track_group_frame_step_lidar(kba_track_group* g, const kba_frame_step_request* req, const kba_frame_lidar* lid,
+                                     const kba_options* opt, kba_frame_step_out* out, kba_result* res) {
+    return group_frame_step(g, req, false, opt, out, res, "kba_track_group_frame_step_lidar: ", true, lid);
+}
+int kba_track_group_frame_step_lidar_opts(kba_track_group* g, const kba_frame_step_request* req, const kba_frame_lidar* lid,
+                                          const kba_options* opts, kba_frame_step_out* out, kba_result* res) {
+    return group_frame_step(g, req, true, opts, out, res, "kba_track_group_frame_step_lidar_opts: ", true, lid);
 }
 
 // ---------------------------------------------------------------------------------------------------------------------

@@ -1,7 +1,10 @@
 // kba_kernels.h -- host-visible launch interface of kba_kernels.cu
 #pragma once
+#include <vector>
+
 #include <cuda_runtime.h>
 
+#include "kba_b200.h"
 #include "kba_device.cuh"
 
 namespace kba {
@@ -507,6 +510,57 @@ struct StepLaunch {
     int n_win = 0;
 };
 void launch_frame_step_gather(const StepLaunch& l, cudaStream_t s);
+
+// ---- lidar depth (kba_lidar.cu, compiled with -fmad=false) ----
+// The host halves of kba_lidar_depth_batch, shared with the frame step's lidar form (kba_track_frame_step_lidar): a plan of the
+// call's views -- their parameters in the kernels' single precision and the offsets of their cells, sorted point records, blocks
+// and features --, the handle's grow-only workspace for the used clouds and the scratch, and one launch sequence (memset, count,
+// scan, fill and feature kernels).  The batch's feature pass reads packed (u, v) pairs and writes depths in feature order; the
+// frame step's reads feature k as staged measurement idx[k]: u, v from the staged columns, its depth into the staged d column.
+// Both are one template of k_lidar_feature, so the depths are the same bit for bit.
+struct LidarParams {
+    float R[9], t[3], f, cx, cy;
+    int width, height, cells_x, cells_y;
+    float hw, hh, offx, offy, bw;
+    int hist_min_count, min_points;
+    float depth_min, depth_max, local_tol, crossnorm_min, viewray_min;
+    int local_enabled;
+    // where the view's data sits in the call's concatenated device arrays
+    long long cloud_off;       // floats, into the clouds
+    int n_points, stride;
+    int cell_off;              // cells_x * cells_y + 1 entries of counts, cursors and starts
+    int sort_off;              // n_points sorted point records
+};
+struct LidarPlan {
+    std::vector<LidarParams> par;                // one per view
+    std::vector<int> blk_off{0}, feat_off{0};    // prefixes over the views: blocks of 256 points, features
+    std::vector<long long> cloud_off;            // per cloud: floats into the workspace's clouds; -1: no view names it
+    long long cells = 0, pairs = 0, blocks = 0, feats = 0;
+    size_t b_clouds = 0;
+    explicit LidarPlan(int n_clouds) : cloud_off(n_clouds, -1) {}
+    // a view of n_feat features on cloud c (checked by the caller) with options o; KBA_ERR_CAPACITY when the call's cells,
+    // (view, point) pairs or 2 * features pass INT32_MAX
+    int add(int c, const kba_lidar_cloud& cl, const double* T_cam_lidar, const double* intr, const kba_lidar_options* o, int n_feat);
+    size_t pack_bytes() const;                   // what the launch reads from d_pack: view parameters | block | feature prefix
+    void pack(void* dst) const;
+};
+struct LidarWs {                                 // the plan's part of the handle's workspace
+    float* clouds = nullptr;
+    int* cnt = nullptr, *cur = nullptr, *start = nullptr;
+    void* sorted = nullptr;
+    void* extra = nullptr;                       // the caller's `extra` bytes, 256-byte aligned
+};
+int lidar_workspace(kba_handle* h, const LidarPlan& p, size_t extra, LidarWs& ws);
+// one copy per cloud a view names, from the caller's memory into the workspace
+cudaError_t lidar_copy_clouds(const LidarPlan& p, const kba_lidar_cloud* clouds, const LidarWs& ws, cudaStream_t s);
+struct LidarStaged {                             // the frame step's features: feature k is staged measurement idx[k]
+    const float* u = nullptr, *v = nullptr;      // the staged columns
+    const int* idx = nullptr;                    // [feats] measurement rows, view by view
+    float* d = nullptr;                          // the staged d column: d[idx[k]] = depth
+    int n_copy = 0;                              // the first n_copy features' depths also go to copy[k] (the download)
+    float* copy = nullptr;
+};
+cudaError_t launch_lidar_staged(const LidarPlan& p, const LidarWs& ws, const void* d_pack, const LidarStaged& f, cudaStream_t s);
 
 cudaError_t configure_pack();
 void launch_pack(const BatchDev& bd, const PackRaw& raw, cudaStream_t s);

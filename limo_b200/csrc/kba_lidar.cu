@@ -1,12 +1,14 @@
 // kba_lidar.cu -- lidar depth extraction on sm_90a (BASELINE config 4; C ABI: kba_lidar_depth_batch and kba_lidar_depth, its
-// one-view case, in kba_b200.h).  A call works on "views": a cloud seen by one camera with one feature list.  Per-view
+// one-view case, in kba_b200.h; the frame step's lidar form, kba_track_frame_step_lidar, runs the same plan and kernels from
+// kba_api.cu through kba_kernels.h).  A call works on "views": a cloud seen by one camera with one feature list.  Per-view
 // parameters live in a device array; each view's cell counts, starts and cursors sit at its own offset of one concatenated
 // array, and its sorted point records in a segment of its cloud's n_points.
 //   k_lidar_bin<false>: all (view, point) pairs: project the cloud (coalesced float loads), count points per 16x16-pixel cell
 //   k_lidar_scan      : one CTA per view: exclusive scan of its cell counts
 //   k_lidar_bin<true> : project again and scatter (u, v, x, y, z, index) into each view's cell-sorted order
 //   k_lidar_feature   : one warp per feature of all views: gather the pixel rectangle from the overlapping cells, depth
-//                       histogram, largest triangle, plane / view-ray intersection, depth gates
+//                       histogram, largest triangle, plane / view-ray intersection, depth gates; templated on where a feature
+//                       reads (u, v) and writes its depth (the batch's packed features, or the frame step's staged rows)
 // The bin passes map a block to its view by a per-view block-offset prefix (binary search), the feature pass a warp by the
 // feature-offset prefix: no CTA idles on a view smaller than the largest.
 // Compiled with -fmad=false: the arithmetic is single precision with the operation order of the specification so that the
@@ -21,26 +23,15 @@
 #include <cuda_runtime.h>
 
 #include "kba_b200.h"
+#include "kba_kernels.h"
 
 namespace {
+
+using kba::LidarParams;
 
 constexpr int kCell = 16;      // pixels per cell side
 constexpr int kMaxNb = 96;     // neighbours kept per feature
 constexpr int kBins = 64;
-
-struct LidarParams {
-    float R[9], t[3], f, cx, cy;
-    int width, height, cells_x, cells_y;
-    float hw, hh, offx, offy, bw;
-    int hist_min_count, min_points;
-    float depth_min, depth_max, local_tol, crossnorm_min, viewray_min;
-    int local_enabled;
-    // where the view's data sits in the call's concatenated device arrays
-    long long cloud_off;       // floats, into the clouds
-    int n_points, stride;
-    int cell_off;              // cells_x * cells_y + 1 entries of counts, cursors and starts
-    int sort_off;              // n_points sorted point records
-};
 
 struct ProjPt { float u, v, x, y, z; int idx; };
 
@@ -115,14 +106,34 @@ __device__ __forceinline__ int bin_of(float z, float zmin, float bw) {
     return b > kBins - 1 ? kBins - 1 : b;
 }
 
+// the feature pass's addressing: where feature k reads its (u, v) and writes its depth
+struct PackedFeatures {        // kba_lidar_depth_batch: (u, v) pairs and depths in feature order
+    const float* __restrict__ uv;
+    float* __restrict__ out;
+    __device__ __forceinline__ void load(int k, float& fu, float& fv) const { fu = uv[2 * (size_t)k]; fv = uv[2 * (size_t)k + 1]; }
+    __device__ __forceinline__ void store(int k, float d) const { out[k] = d; }
+};
+struct StagedFeatures {        // the frame step: feature k is staged measurement idx[k] (kba::LidarStaged)
+    kba::LidarStaged s;
+    __device__ __forceinline__ void load(int k, float& fu, float& fv) const {
+        const int m = __ldg(s.idx + k);
+        fu = __ldg(s.u + m); fv = __ldg(s.v + m);
+    }
+    __device__ __forceinline__ void store(int k, float d) const {
+        s.d[__ldg(s.idx + k)] = d;
+        if (k < s.n_copy) s.copy[k] = d;
+    }
+};
+
 // feat_off[n_views + 1]: the views' features concatenated, n_feats in all.  The result does not depend on the order in which
 // the fill pass's atomics placed the points inside a cell: the histogram counts and the nearest depth are order-free, the
 // largest triangle is chosen by area and then by the points' original indices, and a rectangle with more than kMaxNb points
-// gives -1 whatever was gathered.  That is what makes the depths bit-identical to the sequential specification.
+// gives -1 whatever was gathered.  That is what makes the depths bit-identical to the sequential specification, whichever
+// addressing the features come with.
+template <class Feats>
 __global__ void __launch_bounds__(128) k_lidar_feature(const LidarParams* __restrict__ par, const int* __restrict__ feat_off,
                                                        int n_views, const ProjPt* __restrict__ sorted_all,
-                                                       const int* __restrict__ cell_start_all, const float* __restrict__ feats,
-                                                       int n_feats, float* __restrict__ out) {
+                                                       const int* __restrict__ cell_start_all, const Feats feats, int n_feats) {
     __shared__ ProjPt s_nb[4][kMaxNb];
     __shared__ int s_cnt[4][kBins];
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -133,7 +144,8 @@ __global__ void __launch_bounds__(128) k_lidar_feature(const LidarParams* __rest
     const int* cell_start = cell_start_all + P.cell_off;
     ProjPt* nb = s_nb[warp];
     int* cnt = s_cnt[warp];
-    const float fu = feats[2 * (size_t)k], fv = feats[2 * (size_t)k + 1];
+    float fu, fv;
+    feats.load(k, fu, fv);
     const float cu = fu + P.offx, cv = fv + P.offy;
     // ---- gather the rectangle ----
     const int cx0 = max(0, (int)floorf((cu - P.hw) / kCell)), cx1 = min(P.cells_x - 1, (int)floorf((cu + P.hw) / kCell));
@@ -240,7 +252,7 @@ __global__ void __launch_bounds__(128) k_lidar_feature(const LidarParams* __rest
             }
         }
     }
-    if (lane == 0) out[k] = result;
+    if (lane == 0) feats.store(k, result);
 }
 
 void quat_R(const double* q, float* R) {
@@ -251,9 +263,7 @@ void quat_R(const double* q, float* R) {
 }
 
 // a view's pose, intrinsics and options in the kernels' single precision; a negative image size has no cells
-void view_params(const kba_lidar_view& v, const kba_lidar_options* o, LidarParams& P) {
-    const double* T = v.T_cam_lidar;
-    const double* intr = v.intr;
+void view_params(const double* T, const double* intr, const kba_lidar_options* o, LidarParams& P) {
     quat_R(T, P.R);
     P.t[0] = (float)T[4]; P.t[1] = (float)T[5]; P.t[2] = (float)T[6];
     P.f = (float)intr[0]; P.cx = (float)intr[1]; P.cy = (float)intr[2];
@@ -268,6 +278,27 @@ void view_params(const kba_lidar_view& v, const kba_lidar_options* o, LidarParam
 }
 
 size_t al(size_t b) { return (b + 255) & ~(size_t)255; }
+
+// the workspace's scratch: cell counts, cursors and starts (each of cell_bytes), sorted point records
+size_t cell_bytes(const kba::LidarPlan& p) { return al(sizeof(int) * (size_t)p.cells); }
+size_t sorted_bytes(const kba::LidarPlan& p) { return al(sizeof(ProjPt) * (size_t)std::max(p.pairs, 1LL)); }
+
+// the launch sequence of plan p, its pack() at d_pack, on a workspace whose clouds are copied ahead of it on s
+template <class Feats>
+cudaError_t launch_lidar(const kba::LidarPlan& p, const kba::LidarWs& ws, const void* d_pack, const Feats& f, cudaStream_t s) {
+    const int nw = (int)p.par.size();
+    const LidarParams* d_par = (const LidarParams*)d_pack;
+    const int* d_blk = (const int*)(d_par + nw);
+    const int* d_fo = d_blk + nw + 1;
+    ProjPt* sorted = (ProjPt*)ws.sorted;
+    const cudaError_t e = cudaMemsetAsync(ws.cnt, 0, 2 * cell_bytes(p), s);  // the cursors follow the counts
+    if (e != cudaSuccess) return e;
+    if (p.blocks > 0) k_lidar_bin<false><<<(unsigned)p.blocks, 256, 0, s>>>(d_par, d_blk, nw, ws.clouds, ws.cnt, nullptr, nullptr, nullptr);
+    k_lidar_scan<<<nw, 1024, 0, s>>>(d_par, ws.cnt, ws.start);
+    if (p.blocks > 0) k_lidar_bin<true><<<(unsigned)p.blocks, 256, 0, s>>>(d_par, d_blk, nw, ws.clouds, ws.cnt, ws.start, ws.cur, sorted);
+    k_lidar_feature<Feats><<<(unsigned)((p.feats + 3) / 4), 128, 0, s>>>(d_par, d_fo, nw, sorted, ws.start, f, (int)p.feats);
+    return cudaSuccess;
+}
 
 }  // namespace
 
@@ -286,6 +317,68 @@ extern "C" int kba_internal_stream(kba_handle* h, cudaStream_t* s, int* device);
 extern "C" int kba_internal_fail(int code, const char* msg);
 extern "C" int kba_internal_workspace(kba_handle* h, size_t bytes, void** out);
 
+namespace kba {
+
+int LidarPlan::add(int c, const kba_lidar_cloud& cl, const double* T, const double* intr, const kba_lidar_options* o, int n_feat) {
+    if (cloud_off[c] < 0) {
+        cloud_off[c] = (long long)(b_clouds / sizeof(float));
+        b_clouds += al(sizeof(float) * (size_t)cl.n_points * cl.stride);
+    }
+    LidarParams P;
+    view_params(T, intr, o, P);
+    P.cloud_off = cloud_off[c]; P.n_points = cl.n_points; P.stride = cl.stride;
+    P.cell_off = (int)std::min<long long>(cells, INT_MAX); P.sort_off = (int)std::min<long long>(pairs, INT_MAX);
+    cells += (long long)P.cells_x * P.cells_y + 1;
+    pairs += cl.n_points;
+    blocks += (cl.n_points + 255) / 256;
+    feats += n_feat;
+    if (cells > INT_MAX || pairs > INT_MAX || 2 * feats > INT_MAX) return KBA_ERR_CAPACITY;
+    par.push_back(P);
+    blk_off.push_back((int)blocks); feat_off.push_back((int)feats);
+    return KBA_OK;
+}
+
+size_t LidarPlan::pack_bytes() const { return sizeof(LidarParams) * par.size() + 2 * sizeof(int) * (par.size() + 1); }
+
+void LidarPlan::pack(void* dst) const {
+    char* d = (char*)dst;
+    const size_t nw = par.size();
+    memcpy(d, par.data(), sizeof(LidarParams) * nw); d += sizeof(LidarParams) * nw;
+    memcpy(d, blk_off.data(), sizeof(int) * (nw + 1)); d += sizeof(int) * (nw + 1);
+    memcpy(d, feat_off.data(), sizeof(int) * (nw + 1));
+}
+
+// one device workspace owned by the handle (grow-only): clouds | cell counts | cursors | starts | sorted point records | extra
+int lidar_workspace(kba_handle* h, const LidarPlan& p, size_t extra, LidarWs& ws) {
+    const size_t b_cell = cell_bytes(p), b_sorted = sorted_bytes(p);
+    void* base = nullptr;
+    if (kba_internal_workspace(h, p.b_clouds + 3 * b_cell + b_sorted + al(extra), &base) != KBA_OK) return KBA_ERR_CUDA;
+    char* wp = (char*)base;
+    ws.clouds = (float*)wp; wp += p.b_clouds;
+    ws.cnt = (int*)wp; wp += b_cell;
+    ws.cur = (int*)wp; wp += b_cell;
+    ws.start = (int*)wp; wp += b_cell;
+    ws.sorted = wp; wp += b_sorted;
+    ws.extra = wp;
+    return KBA_OK;
+}
+
+cudaError_t lidar_copy_clouds(const LidarPlan& p, const kba_lidar_cloud* clouds, const LidarWs& ws, cudaStream_t s) {
+    for (size_t c = 0; c < p.cloud_off.size(); ++c) {
+        if (p.cloud_off[c] < 0 || clouds[c].n_points == 0) continue;
+        const cudaError_t e = cudaMemcpyAsync(ws.clouds + p.cloud_off[c], clouds[c].points,
+                                              sizeof(float) * (size_t)clouds[c].n_points * clouds[c].stride, cudaMemcpyHostToDevice, s);
+        if (e != cudaSuccess) return e;
+    }
+    return cudaSuccess;
+}
+
+cudaError_t launch_lidar_staged(const LidarPlan& p, const LidarWs& ws, const void* d_pack, const LidarStaged& f, cudaStream_t s) {
+    return launch_lidar(p, ws, d_pack, StagedFeatures{f}, s);
+}
+
+}  // namespace kba
+
 namespace {
 
 int fail_at(int code, const char* fn, const char* what, long long i, const char* msg) {
@@ -293,7 +386,7 @@ int fail_at(int code, const char* fn, const char* what, long long i, const char*
     return kba_internal_fail(code, m.c_str());
 }
 
-// the host code of every lidar call: opts[0] for every view, or opts[i] for view i (per_view)
+// the host code of every lidar depth batch: opts[0] for every view, or opts[i] for view i (per_view)
 int lidar_batch(kba_handle* h, int32_t n_clouds, const kba_lidar_cloud* clouds, int32_t n_views, const kba_lidar_view* views,
                 const kba_lidar_options* opts, bool per_view, float* device_ms, const char* fn) {
     const std::string name(fn);
@@ -315,92 +408,55 @@ int lidar_batch(kba_handle* h, int32_t n_clouds, const kba_lidar_cloud* clouds, 
         return KBA_OK;
     }
     if (!opts) return kba_internal_fail(KBA_ERR_BAD_ARG, (name + ": null options").c_str());
-    std::vector<long long> cloud_off(n_clouds, -1);  // floats into the device clouds; -1: no working view names it
-    size_t b_clouds = 0;
+    std::vector<char> named(n_clouds, 0);
     for (int i : work) {
         const int c = views[i].cloud;
-        if (cloud_off[c] >= 0) continue;
+        if (named[c]) continue;
+        named[c] = 1;
         const kba_lidar_cloud& cl = clouds[c];
         if (cl.n_points < 0) return fail_at(KBA_ERR_BAD_ARG, fn, "cloud", c, "negative n_points");
         if (cl.stride < 3) return fail_at(KBA_ERR_BAD_ARG, fn, "cloud", c, "stride < 3");
         if (cl.n_points > 0 && !cl.points) return fail_at(KBA_ERR_BAD_ARG, fn, "cloud", c, "null points");
-        cloud_off[c] = (long long)(b_clouds / sizeof(float));
-        b_clouds += al(sizeof(float) * (size_t)cl.n_points * cl.stride);
+    }
+    kba::LidarPlan plan(n_clouds);
+    for (int i : work) {
+        const kba_lidar_view& v = views[i];
+        if (plan.add(v.cloud, clouds[v.cloud], v.T_cam_lidar, v.intr, per_view ? &opts[i] : opts, v.n_features) != KBA_OK)
+            return fail_at(KBA_ERR_CAPACITY, fn, "view", i, "the call's cells, (view, point) pairs or features exceed 32-bit indexing");
     }
     const int nw = (int)work.size();
-    std::vector<LidarParams> par(nw);
-    std::vector<int> blk_off(nw + 1, 0), feat_off(nw + 1, 0);
-    long long cells = 0, pairs = 0, blocks = 0, feats = 0;
-    for (int w = 0; w < nw; ++w) {
-        const int i = work[w];
-        const kba_lidar_view& v = views[i];
-        const kba_lidar_cloud& cl = clouds[v.cloud];
-        LidarParams& P = par[w];
-        view_params(v, per_view ? &opts[i] : opts, P);
-        P.cloud_off = cloud_off[v.cloud]; P.n_points = cl.n_points; P.stride = cl.stride;
-        P.cell_off = (int)std::min<long long>(cells, INT_MAX); P.sort_off = (int)std::min<long long>(pairs, INT_MAX);
-        cells += (long long)P.cells_x * P.cells_y + 1;
-        pairs += cl.n_points;
-        blocks += (cl.n_points + 255) / 256;
-        feats += v.n_features;
-        if (cells > INT_MAX || pairs > INT_MAX || 2 * feats > INT_MAX)
-            return fail_at(KBA_ERR_CAPACITY, fn, "view", i, "the call's cells, (view, point) pairs or features exceed 32-bit indexing");
-        blk_off[w + 1] = (int)blocks; feat_off[w + 1] = (int)feats;
-    }
+    const size_t feats = (size_t)plan.feats;
     cudaStream_t s;
     int device;
     if (kba_internal_stream(h, &s, &device) != KBA_OK) return KBA_ERR_BAD_ARG;
-    // one device workspace owned by the handle (grow-only):
-    //   clouds | packed upload (features | view parameters | block and feature prefixes) | depths | cell counts, cursors | cell
-    //   starts | sorted point records
-    const size_t b_feat = al(sizeof(float) * 2 * (size_t)feats), b_par = al(sizeof(LidarParams) * nw), b_pre = al(sizeof(int) * (nw + 1)),
-                 b_pack = b_feat + b_par + 2 * b_pre, b_out = al(sizeof(float) * (size_t)feats), b_cell = al(sizeof(int) * (size_t)cells),
-                 b_sorted = al(sizeof(ProjPt) * (size_t)std::max(pairs, 1LL));
-    void* ws = nullptr;
-    if (kba_internal_workspace(h, b_clouds + b_pack + b_out + 3 * b_cell + b_sorted, &ws) != KBA_OK) return KBA_ERR_CUDA;
-    char* wp = (char*)ws;
-    float* d_clouds = (float*)wp; wp += b_clouds;
-    char* d_pack = wp; wp += b_pack;
-    const float* d_feats = (const float*)d_pack;
-    const LidarParams* d_par = (const LidarParams*)(d_pack + b_feat);
-    const int* d_blk = (const int*)(d_pack + b_feat + b_par);
-    const int* d_fo = (const int*)(d_pack + b_feat + b_par + b_pre);
-    float* d_out = (float*)wp; wp += b_out;
-    int* d_cnt = (int*)wp; wp += b_cell;
-    int* d_cur = (int*)wp; wp += b_cell;  // right after the counts: one memset clears both
-    int* d_start = (int*)wp; wp += b_cell;
-    ProjPt* d_sorted = (ProjPt*)wp;
+    // the workspace's extra part: the packed upload (view parameters and prefixes | features) | depths
+    const size_t b_par = al(plan.pack_bytes()), b_pack = b_par + al(sizeof(float) * 2 * feats);
+    kba::LidarWs ws;
+    if (kba::lidar_workspace(h, plan, b_pack + al(sizeof(float) * feats), ws) != KBA_OK) return KBA_ERR_CUDA;
+    char* d_pack = (char*)ws.extra;
+    float* d_out = (float*)(d_pack + b_pack);
     // host staging of the packed upload and of the depths, grow-only per host thread
     static thread_local std::vector<char> pack;
     static thread_local std::vector<float> depths;
     if (pack.size() < b_pack) pack.resize(b_pack);
-    if (depths.size() < (size_t)feats) depths.resize((size_t)feats);
+    if (depths.size() < feats) depths.resize(feats);
+    plan.pack(pack.data());
     for (int w = 0; w < nw; ++w) {
         const kba_lidar_view& v = views[work[w]];
-        memcpy(pack.data() + sizeof(float) * 2 * (size_t)feat_off[w], v.features_uv, sizeof(float) * 2 * (size_t)v.n_features);
+        memcpy(pack.data() + b_par + sizeof(float) * 2 * (size_t)plan.feat_off[w], v.features_uv, sizeof(float) * 2 * (size_t)v.n_features);
     }
-    memcpy(pack.data() + b_feat, par.data(), sizeof(LidarParams) * nw);
-    memcpy(pack.data() + b_feat + b_par, blk_off.data(), sizeof(int) * (nw + 1));
-    memcpy(pack.data() + b_feat + b_par + b_pre, feat_off.data(), sizeof(int) * (nw + 1));
     cudaEvent_t e0 = nullptr, e1 = nullptr;
     cudaError_t err = cudaSuccess;
     auto chk = [&](cudaError_t e) { if (err == cudaSuccess && e != cudaSuccess) err = e; };
     chk(cudaSetDevice(device));
     if (device_ms) { chk(cudaEventCreate(&e0)); chk(cudaEventCreate(&e1)); }
     if (err == cudaSuccess) {
-        for (int c = 0; c < n_clouds; ++c)
-            if (cloud_off[c] >= 0 && clouds[c].n_points > 0)
-                chk(cudaMemcpyAsync(d_clouds + cloud_off[c], clouds[c].points, sizeof(float) * (size_t)clouds[c].n_points * clouds[c].stride,
-                                    cudaMemcpyHostToDevice, s));
+        chk(kba::lidar_copy_clouds(plan, clouds, ws, s));
         chk(cudaMemcpyAsync(d_pack, pack.data(), b_pack, cudaMemcpyHostToDevice, s));
         if (e0) chk(cudaEventRecord(e0, s));
-        chk(cudaMemsetAsync(d_cnt, 0, 2 * b_cell, s));
-        if (blocks > 0) k_lidar_bin<false><<<(unsigned)blocks, 256, 0, s>>>(d_par, d_blk, nw, d_clouds, d_cnt, nullptr, nullptr, nullptr);
-        k_lidar_scan<<<nw, 1024, 0, s>>>(d_par, d_cnt, d_start);
-        if (blocks > 0) k_lidar_bin<true><<<(unsigned)blocks, 256, 0, s>>>(d_par, d_blk, nw, d_clouds, d_cnt, d_start, d_cur, d_sorted);
-        k_lidar_feature<<<(unsigned)((feats + 3) / 4), 128, 0, s>>>(d_par, d_fo, nw, d_sorted, d_start, d_feats, (int)feats, d_out);
+        if (err == cudaSuccess) chk(launch_lidar(plan, ws, d_pack, PackedFeatures{(const float*)(d_pack + b_par), d_out}, s));
         if (e1) chk(cudaEventRecord(e1, s));
-        chk(cudaMemcpyAsync(depths.data(), d_out, sizeof(float) * (size_t)feats, cudaMemcpyDeviceToHost, s));
+        chk(cudaMemcpyAsync(depths.data(), d_out, sizeof(float) * feats, cudaMemcpyDeviceToHost, s));
         chk(cudaStreamSynchronize(s));
         chk(cudaGetLastError());
         if (err == cudaSuccess && device_ms) chk(cudaEventElapsedTime(device_ms, e0, e1));
@@ -410,7 +466,7 @@ int lidar_batch(kba_handle* h, int32_t n_clouds, const kba_lidar_cloud* clouds, 
     if (err != cudaSuccess) return kba_internal_fail(KBA_ERR_CUDA, cudaGetErrorString(err));
     for (int w = 0; w < nw; ++w) {
         const kba_lidar_view& v = views[work[w]];
-        memcpy(v.depth_out, depths.data() + feat_off[w], sizeof(float) * (size_t)v.n_features);
+        memcpy(v.depth_out, depths.data() + plan.feat_off[w], sizeof(float) * (size_t)v.n_features);
     }
     return KBA_OK;
 }
