@@ -1370,6 +1370,100 @@ int kba_track_group_frame_step_lidar(kba_track_group* g, const kba_frame_step_re
 int kba_track_group_frame_step_lidar_opts(kba_track_group* g, const kba_frame_step_request* req, const kba_frame_lidar* lid,
                                           const kba_options* opts, kba_frame_step_out* out, kba_result* res);
 
+/* ---- limo's camera callback as one store call: the frame step and, when it is due, the solve block -----------------------
+ * What limo's camera callback runs on the stored window (mono_lidar.cpp:88-372, mono_standalone.cpp:134-183), minus the motion
+ * prior (the caller passes pose7): the frame step, then -- when it is due (more than two keyframes and enough time since the last
+ * solve, mono_lidar.cpp:243-244) -- the solve block on the landmarks the push leaves active.  Every output, both results and every
+ * store afterwards equal, bit for bit, what this chain of store calls gives:
+ *   1. kba_track_frame_step on req->step (with lid: kba_track_frame_step_lidar on req->step and lid), with opt_adjust;
+ *   2. the solve rule: KBA_STEP_SOLVE_ALWAYS solves, KBA_STEP_SOLVE_IF_SELECTED solves iff the frame was selected (a caller whose
+ *      keyframe count reaches 3 only with this frame), KBA_STEP_SOLVE_NEVER does not; the caller evaluates limo's time rule;
+ *   3. the solve block's lists after the push (bundle_adjuster_keyframes.cpp:289-330): the keyframes step.kf_slot, followed by
+ *      step.kf_new if the frame was selected; the landmarks, in candidate order, the candidates lm_slot[j] whose tag lm_new[j] is
+ *        -2 (active before the frame): always;  -1 (an existing landmark the frame measures): iff the frame was selected;
+ *        k >= 0 (step.new_slot[k], lm_slot[j] == new_slot[k]): iff the frame was selected and the creation set bit 0 of flags[k];
+ *      with lm_ground[j] (NULL: none is ground) as the listed landmarks' is_ground_plane;
+ *   4. if it is due, kba_track_keyframe_solve on those lists with the request's other fields (as kba_kfsolve_request takes them)
+ *      and opt_solve.
+ * Outputs (caller-owned): step, as the frame step writes it; solved (the solve block ran); n_lm, the list's length, and
+ * lm_index [n_cand], each candidate's position in the list or -1 (both written only when solved); solve, as
+ * kba_track_keyframe_solve writes it, its landmark arrays indexed by the compacted list (kf_active, kf_common sized for
+ * step.n_kf + 1, the landmark arrays and rank.cand / category for n_cand); res_adjust as the frame step's res; res_solve as the
+ * solve block's res (idle when it does not run).
+ * On the device: the first upload stages everything the frame step stages and, for each request that may solve, the solve block's
+ * lists, tags, tracklets, classes, outliers and AddDepth entries; its launch sequence and download are the frame step's.  The host
+ * composes the verdicts and decides which tracks solve.  Then one upload of the push's, the creation's and the solve block's
+ * argument records, and one launch sequence: k_arena_compact, k_store_append, the creation's kernels, k_cs_lists (the post-push
+ * landmark list, compacted by tag, verdict and creation flag into the solve block's staged list; its length stays in device
+ * memory, where the deactivation and k_kfs_labels read it) and the solve block's first part (k_up_*, k_kfs_labels, k_sel_*,
+ * k_rk_prep, k_rk_depth); one download brings back the creation's and the solve block's first outputs.  From there the sequence is
+ * kba_track_keyframe_solve's.  A selected, solving frame synchronises three times (the chain: four) before the solve's own.
+ * Checks: every check that needs only the request runs before anything is uploaded, and a refusal there writes no output and
+ * changes no store: the frame step's own; an unknown solve policy; for requests that may solve, the solve block's request checks
+ * on the candidate bound n_cand (the keyframe list step.kf_slot), a null lm_slot, lm_new or lm_index with n_cand > 0, a tag below
+ * -2 or at least n_new, and a k >= 0 tag named twice or not at new_slot[k] (KBA_ERR_BAD_ARG).  The solve block's late refusals
+ * stay late: no keyframe kept, the solve's checks on the kept keyframes, a failing or missing draw function, the ranked solve's
+ * checks.  After one, the frame step is done: out.step and res_adjust are written, every store holds the frame step's writes,
+ * solved = 0 and the call returns the solve block's code -- what the chain leaves behind (all-or-nothing over the solving tracks).
+ * Transfers (kba_track_transfer_bytes / kba_track_group_transfer_bytes), P the requests that may solve (solve != NEVER), each
+ * with K = step.n_kf + 1 and L = n_cand, D of them solving, R_s the size of one window's argument records (a constant of the
+ * library build, k_cs_lists' record included), D_w and B_w the draws and the selection bound of a solving request as
+ * kba_track_keyframe_solve states them, each request's arrays padded as in kba_track_keyframe_solve:
+ *         h2d = the frame step's + sum over P of (8 n_depth + 4 (K + 2 L + n_outlier + n_trk) + L + n_trk)
+ *               + (D ? R_s P + 8 D + 4 sum(D_w) + the solve's : 0)
+ *         d2h = the frame step's + (D ? 4 P + sum over P of (12 + 9 K + 7 L + n_trk) + 8 D + 5 sum(B_w) + the solve's : 0)
+ * where the solve's are kba_track_solve_ranked's (kba_track_group_solve_ranked's) over the D solving requests.
+ * Allocations: the two calls' (their staging, grow-only, is shared with kba_track_frame_step and kba_track_keyframe_solve).
+ * The group forms serve one request per track (req[n_tracks], lid: NULL or lid[n_tracks], out[n_tracks], res_*[n_tracks]):
+ * step.n_kf == 0 sits the call out; a request with solve == NEVER or an unmet IF_SELECTED only runs the frame step; a failing
+ * request returns its code and kba_last_error names its track; _opts takes one adjustment and one solve kba_options per track.
+ * A single call is the group call's one-track case. */
+#define KBA_STEP_SOLVE_NEVER 0
+#define KBA_STEP_SOLVE_ALWAYS 1
+#define KBA_STEP_SOLVE_IF_SELECTED 2
+typedef struct kba_camera_step_request {
+    kba_frame_step_request step;  /* step.kf_slot: the active keyframes before the frame                                      */
+    uint8_t solve;              /* KBA_STEP_SOLVE_*                                                                           */
+    uint8_t reserved_[3];
+    int32_t n_cand;
+    int32_t min_connecting, min_window, max_window;
+    int32_t n_trk;
+    const int32_t* lm_slot;     /* [n_cand] the landmarks the push could leave active, ascending landmark id                   */
+    const int32_t* lm_new;      /* [n_cand] their tags: -2 active before the frame, -1 measured by it, k >= 0 step.new_slot[k]  */
+    const uint8_t* lm_ground;   /* [n_cand] is_ground_plane of the candidates, or NULL (none)                                  */
+    const kba_tracklet* trk;    /* [n_trk] the current frame's tracklets                                                       */
+    const kba_label_class* classes;  /* [n_class] */
+    int32_t n_class;
+    int32_t n_outlier;
+    const int32_t* outlier_slot;     /* [n_outlier] the caller's current outlier set                                           */
+    double shrubbery_weight;
+    const kba_select_params* params; /* the ranking, as kba_kfsolve_request                                                    */
+    int32_t max_near, max_middle, max_far;
+    int32_t n_depth;
+    const kba_depth_entry* depth;
+    int32_t (*draw)(void* ctx, int32_t n, int32_t* out);
+    void* draw_ctx;
+    const kba_window* sel;      /* the solve's scalars and ground mode, as kba_kfsolve_request                                 */
+} kba_camera_step_request;
+typedef struct kba_camera_step_out {  /* caller-owned */
+    kba_frame_step_out step;
+    uint8_t solved;             /* the solve block ran                                                                        */
+    uint8_t reserved_[3];
+    int32_t n_lm;               /* the solve's landmark list length (written when solved)                                     */
+    int32_t* lm_index;          /* [n_cand] each candidate's position in that list, or -1 (written when solved)               */
+    kba_kfsolve_out solve;      /* landmark arrays indexed by the compacted list                                              */
+} kba_camera_step_out;
+int kba_track_camera_step(kba_track* t, const kba_camera_step_request* req, const kba_frame_lidar* lid, const kba_options* opt_adjust,
+                          const kba_options* opt_solve, kba_camera_step_out* out, kba_result* res_adjust, kba_result* res_solve);
+/* req[n_tracks], lid NULL or lid[n_tracks], out[n_tracks], res_adjust[n_tracks], res_solve[n_tracks] */
+int kba_track_group_camera_step(kba_track_group* g, const kba_camera_step_request* req, const kba_frame_lidar* lid,
+                                const kba_options* opt_adjust, const kba_options* opt_solve, kba_camera_step_out* out,
+                                kba_result* res_adjust, kba_result* res_solve);
+/* opts_adjust[n_tracks], opts_solve[n_tracks]: track i's adjustment and solve run with its entries */
+int kba_track_group_camera_step_opts(kba_track_group* g, const kba_camera_step_request* req, const kba_frame_lidar* lid,
+                                     const kba_options* opts_adjust, const kba_options* opts_solve, kba_camera_step_out* out,
+                                     kba_result* res_adjust, kba_result* res_solve);
+
 #ifdef __cplusplus
 }
 #endif

@@ -5,12 +5,13 @@ computing call fails with KBA_ERR_CUDA when no sm_90 (H100) device is present.
 """
 import ctypes as C
 import functools
+import inspect
 import itertools
 import os
 
 import numpy as np
 
-from .capi_types import (KbaCounters, KbaCreateOut, KbaCreateRequest, KbaDeactivateOut, KbaDeactivateRequest, KbaDepthEntry, KbaDepthOut, KbaDepthRequest, KbaDrawFn, KbaEvalOut, KbaEvaluateOut, KbaFlowOut, KbaFlowRequest, KbaFrameLidar, KbaFrameStepOut, KbaFrameStepRequest, KbaKfsolveOut, KbaKfsolveRequest, KbaLabelClass, KbaLandmarkWrite, KbaLidarCloud, KbaLidarOptions, KbaLidarView, KbaOptions, KbaPoseWrite, KbaPushRequest, KbaRankedRequest, KbaRankOut, KbaRankRequest, KbaReclaimOut, KbaReclaimRequest, KbaResult, KbaSelectOut, KbaSelectParams, KbaSelectRequest, KbaTracklet,
+from .capi_types import (KbaCameraStepOut, KbaCameraStepRequest, STEP_SOLVE, KbaCounters, KbaCreateOut, KbaCreateRequest, KbaDeactivateOut, KbaDeactivateRequest, KbaDepthEntry, KbaDepthOut, KbaDepthRequest, KbaDrawFn, KbaEvalOut, KbaEvaluateOut, KbaFlowOut, KbaFlowRequest, KbaFrameLidar, KbaFrameStepOut, KbaFrameStepRequest, KbaKfsolveOut, KbaKfsolveRequest, KbaLabelClass, KbaLandmarkWrite, KbaLidarCloud, KbaLidarOptions, KbaLidarView, KbaOptions, KbaPoseWrite, KbaPushRequest, KbaRankedRequest, KbaRankOut, KbaRankRequest, KbaReclaimOut, KbaReclaimRequest, KbaResult, KbaSelectOut, KbaSelectParams, KbaSelectRequest, KbaTracklet,
                          KbaSnapshotHeader, KbaTrackCaps, KbaTrackFrame, KbaTrackRequest, KbaWindow, Result, Window, c_double_p, c_float_p, c_int32_p,
                          c_uint8_p)
 
@@ -39,7 +40,8 @@ SYMBOLS = ["kba_version", "kba_last_error", "kba_default_options", "kba_create",
            "kba_track_group_snapshot_sizes", "kba_track_group_save", "kba_track_evaluate", "kba_track_group_evaluate",
            "kba_track_group_evaluate_opts", "kba_track_keyframe_solve", "kba_track_group_keyframe_solve",
            "kba_track_group_keyframe_solve_opts", "kba_track_frame_step", "kba_track_group_frame_step", "kba_track_group_frame_step_opts",
-           "kba_track_frame_step_lidar", "kba_track_group_frame_step_lidar", "kba_track_group_frame_step_lidar_opts"]
+           "kba_track_frame_step_lidar", "kba_track_group_frame_step_lidar", "kba_track_group_frame_step_lidar_opts",
+           "kba_track_camera_step", "kba_track_group_camera_step", "kba_track_group_camera_step_opts"]
 
 
 class KbaError(RuntimeError):
@@ -185,6 +187,9 @@ def lib():
         for f in (L.kba_track_frame_step_lidar, L.kba_track_group_frame_step_lidar, L.kba_track_group_frame_step_lidar_opts):
             f.argtypes = [vp, C.POINTER(KbaFrameStepRequest), C.POINTER(KbaFrameLidar), C.POINTER(KbaOptions), C.POINTER(KbaFrameStepOut),
                           C.POINTER(KbaResult)]
+        for f in (L.kba_track_camera_step, L.kba_track_group_camera_step, L.kba_track_group_camera_step_opts):
+            f.argtypes = [vp, C.POINTER(KbaCameraStepRequest), C.POINTER(KbaFrameLidar), C.POINTER(KbaOptions), C.POINTER(KbaOptions),
+                          C.POINTER(KbaCameraStepOut), C.POINTER(KbaResult), C.POINTER(KbaResult)]
         L.kba_lidar_default_options.argtypes = [C.POINTER(KbaLidarOptions)]
         L.kba_lidar_default_options.restype = None
         fp = C.POINTER(C.c_float)
@@ -891,6 +896,16 @@ class Track:
         return _frame_step_call(self._p, lib().kba_track_frame_step, lib().kba_track_frame_step_lidar, [kw],
                                 C.byref(opt or default_options()), iterations_capacity, [self.n_cam])[0]
 
+    def camera_step(self, opt_adjust=None, opt_solve=None, iterations_capacity=256, **kw):
+        """limo's camera callback -- the frame step and, when due, the solve block on the landmarks the push leaves active -- as one
+        call (kba_track_camera_step).  Keywords: those of frame_step (d or a cloud), solve ("never", "always", "if_selected"),
+        cand_slots / cand_tags / cand_ground (the solve's candidate list: ascending landmark id; tag -2 active before the frame,
+        -1 measured by it, k >= 0 new_slots[k]) and the keywords of keyframe_solve but its lists.  opt_adjust, opt_solve: the
+        adjustment's and the solve's options.  Returns a dict: step (frame_step's dict), solved, and when solved n_lm, lm_index
+        (each candidate's position in the solve's list, or -1) and solve (keyframe_solve's dict, its landmark arrays for the list)."""
+        return _camera_step_call(self._p, lib().kba_track_camera_step, [kw], [self], C.byref(opt_adjust or default_options()),
+                                 C.byref(opt_solve or default_options()), iterations_capacity)[0]
+
     def transfer_bytes(self):
         a, b, c = C.c_int64(), C.c_int64(), C.c_int64()
         _check(lib().kba_track_transfer_bytes(self._p, C.byref(a), C.byref(b), C.byref(c)))
@@ -968,6 +983,78 @@ def _frame_step_call(p, fn, fn_lidar, requests, o, capacity, n_cam):
     args = [req.ctypes.data_as(C.POINTER(KbaFrameStepRequest))] + [x.ctypes.data_as(C.POINTER(KbaFrameLidar)) for x in lid]
     _check(f(p, *args, o, out.ctypes.data_as(C.POINTER(KbaFrameStepOut)), ress))
     return [None if r is None else result(i, ress) for i, r in enumerate(requests)]
+
+
+_STEP_KEYS = frozenset(inspect.signature(_frame_step_args).parameters)
+
+
+def _camera_step_solve(track, capacity, kf_slots, kf_new, solve="never", cand_slots=(), cand_tags=(), cand_ground=None, **kw):
+    """the solve block's part of one camera step request of track: solve ("never", "always", "if_selected"), the candidates of
+    the solve's landmark list (cand_slots in ascending landmark id, cand_tags: -2 active before the frame, -1 measured by it,
+    k >= 0 new_slots[k]; cand_ground their is_ground_plane) and the other keywords of Track.keyframe_solve, over the keyframes
+    kf_slots followed by kf_new.  Returns (request with its step part zero, output with its step part zero, the KbaResult the
+    solve fills, keep, result(out, res_solve) -> (n_lm, lm_index, keyframe_solve's dict))."""
+    if solve not in STEP_SOLVE:
+        raise ValueError("solve must be one of %s, got %r" % (sorted(STEP_SOLVE), solve))
+    if solve == "never":
+        return KbaCameraStepRequest(), KbaCameraStepOut(), KbaResult(), (), None
+    kf = list(_arr(kf_slots, np.int32, -1)) + [int(kf_new)]
+    q, o, kkeep, kdone, krc = track._keyframe_solve_request(capacity, kf, cand_slots, lm_ground=cand_ground, **kw)
+    tags = _arr(cand_tags, np.int32, -1)
+    if len(tags) != q.n_lm:
+        raise ValueError("cand_tags has %d tags for %d candidates" % (len(tags), q.n_lm))
+    index = np.full(q.n_lm, -1, np.int32)
+    r = KbaCameraStepRequest(solve=STEP_SOLVE[solve], n_cand=q.n_lm, lm_new=_p(tags, c_int32_p))
+    for f, _ in KbaKfsolveRequest._fields_:
+        if f not in ("n_kf", "n_lm", "kf_slot"):
+            setattr(r, f, getattr(q, f))
+    out = KbaCameraStepOut(lm_index=_p(index, c_int32_p), solve=o)
+
+    def result(c, res_solve):
+        d = kdone(c.solve, res_solve)
+        for k in ("lm_active", "lm_outlier", "lm_ground"):
+            d[k] = d[k][:c.n_lm].copy()
+        return c.n_lm, index.copy(), d
+    return r, out, krc, (kkeep, tags, index), result
+
+
+def _camera_step_call(p, fn, requests, tracks, o_adjust, o_solve, capacity):
+    """a camera step of the track or group p through fn: the frame step's records of every request built at once (as for
+    frame_step), the solve block's part per request that may solve.  One result dict per request, None for a track that sits
+    out.  Every request carries a cloud or none does (the lidar form is the call with lid, the other one without)."""
+    n = len(requests)
+    steps = [None if r is None else {k: v for k, v in r.items() if k in _STEP_KEYS} for r in requests]
+    lidars = {"cloud" in r for r in steps if r is not None}
+    if len(lidars) > 1:
+        raise ValueError("%s: a call's requests all carry a cloud or none does" % fn.__name__)
+    lidar = lidars == {True}
+    freq, fout, fress, fkeep, fresult, *flid = _frame_step_records(fn, steps, capacity, lidar, [t.n_cam for t in tracks])
+    reqs, outs, rs = (KbaCameraStepRequest * n)(), (KbaCameraStepOut * n)(), (KbaResult * n)()
+    keep, done = [], {}
+    sq, so = C.sizeof(KbaFrameStepRequest), C.sizeof(KbaFrameStepOut)
+    for i, r in enumerate(requests):
+        if r is None:
+            continue
+        rest = {k: v for k, v in r.items() if k not in _STEP_KEYS}
+        q, ob, rc, k, d = _built(fn, i, rest, _camera_step_solve, tracks[i], capacity, r.get("kf_slots", ()), r.get("kf_new", 0))
+        reqs[i], outs[i], rs[i] = q, ob, rc
+        C.memmove(C.addressof(reqs[i]), freq.ctypes.data + sq * i, sq)  # the step part, at offset 0 of both structs
+        C.memmove(C.addressof(outs[i]), fout.ctypes.data + so * i, so)
+        keep.append(k)
+        done[i] = d
+    lid = flid[0].ctypes.data_as(C.POINTER(KbaFrameLidar)) if lidar else None
+    _check(fn(p, reqs, lid, o_adjust, o_solve, outs, fress, rs))
+    results = [None] * n
+    for i, r in enumerate(requests):
+        if r is None:
+            continue
+        C.memmove(fout.ctypes.data + so * i, C.addressof(outs[i]), so)
+        res = dict(step=fresult(i, fress), solved=bool(outs[i].solved), n_lm=None, lm_index=None, solve=None)
+        if outs[i].solved:
+            res["n_lm"], res["lm_index"], res["solve"] = done[i](outs[i], rs[i])
+        results[i] = res
+    del keep, fkeep
+    return results
 
 
 def _no_keyframes(q):  # n_kf = 0 would sit the track out: a request without keyframes is an error, as for one track
@@ -1164,6 +1251,25 @@ class TrackGroup:
         fn, o = _options(opt, len(self.tracks), L.kba_track_group_frame_step, L.kba_track_group_frame_step_opts)
         fn_lidar, _ = _options(opt, len(self.tracks), L.kba_track_group_frame_step_lidar, L.kba_track_group_frame_step_lidar_opts)
         return _frame_step_call(self._p, fn, fn_lidar, requests, o, iterations_capacity, [t.n_cam for t in self.tracks])
+
+    def camera_step(self, requests, opt_adjust=None, opt_solve=None, iterations_capacity=256):
+        """limo's camera callback for every track (kba_track_group_camera_step): each entry None (the track sits the call out) or
+        a dict with the keywords of Track.camera_step.  opt_adjust, opt_solve: one KbaOptions each, or one per track (both lists:
+        kba_track_group_camera_step_opts).  Returns one result dict per track (Track.camera_step's), None for a track that sat
+        out."""
+        assert len(requests) == len(self.tracks)
+        L, n = lib(), len(self.tracks)
+        per_track = not (opt_adjust is None or isinstance(opt_adjust, KbaOptions)) or \
+            not (opt_solve is None or isinstance(opt_solve, KbaOptions))
+        fn = L.kba_track_group_camera_step_opts if per_track else L.kba_track_group_camera_step
+        if per_track:
+            oa = [opt_adjust] * n if opt_adjust is None or isinstance(opt_adjust, KbaOptions) else opt_adjust
+            os_ = [opt_solve] * n if opt_solve is None or isinstance(opt_solve, KbaOptions) else opt_solve
+            _, o_adjust = _options(list(oa), n, None, fn)
+            _, o_solve = _options(list(os_), n, None, fn)
+        else:
+            o_adjust, o_solve = C.byref(opt_adjust or default_options()), C.byref(opt_solve or default_options())
+        return _camera_step_call(self._p, fn, requests, self.tracks, o_adjust, o_solve, iterations_capacity)
 
     def push_keyframes(self, requests):
         """one keyframe into every track's store in one call (kba_track_group_push_keyframes): each entry None (the track sits the

@@ -359,6 +359,24 @@ class KbaFrameLidar(C.Structure):
     ]
 
 
+STEP_SOLVE = {"never": 0, "always": 1, "if_selected": 2}  # KBA_STEP_SOLVE_*
+
+
+class KbaCameraStepRequest(C.Structure):
+    _fields_ = [("step", KbaFrameStepRequest), ("solve", C.c_uint8), ("reserved_", C.c_uint8 * 3), ("n_cand", C.c_int32),
+                ("min_connecting", C.c_int32), ("min_window", C.c_int32), ("max_window", C.c_int32), ("n_trk", C.c_int32),
+                ("lm_slot", c_int32_p), ("lm_new", c_int32_p), ("lm_ground", c_uint8_p), ("trk", C.POINTER(KbaTracklet)),
+                ("classes", C.POINTER(KbaLabelClass)), ("n_class", C.c_int32), ("n_outlier", C.c_int32), ("outlier_slot", c_int32_p),
+                ("shrubbery_weight", C.c_double), ("params", C.c_void_p), ("max_near", C.c_int32), ("max_middle", C.c_int32),
+                ("max_far", C.c_int32), ("n_depth", C.c_int32), ("depth", C.POINTER(KbaDepthEntry)), ("draw", KbaDrawFn),
+                ("draw_ctx", C.c_void_p), ("sel", C.c_void_p)]
+
+
+class KbaCameraStepOut(C.Structure):
+    _fields_ = [("step", KbaFrameStepOut), ("solved", C.c_uint8), ("reserved_", C.c_uint8 * 3), ("n_lm", C.c_int32),
+                ("lm_index", c_int32_p), ("solve", KbaKfsolveOut)]
+
+
 def _ptr(a, ctype):
     if a is None:
         return C.cast(None, C.POINTER(ctype))

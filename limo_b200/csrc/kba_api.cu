@@ -4047,6 +4047,8 @@ struct KfsWin {
     size_t u_kf, u_lm, u_out, u_trk, u_gin, u_cls, u_depth;
     size_t d_cnt, d_common, d_post, d_kfa, d_lma, d_lmo, d_gr, d_tro;
     size_t x_fixed, x_cand, x_elig, x_shrub;
+    size_t u_tag = 0, d_nlm = 0, d_index = 0;  // the camera step's: candidate tags, the list's length, the candidates' positions
+    int kn = 0, ln = 0;                    // the keyframes and landmarks listed (the camera step's: after the push)
     int K = 0, N = 0, bound = 0, p_out = 0;
     std::vector<int> kf, fixed;
 };
@@ -4060,25 +4062,56 @@ static void kfs_abandon(cudaStream_t s, const std::vector<KfsWin>& ws) {
     cudaStreamSynchronize(s);
 }
 
-// one keyframe solve of the tracks of s (group = false: a single call), req[i] / out[i] / res[i] track i's
-static int set_keyframe_solve(TrackSet& s, bool group, const std::string& who, const kba_kfsolve_request* req, bool per_track,
-                              const kba_options* opts, kba_kfsolve_out* out, kba_result* res) {
-    const int n = (int)s.tracks.size();
-    auto sits_out = [&](int i) { return group && req[i].n_kf == 0; };
-    SolveTotals tot;
-    std::string owhy;
-    const int orc = solve_options_check(n, opts, per_track, "track ", [&](int i) { return !sits_out(i); }, tot, owhy);
-    if (orc != KBA_OK) return fail(orc, who + owhy);
-    // ---- every check that needs only the request; the scratch of each step at its first use
+// one keyframe solve of the tracks of s (group = false: a single call), req[i] / out[i] / res[i] track i's, in the phases the
+// camera step (set_camera_step) shares: the request checks (check), the staging's layout and lists (stage), the argument records
+// (records), the first part's launches (launch_first: deactivation, labels and lists, the ranking's first part), and after its
+// download the rest (rest: the checks on the kept keyframes, the draws, the ranking's second part, the weights, the solve and the
+// outputs).  In the camera step (cs), each request's landmark list is the candidate bound, compacted by k_cs_lists into the list
+// the deactivation and k_kfs_labels read, and its keyframe list may end with the frame's pending slot (kn: the keyframes listed).
+extern "C++" {  // member templates have C++ linkage
+struct KfsCall {
+    TrackSet& s;
+    bool group;
+    const std::string& who;
+    const kba_kfsolve_request* req;
+    bool per_track;
+    const kba_options* opts;
+    kba_kfsolve_out* out;
+    kba_result* res;
+    bool cs = false;
     std::vector<KfsWin> ws;
-    for (int i = 0; i < n; ++i) {
-        if (sits_out(i)) continue;
+    int W = 0, max_trk = 0;
+    Bump up, dn, dx;
+    size_t o_up_rec = 0, o_kfs = 0, o_sel = 0, o_rank = 0, o_cs = 0, o_mid = 0, rec_end = 0, up1 = 0, o_p2 = 0, down1 = 0, o_x = 0, o_res = 0;
+    UpkeepGrid ug;
+    SelectGrid sg;
+    RankGrid rg;
+    StoreStage* st = nullptr;
+    UpkeepLaunch ul;
+    Transfer sum;
+
+    KfsCall(TrackSet& s_, bool group_, const std::string& who_, const kba_kfsolve_request* req_, bool per_track_, const kba_options* opts_,
+            kba_kfsolve_out* out_, kba_result* res_)
+        : s(s_), group(group_), who(who_), req(req_), per_track(per_track_), opts(opts_), out(out_), res(res_) {}
+
+    // the options of the tracks live(i) names, before any request
+    template <class Live>
+    int check_options(Live live) {
+        SolveTotals tot;
+        std::string owhy;
+        const int orc = solve_options_check((int)s.tracks.size(), opts, per_track, "track ", live, tot, owhy);
+        return orc != KBA_OK ? fail(orc, who + owhy) : KBA_OK;
+    }
+
+    // every check of track i's request that needs only the request; the scratch of each step at its first use.  The last
+    // kf_pending keyframes of the list are not pushed yet (the camera step's kf_new, which its frame step checks).
+    int check(int i, int kf_pending) {
         kba_track* t = s.tracks[i];
         const kba_kfsolve_request& q = req[i];
         std::string why;
         int rc = kfsolve_check(t, q, out + i, why);
         if (rc == KBA_OK) {
-            const kba_deactivate_request dq{q.n_kf, q.n_lm, q.min_connecting, q.min_window, q.max_window, 0, q.kf_slot, q.lm_slot};
+            const kba_deactivate_request dq{q.n_kf - kf_pending, q.n_lm, q.min_connecting, q.min_window, q.max_window, 0, q.kf_slot, q.lm_slot};
             kba_deactivate_out dout{out[i].kf_active, out[i].kf_common, out[i].lm_active};
             UpkeepReq ur = upkeep_req(t, dq, &dout);
             rc = upkeep_check(ur, why);
@@ -4086,275 +4119,331 @@ static int set_keyframe_solve(TrackSet& s, bool group, const std::string& who, c
             if (rc == KBA_OK && !t->rank) rc = rank_alloc(t, why);
             if (rc == KBA_OK) rc = kfs_bufs(t, why);
             KfsWin w;
-            w.t = t; w.i = i; w.max_meas = ur.max_meas;
+            w.t = t; w.i = i; w.max_meas = ur.max_meas; w.kn = q.n_kf; w.ln = q.n_lm;
             ws.push_back(w);
         }
-        if (rc != KBA_OK) return fail(rc, who + track_prefix(group, i) + why);
+        return rc != KBA_OK ? fail(rc, who + track_prefix(group, i) + why) : KBA_OK;
     }
-    if (ws.empty()) {  // no upload, no launch
+
+    // the layout (records | AddDepth entries | int lists | byte lists, then the draws' block; out = the first download | device-only
+    // lists | the ranking's outputs), the staging grown to it, and every window's lists in the host staging
+    int stage() {
+        W = (int)ws.size();
+        o_up_rec = up.take(sizeof(UpkeepArgs) * (size_t)(W - 1)); o_kfs = up.take(sizeof(KfsArgs) * (size_t)W);
+        o_sel = up.take(sizeof(SelectArgs) * (size_t)W); o_rank = up.take(sizeof(RankArgs) * (size_t)W);
+        if (cs) o_cs = up.take(sizeof(CsArgs) * (size_t)W);
+        rec_end = up.at;
+        o_mid = dn.take(4 * (size_t)W);
+        size_t sum_lm = 0, max_draws = 0;
+        for (KfsWin& w : ws) {
+            const kba_kfsolve_request& q = req[w.i];
+            const size_t K = (size_t)q.n_kf, L = (size_t)q.n_lm, O = (size_t)q.n_outlier, T = (size_t)q.n_trk;
+            w.u_depth = up.take(8 * (size_t)q.n_depth);
+            w.u_kf = up.take(4 * K, 4); w.u_lm = up.take(4 * L, 4); w.u_out = up.take(4 * O, 4); w.u_trk = up.take(4 * T, 4);
+            if (cs) w.u_tag = up.take(4 * L, 4);
+            w.d_cnt = dn.take(8); w.d_common = dn.take(4 * K, 4); w.d_post = dn.take(4 * K, 4);
+            if (cs) { w.d_nlm = dn.take(4, 4); w.d_index = dn.take(4 * L, 4); }
+            w.x_cand = dx.take(4 * L);
+            sum_lm += L; max_draws += L > 0 ? L - 1 : 0;
+            ug.max_kf = std::max(ug.max_kf, q.n_kf); ug.max_lm = std::max(ug.max_lm, q.n_lm); ug.max_meas = std::max(ug.max_meas, w.max_meas);
+            sg.max_init = std::max(sg.max_init, std::max(std::max(q.n_kf, q.n_lm), w.t->n_cam));
+            rg.max_depth = std::max(rg.max_depth, q.n_depth);
+            max_trk = std::max(max_trk, q.n_trk);
+        }
+        for (KfsWin& w : ws) {  // the byte lists after every window's ints
+            const kba_kfsolve_request& q = req[w.i];
+            const size_t K = (size_t)q.n_kf, L = (size_t)q.n_lm, T = (size_t)q.n_trk;
+            w.u_gin = up.take(L, 1); w.u_cls = up.take(T, 1);
+            w.d_kfa = dn.take(K, 1); w.d_lma = dn.take(L, 1); w.d_lmo = dn.take(L, 1); w.d_gr = dn.take(L, 1); w.d_tro = dn.take(T, 1);
+            w.x_fixed = dx.take(K, 1); w.x_elig = dx.take(L, 1); w.x_shrub = dx.take(T, 1);
+        }
+        sg.max_kf = ug.max_kf; sg.max_cand = ug.max_lm; sg.max_meas = ug.max_meas;
+        rg.max_kf = sg.max_kf; rg.max_cand = sg.max_cand;
+        up1 = up.at; o_p2 = up.take(8 * (size_t)W + 4 * max_draws); down1 = dn.at;
+        o_x = (down1 + 7) & ~(size_t)7; o_res = o_x + ((dx.at + 7) & ~(size_t)7);
+        const size_t out_need = o_res + 8 * (size_t)W + 5 * sum_lm;
+        std::unique_ptr<StoreStage>& stage = s.stage[kKfSolveCall];
+        if (!stage || stage->up.n < up.at || stage->out.n < out_need) {  // grow-only: a call no larger than an earlier one allocates nothing
+            std::unique_ptr<StoreStage> fresh(new StoreStage());
+            if (fresh->alloc(std::max(up.at, stage ? stage->up.n : 0), std::max(out_need, stage ? stage->out.n : 0)))
+                return fail(KBA_ERR_CUDA, who + "out of memory for the keyframe solve staging");
+            stage = std::move(fresh);
+        }
+        st = stage.get();
+        unsigned char* uh = st->up.h;
+        for (KfsWin& w : ws) {
+            const kba_kfsolve_request& q = req[w.i];
+            memcpy(uh + w.u_kf, q.kf_slot, 4 * (size_t)q.n_kf);
+            if (q.n_lm) memcpy(uh + w.u_lm, q.lm_slot, 4 * (size_t)q.n_lm);
+            if (q.n_outlier) memcpy(uh + w.u_out, q.outlier_slot, 4 * (size_t)q.n_outlier);
+            if (q.lm_ground) memcpy(uh + w.u_gin, q.lm_ground, (size_t)q.n_lm); else memset(uh + w.u_gin, 0, (size_t)q.n_lm);
+            int* ts = reinterpret_cast<int*>(uh + w.u_trk);
+            for (int i = 0; i < q.n_trk; ++i) {
+                const int c = label_classes(q, q.trk[i].label);
+                ts[i] = q.trk[i].lm_slot;
+                uh[w.u_cls + i] = (unsigned char)(((q.trk[i].is_outlier || (c & KBA_LABEL_OUTLIER)) ? kKfsMarked : 0) |
+                                                  ((c & KBA_LABEL_SHRUBBERY) ? kKfsShrub : 0) | ((c & KBA_LABEL_GROUND) ? kKfsGround : 0));
+            }
+            int* de = reinterpret_cast<int*>(uh + w.u_depth);
+            for (int e = 0; e < q.n_depth; ++e) { de[2 * e] = q.depth[e].ind; de[2 * e + 1] = q.depth[e].wanted; }
+        }
+        return KBA_OK;
+    }
+
+    // every window's argument records, on the keyframes it lists now (kn); cs: the camera step's list records, created[v] the
+    // creation's flags of window v's frame (null: not selected)
+    int records(const std::vector<const unsigned char*>* created = nullptr) {
+        cudaStream_t st_s = s.h->stream;
+        unsigned char* uh = st->up.h, *od = st->out.d;
+        const unsigned char* ud = st->up.d;
+        ul.rest = reinterpret_cast<const UpkeepArgs*>(ud + o_up_rec);
+        ul.n_win = W;
+        KfsArgs* kfs_h = reinterpret_cast<KfsArgs*>(uh + o_kfs);
+        SelectArgs* sel_h = reinterpret_cast<SelectArgs*>(uh + o_sel);
+        RankArgs* rank_h = reinterpret_cast<RankArgs*>(uh + o_rank);
+        for (int v = 0; v < W; ++v) {
+            KfsWin& w = ws[v];
+            kba_track* t = w.t;
+            const kba_kfsolve_request& q = req[w.i];
+            const int* n_lm_d = nullptr;
+            if (cs) {
+                CsArgs c;
+                c.lm_slot = reinterpret_cast<int*>(st->up.d + w.u_lm); c.ground = st->up.d + w.u_gin;
+                c.tag = reinterpret_cast<const int*>(ud + w.u_tag); c.created = (*created)[v];
+                c.n_cand = q.n_lm; c.selected = c.created != nullptr;
+                c.index = reinterpret_cast<int*>(od + w.d_index); c.n_lm = reinterpret_cast<int*>(od + w.d_nlm);
+                reinterpret_cast<CsArgs*>(uh + o_cs)[v] = c;
+                n_lm_d = c.n_lm;
+            }
+            // the deactivation
+            UpkeepBufs& ub = *t->upkeep;
+            if (ub.stamp >= 0xfffffff0u) {  // the stamps wrap: the map starts over from all 0
+                CU(cudaMemsetAsync(ub.map, 0, sizeof(unsigned long long) * (size_t)t->td.lm_cap, st_s));
+                ub.stamp = 0;
+            }
+            UpkeepArgs a;
+            a.td = t->td;
+            a.kf_slot = reinterpret_cast<const int*>(ud + w.u_kf); a.lm_slot = reinterpret_cast<const int*>(ud + w.u_lm);
+            a.n_kf = w.kn; a.n_lm = q.n_lm; a.n_lm_d = n_lm_d;
+            a.stamp = ub.stamp + 1; ub.stamp += 2;
+            a.map = ub.map;
+            a.min_connecting = q.min_connecting; a.min_window = q.min_window; a.max_window = q.max_window;
+            a.kf_common = reinterpret_cast<int*>(od + w.d_common); a.kf_active = od + w.d_kfa; a.lm_active = od + w.d_lma;
+            if (v == 0) ul.w0 = a;
+            else memcpy(uh + o_up_rec + sizeof(UpkeepArgs) * (size_t)(v - 1), &a, sizeof(UpkeepArgs));
+            // the labels and the post-deactivation lists
+            KfsArgs k;
+            k.kf_slot = a.kf_slot; k.lm_slot = a.lm_slot; k.kf_active = a.kf_active; k.lm_active = a.lm_active;
+            k.ground_in = ud + w.u_gin; k.out_slot = reinterpret_cast<const int*>(ud + w.u_out);
+            k.trk_slot = reinterpret_cast<const int*>(ud + w.u_trk); k.trk_cls = ud + w.u_cls;
+            k.n_kf = w.kn; k.n_lm = q.n_lm; k.n_lm_d = n_lm_d; k.n_out = q.n_outlier; k.n_trk = q.n_trk;
+            k.lm_at = t->kfs->lm_at; k.last = t->kfs->last;
+            k.lm_out = od + w.d_lmo; k.ground = od + w.d_gr; k.trk_out = od + w.d_tro; k.shrub = od + o_x + w.x_shrub;
+            k.kf_post = reinterpret_cast<int*>(od + w.d_post); k.fixed = od + o_x + w.x_fixed;
+            k.cand = reinterpret_cast<int*>(od + o_x + w.x_cand); k.elig = od + o_x + w.x_elig;
+            k.counts = reinterpret_cast<int*>(od + w.d_cnt);
+            k.sel = reinterpret_cast<SelectArgs*>(st->up.d + o_sel) + v; k.rank = reinterpret_cast<RankArgs*>(st->up.d + o_rank) + v;
+            k.lm_weight = t->td.lm_weight; k.shrub_weight = q.shrubbery_weight;
+            kfs_h[v] = k;
+            // the ranking's chain on the device-built lists; k_kfs_labels writes its n_kf and n_cand
+            const size_t L = (size_t)t->td.lm_cap;
+            unsigned char* qd = t->rank->qty;
+            SelectArgs sa = t->select->a;
+            sa.td = t->td;
+            sa.kf_slot = k.kf_post; sa.lm_slot = k.cand; sa.n_kf = 0; sa.n_cand = 0;
+            for (int c = 0; c < 3; ++c) sa.leaf[c] = q.params->voxel_size[c];
+            sa.roi_far = q.params->roi_far; sa.roi_middle = q.params->roi_middle;
+            sa.flow = reinterpret_cast<double*>(qd); sa.seen = reinterpret_cast<int*>(qd + 8 * L); sa.near_order = reinterpret_cast<int*>(qd + 12 * L);
+            sa.counters = reinterpret_cast<int*>(qd + 16 * L); sa.n_near = sa.counters + 1;
+            sa.cheiral = qd + 16 * L + 16; sa.bin = reinterpret_cast<signed char*>(qd + 17 * L + 16);
+            sel_h[v] = sa;
+            RankArgs ra;
+            ra.td = t->td;
+            ra.kf_slot = sa.kf_slot; ra.lm_slot = sa.lm_slot; ra.elig = k.elig;
+            ra.depth = reinterpret_cast<const int*>(ud + w.u_depth);
+            ra.n_kf = 0; ra.n_cand = 0; ra.n_depth = q.n_depth;
+            ra.max_near = q.max_near; ra.max_middle = q.max_middle; ra.max_far = q.max_far;
+            ra.cheiral = sa.cheiral; ra.bin = sa.bin; ra.near_order = sa.near_order; ra.n_near = sa.n_near; ra.flow = sa.flow; ra.seen = sa.seen;
+            RankBufs& rb = *t->rank;
+            ra.cand_of = sa.cand_of; ra.mark = rb.mark; ra.dcand = rb.dcand; ra.dcost = rb.dcost; ra.dcnt = rb.dcnt;
+            ra.sel_slot = rb.sel_slot; ra.gp = rb.gp;
+            rank_h[v] = ra;
+            t->rank->valid = false;  // replaced by this call's, or none if it is refused
+        }
+        return KBA_OK;
+    }
+
+    // the first part's launch sequence (cs: k_cs_lists first), enqueued after the upload of the records and lists
+    cudaError_t launch_first() {
+        cudaStream_t st_s = s.h->stream;
+        const unsigned char* ud = st->up.d;
+        cudaError_t e = cudaMemsetAsync(st->out.d + o_mid, 0, 4 * (size_t)W, st_s);
+        if (e != cudaSuccess) return e;
+        if (cs) launch_cs_lists(reinterpret_cast<const CsArgs*>(ud + o_cs), W, st_s);
+        SelectLaunch sl;
+        sl.all = reinterpret_cast<const SelectArgs*>(ud + o_sel); sl.n_win = W;
+        RankLaunch rl;
+        rl.all = reinterpret_cast<const RankArgs*>(ud + o_rank); rl.n_win = W;
+        rl.n_mid = reinterpret_cast<int*>(st->out.d + o_mid);
+        launch_deactivate(ul, ug, st_s);
+        launch_kfs_labels(reinterpret_cast<const KfsArgs*>(ud + o_kfs), W, st_s);
+        launch_select(sl, sg, st_s);
+        launch_rank_prepare(rl, rg, st_s);
+        return cudaGetLastError();
+    }
+
+    // after the first download: the checks on the kept keyframes, the draws, the ranking's second part, the ranked solve's checks,
+    // the shrubbery weights, the solve and the outputs.  Every refusal comes before the store is written.
+    int rest() {
+        kba_handle* h = s.h;
+        cudaStream_t st_s = h->stream;
+        const int n = (int)s.tracks.size();
+        unsigned char* uh = st->up.h, *od = st->out.d;
+        const unsigned char* ud = st->up.d;
+        const unsigned char* oh = st->out.h;
+        const int* n_mid = reinterpret_cast<const int*>(oh + o_mid);
+        int* p2 = reinterpret_cast<int*>(uh + o_p2);
+        int* draws = p2 + 2 * W;
+        size_t n_draws = 0, n_out = 0;
+        std::vector<TrackRequest> qs(n);
+        for (int v = 0; v < W; ++v) {
+            KfsWin& w = ws[v];
+            const kba_kfsolve_request& q = req[w.i];
+            const int* cnt = reinterpret_cast<const int*>(oh + w.d_cnt);
+            w.K = cnt[0]; w.N = cnt[1];
+            if (cs) w.ln = *reinterpret_cast<const int*>(oh + w.d_nlm);
+            std::string why;
+            int rc = KBA_OK;
+            if (w.K == 0) { why = "no keyframes or a negative size"; rc = KBA_ERR_BAD_ARG; }
+            if (rc == KBA_OK) {
+                const int* post = reinterpret_cast<const int*>(oh + w.d_post);
+                w.kf.assign(post, post + w.K);
+                w.fixed.assign(w.K, 0);
+                w.fixed[0] = 1;
+                for (int e = 0; e < q.n_depth && rc == KBA_OK; ++e)  // the AddDepth heap of an entry lives in shared memory
+                    if (q.depth[e].ind < w.K && std::min(q.depth[e].wanted, w.t->m_cnt[w.kf[q.depth[e].ind]]) > kRankMaxCand) {
+                        why = "an AddDepth entry keeps more than 57344 landmarks"; rc = KBA_ERR_CAPACITY;
+                    }
+            }
+            if (rc == KBA_OK) {
+                // the solve's keyframe checks; the ranking's ground candidates are not known yet: on a window without any
+                kba_window sel0 = *q.sel;
+                sel0.n_gp = 0;
+                std::vector<uint8_t> f8(w.fixed.begin(), w.fixed.end());
+                TrackRequest q0 = track_request(w.K, w.kf.data(), f8.data(), 0, nullptr, &sel0, true);
+                rc = track_check(w.t, q0, why);
+            }
+            if (rc == KBA_OK) {
+                const int nm = n_mid[v], D = std::max(nm - 1, 0), N = w.N;
+                long long b = std::min(q.max_near, N) + (long long)std::min(q.max_middle, nm) + std::min(q.max_far, N);
+                int heap = std::max(std::min(q.max_near, N), std::min(q.max_far, N));
+                for (int e = 0; e < q.n_depth; ++e) {
+                    b += std::min(q.depth[e].wanted, N);
+                    if (q.depth[e].ind < w.K) heap = std::max(heap, std::min(q.depth[e].wanted, w.t->m_cnt[w.kf[q.depth[e].ind]]));
+                }
+                w.bound = (int)std::min<long long>(b, N);
+                rg.heap_ints = std::max(rg.heap_ints, heap);
+                rg.mid_ints = std::max(rg.mid_ints, nm);
+                p2[2 * v] = (int)n_draws; p2[2 * v + 1] = (int)n_out;
+                w.p_out = (int)n_out;
+                n_out += (size_t)w.bound;
+                if (D > 0) {
+                    if (!q.draw) { why = "the middle bin needs " + std::to_string(D) + " draws and there is no draw function"; rc = KBA_ERR_BAD_ARG; }
+                    else if (q.draw(q.draw_ctx, D, draws + n_draws) != 0) { why = "the draw function failed"; rc = KBA_ERR_BAD_ARG; }
+                    n_draws += (size_t)D;
+                }
+            }
+            if (rc != KBA_OK) {
+                kfs_abandon(st_s, ws);
+                return fail(rc, who + track_prefix(group, w.i) + why);
+            }
+        }
+        // ---- the ranking's second part
+        RankLaunch rl;
+        rl.all = reinterpret_cast<const RankArgs*>(ud + o_rank); rl.n_win = W;
+        rl.n_mid = reinterpret_cast<int*>(od + o_mid);
+        const size_t p2_bytes = 8 * (size_t)W + 4 * n_draws;
+        CU(cudaMemcpyAsync(st->up.d + o_p2, uh + o_p2, p2_bytes, cudaMemcpyHostToDevice, st_s));
+        rl.p2 = reinterpret_cast<const int*>(ud + o_p2);
+        rl.res = reinterpret_cast<int*>(od + o_res);
+        rl.out_cand = reinterpret_cast<int*>(od + o_res + 8 * (size_t)W);
+        rl.out_cat = reinterpret_cast<signed char*>(od + o_res + 8 * (size_t)W + 4 * n_out);
+        launch_rank(rl, rg, st_s);
+        CU(cudaGetLastError());
+        const size_t down2 = 8 * (size_t)W + 5 * n_out;
+        CU(cudaMemcpyAsync(st->out.h + o_res, st->out.d + o_res, down2, cudaMemcpyDeviceToHost, st_s));
+        CU(wait_stream(h));
+        sum.h2d += (int64_t)p2_bytes; sum.d2h += (int64_t)down2;
+        const int* rres = reinterpret_cast<const int*>(oh + o_res);
+        for (int v = 0; v < W; ++v) {
+            KfsWin& w = ws[v];
+            RankBufs& rb = *w.t->rank;
+            rb.kf = w.kf; rb.n_sel = rres[2 * v]; rb.n_ground = rres[2 * v + 1]; rb.gen = w.t->gen; rb.valid = true;
+        }
+        // ---- the ranked solve's checks, the shrubbery weights, the solve
+        std::vector<std::vector<uint8_t>> fixed8(n);
+        for (const KfsWin& w : ws) {
+            fixed8[w.i].assign(w.fixed.begin(), w.fixed.end());
+            qs[w.i] = track_request(w.K, w.kf.data(), fixed8[w.i].data(), 0, nullptr, req[w.i].sel, true);
+            TrackRequest q = qs[w.i];
+            std::string why;
+            const int rc = ranked_check(w.t, q, why);
+            if (rc != KBA_OK) return fail(rc, who + track_prefix(group, w.i) + why);
+        }
+        launch_kfs_weights(reinterpret_cast<const KfsArgs*>(ud + o_kfs), W, max_trk, st_s);
+        CU(cudaGetLastError());
+        for (const KfsWin& w : ws) { w.t->gen++; w.t->rank->gen = w.t->gen; }  // the weights do not enter the ranking
+        int rc = set_solve(s, group, who, qs.data(), per_track, opts, res);
+        if (rc != KBA_OK) return rc;
+        sum.h2d += s.last->h2d; sum.d2h += s.last->d2h;
+        // ---- the outputs
+        const unsigned char* hc = oh + o_res + 8 * (size_t)W;
+        for (int v = 0; v < W; ++v) {
+            const KfsWin& w = ws[v];
+            const kba_kfsolve_request& q = req[w.i];
+            kba_kfsolve_out& o = out[w.i];
+            memcpy(o.kf_active, oh + w.d_kfa, (size_t)w.kn); memcpy(o.kf_common, oh + w.d_common, 4 * (size_t)w.kn);
+            if (w.ln) {
+                memcpy(o.lm_active, oh + w.d_lma, (size_t)w.ln); memcpy(o.lm_outlier, oh + w.d_lmo, (size_t)w.ln);
+                memcpy(o.lm_ground, oh + w.d_gr, (size_t)w.ln);
+            }
+            if (q.n_trk) memcpy(o.trk_outlier, oh + w.d_tro, (size_t)q.n_trk);
+            const int n_sel = rres[2 * v];
+            o.rank.n_sel = n_sel; o.rank.n_ground = rres[2 * v + 1]; o.rank.n_draws = std::max(n_mid[v] - 1, 0);
+            if (n_sel) { memcpy(o.rank.cand, hc + 4 * (size_t)w.p_out, 4 * (size_t)n_sel); memcpy(o.rank.category, hc + 4 * n_out + w.p_out, (size_t)n_sel); }
+        }
+        st->counts = sum;
+        s.last = &st->counts;
+        return KBA_OK;
+    }
+};
+}
+
+static int set_keyframe_solve(TrackSet& s, bool group, const std::string& who, const kba_kfsolve_request* req, bool per_track,
+                              const kba_options* opts, kba_kfsolve_out* out, kba_result* res) {
+    const int n = (int)s.tracks.size();
+    auto sits_out = [&](int i) { return group && req[i].n_kf == 0; };
+    KfsCall c(s, group, who, req, per_track, opts, out, res);
+    int rc = c.check_options([&](int i) { return !sits_out(i); });
+    for (int i = 0; i < n && rc == KBA_OK; ++i)
+        if (!sits_out(i)) rc = c.check(i, 0);
+    if (rc != KBA_OK) return rc;
+    if (c.ws.empty()) {  // no upload, no launch
         for (int i = 0; i < n; ++i) idle_result(res[i]);
         s.last = &kNoTransfer;
         return KBA_OK;
     }
     kba_handle* h = s.h;
     CU(cudaSetDevice(h->device));
-    cudaStream_t st_s = h->stream;
-    const int W = (int)ws.size();
-    // ---- layout: up = records | AddDepth entries | int lists | byte lists, then the draws' block; out = the first download |
-    // device-only lists | the ranking's outputs
-    Bump up, dn, dx;
-    const size_t o_up_rec = up.take(sizeof(UpkeepArgs) * (size_t)(W - 1)), o_kfs = up.take(sizeof(KfsArgs) * (size_t)W);
-    const size_t o_sel = up.take(sizeof(SelectArgs) * (size_t)W), o_rank = up.take(sizeof(RankArgs) * (size_t)W);
-    const size_t o_mid = dn.take(4 * (size_t)W);
-    size_t sum_lm = 0, sum_trk = 0, max_draws = 0;
-    UpkeepGrid ug;
-    SelectGrid sg;
-    RankGrid rg;
-    int max_trk = 0;
-    for (KfsWin& w : ws) {
-        const kba_kfsolve_request& q = req[w.i];
-        const size_t K = (size_t)q.n_kf, L = (size_t)q.n_lm, O = (size_t)q.n_outlier, T = (size_t)q.n_trk;
-        w.u_depth = up.take(8 * (size_t)q.n_depth);
-        w.u_kf = up.take(4 * K, 4); w.u_lm = up.take(4 * L, 4); w.u_out = up.take(4 * O, 4); w.u_trk = up.take(4 * T, 4);
-        w.d_cnt = dn.take(8); w.d_common = dn.take(4 * K, 4); w.d_post = dn.take(4 * K, 4);
-        w.x_cand = dx.take(4 * L);
-        sum_lm += L; sum_trk += T; max_draws += L > 0 ? L - 1 : 0;
-        ug.max_kf = std::max(ug.max_kf, q.n_kf); ug.max_lm = std::max(ug.max_lm, q.n_lm); ug.max_meas = std::max(ug.max_meas, w.max_meas);
-        sg.max_init = std::max(sg.max_init, std::max(std::max(q.n_kf, q.n_lm), w.t->n_cam));
-        rg.max_depth = std::max(rg.max_depth, q.n_depth);
-        max_trk = std::max(max_trk, q.n_trk);
-    }
-    for (KfsWin& w : ws) {  // the byte lists after every window's ints
-        const kba_kfsolve_request& q = req[w.i];
-        const size_t K = (size_t)q.n_kf, L = (size_t)q.n_lm, T = (size_t)q.n_trk;
-        w.u_gin = up.take(L, 1); w.u_cls = up.take(T, 1);
-        w.d_kfa = dn.take(K, 1); w.d_lma = dn.take(L, 1); w.d_lmo = dn.take(L, 1); w.d_gr = dn.take(L, 1); w.d_tro = dn.take(T, 1);
-        w.x_fixed = dx.take(K, 1); w.x_elig = dx.take(L, 1); w.x_shrub = dx.take(T, 1);
-    }
-    sg.max_kf = ug.max_kf; sg.max_cand = ug.max_lm; sg.max_meas = ug.max_meas;
-    rg.max_kf = sg.max_kf; rg.max_cand = sg.max_cand;
-    const size_t up1 = up.at, o_p2 = up.take(8 * (size_t)W + 4 * max_draws), down1 = dn.at;
-    const size_t o_x = (down1 + 7) & ~(size_t)7, o_res = o_x + ((dx.at + 7) & ~(size_t)7);
-    const size_t out_need = o_res + 8 * (size_t)W + 5 * sum_lm;
-    std::unique_ptr<StoreStage>& stage = s.stage[kKfSolveCall];
-    if (!stage || stage->up.n < up.at || stage->out.n < out_need) {  // grow-only: a call no larger than an earlier one allocates nothing
-        std::unique_ptr<StoreStage> fresh(new StoreStage());
-        if (fresh->alloc(std::max(up.at, stage ? stage->up.n : 0), std::max(out_need, stage ? stage->out.n : 0)))
-            return fail(KBA_ERR_CUDA, who + "out of memory for the keyframe solve staging");
-        stage = std::move(fresh);
-    }
-    StoreStage& st = *stage;
-    unsigned char* uh = st.up.h, *od = st.out.d;
-    const unsigned char* ud = st.up.d;
-    // ---- records and lists
-    UpkeepLaunch ul;
-    ul.rest = reinterpret_cast<const UpkeepArgs*>(ud + o_up_rec);
-    ul.n_win = W;
-    KfsArgs* kfs_h = reinterpret_cast<KfsArgs*>(uh + o_kfs);
-    SelectArgs* sel_h = reinterpret_cast<SelectArgs*>(uh + o_sel);
-    RankArgs* rank_h = reinterpret_cast<RankArgs*>(uh + o_rank);
-    for (int v = 0; v < W; ++v) {
-        KfsWin& w = ws[v];
-        kba_track* t = w.t;
-        const kba_kfsolve_request& q = req[w.i];
-        memcpy(uh + w.u_kf, q.kf_slot, 4 * (size_t)q.n_kf);
-        if (q.n_lm) memcpy(uh + w.u_lm, q.lm_slot, 4 * (size_t)q.n_lm);
-        if (q.n_outlier) memcpy(uh + w.u_out, q.outlier_slot, 4 * (size_t)q.n_outlier);
-        if (q.lm_ground) memcpy(uh + w.u_gin, q.lm_ground, (size_t)q.n_lm); else memset(uh + w.u_gin, 0, (size_t)q.n_lm);
-        int* ts = reinterpret_cast<int*>(uh + w.u_trk);
-        for (int i = 0; i < q.n_trk; ++i) {
-            const int c = label_classes(q, q.trk[i].label);
-            ts[i] = q.trk[i].lm_slot;
-            uh[w.u_cls + i] = (unsigned char)(((q.trk[i].is_outlier || (c & KBA_LABEL_OUTLIER)) ? kKfsMarked : 0) |
-                                              ((c & KBA_LABEL_SHRUBBERY) ? kKfsShrub : 0) | ((c & KBA_LABEL_GROUND) ? kKfsGround : 0));
-        }
-        int* de = reinterpret_cast<int*>(uh + w.u_depth);
-        for (int e = 0; e < q.n_depth; ++e) { de[2 * e] = q.depth[e].ind; de[2 * e + 1] = q.depth[e].wanted; }
-        // the deactivation
-        UpkeepBufs& ub = *t->upkeep;
-        if (ub.stamp >= 0xfffffff0u) {  // the stamps wrap: the map starts over from all 0
-            CU(cudaMemsetAsync(ub.map, 0, sizeof(unsigned long long) * (size_t)t->td.lm_cap, st_s));
-            ub.stamp = 0;
-        }
-        UpkeepArgs a;
-        a.td = t->td;
-        a.kf_slot = reinterpret_cast<const int*>(ud + w.u_kf); a.lm_slot = reinterpret_cast<const int*>(ud + w.u_lm);
-        a.n_kf = q.n_kf; a.n_lm = q.n_lm;
-        a.stamp = ub.stamp + 1; ub.stamp += 2;
-        a.map = ub.map;
-        a.min_connecting = q.min_connecting; a.min_window = q.min_window; a.max_window = q.max_window;
-        a.kf_common = reinterpret_cast<int*>(od + w.d_common); a.kf_active = od + w.d_kfa; a.lm_active = od + w.d_lma;
-        if (v == 0) ul.w0 = a;
-        else memcpy(uh + o_up_rec + sizeof(UpkeepArgs) * (size_t)(v - 1), &a, sizeof(UpkeepArgs));
-        // the labels and the post-deactivation lists
-        KfsArgs k;
-        k.kf_slot = a.kf_slot; k.lm_slot = a.lm_slot; k.kf_active = a.kf_active; k.lm_active = a.lm_active;
-        k.ground_in = ud + w.u_gin; k.out_slot = reinterpret_cast<const int*>(ud + w.u_out);
-        k.trk_slot = reinterpret_cast<const int*>(ud + w.u_trk); k.trk_cls = ud + w.u_cls;
-        k.n_kf = q.n_kf; k.n_lm = q.n_lm; k.n_out = q.n_outlier; k.n_trk = q.n_trk;
-        k.lm_at = t->kfs->lm_at; k.last = t->kfs->last;
-        k.lm_out = od + w.d_lmo; k.ground = od + w.d_gr; k.trk_out = od + w.d_tro; k.shrub = od + o_x + w.x_shrub;
-        k.kf_post = reinterpret_cast<int*>(od + w.d_post); k.fixed = od + o_x + w.x_fixed;
-        k.cand = reinterpret_cast<int*>(od + o_x + w.x_cand); k.elig = od + o_x + w.x_elig;
-        k.counts = reinterpret_cast<int*>(od + w.d_cnt);
-        k.sel = reinterpret_cast<SelectArgs*>(st.up.d + o_sel) + v; k.rank = reinterpret_cast<RankArgs*>(st.up.d + o_rank) + v;
-        k.lm_weight = t->td.lm_weight; k.shrub_weight = q.shrubbery_weight;
-        kfs_h[v] = k;
-        // the ranking's chain on the device-built lists; k_kfs_labels writes its n_kf and n_cand
-        const size_t L = (size_t)t->td.lm_cap;
-        unsigned char* qd = t->rank->qty;
-        SelectArgs sa = t->select->a;
-        sa.td = t->td;
-        sa.kf_slot = k.kf_post; sa.lm_slot = k.cand; sa.n_kf = 0; sa.n_cand = 0;
-        for (int c = 0; c < 3; ++c) sa.leaf[c] = q.params->voxel_size[c];
-        sa.roi_far = q.params->roi_far; sa.roi_middle = q.params->roi_middle;
-        sa.flow = reinterpret_cast<double*>(qd); sa.seen = reinterpret_cast<int*>(qd + 8 * L); sa.near_order = reinterpret_cast<int*>(qd + 12 * L);
-        sa.counters = reinterpret_cast<int*>(qd + 16 * L); sa.n_near = sa.counters + 1;
-        sa.cheiral = qd + 16 * L + 16; sa.bin = reinterpret_cast<signed char*>(qd + 17 * L + 16);
-        sel_h[v] = sa;
-        RankArgs ra;
-        ra.td = t->td;
-        ra.kf_slot = sa.kf_slot; ra.lm_slot = sa.lm_slot; ra.elig = k.elig;
-        ra.depth = reinterpret_cast<const int*>(ud + w.u_depth);
-        ra.n_kf = 0; ra.n_cand = 0; ra.n_depth = q.n_depth;
-        ra.max_near = q.max_near; ra.max_middle = q.max_middle; ra.max_far = q.max_far;
-        ra.cheiral = sa.cheiral; ra.bin = sa.bin; ra.near_order = sa.near_order; ra.n_near = sa.n_near; ra.flow = sa.flow; ra.seen = sa.seen;
-        RankBufs& rb = *t->rank;
-        ra.cand_of = sa.cand_of; ra.mark = rb.mark; ra.dcand = rb.dcand; ra.dcost = rb.dcost; ra.dcnt = rb.dcnt;
-        ra.sel_slot = rb.sel_slot; ra.gp = rb.gp;
-        rank_h[v] = ra;
-        t->rank->valid = false;  // replaced by this call's, or none if it is refused
-    }
+    if ((rc = c.stage()) != KBA_OK || (rc = c.records()) != KBA_OK) return rc;
     // ---- one upload, one launch sequence (deactivation, labels and lists, the ranking's first part), one download
-    const KfsArgs* kfs_d = reinterpret_cast<const KfsArgs*>(ud + o_kfs);
-    SelectLaunch sl;
-    sl.all = reinterpret_cast<const SelectArgs*>(ud + o_sel); sl.n_win = W;
-    RankLaunch rl;
-    rl.all = reinterpret_cast<const RankArgs*>(ud + o_rank); rl.n_win = W;
-    rl.n_mid = reinterpret_cast<int*>(od + o_mid);
-    CU(cudaMemcpyAsync(st.up.d, st.up.h, up1, cudaMemcpyHostToDevice, st_s));
-    CU(cudaMemsetAsync(rl.n_mid, 0, 4 * (size_t)W, st_s));
-    launch_deactivate(ul, ug, st_s);
-    launch_kfs_labels(kfs_d, W, st_s);
-    launch_select(sl, sg, st_s);
-    launch_rank_prepare(rl, rg, st_s);
-    CU(cudaGetLastError());
-    CU(cudaMemcpyAsync(st.out.h, st.out.d, down1, cudaMemcpyDeviceToHost, st_s));
+    StoreStage& st = *c.st;
+    CU(cudaMemcpyAsync(st.up.d, st.up.h, c.up1, cudaMemcpyHostToDevice, h->stream));
+    CU(c.launch_first());
+    CU(cudaMemcpyAsync(st.out.h, st.out.d, c.down1, cudaMemcpyDeviceToHost, h->stream));
     CU(wait_stream(h));
-    Transfer sum;
-    sum.h2d = (int64_t)up1; sum.d2h = (int64_t)down1;
-    const unsigned char* oh = st.out.h;
-    // ---- the checks of the ranking and of the solve on the post-deactivation lists, then the draws
-    const int* n_mid = reinterpret_cast<const int*>(oh + o_mid);
-    int* p2 = reinterpret_cast<int*>(uh + o_p2);
-    int* draws = p2 + 2 * W;
-    size_t n_draws = 0, n_out = 0;
-    std::vector<TrackRequest> qs(n);
-    for (int v = 0; v < W; ++v) {
-        KfsWin& w = ws[v];
-        const kba_kfsolve_request& q = req[w.i];
-        const int* cnt = reinterpret_cast<const int*>(oh + w.d_cnt);
-        w.K = cnt[0]; w.N = cnt[1];
-        std::string why;
-        int rc = KBA_OK;
-        if (w.K == 0) { why = "no keyframes or a negative size"; rc = KBA_ERR_BAD_ARG; }
-        if (rc == KBA_OK) {
-            const int* post = reinterpret_cast<const int*>(oh + w.d_post);
-            w.kf.assign(post, post + w.K);
-            w.fixed.assign(w.K, 0);
-            w.fixed[0] = 1;
-            for (int e = 0; e < q.n_depth && rc == KBA_OK; ++e)  // the AddDepth heap of an entry lives in shared memory
-                if (q.depth[e].ind < w.K && std::min(q.depth[e].wanted, w.t->m_cnt[w.kf[q.depth[e].ind]]) > kRankMaxCand) {
-                    why = "an AddDepth entry keeps more than 57344 landmarks"; rc = KBA_ERR_CAPACITY;
-                }
-        }
-        if (rc == KBA_OK) {
-            // the solve's keyframe checks; the ranking's ground candidates are not known yet: on a window without any
-            kba_window sel0 = *q.sel;
-            sel0.n_gp = 0;
-            std::vector<uint8_t> f8(w.fixed.begin(), w.fixed.end());
-            TrackRequest q0 = track_request(w.K, w.kf.data(), f8.data(), 0, nullptr, &sel0, true);
-            rc = track_check(w.t, q0, why);
-        }
-        if (rc == KBA_OK) {
-            const int nm = n_mid[v], D = std::max(nm - 1, 0), N = w.N;
-            long long b = std::min(q.max_near, N) + (long long)std::min(q.max_middle, nm) + std::min(q.max_far, N);
-            int heap = std::max(std::min(q.max_near, N), std::min(q.max_far, N));
-            for (int e = 0; e < q.n_depth; ++e) {
-                b += std::min(q.depth[e].wanted, N);
-                if (q.depth[e].ind < w.K) heap = std::max(heap, std::min(q.depth[e].wanted, w.t->m_cnt[w.kf[q.depth[e].ind]]));
-            }
-            w.bound = (int)std::min<long long>(b, N);
-            rg.heap_ints = std::max(rg.heap_ints, heap);
-            rg.mid_ints = std::max(rg.mid_ints, nm);
-            p2[2 * v] = (int)n_draws; p2[2 * v + 1] = (int)n_out;
-            w.p_out = (int)n_out;
-            n_out += (size_t)w.bound;
-            if (D > 0) {
-                if (!q.draw) { why = "the middle bin needs " + std::to_string(D) + " draws and there is no draw function"; rc = KBA_ERR_BAD_ARG; }
-                else if (q.draw(q.draw_ctx, D, draws + n_draws) != 0) { why = "the draw function failed"; rc = KBA_ERR_BAD_ARG; }
-                n_draws += (size_t)D;
-            }
-        }
-        if (rc != KBA_OK) {
-            kfs_abandon(st_s, ws);
-            return fail(rc, who + track_prefix(group, w.i) + why);
-        }
-    }
-    // ---- the ranking's second part
-    const size_t p2_bytes = 8 * (size_t)W + 4 * n_draws;
-    CU(cudaMemcpyAsync(st.up.d + o_p2, uh + o_p2, p2_bytes, cudaMemcpyHostToDevice, st_s));
-    rl.p2 = reinterpret_cast<const int*>(ud + o_p2);
-    rl.res = reinterpret_cast<int*>(od + o_res);
-    rl.out_cand = reinterpret_cast<int*>(od + o_res + 8 * (size_t)W);
-    rl.out_cat = reinterpret_cast<signed char*>(od + o_res + 8 * (size_t)W + 4 * n_out);
-    launch_rank(rl, rg, st_s);
-    CU(cudaGetLastError());
-    const size_t down2 = 8 * (size_t)W + 5 * n_out;
-    CU(cudaMemcpyAsync(st.out.h + o_res, st.out.d + o_res, down2, cudaMemcpyDeviceToHost, st_s));
-    CU(wait_stream(h));
-    sum.h2d += (int64_t)p2_bytes; sum.d2h += (int64_t)down2;
-    const int* rres = reinterpret_cast<const int*>(oh + o_res);
-    for (int v = 0; v < W; ++v) {
-        KfsWin& w = ws[v];
-        RankBufs& rb = *w.t->rank;
-        rb.kf = w.kf; rb.n_sel = rres[2 * v]; rb.n_ground = rres[2 * v + 1]; rb.gen = w.t->gen; rb.valid = true;
-    }
-    // ---- the ranked solve's checks, the shrubbery weights, the solve
-    std::vector<std::vector<uint8_t>> fixed8(n);
-    for (const KfsWin& w : ws) {
-        fixed8[w.i].assign(w.fixed.begin(), w.fixed.end());
-        qs[w.i] = track_request(w.K, w.kf.data(), fixed8[w.i].data(), 0, nullptr, req[w.i].sel, true);
-        TrackRequest q = qs[w.i];
-        std::string why;
-        const int rc = ranked_check(w.t, q, why);
-        if (rc != KBA_OK) return fail(rc, who + track_prefix(group, w.i) + why);
-    }
-    launch_kfs_weights(kfs_d, W, max_trk, st_s);
-    CU(cudaGetLastError());
-    for (const KfsWin& w : ws) { w.t->gen++; w.t->rank->gen = w.t->gen; }  // the weights do not enter the ranking
-    int rc = set_solve(s, group, who, qs.data(), per_track, opts, res);
-    if (rc != KBA_OK) return rc;
-    sum.h2d += s.last->h2d; sum.d2h += s.last->d2h;
-    // ---- the outputs
-    const unsigned char* hc = oh + o_res + 8 * (size_t)W;
-    for (int v = 0; v < W; ++v) {
-        const KfsWin& w = ws[v];
-        const kba_kfsolve_request& q = req[w.i];
-        kba_kfsolve_out& o = out[w.i];
-        memcpy(o.kf_active, oh + w.d_kfa, (size_t)q.n_kf); memcpy(o.kf_common, oh + w.d_common, 4 * (size_t)q.n_kf);
-        if (q.n_lm) {
-            memcpy(o.lm_active, oh + w.d_lma, (size_t)q.n_lm); memcpy(o.lm_outlier, oh + w.d_lmo, (size_t)q.n_lm);
-            memcpy(o.lm_ground, oh + w.d_gr, (size_t)q.n_lm);
-        }
-        if (q.n_trk) memcpy(o.trk_outlier, oh + w.d_tro, (size_t)q.n_trk);
-        const int n_sel = rres[2 * v];
-        o.rank.n_sel = n_sel; o.rank.n_ground = rres[2 * v + 1]; o.rank.n_draws = std::max(n_mid[v] - 1, 0);
-        if (n_sel) { memcpy(o.rank.cand, hc + 4 * (size_t)w.p_out, 4 * (size_t)n_sel); memcpy(o.rank.category, hc + 4 * n_out + w.p_out, (size_t)n_sel); }
-    }
-    st.counts = sum;
-    s.last = &st.counts;
-    return KBA_OK;
+    c.sum.h2d = (int64_t)c.up1; c.sum.d2h = (int64_t)c.down1;
+    return c.rest();
 }
 
 int kba_track_keyframe_solve(kba_track* t, const kba_kfsolve_request* req, const kba_options* opt, kba_kfsolve_out* out, kba_result* res) {
@@ -4481,10 +4570,22 @@ static int step_check(kba_track* t, const kba_frame_step_request& q, const kba_f
     return KBA_OK;
 }
 
+// what a call adds to the frame step's phases (the camera step's solve block, set_camera_step): its checks and staging after the
+// frame step's checks, its upload with the frame step's first upload, whether it runs after the verdicts, and its launch sequence
+// right after the push's and the creation's kernels, ahead of the second download.  Its transfers are its own to count.
+struct StepHook {
+    virtual int checked() = 0;
+    virtual cudaError_t upload(cudaStream_t s) = 0;
+    virtual bool due(const std::vector<StepWin>& ws) = 0;
+    // created[v]: the creation's flags in device memory of ws[v]'s frame, null when it is not selected
+    virtual cudaError_t launch(const std::vector<const unsigned char*>& created, cudaStream_t s) = 0;
+};
+
 // one frame step of the tracks of s (group = false: a single call), req[i] / out[i] / res[i] / lid[i] track i's; lid null: the
 // requests' d columns are the depths, else the lidar kernels extract them from lid[i]'s cloud into the staged d column
 static int set_frame_step(TrackSet& s, bool group, const std::string& who, const kba_frame_step_request* req, bool per_track,
-                          const kba_options* opts, kba_frame_step_out* out, kba_result* res, const kba_frame_lidar* lid) {
+                          const kba_options* opts, kba_frame_step_out* out, kba_result* res, const kba_frame_lidar* lid,
+                          StepHook* hook = nullptr) {
     const int n = (int)s.tracks.size();
     std::vector<StepWin> ws;
     for (int i = 0; i < n; ++i) {
@@ -4495,6 +4596,10 @@ static int set_frame_step(TrackSet& s, bool group, const std::string& who, const
         const int rc = step_check(w.t, req[i], out + i, &opts[per_track ? i : 0], lid ? lid + i : nullptr, w, why);
         if (rc != KBA_OK) return fail(rc, who + track_prefix(group, i) + why);
         ws.push_back(std::move(w));
+    }
+    if (hook) {
+        const int rc = hook->checked();
+        if (rc != KBA_OK) return rc;
     }
     // the lidar views (cloud v is ws[v]'s), those of the frames whose depths are downloaded first: their features lead the
     // feature order, so the download is the first n_copy depths in that order
@@ -4690,7 +4795,8 @@ static int set_frame_step(TrackSet& s, bool group, const std::string& who, const
         for (const StepWin& w : ws) cudaMemsetAsync(w.t->upkeep->map, 0, sizeof(unsigned long long) * (size_t)w.t->td.lm_cap, cs);
         cudaStreamSynchronize(cs);
     };
-    cudaError_t e = plan.par.empty() ? cudaSuccess : lidar_copy_clouds(plan, clouds.data(), lws, cs);
+    cudaError_t e = hook ? hook->upload(cs) : cudaSuccess;
+    if (e == cudaSuccess && !plan.par.empty()) e = lidar_copy_clouds(plan, clouds.data(), lws, cs);
     if (e == cudaSuccess) e = cudaMemcpyAsync(st.up.d, uh, up1, cudaMemcpyHostToDevice, cs);
     if (e == cudaSuccess && !plan.par.empty()) e = launch_lidar_staged(plan, lws, ud + o_lpack, lf, cs);  // the d column
     if (e == cudaSuccess) {
@@ -4733,8 +4839,9 @@ static int set_frame_step(TrackSet& s, bool group, const std::string& who, const
         if (w.selected) sel.push_back(v);
     }
     int64_t up_bytes = (int64_t)up1 + cloud_bytes, down_bytes = (int64_t)down1;
+    const bool hooked = hook && hook->due(ws);
     // ---- the push and the creation of the selected windows: one upload of records, one launch sequence, one download
-    if (!sel.empty()) {
+    if (!sel.empty() || hooked) {
         const int S = (int)sel.size();
         std::vector<CompactTrack> ct;
         std::vector<CompactRun> runs;
@@ -4775,17 +4882,24 @@ static int set_frame_step(TrackSet& s, bool group, const std::string& who, const
         if (!ct.empty()) memcpy(uh + o_ct, ct.data(), sizeof(CompactTrack) * ct.size());
         if (!runs.empty()) memcpy(uh + o_run, runs.data(), sizeof(CompactRun) * runs.size());
         CreateLaunch cl;
-        cl.w0 = cr[0];
+        if (S > 0) cl.w0 = cr[0];
         cl.rest = reinterpret_cast<const CreateArgs*>(ud + o_cr) + 1;
         cl.n_win = S;
-        e = cudaMemcpyAsync(st.up.d + up2_0, uh + up2_0, u2.at - up2_0, cudaMemcpyHostToDevice, cs);
-        if (e == cudaSuccess) {
-            launch_store_push(reinterpret_cast<const CompactTrack*>(ud + o_ct), reinterpret_cast<const CompactRun*>(ud + o_run), (int)runs.size(),
-                              max_run, reinterpret_cast<const StoreAppend*>(ud + o_app), S, max_rows, cols_d, N, cs);
-            launch_create(cl, cg, cs);
-            e = cudaGetLastError();
+        if (S > 0) {
+            e = cudaMemcpyAsync(st.up.d + up2_0, uh + up2_0, u2.at - up2_0, cudaMemcpyHostToDevice, cs);
+            if (e == cudaSuccess) {
+                launch_store_push(reinterpret_cast<const CompactTrack*>(ud + o_ct), reinterpret_cast<const CompactRun*>(ud + o_run),
+                                  (int)runs.size(), max_run, reinterpret_cast<const StoreAppend*>(ud + o_app), S, max_rows, cols_d, N, cs);
+                launch_create(cl, cg, cs);
+                e = cudaGetLastError();
+            }
         }
-        if (e == cudaSuccess) e = cudaMemcpyAsync(st.out.h + dn2_0, od + dn2_0, dc.at - dn2_0, cudaMemcpyDeviceToHost, cs);
+        if (e == cudaSuccess && hooked) {
+            std::vector<const unsigned char*> created(ws.size(), nullptr);
+            for (int j = 0; j < S; ++j) created[sel[j]] = cr[j].flags;
+            e = hook->launch(created, cs);
+        }
+        if (e == cudaSuccess && S > 0) e = cudaMemcpyAsync(st.out.h + dn2_0, od + dn2_0, dc.at - dn2_0, cudaMemcpyDeviceToHost, cs);
         if (e == cudaSuccess) e = wait_stream(h);
         if (e != cudaSuccess) {
             // as create_run: the slot -> request maps go back to all -1
@@ -4869,6 +4983,185 @@ int kba_track_group_frame_step_lidar(kba_track_group* g, const kba_frame_step_re
 int kba_track_group_frame_step_lidar_opts(kba_track_group* g, const kba_frame_step_request* req, const kba_frame_lidar* lid,
                                           const kba_options* opts, kba_frame_step_out* out, kba_result* res) {
     return group_frame_step(g, req, true, opts, out, res, "kba_track_group_frame_step_lidar_opts: ", true, lid);
+}
+
+// ---------------------------------------------------------------------------------------------------------------------
+// limo's camera callback as one store call (include/kba_b200.h, kba_track_camera_step and its group forms; kernels in
+// kba_camerastep.cu and those of the two calls it joins).  The frame step's phases (set_frame_step) run with the solve block's
+// (KfsCall) hooked in: the solve's lists go up with the frame's, and once the verdicts are known its records go up with the push's,
+// k_cs_lists builds the post-push landmark lists right after the creation, and the solve block's first part follows in the same
+// launch sequence.  The solve block's rest runs after the frame step's outputs are written.
+// ---------------------------------------------------------------------------------------------------------------------
+struct CameraStep : StepHook {
+    const kba_camera_step_request* req;
+    bool group;
+    const std::string& who;
+    KfsCall& c;
+    std::vector<kba_kfsolve_request>& kq;
+    std::vector<std::vector<int32_t>>& kf;
+    std::vector<char> may_solve;
+    int64_t lists_up = 0;                 // the solve's lists in the first upload
+
+    CameraStep(const kba_camera_step_request* r, bool g, const std::string& w, KfsCall& c_, std::vector<kba_kfsolve_request>& kq_,
+               std::vector<std::vector<int32_t>>& kf_)
+        : req(r), group(g), who(w), c(c_), kq(kq_), kf(kf_) {}
+
+    // after the frame step's checks (kf_slot, n_kf, kf_new and new_slot are valid): the policy, the tags and the solve block's
+    // request checks on the candidate bound, then its staging
+    int checked() override {
+        const int n = (int)c.s.tracks.size();
+        for (int i = 0; i < n; ++i) {
+            const kba_camera_step_request& q = req[i];
+            if (!may_solve[i]) continue;
+            const kba_frame_step_request& f = q.step;
+            std::string why;
+            int rc = KBA_OK;
+            if (q.n_cand < 0) { why = "a negative size"; rc = KBA_ERR_BAD_ARG; }
+            else if (q.n_cand > 0 && (!q.lm_slot || !q.lm_new)) { why = "null argument"; rc = KBA_ERR_BAD_ARG; }
+            std::vector<char> named((size_t)f.n_new, 0);
+            for (int j = 0; j < q.n_cand && rc == KBA_OK; ++j) {
+                const int k = q.lm_new[j];
+                if (k < kCsActive || k >= f.n_new) { why = "candidate tag out of range"; rc = KBA_ERR_BAD_ARG; }
+                else if (k >= 0 && (named[k] || q.lm_slot[j] != f.new_slot[k])) {
+                    why = "a new landmark's tag named twice or not at its new_slot"; rc = KBA_ERR_BAD_ARG;
+                } else if (k >= 0) named[k] = 1;
+            }
+            if (rc != KBA_OK) return fail(rc, who + track_prefix(group, i) + why);
+            kf[i].assign(f.kf_slot, f.kf_slot + f.n_kf);
+            kf[i].push_back(f.kf_new);
+            kba_kfsolve_request& k = kq[i];
+            k.n_kf = f.n_kf + 1; k.n_lm = q.n_cand;
+            k.min_connecting = q.min_connecting; k.min_window = q.min_window; k.max_window = q.max_window;
+            k.n_trk = q.n_trk; k.kf_slot = kf[i].data(); k.lm_slot = q.lm_slot; k.lm_ground = q.lm_ground; k.trk = q.trk;
+            k.classes = q.classes; k.n_class = q.n_class; k.n_outlier = q.n_outlier; k.outlier_slot = q.outlier_slot;
+            k.shrubbery_weight = q.shrubbery_weight; k.params = q.params;
+            k.max_near = q.max_near; k.max_middle = q.max_middle; k.max_far = q.max_far;
+            k.n_depth = q.n_depth; k.depth = q.depth; k.draw = q.draw; k.draw_ctx = q.draw_ctx; k.sel = q.sel;
+            if ((rc = c.check(i, 1)) != KBA_OK) return rc;
+            KfsWin& w = c.ws.back();
+            w.max_meas = std::max(w.max_meas, f.n_meas);  // kf_new, the newest keyframe if the frame is pushed
+        }
+        if (c.ws.empty()) return KBA_OK;
+        const int rc = c.stage();
+        if (rc != KBA_OK) return rc;
+        for (const KfsWin& w : c.ws)
+            if (kq[w.i].n_lm) memcpy(c.st->up.h + w.u_tag, req[w.i].lm_new, 4 * (size_t)kq[w.i].n_lm);
+        return KBA_OK;
+    }
+
+    // the lists, ahead of the records (which wait for the verdicts)
+    cudaError_t upload(cudaStream_t s) override {
+        if (c.ws.empty()) return cudaSuccess;
+        lists_up = (int64_t)(c.up1 - c.rec_end);
+        return cudaMemcpyAsync(c.st->up.d + c.rec_end, c.st->up.h + c.rec_end, c.up1 - c.rec_end, cudaMemcpyHostToDevice, s);
+    }
+
+    std::vector<int> step_of;             // c.ws[v]'s window in the frame step
+
+    // the solve rule: the windows that solve are kept, with the keyframes they list now
+    bool due(const std::vector<StepWin>& ws) override {
+        std::vector<int> win_of(c.s.tracks.size(), -1);
+        for (int v = 0; v < (int)ws.size(); ++v) win_of[ws[v].i] = v;
+        std::vector<KfsWin> keep;
+        for (KfsWin& w : c.ws) {
+            const StepWin& sw = ws[win_of[w.i]];
+            if (req[w.i].solve == KBA_STEP_SOLVE_IF_SELECTED && !sw.selected) continue;
+            w.kn = sw.q->n_kf + (sw.selected ? 1 : 0);
+            keep.push_back(w);
+            step_of.push_back(win_of[w.i]);
+        }
+        c.ws.swap(keep);
+        c.W = (int)c.ws.size();
+        return c.W > 0;
+    }
+
+    cudaError_t launch(const std::vector<const unsigned char*>& created, cudaStream_t s) override {
+        std::vector<const unsigned char*> cr(c.ws.size());
+        for (size_t v = 0; v < c.ws.size(); ++v) cr[v] = created[step_of[v]];
+        if (c.records(&cr) != KBA_OK) return cudaErrorUnknown;
+        cudaError_t e = cudaMemcpyAsync(c.st->up.d, c.st->up.h, c.rec_end, cudaMemcpyHostToDevice, s);
+        if (e == cudaSuccess) e = c.launch_first();
+        if (e == cudaSuccess) e = cudaMemcpyAsync(c.st->out.h, c.st->out.d, c.down1, cudaMemcpyDeviceToHost, s);
+        return e;
+    }
+};
+
+static int set_camera_step(TrackSet& s, bool group, const std::string& who, const kba_camera_step_request* req, const kba_frame_lidar* lid,
+                           bool per_track, const kba_options* opts_adjust, const kba_options* opts_solve, kba_camera_step_out* out,
+                           kba_result* res_adjust, kba_result* res_solve) {
+    const int n = (int)s.tracks.size();
+    std::vector<kba_frame_step_request> fq(n);
+    std::vector<kba_frame_step_out> fo(n);
+    std::vector<kba_kfsolve_request> kq(n);
+    std::vector<kba_kfsolve_out> ko(n);
+    std::vector<std::vector<int32_t>> kf(n);
+    KfsCall c(s, group, who, kq.data(), per_track, opts_solve, ko.data(), res_solve);
+    c.cs = true;
+    CameraStep cs(req, group, who, c, kq, kf);
+    cs.may_solve.assign(n, 0);
+    for (int i = 0; i < n; ++i) {
+        fq[i] = req[i].step; fo[i] = out[i].step; ko[i] = out[i].solve;
+        if (group && req[i].step.n_kf == 0) continue;
+        if (req[i].solve > KBA_STEP_SOLVE_IF_SELECTED) return fail(KBA_ERR_BAD_ARG, who + track_prefix(group, i) + "unknown solve policy");
+        if (req[i].solve != KBA_STEP_SOLVE_NEVER) {
+            if (!out[i].lm_index && req[i].n_cand > 0) return fail(KBA_ERR_BAD_ARG, who + track_prefix(group, i) + "null argument");
+            cs.may_solve[i] = 1;
+        }
+    }
+    int rc = c.check_options([&](int i) { return cs.may_solve[i] != 0; });
+    if (rc != KBA_OK) return rc;
+    rc = set_frame_step(s, group, who, fq.data(), per_track, opts_adjust, fo.data(), res_adjust, lid, &cs);
+    if (rc != KBA_OK) return rc;
+    // the frame step is done: its outputs are the caller's whatever the solve block does
+    Transfer sum = *s.last;
+    sum.h2d += cs.lists_up;
+    for (int i = 0; i < n; ++i) {
+        if (group && req[i].step.n_kf == 0) continue;
+        out[i].step = fo[i];
+        out[i].solved = 0;
+    }
+    if (c.W == 0) {  // no track solves
+        for (int i = 0; i < n; ++i) idle_result(res_solve[i]);
+        if (c.st) {
+            c.st->counts = sum;
+            s.last = &c.st->counts;
+        }
+        return KBA_OK;
+    }
+    c.sum.h2d = sum.h2d + (int64_t)c.rec_end; c.sum.d2h = sum.d2h + (int64_t)c.down1;
+    rc = c.rest();
+    if (rc != KBA_OK) return rc;
+    for (const KfsWin& w : c.ws) {
+        kba_camera_step_out& o = out[w.i];
+        o.solve = ko[w.i];  // the ranking's counts
+        o.solved = 1;
+        o.n_lm = w.ln;
+        if (req[w.i].n_cand) memcpy(o.lm_index, c.st->out.h + w.d_index, 4 * (size_t)req[w.i].n_cand);
+    }
+    return KBA_OK;
+}
+
+int kba_track_camera_step(kba_track* t, const kba_camera_step_request* req, const kba_frame_lidar* lid, const kba_options* opt_adjust,
+                          const kba_options* opt_solve, kba_camera_step_out* out, kba_result* res_adjust, kba_result* res_solve) {
+    static const std::string who = "kba_track_camera_step: ";
+    if (!t || !req || !opt_adjust || !opt_solve || !out || !res_adjust || !res_solve) return fail(KBA_ERR_BAD_ARG, who + "null argument");
+    return set_camera_step(t->set, false, who, req, lid, false, opt_adjust, opt_solve, out, res_adjust, res_solve);
+}
+
+static int group_camera_step(kba_track_group* g, const kba_camera_step_request* req, const kba_frame_lidar* lid, bool per_track,
+                             const kba_options* opts_adjust, const kba_options* opts_solve, kba_camera_step_out* out, kba_result* res_adjust,
+                             kba_result* res_solve, const std::string& who) {
+    if (!g || !req || !opts_adjust || !opts_solve || !out || !res_adjust || !res_solve) return fail(KBA_ERR_BAD_ARG, who + "null argument");
+    return set_camera_step(g->set, true, who, req, lid, per_track, opts_adjust, opts_solve, out, res_adjust, res_solve);
+}
+int kba_track_group_camera_step(kba_track_group* g, const kba_camera_step_request* req, const kba_frame_lidar* lid, const kba_options* opt_adjust,
+                                const kba_options* opt_solve, kba_camera_step_out* out, kba_result* res_adjust, kba_result* res_solve) {
+    return group_camera_step(g, req, lid, false, opt_adjust, opt_solve, out, res_adjust, res_solve, "kba_track_group_camera_step: ");
+}
+int kba_track_group_camera_step_opts(kba_track_group* g, const kba_camera_step_request* req, const kba_frame_lidar* lid,
+                                     const kba_options* opts_adjust, const kba_options* opts_solve, kba_camera_step_out* out,
+                                     kba_result* res_adjust, kba_result* res_solve) {
+    return group_camera_step(g, req, lid, true, opts_adjust, opts_solve, out, res_adjust, res_solve, "kba_track_group_camera_step_opts: ");
 }
 
 // ---------------------------------------------------------------------------------------------------------------------

@@ -250,6 +250,7 @@ struct UpkeepArgs {
     const int* kf_slot = nullptr;          // [n_kf]
     const int* lm_slot = nullptr;          // [n_lm]
     int n_kf = 0, n_lm = 0;
+    const int* n_lm_d = nullptr;           // or null: the deactivation reads n_lm from here (k_cs_lists writes it), n_lm its bound
     int min_connecting = 0, min_window = 0, max_window = 0;
     unsigned stamp = 0;                    // deactivation uses stamp (newest keyframe) and stamp + 1 (surviving keyframes)
     unsigned long long* map = nullptr;     // [lm_cap] scratch, by slot
@@ -402,6 +403,7 @@ struct KfsArgs {
     const int* trk_slot = nullptr;         // [n_trk] slot or -1
     const unsigned char* trk_cls = nullptr;    // [n_trk] kKfs* bits
     int n_kf = 0, n_lm = 0, n_out = 0, n_trk = 0;
+    const int* n_lm_d = nullptr;           // or null: n_lm is read from here (k_cs_lists writes it), the field is its bound
     int* lm_at = nullptr;                  // [lm_cap] scratch, -1 between calls
     int* last = nullptr;                   // [lm_cap] scratch
     unsigned char* lm_out = nullptr;       // [n_lm] outputs
@@ -420,6 +422,24 @@ struct KfsArgs {
 };
 void launch_kfs_labels(const KfsArgs* args, int n_win, cudaStream_t s);
 void launch_kfs_weights(const KfsArgs* args, int n_win, int max_trk, cudaStream_t s);
+
+// ---- limo's camera callback on a track's store (kba_track_camera_step and its group forms, kba_camerastep.cu) ----
+// One CTA per solving window, between the push's creation kernels and the solve block's first part (launch_deactivate,
+// launch_kfs_labels, ...) of the same sequence: the candidate list staged as the solve block's landmark list is compacted in
+// place, in list order, to the landmarks the push leaves active, and its length goes to n_lm, which the deactivation and
+// k_kfs_labels read (UpkeepArgs::n_lm_d, KfsArgs::n_lm_d).
+constexpr int kCsActive = -2, kCsMeasured = -1;  // tags: active before the frame; measured by it (listed iff it is selected)
+struct CsArgs {
+    int* lm_slot = nullptr;                // [n_cand] the candidates in, the solve's list out (in place)
+    unsigned char* ground = nullptr;       // [n_cand] their is_ground_plane, compacted alongside
+    const int* tag = nullptr;              // [n_cand] kCsActive, kCsMeasured or k >= 0: new_slot[k], listed iff created
+    const unsigned char* created = nullptr;  // [n_new] the creation's flags (bit 0: created); null when the frame is not selected
+    int n_cand = 0;
+    int selected = 0;
+    int* index = nullptr;                  // [n_cand] out: each candidate's position in the list, or -1
+    int* n_lm = nullptr;                   // out: the list's length
+};
+void launch_cs_lists(const CsArgs* args, int n_win, cudaStream_t s);
 
 // ---- evaluation of stored windows at the store's state (kba_track_evaluate / kba_track_group_evaluate, kba_evaluate.cu) ----
 // Run after launch_track_gather on the same batch, in place of the packing and the solve: the outputs of window w go to its

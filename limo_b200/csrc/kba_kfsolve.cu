@@ -5,40 +5,12 @@
 // Windows: one CTA per window (a track group's request; a single call is W = 1).  Everything is integer work in a fixed order:
 // each list keeps its input order (block-wide compaction), and "the last tracklet of a slot decides" is an atomicMax over
 // tracklet indices, whose result does not depend on scheduling.
+#include "kba_compact.cuh"
 #include "kba_kernels.h"
 
 namespace kba {
 
 namespace {
-
-// the positions of the elements of [0, n) for which keep(c) holds, in order: emit(c, position); returns how many.  Every thread of
-// the block calls it (blockDim.x = 1024).
-template <class Keep, class Emit>
-__device__ int block_compact(int n, Keep keep, Emit emit) {
-    __shared__ int warp_sum[32];
-    const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5, n_warps = blockDim.x >> 5;
-    int base = 0;
-    for (int c0 = 0; c0 < n; c0 += blockDim.x) {
-        const int c = c0 + threadIdx.x;
-        const bool f = c < n && keep(c);
-        const unsigned m = __ballot_sync(0xffffffffu, f);
-        if (lane == 0) warp_sum[wid] = __popc(m);
-        __syncthreads();
-        if (wid == 0) {
-            int v = lane < n_warps ? warp_sum[lane] : 0;
-            for (int o = 1; o < 32; o <<= 1) {
-                const int u = __shfl_up_sync(0xffffffffu, v, o);
-                if (lane >= o) v += u;
-            }
-            warp_sum[lane] = v;  // inclusive sums over the warps
-        }
-        __syncthreads();
-        if (f) emit(c, base + (wid ? warp_sum[wid - 1] : 0) + __popc(m & ((1u << lane) - 1u)));
-        base += warp_sum[n_warps - 1];
-        __syncthreads();
-    }
-    return base;
-}
 
 // updateLabels (bundle_adjuster_keyframes.cpp:388-431 as the facade states it) over the deactivation's outputs, then the
 // post-deactivation keyframes (the oldest one fixed) and the ranking's candidates (still active, not outliers) with their
@@ -47,7 +19,8 @@ __device__ int block_compact(int n, Keep keep, Emit emit) {
 __global__ void __launch_bounds__(1024) k_kfs_labels(const KfsArgs* args) {
     const KfsArgs& a = args[blockIdx.x];
     const int t = threadIdx.x, B = blockDim.x;
-    for (int j = t; j < a.n_lm; j += B) {
+    const int n_lm = a.n_lm_d ? *a.n_lm_d : a.n_lm;
+    for (int j = t; j < n_lm; j += B) {
         a.lm_at[a.lm_slot[j]] = j;
         a.lm_out[j] = 0;
         a.ground[j] = a.ground_in ? (a.ground_in[j] != 0) : 0;
@@ -65,7 +38,7 @@ __global__ void __launch_bounds__(1024) k_kfs_labels(const KfsArgs* args) {
         if (a.lm_active[j]) atomicMax(&a.last[j], i);
     }
     __syncthreads();
-    for (int j = t; j < a.n_lm; j += B)
+    for (int j = t; j < n_lm; j += B)
         if (a.last[j] >= 0) a.ground[j] = (a.trk_cls[a.last[j]] & kKfsGround) ? 1 : 0;
     for (int i = t; i < a.n_trk; i += B) {
         const int s = a.trk_slot[i], j = s >= 0 ? a.lm_at[s] : -1;
@@ -76,9 +49,9 @@ __global__ void __launch_bounds__(1024) k_kfs_labels(const KfsArgs* args) {
     __syncthreads();
     const int K = block_compact(a.n_kf, [&](int k) { return a.kf_active[k] != 0; },
                                 [&](int k, int o) { a.kf_post[o] = a.kf_slot[k]; a.fixed[o] = o == 0 ? 1 : 0; });
-    const int N = block_compact(a.n_lm, [&](int j) { return a.lm_active[j] && !a.lm_out[j]; },
+    const int N = block_compact(n_lm, [&](int j) { return a.lm_active[j] && !a.lm_out[j]; },
                                 [&](int j, int o) { a.cand[o] = a.lm_slot[j]; a.elig[o] = a.ground[j]; });
-    for (int j = t; j < a.n_lm; j += B) a.lm_at[a.lm_slot[j]] = -1;
+    for (int j = t; j < n_lm; j += B) a.lm_at[a.lm_slot[j]] = -1;
     if (t == 0) {
         a.counts[0] = K; a.counts[1] = N;
         // no keyframe kept (the host refuses the request): the chain runs on the newest listed keyframe and no candidate, so that

@@ -83,7 +83,7 @@ __global__ void __launch_bounds__(256) k_up_mark_active(const __grid_constant__ 
 __global__ void __launch_bounds__(256) k_up_flag(const __grid_constant__ UpkeepLaunch l) {
     const UpkeepArgs& a = win(l);
     const int j = blockIdx.x * blockDim.x + threadIdx.x;
-    if (j < a.n_lm) a.lm_active[j] = a.map[a.lm_slot[j]] == stamped(a.stamp + 1, 0);
+    if (j < (a.n_lm_d ? *a.n_lm_d : a.n_lm)) a.lm_active[j] = a.map[a.lm_slot[j]] == stamped(a.stamp + 1, 0);
 }
 
 // ---- AddDepth costs -----------------------------------------------------------------------------------------------------------
