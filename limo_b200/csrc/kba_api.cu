@@ -1100,6 +1100,19 @@ struct SolveTotals {
     double time_cap = 0;    // host safety cap (seconds per inner solve), <= 0: none -- some window has no time limit
 };
 
+// The trimming quantiles of every path (k_trim_select, k_ev_finish, k_adjust_pose): a group rejects its landmarks of rank
+// >= (int)(N * quantile), so a NaN or negative quantile would reject every landmark with a residual and one above 1 none.
+static int quantile_check(const kba_options* o, std::string& why) {
+    const std::pair<const char*, double> q[3] = {
+        {"depth_quantile", o->depth_quantile}, {"reprojection_quantile", o->reprojection_quantile}, {"gp_quantile", o->gp_quantile}};
+    for (const auto& e : q)
+        if (!(e.second >= 0.0 && e.second <= 1.0)) {
+            why = std::string("kba_options.") + e.first + " must lie in [0, 1] (got " + std::to_string(e.second) + ")";
+            return KBA_ERR_BAD_ARG;
+        }
+    return KBA_OK;
+}
+
 // Every check of a solve's options, before anything is uploaded.  opts[i] is unit i's (per_unit, n entries) or opts[0] every
 // unit's; live(i) false: unit i sits the solve out and its entry is not read.  Errors name the unit ("window 3: ...") when the
 // options are per unit.
@@ -1116,6 +1129,7 @@ static int solve_options_check(int n, const kba_options* opts, bool per_unit, co
             why = at + "kba_options.precision differs from " + unit + std::to_string(first) + "'s: the precision is the same for the whole batch";
             return KBA_ERR_BAD_ARG;
         }
+        if (quantile_check(o, why) != KBA_OK) { why = at + why; return KBA_ERR_BAD_ARG; }
         if (o->num_trim_rounds > 6 || (o->num_trim_rounds < 0 && o->num_rounds_option > 6)) {
             why = at + "at most 6 trimming rounds (KBA_MAX_SOLVES = 8 inner solves incl. one retry and the final solve)";
             return KBA_ERR_CAPACITY;
@@ -3160,6 +3174,7 @@ static int frame_check(kba_track* t, const kba_track_frame* f, const kba_options
 
 static int options_check(const kba_options* opt, std::string& why) {
     if (opt->precision != 0) { why = "a frame is solved in FP64 only (kba_options.precision must be 0)"; return KBA_ERR_BAD_ARG; }
+    if (quantile_check(opt, why) != KBA_OK) return KBA_ERR_BAD_ARG;
     if (opt->num_trim_rounds > 6 || (opt->num_trim_rounds < 0 && opt->num_rounds_option > 6)) {
         why = "at most 6 trimming rounds (KBA_MAX_SOLVES = 8 inner solves incl. one retry and the final solve)"; return KBA_ERR_CAPACITY;
     }
